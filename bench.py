@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — images/sec end-to-end (c2i, 16x16 tokens) on N B200s, plus roofline and CPU baseline.
+"""bench.py — images/sec end-to-end (c2i, 16x16 tokens) on N H100s, plus roofline; reference GPU / CPU legs on request.
 
     python bench.py --gpus N --steps K --warmup W            (N>1: launched by torchrun, one rank per GPU)
     python bench.py --impl reference --gpus N --steps K --warmup W
@@ -45,16 +45,24 @@ def parse():
     p.add_argument("--t2i", action="store_true",
                    help="text-conditioned workload (BASELINE configs[4]): T=120 synthetic T5 features with ragged left-padded masks, "
                         "caption-MLP prefill + S tokens; use with --gpt-model GPT-XL --image-size 512 --batch 8 --cfg-scale 7.5 --top-k 1000")
-    p.add_argument("--no-cpu-baseline", action="store_true")
+    p.add_argument("--cpu-baseline", action="store_true",
+                   help="also time a bounded sample of the reference's CPU path (a subprocess of up to 10 minutes)")
+    p.add_argument("--no-cpu-baseline", action="store_true", help="accepted for compatibility: the CPU leg is off unless --cpu-baseline")
     p.add_argument("--no-roofline", action="store_true")
+    p.add_argument("--gpu-reference", action="store_true",
+                   help="also time the reference's PyTorch-GPU path (oracle port, bf16, eager + torch.compile) on this GPU "
+                        "(a subprocess of up to 15 minutes; `--impl gpu-reference` runs it alone)")
     p.add_argument("--no-gpu-reference", action="store_true",
-                   help="skip the leg that times the reference's PyTorch-GPU path (oracle port, bf16, eager + torch.compile) on this GPU")
+                   help="accepted for compatibility: the GPU reference leg is off unless --gpu-reference")
     p.add_argument("--gpu-reference-batches", default="64,32", help="per-GPU batch sizes of the gpu_reference leg (first = --batch)")
     p.add_argument("--no-operating-points", action="store_true", help="skip the extra B=32 (north_star B=256 / 8 GPUs) timing of our arm")
     p.add_argument("--seed", type=int, default=0)
     p.add_argument("--latency", action="store_true", help="accepted for compatibility: the batch-1 latency leg now always runs")
     p.add_argument("--no-latency", action="store_true",
                    help="skip the per-token decode latency leg at batch 1 (R=2 rows under CFG, AR sampling only, < 2 s)")
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="after the timed steps, write what the last timed step returned (the fp32 pixels) as DIR/<name>.npy; "
+                        "inputs are seeded, so two builds run with the same arguments can be compared output for output")
     return p.parse_args()
 
 
@@ -87,7 +95,7 @@ def peaks():
         d = json.load(open(path))
         return dict(hbm_gbs=d["hbm_gbs"], bf16_tflops=d["bf16_tflops"], bf16_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_sustained=989.0, source="fallback (H100 SXM data sheet, 700 W)")
 
 
 class ClockSampler:
@@ -290,7 +298,7 @@ def run_reference(args, rank):
 
 # ---------------------------------------------------------------------------------------------- GPU reference leg
 def run_gpu_reference(args):
-    """The reference's own PyTorch path on THIS GPU (BASELINE.md 3.1): oracle port (bit-identical to the live reference, takes
+    """The reference's own PyTorch path on THIS GPU (the north_star's comparator): oracle port (bit-identical to the live reference, takes
     device tensors), bf16 GPT + fp32/TF32 VQ decode, eager and torch.compile(mode="reduce-overhead", fullgraph=True), same
     batch / cfg / top-k / tokens as our arm, CUDA-event timed. See oracle/gpu_baseline.py."""
     import torch
@@ -396,12 +404,14 @@ def run_ours(args):
             dist.barrier()
         torch.cuda.synchronize()
 
+    last = {}
+
     def timed(fn, steps):
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         barrier()
         ev0.record()
         for _ in range(steps):
-            fn()
+            last["out"] = fn()
         pipe.wait()            # every decode (and D2H) submitted above is inside the timed region
         ev1.record()
         barrier()
@@ -429,6 +439,8 @@ def run_ours(args):
     lib.lg_reset_launch_count()
     ms = timed(lambda: step_resident(labels_dev), args.steps)
     launches = int(lib.lg_launch_count())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"pixels": last["out"]})
     ms_e2e = timed(step_e2e, args.steps)
     clocks = sampler.stop() if rank == 0 else None
     log(f"rank {rank}: timed {ms / args.steps:.1f} ms/step resident, {ms_e2e / args.steps:.1f} ms/step e2e")
@@ -442,7 +454,7 @@ def run_ours(args):
                                    f"batch={B} per GPU (R={R} rows), AR sampling + VQ-16 decode to fp32 pixels",
                        "kv_cache_bytes": int(4 * model_dims(args.gpt_model)[0] * R * model_dims(args.gpt_model)[2] * ((T + S + 7) // 8 * 8)),
                        "global_batch": world * B, "parallelism": f"replica-dp{world}", "weights": "random-init, output head normal(0.02)",
-                       "l2": "working set per step (0.65 GB weights + KV cache up to 3.3 GB + 1 GB activations) exceeds the 126 MB L2; no flush needed",
+                       "l2": "working set per step (0.65 GB weights + KV cache up to 3.3 GB + 1 GB activations) exceeds the 50 MB L2; no flush needed",
                        "weight_broadcast_bytes": bcast_bytes,
                        "pipeline": "VQ decode of batch i on a second stream overlaps the AR sampling of batch i+1; all of it inside the timed region" if use_pipe else "sequential"},
             "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": int(host_labels.numel() * host_labels.element_size()),
@@ -607,8 +619,15 @@ def run_ours(args):
                                                 "note": "north_star headline shape: GPT-L 256-token c2i at B=256 over 8 GPUs = 32 images per GPU"}}
         gpt._workspace, gpt._ws_shape = None, (0, 0)
 
-    # ---------------- reference PyTorch-GPU path on this same GPU (BASELINE.md 3.1; the number north_star asks us to beat), rank 0, N=1
-    if rank == 0 and world == 1 and not args.no_gpu_reference and not args.t2i:
+    # ---------------- reference PyTorch-GPU path on this same GPU (the number north_star asks us to beat), rank 0, N=1
+    # The two reference legs below take up to 25 minutes together (torch.compile of the reference, a CPU sample), so they
+    # run on request only; the `--impl reference` / `--impl gpu-reference` arms time the same paths on their own.
+    if rank == 0 and not (args.gpu_reference and not args.no_gpu_reference):
+        line["gpu_reference"] = {"skipped": "not requested (--gpu-reference, or bench.py --impl gpu-reference)"}
+    if rank == 0 and not (args.cpu_baseline and not args.no_cpu_baseline):
+        line["cpu_baseline"] = {"value": None, "unit": UNIT, "cores": host_cores(), "kind": "port",
+                                "sample": "not requested (--cpu-baseline, or bench.py --impl reference)"}
+    if rank == 0 and world == 1 and args.gpu_reference and not args.no_gpu_reference and not args.t2i:
         try:
             r = subprocess.run([sys.executable, os.path.abspath(__file__), "--impl", "gpu-reference", "--gpt-model", args.gpt_model,
                                 "--image-size", str(args.image_size), "--cfg-scale", str(args.cfg_scale), "--top-k", str(args.top_k),
@@ -634,7 +653,7 @@ def run_ours(args):
         log("gpu reference leg done")
 
     # ---------------- CPU baseline leg (rank 0, N=1 only): bounded sample of the same workload on the host cores
-    if rank == 0 and world == 1 and not args.no_cpu_baseline and not args.t2i:
+    if rank == 0 and world == 1 and args.cpu_baseline and not args.no_cpu_baseline and not args.t2i:
         try:
             r = subprocess.run([sys.executable, os.path.abspath(__file__), "--impl", "reference", "--steps", "1", "--warmup", "1",
                                 "--gpt-model", args.gpt_model, "--image-size", str(args.image_size), "--batch", str(B)],
@@ -650,6 +669,27 @@ def run_ours(args):
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """Write each tensor as out_dir/<name>.npy in float32. A tensor above the 64 MB budget is cut to a fixed, seeded
+    sample of its leading-dimension entries (the same sorted indices on every run)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    budget = DUMP_LIMIT_BYTES // max(1, len(arrays))
+    for name, t in arrays.items():
+        t = t.detach().float().cpu()
+        if t.numel() * 4 > budget:
+            per = max(1, t[0].numel() * 4)
+            keep = max(1, min(t.shape[0], budget // per))
+            idx = torch.randperm(t.shape[0], generator=torch.Generator().manual_seed(0))[:keep].sort().values
+            t = t[idx]
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.numpy())
+    log(f"outputs written to {out_dir}: {', '.join(arrays)}")
 
 
 _REAL_STDOUT = None

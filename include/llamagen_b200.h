@@ -1,5 +1,5 @@
 /*
- * llamagen_b200 — C-ABI of the B200-native autoregressive image-sampling engine.
+ * llamagen_b200 — C-ABI of the H100-native (sm_90a) autoregressive image-sampling engine.
  *
  * Drop-in boundary for ONE hot path of FoundationVision/LlamaGen (reference paths are
  * relative to the reference checkout):
@@ -144,7 +144,7 @@ int  lg_vq_decode(lg_vq* v, const int32_t* codes, int B, int grid, void* dev_ws,
                   float* out_nchw, void* stream);
 /* decode_code followed by the samplers' pixel finishing (sample_c2i_ddp.py:141-143 without the optional resize):
  * clamp(127.5*x + 128, 0, 255) -> uint8, NHWC [B,H,W,3], written straight from conv_out's accumulator drain (no fp32 image in
- * HBM). Needs the tcgen05 conv path (every registry VQ model); bytes equal lg_vq_decode + lg_pixels_to_u8. */
+ * HBM). Needs the wgmma conv path (every registry VQ model); bytes equal lg_vq_decode + lg_pixels_to_u8. */
 int  lg_vq_decode_u8(lg_vq* v, const int32_t* codes, int B, int grid, void* dev_ws, size_t ws_bytes,
                      uint8_t* out_nhwc, void* stream);
 /* VectorQuantizer.forward index path (vq_model.py:215-233): z dev f32 NCHW [B, e_dim, g, g] -> idx int64 [B*g*g]. */

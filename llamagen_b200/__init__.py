@@ -1,4 +1,4 @@
-"""llamagen_b200 — B200-native (sm_100a) drop-in for LlamaGen's sampling hot path.
+"""llamagen_b200 — H100-native (sm_90a) drop-in for LlamaGen's sampling hot path.
 
 Public surface mirrors the reference modules on the path (SURVEY §8b):
     GPT_models, generate          <- autoregressive/models/gpt.py, autoregressive/models/generate.py

@@ -1,4 +1,4 @@
-"""In-tree build of libllamagen_b200.so (sm_100a only).
+"""In-tree build of libllamagen_b200.so (sm_90a only).
 
 nvcc cross-compiles without a GPU; the resulting .so has no dependency on libcuda/libcudart at load
 time (cudart is linked statically, driver entry points are resolved lazily), so it can be dlopen'ed on
@@ -19,7 +19,7 @@ OUT_DIR = os.path.join(HERE, os.environ.get("LG_LIB_DIR", "lib"))
 LIB = os.path.join(OUT_DIR, "libllamagen_b200.so")
 EXTRA_DEFS = os.environ.get("LG_NVCC_DEFS", "").split()
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 CFLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
           "--expt-extended-lambda", "-Xptxas", "-v"]
 

@@ -15,9 +15,8 @@ namespace {
 using namespace tma;
 
 #ifndef LG_ATTN_KC
-#define LG_ATTN_KC 32   // keys per stage. Round 1 (one chain): 48 keys / 3 warps / 8 CTAs per SM beat 64 / 4 / 6 (314.9 vs 319.7 ms/step).
-                        // Round 2 (two chains, final tree): 32 keys / 2 warps / 12 CTAs per SM -> 274.7 ms/step vs 279.7 for 48 / 3 / 8
-                        // (profiles/r2_s22_sweep_attn_kc.txt): the smaller CTAs leave shared memory for the other chain's GEMM CTAs.
+#define LG_ATTN_KC 32   // keys per stage: 32 keys / 2 warps per CTA leave shared memory for the other chain's GEMM CTAs
+                        // (build with -DLG_ATTN_KC=48 or 64 for 3 or 4 warps per CTA)
 #endif
 constexpr int kKC = LG_ATTN_KC;   // keys per stage (64 -> 4 warps, 6 CTAs/SM; 48 -> 3 warps, 8 CTAs/SM)
 constexpr int kStagesA = 2;       // 2 stages of K+V per CTA; contexts here are <= 1144 keys
@@ -497,7 +496,7 @@ int launch_v2(const CUtensorMap& kmap, const CUtensorMap& vmap, const AttnTmaArg
     constexpr int WARP_BYTES = kStagesV2 * 2 * TILE_BYTES;
     const size_t smem = 1024 + (size_t)kWarpsV2 * WARP_BYTES + kWarpsV2 * kStagesV2 * sizeof(uint64_t);
     static DevOnce attr;
-    static int sms = 148;
+    static int sms = 132;
     if (lg_first_on_device(attr)) {
         LG_CUDA_OK(cudaFuncSetAttribute(attn_tma_v2_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         int dev = 0;
@@ -716,7 +715,7 @@ int launch_attention_tma(const AttnArgs& a, cudaStream_t st) {
     if (a.qkv_partial) {     // fused QKV epilogue
         // few (row, head) items (batch-1 latency path): a 6-stage ring holds a whole 288-key context, so every K/V byte is
         // requested before the dependency wait instead of two stages at a time
-        if (a.hd == 64 && a.R * a.H <= 2 * 148 && lg_env_flag("LG_ATTN_DEEP", 1)) return launch_t<64, true, kDeepStages>(km, vm, km16, vm16, t, st);
+        if (a.hd == 64 && a.R * a.H <= 2 * 132 && lg_env_flag("LG_ATTN_DEEP", 1)) return launch_t<64, true, kDeepStages>(km, vm, km16, vm16, t, st);
         // deeper sequential ring (A/B switch): more keys requested before the dependency wait, fewer refill round trips
         const int nst = lg_env_flag("LG_ATTN_NST", 2);
         if (a.hd == 64 && nst == 3) return launch_t<64, true, 3, false>(km, vm, km16, vm16, t, st);
@@ -724,10 +723,9 @@ int launch_attention_tma(const AttnArgs& a, cudaStream_t st) {
         if (a.hd == 64) return launch_t<64, true>(km, vm, km16, vm16, t, st);
         return launch_t<128, true>(km, vm, km16, vm16, t, st);
     }
-    // v2 (persistent warp-per-item, LG_ATTN_V2=1) measured SLOWER than the CTA-per-item kernel on B200 (25.7 vs
-    // 19.1 us at R=128, c=128: with one warp per scheduler the ldmatrix->mma->softmax chain is latency-bound), so it
-    // stays opt-in; profiles/ keeps both ncu captures.
-    const bool v2 = lg_env_flag("LG_ATTN_V2", 0) && a.R * a.H >= 4 * 148 && a.hd == 64 && !a.pos.rows;   // (hd 64 only)
+    // v2 (persistent warp-per-item, LG_ATTN_V2=1) stays opt-in: with one warp per scheduler its ldmatrix->mma->softmax chain is
+    // latency-bound, which made it slower than the CTA-per-item kernel where it was measured.
+    const bool v2 = lg_env_flag("LG_ATTN_V2", 0) && a.R * a.H >= 4 * 132 && a.hd == 64 && !a.pos.rows;   // (hd 64 only)
     if (v2) return launch_v2<64>(km, vm, t, st);
     if (a.hd == 64) return launch_t<64, false>(km, vm, km16, vm16, t, st);
     return launch_t<128, false>(km, vm, km16, vm16, t, st);

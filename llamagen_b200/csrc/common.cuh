@@ -1,4 +1,4 @@
-// Shared device/host helpers for the llamagen_b200 CUDA library (sm_100a only).
+// Shared device/host helpers for the llamagen_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>

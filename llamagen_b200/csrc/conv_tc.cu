@@ -1,28 +1,29 @@
-// Blackwell-native implicit-GEMM convolution for the VQ decoder (vq_model.py:128-194):
+// Hopper implicit-GEMM convolution for the VQ decoder (vq_model.py:128-194):
 //   out[pixel, co] = bias[co] + sum_{tap, ci} in[pixel + tap][ci] * W[co][tap][ci]  (+ residual)
-// on tcgen05 tensor cores with the accumulator in TMEM.
+// on wgmma tensor cores with the accumulator in registers.
 //
-//  * A operand (UMMA M = 128 pixels): an 8x16-pixel patch x 64 channels of the bf16 NHWC activation, fetched by
-//    ONE 4-D TMA box per (tap, channel chunk). The tap offset is just a signed shift of the box origin and the
+//  * A operand (128 pixels = two warpgroups of M = 64): an 8x16-pixel patch x 64 channels of the bf16 NHWC activation,
+//    fetched by ONE 4-D TMA box per (tap, channel chunk). The tap offset is just a signed shift of the box origin and the
 //    3x3 zero padding is TMA's out-of-bounds fill — no im2col buffer, no address arithmetic on the SM.
-//  * B operand (UMMA N = Cout tile <= 128): the weight slab [Cout][tap*Cin + ci] (bf16, K-major), 2-D TMA.
+//  * B operand (N = Cout tile, a power of two <= 128): the weight slab [Cout][tap*Cin + ci] (bf16, K-major), 2-D TMA.
 //  * nearest-2x upsample + 3x3 conv (Upsample, vq_model.py:374-378) is evaluated as four 2x2 "phase" convolutions
 //    on the low-resolution input with pre-summed weights: 16 tap-GEMMs instead of 36 (2.25x fewer FLOPs) and the
 //    upsampled tensor never exists.
-//  * epilogue: all 8 warps drain TMEM (lane = pixel), add bias (+ residual), write bf16 NHWC (or fp32 NCHW for conv_out).
+//  * epilogue: the consumer warpgroups add bias (+ residual) to their registers and write bf16 NHWC (or fp32 NCHW / uint8
+//    for conv_out).
+// Warp roles (288 threads): warps 0-7 = two consumer warpgroups, warp 8 = TMA producer.
 #include "kernels.cuh"
 #include "tma_utils.cuh"
-#include "umma_utils.cuh"
+#include "wgmma_utils.cuh"
 #include <algorithm>
 
 namespace {
 
 using namespace tma;
-using namespace umma;
 
-constexpr int kPix = 128;          // pixels per tile (UMMA M)
+constexpr int kPix = 128;          // pixels per tile (two warpgroups of M = 64)
 constexpr int kCk = 64;            // channels per k-block (128 B)
-constexpr int kConvThreads = 256;
+constexpr int kConvThreads = 288;  // 2 consumer warpgroups + 1 producer warp
 constexpr int kConvStages = 3;     // 3 x 32 KB -> two CTAs per SM overlap prologue / drain with the other's main loop
 constexpr int kATile = kPix * kCk * 2;
 
@@ -33,10 +34,9 @@ struct ConvTcArgs {
     int Ht, Wt;          // extent of the pixel grid the patches tile: the input for modes 0-2, the output for mode 3
     int bh, bw;          // pixel patch, bh*bw == 128
     int tiles_x, tiles_y;
-    int bn;              // Cout tile (multiple of 16, <= 128)
+    int bn;              // Cout tile (power of two in [16, 128])
     int kchunks;         // Cin / 64
     int ntaps;           // 9, 1 or 4
-    int tmem_cols;
     const float* bias;
     const bf16* residual;
     bf16* out_bf;
@@ -48,51 +48,52 @@ struct ConvTcArgs {
     int gn_splits;
 };
 
+// TMA shift of the activation box for k-block i of a tile (tap = i / kchunks)
+__device__ __forceinline__ void conv_tap_offset(const ConvTcArgs& a, int tap, int y0, int x0, int py, int px, int& dy, int& dx) {
+    dy = 0; dx = 0;
+    if (a.mode == 0) { dy = tap / 3 - 1; dx = tap % 3 - 1; }
+    else if (a.mode == 2) { const int ta = tap >> 1, tb = tap & 1; dy = py == 0 ? ta - 1 : ta; dx = px == 0 ? tb - 1 : tb; }
+    // mode 3: the map steps two input pixels per box element, so tap (ky, kx) of output patch (y0, x0) is the box
+    // at input origin (2*y0 + ky, 2*x0 + kx); the right/bottom padding is TMA's out-of-bounds zero fill
+    else if (a.mode == 3) { dy = y0 + tap / 3; dx = x0 + tap % 3; }
+}
+
+template <int BN>
 __global__ void __launch_bounds__(kConvThreads, 2) conv_tc_kernel(const __grid_constant__ CUtensorMap amap,
                                                                   const __grid_constant__ CUtensorMap wmap, ConvTcArgs a) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    const int b_tile_bytes = a.bn * kCk * 2;
-    const int stage_bytes = kATile + ((b_tile_bytes + 1023) / 1024) * 1024;
+    constexpr int b_tile_bytes = BN * kCk * 2;
+    constexpr int stage_bytes = kATile + ((b_tile_bytes + 1023) / 1024) * 1024;
     uint8_t* tiles = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(tiles + kConvStages * stage_bytes);
     uint64_t* empty_bar = full_bar + kConvStages;
-    uint64_t* tmem_full_bar = empty_bar + kConvStages;
-    uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
 
-    uint64_t* tmem_empty_bar = reinterpret_cast<uint64_t*>(tmem_base_slot + 2);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tiles_per_img = a.tiles_x * a.tiles_y;
     const int nkb = a.ntaps * a.kchunks;
     const int total_tiles = a.gx * a.gy * a.gz;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         prefetch_map(&amap);
         prefetch_map(&wmap);
-        for (int s = 0; s < kConvStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(tmem_full_bar, 1);
-        mbar_init(tmem_empty_bar, kConvThreads / 32);
+        for (int s = 0; s < kConvStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_base_slot, (uint32_t)a.tmem_cols);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_base_slot;
 
     // Persistent tile loop: CTA c processes tiles c, c + gridDim.x, ...  (tile = ((phase * gy) + cout_tile) * gx + pixel_patch).
     // With gridDim.x == total_tiles this is the one-tile-per-CTA kernel; a smaller grid caps how many SMs the decoder may occupy,
     // which is what lets the AR sampling of the next batch keep its latency while this batch is decoded (pipeline.py).
     uint32_t it0 = 0;                      // k-blocks issued / consumed before the current tile (ring position carries across tiles)
-    uint32_t tcount = 0;                   // tiles this CTA has finished
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, it0 += (uint32_t)nkb, ++tcount) {
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, it0 += (uint32_t)nkb) {
     const int bxi = tile % a.gx, byz = tile / a.gx;
     const int b = bxi / tiles_per_img;
     const int trem = bxi - b * tiles_per_img;
     const int y0 = (trem / a.tiles_x) * a.bh, x0 = (trem % a.tiles_x) * a.bw;
-    const int n0 = (byz % a.gy) * a.bn;
+    const int n0 = (byz % a.gy) * BN;
     const int phase = byz / a.gy, py = phase >> 1, px = phase & 1;
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (elect_one()) {
             const uint32_t tx = (uint32_t)(kATile + b_tile_bytes);
             for (int i = 0; i < nkb; ++i) {
@@ -100,12 +101,8 @@ __global__ void __launch_bounds__(kConvThreads, 2) conv_tc_kernel(const __grid_c
                 const int s = (int)(it % kConvStages);
                 const uint32_t ph = (it / kConvStages) & 1u;
                 const int tap = i / a.kchunks, cc = i - tap * a.kchunks;
-                int dy = 0, dx = 0;
-                if (a.mode == 0) { dy = tap / 3 - 1; dx = tap % 3 - 1; }
-                else if (a.mode == 2) { const int ta = tap >> 1, tb = tap & 1; dy = py == 0 ? ta - 1 : ta; dx = px == 0 ? tb - 1 : tb; }
-                // mode 3: the map steps two input pixels per box element, so tap (ky, kx) of output patch (y0, x0) is the box
-                // at input origin (2*y0 + ky, 2*x0 + kx); the right/bottom padding is TMA's out-of-bounds zero fill
-                else if (a.mode == 3) { dy = y0 + tap / 3; dx = x0 + tap % 3; }
+                int dy, dx;
+                conv_tap_offset(a, tap, y0, x0, py, px, dy, dx);
                 mbar_wait(&empty_bar[s], ph ^ 1);
                 mbar_expect_tx(&full_bar[s], tx);
                 uint8_t* sa = tiles + s * stage_bytes;
@@ -114,160 +111,107 @@ __global__ void __launch_bounds__(kConvThreads, 2) conv_tc_kernel(const __grid_c
             }
         }
         __syncwarp();
-    } else if (warp == 1) {
-        const uint32_t idesc = make_idesc(a.bn);
-        // the accumulator is reused: every warp must have drained the previous tile before the first MMA overwrites it
-        mbar_wait(tmem_empty_bar, (tcount & 1u) ^ 1u);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        for (int i = 0; i < nkb; ++i) {
-            const uint32_t it = it0 + (uint32_t)i;
-            const int s = (int)(it % kConvStages);
-            const uint32_t ph = (it / kConvStages) & 1u;
-            mbar_wait(&full_bar[s], ph);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (elect_one()) {
-                const uint32_t sa = smem_u32(tiles + s * stage_bytes);
-                const uint64_t adesc = make_desc_sw128(sa);
-                const uint64_t bdesc = make_desc_sw128(sa + kATile);
-#pragma unroll
-                for (int k = 0; k < kCk / 16; ++k)
-                    umma_bf16(tmem_base, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, (uint32_t)((i | k) != 0));
-                umma_commit(&empty_bar[s]);
-                if (i == nkb - 1) umma_commit(tmem_full_bar);
-            }
-            __syncwarp();
-        }
+        continue;
     }
 
-    // ---------------------------------------------------------------------- drain: lane = pixel of the patch
-    {
-        const int q = warp & 3, half = warp >> 2;
-        const int pix = q * 32 + lane;
+    // ---------------------------------------------------------------------- consumers: warpgroup g owns pixels [64 g, 64 g + 64)
+    const int g = warp >> 2;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int i = 0; i < nkb; ++i) {
+        const uint32_t it = it0 + (uint32_t)i;
+        const int s = (int)(it % kConvStages);
+        mbar_wait(&full_bar[s], (it / kConvStages) & 1u);
+        const uint32_t sa = smem_u32(tiles + s * stage_bytes);
+        wg::fence_regs<BN / 2>(acc);
+        wg::fence();
+        wg::mma_kblock<BN>(acc, sa + g * (kATile / 2), sa + kATile);
+        wg::commit();
+        wg::wait<1>();
+        wg::fence_regs<BN / 2>(acc);
+        if (i > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[(it - 1) % kConvStages]);
+    }
+    wg::wait<0>();
+    wg::fence_regs<BN / 2>(acc);
+    if (nkb > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[(it0 + (uint32_t)nkb - 1) % kConvStages]);
+
+    // ---------------------------------------------------------------------- epilogue: fragment row = pixel of the patch
+#pragma unroll
+    for (int i = 0; i < BN / 2; i += 2) {
+        const int pix = 64 * g + wg::frag_row(i);
         const int iy = pix / a.bw, ix = pix - iy * a.bw;
         int oy = y0 + iy, ox = x0 + ix;
-        const bool inb = oy < a.Ht && ox < a.Wt;       // patches may overhang the image (TMA zero-filled the reads)
+        if (oy >= a.Ht || ox >= a.Wt) continue;        // patches may overhang the image (TMA zero-filled the reads)
         if (a.mode == 2) { oy = 2 * oy + py; ox = 2 * ox + px; }
-        const int cols_half = ((a.bn / 16 + 1) / 2) * 16;
-        const int c_begin = half * cols_half, c_end = min(a.bn, c_begin + cols_half);
-        mbar_wait(tmem_full_bar, tcount & 1u);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+        const int n = n0 + wg::frag_col(i);            // even; (n, n + 1) are this thread's pair
+        if (n >= a.Cout) continue;
+        const bool two = n + 1 < a.Cout;
+        const float f0 = acc[i] + a.bias[n], f1 = two ? acc[i + 1] + a.bias[n + 1] : 0.f;
         const size_t opix = ((size_t)b * a.Hout + oy) * a.Wout + ox;
-        for (int c0 = c_begin; c0 < c_end; c0 += 16) {
-            uint32_t v[16];
-            tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
-            const int n = n0 + c0;
-            if (!inb || n >= a.Cout) continue;
-            float f[16];
-            if (n + 16 <= a.Cout) {
-                const float4* bp = reinterpret_cast<const float4*>(a.bias + n);
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const float4 bv = __ldg(bp + j);
-                    f[4 * j] = __uint_as_float(v[4 * j]) + bv.x;
-                    f[4 * j + 1] = __uint_as_float(v[4 * j + 1]) + bv.y;
-                    f[4 * j + 2] = __uint_as_float(v[4 * j + 2]) + bv.z;
-                    f[4 * j + 3] = __uint_as_float(v[4 * j + 3]) + bv.w;
-                }
-            } else {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) f[j] = __uint_as_float(v[j]) + (n + j < a.Cout ? a.bias[n + j] : 0.f);
-            }
-            if (a.out_u8) {         // conv_out -> clamp(127.5*x + 128, 0, 255) -> uint8 NHWC, same two roundings as torch's mul then add
-#pragma unroll
-                for (int j = 0; j < 16; ++j)
-                    if (n + j < a.Cout)
-                        a.out_u8[opix * a.Cout + n + j] = (uint8_t)fminf(fmaxf(__fadd_rn(__fmul_rn(127.5f, f[j]), 128.0f), 0.f), 255.f);
-                continue;
-            }
-            if (a.out_nchw) {       // conv_out: fp32 NCHW, Cout = 3
-#pragma unroll
-                for (int j = 0; j < 16; ++j)
-                    if (n + j < a.Cout) a.out_nchw[(((size_t)b * a.Cout + n + j) * a.Hout + oy) * a.Wout + ox] = f[j];
-                continue;
-            }
-            bf16* op = a.out_bf + opix * a.Cout + n;
-            if (a.residual) {
-                const uint4* rp = reinterpret_cast<const uint4*>(a.residual + opix * a.Cout + n);
-#pragma unroll
-                for (int hh = 0; hh < 2; ++hh) {
-                    const uint4 r = rp[hh];
-                    const uint32_t w[4] = {r.x, r.y, r.z, r.w};
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        f[8 * hh + 2 * j] += __uint_as_float(w[j] << 16);
-                        f[8 * hh + 2 * j + 1] += __uint_as_float(w[j] & 0xffff0000u);
-                    }
-                }
-            }
-            uint32_t pk[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                __nv_bfloat162 t = __floats2bfloat162_rn(f[2 * j], f[2 * j + 1]);
-                pk[j] = *reinterpret_cast<uint32_t*>(&t);
-            }
-            reinterpret_cast<uint4*>(op)[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-            reinterpret_cast<uint4*>(op)[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
+        if (a.out_u8) {         // conv_out -> clamp(127.5*x + 128, 0, 255) -> uint8 NHWC, same two roundings as torch's mul then add
+            a.out_u8[opix * a.Cout + n] = (uint8_t)fminf(fmaxf(__fadd_rn(__fmul_rn(127.5f, f0), 128.0f), 0.f), 255.f);
+            if (two) a.out_u8[opix * a.Cout + n + 1] = (uint8_t)fminf(fmaxf(__fadd_rn(__fmul_rn(127.5f, f1), 128.0f), 0.f), 255.f);
+            continue;
         }
-        // this warp's TMEM reads of the tile are complete (tcgen05.wait::ld inside tmem_ld16): hand the accumulator back
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(tmem_empty_bar);
+        if (a.out_nchw) {       // conv_out: fp32 NCHW, Cout = 3
+            a.out_nchw[(((size_t)b * a.Cout + n) * a.Hout + oy) * a.Wout + ox] = f0;
+            if (two) a.out_nchw[(((size_t)b * a.Cout + n + 1) * a.Hout + oy) * a.Wout + ox] = f1;
+            continue;
+        }
+        // bf16 NHWC: Cout % 16 == 0, so the pair is complete and 4-byte aligned
+        float v0 = f0, v1 = f1;
+        if (a.residual) {
+            const uint32_t r = *reinterpret_cast<const uint32_t*>(a.residual + opix * a.Cout + n);
+            v0 += __uint_as_float(r << 16);
+            v1 += __uint_as_float(r & 0xffff0000u);
+        }
+        *reinterpret_cast<__nv_bfloat162*>(a.out_bf + opix * a.Cout + n) = __floats2bfloat162_rn(v0, v1);
     }
     }   // tile loop
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, (uint32_t)a.tmem_cols);
 }
 
 // ---------------------------------------------------------------------------------------------------
 // Weights-as-A variant for Cout % 128 == 0 (every ResnetBlock / Upsample / Downsample conv of the VQ models).
 //
-// Why: in the SS form a tcgen05.mma with M = 128 costs ~170 cycles whatever N is (the A operand is fetched at about one row per
-// cycle, DESIGN.md 9.2), so the kernel above (A = 128 pixels, N = Cout tile <= 128) tops out at 128*128*16*2 flop / 170 cycles =
-// 867 TFLOP/s on 148 SMs - exactly what it measures (873). Here A = the 128-row weight slab and B = a 16x16-pixel patch (two 4-D
-// TMA boxes = 256 pixels), so every instruction does twice the work: N = 256, the UMMA maximum.
+// A = the 128-row weight slab (two warpgroups of 64 output channels) and B = a 16x16-pixel patch (two 4-D TMA boxes =
+// 256 pixels), so every wgmma is m64n256k16, the largest shape: the 64 x 16 A slice fetched from shared memory is reused
+// across 256 pixels instead of 128.
 //
-// TMEM holds the tile as [lane = output channel][column = pixel]. The drain goes through shared memory 64 pixels at a time
-// (fp32 [64][128] in a retired B stage) so that global traffic stays 16-byte vectors along the NHWC channel axis and
-// acc + bias + residual is rounded to bf16 once, as in the kernel above.
+// The drain goes through shared memory 64 pixels at a time (fp32 [64][128] in a retired B stage) so that global traffic
+// stays 16-byte vectors along the NHWC channel axis and acc + bias + residual is rounded to bf16 once, as in the kernel above.
 // ---------------------------------------------------------------------------------------------------
-constexpr int kWStages = 2;                      // 2 x 48 KB: two CTAs per SM overlap one tile's drain with the other's MMAs
+constexpr int kWStages = 2;                      // 2 x 48 KB
 constexpr int kWATile = 128 * kCk * 2;           // weights: 128 couts x 64 ch = 16 KB
 constexpr int kWBTile = 256 * kCk * 2;           // pixels: 256 x 64 ch = 32 KB (two 8x16 boxes)
 constexpr int kWStage = kWATile + kWBTile;
+// drain staging row stride (floats): 132 instead of 128 moves the 4 lanes that share a fragment row (columns 2 apart) to different
+// banks; 64 rows x 132 floats = 33 KB spill 1 KB past stage 0's B tile into stage 1's A tile, which is also held during the drain
+constexpr int kStgLd = 132;
 
-__global__ void __launch_bounds__(kConvThreads, 2) conv_tcw_kernel(const __grid_constant__ CUtensorMap amap,
+__global__ void __launch_bounds__(kConvThreads, 1) conv_tcw_kernel(const __grid_constant__ CUtensorMap amap,
                                                                    const __grid_constant__ CUtensorMap wmap, ConvTcArgs a) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* tiles = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(tiles + kWStages * kWStage);
     uint64_t* empty_bar = full_bar + kWStages;
-    uint64_t* tmem_full_bar = empty_bar + kWStages;
-    uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
-    uint64_t* tmem_empty_bar = reinterpret_cast<uint64_t*>(tmem_base_slot + 2);
-    float* bias_s = reinterpret_cast<float*>(tmem_empty_bar + 1);     // [128]
+    float* bias_s = reinterpret_cast<float*>(empty_bar + kWStages);     // [128]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tiles_per_img = a.tiles_x * a.tiles_y;
     const int nkb = a.ntaps * a.kchunks;
     const int total_tiles = a.gx * a.gy * a.gz;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         prefetch_map(&amap);
         prefetch_map(&wmap);
-        for (int s = 0; s < kWStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(tmem_full_bar, 1);
-        mbar_init(tmem_empty_bar, kConvThreads / 32);
+        for (int s = 0; s < kWStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_base_slot, 256u);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_base_slot;
 
-    uint32_t it0 = 0, tcount = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, it0 += (uint32_t)nkb, ++tcount) {
+    uint32_t it0 = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, it0 += (uint32_t)nkb) {
         const int bxi = tile % a.gx, byz = tile / a.gx;
         const int b = bxi / tiles_per_img;
         const int trem = bxi - b * tiles_per_img;
@@ -275,17 +219,16 @@ __global__ void __launch_bounds__(kConvThreads, 2) conv_tcw_kernel(const __grid_
         const int n0 = (byz % a.gy) * 128;
         const int phase = byz / a.gy, py = phase >> 1, px = phase & 1;
 
-        if (warp == 0) {
+        if (warp == 8) {
             if (elect_one()) {
                 for (int i = 0; i < nkb; ++i) {
                     const uint32_t it = it0 + (uint32_t)i;
                     const int s = (int)(it % kWStages);
                     const uint32_t ph = (it / kWStages) & 1u;
                     const int tap = i / a.kchunks, cc = i - tap * a.kchunks;
-                    int dy = 0, dx = 0, ys = 8;
-                    if (a.mode == 0) { dy = tap / 3 - 1; dx = tap % 3 - 1; }
-                    else if (a.mode == 2) { const int ta = tap >> 1, tb = tap & 1; dy = py == 0 ? ta - 1 : ta; dx = px == 0 ? tb - 1 : tb; }
-                    else if (a.mode == 3) { dy = y0 + tap / 3; dx = x0 + tap % 3; ys = 16; }   // stride-2 map: coordinates are input pixels
+                    int dy, dx;
+                    conv_tap_offset(a, tap, y0, x0, py, px, dy, dx);
+                    const int ys = a.mode == 3 ? 16 : 8;      // stride-2 map: coordinates are input pixels
                     mbar_wait(&empty_bar[s], ph ^ 1);
                     mbar_expect_tx(&full_bar[s], (uint32_t)kWStage);
                     uint8_t* sa = tiles + s * kWStage;
@@ -295,57 +238,54 @@ __global__ void __launch_bounds__(kConvThreads, 2) conv_tcw_kernel(const __grid_
                 }
             }
             __syncwarp();
-        } else if (warp == 1) {
-            const uint32_t idesc = make_idesc(256);
-            mbar_wait(tmem_empty_bar, (tcount & 1u) ^ 1u);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            for (int i = 0; i < nkb; ++i) {
-                const uint32_t it = it0 + (uint32_t)i;
-                const int s = (int)(it % kWStages);
-                const uint32_t ph = (it / kWStages) & 1u;
-                mbar_wait(&full_bar[s], ph);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                if (elect_one()) {
-                    const uint32_t sa = smem_u32(tiles + s * kWStage);
-                    const uint64_t adesc = make_desc_sw128(sa);
-                    const uint64_t bdesc = make_desc_sw128(sa + kWATile);
-#pragma unroll
-                    for (int k = 0; k < kCk / 16; ++k)
-                        umma_bf16(tmem_base, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, (uint32_t)((i | k) != 0));
-                    // the last two k-blocks do not release their stages through the ring: the drain reuses stage memory, so the
-                    // producer may only refill after every warp has left the drain (tmem_empty)
-                    if (i < nkb - kWStages) umma_commit(&empty_bar[s]);
-                    if (i == nkb - 1) umma_commit(tmem_full_bar);
-                }
-                __syncwarp();
-            }
+            continue;
         }
-        if (threadIdx.x >= 64 && threadIdx.x < 192) bias_s[threadIdx.x - 64] = n0 + (int)threadIdx.x - 64 < a.Cout ? a.bias[n0 + threadIdx.x - 64] : 0.f;
+
+        // ------------------------------------------------------------------ consumers: warpgroup g owns couts [64 g, 64 g + 64)
+        const int g = warp >> 2;
+        float acc[128];
+#pragma unroll
+        for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+        for (int i = 0; i < nkb; ++i) {
+            const uint32_t it = it0 + (uint32_t)i;
+            const int s = (int)(it % kWStages);
+            mbar_wait(&full_bar[s], (it / kWStages) & 1u);
+            const uint32_t sa = smem_u32(tiles + s * kWStage);
+            wg::fence_regs<128>(acc);
+            wg::fence();
+            wg::mma_kblock<256>(acc, sa + g * (kWATile / 2), sa + kWATile);
+            wg::commit();
+            wg::wait<1>();
+            wg::fence_regs<128>(acc);
+            // the last two k-blocks do not release their stages through the ring: the drain reuses stage memory, so the
+            // producer may only refill after both warpgroups have left the drain
+            if (i > 0 && i - 1 < nkb - kWStages && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[(it - 1) % kWStages]);
+        }
+        wg::wait<0>();
+        wg::fence_regs<128>(acc);
+        if (threadIdx.x < 128) bias_s[threadIdx.x] = n0 + (int)threadIdx.x < a.Cout ? a.bias[n0 + threadIdx.x] : 0.f;
+        // both warpgroups' MMAs have retired and neither stage has been released (nkb >= kWStages), so all stage memory is idle:
+        // staging buffer = the B half of stage 0 (+ 1 KB of stage 1)
+        wg::consumer_sync();
 
         // ------------------------------------------------------------------ drain: 4 rounds of 64 pixels through shared memory
-        mbar_wait(tmem_full_bar, tcount & 1u);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        // every MMA has retired (tmem_full), so all stage memory is idle: staging buffer = the B half of stage 0
-        float* stg = reinterpret_cast<float*>(tiles + kWATile);            // [64 pixels][128 channels] fp32 = 32 KB
-        const int q = warp & 3, half = warp >> 2;
-        const int ch = q * 32 + lane;                                      // output channel inside the tile = TMEM lane
+        float* stg = reinterpret_cast<float*>(tiles + kWATile);            // [64 pixels][kStgLd] fp32
         float gs[8], gq[8];                                                // GroupNorm statistics of this thread's 8 channels
 #pragma unroll
         for (int j = 0; j < 8; ++j) { gs[j] = 0.f; gq[j] = 0.f; }
-        for (int rnd = 0; rnd < 4; ++rnd) {
-            // TMEM -> staging: this warp takes 32 of the round's 64 pixel columns
-            {
-                const int c0 = rnd * 64 + half * 32;
-                uint32_t v[32];
-                tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
 #pragma unroll
-                for (int j = 0; j < 32; ++j) stg[(half * 32 + j) * 128 + ch] = __uint_as_float(v[j]);
+        for (int rnd = 0; rnd < 4; ++rnd) {
+            // registers -> staging: the fragment columns [64 rnd, 64 rnd + 64) are registers [32 rnd, 32 rnd + 32)
+#pragma unroll
+            for (int j = 0; j < 32; ++j) {
+                const int i = rnd * 32 + j;
+                stg[(wg::frag_col(i) - rnd * 64) * kStgLd + 64 * g + wg::frag_row(i)] = acc[i];
             }
-            __syncthreads();
+            wg::consumer_sync();
             // staging -> global: 64 pixels x 16 chunks of 8 channels; thread -> 4 chunks
 #pragma unroll
             for (int u = 0; u < 4; ++u) {
-                const int idx = u * kConvThreads + (int)threadIdx.x;      // [0, 1024)
+                const int idx = u * 256 + (int)threadIdx.x;               // [0, 1024)
                 const int pl = idx >> 4, c8 = (idx & 15) * 8;             // pixel inside the round, first of 8 channels
                 const int n = rnd * 64 + pl;                               // pixel column of the tile: box = n / 128, row-major 8x16 inside
                 const int iy = (n >> 7) * 8 + ((n & 127) >> 4), ix = n & 15;
@@ -353,8 +293,8 @@ __global__ void __launch_bounds__(kConvThreads, 2) conv_tcw_kernel(const __grid_
                 if (oy >= a.Ht || ox >= a.Wt) continue;                   // the patch may overhang the image
                 if (a.mode == 2) { oy = 2 * oy + py; ox = 2 * ox + px; }
                 const size_t off = (((size_t)b * a.Hout + oy) * a.Wout + ox) * a.Cout + n0 + c8;
-                const float4 f0 = *reinterpret_cast<const float4*>(stg + pl * 128 + c8);
-                const float4 f1 = *reinterpret_cast<const float4*>(stg + pl * 128 + c8 + 4);
+                const float4 f0 = *reinterpret_cast<const float4*>(stg + pl * kStgLd + c8);
+                const float4 f1 = *reinterpret_cast<const float4*>(stg + pl * kStgLd + c8 + 4);
                 float f[8] = {f0.x, f0.y, f0.z, f0.w, f1.x, f1.y, f1.z, f1.w};
 #pragma unroll
                 for (int j = 0; j < 8; ++j) f[j] += bias_s[c8 + j];
@@ -383,7 +323,7 @@ __global__ void __launch_bounds__(kConvThreads, 2) conv_tcw_kernel(const __grid_
                     }
                 }
             }
-            __syncthreads();
+            wg::consumer_sync();
         }
         if (a.gn_partial) {
             // thread t owns channels (t & 15) * 8 .. +7 of the tile for 16 of its pixels: combine the 16 threads of a channel column
@@ -391,7 +331,7 @@ __global__ void __launch_bounds__(kConvThreads, 2) conv_tcw_kernel(const __grid_
             float* part = stg;                                             // [256 threads][16]
 #pragma unroll
             for (int j = 0; j < 8; ++j) { part[threadIdx.x * 16 + j] = gs[j]; part[threadIdx.x * 16 + 8 + j] = gq[j]; }
-            __syncthreads();
+            wg::consumer_sync();
             const int ngrp = 128 / a.gn_cpg;
             if ((int)threadIdx.x < ngrp) {
                 float ts = 0.f, tq = 0.f;
@@ -404,21 +344,14 @@ __global__ void __launch_bounds__(kConvThreads, 2) conv_tcw_kernel(const __grid_
                 o[0] = ts;
                 o[1] = tq;
             }
-            __syncthreads();
+            wg::consumer_sync();
         }
-        // hand the accumulator AND the stage memory back: the MMA warp waits on tmem_empty before the next tile's first MMA, the
-        // producer on the two stage-empty barriers released here
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(tmem_empty_bar);
-        if (threadIdx.x == 0) {
+        // hand the stage memory back: the producer waits on the stage-empty barriers released here
+        if ((threadIdx.x & 127) == 0) {
             const int nrel = nkb < kWStages ? nkb : kWStages;
             for (int i = nkb - nrel; i < nkb; ++i) mbar_arrive(&empty_bar[(it0 + (uint32_t)i) % kWStages]);
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, 256u);
 }
 
 // W'[phase][co][a*2+b][ci] = sum of the 3x3 taps that land on input offset (a, b) for output parity (py, px)
@@ -444,7 +377,7 @@ __global__ void upsample_phase_weights_kernel(const float* __restrict__ w /*[Cou
 }  // namespace
 
 int conv_tc_make_phase_weights(const float* w_f32, bf16* out, int cout, int cin, cudaStream_t st) {
-    upsample_phase_weights_kernel<<<148 * 4, 256, 0, st>>>(w_f32, out, cout, cin);
+    upsample_phase_weights_kernel<<<132 * 4, 256, 0, st>>>(w_f32, out, cout, cin);
     LG_LAUNCH_CHECK();
     return 0;
 }
@@ -459,6 +392,21 @@ bool conv_tc_supported(int Hin, int Win, int Cin, int Cout, int ksize, int up, b
     if (up && ksize != 3) return false;
     if (up == 2 && (Hin % 2 || Win % 2 || Win < 16 || Hin < 16)) return false;
     return ksize == 1 || ksize == 3;
+}
+
+template <int BN>
+static int launch_conv_tc_t(const CUtensorMap& amap, const CUtensorMap& wmap, const ConvTcArgs& a, dim3 grid, cudaStream_t st) {
+    constexpr int b_tile_bytes = BN * kCk * 2;
+    constexpr int stage_bytes = kATile + ((b_tile_bytes + 1023) / 1024) * 1024;
+    const size_t smem = 1024 + (size_t)kConvStages * stage_bytes + 2 * kConvStages * sizeof(uint64_t);
+    static DevOnce attr;
+    if (lg_first_on_device(attr)) {
+        LG_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024));
+    }
+    LG_REQUIRE(smem <= 110 * 1024, "conv_tc: shared memory %zu too large", smem);
+    conv_tc_kernel<BN><<<grid, kConvThreads, smem, st>>>(amap, wmap, a);
+    LG_LAUNCH_CHECK();
+    return 0;
 }
 
 // weights: up == 0 or 2 (stride-2 Downsample) -> [Cout][k*k][Cin] bf16 ; up == 1 -> phase weights [4][Cout][4][Cin] bf16
@@ -479,10 +427,9 @@ int launch_conv_tc(const bf16* in, int B, int Hin, int Win, int Cin, const bf16*
     a.bh = kPix / a.bw;
     a.tiles_x = cdiv(a.Wt, a.bw);
     a.tiles_y = cdiv(a.Ht, a.bh);
-    a.bn = std::min(128, ((Cout + 15) / 16) * 16);
+    a.bn = 16;
+    while (a.bn < 128 && a.bn < Cout) a.bn *= 2;
     a.kchunks = Cin / kCk;
-    a.tmem_cols = 32;
-    while (a.tmem_cols < a.bn) a.tmem_cols *= 2;
     a.bias = bias; a.residual = residual; a.out_bf = out_bf; a.out_nchw = out_nchw; a.out_u8 = out_u8;
 
     CUtensorMap amap, wmap;
@@ -491,17 +438,11 @@ int launch_conv_tc(const bf16* in, int B, int Hin, int Win, int Cin, const bf16*
     const uint64_t wrows = (uint64_t)(up ? 4 : 1) * Cout, wcols = (uint64_t)a.ntaps * Cin;
     LG_TRY(tma::make_map_2d(&wmap, weights, wrows, wcols, wcols, (uint32_t)a.bn, kCk));
 
-    const int b_tile_bytes = a.bn * kCk * 2;
-    const int stage_bytes = kATile + ((b_tile_bytes + 1023) / 1024) * 1024;
-    const size_t smem = 1024 + (size_t)kConvStages * stage_bytes + (2 * kConvStages + 2) * sizeof(uint64_t) + 16;
-    static DevOnce attr;
-    if (lg_first_on_device(attr)) {
-        LG_CUDA_OK(cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024));
-    }
-    LG_REQUIRE(smem <= 110 * 1024, "conv_tc: shared memory %zu too large", smem);
     // CTA budget: 0 = one CTA per tile; > 0 = persistent CTAs (lg_vq_set_cta_budget / LG_CONV_CTAS), e.g. 64 while the next batch samples
     const int budget = g_conv_cta_budget >= 0 ? g_conv_cta_budget : lg_env_flag("LG_CONV_CTAS", 0);
-    if (Cout % 128 == 0 && a.Ht >= 16 && a.Wt >= 16 && out_bf && !out_nchw && !out_u8 && lg_env_flag("LG_CONV_SWAP", 1)) {
+    // the weights-as-A kernel drains through its stage memory, which needs every stage held by the tile (>= kWStages k-blocks)
+    if (Cout % 128 == 0 && a.Ht >= 16 && a.Wt >= 16 && out_bf && !out_nchw && !out_u8 && a.ntaps * a.kchunks >= kWStages &&
+        lg_env_flag("LG_CONV_SWAP", 1)) {
         // weights-as-A kernel: 128 couts x a 16x16-pixel patch (two 8x16 boxes) per tile
         ConvTcArgs w = a;
         w.bw = 16; w.bh = 8;
@@ -518,7 +459,7 @@ int launch_conv_tc(const bf16* in, int B, int Hin, int Win, int Cin, const bf16*
         LG_TRY(tma::make_map_nhwc(&amap2, in, (uint64_t)B, (uint64_t)Hin, (uint64_t)Win, (uint64_t)Cin, 8u, 16u, kCk, down ? 2u : 1u));
         const uint64_t wrows2 = (uint64_t)(up ? 4 : 1) * Cout, wcols2 = (uint64_t)a.ntaps * Cin;
         LG_TRY(tma::make_map_2d(&wmap2, weights, wrows2, wcols2, wcols2, 128u, kCk));
-        const size_t smem2 = 1024 + (size_t)kWStages * kWStage + (2 * kWStages + 2) * sizeof(uint64_t) + 16 + 128 * sizeof(float);
+        const size_t smem2 = 1024 + (size_t)kWStages * kWStage + 2 * kWStages * sizeof(uint64_t) + 128 * sizeof(float);
         static DevOnce attr2;
         if (lg_first_on_device(attr2)) {
             LG_CUDA_OK(cudaFuncSetAttribute(conv_tcw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024));
@@ -535,7 +476,10 @@ int launch_conv_tc(const bf16* in, int B, int Hin, int Win, int Cin, const bf16*
     const long long total = (long long)a.gx * a.gy * a.gz;
     LG_REQUIRE(total < (1ll << 31), "conv_tc: too many tiles");
     dim3 grid((unsigned)(budget > 0 ? std::min<long long>(total, budget) : total));
-    conv_tc_kernel<<<grid, kConvThreads, smem, st>>>(amap, wmap, a);
-    LG_LAUNCH_CHECK();
-    return 0;
+    switch (a.bn) {
+        case 16: return launch_conv_tc_t<16>(amap, wmap, a, grid, st);
+        case 32: return launch_conv_tc_t<32>(amap, wmap, a, grid, st);
+        case 64: return launch_conv_tc_t<64>(amap, wmap, a, grid, st);
+        default: return launch_conv_tc_t<128>(amap, wmap, a, grid, st);
+    }
 }

@@ -599,7 +599,7 @@ static int pd_sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     if (!sms[dev & 31]) cudaDeviceGetAttribute(&sms[dev & 31], cudaDevAttrMultiProcessorCount, dev);
-    return sms[dev & 31] > 0 ? sms[dev & 31] : 148;
+    return sms[dev & 31] > 0 ? sms[dev & 31] : 132;
 }
 static int pd_nsplit(int R, int H) {
     const int forced = lg_env_flag("LG_PD_NSPLIT", 0);            // test hook: force the number of context slices (1..8)

@@ -301,8 +301,8 @@ int lg_engine::forward(int M, int Tq, PosArg pos, const float* emb_mask, int B, 
     if (!skip_first_norm) LG_PROF(PC_EMBED_MISC, st, launch_rmsnorm(ws.h, layers[0].attn_norm, ws.xn, M, D, cfg.norm_eps, dt, st));
     skip_first_norm = false;
     // Direct-epilogue GEMMs (gemm_dx.cu, 6 kernels per layer instead of 8) are validated but OFF by default: a CTA that owns the full
-    // reduction issues 64 dependent tcgen05.mma steps (~0.37 us per 64-wide k-block whatever the UMMA N, measured), so each of the
-    // two kernels costs 10-13 us against 4.4 + 3.2 us for the split-K GEMM + row kernel it replaces (392 vs 292 ms/step).
+    // reduction runs its k-blocks as one dependent MMA chain on a single feature tile, so it is serial where the split-K GEMM spreads
+    // the same bytes over ksplit CTAs. It has not been measured against the split-K path on the H100.
     const bool dx = Tq == 1 && M <= 256 && lg_env_flag("LG_DIRECT", 0) && gemm_dx_supported(M, D, D, dt, DX_RESID, false) &&
                         gemm_dx_supported(M, F, D, dt, DX_SWIGLU, true);
     for (int l = 0; l < L; ++l) {
@@ -321,7 +321,7 @@ int lg_engine::forward(int M, int Tq, PosArg pos, const float* emb_mask, int B, 
         AttnArgs aa = attn_args(l);
         // decode steps on the TMA path: the attention kernel is also the QKV epilogue (one dependent kernel less)
         const bool fuse_qkv = lg_env_flag("LG_FUSE_QKV", 1) && attn_tma_enabled() && attn_tma_supported(aa) &&
-                              !(lg_env_flag("LG_ATTN_V2", 0) && R * H >= 4 * 148 && hd == 64);
+                              !(lg_env_flag("LG_ATTN_V2", 0) && R * H >= 4 * 132 && hd == 64);
         if (fuse_qkv) {
             aa.qkv_partial = ws.partial; aa.qkv_ksplit = ks; aa.freqs = freqs;
         } else {
@@ -529,11 +529,16 @@ int lg_engine_set_workspace(lg_engine* e, void* dev_ws, size_t bytes, int rows, 
     // n equal sub-batch workspaces inside the same memory (every region scales with rows, so chain g takes the g-th
     // 1/n of every region; the K/V parts stay inside the zero-initialised cache regions).
     e->n_sub = 0;
-    // Chain-count policy: every chain streams ALL the weights, so two chains only pay while a layer's weights survive in the 126 MB L2
-    // between the chains' visits (GPT-L 27 MB, GPT-XL 39 MB: 2 chains 292 vs 315 ms and 1 078 vs 1 174 ms per step). GPT-3B's layer is
-    // 258 MB: two chains read 12.4 GB per token instead of 6.2 (2 238 vs 1 629 ms per step, profiles/r2_s13_sweep_c4.txt) -> one chain.
-    const double layer_mb = (4.0 * e->cfg.dim * e->cfg.dim + 3.0 * e->cfg.dim * e->cfg.ffn_dim) * e->esz / 1.0e6;
-    int n = lg_env_flag("LG_SPLIT", layer_mb <= 100.0 ? 2 : 1);
+    // Chain-count policy: every chain streams ALL the weights, so two chains only pay while a layer's weights survive in L2 between
+    // the chains' visits, next to the KV and activation traffic of the other chain; otherwise they double the HBM weight traffic.
+    // Two chains run while a layer is at most a third of the L2. On an H100 80GB HBM3 (50 MB L2; both settings alternated twice in
+    // one run) one chain is faster for GPT-L (27 MB per layer, c2i 256 px, B = 64: 431 vs 469 ms/step) and GPT-XL (39 MB, 384 px,
+    // B = 32: 1659 vs 1849 ms/step).
+    // LG_SPLIT forces the chain count.
+    const double layer_bytes = (4.0 * e->cfg.dim * e->cfg.dim + 3.0 * e->cfg.dim * e->cfg.ffn_dim) * e->esz;
+    int l2_bytes = 0, dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&l2_bytes, cudaDevAttrL2CacheSize, dev) != cudaSuccess) l2_bytes = 0;
+    int n = lg_env_flag("LG_SPLIT", 3.0 * layer_bytes <= (double)l2_bytes ? 2 : 1);
     if (n > lg_engine::kMaxChains) n = lg_engine::kMaxChains;
     while (n >= 2 && (rows % n != 0 || (rows / n) % 2 != 0 || rows / n < 16)) --n;
     if (n >= 2 && e->cfg.dtype == LG_DTYPE_BF16 && tmp.have_maps) {
@@ -818,8 +823,8 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
     }
     // ---- decode loop (generate.py:105-123): per chain one captured graph of `unroll` consecutive steps (the loop
     // state is device-resident, so every step has identical kernel arguments), replayed, chains interleaved; the
-    // remainder runs through a second single-step graph. LG_GRAPH_UNROLL > 1 was measured neutral on B200 (the gap
-    // between graph launches is already hidden by the second chain), so the default is one step per graph.
+    // remainder runs through a second single-step graph. The default is one step per graph (LG_GRAPH_UNROLL > 1 captures more):
+    // with two chains the gap between graph launches of one chain is covered by the other chain's kernels.
     int ret = 0;
     const int unroll = std::max(1, std::min(lg_env_flag("LG_GRAPH_UNROLL", 1), remaining));
     auto capture = [&](Chain& k, int nsteps, cudaGraph_t* graph, cudaGraphExec_t* exec, uint64_t* launches) -> int {
@@ -933,7 +938,7 @@ __global__ void round_bf16_kernel(float* p, size_t n) {
 }
 }  // namespace
 static int round_logits_inplace(float* logits, size_t n, cudaStream_t st) {
-    const int blocks = (int)std::min<size_t>((n + 255) / 256, 148 * 8);
+    const int blocks = (int)std::min<size_t>((n + 255) / 256, 132 * 8);
     (void)lg_launch(round_bf16_kernel, dim3(blocks), dim3(256), 0, st, logits, n);
     LG_LAUNCH_CHECK();
     return 0;

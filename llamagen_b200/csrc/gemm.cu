@@ -88,7 +88,7 @@ __global__ void __launch_bounds__(kSkinnyWarps * 32) gemm_skinny_kernel(const T*
 
 struct Plan {
     bool skinny;
-    bool tc;      // tcgen05 / TMEM / TMA kernel (gemm_tc.cu)
+    bool tc;      // wgmma / TMA kernel (gemm_tc.cu)
     int bm;       // mma tile rows
     int ksplit;
 };
@@ -96,8 +96,8 @@ struct Plan {
 Plan make_plan(int M, int N, int K, int dtype) {
     Plan p;
     p.tc = false;
-    // bf16: the tcgen05 kernel is used for every row count (a batch-1 step pads its 2 rows to the minimum UMMA N = 16;
-    // measured 2.5-3.5 us per GEMM vs 6.2 us for the CUDA-core skinny kernel, which stays for the fp32 exact mode).
+    // bf16: the wgmma kernel is used for every row count (a batch-1 step pads its 2 rows to the minimum N = 16); the CUDA-core
+    // skinny kernel stays for the fp32 exact mode.
     const bool tc_ok = lg_env_flag("LG_GEMM_TC", 1) && gemm_tc_supported(M, N, K, dtype) && N % 128 == 0;
     p.skinny = (dtype == LG_DTYPE_F32) || (M <= kSkinnyRT && !tc_ok);
     if (!p.skinny && tc_ok) {
@@ -109,13 +109,13 @@ Plan make_plan(int M, int N, int K, int dtype) {
     if (p.skinny) {
         p.bm = kSkinnyRT;
         const long long ctas = (long long)cdiv(N, 2 * kSkinnyWarps) * cdiv(M, kSkinnyRT);
-        int ks = (int)std::max<long long>(1, 296 / std::max<long long>(ctas, 1));
+        int ks = (int)std::max<long long>(1, 264 / std::max<long long>(ctas, 1));
         ks = std::min(ks, std::max(1, K / 512));
         p.ksplit = std::min(ks, 16);
     } else {
         p.bm = M <= 32 ? 32 : (M <= 64 ? 64 : 128);
         const long long tiles = (long long)cdiv(M, p.bm) * cdiv(N, 128);
-        int ks = (int)std::max<long long>(1, 148 / std::max<long long>(tiles, 1));
+        int ks = (int)std::max<long long>(1, 132 / std::max<long long>(tiles, 1));
         ks = std::min(ks, std::max(1, (K / mma::BK) / 4));
         p.ksplit = std::min(ks, 16);
     }

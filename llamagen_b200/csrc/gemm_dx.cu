@@ -1,4 +1,4 @@
-// "Direct" tcgen05 GEMM for the decode step: one CTA = (128-feature weight tile) x (row block) over the FULL reduction, so
+// "Direct" wgmma GEMM for the decode step: one CTA = (128-feature weight tile) x (row block) over the FULL reduction, so
 // there is no split-K slab and no separate row-epilogue kernel — the consumer of gpt.py's op is fused on both sides:
 //
 //   prologue (optional)  x_hat = RMSNorm(x) * w          gpt.py:143-148   (the CTA holds its rows over all of K in shared memory)
@@ -8,42 +8,37 @@
 //            DX_F32      y as fp32 (tests)
 //
 // A decode layer then is  QKV (split-K slabs) -> attention (reduces them) -> WO' [DX_RESID] -> W13' [norm + DX_SWIGLU] ->
-// W2 (slabs) -> residual_norm : 6 dependent kernels instead of 8 (each one costs 3-5 us of dependent latency, far more than
-// its bytes or flops; profiles/r2_timeline_*.json).
+// W2 (slabs) -> residual_norm : 6 dependent kernels instead of 8 (at decode sizes a kernel's dependent latency outweighs its
+// bytes or flops).
 //
-// Data path: weights are the UMMA A operand (M = 128 features = TMEM lanes) streamed by TMA through an mbarrier ring that is
-// filled BEFORE the programmatic-dependency wait (weights never depend on activations); the activation rows of the CTA are the
-// B operand (UMMA N = 16/32/64 rows), resident in shared memory for all of K as nkb swizzle-128B tiles. With a norm prologue six
-// warps rewrite those tiles in place (row sum of squares, then bf16(bf16(x * rstd) * w), the reference's rounding points) and
-// hand them to the async proxy with fence.proxy.async before the first MMA. The accumulator lives in TMEM and is drained by all
-// eight warps (lane = feature, column = row).
+// Data path: weights are the wgmma A operand (128 features = two warpgroups of M = 64) streamed by TMA through an mbarrier
+// ring that is filled BEFORE the programmatic-dependency wait (weights never depend on activations); the activation rows of
+// the CTA are the B operand (N = 16/32/64 rows), resident in shared memory for all of K as nkb swizzle-128B tiles. With a
+// norm prologue the eight consumer warps rewrite those tiles in place (row sum of squares, then bf16(bf16(x * rstd) * w),
+// the reference's rounding points) and hand them to the async proxy with fence.proxy.async before the first MMA. The
+// accumulator lives in registers (feature = fragment row, activation row = fragment column).
 #include "kernels.cuh"
 #include "tma_utils.cuh"
-#include "umma_utils.cuh"
+#include "wgmma_utils.cuh"
 #include <algorithm>
 
 namespace {
 
 using namespace tma;
-using namespace umma;
 
-constexpr int kTileN = 128;                      // weight rows per CTA (UMMA M); paired: 64 of Wa followed by 64 of Wb
+constexpr int kTileN = 128;                      // weight rows per CTA; paired: 64 of Wa followed by 64 of Wb
 constexpr int kBK = 64;                          // bf16 elements per k-block = one 128-byte swizzle row
 constexpr int kWBytes = kTileN * kBK * 2;        // 16 KB weight stage
 constexpr int kMaxSt = 12;
-constexpr int kThreadsDx = 256;
+constexpr int kThreadsDx = 288;                  // warps 0-7: two consumer warpgroups, warp 8: TMA producer
+constexpr int kConsumers = 256;
 constexpr size_t kMaxXBytes = 128 * 1024;        // resident activation rows of one CTA (leaves >= 5 weight stages)
-constexpr int kNormWarps = 6;                    // warps 2..7 run the norm prologue
-constexpr int kMiscBytes = 2 * kMaxSt * 8 + 3 * 8 + 8 + 64 * 4 + 192 * 4;   // barriers, TMEM slot, rstd[64], red[192]
+constexpr int kMiscBytes = 2 * kMaxSt * 8 + 8 + 64 * 4 + kConsumers * 4;   // barriers, rstd[64], red[256]
 
 struct DxArgs {
     int M, N, K;          // activation rows, output features (paired: F), reduction
-    int rblk;             // rows per CTA = UMMA N (16, 32 or 64)
     int nkb;              // k-blocks of 64
     int stages;           // weight ring depth
-    int tmem_cols;
-    int ts;               // 1: the weight slice of every MMA step is copied smem -> TMEM (tcgen05.cp) and read from there (TS form)
-    int nacc;             // independent TMEM accumulators the k-blocks rotate over (summed in the drain, fixed order)
     int mode, paired;
     const bf16* normw; float eps;
     float* out_f32; bf16* h; bf16* ff;
@@ -71,57 +66,50 @@ __device__ __forceinline__ uint32_t mul_bf16x2(uint32_t a, uint32_t b) {
     return *reinterpret_cast<uint32_t*>(&r);
 }
 
+// RB: rows per CTA = wgmma N (16, 32 or 64)
+template <int RB>
 __global__ void __launch_bounds__(kThreadsDx, 1) gemm_dx_kernel(const __grid_constant__ CUtensorMap map_wa,
                                                                 const __grid_constant__ CUtensorMap map_wb,
                                                                 const __grid_constant__ CUtensorMap map_x, DxArgs a) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* base = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    const int xtile = a.rblk * 128;                                  // one [rblk rows][64 k] bf16 tile (2/4/8 KB)
+    constexpr int xtile = RB * 128;                                  // one [RB rows][64 k] bf16 tile (2/4/8 KB)
     uint8_t* xres = base;                                            // nkb resident activation tiles
     uint8_t* ring = xres + (size_t)a.nkb * xtile;                    // weight stages (1024-aligned: xtile is a multiple of 2 KB)
     uint64_t* full = reinterpret_cast<uint64_t*>(ring + (size_t)a.stages * kWBytes);
     uint64_t* empty = full + kMaxSt;
     uint64_t* xfull = empty + kMaxSt;
-    uint64_t* xready = xfull + 1;
-    uint64_t* tmem_full = xready + 1;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full + 1);
-    float* rstd_s = reinterpret_cast<float*>(tmem_slot + 2);         // [64]
-    float* red = rstd_s + 64;                                        // [192]
-    bf16* gbuf = reinterpret_cast<bf16*>(red + 192);                 // [nkb * 64] norm weights (zero beyond K)
+    float* rstd_s = reinterpret_cast<float*>(xfull + 1);             // [64]
+    float* red = rstd_s + 64;                                        // [256]
+    bf16* gbuf = reinterpret_cast<bf16*>(((uintptr_t)(red + kConsumers) + 15) & ~(uintptr_t)15);   // [nkb * 64] norm weights (zero beyond K), read as uint4
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int nt = blockIdx.x;
-    const int row0 = (int)blockIdx.y * a.rblk;
-    const int Mb = min(a.rblk, a.M - row0);
+    const int row0 = (int)blockIdx.y * RB;
+    const int Mb = min(RB, a.M - row0);
     const bool norm = a.normw != nullptr;
     if (tid == 0) DX_TRACE(0);
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         prefetch_map(&map_wa);
         prefetch_map(&map_wb);
         prefetch_map(&map_x);
-        for (int s = 0; s < a.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
+        for (int s = 0; s < a.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
         mbar_init(xfull, 1);
-        mbar_init(xready, kNormWarps);
-        mbar_init(tmem_full, 1);
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, (uint32_t)a.tmem_cols);
-    if (norm && warp >= 2) {
+    if (norm && warp < 8) {
         // the norm weight is a parameter: staged before the dependency wait
         const int n8 = a.nkb * 8, k8 = a.K / 8;
-        for (int i = tid - 64; i < n8; i += kNormWarps * 32)
+        for (int i = tid; i < n8; i += kConsumers)
             reinterpret_cast<uint4*>(gbuf)[i] = i < k8 ? __ldg(reinterpret_cast<const uint4*>(a.normw) + i) : make_uint4(0u, 0u, 0u, 0u);
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
     if (tid == 0) DX_TRACE(1);
     lg_pdl_launch_dependents();
-    if (warp != 0) lg_pdl_wait();     // warp 0 waits after it has requested the first weight tiles
+    if (warp != 8) lg_pdl_wait();     // the producer waits after it has requested the first weight tiles
 
-    if (warp == 0) {
+    if (warp == 8) {
         // ------------------------------------------------------------------ TMA producer
         if (elect_one()) {
             auto load_w = [&](int i, int s) {
@@ -165,59 +153,17 @@ __global__ void __launch_bounds__(kThreadsDx, 1) gemm_dx_kernel(const __grid_con
             }
         }
         __syncwarp();
-        lg_pdl_wait();
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------ MMA issuer
-        mbar_wait(norm ? xready : xfull, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        if (lane == 0) DX_TRACE(6);
-        const uint32_t idesc = make_idesc(a.rblk);
-        for (int i = 0; i < a.nkb; ++i) {
-            const int s = i % a.stages;
-            mbar_wait(&full[s], (uint32_t)((i / a.stages) & 1));
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (i == a.nkb - 1 && lane == 0) DX_TRACE(7);
-            if (elect_one()) {
-                const uint64_t wdesc = make_desc_sw128(smem_u32(ring + (size_t)s * kWBytes));
-                const uint64_t xdesc = make_desc_sw128(smem_u32(xres + (size_t)i * xtile));
-#pragma unroll
-                // consecutive k-blocks go to different accumulators: tcgen05.mma into ONE accumulator is a dependent chain (~150 cycles
-                // per instruction at N <= 64, measured), independent accumulators let the operand fetches overlap
-                const uint32_t acc = tmem_base + (uint32_t)((i % a.nacc) * a.rblk);
-                if (a.ts) {
-                    // TS form: in the SS form the tensor core fetches the 128 weight rows of every K=16 step from shared memory at
-                    // ~1 row per cycle (~0.37 us per k-block whatever N, profiles/r2_s9_dx_probe_*); tcgen05.cp moves the same 4 KB
-                    // slice into TMEM (128 lanes x 256 bit, a ring of 16 slots behind the accumulators) and the MMA reads A from there.
-                    // cp and mma execute in issue order, so no extra synchronisation is needed between them.
-#pragma unroll
-                    for (int k = 0; k < kBK / 16; ++k) {
-                        const uint32_t aslot = tmem_base + 128u + (uint32_t)(((i * (kBK / 16) + k) & 15) * 8);
-                        asm volatile("tcgen05.cp.cta_group::1.128x256b [%0], %1;" ::"r"(aslot), "l"(wdesc + (uint64_t)(2 * k)) : "memory");
-                        asm volatile(
-                            "{\n\t.reg .pred p;\n\t"
-                            "setp.ne.b32 p, %4, 0;\n\t"
-                            "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-                            ::"r"(acc), "r"(aslot), "l"(xdesc + (uint64_t)(2 * k)), "r"(idesc), "r"((uint32_t)((i >= a.nacc) | (k != 0))));
-                    }
-                } else {
-#pragma unroll
-                    for (int k = 0; k < kBK / 16; ++k)
-                        umma_bf16(acc, wdesc + (uint64_t)(2 * k), xdesc + (uint64_t)(2 * k), idesc, (uint32_t)((i >= a.nacc) | (k != 0)));
-                }
-                umma_commit(&empty[s]);
-                if (i == a.nkb - 1) umma_commit(tmem_full);
-            }
-            __syncwarp();
-        }
-    } else if (norm) {
-        // ------------------------------------------------------------------ RMSNorm prologue on the resident rows (warps 2..7)
+        return;
+    }
+
+    mbar_wait(xfull, 0);
+    if (norm) {
+        // ------------------------------------------------------------------ RMSNorm prologue on the resident rows
         // thread -> (row, group); a group walks the (k-block, 16-byte chunk) pairs g, g + G, ...  Lanes of a warp hold
         // consecutive rows of the same chunk: with the 128-byte swizzle that is the conflict-free pattern for 128-bit accesses.
-        const int t = tid - 64;
-        const int row = t % a.rblk, grp = t / a.rblk, G = (kNormWarps * 32) / a.rblk;
+        const int row = tid % RB, grp = tid / RB, G = kConsumers / RB;
         const int npairs = a.nkb * 8;
-        mbar_wait(xfull, 0);
-        if (tid == 64) DX_TRACE(5);
+        if (tid == 0) DX_TRACE(5);
         float ss = 0.f;
         for (int j = grp; j < npairs; j += G) {
             const int kb = j >> 3, c = j & 7;
@@ -230,14 +176,14 @@ __global__ void __launch_bounds__(kThreadsDx, 1) gemm_dx_kernel(const __grid_con
                 ss = fmaf(hi, hi, ss);
             }
         }
-        red[grp * a.rblk + row] = ss;
-        asm volatile("bar.sync 1, %0;" ::"n"(kNormWarps * 32) : "memory");
-        if (t < a.rblk) {
+        red[grp * RB + row] = ss;
+        wg::consumer_sync();
+        if (tid < RB) {
             float tot = 0.f;
-            for (int g2 = 0; g2 < G; ++g2) tot += red[g2 * a.rblk + t];      // fixed order: deterministic
-            rstd_s[t] = 1.0f / sqrtf(tot / (float)a.K + a.eps);
+            for (int g2 = 0; g2 < G; ++g2) tot += red[g2 * RB + tid];      // fixed order: deterministic
+            rstd_s[tid] = 1.0f / sqrtf(tot / (float)a.K + a.eps);
         }
-        asm volatile("bar.sync 1, %0;" ::"n"(kNormWarps * 32) : "memory");
+        wg::consumer_sync();
         const float rs = rstd_s[row];
         for (int j = grp; j < npairs; j += G) {
             const int kb = j >> 3, c = j & 7;
@@ -255,90 +201,63 @@ __global__ void __launch_bounds__(kThreadsDx, 1) gemm_dx_kernel(const __grid_con
             *px = make_uint4(o[0], o[1], o[2], o[3]);
         }
         fence_proxy_async();          // generic-proxy writes -> visible to the tensor core's async-proxy reads
-        __syncwarp();
-        if (lane == 0) mbar_arrive(xready);
+        wg::consumer_sync();
     }
 
-    // ---------------------------------------------------------------------- drain: TMEM -> registers -> epilogue
-    const int q = warp & 3, half = warp >> 2;
-    const int nl = q * 32 + lane;                                    // feature inside the tile (TMEM lane)
-    const int cpw = max(16, a.rblk / 2);                             // columns (rows of the block) per warp
-    const int c_begin = half * cpw;
-    const bool active = c_begin < a.rblk;
-    float hv[32];
-    if (a.mode == DX_RESID && active) {
-        // residual operand: written two kernels ago, loaded while the MMAs run
-        const bf16* hp = a.h + (size_t)(row0 + c_begin) * a.N + (size_t)nt * kTileN + nl;
+    // ---------------------------------------------------------------------- MMA: warpgroup g owns features [64 g, 64 g + 64)
+    if (tid == 0) DX_TRACE(6);
+    const int g = warp >> 2;
+    float acc[RB / 2];
 #pragma unroll
-        for (int j = 0; j < 32; ++j) hv[j] = (j < cpw && c_begin + j < Mb) ? __bfloat162float(hp[(size_t)j * a.N]) : 0.f;
+    for (int i = 0; i < RB / 2; ++i) acc[i] = 0.f;
+    for (int i = 0; i < a.nkb; ++i) {
+        const int s = i % a.stages;
+        mbar_wait(&full[s], (uint32_t)((i / a.stages) & 1));
+        if (i == a.nkb - 1 && tid == 0) DX_TRACE(7);
+        wg::fence_regs<RB / 2>(acc);
+        wg::fence();
+        wg::mma_kblock<RB>(acc, smem_u32(ring + (size_t)s * kWBytes) + g * (kWBytes / 2), smem_u32(xres + (size_t)i * xtile));
+        wg::commit();
+        wg::wait<1>();
+        wg::fence_regs<RB / 2>(acc);
+        if (i > 0 && (tid & 127) == 0) mbar_arrive(&empty[(i - 1) % a.stages]);
     }
-    mbar_wait(tmem_full, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    if (tid == 64) DX_TRACE(8);
-    // accumulator columns [c, c + 16) of this warp's lane quarter, summed over the nacc accumulators in index order
-    auto load_acc = [&](int c, uint32_t* v) {
-        tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c, v);
-        for (int t = 1; t < a.nacc; ++t) {
-            uint32_t w[16];
-            tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(t * a.rblk + c), w);
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(w[j]));
-        }
-    };
-    float* stash = reinterpret_cast<float*>(ring);                   // [rblk][64] fp32, free once every MMA has retired
+    wg::wait<0>();
+    wg::fence_regs<RB / 2>(acc);
+    if (tid == 0) DX_TRACE(8);
+
+    // ---------------------------------------------------------------------- epilogue from registers
     if (a.mode == DX_SWIGLU) {
-        if (active && q >= 2) {
-            for (int c0 = 0; c0 < cpw; c0 += 16) {
-                uint32_t v[16];
-                load_acc(c_begin + c0, v);
+        float* stash = reinterpret_cast<float*>(ring);               // [RB][64] fp32, free once both warpgroups' MMAs retired
+        wg::consumer_sync();
+        if (g == 1) {
 #pragma unroll
-                for (int j = 0; j < 16; ++j) stash[(c_begin + c0 + j) * 64 + (nl - 64)] = round_bf16(__uint_as_float(v[j]));
-            }
+            for (int i = 0; i < RB / 2; ++i) stash[wg::frag_col(i) * 64 + wg::frag_row(i)] = round_bf16(acc[i]);
         }
-        __syncthreads();
-        if (active && q < 2) {
-            const size_t f = (size_t)nt * 64 + nl;
-            for (int c0 = 0; c0 < cpw; c0 += 16) {
-                uint32_t v[16];
-                load_acc(c_begin + c0, v);
+        wg::consumer_sync();
+        if (g == 0) {
 #pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const int c = c_begin + c0 + j;
-                    if (c < Mb) {
-                        const float av = round_bf16(__uint_as_float(v[j])), bv = stash[c * 64 + nl];
-                        const float sv = round_bf16(av / (1.0f + expf(-av)));
-                        a.ff[(size_t)(row0 + c) * a.N + f] = __float2bfloat16_rn(sv * bv);
-                    }
+            for (int i = 0; i < RB / 2; ++i) {
+                const int c = wg::frag_col(i), nl = wg::frag_row(i);
+                if (c < Mb) {
+                    const float av = round_bf16(acc[i]), bv = stash[c * 64 + nl];
+                    const float sv = round_bf16(av / (1.0f + expf(-av)));
+                    a.ff[(size_t)(row0 + c) * a.N + (size_t)nt * 64 + nl] = __float2bfloat16_rn(sv * bv);
                 }
             }
         }
-    } else if (active) {
-        const size_t n = (size_t)nt * kTileN + nl;
+    } else {
 #pragma unroll
-        for (int c0 = 0; c0 < 32; c0 += 16) {
-            if (c0 >= cpw) break;
-            uint32_t v[16];
-            load_acc(c_begin + c0, v);
-            if (a.mode == DX_RESID) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const int c = c_begin + c0 + j;
-                    if (c < Mb) a.h[(size_t)(row0 + c) * a.N + n] = __float2bfloat16_rn(hv[c0 + j] + round_bf16(__uint_as_float(v[j])));
-                }
-            } else {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const int c = c_begin + c0 + j;
-                    if (c < Mb) a.out_f32[(size_t)(row0 + c) * a.N + n] = __uint_as_float(v[j]);
-                }
-            }
+        for (int i = 0; i < RB / 2; ++i) {
+            const int c = wg::frag_col(i);
+            const size_t n = (size_t)nt * kTileN + 64 * g + wg::frag_row(i);
+            if (c >= Mb) continue;
+            const size_t o = (size_t)(row0 + c) * a.N + n;
+            if (a.mode == DX_RESID) a.h[o] = __float2bfloat16_rn(__bfloat162float(a.h[o]) + round_bf16(acc[i]));
+            else a.out_f32[o] = acc[i];
         }
     }
-    if (tid == 64) DX_TRACE(9);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, (uint32_t)a.tmem_cols);
-    if (tid == 0) DX_TRACE(10);
+    if (tid == 0) DX_TRACE(9);
 }
 
 int pick_rblk(int M, int K) {
@@ -363,6 +282,18 @@ bool gemm_dx_supported(int M, int N, int K, int dtype, int mode, bool norm) {
     return true;
 }
 
+template <int RB>
+static int launch_dx_t(const CUtensorMap& mwa, const CUtensorMap& mwb, const CUtensorMap& mx, const DxArgs& a, dim3 grid,
+                       size_t smem, cudaStream_t st) {
+    static DevOnce attr;
+    if (lg_first_on_device(attr)) {
+        LG_CUDA_OK(cudaFuncSetAttribute(gemm_dx_kernel<RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    }
+    (void)lg_launch(gemm_dx_kernel<RB>, grid, dim3(kThreadsDx), smem, st, mwa, mwb, mx, a);
+    LG_LAUNCH_CHECK();
+    return 0;
+}
+
 int launch_gemm_dx(const GemmDx& g, cudaStream_t st, const GemmNext* next) {
     const bool norm = g.normw != nullptr;
     LG_REQUIRE(gemm_dx_supported(g.M, g.N, g.K, LG_DTYPE_BF16, g.mode, norm), "gemm_dx: unsupported shape %d %d %d mode %d", g.M, g.N, g.K, g.mode);
@@ -373,19 +304,12 @@ int launch_gemm_dx(const GemmDx& g, cudaStream_t st, const GemmNext* next) {
     LG_REQUIRE((g.mode == DX_F32 && g.out_f32) || (g.mode == DX_RESID && g.h) || (g.mode == DX_SWIGLU && g.ff), "gemm_dx: missing output");
     DxArgs a{};
     a.M = g.M; a.N = g.N; a.K = g.K;
-    a.rblk = pick_rblk(g.M, g.K);
+    const int rblk = pick_rblk(g.M, g.K);
     a.nkb = cdiv(g.K, kBK);
     a.mode = g.mode; a.paired = paired ? 1 : 0;
     a.normw = (const bf16*)g.normw; a.eps = g.eps;
     a.out_f32 = g.out_f32; a.h = (bf16*)g.h; a.ff = (bf16*)g.ff;
-    a.nacc = std::max(1, std::min(std::min(lg_env_flag("LG_DX_NACC", 4), 4), a.nkb));
-    while (a.nacc & (a.nacc - 1)) --a.nacc;                         // 1, 2 or 4
-    a.ts = lg_env_flag("LG_DX_TS", 0) ? 1 : 0;
-    if (a.ts && a.nacc * a.rblk > 128) a.nacc = 128 / a.rblk;     // accumulators in columns [0, 128), the A ring in [128, 256)
-    a.tmem_cols = 32;
-    while (a.tmem_cols < a.nacc * a.rblk) a.tmem_cols *= 2;
-    if (a.ts) a.tmem_cols = 256;
-    const size_t xbytes = (size_t)a.nkb * a.rblk * 128;
+    const size_t xbytes = (size_t)a.nkb * rblk * 128;
     const size_t fixed = 1024 + xbytes + kMiscBytes + (norm ? (size_t)a.nkb * kBK * 2 : 0) + 64;
     int stages = (int)std::min<size_t>(kMaxSt, (227 * 1024 - fixed) / kWBytes);
     stages = std::min(stages, std::max(2, lg_env_flag("LG_DX_STAGES", kMaxSt)));
@@ -401,17 +325,13 @@ int launch_gemm_dx(const GemmDx& g, cudaStream_t st, const GemmNext* next) {
     const int wbox = paired ? kTileN / 2 : kTileN;
     LG_TRY(tma::make_map_2d(&mwa, g.Wa, (uint64_t)g.N, (uint64_t)g.K, (uint64_t)g.K, wbox, kBK));
     LG_TRY(tma::make_map_2d(&mwb, paired ? g.Wb : g.Wa, (uint64_t)g.N, (uint64_t)g.K, (uint64_t)g.K, wbox, kBK));
-    LG_TRY(tma::make_map_2d(&mx, g.X, (uint64_t)g.M, (uint64_t)g.K, (uint64_t)g.ldx, (uint32_t)a.rblk, kBK));   // rows >= M read as zero
+    LG_TRY(tma::make_map_2d(&mx, g.X, (uint64_t)g.M, (uint64_t)g.K, (uint64_t)g.ldx, (uint32_t)rblk, kBK));   // rows >= M read as zero
 
     const size_t smem = fixed + (size_t)stages * kWBytes;
-    static DevOnce attr;
-    if (lg_first_on_device(attr)) {
-        LG_CUDA_OK(cudaFuncSetAttribute(gemm_dx_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    }
     LG_REQUIRE(smem <= 227 * 1024, "gemm_dx: shared memory %zu too large", smem);
-    dim3 grid(paired ? g.N / 64 : g.N / kTileN, cdiv(g.M, a.rblk));
+    dim3 grid(paired ? g.N / 64 : g.N / kTileN, cdiv(g.M, rblk));
     LG_REQUIRE(grid.y <= 65535, "gemm_dx: too many row blocks");
-    (void)lg_launch(gemm_dx_kernel, dim3(grid), dim3(kThreadsDx), smem, st, mwa, mwb, mx, a);
-    LG_LAUNCH_CHECK();
-    return 0;
+    if (rblk == 16) return launch_dx_t<16>(mwa, mwb, mx, a, grid, smem, st);
+    if (rblk == 32) return launch_dx_t<32>(mwa, mwb, mx, a, grid, smem, st);
+    return launch_dx_t<64>(mwa, mwb, mx, a, grid, smem, st);
 }

@@ -1,53 +1,44 @@
-// Blackwell-native weight-streaming GEMM: tcgen05.mma (UMMA) with the accumulator in TMEM, operands staged
-// in shared memory by TMA (cp.async.bulk.tensor) through an mbarrier full/empty ring.
+// Hopper weight-streaming GEMM: wgmma with the accumulator in registers, operands staged in shared memory by TMA
+// (cp.async.bulk.tensor) through an mbarrier full/empty ring.
 //
 //   y[r, n] = sum_k x[r, k] * W[n, k]        (nn.Linear without bias, gpt.py:161-163,199-200,287)
 //
-// "Swap-AB" orientation for decode: the WEIGHT tile is the UMMA A operand (M = 128 output features = the
-// 128 TMEM lanes), the activations are the B operand (N = rows padded to 16, <= 256 = TMEM columns), so a
-// skinny batch never wastes the 128-row MMA shape and each CTA streams a [128 x Kslice] weight slab from
-// HBM exactly once. One CTA = one (n-tile, k-slice); split-K slabs (fp32) are reduced by the row-wise
-// epilogue kernels in xf_kernels.cu, exactly like the mma.sync path it replaces (gemm.cu).
+// "Swap-AB" orientation for decode: the WEIGHT tile is the MMA A operand (128 output features = two warpgroups of
+// M = 64), the activations are the B operand (N = rows padded to a power of two in [16, 256]), so a skinny batch never
+// wastes the 64-row MMA shape and each CTA streams a [128 x Kslice] weight slab from HBM exactly once. One CTA = one
+// (n-tile, k-slice); split-K slabs (fp32) are reduced by the row-wise epilogue kernels in xf_kernels.cu, exactly like the
+// mma.sync path (gemm.cu).
 //
-// Warp roles (256 threads): warp 0 = TMA producer (one elected lane), warp 1 = MMA issuer (one elected lane)
-// + TMEM allocator; when the accumulator is complete all 8 warps drain it (TMEM lane quarter = warp % 4,
-// column half = warp / 4). The drain is written as a pointer walk (one IADD + one STG per value): a lone warp per
-// scheduler is latency-bound, so every instruction in this loop costs ~4 cycles (measured: the first version
-// spent 4.8 us of a 7 us kernel here).
+// Warp roles (288 threads): warps 0-7 = two consumer warpgroups (features [0, 64) and [64, 128) of the tile), warp 8 = TMA
+// producer (one elected lane). Each consumer warpgroup stores its accumulator straight from registers into the fp32 slab.
 #include "kernels.cuh"
 #include "tma_utils.cuh"
-#include "umma_utils.cuh"
+#include "wgmma_utils.cuh"
 #include <mutex>
 #include <unordered_map>
 
 namespace {
 
-constexpr int kBlockN = 128;    // weight rows per CTA  (UMMA M)
+constexpr int kBlockN = 128;    // weight rows per CTA (two warpgroups of M = 64)
 constexpr int kBlockK = 64;     // bf16 elements per k-block = 128 B = one swizzle-128B row
 constexpr int kMaxStages = 8;
-constexpr int kThreads = 256;   // 8 warps: TMA producer, MMA issuer, then ALL of them drain the accumulator
+constexpr int kThreads = 288;   // 2 consumer warpgroups + 1 producer warp
 constexpr int kATileBytes = kBlockN * kBlockK * 2;   // 16 KB
-constexpr int kMaxRowsPerCta = 256;                  // UMMA N <= 256 = TMEM columns of one accumulator
+constexpr int kMaxRowsPerCta = 256;                  // wgmma N <= 256
 
 using namespace tma;
-
-using namespace umma;
 
 struct TcArgs {
     int M, N, K;          // activations rows, weight rows, reduction
     int n_split;          // weight rows [0, n_split) come from map_wa, the rest from map_wb
-    int rpad;             // rows of one row block rounded up to 16 (UMMA N); M > 256 is cut into gridDim.z blocks of rblk rows
-    int rblk;             // rows per row block (== M when gridDim.z == 1)
+    int rblk;             // rows per row block (== M when gridDim.z == 1); M > 256 is cut into gridDim.z blocks of rblk rows
     int kblocks_per_split;
-    int tmem_cols;        // power of two >= max(32, rpad)
-    int stages;           // smem ring depth (<= kMaxStages), sized to fit 227 KB
-    int swap;             // 1: weights are the UMMA A operand (TMEM lane = feature); 0: activations are A (TMEM lane = row)
+    int stages;           // smem ring depth (<= kMaxStages)
     float* partial;       // [ksplit][M][N]
     const char* pf0; unsigned long long pfb0;   // next GEMM's weights to pull into L2 (see GemmNext)
     const char* pf1; unsigned long long pfb1;
     unsigned long long* trace;   // debug: [cta][8] %globaltimer stamps of the pipeline phases (nullable)
     unsigned long long whint;    // L2 eviction hint of the weight tiles (0: default policy)
-    int ld32;                    // drain with 32-column TMEM loads where possible
 };
 
 __device__ __forceinline__ unsigned long long gtime() {
@@ -60,19 +51,18 @@ __device__ __forceinline__ unsigned long long gtime() {
         if (a.trace) a.trace[(size_t)(blockIdx.y * gridDim.x + blockIdx.x) * 8 + (slot)] = gtime(); \
     } while (0)
 
-__device__ __forceinline__ void gemm_tc_body(const CUtensorMap& map_wa, const CUtensorMap& map_wb, const CUtensorMap& map_x,
-                                             const TcArgs& a) {
+// RP: rows of one row block padded to a power of two (wgmma N); the activation box has RP rows, rows >= M read as zero
+template <int RP>
+__global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_constant__ CUtensorMap map_wa,
+                                                              const __grid_constant__ CUtensorMap map_wb,
+                                                              const __grid_constant__ CUtensorMap map_x, TcArgs a) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    // stage s: A tile at s*stage_bytes (1024-aligned), B tile right after
-    const int b_tile_bytes = a.rpad * kBlockK * 2;
-    // activations tile: rpad rows are loaded; when it is the UMMA A operand (M = 128) the full 128-row slot is reserved
-    const int stage_bytes = kATileBytes + (a.swap ? ((b_tile_bytes + 1023) / 1024) * 1024 : kATileBytes);
+    constexpr int b_tile_bytes = RP * kBlockK * 2;
+    constexpr int stage_bytes = kATileBytes + ((b_tile_bytes + 1023) / 1024) * 1024;
     uint8_t* tiles = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     const int kStages = a.stages;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(tiles + kStages * stage_bytes);
     uint64_t* empty_bar = full_bar + kMaxStages;
-    uint64_t* tmem_full_bar = empty_bar + kMaxStages;
-    uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n0 = blockIdx.x * kBlockN;
@@ -84,24 +74,19 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& map_wa, const CU
     const int kb0 = ks * a.kblocks_per_split;
     const int nkb = max(0, min(a.kblocks_per_split, total_kb - kb0));
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         prefetch_map(&map_wa);
         prefetch_map(&map_wb);
         prefetch_map(&map_x);
-        for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(tmem_full_bar, 1);
+        for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_base_slot, (uint32_t)a.tmem_cols);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_base_slot;
     if (threadIdx.x == 0) TC_TRACE(1);
     lg_pdl_launch_dependents();
-    if (warp != 0) lg_pdl_wait();   // warp 0 waits after it has requested the first weight tiles
+    if (warp != 8) lg_pdl_wait();   // the producer waits after it has requested the first weight tiles
 
-    if (warp == 0) {
+    if (warp == 8) {
         // ------------------------------------------------------------------ TMA producer
         if (elect_one()) {
             const bool second = n0 >= a.n_split;
@@ -147,124 +132,41 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& map_wa, const CU
             }
             TC_TRACE(2);
         }
-        __syncwarp();      // reconverge: the drain below uses warp-collective (.sync.aligned) TMEM loads
-        lg_pdl_wait();
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------ MMA issuer
-        const uint32_t idesc = make_idesc(a.swap ? a.rpad : kBlockN);
-        for (int i = 0; i < nkb; ++i) {
-            const int s = i % kStages;
-            const uint32_t ph = (uint32_t)((i / kStages) & 1);
-            mbar_wait(&full_bar[s], ph);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (i == 0 && lane == 0) TC_TRACE(3);
-            if (i == nkb - 1 && lane == 0) TC_TRACE(4);
-            if (elect_one()) {
-                const uint32_t sa = smem_u32(tiles + s * stage_bytes);
-                const uint64_t wdesc = make_desc_sw128(sa);
-                const uint64_t xdesc = make_desc_sw128(sa + kATileBytes);
-                const uint64_t adesc = a.swap ? wdesc : xdesc, bdesc = a.swap ? xdesc : wdesc;
-#pragma unroll
-                for (int k = 0; k < kBlockK / 16; ++k) {
-                    // advance 16 bf16 = 32 bytes inside the 128-byte swizzle span: +2 in the (addr >> 4) field
-                    umma_bf16(tmem_base, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, (uint32_t)((i | k) != 0));
-                }
-                umma_commit(&empty_bar[s]);                       // frees the smem slot when these MMAs retire
-                if (i == nkb - 1) umma_commit(tmem_full_bar);     // accumulator complete
-            }
-            __syncwarp();
-        }
+        __syncwarp();
+        return;
     }
-    // ---------------------------------------------------------------------- drain: TMEM -> registers -> fp32 slab
-    if (a.swap) {
-        const int q = warp & 3;                       // TMEM lane quarter this warp may access
-        const int half = warp >> 2;                   // which half of the columns (activation rows) it drains
-        const int n = n0 + q * 32 + lane;
-        const int cols_half = ((a.rpad / 16 + 1) / 2) * 16;
-        const int c_begin = half * cols_half, c_end = min(a.rpad, c_begin + cols_half);
-        {
-        float* out = a.partial + (size_t)ks * a.M * a.N + (size_t)row0 * a.N;
-        if (nkb > 0) {
-            mbar_wait(tmem_full_bar, 0);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (threadIdx.x == 64) TC_TRACE(5);
-            float* p = out + (size_t)c_begin * a.N + n;
-            const size_t stride = (size_t)a.N;
-            int c0 = c_begin;
-            // 32 columns per TMEM load while a full 32-row group of valid rows remains (64-row decode chains: ONE load per warp)
-            if (a.ld32) {
-                for (; c0 + 32 <= c_end && c0 + 32 <= Mb; c0 += 32) {
-                    uint32_t v[32];
-                    tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
-                    if (n < a.N) {
+    // ---------------------------------------------------------------------- consumers: warpgroup g owns features [64 g, 64 g + 64)
+    const int g = warp >> 2;
+    float acc[RP / 2];
 #pragma unroll
-                        for (int j = 0; j < 32; ++j) { *p = __uint_as_float(v[j]); p += stride; }
-                    } else {
-                        p += 32 * stride;
-                    }
-                }
-            }
-            for (; c0 < c_end; c0 += 16) {
-                uint32_t v[16];
-                tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
-                if (n < a.N) {
-                    if (c0 + 16 <= Mb) {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) { *p = __uint_as_float(v[j]); p += stride; }
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) {
-                            if (c0 + j < Mb) *p = __uint_as_float(v[j]);
-                            p += stride;
-                        }
-                    }
-                }
-            }
-        } else if (n < a.N) {
-            for (int r = c_begin; r < min(c_end, Mb); ++r) out[(size_t)r * a.N + n] = 0.f;
-        }
-        }
-    } else {
-        // activations are the A operand: TMEM lane = row r, columns = 128 features -> 64-byte vector stores per thread
-        const int q = warp & 3, half = warp >> 2;
-        const int r = q * 32 + lane;
-        const int c_begin = half * (kBlockN / 2), c_end = c_begin + kBlockN / 2;
-        float* out = a.partial + (size_t)ks * a.M * a.N + (size_t)r * a.N + n0;
-        if (nkb > 0) {
-            mbar_wait(tmem_full_bar, 0);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (threadIdx.x == 64) TC_TRACE(5);
-            for (int c0 = c_begin; c0 < c_end; c0 += 16) {
-                uint32_t v[16];
-                tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
-                if (r < a.M && n0 + c0 + 16 <= a.N) {
-                    float4* p4 = reinterpret_cast<float4*>(out + c0);
-#pragma unroll
-                    for (int j = 0; j < 4; ++j)
-                        p4[j] = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]),
-                                            __uint_as_float(v[4 * j + 3]));
-                } else if (r < a.M) {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j)
-                        if (n0 + c0 + j < a.N) out[c0 + j] = __uint_as_float(v[j]);
-                }
-            }
-        } else if (r < a.M) {
-            for (int c = c_begin; c < c_end; ++c)
-                if (n0 + c < a.N) out[c] = 0.f;
-        }
+    for (int i = 0; i < RP / 2; ++i) acc[i] = 0.f;
+    for (int i = 0; i < nkb; ++i) {
+        const int s = i % kStages;
+        const uint32_t ph = (uint32_t)((i / kStages) & 1);
+        mbar_wait(&full_bar[s], ph);
+        if (i == 0 && threadIdx.x == 0) TC_TRACE(3);
+        if (i == nkb - 1 && threadIdx.x == 0) TC_TRACE(4);
+        const uint32_t sa = smem_u32(tiles + s * stage_bytes);
+        wg::fence_regs<RP / 2>(acc);
+        wg::fence();
+        wg::mma_kblock<RP>(acc, sa + g * (kATileBytes / 2), sa + kATileBytes);
+        wg::commit();
+        wg::wait<1>();                                  // the previous k-block's MMAs have retired: release its stage
+        wg::fence_regs<RP / 2>(acc);
+        if (i > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[(i - 1) % kStages]);
     }
-    if (threadIdx.x == 64) TC_TRACE(6);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, (uint32_t)a.tmem_cols);
+    wg::wait<0>();
+    wg::fence_regs<RP / 2>(acc);
+    // ---------------------------------------------------------------------- drain: registers -> fp32 slab [row][feature]
+    if (threadIdx.x == 0) TC_TRACE(5);
+    float* out = a.partial + (size_t)ks * a.M * a.N + (size_t)row0 * a.N;
+#pragma unroll
+    for (int i = 0; i < RP / 2; ++i) {
+        const int n = n0 + 64 * g + wg::frag_row(i), r = wg::frag_col(i);
+        if (n < a.N && r < Mb) out[(size_t)r * a.N + n] = acc[i];
+    }
+    if (threadIdx.x == 0) TC_TRACE(6);
     if (threadIdx.x == 0) TC_TRACE(7);
-}
-
-__global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_constant__ CUtensorMap map_wa,
-                                                              const __grid_constant__ CUtensorMap map_wb,
-                                                              const __grid_constant__ CUtensorMap map_x, TcArgs a) {
-    gemm_tc_body(map_wa, map_wb, map_x, a);
 }
 
 // ---------------------------------------------------------------------------------------------- host side
@@ -322,18 +224,39 @@ int make_map_nhwc(CUtensorMap* m, const void* base, uint64_t B, uint64_t H, uint
 static unsigned long long* g_tc_trace = nullptr;
 extern "C" void lg_debug_set_tc_trace(unsigned long long* dev_buf) { g_tc_trace = dev_buf; }
 
-// Plan: number of k-slices so that (N/128) * ksplit is ~104 CTAs (measured best on B200 for the decode shapes:
-// 148 -> 350 ms/step, 112 -> 341, 96 -> 340, 72 -> 352; fewer, fatter slices halve the fp32 slab traffic), >= 2 k-blocks per slice.
+// Plan: number of k-slices so that (N/128) * ksplit is about LG_TC_CTAS CTAs (default 92, ~0.7 per SM of an H100; fewer,
+// fatter slices halve the fp32 slab traffic), >= 2 k-blocks per slice.
 int gemm_tc_ksplit(int M, int N, int K) {
     // row blocks (M > 256: t2i prefill) already multiply the CTA count
     const int tiles = cdiv(N, kBlockN) * cdiv(M, kMaxRowsPerCta), kb = cdiv(K, kBlockK);
-    int ks = std::max(1, lg_env_flag("LG_TC_CTAS", 104) / std::max(tiles, 1));
+    int ks = std::max(1, lg_env_flag("LG_TC_CTAS", 92) / std::max(tiles, 1));
     ks = std::min(ks, std::max(1, kb / 2));
     return std::min(ks, 16);
 }
 
 bool gemm_tc_supported(int M, int N, int K, int dtype) {
     return dtype == LG_DTYPE_BF16 && M >= 1 && K % 8 == 0 && N % 2 == 0;
+}
+
+template <int RP>
+static int gemm_tc_launch_t(const CUtensorMap& mwa, const CUtensorMap& mwb, const CUtensorMap& mx, TcArgs& a, dim3 grid,
+                            cudaStream_t st) {
+    constexpr int b_tile_bytes = RP * kBlockK * 2;
+    constexpr int stage_bytes = kATileBytes + ((b_tile_bytes + 1023) / 1024) * 1024;
+    a.stages = std::min(std::min(kMaxStages, lg_env_flag("LG_TC_STAGES", 4)), (int)((225 * 1024 - 1024) / stage_bytes));
+    // 4 stages instead of filling shared memory: a CTA never owns more than ~8 k-blocks, and the smaller footprint lets the
+    // PDL-launched next kernel become resident next to this one.
+    a.stages = std::min(a.stages, std::max(2, a.kblocks_per_split));   // never more stages than k-blocks
+    LG_REQUIRE(a.stages >= 2, "gemm_tc: tile too large for a 2-stage ring");
+    const size_t smem = 1024 + (size_t)a.stages * stage_bytes + 2 * kMaxStages * sizeof(uint64_t);
+    static DevOnce attr;
+    if (lg_first_on_device(attr)) {
+        LG_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<RP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    }
+    LG_REQUIRE(smem <= 227 * 1024, "gemm_tc: shared memory %zu too large", smem);
+    (void)lg_launch(gemm_tc_kernel<RP>, grid, dim3(kThreads), smem, st, mwa, mwb, mx, a);
+    LG_LAUNCH_CHECK();
+    return 0;
 }
 
 static int gemm_tc_launch(const void* X, int ldx, const void* Wa, const void* Wb, int n_split, int M, int N, int K,
@@ -348,48 +271,32 @@ static int gemm_tc_launch(const void* X, int ldx, const void* Wa, const void* Wb
     a.rblk = M <= kMaxRowsPerCta ? M : kMaxRowsPerCta;
     const int zblocks = cdiv(M, a.rblk);
     LG_REQUIRE(zblocks <= 65535, "gemm_tc: %d row blocks not launchable", zblocks);
-    a.rpad = ((a.rblk + 15) / 16) * 16;
+    int rpad = 16;
+    while (rpad < a.rblk) rpad *= 2;
     const int ks = gemm_tc_ksplit(M, N, K);
     const int kb = cdiv(K, kBlockK);
     a.kblocks_per_split = cdiv(kb, ks);
-    // rows-as-lanes (swap = 0, 64-byte vector stores per thread) was measured SLOWER than features-as-lanes on B200:
-    // each warp store then touches 32 different 128-byte lines (drain 2.8-3.2 us vs 1.1 us), so it stays opt-in.
-    a.swap = (lg_env_flag("LG_TC_NOSWAP", 0) && M > 64 && M <= kBlockN && zblocks == 1) ? 0 : 1;
-    a.tmem_cols = 32;
-    while (a.tmem_cols < (a.swap ? a.rpad : kBlockN)) a.tmem_cols *= 2;
     a.partial = partial;
     if (ksplit_out) *ksplit_out = ks;
 
     CUtensorMap mwa, mwb, mx;
     LG_TRY(tma::make_map_2d(&mwa, Wa, (uint64_t)std::min(n_split, N), (uint64_t)K, (uint64_t)K, kBlockN, kBlockK));
     LG_TRY(tma::make_map_2d(&mwb, Wb, (uint64_t)std::max(N - n_split, Wb == Wa ? N : 1), (uint64_t)K, (uint64_t)K, kBlockN, kBlockK));
-    LG_TRY(tma::make_map_2d(&mx, X, (uint64_t)M, (uint64_t)K, (uint64_t)ldx, (uint32_t)a.rpad, kBlockK));   // rows >= M read as zero
+    LG_TRY(tma::make_map_2d(&mx, X, (uint64_t)M, (uint64_t)K, (uint64_t)ldx, (uint32_t)rpad, kBlockK));   // rows >= M read as zero
 
-    const int b_tile_bytes = a.rpad * kBlockK * 2;
-    const int stage_bytes = kATileBytes + (a.swap ? ((b_tile_bytes + 1023) / 1024) * 1024 : kATileBytes);
-    a.stages = std::min(std::min(kMaxStages, lg_env_flag("LG_TC_STAGES", 4)), (int)((225 * 1024 - 1024) / stage_bytes));
-    // 4 stages (96 KB at the R = 64 rows of a decode chain) instead of filling shared memory: a CTA never owns more than ~8
-    // k-blocks, and the smaller footprint lets the PDL-launched next kernel become resident next to this one (filling
-    // shared memory: 335 ms/step, 3 stages at R = 128: 320). With two 64-row chains, 4 stages let the QKV GEMM request its
-    // whole K range before the dependency wait: 3 -> 4 stages = 297.2 -> 294.9 ms/step (2 runs each), 5 no better.
-    a.stages = std::min(a.stages, std::max(2, a.kblocks_per_split));   // never more stages than k-blocks
     a.trace = g_tc_trace;
-    a.ld32 = lg_env_flag("LG_TC_LD32", 1);
     a.whint = (lg_env_flag("LG_L2_HINT", 1) & 2) ? tma::kL2EvictLast : 0ull;
     const bool pf = next && lg_env_flag("LG_L2_PREFETCH", 1);
     a.pf0 = pf ? (const char*)next->p0 : nullptr; a.pfb0 = pf ? next->b0 : 0;
     a.pf1 = pf ? (const char*)next->p1 : nullptr; a.pfb1 = pf ? next->b1 : 0;
-    LG_REQUIRE(a.stages >= 2, "gemm_tc: tile too large for a 2-stage ring");
-    const size_t smem = 1024 + (size_t)a.stages * stage_bytes + (2 * kMaxStages + 1) * sizeof(uint64_t) + 16;
-    static DevOnce attr;
-    if (lg_first_on_device(attr)) {
-        LG_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    const dim3 grid(cdiv(N, kBlockN), ks, zblocks);
+    switch (rpad) {
+        case 16: return gemm_tc_launch_t<16>(mwa, mwb, mx, a, grid, st);
+        case 32: return gemm_tc_launch_t<32>(mwa, mwb, mx, a, grid, st);
+        case 64: return gemm_tc_launch_t<64>(mwa, mwb, mx, a, grid, st);
+        case 128: return gemm_tc_launch_t<128>(mwa, mwb, mx, a, grid, st);
+        default: return gemm_tc_launch_t<256>(mwa, mwb, mx, a, grid, st);
     }
-    LG_REQUIRE(smem <= 227 * 1024, "gemm_tc: shared memory %zu too large", smem);
-    dim3 grid(cdiv(N, kBlockN), ks, zblocks);
-    (void)lg_launch(gemm_tc_kernel, dim3(grid), dim3(kThreads), smem, st, mwa, mwb, mx, a);
-    LG_LAUNCH_CHECK();
-    return 0;
 }
 
 int gemm_tc_partial(const void* X, int ldx, const void* Wa, const void* Wb, int n_split, int M, int N, int K,

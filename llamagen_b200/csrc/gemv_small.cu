@@ -1,6 +1,6 @@
 // Decode GEMMs for R <= 8 activation rows (the batch-1 latency path; R = 2 with classifier-free guidance).
 //
-// At R <= 8 a 128-wide tcgen05 tile is > 90 % padding and the split-K slabs + row-epilogue kernels of the batched path
+// At R <= 8 a 16-wide wgmma N tile is >= 50 % padding and the split-K slabs + row-epilogue kernels of the batched path
 // dominate the token time (8 dependent kernels per layer). Here every CTA OWNS a few output columns over the full K, so
 // there is no split-K, no slab and no separate epilogue kernel: RMSNorm moves into the prologue, residual add /
 // SwiGLU gate / fp32 store into the epilogue, and a layer is 5 dependent kernels

@@ -138,7 +138,7 @@ int launch_attention_tma(const AttnArgs& a, cudaStream_t st);
 // t2i condition prefill (1 < Tq <= 128, hd 64, bf16): TMA-staged Q/K/V, mma.sync QK^T and PV, one CTA per (row, head)
 bool attn_prefill_tc_supported(const AttnArgs& a);
 int launch_attention_prefill_tc(const AttnArgs& a, cudaStream_t st);
-// conv_tc.cu — tcgen05 implicit-GEMM convolution over bf16 NHWC activations (TMA 4-D boxes, TMEM accumulator)
+// conv_tc.cu — wgmma implicit-GEMM convolution over bf16 NHWC activations (TMA 4-D boxes, register accumulators)
 bool conv_tc_supported(int Hin, int Win, int Cin, int Cout, int ksize, int up, bool nchw_out);
 void conv_tc_set_cta_budget(int ctas);   // > 0: persistent conv CTAs (at most `ctas`), 0: one CTA per tile, -1: LG_CONV_CTAS
 int conv_tc_make_phase_weights(const float* w_f32, bf16* out, int cout, int cin, cudaStream_t st);
@@ -146,13 +146,13 @@ int launch_conv_tc(const bf16* in, int B, int Hin, int Win, int Cin, const bf16*
                    int ksize, int up, const bf16* residual, bf16* out_bf, float* out_nchw, cudaStream_t st, uint8_t* out_u8 = nullptr,
                    float* gn_partial = nullptr, size_t gn_floats = 0, int* gn_splits = nullptr);   // *gn_splits > 0: the drain also wrote the
                    // output's GroupNorm(32) partial statistics [B][*gn_splits][32][2] into gn_partial
-// gemm_tc.cu — tcgen05/TMEM/TMA weight-streaming GEMM (bf16, M <= 256)
+// gemm_tc.cu — wgmma/TMA weight-streaming GEMM (bf16, row blocks of <= 256)
 int gemm_tc_ksplit(int M, int N, int K);
 bool gemm_tc_supported(int M, int N, int K, int dtype);
 int gemm_tc_partial(const void* X, int ldx, const void* Wa, const void* Wb, int n_split, int M, int N, int K,
                     float* partial, int* ksplit_out, cudaStream_t st, const GemmNext* next = nullptr);
 
-// gemm_dx.cu — "direct" tcgen05 GEMM of the decode step: (feature tile) x (row block) CTAs over the FULL K (no split-K slab), the
+// gemm_dx.cu — "direct" wgmma GEMM of the decode step: (feature tile) x (row block) CTAs over the FULL K (no split-K slab), the
 // activation rows resident in shared memory; optional RMSNorm prologue on those rows, epilogue by mode
 enum { DX_F32 = 0, DX_RESID = 1, DX_SWIGLU = 2 };
 struct GemmDx {

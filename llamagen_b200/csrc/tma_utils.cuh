@@ -1,4 +1,4 @@
-// mbarrier / TMA (cp.async.bulk.tensor) / tensor-map helpers shared by the sm_100a kernels.
+// mbarrier / TMA (cp.async.bulk.tensor) / tensor-map helpers shared by the sm_90a kernels.
 #pragma once
 #include "common.cuh"
 #include <cuda.h>

@@ -1,4 +1,4 @@
-// VQ tokenizer decode path + codebook argmin on sm_100a (see include/llamagen_b200.h).
+// VQ tokenizer decode path + codebook argmin on sm_90a (see include/llamagen_b200.h).
 //
 // Replaces tokenizer/tokenizer_image/vq_model.py:
 //   decode_code :52-55 = get_codebook_entry :261-276 -> post_quant_conv :48 -> Decoder.forward :173-194
@@ -542,7 +542,7 @@ int make_conv(lg_vq* v, const std::string& name, int cout, int cin, int k, ConvW
     LG_REQUIRE(cin % 8 == 0, "conv '%s': Cin=%d must be a multiple of 8", name.c_str(), cin);
     bf16* d = nullptr;
     LG_TRY(dev_alloc(v, (size_t)cout * cin * k * k, &d));
-    repack_conv_kernel<<<148 * 4, 256, 0, st>>>(w, d, cout, cin, k * k);
+    repack_conv_kernel<<<132 * 4, 256, 0, st>>>(w, d, cout, cin, k * k);
     LG_LAUNCH_CHECK();
     cw->w = d; cw->bias = b; cw->cout = cout; cw->cin = cin; cw->k = k;
     return 0;
@@ -663,7 +663,7 @@ int run_conv(const ConvW& cw, const bf16* in, int B, int Hin, int Win, int up, c
         if (ws && splits > 0) { ws->gn_src = out_bf; ws->gn_splits = splits; }
         return 0;
     }
-    LG_REQUIRE(!out_u8, "uint8 output needs the tcgen05 conv path (Cin %% 64 == 0, LG_CONV_TC=1)");
+    LG_REQUIRE(!out_u8, "uint8 output needs the wgmma conv path (Cin %% 64 == 0, LG_CONV_TC=1)");
     const int Hout = up == 1 ? 2 * Hin : (up == 2 ? Hin / 2 : Hin), Wout = up == 1 ? 2 * Win : (up == 2 ? Win / 2 : Win);
     const int M = B * Hout * Wout, K = cw.k * cw.k * cw.cin;
     mma::ConvA al{in, Hin, Win, cw.cin, Hout, Wout, cw.k, up, M};
@@ -831,7 +831,7 @@ int lg_vq_finalize(lg_vq* v, void* stream) {
         if (lv.up) {
             const std::string un = "decoder.conv_blocks." + std::to_string(bi) + ".upsample.conv";
             LG_TRY(make_conv(v, un, block_in, block_in, 3, &lv.upconv, st));
-            if (block_in % 64 == 0) {   // pre-summed 2x2 phase weights for the tcgen05 upsample path (conv_tc.cu)
+            if (block_in % 64 == 0) {   // pre-summed 2x2 phase weights for the wgmma upsample path (conv_tc.cu)
                 const float* wf = nullptr;
                 LG_TRY(get(v, un + ".weight", {block_in, block_in, 3, 3}, &wf));
                 LG_TRY(dev_alloc(v, (size_t)16 * block_in * block_in, &lv.upconv.w_phase));
@@ -984,7 +984,7 @@ int lg_vq_encode(lg_vq* v, const float* x_nchw, int B, int H, int W, void* dev_w
             const long long items = (long long)bc * h * (wd / 4) * (c.ch / 8);
             const size_t smem = (size_t)28 * c.ch * sizeof(float);
             prof_begin(PC_VQ_CONV, st);
-            conv_in_rgb_kernel<<<(unsigned)std::min<long long>(cdiv(items, 256), 148 * 8), 256, smem, st>>>(x_nchw + (size_t)b0 * 3 * H * W, v->enc_in_w,
+            conv_in_rgb_kernel<<<(unsigned)std::min<long long>(cdiv(items, 256), 132 * 8), 256, smem, st>>>(x_nchw + (size_t)b0 * 3 * H * W, v->enc_in_w,
                                                                                 v->enc_in_b, w.X, bc, h, wd, c.ch);
             prof_end(st);
             LG_LAUNCH_CHECK();

@@ -405,7 +405,7 @@ int launch_residual_norm(const float* partial, int ksplit, int M, int D, void* h
 
 int launch_silu_mul(const float* partial, int ksplit, int M, int F, void* out, int dtype, cudaStream_t st) {
     LG_REQUIRE(F % 4 == 0, "ffn dim %d must be a multiple of 4", F);
-    const int blocks = (int)std::min<long long>(((long long)M * F / 4 + 255) / 256, 148 * 16);
+    const int blocks = (int)std::min<long long>(((long long)M * F / 4 + 255) / 256, 132 * 16);
     return dispatch_dtype(
         dtype,
         [&] { (void)lg_launch(silu_mul_kernel<float>, dim3(blocks), dim3(256), 0, st, partial, ksplit, M, F, (float*)out); LG_LAUNCH_CHECK(); return 0; },
@@ -414,7 +414,7 @@ int launch_silu_mul(const float* partial, int ksplit, int M, int F, void* out, i
 
 int launch_store_act(const float* partial, int ksplit, int M, int N, void* out, int gelu, int dtype, cudaStream_t st) {
     const size_t total = (size_t)M * N;
-    const int blocks = (int)std::min<size_t>((total + 255) / 256, 148 * 16);
+    const int blocks = (int)std::min<size_t>((total + 255) / 256, 132 * 16);
     return dispatch_dtype(
         dtype,
         [&] { (void)lg_launch(store_act_kernel<float>, dim3(blocks), dim3(256), 0, st, partial, ksplit, total, gelu, (float*)out); LG_LAUNCH_CHECK(); return 0; },
@@ -423,7 +423,7 @@ int launch_store_act(const float* partial, int ksplit, int M, int N, void* out, 
 
 int launch_reduce_f32(const float* partial, int ksplit, int M, int N, float* out, cudaStream_t st) {
     const size_t total = (size_t)M * N;
-    const int blocks = (int)std::min<size_t>((total + 255) / 256, 148 * 16);
+    const int blocks = (int)std::min<size_t>((total + 255) / 256, 132 * 16);
     (void)lg_launch(reduce_f32_kernel, dim3(blocks), dim3(256), 0, st, partial, ksplit, total, out);
     LG_LAUNCH_CHECK();
     return 0;

@@ -3,7 +3,7 @@
 Only the *interface* lives here: a parameter container whose state_dict names/shapes equal the
 reference's (SURVEY §5: `layers.{i}.attention.wqkv.weight`, `cls_embedding.embedding_table.weight`, ...),
 the `GPT_models` registry (gpt.py:438-467) and the `ModelArgs` fields the inference path reads
-(gpt.py:23-50).  All compute is done by the sm_100a kernels behind the C-ABI engine
+(gpt.py:23-50).  All compute is done by the sm_90a kernels behind the C-ABI engine
 (include/llamagen_b200.h); there is no PyTorch forward and no CPU path.
 """
 from __future__ import annotations
@@ -169,7 +169,7 @@ class Transformer(nn.Module):
         p = self.tok_embeddings.weight
         _lib.require_cuda(p, "Transformer.engine")
         if p.dtype not in (torch.float32, torch.bfloat16):
-            raise _lib.LgError(f"unsupported precision {p.dtype}: the sm_100a engine implements bf16 and fp32")
+            raise _lib.LgError(f"unsupported precision {p.dtype}: the sm_90a engine implements bf16 and fp32")
         sig = self._signature()
         if self._engine is not None and sig == self._engine_sig:
             return self._engine

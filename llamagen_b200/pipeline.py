@@ -26,9 +26,8 @@ class SamplePipeline:
         self.decode_stream = torch.cuda.Stream(device=dev)
         self._last = None
         # While batch i is decoded the AR loop of batch i+1 is running. LG_PIPE_CONV_CTAS = N > 0 runs the decoder's convolutions as
-        # N persistent CTAs (a cap on the SMs they occupy); 0 = one CTA per tile (default). Measured on B200 (GPT-L, B = 64, DESIGN.md
-        # section 9): 0 -> 288.1 ms/step, 128 -> 290.6, 64 -> 300.4, 32 -> 317.5: the sampler loses more from a long-lived background
-        # decode than from a short full-machine burst, so the cap stays off; what does help is the sampler's stream priority.
+        # N persistent CTAs (a cap on the SMs they occupy); 0 = one CTA per tile (default): the sampler loses more from a long-lived
+        # background decode than from a short full-machine burst, so the cap stays off; what does help is the sampler's stream priority.
         self.conv_ctas = int(os.environ.get("LG_PIPE_CONV_CTAS", "0"))
 
     def submit(self, cond, grid: int, to_uint8_host=None, emb_masks=None):

@@ -1,5 +1,5 @@
 """`python -m llamagen_b200.sample.sample_c2i` — same flags and output file as
-autoregressive/sample/sample_c2i.py:101-123 (sample_{gpt_type}.png), executed by the sm_100a engine."""
+autoregressive/sample/sample_c2i.py:101-123 (sample_{gpt_type}.png), executed by the sm_90a engine."""
 import argparse
 import time
 
@@ -13,7 +13,7 @@ def main(args):
     torch.manual_seed(args.seed)
     torch.set_grad_enabled(False)
     if not torch.cuda.is_available():
-        raise SystemExit("llamagen_b200 has no CPU path: a CUDA (sm_100a) device is required")
+        raise SystemExit("llamagen_b200 has no CPU path: a CUDA (sm_90a) device is required")
     device = "cuda"
     vq_model = load_vq(args, device)
     latent_size = args.image_size // args.downsample_size

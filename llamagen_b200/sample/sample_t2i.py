@@ -37,7 +37,7 @@ def main(args):
     torch.manual_seed(args.seed)
     torch.set_grad_enabled(False)
     if not torch.cuda.is_available():
-        raise SystemExit("llamagen_b200 has no CPU path: a CUDA (sm_100a) device is required")
+        raise SystemExit("llamagen_b200 has no CPU path: a CUDA (sm_90a) device is required")
     device = "cuda"
     vq_model = load_vq(args, device)
     latent_size = args.image_size // args.downsample_size

@@ -36,7 +36,7 @@ def prompt_indices(n, rank, world, total):
 
 def main(args):
     if not torch.cuda.is_available():
-        raise SystemExit("llamagen_b200 has no CPU path: a CUDA (sm_100a) device is required")
+        raise SystemExit("llamagen_b200 has no CPU path: a CUDA (sm_90a) device is required")
     torch.set_grad_enabled(False)
     rank, world, local = lgd.init_from_env("nccl")
     device = torch.device("cuda", local)

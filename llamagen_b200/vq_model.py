@@ -2,7 +2,7 @@
 
 A parameter container with the reference's state_dict names/shapes (so `load_state_dict(ckpt["model"])`
 of a LlamaGen tokenizer checkpoint works unchanged, strict=True included), the `VQ_models` registry
-(vq_model.py:418-424) and `decode_code` (vq_model.py:52-55) executed by the sm_100a implicit-GEMM
+(vq_model.py:418-424) and `decode_code` (vq_model.py:52-55) executed by the sm_90a implicit-GEMM
 decoder behind the C-ABI (lg_vq_decode).  The encode-side argmin-L2 (vq_model.py:215-233) is exposed
 as `quantize_indices` (lg_vq_argmin).  The conv encoder itself is the next-tier row of SURVEY §8(f).
 """

@@ -1,6 +1,6 @@
-"""Generate golden vectors by RUNNING THE REFERENCE (imported from /root/reference) on tiny seeded models.
+"""Generate golden vectors by RUNNING THE REFERENCE (a LlamaGen checkout) on tiny seeded models.
 
-Run in the authoring container only:  python tests/golden/make_golden.py
+Run:  python tests/golden/make_golden.py <llamagen checkout>
 Outputs (committed, small):
   tests/golden/gpt_c2i.pt  gpt_t2i.pt   : state_dict + inputs + reference generate() greedy tokens and logits
   tests/golden/vq_tiny.pt               : state_dict + codes + reference decode_code pixels + argmin indices
@@ -13,7 +13,7 @@ import sys
 
 import torch
 
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, sys.argv[1])
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 from autoregressive.models.generate import generate, sample, top_k_top_p_filtering  # noqa: E402
@@ -113,6 +113,27 @@ def vq_enc_case(seed):
                 indices=info[2].clone())
 
 
+def save_golden(case, name, part_bytes=900 * 1024):
+    """torch.save `case` as HERE/name; a state_dict that would push the file past 1 MB goes to name.sd<i>.pt parts of at
+    most `part_bytes` tensor bytes each (tests/util.py:load_golden joins them)."""
+    stem = os.path.join(HERE, name[:-3])
+    sd = case.get("state_dict")
+    if sd is not None and sum(t.numel() * t.element_size() for t in sd.values()) > part_bytes:
+        parts, cur, size = [], {}, 0
+        for k, t in sd.items():
+            nb = t.numel() * t.element_size()
+            if cur and size + nb > part_bytes:
+                parts.append(cur)
+                cur, size = {}, 0
+            cur[k] = t
+            size += nb
+        parts.append(cur)
+        for i, part in enumerate(parts):
+            torch.save(part, f"{stem}.sd{i}.pt")
+        case = dict(case, state_dict=None, state_dict_parts=len(parts))
+    torch.save(case, stem + ".pt")
+
+
 def sampling_case(seed):
     torch.manual_seed(seed)
     V = 1024
@@ -128,11 +149,11 @@ def sampling_case(seed):
 
 
 if __name__ == "__main__":
-    torch.save(gpt_case("c2i", 0), os.path.join(HERE, "gpt_c2i.pt"))
-    torch.save(gpt_case("t2i", 1), os.path.join(HERE, "gpt_t2i.pt"))
-    torch.save(vq_case(2), os.path.join(HERE, "vq_tiny.pt"))
-    torch.save(sampling_case(3), os.path.join(HERE, "sampling.pt"))
-    torch.save(vq_enc_case(4), os.path.join(HERE, "vq_enc_tiny.pt"))
+    save_golden(gpt_case("c2i", 0), "gpt_c2i.pt")
+    save_golden(gpt_case("t2i", 1), "gpt_t2i.pt")
+    save_golden(vq_case(2), "vq_tiny.pt")
+    save_golden(sampling_case(3), "sampling.pt")
+    save_golden(vq_enc_case(4), "vq_enc_tiny.pt")
     for f in sorted(os.listdir(HERE)):
         if f.endswith(".pt"):
             print(f, os.path.getsize(os.path.join(HERE, f)) // 1024, "KiB")

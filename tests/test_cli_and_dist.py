@@ -13,16 +13,14 @@ import torch.multiprocessing as mp
 from conftest import ROOT
 
 
-def _ref_flags(path):
-    return set(re.findall(r'add_argument\(\s*"(--[a-z0-9\-]+)"', open(path).read()))
-
-
 @pytest.mark.parametrize("script", ["sample_c2i", "sample_t2i", "sample_c2i_ddp"])
-def test_cli_accepts_every_reference_flag(reference_path, script):
+def test_cli_accepts_every_reference_flag(script):
+    """Every flag the reference sampling scripts declare (recorded in tests/golden/reference_api.pt) is accepted."""
     import importlib
+    from util import load_golden
     mod = importlib.import_module(f"llamagen_b200.sample.{script}")
     ours = {a for act in mod.build_parser()._actions for a in act.option_strings}
-    ref = _ref_flags(os.path.join(reference_path, "autoregressive", "sample", f"{script}.py"))
+    ref = set(load_golden("reference_api.pt")["cli_flags"][script])
     assert ref <= ours, f"missing flags: {sorted(ref - ours)}"
 
 

@@ -19,7 +19,7 @@ SHAPES = [  # (M, N, K)
 @pytest.mark.parametrize("M,N,K", SHAPES)
 @pytest.mark.parametrize("path", ["mma", "tcgen05"])
 def test_gemm_bf16(M, N, K, path, monkeypatch):
-    """path=tcgen05 routes 8 < M <= 256 through the UMMA/TMEM/TMA kernel (gemm_tc.cu); other shapes fall back."""
+    """path=tcgen05 (test id kept stable; the kernel is wgmma + TMA) routes 8 < M <= 256 through gemm_tc.cu; other shapes fall back."""
     monkeypatch.setenv("LG_GEMM_TC", "1" if path == "tcgen05" else "0")
     torch.manual_seed(M * 7 + N + K)
     x = (torch.randn(M, K, device="cuda") * 0.5).bfloat16()

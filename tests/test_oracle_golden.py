@@ -1,16 +1,16 @@
 """CPU: the oracle restatement must reproduce the golden vectors the REFERENCE produced
-(tests/golden/make_golden.py). This is what pins the oracle on machines without /root/reference."""
+(tests/golden/make_golden.py). This is what pins the oracle without a reference checkout."""
 import os
 
 import pytest
 import torch
 
-from conftest import GOLDEN
+from util import load_golden
 from oracle import GPTOracle, VQOracle, sample_oracle, top_k_top_p_oracle
 
 
 def _load(name):
-    return torch.load(os.path.join(GOLDEN, name), map_location="cpu", weights_only=False)
+    return load_golden(name)
 
 
 @pytest.mark.parametrize("name", ["gpt_c2i.pt", "gpt_t2i.pt"])

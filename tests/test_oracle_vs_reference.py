@@ -1,105 +1,74 @@
-"""CPU, authoring container only: the oracle against the LIVE reference on fresh seeds (skipped on the GPU
-box, where /root/reference does not exist)."""
+"""CPU: the oracle against outputs of the reference LlamaGen code recorded in tests/golden/reference_api.pt
+(tests/golden/make_reference_api.py): greedy generate() tokens, the 2-D RoPE table, the model registries, VQ
+decode / encode of a tiny model, and the sample scripts' center crop."""
 import pytest
 import torch
 
 from oracle import GPTOracle, VQOracle, rope_table_2d_oracle
+from util import load_golden, seeded_state_dict
+
+
+@pytest.fixture(scope="module")
+def ref():
+    return load_golden("reference_api.pt")
 
 
 @pytest.mark.parametrize("model_type,cls", [("c2i", 1), ("t2i", 120)])
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
-def test_generate_matches_live_reference(reference_path, model_type, cls, dtype):
-    from autoregressive.models.generate import generate
-    from autoregressive.models.gpt import ModelArgs, Transformer
-    torch.manual_seed(11)
-    cfg = dict(n_layer=2, n_head=2, dim=128, vocab_size=256, block_size=16, cls_token_num=cls, model_type=model_type,
-               num_classes=7, caption_dim=64, norm_eps=1e-5, rope_base=10000)
-    m = Transformer(ModelArgs(**cfg)).eval()
-    m.output.weight.data.normal_(std=0.02)
-    m = m.to(dtype)
-    B = 2
-    if model_type == "c2i":
-        cond, em = torch.tensor([3, 6]), None
-    else:
-        em = torch.zeros(B, cls)
-        em[0, -5:] = 1
-        em[1, -77:] = 1
-        cond = (torch.randn(B, cls, 64) * em[:, :, None]).to(dtype)
-    ref = generate(m, cond, 16, emb_masks=em, cfg_scale=3.0, temperature=1.0, top_k=0, top_p=1.0, sample_logits=False)
-    toks, _ = GPTOracle(m.state_dict(), cfg).generate(cond, 16, emb_masks=em, cfg_scale=3.0, sample_logits=False)
-    assert torch.equal(ref, toks)
+def test_generate_matches_live_reference(ref, model_type, cls, dtype):
+    case = ref["generate"][f"{model_type}_{str(dtype)[6:]}"]
+    assert case["cfg"]["cls_token_num"] == cls
+    sd = {k: v.to(dtype) for k, v in seeded_state_dict(case["shapes"], case["seed"]).items()}
+    toks, _ = GPTOracle(sd, case["cfg"]).generate(case["cond"], 16, emb_masks=case["emb_masks"], cfg_scale=3.0, sample_logits=False)
+    assert torch.equal(case["tokens"], toks)
 
 
-def test_rope_table_matches_live_reference(reference_path):
-    from autoregressive.models.gpt import precompute_freqs_cis_2d
+def test_rope_table_matches_live_reference(ref):
     from llamagen_b200.gpt import rope_table_2d
-    for grid, hd, cls in ((16, 64, 1), (24, 100, 1), (32, 64, 120)):
-        ref = precompute_freqs_cis_2d(grid, hd, 10000, cls)
-        assert torch.equal(ref, rope_table_2d_oracle(grid, hd, 10000, cls))
-        assert torch.equal(ref, rope_table_2d(grid, hd, 10000, cls))
+    for (grid, hd, cls), table in ref["rope"].items():
+        assert torch.equal(table, rope_table_2d_oracle(grid, hd, 10000, cls))
+        assert torch.equal(table, rope_table_2d(grid, hd, 10000, cls))
 
 
-def test_registry_matches_live_reference(reference_path):
+def test_registry_matches_live_reference(ref):
     """Same keys, same parameter names and shapes as the reference registries (drop-in boundary §8b)."""
-    from autoregressive.models.gpt import GPT_models as RefGPT
     from llamagen_b200 import GPT_models
-    assert set(RefGPT) == set(GPT_models)
+    assert set(ref["gpt_names"]) == set(GPT_models)
     for kw in (dict(model_type="c2i", cls_token_num=1, block_size=256), dict(model_type="t2i", cls_token_num=120, block_size=256)):
-        a = RefGPT["GPT-B"](**kw).state_dict()
         b = GPT_models["GPT-B"](**kw).state_dict()
-        assert {k: tuple(v.shape) for k, v in a.items()} == {k: tuple(v.shape) for k, v in b.items()}
+        assert ref["gpt_registry"][kw["model_type"]] == {k: tuple(v.shape) for k, v in b.items()}
 
 
-def test_vq_registry_matches_live_reference(reference_path):
-    from tokenizer.tokenizer_image.vq_model import VQ_models as RefVQ
+def test_vq_registry_matches_live_reference(ref):
     from llamagen_b200 import VQ_models
-    assert set(RefVQ) == set(VQ_models)
-    for name in RefVQ:
-        a = RefVQ[name](codebook_size=16384, codebook_embed_dim=8).state_dict()
+    assert set(ref["vq_registry"]) == set(VQ_models)
+    for name, shapes in ref["vq_registry"].items():
         b = VQ_models[name](codebook_size=16384, codebook_embed_dim=8).state_dict()
-        assert {k: tuple(v.shape) for k, v in a.items()} == {k: tuple(v.shape) for k, v in b.items()}
+        assert shapes == {k: tuple(v.shape) for k, v in b.items()}
 
 
-def test_vq_decode_matches_live_reference(reference_path):
-    import torch.nn as nn
-    from tokenizer.tokenizer_image.vq_model import Decoder, VectorQuantizer
-    torch.manual_seed(5)
-    dec = Decoder(z_channels=32, ch=32, ch_mult=(1, 2, 2)).eval()
-    quant = VectorQuantizer(128, 8, 0.25, 0.0, True, True).eval()
-    pqc = nn.Conv2d(8, 32, 1).eval()
-    sd = {"decoder." + k: v for k, v in dec.state_dict().items()}
-    sd.update({"quantize.embedding.weight": quant.embedding.weight.data, "post_quant_conv.weight": pqc.weight.data,
-               "post_quant_conv.bias": pqc.bias.data})
-    codes = torch.randint(0, 128, (1, 9))
-    with torch.no_grad():
-        ref = dec(pqc(quant.get_codebook_entry(codes, [1, 8, 3, 3], True)))
-    assert torch.equal(ref, VQOracle(sd, ch_mult=(1, 2, 2)).decode_code(codes, [1, 8, 3, 3]))
+def test_vq_decode_matches_live_reference(ref):
+    case = ref["vq_decode"]
+    sd = seeded_state_dict(case["shapes"], case["seed"], fan_in=True)
+    assert torch.equal(case["pixels"], VQOracle(sd, ch_mult=(1, 2, 2)).decode_code(case["codes"], [1, 8, 3, 3]))
 
 
-def test_vq_encode_matches_live_reference(reference_path):
-    import torch.nn as nn
-    from tokenizer.tokenizer_image.vq_model import Encoder, VectorQuantizer
-    torch.manual_seed(6)
-    enc = Encoder(ch=32, ch_mult=(1, 2, 2), z_channels=32).eval()
-    quant = VectorQuantizer(128, 8, 0.25, 0.0, True, True).eval()
-    qc = nn.Conv2d(32, 8, 1).eval()
-    sd = {"encoder." + k: v for k, v in enc.state_dict().items()}
-    sd.update({"quantize.embedding.weight": quant.embedding.weight.data, "quant_conv.weight": qc.weight.data,
-               "quant_conv.bias": qc.bias.data})
-    x = torch.rand(1, 3, 24, 16) * 2 - 1
-    with torch.no_grad():
-        zq, _, info = quant(qc(enc(x)))
-    q, idx = VQOracle(sd, ch_mult=(1, 2, 2)).encode(x)
-    assert torch.equal(idx, info[2]) and torch.equal(q, zq)
+def test_vq_encode_matches_live_reference(ref):
+    case = ref["vq_encode"]
+    sd = seeded_state_dict(case["shapes"], case["seed"], fan_in=True)
+    q, idx = VQOracle(sd, ch_mult=(1, 2, 2)).encode(case["x"])
+    assert torch.equal(idx, case["indices"]) and torch.equal(q, case["quant"])
 
 
-def test_center_crop_matches_live_reference(reference_path):
+def test_center_crop_matches_live_reference(ref):
+    import hashlib
+
     import numpy as np
     from PIL import Image
-    from dataset.augmentation import center_crop_arr
     from llamagen_b200.sample.vq_demo import center_crop
     rng = np.random.default_rng(1)
     for shape in [(300, 420), (1100, 900), (256, 256), (513, 2000)]:
         im = Image.fromarray(rng.integers(0, 255, (*shape, 3), dtype=np.uint8))
         for s in (256, 384):
-            assert (np.array(center_crop(im, s)) == np.array(center_crop_arr(im, s))).all()
+            a = np.array(center_crop(im, s))
+            assert (a.shape, hashlib.sha256(a.tobytes()).hexdigest()) == ref["center_crop"][(shape, s)]

@@ -2,7 +2,7 @@
 
 Every test runs the bf16 engine teacher-forced on the fp32 oracle's greedy stream and compares the CFG-mixed logits of
 EVERY step with (a) the fp32 oracle on the same bf16-rounded weights and (b) the bf16 oracle (like for like). The oracle
-(oracle/gpt_oracle.py, pinned to the live reference) takes device tensors, so it runs on the same B200 in plain torch
+(oracle/gpt_oracle.py, pinned to the live reference) takes device tensors, so it runs on the same GPU in plain torch
 (fp32 matmuls with TF32 off) — a CPU run of GPT-L at R=128 for 256 steps would take minutes per case.
 
 Bound (same protocol as tests/test_gpt_gpu.py::_bf16_parity): the engine may deviate from either oracle by at most
@@ -12,7 +12,7 @@ the bounds (pytest -s) and appended to gpurun_out/parity_report.jsonl so a regre
 
     C2  GPT-L  c2i 16x16, B=64 (R=128, two decode chains), all 256 tokens      <- the benchmarked configuration
     C2' GPT-L  c2i 16x16, B=32 (R=64), all 256 tokens                          <- north_star's per-GPU point (B=256 / 8 GPUs)
-    C3  GPT-XL c2i 24x24, contexts to 577 keys, R=4 (small-row path) and R=16 (tcgen05 path)
+    C3  GPT-XL c2i 24x24, contexts to 577 keys, R=4 (small-row path) and R=16 (wgmma path)
     C5  GPT-XL t2i 32x32, T=120 prefill with ragged emb_masks + 1024 tokens (context 1144), R=4 and R=16
     C4  GPT-3B (head_dim 100) full depth, R=32, 40 tokens
 """
@@ -105,7 +105,7 @@ def test_c2_gpt_l_bench_config_full_sequence(B):
 @pytest.mark.parametrize("B", [2, 8])
 def test_c3_gpt_xl_c2i_24x24(B):
     """BASELINE configs[2] shape: GPT-XL c2i 24x24 = 576 tokens (contexts to 577 keys). B=2 -> R=4 (small-row path),
-    B=8 -> R=16 (tcgen05 GEMMs + TMA attention)."""
+    B=8 -> R=16 (wgmma GEMMs + TMA attention)."""
     m = _registry("GPT-XL", 2, block_size=576, vocab_size=16384)
     torch.manual_seed(10 + B)
     parity_on_device(f"C3 GPT-XL c2i S=576 B={B}", m, torch.randint(0, 1000, (B,)), 576)

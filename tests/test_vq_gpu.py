@@ -1,6 +1,6 @@
 """GPU parity of the VQ decode path (lg_vq_decode) and the codebook argmin (lg_vq_argmin).
 
-Tolerance (stated, SURVEY §8c): the sm_100a decoder feeds bf16 operands to the tensor cores with fp32
+Tolerance (stated, SURVEY §8c): the sm_90a decoder feeds bf16 operands to the tensor cores with fp32
 accumulation and keeps activations in bf16; the oracle's own bf16-vs-fp32 spread on this decoder is
 max-abs 0.146 / mean-abs 0.010 at output std 0.39, so we require max-abs <= 0.2 and mean-abs <= 0.02
 against the fp32 oracle, and <= 1 LSB mean error after the uint8 conversion of sample_c2i_ddp.py:143."""
@@ -49,7 +49,7 @@ def test_tiny_argmin_matches_reference_golden():
 @pytest.mark.parametrize("conv", ["tcgen05", "mma"])
 @pytest.mark.parametrize("name,g,B", [("VQ-16", 16, 3), ("VQ-16", 24, 1), ("VQ-8", 16, 2)])
 def test_full_decoder_vs_oracle(name, g, B, conv, monkeypatch):
-    """conv=tcgen05: TMA 4-D box + UMMA/TMEM implicit GEMM (conv_tc.cu, incl. the 2x2 phase form of upsample+conv and
+    """conv=tcgen05 (test id kept stable): TMA 4-D box + wgmma implicit GEMM (conv_tc.cu, incl. the 2x2 phase form of upsample+conv and
     24x24 grids whose 8x16 patches overhang the image); conv=mma: the mma.sync + cp.async gather path."""
     monkeypatch.setenv("LG_CONV_TC", "1" if conv == "tcgen05" else "0")
     from llamagen_b200 import VQ_models
@@ -65,8 +65,8 @@ def test_full_decoder_vs_oracle(name, g, B, conv, monkeypatch):
 
 @pytest.mark.parametrize("variant", ["n128_tiles", "persistent_8_ctas", "no_gn_fuse", "cta_budget_api"])
 def test_conv_kernel_variants_agree(variant, monkeypatch):
-    """The shipped decoder = weights-as-A convs (UMMA N = 256, conv_tcw_kernel) with the GroupNorm statistics in their drain. It must
-    agree with: the pixels-as-A kernel (N <= 128), the same kernels looping as 8 persistent CTAs (many tiles per CTA: ring / TMEM
+    """The shipped decoder = weights-as-A convs (wgmma N = 256, conv_tcw_kernel) with the GroupNorm statistics in their drain. It must
+    agree with: the pixels-as-A kernel (N <= 128), the same kernels looping as 8 persistent CTAs (many tiles per CTA: ring / accumulator
     phases carried across tiles), the stand-alone statistics pass, and the C-ABI CTA budget. Same bf16 rounding points everywhere;
     only fp32 summation orders differ."""
     from llamagen_b200 import VQ_models, _lib

@@ -7,7 +7,15 @@ from conftest import GOLDEN
 
 
 def load_golden(name):
-    return torch.load(os.path.join(GOLDEN, name), map_location="cpu", weights_only=False)
+    """A golden case; a state_dict stored as name.sd<i>.pt parts (files stay under 1 MB) is joined back in key order."""
+    case = torch.load(os.path.join(GOLDEN, name), map_location="cpu", weights_only=False)
+    n = case.pop("state_dict_parts", 0) if isinstance(case, dict) else 0
+    if n:
+        sd = {}
+        for i in range(n):
+            sd.update(torch.load(os.path.join(GOLDEN, f"{name[:-3]}.sd{i}.pt"), map_location="cpu", weights_only=False))
+        case["state_dict"] = sd
+    return case
 
 
 def build_gpt(cfg: dict, state_dict, dtype, device="cuda"):
@@ -64,4 +72,20 @@ def gemm_dx(x, wa, wb=None, mode=0, normw=None, eps=1e-5, h=None):
     _lib.check(lib.lg_test_gemm_dx(_lib.ptr(x), _lib.ptr(wa), _lib.ptr(wb) if wb is not None else None, M, N, K, mode,
                                    _lib.ptr(normw) if normw is not None else None, ctypes.c_float(eps), _lib.ptr(out),
                                    _lib.current_stream(x.device)), "lg_test_gemm_dx")
+    return out
+
+
+def seeded_state_dict(shapes: dict, seed: int, fan_in: bool = False) -> dict:
+    """Deterministic weights for a parameter layout {name: shape}: N(0, 0.02) for matrices (N(0, 1 / fan_in) with
+    `fan_in`, which keeps conv activations at unit scale), 1 + N(0, 0.02) for vectors (norm weights, biases). The golden
+    cases built by tests/golden/make_reference_api.py load these into the reference model, so a test can rebuild the
+    same model without it."""
+    g = torch.Generator().manual_seed(seed)
+    out = {}
+    for k in sorted(shapes):
+        t = torch.randn(tuple(shapes[k]), generator=g)
+        if t.dim() == 1:
+            out[k] = 1.0 + 0.02 * t
+        else:
+            out[k] = t / (t[0].numel() ** 0.5) if fan_in else 0.02 * t
     return out

@@ -75,8 +75,9 @@ def main():
         peaks = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm = float(peaks.get("hbm_gbs", peaks.get("hbm_GBps", 6569.6))) if isinstance(peaks, dict) else 6569.6
-    tf = float(peaks.get("bf16_tflops_sustained", 1412.5)) if isinstance(peaks, dict) else 1412.5
+    # fallback: H100 SXM data sheet (3.35 TB/s HBM3, 989 TFLOP/s dense bf16 at 700 W), not rates measured here
+    hbm = float(peaks.get("hbm_gbs", peaks.get("hbm_GBps", 3350.0))) if isinstance(peaks, dict) else 3350.0
+    tf = float(peaks.get("bf16_tflops_sustained", 989.0)) if isinstance(peaks, dict) else 989.0
     torch.manual_seed(0)
     m = VQ_models["VQ-16"](codebook_size=16384, codebook_embed_dim=8).cuda().eval()
     B, S = args.batch, args.size

@@ -1,4 +1,4 @@
-"""Phase timing of the tcgen05 GEMM (debug %globaltimer stamps) for the decode shapes at R rows."""
+"""Phase timing of the wgmma GEMM (debug %globaltimer stamps) for the decode shapes at R rows."""
 import ctypes, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))

@@ -1,11 +1,11 @@
-"""Count Blackwell / tensor / async-copy SASS mnemonics per kernel of the built library (CPU-only evidence of what the
-kernels are made of).  Usage: cuobjdump -sass llamagen_b200/lib/libllamagen_b200.so | python tools/sass_summary.py > profiles/..."""
+"""Count Hopper tensor / async-copy SASS mnemonics per kernel of the built library (CPU-only evidence of what the
+kernels are made of).  Usage: cuobjdump -sass llamagen_b200/lib/libllamagen_b200.so | python tools/sass_summary.py"""
 import collections
 import re
 import subprocess
 import sys
 
-KEYS = ("UTCHMMA", "UTMALDG", "UBLKPF", "UTCBAR", "LDTM", "HMMA", "LDSM", "LDGSTS", "SYNCS", "ELECT", "ATOMS", "ATOMG", "ATOM.", "RED.", "REDUX")
+KEYS = ("HGMMA", "UTMALDG", "UBLKPF", "HMMA", "LDSM", "LDGSTS", "SYNCS", "ELECT", "ATOMS", "ATOMG", "ATOM.", "RED.", "REDUX")
 counts = collections.defaultdict(collections.Counter)
 cur = None
 for line in sys.stdin:
@@ -31,8 +31,8 @@ def demangle(n):
 
 
 print("# cuobjdump -sass of the in-tree library: occurrences of selected mnemonics per kernel")
-print("# UTCHMMA = tcgen05.mma   UTMALDG = TMA tensor load   UBLKPF = cp.async.bulk.prefetch.L2   LDTM = tcgen05.ld   UTCBAR = tcgen05.commit")
-print("# HMMA = mma.sync   LDSM = ldmatrix   LDGSTS = cp.async   SYNCS = mbarrier ops   ATOMS = shared-memory atomics (TMEM allocator,")
+print("# HGMMA = wgmma   UTMALDG = TMA tensor load   UBLKPF = cp.async.bulk.prefetch.L2")
+print("# HMMA = mma.sync   LDSM = ldmatrix   LDGSTS = cp.async   SYNCS = mbarrier ops   ATOMS = shared-memory atomics (")
 print("# integer histogram counters of the sampler)   ATOMG / ATOM. / RED. = global atomics: only integer control counters (grid barrier of decode_small_persistent_kernel, arrival ticket of sample_kernel's fused tail); no float atomics, none on a data path")
 rows = sorted((demangle(fn), dict(c)) for fn, c in counts.items() if c)
 for d, c in rows:

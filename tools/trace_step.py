@@ -1,5 +1,5 @@
 """Kernel timeline of one bench step via torch.profiler (CUPTI): per-kernel totals and the idle gaps between
-kernels inside the CUDA-graph replay.  Usage: python tools/trace_step.py [--batch 64] [--out profiles/trace.json]"""
+kernels inside the CUDA-graph replay.  Usage: python tools/trace_step.py [--batch 64] [--out trace.json]"""
 import argparse, collections, json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
