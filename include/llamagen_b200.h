@@ -192,6 +192,25 @@ int  lg_test_gemm(const void* x, const void* w, int M, int N, int K, int dtype, 
 int  lg_test_gemm_dx(const void* x, const void* wa, const void* wb, int M, int N, int K, int mode, const void* normw,
                      float eps, void* out, void* stream);
 
+/* One VQ decoder/encoder convolution through the decoder's own dispatch (the mma.sync gather kernel or either wgmma kernel,
+ * honouring LG_CONV_TC, LG_CONV_SWAP, LG_GN_FUSE and the CTA budget), optionally followed by GroupNorm(32, eps 1e-6)
+ * [+ swish] of its output the way a ResnetBlock hands one to the other (statistics taken from the conv's drain when it wrote them).
+ * x bf16 NHWC [B,Hin,Win,Cin]; w f32 [Cout][Cin][k][k] (checkpoint layout, repacked here like lg_vq_finalize), bias f32 [Cout].
+ * up: 0 = same size, 1 = nearest-2x upsample folded in (k = 3), 2 = Downsample (k = 3, stride 2 over the input zero-padded
+ * right/bottom by one). residual: bf16 NHWC or NULL, may alias out_bf. Exactly one output: out_bf (bf16 NHWC), out_nchw (f32 NCHW)
+ * or out_u8 (clamp(127.5*y + 128, 0, 255) as uint8 NHWC). gn_gamma / gn_beta: f32 [Cout] or NULL; gn_out: bf16 NHWC.
+ * *path: 0 = mma.sync gather kernel, 1 = conv_tc_kernel, 2 = conv_tcw_kernel. *gn_splits: splits of the GroupNorm partial
+ * statistics the conv's drain wrote (0: none), copied to gn_partial [B][splits][32][2] (sum, sum of squares) when non-NULL.
+ * Scratch: 256-byte aligned; the call fails with the size it needs when it is too small. */
+int  lg_test_vq_conv(const void* x, int B, int Hin, int Win, int Cin, const float* w, const float* bias, int Cout, int ksize, int up,
+                     const void* residual, void* out_bf, float* out_nchw, uint8_t* out_u8, const float* gn_gamma,
+                     const float* gn_beta, int gn_swish, void* gn_out, float* gn_partial, size_t gn_partial_floats,
+                     void* dev_scratch, size_t scratch_bytes, int* path, int* gn_splits, void* stream);
+/* The stand-alone GroupNorm(32, eps 1e-6) [+ swish] of the VQ models (statistics pass + apply pass): x, y bf16 NHWC [B,HW,C],
+ * gamma / beta f32 [C]. Scratch: at least B * 64 * 64 floats. */
+int  lg_test_group_norm(const void* x, int B, int HW, int C, const float* gamma, const float* beta, int swish, void* y,
+                        void* dev_scratch, size_t scratch_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -81,6 +81,11 @@ SIGNATURES = {
                              c_void_p]),
     "lg_test_gemm_dx": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_float, c_void_p,
                                 c_void_p]),
+    "lg_test_vq_conv": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
+                                c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_size_t,
+                                c_void_p, c_size_t, POINTER(c_int), POINTER(c_int), c_void_p]),
+    "lg_test_group_norm": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_size_t,
+                                   c_void_p]),
 }
 
 _lib = None

@@ -412,8 +412,9 @@ static int launch_conv_tc_t(const CUtensorMap& amap, const CUtensorMap& wmap, co
 // weights: up == 0 or 2 (stride-2 Downsample) -> [Cout][k*k][Cin] bf16 ; up == 1 -> phase weights [4][Cout][4][Cin] bf16
 int launch_conv_tc(const bf16* in, int B, int Hin, int Win, int Cin, const bf16* weights, const float* bias, int Cout,
                    int ksize, int up, const bf16* residual, bf16* out_bf, float* out_nchw, cudaStream_t st, uint8_t* out_u8,
-                   float* gn_partial, size_t gn_floats, int* gn_splits) {
+                   float* gn_partial, size_t gn_floats, int* gn_splits, int* path) {
     if (gn_splits) *gn_splits = 0;
+    if (path) *path = 1;
     ConvTcArgs a;
     a.gn_partial = nullptr; a.gn_cpg = 0; a.gn_splits = 0;
     a.B = B; a.Hin = Hin; a.Win = Win; a.Cin = Cin; a.Cout = Cout;
@@ -470,6 +471,7 @@ int launch_conv_tc(const bf16* in, int B, int Hin, int Win, int Cin, const bf16*
         dim3 grid2((unsigned)(budget > 0 ? std::min<long long>(total2, budget) : total2));
         conv_tcw_kernel<<<grid2, kConvThreads, smem2, st>>>(amap2, wmap2, w);
         LG_LAUNCH_CHECK();
+        if (path) *path = 2;
         return 0;
     }
     a.gx = B * a.tiles_x * a.tiles_y; a.gy = cdiv(Cout, a.bn); a.gz = up ? 4 : 1;

@@ -144,8 +144,9 @@ void conv_tc_set_cta_budget(int ctas);   // > 0: persistent conv CTAs (at most `
 int conv_tc_make_phase_weights(const float* w_f32, bf16* out, int cout, int cin, cudaStream_t st);
 int launch_conv_tc(const bf16* in, int B, int Hin, int Win, int Cin, const bf16* weights, const float* bias, int Cout,
                    int ksize, int up, const bf16* residual, bf16* out_bf, float* out_nchw, cudaStream_t st, uint8_t* out_u8 = nullptr,
-                   float* gn_partial = nullptr, size_t gn_floats = 0, int* gn_splits = nullptr);   // *gn_splits > 0: the drain also wrote the
-                   // output's GroupNorm(32) partial statistics [B][*gn_splits][32][2] into gn_partial
+                   float* gn_partial = nullptr, size_t gn_floats = 0, int* gn_splits = nullptr,    // *gn_splits > 0: the drain also wrote the
+                   int* path = nullptr);   // output's GroupNorm(32) partial statistics [B][*gn_splits][32][2] into gn_partial;
+                                           // *path: 1 = conv_tc_kernel, 2 = conv_tcw_kernel was launched
 // gemm_tc.cu — wgmma/TMA weight-streaming GEMM (bf16, row blocks of <= 256)
 int gemm_tc_ksplit(int M, int N, int K);
 bool gemm_tc_supported(int M, int N, int K, int dtype);

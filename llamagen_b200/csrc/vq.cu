@@ -161,9 +161,10 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const bf16* __restrict__ 
 __global__ void __launch_bounds__(256) gn_apply_kernel(const bf16* __restrict__ x, const float* __restrict__ partial, int splits,
                                                        const float* __restrict__ gamma, const float* __restrict__ beta,
                                                        bf16* __restrict__ y, int HW, int C, int swish) {
-    __shared__ float mean[32], rstd[32];
+    __shared__ float mean[32], rstd[32], var_s[32];
     __shared__ float red[8][32][2];
     const int b = blockIdx.y;
+    const size_t img = (size_t)b * HW * C;
     {   // combine the per-split partials: 8 interleaved subsets in parallel, then a fixed-order sum (deterministic)
         const int g = threadIdx.x & 31, sub = threadIdx.x >> 5;
         float gs = 0.f, gq = 0.f;
@@ -184,15 +185,41 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const bf16* __restrict__ 
         const float mu = gs / cnt;
         const float var = fmaxf(gq / cnt - mu * mu, 0.f);
         mean[threadIdx.x] = mu;
+        var_s[threadIdx.x] = var;
         rstd[threadIdx.x] = 1.0f / sqrtf(var + 1e-6f);
     }
     __syncthreads();
+    // E[x^2] - mean^2 from fp32 sums cancels catastrophically once |mean| >> std (at |mean| / std = 100 the variance is off by
+    // several percent). Such groups are recomputed here by a corrected two-pass sum around the first-pass mean over the whole
+    // image: every block of the image does the same arithmetic, so the result stays deterministic, and well-conditioned groups keep
+    // the one-pass statistics untouched.
+    const int cpg = C / 32;
+    for (int g = 0; g < 32; ++g) {
+        const float mu0 = mean[g];
+        if (!(mu0 * mu0 > 64.f * var_s[g])) continue;                 // |mean| / std <= 8: the one-pass variance is accurate
+        const int n = HW * cpg;
+        float s1 = 0.f, s2 = 0.f;
+        for (int i = threadIdx.x; i < n; i += 256) {
+            const int p = i / cpg;
+            const float d = __bfloat162float(x[img + (size_t)p * C + g * cpg + (i - p * cpg)]) - mu0;
+            s1 += d;
+            s2 = fmaf(d, d, s2);
+        }
+        s1 = block_sum(s1, &red[0][0][0]);
+        s2 = block_sum(s2, &red[0][0][0]);
+        if (threadIdx.x == 0) {
+            const float dm = s1 / (float)n;
+            mean[g] = mu0 + dm;
+            rstd[g] = 1.0f / sqrtf(fmaxf(s2 / (float)n - dm * dm, 0.f) + 1e-6f);
+        }
+        __syncthreads();
+    }
     // Each thread owns one 8-channel column for the whole kernel: 256 threads step over the image in multiples of
     // C/8 vectors, so the per-channel scale/shift (rstd*gamma, beta - mean*rstd*gamma) is computed ONCE and the
     // inner loop is one FMA + swish per element (the first version recomputed channel/group indices with integer
     // divisions per element and ran at 19 % of HBM bandwidth).
     const int vpp = C / 8;                               // vectors per pixel; divides 256 (checked on the host)
-    const int vec_per_img = HW * vpp, cpg = C / 32;
+    const int vec_per_img = HW * vpp;
     int per = (vec_per_img + gridDim.x - 1) / gridDim.x;
     per = (per + 255) / 256 * 256;                       // keep every block's start a multiple of 256 (hence of vpp)
     const int v0 = blockIdx.x * per, v1 = min(vec_per_img, v0 + per);
@@ -204,7 +231,6 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const bf16* __restrict__ 
         sa[j] = rstd[g] * gamma[c];
         sb[j] = beta[c] - mean[g] * sa[j];
     }
-    const size_t img = (size_t)b * HW * C;
 #pragma unroll 4
     for (int i = v0 + threadIdx.x; i < v1; i += 256) {
         float v[8];
@@ -652,18 +678,21 @@ int chunk_images(const lg_vq* v, int B, int g) {
 
 // ---- layer launchers --------------------------------------------------------------------------------
 // up: 0 = same resolution, 1 = nearest-2x upsample folded in, 2 = Downsample (pad right/bottom, stride 2)
+// *path (optional): 0 = mma.sync gather kernel, 1 = conv_tc_kernel, 2 = conv_tcw_kernel
 int run_conv(const ConvW& cw, const bf16* in, int B, int Hin, int Win, int up, const bf16* residual, bf16* out_bf,
-             float* out_nchw, cudaStream_t st, uint8_t* out_u8 = nullptr, VqWs* ws = nullptr) {
+             float* out_nchw, cudaStream_t st, uint8_t* out_u8 = nullptr, VqWs* ws = nullptr, int* path = nullptr) {
     if (ws && out_bf && ws->gn_src == out_bf) ws->gn_src = nullptr;          // the tensor the statistics described is being overwritten
     if (lg_env_flag("LG_CONV_TC", 1) && conv_tc_supported(Hin, Win, cw.cin, cw.cout, cw.k, up, out_nchw != nullptr || out_u8 != nullptr) &&
         (up != 1 || cw.w_phase)) {
         int splits = 0;
         LG_PROF(PC_VQ_CONV, st, launch_conv_tc(in, B, Hin, Win, cw.cin, up == 1 ? cw.w_phase : cw.w, cw.bias, cw.cout, cw.k, up, residual,
-                                               out_bf, out_nchw, st, out_u8, ws ? ws->gn : nullptr, ws ? ws->gn_floats : 0, ws ? &splits : nullptr));
+                                               out_bf, out_nchw, st, out_u8, ws ? ws->gn : nullptr, ws ? ws->gn_floats : 0, ws ? &splits : nullptr,
+                                               path));
         if (ws && splits > 0) { ws->gn_src = out_bf; ws->gn_splits = splits; }
         return 0;
     }
     LG_REQUIRE(!out_u8, "uint8 output needs the wgmma conv path (Cin %% 64 == 0, LG_CONV_TC=1)");
+    if (path) *path = 0;
     const int Hout = up == 1 ? 2 * Hin : (up == 2 ? Hin / 2 : Hin), Wout = up == 1 ? 2 * Win : (up == 2 ? Win / 2 : Win);
     const int M = B * Hout * Wout, K = cw.k * cw.k * cw.cin;
     mma::ConvA al{in, Hin, Win, cw.cin, Hout, Wout, cw.k, up, M};
@@ -1028,6 +1057,65 @@ int lg_pixels_to_u8(const float* in_nchw, int B, int C, int H, int W, int out_h,
     else pixels_to_u8_kernel<1><<<(unsigned)cdiv(n, 256), 256, 0, st>>>(in_nchw, B, C, H, W, out_h, out_w, out_nhwc);
     LG_LAUNCH_CHECK();
     return 0;
+}
+
+int lg_test_vq_conv(const void* x, int B, int Hin, int Win, int Cin, const float* w, const float* bias, int Cout, int ksize, int up,
+                    const void* residual, void* out_bf, float* out_nchw, uint8_t* out_u8, const float* gn_gamma, const float* gn_beta,
+                    int gn_swish, void* gn_out, float* gn_partial, size_t gn_partial_floats, void* dev_scratch, size_t scratch_bytes,
+                    int* path, int* gn_splits, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    LG_REQUIRE(x && w && bias && dev_scratch && path && gn_splits && B > 0 && Hin > 0 && Win > 0 && Cout > 0,
+               "lg_test_vq_conv: bad argument");
+    LG_REQUIRE((out_bf != nullptr) + (out_nchw != nullptr) + (out_u8 != nullptr) == 1, "lg_test_vq_conv: exactly one output");
+    LG_REQUIRE(ksize == 3 || (ksize == 1 && up == 0), "lg_test_vq_conv: ksize %d with up %d", ksize, up);
+    LG_REQUIRE(up >= 0 && up <= 2 && (up != 2 || (Hin % 2 == 0 && Win % 2 == 0)), "lg_test_vq_conv: bad up %d for %dx%d", up, Hin, Win);
+    LG_REQUIRE(Cin % 8 == 0, "lg_test_vq_conv: Cin=%d must be a multiple of 8", Cin);
+    LG_REQUIRE(((uintptr_t)dev_scratch & 255) == 0, "lg_test_vq_conv: scratch must be 256-byte aligned");
+    const bool gn = gn_gamma != nullptr;
+    LG_REQUIRE(!gn || (gn_beta && gn_out && out_bf && Cout % 32 == 0 && Cout <= 512 && 256 % (Cout / 8) == 0),
+               "lg_test_vq_conv: GroupNorm needs gamma, beta, gn_out, a bf16 output and a supported channel count (%d)", Cout);
+    const int Hout = up == 1 ? 2 * Hin : (up == 2 ? Hin / 2 : Hin), Wout = up == 1 ? 2 * Win : (up == 2 ? Win / 2 : Win);
+    // scratch: repacked weights, phase weights, GroupNorm partials (64 stand-alone splits or one per 16x16 tile and phase)
+    const bool phase = up == 1 && Cin % 64 == 0;
+    const size_t wq_bytes = a256((size_t)Cout * Cin * ksize * ksize * sizeof(bf16));
+    const size_t wp_bytes = phase ? a256((size_t)16 * Cout * Cin * sizeof(bf16)) : 0;
+    const size_t gn_floats = (size_t)B * std::max(64, cdiv(Hin, 16) * cdiv(Win, 16) * 4) * 64;
+    const size_t need = wq_bytes + wp_bytes + gn_floats * sizeof(float);
+    LG_REQUIRE(scratch_bytes >= need, "lg_test_vq_conv: scratch %zu < %zu", scratch_bytes, need);
+    char* s = (char*)dev_scratch;
+    ConvW cw;
+    cw.w = (bf16*)s; cw.bias = bias; cw.cout = Cout; cw.cin = Cin; cw.k = ksize;
+    repack_conv_kernel<<<132 * 4, 256, 0, st>>>(w, cw.w, Cout, Cin, ksize * ksize);
+    LG_LAUNCH_CHECK();
+    if (phase) {
+        cw.w_phase = (bf16*)(s + wq_bytes);
+        LG_TRY(conv_tc_make_phase_weights(w, cw.w_phase, Cout, Cin, st));
+    }
+    VqWs ws{};
+    ws.gn = (float*)(s + wq_bytes + wp_bytes);
+    ws.gn_floats = gn_floats;
+    LG_TRY(run_conv(cw, (const bf16*)x, B, Hin, Win, up, (const bf16*)residual, (bf16*)out_bf, out_nchw, st, out_u8, &ws, path));
+    *gn_splits = ws.gn_src == out_bf && out_bf ? ws.gn_splits : 0;
+    if (gn_partial && *gn_splits > 0) {
+        const size_t n = (size_t)B * *gn_splits * 64;
+        LG_REQUIRE(gn_partial_floats >= n, "lg_test_vq_conv: gn_partial %zu < %zu floats", gn_partial_floats, n);
+        LG_CUDA_OK(cudaMemcpyAsync(gn_partial, ws.gn, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    }
+    if (gn) {
+        const NormW nw{gn_gamma, gn_beta, Cout};
+        LG_TRY(run_gn(nw, (const bf16*)out_bf, (bf16*)gn_out, B, Hout * Wout, gn_swish, ws.gn, st, &ws));
+    }
+    return 0;
+}
+
+int lg_test_group_norm(const void* x, int B, int HW, int C, const float* gamma, const float* beta, int swish, void* y,
+                       void* dev_scratch, size_t scratch_bytes, void* stream) {
+    LG_REQUIRE(x && gamma && beta && y && dev_scratch && B > 0 && HW > 0, "lg_test_group_norm: bad argument");
+    LG_REQUIRE(C % 32 == 0 && C <= 512 && 256 % (C / 8) == 0, "lg_test_group_norm: unsupported channel count %d", C);
+    const size_t need = (size_t)B * 64 * 64 * sizeof(float);       // gn_stats_kernel: at most 64 splits x 32 groups x (sum, sum sq)
+    LG_REQUIRE(scratch_bytes >= need, "lg_test_group_norm: scratch %zu < %zu", scratch_bytes, need);
+    const NormW nw{gamma, beta, C};
+    return run_gn(nw, (const bf16*)x, (bf16*)y, B, HW, swish, (float*)dev_scratch, (cudaStream_t)stream);
 }
 
 }  // extern "C"
