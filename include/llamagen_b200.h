@@ -31,7 +31,8 @@ extern "C" {
 
 #define LG_ABI_VERSION 1
 
-enum { LG_DTYPE_F32 = 0, LG_DTYPE_BF16 = 1 };
+/* LG_DTYPE_F16 (IEEE half) runs the same tensor-core kernels as LG_DTYPE_BF16; values past +-65504 become +-inf, as in torch. */
+enum { LG_DTYPE_F32 = 0, LG_DTYPE_BF16 = 1, LG_DTYPE_F16 = 2 };
 enum { LG_MODEL_C2I = 0, LG_MODEL_T2I = 1 };
 
 /* Mirrors autoregressive/models/gpt.py:23-50 (ModelArgs) — only the fields the inference path reads. */
@@ -46,7 +47,7 @@ typedef struct lg_model_cfg {
     int32_t num_classes;   /* c2i null class index == num_classes (generate.py:130) */
     int32_t caption_dim;   /* t2i feature width (2048) */
     int32_t model_type;    /* LG_MODEL_* */
-    int32_t dtype;         /* LG_DTYPE_* of weights, activations and KV cache */
+    int32_t dtype;         /* LG_DTYPE_F32, _BF16 or _F16: weights, activations and KV cache */
     float   norm_eps;      /* RMSNorm eps, gpt.py:31 */
 } lg_model_cfg;
 
@@ -108,7 +109,8 @@ int  lg_sample_rows(const float* logits, int B, int V, int mix_cfg, int round_dt
 /* Fused CFG-mix + temperature + top-k + top-p + softmax + (argmax | multinomial): generate.py:57-66,95-97.
  * logits f32 [rows, V] (rows = 2B when mix_cfg, cond rows first); writes out_idx int32 [B] and, when
  * non-NULL, out_probs f32 [B, V] (the post-filter softmax the reference returns as `probs`).
- * round_dtype: LG_DTYPE_BF16 rounds raw logits to bf16 first (the reference's `.float()` of a bf16 head). */
+ * round_dtype: LG_DTYPE_BF16 / LG_DTYPE_F16 round raw logits to bf16 / fp16 first (the reference's `.float()` of a 16-bit head);
+ * LG_DTYPE_F32 uses them as they are. */
 int  lg_sample(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc,
                uint64_t step, int32_t* out_idx, float* out_probs, void* stream);
 /* Whole generate(): prefill + (S-1) decode steps, tokens never leave the device.
@@ -181,7 +183,7 @@ const char* lg_profile_class_name(int cls);   /* NULL past the last class */
 int         lg_vq_set_cta_budget(int ctas);
 
 /* ---- stand-alone kernels exported for unit parity tests ------------------------------------------- */
-/* y[M,N] (f32) = x[M,K] * w[N,K]^T, operands in `dtype`; the same dispatch the engine uses. */
+/* y[M,N] (f32) = x[M,K] * w[N,K]^T, operands in `dtype` (LG_DTYPE_F32, _BF16 or _F16); the same dispatch the engine uses. */
 int  lg_test_gemm(const void* x, const void* w, int M, int N, int K, int dtype, float* y,
                   void* dev_scratch, size_t scratch_bytes, void* stream);
 

@@ -13,12 +13,21 @@ from ctypes import (POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("LG_LIB_PATH") or os.path.join(HERE, "lib", "libllamagen_b200.so")
 
-LG_DTYPE_F32, LG_DTYPE_BF16 = 0, 1
+LG_DTYPE_F32, LG_DTYPE_BF16, LG_DTYPE_F16 = 0, 1, 2
 LG_MODEL_C2I, LG_MODEL_T2I = 0, 1
 
 
 class LgError(RuntimeError):
     """Raised when a C-ABI call returns a negative status (message from lg_last_error())."""
+
+
+def dtype_code(dtype) -> int:
+    """LG_DTYPE_* of a torch dtype (float32, bfloat16 or float16); any other dtype raises LgError."""
+    import torch
+    codes = {torch.float32: LG_DTYPE_F32, torch.bfloat16: LG_DTYPE_BF16, torch.float16: LG_DTYPE_F16}
+    if dtype not in codes:
+        raise LgError(f"unsupported precision {dtype}: the sm_90a engine implements fp32, bf16 and fp16")
+    return codes[dtype]
 
 
 class ModelCfg(Structure):

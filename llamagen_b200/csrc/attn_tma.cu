@@ -1,4 +1,4 @@
-// Decode attention (one query per sequence row) for bf16 KV caches: the K and V prefixes of one (row, head)
+// Decode attention (one query per sequence row) for bf16 or fp16 KV caches: the K and V prefixes of one (row, head)
 // are contiguous [c, hd] streams in HBM, so they are pulled by TMA (cp.async.bulk.tensor, 128-byte swizzle)
 // through a 3-stage mbarrier ring — no registers are spent on loads in flight — and the two tiny matrix
 // products (q.K^T and P.V, M = 1 query padded to the m16 MMA shape) run on the tensor cores with ldmatrix
@@ -9,6 +9,7 @@
 #include "kernels.cuh"
 #include "tma_utils.cuh"
 #include <algorithm>
+#include <type_traits>
 
 namespace {
 
@@ -36,18 +37,16 @@ __device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t& r0, uint32_t&
     asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];\n"
                  : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
 }
+// T = bf16 or f16: the operand type of the MMA and the storage type of q, the KV cache and the output
+template <typename T = bf16>
 __device__ __forceinline__ void mma16816(float* c, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+    mma_m16n8k16<T>(c, a0, a1, a2, a3, b0, b1);
 }
 __device__ __forceinline__ uint32_t swz(int r, int c) { return (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4)); }
-__device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
-    __nv_bfloat162 p = __floats2bfloat162_rn(a, b);
-    return *reinterpret_cast<uint32_t*>(&p);
-}
+template <typename T = bf16>
+__device__ __forceinline__ uint32_t pack16(float a, float b) { return ElemTraits<T>::pack2(a, b); }
 
-struct AttnTmaArgs {
+struct AttnTmaArgs {   // the 16-bit tensors are bf16 or fp16 (the kernel's T); declared bf16 for their 2-byte element arithmetic
     const bf16* q;     // [R, D] (unfused path)
     bf16* out;         // [R, D]
     int R, H, maxS;
@@ -70,7 +69,7 @@ struct AttnTmaArgs {
 // (for future steps) and attends to it straight from shared memory. Every TMA load then only touches rows written
 // in EARLIER steps, so the whole KV stream is requested before the programmatic-dependency wait and overlaps the
 // QKV GEMM; one dependent kernel per layer disappears.
-template <int HD, bool FUSED, int NST, bool PAR_ = (NST > 2)>
+template <typename T, int HD, bool FUSED, int NST, bool PAR_ = (NST > 2)>
 __global__ void __launch_bounds__(kWarps * 32 * (PAR_ ? NST : 1), PAR_ ? 1 : (HD == 64 ? (NST > 2 ? 4 : kCtasPerSm64) : (kKC == 32 ? 5 : 4))) attn_tma_kernel(const __grid_constant__ CUtensorMap kmap,
                                                                const __grid_constant__ CUtensorMap vmap,
                                                                const __grid_constant__ CUtensorMap kmap16,
@@ -87,7 +86,7 @@ __global__ void __launch_bounds__(kWarps * 32 * (PAR_ ? NST : 1), PAR_ ? 1 : (HD
     uint8_t* tiles = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(tiles + NST * 2 * TILE_BYTES);
     float* merge = reinterpret_cast<float*>(full_bar + NST);            // [NSLOT][HD + 2]
-    bf16* qbuf = reinterpret_cast<bf16*>(merge + NSLOT * (HD + 2));            // [3][HD]: q, k_new, v_new (FUSED)
+    T* qbuf = reinterpret_cast<T*>(merge + NSLOT * (HD + 2));                  // [3][HD]: q, k_new, v_new (FUSED)
 
     const int h = blockIdx.x, r = blockIdx.y;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, tg = lane & 3;
@@ -167,7 +166,8 @@ __global__ void __launch_bounds__(kWarps * 32 * (PAR_ ? NST : 1), PAR_ ? 1 : (HD
                     sv.x += t.x; sv.y += t.y; sv.z += t.z; sv.w += t.w;
                 }
             }
-            float x0 = round_bf16(sv.x), x1 = round_bf16(sv.y), x2 = round_bf16(sv.z), x3 = round_bf16(sv.w);
+            float x0 = ElemTraits<T>::round(sv.x), x1 = ElemTraits<T>::round(sv.y), x2 = ElemTraits<T>::round(sv.z),
+                  x3 = ElemTraits<T>::round(sv.w);
             if (sec < 2 && live) {   // apply_rotary_emb (gpt.py:420-430): adjacent pairs, fp32, separate roundings
                 // first pass: the angles were fetched before the dependency wait; a second pass (HD = 128 on 64 threads) loads its own
                 const float4 cs = it == (int)threadIdx.x ? cs_pre
@@ -179,8 +179,8 @@ __global__ void __launch_bounds__(kWarps * 32 * (PAR_ ? NST : 1), PAR_ ? 1 : (HD
                 x0 = y0; x1 = y1; x2 = y2; x3 = y3;
             }
             uint2 pk;
-            pk.x = pack_bf16(x0, x1);
-            pk.y = pack_bf16(x2, x3);
+            pk.x = pack16<T>(x0, x1);
+            pk.y = pack16<T>(x2, x3);
             *reinterpret_cast<uint2*>(qbuf + sec * HD + e) = pk;
             if (sec > 0 && live) {
                 bf16* cache = sec == 1 ? a.kcache : a.vcache;
@@ -230,8 +230,8 @@ __global__ void __launch_bounds__(kWarps * 32 * (PAR_ ? NST : 1), PAR_ ? 1 : (HD
                 const int row = wk * 16 + (lane & 7) + ((lane >> 4) << 3);
                 const int chunk = (kk * 2 + ((lane >> 3) & 1)) & 7;
                 ldsm_x4(kt + (kk / 4) * SUB_BYTES + swz(row, chunk), b0, b1, b2, b3);
-                mma16816(sc[0], qa[kk][0], 0u, qa[kk][1], 0u, b0, b1);
-                mma16816(sc[1], qa[kk][0], 0u, qa[kk][1], 0u, b2, b3);
+                mma16816<T>(sc[0], qa[kk][0], 0u, qa[kk][1], 0u, b0, b1);
+                mma16816<T>(sc[1], qa[kk][0], 0u, qa[kk][1], 0u, b2, b3);
             }
             // ---- online softmax on MMA row 0 (held by the quad g == 0; other quads carry zero rows)
             float pv[4];
@@ -262,17 +262,17 @@ __global__ void __launch_bounds__(kWarps * 32 * (PAR_ ? NST : 1), PAR_ ? 1 : (HD
             mx = mn;
 #pragma unroll
             for (int i = 0; i < HD / 8; ++i) { o[i][0] *= corr; o[i][1] *= corr; }
-            // ---- O += P V : P (bf16) is already in A-fragment layout (C layout of S == A layout of P)
-            const uint32_t pa0 = pack_bf16(pv[0], pv[1]);   // keys tg*2, +1
-            const uint32_t pa2 = pack_bf16(pv[2], pv[3]);   // keys 8 + tg*2, +1
+            // ---- O += P V : P (packed to T) is already in A-fragment layout (C layout of S == A layout of P)
+            const uint32_t pa0 = pack16<T>(pv[0], pv[1]);   // keys tg*2, +1
+            const uint32_t pa2 = pack16<T>(pv[2], pv[3]);   // keys 8 + tg*2, +1
 #pragma unroll
             for (int np = 0; np < HD / 16; ++np) {
                 uint32_t b0, b1, b2, b3;
                 const int row = wk * 16 + (lane & 7) + (((lane >> 3) & 1) << 3);
                 const int chunk = (np * 2 + (lane >> 4)) & 7;
                 ldsm_x4_t(vt + (np / 4) * SUB_BYTES + swz(row, chunk), b0, b1, b2, b3);
-                mma16816(o[2 * np], pa0, 0u, pa2, 0u, b0, b1);
-                mma16816(o[2 * np + 1], pa0, 0u, pa2, 0u, b2, b3);
+                mma16816<T>(o[2 * np], pa0, 0u, pa2, 0u, b0, b1);
+                mma16816<T>(o[2 * np + 1], pa0, 0u, pa2, 0u, b2, b3);
             }
         }
         if (PAR) {
@@ -301,19 +301,19 @@ __global__ void __launch_bounds__(kWarps * 32 * (PAR_ ? NST : 1), PAR_ ? 1 : (HD
 #pragma unroll
         for (int i = 0; i < HD / 32; ++i) {
             const int e = lane * (HD / 32) + i;
-            dot = fmaf(__bfloat162float(qbuf[e]), __bfloat162float(qbuf[HD + e]), dot);
+            dot = fmaf(ElemTraits<T>::to_f(qbuf[e]), ElemTraits<T>::to_f(qbuf[HD + e]), dot);
         }
         dot = warp_sum(dot);
         float* crow = merge + NW * (HD + 2);
 #pragma unroll
         for (int i = 0; i < HD / 32; ++i) {
             const int e = lane * (HD / 32) + i;
-            crow[e] = __bfloat162float(qbuf[2 * HD + e]);
+            crow[e] = ElemTraits<T>::to_f(qbuf[2 * HD + e]);
         }
         if (lane == 0) { crow[HD] = dot * a.scale; crow[HD + 1] = 1.f; }
     }
     __syncthreads();
-    bf16* op = a.out + (size_t)r * D + (size_t)h * hdr;
+    T* op = reinterpret_cast<T*>(a.out) + (size_t)r * D + (size_t)h * hdr;
     for (int e = threadIdx.x; e < hdr; e += blockDim.x) {
         float M_ = -INFINITY;
 #pragma unroll
@@ -326,7 +326,7 @@ __global__ void __launch_bounds__(kWarps * 32 * (PAR_ ? NST : 1), PAR_ ? 1 : (HD
             L += merge[w * (HD + 2) + HD + 1] * c;
             O += merge[w * (HD + 2) + e] * c;
         }
-        op[e] = __float2bfloat16_rn(O / L);
+        op[e] = ElemTraits<T>::from_f(O / L);
     }
 }
 
@@ -459,8 +459,8 @@ __global__ void __launch_bounds__(kWarpsV2 * 32, 1) attn_tma_v2_kernel(const __g
                 mx = mn;
 #pragma unroll
                 for (int i = 0; i < HD / 8; ++i) { o[i][0] *= corr; o[i][1] *= corr; }
-                const uint32_t pa0 = pack_bf16(pv[0], pv[1]);
-                const uint32_t pa2 = pack_bf16(pv[2], pv[3]);
+                const uint32_t pa0 = pack16(pv[0], pv[1]);
+                const uint32_t pa2 = pack16(pv[2], pv[3]);
 #pragma unroll
                 for (int np = 0; np < HD / 16; ++np) {
                     uint32_t b0, b1, b2, b3;
@@ -483,7 +483,7 @@ __global__ void __launch_bounds__(kWarpsV2 * 32, 1) attn_tma_v2_kernel(const __g
             const float inv = 1.0f / l;
 #pragma unroll
             for (int i = 0; i < HD / 8; ++i)
-                *reinterpret_cast<uint32_t*>(op + i * 8 + tg * 2) = pack_bf16(o[i][0] * inv, o[i][1] * inv);
+                *reinterpret_cast<uint32_t*>(op + i * 8 + tg * 2) = pack16(o[i][0] * inv, o[i][1] * inv);
         }
 #pragma unroll
         for (int kk = 0; kk < HD / 16; ++kk) { qa[kk][0] = qn[kk][0]; qa[kk][1] = qn[kk][1]; }
@@ -510,19 +510,19 @@ int launch_v2(const CUtensorMap& kmap, const CUtensorMap& vmap, const AttnTmaArg
     return 0;
 }
 
-template <int HD, bool FUSED, int NST = kStagesA, bool PAR = (NST > 2)>
+template <typename T, int HD, bool FUSED, int NST = kStagesA, bool PAR = (NST > 2)>
 int launch_t(const CUtensorMap& kmap, const CUtensorMap& vmap, const CUtensorMap& kmap16, const CUtensorMap& vmap16,
              const AttnTmaArgs& a, cudaStream_t st) {
     constexpr int TILE_BYTES = (HD / 64) * kKC * 128;
     constexpr int NW = PAR ? NST * kWarps : kWarps;
     const size_t smem = 1024 + (size_t)NST * 2 * TILE_BYTES + NST * sizeof(uint64_t) +
-                        (NW + 1) * (HD + 2) * sizeof(float) + 3 * HD * sizeof(bf16) + 16;
+                        (NW + 1) * (HD + 2) * sizeof(float) + 3 * HD * sizeof(T) + 16;
     static DevOnce attr;
     if (lg_first_on_device(attr)) {
-        LG_CUDA_OK(cudaFuncSetAttribute(attn_tma_kernel<HD, FUSED, NST, PAR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        LG_CUDA_OK(cudaFuncSetAttribute(attn_tma_kernel<T, HD, FUSED, NST, PAR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
     dim3 grid(a.H, a.R);
-    (void)lg_launch(attn_tma_kernel<HD, FUSED, NST, PAR>, dim3(grid), dim3(NW * 32), smem, st, kmap, vmap, kmap16, vmap16, a);
+    (void)lg_launch(attn_tma_kernel<T, HD, FUSED, NST, PAR>, dim3(grid), dim3(NW * 32), smem, st, kmap, vmap, kmap16, vmap16, a);
     LG_LAUNCH_CHECK();
     return 0;
 }
@@ -539,12 +539,13 @@ int launch_t(const CUtensorMap& kmap, const CUtensorMap& vmap, const CUtensorMap
 constexpr int kPfRows = 128;                                   // query / key rows staged per (row, head)
 constexpr int kPfBoxes = (kPfRows + kKC - 1) / kKC;            // K (or V) boxes of kKC rows
 
+template <typename T>
 __global__ void __launch_bounds__(256, 2) attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap qmap,
                                                                  const __grid_constant__ CUtensorMap kmap,
-                                                                 const __grid_constant__ CUtensorMap vmap, AttnTmaArgs a, int T) {
+                                                                 const __grid_constant__ CUtensorMap vmap, AttnTmaArgs a, int Tq) {
     constexpr int HD = 64;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* qs = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);   // [128][64] bf16, swizzle-128B
+    uint8_t* qs = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);   // [128][64] T, swizzle-128B
     uint8_t* ks = qs + kPfRows * 128;                                                              // [kPfBoxes * kKC][64]
     uint8_t* vs = ks + kPfBoxes * kKC * 128;
     uint64_t* bar = reinterpret_cast<uint64_t*>(vs + kPfBoxes * kKC * 128);
@@ -563,7 +564,7 @@ __global__ void __launch_bounds__(256, 2) attn_prefill_tc_kernel(const __grid_co
     lg_pdl_sync();                                   // q and the K/V rows were written by the QKV epilogue just before
     if (threadIdx.x == 0) {
         mbar_expect_tx(bar, (uint32_t)(kPfRows * 128 + 2 * kPfBoxes * kKC * 128));
-        load_2d(qs, &qmap, bar, h * HD, r * T);
+        load_2d(qs, &qmap, bar, h * HD, r * Tq);
         for (int i = 0; i < kPfBoxes; ++i) {
             load_2d(ks + i * kKC * 128, &kmap, bar, 0, (int)(row0 + (long long)i * kKC));
             load_2d(vs + i * kKC * 128, &vmap, bar, 0, (int)(row0 + (long long)i * kKC));
@@ -571,7 +572,7 @@ __global__ void __launch_bounds__(256, 2) attn_prefill_tc_kernel(const __grid_co
     }
     mbar_wait(bar, 0);
     const int q0 = warp * 16;                        // this warp's query rows [q0, q0 + 16)
-    if (q0 >= T) return;
+    if (q0 >= Tq) return;
     const uint32_t qb = smem_u32(qs), kb = smem_u32(ks), vb = smem_u32(vs);
     const int nkb = warp + 1;                        // 16-key blocks at or below the causal diagonal of these rows
 
@@ -588,8 +589,8 @@ __global__ void __launch_bounds__(256, 2) attn_prefill_tc_kernel(const __grid_co
                 uint32_t b0, b1, b2, b3;
                 const int row = kb16 * 16 + (lane & 7) + ((lane >> 4) << 3);
                 ldsm_x4(kb + swz(row, (kk * 2 + ((lane >> 3) & 1)) & 7), b0, b1, b2, b3);
-                mma16816(sc[2 * kb16], a0, a1, a2, a3, b0, b1);
-                mma16816(sc[2 * kb16 + 1], a0, a1, a2, a3, b2, b3);
+                mma16816<T>(sc[2 * kb16], a0, a1, a2, a3, b0, b1);
+                mma16816<T>(sc[2 * kb16 + 1], a0, a1, a2, a3, b2, b3);
             }
         }
     }
@@ -635,42 +636,42 @@ __global__ void __launch_bounds__(256, 2) attn_prefill_tc_kernel(const __grid_co
 #pragma unroll
     for (int kb16 = 0; kb16 < 8; ++kb16) {
         if (kb16 < nkb) {
-            const uint32_t pa0 = pack_bf16(sc[2 * kb16][0], sc[2 * kb16][1]), pa1 = pack_bf16(sc[2 * kb16][2], sc[2 * kb16][3]);
-            const uint32_t pa2 = pack_bf16(sc[2 * kb16 + 1][0], sc[2 * kb16 + 1][1]), pa3 = pack_bf16(sc[2 * kb16 + 1][2], sc[2 * kb16 + 1][3]);
+            const uint32_t pa0 = pack16<T>(sc[2 * kb16][0], sc[2 * kb16][1]), pa1 = pack16<T>(sc[2 * kb16][2], sc[2 * kb16][3]);
+            const uint32_t pa2 = pack16<T>(sc[2 * kb16 + 1][0], sc[2 * kb16 + 1][1]), pa3 = pack16<T>(sc[2 * kb16 + 1][2], sc[2 * kb16 + 1][3]);
 #pragma unroll
             for (int np = 0; np < HD / 16; ++np) {
                 uint32_t b0, b1, b2, b3;
                 const int row = kb16 * 16 + (lane & 7) + (((lane >> 3) & 1) << 3);
                 ldsm_x4_t(vb + swz(row, (np * 2 + (lane >> 4)) & 7), b0, b1, b2, b3);
-                mma16816(o[2 * np], pa0, pa1, pa2, pa3, b0, b1);
-                mma16816(o[2 * np + 1], pa0, pa1, pa2, pa3, b2, b3);
+                mma16816<T>(o[2 * np], pa0, pa1, pa2, pa3, b0, b1);
+                mma16816<T>(o[2 * np + 1], pa0, pa1, pa2, pa3, b2, b3);
             }
         }
     }
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
         const int t = q0 + g + hh * 8;
-        if (t < T) {
+        if (t < Tq) {
             const float inv = 1.0f / l[hh];
-            bf16* op = a.out + ((size_t)r * T + t) * D + (size_t)h * HD;
+            T* op = reinterpret_cast<T*>(a.out) + ((size_t)r * Tq + t) * D + (size_t)h * HD;
 #pragma unroll
             for (int i = 0; i < HD / 8; ++i)
-                *reinterpret_cast<uint32_t*>(op + i * 8 + tg * 2) = pack_bf16(o[i][2 * hh] * inv, o[i][2 * hh + 1] * inv);
+                *reinterpret_cast<uint32_t*>(op + i * 8 + tg * 2) = pack16<T>(o[i][2 * hh] * inv, o[i][2 * hh + 1] * inv);
         }
     }
 }
 
-// KV-cache tensor maps: the whole K (or V) region of the workspace as one [rows, hd] bf16 matrix
-int attn_tma_make_map(void* map_out, const void* cache_base, long long total_rows, int hdp, int tail16) {
+// KV-cache tensor maps: the whole K (or V) region of the workspace as one [rows, hd] bf16 / fp16 matrix
+int attn_tma_make_map(void* map_out, const void* cache_base, long long total_rows, int hdp, int dtype, int tail16) {
     // hdp = cache row width in elements (64, 128, or 112 for head_dim 100: the second 64-wide box then reads 112..127 as zeros)
     return tma::make_map_2d(reinterpret_cast<CUtensorMap*>(map_out), cache_base, (uint64_t)total_rows, (uint64_t)hdp, (uint64_t)hdp,
-                            tail16 ? 16 : kKC, 64);
+                            tail16 ? 16 : kKC, 64, dtype);
 }
 
 bool attn_tma_enabled() { return lg_env_flag("LG_ATTN_TMA", 1) != 0; }
 
 bool attn_prefill_tc_supported(const AttnArgs& a) {
-    return a.dtype == LG_DTYPE_BF16 && a.hd == 64 && (a.hdp == 0 || a.hdp == 64) && a.Tq > 1 && a.Tq <= kPfRows && a.kmap && a.vmap &&
+    return lg_dtype_is16(a.dtype) && a.hd == 64 && (a.hdp == 0 || a.hdp == 64) && a.Tq > 1 && a.Tq <= kPfRows && a.kmap && a.vmap &&
            a.pos.dev == nullptr && a.pos.rows == nullptr && a.pos.value == 0 && a.R <= 65535 && a.maxS >= kPfBoxes * kKC &&
            lg_env_flag("LG_ATTN_PREFILL_TC", 1) != 0;
 }
@@ -681,14 +682,16 @@ int launch_attention_prefill_tc(const AttnArgs& a, cudaStream_t st) {
     t.row_base = a.cache_row_base; t.emb_mask = a.emb_mask; t.B = a.B; t.Tc = a.Tc; t.scale = a.scale;
     t.hd = a.hd; t.hdp = a.hd;
     CUtensorMap qmap;
-    LG_TRY(tma::make_map_2d(&qmap, a.q, (uint64_t)a.R * a.Tq, (uint64_t)a.H * a.hd, (uint64_t)a.H * a.hd, kPfRows, 64));
+    LG_TRY(tma::make_map_2d(&qmap, a.q, (uint64_t)a.R * a.Tq, (uint64_t)a.H * a.hd, (uint64_t)a.H * a.hd, kPfRows, 64, a.dtype));
     const size_t smem = 1024 + (size_t)kPfRows * 128 + 2 * (size_t)kPfBoxes * kKC * 128 + 16;
-    static DevOnce attr;
-    if (lg_first_on_device(attr)) {
-        LG_CUDA_OK(cudaFuncSetAttribute(attn_prefill_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const bool half = a.dtype == LG_DTYPE_F16;
+    auto kern = half ? attn_prefill_tc_kernel<f16> : attn_prefill_tc_kernel<bf16>;
+    static DevOnce attr[2];
+    if (lg_first_on_device(attr[half])) {
+        LG_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
     dim3 grid(a.H, a.R);
-    (void)lg_launch(attn_prefill_tc_kernel, dim3(grid), dim3(256), smem, st, qmap, *reinterpret_cast<const CUtensorMap*>(a.kmap),
+    (void)lg_launch(kern, dim3(grid), dim3(256), smem, st, qmap, *reinterpret_cast<const CUtensorMap*>(a.kmap),
                     *reinterpret_cast<const CUtensorMap*>(a.vmap), t, a.Tq);
     LG_LAUNCH_CHECK();
     return 0;
@@ -696,10 +699,11 @@ int launch_attention_prefill_tc(const AttnArgs& a, cudaStream_t st) {
 
 bool attn_tma_supported(const AttnArgs& a) {
     const bool shape = a.hd == 64 || a.hd == 128 || (a.hd == 100 && a.hdp == 112);
-    return a.dtype == LG_DTYPE_BF16 && a.Tq == 1 && shape && a.kmap && a.vmap && a.kmap16 && a.vmap16 && a.R <= 65535;
+    return lg_dtype_is16(a.dtype) && a.Tq == 1 && shape && a.kmap && a.vmap && a.kmap16 && a.vmap16 && a.R <= 65535;
 }
 
-int launch_attention_tma(const AttnArgs& a, cudaStream_t st) {
+template <typename T>
+static int launch_attention_tma_t(const AttnArgs& a, cudaStream_t st) {
     AttnTmaArgs t;
     t.q = (const bf16*)a.q; t.out = (bf16*)a.out; t.R = a.R; t.H = a.H; t.maxS = a.maxS;
     t.pos_dev = a.pos.dev; t.pos_value = a.pos.value; t.pos_rows = a.pos.rows; t.row_base = a.cache_row_base;
@@ -715,18 +719,22 @@ int launch_attention_tma(const AttnArgs& a, cudaStream_t st) {
     if (a.qkv_partial) {     // fused QKV epilogue
         // few (row, head) items (batch-1 latency path): a 6-stage ring holds a whole 288-key context, so every K/V byte is
         // requested before the dependency wait instead of two stages at a time
-        if (a.hd == 64 && a.R * a.H <= 2 * 132 && lg_env_flag("LG_ATTN_DEEP", 1)) return launch_t<64, true, kDeepStages>(km, vm, km16, vm16, t, st);
+        if (a.hd == 64 && a.R * a.H <= 2 * 132 && lg_env_flag("LG_ATTN_DEEP", 1)) return launch_t<T, 64, true, kDeepStages>(km, vm, km16, vm16, t, st);
         // deeper sequential ring (A/B switch): more keys requested before the dependency wait, fewer refill round trips
         const int nst = lg_env_flag("LG_ATTN_NST", 2);
-        if (a.hd == 64 && nst == 3) return launch_t<64, true, 3, false>(km, vm, km16, vm16, t, st);
-        if (a.hd == 64 && nst == 4) return launch_t<64, true, 4, false>(km, vm, km16, vm16, t, st);
-        if (a.hd == 64) return launch_t<64, true>(km, vm, km16, vm16, t, st);
-        return launch_t<128, true>(km, vm, km16, vm16, t, st);
+        if (a.hd == 64 && nst == 3) return launch_t<T, 64, true, 3, false>(km, vm, km16, vm16, t, st);
+        if (a.hd == 64 && nst == 4) return launch_t<T, 64, true, 4, false>(km, vm, km16, vm16, t, st);
+        if (a.hd == 64) return launch_t<T, 64, true>(km, vm, km16, vm16, t, st);
+        return launch_t<T, 128, true>(km, vm, km16, vm16, t, st);
     }
     // v2 (persistent warp-per-item, LG_ATTN_V2=1) stays opt-in: with one warp per scheduler its ldmatrix->mma->softmax chain is
-    // latency-bound, which made it slower than the CTA-per-item kernel where it was measured.
-    const bool v2 = lg_env_flag("LG_ATTN_V2", 0) && a.R * a.H >= 4 * 132 && a.hd == 64 && !a.pos.rows;   // (hd 64 only)
+    // latency-bound, which made it slower than the CTA-per-item kernel where it was measured. bf16 only.
+    const bool v2 = std::is_same<T, bf16>::value && lg_env_flag("LG_ATTN_V2", 0) && a.R * a.H >= 4 * 132 && a.hd == 64 && !a.pos.rows;
     if (v2) return launch_v2<64>(km, vm, t, st);
-    if (a.hd == 64) return launch_t<64, false>(km, vm, km16, vm16, t, st);
-    return launch_t<128, false>(km, vm, km16, vm16, t, st);
+    if (a.hd == 64) return launch_t<T, 64, false>(km, vm, km16, vm16, t, st);
+    return launch_t<T, 128, false>(km, vm, km16, vm16, t, st);
+}
+
+int launch_attention_tma(const AttnArgs& a, cudaStream_t st) {
+    return a.dtype == LG_DTYPE_F16 ? launch_attention_tma_t<f16>(a, st) : launch_attention_tma_t<bf16>(a, st);
 }

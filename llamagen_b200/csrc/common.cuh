@@ -2,6 +2,8 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
+#include <cuda.h>
 #include <stdint.h>
 #include <string>
 #include <cstdio>
@@ -10,6 +12,21 @@
 #include "../../include/llamagen_b200.h"
 
 typedef __nv_bfloat16 bf16;
+typedef __half f16;
+
+// The one place an LG_DTYPE_* becomes a storage format: element size in bytes and the TMA data type of the 16-bit tensor
+// kernels (LG_DTYPE_F32 has no TMA path; its format is reported for completeness).
+struct DtypeInfo {
+    int esz;
+    CUtensorMapDataType tma;
+};
+inline DtypeInfo lg_dtype_info(int dtype) {
+    if (dtype == LG_DTYPE_F16) return {2, CU_TENSOR_MAP_DATA_TYPE_FLOAT16};
+    if (dtype == LG_DTYPE_BF16) return {2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16};
+    return {4, CU_TENSOR_MAP_DATA_TYPE_FLOAT32};
+}
+// bf16 and fp16 share every tensor-core kernel (same shared-memory layouts and MMA rates on sm_90a)
+inline bool lg_dtype_is16(int dtype) { return dtype == LG_DTYPE_BF16 || dtype == LG_DTYPE_F16; }
 
 // ---------------------------------------------------------------------------------------------
 // host-side error plumbing: every extern "C" entry point returns <0 and records a message.
@@ -131,9 +148,47 @@ template <> struct ElemTraits<bf16> {
     __device__ __forceinline__ static float to_f(bf16 v) { return __bfloat162float(v); }
     __device__ __forceinline__ static bf16 from_f(float v) { return __float2bfloat16_rn(v); }
     __device__ __forceinline__ static float round(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
+    // two packed elements <-> floats (element 0 in the low half)
+    __device__ __forceinline__ static float lo(uint32_t w) { return __uint_as_float(w << 16); }
+    __device__ __forceinline__ static float hi(uint32_t w) { return __uint_as_float(w & 0xffff0000u); }
+    __device__ __forceinline__ static uint32_t pack2(float a, float b) {
+        __nv_bfloat162 p = __floats2bfloat162_rn(a, b);
+        return *reinterpret_cast<uint32_t*>(&p);
+    }
+};
+// IEEE half: round-to-nearest-even, overflow to +-inf like torch (no saturation)
+template <> struct ElemTraits<f16> {
+    static constexpr int dtype = LG_DTYPE_F16;
+    __device__ __forceinline__ static float to_f(f16 v) { return __half2float(v); }
+    __device__ __forceinline__ static f16 from_f(float v) { return __float2half_rn(v); }
+    __device__ __forceinline__ static float round(float v) { return __half2float(__float2half_rn(v)); }
+    __device__ __forceinline__ static float lo(uint32_t w) { return __half2float(__ushort_as_half((unsigned short)(w & 0xffffu))); }
+    __device__ __forceinline__ static float hi(uint32_t w) { return __half2float(__ushort_as_half((unsigned short)(w >> 16))); }
+    __device__ __forceinline__ static uint32_t pack2(float a, float b) {
+        __half2 p = __floats2half2_rn(a, b);
+        return *reinterpret_cast<uint32_t*>(&p);
+    }
 };
 
 __device__ __forceinline__ float round_bf16(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
+
+#ifdef __CUDACC__
+// mma.sync m16n8k16 with fp32 accumulators; T selects the .bf16 or .f16 operand type (register layouts are identical)
+template <typename T>
+__device__ __forceinline__ void mma_m16n8k16(float* c, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1);
+template <>
+__device__ __forceinline__ void mma_m16n8k16<bf16>(float* c, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
+                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+template <>
+__device__ __forceinline__ void mma_m16n8k16<f16>(float* c, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
+                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+#endif
 
 // Load VEC contiguous elements of T as floats (VEC*sizeof(T) is 8, 16 or 32 bytes, pointer aligned to
 // min(16, VEC*sizeof(T))).
@@ -156,6 +211,26 @@ template <> struct VecLoad<bf16, 4> {
         o[1] = __uint_as_float(u.x & 0xffff0000u);
         o[2] = __uint_as_float(u.y << 16);
         o[3] = __uint_as_float(u.y & 0xffff0000u);
+    }
+};
+template <> struct VecLoad<f16, 8> {
+    __device__ __forceinline__ static void load(const f16* p, float* o) {
+        uint4 u = *reinterpret_cast<const uint4*>(p);
+        const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            o[2 * i] = ElemTraits<f16>::lo(w[i]);
+            o[2 * i + 1] = ElemTraits<f16>::hi(w[i]);
+        }
+    }
+};
+template <> struct VecLoad<f16, 4> {
+    __device__ __forceinline__ static void load(const f16* p, float* o) {
+        uint2 u = *reinterpret_cast<const uint2*>(p);
+        o[0] = ElemTraits<f16>::lo(u.x);
+        o[1] = ElemTraits<f16>::hi(u.x);
+        o[2] = ElemTraits<f16>::lo(u.y);
+        o[3] = ElemTraits<f16>::hi(u.y);
     }
 };
 template <> struct VecLoad<float, 8> {

@@ -113,7 +113,7 @@ struct Workspace {
     int* counters = nullptr;  // [0] = pos, [1] = step (chain g of a split uses [2g], [2g+1])
     size_t layer_cache_bytes = 0;
     size_t partial_floats = 0;
-    alignas(64) unsigned char kmap[128];   // CUtensorMap over the K / V cache regions (bf16 only)
+    alignas(64) unsigned char kmap[128];   // CUtensorMap over the K / V cache regions (bf16 / fp16 only)
     alignas(64) unsigned char vmap[128];
     alignas(64) unsigned char kmap16[128];  // same regions, 16-row boxes (tail chunk of the decode attention)
     alignas(64) unsigned char vmap16[128];
@@ -130,7 +130,7 @@ struct lg_engine {
     lg_model_cfg cfg;
     int device = 0;
     int hd = 0;
-    int hdp = 0;                          // KV-cache row width in elements: hd, or 112 for head_dim 100 in bf16 (GPT-3B) so that the rows
+    int hdp = 0;                          // KV-cache row width in elements: hd, or 112 for head_dim 100 in bf16 / fp16 (GPT-3B) so that the rows
                                           // are 16-byte multiples and the TMA attention kernel can stream them (dims 100..111 stay zero)
     size_t esz = 2;
     std::unordered_map<std::string, Tensor> w;
@@ -282,19 +282,19 @@ int lg_engine::forward(int M, int Tq, PosArg pos, const float* emb_mask, int B, 
         skip_first_norm = false;
         for (int l = 0; l < L; ++l) {
             const Layer& ly = layers[l];
-            GemvSmall gq{ly.wqkv, nullptr, 3 * D, D, M, ws.h, ly.attn_norm, cfg.norm_eps, ws.partial, nullptr, nullptr};
+            GemvSmall gq{ly.wqkv, nullptr, 3 * D, D, M, ws.h, ly.attn_norm, cfg.norm_eps, ws.partial, nullptr, nullptr, dt};
             LG_PROF(PC_GEMM_QKV, st, launch_gemv_small(gq, st));
             AttnArgs aa = attn_args(l);
             aa.qkv_partial = ws.partial; aa.qkv_ksplit = 1; aa.freqs = freqs;
             LG_PROF(PC_ATTENTION, st, launch_attention(aa, st));
-            GemvSmall go{ly.wo, nullptr, D, D, M, ws.attn, nullptr, 0.f, nullptr, ws.h, nullptr};
+            GemvSmall go{ly.wo, nullptr, D, D, M, ws.attn, nullptr, 0.f, nullptr, ws.h, nullptr, dt};
             LG_PROF(PC_GEMM_WO, st, launch_gemv_small(go, st));
-            GemvSmall g13{ly.w1, ly.w3, F, D, M, ws.h, ly.ffn_norm, cfg.norm_eps, nullptr, nullptr, ws.ff};
+            GemvSmall g13{ly.w1, ly.w3, F, D, M, ws.h, ly.ffn_norm, cfg.norm_eps, nullptr, nullptr, ws.ff, dt};
             LG_PROF(PC_GEMM_W13, st, launch_gemv_small(g13, st));
-            GemvSmall g2{ly.w2, nullptr, D, F, M, ws.ff, nullptr, 0.f, nullptr, ws.h, nullptr};
+            GemvSmall g2{ly.w2, nullptr, D, F, M, ws.ff, nullptr, 0.f, nullptr, ws.h, nullptr, dt};
             LG_PROF(PC_GEMM_W2, st, launch_gemv_small(g2, st));
         }
-        GemvSmall gh{output, nullptr, V, D, M, ws.h, final_norm, cfg.norm_eps, logits_out, nullptr, nullptr};
+        GemvSmall gh{output, nullptr, V, D, M, ws.h, final_norm, cfg.norm_eps, logits_out, nullptr, nullptr, dt};
         LG_PROF(PC_GEMM_HEAD, st, launch_gemv_small(gh, st));
         return 0;
     }
@@ -388,7 +388,7 @@ void lg_reset_launch_count(void) { g_lg_launches.store(0); }
 
 int lg_engine_create(const lg_model_cfg* cfg, int device, lg_engine** out) {
     LG_REQUIRE(cfg && out, "lg_engine_create: null argument");
-    LG_REQUIRE(cfg->dtype == LG_DTYPE_F32 || cfg->dtype == LG_DTYPE_BF16, "unsupported dtype %d (f32 and bf16 only)", cfg->dtype);
+    LG_REQUIRE(cfg->dtype == LG_DTYPE_F32 || lg_dtype_is16(cfg->dtype), "unsupported dtype %d (f32, bf16 and f16 only)", cfg->dtype);
     LG_REQUIRE(cfg->model_type == LG_MODEL_C2I || cfg->model_type == LG_MODEL_T2I, "please check model type");
     LG_REQUIRE(cfg->n_layer > 0 && cfg->n_head > 0 && cfg->dim > 0 && cfg->dim % cfg->n_head == 0, "bad model dims");
     const int hd = cfg->dim / cfg->n_head;
@@ -398,8 +398,8 @@ int lg_engine_create(const lg_model_cfg* cfg, int device, lg_engine** out) {
     e->cfg = *cfg;
     e->device = device;
     e->hd = hd;
-    e->hdp = (hd == 100 && cfg->dtype == LG_DTYPE_BF16 && lg_env_flag("LG_HD_PAD", 1)) ? 112 : hd;
-    e->esz = cfg->dtype == LG_DTYPE_F32 ? 4 : 2;
+    e->hdp = (hd == 100 && lg_dtype_is16(cfg->dtype) && lg_env_flag("LG_HD_PAD", 1)) ? 112 : hd;
+    e->esz = (size_t)lg_dtype_info(cfg->dtype).esz;
     const char* ng = getenv("LG_NO_GRAPH");
     e->use_graph = !(ng && ng[0] == '1');
     *out = e;
@@ -514,13 +514,14 @@ int lg_engine_set_workspace(lg_engine* e, void* dev_ws, size_t bytes, int rows, 
     // still be running kernels on memory the caching allocator has just recycled.
     e->ws_needs_zero = true;
     tmp.have_maps = false;
-    if (e->cfg.dtype == LG_DTYPE_BF16 && (e->hd == 64 || e->hd == 128 || e->hdp == 112)) {
+    const int dt = e->cfg.dtype;
+    if (lg_dtype_is16(dt) && (e->hd == 64 || e->hd == 128 || e->hdp == 112)) {
         const long long total_rows = (long long)e->cfg.n_layer * rows * e->cfg.n_head * max_seq;
         if (total_rows < (1ll << 31)) {
-            LG_TRY(attn_tma_make_map(tmp.kmap, tmp.kcache, total_rows, e->hdp));
-            LG_TRY(attn_tma_make_map(tmp.vmap, tmp.vcache, total_rows, e->hdp));
-            LG_TRY(attn_tma_make_map(tmp.kmap16, tmp.kcache, total_rows, e->hdp, 1));
-            LG_TRY(attn_tma_make_map(tmp.vmap16, tmp.vcache, total_rows, e->hdp, 1));
+            LG_TRY(attn_tma_make_map(tmp.kmap, tmp.kcache, total_rows, e->hdp, dt));
+            LG_TRY(attn_tma_make_map(tmp.vmap, tmp.vcache, total_rows, e->hdp, dt));
+            LG_TRY(attn_tma_make_map(tmp.kmap16, tmp.kcache, total_rows, e->hdp, dt, 1));
+            LG_TRY(attn_tma_make_map(tmp.vmap16, tmp.vcache, total_rows, e->hdp, dt, 1));
             tmp.have_maps = true;
         }
     }
@@ -541,7 +542,7 @@ int lg_engine_set_workspace(lg_engine* e, void* dev_ws, size_t bytes, int rows, 
     int n = lg_env_flag("LG_SPLIT", 3.0 * layer_bytes <= (double)l2_bytes ? 2 : 1);
     if (n > lg_engine::kMaxChains) n = lg_engine::kMaxChains;
     while (n >= 2 && (rows % n != 0 || (rows / n) % 2 != 0 || rows / n < 16)) --n;
-    if (n >= 2 && e->cfg.dtype == LG_DTYPE_BF16 && tmp.have_maps) {
+    if (n >= 2 && lg_dtype_is16(dt) && tmp.have_maps) {
         const lg_model_cfg& c = e->cfg;
         const int hr = rows / n;
         const int Tc = c.model_type == LG_MODEL_T2I ? c.cls_token_num : 1;
@@ -568,10 +569,10 @@ int lg_engine_set_workspace(lg_engine* e, void* dev_ws, size_t bytes, int rows, 
                 w.tokens = tmp.tokens + (size_t)g * hr;
                 w.counters = tmp.counters + 2 * g;
                 const long long total_rows = (long long)c.n_layer * hr * c.n_head * max_seq;
-                LG_TRY(attn_tma_make_map(w.kmap, w.kcache, total_rows, e->hdp));
-                LG_TRY(attn_tma_make_map(w.vmap, w.vcache, total_rows, e->hdp));
-                LG_TRY(attn_tma_make_map(w.kmap16, w.kcache, total_rows, e->hdp, 1));
-                LG_TRY(attn_tma_make_map(w.vmap16, w.vcache, total_rows, e->hdp, 1));
+                LG_TRY(attn_tma_make_map(w.kmap, w.kcache, total_rows, e->hdp, dt));
+                LG_TRY(attn_tma_make_map(w.vmap, w.vcache, total_rows, e->hdp, dt));
+                LG_TRY(attn_tma_make_map(w.kmap16, w.kcache, total_rows, e->hdp, dt, 1));
+                LG_TRY(attn_tma_make_map(w.vmap16, w.vcache, total_rows, e->hdp, dt, 1));
                 w.have_maps = true;
                 e->sub[g] = w;
             }
@@ -592,7 +593,8 @@ static int check_ready(lg_engine* e, int rows, int seq) {
     return 0;
 }
 
-static int round_logits_inplace(float* logits, size_t n, cudaStream_t st);
+// 16-bit engines: the head's logits are a bf16 / fp16 tensor in the reference (gpt.py:368 `.float()` of it); no-op for fp32
+static int round_logits_inplace(float* logits, size_t n, int dtype, cudaStream_t st);
 
 int lg_prefill(lg_engine* e, const void* cond, const float* emb_mask, int B, int T, int use_cfg, float* logits_out,
                void* stream) {
@@ -607,7 +609,7 @@ int lg_prefill(lg_engine* e, const void* cond, const float* emb_mask, int B, int
     LG_TRY(e->embed_cond(cond, B, R, T, st));
     PosArg pos{nullptr, 0};
     LG_TRY(e->forward(R * T, T, pos, emb_mask, B, logits_out, false, st));
-    if (e->cfg.dtype == LG_DTYPE_BF16) LG_TRY(round_logits_inplace(logits_out, (size_t)R * e->cfg.vocab_size, st));
+    LG_TRY(round_logits_inplace(logits_out, (size_t)R * e->cfg.vocab_size, e->cfg.dtype, st));
     return 0;
 }
 
@@ -623,7 +625,7 @@ int lg_decode_step(lg_engine* e, const int32_t* tokens, int B, int pos, int use_
     else LG_TRY(launch_embed(e->tok_emb, tokens, B, R, -1, e->cfg.dim, e->cfg.dtype, e->ws.h, st));
     PosArg p{nullptr, pos};
     LG_TRY(e->forward(R, 1, p, nullptr, B, logits_out, false, st));
-    if (e->cfg.dtype == LG_DTYPE_BF16) LG_TRY(round_logits_inplace(logits_out, (size_t)R * e->cfg.vocab_size, st));
+    LG_TRY(round_logits_inplace(logits_out, (size_t)R * e->cfg.vocab_size, e->cfg.dtype, st));
     return 0;
 }
 
@@ -642,7 +644,7 @@ int lg_decode_rows(lg_engine* e, const int32_t* tokens, const int32_t* pos_rows,
     PosArg p{nullptr, 0, pos_rows};
     e->pd_tokens = nullptr;
     LG_TRY(e->forward(R, 1, p, nullptr, B, logits_out, false, st));
-    if (e->cfg.dtype == LG_DTYPE_BF16) LG_TRY(round_logits_inplace(logits_out, (size_t)R * e->cfg.vocab_size, st));
+    LG_TRY(round_logits_inplace(logits_out, (size_t)R * e->cfg.vocab_size, e->cfg.dtype, st));
     return 0;
 }
 
@@ -650,7 +652,7 @@ int lg_sample_rows(const float* logits, int B, int V, int mix_cfg, int round_dty
                    const int32_t* step_rows, int32_t* out_idx, int32_t* out_seq, int seq_stride, void* stream) {
     LG_REQUIRE(logits && sc && seed_rows && step_rows && (out_idx || out_seq), "lg_sample_rows: null argument");
     SampleArgs a{};
-    a.logits = logits; a.B = B; a.V = V; a.mix_cfg = mix_cfg; a.round_bf16 = round_dtype == LG_DTYPE_BF16;
+    a.logits = logits; a.B = B; a.V = V; a.mix_cfg = mix_cfg; a.round_dtype = lg_dtype_is16(round_dtype) ? round_dtype : LG_DTYPE_F32;
     a.cfg_scale = sc->cfg_scale; a.cfg_interval = sc->cfg_interval; a.temperature = sc->temperature;
     a.top_k = sc->top_k; a.top_p = sc->top_p; a.greedy = sc->greedy; a.seed = sc->seed; a.step = 0;
     a.seed_rows = seed_rows; a.step_rows = step_rows;
@@ -662,7 +664,7 @@ int lg_sample(const float* logits, int B, int V, int mix_cfg, int round_dtype, c
               int32_t* out_idx, float* out_probs, void* stream) {
     LG_REQUIRE(logits && sc && out_idx, "lg_sample: null argument");
     SampleArgs a{};
-    a.logits = logits; a.B = B; a.V = V; a.mix_cfg = mix_cfg; a.round_bf16 = round_dtype == LG_DTYPE_BF16;
+    a.logits = logits; a.B = B; a.V = V; a.mix_cfg = mix_cfg; a.round_dtype = lg_dtype_is16(round_dtype) ? round_dtype : LG_DTYPE_F32;
     a.cfg_scale = sc->cfg_scale; a.cfg_interval = sc->cfg_interval; a.temperature = sc->temperature;
     a.top_k = sc->top_k; a.top_p = sc->top_p; a.greedy = sc->greedy; a.seed = sc->seed; a.step = step;
     a.out_idx = out_idx; a.out_probs = out_probs;
@@ -750,7 +752,7 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
         k.emb_mask = emb_mask ? emb_mask + boff * T : nullptr;
         SampleArgs& sa = k.sa;
         sa.logits = k.w.logits; sa.B = k.B; sa.V = c.vocab_size; sa.mix_cfg = use_cfg;
-        sa.round_bf16 = c.dtype == LG_DTYPE_BF16;
+        sa.round_dtype = c.dtype;   // LG_DTYPE_F32 (0): no rounding
         sa.cfg_scale = sc->cfg_scale; sa.cfg_interval = sc->cfg_interval; sa.temperature = sc->temperature;
         sa.top_k = sc->top_k; sa.top_p = sc->top_p; sa.greedy = sc->greedy; sa.seed = sc->seed;
         sa.row_offset = (int)boff;
@@ -759,9 +761,9 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
         sa.dbg_logits = dbg_logits; sa.dbg_batch = B;
     }
 
-    // Fused tail (bf16): the sample kernel writes the next step's input rows (token embedding, and on the batched path the layer-0
+    // Fused tail (bf16 / fp16): the sample kernel writes the next step's input rows (token embedding, and on the batched path the layer-0
     // RMSNorm) and advances the device-resident counters, so a decode iteration loses its embed / rmsnorm / advance kernels.
-    const bool fuse_tail = c.dtype == LG_DTYPE_BF16 && lg_env_flag("LG_FUSE_TAIL", 1) && c.dim % 2 == 0;
+    const bool fuse_tail = lg_dtype_is16(c.dtype) && lg_env_flag("LG_FUSE_TAIL", 1) && c.dim % 2 == 0;
     auto tail_on = [&](Chain& k) -> bool {
         e->ws = k.w;
         return fuse_tail && !e->persist_usable(k.R);
@@ -936,10 +938,16 @@ __global__ void round_bf16_kernel(float* p, size_t n) {
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
         p[i] = round_bf16(p[i]);
 }
+__global__ void round_f16_kernel(float* p, size_t n) {
+    lg_pdl_sync();
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+        p[i] = ElemTraits<f16>::round(p[i]);   // past +-65504 -> +-inf, like torch's fp16 head
+}
 }  // namespace
-static int round_logits_inplace(float* logits, size_t n, cudaStream_t st) {
+static int round_logits_inplace(float* logits, size_t n, int dtype, cudaStream_t st) {
+    if (!lg_dtype_is16(dtype)) return 0;
     const int blocks = (int)std::min<size_t>((n + 255) / 256, 132 * 8);
-    (void)lg_launch(round_bf16_kernel, dim3(blocks), dim3(256), 0, st, logits, n);
+    (void)lg_launch(dtype == LG_DTYPE_F16 ? round_f16_kernel : round_bf16_kernel, dim3(blocks), dim3(256), 0, st, logits, n);
     LG_LAUNCH_CHECK();
     return 0;
 }

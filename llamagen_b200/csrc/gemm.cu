@@ -2,7 +2,8 @@
 // Two kernels, both produce fp32 split-K slabs consumed by the row-wise epilogues in xf_kernels.cu:
 //   * gemm_skinny_kernel : M <= 8 rows per tile on CUDA cores, 128-bit weight streaming. Used for the
 //     batch-1 latency path (HBM-bound GEMV regime) and for the fp32 "exact" mode at any M.
-//   * mma::gemm_mma_kernel: bf16 tensor-core tiles for M > 8.
+//   * mma::gemm_mma_kernel: bf16 / fp16 tensor-core tiles for M > 8 (the fallback of the wgmma kernel, gemm_tc.cu).
+// bf16 and fp16 take the same path for every shape; only the MMA operand type differs.
 #include "kernels.cuh"
 #include "gemm_mma.cuh"
 #include <algorithm>
@@ -96,7 +97,7 @@ struct Plan {
 Plan make_plan(int M, int N, int K, int dtype) {
     Plan p;
     p.tc = false;
-    // bf16: the wgmma kernel is used for every row count (a batch-1 step pads its 2 rows to the minimum N = 16); the CUDA-core
+    // bf16 / fp16: the wgmma kernel is used for every row count (a batch-1 step pads its 2 rows to the minimum N = 16); the CUDA-core
     // skinny kernel stays for the fp32 exact mode.
     const bool tc_ok = lg_env_flag("LG_GEMM_TC", 1) && gemm_tc_supported(M, N, K, dtype) && N % 128 == 0;
     p.skinny = (dtype == LG_DTYPE_F32) || (M <= kSkinnyRT && !tc_ok);
@@ -149,6 +150,10 @@ int gemm_partial(const void* X, int ldx, const void* Wa, const void* Wb, int n_s
             }
             (void)lg_launch(gemm_skinny_kernel<float>, dim3(grid), dim3(kSkinnyWarps * 32), smem, st, 
                 (const float*)X, ldx, (const float*)Wa, (const float*)Wb, n_split, M, N, K, kper, partial);
+        } else if (dtype == LG_DTYPE_F16) {
+            const size_t smem = (size_t)kSkinnyRT * kSkinnyKC * sizeof(f16);
+            (void)lg_launch(gemm_skinny_kernel<f16>, dim3(grid), dim3(kSkinnyWarps * 32), smem, st,
+                (const f16*)X, ldx, (const f16*)Wa, (const f16*)Wb, n_split, M, N, K, kper, partial);
         } else {
             const size_t smem = (size_t)kSkinnyRT * kSkinnyKC * sizeof(bf16);
             (void)lg_launch(gemm_skinny_kernel<bf16>, dim3(grid), dim3(kSkinnyWarps * 32), smem, st, 
@@ -159,11 +164,17 @@ int gemm_partial(const void* X, int ldx, const void* Wa, const void* Wb, int n_s
     }
     if (p.tc) {
         if (n_split % 128 != 0 && n_split != N) return lg_fail("gemm: weight segment boundary %d not tile aligned", n_split);
-        return gemm_tc_partial(X, ldx, Wa, Wb, n_split, M, N, K, partial, nullptr, st, next);
+        return gemm_tc_partial(X, ldx, Wa, Wb, n_split, M, N, K, dtype, partial, nullptr, st, next);
     }
-    mma::DenseA al{(const bf16*)X, ldx, 0, M};
+    LG_REQUIRE(lg_dtype_is16(dtype), "gemm: unsupported dtype %d", dtype);
+    mma::DenseA al{(const bf16*)X, ldx, 0, M};   // raw 16-bit elements: the same loaders serve fp16
     mma::BRows bw{(const bf16*)Wa, (const bf16*)Wb, n_split, K, 0, N};
     mma::EpiPartial epi{partial, M, N};
+    if (dtype == LG_DTYPE_F16) {
+        if (p.bm == 32) return mma::launch_gemm_mma<32, 128, 1, 8, 4, f16>(al, bw, M, N, K, p.ksplit, 1, epi, st);
+        if (p.bm == 64) return mma::launch_gemm_mma<64, 128, 2, 4, 4, f16>(al, bw, M, N, K, p.ksplit, 1, epi, st);
+        return mma::launch_gemm_mma<128, 128, 2, 4, 3, f16>(al, bw, M, N, K, p.ksplit, 1, epi, st);
+    }
     if (p.bm == 32) return mma::launch_gemm_mma<32, 128, 1, 8, 4>(al, bw, M, N, K, p.ksplit, 1, epi, st);
     if (p.bm == 64) return mma::launch_gemm_mma<64, 128, 2, 4, 4>(al, bw, M, N, K, p.ksplit, 1, epi, st);
     return mma::launch_gemm_mma<128, 128, 2, 4, 3>(al, bw, M, N, K, p.ksplit, 1, epi, st);

@@ -1,4 +1,4 @@
-// bf16 tensor-core GEMM main loop, C[M,N] = A[M,K] * B[N,K]^T, fp32 accumulate (round-1 workhorse:
+// bf16 / fp16 tensor-core GEMM main loop, C[M,N] = A[M,K] * B[N,K]^T, fp32 accumulate (round-1 workhorse:
 // mma.sync m16n8k16 fed by a multi-stage cp.async pipeline; BK = 64 so every shared-memory row is one
 // 128-byte line, XOR-swizzled by (row & 7) -> conflict-free cp.async stores and ldmatrix loads).
 //
@@ -7,6 +7,8 @@
 //   * implicit-GEMM convolution over NHWC activations (zero padding and the nearest-2x upsample of
 //     vq_model.py:374-378 are folded into the address computation, nothing is materialised).
 // The epilogue is a functor called with two adjacent output columns (n, n+1) of one row.
+// T (bf16 by default, f16 for fp16 transformers) only selects the MMA operand type: loads move raw 16-bit elements, so the
+// loaders address fp16 tensors through the same bf16-typed pointers.
 #pragma once
 #include "common.cuh"
 
@@ -27,11 +29,6 @@ template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile(
 __device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
     asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];\n"
                  : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void mma_bf16(float* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
 // byte offset of 16-byte chunk `c` (0..7) of row `r` inside a [rows][128 B] swizzled tile
@@ -115,7 +112,7 @@ struct EpiPartial {          // fp32 slabs [z][M][N]
     }
 };
 
-template <int BM, int BN, int WARPS_M, int WARPS_N, int STAGES, class AL, class Epi>
+template <int BM, int BN, int WARPS_M, int WARPS_N, int STAGES, class AL, class Epi, typename T = bf16>
 __global__ void __launch_bounds__(kThreads) gemm_mma_kernel(AL al, BRows bw, int M, int N, int K, int kper,
                                                             int ksplit, Epi epi) {
     lg_pdl_sync();
@@ -204,8 +201,8 @@ __global__ void __launch_bounds__(kThreads) gemm_mma_kernel(AL al, BRows bw, int
                 ldmatrix_x4(sb + swz(r, kk * 2 + ((lane >> 3) & 1)), b0, b1, b2, b3);
 #pragma unroll
                 for (int mt = 0; mt < MT; ++mt) {
-                    mma_bf16(acc[mt][2 * np], af[mt], b0, b1);
-                    mma_bf16(acc[mt][2 * np + 1], af[mt], b2, b3);
+                    mma_m16n8k16<T>(acc[mt][2 * np], af[mt][0], af[mt][1], af[mt][2], af[mt][3], b0, b1);
+                    mma_m16n8k16<T>(acc[mt][2 * np + 1], af[mt][0], af[mt][1], af[mt][2], af[mt][3], b2, b3);
                 }
             }
         }
@@ -226,10 +223,10 @@ __global__ void __launch_bounds__(kThreads) gemm_mma_kernel(AL al, BRows bw, int
     }
 }
 
-template <int BM, int BN, int WARPS_M, int WARPS_N, int STAGES, class AL, class Epi>
+template <int BM, int BN, int WARPS_M, int WARPS_N, int STAGES, typename T = bf16, class AL, class Epi>
 int launch_gemm_mma(const AL& al, const BRows& bw, int M, int N, int K, int ksplit, int nbatch, const Epi& epi,
                     cudaStream_t st) {
-    auto kern = gemm_mma_kernel<BM, BN, WARPS_M, WARPS_N, STAGES, AL, Epi>;
+    auto kern = gemm_mma_kernel<BM, BN, WARPS_M, WARPS_N, STAGES, AL, Epi, T>;
     constexpr int smem = STAGES * (BM + BN) * 128;
     static DevOnce attr_set;
     if (lg_first_on_device(attr_set)) {

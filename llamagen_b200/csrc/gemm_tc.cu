@@ -51,8 +51,9 @@ __device__ __forceinline__ unsigned long long gtime() {
         if (a.trace) a.trace[(size_t)(blockIdx.y * gridDim.x + blockIdx.x) * 8 + (slot)] = gtime(); \
     } while (0)
 
-// RP: rows of one row block padded to a power of two (wgmma N); the activation box has RP rows, rows >= M read as zero
-template <int RP>
+// RP: rows of one row block padded to a power of two (wgmma N); the activation box has RP rows, rows >= M read as zero.
+// T: operand type (bf16 or f16), only the wgmma instruction depends on it.
+template <int RP, typename T>
 __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_constant__ CUtensorMap map_wa,
                                                               const __grid_constant__ CUtensorMap map_wb,
                                                               const __grid_constant__ CUtensorMap map_x, TcArgs a) {
@@ -149,7 +150,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         const uint32_t sa = smem_u32(tiles + s * stage_bytes);
         wg::fence_regs<RP / 2>(acc);
         wg::fence();
-        wg::mma_kblock<RP>(acc, sa + g * (kATileBytes / 2), sa + kATileBytes);
+        wg::mma_kblock<RP, T>(acc, sa + g * (kATileBytes / 2), sa + kATileBytes);
         wg::commit();
         wg::wait<1>();                                  // the previous k-block's MMAs have retired: release its stage
         wg::fence_regs<RP / 2>(acc);
@@ -189,14 +190,16 @@ static EncodeTiledFn get_encode() {
     return fn;
 }
 int make_map_2d(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, uint32_t box_rows,
-                uint32_t box_cols) {
+                uint32_t box_cols, int dtype) {
     EncodeTiledFn enc = get_encode();
     LG_REQUIRE(enc, "cuTensorMapEncodeTiled is not available from the driver");
+    LG_REQUIRE(lg_dtype_is16(dtype), "make_map_2d: dtype %d has no 16-bit tensor map", dtype);
+    const DtypeInfo di = lg_dtype_info(dtype);
     cuuint64_t dims[2] = {cols, rows};
-    cuuint64_t strides[1] = {ld_elems * 2};
+    cuuint64_t strides[1] = {ld_elems * (cuuint64_t)di.esz};
     cuuint32_t box[2] = {box_cols, box_rows};
     cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
+    CUresult r = enc(m, di.tma, 2, const_cast<void*>(base), dims, strides, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     LG_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(2d) failed (%d) rows=%llu cols=%llu ld=%llu box=%ux%u", (int)r,
@@ -235,10 +238,10 @@ int gemm_tc_ksplit(int M, int N, int K) {
 }
 
 bool gemm_tc_supported(int M, int N, int K, int dtype) {
-    return dtype == LG_DTYPE_BF16 && M >= 1 && K % 8 == 0 && N % 2 == 0;
+    return lg_dtype_is16(dtype) && M >= 1 && K % 8 == 0 && N % 2 == 0;
 }
 
-template <int RP>
+template <int RP, typename T>
 static int gemm_tc_launch_t(const CUtensorMap& mwa, const CUtensorMap& mwb, const CUtensorMap& mx, TcArgs& a, dim3 grid,
                             cudaStream_t st) {
     constexpr int b_tile_bytes = RP * kBlockK * 2;
@@ -251,17 +254,19 @@ static int gemm_tc_launch_t(const CUtensorMap& mwa, const CUtensorMap& mwb, cons
     const size_t smem = 1024 + (size_t)a.stages * stage_bytes + 2 * kMaxStages * sizeof(uint64_t);
     static DevOnce attr;
     if (lg_first_on_device(attr)) {
-        LG_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<RP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        LG_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<RP, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     }
     LG_REQUIRE(smem <= 227 * 1024, "gemm_tc: shared memory %zu too large", smem);
-    (void)lg_launch(gemm_tc_kernel<RP>, grid, dim3(kThreads), smem, st, mwa, mwb, mx, a);
+    (void)lg_launch(gemm_tc_kernel<RP, T>, grid, dim3(kThreads), smem, st, mwa, mwb, mx, a);
     LG_LAUNCH_CHECK();
     return 0;
 }
 
+template <typename T>
 static int gemm_tc_launch(const void* X, int ldx, const void* Wa, const void* Wb, int n_split, int M, int N, int K,
                           float* partial, int* ksplit_out, cudaStream_t st, const GemmNext* next) {
-    LG_REQUIRE(gemm_tc_supported(M, N, K, LG_DTYPE_BF16), "gemm_tc: unsupported shape %d %d %d", M, N, K);
+    constexpr int dt = ElemTraits<T>::dtype;
+    LG_REQUIRE(gemm_tc_supported(M, N, K, dt), "gemm_tc: unsupported shape %d %d %d", M, N, K);
     if (Wb == nullptr) { Wb = Wa; n_split = N; }
     LG_REQUIRE(n_split % kBlockN == 0 || n_split == N, "gemm_tc: weight segment boundary %d must be a multiple of %d", n_split, kBlockN);
     LG_REQUIRE(((uintptr_t)X & 15) == 0 && ((uintptr_t)Wa & 15) == 0 && ((uintptr_t)Wb & 15) == 0 && ldx % 8 == 0,
@@ -280,9 +285,9 @@ static int gemm_tc_launch(const void* X, int ldx, const void* Wa, const void* Wb
     if (ksplit_out) *ksplit_out = ks;
 
     CUtensorMap mwa, mwb, mx;
-    LG_TRY(tma::make_map_2d(&mwa, Wa, (uint64_t)std::min(n_split, N), (uint64_t)K, (uint64_t)K, kBlockN, kBlockK));
-    LG_TRY(tma::make_map_2d(&mwb, Wb, (uint64_t)std::max(N - n_split, Wb == Wa ? N : 1), (uint64_t)K, (uint64_t)K, kBlockN, kBlockK));
-    LG_TRY(tma::make_map_2d(&mx, X, (uint64_t)M, (uint64_t)K, (uint64_t)ldx, (uint32_t)rpad, kBlockK));   // rows >= M read as zero
+    LG_TRY(tma::make_map_2d(&mwa, Wa, (uint64_t)std::min(n_split, N), (uint64_t)K, (uint64_t)K, kBlockN, kBlockK, dt));
+    LG_TRY(tma::make_map_2d(&mwb, Wb, (uint64_t)std::max(N - n_split, Wb == Wa ? N : 1), (uint64_t)K, (uint64_t)K, kBlockN, kBlockK, dt));
+    LG_TRY(tma::make_map_2d(&mx, X, (uint64_t)M, (uint64_t)K, (uint64_t)ldx, (uint32_t)rpad, kBlockK, dt));   // rows >= M read as zero
 
     a.trace = g_tc_trace;
     a.whint = (lg_env_flag("LG_L2_HINT", 1) & 2) ? tma::kL2EvictLast : 0ull;
@@ -291,15 +296,17 @@ static int gemm_tc_launch(const void* X, int ldx, const void* Wa, const void* Wb
     a.pf1 = pf ? (const char*)next->p1 : nullptr; a.pfb1 = pf ? next->b1 : 0;
     const dim3 grid(cdiv(N, kBlockN), ks, zblocks);
     switch (rpad) {
-        case 16: return gemm_tc_launch_t<16>(mwa, mwb, mx, a, grid, st);
-        case 32: return gemm_tc_launch_t<32>(mwa, mwb, mx, a, grid, st);
-        case 64: return gemm_tc_launch_t<64>(mwa, mwb, mx, a, grid, st);
-        case 128: return gemm_tc_launch_t<128>(mwa, mwb, mx, a, grid, st);
-        default: return gemm_tc_launch_t<256>(mwa, mwb, mx, a, grid, st);
+        case 16: return gemm_tc_launch_t<16, T>(mwa, mwb, mx, a, grid, st);
+        case 32: return gemm_tc_launch_t<32, T>(mwa, mwb, mx, a, grid, st);
+        case 64: return gemm_tc_launch_t<64, T>(mwa, mwb, mx, a, grid, st);
+        case 128: return gemm_tc_launch_t<128, T>(mwa, mwb, mx, a, grid, st);
+        default: return gemm_tc_launch_t<256, T>(mwa, mwb, mx, a, grid, st);
     }
 }
 
-int gemm_tc_partial(const void* X, int ldx, const void* Wa, const void* Wb, int n_split, int M, int N, int K,
+int gemm_tc_partial(const void* X, int ldx, const void* Wa, const void* Wb, int n_split, int M, int N, int K, int dtype,
                     float* partial, int* ksplit_out, cudaStream_t st, const GemmNext* next) {
-    return gemm_tc_launch(X, ldx, Wa, Wb, n_split, M, N, K, partial, ksplit_out, st, next);
+    if (dtype == LG_DTYPE_F16) return gemm_tc_launch<f16>(X, ldx, Wa, Wb, n_split, M, N, K, partial, ksplit_out, st, next);
+    LG_REQUIRE(dtype == LG_DTYPE_BF16, "gemm_tc: unsupported dtype %d", dtype);
+    return gemm_tc_launch<bf16>(X, ldx, Wa, Wb, n_split, M, N, K, partial, ksplit_out, st, next);
 }

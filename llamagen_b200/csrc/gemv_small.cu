@@ -6,7 +6,7 @@
 // SwiGLU gate / fp32 store into the epilogue, and a layer is 5 dependent kernels
 //     qkv' (norm prologue) -> attention (fused RoPE + KV write, attn_tma.cu) -> wo' (+residual) -> w13' (norm, SwiGLU) -> w2' (+residual).
 //
-// Math: mma.sync m16n8k16 (bf16 x bf16 -> fp32), weights as the M operand (16 weight rows), activations as the N operand
+// Math: mma.sync m16n8k16 (bf16 x bf16 or fp16 x fp16 -> fp32), weights as the M operand (16 weight rows), activations as the N operand
 // (8 rows). Both operands are fetched with 128-bit loads: lane (g, t) loads 8 consecutive k of weight rows g / g+8 from
 // HBM and of activation row g from shared memory, and feeds registers {0,1} to one MMA and {2,3} to the next — the k
 // permutation this implies is the same on both operands, so the dot products are exact. The 8 warps of a CTA interleave
@@ -15,39 +15,34 @@
 // the programmatic-dependency wait.
 //
 // Rounding points are those of the batched path (xf_kernels.cu: residual_norm_kernel, silu_mul_kernel), i.e. of the
-// reference's bf16 tensors (gpt.py:143-148,167,255-256).
+// reference's bf16 / fp16 tensors (gpt.py:143-148,167,255-256).
 #include "kernels.cuh"
 
 namespace {
 
 constexpr int kWarps = 8, kThreads = 256;
 
+// 16-bit tensors of element type T (bf16 or f16)
+template <typename T>
 struct GemvArgs {
-    const bf16* Wa;        // [N][K]
-    const bf16* Wb;        // paired form (SwiGLU): second matrix [N][K], else null
+    const T* Wa;           // [N][K]
+    const T* Wb;           // paired form (SwiGLU): second matrix [N][K], else null
     int N, K, R;
     int pro;               // 0: x = in    1: x = rmsnorm(in) * normw
-    const bf16* in;        // [R][K]
-    const bf16* normw;     // [K]
+    const T* in;           // [R][K]
+    const T* normw;        // [K]
     float eps;
-    int epi;               // 0: out_f32[r][n] = acc   1: h[r][n] = bf(h + bf(acc))   2: ff[r][n] = bf(bf(silu(bf(a))) * bf(b))
+    int epi;               // 0: out_f32[r][n] = acc   1: h[r][n] = T(h + T(acc))   2: ff[r][n] = T(T(silu(T(a))) * T(b))
     float* out_f32;
-    bf16* h;
-    bf16* ff;
+    T* h;
+    T* ff;
 };
-
-__device__ __forceinline__ void mma16816(float* c, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
-
-__device__ __forceinline__ float bf_round(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
 
 // ROWS weight rows per CTA: 8 (upper half of one m16 tile), 16 (one tile) or 32 (two tiles; in the paired form tile 0 comes
 // from Wa and tile 1 from the same rows of Wb). PF = chunks of 32 k kept in flight per warp.
-template <int ROWS, int PF>
-__global__ void __launch_bounds__(kThreads) gemv_small_kernel(GemvArgs a) {
+template <int ROWS, int PF, typename T>
+__global__ void __launch_bounds__(kThreads) gemv_small_kernel(GemvArgs<T> a) {
+    using TR = ElemTraits<T>;
     constexpr int MT = ROWS == 32 ? 2 : 1;          // m16 tiles
     constexpr int HALVES = ROWS == 8 ? 1 : 2;       // row halves (g, g+8) loaded per tile
     extern __shared__ __align__(16) uint8_t smem[];
@@ -62,12 +57,12 @@ __global__ void __launch_bounds__(kThreads) gemv_small_kernel(GemvArgs a) {
     const int nchunks = K / 32;
     const int my_chunks = (nchunks - warp + kWarps - 1) / kWarps;     // chunks warp, warp+8, ...
 
-    const bf16* wrow[MT][HALVES];
+    const T* wrow[MT][HALVES];
 #pragma unroll
     for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
         for (int hh = 0; hh < HALVES; ++hh) {
-            const bf16* base = (a.Wb && mt == 1) ? a.Wb : a.Wa;
+            const T* base = (a.Wb && mt == 1) ? a.Wb : a.Wa;
             const int row = n0 + ((a.Wb || mt == 0) ? 0 : 16) + g + 8 * hh;
             wrow[mt][hh] = base + (size_t)row * K + t * 8;
         }
@@ -100,7 +95,7 @@ __global__ void __launch_bounds__(kThreads) gemv_small_kernel(GemvArgs a) {
     // residual epilogue: request this thread's h element now, it is only needed after the main loop
     const int ei = threadIdx.x >> 3, er = threadIdx.x & 7;
     float h_old = 0.f;
-    if (a.epi == 1 && er < R && ei < ROWS) h_old = __bfloat162float(a.h[(size_t)er * a.N + n0 + ei]);
+    if (a.epi == 1 && er < R && ei < ROWS) h_old = TR::to_f(a.h[(size_t)er * a.N + n0 + ei]);
 
     // ---------------------------------------------------------------- prologue: activations -> shared memory
     {
@@ -114,7 +109,7 @@ __global__ void __launch_bounds__(kThreads) gemv_small_kernel(GemvArgs a) {
                     const uint32_t w[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
                     for (int q = 0; q < 4; ++q) {
-                        const float lo = __uint_as_float(w[q] << 16), hi = __uint_as_float(w[q] & 0xffff0000u);
+                        const float lo = TR::lo(w[q]), hi = TR::hi(w[q]);
                         ss = fmaf(lo, lo, ss);
                         ss = fmaf(hi, hi, ss);
                     }
@@ -145,10 +140,9 @@ __global__ void __launch_bounds__(kThreads) gemv_small_kernel(GemvArgs a) {
 #pragma unroll
                     for (int q = 0; q < 4; ++q) {
                         // (x.float() * rsqrt(mean(x^2) + eps)).type_as(x) * weight   (gpt.py:143-148)
-                        const float lo = bf_round(__uint_as_float(w[q] << 16) * rinv) * __uint_as_float(n[q] << 16);
-                        const float hi = bf_round(__uint_as_float(w[q] & 0xffff0000u) * rinv) * __uint_as_float(n[q] & 0xffff0000u);
-                        __nv_bfloat162 pk = __floats2bfloat162_rn(lo, hi);
-                        o[q] = *reinterpret_cast<uint32_t*>(&pk);
+                        const float lo = TR::round(TR::lo(w[q]) * rinv) * TR::lo(n[q]);
+                        const float hi = TR::round(TR::hi(w[q]) * rinv) * TR::hi(n[q]);
+                        o[q] = TR::pack2(lo, hi);
                     }
                     *px = make_uint4(o[0], o[1], o[2], o[3]);
                 }
@@ -175,8 +169,8 @@ __global__ void __launch_bounds__(kThreads) gemv_small_kernel(GemvArgs a) {
                 for (int mt = 0; mt < MT; ++mt) {
                     const uint4 w0 = wbuf[s][mt][0];
                     const uint4 w1 = HALVES == 2 ? wbuf[s][mt][HALVES - 1] : make_uint4(0u, 0u, 0u, 0u);
-                    mma16816(acc[mt], w0.x, w1.x, w0.y, w1.y, xb.x, xb.y);
-                    mma16816(acc[mt], w0.z, w1.z, w0.w, w1.w, xb.z, xb.w);
+                    mma_m16n8k16<T>(acc[mt], w0.x, w1.x, w0.y, w1.y, xb.x, xb.y);
+                    mma_m16n8k16<T>(acc[mt], w0.z, w1.z, w0.w, w1.w, xb.z, xb.w);
                 }
             }
             load_chunk(s, it + PF);
@@ -201,10 +195,10 @@ __global__ void __launch_bounds__(kThreads) gemv_small_kernel(GemvArgs a) {
             av += red[((w * MT + 0) * 16 + i) * 8 + r];
             bv += red[((w * MT + (MT - 1)) * 16 + i) * 8 + r];
         }
-        av = bf_round(av);
-        bv = bf_round(bv);
-        const float sv = bf_round(av / (1.0f + expf(-av)));  // F.silu(w1 x) * w3 x in bf16 tensors (gpt.py:167)
-        a.ff[(size_t)r * a.N + n0 + i] = __float2bfloat16_rn(sv * bv);
+        av = TR::round(av);
+        bv = TR::round(bv);
+        const float sv = TR::round(av / (1.0f + expf(-av)));  // F.silu(w1 x) * w3 x in T tensors (gpt.py:167)
+        a.ff[(size_t)r * a.N + n0 + i] = TR::from_f(sv * bv);
         return;
     }
     if (i >= ROWS) return;
@@ -215,44 +209,49 @@ __global__ void __launch_bounds__(kThreads) gemv_small_kernel(GemvArgs a) {
     const size_t o = (size_t)r * a.N + n0 + i;
     if (a.epi == 0) {
         a.out_f32[o] = v;
-    } else {                                                 // h = x + f(x), both bf16 tensors (gpt.py:255-256)
-        a.h[o] = __float2bfloat16_rn(h_old + bf_round(v));
+    } else {                                                 // h = x + f(x), both T tensors (gpt.py:255-256)
+        a.h[o] = TR::from_f(h_old + TR::round(v));
     }
 }
 
-template <int ROWS, int PF>
-int launch_t(const GemvArgs& a, cudaStream_t st) {
+template <int ROWS, int PF, typename T>
+int launch_t(const GemvArgs<T>& a, cudaStream_t st) {
     constexpr int MT = ROWS == 32 ? 2 : 1;
     const size_t smem = (size_t)(kWarps * MT * 16 * 8 + 64) * sizeof(float) + (size_t)a.R * (a.K * 2 + 16);
     static DevOnce attr;
     if (lg_first_on_device(attr)) {
-        LG_CUDA_OK(cudaFuncSetAttribute(gemv_small_kernel<ROWS, PF>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+        LG_CUDA_OK(cudaFuncSetAttribute(gemv_small_kernel<ROWS, PF, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     }
     LG_REQUIRE(smem <= 100 * 1024, "gemv_small: %zu bytes of shared memory (R=%d K=%d)", smem, a.R, a.K);
     const int rows_per_cta = a.Wb ? 16 : ROWS;
-    (void)lg_launch(gemv_small_kernel<ROWS, PF>, dim3(a.N / rows_per_cta), dim3(kThreads), smem, st, a);
+    (void)lg_launch(gemv_small_kernel<ROWS, PF, T>, dim3(a.N / rows_per_cta), dim3(kThreads), smem, st, a);
     LG_LAUNCH_CHECK();
     return 0;
 }
 
-}  // namespace
-
-bool gemv_small_supported(int R, int N, int K, int dtype, bool paired) {
-    if (dtype != LG_DTYPE_BF16 || R < 1 || R > 8 || K % 32 != 0 || K < 256) return false;
-    if ((size_t)R * (K * 2 + 16) > 90 * 1024) return false;
-    return N % (paired ? 16 : 32) == 0;      // every row granularity used below divides N
-}
-
-int launch_gemv_small(const GemvSmall& g, cudaStream_t st) {
-    LG_REQUIRE(gemv_small_supported(g.R, g.N, g.K, LG_DTYPE_BF16, g.Wb != nullptr), "gemv_small: unsupported shape R=%d N=%d K=%d", g.R,
-               g.N, g.K);
-    GemvArgs a;
-    a.Wa = (const bf16*)g.Wa; a.Wb = (const bf16*)g.Wb; a.N = g.N; a.K = g.K; a.R = g.R;
-    a.pro = g.normw ? 1 : 0; a.in = (const bf16*)g.in; a.normw = (const bf16*)g.normw; a.eps = g.eps;
-    a.epi = g.Wb ? 2 : (g.out_f32 ? 0 : 1); a.out_f32 = g.out_f32; a.h = (bf16*)g.h; a.ff = (bf16*)g.ff;
+template <typename T>
+int launch_typed(const GemvSmall& g, cudaStream_t st) {
+    GemvArgs<T> a;
+    a.Wa = (const T*)g.Wa; a.Wb = (const T*)g.Wb; a.N = g.N; a.K = g.K; a.R = g.R;
+    a.pro = g.normw ? 1 : 0; a.in = (const T*)g.in; a.normw = (const T*)g.normw; a.eps = g.eps;
+    a.epi = g.Wb ? 2 : (g.out_f32 ? 0 : 1); a.out_f32 = g.out_f32; a.h = (T*)g.h; a.ff = (T*)g.ff;
     if (g.Wb) return launch_t<32, 4>(a, st);
     // Row granularity: enough CTAs to pull the matrix from all SMs (8 rows/CTA below ~2.4k outputs), fatter CTAs for the head
     if (g.N <= 2048) return launch_t<8, 12>(a, st);
     if (g.N <= 8192) return launch_t<16, 4>(a, st);
     return launch_t<32, 4>(a, st);
+}
+
+}  // namespace
+
+bool gemv_small_supported(int R, int N, int K, int dtype, bool paired) {
+    if (!lg_dtype_is16(dtype) || R < 1 || R > 8 || K % 32 != 0 || K < 256) return false;
+    if ((size_t)R * (K * 2 + 16) > 90 * 1024) return false;
+    return N % (paired ? 16 : 32) == 0;      // every row granularity used below divides N
+}
+
+int launch_gemv_small(const GemvSmall& g, cudaStream_t st) {
+    LG_REQUIRE(gemv_small_supported(g.R, g.N, g.K, g.dtype, g.Wb != nullptr), "gemv_small: unsupported shape R=%d N=%d K=%d dtype %d",
+               g.R, g.N, g.K, g.dtype);
+    return g.dtype == LG_DTYPE_F16 ? launch_typed<f16>(g, st) : launch_typed<bf16>(g, st);
 }

@@ -9,7 +9,8 @@ struct SampleArgs {
     const float* logits;   // [rows, V], cond rows first
     int B, V;
     int mix_cfg;           // rows == 2B and CFG mixing requested
-    int round_bf16;        // round raw logits to bf16 before use (bf16 head output, gpt.py:368)
+    int round_dtype;       // LG_DTYPE_BF16 / LG_DTYPE_F16: round raw logits to that type before use (16-bit head output,
+                           // gpt.py:368); LG_DTYPE_F32 (0): use them as they are
     float cfg_scale;
     int cfg_interval;
     float temperature;
@@ -31,10 +32,10 @@ struct SampleArgs {
     // continuous batching (lg_sample_rows): every image is its own request with its own RNG seed and token index
     const uint64_t* seed_rows = nullptr;   // [B] or null
     const int* step_rows = nullptr;        // [B] or null
-    // fused tail of a decode iteration (bf16 only): the CTA that picked image b's token also writes the next step's input rows b and
+    // fused tail of a decode iteration (16-bit models; rows in round_dtype): the CTA that picked image b's token also writes the next step's input rows b and
     // B + b (token embedding, gpt.py:352; optionally its RMSNorm for layer 0, gpt.py:143-148) and the last CTA to finish advances the
     // device-resident position / step counters - three dependent kernels (embed, rmsnorm, advance) fewer per token
-    const void* emb_table = nullptr;       // tok_embeddings [V][D] bf16 (null: no fused tail)
+    const void* emb_table = nullptr;       // tok_embeddings [V][D] (null: no fused tail)
     void* emb_h = nullptr;                 // [R][D] next step's residual stream
     void* emb_xn = nullptr;                // [R][D] RMSNorm(h) * norm_w, or null
     const void* emb_norm_w = nullptr;      // [D]
@@ -130,12 +131,13 @@ struct AttnArgs {
     const float* qkv_partial = nullptr; int qkv_ksplit = 0; const float* freqs = nullptr;
 };
 int launch_attention(const AttnArgs& a, cudaStream_t st);
-// attn_tma.cu — TMA + tensor-core decode attention for bf16 caches
-int attn_tma_make_map(void* map_out /*CUtensorMap, 128 B*/, const void* cache_base, long long total_rows, int hdp, int tail16 = 0);
+// attn_tma.cu — TMA + tensor-core decode attention for bf16 / fp16 caches (dtype: LG_DTYPE_BF16 or LG_DTYPE_F16)
+int attn_tma_make_map(void* map_out /*CUtensorMap, 128 B*/, const void* cache_base, long long total_rows, int hdp, int dtype,
+                      int tail16 = 0);
 bool attn_tma_supported(const AttnArgs& a);
 bool attn_tma_enabled();
 int launch_attention_tma(const AttnArgs& a, cudaStream_t st);
-// t2i condition prefill (1 < Tq <= 128, hd 64, bf16): TMA-staged Q/K/V, mma.sync QK^T and PV, one CTA per (row, head)
+// t2i condition prefill (1 < Tq <= 128, hd 64, bf16 / fp16): TMA-staged Q/K/V, mma.sync QK^T and PV, one CTA per (row, head)
 bool attn_prefill_tc_supported(const AttnArgs& a);
 int launch_attention_prefill_tc(const AttnArgs& a, cudaStream_t st);
 // conv_tc.cu — wgmma implicit-GEMM convolution over bf16 NHWC activations (TMA 4-D boxes, register accumulators)
@@ -147,10 +149,10 @@ int launch_conv_tc(const bf16* in, int B, int Hin, int Win, int Cin, const bf16*
                    float* gn_partial = nullptr, size_t gn_floats = 0, int* gn_splits = nullptr,    // *gn_splits > 0: the drain also wrote the
                    int* path = nullptr);   // output's GroupNorm(32) partial statistics [B][*gn_splits][32][2] into gn_partial;
                                            // *path: 1 = conv_tc_kernel, 2 = conv_tcw_kernel was launched
-// gemm_tc.cu — wgmma/TMA weight-streaming GEMM (bf16, row blocks of <= 256)
+// gemm_tc.cu — wgmma/TMA weight-streaming GEMM (bf16 or fp16, row blocks of <= 256)
 int gemm_tc_ksplit(int M, int N, int K);
 bool gemm_tc_supported(int M, int N, int K, int dtype);
-int gemm_tc_partial(const void* X, int ldx, const void* Wa, const void* Wb, int n_split, int M, int N, int K,
+int gemm_tc_partial(const void* X, int ldx, const void* Wa, const void* Wb, int n_split, int M, int N, int K, int dtype,
                     float* partial, int* ksplit_out, cudaStream_t st, const GemmNext* next = nullptr);
 
 // gemm_dx.cu — "direct" wgmma GEMM of the decode step: (feature tile) x (row block) CTAs over the FULL K (no split-K slab), the
@@ -172,11 +174,12 @@ int launch_gemm_dx(const GemmDx& g, cudaStream_t st, const GemmNext* next = null
 // gemv_small.cu — decode GEMMs for R <= 8 rows: CTA-owned output columns (no split-K), RMSNorm in the prologue (normw != null),
 // epilogue by destination: out_f32 [R][N] | h (in-place residual add) | ff (SwiGLU gate of the Wa/Wb row pair)
 struct GemvSmall {
-    const void* Wa; const void* Wb;   // [N][K] bf16; Wb only for the paired (w1 | w3) form
+    const void* Wa; const void* Wb;   // [N][K]; Wb only for the paired (w1 | w3) form
     int N, K, R;
-    const void* in;                   // [R][K] bf16
+    const void* in;                   // [R][K]
     const void* normw; float eps;     // RMSNorm weight [K] or null
     float* out_f32; void* h; void* ff;
+    int dtype;                        // LG_DTYPE_BF16 or LG_DTYPE_F16: every 16-bit tensor above
 };
 bool gemv_small_supported(int R, int N, int K, int dtype, bool paired);
 int launch_gemv_small(const GemvSmall& g, cudaStream_t st);

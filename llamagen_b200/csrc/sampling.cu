@@ -31,7 +31,10 @@ __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
     return x ^ (x >> 31);
 }
 
+// E: the 16-bit type of the rounding (a.round_dtype != LG_DTYPE_F32) and of the fused tail's rows
+template <typename E>
 __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
+    using TR = ElemTraits<E>;
     lg_pdl_sync();
     extern __shared__ float sh[];  // V floats: the working logits row, later exp() values
     __shared__ float red[33];
@@ -57,9 +60,9 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
     float* dbg = a.dbg_logits ? a.dbg_logits + ((size_t)step * dbgB + a.row_offset + b) * V : nullptr;
 
     auto mix1 = [&](float c, float u) -> float {
-        if (a.round_bf16) c = round_bf16(c);
+        if (a.round_dtype) c = TR::round(c);
         if (!mix) return c;
-        if (a.round_bf16) u = round_bf16(u);
+        if (a.round_dtype) u = TR::round(u);
         return __fadd_rn(u, __fmul_rn(__fsub_rn(c, u), a.cfg_scale));
     };
     if ((V & 3) == 0) {
@@ -412,12 +415,12 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
     if (a.emb_table) {
         __syncthreads();
         const int D = a.emb_D;
-        const bf16* src = reinterpret_cast<const bf16*>(a.emb_table) + (size_t)s_next * D;
+        const E* src = reinterpret_cast<const E*>(a.emb_table) + (size_t)s_next * D;
         // thread -> 2 consecutive elements per pass (D even); the same token feeds the cond and the uncond row (generate.py:91)
         for (int i = tid * 2; i < D; i += kSampleThreads * 2) {
             const uint32_t w = *reinterpret_cast<const uint32_t*>(src + i);
             for (int row = b; row < a.emb_rows; row += B)
-                *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(a.emb_h) + (size_t)row * D + i) = w;
+                *reinterpret_cast<uint32_t*>(reinterpret_cast<E*>(a.emb_h) + (size_t)row * D + i) = w;
         }
         if (a.emb_xn) {
             // sum of squares in rmsnorm_kernel's order (256 threads striding the row, then the same block reduction tree: the other
@@ -425,21 +428,21 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
             float ss = 0.f;
             if (tid < 256)
                 for (int i = tid; i < D; i += 256) {
-                    const float v = __bfloat162float(src[i]);
+                    const float v = TR::to_f(src[i]);
                     ss = fmaf(v, v, ss);
                 }
             const float tot = block_sum(ss, red);
             const float rinv = 1.0f / sqrtf(tot / (float)D + a.emb_eps);
-            const bf16* nw = reinterpret_cast<const bf16*>(a.emb_norm_w);
+            const E* nw = reinterpret_cast<const E*>(a.emb_norm_w);
             for (int i = tid * 2; i < D; i += kSampleThreads * 2) {
                 const uint32_t w = *reinterpret_cast<const uint32_t*>(src + i);
                 const uint32_t g2 = *reinterpret_cast<const uint32_t*>(nw + i);
-                // norm(x.float()).type_as(x) * weight: two bf16 roundings, as rmsnorm_kernel / residual_norm_kernel
-                const float lo = round_bf16(__uint_as_float(w << 16) * rinv) * __uint_as_float(g2 << 16);
-                const float hi = round_bf16(__uint_as_float(w & 0xffff0000u) * rinv) * __uint_as_float(g2 & 0xffff0000u);
-                __nv_bfloat162 pk = __floats2bfloat162_rn(lo, hi);
+                // norm(x.float()).type_as(x) * weight: two E roundings, as rmsnorm_kernel / residual_norm_kernel
+                const float lo = TR::round(TR::lo(w) * rinv) * TR::lo(g2);
+                const float hi = TR::round(TR::hi(w) * rinv) * TR::hi(g2);
+                const uint32_t pk = TR::pack2(lo, hi);
                 for (int row = b; row < a.emb_rows; row += B)
-                    *reinterpret_cast<__nv_bfloat162*>(reinterpret_cast<bf16*>(a.emb_xn) + (size_t)row * D + i) = pk;
+                    *reinterpret_cast<uint32_t*>(reinterpret_cast<E*>(a.emb_xn) + (size_t)row * D + i) = pk;
             }
         }
     }
@@ -464,11 +467,15 @@ int launch_sample(const SampleArgs& a, cudaStream_t st) {
     LG_REQUIRE(a.B > 0 && a.V > 0, "lg_sample: bad shape B=%d V=%d", a.B, a.V);
     const size_t smem = (size_t)a.V * sizeof(float);
     LG_REQUIRE(smem <= 200 * 1024, "lg_sample: vocab %d too large for the shared-memory row stage", a.V);
-    static DevOnce attr_set;
-    if (lg_first_on_device(attr_set)) {
-        LG_CUDA_OK(cudaFuncSetAttribute(sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    LG_REQUIRE(a.round_dtype == LG_DTYPE_F32 || lg_dtype_is16(a.round_dtype), "lg_sample: unsupported round dtype %d", a.round_dtype);
+    LG_REQUIRE(!a.emb_table || a.round_dtype != LG_DTYPE_F32, "lg_sample: the fused tail needs a 16-bit round dtype");
+    const bool half = a.round_dtype == LG_DTYPE_F16;
+    auto kern = half ? sample_kernel<f16> : sample_kernel<bf16>;
+    static DevOnce attr_set[2];
+    if (lg_first_on_device(attr_set[half])) {
+        LG_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     }
-    (void)lg_launch(sample_kernel, dim3(a.B), dim3(kSampleThreads), smem, st, a);
+    (void)lg_launch(kern, dim3(a.B), dim3(kSampleThreads), smem, st, a);
     LG_LAUNCH_CHECK();
     return 0;
 }

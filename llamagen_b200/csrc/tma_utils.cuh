@@ -74,10 +74,10 @@ __device__ __forceinline__ void load_4d(void* smem_dst, const CUtensorMap* map, 
         : "memory");
 }
 
-// host: 2-D bf16 row-major [rows, cols] (cols contiguous, `ld_elems` between rows); box [box_rows, box_cols];
-// 128-byte swizzle (box_cols * 2 bytes must be <= 128); out-of-bounds elements read as zero.
+// host: 2-D row-major [rows, cols] of a 16-bit LG_DTYPE_* (bf16 or fp16; cols contiguous, `ld_elems` between rows); box
+// [box_rows, box_cols]; 128-byte swizzle (box_cols * 2 bytes must be <= 128); out-of-bounds elements read as zero.
 int make_map_2d(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, uint32_t box_rows,
-                uint32_t box_cols);
+                uint32_t box_cols, int dtype = LG_DTYPE_BF16);
 // host: 4-D bf16 NHWC activation [B, H, W, C]; box [1, box_h, box_w, box_c]; 128-byte swizzle; OOB -> zero
 // (signed start coordinates give the conv's zero padding for free).
 int make_map_nhwc(CUtensorMap* m, const void* base, uint64_t B, uint64_t H, uint64_t W, uint64_t C, uint32_t box_h,

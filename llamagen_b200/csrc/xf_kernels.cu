@@ -104,6 +104,12 @@ template <> __device__ __forceinline__ void store4<bf16>(bf16* p, float a, float
     u.y = *reinterpret_cast<uint32_t*>(&hi);
     *reinterpret_cast<uint2*>(p) = u;
 }
+template <> __device__ __forceinline__ void store4<f16>(f16* p, float a, float b, float c, float d) {
+    uint2 u;
+    u.x = ElemTraits<f16>::pack2(a, b);
+    u.y = ElemTraits<f16>::pack2(c, d);
+    *reinterpret_cast<uint2*>(p) = u;
+}
 template <typename T> __device__ __forceinline__ void load4(const T* p, float* o) { VecLoad<T, 4>::load(p, o); }
 
 // One CTA per row, one thread per 4 consecutive output features (two RoPE pairs), all loads up front.
@@ -337,10 +343,12 @@ __global__ void set_counters_kernel(int* pos, int pv, int* step, int sv) {
     if (step) *step = sv;
 }
 
-template <typename F32, typename BF>
-int dispatch_dtype(int dtype, F32 f32, BF bf) {
-    if (dtype == LG_DTYPE_F32) return f32();
-    if (dtype == LG_DTYPE_BF16) return bf();
+// f is called with a value of the element type: f(T{}) for T = float, bf16 or f16
+template <typename F>
+int dispatch_dtype(int dtype, F f) {
+    if (dtype == LG_DTYPE_F32) return f(float{});
+    if (dtype == LG_DTYPE_BF16) return f(bf16{});
+    if (dtype == LG_DTYPE_F16) return f(f16{});
     return lg_fail("unsupported dtype %d", dtype);
 }
 
@@ -349,48 +357,66 @@ int dispatch_dtype(int dtype, F32 f32, BF bf) {
 int launch_embed(const void* table, const int32_t* src, int B, int R, int null_idx, int D, int dtype, void* out,
                  cudaStream_t st) {
     return dispatch_dtype(
-        dtype,
-        [&] { (void)lg_launch(embed_kernel<float>, dim3(R), dim3(128), 0, st, (const float*)table, src, B, null_idx, D, (float*)out); LG_LAUNCH_CHECK(); return 0; },
-        [&] { (void)lg_launch(embed_kernel<bf16>, dim3(R), dim3(128), 0, st, (const bf16*)table, src, B, null_idx, D, (bf16*)out); LG_LAUNCH_CHECK(); return 0; });
+        dtype, [&](auto z) {
+            using E = decltype(z);
+            (void)lg_launch(embed_kernel<E>, dim3(R), dim3(128), 0, st, (const E*)table, src, B, null_idx, D, (E*)out);
+            LG_LAUNCH_CHECK();
+            return 0;
+        });
 }
 
 int launch_embed_rows(const void* cls_table, const void* tok_table, const int32_t* src, const int* pos_rows, int B, int R, int null_idx,
                       int D, int dtype, void* out, cudaStream_t st) {
     return dispatch_dtype(
-        dtype,
-        [&] { (void)lg_launch(embed_rows_kernel<float>, dim3(R), dim3(128), 0, st, (const float*)cls_table, (const float*)tok_table, src, pos_rows, B, null_idx, D, (float*)out); LG_LAUNCH_CHECK(); return 0; },
-        [&] { (void)lg_launch(embed_rows_kernel<bf16>, dim3(R), dim3(128), 0, st, (const bf16*)cls_table, (const bf16*)tok_table, src, pos_rows, B, null_idx, D, (bf16*)out); LG_LAUNCH_CHECK(); return 0; });
+        dtype, [&](auto z) {
+            using E = decltype(z);
+            (void)lg_launch(embed_rows_kernel<E>, dim3(R), dim3(128), 0, st, (const E*)cls_table, (const E*)tok_table, src, pos_rows, B, null_idx, D, (E*)out);
+            LG_LAUNCH_CHECK();
+            return 0;
+        });
 }
 
 int launch_build_caption_rows(const void* cond, const void* uncond, int B, int R, int T, int C, int dtype, void* out,
                               cudaStream_t st) {
     return dispatch_dtype(
-        dtype,
-        [&] { (void)lg_launch(caption_rows_kernel<float>, dim3(R * T), dim3(128), 0, st, (const float*)cond, (const float*)uncond, B, T, C, (float*)out); LG_LAUNCH_CHECK(); return 0; },
-        [&] { (void)lg_launch(caption_rows_kernel<bf16>, dim3(R * T), dim3(128), 0, st, (const bf16*)cond, (const bf16*)uncond, B, T, C, (bf16*)out); LG_LAUNCH_CHECK(); return 0; });
+        dtype, [&](auto z) {
+            using E = decltype(z);
+            (void)lg_launch(caption_rows_kernel<E>, dim3(R * T), dim3(128), 0, st, (const E*)cond, (const E*)uncond, B, T, C, (E*)out);
+            LG_LAUNCH_CHECK();
+            return 0;
+        });
 }
 
 int launch_gather_last(const void* in, int R, int T, int D, int dtype, void* out, cudaStream_t st) {
     return dispatch_dtype(
-        dtype,
-        [&] { (void)lg_launch(gather_last_kernel<float>, dim3(R), dim3(128), 0, st, (const float*)in, T, D, (float*)out); LG_LAUNCH_CHECK(); return 0; },
-        [&] { (void)lg_launch(gather_last_kernel<bf16>, dim3(R), dim3(128), 0, st, (const bf16*)in, T, D, (bf16*)out); LG_LAUNCH_CHECK(); return 0; });
+        dtype, [&](auto z) {
+            using E = decltype(z);
+            (void)lg_launch(gather_last_kernel<E>, dim3(R), dim3(128), 0, st, (const E*)in, T, D, (E*)out);
+            LG_LAUNCH_CHECK();
+            return 0;
+        });
 }
 
 int launch_rmsnorm(const void* x, const void* w, void* xn, int M, int D, float eps, int dtype, cudaStream_t st) {
     return dispatch_dtype(
-        dtype,
-        [&] { (void)lg_launch(rmsnorm_kernel<float>, dim3(M), dim3(256), 0, st, (const float*)x, (const float*)w, (float*)xn, D, eps); LG_LAUNCH_CHECK(); return 0; },
-        [&] { (void)lg_launch(rmsnorm_kernel<bf16>, dim3(M), dim3(256), 0, st, (const bf16*)x, (const bf16*)w, (bf16*)xn, D, eps); LG_LAUNCH_CHECK(); return 0; });
+        dtype, [&](auto z) {
+            using E = decltype(z);
+            (void)lg_launch(rmsnorm_kernel<E>, dim3(M), dim3(256), 0, st, (const E*)x, (const E*)w, (E*)xn, D, eps);
+            LG_LAUNCH_CHECK();
+            return 0;
+        });
 }
 
 int launch_qkv_epilogue(const QkvEpiArgs& a, cudaStream_t st) {
     LG_REQUIRE(a.hd % 4 == 0 && a.D % 4 == 0, "head_dim %d / dim %d must be multiples of 4", a.hd, a.D);
     const int threads = std::min(1024, ((3 * a.D / 4 + 31) / 32) * 32);
     return dispatch_dtype(
-        a.dtype,
-        [&] { (void)lg_launch(qkv_epilogue_kernel<float>, dim3(a.M), dim3(threads), 0, st, a); LG_LAUNCH_CHECK(); return 0; },
-        [&] { (void)lg_launch(qkv_epilogue_kernel<bf16>, dim3(a.M), dim3(threads), 0, st, a); LG_LAUNCH_CHECK(); return 0; });
+        a.dtype, [&](auto z) {
+            using E = decltype(z);
+            (void)lg_launch(qkv_epilogue_kernel<E>, dim3(a.M), dim3(threads), 0, st, a);
+            LG_LAUNCH_CHECK();
+            return 0;
+        });
 }
 
 int launch_residual_norm(const float* partial, int ksplit, int M, int D, void* h, const void* norm_w, void* xn,
@@ -398,27 +424,36 @@ int launch_residual_norm(const float* partial, int ksplit, int M, int D, void* h
     LG_REQUIRE(D % 4 == 0 && D <= 4096, "dim %d must be a multiple of 4 and <= 4096", D);
     const int threads = ((D / 4 + 31) / 32) * 32;
     return dispatch_dtype(
-        dtype,
-        [&] { (void)lg_launch(residual_norm_kernel<float>, dim3(M), dim3(threads), 0, st, partial, ksplit, M, D, (float*)h, (const float*)norm_w, (float*)xn, eps); LG_LAUNCH_CHECK(); return 0; },
-        [&] { (void)lg_launch(residual_norm_kernel<bf16>, dim3(M), dim3(threads), 0, st, partial, ksplit, M, D, (bf16*)h, (const bf16*)norm_w, (bf16*)xn, eps); LG_LAUNCH_CHECK(); return 0; });
+        dtype, [&](auto z) {
+            using E = decltype(z);
+            (void)lg_launch(residual_norm_kernel<E>, dim3(M), dim3(threads), 0, st, partial, ksplit, M, D, (E*)h, (const E*)norm_w, (E*)xn, eps);
+            LG_LAUNCH_CHECK();
+            return 0;
+        });
 }
 
 int launch_silu_mul(const float* partial, int ksplit, int M, int F, void* out, int dtype, cudaStream_t st) {
     LG_REQUIRE(F % 4 == 0, "ffn dim %d must be a multiple of 4", F);
     const int blocks = (int)std::min<long long>(((long long)M * F / 4 + 255) / 256, 132 * 16);
     return dispatch_dtype(
-        dtype,
-        [&] { (void)lg_launch(silu_mul_kernel<float>, dim3(blocks), dim3(256), 0, st, partial, ksplit, M, F, (float*)out); LG_LAUNCH_CHECK(); return 0; },
-        [&] { (void)lg_launch(silu_mul_kernel<bf16>, dim3(blocks), dim3(256), 0, st, partial, ksplit, M, F, (bf16*)out); LG_LAUNCH_CHECK(); return 0; });
+        dtype, [&](auto z) {
+            using E = decltype(z);
+            (void)lg_launch(silu_mul_kernel<E>, dim3(blocks), dim3(256), 0, st, partial, ksplit, M, F, (E*)out);
+            LG_LAUNCH_CHECK();
+            return 0;
+        });
 }
 
 int launch_store_act(const float* partial, int ksplit, int M, int N, void* out, int gelu, int dtype, cudaStream_t st) {
     const size_t total = (size_t)M * N;
     const int blocks = (int)std::min<size_t>((total + 255) / 256, 132 * 16);
     return dispatch_dtype(
-        dtype,
-        [&] { (void)lg_launch(store_act_kernel<float>, dim3(blocks), dim3(256), 0, st, partial, ksplit, total, gelu, (float*)out); LG_LAUNCH_CHECK(); return 0; },
-        [&] { (void)lg_launch(store_act_kernel<bf16>, dim3(blocks), dim3(256), 0, st, partial, ksplit, total, gelu, (bf16*)out); LG_LAUNCH_CHECK(); return 0; });
+        dtype, [&](auto z) {
+            using E = decltype(z);
+            (void)lg_launch(store_act_kernel<E>, dim3(blocks), dim3(256), 0, st, partial, ksplit, total, gelu, (E*)out);
+            LG_LAUNCH_CHECK();
+            return 0;
+        });
 }
 
 int launch_reduce_f32(const float* partial, int ksplit, int M, int N, float* out, cudaStream_t st) {
@@ -445,12 +480,17 @@ int launch_attention(const AttnArgs& a, cudaStream_t st) {
     if (attn_prefill_tc_supported(a) && attn_tma_enabled() && a.qkv_partial == nullptr) return launch_attention_prefill_tc(a, st);
     LG_REQUIRE(a.qkv_partial == nullptr, "attention: fused QKV epilogue requested on a path that does not support it");
     LG_REQUIRE((long long)a.R * a.Tq <= 65535, "attention: too many query rows (%d x %d)", a.R, a.Tq);
-    LG_REQUIRE(a.hdp == 0 || a.hdp == a.hd || (a.hd == 100 && a.hdp == 112 && a.dtype == LG_DTYPE_BF16), "attention: unsupported KV row stride %d for head_dim %d", a.hdp, a.hd);
+    LG_REQUIRE(a.hdp == 0 || a.hdp == a.hd || (a.hd == 100 && a.hdp == 112 && lg_dtype_is16(a.dtype)), "attention: unsupported KV row stride %d for head_dim %d", a.hdp, a.hd);
     if (a.dtype == LG_DTYPE_BF16) {
         if (a.hd == 64) return launch_attention_t<bf16, 64, 8, 8>(a, st);
         if (a.hd == 128) return launch_attention_t<bf16, 128, 8, 16>(a, st);
         if (a.hd == 100 && a.hdp == 112) return launch_attention_t<bf16, 100, 4, 32, 112>(a, st);
         if (a.hd == 100) return launch_attention_t<bf16, 100, 4, 32>(a, st);
+    } else if (a.dtype == LG_DTYPE_F16) {
+        if (a.hd == 64) return launch_attention_t<f16, 64, 8, 8>(a, st);
+        if (a.hd == 128) return launch_attention_t<f16, 128, 8, 16>(a, st);
+        if (a.hd == 100 && a.hdp == 112) return launch_attention_t<f16, 100, 4, 32, 112>(a, st);
+        if (a.hd == 100) return launch_attention_t<f16, 100, 4, 32>(a, st);
     } else if (a.dtype == LG_DTYPE_F32) {
         if (a.hd == 64) return launch_attention_t<float, 64, 8, 8>(a, st);
         if (a.hd == 128) return launch_attention_t<float, 128, 8, 16>(a, st);

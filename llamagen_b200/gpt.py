@@ -168,15 +168,13 @@ class Transformer(nn.Module):
         """Create / refresh the C engine for the parameters' current device + dtype."""
         p = self.tok_embeddings.weight
         _lib.require_cuda(p, "Transformer.engine")
-        if p.dtype not in (torch.float32, torch.bfloat16):
-            raise _lib.LgError(f"unsupported precision {p.dtype}: the sm_90a engine implements bf16 and fp32")
+        dt = _lib.dtype_code(p.dtype)   # fp32, bf16 or fp16; raises for anything else
         sig = self._signature()
         if self._engine is not None and sig == self._engine_sig:
             return self._engine
         self._drop_engine()
         lib = _lib.load()
         c = self.config
-        dt = _lib.LG_DTYPE_BF16 if p.dtype == torch.bfloat16 else _lib.LG_DTYPE_F32
         cfg = _lib.ModelCfg(c.n_layer, c.n_head, c.dim, c.ffn_dim, c.vocab_size, c.cls_token_num, c.block_size,
                             c.num_classes, c.caption_dim,
                             _lib.LG_MODEL_C2I if c.model_type == "c2i" else _lib.LG_MODEL_T2I, dt, c.norm_eps)
@@ -187,7 +185,7 @@ class Transformer(nn.Module):
         for name, t in self.state_dict().items():
             if not t.is_contiguous():
                 raise _lib.LgError(f"parameter {name} must be contiguous")
-            t_dt = _lib.LG_DTYPE_BF16 if t.dtype == torch.bfloat16 else _lib.LG_DTYPE_F32
+            t_dt = _lib.dtype_code(t.dtype)
             _lib.check(lib.lg_engine_bind_weight(handle, name.encode(), _lib.ptr(t), _lib.shape_array(t.shape),
                                                  t.dim(), t_dt), f"bind {name}")
         self.freqs_cis = self.freqs_cis.to(device=p.device, dtype=torch.float32).contiguous()

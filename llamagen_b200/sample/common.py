@@ -31,8 +31,6 @@ def load_vq(args, device):
 
 def load_gpt(args, device, latent_size):
     precision = {"none": torch.float32, "bf16": torch.bfloat16, "fp16": torch.float16}[args.precision]
-    if precision == torch.float16:
-        raise SystemExit("--precision fp16 is not implemented by the sm_90a engine; use bf16 (default) or none (fp32)")
     gpt_model = GPT_models[args.gpt_model](
         vocab_size=args.codebook_size, block_size=latent_size ** 2, num_classes=args.num_classes,
         cls_token_num=args.cls_token_num, model_type=args.gpt_type).to(device=device, dtype=precision)

@@ -130,7 +130,7 @@ class LLM:
         _lib.check(lib.lg_decode_rows(handle, _lib.ptr(st["tok"]), _lib.ptr(st["pos"]), B, use_cfg, _lib.ptr(st["logits"]), stream),
                    "lg_decode_rows")
         sc = _lib.SampleCfg(self.cfg_scale, -1, float(params.temperature), max(0, int(params.top_k)), float(params.top_p), 0, 0)
-        dt = _lib.LG_DTYPE_BF16 if self.model.tok_embeddings.weight.dtype == torch.bfloat16 else _lib.LG_DTYPE_F32
+        dt = _lib.dtype_code(self.model.tok_embeddings.weight.dtype)   # 16-bit models round the head's logits to their dtype
         _lib.check(lib.lg_sample_rows(_lib.ptr(st["logits"]), B, self.model.vocab_size, use_cfg, dt, ctypes.byref(sc),
                                       _lib.ptr(st["seeds"]), _lib.ptr(st["pos"]), _lib.ptr(st["tok"]), _lib.ptr(st["out"]), S, stream),
                    "lg_sample_rows")
