@@ -32,7 +32,8 @@ extern "C" {
 #define LG_ABI_VERSION 1
 
 /* LG_DTYPE_F16 (IEEE half) runs the same tensor-core kernels as LG_DTYPE_BF16; values past +-65504 become +-inf, as in torch. */
-enum { LG_DTYPE_F32 = 0, LG_DTYPE_BF16 = 1, LG_DTYPE_F16 = 2 };
+/* LG_DTYPE_E4M3 (fp8 e4m3, finite, max +-448) is a KV-cache storage type only (lg_engine_set_kv_cache); never a model dtype. */
+enum { LG_DTYPE_F32 = 0, LG_DTYPE_BF16 = 1, LG_DTYPE_F16 = 2, LG_DTYPE_E4M3 = 3 };
 enum { LG_MODEL_C2I = 0, LG_MODEL_T2I = 1 };
 
 /* Mirrors autoregressive/models/gpt.py:23-50 (ModelArgs) — only the fields the inference path reads. */
@@ -85,6 +86,13 @@ int  lg_engine_finalize(lg_engine* e);
  * of up to max_seq positions (cls_token_num + new tokens). Replaces setup_caches (gpt.py:316-330). */
 int  lg_engine_workspace_bytes(lg_engine* e, int rows, int max_seq, size_t* bytes);
 int  lg_engine_set_workspace(lg_engine* e, void* dev_ws, size_t bytes, int rows, int max_seq);
+/* KV-cache storage of a bf16 / fp16 model. kv_dtype = LG_DTYPE_E4M3 stores K and V as fp8 e4m3 (one byte per element, half
+ * the cache bytes): the stored byte is e4m3_satfinite_rne(x / s) of the model-dtype value x (K after RoPE), and every read,
+ * including the current step's own key and value, sees e4m3 * s. scales: host float [n_layer][2] = (k, v) per layer, each a
+ * power of two in [2^-8, 2^7], or NULL for all 1.0. kv_dtype = the model's dtype restores the default 16-bit cache.
+ * Call after lg_engine_create / lg_engine_finalize and before lg_engine_workspace_bytes / lg_engine_set_workspace: the call
+ * drops the workspace, so compute calls fail until lg_engine_set_workspace runs again. fp32 models are refused. */
+int  lg_engine_set_kv_cache(lg_engine* e, int kv_dtype, const float* scales);
 
 /* Prefill over the condition (generate.py:77-86 / gpt.py:348-349).
  *  c2i: cond = dev int32 [B] class labels.      t2i: cond = dev [B, T, caption_dim] features (cfg.dtype),

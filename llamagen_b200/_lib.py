@@ -14,6 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("LG_LIB_PATH") or os.path.join(HERE, "lib", "libllamagen_b200.so")
 
 LG_DTYPE_F32, LG_DTYPE_BF16, LG_DTYPE_F16 = 0, 1, 2
+LG_DTYPE_E4M3 = 3   # fp8 e4m3: KV-cache storage only (lg_engine_set_kv_cache)
 LG_MODEL_C2I, LG_MODEL_T2I = 0, 1
 
 
@@ -60,6 +61,7 @@ SIGNATURES = {
     "lg_engine_finalize": (c_int, [c_void_p]),
     "lg_engine_workspace_bytes": (c_int, [c_void_p, c_int, c_int, POINTER(c_size_t)]),
     "lg_engine_set_workspace": (c_int, [c_void_p, c_void_p, c_size_t, c_int, c_int]),
+    "lg_engine_set_kv_cache": (c_int, [c_void_p, c_int, POINTER(c_float)]),
     "lg_prefill": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "lg_decode_step": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "lg_decode_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+#include <cuda_fp8.h>
 #include <cuda.h>
 #include <stdint.h>
 #include <string>
@@ -23,6 +24,7 @@ struct DtypeInfo {
 inline DtypeInfo lg_dtype_info(int dtype) {
     if (dtype == LG_DTYPE_F16) return {2, CU_TENSOR_MAP_DATA_TYPE_FLOAT16};
     if (dtype == LG_DTYPE_BF16) return {2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16};
+    if (dtype == LG_DTYPE_E4M3) return {1, CU_TENSOR_MAP_DATA_TYPE_UINT8};   // fp8 KV cache: raw bytes, decoded in registers
     return {4, CU_TENSOR_MAP_DATA_TYPE_FLOAT32};
 }
 // bf16 and fp16 share every tensor-core kernel (same shared-memory layouts and MMA rates on sm_90a)
@@ -172,6 +174,30 @@ template <> struct ElemTraits<f16> {
 
 __device__ __forceinline__ float round_bf16(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
 
+// ---------------------------------------------------------------------------------------------
+// fp8 e4m3 KV cache (LG_DTYPE_E4M3): one instruction each way on sm_90a. Every e4m3 value is exact in fp16 and in bf16.
+// ---------------------------------------------------------------------------------------------
+typedef __nv_fp8_e4m3 e4m3;   // storage tag of the fp8 cache (1 byte)
+// (a, b) -> two e4m3 bytes, a in the low byte: clamp to +-448 (inf too), round to nearest even
+__device__ __forceinline__ uint32_t e4m3x2_pack(float a, float b) {
+    uint16_t r;
+    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(b), "f"(a));
+    return r;
+}
+// two e4m3 bytes (low 16 bits of v) -> f16x2, the low byte in the low half
+__device__ __forceinline__ uint32_t e4m3x2_to_f16x2(uint32_t v) {
+    uint32_t r;
+    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(r) : "h"((uint16_t)v));
+    return r;
+}
+// two e4m3 bytes -> a packed pair of T (bf16 widens through fp32, exactly)
+template <typename T> __device__ __forceinline__ uint32_t e4m3x2_to(uint32_t v);
+template <> __device__ __forceinline__ uint32_t e4m3x2_to<f16>(uint32_t v) { return e4m3x2_to_f16x2(v); }
+template <> __device__ __forceinline__ uint32_t e4m3x2_to<bf16>(uint32_t v) {
+    const uint32_t h = e4m3x2_to_f16x2(v);
+    return ElemTraits<bf16>::pack2(ElemTraits<f16>::lo(h), ElemTraits<f16>::hi(h));
+}
+
 #ifdef __CUDACC__
 // mma.sync m16n8k16 with fp32 accumulators; T selects the .bf16 or .f16 operand type (register layouts are identical)
 template <typename T>
@@ -231,6 +257,30 @@ template <> struct VecLoad<f16, 4> {
         o[1] = ElemTraits<f16>::hi(u.x);
         o[2] = ElemTraits<f16>::lo(u.y);
         o[3] = ElemTraits<f16>::hi(u.y);
+    }
+};
+template <> struct VecLoad<e4m3, 8> {   // fp8 cache: the undecoded e4m3 values (the scale is folded in by the caller)
+    __device__ __forceinline__ static void load(const e4m3* p, float* o) {
+        uint2 u = *reinterpret_cast<const uint2*>(p);
+        const uint32_t w[2] = {u.x, u.y};
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const uint32_t lo = e4m3x2_to_f16x2(w[i]), hi = e4m3x2_to_f16x2(w[i] >> 16);
+            o[4 * i] = ElemTraits<f16>::lo(lo);
+            o[4 * i + 1] = ElemTraits<f16>::hi(lo);
+            o[4 * i + 2] = ElemTraits<f16>::lo(hi);
+            o[4 * i + 3] = ElemTraits<f16>::hi(hi);
+        }
+    }
+};
+template <> struct VecLoad<e4m3, 4> {
+    __device__ __forceinline__ static void load(const e4m3* p, float* o) {
+        const uint32_t w = *reinterpret_cast<const uint32_t*>(p);
+        const uint32_t lo = e4m3x2_to_f16x2(w), hi = e4m3x2_to_f16x2(w >> 16);
+        o[0] = ElemTraits<f16>::lo(lo);
+        o[1] = ElemTraits<f16>::hi(lo);
+        o[2] = ElemTraits<f16>::lo(hi);
+        o[3] = ElemTraits<f16>::hi(hi);
     }
 };
 template <> struct VecLoad<float, 8> {

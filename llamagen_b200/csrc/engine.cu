@@ -8,6 +8,7 @@
 // HBM, so one captured CUDA graph of a decode step is replayed S-2 times with no host round trip.
 #include "kernels.cuh"
 #include <algorithm>
+#include <cmath>
 #include <cstdarg>
 #include <cstdlib>
 #include <cstring>
@@ -133,6 +134,10 @@ struct lg_engine {
     int hdp = 0;                          // KV-cache row width in elements: hd, or 112 for head_dim 100 in bf16 / fp16 (GPT-3B) so that the rows
                                           // are 16-byte multiples and the TMA attention kernel can stream them (dims 100..111 stay zero)
     size_t esz = 2;
+    // KV-cache storage (lg_engine_set_kv_cache): the model dtype, or fp8 e4m3 with per-layer power-of-two (k, v) scales
+    bool kv_f8 = false;
+    size_t kv_esz = 2;                    // bytes per cached element
+    std::vector<float> kv_scales;         // [n_layer][2] (fp8 only)
     std::unordered_map<std::string, Tensor> w;
     std::vector<Layer> layers;
     const void *tok_emb = nullptr, *cls_table = nullptr, *cap_fc1 = nullptr, *cap_fc2 = nullptr, *uncond = nullptr;
@@ -161,7 +166,7 @@ struct lg_engine {
     }
     // R <= 8 decode steps can run as ONE persistent cooperative kernel per token (decode_persist.cu)
     bool persist_usable(int R) const {
-        return lg_env_flag("LG_PERSIST", 0) && d_layers && cfg.dtype == LG_DTYPE_BF16 && ws.have_maps &&
+        return lg_env_flag("LG_PERSIST", 0) && d_layers && cfg.dtype == LG_DTYPE_BF16 && !kv_f8 && ws.have_maps &&
                decode_persist_supported(R, cfg.dim, cfg.ffn_dim, cfg.vocab_size, cfg.n_head, hd, cfg.dtype) &&
                decode_persist_part_floats(R, cfg.n_head, hd) <= ws.partial_floats;
     }
@@ -198,7 +203,7 @@ size_t lg_engine::carve(Workspace& o, char* base, int rows, int max_seq) const {
         off += align_up(bytes);
         return p;
     };
-    o.layer_cache_bytes = (size_t)rows * H * max_seq * hdp * esz;
+    o.layer_cache_bytes = (size_t)rows * H * max_seq * hdp * kv_esz;
     o.kcache = take(o.layer_cache_bytes * L);
     o.vcache = take(o.layer_cache_bytes * L);
     o.h = take(Mmax * D * esz);
@@ -256,6 +261,10 @@ int lg_engine::forward(int M, int Tq, PosArg pos, const float* emb_mask, int B, 
         aa.out = ws.attn; aa.R = R; aa.Tq = Tq; aa.H = H; aa.hd = hd;
         aa.maxS = ws.max_seq; aa.pos = pos; aa.emb_mask = emb_mask; aa.B = B; aa.hdp = hdp;
         aa.Tc = cfg.cls_token_num; aa.scale = 1.0f / sqrtf((float)hd); aa.dtype = dt;
+        if (kv_f8) {   // the K scale folds into the softmax scale, the V scale into O / L, the writers divide by them
+            const float ks = kv_scales[2 * l], vs = kv_scales[2 * l + 1];
+            aa.kv_f8 = 1; aa.scale *= ks; aa.k_inv = 1.0f / ks; aa.v_inv = 1.0f / vs; aa.v_scale = vs;
+        }
         if (ws.have_maps) {
             aa.kmap = ws.kmap; aa.vmap = ws.vmap; aa.kmap16 = ws.kmap16; aa.vmap16 = ws.vmap16;
             aa.cache_row_base = (long long)l * ws.rows * H * ws.max_seq;
@@ -319,9 +328,11 @@ int lg_engine::forward(int M, int Tq, PosArg pos, const float* emb_mask, int B, 
         qa.partial = ws.partial; qa.ksplit = ks; qa.M = M; qa.Tq = Tq; qa.D = D; qa.H = H; qa.hd = hd;
         qa.pos = pos; qa.freqs = freqs; qa.q = ws.q; qa.kcache = kc; qa.vcache = vc; qa.maxS = ws.max_seq; qa.dtype = dt; qa.hdp = hdp;
         AttnArgs aa = attn_args(l);
-        // decode steps on the TMA path: the attention kernel is also the QKV epilogue (one dependent kernel less)
+        qa.kv_f8 = aa.kv_f8; qa.k_inv = aa.k_inv; qa.v_inv = aa.v_inv;
+        // decode steps on the TMA path: the attention kernel is also the QKV epilogue (one dependent kernel less); LG_ATTN_V2 unfuses
+        // it for its bf16-cache kernel only
         const bool fuse_qkv = lg_env_flag("LG_FUSE_QKV", 1) && attn_tma_enabled() && attn_tma_supported(aa) &&
-                              !(lg_env_flag("LG_ATTN_V2", 0) && R * H >= 4 * 132 && hd == 64);
+                              !(!kv_f8 && lg_env_flag("LG_ATTN_V2", 0) && R * H >= 4 * 132 && hd == 64);
         if (fuse_qkv) {
             aa.qkv_partial = ws.partial; aa.qkv_ksplit = ks; aa.freqs = freqs;
         } else {
@@ -400,6 +411,7 @@ int lg_engine_create(const lg_model_cfg* cfg, int device, lg_engine** out) {
     e->hd = hd;
     e->hdp = (hd == 100 && lg_dtype_is16(cfg->dtype) && lg_env_flag("LG_HD_PAD", 1)) ? 112 : hd;
     e->esz = (size_t)lg_dtype_info(cfg->dtype).esz;
+    e->kv_esz = e->esz;
     const char* ng = getenv("LG_NO_GRAPH");
     e->use_graph = !(ng && ng[0] == '1');
     *out = e;
@@ -515,13 +527,14 @@ int lg_engine_set_workspace(lg_engine* e, void* dev_ws, size_t bytes, int rows, 
     e->ws_needs_zero = true;
     tmp.have_maps = false;
     const int dt = e->cfg.dtype;
+    const int kvdt = e->kv_f8 ? LG_DTYPE_E4M3 : dt;   // storage type of the cache regions
     if (lg_dtype_is16(dt) && (e->hd == 64 || e->hd == 128 || e->hdp == 112)) {
         const long long total_rows = (long long)e->cfg.n_layer * rows * e->cfg.n_head * max_seq;
         if (total_rows < (1ll << 31)) {
-            LG_TRY(attn_tma_make_map(tmp.kmap, tmp.kcache, total_rows, e->hdp, dt));
-            LG_TRY(attn_tma_make_map(tmp.vmap, tmp.vcache, total_rows, e->hdp, dt));
-            LG_TRY(attn_tma_make_map(tmp.kmap16, tmp.kcache, total_rows, e->hdp, dt, 1));
-            LG_TRY(attn_tma_make_map(tmp.vmap16, tmp.vcache, total_rows, e->hdp, dt, 1));
+            LG_TRY(attn_tma_make_map(tmp.kmap, tmp.kcache, total_rows, e->hdp, kvdt));
+            LG_TRY(attn_tma_make_map(tmp.vmap, tmp.vcache, total_rows, e->hdp, kvdt));
+            LG_TRY(attn_tma_make_map(tmp.kmap16, tmp.kcache, total_rows, e->hdp, kvdt, 1));
+            LG_TRY(attn_tma_make_map(tmp.vmap16, tmp.vcache, total_rows, e->hdp, kvdt, 1));
             tmp.have_maps = true;
         }
     }
@@ -555,7 +568,7 @@ int lg_engine_set_workspace(lg_engine* e, void* dev_ws, size_t bytes, int rows, 
             for (int g = 0; g < n; ++g) {
                 Workspace w = tmp;
                 w.rows = hr;
-                w.layer_cache_bytes = (size_t)hr * c.n_head * max_seq * e->hdp * esz;
+                w.layer_cache_bytes = (size_t)hr * c.n_head * max_seq * e->hdp * e->kv_esz;
                 w.kcache = tmp.kcache + (size_t)g * w.layer_cache_bytes * c.n_layer;
                 w.vcache = tmp.vcache + (size_t)g * w.layer_cache_bytes * c.n_layer;
                 w.h = tmp.h + (size_t)g * Mh * c.dim * esz;
@@ -569,16 +582,46 @@ int lg_engine_set_workspace(lg_engine* e, void* dev_ws, size_t bytes, int rows, 
                 w.tokens = tmp.tokens + (size_t)g * hr;
                 w.counters = tmp.counters + 2 * g;
                 const long long total_rows = (long long)c.n_layer * hr * c.n_head * max_seq;
-                LG_TRY(attn_tma_make_map(w.kmap, w.kcache, total_rows, e->hdp, dt));
-                LG_TRY(attn_tma_make_map(w.vmap, w.vcache, total_rows, e->hdp, dt));
-                LG_TRY(attn_tma_make_map(w.kmap16, w.kcache, total_rows, e->hdp, dt, 1));
-                LG_TRY(attn_tma_make_map(w.vmap16, w.vcache, total_rows, e->hdp, dt, 1));
+                LG_TRY(attn_tma_make_map(w.kmap, w.kcache, total_rows, e->hdp, kvdt));
+                LG_TRY(attn_tma_make_map(w.vmap, w.vcache, total_rows, e->hdp, kvdt));
+                LG_TRY(attn_tma_make_map(w.kmap16, w.kcache, total_rows, e->hdp, kvdt, 1));
+                LG_TRY(attn_tma_make_map(w.vmap16, w.vcache, total_rows, e->hdp, kvdt, 1));
                 w.have_maps = true;
                 e->sub[g] = w;
             }
             e->n_sub = n;
         }
     }
+    return 0;
+}
+
+int lg_engine_set_kv_cache(lg_engine* e, int kv_dtype, const float* scales) {
+    LG_REQUIRE(e, "lg_engine_set_kv_cache: null engine");
+    const int dt = e->cfg.dtype;
+    LG_REQUIRE(lg_dtype_is16(dt), "lg_engine_set_kv_cache: an fp8 KV cache needs a bf16 or fp16 model (model dtype %d)", dt);
+    LG_REQUIRE(kv_dtype == dt || kv_dtype == LG_DTYPE_E4M3,
+               "lg_engine_set_kv_cache: unsupported KV-cache dtype %d (LG_DTYPE_E4M3 or the model dtype %d)", kv_dtype, dt);
+    std::vector<float> sc;
+    if (kv_dtype == LG_DTYPE_E4M3) {
+        sc.assign((size_t)2 * e->cfg.n_layer, 1.0f);
+        for (size_t i = 0; scales && i < sc.size(); ++i) {
+            const float s = scales[i];
+            int ex = 0;
+            // powers of two keep x / s exact and e4m3 * s exact in bf16 and fp16 (448 * 2^7 < 65504)
+            const bool pow2 = std::isfinite(s) && s > 0.f && std::frexp(s, &ex) == 0.5f && ex - 1 >= -8 && ex - 1 <= 7;
+            LG_REQUIRE(pow2, "lg_engine_set_kv_cache: %s scale of layer %d is %g; scales must be powers of two in [2^-8, 2^7]",
+                       i % 2 ? "V" : "K", (int)(i / 2), (double)s);
+            sc[i] = s;
+        }
+    }
+    // the carving and the tensor maps depend on the element size: the caller sets a new workspace
+    e->kv_f8 = kv_dtype == LG_DTYPE_E4M3;
+    e->kv_esz = e->kv_f8 ? 1 : e->esz;
+    e->kv_scales = sc;
+    e->full = Workspace();
+    e->ws = Workspace();
+    e->n_sub = 0;
+    e->ws_needs_zero = false;
     return 0;
 }
 

@@ -193,14 +193,16 @@ int make_map_2d(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, 
                 uint32_t box_cols, int dtype) {
     EncodeTiledFn enc = get_encode();
     LG_REQUIRE(enc, "cuTensorMapEncodeTiled is not available from the driver");
-    LG_REQUIRE(lg_dtype_is16(dtype), "make_map_2d: dtype %d has no 16-bit tensor map", dtype);
+    LG_REQUIRE(lg_dtype_is16(dtype) || dtype == LG_DTYPE_E4M3, "make_map_2d: dtype %d has no tensor map", dtype);
     const DtypeInfo di = lg_dtype_info(dtype);
     cuuint64_t dims[2] = {cols, rows};
     cuuint64_t strides[1] = {ld_elems * (cuuint64_t)di.esz};
     cuuint32_t box[2] = {box_cols, box_rows};
     cuuint32_t estr[2] = {1, 1};
+    // 128-byte swizzle; fp8 KV boxes of 64 bytes use the 64-byte swizzle
+    const CUtensorMapSwizzle swz = box_cols * di.esz == 64 && dtype == LG_DTYPE_E4M3 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
     CUresult r = enc(m, di.tma, 2, const_cast<void*>(base), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     LG_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(2d) failed (%d) rows=%llu cols=%llu ld=%llu box=%ux%u", (int)r,
                (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld_elems, box_rows, box_cols);

@@ -97,6 +97,9 @@ struct QkvEpiArgs {
     int maxS;
     int dtype;
     int hdp = 0;                        // elements between consecutive cache rows (0: hd). GPT-3B's hd = 100 is stored in 112-wide rows
+    // fp8 KV cache (lg_engine_set_kv_cache): K / V are stored as e4m3(x * inv) with inv = 1 / (this layer's power-of-two scale)
+    int kv_f8 = 0;
+    float k_inv = 1.f, v_inv = 1.f;
 };
 int launch_qkv_epilogue(const QkvEpiArgs& a, cudaStream_t st);
 
@@ -129,9 +132,14 @@ struct AttnArgs {
     long long cache_row_base = 0;
     // fused QKV epilogue (TMA path, Tq == 1): the attention kernel reduces the QKV GEMM's split-K slabs itself
     const float* qkv_partial = nullptr; int qkv_ksplit = 0; const float* freqs = nullptr;
+    // fp8 KV cache: the caches hold e4m3 codes; `scale` already includes the K scale, the output is multiplied by v_scale, and the
+    // fused writer stores e4m3(k * k_inv), e4m3(v * v_inv)
+    int kv_f8 = 0;
+    float k_inv = 1.f, v_inv = 1.f, v_scale = 1.f;
 };
 int launch_attention(const AttnArgs& a, cudaStream_t st);
-// attn_tma.cu — TMA + tensor-core decode attention for bf16 / fp16 caches (dtype: LG_DTYPE_BF16 or LG_DTYPE_F16)
+// attn_tma.cu — TMA + tensor-core decode attention for bf16 / fp16 caches (dtype: LG_DTYPE_BF16 or LG_DTYPE_F16) and fp8 caches of
+// those models (map dtype LG_DTYPE_E4M3: 64- or 128-byte boxes)
 int attn_tma_make_map(void* map_out /*CUtensorMap, 128 B*/, const void* cache_base, long long total_rows, int hdp, int dtype,
                       int tail16 = 0);
 bool attn_tma_supported(const AttnArgs& a);

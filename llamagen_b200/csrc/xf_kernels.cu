@@ -7,6 +7,7 @@
 // model dtype T is rounded to T at the same point here (ElemTraits<T>::round).
 #include "kernels.cuh"
 #include <algorithm>
+#include <type_traits>
 
 namespace {
 
@@ -111,9 +112,13 @@ template <> __device__ __forceinline__ void store4<f16>(f16* p, float a, float b
     *reinterpret_cast<uint2*>(p) = u;
 }
 template <typename T> __device__ __forceinline__ void load4(const T* p, float* o) { VecLoad<T, 4>::load(p, o); }
+__device__ __forceinline__ void store4_e4m3(e4m3* p, float a, float b, float c, float d) {
+    *reinterpret_cast<uint32_t*>(p) = e4m3x2_pack(a, b) | (e4m3x2_pack(c, d) << 16);
+}
 
 // One CTA per row, one thread per 4 consecutive output features (two RoPE pairs), all loads up front.
-template <typename T>
+// F8: the K / V rows go to an fp8 cache as e4m3(x * inv), x the model-dtype value the 16-bit cache would hold.
+template <typename T, bool F8 = false>
 __global__ void __launch_bounds__(1024) qkv_epilogue_kernel(QkvEpiArgs a) {
     lg_pdl_sync();
     const int m = blockIdx.x, r = m / a.Tq, t = m % a.Tq;
@@ -131,13 +136,26 @@ __global__ void __launch_bounds__(1024) qkv_epilogue_kernel(QkvEpiArgs a) {
         const float x0 = TR<T>::round(sv.x), x1 = TR<T>::round(sv.y), x2 = TR<T>::round(sv.z), x3 = TR<T>::round(sv.w);
         const int sec = n / D, within = n - sec * D, head = within / hd, e = within - head * hd;   // hd % 4 == 0
         if (sec == 2) {
-            store4<T>(vc + (((size_t)r * a.H + head) * a.maxS + p) * hdp + e, x0, x1, x2, x3);
+            if constexpr (F8) {
+                const float s = a.v_inv;
+                store4_e4m3(reinterpret_cast<e4m3*>(a.vcache) + (((size_t)r * a.H + head) * a.maxS + p) * hdp + e, x0 * s, x1 * s, x2 * s, x3 * s);
+            } else {
+                store4<T>(vc + (((size_t)r * a.H + head) * a.maxS + p) * hdp + e, x0, x1, x2, x3);
+            }
         } else {
             const float4 cs = *reinterpret_cast<const float4*>(fr + (e >> 1) * 2);   // (cos, sin) of two pairs
             const float y0 = __fsub_rn(__fmul_rn(x0, cs.x), __fmul_rn(x1, cs.y));
             const float y1 = __fadd_rn(__fmul_rn(x1, cs.x), __fmul_rn(x0, cs.y));
             const float y2 = __fsub_rn(__fmul_rn(x2, cs.z), __fmul_rn(x3, cs.w));
             const float y3 = __fadd_rn(__fmul_rn(x3, cs.z), __fmul_rn(x2, cs.w));
+            if constexpr (F8) {
+                if (sec == 1) {   // the key is rounded to T after RoPE (as the 16-bit cache stores it), then quantised
+                    const float s = a.k_inv;
+                    store4_e4m3(reinterpret_cast<e4m3*>(a.kcache) + (((size_t)r * a.H + head) * a.maxS + p) * hdp + e,
+                                TR<T>::round(y0) * s, TR<T>::round(y1) * s, TR<T>::round(y2) * s, TR<T>::round(y3) * s);
+                    continue;
+                }
+            }
             T* dst = sec == 0 ? q + (size_t)m * D + within : kc + (((size_t)r * a.H + head) * a.maxS + p) * hdp + e;
             store4<T>(dst, y0, y1, y2, y3);
         }
@@ -225,7 +243,8 @@ __global__ void reduce_f32_kernel(const float* __restrict__ partial, int ks, siz
 // contiguous head elements (128-bit loads for hd=64 bf16); every lane group runs an independent online
 // softmax over its keys; groups merge by shuffles, warps merge through shared memory.
 // Mask (gpt.py:354 + generate.py:154-163): key j visible iff j <= qpos and (j >= Tc or emb_mask[r%B, j] != 0 or j == qpos).
-template <typename T, int HD, int VEC, int LPK, int HDP = HD>
+// KV = e4m3 (fp8 cache): K and V are read as their e4m3 codes; a.scale carries the K scale and the output is multiplied by a.v_scale.
+template <typename T, int HD, int VEC, int LPK, int HDP = HD, typename KV = T>
 __global__ void __launch_bounds__(256) attention_kernel(AttnArgs a) {
     lg_pdl_sync();
     constexpr int KPW = 32 / LPK;  // keys per warp per iteration
@@ -242,8 +261,8 @@ __global__ void __launch_bounds__(256) attention_kernel(AttnArgs a) {
     constexpr int hdp = HDP;                            // cache row stride (compile-time: the address math sits in the inner loop)
 
     const T* qp = reinterpret_cast<const T*>(a.q) + (size_t)m * D + (size_t)h * HD;
-    const T* kbase = reinterpret_cast<const T*>(a.kcache) + ((size_t)r * a.H + h) * (size_t)a.maxS * hdp;
-    const T* vbase = reinterpret_cast<const T*>(a.vcache) + ((size_t)r * a.H + h) * (size_t)a.maxS * hdp;
+    const KV* kbase = reinterpret_cast<const KV*>(a.kcache) + ((size_t)r * a.H + h) * (size_t)a.maxS * hdp;
+    const KV* vbase = reinterpret_cast<const KV*>(a.vcache) + ((size_t)r * a.H + h) * (size_t)a.maxS * hdp;
     const float* mrow = a.emb_mask ? a.emb_mask + (size_t)(r % a.B) * a.Tc : nullptr;
 
     float qv[VEC];
@@ -268,8 +287,8 @@ __global__ void __launch_bounds__(256) attention_kernel(AttnArgs a) {
 #pragma unroll
             for (int i = 0; i < VEC; ++i) { kv[u][i] = 0.f; vv[u][i] = 0.f; }
             if (j < nkeys && active) {
-                VecLoad<T, VEC>::load(kbase + (size_t)j * hdp + li * VEC, kv[u]);
-                VecLoad<T, VEC>::load(vbase + (size_t)j * hdp + li * VEC, vv[u]);
+                VecLoad<KV, VEC>::load(kbase + (size_t)j * hdp + li * VEC, kv[u]);
+                VecLoad<KV, VEC>::load(vbase + (size_t)j * hdp + li * VEC, vv[u]);
             }
         }
 #pragma unroll
@@ -328,7 +347,8 @@ __global__ void __launch_bounds__(256) attention_kernel(AttnArgs a) {
             L += smem[(size_t)w * (HD + 2) + HD + 1] * c;
             O += smem[(size_t)w * (HD + 2) + e] * c;
         }
-        op[e] = TR<T>::from_f(O / L);
+        if constexpr (std::is_same<KV, e4m3>::value) op[e] = TR<T>::from_f(O / L * a.v_scale);
+        else op[e] = TR<T>::from_f(O / L);
     }
 }
 
@@ -410,6 +430,13 @@ int launch_rmsnorm(const void* x, const void* w, void* xn, int M, int D, float e
 int launch_qkv_epilogue(const QkvEpiArgs& a, cudaStream_t st) {
     LG_REQUIRE(a.hd % 4 == 0 && a.D % 4 == 0, "head_dim %d / dim %d must be multiples of 4", a.hd, a.D);
     const int threads = std::min(1024, ((3 * a.D / 4 + 31) / 32) * 32);
+    if (a.kv_f8) {
+        LG_REQUIRE(lg_dtype_is16(a.dtype), "qkv epilogue: an fp8 KV cache needs a bf16 or fp16 model (dtype %d)", a.dtype);
+        (void)lg_launch(a.dtype == LG_DTYPE_F16 ? qkv_epilogue_kernel<f16, true> : qkv_epilogue_kernel<bf16, true>, dim3(a.M), dim3(threads), 0,
+                        st, a);
+        LG_LAUNCH_CHECK();
+        return 0;
+    }
     return dispatch_dtype(
         a.dtype, [&](auto z) {
             using E = decltype(z);
@@ -464,13 +491,13 @@ int launch_reduce_f32(const float* partial, int ksplit, int M, int N, float* out
     return 0;
 }
 
-template <typename T, int HD, int VEC, int LPK, int HDP = HD>
+template <typename T, int HD, int VEC, int LPK, int HDP = HD, typename KV = T>
 static int launch_attention_t(const AttnArgs& a, cudaStream_t st) {
     const long long ctas = (long long)a.R * a.Tq * a.H;
     const int nwarps = ctas >= 592 ? 4 : 8;
     const size_t smem = (size_t)nwarps * (HD + 2) * sizeof(float);
     dim3 grid(a.H, a.R * a.Tq);
-    (void)lg_launch(attention_kernel<T, HD, VEC, LPK, HDP>, dim3(grid), dim3(nwarps * 32), smem, st, a);
+    (void)lg_launch(attention_kernel<T, HD, VEC, LPK, HDP, KV>, dim3(grid), dim3(nwarps * 32), smem, st, a);
     LG_LAUNCH_CHECK();
     return 0;
 }
@@ -481,6 +508,20 @@ int launch_attention(const AttnArgs& a, cudaStream_t st) {
     LG_REQUIRE(a.qkv_partial == nullptr, "attention: fused QKV epilogue requested on a path that does not support it");
     LG_REQUIRE((long long)a.R * a.Tq <= 65535, "attention: too many query rows (%d x %d)", a.R, a.Tq);
     LG_REQUIRE(a.hdp == 0 || a.hdp == a.hd || (a.hd == 100 && a.hdp == 112 && lg_dtype_is16(a.dtype)), "attention: unsupported KV row stride %d for head_dim %d", a.hdp, a.hd);
+    if (a.kv_f8) {   // fp8 cache of a 16-bit model
+        if (a.dtype == LG_DTYPE_BF16) {
+            if (a.hd == 64) return launch_attention_t<bf16, 64, 8, 8, 64, e4m3>(a, st);
+            if (a.hd == 128) return launch_attention_t<bf16, 128, 8, 16, 128, e4m3>(a, st);
+            if (a.hd == 100 && a.hdp == 112) return launch_attention_t<bf16, 100, 4, 32, 112, e4m3>(a, st);
+            if (a.hd == 100) return launch_attention_t<bf16, 100, 4, 32, 100, e4m3>(a, st);
+        } else if (a.dtype == LG_DTYPE_F16) {
+            if (a.hd == 64) return launch_attention_t<f16, 64, 8, 8, 64, e4m3>(a, st);
+            if (a.hd == 128) return launch_attention_t<f16, 128, 8, 16, 128, e4m3>(a, st);
+            if (a.hd == 100 && a.hdp == 112) return launch_attention_t<f16, 100, 4, 32, 112, e4m3>(a, st);
+            if (a.hd == 100) return launch_attention_t<f16, 100, 4, 32, 100, e4m3>(a, st);
+        }
+        return lg_fail("attention: no fp8 KV-cache kernel for head_dim %d / dtype %d", a.hd, a.dtype);
+    }
     if (a.dtype == LG_DTYPE_BF16) {
         if (a.hd == 64) return launch_attention_t<bf16, 64, 8, 8>(a, st);
         if (a.hd == 128) return launch_attention_t<bf16, 128, 8, 16>(a, st);

@@ -157,12 +157,28 @@ class Transformer(nn.Module):
         self._engine_sig = None
         self._workspace = None
         self._ws_shape = (0, 0)
+        self._kv_cache = ("auto", None)
         self.requires_grad_(False)
 
     # ------------------------------------------------------------------ engine plumbing
+    def set_kv_cache(self, dtype: str = "auto", scales=None):
+        """KV-cache storage of a bf16 / fp16 model: "auto" (the model dtype) or "fp8" (e4m3, half the cache bytes).
+        scales: [n_layer, 2] per-layer (k, v) scales for fp8, each a power of two in [2^-8, 2^7]; None = all 1.0. K and V are
+        stored as e4m3(x / s) and read back as e4m3 * s. Takes effect at the next setup_caches(), which re-creates the workspace."""
+        if dtype not in ("auto", "fp8"):
+            raise ValueError(f"kv cache dtype must be 'auto' or 'fp8', got {dtype!r}")
+        if scales is not None:
+            if dtype != "fp8":
+                raise ValueError("KV-cache scales apply to the fp8 cache only")
+            s = torch.as_tensor(scales, dtype=torch.float32).detach().cpu()
+            if tuple(s.shape) != (self.n_layer, 2):
+                raise ValueError(f"KV-cache scales must have shape [{self.n_layer}, 2], got {tuple(s.shape)}")
+            scales = tuple(float(x) for x in s.reshape(-1))
+        self._kv_cache = (dtype, scales)
+
     def _signature(self):
         p = self.tok_embeddings.weight
-        return (p.device, p.dtype, tuple(t.data_ptr() for t in self.state_dict().values()))
+        return (p.device, p.dtype, tuple(t.data_ptr() for t in self.state_dict().values()), self._kv_cache)
 
     def engine(self):
         """Create / refresh the C engine for the parameters' current device + dtype."""
@@ -193,6 +209,14 @@ class Transformer(nn.Module):
                                              _lib.shape_array(self.freqs_cis.shape), 3, _lib.LG_DTYPE_F32),
                    "bind freqs_cis")
         _lib.check(lib.lg_engine_finalize(handle), "lg_engine_finalize")
+        kv_dtype, kv_scales = self._kv_cache
+        if kv_dtype == "fp8":
+            arr = (ctypes.c_float * len(kv_scales))(*kv_scales) if kv_scales is not None else None
+            status = lib.lg_engine_set_kv_cache(handle, _lib.LG_DTYPE_E4M3, arr)
+            if status < 0:
+                msg = lib.lg_last_error()
+                lib.lg_engine_destroy(handle)
+                raise _lib.LgError(f"lg_engine_set_kv_cache: {msg.decode() if msg else 'unknown error'}")
         self._engine, self._engine_sig = handle, sig
         self._workspace, self._ws_shape = None, (0, 0)
         return handle
