@@ -90,6 +90,9 @@ SIGNATURES = {
     "lg_profile_class_name": (c_char_p, [c_int]),
     "lg_test_gemm": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t,
                              c_void_p]),
+    "lg_test_attention": (c_int, [c_int, c_int, c_float, c_float, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                  c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int,
+                                  c_void_p, c_int, c_void_p, c_void_p, POINTER(c_int), c_void_p]),
     "lg_test_gemm_dx": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_float, c_void_p,
                                 c_void_p]),
     "lg_test_vq_conv": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,

@@ -22,7 +22,8 @@ using namespace tma;
 constexpr int kKC = LG_ATTN_KC;   // keys per stage (64 -> 4 warps, 6 CTAs/SM; 48 -> 3 warps, 8 CTAs/SM)
 constexpr int kStagesA = 2;       // 2 stages of K+V per CTA; contexts here are <= 1144 keys
 constexpr int kWarps = kKC / 16;  // each warp owns 16 keys of a stage
-constexpr int kDeepStages = kKC == 32 ? 8 : 6;   // few-item (batch-1) variant: the whole <= 256/288-key context is requested before the dependency wait
+constexpr int kDeepStages = kKC == 32 ? 8 : 6;   // few-item (batch-1) variant: a whole context of up to NST * kKC keys (256 at kKC = 32)
+                                                 // is requested before the dependency wait
 #ifdef LG_ATTN_CTAS
 constexpr int kCtasPerSm64 = LG_ATTN_CTAS;
 #else
@@ -852,6 +853,10 @@ int attn_tma_make_map(void* map_out, const void* cache_base, long long total_row
                             tail16 ? 16 : kKC, dtype == LG_DTYPE_E4M3 ? (hdp == 64 ? 64 : 128) : 64, dtype);
 }
 
+bool attn_tma_maps_usable(int dtype, int hd, int hdp, long long total_rows) {
+    return lg_dtype_is16(dtype) && (hd == 64 || hd == 128 || hdp == 112) && total_rows < (1ll << 31);
+}
+
 bool attn_tma_enabled() { return lg_env_flag("LG_ATTN_TMA", 1) != 0; }
 
 bool attn_prefill_tc_supported(const AttnArgs& a) {
@@ -860,7 +865,7 @@ bool attn_prefill_tc_supported(const AttnArgs& a) {
            lg_env_flag("LG_ATTN_PREFILL_TC", 1) != 0;
 }
 
-int launch_attention_prefill_tc(const AttnArgs& a, cudaStream_t st) {
+int launch_attention_prefill_tc(const AttnArgs& a, cudaStream_t st, int* path) {
     AttnTmaArgs t{};
     t.q = (const bf16*)a.q; t.out = (bf16*)a.out; t.R = a.R; t.H = a.H; t.maxS = a.maxS;
     t.row_base = a.cache_row_base; t.emb_mask = a.emb_mask; t.B = a.B; t.Tc = a.Tc; t.scale = a.scale;
@@ -881,6 +886,7 @@ int launch_attention_prefill_tc(const AttnArgs& a, cudaStream_t st) {
     (void)lg_launch(kern, dim3(grid), dim3(256), smem, st, qmap, *reinterpret_cast<const CUtensorMap*>(a.kmap),
                     *reinterpret_cast<const CUtensorMap*>(a.vmap), t, a.Tq, f8s);
     LG_LAUNCH_CHECK();
+    set_attn_path(path, 3, 1, 0);
     return 0;
 }
 
@@ -890,7 +896,7 @@ bool attn_tma_supported(const AttnArgs& a) {
 }
 
 template <typename T, bool F8 = false>
-static int launch_attention_tma_t(const AttnArgs& a, cudaStream_t st) {
+static int launch_attention_tma_t(const AttnArgs& a, cudaStream_t st, int* path) {
     AttnTmaArgs t;
     const KvScales f8s{a.k_inv, a.v_inv, a.v_scale};
     t.q = (const bf16*)a.q; t.out = (bf16*)a.out; t.R = a.R; t.H = a.H; t.maxS = a.maxS;
@@ -904,27 +910,33 @@ static int launch_attention_tma_t(const AttnArgs& a, cudaStream_t st) {
     const CUtensorMap& vm = *reinterpret_cast<const CUtensorMap*>(a.vmap);
     const CUtensorMap& km16 = *reinterpret_cast<const CUtensorMap*>(a.kmap16);
     const CUtensorMap& vm16 = *reinterpret_cast<const CUtensorMap*>(a.vmap16);
+    const int fused = a.qkv_partial ? 1 : 0;
+    auto ran = [&](int rc, int kernel, int stages) {
+        if (rc == 0) set_attn_path(path, kernel, stages, fused);
+        return rc;
+    };
     if (a.qkv_partial) {     // fused QKV epilogue
-        // few (row, head) items (batch-1 latency path): a 6-stage ring holds a whole 288-key context, so every K/V byte is
-        // requested before the dependency wait instead of two stages at a time
+        // few (row, head) items (batch-1 latency path): an 8-stage ring (kKC = 32) holds a whole 256-key context, so every K/V byte
+        // is requested before the dependency wait instead of two stages at a time
         if (a.hd == 64 && a.R * a.H <= 2 * 132 && lg_env_flag("LG_ATTN_DEEP", 1))
-            return launch_t<T, 64, true, kDeepStages, (kDeepStages > 2), F8>(km, vm, km16, vm16, t, st, f8s);
+            return ran(launch_t<T, 64, true, kDeepStages, (kDeepStages > 2), F8>(km, vm, km16, vm16, t, st, f8s), 1, kDeepStages);
         // deeper sequential ring (A/B switch): more keys requested before the dependency wait, fewer refill round trips
         const int nst = lg_env_flag("LG_ATTN_NST", 2);
-        if (a.hd == 64 && nst == 3) return launch_t<T, 64, true, 3, false, F8>(km, vm, km16, vm16, t, st, f8s);
-        if (a.hd == 64 && nst == 4) return launch_t<T, 64, true, 4, false, F8>(km, vm, km16, vm16, t, st, f8s);
-        if (a.hd == 64) return launch_t<T, 64, true, kStagesA, false, F8>(km, vm, km16, vm16, t, st, f8s);
-        return launch_t<T, 128, true, kStagesA, false, F8>(km, vm, km16, vm16, t, st, f8s);
+        if (a.hd == 64 && nst == 3) return ran(launch_t<T, 64, true, 3, false, F8>(km, vm, km16, vm16, t, st, f8s), 1, 3);
+        if (a.hd == 64 && nst == 4) return ran(launch_t<T, 64, true, 4, false, F8>(km, vm, km16, vm16, t, st, f8s), 1, 4);
+        if (a.hd == 64) return ran(launch_t<T, 64, true, kStagesA, false, F8>(km, vm, km16, vm16, t, st, f8s), 1, kStagesA);
+        return ran(launch_t<T, 128, true, kStagesA, false, F8>(km, vm, km16, vm16, t, st, f8s), 1, kStagesA);
     }
     // v2 (persistent warp-per-item, LG_ATTN_V2=1) stays opt-in: with one warp per scheduler its ldmatrix->mma->softmax chain is
     // latency-bound, which made it slower than the CTA-per-item kernel where it was measured. bf16 caches only.
     const bool v2 = !F8 && std::is_same<T, bf16>::value && lg_env_flag("LG_ATTN_V2", 0) && a.R * a.H >= 4 * 132 && a.hd == 64 && !a.pos.rows;
-    if (v2) return launch_v2<64>(km, vm, t, st);
-    if (a.hd == 64) return launch_t<T, 64, false, kStagesA, false, F8>(km, vm, km16, vm16, t, st, f8s);
-    return launch_t<T, 128, false, kStagesA, false, F8>(km, vm, km16, vm16, t, st, f8s);
+    if (v2) return ran(launch_v2<64>(km, vm, t, st), 2, kStagesV2);
+    if (a.hd == 64) return ran(launch_t<T, 64, false, kStagesA, false, F8>(km, vm, km16, vm16, t, st, f8s), 1, kStagesA);
+    return ran(launch_t<T, 128, false, kStagesA, false, F8>(km, vm, km16, vm16, t, st, f8s), 1, kStagesA);
 }
 
-int launch_attention_tma(const AttnArgs& a, cudaStream_t st) {
-    if (a.kv_f8) return a.dtype == LG_DTYPE_F16 ? launch_attention_tma_t<f16, true>(a, st) : launch_attention_tma_t<bf16, true>(a, st);
-    return a.dtype == LG_DTYPE_F16 ? launch_attention_tma_t<f16>(a, st) : launch_attention_tma_t<bf16>(a, st);
+int launch_attention_tma(const AttnArgs& a, cudaStream_t st, int* path) {
+    if (a.kv_f8)
+        return a.dtype == LG_DTYPE_F16 ? launch_attention_tma_t<f16, true>(a, st, path) : launch_attention_tma_t<bf16, true>(a, st, path);
+    return a.dtype == LG_DTYPE_F16 ? launch_attention_tma_t<f16>(a, st, path) : launch_attention_tma_t<bf16>(a, st, path);
 }

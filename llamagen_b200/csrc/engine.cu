@@ -528,15 +528,13 @@ int lg_engine_set_workspace(lg_engine* e, void* dev_ws, size_t bytes, int rows, 
     tmp.have_maps = false;
     const int dt = e->cfg.dtype;
     const int kvdt = e->kv_f8 ? LG_DTYPE_E4M3 : dt;   // storage type of the cache regions
-    if (lg_dtype_is16(dt) && (e->hd == 64 || e->hd == 128 || e->hdp == 112)) {
-        const long long total_rows = (long long)e->cfg.n_layer * rows * e->cfg.n_head * max_seq;
-        if (total_rows < (1ll << 31)) {
-            LG_TRY(attn_tma_make_map(tmp.kmap, tmp.kcache, total_rows, e->hdp, kvdt));
-            LG_TRY(attn_tma_make_map(tmp.vmap, tmp.vcache, total_rows, e->hdp, kvdt));
-            LG_TRY(attn_tma_make_map(tmp.kmap16, tmp.kcache, total_rows, e->hdp, kvdt, 1));
-            LG_TRY(attn_tma_make_map(tmp.vmap16, tmp.vcache, total_rows, e->hdp, kvdt, 1));
-            tmp.have_maps = true;
-        }
+    const long long total_rows = (long long)e->cfg.n_layer * rows * e->cfg.n_head * max_seq;
+    if (attn_tma_maps_usable(dt, e->hd, e->hdp, total_rows)) {
+        LG_TRY(attn_tma_make_map(tmp.kmap, tmp.kcache, total_rows, e->hdp, kvdt));
+        LG_TRY(attn_tma_make_map(tmp.vmap, tmp.vcache, total_rows, e->hdp, kvdt));
+        LG_TRY(attn_tma_make_map(tmp.kmap16, tmp.kcache, total_rows, e->hdp, kvdt, 1));
+        LG_TRY(attn_tma_make_map(tmp.vmap16, tmp.vcache, total_rows, e->hdp, kvdt, 1));
+        tmp.have_maps = true;
     }
     e->full = tmp;
     e->ws = tmp;
@@ -595,6 +593,12 @@ int lg_engine_set_workspace(lg_engine* e, void* dev_ws, size_t bytes, int rows, 
     return 0;
 }
 
+// powers of two keep x / s exact and e4m3 * s exact in bf16 and fp16 (448 * 2^7 < 65504)
+static bool kv_scale_ok(float s) {
+    int ex = 0;
+    return std::isfinite(s) && s > 0.f && std::frexp(s, &ex) == 0.5f && ex - 1 >= -8 && ex - 1 <= 7;
+}
+
 int lg_engine_set_kv_cache(lg_engine* e, int kv_dtype, const float* scales) {
     LG_REQUIRE(e, "lg_engine_set_kv_cache: null engine");
     const int dt = e->cfg.dtype;
@@ -606,10 +610,7 @@ int lg_engine_set_kv_cache(lg_engine* e, int kv_dtype, const float* scales) {
         sc.assign((size_t)2 * e->cfg.n_layer, 1.0f);
         for (size_t i = 0; scales && i < sc.size(); ++i) {
             const float s = scales[i];
-            int ex = 0;
-            // powers of two keep x / s exact and e4m3 * s exact in bf16 and fp16 (448 * 2^7 < 65504)
-            const bool pow2 = std::isfinite(s) && s > 0.f && std::frexp(s, &ex) == 0.5f && ex - 1 >= -8 && ex - 1 <= 7;
-            LG_REQUIRE(pow2, "lg_engine_set_kv_cache: %s scale of layer %d is %g; scales must be powers of two in [2^-8, 2^7]",
+            LG_REQUIRE(kv_scale_ok(s), "lg_engine_set_kv_cache: %s scale of layer %d is %g; scales must be powers of two in [2^-8, 2^7]",
                        i % 2 ? "V" : "K", (int)(i / 2), (double)s);
             sc[i] = s;
         }
@@ -961,6 +962,72 @@ int lg_test_gemm(const void* x, const void* w, int M, int N, int K, int dtype, f
     GemmPlan plan;
     LG_TRY(gemm_partial(x, K, w, nullptr, 0, M, N, K, dtype, (float*)dev_scratch, &plan, st));
     return launch_reduce_f32((const float*)dev_scratch, plan.ksplit, M, N, y, st);
+}
+
+int lg_test_attention(int dtype, int kv_dtype, float k_scale, float v_scale, int R, int Tq, int H, int hd, int hdp, int max_seq,
+                      void* kcache, void* vcache, int n_layer, int layer, int pos_value, const int32_t* pos_dev,
+                      const int32_t* pos_rows, const float* emb_mask, int B, int Tc, const void* q, const float* qkv_partial,
+                      int ksplit, const float* freqs, int fuse, void* q_out, void* out, int* path, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    auto a16 = [](const void* p) { return ((uintptr_t)p & 15) == 0; };
+    const bool f8 = kv_dtype == LG_DTYPE_E4M3;
+    LG_REQUIRE(dtype == LG_DTYPE_F32 || lg_dtype_is16(dtype), "lg_test_attention: unsupported model dtype %d", dtype);
+    LG_REQUIRE(kv_dtype == dtype || (f8 && lg_dtype_is16(dtype)),
+               "lg_test_attention: KV dtype %d with model dtype %d (the model dtype, or LG_DTYPE_E4M3 for a bf16 / fp16 model)", kv_dtype,
+               dtype);
+    LG_REQUIRE(f8 ? kv_scale_ok(k_scale) && kv_scale_ok(v_scale) : k_scale == 1.f && v_scale == 1.f,
+               "lg_test_attention: K / V scales %g / %g (fp8: powers of two in [2^-8, 2^7], otherwise 1)", (double)k_scale, (double)v_scale);
+    LG_REQUIRE(R > 0 && Tq > 0 && H > 0 && max_seq > 0 && n_layer > 0 && layer >= 0 && layer < n_layer && (long long)R * Tq <= 65535,
+               "lg_test_attention: bad shape R=%d Tq=%d H=%d max_seq=%d layer %d of %d", R, Tq, H, max_seq, layer, n_layer);
+    LG_REQUIRE(hd == 64 || hd == 100 || hd == 128, "lg_test_attention: unsupported head_dim %d (64, 100, 128)", hd);
+    LG_REQUIRE(hdp == hd || (hd == 100 && hdp == 112 && lg_dtype_is16(dtype)), "lg_test_attention: row width %d for head_dim %d", hdp, hd);
+    LG_REQUIRE(kcache && vcache && out && a16(kcache) && a16(vcache) && a16(out) && a16(q) && a16(q_out) && a16(qkv_partial) && a16(freqs),
+               "lg_test_attention: null or misaligned (16 bytes) buffer");
+    if (pos_rows) {
+        LG_REQUIRE(pos_dev == nullptr && pos_value == 0, "lg_test_attention: per-row positions take no counter and no value");
+    } else {
+        LG_REQUIRE(pos_value >= 0 && (pos_dev || pos_value + Tq <= max_seq), "lg_test_attention: position %d + Tq %d exceeds max_seq %d",
+                   pos_value, Tq, max_seq);
+    }
+    LG_REQUIRE(!emb_mask || (B > 0 && Tc > 0 && Tc <= max_seq), "lg_test_attention: emb_mask needs B > 0 and 0 < Tc <= max_seq (B=%d Tc=%d)",
+               B, Tc);
+    LG_REQUIRE((q != nullptr) != (qkv_partial != nullptr), "lg_test_attention: pass exactly one of q and qkv_partial");
+    LG_REQUIRE(q ? fuse == 0 : (ksplit > 0 && freqs && (fuse == 1 || (fuse == 0 && q_out))),
+               "lg_test_attention: q takes fuse = 0; qkv_partial needs ksplit > 0, freqs and fuse = 1 or q_out");
+    const long long total_rows = (long long)n_layer * R * H * max_seq;
+    const size_t layer_bytes = (size_t)R * H * max_seq * hdp * (f8 ? 1 : lg_dtype_info(dtype).esz);
+    AttnArgs aa;
+    aa.q = q ? q : q_out; aa.out = out;
+    aa.kcache = (char*)kcache + (size_t)layer * layer_bytes; aa.vcache = (char*)vcache + (size_t)layer * layer_bytes;
+    aa.R = R; aa.Tq = Tq; aa.H = H; aa.hd = hd; aa.maxS = max_seq; aa.hdp = hdp;
+    aa.pos = PosArg{pos_dev, pos_value, pos_rows};
+    aa.emb_mask = emb_mask; aa.B = emb_mask ? B : 1; aa.Tc = emb_mask ? Tc : 0;
+    aa.scale = 1.0f / sqrtf((float)hd); aa.dtype = dtype;
+    if (f8) { aa.kv_f8 = 1; aa.scale *= k_scale; aa.k_inv = 1.0f / k_scale; aa.v_inv = 1.0f / v_scale; aa.v_scale = v_scale; }
+    alignas(64) unsigned char maps[4][128];   // as lg_engine_set_workspace builds them: over every layer of the buffer
+    if (attn_tma_maps_usable(dtype, hd, hdp, total_rows)) {
+        const int kvdt = f8 ? LG_DTYPE_E4M3 : dtype;
+        LG_TRY(attn_tma_make_map(maps[0], kcache, total_rows, hdp, kvdt));
+        LG_TRY(attn_tma_make_map(maps[1], vcache, total_rows, hdp, kvdt));
+        LG_TRY(attn_tma_make_map(maps[2], kcache, total_rows, hdp, kvdt, 1));
+        LG_TRY(attn_tma_make_map(maps[3], vcache, total_rows, hdp, kvdt, 1));
+        aa.kmap = maps[0]; aa.vmap = maps[1]; aa.kmap16 = maps[2]; aa.vmap16 = maps[3];
+        aa.cache_row_base = (long long)layer * R * H * max_seq;
+    }
+    if (qkv_partial) {
+        if (fuse) {
+            LG_REQUIRE(attn_tma_enabled() && attn_tma_supported(aa), "lg_test_attention: the fused QKV epilogue needs the TMA decode kernel");
+            aa.qkv_partial = qkv_partial; aa.qkv_ksplit = ksplit; aa.freqs = freqs;
+        } else {
+            QkvEpiArgs qa;
+            qa.partial = qkv_partial; qa.ksplit = ksplit; qa.M = R * Tq; qa.Tq = Tq; qa.D = H * hd; qa.H = H; qa.hd = hd;
+            qa.pos = aa.pos; qa.freqs = freqs; qa.q = q_out; qa.kcache = const_cast<void*>(aa.kcache); qa.vcache = const_cast<void*>(aa.vcache);
+            qa.maxS = max_seq; qa.dtype = dtype; qa.hdp = hdp;
+            qa.kv_f8 = aa.kv_f8; qa.k_inv = aa.k_inv; qa.v_inv = aa.v_inv;
+            LG_TRY(launch_qkv_epilogue(qa, st));
+        }
+    }
+    return launch_attention(aa, st, path);
 }
 
 int lg_test_gemm_dx(const void* x, const void* wa, const void* wb, int M, int N, int K, int mode, const void* normw, float eps,

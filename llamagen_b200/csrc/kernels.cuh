@@ -137,17 +137,26 @@ struct AttnArgs {
     int kv_f8 = 0;
     float k_inv = 1.f, v_inv = 1.f, v_scale = 1.f;
 };
-int launch_attention(const AttnArgs& a, cudaStream_t st);
+// path (optional, int[3]): the kernel that was launched (0 = attention_kernel, 1 = attn_tma_kernel, 2 = attn_tma_v2_kernel,
+// 3 = attn_prefill_tc_kernel), its TMA ring depth (0 for attention_kernel, 1 for the single-stage prefill) and whether it fused the
+// QKV epilogue
+int launch_attention(const AttnArgs& a, cudaStream_t st, int* path = nullptr);
+inline void set_attn_path(int* path, int kernel, int stages, int fused) {
+    if (path) { path[0] = kernel; path[1] = stages; path[2] = fused; }
+}
 // attn_tma.cu — TMA + tensor-core decode attention for bf16 / fp16 caches (dtype: LG_DTYPE_BF16 or LG_DTYPE_F16) and fp8 caches of
 // those models (map dtype LG_DTYPE_E4M3: 64- or 128-byte boxes)
 int attn_tma_make_map(void* map_out /*CUtensorMap, 128 B*/, const void* cache_base, long long total_rows, int hdp, int dtype,
                       int tail16 = 0);
+// whether KV-cache tensor maps are built for a workspace (and the TMA attention kernels can run): 16-bit model, hd 64 / 128 or
+// hd 100 in 112-wide rows, fewer than 2^31 cache rows over all layers
+bool attn_tma_maps_usable(int dtype, int hd, int hdp, long long total_rows);
 bool attn_tma_supported(const AttnArgs& a);
 bool attn_tma_enabled();
-int launch_attention_tma(const AttnArgs& a, cudaStream_t st);
+int launch_attention_tma(const AttnArgs& a, cudaStream_t st, int* path = nullptr);
 // t2i condition prefill (1 < Tq <= 128, hd 64, bf16 / fp16): TMA-staged Q/K/V, mma.sync QK^T and PV, one CTA per (row, head)
 bool attn_prefill_tc_supported(const AttnArgs& a);
-int launch_attention_prefill_tc(const AttnArgs& a, cudaStream_t st);
+int launch_attention_prefill_tc(const AttnArgs& a, cudaStream_t st, int* path = nullptr);
 // conv_tc.cu — wgmma implicit-GEMM convolution over bf16 NHWC activations (TMA 4-D boxes, register accumulators)
 bool conv_tc_supported(int Hin, int Win, int Cin, int Cout, int ksize, int up, bool nchw_out);
 void conv_tc_set_cta_budget(int ctas);   // > 0: persistent conv CTAs (at most `ctas`), 0: one CTA per tile, -1: LG_CONV_CTAS

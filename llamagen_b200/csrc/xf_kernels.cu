@@ -502,10 +502,11 @@ static int launch_attention_t(const AttnArgs& a, cudaStream_t st) {
     return 0;
 }
 
-int launch_attention(const AttnArgs& a, cudaStream_t st) {
-    if (attn_tma_supported(a) && attn_tma_enabled()) return launch_attention_tma(a, st);
-    if (attn_prefill_tc_supported(a) && attn_tma_enabled() && a.qkv_partial == nullptr) return launch_attention_prefill_tc(a, st);
+int launch_attention(const AttnArgs& a, cudaStream_t st, int* path) {
+    if (attn_tma_supported(a) && attn_tma_enabled()) return launch_attention_tma(a, st, path);
+    if (attn_prefill_tc_supported(a) && attn_tma_enabled() && a.qkv_partial == nullptr) return launch_attention_prefill_tc(a, st, path);
     LG_REQUIRE(a.qkv_partial == nullptr, "attention: fused QKV epilogue requested on a path that does not support it");
+    set_attn_path(path, 0, 0, 0);
     LG_REQUIRE((long long)a.R * a.Tq <= 65535, "attention: too many query rows (%d x %d)", a.R, a.Tq);
     LG_REQUIRE(a.hdp == 0 || a.hdp == a.hd || (a.hd == 100 && a.hdp == 112 && lg_dtype_is16(a.dtype)), "attention: unsupported KV row stride %d for head_dim %d", a.hdp, a.hd);
     if (a.kv_f8) {   // fp8 cache of a 16-bit model

@@ -162,7 +162,7 @@ def test_sampling_run_is_seed_reproducible_and_in_range():
 
 
 def test_attention_kernels_agree_large_batch_t2i(monkeypatch):
-    """The persistent warp-per-item TMA attention (taken when rows*heads >= 592), the CTA-per-item TMA kernel and
+    """The persistent warp-per-item TMA attention (taken when rows*heads >= 4 * 132 = 528), the CTA-per-item TMA kernel and
     the CUDA-core kernel must agree on a masked t2i decode at a batch large enough to select each of them."""
     g = load_golden("gpt_t2i.pt")
     B, S = 160, 6
@@ -257,8 +257,8 @@ def test_small_row_decode_path(B, monkeypatch):
 
 
 def test_small_grid_attention_parallel_chunks_long_context(monkeypatch):
-    """Few (row, head) items take the 6-stage attention whose warp groups process the chunks of a context concurrently
-    (attn_tma.cu, NST = 6). A 400-token context (> 6 x 48 keys) also exercises the per-group stage refill. It must agree
+    """Few (row, head) items take the 8-stage attention whose warp groups process the chunks of a context concurrently
+    (attn_tma.cu, NST = 8). A 400-token context (> 8 x 32 keys) also exercises the per-group stage refill. It must agree
     with the 2-stage kernel (same arithmetic per key, different merge order) and stay greedy-identical where decisive."""
     from llamagen_b200.gpt import ModelArgs, Transformer
     torch.manual_seed(4)
@@ -278,7 +278,7 @@ def test_small_grid_attention_parallel_chunks_long_context(monkeypatch):
 
 def test_small_row_path_t2i_masked_condition(monkeypatch):
     """t2i decode at R = 6 rows on the small-row path: the 120-token condition prefix is masked per image (emb_masks,
-    generate.py:154-163) inside the 6-stage attention; the batched path is the reference point."""
+    generate.py:154-163) inside the 8-stage attention; the batched path is the reference point."""
     from llamagen_b200.gpt import ModelArgs, Transformer
     torch.manual_seed(8)
     m = Transformer(ModelArgs(n_layer=3, n_head=4, dim=256, block_size=64, vocab_size=1024, cls_token_num=120, caption_dim=64,
