@@ -195,8 +195,8 @@ int         lg_vq_set_cta_budget(int ctas);
 int  lg_test_gemm(const void* x, const void* w, int M, int N, int K, int dtype, float* y,
                   void* dev_scratch, size_t scratch_bytes, void* stream);
 
-/* One transformer attention call through the engine's own dispatch (honouring LG_ATTN_TMA, LG_ATTN_PREFILL_TC, LG_ATTN_NST,
- * LG_ATTN_DEEP and LG_ATTN_V2). dtype: the model dtype (LG_DTYPE_F32, _BF16 or _F16); kv_dtype: dtype, or LG_DTYPE_E4M3 for a
+/* One transformer attention call through the engine's own dispatch (honouring LG_ATTN_TMA, LG_ATTN_PREFILL_TC, LG_ATTN_NST
+ * and LG_ATTN_DEEP). dtype: the model dtype (LG_DTYPE_F32, _BF16 or _F16); kv_dtype: dtype, or LG_DTYPE_E4M3 for a
  * 16-bit model with k_scale / v_scale powers of two in [2^-8, 2^7] (otherwise both 1). kcache / vcache: dev [n_layer][R][H][max_seq]
  * [hdp] in the KV dtype; `layer` is the one attended to. The tensor maps span all n_layer layers, as lg_engine_set_workspace builds
  * them. Query row m = r * Tq + t sits at position pos(r) + t, pos(r) = pos_rows ? pos_rows[r] : (pos_dev ? *pos_dev : 0) + pos_value,
@@ -204,20 +204,13 @@ int  lg_test_gemm(const void* x, const void* w, int M, int N, int K, int dtype, 
  * Input: q (dev [R * Tq][H * hd], post-RoPE) or the QKV GEMM's split-K slabs qkv_partial (dev f32 [ksplit][R * Tq][3 * H * hd]) with
  * freqs (dev f32 [max_seq][hd / 2][2]): fuse = 0 runs the QKV epilogue (q -> q_out, K / V rows written at the query positions) and
  * then the attention; fuse = 1 lets the TMA decode kernel do the epilogue itself (Tq = 1). out: dev [R * Tq][H * hd].
- * path (int[3]) or NULL: kernel (0 = attention_kernel, 1 = attn_tma_kernel, 2 = attn_tma_v2_kernel, 3 = attn_prefill_tc_kernel),
+ * path (int[3]) or NULL: kernel (0 = attention_kernel, 1 = attn_tma_kernel, 3 = attn_prefill_tc_kernel; 2 is unused),
  * TMA ring depth (0 for attention_kernel) and whether the QKV epilogue was fused. Every argument is checked before any launch;
  * the caller keeps *pos_dev + pos_value + Tq <= max_seq and pos_rows[r] < max_seq. */
 int  lg_test_attention(int dtype, int kv_dtype, float k_scale, float v_scale, int R, int Tq, int H, int hd, int hdp, int max_seq,
                        void* kcache, void* vcache, int n_layer, int layer, int pos_value, const int32_t* pos_dev,
                        const int32_t* pos_rows, const float* emb_mask, int B, int Tc, const void* q, const float* qkv_partial,
                        int ksplit, const float* freqs, int fuse, void* q_out, void* out, int* path, void* stream);
-
-/* The decode step's direct-epilogue GEMM (csrc/gemm_dx.cu) on its own. mode 0: y (f32 [M,N]) = norm(x) * wa^T; mode 1: h (bf16
- * [M,N], in place) = bf16(h + bf16(norm(x) * wa^T)) — the residual add of gpt.py:255-256; mode 2: ff (bf16 [M,N]) =
- * silu(norm(x) * wa^T) * (norm(x) * wb^T) — gpt.py:167. norm(x) = RMSNorm(x) * normw (gpt.py:143-148) when normw != NULL, else x.
- * x [M,K], wa/wb [N,K], normw [K]: bf16 device pointers. */
-int  lg_test_gemm_dx(const void* x, const void* wa, const void* wb, int M, int N, int K, int mode, const void* normw,
-                     float eps, void* out, void* stream);
 
 /* One VQ decoder/encoder convolution through the decoder's own dispatch (the mma.sync gather kernel or either wgmma kernel,
  * honouring LG_CONV_TC, LG_CONV_SWAP, LG_GN_FUSE and the CTA budget), optionally followed by GroupNorm(32, eps 1e-6)

@@ -8,8 +8,6 @@
 // only the valid prefix [0, pos] is read. Mask rule: generate.py:154-163 (emb_masks on the condition keys).
 #include "kernels.cuh"
 #include "tma_utils.cuh"
-#include <algorithm>
-#include <type_traits>
 
 namespace {
 
@@ -448,186 +446,6 @@ __global__ void __launch_bounds__(kWarps * 32 * (PAR_ ? NST : 1), PAR_ ? 1 : (HD
     }
 }
 
-// ---------------------------------------------------------------------------------------------------
-// v2: persistent, one WARP per (row, head) work item. Every warp owns a private 3-stage TMA ring (its own
-// mbarriers), so there is no CTA-wide synchronisation at all, the ring keeps streaming across item
-// boundaries (the next item's first chunks are requested while the current item is still being reduced),
-// and q for the next item is prefetched into registers. 4 warps x 3 stages x 16 KB = 192 KB of loads in
-// flight per SM.
-// ---------------------------------------------------------------------------------------------------
-constexpr int kWarpsV2 = 4;
-constexpr int kStagesV2 = 3;
-
-template <int HD>
-__global__ void __launch_bounds__(kWarpsV2 * 32, 1) attn_tma_v2_kernel(const __grid_constant__ CUtensorMap kmap,
-                                                                       const __grid_constant__ CUtensorMap vmap, AttnTmaArgs a) {
-    constexpr int NSUB = HD / 64;
-    constexpr int SUB_BYTES = kKC * 128;
-    constexpr int TILE_BYTES = NSUB * SUB_BYTES;
-    constexpr int WARP_BYTES = kStagesV2 * 2 * TILE_BYTES;
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* tiles_all = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(tiles_all + kWarpsV2 * WARP_BYTES);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, tg = lane & 3;
-    uint8_t* tiles = tiles_all + warp * WARP_BYTES;
-    uint64_t* full_bar = bars + warp * kStagesV2;
-    if (lane == 0) {
-        if (warp == 0) { prefetch_map(&kmap); prefetch_map(&vmap); }
-        for (int s = 0; s < kStagesV2; ++s) mbar_init(&full_bar[s], 1);
-        fence_barrier_init();
-    }
-    __syncwarp();
-    lg_pdl_sync();     // K/V rows of this step and the position counter come from earlier kernels
-    const int qpos = (a.pos_dev ? *a.pos_dev : 0) + a.pos_value;
-    const int nkeys = qpos + 1;
-    const int nchunks = (nkeys + kKC - 1) / kKC;
-    const int D = a.H * HD;
-    const int nitems = a.R * a.H;
-    const int wid = blockIdx.x * kWarpsV2 + warp, nw = gridDim.x * kWarpsV2;
-    const int my_items = wid < nitems ? (nitems - wid + nw - 1) / nw : 0;
-    const long long total = (long long)my_items * nchunks;       // flattened (item, chunk) stream of this warp
-
-    auto issue = [&](long long f) {                               // lane 0 only
-        const int it = (int)(f / nchunks), ci = (int)(f - (long long)it * nchunks);
-        const int item = wid + it * nw;
-        const long long row0 = a.row_base + (long long)item * a.maxS;     // item = r*H + h
-        const int s = (int)(f % kStagesV2);
-        uint8_t* kt = tiles + s * 2 * TILE_BYTES;
-        uint8_t* vt = kt + TILE_BYTES;
-        mbar_expect_tx(&full_bar[s], 2 * TILE_BYTES);
-#pragma unroll
-        for (int sub = 0; sub < NSUB; ++sub) {
-            load_2d(kt + sub * SUB_BYTES, &kmap, &full_bar[s], sub * 64, (int)(row0 + (long long)ci * kKC));
-            load_2d(vt + sub * SUB_BYTES, &vmap, &full_bar[s], sub * 64, (int)(row0 + (long long)ci * kKC));
-        }
-    };
-    if (lane == 0)
-        for (long long f = 0; f < total && f < kStagesV2; ++f) issue(f);
-
-    auto load_q = [&](int item, uint32_t (*qa)[2]) {
-        const bf16* qp = a.q + (size_t)(item / a.H) * D + (size_t)(item % a.H) * HD;
-#pragma unroll
-        for (int kk = 0; kk < HD / 16; ++kk) {
-            qa[kk][0] = 0; qa[kk][1] = 0;
-            if (g == 0) {
-                qa[kk][0] = *reinterpret_cast<const uint32_t*>(qp + kk * 16 + tg * 2);
-                qa[kk][1] = *reinterpret_cast<const uint32_t*>(qp + kk * 16 + 8 + tg * 2);
-            }
-        }
-    };
-    uint32_t qa[HD / 16][2], qn[HD / 16][2];
-    if (my_items > 0) load_q(wid, qa);
-
-    long long f = 0;
-    for (int it = 0; it < my_items; ++it) {
-        const int item = wid + it * nw;
-        const int r = item / a.H;
-        if (it + 1 < my_items) load_q(item + nw, qn);             // prefetch the next item's query
-        const float* mrow = a.emb_mask ? a.emb_mask + (size_t)(r % a.B) * a.Tc : nullptr;
-        float o[HD / 8][2];
-#pragma unroll
-        for (int i = 0; i < HD / 8; ++i) { o[i][0] = 0.f; o[i][1] = 0.f; }
-        float mx = -INFINITY, l = 0.f;
-
-        for (int ci = 0; ci < nchunks; ++ci, ++f) {
-            const int s = (int)(f % kStagesV2);
-            mbar_wait(&full_bar[s], (uint32_t)((f / kStagesV2) & 1));
-            const uint32_t kt = smem_u32(tiles + s * 2 * TILE_BYTES);
-            const uint32_t vt = kt + TILE_BYTES;
-#pragma unroll 1
-            for (int sub16 = 0; sub16 < kKC / 16; ++sub16) {
-                const int j0 = ci * kKC + sub16 * 16;
-                if (j0 >= nkeys) break;
-                float sc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
-#pragma unroll
-                for (int kk = 0; kk < HD / 16; ++kk) {
-                    uint32_t b0, b1, b2, b3;
-                    const int row = sub16 * 16 + (lane & 7) + ((lane >> 4) << 3);
-                    const int chunk = (kk * 2 + ((lane >> 3) & 1)) & 7;
-                    ldsm_x4(kt + (kk / 4) * SUB_BYTES + swz(row, chunk), b0, b1, b2, b3);
-                    mma16816(sc[0], qa[kk][0], 0u, qa[kk][1], 0u, b0, b1);
-                    mma16816(sc[1], qa[kk][0], 0u, qa[kk][1], 0u, b2, b3);
-                }
-                float pv[4];
-                float lmax = -INFINITY;
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const int j = j0 + (i >> 1) * 8 + tg * 2 + (i & 1);
-                    bool vis = j < nkeys;
-                    if (vis && mrow && j < a.Tc && j != qpos) vis = mrow[j] != 0.f;
-                    pv[i] = vis ? sc[i >> 1][i & 1] * a.scale : -INFINITY;
-                    lmax = fmaxf(lmax, pv[i]);
-                }
-                lmax = fmaxf(lmax, __shfl_xor_sync(0xffffffffu, lmax, 1));
-                lmax = fmaxf(lmax, __shfl_xor_sync(0xffffffffu, lmax, 2));
-                const float mn = fmaxf(mx, lmax);
-                float corr = 1.f, lsum = 0.f;
-                if (mn != -INFINITY) {
-                    corr = __expf(mx - mn);
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) { pv[i] = __expf(pv[i] - mn); lsum += pv[i]; }
-                } else {
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) pv[i] = 0.f;
-                }
-                lsum += __shfl_xor_sync(0xffffffffu, lsum, 1);
-                lsum += __shfl_xor_sync(0xffffffffu, lsum, 2);
-                l = l * corr + lsum;
-                mx = mn;
-#pragma unroll
-                for (int i = 0; i < HD / 8; ++i) { o[i][0] *= corr; o[i][1] *= corr; }
-                const uint32_t pa0 = pack16(pv[0], pv[1]);
-                const uint32_t pa2 = pack16(pv[2], pv[3]);
-#pragma unroll
-                for (int np = 0; np < HD / 16; ++np) {
-                    uint32_t b0, b1, b2, b3;
-                    const int row = sub16 * 16 + (lane & 7) + (((lane >> 3) & 1) << 3);
-                    const int chunk = (np * 2 + (lane >> 4)) & 7;
-                    ldsm_x4_t(vt + (np / 4) * SUB_BYTES + swz(row, chunk), b0, b1, b2, b3);
-                    float c0[4] = {o[2 * np][0], o[2 * np][1], 0.f, 0.f};
-                    float c1[4] = {o[2 * np + 1][0], o[2 * np + 1][1], 0.f, 0.f};
-                    mma16816(c0, pa0, 0u, pa2, 0u, b0, b1);
-                    mma16816(c1, pa0, 0u, pa2, 0u, b2, b3);
-                    o[2 * np][0] = c0[0]; o[2 * np][1] = c0[1];
-                    o[2 * np + 1][0] = c1[0]; o[2 * np + 1][1] = c1[1];
-                }
-            }
-            __syncwarp();                                          // all lanes are done reading stage s
-            if (lane == 0 && f + kStagesV2 < total) issue(f + kStagesV2);
-        }
-        if (g == 0) {
-            bf16* op = a.out + (size_t)r * D + (size_t)(item % a.H) * HD;
-            const float inv = 1.0f / l;
-#pragma unroll
-            for (int i = 0; i < HD / 8; ++i)
-                *reinterpret_cast<uint32_t*>(op + i * 8 + tg * 2) = pack16(o[i][0] * inv, o[i][1] * inv);
-        }
-#pragma unroll
-        for (int kk = 0; kk < HD / 16; ++kk) { qa[kk][0] = qn[kk][0]; qa[kk][1] = qn[kk][1]; }
-    }
-}
-
-template <int HD>
-int launch_v2(const CUtensorMap& kmap, const CUtensorMap& vmap, const AttnTmaArgs& a, cudaStream_t st) {
-    constexpr int TILE_BYTES = (HD / 64) * kKC * 128;
-    constexpr int WARP_BYTES = kStagesV2 * 2 * TILE_BYTES;
-    const size_t smem = 1024 + (size_t)kWarpsV2 * WARP_BYTES + kWarpsV2 * kStagesV2 * sizeof(uint64_t);
-    static DevOnce attr;
-    static int sms = 132;
-    if (lg_first_on_device(attr)) {
-        LG_CUDA_OK(cudaFuncSetAttribute(attn_tma_v2_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    }
-    const int nitems = a.R * a.H;
-    const int ctas = std::min(sms, (nitems + kWarpsV2 - 1) / kWarpsV2);
-    (void)lg_launch(attn_tma_v2_kernel<HD>, dim3(ctas), dim3(kWarpsV2 * 32), smem, st, kmap, vmap, a);
-    LG_LAUNCH_CHECK();
-    return 0;
-}
-
 template <typename T, int HD, bool FUSED, int NST = kStagesA, bool PAR = (NST > 2), bool F8 = false>
 int launch_t(const CUtensorMap& kmap, const CUtensorMap& vmap, const CUtensorMap& kmap16, const CUtensorMap& vmap16,
              const AttnTmaArgs& a, cudaStream_t st, const KvScales& f8s) {
@@ -921,16 +739,11 @@ static int launch_attention_tma_t(const AttnArgs& a, cudaStream_t st, int* path)
         if (a.hd == 64 && a.R * a.H <= 2 * 132 && lg_env_flag("LG_ATTN_DEEP", 1))
             return ran(launch_t<T, 64, true, kDeepStages, (kDeepStages > 2), F8>(km, vm, km16, vm16, t, st, f8s), 1, kDeepStages);
         // deeper sequential ring (A/B switch): more keys requested before the dependency wait, fewer refill round trips
-        const int nst = lg_env_flag("LG_ATTN_NST", 2);
-        if (a.hd == 64 && nst == 3) return ran(launch_t<T, 64, true, 3, false, F8>(km, vm, km16, vm16, t, st, f8s), 1, 3);
-        if (a.hd == 64 && nst == 4) return ran(launch_t<T, 64, true, 4, false, F8>(km, vm, km16, vm16, t, st, f8s), 1, 4);
+        if (a.hd == 64 && lg_env_flag("LG_ATTN_NST", 2) == 3)
+            return ran(launch_t<T, 64, true, 3, false, F8>(km, vm, km16, vm16, t, st, f8s), 1, 3);
         if (a.hd == 64) return ran(launch_t<T, 64, true, kStagesA, false, F8>(km, vm, km16, vm16, t, st, f8s), 1, kStagesA);
         return ran(launch_t<T, 128, true, kStagesA, false, F8>(km, vm, km16, vm16, t, st, f8s), 1, kStagesA);
     }
-    // v2 (persistent warp-per-item, LG_ATTN_V2=1) stays opt-in: with one warp per scheduler its ldmatrix->mma->softmax chain is
-    // latency-bound, which made it slower than the CTA-per-item kernel where it was measured. bf16 caches only.
-    const bool v2 = !F8 && std::is_same<T, bf16>::value && lg_env_flag("LG_ATTN_V2", 0) && a.R * a.H >= 4 * 132 && a.hd == 64 && !a.pos.rows;
-    if (v2) return ran(launch_v2<64>(km, vm, t, st), 2, kStagesV2);
     if (a.hd == 64) return ran(launch_t<T, 64, false, kStagesA, false, F8>(km, vm, km16, vm16, t, st, f8s), 1, kStagesA);
     return ran(launch_t<T, 128, false, kStagesA, false, F8>(km, vm, km16, vm16, t, st, f8s), 1, kStagesA);
 }

@@ -149,9 +149,6 @@ struct lg_engine {
     Workspace full, sub[kMaxChains];      // sub[g]: rows/n_sub each, carved INSIDE the regions of `full` (multi-chain decode)
     int n_sub = 0;                        // 0: no split available
     bool use_graph = true;
-    PdLayerW* d_layers = nullptr;         // device copy of the per-layer weight pointers (persistent small-row decode kernel)
-    const int32_t* pd_tokens = nullptr;   // set by the caller of forward() when the step's token ids are in device memory and the
-                                          // embedding lookup has NOT been launched (the persistent kernel gathers the rows itself)
     bool ws_needs_zero = false;           // KV cache + counters of `full` still have to be zero-filled (done on the caller's stream)
     bool skip_first_norm = false;         // set by the decode loop when the sample kernel's fused tail already wrote xn = RMSNorm_0(h)
     cudaStream_t works[kMaxChains] = {};   // engine-owned streams (one per chain)
@@ -162,13 +159,6 @@ struct lg_engine {
             if (ev_joins[i]) cudaEventDestroy(ev_joins[i]);
         }
         if (ev_fork) cudaEventDestroy(ev_fork);
-        if (d_layers) cudaFree(d_layers);
-    }
-    // R <= 8 decode steps can run as ONE persistent cooperative kernel per token (decode_persist.cu)
-    bool persist_usable(int R) const {
-        return lg_env_flag("LG_PERSIST", 0) && d_layers && cfg.dtype == LG_DTYPE_BF16 && !kv_f8 && ws.have_maps &&
-               decode_persist_supported(R, cfg.dim, cfg.ffn_dim, cfg.vocab_size, cfg.n_head, hd, cfg.dtype) &&
-               decode_persist_part_floats(R, cfg.n_head, hd) <= ws.partial_floats;
     }
 
     // R <= 8 decode steps on the column-owner GEMV path (gemv_small.cu); shared by forward() and the decode loop's fused tail
@@ -223,12 +213,11 @@ size_t lg_engine::carve(Workspace& o, char* base, int rows, int max_seq) const {
         if (cfg.model_type == LG_MODEL_T2I) pf = std::max(pf, gemm_partial_floats(M, D, cfg.caption_dim, cfg.dtype));
     }
     pf = std::max(pf, gemm_partial_floats(rows, V, D, cfg.dtype));
-    if (cfg.dtype == LG_DTYPE_BF16) pf = std::max(pf, (size_t)std::min(rows, 8) * H * 8 * (hd + 2));   // decode_persist.cu partials
     o.partial_floats = pf;
     o.partial = (float*)take(pf * sizeof(float));
     o.logits = (float*)take((size_t)rows * V * sizeof(float));
     o.tokens = (int32_t*)take((size_t)rows * sizeof(int32_t));
-    o.counters = (int*)take(128 * sizeof(int));   // [0, 16): pos/step per chain (<= 8 chains); [96, 98): grid-barrier counters of decode_persist.cu
+    o.counters = (int*)take(128 * sizeof(int));   // [0, 16): pos/step per chain (<= 8 chains)
     o.rows = rows;
     o.max_seq = max_seq;
     return off;
@@ -271,21 +260,6 @@ int lg_engine::forward(int M, int Tq, PosArg pos, const float* emb_mask, int B, 
         }
         return aa;
     };
-    // ---- R <= 8 decode step as ONE persistent cooperative kernel (decode_persist.cu): the caller passed the token ids
-    if (Tq == 1 && M <= 8 && pd_tokens) {
-        const int32_t* toks = pd_tokens;
-        pd_tokens = nullptr;
-        PdLaunch p{};
-        p.L = L; p.D = D; p.F = F; p.V = V; p.H = H; p.hd = hd; p.R = M; p.B = B; p.Tc = cfg.cls_token_num; p.maxS = ws.max_seq;
-        p.eps = cfg.norm_eps; p.scale = 1.0f / sqrtf((float)hd);
-        p.layers = d_layers; p.final_norm = final_norm; p.output = output; p.tok_emb = tok_emb; p.freqs = freqs;
-        p.kcache = ws.kcache; p.vcache = ws.vcache; p.layer_elems = ws.layer_cache_bytes / esz;
-        p.h = ws.h; p.q = ws.q; p.ff = ws.ff; p.part = ws.partial; p.part_floats = ws.partial_floats; p.logits = logits_out;
-        p.tokens = toks; p.pos_dev = pos.dev; p.pos_value = pos.value; p.emb_mask = emb_mask;
-        p.bar = (unsigned int*)(ws.counters + 96);
-        LG_PROF(PC_PERSIST, st, launch_decode_persist(p, st));
-        return 0;
-    }
     // ---- R <= 8 decode step (batch-1 latency path, gemv_small.cu): 5 dependent kernels per layer, no slabs
     if (Tq == 1 && small_row_path(M, attn_args(0))) {
         skip_first_norm = false;
@@ -309,11 +283,6 @@ int lg_engine::forward(int M, int Tq, PosArg pos, const float* emb_mask, int B, 
     }
     if (!skip_first_norm) LG_PROF(PC_EMBED_MISC, st, launch_rmsnorm(ws.h, layers[0].attn_norm, ws.xn, M, D, cfg.norm_eps, dt, st));
     skip_first_norm = false;
-    // Direct-epilogue GEMMs (gemm_dx.cu, 6 kernels per layer instead of 8) are validated but OFF by default: a CTA that owns the full
-    // reduction runs its k-blocks as one dependent MMA chain on a single feature tile, so it is serial where the split-K GEMM spreads
-    // the same bytes over ksplit CTAs. It has not been measured against the split-K path on the H100.
-    const bool dx = Tq == 1 && M <= 256 && lg_env_flag("LG_DIRECT", 0) && gemm_dx_supported(M, D, D, dt, DX_RESID, false) &&
-                        gemm_dx_supported(M, F, D, dt, DX_SWIGLU, true);
     for (int l = 0; l < L; ++l) {
         const Layer& ly = layers[l];
         char* kc = ws.kcache + (size_t)l * ws.layer_cache_bytes;
@@ -329,29 +298,18 @@ int lg_engine::forward(int M, int Tq, PosArg pos, const float* emb_mask, int B, 
         qa.pos = pos; qa.freqs = freqs; qa.q = ws.q; qa.kcache = kc; qa.vcache = vc; qa.maxS = ws.max_seq; qa.dtype = dt; qa.hdp = hdp;
         AttnArgs aa = attn_args(l);
         qa.kv_f8 = aa.kv_f8; qa.k_inv = aa.k_inv; qa.v_inv = aa.v_inv;
-        // decode steps on the TMA path: the attention kernel is also the QKV epilogue (one dependent kernel less); LG_ATTN_V2 unfuses
-        // it for its bf16-cache kernel only
-        const bool fuse_qkv = lg_env_flag("LG_FUSE_QKV", 1) && attn_tma_enabled() && attn_tma_supported(aa) &&
-                              !(!kv_f8 && lg_env_flag("LG_ATTN_V2", 0) && R * H >= 4 * 132 && hd == 64);
+        // decode steps on the TMA path: the attention kernel is also the QKV epilogue (one dependent kernel less)
+        const bool fuse_qkv = lg_env_flag("LG_FUSE_QKV", 1) && attn_tma_enabled() && attn_tma_supported(aa);
         if (fuse_qkv) {
             aa.qkv_partial = ws.partial; aa.qkv_ksplit = ks; aa.freqs = freqs;
         } else {
             LG_PROF(PC_QKV_EPI, st, launch_qkv_epilogue(qa, st));
         }
         LG_PROF(PC_ATTENTION, st, launch_attention(aa, st));
-        if (dx) {
-            // decode step: WO with the residual add in its drain, then w1|w3 with the RMSNorm on its resident rows and the SwiGLU
-            // gate in its drain (gemm_dx.cu) — two dependent kernels instead of four, no split-K slabs
-            GemmDx go{ws.attn, D, ly.wo, nullptr, M, D, D, DX_RESID, nullptr, 0.f, nullptr, ws.h, nullptr};
-            LG_PROF(PC_GEMM_WO, st, launch_gemm_dx(go, st, &nx_w13));
-            GemmDx g13{ws.h, D, ly.w1, ly.w3, M, F, D, DX_SWIGLU, ly.ffn_norm, cfg.norm_eps, nullptr, nullptr, ws.ff};
-            LG_PROF(PC_GEMM_W13, st, launch_gemm_dx(g13, st, &nx_w2));
-        } else {
-            LG_PROF(PC_GEMM_WO, st, gemm(ws.attn, M, D, D, ly.wo, nullptr, 0, &ks, nullptr, st, &nx_w13));
-            LG_PROF(PC_RESNORM, st, launch_residual_norm(ws.partial, ks, M, D, ws.h, ly.ffn_norm, ws.xn, cfg.norm_eps, dt, st));
-            LG_PROF(PC_GEMM_W13, st, gemm(ws.xn, M, 2 * F, D, ly.w1, ly.w3, F, &ks, nullptr, st, &nx_w2));
-            LG_PROF(PC_SILU, st, launch_silu_mul(ws.partial, ks, M, F, ws.ff, dt, st));
-        }
+        LG_PROF(PC_GEMM_WO, st, gemm(ws.attn, M, D, D, ly.wo, nullptr, 0, &ks, nullptr, st, &nx_w13));
+        LG_PROF(PC_RESNORM, st, launch_residual_norm(ws.partial, ks, M, D, ws.h, ly.ffn_norm, ws.xn, cfg.norm_eps, dt, st));
+        LG_PROF(PC_GEMM_W13, st, gemm(ws.xn, M, 2 * F, D, ly.w1, ly.w3, F, &ks, nullptr, st, &nx_w2));
+        LG_PROF(PC_SILU, st, launch_silu_mul(ws.partial, ks, M, F, ws.ff, dt, st));
         LG_PROF(PC_GEMM_W2, st, gemm(ws.ff, M, D, F, ly.w2, nullptr, 0, &ks, nullptr, st, &nx_qkv));
         const void* next_norm = (l + 1 < L) ? layers[l + 1].attn_norm : final_norm;
         LG_PROF(PC_RESNORM, st, launch_residual_norm(ws.partial, ks, M, D, ws.h, next_norm, ws.xn, cfg.norm_eps, dt, st));
@@ -488,17 +446,6 @@ int lg_engine_finalize(lg_engine* e) {
     const void* fr = nullptr;
     LG_TRY(need(e, "freqs_cis", LG_DTYPE_F32, {c.cls_token_num + c.block_size, e->hd / 2, 2}, &fr));
     e->freqs = (const float*)fr;
-    if (dt == LG_DTYPE_BF16) {
-        DeviceGuard guard(e->device);
-        std::vector<PdLayerW> hl(c.n_layer);
-        for (int l = 0; l < c.n_layer; ++l) {
-            const Layer& ly = e->layers[l];
-            hl[l] = PdLayerW{(const bf16*)ly.wqkv, (const bf16*)ly.wo, (const bf16*)ly.w1, (const bf16*)ly.w3, (const bf16*)ly.w2,
-                             (const bf16*)ly.attn_norm, (const bf16*)ly.ffn_norm};
-        }
-        if (!e->d_layers) LG_CUDA_OK(cudaMalloc(&e->d_layers, sizeof(PdLayerW) * c.n_layer));
-        LG_CUDA_OK(cudaMemcpy(e->d_layers, hl.data(), sizeof(PdLayerW) * c.n_layer, cudaMemcpyHostToDevice));
-    }
     e->finalized = true;
     return 0;
 }
@@ -665,8 +612,7 @@ int lg_decode_step(lg_engine* e, const int32_t* tokens, int B, int pos, int use_
     LG_TRY(check_ready(e, R, pos + 1));
     LG_TRY(e->zero_fill_if_needed(st));
     LG_REQUIRE(tokens && logits_out && B > 0 && pos >= 0, "lg_decode_step: bad argument");
-    if (e->persist_usable(R)) e->pd_tokens = tokens;
-    else LG_TRY(launch_embed(e->tok_emb, tokens, B, R, -1, e->cfg.dim, e->cfg.dtype, e->ws.h, st));
+    LG_TRY(launch_embed(e->tok_emb, tokens, B, R, -1, e->cfg.dim, e->cfg.dtype, e->ws.h, st));
     PosArg p{nullptr, pos};
     LG_TRY(e->forward(R, 1, p, nullptr, B, logits_out, false, st));
     LG_TRY(round_logits_inplace(logits_out, (size_t)R * e->cfg.vocab_size, e->cfg.dtype, st));
@@ -686,7 +632,6 @@ int lg_decode_rows(lg_engine* e, const int32_t* tokens, const int32_t* pos_rows,
     LG_REQUIRE(e->cfg.model_type == LG_MODEL_C2I && e->cfg.cls_token_num == 1, "lg_decode_rows: class-conditional models only");
     LG_TRY(launch_embed_rows(e->cls_table, e->tok_emb, tokens, pos_rows, B, R, e->cfg.num_classes, e->cfg.dim, e->cfg.dtype, e->ws.h, st));
     PosArg p{nullptr, 0, pos_rows};
-    e->pd_tokens = nullptr;
     LG_TRY(e->forward(R, 1, p, nullptr, B, logits_out, false, st));
     LG_TRY(round_logits_inplace(logits_out, (size_t)R * e->cfg.vocab_size, e->cfg.dtype, st));
     return 0;
@@ -777,8 +722,8 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
     const lg_model_cfg& c = e->cfg;
 
     // Multi-chain decode: at large batch every kernel of a decode step is latency-bound (a few microseconds of
-    // dependent load -> compute -> store), so the batch is cut into LG_SPLIT (default 2, max 8) independent chains (their own KV-cache half,
-    // stream and CUDA graph) whose kernels interleave on the GPU. Each image's arithmetic is unchanged, so the result
+    // dependent load -> compute -> store), so the batch is cut into n_sub independent chains (the chain-count policy of
+    // lg_engine_set_workspace, which LG_SPLIT overrides; each chain has its own KV-cache slice, stream and CUDA graph) whose kernels interleave on the GPU. Each image's arithmetic is unchanged, so the result
     // is bit-identical to the single-chain run.
     const bool split = e->n_sub >= 2 && lg_env_flag("LG_SPLIT", 2) >= 2 && R == e->full.rows && B % e->n_sub == 0 &&
                        !prof_enabled() && !lg_debug_sync();
@@ -808,10 +753,6 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
     // Fused tail (bf16 / fp16): the sample kernel writes the next step's input rows (token embedding, and on the batched path the layer-0
     // RMSNorm) and advances the device-resident counters, so a decode iteration loses its embed / rmsnorm / advance kernels.
     const bool fuse_tail = lg_dtype_is16(c.dtype) && lg_env_flag("LG_FUSE_TAIL", 1) && c.dim % 2 == 0;
-    auto tail_on = [&](Chain& k) -> bool {
-        e->ws = k.w;
-        return fuse_tail && !e->persist_usable(k.R);
-    };
     auto arm_tail = [&](Chain& k, bool advance) {
         SampleArgs& sa = k.sa;
         e->ws = k.w;
@@ -830,17 +771,14 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
         e->ws = k.w;
         int* d_pos = k.w.counters;
         int* d_step = k.w.counters + 1;
-        const bool tail = tail_on(k);
-        if (tail) {
+        if (fuse_tail) {
             e->skip_first_norm = k.sa.emb_xn != nullptr;     // the previous iteration's sample kernel left h (and xn) in place
-        } else if (e->persist_usable(k.R)) {
-            e->pd_tokens = k.w.tokens;
         } else {
             LG_PROF(PC_EMBED_MISC, k.st, launch_embed(e->tok_emb, k.w.tokens, k.B, k.R, -1, c.dim, c.dtype, k.w.h, k.st));
         }
         LG_TRY(e->forward(k.R, 1, PosArg{d_pos, 0}, k.emb_mask, k.B, k.w.logits, false, k.st));
         LG_PROF(PC_SAMPLE, k.st, launch_sample(k.sa, k.st));
-        if (!tail) LG_PROF(PC_EMBED_MISC, k.st, launch_advance(d_pos, d_step, k.st));
+        if (!fuse_tail) LG_PROF(PC_EMBED_MISC, k.st, launch_advance(d_pos, d_step, k.st));
         return 0;
     };
 
@@ -851,7 +789,7 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
         LG_TRY(e->embed_cond(k.cond, k.B, k.R, T, k.st));
         LG_TRY(e->forward(k.R * T, T, PosArg{nullptr, 0}, k.emb_mask, k.B, k.w.logits, false, k.st));
         k.sa.step = 0; k.sa.step_dev = nullptr;
-        const bool tail = S > 1 && tail_on(k);
+        const bool tail = S > 1 && fuse_tail;
         if (tail) arm_tail(k, false);            // the prefill's sample prepares the first decode step's rows; counters are set below
         LG_TRY(launch_sample(k.sa, k.st));
         if (S == 1) continue;
@@ -867,18 +805,15 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
             for (int g = 0; g < nchains; ++g) LG_TRY(body(ch[g]));
         return 0;
     }
-    // ---- decode loop (generate.py:105-123): per chain one captured graph of `unroll` consecutive steps (the loop
-    // state is device-resident, so every step has identical kernel arguments), replayed, chains interleaved; the
-    // remainder runs through a second single-step graph. The default is one step per graph (LG_GRAPH_UNROLL > 1 captures more):
-    // with two chains the gap between graph launches of one chain is covered by the other chain's kernels.
+    // ---- decode loop (generate.py:105-123): per chain one captured graph of one decode step (the loop state is
+    // device-resident, so every step has identical kernel arguments), replayed, chains interleaved: with two chains the
+    // gap between graph launches of one chain is covered by the other chain's kernels.
     int ret = 0;
-    const int unroll = std::max(1, std::min(lg_env_flag("LG_GRAPH_UNROLL", 1), remaining));
-    auto capture = [&](Chain& k, int nsteps, cudaGraph_t* graph, cudaGraphExec_t* exec, uint64_t* launches) -> int {
+    auto capture = [&](Chain& k, cudaGraph_t* graph, cudaGraphExec_t* exec, uint64_t* launches) -> int {
         cudaError_t ce = cudaStreamBeginCapture(k.st, cudaStreamCaptureModeRelaxed);
         if (ce != cudaSuccess) return lg_fail("cudaStreamBeginCapture failed: %s", cudaGetErrorString(ce));
         const uint64_t before = g_lg_launches.load();
-        int rc = 0;
-        for (int i = 0; i < nsteps && rc == 0; ++i) rc = body(k);
+        const int rc = body(k);
         *launches = g_lg_launches.load() - before;
         ce = cudaStreamEndCapture(k.st, graph);
         g_lg_launches.fetch_sub(*launches);  // the capture pass launched nothing
@@ -888,31 +823,13 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
         if (ce != cudaSuccess) return lg_fail("cudaGraphInstantiate failed: %s", cudaGetErrorString(ce));
         return 0;
     };
-    cudaGraph_t g1[lg_engine::kMaxChains] = {};
-    cudaGraphExec_t e1[lg_engine::kMaxChains] = {};
-    uint64_t l1[lg_engine::kMaxChains] = {};
-    const int nbig = remaining / unroll, nsmall = remaining - nbig * unroll;
-    for (int g = 0; g < nchains && ret == 0; ++g) {
-        ret = capture(ch[g], unroll, &ch[g].graph, &ch[g].exec, &ch[g].per_step);
-        if (ret == 0 && nsmall > 0 && unroll > 1) ret = capture(ch[g], 1, &g1[g], &e1[g], &l1[g]);
-    }
-    for (int i = 0; i < nbig && ret == 0; ++i) {
+    for (int g = 0; g < nchains && ret == 0; ++g) ret = capture(ch[g], &ch[g].graph, &ch[g].exec, &ch[g].per_step);
+    for (int i = 0; i < remaining && ret == 0; ++i) {
         for (int g = 0; g < nchains; ++g) {
             const cudaError_t ce = cudaGraphLaunch(ch[g].exec, ch[g].st);
             if (ce != cudaSuccess) { ret = lg_fail("cudaGraphLaunch failed: %s", cudaGetErrorString(ce)); break; }
             g_lg_launches.fetch_add(ch[g].per_step);
         }
-    }
-    for (int i = 0; i < nsmall && ret == 0 && unroll > 1; ++i) {
-        for (int g = 0; g < nchains; ++g) {
-            const cudaError_t ce = cudaGraphLaunch(e1[g], ch[g].st);
-            if (ce != cudaSuccess) { ret = lg_fail("cudaGraphLaunch failed: %s", cudaGetErrorString(ce)); break; }
-            g_lg_launches.fetch_add(l1[g]);
-        }
-    }
-    for (int g = 0; g < nchains; ++g) {
-        if (e1[g]) cudaGraphExecDestroy(e1[g]);
-        if (g1[g]) cudaGraphDestroy(g1[g]);
     }
     for (int g = 0; g < nchains; ++g) {
         if (ch[g].exec) cudaGraphExecDestroy(ch[g].exec);
@@ -949,7 +866,7 @@ int lg_profile_read(int cls, double* total_ms, uint64_t* launches) {
 const char* lg_profile_class_name(int cls) {
     static const char* names[PC_COUNT] = {"gemm_qkv", "qkv_rope_kvwrite", "attention", "gemm_wo", "residual_rmsnorm",
                                           "gemm_w13", "silu_mul", "gemm_w2", "gemm_head", "sample", "embed_misc",
-                                          "vq_conv_gemm", "vq_gn_stats", "vq_gn_apply", "vq_attn", "vq_misc", "persistent_decode"};
+                                          "vq_conv_gemm", "vq_gn_stats", "vq_gn_apply", "vq_attn", "vq_misc"};
     return (cls >= 0 && cls < PC_COUNT) ? names[cls] : nullptr;
 }
 
@@ -1028,16 +945,6 @@ int lg_test_attention(int dtype, int kv_dtype, float k_scale, float v_scale, int
         }
     }
     return launch_attention(aa, st, path);
-}
-
-int lg_test_gemm_dx(const void* x, const void* wa, const void* wb, int M, int N, int K, int mode, const void* normw, float eps,
-                    void* out, void* stream) {
-    LG_REQUIRE(x && wa && out && mode >= DX_F32 && mode <= DX_SWIGLU, "lg_test_gemm_dx: bad argument");
-    GemmDx g{x, K, wa, wb, M, N, K, mode, normw, eps, nullptr, nullptr, nullptr};
-    if (mode == DX_F32) g.out_f32 = (float*)out;
-    else if (mode == DX_RESID) g.h = out;
-    else g.ff = out;
-    return launch_gemm_dx(g, (cudaStream_t)stream);
 }
 
 }  // extern "C"

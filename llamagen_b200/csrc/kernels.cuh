@@ -137,7 +137,7 @@ struct AttnArgs {
     int kv_f8 = 0;
     float k_inv = 1.f, v_inv = 1.f, v_scale = 1.f;
 };
-// path (optional, int[3]): the kernel that was launched (0 = attention_kernel, 1 = attn_tma_kernel, 2 = attn_tma_v2_kernel,
+// path (optional, int[3]): the kernel that was launched (0 = attention_kernel, 1 = attn_tma_kernel,
 // 3 = attn_prefill_tc_kernel), its TMA ring depth (0 for attention_kernel, 1 for the single-stage prefill) and whether it fused the
 // QKV epilogue
 int launch_attention(const AttnArgs& a, cudaStream_t st, int* path = nullptr);
@@ -172,22 +172,6 @@ bool gemm_tc_supported(int M, int N, int K, int dtype);
 int gemm_tc_partial(const void* X, int ldx, const void* Wa, const void* Wb, int n_split, int M, int N, int K, int dtype,
                     float* partial, int* ksplit_out, cudaStream_t st, const GemmNext* next = nullptr);
 
-// gemm_dx.cu — "direct" wgmma GEMM of the decode step: (feature tile) x (row block) CTAs over the FULL K (no split-K slab), the
-// activation rows resident in shared memory; optional RMSNorm prologue on those rows, epilogue by mode
-enum { DX_F32 = 0, DX_RESID = 1, DX_SWIGLU = 2 };
-struct GemmDx {
-    const void* X; int ldx;            // [M][K] bf16
-    const void* Wa; const void* Wb;    // [N][K] bf16; Wb only for DX_SWIGLU (w1 | w3, N = F)
-    int M, N, K;
-    int mode;
-    const void* normw; float eps;      // RMSNorm weight [K] applied to X (null: none)
-    float* out_f32;                    // DX_F32:    y [M][N]
-    void* h;                           // DX_RESID:  h[M][N] = bf16(h + bf16(y)) in place
-    void* ff;                          // DX_SWIGLU: ff[M][N] = silu(y1) * y3
-};
-bool gemm_dx_supported(int M, int N, int K, int dtype, int mode, bool norm);
-int launch_gemm_dx(const GemmDx& g, cudaStream_t st, const GemmNext* next = nullptr);
-
 // gemv_small.cu — decode GEMMs for R <= 8 rows: CTA-owned output columns (no split-K), RMSNorm in the prologue (normw != null),
 // epilogue by destination: out_f32 [R][N] | h (in-place residual add) | ff (SwiGLU gate of the Wa/Wb row pair)
 struct GemvSmall {
@@ -201,25 +185,6 @@ struct GemvSmall {
 bool gemv_small_supported(int R, int N, int K, int dtype, bool paired);
 int launch_gemv_small(const GemvSmall& g, cudaStream_t st);
 
-// decode_persist.cu — one cooperative launch per token for R <= 8 rows: every layer + the head, phases separated by grid
-// barriers, weights and old K/V rows streamed through a shared-memory ring by a producer warp that never waits on activations.
-struct PdLayerW { const bf16 *wqkv, *wo, *w1, *w3, *w2, *attn_norm, *ffn_norm; };
-struct PdLaunch {
-    int L, D, F, V, H, hd, R, B, Tc, maxS;
-    float eps, scale;
-    const PdLayerW* layers;            // DEVICE array [L]
-    const void *final_norm, *output, *tok_emb;
-    const float* freqs;
-    void *kcache, *vcache; size_t layer_elems;     // layer 0 base, elements between layers
-    void *h, *q, *ff; float* part; size_t part_floats; float* logits;
-    const int32_t* tokens; const int* pos_dev; int pos_value;
-    const float* emb_mask;
-    unsigned int* bar;                 // 2 zero-initialised counters
-};
-bool decode_persist_supported(int R, int D, int F, int V, int H, int hd, int dtype);
-size_t decode_persist_part_floats(int R, int H, int hd);      // fp32 scratch the attention partials need
-int launch_decode_persist(const PdLaunch& p, cudaStream_t st);
-
 // *pos += 1; *step += 1  (device-side loop counters for graph replay)
 int launch_advance(int* pos, int* step, cudaStream_t st);
 int launch_set_counters(int* pos, int pos_v, int* step, int step_v, cudaStream_t st);
@@ -230,7 +195,7 @@ int launch_set_counters(int* pos, int pos_v, int* step, int step_v, cudaStream_t
 // ------------------------------------------------------------------------------------------------
 enum ProfClass {
     PC_GEMM_QKV = 0, PC_QKV_EPI, PC_ATTENTION, PC_GEMM_WO, PC_RESNORM, PC_GEMM_W13, PC_SILU, PC_GEMM_W2,
-    PC_GEMM_HEAD, PC_SAMPLE, PC_EMBED_MISC, PC_VQ_CONV, PC_VQ_GN_STATS, PC_VQ_GN_APPLY, PC_VQ_ATTN, PC_VQ_MISC, PC_PERSIST,
+    PC_GEMM_HEAD, PC_SAMPLE, PC_EMBED_MISC, PC_VQ_CONV, PC_VQ_GN_STATS, PC_VQ_GN_APPLY, PC_VQ_ATTN, PC_VQ_MISC,
     PC_COUNT
 };
 bool prof_enabled();

@@ -1,4 +1,4 @@
-// wgmma (Hopper warpgroup MMA) helpers shared by the tensor-core kernels (gemm_tc.cu, gemm_dx.cu, conv_tc.cu).
+// wgmma (Hopper warpgroup MMA) helpers shared by the tensor-core kernels (gemm_tc.cu, conv_tc.cu).
 //
 // Both operands are K-major bf16 (or fp16) tiles in shared memory written by TMA with the 128-byte swizzle: rows of 64 elements
 // (128 B), 8-row groups 1024 B apart, tile bases 1024-aligned. One warpgroup (128 threads) computes a 64 x N fp32

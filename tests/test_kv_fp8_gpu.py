@@ -208,7 +208,7 @@ def test_fp8_changes_logits_and_shrinks_workspace():
 
 
 def _run_env(monkeypatch, env, build, cond, S, teacher):
-    for k in ("LG_ATTN_TMA", "LG_NO_GRAPH", "LG_SPLIT", "LG_FUSE_TAIL", "LG_ATTN_NST", "LG_PERSIST", "LG_ATTN_V2"):
+    for k in ("LG_ATTN_TMA", "LG_NO_GRAPH", "LG_SPLIT", "LG_FUSE_TAIL", "LG_ATTN_NST"):
         monkeypatch.delenv(k, raising=False)
     for k, v in env.items():
         monkeypatch.setenv(k, v)
@@ -221,8 +221,7 @@ def _run_env(monkeypatch, env, build, cond, S, teacher):
 
 
 def test_fp8_paths_agree(monkeypatch):
-    """CUDA-core attention within the bound of the default; the ring-depth, chain-count and tail switches bit-identical to it,
-    and LG_ATTN_V2 (R * H >= 528) bit-identical too: an fp8 cache never selects the bf16-only v2 kernel."""
+    """CUDA-core attention within the bound of the default; the ring-depth, chain-count, tail and graph switches bit-identical to it."""
     S, B = 8, 24
     cond = torch.randint(0, 1000, (B,), generator=torch.Generator().manual_seed(3))
 
@@ -236,27 +235,11 @@ def test_fp8_paths_agree(monkeypatch):
     base = _run_env(monkeypatch, {"LG_SPLIT": "1"}, build, cond, S, teacher)
     _, logits, _ = _run_env(monkeypatch, {"LG_ATTN_TMA": "0", "LG_SPLIT": "1"}, build, cond, S, teacher)
     assert (logits - base[1]).abs().max().item() <= tol
-    for env in ({"LG_ATTN_NST": "3", "LG_SPLIT": "1"}, {"LG_ATTN_NST": "4", "LG_SPLIT": "1"}, {"LG_SPLIT": "2"},
-                {"LG_FUSE_TAIL": "0", "LG_SPLIT": "1"}, {"LG_NO_GRAPH": "1", "LG_FUSE_TAIL": "0", "LG_SPLIT": "1"},
-                {"LG_ATTN_V2": "1", "LG_SPLIT": "1"}):
+    for env in ({"LG_ATTN_NST": "3", "LG_SPLIT": "1"}, {"LG_SPLIT": "2"}, {"LG_FUSE_TAIL": "0", "LG_SPLIT": "1"},
+                {"LG_NO_GRAPH": "1", "LG_FUSE_TAIL": "0", "LG_SPLIT": "1"}):
         other = _run_env(monkeypatch, env, build, cond, S, teacher)
         for i in range(3):
             assert torch.equal(other[i], base[i]), (env, i)
-
-
-def test_fp8_persist_switch_is_ignored(monkeypatch):
-    """LG_PERSIST=1 at B = 1: the persistent bf16-cache decode kernel is never selected for an fp8 cache."""
-    g = load_golden("gpt_c2i.pt")
-    cond = g["cond"][:1]
-    teacher = torch.randint(0, 512, (1, 10), generator=torch.Generator().manual_seed(2), dtype=torch.int32)
-
-    def build():
-        return build_gpt(g["cfg"], g["state_dict"], torch.bfloat16)
-
-    base = _run_env(monkeypatch, {}, build, cond, 10, teacher)
-    other = _run_env(monkeypatch, {"LG_PERSIST": "1"}, build, cond, 10, teacher)
-    for i in range(3):
-        assert torch.equal(other[i], base[i]), i
 
 
 def test_serve_llm_fp8_matches_generate():

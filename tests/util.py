@@ -57,24 +57,6 @@ def test_gemm(x, w):
     return y
 
 
-def gemm_dx(x, wa, wb=None, mode=0, normw=None, eps=1e-5, h=None):
-    """The decode step's direct-epilogue GEMM (lg_test_gemm_dx): mode 0 -> y fp32, 1 -> h updated in place (returned), 2 -> ff."""
-    from llamagen_b200 import _lib
-    lib = _lib.load()
-    M, K = x.shape
-    N = wa.shape[0]
-    if mode == 0:
-        out = torch.empty(M, N, dtype=torch.float32, device=x.device)
-    elif mode == 1:
-        out = h.clone()
-    else:
-        out = torch.empty(M, N, dtype=torch.bfloat16, device=x.device)
-    _lib.check(lib.lg_test_gemm_dx(_lib.ptr(x), _lib.ptr(wa), _lib.ptr(wb) if wb is not None else None, M, N, K, mode,
-                                   _lib.ptr(normw) if normw is not None else None, ctypes.c_float(eps), _lib.ptr(out),
-                                   _lib.current_stream(x.device)), "lg_test_gemm_dx")
-    return out
-
-
 def seeded_state_dict(shapes: dict, seed: int, fan_in: bool = False) -> dict:
     """Deterministic weights for a parameter layout {name: shape}: N(0, 0.02) for matrices (N(0, 1 / fan_in) with
     `fan_in`, which keeps conv activations at unit scale), 1 + N(0, 0.02) for vectors (norm weights, biases). The golden

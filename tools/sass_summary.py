@@ -33,7 +33,7 @@ def demangle(n):
 print("# cuobjdump -sass of the in-tree library: occurrences of selected mnemonics per kernel")
 print("# HGMMA = wgmma   UTMALDG = TMA tensor load   UBLKPF = cp.async.bulk.prefetch.L2")
 print("# HMMA = mma.sync   LDSM = ldmatrix   LDGSTS = cp.async   SYNCS = mbarrier ops   ATOMS = shared-memory atomics (")
-print("# integer histogram counters of the sampler)   ATOMG / ATOM. / RED. = global atomics: only integer control counters (grid barrier of decode_small_persistent_kernel, arrival ticket of sample_kernel's fused tail); no float atomics, none on a data path")
+print("# integer histogram counters of the sampler)   ATOMG / ATOM. / RED. = global atomics: only integer control counters (arrival ticket of sample_kernel's fused tail); no float atomics, none on a data path")
 rows = sorted((demangle(fn), dict(c)) for fn, c in counts.items() if c)
 for d, c in rows:
     print(f"{d}: {c}")
