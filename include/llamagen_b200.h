@@ -185,7 +185,7 @@ int         lg_profile_read(int cls, double* total_ms, uint64_t* launches);
 const char* lg_profile_class_name(int cls);   /* NULL past the last class */
 
 /* Cap the number of CTAs (hence SMs) the VQ decoder's tensor-core convolutions occupy: ctas > 0 runs them as that many persistent
- * CTAs, 0 restores one CTA per tile, -1 defers to the LG_CONV_CTAS environment variable (default). Process-wide; used by
+ * CTAs, 0 (or any negative value) restores one CTA per tile (the default). Process-wide; used by
  * SamplePipeline so that decoding batch i does not evict the latency-bound AR sampling of batch i+1 from the SMs
  * (the reference runs the two back to back, sample_c2i_ddp.py:128-143). */
 int         lg_vq_set_cta_budget(int ctas);
@@ -198,8 +198,9 @@ int  lg_test_gemm(const void* x, const void* w, int M, int N, int K, int dtype, 
 /* One transformer attention call through the engine's own dispatch (honouring LG_ATTN_TMA, LG_ATTN_PREFILL_TC, LG_ATTN_NST
  * and LG_ATTN_DEEP). dtype: the model dtype (LG_DTYPE_F32, _BF16 or _F16); kv_dtype: dtype, or LG_DTYPE_E4M3 for a
  * 16-bit model with k_scale / v_scale powers of two in [2^-8, 2^7] (otherwise both 1). kcache / vcache: dev [n_layer][R][H][max_seq]
- * [hdp] in the KV dtype; `layer` is the one attended to. The tensor maps span all n_layer layers, as lg_engine_set_workspace builds
- * them. Query row m = r * Tq + t sits at position pos(r) + t, pos(r) = pos_rows ? pos_rows[r] : (pos_dev ? *pos_dev : 0) + pos_value,
+ * [hdp] in the KV dtype, hdp = the engine's row width: 112 for hd 100 in a bf16 / fp16 model, hd otherwise (dims hd..hdp-1 are
+ * padding and do not affect the result); `layer` is the one attended to. The tensor maps span all n_layer layers, as
+ * lg_engine_set_workspace builds them. Query row m = r * Tq + t sits at position pos(r) + t, pos(r) = pos_rows ? pos_rows[r] : (pos_dev ? *pos_dev : 0) + pos_value,
  * and attends keys j <= its position with j >= Tc or emb_mask[r % B][j] != 0 or j == its position (emb_mask dev f32 [B][Tc] or NULL).
  * Input: q (dev [R * Tq][H * hd], post-RoPE) or the QKV GEMM's split-K slabs qkv_partial (dev f32 [ksplit][R * Tq][3 * H * hd]) with
  * freqs (dev f32 [max_seq][hd / 2][2]): fuse = 0 runs the QKV epilogue (q -> q_out, K / V rows written at the query positions) and

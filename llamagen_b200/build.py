@@ -14,7 +14,6 @@ from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-# A/B builds: LG_NVCC_DEFS="-DLG_ATTN_KC=48" LG_LIB_DIR=lib_kc48 python -m llamagen_b200.build ; run with LG_LIB_PATH=...
 OUT_DIR = os.path.join(HERE, os.environ.get("LG_LIB_DIR", "lib"))
 LIB = os.path.join(OUT_DIR, "libllamagen_b200.so")
 EXTRA_DEFS = os.environ.get("LG_NVCC_DEFS", "").split()

@@ -13,20 +13,11 @@ namespace {
 
 using namespace tma;
 
-#ifndef LG_ATTN_KC
-#define LG_ATTN_KC 32   // keys per stage: 32 keys / 2 warps per CTA leave shared memory for the other chain's GEMM CTAs
-                        // (build with -DLG_ATTN_KC=48 or 64 for 3 or 4 warps per CTA)
-#endif
-constexpr int kKC = LG_ATTN_KC;   // keys per stage (64 -> 4 warps, 6 CTAs/SM; 48 -> 3 warps, 8 CTAs/SM)
+constexpr int kKC = 32;           // keys per stage: 32 keys / 2 warps per CTA leave shared memory for the other chain's GEMM CTAs
 constexpr int kStagesA = 2;       // 2 stages of K+V per CTA; contexts here are <= 1144 keys
 constexpr int kWarps = kKC / 16;  // each warp owns 16 keys of a stage
-constexpr int kDeepStages = kKC == 32 ? 8 : 6;   // few-item (batch-1) variant: a whole context of up to NST * kKC keys (256 at kKC = 32)
-                                                 // is requested before the dependency wait
-#ifdef LG_ATTN_CTAS
-constexpr int kCtasPerSm64 = LG_ATTN_CTAS;
-#else
-constexpr int kCtasPerSm64 = kKC == 48 ? 8 : (kKC == 32 ? 12 : 6);
-#endif
+constexpr int kDeepStages = 8;    // few-item (batch-1) variant: a whole context of up to 256 keys is requested before the dependency wait
+constexpr int kCtasPerSm64 = 12;  // launch bound of the sequential hd-64 kernels (5 for hd 128)
 
 __device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
     asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];\n"
@@ -95,7 +86,7 @@ struct KvScales {
 // and transposes bytes with prmt (the output dims come out permuted and are put back in the merge). The fused writer stores
 // e4m3(x * inv) and the step attends to those codes too; the K scale is in a.scale and the V scale multiplies O / L.
 template <typename T, int HD, bool FUSED, int NST, bool PAR_ = (NST > 2), bool F8 = false>
-__global__ void __launch_bounds__(kWarps * 32 * (PAR_ ? NST : 1), PAR_ ? 1 : (HD == 64 ? (NST > 2 ? 4 : kCtasPerSm64) : (kKC == 32 ? 5 : 4))) attn_tma_kernel(const __grid_constant__ CUtensorMap kmap,
+__global__ void __launch_bounds__(kWarps * 32 * (PAR_ ? NST : 1), PAR_ ? 1 : (HD == 64 ? (NST > 2 ? 4 : kCtasPerSm64) : 5)) attn_tma_kernel(const __grid_constant__ CUtensorMap kmap,
                                                                const __grid_constant__ CUtensorMap vmap,
                                                                const __grid_constant__ CUtensorMap kmap16,
                                                                const __grid_constant__ CUtensorMap vmap16, AttnTmaArgs a,
@@ -722,7 +713,7 @@ static int launch_attention_tma_t(const AttnArgs& a, cudaStream_t st, int* path)
     t.emb_mask = a.emb_mask; t.B = a.B; t.Tc = a.Tc; t.scale = a.scale;
     t.partial = a.qkv_partial; t.ksplit = a.qkv_ksplit; t.freqs = a.freqs;
     t.kcache = (bf16*)const_cast<void*>(a.kcache); t.vcache = (bf16*)const_cast<void*>(a.vcache);
-    t.kvhint = (lg_env_flag("LG_L2_HINT", 1) & 1) ? tma::kL2EvictFirst : 0ull;
+    t.kvhint = tma::kL2EvictFirst;   // each K/V byte is read once per step
     t.hd = a.hd; t.hdp = a.hdp ? a.hdp : a.hd;
     const CUtensorMap& km = *reinterpret_cast<const CUtensorMap*>(a.kmap);
     const CUtensorMap& vm = *reinterpret_cast<const CUtensorMap*>(a.vmap);

@@ -382,7 +382,7 @@ int conv_tc_make_phase_weights(const float* w_f32, bf16* out, int cout, int cin,
     return 0;
 }
 
-static int g_conv_cta_budget = -1;      // -1: read LG_CONV_CTAS at every launch
+static int g_conv_cta_budget = 0;
 void conv_tc_set_cta_budget(int ctas) { g_conv_cta_budget = ctas; }
 
 bool conv_tc_supported(int Hin, int Win, int Cin, int Cout, int ksize, int up, bool nchw_out) {
@@ -439,8 +439,8 @@ int launch_conv_tc(const bf16* in, int B, int Hin, int Win, int Cin, const bf16*
     const uint64_t wrows = (uint64_t)(up ? 4 : 1) * Cout, wcols = (uint64_t)a.ntaps * Cin;
     LG_TRY(tma::make_map_2d(&wmap, weights, wrows, wcols, wcols, (uint32_t)a.bn, kCk));
 
-    // CTA budget: 0 = one CTA per tile; > 0 = persistent CTAs (lg_vq_set_cta_budget / LG_CONV_CTAS), e.g. 64 while the next batch samples
-    const int budget = g_conv_cta_budget >= 0 ? g_conv_cta_budget : lg_env_flag("LG_CONV_CTAS", 0);
+    // CTA budget: 0 = one CTA per tile; > 0 = persistent CTAs (lg_vq_set_cta_budget), e.g. 64 while the next batch samples
+    const int budget = g_conv_cta_budget;
     // the weights-as-A kernel drains through its stage memory, which needs every stage held by the tile (>= kWStages k-blocks)
     if (Cout % 128 == 0 && a.Ht >= 16 && a.Wt >= 16 && out_bf && !out_nchw && !out_u8 && a.ntaps * a.kchunks >= kWStages &&
         lg_env_flag("LG_CONV_SWAP", 1)) {

@@ -367,7 +367,7 @@ int lg_engine_create(const lg_model_cfg* cfg, int device, lg_engine** out) {
     e->cfg = *cfg;
     e->device = device;
     e->hd = hd;
-    e->hdp = (hd == 100 && lg_dtype_is16(cfg->dtype) && lg_env_flag("LG_HD_PAD", 1)) ? 112 : hd;
+    e->hdp = attn_kv_row_width(cfg->dtype, hd);
     e->esz = (size_t)lg_dtype_info(cfg->dtype).esz;
     e->kv_esz = e->esz;
     const char* ng = getenv("LG_NO_GRAPH");
@@ -678,7 +678,7 @@ int lg_generate(lg_engine* e, const void* cond, const float* emb_mask, int B, in
         int prio_lo = 0, prio_hi = 0;
         LG_CUDA_OK(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
         for (int i = 0; i < lg_engine::kMaxChains; ++i) {
-            LG_CUDA_OK(cudaStreamCreateWithPriority(&e->works[i], cudaStreamNonBlocking, lg_env_flag("LG_AR_PRIORITY", 1) ? prio_hi : prio_lo));
+            LG_CUDA_OK(cudaStreamCreateWithPriority(&e->works[i], cudaStreamNonBlocking, prio_hi));
             LG_CUDA_OK(cudaEventCreateWithFlags(&e->ev_joins[i], cudaEventDisableTiming));
         }
         LG_CUDA_OK(cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming));
@@ -839,7 +839,7 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
 }
 
 int lg_vq_set_cta_budget(int ctas) {
-    conv_tc_set_cta_budget(ctas < -1 ? -1 : ctas);
+    conv_tc_set_cta_budget(ctas < 0 ? 0 : ctas);
     return 0;
 }
 int lg_set_pdl(int on) {
@@ -897,7 +897,7 @@ int lg_test_attention(int dtype, int kv_dtype, float k_scale, float v_scale, int
     LG_REQUIRE(R > 0 && Tq > 0 && H > 0 && max_seq > 0 && n_layer > 0 && layer >= 0 && layer < n_layer && (long long)R * Tq <= 65535,
                "lg_test_attention: bad shape R=%d Tq=%d H=%d max_seq=%d layer %d of %d", R, Tq, H, max_seq, layer, n_layer);
     LG_REQUIRE(hd == 64 || hd == 100 || hd == 128, "lg_test_attention: unsupported head_dim %d (64, 100, 128)", hd);
-    LG_REQUIRE(hdp == hd || (hd == 100 && hdp == 112 && lg_dtype_is16(dtype)), "lg_test_attention: row width %d for head_dim %d", hdp, hd);
+    LG_REQUIRE(hdp == attn_kv_row_width(dtype, hd), "lg_test_attention: row width %d for head_dim %d", hdp, hd);
     LG_REQUIRE(kcache && vcache && out && a16(kcache) && a16(vcache) && a16(out) && a16(q) && a16(q_out) && a16(qkv_partial) && a16(freqs),
                "lg_test_attention: null or misaligned (16 bytes) buffer");
     if (pos_rows) {

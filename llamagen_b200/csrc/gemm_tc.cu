@@ -21,7 +21,9 @@ namespace {
 
 constexpr int kBlockN = 128;    // weight rows per CTA (two warpgroups of M = 64)
 constexpr int kBlockK = 64;     // bf16 elements per k-block = 128 B = one swizzle-128B row
-constexpr int kMaxStages = 8;
+constexpr int kMaxStages = 8;   // barrier slots in shared memory
+constexpr int kRingStages = 4;  // stages the host launches with (fewer when a CTA owns fewer k-blocks)
+constexpr int kTargetCtas = 92; // split-K CTA target per GEMM (~0.7 per SM of an H100)
 constexpr int kThreads = 288;   // 2 consumer warpgroups + 1 producer warp
 constexpr int kATileBytes = kBlockN * kBlockK * 2;   // 16 KB
 constexpr int kMaxRowsPerCta = 256;                  // wgmma N <= 256
@@ -37,19 +39,8 @@ struct TcArgs {
     float* partial;       // [ksplit][M][N]
     const char* pf0; unsigned long long pfb0;   // next GEMM's weights to pull into L2 (see GemmNext)
     const char* pf1; unsigned long long pfb1;
-    unsigned long long* trace;   // debug: [cta][8] %globaltimer stamps of the pipeline phases (nullable)
     unsigned long long whint;    // L2 eviction hint of the weight tiles (0: default policy)
 };
-
-__device__ __forceinline__ unsigned long long gtime() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
-#define TC_TRACE(slot)                                                                            \
-    do {                                                                                          \
-        if (a.trace) a.trace[(size_t)(blockIdx.y * gridDim.x + blockIdx.x) * 8 + (slot)] = gtime(); \
-    } while (0)
 
 // RP: rows of one row block padded to a power of two (wgmma N); the activation box has RP rows, rows >= M read as zero.
 // T: operand type (bf16 or f16), only the wgmma instruction depends on it.
@@ -70,7 +61,6 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     const int ks = blockIdx.y;
     const int row0 = (int)blockIdx.z * a.rblk;               // first activation row of this CTA's row block (t2i prefill: M = R*120)
     const int Mb = min(a.rblk, a.M - row0);                  // valid rows in the block
-    if (threadIdx.x == 0) TC_TRACE(0);
     const int total_kb = (a.K + kBlockK - 1) / kBlockK;
     const int kb0 = ks * a.kblocks_per_split;
     const int nkb = max(0, min(a.kblocks_per_split, total_kb - kb0));
@@ -83,7 +73,6 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         fence_barrier_init();
     }
     __syncthreads();
-    if (threadIdx.x == 0) TC_TRACE(1);
     lg_pdl_launch_dependents();
     if (warp != 8) lg_pdl_wait();   // the producer waits after it has requested the first weight tiles
 
@@ -131,7 +120,6 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                     }
                 }
             }
-            TC_TRACE(2);
         }
         __syncwarp();
         return;
@@ -145,8 +133,6 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         const int s = i % kStages;
         const uint32_t ph = (uint32_t)((i / kStages) & 1);
         mbar_wait(&full_bar[s], ph);
-        if (i == 0 && threadIdx.x == 0) TC_TRACE(3);
-        if (i == nkb - 1 && threadIdx.x == 0) TC_TRACE(4);
         const uint32_t sa = smem_u32(tiles + s * stage_bytes);
         wg::fence_regs<RP / 2>(acc);
         wg::fence();
@@ -159,15 +145,12 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     wg::wait<0>();
     wg::fence_regs<RP / 2>(acc);
     // ---------------------------------------------------------------------- drain: registers -> fp32 slab [row][feature]
-    if (threadIdx.x == 0) TC_TRACE(5);
     float* out = a.partial + (size_t)ks * a.M * a.N + (size_t)row0 * a.N;
 #pragma unroll
     for (int i = 0; i < RP / 2; ++i) {
         const int n = n0 + 64 * g + wg::frag_row(i), r = wg::frag_col(i);
         if (n < a.N && r < Mb) out[(size_t)r * a.N + n] = acc[i];
     }
-    if (threadIdx.x == 0) TC_TRACE(6);
-    if (threadIdx.x == 0) TC_TRACE(7);
 }
 
 // ---------------------------------------------------------------------------------------------- host side
@@ -226,15 +209,12 @@ int make_map_nhwc(CUtensorMap* m, const void* base, uint64_t B, uint64_t H, uint
 }
 }  // namespace tma
 
-static unsigned long long* g_tc_trace = nullptr;
-extern "C" void lg_debug_set_tc_trace(unsigned long long* dev_buf) { g_tc_trace = dev_buf; }
-
-// Plan: number of k-slices so that (N/128) * ksplit is about LG_TC_CTAS CTAs (default 92, ~0.7 per SM of an H100; fewer,
-// fatter slices halve the fp32 slab traffic), >= 2 k-blocks per slice.
+// Plan: number of k-slices so that (N/128) * ksplit is about kTargetCtas CTAs (fewer, fatter slices than one per SM halve the
+// fp32 slab traffic), >= 2 k-blocks per slice.
 int gemm_tc_ksplit(int M, int N, int K) {
     // row blocks (M > 256: t2i prefill) already multiply the CTA count
     const int tiles = cdiv(N, kBlockN) * cdiv(M, kMaxRowsPerCta), kb = cdiv(K, kBlockK);
-    int ks = std::max(1, lg_env_flag("LG_TC_CTAS", 92) / std::max(tiles, 1));
+    int ks = std::max(1, kTargetCtas / std::max(tiles, 1));
     ks = std::min(ks, std::max(1, kb / 2));
     return std::min(ks, 16);
 }
@@ -248,17 +228,15 @@ static int gemm_tc_launch_t(const CUtensorMap& mwa, const CUtensorMap& mwb, cons
                             cudaStream_t st) {
     constexpr int b_tile_bytes = RP * kBlockK * 2;
     constexpr int stage_bytes = kATileBytes + ((b_tile_bytes + 1023) / 1024) * 1024;
-    a.stages = std::min(std::min(kMaxStages, lg_env_flag("LG_TC_STAGES", 4)), (int)((225 * 1024 - 1024) / stage_bytes));
     // 4 stages instead of filling shared memory: a CTA never owns more than ~8 k-blocks, and the smaller footprint lets the
     // PDL-launched next kernel become resident next to this one.
-    a.stages = std::min(a.stages, std::max(2, a.kblocks_per_split));   // never more stages than k-blocks
-    LG_REQUIRE(a.stages >= 2, "gemm_tc: tile too large for a 2-stage ring");
+    static_assert(1024 + kRingStages * stage_bytes + 2 * kMaxStages * sizeof(uint64_t) <= 227 * 1024, "gemm_tc: ring too large");
+    a.stages = std::min(kRingStages, std::max(2, a.kblocks_per_split));   // never more stages than k-blocks
     const size_t smem = 1024 + (size_t)a.stages * stage_bytes + 2 * kMaxStages * sizeof(uint64_t);
     static DevOnce attr;
     if (lg_first_on_device(attr)) {
         LG_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<RP, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     }
-    LG_REQUIRE(smem <= 227 * 1024, "gemm_tc: shared memory %zu too large", smem);
     (void)lg_launch(gemm_tc_kernel<RP, T>, grid, dim3(kThreads), smem, st, mwa, mwb, mx, a);
     LG_LAUNCH_CHECK();
     return 0;
@@ -291,11 +269,9 @@ static int gemm_tc_launch(const void* X, int ldx, const void* Wa, const void* Wb
     LG_TRY(tma::make_map_2d(&mwb, Wb, (uint64_t)std::max(N - n_split, Wb == Wa ? N : 1), (uint64_t)K, (uint64_t)K, kBlockN, kBlockK, dt));
     LG_TRY(tma::make_map_2d(&mx, X, (uint64_t)M, (uint64_t)K, (uint64_t)ldx, (uint32_t)rpad, kBlockK, dt));   // rows >= M read as zero
 
-    a.trace = g_tc_trace;
-    a.whint = (lg_env_flag("LG_L2_HINT", 1) & 2) ? tma::kL2EvictLast : 0ull;
-    const bool pf = next && lg_env_flag("LG_L2_PREFETCH", 1);
-    a.pf0 = pf ? (const char*)next->p0 : nullptr; a.pfb0 = pf ? next->b0 : 0;
-    a.pf1 = pf ? (const char*)next->p1 : nullptr; a.pfb1 = pf ? next->b1 : 0;
+    a.whint = 0ull;   // the weight tiles take the default L2 policy
+    a.pf0 = next ? (const char*)next->p0 : nullptr; a.pfb0 = next ? next->b0 : 0;
+    a.pf1 = next ? (const char*)next->p1 : nullptr; a.pfb1 = next ? next->b1 : 0;
     const dim3 grid(cdiv(N, kBlockN), ks, zblocks);
     switch (rpad) {
         case 16: return gemm_tc_launch_t<16, T>(mwa, mwb, mx, a, grid, st);

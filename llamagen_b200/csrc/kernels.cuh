@@ -137,6 +137,9 @@ struct AttnArgs {
     int kv_f8 = 0;
     float k_inv = 1.f, v_inv = 1.f, v_scale = 1.f;
 };
+// KV-cache row width in elements: head_dim 100 of a bf16 / fp16 model (GPT-3B) is stored in 112-wide rows, 16-byte multiples that
+// the TMA attention kernels can stream (dims 100..111 stay zero); every other cache row is hd wide
+inline int attn_kv_row_width(int dtype, int hd) { return hd == 100 && lg_dtype_is16(dtype) ? 112 : hd; }
 // path (optional, int[3]): the kernel that was launched (0 = attention_kernel, 1 = attn_tma_kernel,
 // 3 = attn_prefill_tc_kernel), its TMA ring depth (0 for attention_kernel, 1 for the single-stage prefill) and whether it fused the
 // QKV epilogue
@@ -159,7 +162,7 @@ bool attn_prefill_tc_supported(const AttnArgs& a);
 int launch_attention_prefill_tc(const AttnArgs& a, cudaStream_t st, int* path = nullptr);
 // conv_tc.cu — wgmma implicit-GEMM convolution over bf16 NHWC activations (TMA 4-D boxes, register accumulators)
 bool conv_tc_supported(int Hin, int Win, int Cin, int Cout, int ksize, int up, bool nchw_out);
-void conv_tc_set_cta_budget(int ctas);   // > 0: persistent conv CTAs (at most `ctas`), 0: one CTA per tile, -1: LG_CONV_CTAS
+void conv_tc_set_cta_budget(int ctas);   // > 0: persistent conv CTAs (at most `ctas`), 0: one CTA per tile (default)
 int conv_tc_make_phase_weights(const float* w_f32, bf16* out, int cout, int cin, cudaStream_t st);
 int launch_conv_tc(const bf16* in, int B, int Hin, int Win, int Cin, const bf16* weights, const float* bias, int Cout,
                    int ksize, int up, const bf16* residual, bf16* out_bf, float* out_nchw, cudaStream_t st, uint8_t* out_u8 = nullptr,

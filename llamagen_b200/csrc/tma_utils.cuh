@@ -52,11 +52,9 @@ __device__ __forceinline__ void load_2d(void* smem_dst, const CUtensorMap* map, 
         ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
         : "memory");
 }
-// L2 eviction-priority hints for bulk tensor loads (the encodings createpolicy.fractional.L2::evict_* produce with fraction 1.0):
-// KV-cache streams are read once per step (evict_first), weights are re-read by the second decode chain and by the next token
-// (evict_last). hint == 0 keeps the default policy.
+// L2 eviction-priority hint for bulk tensor loads (the encoding createpolicy.fractional.L2::evict_first produces with fraction 1.0):
+// KV-cache streams are read once per step. hint == 0 keeps the default policy, which the weight tiles use.
 constexpr uint64_t kL2EvictFirst = 0x12F0000000000000ull;
-constexpr uint64_t kL2EvictLast = 0x14F0000000000000ull;
 __device__ __forceinline__ void load_2d_hint(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, uint64_t hint) {
     if (hint == 0) {
         load_2d(smem_dst, map, bar, c0, c1);

@@ -716,7 +716,7 @@ int run_gn(const NormW& nw, const bf16* x, bf16* y, int B, int HW, int swish, fl
         LG_LAUNCH_CHECK();
     }
     if (ws) ws->gn_src = nullptr;                // gnbuf is consumed below; y (and any later writer of x) invalidates it anyway
-    int chunks = (int)std::min<long long>(lg_env_flag("LG_GN_CHUNKS", 256), std::max<long long>(1, (long long)HW * (nw.c / 8) / 1024));
+    int chunks = (int)std::min<long long>(256, std::max<long long>(1, (long long)HW * (nw.c / 8) / 1024));
     prof_begin(PC_VQ_GN_APPLY, st);
     gn_apply_kernel<<<dim3(chunks, B), 256, 0, st>>>(x, gnbuf, splits, nw.gamma, nw.beta, y, HW, nw.c, swish);
     prof_end(st);

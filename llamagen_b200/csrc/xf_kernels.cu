@@ -508,31 +508,27 @@ int launch_attention(const AttnArgs& a, cudaStream_t st, int* path) {
     LG_REQUIRE(a.qkv_partial == nullptr, "attention: fused QKV epilogue requested on a path that does not support it");
     set_attn_path(path, 0, 0, 0);
     LG_REQUIRE((long long)a.R * a.Tq <= 65535, "attention: too many query rows (%d x %d)", a.R, a.Tq);
-    LG_REQUIRE(a.hdp == 0 || a.hdp == a.hd || (a.hd == 100 && a.hdp == 112 && lg_dtype_is16(a.dtype)), "attention: unsupported KV row stride %d for head_dim %d", a.hdp, a.hd);
+    LG_REQUIRE((a.hdp ? a.hdp : a.hd) == attn_kv_row_width(a.dtype, a.hd), "attention: KV row width %d for head_dim %d", a.hdp, a.hd);
     if (a.kv_f8) {   // fp8 cache of a 16-bit model
         if (a.dtype == LG_DTYPE_BF16) {
             if (a.hd == 64) return launch_attention_t<bf16, 64, 8, 8, 64, e4m3>(a, st);
             if (a.hd == 128) return launch_attention_t<bf16, 128, 8, 16, 128, e4m3>(a, st);
-            if (a.hd == 100 && a.hdp == 112) return launch_attention_t<bf16, 100, 4, 32, 112, e4m3>(a, st);
-            if (a.hd == 100) return launch_attention_t<bf16, 100, 4, 32, 100, e4m3>(a, st);
+            if (a.hd == 100) return launch_attention_t<bf16, 100, 4, 32, 112, e4m3>(a, st);
         } else if (a.dtype == LG_DTYPE_F16) {
             if (a.hd == 64) return launch_attention_t<f16, 64, 8, 8, 64, e4m3>(a, st);
             if (a.hd == 128) return launch_attention_t<f16, 128, 8, 16, 128, e4m3>(a, st);
-            if (a.hd == 100 && a.hdp == 112) return launch_attention_t<f16, 100, 4, 32, 112, e4m3>(a, st);
-            if (a.hd == 100) return launch_attention_t<f16, 100, 4, 32, 100, e4m3>(a, st);
+            if (a.hd == 100) return launch_attention_t<f16, 100, 4, 32, 112, e4m3>(a, st);
         }
         return lg_fail("attention: no fp8 KV-cache kernel for head_dim %d / dtype %d", a.hd, a.dtype);
     }
     if (a.dtype == LG_DTYPE_BF16) {
         if (a.hd == 64) return launch_attention_t<bf16, 64, 8, 8>(a, st);
         if (a.hd == 128) return launch_attention_t<bf16, 128, 8, 16>(a, st);
-        if (a.hd == 100 && a.hdp == 112) return launch_attention_t<bf16, 100, 4, 32, 112>(a, st);
-        if (a.hd == 100) return launch_attention_t<bf16, 100, 4, 32>(a, st);
+        if (a.hd == 100) return launch_attention_t<bf16, 100, 4, 32, 112>(a, st);
     } else if (a.dtype == LG_DTYPE_F16) {
         if (a.hd == 64) return launch_attention_t<f16, 64, 8, 8>(a, st);
         if (a.hd == 128) return launch_attention_t<f16, 128, 8, 16>(a, st);
-        if (a.hd == 100 && a.hdp == 112) return launch_attention_t<f16, 100, 4, 32, 112>(a, st);
-        if (a.hd == 100) return launch_attention_t<f16, 100, 4, 32>(a, st);
+        if (a.hd == 100) return launch_attention_t<f16, 100, 4, 32, 112>(a, st);
     } else if (a.dtype == LG_DTYPE_F32) {
         if (a.hd == 64) return launch_attention_t<float, 64, 8, 8>(a, st);
         if (a.hd == 128) return launch_attention_t<float, 128, 8, 16>(a, st);

@@ -57,7 +57,7 @@ class SamplePipeline:
                     u8 = to_uint8_nhwc(pixels, size=(to_uint8_host.shape[1], to_uint8_host.shape[2]))
                     to_uint8_host.copy_(u8, non_blocking=True)
             if self.conv_ctas > 0:
-                _lib.load().lg_vq_set_cta_budget(-1)
+                _lib.load().lg_vq_set_cta_budget(0)
         self._last = pixels
         return pixels
 

@@ -178,13 +178,14 @@ class Case:
 
 
 def dispatchable():
-    """Every (kernel, stages, fused, dtype, kv, hd, hdp) launch_attention can select (default LG_ATTN_KC)."""
+    """Every (kernel, stages, fused, dtype, kv, hd, hdp) launch_attention can select: fp32 rows are hd wide, bf16 / fp16 store hd 100
+    in 112-wide rows."""
     out = {(0, 0, 0, "f32", "auto", hd, hd) for hd in (64, 128, 100)}
     for dt in ("bf16", "f16"):
         for kv in ("auto", "fp8"):
             for hd, hdp in ((64, 64), (128, 128), (100, 112)):
                 out |= {(1, 2, 0, dt, kv, hd, hdp), (1, 2, 1, dt, kv, hd, hdp), (0, 0, 0, dt, kv, hd, hdp)}
-            out |= {(0, 0, 0, dt, kv, 100, 100), (3, 1, 0, dt, kv, 64, 64)}
+            out.add((3, 1, 0, dt, kv, 64, 64))
             out |= {(1, st, 1, dt, kv, 64, 64) for st in (3, 8)}
     return out
 
@@ -212,7 +213,6 @@ def _cases():
                 cs.append(Case(f"cc_notma_{tag}", dt, kv, hd, 3, 2, 230, (0, 0, 0), hdp=hdp, pos=pos, scales=sc,
                                env={"LG_ATTN_TMA": "0"}))
             sc = FP8_SCALES[i % 3] if kv == "fp8" else (1.0, 1.0)
-            cs.append(Case(f"cc_hd100_{dt}_{kv}", dt, kv, 100, 3, 2, 230, (0, 0, 0), pos=("scalar", 203), scales=sc))
             cs.append(Case(f"fused_nst3_{dt}_{kv}", dt, kv, 64, 17, 16, 300, (1, 3, 1), pos=("dev", 290), inp="fused",
                            scales=sc, env={"LG_ATTN_NST": "3"}))
             cs.append(Case(f"fused_s300_{dt}_{kv}", dt, kv, 64, 17, 16, 300, (1, 2, 1), pos=("dev", 290), inp="fused", scales=sc))
@@ -251,7 +251,8 @@ def _cases():
            Case("rows_deep_bf16", "bf16", "auto", 64, 12, 2, 301, (1, 8, 1), pos=("rows", rows), inp="fused"),
            Case("rows_fused_f16_112", "f16", "auto", 100, 12, 2, 301, (1, 2, 1), hdp=112, pos=("rows", rows), inp="fused"),
            Case("rows_cc_f32", "f32", "auto", 128, 12, 2, 301, (0, 0, 0), pos=("rows", rows)),
-           Case("rows_cc_bf16_fp8", "bf16", "fp8", 100, 12, 2, 301, (0, 0, 0), pos=("rows", rows), scales=FP8_SCALES[2])]
+           Case("rows_cc_bf16_fp8_112", "bf16", "fp8", 100, 12, 2, 301, (0, 0, 0), hdp=112, pos=("rows", rows), scales=FP8_SCALES[2],
+                env={"LG_ATTN_TMA": "0"})]
     # decode with an emb-mask, query positions inside and past the condition (the j == qpos exemption)
     mrows = [50, 119, 120, 300]
     cs += [Case("mask_tma_bf16", "bf16", "auto", 64, 4, 2, 301, (1, 2, 0), pos=("rows", mrows), mask=MASK4),
@@ -617,7 +618,8 @@ def test_argument_validation():
 
     for kw, msg in [(dict(dt=0, kvdt=LG_E4M3), "KV dtype"), (dict(kvdt=LG_E4M3, ks=3.0), "scales"), (dict(ks=0.5), "scales"),
                     (dict(pos=S), "exceeds max_seq"), (dict(pos=S - 1, Tq=2), "exceeds max_seq"), (dict(hd_=96, hdp=96), "head_dim"),
-                    (dict(dt=0, kvdt=0, hd_=100, hdp=112), "row width"), (dict(layer=2), "bad shape"), (dict(qq=None), "exactly one"),
+                    (dict(dt=0, kvdt=0, hd_=100, hdp=112), "row width"), (dict(hd_=100, hdp=100), "row width"),
+                    (dict(dt=2, kvdt=2, hd_=100, hdp=100), "row width"), (dict(layer=2), "bad shape"), (dict(qq=None), "exactly one"),
                     (dict(pp=part), "exactly one"), (dict(qq=None, pp=part), "fuse"), (dict(fuse=1), "fuse"),
                     (dict(qq=None, pp=part, fuse=1, Tq=2), "fused QKV"), (dict(qq=None, pp=part, fuse=1, dt=0, kvdt=0), "fused QKV")]:
         rc, err = call(**kw)

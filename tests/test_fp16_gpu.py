@@ -106,10 +106,8 @@ def test_gpt_l_f16_teacher_forced(B):
     _f16_parity(m, torch.randint(0, 1000, (B,)), 6)
 
 
-@pytest.mark.parametrize("hd_pad", ["1", "0"])
-def test_gpt_3b_head_dim_100_f16(hd_pad, monkeypatch):
-    """GPT-3B's head_dim 100: 112-wide KV rows on the TMA attention (LG_HD_PAD=1, default) or 100-wide rows on the CUDA-core kernel."""
-    monkeypatch.setenv("LG_HD_PAD", hd_pad)
+def test_gpt_3b_head_dim_100_f16():
+    """GPT-3B's head_dim 100: 112-wide KV rows on the TMA attention."""
     from llamagen_b200.gpt import ModelArgs, Transformer
     torch.manual_seed(3)
     m = Transformer(ModelArgs(n_layer=4, n_head=32, dim=3200, block_size=576, vocab_size=16384))

@@ -78,7 +78,7 @@ def _check_cache_bytes(m, o16, scales=None):
     c = m.config
     L, H, hd = c.n_layer, c.n_head, c.dim // c.n_head
     rows, maxS = m._ws_shape
-    hdp = 112 if hd == 100 and os.environ.get("LG_HD_PAD", "1") != "0" else hd
+    hdp = 112 if hd == 100 else hd
     ws = m._workspace
     off = (ws.data_ptr() + 255) // 256 * 256 - ws.data_ptr()
     layer = rows * H * maxS * hdp
@@ -124,10 +124,8 @@ def test_gpt_l_fp8_teacher_forced(B, dtype, one_chain):
     _check_cache_bytes(m, o16)
 
 
-@pytest.mark.parametrize("hd_pad", ["1", "0"])
-def test_gpt_3b_head_dim_100_fp8(hd_pad, monkeypatch, one_chain):
-    """hd 100: 112-byte fp8 rows on the TMA kernel (LG_HD_PAD=1) or 100-byte rows on the CUDA-core kernel (LG_HD_PAD=0)."""
-    monkeypatch.setenv("LG_HD_PAD", hd_pad)
+def test_gpt_3b_head_dim_100_fp8(one_chain):
+    """hd 100: 112-byte fp8 rows on the TMA kernel."""
     from llamagen_b200.gpt import ModelArgs, Transformer
     torch.manual_seed(3)
     m = Transformer(ModelArgs(n_layer=4, n_head=32, dim=3200, block_size=576, vocab_size=16384))

@@ -441,7 +441,7 @@ def test_conv_cta_budget_is_bit_identical(cid, budget):
         lib.lg_vq_set_cta_budget(budget)
         y1, p1, s1, part1, _ = _run_case(c, x, w, bias, res)
     finally:
-        lib.lg_vq_set_cta_budget(-1)
+        lib.lg_vq_set_cta_budget(0)
     assert p0 == p1 == c.path and s0 == s1
     assert torch.equal(y0, y1)
     assert (part0 is None and part1 is None) or torch.equal(part0, part1)
