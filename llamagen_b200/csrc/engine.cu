@@ -102,23 +102,78 @@ struct Tensor {
 
 size_t align_up(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
 
+constexpr int kCounterInts = 128;   // device loop state: pos / step of chain g at [2g, 2g+1], the sampler's ticket at 64 + 2g
+
+// CUtensorMaps over a whole K and a whole V cache region: kKC-row boxes, and 16-row boxes for the tail chunk of the decode attention
+struct alignas(64) KvMaps {
+    unsigned char k[128], v[128], k16[128], v16[128];
+    bool usable = false;   // built: a bf16 / fp16 cache the TMA attention kernels can stream (attn_tma_maps_usable)
+};
+
+// Fills `m` for a K / V cache pair of total_rows rows of hdp elements each, stored in kv_dtype, of a model in `dtype` with head_dim hd
+int make_kv_maps(KvMaps& m, int dtype, int hd, int hdp, int kv_dtype, const void* kcache, const void* vcache, long long total_rows) {
+    m.usable = attn_tma_maps_usable(dtype, hd, hdp, total_rows);
+    if (!m.usable) return 0;
+    LG_TRY(attn_tma_make_map(m.k, kcache, total_rows, hdp, kv_dtype));
+    LG_TRY(attn_tma_make_map(m.v, vcache, total_rows, hdp, kv_dtype));
+    LG_TRY(attn_tma_make_map(m.k16, kcache, total_rows, hdp, kv_dtype, 1));
+    LG_TRY(attn_tma_make_map(m.v16, vcache, total_rows, hdp, kv_dtype, 1));
+    return 0;
+}
+
+// One attention call over layer `layer` of a K / V cache pair laid out [layer][rows, H, max_seq, hdp] (DESIGN §3): the geometry, the
+// softmax scale with an fp8 cache's scales folded in (kv_scales: this layer's {K, V} scales, null for a cache in the model dtype) and
+// the tensor maps over the whole pair. The caller sets q, out, the positions and the emb-mask.
+AttnArgs make_attn_args(int dtype, int H, int hd, int hdp, int rows, int max_seq, char* kcache, char* vcache, const KvMaps& maps,
+                        const float* kv_scales, int layer, int R, int Tq) {
+    AttnArgs aa{};
+    const long long row0 = (long long)layer * rows * H * max_seq;
+    const size_t row_bytes = (size_t)hdp * (kv_scales ? 1 : lg_dtype_info(dtype).esz);
+    aa.kcache = kcache + (size_t)row0 * row_bytes; aa.vcache = vcache + (size_t)row0 * row_bytes;
+    aa.R = R; aa.Tq = Tq; aa.H = H; aa.hd = hd; aa.hdp = hdp; aa.maxS = max_seq; aa.dtype = dtype;
+    aa.scale = 1.0f / sqrtf((float)hd);
+    if (kv_scales) {   // the K scale folds into the softmax scale, the V scale into O / L, the writers divide by them
+        const float ks = kv_scales[0], vs = kv_scales[1];
+        aa.kv_f8 = 1; aa.scale *= ks; aa.k_inv = 1.0f / ks; aa.v_inv = 1.0f / vs; aa.v_scale = vs;
+    }
+    if (maps.usable) {
+        aa.kmap = maps.k; aa.vmap = maps.v; aa.kmap16 = maps.k16; aa.vmap16 = maps.v16;
+        aa.cache_row_base = row0;
+    }
+    return aa;
+}
+
+// The separate QKV epilogue that writes q and the K / V rows `aa` attends over, from the QKV GEMM's split-K slabs
+QkvEpiArgs make_qkv_epi_args(const AttnArgs& aa, const float* partial, int ksplit, const float* freqs) {
+    QkvEpiArgs qa;
+    qa.partial = partial; qa.ksplit = ksplit; qa.M = aa.R * aa.Tq; qa.Tq = aa.Tq; qa.D = aa.H * aa.hd; qa.H = aa.H; qa.hd = aa.hd;
+    qa.pos = aa.pos; qa.freqs = freqs; qa.q = const_cast<void*>(aa.q);
+    qa.kcache = const_cast<void*>(aa.kcache); qa.vcache = const_cast<void*>(aa.vcache);
+    qa.maxS = aa.maxS; qa.dtype = aa.dtype; qa.hdp = aa.hdp;
+    qa.kv_f8 = aa.kv_f8; qa.k_inv = aa.k_inv; qa.v_inv = aa.v_inv;
+    return qa;
+}
+
+SampleArgs make_sample_args(const lg_sample_cfg& sc, const float* logits, int B, int V, int mix_cfg, int round_dtype) {
+    SampleArgs a{};
+    a.logits = logits; a.B = B; a.V = V; a.mix_cfg = mix_cfg; a.round_dtype = lg_dtype_is16(round_dtype) ? round_dtype : LG_DTYPE_F32;
+    a.cfg_scale = sc.cfg_scale; a.cfg_interval = sc.cfg_interval; a.temperature = sc.temperature;
+    a.top_k = sc.top_k; a.top_p = sc.top_p; a.greedy = sc.greedy; a.seed = sc.seed;
+    return a;
+}
+
+// The workspace (lg_engine::carve), or one decode chain's view of it
 struct Workspace {
-    char* base = nullptr;
-    size_t bytes = 0;
+    char* base = nullptr;     // start of the whole workspace
     int rows = 0, max_seq = 0;
-    // carved pointers
     char *kcache = nullptr, *vcache = nullptr;
+    size_t cache_bytes = 0;   // the K and V regions together, from kcache on (what the first use zero-fills)
     char *h = nullptr, *xn = nullptr, *q = nullptr, *attn = nullptr, *ff = nullptr, *x0 = nullptr;
     float *partial = nullptr, *logits = nullptr;
-    int32_t* tokens = nullptr;
-    int* counters = nullptr;  // [0] = pos, [1] = step (chain g of a split uses [2g], [2g+1])
-    size_t layer_cache_bytes = 0;
     size_t partial_floats = 0;
-    alignas(64) unsigned char kmap[128];   // CUtensorMap over the K / V cache regions (bf16 / fp16 only)
-    alignas(64) unsigned char vmap[128];
-    alignas(64) unsigned char kmap16[128];  // same regions, 16-row boxes (tail chunk of the decode attention)
-    alignas(64) unsigned char vmap16[128];
-    bool have_maps = false;
+    int32_t* tokens = nullptr;
+    int* counters = nullptr;  // [0] = pos, [1] = step, [64] = the fused sampler tail's ticket
+    KvMaps maps;
 };
 
 struct Layer {
@@ -144,13 +199,11 @@ struct lg_engine {
     const void *final_norm = nullptr, *output = nullptr;
     const float* freqs = nullptr;
     bool finalized = false;
-    Workspace ws;                         // ACTIVE workspace (full, or one of the two halves while a group is issued)
-    static constexpr int kMaxChains = 8;
-    Workspace full, sub[kMaxChains];      // sub[g]: rows/n_sub each, carved INSIDE the regions of `full` (multi-chain decode)
+    static constexpr int kMaxChains = 2;
+    Workspace full, sub[kMaxChains];      // sub[g]: chain g's view of `full` (multi-chain decode)
     int n_sub = 0;                        // 0: no split available
     bool use_graph = true;
     bool ws_needs_zero = false;           // KV cache + counters of `full` still have to be zero-filled (done on the caller's stream)
-    bool skip_first_norm = false;         // set by the decode loop when the sample kernel's fused tail already wrote xn = RMSNorm_0(h)
     cudaStream_t works[kMaxChains] = {};   // engine-owned streams (one per chain)
     cudaEvent_t ev_fork = nullptr, ev_joins[kMaxChains] = {};
     ~lg_engine() {
@@ -168,40 +221,55 @@ struct lg_engine {
                gemv_small_supported(M, 3 * D, D, dt, false) && gemv_small_supported(M, D, D, dt, false) &&
                gemv_small_supported(M, F, D, dt, true) && gemv_small_supported(M, D, F, dt, false) && gemv_small_supported(M, V, D, dt, false);
     }
-    size_t carve(Workspace& o, char* base, int rows, int max_seq) const;
+    size_t carve(Workspace& o, char* base, int rows, int max_seq, int g = 0, int n = 1) const;
+    // K / V tensor maps over every layer of a workspace or chain view
+    int make_maps(Workspace& w) const {
+        return make_kv_maps(w.maps, cfg.dtype, hd, hdp, kv_f8 ? LG_DTYPE_E4M3 : cfg.dtype, w.kcache, w.vcache,
+                            (long long)cfg.n_layer * w.rows * cfg.n_head * w.max_seq);
+    }
+    AttnArgs attn_args(const Workspace& w, int l, int R, int Tq) const {
+        return make_attn_args(cfg.dtype, cfg.n_head, hd, hdp, w.rows, w.max_seq, w.kcache, w.vcache, w.maps,
+                              kv_f8 ? &kv_scales[2 * l] : nullptr, l, R, Tq);
+    }
     int zero_fill_if_needed(cudaStream_t st) {
         if (!ws_needs_zero || !full.base) return 0;
-        LG_CUDA_OK(cudaMemsetAsync(full.kcache, 0, 2 * ((full.layer_cache_bytes * cfg.n_layer + 255) / 256 * 256), st));
-        LG_CUDA_OK(cudaMemsetAsync(full.counters, 0, 128 * sizeof(int), st));
+        LG_CUDA_OK(cudaMemsetAsync(full.kcache, 0, full.cache_bytes, st));
+        LG_CUDA_OK(cudaMemsetAsync(full.counters, 0, kCounterInts * sizeof(int), st));
         ws_needs_zero = false;
         return 0;
     }
-    int forward(int M, int Tq, PosArg pos, const float* emb_mask, int B, float* logits_out, bool round_out,
+    // xn_ready: xn already holds RMSNorm_0(h) (the fused tail of the previous decode step's sample kernel wrote it)
+    int forward(const Workspace& w, int M, int Tq, PosArg pos, const float* emb_mask, int B, float* logits_out, bool xn_ready,
                 cudaStream_t st);
-    int embed_cond(const void* cond, int B, int R, int T, cudaStream_t st);
-    int gemm(const void* x, int M, int N, int K, const void* wa, const void* wb, int n_split, int* ksplit,
+    int embed_cond(const Workspace& w, const void* cond, int B, int R, int T, cudaStream_t st);
+    int gemm(const Workspace& w, const void* x, int M, int N, int K, const void* wa, const void* wb, int n_split, int* ksplit,
              float* direct_out, cudaStream_t st, const GemmNext* next = nullptr);
 };
 
-size_t lg_engine::carve(Workspace& o, char* base, int rows, int max_seq) const {
+// Lays out the workspace for `rows` rows and max_seq positions from `base` (null: sizes only) and returns its bytes. With n > 1, `o`
+// becomes chain g's view of that same layout: the g-th n-th of every region that scales with rows (rows / n rows each), a 64-float
+// aligned n-th of the GEMM partials, and the counters from 2g on.
+size_t lg_engine::carve(Workspace& o, char* base, int rows, int max_seq, int g, int n) const {
     const int L = cfg.n_layer, D = cfg.dim, F = cfg.ffn_dim, V = cfg.vocab_size, H = cfg.n_head;
     const int Tc = cfg.model_type == LG_MODEL_T2I ? cfg.cls_token_num : 1;
     const size_t Mmax = (size_t)rows * Tc;
     size_t off = 0;
-    auto take = [&](size_t bytes) {
-        char* p = base ? base + off : nullptr;
+    auto take = [&](size_t bytes, size_t chain_stride) {
+        char* p = base ? base + off + g * chain_stride : nullptr;
         off += align_up(bytes);
         return p;
     };
-    o.layer_cache_bytes = (size_t)rows * H * max_seq * hdp * kv_esz;
-    o.kcache = take(o.layer_cache_bytes * L);
-    o.vcache = take(o.layer_cache_bytes * L);
-    o.h = take(Mmax * D * esz);
-    o.xn = take(Mmax * D * esz);
-    o.q = take(Mmax * D * esz);
-    o.attn = take(Mmax * D * esz);
-    o.ff = take(Mmax * F * esz);
-    o.x0 = take(cfg.model_type == LG_MODEL_T2I ? Mmax * cfg.caption_dim * esz : 0);
+    auto split = [&](size_t bytes) { return take(bytes, bytes / n); };
+    const size_t cache = (size_t)rows * H * max_seq * hdp * kv_esz * L;
+    o.kcache = split(cache);
+    o.vcache = split(cache);
+    o.cache_bytes = off;
+    o.h = split(Mmax * D * esz);
+    o.xn = split(Mmax * D * esz);
+    o.q = split(Mmax * D * esz);
+    o.attn = split(Mmax * D * esz);
+    o.ff = split(Mmax * F * esz);
+    o.x0 = split(cfg.model_type == LG_MODEL_T2I ? Mmax * cfg.caption_dim * esz : 0);
     size_t pf = 0;
     const int Ms[2] = {rows, (int)Mmax};
     for (int i = 0; i < 2; ++i) {
@@ -213,137 +281,118 @@ size_t lg_engine::carve(Workspace& o, char* base, int rows, int max_seq) const {
         if (cfg.model_type == LG_MODEL_T2I) pf = std::max(pf, gemm_partial_floats(M, D, cfg.caption_dim, cfg.dtype));
     }
     pf = std::max(pf, gemm_partial_floats(rows, V, D, cfg.dtype));
-    o.partial_floats = pf;
-    o.partial = (float*)take(pf * sizeof(float));
-    o.logits = (float*)take((size_t)rows * V * sizeof(float));
-    o.tokens = (int32_t*)take((size_t)rows * sizeof(int32_t));
-    o.counters = (int*)take(128 * sizeof(int));   // [0, 16): pos/step per chain (<= 8 chains)
-    o.rows = rows;
+    o.partial_floats = n == 1 ? pf : pf / n / 64 * 64;
+    o.partial = (float*)take(pf * sizeof(float), o.partial_floats * sizeof(float));
+    o.logits = (float*)split((size_t)rows * V * sizeof(float));
+    o.tokens = (int32_t*)split((size_t)rows * sizeof(int32_t));
+    o.counters = (int*)take(kCounterInts * sizeof(int), 2 * sizeof(int));
+    o.base = base;
+    o.rows = rows / n;
     o.max_seq = max_seq;
     return off;
 }
 
-int lg_engine::gemm(const void* x, int M, int N, int K, const void* wa, const void* wb, int n_split, int* ksplit,
+int lg_engine::gemm(const Workspace& w, const void* x, int M, int N, int K, const void* wa, const void* wb, int n_split, int* ksplit,
                     float* direct_out, cudaStream_t st, const GemmNext* next) {
     // when the plan needs a single slab the GEMM can write straight into `direct_out`
     const size_t need = gemm_partial_floats(M, N, K, cfg.dtype);
     const size_t slabs = need / ((size_t)M * N);
-    float* dst = (direct_out && slabs == 1) ? direct_out : ws.partial;
+    float* dst = (direct_out && slabs == 1) ? direct_out : w.partial;
     // the plan (k-slices) is not monotone in M and depends on run-time switches: never trust the carve-time sizing blindly
-    LG_REQUIRE(dst == direct_out || need <= ws.partial_floats, "gemm %dx%dx%d needs %zu partial floats, workspace holds %zu", M, N, K, need,
-               ws.partial_floats);
+    LG_REQUIRE(dst == direct_out || need <= w.partial_floats, "gemm %dx%dx%d needs %zu partial floats, workspace holds %zu", M, N, K, need,
+               w.partial_floats);
     GemmPlan plan;
     LG_TRY(gemm_partial(x, K, wa, wb, n_split, M, N, K, cfg.dtype, dst, &plan, st, next));
     *ksplit = plan.ksplit;
     return dst == direct_out ? 1 : 0;
 }
 
-int lg_engine::forward(int M, int Tq, PosArg pos, const float* emb_mask, int B, float* logits_out, bool round_out,
+int lg_engine::forward(const Workspace& w, int M, int Tq, PosArg pos, const float* emb_mask, int B, float* logits_out, bool xn_ready,
                        cudaStream_t st) {
-    const int L = cfg.n_layer, D = cfg.dim, F = cfg.ffn_dim, V = cfg.vocab_size, H = cfg.n_head;
+    const int L = cfg.n_layer, D = cfg.dim, F = cfg.ffn_dim, V = cfg.vocab_size;
     const int R = M / Tq;
     const int dt = cfg.dtype;
     int ks = 1;
-    auto attn_args = [&](int l) {
-        AttnArgs aa;
-        aa.q = ws.q; aa.kcache = ws.kcache + (size_t)l * ws.layer_cache_bytes; aa.vcache = ws.vcache + (size_t)l * ws.layer_cache_bytes;
-        aa.out = ws.attn; aa.R = R; aa.Tq = Tq; aa.H = H; aa.hd = hd;
-        aa.maxS = ws.max_seq; aa.pos = pos; aa.emb_mask = emb_mask; aa.B = B; aa.hdp = hdp;
-        aa.Tc = cfg.cls_token_num; aa.scale = 1.0f / sqrtf((float)hd); aa.dtype = dt;
-        if (kv_f8) {   // the K scale folds into the softmax scale, the V scale into O / L, the writers divide by them
-            const float ks = kv_scales[2 * l], vs = kv_scales[2 * l + 1];
-            aa.kv_f8 = 1; aa.scale *= ks; aa.k_inv = 1.0f / ks; aa.v_inv = 1.0f / vs; aa.v_scale = vs;
-        }
-        if (ws.have_maps) {
-            aa.kmap = ws.kmap; aa.vmap = ws.vmap; aa.kmap16 = ws.kmap16; aa.vmap16 = ws.vmap16;
-            aa.cache_row_base = (long long)l * ws.rows * H * ws.max_seq;
-        }
+    auto layer_attn = [&](int l) {
+        AttnArgs aa = attn_args(w, l, R, Tq);
+        aa.q = w.q; aa.out = w.attn; aa.pos = pos; aa.emb_mask = emb_mask; aa.B = B; aa.Tc = cfg.cls_token_num;
         return aa;
     };
     // ---- R <= 8 decode step (batch-1 latency path, gemv_small.cu): 5 dependent kernels per layer, no slabs
-    if (Tq == 1 && small_row_path(M, attn_args(0))) {
-        skip_first_norm = false;
+    if (Tq == 1 && small_row_path(M, attn_args(w, 0, R, Tq))) {
         for (int l = 0; l < L; ++l) {
             const Layer& ly = layers[l];
-            GemvSmall gq{ly.wqkv, nullptr, 3 * D, D, M, ws.h, ly.attn_norm, cfg.norm_eps, ws.partial, nullptr, nullptr, dt};
+            GemvSmall gq{ly.wqkv, nullptr, 3 * D, D, M, w.h, ly.attn_norm, cfg.norm_eps, w.partial, nullptr, nullptr, dt};
             LG_PROF(PC_GEMM_QKV, st, launch_gemv_small(gq, st));
-            AttnArgs aa = attn_args(l);
-            aa.qkv_partial = ws.partial; aa.qkv_ksplit = 1; aa.freqs = freqs;
+            AttnArgs aa = layer_attn(l);
+            aa.qkv_partial = w.partial; aa.qkv_ksplit = 1; aa.freqs = freqs;
             LG_PROF(PC_ATTENTION, st, launch_attention(aa, st));
-            GemvSmall go{ly.wo, nullptr, D, D, M, ws.attn, nullptr, 0.f, nullptr, ws.h, nullptr, dt};
+            GemvSmall go{ly.wo, nullptr, D, D, M, w.attn, nullptr, 0.f, nullptr, w.h, nullptr, dt};
             LG_PROF(PC_GEMM_WO, st, launch_gemv_small(go, st));
-            GemvSmall g13{ly.w1, ly.w3, F, D, M, ws.h, ly.ffn_norm, cfg.norm_eps, nullptr, nullptr, ws.ff, dt};
+            GemvSmall g13{ly.w1, ly.w3, F, D, M, w.h, ly.ffn_norm, cfg.norm_eps, nullptr, nullptr, w.ff, dt};
             LG_PROF(PC_GEMM_W13, st, launch_gemv_small(g13, st));
-            GemvSmall g2{ly.w2, nullptr, D, F, M, ws.ff, nullptr, 0.f, nullptr, ws.h, nullptr, dt};
+            GemvSmall g2{ly.w2, nullptr, D, F, M, w.ff, nullptr, 0.f, nullptr, w.h, nullptr, dt};
             LG_PROF(PC_GEMM_W2, st, launch_gemv_small(g2, st));
         }
-        GemvSmall gh{output, nullptr, V, D, M, ws.h, final_norm, cfg.norm_eps, logits_out, nullptr, nullptr, dt};
+        GemvSmall gh{output, nullptr, V, D, M, w.h, final_norm, cfg.norm_eps, logits_out, nullptr, nullptr, dt};
         LG_PROF(PC_GEMM_HEAD, st, launch_gemv_small(gh, st));
         return 0;
     }
-    if (!skip_first_norm) LG_PROF(PC_EMBED_MISC, st, launch_rmsnorm(ws.h, layers[0].attn_norm, ws.xn, M, D, cfg.norm_eps, dt, st));
-    skip_first_norm = false;
+    if (!xn_ready) LG_PROF(PC_EMBED_MISC, st, launch_rmsnorm(w.h, layers[0].attn_norm, w.xn, M, D, cfg.norm_eps, dt, st));
     for (int l = 0; l < L; ++l) {
         const Layer& ly = layers[l];
-        char* kc = ws.kcache + (size_t)l * ws.layer_cache_bytes;
-        char* vc = ws.vcache + (size_t)l * ws.layer_cache_bytes;
         const size_t eb = esz;
         GemmNext nx_wo{ly.wo, (size_t)D * D * eb, nullptr, 0};
         GemmNext nx_w13{ly.w1, (size_t)F * D * eb, ly.w3, (size_t)F * D * eb};
         GemmNext nx_w2{ly.w2, (size_t)D * F * eb, nullptr, 0};
         GemmNext nx_qkv{(l + 1 < L) ? layers[l + 1].wqkv : output, (l + 1 < L) ? (size_t)3 * D * D * eb : (size_t)V * D * eb, nullptr, 0};
-        LG_PROF(PC_GEMM_QKV, st, gemm(ws.xn, M, 3 * D, D, ly.wqkv, nullptr, 0, &ks, nullptr, st, &nx_wo));
-        QkvEpiArgs qa;
-        qa.partial = ws.partial; qa.ksplit = ks; qa.M = M; qa.Tq = Tq; qa.D = D; qa.H = H; qa.hd = hd;
-        qa.pos = pos; qa.freqs = freqs; qa.q = ws.q; qa.kcache = kc; qa.vcache = vc; qa.maxS = ws.max_seq; qa.dtype = dt; qa.hdp = hdp;
-        AttnArgs aa = attn_args(l);
-        qa.kv_f8 = aa.kv_f8; qa.k_inv = aa.k_inv; qa.v_inv = aa.v_inv;
+        LG_PROF(PC_GEMM_QKV, st, gemm(w, w.xn, M, 3 * D, D, ly.wqkv, nullptr, 0, &ks, nullptr, st, &nx_wo));
+        AttnArgs aa = layer_attn(l);
         // decode steps on the TMA path: the attention kernel is also the QKV epilogue (one dependent kernel less)
         const bool fuse_qkv = lg_env_flag("LG_FUSE_QKV", 1) && attn_tma_enabled() && attn_tma_supported(aa);
         if (fuse_qkv) {
-            aa.qkv_partial = ws.partial; aa.qkv_ksplit = ks; aa.freqs = freqs;
+            aa.qkv_partial = w.partial; aa.qkv_ksplit = ks; aa.freqs = freqs;
         } else {
-            LG_PROF(PC_QKV_EPI, st, launch_qkv_epilogue(qa, st));
+            LG_PROF(PC_QKV_EPI, st, launch_qkv_epilogue(make_qkv_epi_args(aa, w.partial, ks, freqs), st));
         }
         LG_PROF(PC_ATTENTION, st, launch_attention(aa, st));
-        LG_PROF(PC_GEMM_WO, st, gemm(ws.attn, M, D, D, ly.wo, nullptr, 0, &ks, nullptr, st, &nx_w13));
-        LG_PROF(PC_RESNORM, st, launch_residual_norm(ws.partial, ks, M, D, ws.h, ly.ffn_norm, ws.xn, cfg.norm_eps, dt, st));
-        LG_PROF(PC_GEMM_W13, st, gemm(ws.xn, M, 2 * F, D, ly.w1, ly.w3, F, &ks, nullptr, st, &nx_w2));
-        LG_PROF(PC_SILU, st, launch_silu_mul(ws.partial, ks, M, F, ws.ff, dt, st));
-        LG_PROF(PC_GEMM_W2, st, gemm(ws.ff, M, D, F, ly.w2, nullptr, 0, &ks, nullptr, st, &nx_qkv));
+        LG_PROF(PC_GEMM_WO, st, gemm(w, w.attn, M, D, D, ly.wo, nullptr, 0, &ks, nullptr, st, &nx_w13));
+        LG_PROF(PC_RESNORM, st, launch_residual_norm(w.partial, ks, M, D, w.h, ly.ffn_norm, w.xn, cfg.norm_eps, dt, st));
+        LG_PROF(PC_GEMM_W13, st, gemm(w, w.xn, M, 2 * F, D, ly.w1, ly.w3, F, &ks, nullptr, st, &nx_w2));
+        LG_PROF(PC_SILU, st, launch_silu_mul(w.partial, ks, M, F, w.ff, dt, st));
+        LG_PROF(PC_GEMM_W2, st, gemm(w, w.ff, M, D, F, ly.w2, nullptr, 0, &ks, nullptr, st, &nx_qkv));
         const void* next_norm = (l + 1 < L) ? layers[l + 1].attn_norm : final_norm;
-        LG_PROF(PC_RESNORM, st, launch_residual_norm(ws.partial, ks, M, D, ws.h, next_norm, ws.xn, cfg.norm_eps, dt, st));
+        LG_PROF(PC_RESNORM, st, launch_residual_norm(w.partial, ks, M, D, w.h, next_norm, w.xn, cfg.norm_eps, dt, st));
     }
     // head on the last position only (generate.py:58 reads logits[:, -1])
-    const void* xlast = ws.xn;
+    const void* xlast = w.xn;
     if (Tq > 1) {
-        LG_TRY(launch_gather_last(ws.xn, R, Tq, D, dt, ws.q, st));
-        xlast = ws.q;
+        LG_TRY(launch_gather_last(w.xn, R, Tq, D, dt, w.q, st));
+        xlast = w.q;
     }
-    (void)round_out;
     prof_begin(PC_GEMM_HEAD, st);
     GemmNext nx_first{layers[0].wqkv, (size_t)3 * D * D * esz, nullptr, 0};   // the next decode step starts with layer 0
-    const int direct = gemm(xlast, R, V, D, output, nullptr, 0, &ks, logits_out, st, &nx_first);
+    const int direct = gemm(w, xlast, R, V, D, output, nullptr, 0, &ks, logits_out, st, &nx_first);
     prof_end(st);
     if (direct < 0) return direct;
-    if (direct == 0) LG_TRY(launch_reduce_f32(ws.partial, ks, R, V, logits_out, st));
+    if (direct == 0) LG_TRY(launch_reduce_f32(w.partial, ks, R, V, logits_out, st));
     return 0;
 }
 
-int lg_engine::embed_cond(const void* cond, int B, int R, int T, cudaStream_t st) {
+int lg_engine::embed_cond(const Workspace& w, const void* cond, int B, int R, int T, cudaStream_t st) {
     const int D = cfg.dim, dt = cfg.dtype;
     if (cfg.model_type == LG_MODEL_C2I) {
         // LabelEmbedder (gpt.py:78-83); null class = num_classes (generate.py:130)
-        return launch_embed(cls_table, (const int32_t*)cond, B, R, cfg.num_classes, D, dt, ws.h, st);
+        return launch_embed(cls_table, (const int32_t*)cond, B, R, cfg.num_classes, D, dt, w.h, st);
     }
     // CaptionEmbedder: cap_proj = fc2(gelu_tanh(fc1(x))) (gpt.py:110-131); uncond rows = uncond_embedding
     const int C = cfg.caption_dim, M = R * T;
     int ks = 1;
-    LG_TRY(launch_build_caption_rows(cond, uncond, B, R, T, C, dt, ws.x0, st));
-    LG_TRY(gemm(ws.x0, M, D, C, cap_fc1, nullptr, 0, &ks, nullptr, st));
-    LG_TRY(launch_store_act(ws.partial, ks, M, D, ws.attn, 1, dt, st));
-    LG_TRY(gemm(ws.attn, M, D, D, cap_fc2, nullptr, 0, &ks, nullptr, st));
-    LG_TRY(launch_store_act(ws.partial, ks, M, D, ws.h, 0, dt, st));
+    LG_TRY(launch_build_caption_rows(cond, uncond, B, R, T, C, dt, w.x0, st));
+    LG_TRY(gemm(w, w.x0, M, D, C, cap_fc1, nullptr, 0, &ks, nullptr, st));
+    LG_TRY(launch_store_act(w.partial, ks, M, D, w.attn, 1, dt, st));
+    LG_TRY(gemm(w, w.attn, M, D, D, cap_fc2, nullptr, 0, &ks, nullptr, st));
+    LG_TRY(launch_store_act(w.partial, ks, M, D, w.h, 0, dt, st));
     return 0;
 }
 
@@ -461,79 +510,36 @@ int lg_engine_set_workspace(lg_engine* e, void* dev_ws, size_t bytes, int rows, 
     LG_REQUIRE(e && dev_ws, "lg_engine_set_workspace: null argument");
     DeviceGuard guard(e->device);
     LG_REQUIRE(((uintptr_t)dev_ws & 255) == 0, "workspace must be 256-byte aligned");
-    Workspace tmp;
-    const size_t needb = e->carve(tmp, (char*)dev_ws, rows, max_seq);
+    Workspace full;
+    const size_t needb = e->carve(full, (char*)dev_ws, rows, max_seq);
     LG_REQUIRE(bytes >= needb, "workspace too small: %zu < %zu", bytes, needb);
-    tmp.base = (char*)dev_ws;
-    tmp.bytes = bytes;
     // The reference zero-fills the KV cache (gpt.py:174-175). The tensor-core attention multiplies masked
     // probabilities (exactly 0) with whatever sits in not-yet-written V rows, so those rows must be finite.
     // The zero-fill is enqueued on the CALLER'S stream by the first prefill / decode / generate that uses this workspace
     // (zero_fill_if_needed): a legacy-NULL-stream memset here would not be ordered against non-blocking streams that may
     // still be running kernels on memory the caching allocator has just recycled.
     e->ws_needs_zero = true;
-    tmp.have_maps = false;
-    const int dt = e->cfg.dtype;
-    const int kvdt = e->kv_f8 ? LG_DTYPE_E4M3 : dt;   // storage type of the cache regions
-    const long long total_rows = (long long)e->cfg.n_layer * rows * e->cfg.n_head * max_seq;
-    if (attn_tma_maps_usable(dt, e->hd, e->hdp, total_rows)) {
-        LG_TRY(attn_tma_make_map(tmp.kmap, tmp.kcache, total_rows, e->hdp, kvdt));
-        LG_TRY(attn_tma_make_map(tmp.vmap, tmp.vcache, total_rows, e->hdp, kvdt));
-        LG_TRY(attn_tma_make_map(tmp.kmap16, tmp.kcache, total_rows, e->hdp, kvdt, 1));
-        LG_TRY(attn_tma_make_map(tmp.vmap16, tmp.vcache, total_rows, e->hdp, kvdt, 1));
-        tmp.have_maps = true;
-    }
-    e->full = tmp;
-    e->ws = tmp;
-    // n equal sub-batch workspaces inside the same memory (every region scales with rows, so chain g takes the g-th
-    // 1/n of every region; the K/V parts stay inside the zero-initialised cache regions).
+    LG_TRY(e->make_maps(full));
+    e->full = full;
     e->n_sub = 0;
     // Chain-count policy: every chain streams ALL the weights, so two chains only pay while a layer's weights survive in L2 between
     // the chains' visits, next to the KV and activation traffic of the other chain; otherwise they double the HBM weight traffic.
     // Two chains run while a layer is at most a third of the L2. On an H100 80GB HBM3 (50 MB L2; both settings alternated twice in
     // one run) one chain is faster for GPT-L (27 MB per layer, c2i 256 px, B = 64: 431 vs 469 ms/step) and GPT-XL (39 MB, 384 px,
     // B = 32: 1659 vs 1849 ms/step).
-    // LG_SPLIT forces the chain count.
+    // LG_SPLIT forces the chain count (at most two).
     const double layer_bytes = (4.0 * e->cfg.dim * e->cfg.dim + 3.0 * e->cfg.dim * e->cfg.ffn_dim) * e->esz;
     int l2_bytes = 0, dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&l2_bytes, cudaDevAttrL2CacheSize, dev) != cudaSuccess) l2_bytes = 0;
     int n = lg_env_flag("LG_SPLIT", 3.0 * layer_bytes <= (double)l2_bytes ? 2 : 1);
     if (n > lg_engine::kMaxChains) n = lg_engine::kMaxChains;
     while (n >= 2 && (rows % n != 0 || (rows / n) % 2 != 0 || rows / n < 16)) --n;
-    if (n >= 2 && lg_dtype_is16(dt) && tmp.have_maps) {
-        const lg_model_cfg& c = e->cfg;
-        const int hr = rows / n;
-        const int Tc = c.model_type == LG_MODEL_T2I ? c.cls_token_num : 1;
-        const size_t Mh = (size_t)hr * Tc, esz = e->esz;
-        Workspace probe;
-        e->carve(probe, nullptr, hr, max_seq);
-        const size_t pf_full = tmp.partial_floats, pf_part = probe.partial_floats;
-        const size_t pf_slot = pf_full / n / 64 * 64;
-        if (pf_part <= pf_slot) {
-            for (int g = 0; g < n; ++g) {
-                Workspace w = tmp;
-                w.rows = hr;
-                w.layer_cache_bytes = (size_t)hr * c.n_head * max_seq * e->hdp * e->kv_esz;
-                w.kcache = tmp.kcache + (size_t)g * w.layer_cache_bytes * c.n_layer;
-                w.vcache = tmp.vcache + (size_t)g * w.layer_cache_bytes * c.n_layer;
-                w.h = tmp.h + (size_t)g * Mh * c.dim * esz;
-                w.xn = tmp.xn + (size_t)g * Mh * c.dim * esz;
-                w.q = tmp.q + (size_t)g * Mh * c.dim * esz;
-                w.attn = tmp.attn + (size_t)g * Mh * c.dim * esz;
-                w.ff = tmp.ff + (size_t)g * Mh * c.ffn_dim * esz;
-                w.x0 = tmp.x0 ? tmp.x0 + (size_t)g * Mh * c.caption_dim * esz : nullptr;
-                w.partial = tmp.partial + (size_t)g * pf_slot;
-                w.logits = tmp.logits + (size_t)g * hr * c.vocab_size;
-                w.tokens = tmp.tokens + (size_t)g * hr;
-                w.counters = tmp.counters + 2 * g;
-                const long long total_rows = (long long)c.n_layer * hr * c.n_head * max_seq;
-                LG_TRY(attn_tma_make_map(w.kmap, w.kcache, total_rows, e->hdp, kvdt));
-                LG_TRY(attn_tma_make_map(w.vmap, w.vcache, total_rows, e->hdp, kvdt));
-                LG_TRY(attn_tma_make_map(w.kmap16, w.kcache, total_rows, e->hdp, kvdt, 1));
-                LG_TRY(attn_tma_make_map(w.vmap16, w.vcache, total_rows, e->hdp, kvdt, 1));
-                w.have_maps = true;
-                e->sub[g] = w;
-            }
+    if (n >= 2 && full.maps.usable) {   // chains run bf16 / fp16 models whose cache the TMA attention kernels stream
+        Workspace need;                 // a chain's GEMMs must fit in its share of the partials
+        e->carve(need, nullptr, rows / n, max_seq);
+        for (int g = 0; g < n; ++g) e->carve(e->sub[g], (char*)dev_ws, rows, max_seq, g, n);
+        if (need.partial_floats <= e->sub[0].partial_floats) {
+            for (int g = 0; g < n; ++g) LG_TRY(e->make_maps(e->sub[g]));
             e->n_sub = n;
         }
     }
@@ -567,7 +573,6 @@ int lg_engine_set_kv_cache(lg_engine* e, int kv_dtype, const float* scales) {
     e->kv_esz = e->kv_f8 ? 1 : e->esz;
     e->kv_scales = sc;
     e->full = Workspace();
-    e->ws = Workspace();
     e->n_sub = 0;
     e->ws_needs_zero = false;
     return 0;
@@ -576,9 +581,8 @@ int lg_engine_set_kv_cache(lg_engine* e, int kv_dtype, const float* scales) {
 static int check_ready(lg_engine* e, int rows, int seq) {
     LG_REQUIRE(e && e->finalized, "engine not finalized");
     LG_REQUIRE(e->full.base, "workspace not set");
-    e->ws = e->full;
-    LG_REQUIRE(rows <= e->ws.rows, "rows %d exceed workspace rows %d", rows, e->ws.rows);
-    LG_REQUIRE(seq <= e->ws.max_seq, "sequence %d exceeds workspace max_seq %d", seq, e->ws.max_seq);
+    LG_REQUIRE(rows <= e->full.rows, "rows %d exceed workspace rows %d", rows, e->full.rows);
+    LG_REQUIRE(seq <= e->full.max_seq, "sequence %d exceeds workspace max_seq %d", seq, e->full.max_seq);
     LG_REQUIRE(seq <= e->cfg.cls_token_num + e->cfg.block_size, "sequence %d exceeds the RoPE table (%d)", seq,
                e->cfg.cls_token_num + e->cfg.block_size);
     return 0;
@@ -597,9 +601,9 @@ int lg_prefill(lg_engine* e, const void* cond, const float* emb_mask, int B, int
     LG_TRY(e->zero_fill_if_needed(st));
     LG_REQUIRE(cond && logits_out && B > 0, "lg_prefill: bad argument");
     LG_REQUIRE(T == e->cfg.cls_token_num, "lg_prefill: T=%d must equal cls_token_num=%d", T, e->cfg.cls_token_num);
-    LG_TRY(e->embed_cond(cond, B, R, T, st));
+    LG_TRY(e->embed_cond(e->full, cond, B, R, T, st));
     PosArg pos{nullptr, 0};
-    LG_TRY(e->forward(R * T, T, pos, emb_mask, B, logits_out, false, st));
+    LG_TRY(e->forward(e->full, R * T, T, pos, emb_mask, B, logits_out, false, st));
     LG_TRY(round_logits_inplace(logits_out, (size_t)R * e->cfg.vocab_size, e->cfg.dtype, st));
     return 0;
 }
@@ -612,9 +616,9 @@ int lg_decode_step(lg_engine* e, const int32_t* tokens, int B, int pos, int use_
     LG_TRY(check_ready(e, R, pos + 1));
     LG_TRY(e->zero_fill_if_needed(st));
     LG_REQUIRE(tokens && logits_out && B > 0 && pos >= 0, "lg_decode_step: bad argument");
-    LG_TRY(launch_embed(e->tok_emb, tokens, B, R, -1, e->cfg.dim, e->cfg.dtype, e->ws.h, st));
+    LG_TRY(launch_embed(e->tok_emb, tokens, B, R, -1, e->cfg.dim, e->cfg.dtype, e->full.h, st));
     PosArg p{nullptr, pos};
-    LG_TRY(e->forward(R, 1, p, nullptr, B, logits_out, false, st));
+    LG_TRY(e->forward(e->full, R, 1, p, nullptr, B, logits_out, false, st));
     LG_TRY(round_logits_inplace(logits_out, (size_t)R * e->cfg.vocab_size, e->cfg.dtype, st));
     return 0;
 }
@@ -630,9 +634,9 @@ int lg_decode_rows(lg_engine* e, const int32_t* tokens, const int32_t* pos_rows,
     LG_TRY(e->zero_fill_if_needed(st));
     LG_REQUIRE(tokens && pos_rows && logits_out && B > 0, "lg_decode_rows: bad argument");
     LG_REQUIRE(e->cfg.model_type == LG_MODEL_C2I && e->cfg.cls_token_num == 1, "lg_decode_rows: class-conditional models only");
-    LG_TRY(launch_embed_rows(e->cls_table, e->tok_emb, tokens, pos_rows, B, R, e->cfg.num_classes, e->cfg.dim, e->cfg.dtype, e->ws.h, st));
+    LG_TRY(launch_embed_rows(e->cls_table, e->tok_emb, tokens, pos_rows, B, R, e->cfg.num_classes, e->cfg.dim, e->cfg.dtype, e->full.h, st));
     PosArg p{nullptr, 0, pos_rows};
-    LG_TRY(e->forward(R, 1, p, nullptr, B, logits_out, false, st));
+    LG_TRY(e->forward(e->full, R, 1, p, nullptr, B, logits_out, false, st));
     LG_TRY(round_logits_inplace(logits_out, (size_t)R * e->cfg.vocab_size, e->cfg.dtype, st));
     return 0;
 }
@@ -640,10 +644,7 @@ int lg_decode_rows(lg_engine* e, const int32_t* tokens, const int32_t* pos_rows,
 int lg_sample_rows(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc, const uint64_t* seed_rows,
                    const int32_t* step_rows, int32_t* out_idx, int32_t* out_seq, int seq_stride, void* stream) {
     LG_REQUIRE(logits && sc && seed_rows && step_rows && (out_idx || out_seq), "lg_sample_rows: null argument");
-    SampleArgs a{};
-    a.logits = logits; a.B = B; a.V = V; a.mix_cfg = mix_cfg; a.round_dtype = lg_dtype_is16(round_dtype) ? round_dtype : LG_DTYPE_F32;
-    a.cfg_scale = sc->cfg_scale; a.cfg_interval = sc->cfg_interval; a.temperature = sc->temperature;
-    a.top_k = sc->top_k; a.top_p = sc->top_p; a.greedy = sc->greedy; a.seed = sc->seed; a.step = 0;
+    SampleArgs a = make_sample_args(*sc, logits, B, V, mix_cfg, round_dtype);
     a.seed_rows = seed_rows; a.step_rows = step_rows;
     a.out_idx = out_idx; a.out_seq = out_seq; a.seq_stride = seq_stride;
     return launch_sample(a, (cudaStream_t)stream);
@@ -652,11 +653,8 @@ int lg_sample_rows(const float* logits, int B, int V, int mix_cfg, int round_dty
 int lg_sample(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc, uint64_t step,
               int32_t* out_idx, float* out_probs, void* stream) {
     LG_REQUIRE(logits && sc && out_idx, "lg_sample: null argument");
-    SampleArgs a{};
-    a.logits = logits; a.B = B; a.V = V; a.mix_cfg = mix_cfg; a.round_dtype = lg_dtype_is16(round_dtype) ? round_dtype : LG_DTYPE_F32;
-    a.cfg_scale = sc->cfg_scale; a.cfg_interval = sc->cfg_interval; a.temperature = sc->temperature;
-    a.top_k = sc->top_k; a.top_p = sc->top_p; a.greedy = sc->greedy; a.seed = sc->seed; a.step = step;
-    a.out_idx = out_idx; a.out_probs = out_probs;
+    SampleArgs a = make_sample_args(*sc, logits, B, V, mix_cfg, round_dtype);
+    a.step = step; a.out_idx = out_idx; a.out_probs = out_probs;
     return launch_sample(a, (cudaStream_t)stream);
 }
 
@@ -691,12 +689,11 @@ int lg_generate(lg_engine* e, const void* cond, const float* emb_mask, int B, in
         cudaEventRecord(e->ev_joins[i], e->works[i]);
         cudaStreamWaitEvent(caller, e->ev_joins[i], 0);
     }
-    if (e->full.base) e->ws = e->full;
     return rc;
 }
 
 namespace {
-// One independent decode chain (a contiguous group of images with its own workspace half, stream and graph).
+// One independent decode chain (a contiguous group of images with its own workspace view, stream and graph).
 struct Chain {
     Workspace w;
     cudaStream_t st = nullptr;
@@ -739,11 +736,8 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
         k.cond = c.model_type == LG_MODEL_C2I ? (const void*)((const int32_t*)cond + boff)
                                               : (const void*)((const char*)cond + boff * T * c.caption_dim * e->esz);
         k.emb_mask = emb_mask ? emb_mask + boff * T : nullptr;
+        k.sa = make_sample_args(*sc, k.w.logits, k.B, c.vocab_size, use_cfg, c.dtype);
         SampleArgs& sa = k.sa;
-        sa.logits = k.w.logits; sa.B = k.B; sa.V = c.vocab_size; sa.mix_cfg = use_cfg;
-        sa.round_dtype = c.dtype;   // LG_DTYPE_F32 (0): no rounding
-        sa.cfg_scale = sc->cfg_scale; sa.cfg_interval = sc->cfg_interval; sa.temperature = sc->temperature;
-        sa.top_k = sc->top_k; sa.top_p = sc->top_p; sa.greedy = sc->greedy; sa.seed = sc->seed;
         sa.row_offset = (int)boff;
         sa.out_seq = out_tokens + boff * S; sa.seq_stride = S; sa.next_tokens = k.w.tokens;
         sa.teacher = teacher ? teacher + boff * S : nullptr;
@@ -755,11 +749,7 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
     const bool fuse_tail = lg_dtype_is16(c.dtype) && lg_env_flag("LG_FUSE_TAIL", 1) && c.dim % 2 == 0;
     auto arm_tail = [&](Chain& k, bool advance) {
         SampleArgs& sa = k.sa;
-        e->ws = k.w;
-        AttnArgs aa{};
-        aa.R = k.R; aa.Tq = 1; aa.H = c.n_head; aa.hd = e->hd; aa.hdp = e->hdp; aa.dtype = c.dtype;
-        if (k.w.have_maps) { aa.kmap = k.w.kmap; aa.vmap = k.w.vmap; aa.kmap16 = k.w.kmap16; aa.vmap16 = k.w.vmap16; }
-        const bool small = e->small_row_path(k.R, aa);
+        const bool small = e->small_row_path(k.R, e->attn_args(k.w, 0, k.R, 1));
         sa.emb_table = e->tok_emb; sa.emb_h = k.w.h; sa.emb_D = c.dim; sa.emb_rows = k.R;
         sa.emb_xn = small ? nullptr : k.w.xn;
         sa.emb_norm_w = e->layers[0].attn_norm; sa.emb_eps = c.norm_eps;
@@ -768,15 +758,12 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
         sa.adv_ticket = advance ? reinterpret_cast<unsigned int*>(k.w.counters + 64) : nullptr;
     };
     auto body = [&](Chain& k) -> int {
-        e->ws = k.w;
         int* d_pos = k.w.counters;
         int* d_step = k.w.counters + 1;
-        if (fuse_tail) {
-            e->skip_first_norm = k.sa.emb_xn != nullptr;     // the previous iteration's sample kernel left h (and xn) in place
-        } else {
-            LG_PROF(PC_EMBED_MISC, k.st, launch_embed(e->tok_emb, k.w.tokens, k.B, k.R, -1, c.dim, c.dtype, k.w.h, k.st));
-        }
-        LG_TRY(e->forward(k.R, 1, PosArg{d_pos, 0}, k.emb_mask, k.B, k.w.logits, false, k.st));
+        // with the fused tail the previous iteration's sample kernel left h (and xn) in place
+        if (!fuse_tail) LG_PROF(PC_EMBED_MISC, k.st, launch_embed(e->tok_emb, k.w.tokens, k.B, k.R, -1, c.dim, c.dtype, k.w.h, k.st));
+        const bool xn_ready = fuse_tail && k.sa.emb_xn != nullptr;
+        LG_TRY(e->forward(k.w, k.R, 1, PosArg{d_pos, 0}, k.emb_mask, k.B, k.w.logits, xn_ready, k.st));
         LG_PROF(PC_SAMPLE, k.st, launch_sample(k.sa, k.st));
         if (!fuse_tail) LG_PROF(PC_EMBED_MISC, k.st, launch_advance(d_pos, d_step, k.st));
         return 0;
@@ -785,9 +772,8 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
     // ---- prefill (generate.py:167-169) + first decode step, eagerly, per chain
     for (int g = 0; g < nchains; ++g) {
         Chain& k = ch[g];
-        e->ws = k.w;
-        LG_TRY(e->embed_cond(k.cond, k.B, k.R, T, k.st));
-        LG_TRY(e->forward(k.R * T, T, PosArg{nullptr, 0}, k.emb_mask, k.B, k.w.logits, false, k.st));
+        LG_TRY(e->embed_cond(k.w, k.cond, k.B, k.R, T, k.st));
+        LG_TRY(e->forward(k.w, k.R * T, T, PosArg{nullptr, 0}, k.emb_mask, k.B, k.w.logits, false, k.st));
         k.sa.step = 0; k.sa.step_dev = nullptr;
         const bool tail = S > 1 && fuse_tail;
         if (tail) arm_tail(k, false);            // the prefill's sample prepares the first decode step's rows; counters are set below
@@ -911,37 +897,19 @@ int lg_test_attention(int dtype, int kv_dtype, float k_scale, float v_scale, int
     LG_REQUIRE((q != nullptr) != (qkv_partial != nullptr), "lg_test_attention: pass exactly one of q and qkv_partial");
     LG_REQUIRE(q ? fuse == 0 : (ksplit > 0 && freqs && (fuse == 1 || (fuse == 0 && q_out))),
                "lg_test_attention: q takes fuse = 0; qkv_partial needs ksplit > 0, freqs and fuse = 1 or q_out");
-    const long long total_rows = (long long)n_layer * R * H * max_seq;
-    const size_t layer_bytes = (size_t)R * H * max_seq * hdp * (f8 ? 1 : lg_dtype_info(dtype).esz);
-    AttnArgs aa;
+    KvMaps maps;   // as the engine builds them: over every layer of the buffer
+    LG_TRY(make_kv_maps(maps, dtype, hd, hdp, f8 ? LG_DTYPE_E4M3 : dtype, kcache, vcache, (long long)n_layer * R * H * max_seq));
+    const float scales[2] = {k_scale, v_scale};
+    AttnArgs aa = make_attn_args(dtype, H, hd, hdp, R, max_seq, (char*)kcache, (char*)vcache, maps, f8 ? scales : nullptr, layer, R, Tq);
     aa.q = q ? q : q_out; aa.out = out;
-    aa.kcache = (char*)kcache + (size_t)layer * layer_bytes; aa.vcache = (char*)vcache + (size_t)layer * layer_bytes;
-    aa.R = R; aa.Tq = Tq; aa.H = H; aa.hd = hd; aa.maxS = max_seq; aa.hdp = hdp;
     aa.pos = PosArg{pos_dev, pos_value, pos_rows};
     aa.emb_mask = emb_mask; aa.B = emb_mask ? B : 1; aa.Tc = emb_mask ? Tc : 0;
-    aa.scale = 1.0f / sqrtf((float)hd); aa.dtype = dtype;
-    if (f8) { aa.kv_f8 = 1; aa.scale *= k_scale; aa.k_inv = 1.0f / k_scale; aa.v_inv = 1.0f / v_scale; aa.v_scale = v_scale; }
-    alignas(64) unsigned char maps[4][128];   // as lg_engine_set_workspace builds them: over every layer of the buffer
-    if (attn_tma_maps_usable(dtype, hd, hdp, total_rows)) {
-        const int kvdt = f8 ? LG_DTYPE_E4M3 : dtype;
-        LG_TRY(attn_tma_make_map(maps[0], kcache, total_rows, hdp, kvdt));
-        LG_TRY(attn_tma_make_map(maps[1], vcache, total_rows, hdp, kvdt));
-        LG_TRY(attn_tma_make_map(maps[2], kcache, total_rows, hdp, kvdt, 1));
-        LG_TRY(attn_tma_make_map(maps[3], vcache, total_rows, hdp, kvdt, 1));
-        aa.kmap = maps[0]; aa.vmap = maps[1]; aa.kmap16 = maps[2]; aa.vmap16 = maps[3];
-        aa.cache_row_base = (long long)layer * R * H * max_seq;
-    }
     if (qkv_partial) {
         if (fuse) {
             LG_REQUIRE(attn_tma_enabled() && attn_tma_supported(aa), "lg_test_attention: the fused QKV epilogue needs the TMA decode kernel");
             aa.qkv_partial = qkv_partial; aa.qkv_ksplit = ksplit; aa.freqs = freqs;
         } else {
-            QkvEpiArgs qa;
-            qa.partial = qkv_partial; qa.ksplit = ksplit; qa.M = R * Tq; qa.Tq = Tq; qa.D = H * hd; qa.H = H; qa.hd = hd;
-            qa.pos = aa.pos; qa.freqs = freqs; qa.q = q_out; qa.kcache = const_cast<void*>(aa.kcache); qa.vcache = const_cast<void*>(aa.vcache);
-            qa.maxS = max_seq; qa.dtype = dtype; qa.hdp = hdp;
-            qa.kv_f8 = aa.kv_f8; qa.k_inv = aa.k_inv; qa.v_inv = aa.v_inv;
-            LG_TRY(launch_qkv_epilogue(qa, st));
+            LG_TRY(launch_qkv_epilogue(make_qkv_epi_args(aa, qkv_partial, ksplit, freqs), st));
         }
     }
     return launch_attention(aa, st, path);

@@ -3,6 +3,8 @@ import ctypes
 import os
 import re
 
+import pytest
+
 from conftest import ROOT
 
 
@@ -42,6 +44,43 @@ def test_error_reporting_without_gpu():
     assert lib.lg_engine_create(ctypes.byref(cfg), 0, ctypes.byref(h)) == 0
     assert lib.lg_engine_finalize(h) < 0 and b"missing weight" in lib.lg_last_error()
     lib.lg_engine_destroy(h)
+
+
+_GPT_L = dict(n_layer=24, n_head=16, dim=1024, ffn_dim=2816, vocab_size=16384, cls_token_num=1, num_classes=1000, caption_dim=0)
+_TINY_T2I = dict(n_layer=2, n_head=4, dim=256, ffn_dim=704, vocab_size=1024, cls_token_num=8, num_classes=0, caption_dim=64)
+_TINY_HD100 = dict(n_layer=2, n_head=2, dim=200, ffn_dim=544, vocab_size=1024, cls_token_num=1, num_classes=10, caption_dim=0)
+
+
+@pytest.mark.parametrize("m, t2i, dtype, kv_fp8, sizes", [
+    (_GPT_L, False, "bf16", False, {(2, 17): 3632896, (128, 257): 3252356096}),
+    (_TINY_T2I, True, "bf16", False, {(2, 17): 316160, (128, 257): 83100672}),
+    (_GPT_L, False, "f16", False, {(2, 17): 3632896, (128, 257): 3252356096}),
+    (_GPT_L, False, "f32", False, {(2, 17): 7002880, (128, 257): 6487933952}),
+    (_TINY_HD100, False, "bf16", False, {(2, 17): 92672, (128, 257): 60867584}),     # 112-wide cache rows
+    (_GPT_L, False, "bf16", True, {(2, 17): 1961728, (128, 257): 1635451904}),
+], ids=["c2i_bf16_hd64", "t2i_bf16_caption", "c2i_f16", "c2i_f32", "c2i_bf16_hd100", "c2i_bf16_kv_fp8"])
+def test_workspace_bytes_are_pinned(m, t2i, dtype, kv_fp8, sizes, monkeypatch):
+    """The workspace layout (KV caches, activations, GEMM partials, logits, tokens, counters) is host arithmetic: its size, computed
+    without a GPU, must not move. The GEMM partials follow the default GEMM plan."""
+    from llamagen_b200 import _lib
+    monkeypatch.delenv("LG_GEMM_TC", raising=False)
+    lib = _lib.load()
+    dt = {"bf16": _lib.LG_DTYPE_BF16, "f16": _lib.LG_DTYPE_F16, "f32": _lib.LG_DTYPE_F32}[dtype]
+    cfg = _lib.ModelCfg(m["n_layer"], m["n_head"], m["dim"], m["ffn_dim"], m["vocab_size"], m["cls_token_num"], 256, m["num_classes"],
+                        m["caption_dim"], _lib.LG_MODEL_T2I if t2i else _lib.LG_MODEL_C2I, dt, 1e-5)
+    h = ctypes.c_void_p()
+    assert lib.lg_engine_create(ctypes.byref(cfg), 0, ctypes.byref(h)) == 0
+    try:
+        if kv_fp8:
+            assert lib.lg_engine_set_kv_cache(h, _lib.LG_DTYPE_E4M3, None) == 0, lib.lg_last_error()
+        got = {}
+        for rows, seq in sizes:
+            n = ctypes.c_size_t()
+            assert lib.lg_engine_workspace_bytes(h, rows, seq, ctypes.byref(n)) == 0, lib.lg_last_error()
+            got[(rows, seq)] = n.value
+        assert got == sizes
+    finally:
+        lib.lg_engine_destroy(h)
 
 
 def test_product_never_imports_oracle():

@@ -188,22 +188,21 @@ def test_attention_kernels_agree_large_batch_t2i(monkeypatch):
 
 
 def test_multi_chain_decode_is_bit_identical(monkeypatch):
-    """Large batches are decoded as LG_SPLIT (default 2, max 4) independent sub-batch chains on their own streams and
-    CUDA graphs. Every image's arithmetic is unchanged, so tokens AND logits must equal the single-chain run bit for bit."""
+    """Large batches can be decoded as two independent half-batch chains (LG_SPLIT=2) on their own streams and CUDA graphs.
+    Every image's arithmetic is unchanged, so tokens, logits AND sampled streams must equal the single-chain run bit for bit."""
     g = load_golden("gpt_c2i.pt")
     B, S = 48, 10
     cond = torch.randint(0, 10, (B,), generator=torch.Generator().manual_seed(3))
     outs = {}
-    for split in ("1", "2", "4"):
+    for split in ("1", "2"):
         monkeypatch.setenv("LG_SPLIT", split)
         m = build_gpt(g["cfg"], g["state_dict"], torch.bfloat16)
         toks, logits = _gen(m, cond, S, None, cfg_scale=4.0)
         from llamagen_b200 import generate
         sampled = generate(m, cond.cuda(), S, cfg_scale=4.0, temperature=1.0, top_k=50, top_p=1.0, sample_logits=True, seed=5).cpu()
         outs[split] = (toks, logits, sampled)
-    for split in ("2", "4"):
-        for i in range(3):
-            assert torch.equal(outs[split][i], outs["1"][i]), (split, i)
+    for i in range(3):
+        assert torch.equal(outs["2"][i], outs["1"][i]), i
 
 
 @pytest.mark.parametrize("B", [1, 3, 4])

@@ -10,7 +10,7 @@ Bound (same protocol as tests/test_gpt_gpu.py::_bf16_parity): the engine may dev
 must agree wherever the fp32 oracle's top-1/top-2 gap exceeds twice that bound. The MEASURED errors are printed next to
 the bounds (pytest -s) and appended to gpurun_out/parity_report.jsonl so a regression inside the slack stays visible.
 
-    C2  GPT-L  c2i 16x16, B=64 (R=128, two decode chains), all 256 tokens      <- the benchmarked configuration
+    C2  GPT-L  c2i 16x16, B=64 (R=128, one decode chain), all 256 tokens       <- the benchmarked configuration
     C2' GPT-L  c2i 16x16, B=32 (R=64), all 256 tokens                          <- north_star's per-GPU point (B=256 / 8 GPUs)
     C3  GPT-XL c2i 24x24, contexts to 577 keys, R=4 (small-row path) and R=16 (wgmma path)
     C5  GPT-XL t2i 32x32, T=120 prefill with ragged emb_masks + 1024 tokens (context 1144), R=4 and R=16
@@ -95,8 +95,9 @@ def parity_on_device(tag, m, cond, S, emb_masks=None, cfg_scale=4.0):
 
 @pytest.mark.parametrize("B", [64, 32])
 def test_c2_gpt_l_bench_config_full_sequence(B):
-    """BASELINE configs[1]: GPT-L c2i 16x16, cfg 4.0. B=64 is the benchmarked batch (R=128 rows, two 64-row decode chains,
-    contexts to 257 keys on attn_tma_kernel); B=32 is the per-GPU batch of north_star's B=256-over-8-GPUs point."""
+    """BASELINE configs[1]: GPT-L c2i 16x16, cfg 4.0. B=64 is the benchmarked batch (R=128 rows in one decode chain: a
+    27 MB GPT-L layer is more than a third of the H100's 50 MB L2; contexts to 257 keys on attn_tma_kernel); B=32 is the
+    per-GPU batch of north_star's B=256-over-8-GPUs point."""
     m = _registry("GPT-L", 1, block_size=256, vocab_size=16384)
     torch.manual_seed(B)
     parity_on_device(f"C2 GPT-L c2i S=256 B={B}", m, torch.randint(0, 1000, (B,)), 256)
