@@ -385,13 +385,38 @@ int conv_tc_make_phase_weights(const float* w_f32, bf16* out, int cout, int cin,
 static int g_conv_cta_budget = 0;
 void conv_tc_set_cta_budget(int ctas) { g_conv_cta_budget = ctas; }
 
-bool conv_tc_supported(int Hin, int Win, int Cin, int Cout, int ksize, int up, bool nchw_out) {
-    if (Cin % 64 != 0) return false;
-    if (Win < 8 || Hin < 8) return false;
-    if (!nchw_out && Cout % 16 != 0) return false;
-    if (up && ksize != 3) return false;
-    if (up == 2 && (Hin % 2 || Win % 2 || Win < 16 || Hin < 16)) return false;
-    return ksize == 1 || ksize == 3;
+// ConvTcArgs shared by both kernels before the patch, Cout tile, tile grid and statistics are chosen
+static ConvTcArgs conv_tc_args(const ConvCall& c) {
+    ConvTcArgs a{};
+    a.B = c.B; a.Hin = c.Hin; a.Win = c.Win; a.Cin = c.cin; a.Cout = c.cout;
+    a.Hout = conv_out_extent(c.Hin, c.up); a.Wout = conv_out_extent(c.Win, c.up);
+    a.mode = c.up == 1 ? 2 : (c.up == 2 ? 3 : (c.k == 1 ? 1 : 0));
+    a.ntaps = c.up == 1 ? 4 : c.k * c.k;
+    a.Ht = c.up == 2 ? a.Hout : c.Hin; a.Wt = c.up == 2 ? a.Wout : c.Win;
+    a.kchunks = c.cin / kCk;
+    a.bias = c.bias; a.residual = c.residual; a.out_bf = c.out_bf; a.out_nchw = c.out_nchw; a.out_u8 = c.out_u8;
+    a.gz = c.up == 1 ? 4 : 1;
+    return a;
+}
+
+ConvPlan conv_plan(const ConvCall& c) {
+    ConvPlan p;
+    const bool pixels_out = c.out_nchw || c.out_u8;          // conv_out: any Cout
+    const bool tc = c.cin % kCk == 0 && c.Hin >= 8 && c.Win >= 8 && (pixels_out || c.cout % 16 == 0) &&
+                    (c.k == 3 || (c.k == 1 && c.up == 0)) && (c.up != 1 || conv_has_phase_weights(c.up, c.cin)) &&
+                    (c.up != 2 || (c.Hin % 2 == 0 && c.Win % 2 == 0 && c.Hin >= 16 && c.Win >= 16));
+    if (!lg_env_flag("LG_CONV_TC", 1) || !tc) return p;
+    p.kernel = 1;
+    // the weights-as-A kernel drains through its stage memory, which needs every stage held by the tile (>= kWStages k-blocks)
+    const ConvTcArgs a = conv_tc_args(c);
+    if (c.cout % 128 != 0 || a.Ht < 16 || a.Wt < 16 || !c.out_bf || a.ntaps * a.kchunks < kWStages || !lg_env_flag("LG_CONV_SWAP", 1))
+        return p;
+    p.kernel = 2;
+    // GroupNorm(32) statistics of the output in the drain: every (image, tile, group) slot is written by exactly one CTA
+    const int splits = cdiv(a.Wt, 16) * cdiv(a.Ht, 16) * a.gz;
+    if (c.gn_partial && 128 % (c.cout / 32) == 0 && (size_t)c.B * splits * 32 * 2 <= c.gn_floats && lg_env_flag("LG_GN_FUSE", 1))
+        p.gn_splits = splits;
+    return p;
 }
 
 template <int BN>
@@ -409,75 +434,46 @@ static int launch_conv_tc_t(const CUtensorMap& amap, const CUtensorMap& wmap, co
     return 0;
 }
 
-// weights: up == 0 or 2 (stride-2 Downsample) -> [Cout][k*k][Cin] bf16 ; up == 1 -> phase weights [4][Cout][4][Cin] bf16
-int launch_conv_tc(const bf16* in, int B, int Hin, int Win, int Cin, const bf16* weights, const float* bias, int Cout,
-                   int ksize, int up, const bf16* residual, bf16* out_bf, float* out_nchw, cudaStream_t st, uint8_t* out_u8,
-                   float* gn_partial, size_t gn_floats, int* gn_splits, int* path) {
-    if (gn_splits) *gn_splits = 0;
-    if (path) *path = 1;
-    ConvTcArgs a;
-    a.gn_partial = nullptr; a.gn_cpg = 0; a.gn_splits = 0;
-    a.B = B; a.Hin = Hin; a.Win = Win; a.Cin = Cin; a.Cout = Cout;
-    const bool down = up == 2;
-    up = up == 1;
-    a.Hout = up ? 2 * Hin : (down ? Hin / 2 : Hin); a.Wout = up ? 2 * Win : (down ? Win / 2 : Win);
-    a.mode = up ? 2 : (down ? 3 : (ksize == 1 ? 1 : 0));
-    a.ntaps = up ? 4 : ksize * ksize;
-    a.Ht = down ? a.Hout : Hin; a.Wt = down ? a.Wout : Win;
+static int launch_conv_tcw(const CUtensorMap& amap, const CUtensorMap& wmap, const ConvTcArgs& a, dim3 grid, cudaStream_t st) {
+    const size_t smem = 1024 + (size_t)kWStages * kWStage + 2 * kWStages * sizeof(uint64_t) + 128 * sizeof(float);
+    static DevOnce attr;
+    if (lg_first_on_device(attr)) {
+        LG_CUDA_OK(cudaFuncSetAttribute(conv_tcw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024));
+    }
+    LG_REQUIRE(smem <= 110 * 1024, "conv_tcw: shared memory %zu too large", smem);
+    conv_tcw_kernel<<<grid, kConvThreads, smem, st>>>(amap, wmap, a);
+    LG_LAUNCH_CHECK();
+    return 0;
+}
+
+int launch_conv_tc(const ConvCall& c, const ConvPlan& p, cudaStream_t st) {
+    LG_REQUIRE(c.up != 1 || c.w_phase, "conv_tc: upsample conv without phase weights");
+    const bool tcw = p.kernel == 2;
+    ConvTcArgs a = conv_tc_args(c);
+    // conv_tc_kernel: an 8x16 (8-wide when Wt < 16) patch x a Cout tile of up to 128; conv_tcw_kernel (Wt >= 16, Cout % 128 == 0):
+    // 128 couts x a 16x16 patch, two 8x16 boxes of the same tensor map
     a.bw = a.Wt >= 16 ? 16 : 8;
     a.bh = kPix / a.bw;
-    a.tiles_x = cdiv(a.Wt, a.bw);
-    a.tiles_y = cdiv(a.Ht, a.bh);
     a.bn = 16;
-    while (a.bn < 128 && a.bn < Cout) a.bn *= 2;
-    a.kchunks = Cin / kCk;
-    a.bias = bias; a.residual = residual; a.out_bf = out_bf; a.out_nchw = out_nchw; a.out_u8 = out_u8;
+    while (a.bn < 128 && a.bn < c.cout) a.bn *= 2;
+    a.tiles_x = cdiv(a.Wt, a.bw);
+    a.tiles_y = cdiv(a.Ht, tcw ? 16 : a.bh);
+    a.gx = c.B * a.tiles_x * a.tiles_y; a.gy = cdiv(c.cout, a.bn);
+    if (p.gn_splits > 0) { a.gn_partial = c.gn_partial; a.gn_cpg = c.cout / 32; a.gn_splits = p.gn_splits; }
 
     CUtensorMap amap, wmap;
-    LG_TRY(tma::make_map_nhwc(&amap, in, (uint64_t)B, (uint64_t)Hin, (uint64_t)Win, (uint64_t)Cin, (uint32_t)a.bh, (uint32_t)a.bw, kCk,
-                              down ? 2u : 1u));
-    const uint64_t wrows = (uint64_t)(up ? 4 : 1) * Cout, wcols = (uint64_t)a.ntaps * Cin;
-    LG_TRY(tma::make_map_2d(&wmap, weights, wrows, wcols, wcols, (uint32_t)a.bn, kCk));
+    LG_TRY(tma::make_map_nhwc(&amap, c.in, (uint64_t)c.B, (uint64_t)c.Hin, (uint64_t)c.Win, (uint64_t)c.cin, (uint32_t)a.bh, (uint32_t)a.bw,
+                              kCk, c.up == 2 ? 2u : 1u));
+    // weights: [Cout][k*k][Cin], or for the upsample the phase weights [4][Cout][4][Cin]
+    const uint64_t wrows = (uint64_t)a.gz * c.cout, wcols = (uint64_t)a.ntaps * c.cin;
+    LG_TRY(tma::make_map_2d(&wmap, c.up == 1 ? c.w_phase : c.w, wrows, wcols, wcols, (uint32_t)a.bn, kCk));
 
-    // CTA budget: 0 = one CTA per tile; > 0 = persistent CTAs (lg_vq_set_cta_budget), e.g. 64 while the next batch samples
-    const int budget = g_conv_cta_budget;
-    // the weights-as-A kernel drains through its stage memory, which needs every stage held by the tile (>= kWStages k-blocks)
-    if (Cout % 128 == 0 && a.Ht >= 16 && a.Wt >= 16 && out_bf && !out_nchw && !out_u8 && a.ntaps * a.kchunks >= kWStages &&
-        lg_env_flag("LG_CONV_SWAP", 1)) {
-        // weights-as-A kernel: 128 couts x a 16x16-pixel patch (two 8x16 boxes) per tile
-        ConvTcArgs w = a;
-        w.bw = 16; w.bh = 8;
-        w.tiles_x = cdiv(a.Wt, 16); w.tiles_y = cdiv(a.Ht, 16);
-        w.bn = 128;
-        w.gx = B * w.tiles_x * w.tiles_y; w.gy = Cout / 128; w.gz = up ? 4 : 1;
-        // GroupNorm(32) statistics of the output in the drain: every (image, tile, group) slot is written by exactly one CTA
-        const int splits = w.tiles_x * w.tiles_y * w.gz, cpg = Cout / 32;
-        if (gn_partial && gn_splits && Cout % 32 == 0 && 128 % cpg == 0 && (size_t)B * splits * 64 <= gn_floats && lg_env_flag("LG_GN_FUSE", 1)) {
-            w.gn_partial = gn_partial; w.gn_cpg = cpg; w.gn_splits = splits;
-            *gn_splits = splits;
-        }
-        CUtensorMap amap2, wmap2;
-        LG_TRY(tma::make_map_nhwc(&amap2, in, (uint64_t)B, (uint64_t)Hin, (uint64_t)Win, (uint64_t)Cin, 8u, 16u, kCk, down ? 2u : 1u));
-        const uint64_t wrows2 = (uint64_t)(up ? 4 : 1) * Cout, wcols2 = (uint64_t)a.ntaps * Cin;
-        LG_TRY(tma::make_map_2d(&wmap2, weights, wrows2, wcols2, wcols2, 128u, kCk));
-        const size_t smem2 = 1024 + (size_t)kWStages * kWStage + 2 * kWStages * sizeof(uint64_t) + 128 * sizeof(float);
-        static DevOnce attr2;
-        if (lg_first_on_device(attr2)) {
-            LG_CUDA_OK(cudaFuncSetAttribute(conv_tcw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024));
-        }
-        LG_REQUIRE(smem2 <= 110 * 1024, "conv_tcw: shared memory %zu too large", smem2);
-        const long long total2 = (long long)w.gx * w.gy * w.gz;
-        LG_REQUIRE(total2 < (1ll << 31), "conv_tcw: too many tiles");
-        dim3 grid2((unsigned)(budget > 0 ? std::min<long long>(total2, budget) : total2));
-        conv_tcw_kernel<<<grid2, kConvThreads, smem2, st>>>(amap2, wmap2, w);
-        LG_LAUNCH_CHECK();
-        if (path) *path = 2;
-        return 0;
-    }
-    a.gx = B * a.tiles_x * a.tiles_y; a.gy = cdiv(Cout, a.bn); a.gz = up ? 4 : 1;
     const long long total = (long long)a.gx * a.gy * a.gz;
     LG_REQUIRE(total < (1ll << 31), "conv_tc: too many tiles");
-    dim3 grid((unsigned)(budget > 0 ? std::min<long long>(total, budget) : total));
+    // CTA budget: 0 = one CTA per tile; > 0 = persistent CTAs (lg_vq_set_cta_budget), e.g. 64 while the next batch samples
+    const int budget = g_conv_cta_budget;
+    const dim3 grid((unsigned)(budget > 0 ? std::min<long long>(total, budget) : total));
+    if (tcw) return launch_conv_tcw(amap, wmap, a, grid, st);
     switch (a.bn) {
         case 16: return launch_conv_tc_t<16>(amap, wmap, a, grid, st);
         case 32: return launch_conv_tc_t<32>(amap, wmap, a, grid, st);

@@ -1,6 +1,7 @@
 // Internal launch API shared by the translation units of libllamagen_b200.so.
 #pragma once
 #include "common.cuh"
+#include <algorithm>
 
 // ------------------------------------------------------------------------------------------------
 // sampling.cu
@@ -160,15 +161,40 @@ int launch_attention_tma(const AttnArgs& a, cudaStream_t st, int* path = nullptr
 // t2i condition prefill (1 < Tq <= 128, hd 64, bf16 / fp16): TMA-staged Q/K/V, mma.sync QK^T and PV, one CTA per (row, head)
 bool attn_prefill_tc_supported(const AttnArgs& a);
 int launch_attention_prefill_tc(const AttnArgs& a, cudaStream_t st, int* path = nullptr);
-// conv_tc.cu — wgmma implicit-GEMM convolution over bf16 NHWC activations (TMA 4-D boxes, register accumulators)
-bool conv_tc_supported(int Hin, int Win, int Cin, int Cout, int ksize, int up, bool nchw_out);
+// VQ convolutions: vq.cu runs them; conv_tc.cu holds the wgmma kernels and chooses the kernel of each call.
+// GroupNorm(32) partial statistics are [B][splits][32 groups][sum, sum of squares] floats. gn_stats_kernel writes at most
+// kGnStatsMaxSplits splits per image; the drain of conv_tcw_kernel writes one per 16x16-pixel tile (and upsample phase) of its input.
+constexpr int kGnStatsMaxSplits = 64;
+// partials capacity that serves every GroupNorm of B images whose convolutions read inputs of at most H x W pixels
+inline size_t gn_partial_capacity(int B, int H, int W) {
+    return (size_t)B * std::max(kGnStatsMaxSplits, cdiv(H, 16) * cdiv(W, 16) * 4) * 32 * 2;
+}
+// up: 0 = same resolution, 1 = nearest-2x upsample folded in, 2 = Downsample (pad right/bottom, stride 2)
+inline int conv_out_extent(int n, int up) { return up == 1 ? 2 * n : (up == 2 ? n / 2 : n); }
+// an upsample conv has pre-summed 2x2 phase weights (conv_tc_make_phase_weights), which the wgmma path needs, exactly when this holds
+inline bool conv_has_phase_weights(int up, int cin) { return up == 1 && cin % 64 == 0; }
+// One convolution: bf16 NHWC input, weights repacked to bf16 [cout][k*k][cin], exactly one output
+struct ConvCall {
+    const bf16* in = nullptr;        // [B][Hin][Win][cin]
+    int B = 0, Hin = 0, Win = 0, cin = 0, cout = 0, k = 0;
+    int up = 0;
+    const bf16* w = nullptr;
+    const bf16* w_phase = nullptr;   // [4 phases][cout][4 taps][cin] when conv_has_phase_weights(up, cin)
+    const float* bias = nullptr;
+    const bf16* residual = nullptr;  // bf16 NHWC like the output, may alias out_bf
+    bf16* out_bf = nullptr;          // bf16 NHWC
+    float* out_nchw = nullptr;       // fp32 NCHW
+    uint8_t* out_u8 = nullptr;       // clamp(127.5 y + 128, 0, 255) as uint8 NHWC
+    float* gn_partial = nullptr;     // non-null: the drain may write the output's GroupNorm partials here (gn_floats capacity)
+    size_t gn_floats = 0;
+};
+// The kernel a call runs on: 0 = mma.sync gather (vq.cu), 1 = conv_tc_kernel, 2 = conv_tcw_kernel; gn_splits > 0: its drain writes
+// that many splits of the output's GroupNorm partials into gn_partial. The only reader of LG_CONV_TC, LG_CONV_SWAP and LG_GN_FUSE.
+struct ConvPlan { int kernel = 0; int gn_splits = 0; };
+ConvPlan conv_plan(const ConvCall& c);
+int launch_conv_tc(const ConvCall& c, const ConvPlan& p, cudaStream_t st);   // p.kernel 1 or 2
 void conv_tc_set_cta_budget(int ctas);   // > 0: persistent conv CTAs (at most `ctas`), 0: one CTA per tile (default)
 int conv_tc_make_phase_weights(const float* w_f32, bf16* out, int cout, int cin, cudaStream_t st);
-int launch_conv_tc(const bf16* in, int B, int Hin, int Win, int Cin, const bf16* weights, const float* bias, int Cout,
-                   int ksize, int up, const bf16* residual, bf16* out_bf, float* out_nchw, cudaStream_t st, uint8_t* out_u8 = nullptr,
-                   float* gn_partial = nullptr, size_t gn_floats = 0, int* gn_splits = nullptr,    // *gn_splits > 0: the drain also wrote the
-                   int* path = nullptr);   // output's GroupNorm(32) partial statistics [B][*gn_splits][32][2] into gn_partial;
-                                           // *path: 1 = conv_tc_kernel, 2 = conv_tcw_kernel was launched
 // gemm_tc.cu — wgmma/TMA weight-streaming GEMM (bf16 or fp16, row blocks of <= 256)
 int gemm_tc_ksplit(int M, int N, int K);
 bool gemm_tc_supported(int M, int N, int K, int dtype);

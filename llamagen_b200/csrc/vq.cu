@@ -76,10 +76,6 @@ __global__ void repack_conv_kernel(const float* __restrict__ src, bf16* __restri
     }
 }
 
-__global__ void copy_f32_kernel(const float* __restrict__ src, float* __restrict__ dst, size_t n) {
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) dst[i] = src[i];
-}
-
 // F.normalize(e, p=2, dim=-1) (vq_model.py:264): e / max(||e||, 1e-12); also the row's squared norm.
 __global__ void normalize_codebook_kernel(const float* __restrict__ e, float* __restrict__ out, float* __restrict__ sq,
                                           int n, int d, int l2) {
@@ -87,11 +83,9 @@ __global__ void normalize_codebook_kernel(const float* __restrict__ e, float* __
     if (i >= n) return;
     float ss = 0.f;
     for (int j = 0; j < d; ++j) ss += e[(size_t)i * d + j] * e[(size_t)i * d + j];
-    const float inv = l2 ? 1.0f / fmaxf(sqrtf(ss), 1e-12f) : 1.0f;
     float s2 = 0.f;
     for (int j = 0; j < d; ++j) {
         const float v = l2 ? e[(size_t)i * d + j] / fmaxf(sqrtf(ss), 1e-12f) : e[(size_t)i * d + j];
-        (void)inv;
         out[(size_t)i * d + j] = v;
         s2 += v * v;
     }
@@ -504,7 +498,11 @@ struct ConvW { bf16* w = nullptr; bf16* w_phase = nullptr; const float* bias = n
 struct NormW { const float* gamma = nullptr; const float* beta = nullptr; int c = 0; };
 struct ResW { NormW n1, n2; ConvW c1, c2, nin; bool has_nin = false; int cin = 0, cout = 0; };
 struct AttnW { NormW norm; ConvW qk, v, proj; float* qk_bias = nullptr; int c = 0; };
-struct LevelW { std::vector<ResW> res; std::vector<AttnW> attn; bool up = false; ConvW upconv; };   // upconv: up- or downsample conv
+// resampling: the level ends in the decoder's Upsample or the encoder's Downsample conv
+struct LevelW { std::vector<ResW> res; std::vector<AttnW> attn; bool resampling = false; ConvW resample; };
+struct MidW { ResW res0; AttnW attn; ResW res1; };
+// Decoder or Encoder (vq_model.py:64-194) less what the two do not share: levels in execution order, mid, norm_out, conv_out
+struct TowerW { std::vector<LevelW> levels; MidW mid; NormW norm_out; ConvW conv_out; };
 
 }  // namespace
 
@@ -514,24 +512,18 @@ struct lg_vq {
     std::unordered_map<std::string, HostTensor> t;
     std::vector<void*> owned;   // cudaMalloc'ed repacked weights
     bool finalized = false;
-    ConvW conv_in, conv_out;
-    ResW mid0, mid2;
-    AttnW mid1;
-    std::vector<LevelW> levels;
-    NormW norm_out;
+    TowerW dec;
+    ConvW conv_in;              // decoder.conv_in
     float* codebook = nullptr;  // normalised [n_e, e_dim]
     float* codebook_sq = nullptr;
     const float* pq_w = nullptr;
     const float* pq_b = nullptr;
     // encoder (optional: built when encoder.* and quant_conv.* are bound)
     bool has_encoder = false;
+    TowerW enc;
     const float* enc_in_w = nullptr;   // fp32 [ch,3,3,3], applied in fp32 by conv_in_rgb_kernel
     const float* enc_in_b = nullptr;
-    std::vector<LevelW> enc_levels;
-    ResW enc_mid0, enc_mid2;
-    AttnW enc_mid1;
-    NormW enc_norm_out;
-    ConvW enc_conv_out, quant_conv;
+    ConvW quant_conv;
 
     ~lg_vq() { for (void* p : owned) cudaFree(p); }
 };
@@ -607,11 +599,36 @@ int make_attn(lg_vq* v, const std::string& p, int c, AttnW* a, cudaStream_t st) 
     LG_CUDA_OK(cudaMemcpyAsync(qk, q.w, (size_t)c * c * sizeof(bf16), cudaMemcpyDeviceToDevice, st));
     LG_CUDA_OK(cudaMemcpyAsync(qk + (size_t)c * c, k.w, (size_t)c * c * sizeof(bf16), cudaMemcpyDeviceToDevice, st));
     LG_TRY(dev_alloc(v, (size_t)2 * c, &a->qk_bias));
-    copy_f32_kernel<<<1, 256, 0, st>>>(q.bias, a->qk_bias, c);
-    LG_LAUNCH_CHECK();
-    copy_f32_kernel<<<1, 256, 0, st>>>(k.bias, a->qk_bias + c, c);
-    LG_LAUNCH_CHECK();
+    LG_CUDA_OK(cudaMemcpyAsync(a->qk_bias, q.bias, (size_t)c * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    LG_CUDA_OK(cudaMemcpyAsync(a->qk_bias + c, k.bias, (size_t)c * sizeof(float), cudaMemcpyDeviceToDevice, st));
     a->qk.w = qk; a->qk.bias = a->qk_bias; a->qk.cout = 2 * c; a->qk.cin = c; a->qk.k = 1;
+    return 0;
+}
+
+int make_mid(lg_vq* v, const std::string& p, int c, MidW* m, cudaStream_t st) {
+    LG_TRY(make_res(v, p + ".0", c, c, &m->res0, st));
+    LG_TRY(make_attn(v, p + ".1", c, &m->attn, st));
+    return make_res(v, p + ".2", c, c, &m->res1, st);
+}
+
+// Appends a level to t: nres ResnetBlocks cin -> cout, each followed by an AttnBlock when `attn`, then the resampling conv when
+// up != 0 (up: the run_conv mode, 1 = Upsample, 2 = Downsample)
+int make_level(lg_vq* v, const std::string& p, int nres, int cin, int cout, bool attn, int up, TowerW* t, cudaStream_t st) {
+    LevelW* lv = &t->levels.emplace_back();
+    for (int j = 0; j < nres; ++j) {
+        LG_TRY(make_res(v, p + ".res." + std::to_string(j), j == 0 ? cin : cout, cout, &lv->res.emplace_back(), st));
+        if (attn) LG_TRY(make_attn(v, p + ".attn." + std::to_string(j), cout, &lv->attn.emplace_back(), st));
+    }
+    lv->resampling = up != 0;
+    if (!lv->resampling) return 0;
+    const std::string name = p + (up == 1 ? ".upsample.conv" : ".downsample.conv");
+    LG_TRY(make_conv(v, name, cout, cout, 3, &lv->resample, st));
+    if (conv_has_phase_weights(up, cout)) {
+        const float* wf = nullptr;
+        LG_TRY(get(v, name + ".weight", {cout, cout, 3, 3}, &wf));
+        LG_TRY(dev_alloc(v, (size_t)16 * cout * cout, &lv->resample.w_phase));
+        LG_TRY(conv_tc_make_phase_weights(wf, lv->resample.w_phase, cout, cout, st));
+    }
     return 0;
 }
 
@@ -622,10 +639,8 @@ struct VqWs {
     size_t bytes;
     int attn_bc;   // images per attention chunk
     size_t gn_floats = 0;            // capacity of gn
-    // GroupNorm statistics produced by the drain of the conv that wrote `gn_src` (conv_tcw_kernel): run_gn skips its statistics pass
-    // when it is asked to normalise exactly that tensor
-    const bf16* gn_src = nullptr;
-    int gn_splits = 0;
+    // c with its drain asked for the GroupNorm partials of its output (into gn)
+    ConvCall stats(ConvCall c) const { c.gn_partial = gn; c.gn_floats = gn_floats; return c; }
 };
 
 size_t a256(size_t v) { return (v + 255) / 256 * 256; }
@@ -654,14 +669,9 @@ VqWs carve_vq(const lg_vq* v, char* base, int Bc, int g) {
     w.VT = (bf16*)take((size_t)Bc * N * Cd * 2);
     w.S = (float*)take((size_t)abc * N * N * 4);
     w.P = (bf16*)take((size_t)abc * N * N * 2);
-    // statistics partials: gn_stats_kernel uses <= 64 splits per image, the conv drains one per 16x16-pixel tile of the largest output
-    {
-        int rmax = g;
-        for (int i = 0; i + 1 < c.n_mult; ++i) rmax *= 2;
-        const size_t splits = std::max<size_t>(64, (size_t)((rmax + 15) / 16) * ((rmax + 15) / 16) * 4);
-        w.gn_floats = (size_t)Bc * splits * 32 * 2;
-        w.gn = (float*)take(w.gn_floats * 4);
-    }
+    const int rmax = g << (c.n_mult - 1);                             // largest resolution: pixels of the decoded image
+    w.gn_floats = gn_partial_capacity(Bc, rmax, rmax);
+    w.gn = (float*)take(w.gn_floats * 4);
     w.Z = (float*)take((size_t)Bc * N * c.codebook_embed_dim * 4);   // encoder output z (fp32 NCHW) ahead of the argmin
     w.bytes = off;
     w.attn_bc = abc;
@@ -677,45 +687,49 @@ int chunk_images(const lg_vq* v, int B, int g) {
 }
 
 // ---- layer launchers --------------------------------------------------------------------------------
-// up: 0 = same resolution, 1 = nearest-2x upsample folded in, 2 = Downsample (pad right/bottom, stride 2)
-// *path (optional): 0 = mma.sync gather kernel, 1 = conv_tc_kernel, 2 = conv_tcw_kernel
-int run_conv(const ConvW& cw, const bf16* in, int B, int Hin, int Win, int up, const bf16* residual, bf16* out_bf,
-             float* out_nchw, cudaStream_t st, uint8_t* out_u8 = nullptr, VqWs* ws = nullptr, int* path = nullptr) {
-    if (ws && out_bf && ws->gn_src == out_bf) ws->gn_src = nullptr;          // the tensor the statistics described is being overwritten
-    if (lg_env_flag("LG_CONV_TC", 1) && conv_tc_supported(Hin, Win, cw.cin, cw.cout, cw.k, up, out_nchw != nullptr || out_u8 != nullptr) &&
-        (up != 1 || cw.w_phase)) {
-        int splits = 0;
-        LG_PROF(PC_VQ_CONV, st, launch_conv_tc(in, B, Hin, Win, cw.cin, up == 1 ? cw.w_phase : cw.w, cw.bias, cw.cout, cw.k, up, residual,
-                                               out_bf, out_nchw, st, out_u8, ws ? ws->gn : nullptr, ws ? ws->gn_floats : 0, ws ? &splits : nullptr,
-                                               path));
-        if (ws && splits > 0) { ws->gn_src = out_bf; ws->gn_splits = splits; }
-        return 0;
+// GroupNorm statistics pass from layer to layer as a count: run_conv returns how many partial-statistics splits its drain wrote
+// (0: none), run_gn takes that count for its input, and the block runners take the count of w.X on entry and return the count
+// for w.X on exit (or a negative error).
+
+// conv cw over `in` (B x H x W) into the bf16 tensor `out` (+ residual), without statistics
+ConvCall conv_call(const ConvW& cw, const bf16* in, int B, int H, int W, bf16* out, const bf16* residual = nullptr) {
+    ConvCall c;
+    c.in = in; c.B = B; c.Hin = H; c.Win = W; c.cin = cw.cin; c.cout = cw.cout; c.k = cw.k;
+    c.w = cw.w; c.w_phase = cw.w_phase; c.bias = cw.bias; c.residual = residual; c.out_bf = out;
+    return c;
+}
+
+// Runs c on the kernel conv_plan picks (*path, optional) and returns the splits its drain wrote into c.gn_partial.
+int run_conv(const ConvCall& c, cudaStream_t st, int* path = nullptr) {
+    const ConvPlan p = conv_plan(c);
+    if (path) *path = p.kernel;
+    if (p.kernel != 0) {
+        LG_PROF(PC_VQ_CONV, st, launch_conv_tc(c, p, st));
+        return p.gn_splits;
     }
-    LG_REQUIRE(!out_u8, "uint8 output needs the wgmma conv path (Cin %% 64 == 0, LG_CONV_TC=1)");
-    if (path) *path = 0;
-    const int Hout = up == 1 ? 2 * Hin : (up == 2 ? Hin / 2 : Hin), Wout = up == 1 ? 2 * Win : (up == 2 ? Win / 2 : Win);
-    const int M = B * Hout * Wout, K = cw.k * cw.k * cw.cin;
-    mma::ConvA al{in, Hin, Win, cw.cin, Hout, Wout, cw.k, up, M};
-    mma::BRows bw{cw.w, cw.w, cw.cout, K, 0, cw.cout};
+    LG_REQUIRE(!c.out_u8, "uint8 output needs the wgmma conv path (Cin %% 64 == 0, LG_CONV_TC=1)");
+    const int Hout = conv_out_extent(c.Hin, c.up), Wout = conv_out_extent(c.Win, c.up);
+    const int M = c.B * Hout * Wout, K = c.k * c.k * c.cin;
+    mma::ConvA al{c.in, c.Hin, c.Win, c.cin, Hout, Wout, c.k, c.up, M};
+    mma::BRows bw{c.w, c.w, c.cout, K, 0, c.cout};
     EpiVq e{};
-    e.bias = cw.bias; e.residual = residual; e.ldr = cw.cout; e.out_bf = out_bf; e.ldo = cw.cout; e.scale = 1.f;
-    e.N = cw.cout;
-    if (out_nchw) { e.out_f32 = out_nchw; e.nchw = 1; e.hw = Hout * Wout; e.out_bf = nullptr; }
-    LG_PROF(PC_VQ_CONV, st, launch_vq_gemm(al, bw, M, cw.cout, K, 1, e, st));
+    e.bias = c.bias; e.residual = c.residual; e.ldr = c.cout; e.out_bf = c.out_bf; e.ldo = c.cout; e.scale = 1.f;
+    e.N = c.cout;
+    if (c.out_nchw) { e.out_f32 = c.out_nchw; e.nchw = 1; e.hw = Hout * Wout; e.out_bf = nullptr; }
+    LG_PROF(PC_VQ_CONV, st, launch_vq_gemm(al, bw, M, c.cout, K, 1, e, st));
     return 0;
 }
 
-int run_gn(const NormW& nw, const bf16* x, bf16* y, int B, int HW, int swish, float* gnbuf, cudaStream_t st, VqWs* ws = nullptr) {
-    int splits = (int)std::min<long long>(64, std::max<long long>(1, (long long)HW * nw.c / 8 / 2048));
-    if (ws && ws->gn_src == x && ws->gn_splits > 0) {
-        splits = ws->gn_splits;                  // the producing conv's drain already wrote the partial statistics of x
-    } else {
+// x_splits: the partials of x a conv's drain left in gnbuf; with none, the statistics pass writes them there first
+int run_gn(const NormW& nw, const bf16* x, int x_splits, bf16* y, int B, int HW, int swish, float* gnbuf, cudaStream_t st) {
+    int splits = x_splits;
+    if (splits == 0) {
+        splits = (int)std::min<long long>(kGnStatsMaxSplits, std::max<long long>(1, (long long)HW * nw.c / 8 / 2048));
         prof_begin(PC_VQ_GN_STATS, st);
         gn_stats_kernel<<<dim3(splits, B), 256, 0, st>>>(x, HW, nw.c, gnbuf);
         prof_end(st);
         LG_LAUNCH_CHECK();
     }
-    if (ws) ws->gn_src = nullptr;                // gnbuf is consumed below; y (and any later writer of x) invalidates it anyway
     int chunks = (int)std::min<long long>(256, std::max<long long>(1, (long long)HW * (nw.c / 8) / 1024));
     prof_begin(PC_VQ_GN_APPLY, st);
     gn_apply_kernel<<<dim3(chunks, B), 256, 0, st>>>(x, gnbuf, splits, nw.gamma, nw.beta, y, HW, nw.c, swish);
@@ -725,25 +739,25 @@ int run_gn(const NormW& nw, const bf16* x, bf16* y, int B, int HW, int swish, fl
 }
 
 // ResnetBlock (vq_model.py:298-314). x lives in w.X and the result is left in w.X.
-int run_res(const ResW& r, VqWs& w, int B, int H, int W, cudaStream_t st) {
+int run_res(const ResW& r, VqWs& w, int B, int H, int W, int xs, cudaStream_t st) {
     const int HW = H * W;
-    LG_TRY(run_gn(r.n1, w.X, w.T, B, HW, 1, w.gn, st, &w));
-    LG_TRY(run_conv(r.c1, w.T, B, H, W, 0, nullptr, w.U, nullptr, st, nullptr, &w));
-    LG_TRY(run_gn(r.n2, w.U, w.T, B, HW, 1, w.gn, st, &w));
+    int s;
+    LG_TRY(run_gn(r.n1, w.X, xs, w.T, B, HW, 1, w.gn, st));
+    LG_TRY(s = run_conv(w.stats(conv_call(r.c1, w.T, B, H, W, w.U)), st));
+    LG_TRY(run_gn(r.n2, w.U, s, w.T, B, HW, 1, w.gn, st));
+    const bf16* shortcut = w.X;                                                     // in-place residual
     if (r.has_nin) {
-        LG_TRY(run_conv(r.nin, w.X, B, H, W, 0, nullptr, w.U, nullptr, st));     // shortcut -> U
-        LG_TRY(run_conv(r.c2, w.T, B, H, W, 0, w.U, w.X, nullptr, st, nullptr, &w));  // X = conv2 + shortcut
-    } else {
-        LG_TRY(run_conv(r.c2, w.T, B, H, W, 0, w.X, w.X, nullptr, st, nullptr, &w));  // in-place residual
+        LG_TRY(run_conv(conv_call(r.nin, w.X, B, H, W, w.U), st));                  // shortcut -> U
+        shortcut = w.U;
     }
-    return 0;
+    return run_conv(w.stats(conv_call(r.c2, w.T, B, H, W, w.X, shortcut)), st);   // X = conv2 + shortcut
 }
 
 // AttnBlock (vq_model.py:327-351), single head over N = H*W tokens, C channels. In/out: w.X.
-int run_attn(const AttnW& a, VqWs& w, int B, int H, int W, cudaStream_t st) {
+int run_attn(const AttnW& a, VqWs& w, int B, int H, int W, int xs, cudaStream_t st) {
     const int N = H * W, C = a.c;
     LG_REQUIRE(N % 8 == 0, "attention block: token count %d must be a multiple of 8", N);
-    LG_TRY(run_gn(a.norm, w.X, w.T, B, N, 0, w.gn, st, &w));                      // hn -> T  [B*N, C]
+    LG_TRY(run_gn(a.norm, w.X, xs, w.T, B, N, 0, w.gn, st));                      // hn -> T  [B*N, C]
     {   // q | k  -> U [B*N, 2C]
         mma::DenseA al{w.T, C, 0, B * N};
         mma::BRows bw{a.qk.w, a.qk.w, 2 * C, C, 0, 2 * C};
@@ -780,7 +794,28 @@ int run_attn(const AttnW& a, VqWs& w, int B, int H, int W, cudaStream_t st) {
         }
     }
     // x = x + proj_out(O)
-    return run_conv(a.proj, w.T, B, H, W, 0, w.X, w.X, nullptr, st, nullptr, &w);
+    return run_conv(w.stats(conv_call(a.proj, w.T, B, H, W, w.X, w.X)), st);
+}
+
+int run_mid(const MidW& m, VqWs& w, int B, int H, int W, int xs, cudaStream_t st) {
+    LG_TRY(xs = run_res(m.res0, w, B, H, W, xs, st));
+    LG_TRY(xs = run_attn(m.attn, w, B, H, W, xs, st));
+    return run_res(m.res1, w, B, H, W, xs, st);
+}
+
+// A level at H x W, then its resampling conv (up: 1 = Upsample, 2 = Downsample) into w.T, which becomes w.X; H and W follow it
+int run_level(const LevelW& lv, int up, VqWs& w, int B, int& H, int& W, int xs, cudaStream_t st) {
+    for (size_t j = 0; j < lv.res.size(); ++j) {
+        LG_TRY(xs = run_res(lv.res[j], w, B, H, W, xs, st));
+        if (!lv.attn.empty()) LG_TRY(xs = run_attn(lv.attn[j], w, B, H, W, xs, st));
+    }
+    if (!lv.resampling) return xs;
+    ConvCall c = w.stats(conv_call(lv.resample, w.X, B, H, W, w.T));
+    c.up = up;
+    LG_TRY(xs = run_conv(c, st));
+    std::swap(w.X, w.T);
+    H = conv_out_extent(H, up); W = conv_out_extent(W, up);
+    return xs;
 }
 
 }  // namespace
@@ -823,7 +858,8 @@ int lg_vq_finalize(lg_vq* v, void* stream) {
     DeviceGuard guard(v->device);
     for (void* p : v->owned) cudaFree(p);
     v->owned.clear();
-    v->levels.clear();
+    v->dec = TowerW{};
+    v->enc = TowerW{};
     const lg_vq_cfg& c = v->cfg;
     const int n = c.n_mult, nrb = c.num_res_blocks;
     int block_in = c.ch * c.ch_mult[n - 1];
@@ -837,42 +873,16 @@ int lg_vq_finalize(lg_vq* v, void* stream) {
     LG_TRY(get(v, "post_quant_conv.weight", {c.z_channels, c.codebook_embed_dim, 1, 1}, &v->pq_w));
     LG_TRY(get(v, "post_quant_conv.bias", {c.z_channels}, &v->pq_b));
     LG_TRY(make_conv(v, "decoder.conv_in", block_in, c.z_channels, 3, &v->conv_in, st));
-    LG_TRY(make_res(v, "decoder.mid.0", block_in, block_in, &v->mid0, st));
-    LG_TRY(make_attn(v, "decoder.mid.1", block_in, &v->mid1, st));
-    LG_TRY(make_res(v, "decoder.mid.2", block_in, block_in, &v->mid2, st));
+    LG_TRY(make_mid(v, "decoder.mid", block_in, &v->dec.mid, st));
     for (int bi = 0; bi < n; ++bi) {
-        const int i_level = n - 1 - bi;
-        const int block_out = c.ch * c.ch_mult[i_level];
-        LevelW lv;
-        for (int j = 0; j < nrb + 1; ++j) {
-            const std::string p = "decoder.conv_blocks." + std::to_string(bi);
-            ResW r;
-            LG_TRY(make_res(v, p + ".res." + std::to_string(j), block_in, block_out, &r, st));
-            lv.res.push_back(r);
-            block_in = block_out;
-            if (i_level == n - 1) {
-                AttnW a;
-                LG_TRY(make_attn(v, p + ".attn." + std::to_string(j), block_in, &a, st));
-                lv.attn.push_back(a);
-            }
-        }
-        lv.up = i_level != 0;
-        if (lv.up) {
-            const std::string un = "decoder.conv_blocks." + std::to_string(bi) + ".upsample.conv";
-            LG_TRY(make_conv(v, un, block_in, block_in, 3, &lv.upconv, st));
-            if (block_in % 64 == 0) {   // pre-summed 2x2 phase weights for the wgmma upsample path (conv_tc.cu)
-                const float* wf = nullptr;
-                LG_TRY(get(v, un + ".weight", {block_in, block_in, 3, 3}, &wf));
-                LG_TRY(dev_alloc(v, (size_t)16 * block_in * block_in, &lv.upconv.w_phase));
-                LG_TRY(conv_tc_make_phase_weights(wf, lv.upconv.w_phase, block_in, block_in, st));
-            }
-        }
-        v->levels.push_back(lv);
+        const int i_level = n - 1 - bi, block_out = c.ch * c.ch_mult[i_level];
+        LG_TRY(make_level(v, "decoder.conv_blocks." + std::to_string(bi), nrb + 1, block_in, block_out, i_level == n - 1,
+                          i_level != 0 ? 1 : 0, &v->dec, st));
+        block_in = block_out;
     }
-    LG_TRY(make_norm(v, "decoder.norm_out", block_in, &v->norm_out));
-    LG_TRY(make_conv(v, "decoder.conv_out", 3, block_in, 3, &v->conv_out, st));
+    LG_TRY(make_norm(v, "decoder.norm_out", block_in, &v->dec.norm_out));
+    LG_TRY(make_conv(v, "decoder.conv_out", 3, block_in, 3, &v->dec.conv_out, st));
     // ---- encoder (vq_model.py:64-97) + quant_conv (:35): only when the caller bound those tensors
-    v->enc_levels.clear();
     v->has_encoder = v->t.count("encoder.conv_in.weight") && v->t.count("quant_conv.weight");
     if (v->has_encoder) {
         LG_REQUIRE(c.ch % 8 == 0, "encoder: ch=%d must be a multiple of 8", c.ch);
@@ -881,28 +891,13 @@ int lg_vq_finalize(lg_vq* v, void* stream) {
         int bin = c.ch;
         for (int i_level = 0; i_level < n; ++i_level) {
             const int bout = c.ch * c.ch_mult[i_level];
-            const std::string p = "encoder.conv_blocks." + std::to_string(i_level);
-            LevelW lv;
-            for (int j = 0; j < nrb; ++j) {
-                ResW r;
-                LG_TRY(make_res(v, p + ".res." + std::to_string(j), bin, bout, &r, st));
-                lv.res.push_back(r);
-                bin = bout;
-                if (i_level == n - 1) {
-                    AttnW a;
-                    LG_TRY(make_attn(v, p + ".attn." + std::to_string(j), bin, &a, st));
-                    lv.attn.push_back(a);
-                }
-            }
-            lv.up = i_level != n - 1;   // here: has a Downsample conv
-            if (lv.up) LG_TRY(make_conv(v, p + ".downsample.conv", bin, bin, 3, &lv.upconv, st));
-            v->enc_levels.push_back(lv);
+            LG_TRY(make_level(v, "encoder.conv_blocks." + std::to_string(i_level), nrb, bin, bout, i_level == n - 1,
+                              i_level != n - 1 ? 2 : 0, &v->enc, st));
+            bin = bout;
         }
-        LG_TRY(make_res(v, "encoder.mid.0", bin, bin, &v->enc_mid0, st));
-        LG_TRY(make_attn(v, "encoder.mid.1", bin, &v->enc_mid1, st));
-        LG_TRY(make_res(v, "encoder.mid.2", bin, bin, &v->enc_mid2, st));
-        LG_TRY(make_norm(v, "encoder.norm_out", bin, &v->enc_norm_out));
-        LG_TRY(make_conv(v, "encoder.conv_out", c.z_channels, bin, 3, &v->enc_conv_out, st));
+        LG_TRY(make_mid(v, "encoder.mid", bin, &v->enc.mid, st));
+        LG_TRY(make_norm(v, "encoder.norm_out", bin, &v->enc.norm_out));
+        LG_TRY(make_conv(v, "encoder.conv_out", c.z_channels, bin, 3, &v->enc.conv_out, st));
         LG_TRY(make_conv(v, "quant_conv", c.codebook_embed_dim, c.z_channels, 1, &v->quant_conv, st));
     }
     LG_CUDA_OK(cudaStreamSynchronize(st));
@@ -936,26 +931,15 @@ static int vq_decode_impl(lg_vq* v, const int32_t* codes, int B, int grid, void*
         lookup_postquant_kernel<<<bc * grid * grid, 256, 0, st>>>(codes + (size_t)b0 * grid * grid, v->codebook, c.codebook_size,
                                                                   c.codebook_embed_dim, v->pq_w, v->pq_b, c.z_channels, w.T);
         LG_LAUNCH_CHECK();
-        w.gn_src = nullptr;
-        LG_TRY(run_conv(v->conv_in, w.T, bc, H, W, 0, nullptr, w.X, nullptr, st, nullptr, &w));
-        LG_TRY(run_res(v->mid0, w, bc, H, W, st));
-        LG_TRY(run_attn(v->mid1, w, bc, H, W, st));
-        LG_TRY(run_res(v->mid2, w, bc, H, W, st));
-        for (size_t li = 0; li < v->levels.size(); ++li) {
-            const LevelW& lv = v->levels[li];
-            for (size_t j = 0; j < lv.res.size(); ++j) {
-                LG_TRY(run_res(lv.res[j], w, bc, H, W, st));
-                if (!lv.attn.empty()) LG_TRY(run_attn(lv.attn[j], w, bc, H, W, st));
-            }
-            if (lv.up) {  // nearest x2 folded into the conv's gather; result -> T, then swap
-                LG_TRY(run_conv(lv.upconv, w.X, bc, H, W, 1, nullptr, w.T, nullptr, st, nullptr, &w));
-                std::swap(w.X, w.T);
-                H *= 2; W *= 2;
-            }
-        }
-        LG_TRY(run_gn(v->norm_out, w.X, w.T, bc, H * W, 1, w.gn, st, &w));
-        LG_TRY(run_conv(v->conv_out, w.T, bc, H, W, 0, nullptr, nullptr, out_nchw ? out_nchw + (size_t)b0 * out_per_img : nullptr, st,
-                        out_u8 ? out_u8 + (size_t)b0 * out_per_img : nullptr));
+        int xs;   // drain-statistics splits of w.X
+        LG_TRY(xs = run_conv(w.stats(conv_call(v->conv_in, w.T, bc, H, W, w.X)), st));
+        LG_TRY(xs = run_mid(v->dec.mid, w, bc, H, W, xs, st));
+        for (const LevelW& lv : v->dec.levels) LG_TRY(xs = run_level(lv, 1, w, bc, H, W, xs, st));
+        LG_TRY(run_gn(v->dec.norm_out, w.X, xs, w.T, bc, H * W, 1, w.gn, st));
+        ConvCall out = conv_call(v->dec.conv_out, w.T, bc, H, W, nullptr);
+        if (out_nchw) out.out_nchw = out_nchw + (size_t)b0 * out_per_img;
+        if (out_u8) out.out_u8 = out_u8 + (size_t)b0 * out_per_img;
+        LG_TRY(run_conv(out, st));
     }
     return 0;
 }
@@ -1018,25 +1002,15 @@ int lg_vq_encode(lg_vq* v, const float* x_nchw, int B, int H, int W, void* dev_w
             prof_end(st);
             LG_LAUNCH_CHECK();
         }
-        for (size_t li = 0; li < v->enc_levels.size(); ++li) {
-            const LevelW& lv = v->enc_levels[li];
-            for (size_t j = 0; j < lv.res.size(); ++j) {
-                LG_TRY(run_res(lv.res[j], w, bc, h, wd, st));
-                if (!lv.attn.empty()) LG_TRY(run_attn(lv.attn[j], w, bc, h, wd, st));
-            }
-            if (lv.up) {
-                LG_TRY(run_conv(lv.upconv, w.X, bc, h, wd, 2, nullptr, w.T, nullptr, st, nullptr, &w));
-                std::swap(w.X, w.T);
-                h /= 2; wd /= 2;
-            }
-        }
-        LG_TRY(run_res(v->enc_mid0, w, bc, h, wd, st));
-        LG_TRY(run_attn(v->enc_mid1, w, bc, h, wd, st));
-        LG_TRY(run_res(v->enc_mid2, w, bc, h, wd, st));
-        LG_TRY(run_gn(v->enc_norm_out, w.X, w.T, bc, h * wd, 1, w.gn, st, &w));
-        LG_TRY(run_conv(v->enc_conv_out, w.T, bc, h, wd, 0, nullptr, w.U, nullptr, st));
+        int xs = 0;   // drain-statistics splits of w.X: conv_in_rgb_kernel writes none
+        for (const LevelW& lv : v->enc.levels) LG_TRY(xs = run_level(lv, 2, w, bc, h, wd, xs, st));
+        LG_TRY(xs = run_mid(v->enc.mid, w, bc, h, wd, xs, st));
+        LG_TRY(run_gn(v->enc.norm_out, w.X, xs, w.T, bc, h * wd, 1, w.gn, st));
+        LG_TRY(run_conv(conv_call(v->enc.conv_out, w.T, bc, h, wd, w.U), st));
         float* z = out_z_nchw ? out_z_nchw + (size_t)b0 * ed * N : w.Z;
-        LG_TRY(run_conv(v->quant_conv, w.U, bc, h, wd, 0, nullptr, nullptr, z, st));
+        ConvCall qc = conv_call(v->quant_conv, w.U, bc, h, wd, nullptr);
+        qc.out_nchw = z;
+        LG_TRY(run_conv(qc, st));
         LG_TRY(lg_vq_argmin(v, z, bc, grid, out_idx + (size_t)b0 * N, stream));
         if (out_quant_nchw) {
             quant_out_kernel<<<cdiv(bc * N, 256), 256, 0, st>>>(z, out_idx + (size_t)b0 * N, v->codebook, bc, N, ed, c.l2_norm,
@@ -1074,36 +1048,35 @@ int lg_test_vq_conv(const void* x, int B, int Hin, int Win, int Cin, const float
     const bool gn = gn_gamma != nullptr;
     LG_REQUIRE(!gn || (gn_beta && gn_out && out_bf && Cout % 32 == 0 && Cout <= 512 && 256 % (Cout / 8) == 0),
                "lg_test_vq_conv: GroupNorm needs gamma, beta, gn_out, a bf16 output and a supported channel count (%d)", Cout);
-    const int Hout = up == 1 ? 2 * Hin : (up == 2 ? Hin / 2 : Hin), Wout = up == 1 ? 2 * Win : (up == 2 ? Win / 2 : Win);
-    // scratch: repacked weights, phase weights, GroupNorm partials (64 stand-alone splits or one per 16x16 tile and phase)
-    const bool phase = up == 1 && Cin % 64 == 0;
+    // scratch: repacked weights, phase weights, GroupNorm partials
+    const bool phase = conv_has_phase_weights(up, Cin);
     const size_t wq_bytes = a256((size_t)Cout * Cin * ksize * ksize * sizeof(bf16));
     const size_t wp_bytes = phase ? a256((size_t)16 * Cout * Cin * sizeof(bf16)) : 0;
-    const size_t gn_floats = (size_t)B * std::max(64, cdiv(Hin, 16) * cdiv(Win, 16) * 4) * 64;
+    const size_t gn_floats = gn_partial_capacity(B, Hin, Win);
     const size_t need = wq_bytes + wp_bytes + gn_floats * sizeof(float);
     LG_REQUIRE(scratch_bytes >= need, "lg_test_vq_conv: scratch %zu < %zu", scratch_bytes, need);
     char* s = (char*)dev_scratch;
-    ConvW cw;
-    cw.w = (bf16*)s; cw.bias = bias; cw.cout = Cout; cw.cin = Cin; cw.k = ksize;
-    repack_conv_kernel<<<132 * 4, 256, 0, st>>>(w, cw.w, Cout, Cin, ksize * ksize);
+    bf16* wq = (bf16*)s;
+    bf16* wp = phase ? (bf16*)(s + wq_bytes) : nullptr;
+    repack_conv_kernel<<<132 * 4, 256, 0, st>>>(w, wq, Cout, Cin, ksize * ksize);
     LG_LAUNCH_CHECK();
-    if (phase) {
-        cw.w_phase = (bf16*)(s + wq_bytes);
-        LG_TRY(conv_tc_make_phase_weights(w, cw.w_phase, Cout, Cin, st));
-    }
-    VqWs ws{};
-    ws.gn = (float*)(s + wq_bytes + wp_bytes);
-    ws.gn_floats = gn_floats;
-    LG_TRY(run_conv(cw, (const bf16*)x, B, Hin, Win, up, (const bf16*)residual, (bf16*)out_bf, out_nchw, st, out_u8, &ws, path));
-    *gn_splits = ws.gn_src == out_bf && out_bf ? ws.gn_splits : 0;
-    if (gn_partial && *gn_splits > 0) {
-        const size_t n = (size_t)B * *gn_splits * 64;
+    if (phase) LG_TRY(conv_tc_make_phase_weights(w, wp, Cout, Cin, st));
+    const ConvW cw{wq, wp, bias, Cout, Cin, ksize};
+    ConvCall c = conv_call(cw, (const bf16*)x, B, Hin, Win, (bf16*)out_bf, (const bf16*)residual);
+    c.up = up; c.out_nchw = out_nchw; c.out_u8 = out_u8;
+    c.gn_partial = (float*)(s + wq_bytes + wp_bytes); c.gn_floats = gn_floats;
+    int splits;
+    LG_TRY(splits = run_conv(c, st, path));
+    *gn_splits = splits;
+    if (gn_partial && splits > 0) {
+        const size_t n = (size_t)B * splits * 32 * 2;
         LG_REQUIRE(gn_partial_floats >= n, "lg_test_vq_conv: gn_partial %zu < %zu floats", gn_partial_floats, n);
-        LG_CUDA_OK(cudaMemcpyAsync(gn_partial, ws.gn, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        LG_CUDA_OK(cudaMemcpyAsync(gn_partial, c.gn_partial, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
     }
     if (gn) {
         const NormW nw{gn_gamma, gn_beta, Cout};
-        LG_TRY(run_gn(nw, (const bf16*)out_bf, (bf16*)gn_out, B, Hout * Wout, gn_swish, ws.gn, st, &ws));
+        const int HWout = conv_out_extent(Hin, up) * conv_out_extent(Win, up);
+        LG_TRY(run_gn(nw, (const bf16*)out_bf, splits, (bf16*)gn_out, B, HWout, gn_swish, c.gn_partial, st));
     }
     return 0;
 }
@@ -1112,10 +1085,10 @@ int lg_test_group_norm(const void* x, int B, int HW, int C, const float* gamma, 
                        void* dev_scratch, size_t scratch_bytes, void* stream) {
     LG_REQUIRE(x && gamma && beta && y && dev_scratch && B > 0 && HW > 0, "lg_test_group_norm: bad argument");
     LG_REQUIRE(C % 32 == 0 && C <= 512 && 256 % (C / 8) == 0, "lg_test_group_norm: unsupported channel count %d", C);
-    const size_t need = (size_t)B * 64 * 64 * sizeof(float);       // gn_stats_kernel: at most 64 splits x 32 groups x (sum, sum sq)
+    const size_t need = (size_t)B * kGnStatsMaxSplits * 32 * 2 * sizeof(float);
     LG_REQUIRE(scratch_bytes >= need, "lg_test_group_norm: scratch %zu < %zu", scratch_bytes, need);
     const NormW nw{gamma, beta, C};
-    return run_gn(nw, (const bf16*)x, (bf16*)y, B, HW, swish, (float*)dev_scratch, (cudaStream_t)stream);
+    return run_gn(nw, (const bf16*)x, 0, (bf16*)y, B, HW, swish, (float*)dev_scratch, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -210,25 +210,16 @@ class VQModel(nn.Module):
         Returns fp32 NCHW [B, 3, H, W] on the model's device."""
         if shape is None or not channel_first:
             raise NotImplementedError("decode_code needs shape=[B, C, g, g] with channel_first=True (the only form the samplers use)")
-        h = self.engine()
-        lib = _lib.load()
-        dev = self.quantize.embedding.weight.device
-        B, g = int(shape[0]), int(shape[2])
-        if int(shape[3]) != g or int(shape[1]) != self.config.codebook_embed_dim:
-            raise ValueError(f"bad latent shape {shape}")
-        codes = code_b.to(device=dev, dtype=torch.int32).reshape(B, g * g).contiguous()
-        up = 2 ** (len(self.config.decoder_ch_mult) - 1)
-        out = torch.empty(B, 3, g * up, g * up, dtype=torch.float32, device=dev)
-        base, nbytes = self._workspace(h, B, g, dev)
-        _lib.check(lib.lg_vq_decode(h, _lib.ptr(codes), B, g, ctypes.c_void_p(base), nbytes, _lib.ptr(out),
-                                    _lib.current_stream(dev)), "lg_vq_decode")
-        return out
+        return self._decode(code_b, shape, uint8=False)
 
     @torch.no_grad()
     def decode_code_uint8(self, code_b, shape):
         """decode_code + the samplers' pixel finishing without a resize (sample_c2i_ddp.py:141-143:
         `clamp(127.5 * x + 128, 0, 255).permute(0, 2, 3, 1).to(uint8)`) in ONE pass: conv_out's accumulator drain writes
         the uint8 NHWC bytes, the fp32 image never exists in HBM. Returns uint8 [B, H, W, 3]."""
+        return self._decode(code_b, shape, uint8=True)
+
+    def _decode(self, code_b, shape, uint8):
         h = self.engine()
         lib = _lib.load()
         dev = self.quantize.embedding.weight.device
@@ -236,11 +227,14 @@ class VQModel(nn.Module):
         if int(shape[3]) != g or int(shape[1]) != self.config.codebook_embed_dim:
             raise ValueError(f"bad latent shape {shape}")
         codes = code_b.to(device=dev, dtype=torch.int32).reshape(B, g * g).contiguous()
-        up = 2 ** (len(self.config.decoder_ch_mult) - 1)
-        out = torch.empty(B, g * up, g * up, 3, dtype=torch.uint8, device=dev)
+        H = g * 2 ** (len(self.config.decoder_ch_mult) - 1)
+        if uint8:
+            out, entry = torch.empty(B, H, H, 3, dtype=torch.uint8, device=dev), "lg_vq_decode_u8"
+        else:
+            out, entry = torch.empty(B, 3, H, H, dtype=torch.float32, device=dev), "lg_vq_decode"
         base, nbytes = self._workspace(h, B, g, dev)
-        _lib.check(lib.lg_vq_decode_u8(h, _lib.ptr(codes), B, g, ctypes.c_void_p(base), nbytes, _lib.ptr(out),
-                                       _lib.current_stream(dev)), "lg_vq_decode_u8")
+        _lib.check(getattr(lib, entry)(h, _lib.ptr(codes), B, g, ctypes.c_void_p(base), nbytes, _lib.ptr(out),
+                                       _lib.current_stream(dev)), entry)
         return out
 
     @torch.no_grad()

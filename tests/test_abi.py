@@ -83,6 +83,31 @@ def test_workspace_bytes_are_pinned(m, t2i, dtype, kv_fp8, sizes, monkeypatch):
         lib.lg_engine_destroy(h)
 
 
+@pytest.mark.parametrize("ch, ch_mult, z, n_e, sizes", [
+    (128, (1, 1, 2, 2, 4), 256, 16384, {(1, 16): 51257344, (64, 16): 3280470016, (3, 24): 349304832,
+                                        (128, 16): 6407168000}),          # 128 images at 16x16: chunks of 125
+    (128, (1, 2, 2, 4), 256, 16384, {(1, 16): 25894912, (64, 32): 6389596160}),
+    (32, (1, 2), 32, 64, {(2, 4): 90112, (4, 16): 3375104}),
+], ids=["vq16", "vq8", "tiny"])
+def test_vq_workspace_bytes_are_pinned(ch, ch_mult, z, n_e, sizes):
+    """The VQ workspace (activations, attention scores, GroupNorm partials, encoder latents) per chunk of images is host
+    arithmetic: its size, computed without a GPU, must not move."""
+    from llamagen_b200 import _lib
+    lib = _lib.load()
+    cfg = _lib.VqCfg(n_e, 8, z, ch, 2, len(ch_mult), (ctypes.c_int32 * 8)(*ch_mult), 1)
+    h = ctypes.c_void_p()
+    assert lib.lg_vq_create(ctypes.byref(cfg), 0, ctypes.byref(h)) == 0, lib.lg_last_error()
+    try:
+        got = {}
+        for B, grid in sizes:
+            n = ctypes.c_size_t()
+            assert lib.lg_vq_workspace_bytes(h, B, grid, ctypes.byref(n)) == 0, lib.lg_last_error()
+            got[(B, grid)] = n.value
+        assert got == sizes
+    finally:
+        lib.lg_vq_destroy(h)
+
+
 def test_product_never_imports_oracle():
     """The shipped package must not route through the CPU oracle (graded constraint ③)."""
     pkg = os.path.join(ROOT, "llamagen_b200")
