@@ -128,6 +128,23 @@ int  lg_generate(lg_engine* e, const void* cond, const float* emb_mask, int B, i
                  const lg_sample_cfg* sc, int32_t* out_tokens, float* dbg_logits,
                  const int32_t* teacher, void* stream);
 
+/* ---- teacher-forced scoring: Transformer.forward(idx, cond_idx, targets) (gpt.py:341-382, eval mode) ----------------------- */
+/* Bytes of caller-provided scratch for lg_score over `rows` sequences (rows = 2B under CFG) of `seq` positions (T + S - 1). */
+int  lg_score_workspace_bytes(lg_engine* e, int rows, int seq, size_t* bytes);
+/* Teacher-forced forward (gpt.py:341-382, eval mode): for each image b the sequence is the condition (T positions, as lg_prefill
+ * embeds it; emb_mask as in lg_prefill) followed by the token embeddings of idx[b, 0..S-2]. Scores the S positions T-1 .. T+S-2.
+ * idx dev int32 [B, S-1] (NULL iff S == 1); targets dev int32 [B, S] or NULL.
+ * use_cfg: rows doubled with the null condition, as lg_prefill does; both halves read the same idx. The scored logits are
+ * uncond + (cond - uncond) * cfg_scale (generate.py:79-82,95-97).
+ * logits_out: NULL or dev f32 [B, S, V]. Holds the head output rounded to the model dtype, as lg_prefill / lg_decode_step return it,
+ * CFG-mixed when use_cfg. nll_out: NULL or dev f32 [B, S], -log_softmax(logits)[target] (needs targets; NaN for a target outside
+ * [0, V)). At least one of the two is given.
+ * Uses only dev_ws (lg_score_workspace_bytes, 256-byte aligned); never touches the workspace of lg_engine_set_workspace, so a
+ * generation's KV cache survives. K and V are kept for one layer at a time, always in the model dtype (also after
+ * lg_engine_set_kv_cache). May process the batch in image chunks that fit ws_bytes; a CFG twin always stays in its image's chunk. */
+int  lg_score(lg_engine* e, const void* cond, const float* emb_mask, const int32_t* idx, const int32_t* targets, int B, int T, int S,
+              int use_cfg, float cfg_scale, void* dev_ws, size_t ws_bytes, float* logits_out, float* nll_out, void* stream);
+
 /* ---- VQ tokenizer: replaces VQModel.decode_code / VectorQuantizer (vq_model.py) ------------------- */
 typedef struct lg_vq_cfg {
     int32_t codebook_size;
@@ -205,8 +222,9 @@ int  lg_test_gemm(const void* x, const void* w, int M, int N, int K, int dtype, 
  * Input: q (dev [R * Tq][H * hd], post-RoPE) or the QKV GEMM's split-K slabs qkv_partial (dev f32 [ksplit][R * Tq][3 * H * hd]) with
  * freqs (dev f32 [max_seq][hd / 2][2]): fuse = 0 runs the QKV epilogue (q -> q_out, K / V rows written at the query positions) and
  * then the attention; fuse = 1 lets the TMA decode kernel do the epilogue itself (Tq = 1). out: dev [R * Tq][H * hd].
- * path (int[3]) or NULL: kernel (0 = attention_kernel, 1 = attn_tma_kernel, 3 = attn_prefill_tc_kernel; 2 is unused),
- * TMA ring depth (0 for attention_kernel) and whether the QKV epilogue was fused. Every argument is checked before any launch;
+ * path (int[3]) or NULL: kernel (0 = attention_kernel, 1 = attn_tma_kernel, 2 = attn_causal_tc_kernel: Tq > 128 from position 0 on a
+ * 16-bit cache in the model dtype, 3 = attn_prefill_tc_kernel), TMA ring depth (0 for attention_kernel) and whether the QKV epilogue
+ * was fused. R * Tq may exceed 65535 only on kernel 2. Every argument is checked before any launch;
  * the caller keeps *pos_dev + pos_value + Tq <= max_seq and pos_rows[r] < max_seq. */
 int  lg_test_attention(int dtype, int kv_dtype, float k_scale, float v_scale, int R, int Tq, int H, int hd, int hdp, int max_seq,
                        void* kcache, void* vcache, int n_layer, int layer, int pos_value, const int32_t* pos_dev,

@@ -654,6 +654,206 @@ __global__ void __launch_bounds__(256, 2) attn_prefill_tc_kernel(const __grid_co
     }
 }
 
+// ---------------------------------------------------------------------------------------------------
+// Long causal attention (Tq > 128 query positions per row, from position 0: the teacher-forced sequence of lg_score, gpt.py:341-368
+// in eval mode): one CTA per (head, row, block of kCqRows queries), 4 warps of 16 query rows each. The key blocks at or below the
+// block's causal diagonal stream through a kCqStages-deep TMA / mbarrier ring in kCqKeys-key blocks (kKC-row boxes of the KV maps);
+// S = Q K^T and O += P V run on mma.sync m16n8k16 with ldmatrix operands, the softmax is online in fp32 registers and P is reused
+// from the score fragments (FlashAttention-2). Q comes straight from global memory into A fragments (rows of 64, 128 or the 100
+// dims of GPT-3B, whose K / V rows are 112 wide: the maps read dims 112..127 as zeros). No R * Tq grid limit.
+// ---------------------------------------------------------------------------------------------------
+constexpr int kCqRows = 64;       // query rows per CTA
+constexpr int kCqKeys = 64;       // keys per ring stage
+constexpr int kCqStages = 2;
+
+template <typename T, int HD>
+__global__ void __launch_bounds__(128) attn_causal_tc_kernel(const __grid_constant__ CUtensorMap kmap,
+                                                             const __grid_constant__ CUtensorMap vmap, AttnTmaArgs a, int Tq) {
+    constexpr int NSUB = HD / 64;
+    constexpr int SUB_BYTES = kCqKeys * 128;      // [kCqKeys keys][64 dims], 128-byte swizzle
+    constexpr int TILE_BYTES = NSUB * SUB_BYTES;
+    constexpr int NT = kCqKeys / 8;               // n8 score tiles per stage
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    uint8_t* tiles = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(tiles + kCqStages * 2 * TILE_BYTES);
+
+    const int h = blockIdx.x, r = blockIdx.y;
+    const int q0 = (gridDim.z - 1 - blockIdx.z) * kCqRows;   // the longest blocks start first
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, tg = lane & 3;
+    const long long row0 = a.row_base + ((long long)r * a.H + h) * a.maxS;
+    const int hdr = a.hd, D = a.H * hdr;
+    const int nkeys = min(q0 + kCqRows, Tq);
+    const int nblk = (nkeys + kCqKeys - 1) / kCqKeys;
+
+    if (threadIdx.x == 0) {
+        prefetch_map(&kmap);
+        prefetch_map(&vmap);
+        for (int s = 0; s < kCqStages; ++s) mbar_init(&full_bar[s], 1);
+        fence_barrier_init();
+    }
+    __syncthreads();
+    lg_pdl_sync();                                   // q and the K / V rows were written by the QKV epilogue just before
+    auto issue = [&](int kb) {
+        const int s = kb % kCqStages;
+        uint8_t* kt = tiles + s * 2 * TILE_BYTES;
+        uint8_t* vt = kt + TILE_BYTES;
+        mbar_expect_tx(&full_bar[s], 2 * TILE_BYTES);
+#pragma unroll
+        for (int sub = 0; sub < NSUB; ++sub)
+#pragma unroll
+            for (int i = 0; i < kCqKeys / kKC; ++i) {
+                const int row = (int)(row0 + (long long)kb * kCqKeys + i * kKC);
+                load_2d(kt + sub * SUB_BYTES + i * kKC * 128, &kmap, &full_bar[s], sub * 64, row);
+                load_2d(vt + sub * SUB_BYTES + i * kKC * 128, &vmap, &full_bar[s], sub * 64, row);
+            }
+    };
+    if (threadIdx.x == 0)
+        for (int kb = 0; kb < min(kCqStages, nblk); ++kb) issue(kb);
+
+    // Q rows t0 = q0 + 16 warp + g and t1 = t0 + 8 as m16n8k16 A fragments (pairs of dims; hdr % 4 == 0, so a pair is all real
+    // or all padding)
+    const int t0 = q0 + warp * 16 + g, t1 = t0 + 8;
+    uint32_t qa[HD / 16][4];
+    {
+        const T* qp = reinterpret_cast<const T*>(a.q) + (size_t)h * hdr;
+        const T* r0p = qp + ((size_t)r * Tq + t0) * D;
+        const T* r1p = qp + ((size_t)r * Tq + t1) * D;
+#pragma unroll
+        for (int kk = 0; kk < HD / 16; ++kk) {
+            const int d0 = kk * 16 + tg * 2, d1 = d0 + 8;
+            qa[kk][0] = (t0 < Tq && d0 < hdr) ? *reinterpret_cast<const uint32_t*>(r0p + d0) : 0u;
+            qa[kk][1] = (t1 < Tq && d0 < hdr) ? *reinterpret_cast<const uint32_t*>(r1p + d0) : 0u;
+            qa[kk][2] = (t0 < Tq && d1 < hdr) ? *reinterpret_cast<const uint32_t*>(r0p + d1) : 0u;
+            qa[kk][3] = (t1 < Tq && d1 < hdr) ? *reinterpret_cast<const uint32_t*>(r1p + d1) : 0u;
+        }
+    }
+    const float* mrow = a.emb_mask ? a.emb_mask + (size_t)(r % a.B) * a.Tc : nullptr;
+    float o[HD / 8][4];
+#pragma unroll
+    for (int i = 0; i < HD / 8; ++i) { o[i][0] = 0.f; o[i][1] = 0.f; o[i][2] = 0.f; o[i][3] = 0.f; }
+    float mx[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};   // running max (quad-uniform) and this lane's share of the sum
+
+    for (int kb = 0; kb < nblk; ++kb) {
+        const int s = kb % kCqStages;
+        mbar_wait(&full_bar[s], (uint32_t)((kb / kCqStages) & 1));
+        const int j0 = kb * kCqKeys;
+        if (j0 <= q0 + warp * 16 + 15) {             // warp-uniform: some key of the block is at or below this warp's diagonal
+            const uint32_t kt = smem_u32(tiles + s * 2 * TILE_BYTES);
+            const uint32_t vt = kt + TILE_BYTES;
+            float sc[NT][4];
+#pragma unroll
+            for (int i = 0; i < NT; ++i) { sc[i][0] = 0.f; sc[i][1] = 0.f; sc[i][2] = 0.f; sc[i][3] = 0.f; }
+#pragma unroll
+            for (int kk = 0; kk < HD / 16; ++kk) {
+#pragma unroll
+                for (int np = 0; np < NT / 2; ++np) {
+                    uint32_t b0, b1, b2, b3;
+                    const int row = np * 16 + (lane & 7) + ((lane >> 4) << 3);
+                    ldsm_x4(kt + (kk / 4) * SUB_BYTES + swz(row, (kk * 2 + ((lane >> 3) & 1)) & 7), b0, b1, b2, b3);
+                    mma16816<T>(sc[2 * np], qa[kk][0], qa[kk][1], qa[kk][2], qa[kk][3], b0, b1);
+                    mma16816<T>(sc[2 * np + 1], qa[kk][0], qa[kk][1], qa[kk][2], qa[kk][3], b2, b3);
+                }
+            }
+            // ---- mask + online softmax; values [..][0..1] belong to row t0, [..][2..3] to row t1
+            float bmax[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+            for (int nt = 0; nt < NT; ++nt) {
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const int t = (e >> 1) ? t1 : t0, j = j0 + nt * 8 + tg * 2 + (e & 1);
+                    bool vis = j <= t;
+                    if (vis && mrow && j < a.Tc && j != t) vis = mrow[j] != 0.f;
+                    const float x = vis ? sc[nt][e] * a.scale : -INFINITY;
+                    sc[nt][e] = x;
+                    bmax[e >> 1] = fmaxf(bmax[e >> 1], x);
+                }
+            }
+            float corr[2];
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+                bmax[hh] = fmaxf(bmax[hh], __shfl_xor_sync(0xffffffffu, bmax[hh], 1));
+                bmax[hh] = fmaxf(bmax[hh], __shfl_xor_sync(0xffffffffu, bmax[hh], 2));
+                const float mn = fmaxf(mx[hh], bmax[hh]);
+                corr[hh] = mn == -INFINITY ? 1.f : __expf(mx[hh] - mn);   // exp(-inf) = 0 when the row saw no visible key yet
+                mx[hh] = mn;
+                l[hh] *= corr[hh];
+            }
+#pragma unroll
+            for (int nt = 0; nt < NT; ++nt) {
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const float m = mx[e >> 1];
+                    const float pv = m == -INFINITY ? 0.f : __expf(sc[nt][e] - m);
+                    sc[nt][e] = pv;
+                    l[e >> 1] += pv;
+                }
+            }
+#pragma unroll
+            for (int i = 0; i < HD / 8; ++i) { o[i][0] *= corr[0]; o[i][1] *= corr[0]; o[i][2] *= corr[1]; o[i][3] *= corr[1]; }
+            // ---- O += P V, P packed to T from the score fragments (C layout of S == A layout of P)
+#pragma unroll
+            for (int kb16 = 0; kb16 < kCqKeys / 16; ++kb16) {
+                const uint32_t pa0 = pack16<T>(sc[2 * kb16][0], sc[2 * kb16][1]), pa1 = pack16<T>(sc[2 * kb16][2], sc[2 * kb16][3]);
+                const uint32_t pa2 = pack16<T>(sc[2 * kb16 + 1][0], sc[2 * kb16 + 1][1]);
+                const uint32_t pa3 = pack16<T>(sc[2 * kb16 + 1][2], sc[2 * kb16 + 1][3]);
+#pragma unroll
+                for (int np = 0; np < HD / 16; ++np) {
+                    uint32_t b0, b1, b2, b3;
+                    const int row = kb16 * 16 + (lane & 7) + (((lane >> 3) & 1) << 3);
+                    ldsm_x4_t(vt + (np / 4) * SUB_BYTES + swz(row, (np * 2 + (lane >> 4)) & 7), b0, b1, b2, b3);
+                    mma16816<T>(o[2 * np], pa0, pa1, pa2, pa3, b0, b1);
+                    mma16816<T>(o[2 * np + 1], pa0, pa1, pa2, pa3, b2, b3);
+                }
+            }
+        }
+        __syncthreads();                             // every warp is done with stage s
+        if (threadIdx.x == 0 && kb + kCqStages < nblk) issue(kb + kCqStages);
+    }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+        l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 1);
+        l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 2);
+    }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+        const int t = hh ? t1 : t0;
+        if (t < Tq) {
+            const float inv = 1.0f / l[hh];          // the diagonal key is always visible: l > 0
+            T* op = reinterpret_cast<T*>(a.out) + ((size_t)r * Tq + t) * D + (size_t)h * hdr;
+#pragma unroll
+            for (int i = 0; i < HD / 8; ++i)
+                if (i * 8 + tg * 2 < hdr) *reinterpret_cast<uint32_t*>(op + i * 8 + tg * 2) = pack16<T>(o[i][2 * hh] * inv, o[i][2 * hh + 1] * inv);
+        }
+    }
+}
+
+bool attn_causal_tc_supported(const AttnArgs& a) {
+    const bool shape = a.hd == 64 || a.hd == 128 || (a.hd == 100 && a.hdp == 112);
+    return lg_dtype_is16(a.dtype) && !a.kv_f8 && shape && a.Tq > kPfRows && a.kmap && a.vmap && a.pos.dev == nullptr &&
+           a.pos.rows == nullptr && a.pos.value == 0 && a.maxS >= a.Tq && a.R <= 65535;
+}
+
+int launch_attention_causal_tc(const AttnArgs& a, cudaStream_t st, int* path) {
+    AttnTmaArgs t{};
+    t.q = (const bf16*)a.q; t.out = (bf16*)a.out; t.R = a.R; t.H = a.H; t.maxS = a.maxS;
+    t.row_base = a.cache_row_base; t.emb_mask = a.emb_mask; t.B = a.B; t.Tc = a.Tc; t.scale = a.scale;
+    t.hd = a.hd; t.hdp = a.hdp ? a.hdp : a.hd;
+    const bool half = a.dtype == LG_DTYPE_F16, wide = a.hd != 64;
+    auto kern = wide ? (half ? attn_causal_tc_kernel<f16, 128> : attn_causal_tc_kernel<bf16, 128>)
+                     : (half ? attn_causal_tc_kernel<f16, 64> : attn_causal_tc_kernel<bf16, 64>);
+    const size_t smem = 1024 + (size_t)kCqStages * 2 * (wide ? 2 : 1) * kCqKeys * 128 + kCqStages * sizeof(uint64_t);
+    static DevOnce attr[4];
+    if (lg_first_on_device(attr[(half ? 1 : 0) + (wide ? 2 : 0)])) {
+        LG_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    }
+    dim3 grid(a.H, a.R, (a.Tq + kCqRows - 1) / kCqRows);
+    (void)lg_launch(kern, dim3(grid), dim3(128), smem, st, *reinterpret_cast<const CUtensorMap*>(a.kmap),
+                    *reinterpret_cast<const CUtensorMap*>(a.vmap), t, a.Tq);
+    LG_LAUNCH_CHECK();
+    set_attn_path(path, 2, kCqStages, 0);
+    return 0;
+}
+
 // KV-cache tensor maps: the whole K (or V) region of the workspace as one [rows, hd] bf16 / fp16 matrix, or (dtype LG_DTYPE_E4M3)
 // one [rows, hdp] byte matrix read in boxes of 64 bytes (hd 64) or 128 bytes (hdp 128 or 112; bytes 112..127 read as zeros)
 int attn_tma_make_map(void* map_out, const void* cache_base, long long total_rows, int hdp, int dtype, int tail16) {

@@ -174,6 +174,10 @@ struct Workspace {
     int32_t* tokens = nullptr;
     int* counters = nullptr;  // [0] = pos, [1] = step, [64] = the fused sampler tail's ticket
     KvMaps maps;
+    // lg_score's view (lg_engine::carve_score): K / V of ONE layer in the model dtype, rewritten by every layer (a teacher-forced pass
+    // never decodes afterwards), and the rows of one head GEMM
+    bool score = false;
+    int head_rows = 0;
 };
 
 struct Layer {
@@ -222,14 +226,22 @@ struct lg_engine {
                gemv_small_supported(M, F, D, dt, true) && gemv_small_supported(M, D, F, dt, false) && gemv_small_supported(M, V, D, dt, false);
     }
     size_t carve(Workspace& o, char* base, int rows, int max_seq, int g = 0, int n = 1) const;
-    // K / V tensor maps over every layer of a workspace or chain view
+    size_t carve_score(Workspace& o, char* base, int rows, int seq) const;
+    // K / V tensor maps over every layer of a workspace or chain view (one layer in the model dtype for a scoring view)
     int make_maps(Workspace& w) const {
+        if (w.score) return make_kv_maps(w.maps, cfg.dtype, hd, hdp, cfg.dtype, w.kcache, w.vcache, (long long)w.rows * cfg.n_head * w.max_seq);
         return make_kv_maps(w.maps, cfg.dtype, hd, hdp, kv_f8 ? LG_DTYPE_E4M3 : cfg.dtype, w.kcache, w.vcache,
                             (long long)cfg.n_layer * w.rows * cfg.n_head * w.max_seq);
     }
     AttnArgs attn_args(const Workspace& w, int l, int R, int Tq) const {
+        if (w.score) return make_attn_args(cfg.dtype, cfg.n_head, hd, hdp, w.rows, w.max_seq, w.kcache, w.vcache, w.maps, nullptr, 0, R, Tq);
         return make_attn_args(cfg.dtype, cfg.n_head, hd, hdp, w.rows, w.max_seq, w.kcache, w.vcache, w.maps,
                               kv_f8 ? &kv_scales[2 * l] : nullptr, l, R, Tq);
+    }
+    AttnArgs layer_attn(const Workspace& w, int l, int R, int Tq, PosArg pos, const float* emb_mask, int B) const {
+        AttnArgs aa = attn_args(w, l, R, Tq);
+        aa.q = w.q; aa.out = w.attn; aa.pos = pos; aa.emb_mask = emb_mask; aa.B = B; aa.Tc = cfg.cls_token_num;
+        return aa;
     }
     int zero_fill_if_needed(cudaStream_t st) {
         if (!ws_needs_zero || !full.base) return 0;
@@ -241,6 +253,8 @@ struct lg_engine {
     // xn_ready: xn already holds RMSNorm_0(h) (the fused tail of the previous decode step's sample kernel wrote it)
     int forward(const Workspace& w, int M, int Tq, PosArg pos, const float* emb_mask, int B, float* logits_out, bool xn_ready,
                 cudaStream_t st);
+    // the transformer blocks over M = R * Tq rows of w.h, leaving RMSNorm_final(h) in w.xn (batched GEMM path)
+    int run_layers(const Workspace& w, int M, int Tq, PosArg pos, const float* emb_mask, int B, bool xn_ready, cudaStream_t st);
     int embed_cond(const Workspace& w, const void* cond, int B, int R, int T, cudaStream_t st);
     int gemm(const Workspace& w, const void* x, int M, int N, int K, const void* wa, const void* wb, int n_split, int* ksplit,
              float* direct_out, cudaStream_t st, const GemmNext* next = nullptr);
@@ -292,6 +306,51 @@ size_t lg_engine::carve(Workspace& o, char* base, int rows, int max_seq, int g, 
     return off;
 }
 
+constexpr int kScoreHeadRows = 2048;   // rows per head GEMM of lg_score: its fp32 slabs stay ~kScoreHeadRows * V floats
+
+// lg_score's scratch for `rows` sequences of `seq` positions, from `base` (null: sizes only): the activations of rows * seq positions,
+// the GEMM partials of that M (and of the caption MLP and one head chunk), and K / V of ONE layer ([rows, H, round8(seq), hdp] in the
+// model dtype, also after lg_engine_set_kv_cache): every layer rewrites it before its attention reads it.
+size_t lg_engine::carve_score(Workspace& o, char* base, int rows, int seq) const {
+    const int D = cfg.dim, F = cfg.ffn_dim, V = cfg.vocab_size, H = cfg.n_head, Tc = cfg.cls_token_num;
+    const bool t2i = cfg.model_type == LG_MODEL_T2I;
+    const int seq8 = (seq + 7) / 8 * 8, M = rows * seq;
+    size_t off = 0;
+    auto take = [&](size_t bytes) {
+        char* p = base ? base + off : nullptr;
+        off += align_up(bytes);
+        return p;
+    };
+    const size_t kv = (size_t)rows * H * seq8 * hdp * esz;
+    o.kcache = take(kv);
+    o.vcache = take(kv);
+    o.cache_bytes = off;
+    o.h = take((size_t)M * D * esz);
+    o.xn = take((size_t)M * D * esz);
+    o.q = take((size_t)M * D * esz);
+    o.attn = take((size_t)M * D * esz);
+    o.ff = take((size_t)M * F * esz);
+    o.x0 = take(t2i ? (size_t)rows * Tc * cfg.caption_dim * esz : 0);
+    size_t pf = 0;
+    pf = std::max(pf, gemm_partial_floats(M, 3 * D, D, cfg.dtype));
+    pf = std::max(pf, gemm_partial_floats(M, D, D, cfg.dtype));
+    pf = std::max(pf, gemm_partial_floats(M, 2 * F, D, cfg.dtype));
+    pf = std::max(pf, gemm_partial_floats(M, D, F, cfg.dtype));
+    if (t2i) {
+        pf = std::max(pf, gemm_partial_floats(rows * Tc, D, cfg.caption_dim, cfg.dtype));
+        pf = std::max(pf, gemm_partial_floats(rows * Tc, D, D, cfg.dtype));
+    }
+    o.head_rows = std::min(rows * std::max(seq - Tc + 1, 1), kScoreHeadRows);
+    pf = std::max(pf, gemm_partial_floats(o.head_rows, V, D, cfg.dtype));
+    o.partial_floats = pf;
+    o.partial = (float*)take(pf * sizeof(float));
+    o.base = base;
+    o.rows = rows;
+    o.max_seq = seq8;
+    o.score = true;
+    return off;
+}
+
 int lg_engine::gemm(const Workspace& w, const void* x, int M, int N, int K, const void* wa, const void* wb, int n_split, int* ksplit,
                     float* direct_out, cudaStream_t st, const GemmNext* next) {
     // when the plan needs a single slab the GEMM can write straight into `direct_out`
@@ -313,18 +372,13 @@ int lg_engine::forward(const Workspace& w, int M, int Tq, PosArg pos, const floa
     const int R = M / Tq;
     const int dt = cfg.dtype;
     int ks = 1;
-    auto layer_attn = [&](int l) {
-        AttnArgs aa = attn_args(w, l, R, Tq);
-        aa.q = w.q; aa.out = w.attn; aa.pos = pos; aa.emb_mask = emb_mask; aa.B = B; aa.Tc = cfg.cls_token_num;
-        return aa;
-    };
     // ---- R <= 8 decode step (batch-1 latency path, gemv_small.cu): 5 dependent kernels per layer, no slabs
     if (Tq == 1 && small_row_path(M, attn_args(w, 0, R, Tq))) {
         for (int l = 0; l < L; ++l) {
             const Layer& ly = layers[l];
             GemvSmall gq{ly.wqkv, nullptr, 3 * D, D, M, w.h, ly.attn_norm, cfg.norm_eps, w.partial, nullptr, nullptr, dt};
             LG_PROF(PC_GEMM_QKV, st, launch_gemv_small(gq, st));
-            AttnArgs aa = layer_attn(l);
+            AttnArgs aa = layer_attn(w, l, R, Tq, pos, emb_mask, B);
             aa.qkv_partial = w.partial; aa.qkv_ksplit = 1; aa.freqs = freqs;
             LG_PROF(PC_ATTENTION, st, launch_attention(aa, st));
             GemvSmall go{ly.wo, nullptr, D, D, M, w.attn, nullptr, 0.f, nullptr, w.h, nullptr, dt};
@@ -338,6 +392,27 @@ int lg_engine::forward(const Workspace& w, int M, int Tq, PosArg pos, const floa
         LG_PROF(PC_GEMM_HEAD, st, launch_gemv_small(gh, st));
         return 0;
     }
+    LG_TRY(run_layers(w, M, Tq, pos, emb_mask, B, xn_ready, st));
+    // head on the last position only (generate.py:58 reads logits[:, -1])
+    const void* xlast = w.xn;
+    if (Tq > 1) {
+        LG_TRY(launch_gather_last(w.xn, R, Tq, D, dt, w.q, st));
+        xlast = w.q;
+    }
+    prof_begin(PC_GEMM_HEAD, st);
+    GemmNext nx_first{layers[0].wqkv, (size_t)3 * D * D * esz, nullptr, 0};   // the next decode step starts with layer 0
+    const int direct = gemm(w, xlast, R, V, D, output, nullptr, 0, &ks, logits_out, st, &nx_first);
+    prof_end(st);
+    if (direct < 0) return direct;
+    if (direct == 0) LG_TRY(launch_reduce_f32(w.partial, ks, R, V, logits_out, st));
+    return 0;
+}
+
+int lg_engine::run_layers(const Workspace& w, int M, int Tq, PosArg pos, const float* emb_mask, int B, bool xn_ready, cudaStream_t st) {
+    const int L = cfg.n_layer, D = cfg.dim, F = cfg.ffn_dim, V = cfg.vocab_size;
+    const int R = M / Tq;
+    const int dt = cfg.dtype;
+    int ks = 1;
     if (!xn_ready) LG_PROF(PC_EMBED_MISC, st, launch_rmsnorm(w.h, layers[0].attn_norm, w.xn, M, D, cfg.norm_eps, dt, st));
     for (int l = 0; l < L; ++l) {
         const Layer& ly = layers[l];
@@ -347,7 +422,7 @@ int lg_engine::forward(const Workspace& w, int M, int Tq, PosArg pos, const floa
         GemmNext nx_w2{ly.w2, (size_t)D * F * eb, nullptr, 0};
         GemmNext nx_qkv{(l + 1 < L) ? layers[l + 1].wqkv : output, (l + 1 < L) ? (size_t)3 * D * D * eb : (size_t)V * D * eb, nullptr, 0};
         LG_PROF(PC_GEMM_QKV, st, gemm(w, w.xn, M, 3 * D, D, ly.wqkv, nullptr, 0, &ks, nullptr, st, &nx_wo));
-        AttnArgs aa = layer_attn(l);
+        AttnArgs aa = layer_attn(w, l, R, Tq, pos, emb_mask, B);
         // decode steps on the TMA path: the attention kernel is also the QKV epilogue (one dependent kernel less)
         const bool fuse_qkv = lg_env_flag("LG_FUSE_QKV", 1) && attn_tma_enabled() && attn_tma_supported(aa);
         if (fuse_qkv) {
@@ -364,18 +439,6 @@ int lg_engine::forward(const Workspace& w, int M, int Tq, PosArg pos, const floa
         const void* next_norm = (l + 1 < L) ? layers[l + 1].attn_norm : final_norm;
         LG_PROF(PC_RESNORM, st, launch_residual_norm(w.partial, ks, M, D, w.h, next_norm, w.xn, cfg.norm_eps, dt, st));
     }
-    // head on the last position only (generate.py:58 reads logits[:, -1])
-    const void* xlast = w.xn;
-    if (Tq > 1) {
-        LG_TRY(launch_gather_last(w.xn, R, Tq, D, dt, w.q, st));
-        xlast = w.q;
-    }
-    prof_begin(PC_GEMM_HEAD, st);
-    GemmNext nx_first{layers[0].wqkv, (size_t)3 * D * D * esz, nullptr, 0};   // the next decode step starts with layer 0
-    const int direct = gemm(w, xlast, R, V, D, output, nullptr, 0, &ks, logits_out, st, &nx_first);
-    prof_end(st);
-    if (direct < 0) return direct;
-    if (direct == 0) LG_TRY(launch_reduce_f32(w.partial, ks, R, V, logits_out, st));
     return 0;
 }
 
@@ -641,6 +704,86 @@ int lg_decode_rows(lg_engine* e, const int32_t* tokens, const int32_t* pos_rows,
     return 0;
 }
 
+int lg_score_workspace_bytes(lg_engine* e, int rows, int seq, size_t* bytes) {
+    LG_REQUIRE(e && bytes && rows > 0 && seq > 0, "lg_score_workspace_bytes: bad argument");
+    LG_REQUIRE(seq >= e->cfg.cls_token_num && seq <= e->cfg.cls_token_num + e->cfg.block_size - 1,
+               "lg_score_workspace_bytes: seq %d outside [cls_token_num, cls_token_num + block_size - 1] = [%d, %d]", seq,
+               e->cfg.cls_token_num, e->cfg.cls_token_num + e->cfg.block_size - 1);
+    Workspace tmp;
+    *bytes = e->carve_score(tmp, nullptr, rows, seq);
+    return 0;
+}
+
+int lg_score(lg_engine* e, const void* cond, const float* emb_mask, const int32_t* idx, const int32_t* targets, int B, int T, int S,
+             int use_cfg, float cfg_scale, void* dev_ws, size_t ws_bytes, float* logits_out, float* nll_out, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    LG_REQUIRE(e && e->finalized, "lg_score: engine not finalized");
+    DeviceGuard guard(e->device);
+    const lg_model_cfg& c = e->cfg;
+    LG_REQUIRE(cond && B > 0, "lg_score: null cond or B=%d", B);
+    LG_REQUIRE(T == c.cls_token_num, "lg_score: T=%d must equal cls_token_num=%d", T, c.cls_token_num);
+    LG_REQUIRE(S >= 1 && S <= c.block_size, "lg_score: S=%d outside [1, block_size=%d]", S, c.block_size);
+    LG_REQUIRE((idx == nullptr) == (S == 1), "lg_score: idx must be NULL exactly when S == 1 (S=%d)", S);
+    LG_REQUIRE(logits_out || nll_out, "lg_score: nothing to write (logits_out and nll_out are both NULL)");
+    LG_REQUIRE(!nll_out || targets, "lg_score: nll_out needs targets");
+    LG_REQUIRE(!emb_mask || c.model_type == LG_MODEL_T2I, "lg_score: emb_mask only applies to t2i models");
+    LG_REQUIRE(!use_cfg || std::isfinite(cfg_scale), "lg_score: cfg_scale %g is not finite", (double)cfg_scale);
+    LG_REQUIRE(dev_ws && ((uintptr_t)dev_ws & 255) == 0, "lg_score: scratch must be non-null and 256-byte aligned");
+    const int nh = use_cfg ? 2 : 1, seq = T + S - 1, D = c.dim, V = c.vocab_size, dt = c.dtype;
+    // images per chunk: the scratch bounds it, and so does attention_kernel's grid (R * seq <= 65535 query rows) when the sequence
+    // is not on a tensor-core path (fp32 models, or LG_ATTN_TMA=0)
+    auto fits = [&](int nb) {
+        Workspace w;
+        if (e->carve_score(w, (char*)dev_ws, nh * nb, seq) > ws_bytes) return false;
+        if ((long long)nh * nb * seq <= 65535) return true;
+        if (e->make_maps(w) != 0) return false;
+        const AttnArgs aa = e->attn_args(w, 0, nh * nb, seq);
+        return attn_tma_enabled() && (attn_causal_tc_supported(aa) || attn_prefill_tc_supported(aa) || attn_tma_supported(aa));
+    };
+    {
+        Workspace one;
+        const size_t need1 = e->carve_score(one, nullptr, nh, seq);
+        LG_REQUIRE(ws_bytes >= need1, "lg_score: scratch of %zu bytes is too small for one image (%zu)", ws_bytes, need1);
+    }
+    int lo = 1, hi = B;   // largest chunk that fits
+    while (lo < hi) {
+        const int mid = lo + (hi - lo + 1) / 2;
+        if (fits(mid)) lo = mid; else hi = mid - 1;
+    }
+    LG_REQUIRE(fits(lo), "lg_score: no chunk of images fits the scratch (%zu bytes) and the attention grid", ws_bytes);
+    const size_t esz = e->esz;
+    for (int b0 = 0; b0 < B; b0 += lo) {
+        const int nb = std::min(lo, B - b0), R = nh * nb;
+        Workspace w;
+        e->carve_score(w, (char*)dev_ws, R, seq);
+        LG_TRY(e->make_maps(w));
+        // K / V rows past the sequence and dims hd..hdp-1 are never written; the tensor-core attention multiplies them by exact zeros
+        LG_CUDA_OK(cudaMemsetAsync(w.kcache, 0, w.cache_bytes, st));
+        const void* cond_c = c.model_type == LG_MODEL_C2I ? (const void*)((const int32_t*)cond + b0)
+                                                          : (const void*)((const char*)cond + (size_t)b0 * T * c.caption_dim * esz);
+        const float* em = emb_mask ? emb_mask + (size_t)b0 * T : nullptr;
+        Workspace wc = w;   // the condition rows [R * T, D] go to ff first, then the sequence embedding assembles h
+        wc.h = w.ff;
+        LG_TRY(e->embed_cond(wc, cond_c, nb, R, T, st));
+        LG_TRY(launch_embed_seq(w.ff, e->tok_emb, idx ? idx + (size_t)b0 * (S - 1) : nullptr, nb, R, T, seq, D, dt, w.h, st));
+        LG_TRY(e->run_layers(w, R * seq, seq, PosArg{nullptr, 0}, em, nb, false, st));
+        LG_TRY(launch_gather_scored(w.xn, nb, nh, seq, T, S, D, dt, w.q, st));
+        // the head in chunks of at most w.head_rows rows (a CFG pair never splits)
+        const int P = nb * S, per = std::max(1, w.head_rows / nh);
+        for (int p0 = 0; p0 < P;) {
+            int np = std::min(per, P - p0);
+            while (np > 1 && gemm_partial_floats(np * nh, V, D, dt) > w.partial_floats) np /= 2;   // the GEMM plan is not monotone in M
+            int ks = 1;
+            LG_TRY(e->gemm(w, (const char*)w.q + (size_t)p0 * nh * D * esz, np * nh, V, D, e->output, nullptr, 0, &ks, nullptr, st));
+            const size_t g0 = (size_t)b0 * S + p0;
+            LG_TRY(launch_score_head(w.partial, ks, np, V, nh, cfg_scale, dt, targets ? targets + g0 : nullptr,
+                                     logits_out ? logits_out + g0 * V : nullptr, nll_out ? nll_out + g0 : nullptr, st));
+            p0 += np;
+        }
+    }
+    return 0;
+}
+
 int lg_sample_rows(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc, const uint64_t* seed_rows,
                    const int32_t* step_rows, int32_t* out_idx, int32_t* out_seq, int seq_stride, void* stream) {
     LG_REQUIRE(logits && sc && seed_rows && step_rows && (out_idx || out_seq), "lg_sample_rows: null argument");
@@ -880,7 +1023,7 @@ int lg_test_attention(int dtype, int kv_dtype, float k_scale, float v_scale, int
                dtype);
     LG_REQUIRE(f8 ? kv_scale_ok(k_scale) && kv_scale_ok(v_scale) : k_scale == 1.f && v_scale == 1.f,
                "lg_test_attention: K / V scales %g / %g (fp8: powers of two in [2^-8, 2^7], otherwise 1)", (double)k_scale, (double)v_scale);
-    LG_REQUIRE(R > 0 && Tq > 0 && H > 0 && max_seq > 0 && n_layer > 0 && layer >= 0 && layer < n_layer && (long long)R * Tq <= 65535,
+    LG_REQUIRE(R > 0 && Tq > 0 && H > 0 && max_seq > 0 && n_layer > 0 && layer >= 0 && layer < n_layer,
                "lg_test_attention: bad shape R=%d Tq=%d H=%d max_seq=%d layer %d of %d", R, Tq, H, max_seq, layer, n_layer);
     LG_REQUIRE(hd == 64 || hd == 100 || hd == 128, "lg_test_attention: unsupported head_dim %d (64, 100, 128)", hd);
     LG_REQUIRE(hdp == attn_kv_row_width(dtype, hd), "lg_test_attention: row width %d for head_dim %d", hdp, hd);
@@ -904,6 +1047,8 @@ int lg_test_attention(int dtype, int kv_dtype, float k_scale, float v_scale, int
     aa.q = q ? q : q_out; aa.out = out;
     aa.pos = PosArg{pos_dev, pos_value, pos_rows};
     aa.emb_mask = emb_mask; aa.B = emb_mask ? B : 1; aa.Tc = emb_mask ? Tc : 0;
+    LG_REQUIRE((long long)R * Tq <= 65535 || (attn_tma_enabled() && attn_causal_tc_supported(aa)),
+               "lg_test_attention: bad shape R=%d Tq=%d: more than 65535 query rows need the causal tensor-core kernel", R, Tq);
     if (qkv_partial) {
         if (fuse) {
             LG_REQUIRE(attn_tma_enabled() && attn_tma_supported(aa), "lg_test_attention: the fused QKV epilogue needs the TMA decode kernel");
@@ -918,21 +1063,19 @@ int lg_test_attention(int dtype, int kv_dtype, float k_scale, float v_scale, int
 }  // extern "C"
 
 namespace {
-__global__ void round_bf16_kernel(float* p, size_t n) {
+// the 16-bit head's logits as the reference materialises them (gpt.py:368: `.float()` of a bf16 / fp16 tensor); past +-65504 an fp16
+// logit becomes +-inf, like torch's fp16 head
+template <typename T>
+__global__ void round_logits_kernel(float* p, size_t n) {
     lg_pdl_sync();
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-        p[i] = round_bf16(p[i]);
-}
-__global__ void round_f16_kernel(float* p, size_t n) {
-    lg_pdl_sync();
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-        p[i] = ElemTraits<f16>::round(p[i]);   // past +-65504 -> +-inf, like torch's fp16 head
+        p[i] = ElemTraits<T>::round(p[i]);
 }
 }  // namespace
 static int round_logits_inplace(float* logits, size_t n, int dtype, cudaStream_t st) {
     if (!lg_dtype_is16(dtype)) return 0;
     const int blocks = (int)std::min<size_t>((n + 255) / 256, 132 * 8);
-    (void)lg_launch(dtype == LG_DTYPE_F16 ? round_f16_kernel : round_bf16_kernel, dim3(blocks), dim3(256), 0, st, logits, n);
+    (void)lg_launch(dtype == LG_DTYPE_F16 ? round_logits_kernel<f16> : round_logits_kernel<bf16>, dim3(blocks), dim3(256), 0, st, logits, n);
     LG_LAUNCH_CHECK();
     return 0;
 }

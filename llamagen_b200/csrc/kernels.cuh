@@ -116,6 +116,16 @@ int launch_reduce_f32(const float* partial, int ksplit, int M, int N, float* out
 // gather last-position rows: out[r,:] = in[(r*T + T-1),:]
 int launch_gather_last(const void* in, int R, int T, int D, int dtype, void* out, cudaStream_t st);
 
+// lg_score: h[r, t] = t < T ? cond_rows[r * T + t] : table[idx[r % B][t - T]] over R * seq rows (idx [B][seq - T])
+int launch_embed_seq(const void* cond_rows, const void* table, const int32_t* idx, int B, int R, int T, int seq, int D, int dtype, void* out,
+                     cudaStream_t st);
+// out row (b * S + s) * nh + half = in row (b + half * B) * seq + T - 1 + s (the scored positions of B images, CFG twins adjacent)
+int launch_gather_scored(const void* in, int B, int nh, int seq, int T, int S, int D, int dtype, void* out, cudaStream_t st);
+// P scored positions from the head's split-K slabs [ksplit][P * nh][V]: logits (dtype-rounded, CFG-mixed when nh == 2) -> logits
+// [P][V] (or null), nll[p] = logsumexp - logit[targets[p]] (or null; NaN for a target outside [0, V))
+int launch_score_head(const float* partial, int ksplit, int P, int V, int nh, float cfg_scale, int dtype, const int32_t* targets,
+                      float* logits, float* nll, cudaStream_t st);
+
 struct AttnArgs {
     const void* q;          // [M, D] post-RoPE
     const void* kcache; const void* vcache;   // [R, H, maxS, hd]
@@ -141,7 +151,7 @@ struct AttnArgs {
 // KV-cache row width in elements: head_dim 100 of a bf16 / fp16 model (GPT-3B) is stored in 112-wide rows, 16-byte multiples that
 // the TMA attention kernels can stream (dims 100..111 stay zero); every other cache row is hd wide
 inline int attn_kv_row_width(int dtype, int hd) { return hd == 100 && lg_dtype_is16(dtype) ? 112 : hd; }
-// path (optional, int[3]): the kernel that was launched (0 = attention_kernel, 1 = attn_tma_kernel,
+// path (optional, int[3]): the kernel that was launched (0 = attention_kernel, 1 = attn_tma_kernel, 2 = attn_causal_tc_kernel,
 // 3 = attn_prefill_tc_kernel), its TMA ring depth (0 for attention_kernel, 1 for the single-stage prefill) and whether it fused the
 // QKV epilogue
 int launch_attention(const AttnArgs& a, cudaStream_t st, int* path = nullptr);
@@ -161,6 +171,10 @@ int launch_attention_tma(const AttnArgs& a, cudaStream_t st, int* path = nullptr
 // t2i condition prefill (1 < Tq <= 128, hd 64, bf16 / fp16): TMA-staged Q/K/V, mma.sync QK^T and PV, one CTA per (row, head)
 bool attn_prefill_tc_supported(const AttnArgs& a);
 int launch_attention_prefill_tc(const AttnArgs& a, cudaStream_t st, int* path = nullptr);
+// teacher-forced sequences (Tq > 128 queries from position 0, bf16 / fp16 cache in the model dtype, hd 64 / 128 / 100-in-112): a CTA
+// per (head, row, 64-query block), K / V blocks through a TMA ring, mma.sync QK^T and PV with an online softmax
+bool attn_causal_tc_supported(const AttnArgs& a);
+int launch_attention_causal_tc(const AttnArgs& a, cudaStream_t st, int* path = nullptr);
 // VQ convolutions: vq.cu runs them; conv_tc.cu holds the wgmma kernels and chooses the kernel of each call.
 // GroupNorm(32) partial statistics are [B][splits][32 groups][sum, sum of squares] floats. gn_stats_kernel writes at most
 // kGnStatsMaxSplits splits per image; the drain of conv_tcw_kernel writes one per 16x16-pixel tile (and upsample phase) of its input.

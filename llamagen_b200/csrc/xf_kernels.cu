@@ -352,6 +352,65 @@ __global__ void __launch_bounds__(256) attention_kernel(AttnArgs a) {
     }
 }
 
+// ---------------------------------------------------------------- teacher-forced scoring (lg_score)
+// h[r, t] = t < T ? the condition embedding cond[r, t] ([R * T, D]) : tok_emb[idx[r % B, t - T]]  (gpt.py:342-344, CFG twins share idx)
+template <typename T>
+__global__ void embed_seq_kernel(const T* __restrict__ cond, const T* __restrict__ table, const int32_t* __restrict__ idx, int B, int T_,
+                                 int seq, int D, T* __restrict__ out) {
+    lg_pdl_sync();
+    const int row = blockIdx.x, r = row / seq, t = row - r * seq;
+    const T* s = t < T_ ? cond + ((size_t)r * T_ + t) * D : table + (size_t)idx[(size_t)(r % B) * (seq - T_) + (t - T_)] * D;
+    T* d = out + (size_t)row * D;
+    for (int i = threadIdx.x; i < D; i += blockDim.x) d[i] = s[i];
+}
+
+// out row (b * S + s) * nh + half = in row (b + half * B) * seq + T - 1 + s: the scored positions, CFG twins adjacent
+template <typename T>
+__global__ void gather_scored_kernel(const T* __restrict__ in, int B, int nh, int seq, int T_, int S, int D, T* __restrict__ out) {
+    lg_pdl_sync();
+    const int o = blockIdx.x, half = o % nh, p = o / nh, b = p / S, s = p - b * S;
+    const T* src = in + ((size_t)(b + half * B) * seq + T_ - 1 + s) * D;
+    T* d = out + (size_t)o * D;
+    for (int i = threadIdx.x; i < D; i += blockDim.x) d[i] = src[i];
+}
+
+constexpr int kScoreThreads = 512;
+// One CTA per scored position p (head rows p * nh .. p * nh + nh - 1 of the split-K slabs): the logit the reference materialises
+// (rounded to T like round_logits_inplace), CFG-mixed as generate.py:79-82 / sampling.cu mix it when nh == 2, written to logits
+// when asked, then nll = logsumexp - logit[target] in fp32 (F.cross_entropy, gpt.py:378).
+template <typename T>
+__global__ void __launch_bounds__(kScoreThreads) score_head_kernel(const float* __restrict__ partial, int ks, int Mh, int V, int nh,
+                                                                   float cfg_scale, const int32_t* __restrict__ targets,
+                                                                   float* __restrict__ logits, float* __restrict__ nll) {
+    lg_pdl_sync();
+    __shared__ float red[33];
+    const int p = blockIdx.x;
+    const size_t slab = (size_t)Mh * V;
+    const float* pc = partial + (size_t)p * nh * V;
+    auto logit = [&](int v) {
+        const float c = TR<T>::round(sum_partials(pc, v, ks, slab));
+        if (nh == 1) return c;
+        const float u = TR<T>::round(sum_partials(pc + V, v, ks, slab));
+        return __fadd_rn(u, __fmul_rn(__fsub_rn(c, u), cfg_scale));
+    };
+    float* lrow = logits ? logits + (size_t)p * V : nullptr;
+    float m = -INFINITY, sum = 0.f;
+    for (int v = threadIdx.x; v < V; v += kScoreThreads) {
+        const float x = logit(v);
+        if (lrow) lrow[v] = x;
+        if (x > m) { sum = sum * expf(m - x) + 1.f; m = x; }
+        else if (x != -INFINITY) sum += expf(x - m);
+    }
+    if (!nll) return;
+    // merge the threads' (max, sum) pairs: block max first, then the rescaled sums
+    const float M_ = block_max(m, red);
+    const float total = block_sum(m == -INFINITY ? 0.f : sum * expf(m - M_), red);
+    if (threadIdx.x == 0) {
+        const int tg = targets[p];
+        nll[p] = (tg >= 0 && tg < V) ? M_ + logf(total) - logit(tg) : __int_as_float(0x7fc00000);
+    }
+}
+
 __global__ void advance_kernel(int* pos, int* step) {
     lg_pdl_sync();
     if (pos) *pos += 1;
@@ -505,6 +564,7 @@ static int launch_attention_t(const AttnArgs& a, cudaStream_t st) {
 int launch_attention(const AttnArgs& a, cudaStream_t st, int* path) {
     if (attn_tma_supported(a) && attn_tma_enabled()) return launch_attention_tma(a, st, path);
     if (attn_prefill_tc_supported(a) && attn_tma_enabled() && a.qkv_partial == nullptr) return launch_attention_prefill_tc(a, st, path);
+    if (attn_causal_tc_supported(a) && attn_tma_enabled() && a.qkv_partial == nullptr) return launch_attention_causal_tc(a, st, path);
     LG_REQUIRE(a.qkv_partial == nullptr, "attention: fused QKV epilogue requested on a path that does not support it");
     set_attn_path(path, 0, 0, 0);
     LG_REQUIRE((long long)a.R * a.Tq <= 65535, "attention: too many query rows (%d x %d)", a.R, a.Tq);
@@ -535,6 +595,40 @@ int launch_attention(const AttnArgs& a, cudaStream_t st, int* path) {
         if (a.hd == 100) return launch_attention_t<float, 100, 4, 32>(a, st);
     }
     return lg_fail("attention: unsupported head_dim %d / dtype %d (supported: 64, 100, 128)", a.hd, a.dtype);
+}
+
+int launch_embed_seq(const void* cond_rows, const void* table, const int32_t* idx, int B, int R, int T, int seq, int D, int dtype, void* out,
+                     cudaStream_t st) {
+    return dispatch_dtype(
+        dtype, [&](auto z) {
+            using E = decltype(z);
+            (void)lg_launch(embed_seq_kernel<E>, dim3(R * seq), dim3(128), 0, st, (const E*)cond_rows, (const E*)table, idx, B, T, seq, D,
+                            (E*)out);
+            LG_LAUNCH_CHECK();
+            return 0;
+        });
+}
+
+int launch_gather_scored(const void* in, int B, int nh, int seq, int T, int S, int D, int dtype, void* out, cudaStream_t st) {
+    return dispatch_dtype(
+        dtype, [&](auto z) {
+            using E = decltype(z);
+            (void)lg_launch(gather_scored_kernel<E>, dim3(B * S * nh), dim3(128), 0, st, (const E*)in, B, nh, seq, T, S, D, (E*)out);
+            LG_LAUNCH_CHECK();
+            return 0;
+        });
+}
+
+int launch_score_head(const float* partial, int ksplit, int P, int V, int nh, float cfg_scale, int dtype, const int32_t* targets,
+                      float* logits, float* nll, cudaStream_t st) {
+    return dispatch_dtype(
+        dtype, [&](auto z) {
+            using E = decltype(z);
+            (void)lg_launch(score_head_kernel<E>, dim3(P), dim3(kScoreThreads), 0, st, partial, ksplit, P * nh, V, nh, cfg_scale, targets,
+                            logits, nll);
+            LG_LAUNCH_CHECK();
+            return 0;
+        });
 }
 
 int launch_advance(int* pos, int* step, cudaStream_t st) {

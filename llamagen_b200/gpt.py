@@ -77,6 +77,41 @@ def rope_table_2d(grid_size: int, head_dim: int, base: float, cls_token_num: int
     return torch.cat([torch.zeros(cls_token_num, head_dim // 2, 2), table]).contiguous()
 
 
+SCORE_SCRATCH_CAP = 4 << 30   # bytes of lg_score scratch a model keeps; a batch that needs more is scored in image chunks
+
+
+def t2i_attn_mask(emb_masks: torch.Tensor, seq: int) -> torch.Tensor:
+    """bool [B, seq, seq]: the attention mask dataset/t2i.py:123-128 builds from emb_masks [B, T] (tril, condition columns times
+    emb_mask, unit diagonal); slicing the dataset's [:-1, :-1] gives the same matrix at seq = max_seq_length - 1."""
+    B, T = emb_masks.shape
+    m = torch.tril(torch.ones(seq, seq, device=emb_masks.device)).repeat(B, 1, 1)
+    m[:, :, :T] = m[:, :, :T] * emb_masks.float()[:, None, :]
+    eye = torch.eye(seq, device=emb_masks.device)
+    return (m * (1 - eye) + eye).bool()
+
+
+def emb_mask_from_attn_mask(mask: torch.Tensor, T: int) -> torch.Tensor:
+    """emb_masks [B, T] (float) of a dataset-style t2i attention mask ([B, 1, seq, seq] or [B, seq, seq], any dtype, nonzero =
+    visible): read from the last query row, then checked on the mask's device against the mask rebuilt from them. Any other
+    mask raises ValueError: the engine's attention implements only this rule."""
+    m = mask
+    if m.dim() == 4:
+        if m.shape[1] != 1:
+            raise ValueError(f"the attention mask must be [B, 1, seq, seq] (one mask for every head), got {tuple(m.shape)}")
+        m = m[:, 0]
+    if m.dim() != 3 or m.shape[1] != m.shape[2] or m.shape[1] < T:
+        raise ValueError(f"the attention mask must be [B, seq, seq] with seq >= {T}, got {tuple(mask.shape)}")
+    m = m != 0
+    seq = m.shape[1]
+    emb = m[:, -1, :T].float()
+    if seq == T:
+        emb[:, T - 1] = 1.0     # the last condition column is then only seen from its own row, through the unit diagonal
+    if not torch.equal(t2i_attn_mask(emb, seq), m):
+        raise ValueError("unsupported attention mask: only the t2i dataset's causal mask with per-image condition padding "
+                         "(dataset/t2i.py:123-128) is implemented")
+    return emb
+
+
 class _Group(nn.Module):
     """Bare namespace so parameters get the reference's dotted names."""
 
@@ -158,6 +193,7 @@ class Transformer(nn.Module):
         self._workspace = None
         self._ws_shape = (0, 0)
         self._kv_cache = ("auto", None)
+        self._score_ws = None
         self.requires_grad_(False)
 
     # ------------------------------------------------------------------ engine plumbing
@@ -254,16 +290,95 @@ class Transformer(nn.Module):
         self.max_batch_size = max_batch_size
         self.max_seq_length = max_seq_length
 
+    # ------------------------------------------------------------------ teacher-forced scoring (lg_score)
+    def _score_scratch(self, rows: int, seq: int, nh: int):
+        """The lg_score scratch for `rows` sequences of `seq` positions, capped at SCORE_SCRATCH_CAP bytes (the engine then scores
+        the batch in image chunks); kept on the model like the setup_caches() workspace. Returns (device pointer, bytes)."""
+        lib, handle = _lib.load(), self.engine()
+        need, one = ctypes.c_size_t(), ctypes.c_size_t()
+        _lib.check(lib.lg_score_workspace_bytes(handle, rows, seq, ctypes.byref(need)), "lg_score_workspace_bytes")
+        _lib.check(lib.lg_score_workspace_bytes(handle, nh, seq, ctypes.byref(one)), "lg_score_workspace_bytes")
+        nbytes = need.value if need.value <= SCORE_SCRATCH_CAP else max(SCORE_SCRATCH_CAP, one.value)
+        dev = self.tok_embeddings.weight.device
+        if self._score_ws is None or self._score_ws.numel() < nbytes + 256 or self._score_ws.device != dev:
+            self._score_ws = None
+            self._score_ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=dev)
+        base = (self._score_ws.data_ptr() + 255) // 256 * 256
+        return ctypes.c_void_p(base), self._score_ws.numel() - (base - self._score_ws.data_ptr())
+
+    def _score(self, cond, idx, targets, emb_masks, cfg_scale: float, want_logits: bool, want_nll: bool):
+        """lg_score over complete sequences: cond (c2i labels [B] / t2i features [B, T, C]), idx [B, S-1] or None (S = 1),
+        targets [B, S] or None. Returns (logits fp32 [B, S, V] or None, nll fp32 [B, S] or None)."""
+        lib, handle = _lib.load(), self.engine()
+        dev = self.tok_embeddings.weight.device
+        if self.model_type == "c2i":
+            cond_dev = cond.to(device=dev, dtype=torch.int32).contiguous()
+            if cond_dev.dim() != 1:
+                raise ValueError("c2i cond must be a 1-D tensor of class labels")
+            T = 1
+        else:
+            cond_dev = cond[:, : self.cls_token_num].to(device=dev, dtype=self.tok_embeddings.weight.dtype).contiguous()
+            T = cond_dev.shape[1]
+        B = cond_dev.shape[0]
+        S = 1 if idx is None else idx.shape[1] + 1
+        if idx is not None and tuple(idx.shape) != (B, S - 1):
+            raise ValueError(f"idx must be [B, S-1] = [{B}, {S - 1}], got {tuple(idx.shape)}")
+        if not 1 <= S <= self.block_size:
+            raise ValueError(f"a scored sequence holds 1 .. block_size={self.block_size} tokens, got {S}")
+        V = self.vocab_size
+        idx_dev = idx.to(device=dev, dtype=torch.int32).contiguous() if idx is not None else None
+        tgt = None
+        if targets is not None:
+            tgt = targets.to(device=dev, dtype=torch.int64)
+            if tuple(tgt.shape) != (B, S):
+                raise ValueError(f"targets must be [B, S] = [{B}, {S}], got {tuple(tgt.shape)}")
+            if bool(((tgt < 0) | (tgt >= V)).any()):
+                raise ValueError(f"targets must lie in [0, vocab_size={V})")
+            tgt = tgt.to(torch.int32).contiguous()
+        em = None
+        if emb_masks is not None:
+            if tuple(emb_masks.shape) != (B, T):
+                raise ValueError(f"emb_masks must be [B, T] = [{B}, {T}], got {tuple(emb_masks.shape)}")
+            em = emb_masks.to(device=dev, dtype=torch.float32).contiguous()
+        use_cfg = cfg_scale > 1.0                               # generate.py:128
+        nh = 2 if use_cfg else 1
+        logits = torch.empty(B, S, V, dtype=torch.float32, device=dev) if want_logits else None
+        nll = torch.empty(B, S, dtype=torch.float32, device=dev) if want_nll else None
+        ws, ws_bytes = self._score_scratch(nh * B, T + S - 1, nh)
+        _lib.check(lib.lg_score(handle, _lib.ptr(cond_dev), _lib.ptr(em), _lib.ptr(idx_dev), _lib.ptr(tgt), B, T, S, int(use_cfg),
+                                float(cfg_scale), ws, ws_bytes, _lib.ptr(logits), _lib.ptr(nll), _lib.current_stream(dev)),
+                   "lg_score")
+        return logits, nll
+
     # ------------------------------------------------------------------ reference-style forward
     def forward(self, idx, cond_idx, input_pos=None, targets=None, mask=None, valid=None, emb_masks=None):
-        """Inference branches of Transformer.forward (gpt.py:348-368) through the engine.
+        """Transformer.forward (gpt.py:341-382) through the engine, eval mode (no dropout).
 
+        teacher-forced: idx [B, L] and cond_idx given -> (fp32 logits [B, L + 1, V] of positions cls_token_num - 1 .. (the
+                 training branch's logits[:, cls_token_num - 1:]), loss): the mean cross entropy over targets [B, L + 1], or its
+                 `valid`-weighted mean. t2i: emb_masks [B, T], or the dataset's attention `mask` ([B, 1, seq, seq] or [B, seq, seq],
+                 dataset/t2i.py:123-128 sliced [:-1, :-1]) from which they are derived. Needs no setup_caches().
         prefill: idx=None, cond_idx given  -> fp32 logits [rows, 1, V] of the LAST condition position
                  (the only one generate() reads, generate.py:58; the reference materialises all T).
         decode : idx [rows, 1], cond_idx=None, input_pos=[p] -> fp32 logits [rows, 1, V].
         rows are taken as given (the caller has already doubled them for CFG, as in the reference)."""
-        if targets is not None or (idx is not None and cond_idx is not None):
-            raise NotImplementedError("training / teacher-forced full-sequence forward is outside the sampling hot path")
+        if idx is not None and cond_idx is not None:
+            if mask is not None:
+                if emb_masks is not None:
+                    raise ValueError("pass either mask or emb_masks, not both")
+                if self.model_type != "t2i":
+                    raise ValueError("an attention mask applies to t2i models only (c2i sequences are plain causal)")
+                emb_masks = emb_mask_from_attn_mask(mask, self.cls_token_num)
+            logits, nll = self._score(cond_idx, idx, targets, emb_masks, 1.0, True, targets is not None)
+            loss = None
+            if valid is not None:                               # gpt.py:373-376
+                w = valid.to(device=nll.device, dtype=torch.float32)[:, None].repeat(1, nll.shape[1]).reshape(-1)
+                loss = (nll.reshape(-1) * w).sum() / torch.clamp(w.sum(), min=1.0)
+            elif targets is not None:                           # gpt.py:377-378
+                loss = nll.mean()
+            return logits, loss
+        if targets is not None:
+            raise ValueError("targets need both idx and cond_idx (the teacher-forced forward)")
         if self.max_batch_size < 0:
             raise _lib.LgError("call setup_caches() before forward() (as generate() does)")
         lib, handle = _lib.load(), self.engine()
