@@ -145,6 +145,30 @@ int  lg_score_workspace_bytes(lg_engine* e, int rows, int seq, size_t* bytes);
 int  lg_score(lg_engine* e, const void* cond, const float* emb_mask, const int32_t* idx, const int32_t* targets, int B, int T, int S,
               int use_cfg, float cfg_scale, void* dev_ws, size_t ws_bytes, float* logits_out, float* nll_out, void* stream);
 
+/* ---- speculative Jacobi decoding (Teng et al. 2024): up to L tokens per forward pass, same distribution as lg_generate ------------ */
+/* Bytes of caller-provided scratch for lg_generate_sjd with B images and window L (use_cfg: rows doubled). */
+int  lg_sjd_workspace_bytes(lg_engine* e, int B, int use_cfg, int L, size_t* bytes);
+/* generate() with a window of L tokens per pass (2 <= L <= 64, L <= S - 1). Token 0 is drawn by the prefill exactly as lg_generate
+ * draws it. Each pass feeds image b's last final token and L - 1 drafts at positions T + s_b - 1 .. T + s_b + L - 2 (s_b: the first
+ * token index the window predicts; near the end of the sequence the window is held at s_b = S - L and re-feeds final tokens), then:
+ *   accept: for token k = n_b, ... (n_b tokens final) in order, draft d_k is accepted iff u_acc(k) * q_k(d_k) < p_k(d_k), q_k the
+ *     distribution it was drawn from; the first rejected k is drawn from normalize(max(0, p_k - q_k)) with u_res(k) by inverse CDF
+ *     (an all-zero residual takes x_k, the redraw below); with every draft accepted, the bonus token s_b + L - 1 is x of that slot.
+ *     Greedy (sc->greedy): accept iff d_k = argmax p_k; a rejected k and the bonus token take argmax p.
+ *   refresh: a draft whose p this pass computed becomes x_k (q_k = p_k); a new index k takes floor(u_init(k) * V) (q = 1 / V).
+ * p_k is the distribution lg_generate samples token k from (rounding, CFG mix with cfg_interval by token index, temperature, top-k,
+ * top-p). x_k is the sample kernel's own draw from p_k (lg_sample_rows with seed_rows = pass_seed(b, pass), step_rows = k; argmax when
+ * greedy). With C1 = 0xA0761D6478BD642F, C2 = 0xE7037ED1A0B428DB, C3 = 0x8EBC6AF09C88C6E3, C4 = 0x9E6C63D0676A9A99,
+ * C5 = 0xD6E8FEB86659FD93 and splitmix64 as in lg_sample, all arithmetic mod 2^64:
+ *   u_purpose(k) = top 24 bits of sm(sm(sm(seed ^ C1 (k + 1)) ^ C2 (b + 1)) ^ C3 purpose) / 2^24, purpose accept 1, residual 2, init 3
+ *   pass_seed(b, pass) = sm(sm(seed ^ C4 (b + 1)) ^ C5 (pass + 1)), pass = 0, 1, ... counting the passes.
+ * A finished image's rows keep running; their outputs are unused. out_tokens dev int32 [B, S]; iters_out dev int32 [1]: the passes run.
+ * dbg_probs: NULL or dev f32 [S - 1][B][L][V], pass j's p rows at [j] (rows of finished images unspecified). Uses the KV cache of
+ * lg_engine_set_workspace (rows >= R, max_seq >= T + S) and dev_ws (lg_sjd_workspace_bytes, 256-byte aligned) for everything else.
+ * The host waits for each pass's done flag before it decides on launching the one after next. */
+int  lg_generate_sjd(lg_engine* e, const void* cond, const float* emb_mask, int B, int T, int S, const lg_sample_cfg* sc, int L,
+                     void* dev_ws, size_t ws_bytes, int32_t* out_tokens, int32_t* iters_out, float* dbg_probs, void* stream);
+
 /* ---- VQ tokenizer: replaces VQModel.decode_code / VectorQuantizer (vq_model.py) ------------------- */
 typedef struct lg_vq_cfg {
     int32_t codebook_size;
@@ -223,13 +247,19 @@ int  lg_test_gemm(const void* x, const void* w, int M, int N, int K, int dtype, 
  * freqs (dev f32 [max_seq][hd / 2][2]): fuse = 0 runs the QKV epilogue (q -> q_out, K / V rows written at the query positions) and
  * then the attention; fuse = 1 lets the TMA decode kernel do the epilogue itself (Tq = 1). out: dev [R * Tq][H * hd].
  * path (int[3]) or NULL: kernel (0 = attention_kernel, 1 = attn_tma_kernel, 2 = attn_causal_tc_kernel: Tq > 128 from position 0 on a
- * 16-bit cache in the model dtype, 3 = attn_prefill_tc_kernel), TMA ring depth (0 for attention_kernel) and whether the QKV epilogue
+ * 16-bit cache in the model dtype, 3 = attn_prefill_tc_kernel, 4 = attn_window_tc_kernel: 2 <= Tq <= 64 at pos_rows on such a cache),
+ * TMA ring depth (0 for attention_kernel) and whether the QKV epilogue
  * was fused. R * Tq may exceed 65535 only on kernel 2. Every argument is checked before any launch;
  * the caller keeps *pos_dev + pos_value + Tq <= max_seq and pos_rows[r] < max_seq. */
 int  lg_test_attention(int dtype, int kv_dtype, float k_scale, float v_scale, int R, int Tq, int H, int hd, int hdp, int max_seq,
                        void* kcache, void* vcache, int n_layer, int layer, int pos_value, const int32_t* pos_dev,
                        const int32_t* pos_rows, const float* emb_mask, int B, int Tc, const void* q, const float* qkv_partial,
                        int ksplit, const float* freqs, int fuse, void* q_out, void* out, int* path, void* stream);
+
+/* The acceptance step of lg_generate_sjd alone, on caller buffers (dev): p, q f32 [B * L][V], qflag, x, win int32 [B * L], nfin,
+ * start int32 [B] (updated), out int32 [B][S] (accepted tokens written). Every image must have nfin < S. */
+int  lg_test_sjd_verify(int B, int S, int L, int V, int greedy, uint64_t seed, const float* p, const float* q, const int32_t* qflag,
+                        const int32_t* x, const int32_t* win, int32_t* nfin, int32_t* start, int32_t* out, void* stream);
 
 /* One VQ decoder/encoder convolution through the decoder's own dispatch (the mma.sync gather kernel or either wgmma kernel,
  * honouring LG_CONV_TC, LG_CONV_SWAP, LG_GN_FUSE and the CTA budget), optionally followed by GroupNorm(32, eps 1e-6)

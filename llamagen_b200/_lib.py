@@ -74,6 +74,11 @@ SIGNATURES = {
     "lg_score_workspace_bytes": (c_int, [c_void_p, c_int, c_int, POINTER(c_size_t)]),
     "lg_score": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_size_t,
                          c_void_p, c_void_p, c_void_p]),
+    "lg_sjd_workspace_bytes": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(c_size_t)]),
+    "lg_generate_sjd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(SampleCfg), c_int, c_void_p, c_size_t,
+                                c_void_p, c_void_p, c_void_p, c_void_p]),
+    "lg_test_sjd_verify": (c_int, [c_int, c_int, c_int, c_int, c_int, c_uint64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                   c_void_p, c_void_p, c_void_p, c_void_p]),
     "lg_vq_create": (c_int, [POINTER(VqCfg), c_int, POINTER(c_void_p)]),
     "lg_vq_destroy": (None, [c_void_p]),
     "lg_vq_bind_weight": (c_int, [c_void_p, c_char_p, c_void_p, POINTER(c_int64), c_int]),

@@ -666,9 +666,11 @@ constexpr int kCqRows = 64;       // query rows per CTA
 constexpr int kCqKeys = 64;       // keys per ring stage
 constexpr int kCqStages = 2;
 
-template <typename T, int HD>
-__global__ void __launch_bounds__(128) attn_causal_tc_kernel(const __grid_constant__ CUtensorMap kmap,
-                                                             const __grid_constant__ CUtensorMap vmap, AttnTmaArgs a, int Tq) {
+//
+// The speculative (Jacobi) decoding window runs the same body with a per-row start (attn_window_tc_kernel): row r's Tq <= kCqRows
+// queries sit at positions a.pos_rows[r] + t and attend keys [0, a.pos_rows[r] + t]; q and out stay [R * Tq, D].
+template <typename T, int HD, bool WINDOW>
+__device__ __forceinline__ void causal_tc_body(const CUtensorMap& kmap, const CUtensorMap& vmap, const AttnTmaArgs& a, int Tq) {
     constexpr int NSUB = HD / 64;
     constexpr int SUB_BYTES = kCqKeys * 128;      // [kCqKeys keys][64 dims], 128-byte swizzle
     constexpr int TILE_BYTES = NSUB * SUB_BYTES;
@@ -682,8 +684,6 @@ __global__ void __launch_bounds__(128) attn_causal_tc_kernel(const __grid_consta
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, tg = lane & 3;
     const long long row0 = a.row_base + ((long long)r * a.H + h) * a.maxS;
     const int hdr = a.hd, D = a.H * hdr;
-    const int nkeys = min(q0 + kCqRows, Tq);
-    const int nblk = (nkeys + kCqKeys - 1) / kCqKeys;
 
     if (threadIdx.x == 0) {
         prefetch_map(&kmap);
@@ -693,6 +693,10 @@ __global__ void __launch_bounds__(128) attn_causal_tc_kernel(const __grid_consta
     }
     __syncthreads();
     lg_pdl_sync();                                   // q and the K / V rows were written by the QKV epilogue just before
+    // absolute position of query 0: read after the dependency wait, since the previous iteration's last kernel moves the positions
+    const int p0 = WINDOW ? a.pos_rows[r] : 0;
+    const int nkeys = p0 + min(q0 + kCqRows, Tq);
+    const int nblk = (nkeys + kCqKeys - 1) / kCqKeys;
     auto issue = [&](int kb) {
         const int s = kb % kCqStages;
         uint8_t* kt = tiles + s * 2 * TILE_BYTES;
@@ -737,7 +741,7 @@ __global__ void __launch_bounds__(128) attn_causal_tc_kernel(const __grid_consta
         const int s = kb % kCqStages;
         mbar_wait(&full_bar[s], (uint32_t)((kb / kCqStages) & 1));
         const int j0 = kb * kCqKeys;
-        if (j0 <= q0 + warp * 16 + 15) {             // warp-uniform: some key of the block is at or below this warp's diagonal
+        if (j0 <= p0 + q0 + warp * 16 + 15) {        // warp-uniform: some key of the block is at or below this warp's diagonal
             const uint32_t kt = smem_u32(tiles + s * 2 * TILE_BYTES);
             const uint32_t vt = kt + TILE_BYTES;
             float sc[NT][4];
@@ -760,7 +764,7 @@ __global__ void __launch_bounds__(128) attn_causal_tc_kernel(const __grid_consta
             for (int nt = 0; nt < NT; ++nt) {
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
-                    const int t = (e >> 1) ? t1 : t0, j = j0 + nt * 8 + tg * 2 + (e & 1);
+                    const int t = p0 + ((e >> 1) ? t1 : t0), j = j0 + nt * 8 + tg * 2 + (e & 1);
                     bool vis = j <= t;
                     if (vis && mrow && j < a.Tc && j != t) vis = mrow[j] != 0.f;
                     const float x = vis ? sc[nt][e] * a.scale : -INFINITY;
@@ -827,32 +831,58 @@ __global__ void __launch_bounds__(128) attn_causal_tc_kernel(const __grid_consta
     }
 }
 
+template <typename T, int HD>
+__global__ void __launch_bounds__(128) attn_causal_tc_kernel(const __grid_constant__ CUtensorMap kmap,
+                                                             const __grid_constant__ CUtensorMap vmap, AttnTmaArgs a, int Tq) {
+    causal_tc_body<T, HD, false>(kmap, vmap, a, Tq);
+}
+
+template <typename T, int HD>
+__global__ void __launch_bounds__(128) attn_window_tc_kernel(const __grid_constant__ CUtensorMap kmap,
+                                                             const __grid_constant__ CUtensorMap vmap, AttnTmaArgs a, int Tq) {
+    causal_tc_body<T, HD, true>(kmap, vmap, a, Tq);
+}
+
 bool attn_causal_tc_supported(const AttnArgs& a) {
     const bool shape = a.hd == 64 || a.hd == 128 || (a.hd == 100 && a.hdp == 112);
     return lg_dtype_is16(a.dtype) && !a.kv_f8 && shape && a.Tq > kPfRows && a.kmap && a.vmap && a.pos.dev == nullptr &&
            a.pos.rows == nullptr && a.pos.value == 0 && a.maxS >= a.Tq && a.R <= 65535;
 }
 
-int launch_attention_causal_tc(const AttnArgs& a, cudaStream_t st, int* path) {
+// window = true: attn_window_tc_kernel (one query block per row, at the row's own position), else attn_causal_tc_kernel
+static int launch_causal_tc(const AttnArgs& a, cudaStream_t st, int* path, bool window) {
     AttnTmaArgs t{};
     t.q = (const bf16*)a.q; t.out = (bf16*)a.out; t.R = a.R; t.H = a.H; t.maxS = a.maxS;
+    t.pos_rows = a.pos.rows;
     t.row_base = a.cache_row_base; t.emb_mask = a.emb_mask; t.B = a.B; t.Tc = a.Tc; t.scale = a.scale;
     t.hd = a.hd; t.hdp = a.hdp ? a.hdp : a.hd;
     const bool half = a.dtype == LG_DTYPE_F16, wide = a.hd != 64;
-    auto kern = wide ? (half ? attn_causal_tc_kernel<f16, 128> : attn_causal_tc_kernel<bf16, 128>)
-                     : (half ? attn_causal_tc_kernel<f16, 64> : attn_causal_tc_kernel<bf16, 64>);
+    auto kern = window ? (wide ? (half ? attn_window_tc_kernel<f16, 128> : attn_window_tc_kernel<bf16, 128>)
+                               : (half ? attn_window_tc_kernel<f16, 64> : attn_window_tc_kernel<bf16, 64>))
+                       : (wide ? (half ? attn_causal_tc_kernel<f16, 128> : attn_causal_tc_kernel<bf16, 128>)
+                               : (half ? attn_causal_tc_kernel<f16, 64> : attn_causal_tc_kernel<bf16, 64>));
     const size_t smem = 1024 + (size_t)kCqStages * 2 * (wide ? 2 : 1) * kCqKeys * 128 + kCqStages * sizeof(uint64_t);
-    static DevOnce attr[4];
-    if (lg_first_on_device(attr[(half ? 1 : 0) + (wide ? 2 : 0)])) {
+    static DevOnce attr[8];
+    if (lg_first_on_device(attr[(half ? 1 : 0) + (wide ? 2 : 0) + (window ? 4 : 0)])) {
         LG_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
     dim3 grid(a.H, a.R, (a.Tq + kCqRows - 1) / kCqRows);
     (void)lg_launch(kern, dim3(grid), dim3(128), smem, st, *reinterpret_cast<const CUtensorMap*>(a.kmap),
                     *reinterpret_cast<const CUtensorMap*>(a.vmap), t, a.Tq);
     LG_LAUNCH_CHECK();
-    set_attn_path(path, 2, kCqStages, 0);
+    set_attn_path(path, window ? 4 : 2, kCqStages, 0);
     return 0;
 }
+
+int launch_attention_causal_tc(const AttnArgs& a, cudaStream_t st, int* path) { return launch_causal_tc(a, st, path, false); }
+
+bool attn_window_tc_supported(const AttnArgs& a) {
+    const bool shape = a.hd == 64 || a.hd == 128 || (a.hd == 100 && a.hdp == 112);
+    return lg_dtype_is16(a.dtype) && !a.kv_f8 && shape && a.Tq >= 2 && a.Tq <= kCqRows && a.kmap && a.vmap && a.pos.rows != nullptr &&
+           a.R <= 65535;
+}
+
+int launch_attention_window_tc(const AttnArgs& a, cudaStream_t st, int* path) { return launch_causal_tc(a, st, path, true); }
 
 // KV-cache tensor maps: the whole K (or V) region of the workspace as one [rows, hd] bf16 / fp16 matrix, or (dtype LG_DTYPE_E4M3)
 // one [rows, hdp] byte matrix read in boxes of 64 bytes (hd 64) or 128 bytes (hdp 128 or 112; bytes 112..127 read as zeros)

@@ -210,12 +210,31 @@ struct lg_engine {
     bool ws_needs_zero = false;           // KV cache + counters of `full` still have to be zero-filled (done on the caller's stream)
     cudaStream_t works[kMaxChains] = {};   // engine-owned streams (one per chain)
     cudaEvent_t ev_fork = nullptr, ev_joins[kMaxChains] = {};
+    int* sjd_done_host = nullptr;         // pinned copy of lg_generate_sjd's done flag
+    cudaEvent_t ev_pass[2] = {};
     ~lg_engine() {
         for (int i = 0; i < kMaxChains; ++i) {
             if (works[i]) cudaStreamDestroy(works[i]);
             if (ev_joins[i]) cudaEventDestroy(ev_joins[i]);
         }
         if (ev_fork) cudaEventDestroy(ev_fork);
+        for (cudaEvent_t ev : ev_pass)
+            if (ev) cudaEventDestroy(ev);
+        if (sjd_done_host) cudaFreeHost(sjd_done_host);
+    }
+    // the engine-owned streams the loops run on, created on first use
+    int ensure_streams() {
+        if (works[0]) return 0;
+        // highest priority: when the VQ decode of the previous batch runs beside the sampler (pipeline.py), a freed SM slot goes to the
+        // sampler's short dependent kernels first
+        int prio_lo = 0, prio_hi = 0;
+        LG_CUDA_OK(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
+        for (int i = 0; i < kMaxChains; ++i) {
+            LG_CUDA_OK(cudaStreamCreateWithPriority(&works[i], cudaStreamNonBlocking, prio_hi));
+            LG_CUDA_OK(cudaEventCreateWithFlags(&ev_joins[i], cudaEventDisableTiming));
+        }
+        LG_CUDA_OK(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
+        return 0;
     }
 
     // R <= 8 decode steps on the column-owner GEMV path (gemv_small.cu); shared by forward() and the decode loop's fused tail
@@ -227,6 +246,7 @@ struct lg_engine {
     }
     size_t carve(Workspace& o, char* base, int rows, int max_seq, int g = 0, int n = 1) const;
     size_t carve_score(Workspace& o, char* base, int rows, int seq) const;
+    size_t carve_sjd(Workspace& o, SjdArgs& sa, char* base, int B, int nh, int L) const;
     // K / V tensor maps over every layer of a workspace or chain view (one layer in the model dtype for a scoring view)
     int make_maps(Workspace& w) const {
         if (w.score) return make_kv_maps(w.maps, cfg.dtype, hd, hdp, cfg.dtype, w.kcache, w.vcache, (long long)w.rows * cfg.n_head * w.max_seq);
@@ -348,6 +368,47 @@ size_t lg_engine::carve_score(Workspace& o, char* base, int rows, int seq) const
     o.rows = rows;
     o.max_seq = seq8;
     o.score = true;
+    return off;
+}
+
+// lg_generate_sjd's scratch for B images (nh rows each) and window L, from `base` (null: sizes only): the activations, GEMM partials
+// and logits of nh * B * L rows, and the loop state (sa's buffers). `o` takes only the row-scaled regions; the caller adds the KV
+// cache of the full workspace.
+size_t lg_engine::carve_sjd(Workspace& o, SjdArgs& sa, char* base, int B, int nh, int L) const {
+    const int D = cfg.dim, F = cfg.ffn_dim, V = cfg.vocab_size;
+    const size_t M = (size_t)nh * B * L, BL = (size_t)B * L;
+    size_t off = 0;
+    auto take = [&](size_t bytes) {
+        char* p = base ? base + off : nullptr;
+        off += align_up(bytes);
+        return p;
+    };
+    o.h = take(M * D * esz);
+    o.xn = take(M * D * esz);
+    o.q = take(M * D * esz);
+    o.attn = take(M * D * esz);
+    o.ff = take(M * F * esz);
+    size_t pf = 0;
+    pf = std::max(pf, gemm_partial_floats((int)M, 3 * D, D, cfg.dtype));
+    pf = std::max(pf, gemm_partial_floats((int)M, D, D, cfg.dtype));
+    pf = std::max(pf, gemm_partial_floats((int)M, 2 * F, D, cfg.dtype));
+    pf = std::max(pf, gemm_partial_floats((int)M, D, F, cfg.dtype));
+    pf = std::max(pf, gemm_partial_floats((int)M, V, D, cfg.dtype));
+    o.partial_floats = pf;
+    o.partial = (float*)take(pf * sizeof(float));
+    o.logits = (float*)take(M * V * sizeof(float));
+    sa.p = (const float*)take(BL * V * sizeof(float));
+    sa.q = (float*)take(BL * V * sizeof(float));
+    sa.seed_rows = (uint64_t*)take(BL * sizeof(uint64_t));
+    sa.qflag = (int32_t*)take(BL * sizeof(int32_t));
+    sa.x = (const int32_t*)take(BL * sizeof(int32_t));
+    sa.win = (int32_t*)take(BL * sizeof(int32_t));
+    sa.step_rows = (int32_t*)take(BL * sizeof(int32_t));
+    sa.nfin = (int32_t*)take(B * sizeof(int32_t));
+    sa.start = (int32_t*)take(B * sizeof(int32_t));
+    sa.shift = (int32_t*)take(B * sizeof(int32_t));
+    sa.pos_rows = (int32_t*)take((size_t)nh * B * sizeof(int32_t));
+    sa.state = (int32_t*)take(kSjdStateInts * sizeof(int32_t));
     return off;
 }
 
@@ -813,17 +874,7 @@ int lg_generate(lg_engine* e, const void* cond, const float* emb_mask, int B, in
     cudaStream_t caller = (cudaStream_t)stream;
     LG_REQUIRE(e, "lg_generate: null engine");
     DeviceGuard guard(e->device);
-    if (!e->works[0]) {
-        // highest priority: when the VQ decode of the previous batch runs beside the sampler (pipeline.py), a freed SM slot goes to the
-        // sampler's short dependent kernels first
-        int prio_lo = 0, prio_hi = 0;
-        LG_CUDA_OK(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
-        for (int i = 0; i < lg_engine::kMaxChains; ++i) {
-            LG_CUDA_OK(cudaStreamCreateWithPriority(&e->works[i], cudaStreamNonBlocking, prio_hi));
-            LG_CUDA_OK(cudaEventCreateWithFlags(&e->ev_joins[i], cudaEventDisableTiming));
-        }
-        LG_CUDA_OK(cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming));
-    }
+    LG_TRY(e->ensure_streams());
     LG_TRY(e->zero_fill_if_needed(caller));
     LG_CUDA_OK(cudaEventRecord(e->ev_fork, caller));
     for (int i = 0; i < lg_engine::kMaxChains; ++i) LG_CUDA_OK(cudaStreamWaitEvent(e->works[i], e->ev_fork, 0));
@@ -965,6 +1016,156 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
         if (ch[g].graph) cudaGraphDestroy(ch[g].graph);
     }
     return ret;
+}
+
+int lg_sjd_workspace_bytes(lg_engine* e, int B, int use_cfg, int L, size_t* bytes) {
+    LG_REQUIRE(e && bytes && B > 0 && L >= 2 && L <= 64, "lg_sjd_workspace_bytes: bad argument (B=%d L=%d)", B, L);
+    Workspace w;
+    SjdArgs sa{};
+    *bytes = e->carve_sjd(w, sa, nullptr, B, use_cfg ? 2 : 1, L);
+    return 0;
+}
+
+static int generate_sjd_impl(lg_engine* e, const Workspace& w, SjdArgs& sa, const void* cond, const float* emb_mask, const lg_sample_cfg& sc,
+                             bool use_cfg, int32_t* iters_out, cudaStream_t st) {
+    const lg_model_cfg& c = e->cfg;
+    const int B = sa.B, S = sa.S, L = sa.L, T = sa.T, V = c.vocab_size, D = c.dim, dt = c.dtype, R = sa.nh * B, M = R * L;
+    static int calls = 0;
+    sa.done_token = ++calls;   // a pass still in flight from an earlier call cannot end this one
+    LG_CUDA_OK(cudaMemsetAsync(sa.state, 0, kSjdStateInts * sizeof(int32_t), st));
+    // prefill and token 0, drawn as lg_generate draws it
+    LG_TRY(e->embed_cond(e->full, cond, B, R, T, st));
+    LG_TRY(e->forward(e->full, R * T, T, PosArg{nullptr, 0}, emb_mask, B, e->full.logits, false, st));
+    SampleArgs s0 = make_sample_args(sc, e->full.logits, B, V, use_cfg, dt);
+    s0.step = 0; s0.out_seq = sa.out; s0.seq_stride = S;
+    LG_TRY(launch_sample(s0, st));
+    LG_TRY(launch_sjd_refresh(sa, 1, st));
+    // one pass: window embedding, the layers over R * L rows at per-row positions, the head over every row, p and x for every slot
+    // (B * L images, CFG twins at rows b * L + i and (B + b) * L + i), acceptance, next window
+    SampleArgs sp = make_sample_args(sc, w.logits, B * L, V, use_cfg, dt);
+    sp.seed_rows = sa.seed_rows; sp.step_rows = sa.step_rows;
+    sp.out_idx = const_cast<int32_t*>(sa.x); sp.out_probs = const_cast<float*>(sa.p);
+    auto pass = [&]() -> int {
+        LG_PROF(PC_EMBED_MISC, st, launch_embed(e->tok_emb, sa.win, B * L, M, -1, D, dt, w.h, st));
+        LG_TRY(e->run_layers(w, M, L, PosArg{nullptr, 0, sa.pos_rows}, emb_mask, B, false, st));
+        int ks = 1;
+        prof_begin(PC_GEMM_HEAD, st);
+        const int direct = e->gemm(w, w.xn, M, V, D, e->output, nullptr, 0, &ks, w.logits, st);
+        prof_end(st);
+        if (direct < 0) return direct;
+        if (direct == 0) LG_TRY(launch_reduce_f32(w.partial, ks, M, V, w.logits, st));
+        LG_PROF(PC_SAMPLE, st, launch_sample(sp, st));
+        LG_PROF(PC_SAMPLE, st, launch_sjd_verify(sa, st));
+        LG_PROF(PC_SAMPLE, st, launch_sjd_refresh(sa, 0, st));
+        LG_CUDA_OK(cudaMemcpyAsync(e->sjd_done_host, sa.state + kSjdDone, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        return 0;
+    };
+    // Every pass has the same kernel arguments (the loop state is on the device), so one captured graph is replayed. The host reads
+    // pass j - 1's done flag after it has enqueued pass j: the GPU never waits for the host, and at most one pass runs after the last
+    // image finished (a no-op: finished images are frozen). At most S - 1 passes: each one makes at least one token final.
+    LG_TRY(pass());   // eagerly first: sets every kernel attribute outside capture
+    LG_CUDA_OK(cudaEventRecord(e->ev_pass[0], st));
+    const bool graph = e->use_graph && !prof_enabled() && !lg_debug_sync() && S - 1 > 2;
+    cudaGraph_t g = nullptr;
+    cudaGraphExec_t exec = nullptr;
+    uint64_t per_pass = 0;
+    int ret = 0;
+    if (graph) {
+        cudaError_t ce = cudaStreamBeginCapture(st, cudaStreamCaptureModeRelaxed);
+        if (ce != cudaSuccess) return lg_fail("cudaStreamBeginCapture failed: %s", cudaGetErrorString(ce));
+        const uint64_t before = g_lg_launches.load();
+        ret = pass();
+        per_pass = g_lg_launches.load() - before;
+        ce = cudaStreamEndCapture(st, &g);
+        g_lg_launches.fetch_sub(per_pass);   // the capture pass launched nothing
+        if (ret == 0 && (ce != cudaSuccess || !g)) ret = lg_fail("stream capture failed: %s", cudaGetErrorString(ce));
+        if (ret == 0) {
+            ce = cudaGraphInstantiate(&exec, g, 0);
+            if (ce != cudaSuccess) ret = lg_fail("cudaGraphInstantiate failed: %s", cudaGetErrorString(ce));
+        }
+    }
+    for (int launched = 1; ret == 0 && launched < S - 1; ++launched) {
+        if (graph) {
+            const cudaError_t ce = cudaGraphLaunch(exec, st);
+            if (ce != cudaSuccess) { ret = lg_fail("cudaGraphLaunch failed: %s", cudaGetErrorString(ce)); break; }
+            g_lg_launches.fetch_add(per_pass);
+        } else {
+            ret = pass();
+            if (ret) break;
+        }
+        cudaError_t ce = cudaEventRecord(e->ev_pass[launched & 1], st);
+        if (ce == cudaSuccess) ce = cudaEventSynchronize(e->ev_pass[(launched - 1) & 1]);
+        if (ce != cudaSuccess) { ret = lg_fail("lg_generate_sjd: waiting for a pass failed: %s", cudaGetErrorString(ce)); break; }
+        if (*(volatile int*)e->sjd_done_host == sa.done_token) break;
+    }
+    if (exec) cudaGraphExecDestroy(exec);
+    if (g) cudaGraphDestroy(g);
+    if (ret) return ret;
+    LG_CUDA_OK(cudaMemcpyAsync(iters_out, sa.state + kSjdIters, sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+    return 0;
+}
+
+int lg_generate_sjd(lg_engine* e, const void* cond, const float* emb_mask, int B, int T, int S, const lg_sample_cfg* sc, int L,
+                    void* dev_ws, size_t ws_bytes, int32_t* out_tokens, int32_t* iters_out, float* dbg_probs, void* stream) {
+    cudaStream_t caller = (cudaStream_t)stream;
+    LG_REQUIRE(e && e->finalized, "lg_generate_sjd: engine not finalized");
+    DeviceGuard guard(e->device);
+    const lg_model_cfg& c = e->cfg;
+    LG_REQUIRE(cond && sc && out_tokens && iters_out && B > 0, "lg_generate_sjd: null argument or B=%d", B);
+    LG_REQUIRE(L >= 2 && L <= 64, "lg_generate_sjd: window L=%d outside [2, 64]", L);
+    LG_REQUIRE(S > L && S <= c.block_size, "lg_generate_sjd: S=%d must lie in [L + 1, block_size=%d] (L=%d)", S, c.block_size, L);
+    LG_REQUIRE(T == c.cls_token_num, "lg_generate_sjd: T=%d must equal cls_token_num=%d", T, c.cls_token_num);
+    LG_REQUIRE(!emb_mask || c.model_type == LG_MODEL_T2I, "lg_generate_sjd: emb_mask only applies to t2i models");
+    LG_REQUIRE((size_t)c.vocab_size * sizeof(float) <= 200 * 1024, "lg_generate_sjd: vocab %d too large for the sampler", c.vocab_size);
+    const bool use_cfg = sc->cfg_scale > 1.0f;   // generate.py:128
+    const int nh = use_cfg ? 2 : 1, R = nh * B;
+    LG_TRY(check_ready(e, R, T + S));
+    LG_REQUIRE((long long)R * L <= 65535, "lg_generate_sjd: %d rows x window %d exceed 65535 query rows", R, L);
+    LG_REQUIRE(dev_ws && ((uintptr_t)dev_ws & 255) == 0, "lg_generate_sjd: scratch must be non-null and 256-byte aligned");
+    Workspace scr;
+    SjdArgs sa{};
+    const size_t need = e->carve_sjd(scr, sa, (char*)dev_ws, B, nh, L);
+    LG_REQUIRE(ws_bytes >= need, "lg_generate_sjd: scratch of %zu bytes is too small (%zu)", ws_bytes, need);
+    Workspace w = e->full;   // the KV cache and its maps of the workspace, everything else from the scratch
+    w.h = scr.h; w.xn = scr.xn; w.q = scr.q; w.attn = scr.attn; w.ff = scr.ff; w.x0 = nullptr;
+    w.partial = scr.partial; w.partial_floats = scr.partial_floats; w.logits = scr.logits;
+    w.tokens = nullptr; w.counters = nullptr;
+    sa.B = B; sa.S = S; sa.L = L; sa.V = c.vocab_size; sa.T = T; sa.nh = nh;
+    sa.greedy = sc->greedy; sa.seed = sc->seed; sa.row_offset = 0;
+    sa.out = out_tokens; sa.dbg = dbg_probs;
+    LG_TRY(e->ensure_streams());
+    if (!e->sjd_done_host) {
+        LG_CUDA_OK(cudaHostAlloc((void**)&e->sjd_done_host, sizeof(int), cudaHostAllocDefault));
+        *e->sjd_done_host = 0;
+        for (cudaEvent_t& ev : e->ev_pass) LG_CUDA_OK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    }
+    // on an engine-owned stream, as lg_generate: the caller's stream may be the legacy default stream, which cannot be captured
+    cudaStream_t st = e->works[0];
+    LG_TRY(e->zero_fill_if_needed(caller));
+    LG_CUDA_OK(cudaEventRecord(e->ev_fork, caller));
+    LG_CUDA_OK(cudaStreamWaitEvent(st, e->ev_fork, 0));
+    const int rc = generate_sjd_impl(e, w, sa, cond, emb_mask, *sc, use_cfg, iters_out, st);
+    cudaEventRecord(e->ev_joins[0], st);
+    cudaStreamWaitEvent(caller, e->ev_joins[0], 0);
+    return rc;
+}
+
+int lg_test_sjd_verify(int B, int S, int L, int V, int greedy, uint64_t seed, const float* p, const float* q, const int32_t* qflag,
+                       const int32_t* x, const int32_t* win, int32_t* nfin, int32_t* start, int32_t* out, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    LG_REQUIRE(p && q && qflag && x && win && nfin && start && out, "lg_test_sjd_verify: null argument");
+    LG_REQUIRE(B > 0 && V > 0 && L >= 2 && L <= 64 && S > L, "lg_test_sjd_verify: bad shape B=%d S=%d L=%d V=%d", B, S, L, V);
+    SjdArgs sa{};
+    sa.B = B; sa.S = S; sa.L = L; sa.V = V; sa.T = 0; sa.nh = 1; sa.greedy = greedy; sa.seed = seed;
+    sa.p = p; sa.q = const_cast<float*>(q); sa.qflag = const_cast<int32_t*>(qflag); sa.x = x; sa.win = const_cast<int32_t*>(win);
+    sa.nfin = nfin; sa.start = start; sa.out = out; sa.done_token = 1;
+    int32_t* tmp = nullptr;   // shift [B], pos_rows [B], loop state
+    LG_CUDA_OK(cudaMallocAsync((void**)&tmp, (2 * (size_t)B + kSjdStateInts) * sizeof(int32_t), st));
+    LG_CUDA_OK(cudaMemsetAsync(tmp, 0, (2 * (size_t)B + kSjdStateInts) * sizeof(int32_t), st));
+    sa.shift = tmp; sa.pos_rows = tmp + B; sa.state = tmp + 2 * B;
+    const int rc = launch_sjd_verify(sa, st);
+    cudaFreeAsync(tmp, st);
+    return rc;
 }
 
 int lg_vq_set_cta_budget(int ctas) {

@@ -49,6 +49,33 @@ struct SampleArgs {
 };
 int launch_sample(const SampleArgs& a, cudaStream_t st);
 
+// Speculative Jacobi decoding (lg_generate_sjd). Image b's window has L slots; slot i feeds token start[b] + i - 1 (win) and its
+// output p (the sample kernel's out_probs) is the distribution of token start[b] + i. Rows of image b are b * L + i.
+enum SjdState { kSjdIters = 0, kSjdDone, kSjdTicket, kSjdActive, kSjdFinished, kSjdLive, kSjdStateInts };
+struct SjdArgs {
+    int B, S, L, V, T, nh;       // nh: 2 with CFG twins (rows b and B + b), else 1
+    int greedy;
+    uint64_t seed;
+    int row_offset;              // added to the image index in every uniform's key
+    const float* p;              // [B * L][V] this pass's p rows
+    float* q;                    // [B * L][V] q of the draft for token start + i (slot i), unless qflag says uniform
+    int32_t* qflag;              // [B * L] 1: that q is uniform, 1 / V
+    const int32_t* x;            // [B * L] the sample kernel's draw from p of slot i
+    int32_t* win;                // [B * L] window input tokens
+    int32_t* nfin;               // [B] tokens final so far
+    int32_t* start;              // [B] first token index the window predicts
+    int32_t* shift;              // [B] start after the pass minus start before it
+    int32_t* pos_rows;           // [nh * B] T + start - 1 (the position of slot 0)
+    uint64_t* seed_rows;         // [B * L] the sample kernel's per-row seeds (redraws)
+    int32_t* step_rows;          // [B * L] token index of each slot
+    int32_t* out;                // [B][S]
+    int32_t* state;              // [kSjdStateInts], zero-initialised
+    float* dbg;                  // [passes][B][L][V] copy of every pass's p rows, or null
+    int done_token;              // written to state[kSjdDone] once every image has S tokens (unique per call)
+};
+int launch_sjd_verify(const SjdArgs& a, cudaStream_t st);
+int launch_sjd_refresh(const SjdArgs& a, int first, cudaStream_t st);
+
 // ------------------------------------------------------------------------------------------------
 // gemm.cu — y_partial[ks][M][N] (f32) = x[M,K] * W[N,K]^T ; W may be two row segments (w1 | w3).
 // ------------------------------------------------------------------------------------------------
@@ -152,7 +179,7 @@ struct AttnArgs {
 // the TMA attention kernels can stream (dims 100..111 stay zero); every other cache row is hd wide
 inline int attn_kv_row_width(int dtype, int hd) { return hd == 100 && lg_dtype_is16(dtype) ? 112 : hd; }
 // path (optional, int[3]): the kernel that was launched (0 = attention_kernel, 1 = attn_tma_kernel, 2 = attn_causal_tc_kernel,
-// 3 = attn_prefill_tc_kernel), its TMA ring depth (0 for attention_kernel, 1 for the single-stage prefill) and whether it fused the
+// 3 = attn_prefill_tc_kernel, 4 = attn_window_tc_kernel), its TMA ring depth (0 for attention_kernel, 1 for the single-stage prefill) and whether it fused the
 // QKV epilogue
 int launch_attention(const AttnArgs& a, cudaStream_t st, int* path = nullptr);
 inline void set_attn_path(int* path, int kernel, int stages, int fused) {
@@ -175,6 +202,10 @@ int launch_attention_prefill_tc(const AttnArgs& a, cudaStream_t st, int* path = 
 // per (head, row, 64-query block), K / V blocks through a TMA ring, mma.sync QK^T and PV with an online softmax
 bool attn_causal_tc_supported(const AttnArgs& a);
 int launch_attention_causal_tc(const AttnArgs& a, cudaStream_t st, int* path = nullptr);
+// speculative-decoding windows (2 <= Tq <= 64 queries per row at per-row positions pos.rows[r] + t, same cache and shapes as the causal
+// kernel): a CTA per (head, row) streams the row's K / V blocks [0, pos.rows[r] + Tq) through the causal kernel's TMA ring
+bool attn_window_tc_supported(const AttnArgs& a);
+int launch_attention_window_tc(const AttnArgs& a, cudaStream_t st, int* path = nullptr);
 // VQ convolutions: vq.cu runs them; conv_tc.cu holds the wgmma kernels and chooses the kernel of each call.
 // GroupNorm(32) partial statistics are [B][splits][32 groups][sum, sum of squares] floats. gn_stats_kernel writes at most
 // kGnStatsMaxSplits splits per image; the drain of conv_tcw_kernel writes one per 16x16-pixel tile (and upsample phase) of its input.

@@ -479,3 +479,193 @@ int launch_sample(const SampleArgs& a, cudaStream_t st) {
     LG_LAUNCH_CHECK();
     return 0;
 }
+
+// ---------------------------------------------------------------------------------------------------
+// Speculative Jacobi decoding (lg_generate_sjd): acceptance and the next window. One pass of the loop feeds image b's window of L
+// tokens (slot i holds token s_b + i - 1, s_b = start[b]) through the model; the sample kernel then writes p_{s_b + i} for every slot
+// (out_probs) and a draw x_i from it (argmax in greedy mode). The uniforms (sjd_uniform, mirrored by tests/sjd_oracle.py) are keyed
+// by (seed, image, token index, purpose); the redraw x_i is the sample kernel's own draw with seed_rows = sjd_pass_seed(seed, b, pass)
+// and step_rows = the token index, so no uniform is used twice.
+namespace {
+
+enum SjdPurpose : uint64_t { kSjdAccept = 1, kSjdResidual = 2, kSjdInit = 3 };
+
+__device__ __forceinline__ float sjd_uniform(uint64_t seed, int b, int k, uint64_t purpose) {
+    const uint64_t r = splitmix64(splitmix64(splitmix64(seed ^ (0xA0761D6478BD642Full * (uint64_t)(k + 1))) ^
+                                             (0xE7037ED1A0B428DBull * (uint64_t)(b + 1))) ^
+                                  (0x8EBC6AF09C88C6E3ull * purpose));
+    return (float)(r >> 40) * (1.0f / 16777216.0f);
+}
+__device__ __forceinline__ uint64_t sjd_pass_seed(uint64_t seed, int b, int pass) {
+    return splitmix64(splitmix64(seed ^ (0x9E6C63D0676A9A99ull * (uint64_t)(b + 1))) ^ (0xD6E8FEB86659FD93ull * (uint64_t)(pass + 1)));
+}
+
+constexpr int kSjdThreads = 512;
+
+// One CTA per image: accept a prefix of the drafts, draw the token that ends it, advance the image's window
+__global__ void __launch_bounds__(kSjdThreads) sjd_verify_kernel(SjdArgs a) {
+    lg_pdl_sync();
+    __shared__ float red[33];
+    __shared__ float s_wtot[32];
+    __shared__ int s_i, s_pick;
+    const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int L = a.L, V = a.V, S = a.S;
+    const int n = a.nfin[b], s = a.start[b];
+    const bool active = n < S;
+    if (active) {
+        const size_t row0 = (size_t)b * L;
+        if (tid == 0) {
+            int i = n - s;
+            for (; i <= L - 2; ++i) {   // the draft for token s + i is fed in slot i + 1 and checked against p_{s + i} (slot i)
+                const int d = a.win[row0 + i + 1], k = s + i;
+                bool acc;
+                if (a.greedy) {
+                    acc = d == a.x[row0 + i];
+                } else {
+                    const float pd = a.p[(row0 + i) * V + d];
+                    const float qd = a.qflag[row0 + i] ? 1.0f / (float)V : a.q[(row0 + i) * V + d];
+                    acc = sjd_uniform(a.seed, b + a.row_offset, k, kSjdAccept) * qd < pd;
+                }
+                if (!acc) break;
+                a.out[(size_t)b * S + k] = d;
+            }
+            s_i = i;
+            s_pick = a.x[row0 + min(i, L - 1)];   // bonus token, greedy correction, or the fallback of an empty residual
+        }
+        __syncthreads();
+        const int i = s_i;
+        if (i <= L - 2 && !a.greedy) {
+            // residual draw: normalize(max(0, p - q)), inverse CDF over contiguous per-thread segments
+            const float* pr = a.p + (row0 + i) * V;
+            const float* qr = a.q + (row0 + i) * V;
+            const bool uni = a.qflag[row0 + i] != 0;
+            const float qu = 1.0f / (float)V;
+            const int seg = (V + kSjdThreads - 1) / kSjdThreads;
+            const int v0 = min(tid * seg, V), v1 = min(v0 + seg, V);
+            float local = 0.f;
+            for (int v = v0; v < v1; ++v) local += fmaxf(0.f, pr[v] - (uni ? qu : qr[v]));
+            float incl = local;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const float t = __shfl_up_sync(0xffffffffu, incl, o);
+                if (lane >= o) incl += t;
+            }
+            if (lane == 31) s_wtot[warp] = incl;
+            __syncthreads();
+            if (warp == 0) {
+                const float w = lane < kSjdThreads / 32 ? s_wtot[lane] : 0.f;
+                float wi = w;
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) {
+                    const float t = __shfl_up_sync(0xffffffffu, wi, o);
+                    if (lane >= o) wi += t;
+                }
+                if (lane < kSjdThreads / 32) s_wtot[lane] = wi - w;
+                if (lane == 31) red[32] = wi;
+            }
+            __syncthreads();
+            const float total = red[32];
+            if (total > 0.f) {
+                const float target = sjd_uniform(a.seed, b + a.row_offset, s + i, kSjdResidual) * total;
+                const float excl = s_wtot[warp] + (incl - local);
+                int last = -1;
+                for (int v = tid; v < V; v += kSjdThreads)
+                    if (pr[v] - (uni ? qu : qr[v]) > 0.f) last = max(last, v);
+                last = (int)block_max((float)last, red);
+                __syncthreads();
+                if (tid == 0) s_pick = last;   // the target past the rounded total: the last positive weight
+                __syncthreads();
+                if (local > 0.f && target >= excl && target < excl + local) {
+                    float c = excl;
+                    for (int v = v0; v < v1; ++v) {
+                        const float e = fmaxf(0.f, pr[v] - (uni ? qu : qr[v]));
+                        c += e;
+                        if (c > target && e > 0.f) { s_pick = v; break; }
+                    }
+                }
+            }
+            __syncthreads();
+        }
+        if (tid == 0) {
+            const int k = s + i, n2 = k + 1, s2 = min(n2, S - L);
+            a.out[(size_t)b * S + k] = s_pick;
+            a.nfin[b] = n2;
+            a.start[b] = s2;
+            a.shift[b] = s2 - s;
+            for (int hh = 0; hh < a.nh; ++hh) a.pos_rows[hh * a.B + b] = a.T + s2 - 1;
+            atomicAdd(&a.state[kSjdActive], 1);
+            if (n2 >= S) atomicAdd(&a.state[kSjdFinished], 1);
+        }
+    }
+    if (tid == 0) {
+        __threadfence();
+        if (atomicAdd(reinterpret_cast<unsigned int*>(&a.state[kSjdTicket]), 1u) == gridDim.x - 1) {
+            const int act = atomicExch(&a.state[kSjdActive], 0);
+            a.state[kSjdLive] = act > 0;
+            if (act > 0) a.state[kSjdIters] += 1;
+            if (atomicAdd(&a.state[kSjdFinished], 0) >= a.B) a.state[kSjdDone] = a.done_token;
+            a.state[kSjdTicket] = 0;
+        }
+    }
+}
+
+// grid (B, L): slot i of image b's next window. first = 1 sets up the window after the prefill (token 0 final, all drafts new).
+__global__ void __launch_bounds__(256) sjd_refresh_kernel(SjdArgs a, int first) {
+    lg_pdl_sync();
+    const int b = blockIdx.x, i = blockIdx.y, L = a.L, V = a.V, S = a.S;
+    const size_t slot = (size_t)b * L + i;
+    if (!first && !a.state[kSjdLive]) return;   // a pass after every image finished changes nothing
+    const int pass = a.state[kSjdIters];        // index of the next pass
+    if (!first && a.dbg) {
+        float* d = a.dbg + ((size_t)(pass - 1) * a.B * L + slot) * V;
+        for (int v = threadIdx.x; v < V; v += blockDim.x) d[v] = a.p[slot * V + v];
+    }
+    int n, s, shift;
+    if (first) {
+        n = 1; s = 1; shift = 1 << 20;
+        if (i == 0 && threadIdx.x == 0) {
+            a.nfin[b] = 1; a.start[b] = 1;
+            for (int hh = 0; hh < a.nh; ++hh) a.pos_rows[hh * a.B + b] = a.T;
+        }
+    } else {
+        n = a.nfin[b]; s = a.start[b]; shift = a.shift[b];
+        if (n >= S) return;                      // finished: its rows keep running on the old window, their outputs unused
+    }
+    const int k = s + i - 1;                     // the token this slot feeds
+    if (threadIdx.x == 0) {
+        a.seed_rows[slot] = sjd_pass_seed(a.seed, b + a.row_offset, pass);
+        a.step_rows[slot] = s + i;
+    }
+    if (k < n) {
+        if (threadIdx.x == 0) a.win[slot] = a.out[(size_t)b * S + k];
+        return;
+    }
+    const int j = k - (s - shift);               // the slot of the pass just run that computed p_k
+    const size_t qs = slot - 1;                  // q of the draft for token k sits at slot k - s
+    if (j <= L - 1) {                            // Jacobi update: redraw from p_k, which becomes its q
+        const float* src = a.p + ((size_t)b * L + j) * V;
+        float* dst = a.q + qs * V;
+        for (int v = threadIdx.x; v < V; v += blockDim.x) dst[v] = src[v];
+        if (threadIdx.x == 0) { a.win[slot] = a.x[(size_t)b * L + j]; a.qflag[qs] = 0; }
+    } else if (threadIdx.x == 0) {               // a new index: uniform over the vocabulary, q = 1 / V
+        const int t = (int)(sjd_uniform(a.seed, b + a.row_offset, k, kSjdInit) * (float)V);
+        a.win[slot] = min(t, V - 1);
+        a.qflag[qs] = 1;
+    }
+}
+
+}  // namespace
+
+int launch_sjd_verify(const SjdArgs& a, cudaStream_t st) {
+    LG_REQUIRE(a.B > 0 && a.L >= 1 && a.L <= 64 && a.S > a.L && a.V > 0, "sjd: bad shape B=%d L=%d S=%d V=%d", a.B, a.L, a.S, a.V);
+    (void)lg_launch(sjd_verify_kernel, dim3(a.B), dim3(kSjdThreads), 0, st, a);
+    LG_LAUNCH_CHECK();
+    return 0;
+}
+
+int launch_sjd_refresh(const SjdArgs& a, int first, cudaStream_t st) {
+    LG_REQUIRE(a.B > 0 && a.L >= 1 && a.L <= 64 && a.S > a.L && a.V > 0, "sjd: bad shape B=%d L=%d S=%d V=%d", a.B, a.L, a.S, a.V);
+    (void)lg_launch(sjd_refresh_kernel, dim3(a.B, a.L), dim3(256), 0, st, a, first);
+    LG_LAUNCH_CHECK();
+    return 0;
+}

@@ -565,6 +565,7 @@ int launch_attention(const AttnArgs& a, cudaStream_t st, int* path) {
     if (attn_tma_supported(a) && attn_tma_enabled()) return launch_attention_tma(a, st, path);
     if (attn_prefill_tc_supported(a) && attn_tma_enabled() && a.qkv_partial == nullptr) return launch_attention_prefill_tc(a, st, path);
     if (attn_causal_tc_supported(a) && attn_tma_enabled() && a.qkv_partial == nullptr) return launch_attention_causal_tc(a, st, path);
+    if (attn_window_tc_supported(a) && attn_tma_enabled() && a.qkv_partial == nullptr) return launch_attention_window_tc(a, st, path);
     LG_REQUIRE(a.qkv_partial == nullptr, "attention: fused QKV epilogue requested on a path that does not support it");
     set_attn_path(path, 0, 0, 0);
     LG_REQUIRE((long long)a.R * a.Tq <= 65535, "attention: too many query rows (%d x %d)", a.R, a.Tq);

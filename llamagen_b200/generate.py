@@ -41,6 +41,10 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
       seed=int             explicit RNG seed for the multinomial draw
       return_logits=True   also return the per-step CFG-mixed logits [S, B, V] (fp32) for parity tests
       teacher=int tensor   [B, S] tokens fed back instead of the sampled ones (teacher forcing)
+      sjd_window=L         speculative Jacobi decoding: up to L tokens per forward pass (2 <= L <= 64; a window longer than
+                           max_new_tokens - 1 is shortened to it). The same distribution as plain sampling but other draws for a
+                           seed, except token 0; greedy decoding gives the same tokens.
+      return_stats=True    with sjd_window: return (tokens, {"iterations": passes, "tokens_per_iteration": ...})
     """
     if not isinstance(model, Transformer):
         raise TypeError("llamagen_b200.generate needs a llamagen_b200 GPT_models[...] instance")
@@ -51,8 +55,17 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
     seed = sampling_kwargs.pop("seed", None)
     return_logits = bool(sampling_kwargs.pop("return_logits", False))
     teacher = sampling_kwargs.pop("teacher", None)
+    sjd_window = sampling_kwargs.pop("sjd_window", None)
+    return_stats = bool(sampling_kwargs.pop("return_stats", False))
     if sampling_kwargs:
         raise TypeError(f"unexpected sampling kwargs: {sorted(sampling_kwargs)}")
+    if sjd_window is not None:
+        if isinstance(sjd_window, bool) or int(sjd_window) != sjd_window or not 2 <= int(sjd_window) <= 64:
+            raise ValueError(f"sjd_window must be an integer in [2, 64], got {sjd_window!r}")
+        if teacher is not None or return_logits:
+            raise ValueError("sjd_window cannot be combined with teacher or return_logits")
+    elif return_stats:
+        raise ValueError("return_stats needs sjd_window")
 
     dev = model.tok_embeddings.weight.device
     _lib.require_cuda(model.tok_embeddings.weight, "generate")
@@ -77,9 +90,15 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
         assert emb_masks.shape[-1] == T
         em = emb_masks.to(device=dev, dtype=torch.float32).contiguous()
 
+    if sjd_window is not None and S < 3:
+        raise ValueError(f"sjd_window needs max_new_tokens >= 3, got {S}")
     model.setup_caches(max_batch_size=rows, max_seq_length=T + S, dtype=model.tok_embeddings.weight.dtype)
     lib, handle = _lib.load(), model.engine()
     out = torch.empty((B, S), dtype=torch.int32, device=dev)
+    if sjd_window is not None:
+        return _generate_sjd(model, lib, handle, cond, cond_dev, em, B, T, S, out, min(int(sjd_window), S - 1), use_cfg, return_stats,
+                             _lib.SampleCfg(float(cfg_scale), int(cfg_interval), temperature, top_k, top_p, 0 if sample_logits else 1,
+                                            _draw_seed() if seed is None else int(seed)))
     dbg = torch.empty((S, B, model.vocab_size), dtype=torch.float32, device=dev) if return_logits else None
     tf = teacher.to(device=dev, dtype=torch.int32).contiguous() if teacher is not None else None
     if tf is not None and tuple(tf.shape) != (B, S):
@@ -91,3 +110,18 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
     if cond.device != dev:
         out = out.to(cond.device)
     return (out, dbg) if return_logits else out
+
+
+def _generate_sjd(model, lib, handle, cond, cond_dev, em, B, T, S, out, L, use_cfg, return_stats, sc, dbg_probs=None):
+    """lg_generate_sjd with window L (already clamped to S - 1); dbg_probs: None or f32 [S - 1, B, L, V] for replay tests."""
+    dev = out.device
+    ws, ws_bytes = model._sjd_scratch(B, use_cfg, L)
+    iters = torch.zeros(1, dtype=torch.int32, device=dev)
+    _lib.check(lib.lg_generate_sjd(handle, _lib.ptr(cond_dev), _lib.ptr(em), B, T, S, ctypes.byref(sc), L, ws, ws_bytes, _lib.ptr(out),
+                                   _lib.ptr(iters), _lib.ptr(dbg_probs), _lib.current_stream(dev)), "lg_generate_sjd")
+    if cond.device != dev:
+        out = out.to(cond.device)
+    if not return_stats:
+        return out
+    n = int(iters.item())
+    return out, {"iterations": n, "tokens_per_iteration": (S - 1) / max(n, 1)}

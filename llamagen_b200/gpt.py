@@ -194,6 +194,7 @@ class Transformer(nn.Module):
         self._ws_shape = (0, 0)
         self._kv_cache = ("auto", None)
         self._score_ws = None
+        self._sjd_ws = None
         self.requires_grad_(False)
 
     # ------------------------------------------------------------------ engine plumbing
@@ -305,6 +306,19 @@ class Transformer(nn.Module):
             self._score_ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=dev)
         base = (self._score_ws.data_ptr() + 255) // 256 * 256
         return ctypes.c_void_p(base), self._score_ws.numel() - (base - self._score_ws.data_ptr())
+
+    def _sjd_scratch(self, B: int, use_cfg: bool, L: int):
+        """The lg_generate_sjd scratch for B images and window L, kept on the model like the setup_caches() workspace.
+        Returns (device pointer, bytes)."""
+        lib, handle = _lib.load(), self.engine()
+        need = ctypes.c_size_t()
+        _lib.check(lib.lg_sjd_workspace_bytes(handle, B, int(use_cfg), L, ctypes.byref(need)), "lg_sjd_workspace_bytes")
+        dev = self.tok_embeddings.weight.device
+        if self._sjd_ws is None or self._sjd_ws.numel() < need.value + 256 or self._sjd_ws.device != dev:
+            self._sjd_ws = None
+            self._sjd_ws = torch.empty(need.value + 256, dtype=torch.uint8, device=dev)
+        base = (self._sjd_ws.data_ptr() + 255) // 256 * 256
+        return ctypes.c_void_p(base), self._sjd_ws.numel() - (base - self._sjd_ws.data_ptr())
 
     def _score(self, cond, idx, targets, emb_masks, cfg_scale: float, want_logits: bool, want_nll: bool):
         """lg_score over complete sequences: cond (c2i labels [B] / t2i features [B, T, C]), idx [B, S-1] or None (S = 1),

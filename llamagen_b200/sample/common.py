@@ -52,6 +52,17 @@ def load_gpt(args, device, latent_size):
     return gpt_model
 
 
+def add_sjd_arg(parser):
+    parser.add_argument("--sjd-window", type=int, default=None,
+                        help="extension: speculative Jacobi decoding with this many tokens per forward pass (2..64)")
+    return parser
+
+
+def sjd_kwargs(args) -> dict:
+    """generate() keywords of --sjd-window (none when it is not given, so the default path is unchanged)."""
+    return {} if args.sjd_window is None else {"sjd_window": args.sjd_window}
+
+
 def add_common_args(parser, t2i: bool):
     parser.add_argument("--gpt-model", type=str, choices=list(GPT_models.keys()), default="GPT-XL" if t2i else "GPT-B")
     parser.add_argument("--gpt-ckpt", type=str, default=None)

@@ -6,7 +6,7 @@ import time
 import torch
 
 from .. import generate
-from .common import add_common_args, load_gpt, load_vq
+from .common import add_common_args, add_sjd_arg, sjd_kwargs, load_gpt, load_vq
 
 
 def main(args):
@@ -26,7 +26,8 @@ def main(args):
     torch.cuda.synchronize()
     t1 = time.time()
     index_sample = generate(gpt_model, c_indices, latent_size ** 2, cfg_scale=args.cfg_scale, cfg_interval=args.cfg_interval,
-                            temperature=args.temperature, top_k=args.top_k, top_p=args.top_p, sample_logits=True)
+                            temperature=args.temperature, top_k=args.top_k, top_p=args.top_p, sample_logits=True,
+                            **sjd_kwargs(args))
     torch.cuda.synchronize()
     print(f"gpt sampling takes about {time.time() - t1:.2f} seconds.")
     t2 = time.time()
@@ -39,7 +40,7 @@ def main(args):
 
 
 def build_parser():
-    parser = add_common_args(argparse.ArgumentParser(), t2i=False)
+    parser = add_sjd_arg(add_common_args(argparse.ArgumentParser(), t2i=False))
     parser.add_argument("--cfg-interval", type=float, default=-1)
     parser.add_argument("--class-labels", type=int, nargs="+", default=None,
                         help="extension: override the 8 hard-coded ImageNet labels (batch size = number of labels)")

@@ -12,7 +12,7 @@ import torch
 
 from .. import generate
 from ..cond import HFT5Encoder, load_t5_feature_files, prepare_condition, synthetic_features
-from .common import add_common_args, load_gpt, load_vq
+from .common import add_common_args, add_sjd_arg, sjd_kwargs, load_gpt, load_vq
 
 PROMPTS = [
     "A portrait photo of a kangaroo wearing an orange hoodie and blue sunglasses standing on the grassin front of the Sydney Opera House holding a sign on the chest that says Welcome Friends!",
@@ -55,7 +55,8 @@ def main(args):
     torch.cuda.synchronize()
     t1 = time.time()
     index_sample = generate(gpt_model, c_indices, latent_size ** 2, emb_masks, cfg_scale=args.cfg_scale,
-                            temperature=args.temperature, top_k=args.top_k, top_p=args.top_p, sample_logits=True)
+                            temperature=args.temperature, top_k=args.top_k, top_p=args.top_p, sample_logits=True,
+                            **sjd_kwargs(args))
     torch.cuda.synchronize()
     print(f"Full sampling takes about {time.time() - t1:.2f} seconds.")
     t2 = time.time()
@@ -68,7 +69,7 @@ def main(args):
 
 
 def build_parser():
-    parser = add_common_args(argparse.ArgumentParser(), t2i=True)
+    parser = add_sjd_arg(add_common_args(argparse.ArgumentParser(), t2i=True))
     parser.add_argument("--t5-path", type=str, default="pretrained_models/t5-ckpt")
     parser.add_argument("--t5-model-type", type=str, default="flan-t5-xl")
     parser.add_argument("--t5-feature-max-len", type=int, default=120)
