@@ -236,8 +236,8 @@ int         lg_vq_set_cta_budget(int ctas);
 int  lg_test_gemm(const void* x, const void* w, int M, int N, int K, int dtype, float* y,
                   void* dev_scratch, size_t scratch_bytes, void* stream);
 
-/* One transformer attention call through the engine's own dispatch (honouring LG_ATTN_TMA, LG_ATTN_PREFILL_TC, LG_ATTN_NST
- * and LG_ATTN_DEEP). dtype: the model dtype (LG_DTYPE_F32, _BF16 or _F16); kv_dtype: dtype, or LG_DTYPE_E4M3 for a
+/* One transformer attention call through the engine's own dispatch, attn_plan (honouring LG_ATTN_TMA, LG_ATTN_PREFILL_TC,
+ * LG_ATTN_NST and LG_ATTN_DEEP). dtype: the model dtype (LG_DTYPE_F32, _BF16 or _F16); kv_dtype: dtype, or LG_DTYPE_E4M3 for a
  * 16-bit model with k_scale / v_scale powers of two in [2^-8, 2^7] (otherwise both 1). kcache / vcache: dev [n_layer][R][H][max_seq]
  * [hdp] in the KV dtype, hdp = the engine's row width: 112 for hd 100 in a bf16 / fp16 model, hd otherwise (dims hd..hdp-1 are
  * padding and do not affect the result); `layer` is the one attended to. The tensor maps span all n_layer layers, as
@@ -255,6 +255,13 @@ int  lg_test_attention(int dtype, int kv_dtype, float k_scale, float v_scale, in
                        void* kcache, void* vcache, int n_layer, int layer, int pos_value, const int32_t* pos_dev,
                        const int32_t* pos_rows, const float* emb_mask, int B, int Tc, const void* q, const float* qkv_partial,
                        int ksplit, const float* freqs, int fuse, void* q_out, void* out, int* path, void* stream);
+/* The dispatch of lg_test_attention without buffers or a GPU: after the same checks of the shape-only arguments, plan (int[3])
+ * receives the (kernel, ring depth, fused) that lg_test_attention reports for the call over an n_layer-layer buffer. pos_kind: 0 =
+ * pos_value alone, 1 = a device counter plus pos_value, 2 = per-row positions (pos_value 0). input: 0 = q, 1 = QKV slabs with
+ * fuse = 0, 2 = QKV slabs with fuse = 1. The tensor maps count as built when lg_test_attention would build them (bf16 / fp16 rows of
+ * a supported width, fewer than 2^31 rows over all layers); none is encoded. */
+int  lg_test_attention_plan(int dtype, int kv_dtype, int R, int Tq, int H, int hd, int hdp, int max_seq, int n_layer, int pos_kind,
+                            int pos_value, int input, int* plan);
 
 /* The acceptance step of lg_generate_sjd alone, on caller buffers (dev): p, q f32 [B * L][V], qflag, x, win int32 [B * L], nfin,
  * start int32 [B] (updated), out int32 [B][S] (accepted tokens written). Every image must have nfin < S. */

@@ -101,6 +101,8 @@ SIGNATURES = {
     "lg_test_attention": (c_int, [c_int, c_int, c_float, c_float, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                                   c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int,
                                   c_void_p, c_int, c_void_p, c_void_p, POINTER(c_int), c_void_p]),
+    "lg_test_attention_plan": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                       POINTER(c_int)]),
     "lg_test_vq_conv": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                                 c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_size_t,
                                 c_void_p, c_size_t, POINTER(c_int), POINTER(c_int), c_void_p]),

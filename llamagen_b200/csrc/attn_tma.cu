@@ -437,9 +437,20 @@ __global__ void __launch_bounds__(kWarps * 32 * (PAR_ ? NST : 1), PAR_ ? 1 : (HD
     }
 }
 
-template <typename T, int HD, bool FUSED, int NST = kStagesA, bool PAR = (NST > 2), bool F8 = false>
-int launch_t(const CUtensorMap& kmap, const CUtensorMap& vmap, const CUtensorMap& kmap16, const CUtensorMap& vmap16,
-             const AttnTmaArgs& a, cudaStream_t st, const KvScales& f8s) {
+// The AttnTmaArgs of a call (kernels 1-4)
+AttnTmaArgs tma_args(const AttnArgs& a) {
+    AttnTmaArgs t{};
+    t.q = (const bf16*)a.q; t.out = (bf16*)a.out; t.R = a.R; t.H = a.H; t.maxS = a.maxS;
+    t.pos_dev = a.pos.dev; t.pos_value = a.pos.value; t.pos_rows = a.pos.rows; t.row_base = a.cache_row_base;
+    t.emb_mask = a.emb_mask; t.B = a.B; t.Tc = a.Tc; t.scale = a.scale;
+    t.partial = a.qkv_partial; t.ksplit = a.qkv_ksplit; t.freqs = a.freqs;
+    t.kcache = (bf16*)const_cast<void*>(a.kcache); t.vcache = (bf16*)const_cast<void*>(a.vcache);
+    t.hd = a.hd; t.hdp = a.hdp ? a.hdp : a.hd;
+    return t;
+}
+
+template <typename T, int HD, bool FUSED, int NST, bool PAR, bool F8>
+int launch_t(const AttnArgs& a, cudaStream_t st) {
     constexpr int TILE_BYTES = F8 ? kKC * (HD == 64 ? 64 : 128) : (HD / 64) * kKC * 128;
     constexpr int NW = PAR ? NST * kWarps : kWarps;
     const size_t smem = 1024 + (size_t)NST * 2 * TILE_BYTES + NST * sizeof(uint64_t) +
@@ -448,8 +459,12 @@ int launch_t(const CUtensorMap& kmap, const CUtensorMap& vmap, const CUtensorMap
     if (lg_first_on_device(attr)) {
         LG_CUDA_OK(cudaFuncSetAttribute(attn_tma_kernel<T, HD, FUSED, NST, PAR, F8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
+    AttnTmaArgs t = tma_args(a);
+    t.kvhint = tma::kL2EvictFirst;   // each K/V byte is read once per step
+    auto map = [](const void* m) -> const CUtensorMap& { return *reinterpret_cast<const CUtensorMap*>(m); };
     dim3 grid(a.H, a.R);
-    (void)lg_launch(attn_tma_kernel<T, HD, FUSED, NST, PAR, F8>, dim3(grid), dim3(NW * 32), smem, st, kmap, vmap, kmap16, vmap16, a, f8s);
+    (void)lg_launch(attn_tma_kernel<T, HD, FUSED, NST, PAR, F8>, dim3(grid), dim3(NW * 32), smem, st, map(a.kmap), map(a.vmap),
+                    map(a.kmap16), map(a.vmap16), t, KvScales{a.k_inv, a.v_inv, a.v_scale});
     LG_LAUNCH_CHECK();
     return 0;
 }
@@ -843,47 +858,6 @@ __global__ void __launch_bounds__(128) attn_window_tc_kernel(const __grid_consta
     causal_tc_body<T, HD, true>(kmap, vmap, a, Tq);
 }
 
-bool attn_causal_tc_supported(const AttnArgs& a) {
-    const bool shape = a.hd == 64 || a.hd == 128 || (a.hd == 100 && a.hdp == 112);
-    return lg_dtype_is16(a.dtype) && !a.kv_f8 && shape && a.Tq > kPfRows && a.kmap && a.vmap && a.pos.dev == nullptr &&
-           a.pos.rows == nullptr && a.pos.value == 0 && a.maxS >= a.Tq && a.R <= 65535;
-}
-
-// window = true: attn_window_tc_kernel (one query block per row, at the row's own position), else attn_causal_tc_kernel
-static int launch_causal_tc(const AttnArgs& a, cudaStream_t st, int* path, bool window) {
-    AttnTmaArgs t{};
-    t.q = (const bf16*)a.q; t.out = (bf16*)a.out; t.R = a.R; t.H = a.H; t.maxS = a.maxS;
-    t.pos_rows = a.pos.rows;
-    t.row_base = a.cache_row_base; t.emb_mask = a.emb_mask; t.B = a.B; t.Tc = a.Tc; t.scale = a.scale;
-    t.hd = a.hd; t.hdp = a.hdp ? a.hdp : a.hd;
-    const bool half = a.dtype == LG_DTYPE_F16, wide = a.hd != 64;
-    auto kern = window ? (wide ? (half ? attn_window_tc_kernel<f16, 128> : attn_window_tc_kernel<bf16, 128>)
-                               : (half ? attn_window_tc_kernel<f16, 64> : attn_window_tc_kernel<bf16, 64>))
-                       : (wide ? (half ? attn_causal_tc_kernel<f16, 128> : attn_causal_tc_kernel<bf16, 128>)
-                               : (half ? attn_causal_tc_kernel<f16, 64> : attn_causal_tc_kernel<bf16, 64>));
-    const size_t smem = 1024 + (size_t)kCqStages * 2 * (wide ? 2 : 1) * kCqKeys * 128 + kCqStages * sizeof(uint64_t);
-    static DevOnce attr[8];
-    if (lg_first_on_device(attr[(half ? 1 : 0) + (wide ? 2 : 0) + (window ? 4 : 0)])) {
-        LG_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    }
-    dim3 grid(a.H, a.R, (a.Tq + kCqRows - 1) / kCqRows);
-    (void)lg_launch(kern, dim3(grid), dim3(128), smem, st, *reinterpret_cast<const CUtensorMap*>(a.kmap),
-                    *reinterpret_cast<const CUtensorMap*>(a.vmap), t, a.Tq);
-    LG_LAUNCH_CHECK();
-    set_attn_path(path, window ? 4 : 2, kCqStages, 0);
-    return 0;
-}
-
-int launch_attention_causal_tc(const AttnArgs& a, cudaStream_t st, int* path) { return launch_causal_tc(a, st, path, false); }
-
-bool attn_window_tc_supported(const AttnArgs& a) {
-    const bool shape = a.hd == 64 || a.hd == 128 || (a.hd == 100 && a.hdp == 112);
-    return lg_dtype_is16(a.dtype) && !a.kv_f8 && shape && a.Tq >= 2 && a.Tq <= kCqRows && a.kmap && a.vmap && a.pos.rows != nullptr &&
-           a.R <= 65535;
-}
-
-int launch_attention_window_tc(const AttnArgs& a, cudaStream_t st, int* path) { return launch_causal_tc(a, st, path, true); }
-
 // KV-cache tensor maps: the whole K (or V) region of the workspace as one [rows, hd] bf16 / fp16 matrix, or (dtype LG_DTYPE_E4M3)
 // one [rows, hdp] byte matrix read in boxes of 64 bytes (hd 64) or 128 bytes (hdp 128 or 112; bytes 112..127 read as zeros)
 int attn_tma_make_map(void* map_out, const void* cache_base, long long total_rows, int hdp, int dtype, int tail16) {
@@ -892,23 +866,55 @@ int attn_tma_make_map(void* map_out, const void* cache_base, long long total_row
                             tail16 ? 16 : kKC, dtype == LG_DTYPE_E4M3 ? (hdp == 64 ? 64 : 128) : 64, dtype);
 }
 
+// Head shapes of the TMA kernels: hd 64 or 128, or hd 100 in 112-wide rows (the maps read 112..127 as zeros)
+static bool tma_head_shape(int hd, int hdp) { return hd == 64 || hd == 128 || (hd == 100 && hdp == 112); }
+
 bool attn_tma_maps_usable(int dtype, int hd, int hdp, long long total_rows) {
-    return lg_dtype_is16(dtype) && (hd == 64 || hd == 128 || hdp == 112) && total_rows < (1ll << 31);
+    return lg_dtype_is16(dtype) && tma_head_shape(hd, hdp) && total_rows < (1ll << 31);
 }
 
-bool attn_tma_enabled() { return lg_env_flag("LG_ATTN_TMA", 1) != 0; }
-
-bool attn_prefill_tc_supported(const AttnArgs& a) {
-    return lg_dtype_is16(a.dtype) && a.hd == 64 && (a.hdp == 0 || a.hdp == 64) && a.Tq > 1 && a.Tq <= kPfRows && a.kmap && a.vmap &&
-           a.pos.dev == nullptr && a.pos.rows == nullptr && a.pos.value == 0 && a.R <= 65535 && a.maxS >= kPfBoxes * kKC &&
-           lg_env_flag("LG_ATTN_PREFILL_TC", 1) != 0;
+AttnPlan attn_plan(const AttnArgs& a) {
+    AttnPlan p;
+    auto plan = [&](int kernel, int stages) { p.kernel = kernel; p.stages = stages; return p; };
+    const bool fused = a.qkv_partial != nullptr;
+    const bool from0 = a.pos.dev == nullptr && a.pos.rows == nullptr && a.pos.value == 0;   // query t sits at position t
+    // kernels 1-4: a 16-bit model whose cache the maps cover, one grid row per sequence row
+    const bool tma = lg_env_flag("LG_ATTN_TMA", 1) && lg_dtype_is16(a.dtype) && tma_head_shape(a.hd, a.hdp) && a.kmap && a.vmap &&
+                     a.R <= 65535;
+    if (tma && a.Tq == 1 && a.kmap16 && a.vmap16) {
+        p.fused = fused;
+        // few (row, head) items (batch-1 latency path): an 8-stage ring (kKC = 32) holds a whole 256-key context, so every K/V byte
+        // is requested before the dependency wait instead of two stages at a time
+        if (fused && a.hd == 64 && a.R * a.H <= 2 * 132 && lg_env_flag("LG_ATTN_DEEP", 1)) return plan(1, kDeepStages);
+        // deeper sequential ring (A/B switch): more keys requested before the dependency wait, fewer refill round trips
+        if (fused && a.hd == 64 && lg_env_flag("LG_ATTN_NST", 2) == 3) return plan(1, 3);
+        return plan(1, kStagesA);
+    }
+    if (tma && !fused && a.hd == 64 && (a.hdp == 0 || a.hdp == 64) && a.Tq > 1 && a.Tq <= kPfRows && from0 && a.maxS >= kPfBoxes * kKC &&
+        lg_env_flag("LG_ATTN_PREFILL_TC", 1))
+        return plan(3, 1);
+    const bool tc16 = tma && !fused && !a.kv_f8;   // kernels 2 and 4: a 16-bit cache in the model dtype
+    if (tc16 && a.Tq > kPfRows && from0 && a.maxS >= a.Tq) return plan(2, kCqStages);
+    if (tc16 && a.Tq >= 2 && a.Tq <= kCqRows && a.pos.rows) return plan(4, kCqStages);
+    if (fused) snprintf(p.error, sizeof(p.error), "attention: fused QKV epilogue requested on a path that does not support it");
+    else if ((long long)a.R * a.Tq > 65535) snprintf(p.error, sizeof(p.error), "attention: too many query rows (%d x %d)", a.R, a.Tq);
+    else if ((a.hdp ? a.hdp : a.hd) != attn_kv_row_width(a.dtype, a.hd))
+        snprintf(p.error, sizeof(p.error), "attention: KV row width %d for head_dim %d", a.hdp, a.hd);
+    else p.kernel = 0;
+    return p;
 }
 
-int launch_attention_prefill_tc(const AttnArgs& a, cudaStream_t st, int* path) {
-    AttnTmaArgs t{};
-    t.q = (const bf16*)a.q; t.out = (bf16*)a.out; t.R = a.R; t.H = a.H; t.maxS = a.maxS;
-    t.row_base = a.cache_row_base; t.emb_mask = a.emb_mask; t.B = a.B; t.Tc = a.Tc; t.scale = a.scale;
-    t.hd = a.hd; t.hdp = a.hd;
+// attn_tma_kernel at the plan's head dim, fusion and ring depth
+template <typename T, bool F8>
+static int launch_decode(const AttnArgs& a, const AttnPlan& p, cudaStream_t st) {
+    const bool hd64 = a.hd == 64;
+    if (!p.fused) return hd64 ? launch_t<T, 64, false, kStagesA, false, F8>(a, st) : launch_t<T, 128, false, kStagesA, false, F8>(a, st);
+    if (p.stages == kDeepStages) return launch_t<T, 64, true, kDeepStages, true, F8>(a, st);
+    if (p.stages == 3) return launch_t<T, 64, true, 3, false, F8>(a, st);
+    return hd64 ? launch_t<T, 64, true, kStagesA, false, F8>(a, st) : launch_t<T, 128, true, kStagesA, false, F8>(a, st);
+}
+
+static int launch_prefill_tc(const AttnArgs& a, cudaStream_t st) {
     CUtensorMap qmap;
     LG_TRY(tma::make_map_2d(&qmap, a.q, (uint64_t)a.R * a.Tq, (uint64_t)a.H * a.hd, (uint64_t)a.H * a.hd, kPfRows, 64, a.dtype));
     const size_t smem = 1024 + (size_t)kPfRows * 128 + 2 * (size_t)kPfBoxes * kKC * (a.kv_f8 ? 64 : 128) + 16;
@@ -921,56 +927,40 @@ int launch_attention_prefill_tc(const AttnArgs& a, cudaStream_t st, int* path) {
         LG_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
     dim3 grid(a.H, a.R);
-    const KvScales f8s{a.k_inv, a.v_inv, a.v_scale};
     (void)lg_launch(kern, dim3(grid), dim3(256), smem, st, qmap, *reinterpret_cast<const CUtensorMap*>(a.kmap),
-                    *reinterpret_cast<const CUtensorMap*>(a.vmap), t, a.Tq, f8s);
+                    *reinterpret_cast<const CUtensorMap*>(a.vmap), tma_args(a), a.Tq, KvScales{a.k_inv, a.v_inv, a.v_scale});
     LG_LAUNCH_CHECK();
-    set_attn_path(path, 3, 1, 0);
     return 0;
 }
 
-bool attn_tma_supported(const AttnArgs& a) {
-    const bool shape = a.hd == 64 || a.hd == 128 || (a.hd == 100 && a.hdp == 112);
-    return lg_dtype_is16(a.dtype) && a.Tq == 1 && shape && a.kmap && a.vmap && a.kmap16 && a.vmap16 && a.R <= 65535;
-}
-
-template <typename T, bool F8 = false>
-static int launch_attention_tma_t(const AttnArgs& a, cudaStream_t st, int* path) {
-    AttnTmaArgs t;
-    const KvScales f8s{a.k_inv, a.v_inv, a.v_scale};
-    t.q = (const bf16*)a.q; t.out = (bf16*)a.out; t.R = a.R; t.H = a.H; t.maxS = a.maxS;
-    t.pos_dev = a.pos.dev; t.pos_value = a.pos.value; t.pos_rows = a.pos.rows; t.row_base = a.cache_row_base;
-    t.emb_mask = a.emb_mask; t.B = a.B; t.Tc = a.Tc; t.scale = a.scale;
-    t.partial = a.qkv_partial; t.ksplit = a.qkv_ksplit; t.freqs = a.freqs;
-    t.kcache = (bf16*)const_cast<void*>(a.kcache); t.vcache = (bf16*)const_cast<void*>(a.vcache);
-    t.kvhint = tma::kL2EvictFirst;   // each K/V byte is read once per step
-    t.hd = a.hd; t.hdp = a.hdp ? a.hdp : a.hd;
-    const CUtensorMap& km = *reinterpret_cast<const CUtensorMap*>(a.kmap);
-    const CUtensorMap& vm = *reinterpret_cast<const CUtensorMap*>(a.vmap);
-    const CUtensorMap& km16 = *reinterpret_cast<const CUtensorMap*>(a.kmap16);
-    const CUtensorMap& vm16 = *reinterpret_cast<const CUtensorMap*>(a.vmap16);
-    const int fused = a.qkv_partial ? 1 : 0;
-    auto ran = [&](int rc, int kernel, int stages) {
-        if (rc == 0) set_attn_path(path, kernel, stages, fused);
-        return rc;
-    };
-    if (a.qkv_partial) {     // fused QKV epilogue
-        // few (row, head) items (batch-1 latency path): an 8-stage ring (kKC = 32) holds a whole 256-key context, so every K/V byte
-        // is requested before the dependency wait instead of two stages at a time
-        if (a.hd == 64 && a.R * a.H <= 2 * 132 && lg_env_flag("LG_ATTN_DEEP", 1))
-            return ran(launch_t<T, 64, true, kDeepStages, (kDeepStages > 2), F8>(km, vm, km16, vm16, t, st, f8s), 1, kDeepStages);
-        // deeper sequential ring (A/B switch): more keys requested before the dependency wait, fewer refill round trips
-        if (a.hd == 64 && lg_env_flag("LG_ATTN_NST", 2) == 3)
-            return ran(launch_t<T, 64, true, 3, false, F8>(km, vm, km16, vm16, t, st, f8s), 1, 3);
-        if (a.hd == 64) return ran(launch_t<T, 64, true, kStagesA, false, F8>(km, vm, km16, vm16, t, st, f8s), 1, kStagesA);
-        return ran(launch_t<T, 128, true, kStagesA, false, F8>(km, vm, km16, vm16, t, st, f8s), 1, kStagesA);
+// window = true: attn_window_tc_kernel (one query block per row, at the row's own position), else attn_causal_tc_kernel
+static int launch_causal_tc(const AttnArgs& a, cudaStream_t st, bool window) {
+    const bool half = a.dtype == LG_DTYPE_F16, wide = a.hd != 64;
+    auto kern = window ? (wide ? (half ? attn_window_tc_kernel<f16, 128> : attn_window_tc_kernel<bf16, 128>)
+                               : (half ? attn_window_tc_kernel<f16, 64> : attn_window_tc_kernel<bf16, 64>))
+                       : (wide ? (half ? attn_causal_tc_kernel<f16, 128> : attn_causal_tc_kernel<bf16, 128>)
+                               : (half ? attn_causal_tc_kernel<f16, 64> : attn_causal_tc_kernel<bf16, 64>));
+    const size_t smem = 1024 + (size_t)kCqStages * 2 * (wide ? 2 : 1) * kCqKeys * 128 + kCqStages * sizeof(uint64_t);
+    static DevOnce attr[8];
+    if (lg_first_on_device(attr[(half ? 1 : 0) + (wide ? 2 : 0) + (window ? 4 : 0)])) {
+        LG_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
-    if (a.hd == 64) return ran(launch_t<T, 64, false, kStagesA, false, F8>(km, vm, km16, vm16, t, st, f8s), 1, kStagesA);
-    return ran(launch_t<T, 128, false, kStagesA, false, F8>(km, vm, km16, vm16, t, st, f8s), 1, kStagesA);
+    dim3 grid(a.H, a.R, (a.Tq + kCqRows - 1) / kCqRows);
+    (void)lg_launch(kern, dim3(grid), dim3(128), smem, st, *reinterpret_cast<const CUtensorMap*>(a.kmap),
+                    *reinterpret_cast<const CUtensorMap*>(a.vmap), tma_args(a), a.Tq);
+    LG_LAUNCH_CHECK();
+    return 0;
 }
 
-int launch_attention_tma(const AttnArgs& a, cudaStream_t st, int* path) {
-    if (a.kv_f8)
-        return a.dtype == LG_DTYPE_F16 ? launch_attention_tma_t<f16, true>(a, st, path) : launch_attention_tma_t<bf16, true>(a, st, path);
-    return a.dtype == LG_DTYPE_F16 ? launch_attention_tma_t<f16>(a, st, path) : launch_attention_tma_t<bf16>(a, st, path);
+int launch_attention_tma(const AttnArgs& a, const AttnPlan& p, cudaStream_t st) {
+    const bool half = a.dtype == LG_DTYPE_F16;
+    switch (p.kernel) {
+        case 1:
+            if (a.kv_f8) return half ? launch_decode<f16, true>(a, p, st) : launch_decode<bf16, true>(a, p, st);
+            return half ? launch_decode<f16, false>(a, p, st) : launch_decode<bf16, false>(a, p, st);
+        case 2: return launch_causal_tc(a, st, false);
+        case 3: return launch_prefill_tc(a, st);
+        case 4: return launch_causal_tc(a, st, true);
+    }
+    return lg_fail("attention: kernel %d is not one of the TMA kernels", p.kernel);
 }

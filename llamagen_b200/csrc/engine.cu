@@ -154,6 +154,10 @@ QkvEpiArgs make_qkv_epi_args(const AttnArgs& aa, const float* partial, int kspli
     return qa;
 }
 
+// Whether the attention kernel of `aa` (a call without QKV slabs) is also its QKV epilogue, one dependent kernel less: decode steps
+// that run on the TMA decode kernel
+bool fuse_qkv(const AttnArgs& aa) { return lg_env_flag("LG_FUSE_QKV", 1) && attn_plan(aa).kernel == 1; }
+
 SampleArgs make_sample_args(const lg_sample_cfg& sc, const float* logits, int B, int V, int mix_cfg, int round_dtype) {
     SampleArgs a{};
     a.logits = logits; a.B = B; a.V = V; a.mix_cfg = mix_cfg; a.round_dtype = lg_dtype_is16(round_dtype) ? round_dtype : LG_DTYPE_F32;
@@ -240,9 +244,9 @@ struct lg_engine {
     // R <= 8 decode steps on the column-owner GEMV path (gemv_small.cu); shared by forward() and the decode loop's fused tail
     bool small_row_path(int M, const AttnArgs& aa) const {
         const int D = cfg.dim, F = cfg.ffn_dim, V = cfg.vocab_size, dt = cfg.dtype;
-        return M <= 8 && lg_env_flag("LG_SMALL_R", 1) && lg_env_flag("LG_FUSE_QKV", 1) && attn_tma_enabled() && attn_tma_supported(aa) &&
-               gemv_small_supported(M, 3 * D, D, dt, false) && gemv_small_supported(M, D, D, dt, false) &&
-               gemv_small_supported(M, F, D, dt, true) && gemv_small_supported(M, D, F, dt, false) && gemv_small_supported(M, V, D, dt, false);
+        return M <= 8 && lg_env_flag("LG_SMALL_R", 1) && fuse_qkv(aa) && gemv_small_supported(M, 3 * D, D, dt, false) &&
+               gemv_small_supported(M, D, D, dt, false) && gemv_small_supported(M, F, D, dt, true) &&
+               gemv_small_supported(M, D, F, dt, false) && gemv_small_supported(M, V, D, dt, false);
     }
     size_t carve(Workspace& o, char* base, int rows, int max_seq, int g = 0, int n = 1) const;
     size_t carve_score(Workspace& o, char* base, int rows, int seq) const;
@@ -484,9 +488,7 @@ int lg_engine::run_layers(const Workspace& w, int M, int Tq, PosArg pos, const f
         GemmNext nx_qkv{(l + 1 < L) ? layers[l + 1].wqkv : output, (l + 1 < L) ? (size_t)3 * D * D * eb : (size_t)V * D * eb, nullptr, 0};
         LG_PROF(PC_GEMM_QKV, st, gemm(w, w.xn, M, 3 * D, D, ly.wqkv, nullptr, 0, &ks, nullptr, st, &nx_wo));
         AttnArgs aa = layer_attn(w, l, R, Tq, pos, emb_mask, B);
-        // decode steps on the TMA path: the attention kernel is also the QKV epilogue (one dependent kernel less)
-        const bool fuse_qkv = lg_env_flag("LG_FUSE_QKV", 1) && attn_tma_enabled() && attn_tma_supported(aa);
-        if (fuse_qkv) {
+        if (fuse_qkv(aa)) {
             aa.qkv_partial = w.partial; aa.qkv_ksplit = ks; aa.freqs = freqs;
         } else {
             LG_PROF(PC_QKV_EPI, st, launch_qkv_epilogue(make_qkv_epi_args(aa, w.partial, ks, freqs), st));
@@ -795,11 +797,8 @@ int lg_score(lg_engine* e, const void* cond, const float* emb_mask, const int32_
     // is not on a tensor-core path (fp32 models, or LG_ATTN_TMA=0)
     auto fits = [&](int nb) {
         Workspace w;
-        if (e->carve_score(w, (char*)dev_ws, nh * nb, seq) > ws_bytes) return false;
-        if ((long long)nh * nb * seq <= 65535) return true;
-        if (e->make_maps(w) != 0) return false;
-        const AttnArgs aa = e->attn_args(w, 0, nh * nb, seq);
-        return attn_tma_enabled() && (attn_causal_tc_supported(aa) || attn_prefill_tc_supported(aa) || attn_tma_supported(aa));
+        return e->carve_score(w, (char*)dev_ws, nh * nb, seq) <= ws_bytes && e->make_maps(w) == 0 &&
+               attn_plan(e->attn_args(w, 0, nh * nb, seq)).kernel >= 0;
     };
     {
         Workspace one;
@@ -1211,54 +1210,87 @@ int lg_test_gemm(const void* x, const void* w, int M, int N, int K, int dtype, f
     return launch_reduce_f32((const float*)dev_scratch, plan.ksplit, M, N, y, st);
 }
 
+// What lg_test_attention and lg_test_attention_plan (fn) check of the shape-only arguments, then the call's AttnArgs (no QKV slabs
+// attached yet) over a K / V buffer of n_layer layers, with `maps` as the engine builds them (without a buffer: only whether it would),
+// held to the dispatch rules: more than 65535 query rows only on kernel 2, slabs fused into the attention (`fused`) only on kernel 1
+static int test_attention_args(const char* fn, KvMaps& maps, AttnArgs& aa, int dtype, int kv_dtype, const float* kv_scales, int R, int Tq,
+                               int H, int hd, int hdp, int max_seq, void* kcache, void* vcache, int n_layer, int layer, PosArg pos,
+                               bool fused) {
+    LG_REQUIRE(dtype == LG_DTYPE_F32 || lg_dtype_is16(dtype), "%s: unsupported model dtype %d", fn, dtype);
+    LG_REQUIRE(kv_dtype == dtype || (kv_dtype == LG_DTYPE_E4M3 && lg_dtype_is16(dtype)),
+               "%s: KV dtype %d with model dtype %d (the model dtype, or LG_DTYPE_E4M3 for a bf16 / fp16 model)", fn, kv_dtype, dtype);
+    LG_REQUIRE(R > 0 && Tq > 0 && H > 0 && max_seq > 0 && n_layer > 0 && layer >= 0 && layer < n_layer,
+               "%s: bad shape R=%d Tq=%d H=%d max_seq=%d layer %d of %d", fn, R, Tq, H, max_seq, layer, n_layer);
+    LG_REQUIRE(hd == 64 || hd == 100 || hd == 128, "%s: unsupported head_dim %d (64, 100, 128)", fn, hd);
+    LG_REQUIRE(hdp == attn_kv_row_width(dtype, hd), "%s: row width %d for head_dim %d", fn, hdp, hd);
+    if (pos.rows) {
+        LG_REQUIRE(pos.dev == nullptr && pos.value == 0, "%s: per-row positions take no counter and no value", fn);
+    } else {
+        LG_REQUIRE(pos.value >= 0 && (pos.dev || pos.value + Tq <= max_seq), "%s: position %d + Tq %d exceeds max_seq %d", fn,
+                   pos.value, Tq, max_seq);
+    }
+    const long long rows = (long long)n_layer * R * H * max_seq;
+    if (kcache) LG_TRY(make_kv_maps(maps, dtype, hd, hdp, kv_dtype, kcache, vcache, rows));
+    else maps.usable = attn_tma_maps_usable(dtype, hd, hdp, rows);
+    aa = make_attn_args(dtype, H, hd, hdp, R, max_seq, (char*)kcache, (char*)vcache, maps, kv_dtype == LG_DTYPE_E4M3 ? kv_scales : nullptr,
+                        layer, R, Tq);
+    aa.pos = pos;
+    const AttnPlan p = attn_plan(aa);
+    LG_REQUIRE((long long)R * Tq <= 65535 || p.kernel == 2,
+               "%s: bad shape R=%d Tq=%d: more than 65535 query rows need the causal tensor-core kernel", fn, R, Tq);
+    LG_REQUIRE(!fused || p.kernel == 1, "%s: the fused QKV epilogue needs the TMA decode kernel", fn);
+    return 0;
+}
+
 int lg_test_attention(int dtype, int kv_dtype, float k_scale, float v_scale, int R, int Tq, int H, int hd, int hdp, int max_seq,
                       void* kcache, void* vcache, int n_layer, int layer, int pos_value, const int32_t* pos_dev,
                       const int32_t* pos_rows, const float* emb_mask, int B, int Tc, const void* q, const float* qkv_partial,
                       int ksplit, const float* freqs, int fuse, void* q_out, void* out, int* path, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     auto a16 = [](const void* p) { return ((uintptr_t)p & 15) == 0; };
-    const bool f8 = kv_dtype == LG_DTYPE_E4M3;
-    LG_REQUIRE(dtype == LG_DTYPE_F32 || lg_dtype_is16(dtype), "lg_test_attention: unsupported model dtype %d", dtype);
-    LG_REQUIRE(kv_dtype == dtype || (f8 && lg_dtype_is16(dtype)),
-               "lg_test_attention: KV dtype %d with model dtype %d (the model dtype, or LG_DTYPE_E4M3 for a bf16 / fp16 model)", kv_dtype,
-               dtype);
-    LG_REQUIRE(f8 ? kv_scale_ok(k_scale) && kv_scale_ok(v_scale) : k_scale == 1.f && v_scale == 1.f,
+    LG_REQUIRE(kv_dtype == LG_DTYPE_E4M3 ? kv_scale_ok(k_scale) && kv_scale_ok(v_scale) : k_scale == 1.f && v_scale == 1.f,
                "lg_test_attention: K / V scales %g / %g (fp8: powers of two in [2^-8, 2^7], otherwise 1)", (double)k_scale, (double)v_scale);
-    LG_REQUIRE(R > 0 && Tq > 0 && H > 0 && max_seq > 0 && n_layer > 0 && layer >= 0 && layer < n_layer,
-               "lg_test_attention: bad shape R=%d Tq=%d H=%d max_seq=%d layer %d of %d", R, Tq, H, max_seq, layer, n_layer);
-    LG_REQUIRE(hd == 64 || hd == 100 || hd == 128, "lg_test_attention: unsupported head_dim %d (64, 100, 128)", hd);
-    LG_REQUIRE(hdp == attn_kv_row_width(dtype, hd), "lg_test_attention: row width %d for head_dim %d", hdp, hd);
     LG_REQUIRE(kcache && vcache && out && a16(kcache) && a16(vcache) && a16(out) && a16(q) && a16(q_out) && a16(qkv_partial) && a16(freqs),
                "lg_test_attention: null or misaligned (16 bytes) buffer");
-    if (pos_rows) {
-        LG_REQUIRE(pos_dev == nullptr && pos_value == 0, "lg_test_attention: per-row positions take no counter and no value");
-    } else {
-        LG_REQUIRE(pos_value >= 0 && (pos_dev || pos_value + Tq <= max_seq), "lg_test_attention: position %d + Tq %d exceeds max_seq %d",
-                   pos_value, Tq, max_seq);
-    }
     LG_REQUIRE(!emb_mask || (B > 0 && Tc > 0 && Tc <= max_seq), "lg_test_attention: emb_mask needs B > 0 and 0 < Tc <= max_seq (B=%d Tc=%d)",
                B, Tc);
     LG_REQUIRE((q != nullptr) != (qkv_partial != nullptr), "lg_test_attention: pass exactly one of q and qkv_partial");
     LG_REQUIRE(q ? fuse == 0 : (ksplit > 0 && freqs && (fuse == 1 || (fuse == 0 && q_out))),
                "lg_test_attention: q takes fuse = 0; qkv_partial needs ksplit > 0, freqs and fuse = 1 or q_out");
-    KvMaps maps;   // as the engine builds them: over every layer of the buffer
-    LG_TRY(make_kv_maps(maps, dtype, hd, hdp, f8 ? LG_DTYPE_E4M3 : dtype, kcache, vcache, (long long)n_layer * R * H * max_seq));
+    KvMaps maps;
+    AttnArgs aa;
     const float scales[2] = {k_scale, v_scale};
-    AttnArgs aa = make_attn_args(dtype, H, hd, hdp, R, max_seq, (char*)kcache, (char*)vcache, maps, f8 ? scales : nullptr, layer, R, Tq);
+    LG_TRY(test_attention_args("lg_test_attention", maps, aa, dtype, kv_dtype, scales, R, Tq, H, hd, hdp, max_seq, kcache, vcache, n_layer,
+                               layer, PosArg{pos_dev, pos_value, pos_rows}, qkv_partial && fuse));
     aa.q = q ? q : q_out; aa.out = out;
-    aa.pos = PosArg{pos_dev, pos_value, pos_rows};
     aa.emb_mask = emb_mask; aa.B = emb_mask ? B : 1; aa.Tc = emb_mask ? Tc : 0;
-    LG_REQUIRE((long long)R * Tq <= 65535 || (attn_tma_enabled() && attn_causal_tc_supported(aa)),
-               "lg_test_attention: bad shape R=%d Tq=%d: more than 65535 query rows need the causal tensor-core kernel", R, Tq);
     if (qkv_partial) {
         if (fuse) {
-            LG_REQUIRE(attn_tma_enabled() && attn_tma_supported(aa), "lg_test_attention: the fused QKV epilogue needs the TMA decode kernel");
             aa.qkv_partial = qkv_partial; aa.qkv_ksplit = ksplit; aa.freqs = freqs;
         } else {
             LG_TRY(launch_qkv_epilogue(make_qkv_epi_args(aa, qkv_partial, ksplit, freqs), st));
         }
     }
     return launch_attention(aa, st, path);
+}
+
+int lg_test_attention_plan(int dtype, int kv_dtype, int R, int Tq, int H, int hd, int hdp, int max_seq, int n_layer, int pos_kind,
+                           int pos_value, int input, int* plan) {
+    // stand-ins for the call's device buffers: the checks and attn_plan only test them for null
+    static const int32_t pos_buf = 0;
+    static const float slab_buf = 0.f;
+    LG_REQUIRE(pos_kind >= 0 && pos_kind <= 2 && input >= 0 && input <= 2 && plan,
+               "lg_test_attention_plan: pos_kind %d or input %d outside 0..2, or null plan", pos_kind, input);
+    KvMaps maps;
+    AttnArgs aa;
+    const float scales[2] = {1.f, 1.f};
+    LG_TRY(test_attention_args("lg_test_attention_plan", maps, aa, dtype, kv_dtype, scales, R, Tq, H, hd, hdp, max_seq, nullptr, nullptr,
+                               n_layer, 0, PosArg{pos_kind == 1 ? &pos_buf : nullptr, pos_value, pos_kind == 2 ? &pos_buf : nullptr},
+                               input == 2));
+    if (input == 2) aa.qkv_partial = &slab_buf;
+    const AttnPlan p = attn_plan(aa);
+    plan[0] = p.kernel; plan[1] = p.stages; plan[2] = p.fused;
+    return 0;
 }
 
 }  // extern "C"

@@ -178,34 +178,32 @@ struct AttnArgs {
 // KV-cache row width in elements: head_dim 100 of a bf16 / fp16 model (GPT-3B) is stored in 112-wide rows, 16-byte multiples that
 // the TMA attention kernels can stream (dims 100..111 stay zero); every other cache row is hd wide
 inline int attn_kv_row_width(int dtype, int hd) { return hd == 100 && lg_dtype_is16(dtype) ? 112 : hd; }
-// path (optional, int[3]): the kernel that was launched (0 = attention_kernel, 1 = attn_tma_kernel, 2 = attn_causal_tc_kernel,
-// 3 = attn_prefill_tc_kernel, 4 = attn_window_tc_kernel), its TMA ring depth (0 for attention_kernel, 1 for the single-stage prefill) and whether it fused the
-// QKV epilogue
+// The kernel an attention call runs on (attn_tma.cu), in this order of preference; the TMA kernels (1-4) need a 16-bit model with
+// tensor maps over its cache (attn_tma_maps_usable), R <= 65535 and LG_ATTN_TMA other than 0.
+//   1 attn_tma_kernel: decode (Tq = 1). fused = 1 when the call brings the QKV GEMM's split-K slabs: the kernel is also their
+//     epilogue. stages: its TMA ring, 8 for fused hd 64 with R * H <= 264 (LG_ATTN_DEEP), 3 for other fused hd 64 under
+//     LG_ATTN_NST=3, 2 otherwise.
+//   3 attn_prefill_tc_kernel: the t2i condition prefill, 1 < Tq <= 128 from position 0, hd 64, fp8 caches too (LG_ATTN_PREFILL_TC).
+//     TMA-staged Q/K/V, mma.sync QK^T and PV, one CTA per (row, head); stages 1.
+//   2 attn_causal_tc_kernel: teacher-forced sequences, Tq > 128 from position 0 on a cache in the model dtype: a CTA per (head, row,
+//     64-query block), K / V blocks through a 2-stage TMA ring, mma.sync QK^T and PV with an online softmax; no R * Tq limit.
+//   4 attn_window_tc_kernel: speculative-decoding windows, 2 <= Tq <= 64 queries per row at pos.rows[r] + t, same caches as kernel 2,
+//     through the same ring.
+//   0 attention_kernel (xf_kernels.cu): CUDA cores, no fused slabs, R * Tq <= 65535, rows attn_kv_row_width wide; stages 0.
+// kernel -1: no kernel takes the call, `error` says why. The only reader of LG_ATTN_TMA, LG_ATTN_PREFILL_TC, LG_ATTN_DEEP and
+// LG_ATTN_NST.
+struct AttnPlan { int kernel = -1; int stages = 0; int fused = 0; char error[96] = {}; };
+AttnPlan attn_plan(const AttnArgs& a);
+// runs `a` on the kernel attn_plan picks; path (optional, int[3]) receives the plan's {kernel, stages, fused}
 int launch_attention(const AttnArgs& a, cudaStream_t st, int* path = nullptr);
-inline void set_attn_path(int* path, int kernel, int stages, int fused) {
-    if (path) { path[0] = kernel; path[1] = stages; path[2] = fused; }
-}
-// attn_tma.cu — TMA + tensor-core decode attention for bf16 / fp16 caches (dtype: LG_DTYPE_BF16 or LG_DTYPE_F16) and fp8 caches of
-// those models (map dtype LG_DTYPE_E4M3: 64- or 128-byte boxes)
+int launch_attention_tma(const AttnArgs& a, const AttnPlan& p, cudaStream_t st);   // p.kernel 1-4
+// KV-cache tensor maps for bf16 / fp16 caches (dtype: LG_DTYPE_BF16 or LG_DTYPE_F16) and fp8 caches of those models (map dtype
+// LG_DTYPE_E4M3: 64- or 128-byte boxes)
 int attn_tma_make_map(void* map_out /*CUtensorMap, 128 B*/, const void* cache_base, long long total_rows, int hdp, int dtype,
                       int tail16 = 0);
 // whether KV-cache tensor maps are built for a workspace (and the TMA attention kernels can run): 16-bit model, hd 64 / 128 or
 // hd 100 in 112-wide rows, fewer than 2^31 cache rows over all layers
 bool attn_tma_maps_usable(int dtype, int hd, int hdp, long long total_rows);
-bool attn_tma_supported(const AttnArgs& a);
-bool attn_tma_enabled();
-int launch_attention_tma(const AttnArgs& a, cudaStream_t st, int* path = nullptr);
-// t2i condition prefill (1 < Tq <= 128, hd 64, bf16 / fp16): TMA-staged Q/K/V, mma.sync QK^T and PV, one CTA per (row, head)
-bool attn_prefill_tc_supported(const AttnArgs& a);
-int launch_attention_prefill_tc(const AttnArgs& a, cudaStream_t st, int* path = nullptr);
-// teacher-forced sequences (Tq > 128 queries from position 0, bf16 / fp16 cache in the model dtype, hd 64 / 128 / 100-in-112): a CTA
-// per (head, row, 64-query block), K / V blocks through a TMA ring, mma.sync QK^T and PV with an online softmax
-bool attn_causal_tc_supported(const AttnArgs& a);
-int launch_attention_causal_tc(const AttnArgs& a, cudaStream_t st, int* path = nullptr);
-// speculative-decoding windows (2 <= Tq <= 64 queries per row at per-row positions pos.rows[r] + t, same cache and shapes as the causal
-// kernel): a CTA per (head, row) streams the row's K / V blocks [0, pos.rows[r] + Tq) through the causal kernel's TMA ring
-bool attn_window_tc_supported(const AttnArgs& a);
-int launch_attention_window_tc(const AttnArgs& a, cudaStream_t st, int* path = nullptr);
 // VQ convolutions: vq.cu runs them; conv_tc.cu holds the wgmma kernels and chooses the kernel of each call.
 // GroupNorm(32) partial statistics are [B][splits][32 groups][sum, sum of squares] floats. gn_stats_kernel writes at most
 // kGnStatsMaxSplits splits per image; the drain of conv_tcw_kernel writes one per 16x16-pixel tile (and upsample phase) of its input.

@@ -562,14 +562,10 @@ static int launch_attention_t(const AttnArgs& a, cudaStream_t st) {
 }
 
 int launch_attention(const AttnArgs& a, cudaStream_t st, int* path) {
-    if (attn_tma_supported(a) && attn_tma_enabled()) return launch_attention_tma(a, st, path);
-    if (attn_prefill_tc_supported(a) && attn_tma_enabled() && a.qkv_partial == nullptr) return launch_attention_prefill_tc(a, st, path);
-    if (attn_causal_tc_supported(a) && attn_tma_enabled() && a.qkv_partial == nullptr) return launch_attention_causal_tc(a, st, path);
-    if (attn_window_tc_supported(a) && attn_tma_enabled() && a.qkv_partial == nullptr) return launch_attention_window_tc(a, st, path);
-    LG_REQUIRE(a.qkv_partial == nullptr, "attention: fused QKV epilogue requested on a path that does not support it");
-    set_attn_path(path, 0, 0, 0);
-    LG_REQUIRE((long long)a.R * a.Tq <= 65535, "attention: too many query rows (%d x %d)", a.R, a.Tq);
-    LG_REQUIRE((a.hdp ? a.hdp : a.hd) == attn_kv_row_width(a.dtype, a.hd), "attention: KV row width %d for head_dim %d", a.hdp, a.hd);
+    const AttnPlan p = attn_plan(a);
+    if (path) { path[0] = p.kernel; path[1] = p.stages; path[2] = p.fused; }
+    LG_REQUIRE(p.kernel >= 0, "%s", p.error);
+    if (p.kernel > 0) return launch_attention_tma(a, p, st);
     if (a.kv_f8) {   // fp8 cache of a 16-bit model
         if (a.dtype == LG_DTYPE_BF16) {
             if (a.hd == 64) return launch_attention_t<bf16, 64, 8, 8, 64, e4m3>(a, st);
