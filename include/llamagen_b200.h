@@ -236,6 +236,26 @@ int         lg_vq_set_cta_budget(int ctas);
 int  lg_test_gemm(const void* x, const void* w, int M, int N, int K, int dtype, float* y,
                   void* dev_scratch, size_t scratch_bytes, void* stream);
 
+/* One linear layer of the transformer as the engine composes it, all tensors in `dtype` unless stated (dev, 16-byte aligned):
+ * x [M][K]; wa [N][K]; wb [N][K] with epi 2 only (the w1 | w3 pair: the GEMM is x [wa; wb]^T, 2N columns, segment boundary N).
+ * small = 0: the batched kernels. norm_in: x' = RMSNorm(x) * norm_in (eps) in scratch (rmsnorm_kernel), then the GEMM on the kernel
+ * gemm_plan picks into fp32 split-K slabs, then the epilogue:
+ *   epi 0: out_f32 [M][N] f32 = the slabs summed (reduce_f32_kernel)        epi 1: h [M][N] += T(acc) (residual_norm_kernel);
+ *   with norm_out also out [M][N] = RMSNorm(h) * norm_out                  epi 2: out [M][N] = silu(T(acc_a)) * T(acc_b)
+ *   epi 3: out [M][N] = T(acc)                                              epi 4: out [M][N] = gelu_tanh(T(acc)) (store_act_kernel)
+ * acc_out (f32 [M][N or 2N], optional): the slabs summed in slab order, as the epilogues sum them.
+ * small = 1: one gemv_small call (bf16 / fp16, M <= 8; norm_in is its RMSNorm prologue; epi 0, 1 without norm_out, or 2; no acc_out).
+ * path (int[4], optional): {kernel, tile, ksplit, row blocks or PF}; kernel 0 = gemm_skinny_kernel, 1 = gemm_mma_kernel,
+ * 2 = gemm_tc_kernel, 3 = gemv_small_kernel (tile: its weight rows per CTA, ksplit 1, then its k chunks in flight PF).
+ * Every argument is checked before any launch. Scratch: 256-byte aligned (NULL when the call needs none); the call fails with the
+ * size it needs when it is too small. */
+int  lg_test_linear(int dtype, int M, int N, int K, const void* x, const void* norm_in, float eps, const void* wa, const void* wb,
+                    int epi, const void* norm_out, void* h, void* out, float* out_f32, float* acc_out, int small, void* dev_scratch,
+                    size_t scratch_bytes, int* path, void* stream);
+/* The path of lg_test_linear without buffers or a GPU, after the same checks of the shape-only arguments: paired = wb is passed.
+ * has_norm_in is accepted for symmetry with lg_test_linear; no dispatch rule depends on it. */
+int  lg_test_linear_plan(int dtype, int M, int N, int K, int paired, int small, int epi, int has_norm_in, int* plan);
+
 /* One transformer attention call through the engine's own dispatch, attn_plan (honouring LG_ATTN_TMA, LG_ATTN_PREFILL_TC,
  * LG_ATTN_NST and LG_ATTN_DEEP). dtype: the model dtype (LG_DTYPE_F32, _BF16 or _F16); kv_dtype: dtype, or LG_DTYPE_E4M3 for a
  * 16-bit model with k_scale / v_scale powers of two in [2^-8, 2^7] (otherwise both 1). kcache / vcache: dev [n_layer][R][H][max_seq]

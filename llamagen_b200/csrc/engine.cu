@@ -312,13 +312,13 @@ size_t lg_engine::carve(Workspace& o, char* base, int rows, int max_seq, int g, 
     const int Ms[2] = {rows, (int)Mmax};
     for (int i = 0; i < 2; ++i) {
         const int M = Ms[i];
-        pf = std::max(pf, gemm_partial_floats(M, 3 * D, D, cfg.dtype));
-        pf = std::max(pf, gemm_partial_floats(M, D, D, cfg.dtype));
-        pf = std::max(pf, gemm_partial_floats(M, 2 * F, D, cfg.dtype));
-        pf = std::max(pf, gemm_partial_floats(M, D, F, cfg.dtype));
-        if (cfg.model_type == LG_MODEL_T2I) pf = std::max(pf, gemm_partial_floats(M, D, cfg.caption_dim, cfg.dtype));
+        pf = std::max(pf, gemm_partial_floats(M, 3 * D, D, 0, cfg.dtype));
+        pf = std::max(pf, gemm_partial_floats(M, D, D, 0, cfg.dtype));
+        pf = std::max(pf, gemm_partial_floats(M, 2 * F, D, F, cfg.dtype));
+        pf = std::max(pf, gemm_partial_floats(M, D, F, 0, cfg.dtype));
+        if (cfg.model_type == LG_MODEL_T2I) pf = std::max(pf, gemm_partial_floats(M, D, cfg.caption_dim, 0, cfg.dtype));
     }
-    pf = std::max(pf, gemm_partial_floats(rows, V, D, cfg.dtype));
+    pf = std::max(pf, gemm_partial_floats(rows, V, D, 0, cfg.dtype));
     o.partial_floats = n == 1 ? pf : pf / n / 64 * 64;
     o.partial = (float*)take(pf * sizeof(float), o.partial_floats * sizeof(float));
     o.logits = (float*)split((size_t)rows * V * sizeof(float));
@@ -356,16 +356,16 @@ size_t lg_engine::carve_score(Workspace& o, char* base, int rows, int seq) const
     o.ff = take((size_t)M * F * esz);
     o.x0 = take(t2i ? (size_t)rows * Tc * cfg.caption_dim * esz : 0);
     size_t pf = 0;
-    pf = std::max(pf, gemm_partial_floats(M, 3 * D, D, cfg.dtype));
-    pf = std::max(pf, gemm_partial_floats(M, D, D, cfg.dtype));
-    pf = std::max(pf, gemm_partial_floats(M, 2 * F, D, cfg.dtype));
-    pf = std::max(pf, gemm_partial_floats(M, D, F, cfg.dtype));
+    pf = std::max(pf, gemm_partial_floats(M, 3 * D, D, 0, cfg.dtype));
+    pf = std::max(pf, gemm_partial_floats(M, D, D, 0, cfg.dtype));
+    pf = std::max(pf, gemm_partial_floats(M, 2 * F, D, F, cfg.dtype));
+    pf = std::max(pf, gemm_partial_floats(M, D, F, 0, cfg.dtype));
     if (t2i) {
-        pf = std::max(pf, gemm_partial_floats(rows * Tc, D, cfg.caption_dim, cfg.dtype));
-        pf = std::max(pf, gemm_partial_floats(rows * Tc, D, D, cfg.dtype));
+        pf = std::max(pf, gemm_partial_floats(rows * Tc, D, cfg.caption_dim, 0, cfg.dtype));
+        pf = std::max(pf, gemm_partial_floats(rows * Tc, D, D, 0, cfg.dtype));
     }
     o.head_rows = std::min(rows * std::max(seq - Tc + 1, 1), kScoreHeadRows);
-    pf = std::max(pf, gemm_partial_floats(o.head_rows, V, D, cfg.dtype));
+    pf = std::max(pf, gemm_partial_floats(o.head_rows, V, D, 0, cfg.dtype));
     o.partial_floats = pf;
     o.partial = (float*)take(pf * sizeof(float));
     o.base = base;
@@ -393,11 +393,11 @@ size_t lg_engine::carve_sjd(Workspace& o, SjdArgs& sa, char* base, int B, int nh
     o.attn = take(M * D * esz);
     o.ff = take(M * F * esz);
     size_t pf = 0;
-    pf = std::max(pf, gemm_partial_floats((int)M, 3 * D, D, cfg.dtype));
-    pf = std::max(pf, gemm_partial_floats((int)M, D, D, cfg.dtype));
-    pf = std::max(pf, gemm_partial_floats((int)M, 2 * F, D, cfg.dtype));
-    pf = std::max(pf, gemm_partial_floats((int)M, D, F, cfg.dtype));
-    pf = std::max(pf, gemm_partial_floats((int)M, V, D, cfg.dtype));
+    pf = std::max(pf, gemm_partial_floats((int)M, 3 * D, D, 0, cfg.dtype));
+    pf = std::max(pf, gemm_partial_floats((int)M, D, D, 0, cfg.dtype));
+    pf = std::max(pf, gemm_partial_floats((int)M, 2 * F, D, F, cfg.dtype));
+    pf = std::max(pf, gemm_partial_floats((int)M, D, F, 0, cfg.dtype));
+    pf = std::max(pf, gemm_partial_floats((int)M, V, D, 0, cfg.dtype));
     o.partial_floats = pf;
     o.partial = (float*)take(pf * sizeof(float));
     o.logits = (float*)take(M * V * sizeof(float));
@@ -419,7 +419,7 @@ size_t lg_engine::carve_sjd(Workspace& o, SjdArgs& sa, char* base, int B, int nh
 int lg_engine::gemm(const Workspace& w, const void* x, int M, int N, int K, const void* wa, const void* wb, int n_split, int* ksplit,
                     float* direct_out, cudaStream_t st, const GemmNext* next) {
     // when the plan needs a single slab the GEMM can write straight into `direct_out`
-    const size_t need = gemm_partial_floats(M, N, K, cfg.dtype);
+    const size_t need = gemm_partial_floats(M, N, K, wb ? n_split : 0, cfg.dtype);
     const size_t slabs = need / ((size_t)M * N);
     float* dst = (direct_out && slabs == 1) ? direct_out : w.partial;
     // the plan (k-slices) is not monotone in M and depends on run-time switches: never trust the carve-time sizing blindly
@@ -832,7 +832,7 @@ int lg_score(lg_engine* e, const void* cond, const float* emb_mask, const int32_
         const int P = nb * S, per = std::max(1, w.head_rows / nh);
         for (int p0 = 0; p0 < P;) {
             int np = std::min(per, P - p0);
-            while (np > 1 && gemm_partial_floats(np * nh, V, D, dt) > w.partial_floats) np /= 2;   // the GEMM plan is not monotone in M
+            while (np > 1 && gemm_partial_floats(np * nh, V, D, 0, dt) > w.partial_floats) np /= 2;   // the GEMM plan is not monotone in M
             int ks = 1;
             LG_TRY(e->gemm(w, (const char*)w.q + (size_t)p0 * nh * D * esz, np * nh, V, D, e->output, nullptr, 0, &ks, nullptr, st));
             const size_t g0 = (size_t)b0 * S + p0;
@@ -1203,11 +1203,77 @@ int lg_test_gemm(const void* x, const void* w, int M, int N, int K, int dtype, f
                  size_t scratch_bytes, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     LG_REQUIRE(x && w && y && dev_scratch, "lg_test_gemm: null argument");
-    const size_t needf = gemm_partial_floats(M, N, K, dtype);
+    const size_t needf = gemm_partial_floats(M, N, K, 0, dtype);
     LG_REQUIRE(scratch_bytes >= needf * sizeof(float), "lg_test_gemm: scratch %zu < %zu", scratch_bytes, needf * sizeof(float));
     GemmPlan plan;
     LG_TRY(gemm_partial(x, K, w, nullptr, 0, M, N, K, dtype, (float*)dev_scratch, &plan, st));
     return launch_reduce_f32((const float*)dev_scratch, plan.ksplit, M, N, y, st);
+}
+
+// What lg_test_linear and lg_test_linear_plan (fn) check of the shape-only arguments, then the call's path {kernel (3: gemv_small),
+// tile, ksplit, row blocks or PF}
+static int test_linear_args(const char* fn, int dtype, int M, int N, int K, bool paired, bool small, int epi, bool norm_out, int* path) {
+    LG_REQUIRE(epi >= 0 && epi <= 4, "%s: epilogue %d outside 0..4", fn, epi);
+    LG_REQUIRE(paired == (epi == 2), "%s: wb goes with the SwiGLU epilogue (2) alone, epilogue %d", fn, epi);
+    LG_REQUIRE(!norm_out || (epi == 1 && !small), "%s: norm_out goes with the batched residual epilogue alone", fn);
+    if (small) {
+        LG_REQUIRE(epi <= 2, "%s: the small path has no store or gelu epilogue (%d)", fn, epi);
+        const GemvSmallPlan p = gemv_small_plan(M, N, K, dtype, paired);
+        LG_REQUIRE(p.rows != 0, "%s: %s", fn, p.error);
+        path[0] = 3; path[1] = p.rows; path[2] = 1; path[3] = p.pf;
+        return 0;
+    }
+    const GemmPlan p = gemm_plan(M, paired ? 2 * N : N, K, paired ? N : 0, dtype);
+    LG_REQUIRE(p.kernel >= 0, "%s: %s", fn, p.error);
+    LG_REQUIRE(epi != 1 || (N % 4 == 0 && N <= 4096), "%s: the residual epilogue needs N %% 4 == 0 and N <= 4096 (N=%d)", fn, N);
+    LG_REQUIRE(epi != 2 || N % 4 == 0, "%s: the SwiGLU epilogue needs N %% 4 == 0 (N=%d)", fn, N);
+    path[0] = p.kernel; path[1] = p.tile; path[2] = p.ksplit; path[3] = p.row_blocks;
+    return 0;
+}
+
+int lg_test_linear(int dtype, int M, int N, int K, const void* x, const void* norm_in, float eps, const void* wa, const void* wb, int epi,
+                   const void* norm_out, void* h, void* out, float* out_f32, float* acc_out, int small, void* dev_scratch,
+                   size_t scratch_bytes, int* path, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    auto a16 = [](const void* p) { return ((uintptr_t)p & 15) == 0; };
+    int pl[4];
+    LG_TRY(test_linear_args("lg_test_linear", dtype, M, N, K, wb != nullptr, small != 0, epi, norm_out != nullptr, pl));
+    LG_REQUIRE(x && wa && a16(x) && a16(wa) && a16(wb) && a16(norm_in) && a16(norm_out) && a16(h) && a16(out) && a16(out_f32) && a16(acc_out),
+               "lg_test_linear: null or misaligned (16 bytes) operand");
+    LG_REQUIRE((out_f32 != nullptr) == (epi == 0) && (h != nullptr) == (epi == 1) && (out != nullptr) == (epi >= 2 || norm_out != nullptr),
+               "lg_test_linear: epilogue %d writes out_f32 (0), h (1), out (1 with norm_out, 2-4) and no other buffer", epi);
+    LG_REQUIRE(!small || !acc_out, "lg_test_linear: the small path keeps its accumulator on chip (acc_out)");
+    const int NN = wb ? 2 * N : N;
+    const size_t pbytes = small ? 0 : align_up(gemm_partial_floats(M, NN, K, wb ? N : 0, dtype) * sizeof(float));
+    const size_t need = pbytes + (!small && norm_in ? (size_t)M * K * lg_dtype_info(dtype).esz : 0);
+    LG_REQUIRE(need == 0 || (dev_scratch && ((uintptr_t)dev_scratch & 255) == 0 && scratch_bytes >= need),
+               "lg_test_linear: scratch %zu < %zu (256-byte aligned)", scratch_bytes, need);
+    if (path) std::copy(pl, pl + 4, path);
+    if (small) {
+        GemvSmall g{wa, wb, N, K, M, x, norm_in, eps, epi == 0 ? out_f32 : nullptr, epi == 1 ? h : nullptr, epi == 2 ? out : nullptr, dtype};
+        return launch_gemv_small(g, st);
+    }
+    float* partial = (float*)dev_scratch;
+    const void* xin = x;
+    if (norm_in) {   // layer 0's attention norm (run_layers)
+        xin = (char*)dev_scratch + pbytes;
+        LG_TRY(launch_rmsnorm(x, norm_in, (void*)xin, M, K, eps, dtype, st));
+    }
+    GemmPlan p;
+    LG_TRY(gemm_partial(xin, K, wa, wb, wb ? N : 0, M, NN, K, dtype, partial, &p, st));
+    if (acc_out) LG_TRY(launch_reduce_f32(partial, p.ksplit, M, NN, acc_out, st));
+    switch (epi) {
+        case 0: return launch_reduce_f32(partial, p.ksplit, M, N, out_f32, st);
+        case 1: return launch_residual_norm(partial, p.ksplit, M, N, h, norm_out, norm_out ? out : nullptr, eps, dtype, st);
+        case 2: return launch_silu_mul(partial, p.ksplit, M, N, out, dtype, st);
+        default: return launch_store_act(partial, p.ksplit, M, N, out, epi == 4, dtype, st);
+    }
+}
+
+int lg_test_linear_plan(int dtype, int M, int N, int K, int paired, int small, int epi, int has_norm_in, int* plan) {
+    (void)has_norm_in;   // no dispatch rule depends on the RMSNorm prologue
+    LG_REQUIRE(plan, "lg_test_linear_plan: null plan");
+    return test_linear_args("lg_test_linear_plan", dtype, M, N, K, paired != 0, small != 0, epi, false, plan);
 }
 
 // What lg_test_attention and lg_test_attention_plan (fn) check of the shape-only arguments, then the call's AttnArgs (no QKV slabs

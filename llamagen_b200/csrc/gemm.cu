@@ -87,57 +87,71 @@ __global__ void __launch_bounds__(kSkinnyWarps * 32) gemm_skinny_kernel(const T*
     }
 }
 
-struct Plan {
-    bool skinny;
-    bool tc;      // wgmma / TMA kernel (gemm_tc.cu)
-    int bm;       // mma tile rows
-    int ksplit;
-};
+}  // namespace
 
-Plan make_plan(int M, int N, int K, int dtype) {
-    Plan p;
-    p.tc = false;
+GemmPlan gemm_plan(int M, int N, int K, int n_split, int dtype) {
+    GemmPlan p;
+    if (M <= 0 || N <= 0 || K <= 0) {
+        snprintf(p.error, sizeof(p.error), "gemm: bad shape %d %d %d", M, N, K);
+        return p;
+    }
+    if (N % 2 != 0 || K % 8 != 0) {
+        snprintf(p.error, sizeof(p.error), "gemm: N=%d must be even and K=%d a multiple of 8", N, K);
+        return p;
+    }
+    if (dtype != LG_DTYPE_F32 && !lg_dtype_is16(dtype)) {
+        snprintf(p.error, sizeof(p.error), "gemm: unsupported dtype %d", dtype);
+        return p;
+    }
+    if (n_split < 0 || n_split > N) {
+        snprintf(p.error, sizeof(p.error), "gemm: weight segment boundary %d outside [0, %d]", n_split, N);
+        return p;
+    }
     // bf16 / fp16: the wgmma kernel is used for every row count (a batch-1 step pads its 2 rows to the minimum N = 16); the CUDA-core
-    // skinny kernel stays for the fp32 exact mode.
-    const bool tc_ok = lg_env_flag("LG_GEMM_TC", 1) && gemm_tc_supported(M, N, K, dtype) && N % 128 == 0;
-    p.skinny = (dtype == LG_DTYPE_F32) || (M <= kSkinnyRT && !tc_ok);
-    if (!p.skinny && tc_ok) {
-        p.tc = true;
-        p.bm = 0;
+    // skinny kernel stays for the fp32 exact mode. A wgmma CTA streams one 128-row weight tile from one segment, so the w1 | w3
+    // boundary must fall on a tile edge; any other boundary (ffn_dim % 128 != 0) goes to the row-wise loaders of the other kernels.
+    const bool one_segment = n_split == 0 || n_split == N;
+    const bool tc_ok = lg_env_flag("LG_GEMM_TC", 1) && lg_dtype_is16(dtype) && N % 128 == 0 && (one_segment || n_split % 128 == 0);
+    if (tc_ok) {
+        const int rblk = std::min(M, 256);
+        p.kernel = 2;
+        p.tile = 16;
+        while (p.tile < rblk) p.tile *= 2;
+        p.row_blocks = cdiv(M, rblk);
         p.ksplit = gemm_tc_ksplit(M, N, K);
         return p;
     }
-    if (p.skinny) {
-        p.bm = kSkinnyRT;
+    if (dtype == LG_DTYPE_F32 || M <= kSkinnyRT) {
+        p.kernel = 0;
+        p.tile = kSkinnyRT;
         const long long ctas = (long long)cdiv(N, 2 * kSkinnyWarps) * cdiv(M, kSkinnyRT);
         int ks = (int)std::max<long long>(1, 264 / std::max<long long>(ctas, 1));
         ks = std::min(ks, std::max(1, K / 512));
         p.ksplit = std::min(ks, 16);
     } else {
-        p.bm = M <= 32 ? 32 : (M <= 64 ? 64 : 128);
-        const long long tiles = (long long)cdiv(M, p.bm) * cdiv(N, 128);
+        p.kernel = 1;
+        p.tile = M <= 32 ? 32 : (M <= 64 ? 64 : 128);
+        const long long tiles = (long long)cdiv(M, p.tile) * cdiv(N, 128);
         int ks = (int)std::max<long long>(1, 132 / std::max<long long>(tiles, 1));
         ks = std::min(ks, std::max(1, (K / mma::BK) / 4));
         p.ksplit = std::min(ks, 16);
     }
+    p.row_blocks = cdiv(M, p.tile);
     return p;
 }
 
-}  // namespace
-
-size_t gemm_partial_floats(int M, int N, int K, int dtype) {
-    const Plan p = make_plan(M, N, K, dtype);
-    return (size_t)p.ksplit * M * N;
+size_t gemm_partial_floats(int M, int N, int K, int n_split, int dtype) {
+    const GemmPlan p = gemm_plan(M, N, K, n_split, dtype);
+    return p.kernel < 0 ? 0 : (size_t)p.ksplit * M * N;
 }
 
 int gemm_partial(const void* X, int ldx, const void* Wa, const void* Wb, int n_split, int M, int N, int K, int dtype,
                  float* partial, GemmPlan* plan, cudaStream_t st, const GemmNext* next) {
-    LG_REQUIRE(M > 0 && N > 0 && K > 0, "gemm: bad shape %d %d %d", M, N, K);
-    LG_REQUIRE(N % 2 == 0 && K % 8 == 0, "gemm: N=%d must be even and K=%d a multiple of 8", N, K);
-    if (Wb == nullptr) { Wb = Wa; n_split = N; }
-    const Plan p = make_plan(M, N, K, dtype);
-    if (plan) plan->ksplit = p.ksplit;
-    if (p.skinny) {
+    if (Wb == nullptr || n_split == 0) { Wb = Wa; n_split = N; }
+    const GemmPlan p = gemm_plan(M, N, K, n_split, dtype);
+    if (plan) *plan = p;
+    if (p.kernel < 0) return lg_fail("%s", p.error);
+    if (p.kernel == 0) {
         // kper: multiple of 256 elements so every lane's 16-byte vector stays inside the slab
         int kper = cdiv(cdiv(K, p.ksplit), 256) * 256;
         dim3 grid(cdiv(N, 2 * kSkinnyWarps), cdiv(M, kSkinnyRT), p.ksplit);
@@ -162,20 +176,16 @@ int gemm_partial(const void* X, int ldx, const void* Wa, const void* Wb, int n_s
         LG_LAUNCH_CHECK();
         return 0;
     }
-    if (p.tc) {
-        if (n_split % 128 != 0 && n_split != N) return lg_fail("gemm: weight segment boundary %d not tile aligned", n_split);
-        return gemm_tc_partial(X, ldx, Wa, Wb, n_split, M, N, K, dtype, partial, nullptr, st, next);
-    }
-    LG_REQUIRE(lg_dtype_is16(dtype), "gemm: unsupported dtype %d", dtype);
+    if (p.kernel == 2) return gemm_tc_partial(X, ldx, Wa, Wb, n_split, M, N, K, dtype, p, partial, st, next);
     mma::DenseA al{(const bf16*)X, ldx, 0, M};   // raw 16-bit elements: the same loaders serve fp16
     mma::BRows bw{(const bf16*)Wa, (const bf16*)Wb, n_split, K, 0, N};
     mma::EpiPartial epi{partial, M, N};
     if (dtype == LG_DTYPE_F16) {
-        if (p.bm == 32) return mma::launch_gemm_mma<32, 128, 1, 8, 4, f16>(al, bw, M, N, K, p.ksplit, 1, epi, st);
-        if (p.bm == 64) return mma::launch_gemm_mma<64, 128, 2, 4, 4, f16>(al, bw, M, N, K, p.ksplit, 1, epi, st);
+        if (p.tile == 32) return mma::launch_gemm_mma<32, 128, 1, 8, 4, f16>(al, bw, M, N, K, p.ksplit, 1, epi, st);
+        if (p.tile == 64) return mma::launch_gemm_mma<64, 128, 2, 4, 4, f16>(al, bw, M, N, K, p.ksplit, 1, epi, st);
         return mma::launch_gemm_mma<128, 128, 2, 4, 3, f16>(al, bw, M, N, K, p.ksplit, 1, epi, st);
     }
-    if (p.bm == 32) return mma::launch_gemm_mma<32, 128, 1, 8, 4>(al, bw, M, N, K, p.ksplit, 1, epi, st);
-    if (p.bm == 64) return mma::launch_gemm_mma<64, 128, 2, 4, 4>(al, bw, M, N, K, p.ksplit, 1, epi, st);
+    if (p.tile == 32) return mma::launch_gemm_mma<32, 128, 1, 8, 4>(al, bw, M, N, K, p.ksplit, 1, epi, st);
+    if (p.tile == 64) return mma::launch_gemm_mma<64, 128, 2, 4, 4>(al, bw, M, N, K, p.ksplit, 1, epi, st);
     return mma::launch_gemm_mma<128, 128, 2, 4, 3>(al, bw, M, N, K, p.ksplit, 1, epi, st);
 }

@@ -219,10 +219,6 @@ int gemm_tc_ksplit(int M, int N, int K) {
     return std::min(ks, 16);
 }
 
-bool gemm_tc_supported(int M, int N, int K, int dtype) {
-    return lg_dtype_is16(dtype) && M >= 1 && K % 8 == 0 && N % 2 == 0;
-}
-
 template <int RP, typename T>
 static int gemm_tc_launch_t(const CUtensorMap& mwa, const CUtensorMap& mwb, const CUtensorMap& mx, TcArgs& a, dim3 grid,
                             cudaStream_t st) {
@@ -244,25 +240,22 @@ static int gemm_tc_launch_t(const CUtensorMap& mwa, const CUtensorMap& mwb, cons
 
 template <typename T>
 static int gemm_tc_launch(const void* X, int ldx, const void* Wa, const void* Wb, int n_split, int M, int N, int K,
-                          float* partial, int* ksplit_out, cudaStream_t st, const GemmNext* next) {
+                          const GemmPlan& p, float* partial, cudaStream_t st, const GemmNext* next) {
     constexpr int dt = ElemTraits<T>::dtype;
-    LG_REQUIRE(gemm_tc_supported(M, N, K, dt), "gemm_tc: unsupported shape %d %d %d", M, N, K);
     if (Wb == nullptr) { Wb = Wa; n_split = N; }
-    LG_REQUIRE(n_split % kBlockN == 0 || n_split == N, "gemm_tc: weight segment boundary %d must be a multiple of %d", n_split, kBlockN);
+    LG_REQUIRE(p.kernel == 2, "gemm_tc: the call is planned on kernel %d", p.kernel);
     LG_REQUIRE(((uintptr_t)X & 15) == 0 && ((uintptr_t)Wa & 15) == 0 && ((uintptr_t)Wb & 15) == 0 && ldx % 8 == 0,
                "gemm_tc: operands must be 16-byte aligned");
     TcArgs a;
     a.M = M; a.N = N; a.K = K; a.n_split = n_split;
     a.rblk = M <= kMaxRowsPerCta ? M : kMaxRowsPerCta;
-    const int zblocks = cdiv(M, a.rblk);
+    const int zblocks = p.row_blocks;
     LG_REQUIRE(zblocks <= 65535, "gemm_tc: %d row blocks not launchable", zblocks);
-    int rpad = 16;
-    while (rpad < a.rblk) rpad *= 2;
-    const int ks = gemm_tc_ksplit(M, N, K);
+    const int rpad = p.tile;
+    const int ks = p.ksplit;
     const int kb = cdiv(K, kBlockK);
     a.kblocks_per_split = cdiv(kb, ks);
     a.partial = partial;
-    if (ksplit_out) *ksplit_out = ks;
 
     CUtensorMap mwa, mwb, mx;
     LG_TRY(tma::make_map_2d(&mwa, Wa, (uint64_t)std::min(n_split, N), (uint64_t)K, (uint64_t)K, kBlockN, kBlockK, dt));
@@ -283,8 +276,8 @@ static int gemm_tc_launch(const void* X, int ldx, const void* Wa, const void* Wb
 }
 
 int gemm_tc_partial(const void* X, int ldx, const void* Wa, const void* Wb, int n_split, int M, int N, int K, int dtype,
-                    float* partial, int* ksplit_out, cudaStream_t st, const GemmNext* next) {
-    if (dtype == LG_DTYPE_F16) return gemm_tc_launch<f16>(X, ldx, Wa, Wb, n_split, M, N, K, partial, ksplit_out, st, next);
+                    const GemmPlan& p, float* partial, cudaStream_t st, const GemmNext* next) {
+    if (dtype == LG_DTYPE_F16) return gemm_tc_launch<f16>(X, ldx, Wa, Wb, n_split, M, N, K, p, partial, st, next);
     LG_REQUIRE(dtype == LG_DTYPE_BF16, "gemm_tc: unsupported dtype %d", dtype);
-    return gemm_tc_launch<bf16>(X, ldx, Wa, Wb, n_split, M, N, K, partial, ksplit_out, st, next);
+    return gemm_tc_launch<bf16>(X, ldx, Wa, Wb, n_split, M, N, K, p, partial, st, next);
 }

@@ -230,28 +230,43 @@ int launch_t(const GemvArgs<T>& a, cudaStream_t st) {
 }
 
 template <typename T>
-int launch_typed(const GemvSmall& g, cudaStream_t st) {
+int launch_typed(const GemvSmall& g, const GemvSmallPlan& p, cudaStream_t st) {
     GemvArgs<T> a;
     a.Wa = (const T*)g.Wa; a.Wb = (const T*)g.Wb; a.N = g.N; a.K = g.K; a.R = g.R;
     a.pro = g.normw ? 1 : 0; a.in = (const T*)g.in; a.normw = (const T*)g.normw; a.eps = g.eps;
     a.epi = g.Wb ? 2 : (g.out_f32 ? 0 : 1); a.out_f32 = g.out_f32; a.h = (T*)g.h; a.ff = (T*)g.ff;
-    if (g.Wb) return launch_t<32, 4>(a, st);
-    // Row granularity: enough CTAs to pull the matrix from all SMs (8 rows/CTA below ~2.4k outputs), fatter CTAs for the head
-    if (g.N <= 2048) return launch_t<8, 12>(a, st);
-    if (g.N <= 8192) return launch_t<16, 4>(a, st);
+    if (p.rows == 8) return launch_t<8, 12>(a, st);
+    if (p.rows == 16) return launch_t<16, 4>(a, st);
     return launch_t<32, 4>(a, st);
 }
 
 }  // namespace
 
-bool gemv_small_supported(int R, int N, int K, int dtype, bool paired) {
-    if (!lg_dtype_is16(dtype) || R < 1 || R > 8 || K % 32 != 0 || K < 256) return false;
-    if ((size_t)R * (K * 2 + 16) > 90 * 1024) return false;
-    return N % (paired ? 16 : 32) == 0;      // every row granularity used below divides N
+GemvSmallPlan gemv_small_plan(int R, int N, int K, int dtype, bool paired) {
+    GemvSmallPlan p;
+    if (!lg_dtype_is16(dtype)) {
+        snprintf(p.error, sizeof(p.error), "gemv_small: dtype %d is not bf16 / fp16", dtype);
+    } else if (R < 1 || R > 8) {
+        snprintf(p.error, sizeof(p.error), "gemv_small: R=%d rows outside 1..8", R);
+    } else if (K % 32 != 0 || K < 256) {
+        snprintf(p.error, sizeof(p.error), "gemv_small: K=%d must be a multiple of 32 and at least 256", K);
+    } else if ((size_t)R * (K * 2 + 16) > 90 * 1024) {
+        snprintf(p.error, sizeof(p.error), "gemv_small: R=%d rows of K=%d exceed 90 KiB of shared memory", R, K);
+    } else if (N <= 0 || N % (paired ? 16 : 32) != 0) {      // every row granularity used below divides N
+        snprintf(p.error, sizeof(p.error), "gemv_small: N=%d must be a positive multiple of %d", N, paired ? 16 : 32);
+    } else if (paired) {
+        p.rows = 32; p.pf = 4;
+    } else if (N <= 2048) {
+        // Row granularity: enough CTAs to pull the matrix from all SMs (8 rows/CTA below ~2.4k outputs), fatter CTAs for the head
+        p.rows = 8; p.pf = 12;
+    } else {
+        p.rows = N <= 8192 ? 16 : 32; p.pf = 4;
+    }
+    return p;
 }
 
 int launch_gemv_small(const GemvSmall& g, cudaStream_t st) {
-    LG_REQUIRE(gemv_small_supported(g.R, g.N, g.K, g.dtype, g.Wb != nullptr), "gemv_small: unsupported shape R=%d N=%d K=%d dtype %d",
-               g.R, g.N, g.K, g.dtype);
-    return g.dtype == LG_DTYPE_F16 ? launch_typed<f16>(g, st) : launch_typed<bf16>(g, st);
+    const GemvSmallPlan p = gemv_small_plan(g.R, g.N, g.K, g.dtype, g.Wb != nullptr);
+    if (p.rows == 0) return lg_fail("%s", p.error);
+    return g.dtype == LG_DTYPE_F16 ? launch_typed<f16>(g, p, st) : launch_typed<bf16>(g, p, st);
 }

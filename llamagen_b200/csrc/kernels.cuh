@@ -79,17 +79,24 @@ int launch_sjd_refresh(const SjdArgs& a, int first, cudaStream_t st);
 // ------------------------------------------------------------------------------------------------
 // gemm.cu — y_partial[ks][M][N] (f32) = x[M,K] * W[N,K]^T ; W may be two row segments (w1 | w3).
 // ------------------------------------------------------------------------------------------------
-struct GemmPlan {
-    int ksplit;            // number of fp32 partial slabs written
-};
+// The kernel a GEMM call runs on; n_split: weight rows [0, n_split) come from Wa, the rest from Wb (0 or N: Wa alone).
+//   2 gemm_tc_kernel (gemm_tc.cu): bf16 / fp16, N % 128 == 0 and a segment boundary on a 128-row tile, unless LG_GEMM_TC=0.
+//     tile: the row pad of a row block (16 ... 256), row_blocks: blocks of min(M, 256) rows.
+//   0 gemm_skinny_kernel: fp32 at any M, and 16-bit at M <= 8 that kernel 2 does not take. tile 8 rows.
+//   1 gemm_mma_kernel: every other 16-bit call. tile: 32, 64 or 128 rows (bm).
+// ksplit: fp32 slabs [ksplit][M][N] written (<= 16). kernel -1: the call is not valid, `error` says why. The only reader of
+// LG_GEMM_TC.
+struct GemmPlan { int kernel = -1; int tile = 0; int ksplit = 0; int row_blocks = 0; char error[96] = {}; };
+GemmPlan gemm_plan(int M, int N, int K, int n_split, int dtype);
 // Weights the NEXT GEMM of the decode chain will stream: the current GEMM's CTAs ask the L2 to fetch them
 // (cp.async.bulk.prefetch.L2) so the next kernel's TMA loads hit L2 instead of paying the HBM latency.
 struct GemmNext {
     const void* p0 = nullptr; size_t b0 = 0;
     const void* p1 = nullptr; size_t b1 = 0;
 };
-// Returns the plan used; partial must hold ksplit_max(M,N,K) * M * N floats (see gemm_partial_floats).
-size_t gemm_partial_floats(int M, int N, int K, int dtype);
+// floats of fp32 slabs the call's plan writes (0 for an invalid call); partial must hold that many
+size_t gemm_partial_floats(int M, int N, int K, int n_split, int dtype);
+// runs the call on the kernel gemm_plan picks; *plan (optional) receives that plan
 int gemm_partial(const void* X, int ldx, const void* Wa, const void* Wb, int n_split, int M, int N, int K,
                  int dtype, float* partial, GemmPlan* plan, cudaStream_t st, const GemmNext* next = nullptr);
 
@@ -240,9 +247,8 @@ void conv_tc_set_cta_budget(int ctas);   // > 0: persistent conv CTAs (at most `
 int conv_tc_make_phase_weights(const float* w_f32, bf16* out, int cout, int cin, cudaStream_t st);
 // gemm_tc.cu — wgmma/TMA weight-streaming GEMM (bf16 or fp16, row blocks of <= 256)
 int gemm_tc_ksplit(int M, int N, int K);
-bool gemm_tc_supported(int M, int N, int K, int dtype);
 int gemm_tc_partial(const void* X, int ldx, const void* Wa, const void* Wb, int n_split, int M, int N, int K, int dtype,
-                    float* partial, int* ksplit_out, cudaStream_t st, const GemmNext* next = nullptr);
+                    const GemmPlan& p, float* partial, cudaStream_t st, const GemmNext* next = nullptr);   // p.kernel 2
 
 // gemv_small.cu — decode GEMMs for R <= 8 rows: CTA-owned output columns (no split-K), RMSNorm in the prologue (normw != null),
 // epilogue by destination: out_f32 [R][N] | h (in-place residual add) | ff (SwiGLU gate of the Wa/Wb row pair)
@@ -254,7 +260,12 @@ struct GemvSmall {
     float* out_f32; void* h; void* ff;
     int dtype;                        // LG_DTYPE_BF16 or LG_DTYPE_F16: every 16-bit tensor above
 };
-bool gemv_small_supported(int R, int N, int K, int dtype, bool paired);
+// The instantiation a call runs on: rows = weight rows per CTA (8, 16 or 32; the paired form is 32: 16 rows of Wa and of Wb), pf =
+// 32-wide k chunks in flight per warp. rows 0: the call is not supported (bf16 / fp16, 1 <= R <= 8, K % 32 == 0, K >= 256,
+// R * (2K + 16) bytes <= 90 KiB, N > 0 a multiple of 32, or of 16 when paired), `error` says why.
+struct GemvSmallPlan { int rows = 0; int pf = 0; char error[96] = {}; };
+GemvSmallPlan gemv_small_plan(int R, int N, int K, int dtype, bool paired);
+inline bool gemv_small_supported(int R, int N, int K, int dtype, bool paired) { return gemv_small_plan(R, N, K, dtype, paired).rows != 0; }
 int launch_gemv_small(const GemvSmall& g, cudaStream_t st);
 
 // *pos += 1; *step += 1  (device-side loop counters for graph replay)

@@ -53,12 +53,13 @@ _TINY_HD100 = dict(n_layer=2, n_head=2, dim=200, ffn_dim=544, vocab_size=1024, c
 
 @pytest.mark.parametrize("m, t2i, dtype, kv_fp8, sizes", [
     (_GPT_L, False, "bf16", False, {(2, 17): 3632896, (128, 257): 3252356096}),
-    (_TINY_T2I, True, "bf16", False, {(2, 17): 316160, (128, 257): 83100672}),
+    # ffn_dim 704: the w1 | w3 boundary is not on a 128-row tile, so that GEMM plans mma.sync (one slab) instead of wgmma (two)
+    (_TINY_T2I, True, "bf16", False, {(2, 17): 234240, (128, 257): 77857792}),
     (_GPT_L, False, "f16", False, {(2, 17): 3632896, (128, 257): 3252356096}),
     (_GPT_L, False, "f32", False, {(2, 17): 7002880, (128, 257): 6487933952}),
     (_TINY_HD100, False, "bf16", False, {(2, 17): 92672, (128, 257): 60867584}),     # 112-wide cache rows
     (_GPT_L, False, "bf16", True, {(2, 17): 1961728, (128, 257): 1635451904}),
-], ids=["c2i_bf16_hd64", "t2i_bf16_caption", "c2i_f16", "c2i_f32", "c2i_bf16_hd100", "c2i_bf16_kv_fp8"])
+], ids=["c2i_bf16_hd64", "t2i_bf16_caption_ffn704", "c2i_f16", "c2i_f32", "c2i_bf16_hd100", "c2i_bf16_kv_fp8"])
 def test_workspace_bytes_are_pinned(m, t2i, dtype, kv_fp8, sizes, monkeypatch):
     """The workspace layout (KV caches, activations, GEMM partials, logits, tokens, counters) is host arithmetic: its size, computed
     without a GPU, must not move. The GEMM partials follow the default GEMM plan."""
