@@ -32,7 +32,8 @@ extern "C" {
 #define LG_ABI_VERSION 1
 
 /* LG_DTYPE_F16 (IEEE half) runs the same tensor-core kernels as LG_DTYPE_BF16; values past +-65504 become +-inf, as in torch. */
-/* LG_DTYPE_E4M3 (fp8 e4m3, finite, max +-448) is a KV-cache storage type only (lg_engine_set_kv_cache); never a model dtype. */
+/* LG_DTYPE_E4M3 (fp8 e4m3, finite, max +-448) is a storage type of a bf16 / fp16 model, never a model dtype: of the KV cache
+ * (lg_engine_set_kv_cache) and of the GEMM weights (lg_engine_bind_weight, "fp8 weights" below). */
 enum { LG_DTYPE_F32 = 0, LG_DTYPE_BF16 = 1, LG_DTYPE_F16 = 2, LG_DTYPE_E4M3 = 3 };
 enum { LG_MODEL_C2I = 0, LG_MODEL_T2I = 1 };
 
@@ -77,11 +78,33 @@ int  lg_engine_create(const lg_model_cfg* cfg, int device, lg_engine** out);
 void lg_engine_destroy(lg_engine* e);
 /* Borrow a checkpoint tensor by its reference state_dict name (SURVEY §5), plus "freqs_cis"
  * (fp32 [cls_token_num+block_size, head_dim/2, 2], gpt.py:404-417).  dtype must equal cfg.dtype
- * except freqs_cis (always f32).  The caller keeps the tensor alive. */
+ * except freqs_cis (always f32) and fp8 weights with their scales (below).  The caller keeps the tensor alive. */
 int  lg_engine_bind_weight(lg_engine* e, const char* name, const void* dev_ptr,
                            const int64_t* shape, int ndim, int dtype);
-/* Validate that every tensor the configured model needs is bound. */
+/* fp8 weights (weight-only, "W8A16") of a bf16 / fp16 model. The six GEMM weights "layers.{i}.attention.wqkv.weight",
+ * "...attention.wo.weight", "...feed_forward.w1.weight", "...w3.weight", "...w2.weight" and "output.weight" may each be bound with
+ * dtype LG_DTYPE_E4M3 as dev uint8 codes [N, K], together with a companion tensor "<name>_scale", dev f32 [N] (LG_DTYPE_F32):
+ *   - scale[n] = 2^e, one per output row; allowed e: [-15, 7] for an fp16 model (every code * scale is then an fp16 value, the
+ *     smallest e4m3 subnormal being 2^-9), [-64, 64] for a bf16 model;
+ *   - the layer computes y[r, n] = scale[n] * sum_k x[r, k] * code[n, k]: codes widened exactly to the model dtype, products and sum
+ *     in fp32 on the tensor cores, the scale applied to the fp32 sum before its first rounding. Activations, KV cache, norms,
+ *     embeddings and every rounding point are those of the 16-bit model, so the engine computes what it computes for the 16-bit
+ *     weight code * scale (up to the order of the fp32 sum);
+ *   - stored K order: the code of column k is byte lg_weight_fp8_stored_index(k) of its row. With k = 64 c + 16 s + 8 h + 2 q + b
+ *     (s, q in 0..3; h, b in 0..1) that is 64 c + 16 q + 4 s + 2 h + b: a permutation inside every 64-wide k-block that makes the
+ *     tensor-core A fragments of one thread contiguous. Hence K % 64 == 0, and the batched kernel needs N % 128 == 0.
+ * Any subset of the six may be fp8, except that w1 and w3 of a layer (one GEMM) go together. lg_quantize_rows_e4m3 produces codes
+ * and scales from a 16-bit weight. An fp8 weight has no 16-bit copy inside the engine: a call no fp8 kernel takes is an error. */
+/* Validate that every tensor the configured model needs is bound. An fp8 weight is refused on an fp32 model, without its scales,
+ * with a scale outside the allowed powers of two (the scales are copied to the host: synchronises), and with a shape the fp8 GEMM
+ * kernel does not take (N % 128, K % 64). */
 int  lg_engine_finalize(lg_engine* e);
+/* w dev [N, K] in dtype (LG_DTYPE_BF16 or _F16, K % 64 == 0) -> codes_out dev uint8 [N, K] in the stored K order and scales_out dev
+ * f32 [N]: scale[n] = 2^e with max_k |w[n, k]| / 2^e in (224, 448], e clamped to the allowed range above, 1 for an all-zero row;
+ * code = e4m3_satfinite_rne(float(w[n, k]) / scale[n]) (cvt.rn.satfinite.e4m3x2.f32, the KV-cache writers' conversion). */
+int  lg_quantize_rows_e4m3(const void* w, int N, int K, int dtype, uint8_t* codes_out, float* scales_out, void* stream);
+/* Byte of a stored row that holds column k's code (k >= 0; no GPU needed). */
+int  lg_weight_fp8_stored_index(int k);
 /* Bytes of caller-provided scratch (KV cache + activations) for `rows` sequences (rows = 2*B under CFG)
  * of up to max_seq positions (cls_token_num + new tokens). Replaces setup_caches (gpt.py:316-330). */
 int  lg_engine_workspace_bytes(lg_engine* e, int rows, int max_seq, size_t* bytes);
@@ -255,6 +278,16 @@ int  lg_test_linear(int dtype, int M, int N, int K, const void* x, const void* n
 /* The path of lg_test_linear without buffers or a GPU, after the same checks of the shape-only arguments: paired = wb is passed.
  * has_norm_in is accepted for symmetry with lg_test_linear; no dispatch rule depends on it. */
 int  lg_test_linear_plan(int dtype, int M, int N, int K, int paired, int small, int epi, int has_norm_in, int* plan);
+
+/* lg_test_linear / lg_test_linear_plan with fp8 weights: wa / wb are dev uint8 codes [N][K] in the stored K order with row scales
+ * wa_scale / wb_scale (dev f32 [N], checked like lg_engine_finalize checks them: synchronises). fp8 weights run on gemm_tc_kernel
+ * (kernel 2: bf16 / fp16, N % 128 == 0 - with wb, N is the segment boundary -, K % 64 == 0, LG_GEMM_TC other than 0) and on
+ * gemv_small_kernel (kernel 3, its 16-bit rules and K % 64 == 0); any other call fails with the plan's message. Where both exist,
+ * the plan equals lg_test_linear_plan's for the same arguments; acc_out holds the scaled sums scale[n] * sum_k x * code. */
+int  lg_test_linear_w8(int dtype, int M, int N, int K, const void* x, const void* norm_in, float eps, const uint8_t* wa,
+                       const float* wa_scale, const uint8_t* wb, const float* wb_scale, int epi, const void* norm_out, void* h, void* out,
+                       float* out_f32, float* acc_out, int small, void* dev_scratch, size_t scratch_bytes, int* path, void* stream);
+int  lg_test_linear_w8_plan(int dtype, int M, int N, int K, int paired, int small, int epi, int has_norm_in, int* plan);
 
 /* One transformer attention call through the engine's own dispatch, attn_plan (honouring LG_ATTN_TMA, LG_ATTN_PREFILL_TC,
  * LG_ATTN_NST and LG_ATTN_DEEP). dtype: the model dtype (LG_DTYPE_F32, _BF16 or _F16); kv_dtype: dtype, or LG_DTYPE_E4M3 for a

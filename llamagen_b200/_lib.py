@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("LG_LIB_PATH") or os.path.join(HERE, "lib", "libllamagen_b200.so")
 
 LG_DTYPE_F32, LG_DTYPE_BF16, LG_DTYPE_F16 = 0, 1, 2
-LG_DTYPE_E4M3 = 3   # fp8 e4m3: KV-cache storage only (lg_engine_set_kv_cache)
+LG_DTYPE_E4M3 = 3   # fp8 e4m3: storage of the KV cache (lg_engine_set_kv_cache) and of GEMM weights (lg_engine_bind_weight)
 LG_MODEL_C2I, LG_MODEL_T2I = 0, 1
 
 
@@ -101,6 +101,11 @@ SIGNATURES = {
     "lg_test_linear": (c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_int, c_void_p,
                                c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_size_t, POINTER(c_int), c_void_p]),
     "lg_test_linear_plan": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_int)]),
+    "lg_quantize_rows_e4m3": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "lg_weight_fp8_stored_index": (c_int, [c_int]),
+    "lg_test_linear_w8": (c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_size_t, POINTER(c_int), c_void_p]),
+    "lg_test_linear_w8_plan": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_int)]),
     "lg_test_attention": (c_int, [c_int, c_int, c_float, c_float, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                                   c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int,
                                   c_void_p, c_int, c_void_p, c_void_p, POINTER(c_int), c_void_p]),
@@ -154,6 +159,14 @@ def ptr(t) -> c_void_p:
 def current_stream(device) -> c_void_p:
     import torch
     return c_void_p(torch.cuda.current_stream(device).cuda_stream)
+
+
+def weight_fp8_stored_index(K: int):
+    """int64 [K]: the byte of a stored fp8 weight row that holds column k's code (lg_weight_fp8_stored_index), so that
+    stored[:, index] is the row in column order and natural.new_empty(...)[:, index] = natural packs one."""
+    import torch
+    lib = load()
+    return torch.tensor([lib.lg_weight_fp8_stored_index(k) for k in range(K)], dtype=torch.int64)
 
 
 def shape_array(shape):

@@ -185,7 +185,8 @@ struct Workspace {
 };
 
 struct Layer {
-    const void *wqkv, *wo, *w1, *w3, *w2, *attn_norm, *ffn_norm;
+    GemmWeight wqkv, wo, w1, w3, w2;   // each in the model dtype or fp8 (w1 and w3 alike: one GEMM streams both)
+    const void *attn_norm, *ffn_norm;
 };
 
 }  // namespace
@@ -204,7 +205,9 @@ struct lg_engine {
     std::unordered_map<std::string, Tensor> w;
     std::vector<Layer> layers;
     const void *tok_emb = nullptr, *cls_table = nullptr, *cap_fc1 = nullptr, *cap_fc2 = nullptr, *uncond = nullptr;
-    const void *final_norm = nullptr, *output = nullptr;
+    const void* final_norm = nullptr;
+    GemmWeight output;
+    size_t layer_weight_bytes = 0;        // GEMM weight bytes of the largest layer as bound (the chain-count policy's measure)
     const float* freqs = nullptr;
     bool finalized = false;
     static constexpr int kMaxChains = 2;
@@ -244,9 +247,15 @@ struct lg_engine {
     // R <= 8 decode steps on the column-owner GEMV path (gemv_small.cu); shared by forward() and the decode loop's fused tail
     bool small_row_path(int M, const AttnArgs& aa) const {
         const int D = cfg.dim, F = cfg.ffn_dim, V = cfg.vocab_size, dt = cfg.dtype;
-        return M <= 8 && lg_env_flag("LG_SMALL_R", 1) && fuse_qkv(aa) && gemv_small_supported(M, 3 * D, D, dt, false) &&
-               gemv_small_supported(M, D, D, dt, false) && gemv_small_supported(M, F, D, dt, true) &&
-               gemv_small_supported(M, D, F, dt, false) && gemv_small_supported(M, V, D, dt, false);
+        if (!(M <= 8 && lg_env_flag("LG_SMALL_R", 1) && fuse_qkv(aa) && gemv_small_supported(M, V, D, dt, false, output.scale != nullptr)))
+            return false;
+        for (const Layer& ly : layers)   // the storage of a weight is per layer
+            if (!(gemv_small_supported(M, 3 * D, D, dt, false, ly.wqkv.scale != nullptr) &&
+                  gemv_small_supported(M, D, D, dt, false, ly.wo.scale != nullptr) &&
+                  gemv_small_supported(M, F, D, dt, true, ly.w1.scale != nullptr) &&
+                  gemv_small_supported(M, D, F, dt, false, ly.w2.scale != nullptr)))
+                return false;
+        return true;
     }
     size_t carve(Workspace& o, char* base, int rows, int max_seq, int g = 0, int n = 1) const;
     size_t carve_score(Workspace& o, char* base, int rows, int seq) const;
@@ -280,7 +289,7 @@ struct lg_engine {
     // the transformer blocks over M = R * Tq rows of w.h, leaving RMSNorm_final(h) in w.xn (batched GEMM path)
     int run_layers(const Workspace& w, int M, int Tq, PosArg pos, const float* emb_mask, int B, bool xn_ready, cudaStream_t st);
     int embed_cond(const Workspace& w, const void* cond, int B, int R, int T, cudaStream_t st);
-    int gemm(const Workspace& w, const void* x, int M, int N, int K, const void* wa, const void* wb, int n_split, int* ksplit,
+    int gemm(const Workspace& w, const void* x, int M, int N, int K, const GemmWeight& wa, const GemmWeight& wb, int n_split, int* ksplit,
              float* direct_out, cudaStream_t st, const GemmNext* next = nullptr);
 };
 
@@ -416,10 +425,11 @@ size_t lg_engine::carve_sjd(Workspace& o, SjdArgs& sa, char* base, int B, int nh
     return off;
 }
 
-int lg_engine::gemm(const Workspace& w, const void* x, int M, int N, int K, const void* wa, const void* wb, int n_split, int* ksplit,
+int lg_engine::gemm(const Workspace& w, const void* x, int M, int N, int K, const GemmWeight& wa, const GemmWeight& wb, int n_split, int* ksplit,
                     float* direct_out, cudaStream_t st, const GemmNext* next) {
     // when the plan needs a single slab the GEMM can write straight into `direct_out`
-    const size_t need = gemm_partial_floats(M, N, K, wb ? n_split : 0, cfg.dtype);
+    const size_t need = gemm_partial_floats(M, N, K, wb.p ? n_split : 0, cfg.dtype, wa.scale != nullptr);
+    LG_REQUIRE(need > 0, "%s", gemm_plan(M, N, K, wb.p ? n_split : 0, cfg.dtype, wa.scale != nullptr).error);
     const size_t slabs = need / ((size_t)M * N);
     float* dst = (direct_out && slabs == 1) ? direct_out : w.partial;
     // the plan (k-slices) is not monotone in M and depends on run-time switches: never trust the carve-time sizing blindly
@@ -465,7 +475,7 @@ int lg_engine::forward(const Workspace& w, int M, int Tq, PosArg pos, const floa
         xlast = w.q;
     }
     prof_begin(PC_GEMM_HEAD, st);
-    GemmNext nx_first{layers[0].wqkv, (size_t)3 * D * D * esz, nullptr, 0};   // the next decode step starts with layer 0
+    GemmNext nx_first{layers[0].wqkv.p, layers[0].wqkv.bytes(3 * D, D, esz), nullptr, 0};   // the next decode step starts with layer 0
     const int direct = gemm(w, xlast, R, V, D, output, nullptr, 0, &ks, logits_out, st, &nx_first);
     prof_end(st);
     if (direct < 0) return direct;
@@ -482,10 +492,11 @@ int lg_engine::run_layers(const Workspace& w, int M, int Tq, PosArg pos, const f
     for (int l = 0; l < L; ++l) {
         const Layer& ly = layers[l];
         const size_t eb = esz;
-        GemmNext nx_wo{ly.wo, (size_t)D * D * eb, nullptr, 0};
-        GemmNext nx_w13{ly.w1, (size_t)F * D * eb, ly.w3, (size_t)F * D * eb};
-        GemmNext nx_w2{ly.w2, (size_t)D * F * eb, nullptr, 0};
-        GemmNext nx_qkv{(l + 1 < L) ? layers[l + 1].wqkv : output, (l + 1 < L) ? (size_t)3 * D * D * eb : (size_t)V * D * eb, nullptr, 0};
+        const bool last = l + 1 == L;     // prefetch sizes are those of the tensors as bound (fp8 codes are one byte)
+        GemmNext nx_wo{ly.wo.p, ly.wo.bytes(D, D, eb), nullptr, 0};
+        GemmNext nx_w13{ly.w1.p, ly.w1.bytes(F, D, eb), ly.w3.p, ly.w3.bytes(F, D, eb)};
+        GemmNext nx_w2{ly.w2.p, ly.w2.bytes(D, F, eb), nullptr, 0};
+        GemmNext nx_qkv{last ? output.p : layers[l + 1].wqkv.p, last ? output.bytes(V, D, eb) : layers[l + 1].wqkv.bytes(3 * D, D, eb), nullptr, 0};
         LG_PROF(PC_GEMM_QKV, st, gemm(w, w.xn, M, 3 * D, D, ly.wqkv, nullptr, 0, &ks, nullptr, st, &nx_wo));
         AttnArgs aa = layer_attn(w, l, R, Tq, pos, emb_mask, B);
         if (fuse_qkv(aa)) {
@@ -587,25 +598,55 @@ static int need(lg_engine* e, const std::string& name, int dtype, std::initializ
     return 0;
 }
 
+// A GEMM weight [N][K] (n_split: the w1 | w3 boundary of the GEMM that streams it, 0 for one segment): in the model dtype, or bound as
+// LG_DTYPE_E4M3 codes with its companion "<name>_scale" fp32 [N]. An fp8 weight is refused on an fp32 model, without its scales, with
+// a scale that is not an allowed power of two, and with a shape the fp8 GEMM kernel does not take.
+static int need_gemm_weight(lg_engine* e, const std::string& name, int64_t N, int64_t K, int NN, int n_split, GemmWeight* out) {
+    const int dt = e->cfg.dtype;
+    auto it = e->w.find(name);
+    const void* p = nullptr;
+    if (it == e->w.end() || it->second.dtype != LG_DTYPE_E4M3) {
+        LG_TRY(need(e, name, dt, {N, K}, &p));
+        *out = GemmWeight(p);
+        return 0;
+    }
+    LG_REQUIRE(lg_dtype_is16(dt), "weight '%s' is fp8: fp8 weights need a bf16 or fp16 model (model dtype %d)", name.c_str(), dt);
+    LG_TRY(need(e, name, LG_DTYPE_E4M3, {N, K}, &p));
+    const void* sc = nullptr;
+    LG_TRY(need(e, name + "_scale", LG_DTYPE_F32, {N}, &sc));
+    const GemmPlan plan = gemm_plan(16, NN, (int)K, n_split, dt, true);
+    LG_REQUIRE(plan.kernel >= 0, "weight '%s' [%lld, %lld] cannot be fp8: %s", name.c_str(), (long long)N, (long long)K, plan.error);
+    DeviceGuard guard(e->device);
+    LG_TRY(w8_check_scales((name + "_scale").c_str(), (const float*)sc, (int)N, dt));
+    *out = GemmWeight(p, (const float*)sc);
+    return 0;
+}
+
 int lg_engine_finalize(lg_engine* e) {
     LG_REQUIRE(e, "null engine");
     const lg_model_cfg& c = e->cfg;
     const int D = c.dim, F = c.ffn_dim, V = c.vocab_size, dt = c.dtype;
     e->layers.resize(c.n_layer);
+    e->layer_weight_bytes = 0;
     for (int l = 0; l < c.n_layer; ++l) {
         const std::string p = "layers." + std::to_string(l) + ".";
         Layer& ly = e->layers[l];
-        LG_TRY(need(e, p + "attention.wqkv.weight", dt, {3 * D, D}, &ly.wqkv));
-        LG_TRY(need(e, p + "attention.wo.weight", dt, {D, D}, &ly.wo));
-        LG_TRY(need(e, p + "feed_forward.w1.weight", dt, {F, D}, &ly.w1));
-        LG_TRY(need(e, p + "feed_forward.w3.weight", dt, {F, D}, &ly.w3));
-        LG_TRY(need(e, p + "feed_forward.w2.weight", dt, {D, F}, &ly.w2));
+        LG_TRY(need_gemm_weight(e, p + "attention.wqkv.weight", 3 * D, D, 3 * D, 0, &ly.wqkv));
+        LG_TRY(need_gemm_weight(e, p + "attention.wo.weight", D, D, D, 0, &ly.wo));
+        LG_TRY(need_gemm_weight(e, p + "feed_forward.w1.weight", F, D, 2 * F, F, &ly.w1));
+        LG_TRY(need_gemm_weight(e, p + "feed_forward.w3.weight", F, D, 2 * F, F, &ly.w3));
+        LG_REQUIRE((ly.w1.scale != nullptr) == (ly.w3.scale != nullptr),
+                   "layer %d: feed_forward.w1 and w3 are streamed by one GEMM and must both be fp8 or both be 16-bit", l);
+        LG_TRY(need_gemm_weight(e, p + "feed_forward.w2.weight", D, F, D, 0, &ly.w2));
+        e->layer_weight_bytes = std::max(e->layer_weight_bytes, ly.wqkv.bytes(3 * D, D, e->esz) + ly.wo.bytes(D, D, e->esz) +
+                                                                    ly.w1.bytes(F, D, e->esz) + ly.w3.bytes(F, D, e->esz) +
+                                                                    ly.w2.bytes(D, F, e->esz));
         LG_TRY(need(e, p + "attention_norm.weight", dt, {D}, &ly.attn_norm));
         LG_TRY(need(e, p + "ffn_norm.weight", dt, {D}, &ly.ffn_norm));
     }
     LG_TRY(need(e, "tok_embeddings.weight", dt, {V, D}, &e->tok_emb));
     LG_TRY(need(e, "norm.weight", dt, {D}, &e->final_norm));
-    LG_TRY(need(e, "output.weight", dt, {V, D}, &e->output));
+    LG_TRY(need_gemm_weight(e, "output.weight", V, D, V, 0, &e->output));
     if (c.model_type == LG_MODEL_C2I) {
         auto it = e->w.find("cls_embedding.embedding_table.weight");
         LG_REQUIRE(it != e->w.end(), "missing weight 'cls_embedding.embedding_table.weight'");
@@ -650,11 +691,12 @@ int lg_engine_set_workspace(lg_engine* e, void* dev_ws, size_t bytes, int rows, 
     e->n_sub = 0;
     // Chain-count policy: every chain streams ALL the weights, so two chains only pay while a layer's weights survive in L2 between
     // the chains' visits, next to the KV and activation traffic of the other chain; otherwise they double the HBM weight traffic.
-    // Two chains run while a layer is at most a third of the L2. On an H100 80GB HBM3 (50 MB L2; both settings alternated twice in
+    // Two chains run while a layer's GEMM weights as bound (fp8 weights count one byte per element) are at most a third of the L2. On an H100 80GB HBM3 (50 MB L2; both settings alternated twice in
     // one run) one chain is faster for GPT-L (27 MB per layer, c2i 256 px, B = 64: 431 vs 469 ms/step) and GPT-XL (39 MB, 384 px,
     // B = 32: 1659 vs 1849 ms/step).
     // LG_SPLIT forces the chain count (at most two).
-    const double layer_bytes = (4.0 * e->cfg.dim * e->cfg.dim + 3.0 * e->cfg.dim * e->cfg.ffn_dim) * e->esz;
+    const double layer_bytes = e->finalized ? (double)e->layer_weight_bytes
+                                            : (4.0 * e->cfg.dim * e->cfg.dim + 3.0 * e->cfg.dim * e->cfg.ffn_dim) * e->esz;
     int l2_bytes = 0, dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&l2_bytes, cudaDevAttrL2CacheSize, dev) != cudaSuccess) l2_bytes = 0;
     int n = lg_env_flag("LG_SPLIT", 3.0 * layer_bytes <= (double)l2_bytes ? 2 : 1);
@@ -1212,18 +1254,19 @@ int lg_test_gemm(const void* x, const void* w, int M, int N, int K, int dtype, f
 
 // What lg_test_linear and lg_test_linear_plan (fn) check of the shape-only arguments, then the call's path {kernel (3: gemv_small),
 // tile, ksplit, row blocks or PF}
-static int test_linear_args(const char* fn, int dtype, int M, int N, int K, bool paired, bool small, int epi, bool norm_out, int* path) {
+static int test_linear_args(const char* fn, int dtype, int M, int N, int K, bool paired, bool small, int epi, bool norm_out, bool w8,
+                            int* path) {
     LG_REQUIRE(epi >= 0 && epi <= 4, "%s: epilogue %d outside 0..4", fn, epi);
     LG_REQUIRE(paired == (epi == 2), "%s: wb goes with the SwiGLU epilogue (2) alone, epilogue %d", fn, epi);
     LG_REQUIRE(!norm_out || (epi == 1 && !small), "%s: norm_out goes with the batched residual epilogue alone", fn);
     if (small) {
         LG_REQUIRE(epi <= 2, "%s: the small path has no store or gelu epilogue (%d)", fn, epi);
-        const GemvSmallPlan p = gemv_small_plan(M, N, K, dtype, paired);
+        const GemvSmallPlan p = gemv_small_plan(M, N, K, dtype, paired, w8);
         LG_REQUIRE(p.rows != 0, "%s: %s", fn, p.error);
         path[0] = 3; path[1] = p.rows; path[2] = 1; path[3] = p.pf;
         return 0;
     }
-    const GemmPlan p = gemm_plan(M, paired ? 2 * N : N, K, paired ? N : 0, dtype);
+    const GemmPlan p = gemm_plan(M, paired ? 2 * N : N, K, paired ? N : 0, dtype, w8);
     LG_REQUIRE(p.kernel >= 0, "%s: %s", fn, p.error);
     LG_REQUIRE(epi != 1 || (N % 4 == 0 && N <= 4096), "%s: the residual epilogue needs N %% 4 == 0 and N <= 4096 (N=%d)", fn, N);
     LG_REQUIRE(epi != 2 || N % 4 == 0, "%s: the SwiGLU epilogue needs N %% 4 == 0 (N=%d)", fn, N);
@@ -1231,23 +1274,28 @@ static int test_linear_args(const char* fn, int dtype, int M, int N, int K, bool
     return 0;
 }
 
-int lg_test_linear(int dtype, int M, int N, int K, const void* x, const void* norm_in, float eps, const void* wa, const void* wb, int epi,
-                   const void* norm_out, void* h, void* out, float* out_f32, float* acc_out, int small, void* dev_scratch,
-                   size_t scratch_bytes, int* path, void* stream) {
-    cudaStream_t st = (cudaStream_t)stream;
+// lg_test_linear / lg_test_linear_w8 (fn) over weights in the model dtype / fp8 weights (w8: wa.scale and, with wb, wb.scale set)
+static int test_linear_run(const char* fn, bool w8, int dtype, int M, int N, int K, const void* x, const void* norm_in, float eps,
+                           const GemmWeight& wa, const GemmWeight& wb, int epi, const void* norm_out, void* h, void* out, float* out_f32,
+                           float* acc_out, int small, void* dev_scratch, size_t scratch_bytes, int* path, cudaStream_t st) {
     auto a16 = [](const void* p) { return ((uintptr_t)p & 15) == 0; };
     int pl[4];
-    LG_TRY(test_linear_args("lg_test_linear", dtype, M, N, K, wb != nullptr, small != 0, epi, norm_out != nullptr, pl));
-    LG_REQUIRE(x && wa && a16(x) && a16(wa) && a16(wb) && a16(norm_in) && a16(norm_out) && a16(h) && a16(out) && a16(out_f32) && a16(acc_out),
-               "lg_test_linear: null or misaligned (16 bytes) operand");
+    LG_TRY(test_linear_args(fn, dtype, M, N, K, wb.p != nullptr, small != 0, epi, norm_out != nullptr, w8, pl));
+    LG_REQUIRE(x && wa.p && a16(x) && a16(wa.p) && a16(wb.p) && a16(norm_in) && a16(norm_out) && a16(h) && a16(out) && a16(out_f32) && a16(acc_out),
+               "%s: null or misaligned (16 bytes) operand", fn);
     LG_REQUIRE((out_f32 != nullptr) == (epi == 0) && (h != nullptr) == (epi == 1) && (out != nullptr) == (epi >= 2 || norm_out != nullptr),
-               "lg_test_linear: epilogue %d writes out_f32 (0), h (1), out (1 with norm_out, 2-4) and no other buffer", epi);
-    LG_REQUIRE(!small || !acc_out, "lg_test_linear: the small path keeps its accumulator on chip (acc_out)");
-    const int NN = wb ? 2 * N : N;
-    const size_t pbytes = small ? 0 : align_up(gemm_partial_floats(M, NN, K, wb ? N : 0, dtype) * sizeof(float));
+               "%s: epilogue %d writes out_f32 (0), h (1), out (1 with norm_out, 2-4) and no other buffer", fn, epi);
+    LG_REQUIRE(!small || !acc_out, "%s: the small path keeps its accumulator on chip (acc_out)", fn);
+    if (w8) {
+        LG_REQUIRE(wa.scale && (wb.p == nullptr) == (wb.scale == nullptr), "%s: every fp8 weight comes with its row scales", fn);
+        LG_TRY(w8_check_scales("wa_scale", wa.scale, N, dtype));
+        if (wb.p) LG_TRY(w8_check_scales("wb_scale", wb.scale, N, dtype));
+    }
+    const int NN = wb.p ? 2 * N : N;
+    const size_t pbytes = small ? 0 : align_up(gemm_partial_floats(M, NN, K, wb.p ? N : 0, dtype, w8) * sizeof(float));
     const size_t need = pbytes + (!small && norm_in ? (size_t)M * K * lg_dtype_info(dtype).esz : 0);
     LG_REQUIRE(need == 0 || (dev_scratch && ((uintptr_t)dev_scratch & 255) == 0 && scratch_bytes >= need),
-               "lg_test_linear: scratch %zu < %zu (256-byte aligned)", scratch_bytes, need);
+               "%s: scratch %zu < %zu (256-byte aligned)", fn, scratch_bytes, need);
     if (path) std::copy(pl, pl + 4, path);
     if (small) {
         GemvSmall g{wa, wb, N, K, M, x, norm_in, eps, epi == 0 ? out_f32 : nullptr, epi == 1 ? h : nullptr, epi == 2 ? out : nullptr, dtype};
@@ -1260,7 +1308,7 @@ int lg_test_linear(int dtype, int M, int N, int K, const void* x, const void* no
         LG_TRY(launch_rmsnorm(x, norm_in, (void*)xin, M, K, eps, dtype, st));
     }
     GemmPlan p;
-    LG_TRY(gemm_partial(xin, K, wa, wb, wb ? N : 0, M, NN, K, dtype, partial, &p, st));
+    LG_TRY(gemm_partial(xin, K, wa, wb, wb.p ? N : 0, M, NN, K, dtype, partial, &p, st));
     if (acc_out) LG_TRY(launch_reduce_f32(partial, p.ksplit, M, NN, acc_out, st));
     switch (epi) {
         case 0: return launch_reduce_f32(partial, p.ksplit, M, N, out_f32, st);
@@ -1270,11 +1318,36 @@ int lg_test_linear(int dtype, int M, int N, int K, const void* x, const void* no
     }
 }
 
+int lg_test_linear(int dtype, int M, int N, int K, const void* x, const void* norm_in, float eps, const void* wa, const void* wb, int epi,
+                   const void* norm_out, void* h, void* out, float* out_f32, float* acc_out, int small, void* dev_scratch,
+                   size_t scratch_bytes, int* path, void* stream) {
+    return test_linear_run("lg_test_linear", false, dtype, M, N, K, x, norm_in, eps, GemmWeight(wa), GemmWeight(wb), epi, norm_out, h, out,
+                           out_f32, acc_out, small, dev_scratch, scratch_bytes, path, (cudaStream_t)stream);
+}
+
+int lg_test_linear_w8(int dtype, int M, int N, int K, const void* x, const void* norm_in, float eps, const uint8_t* wa, const float* wa_scale,
+                      const uint8_t* wb, const float* wb_scale, int epi, const void* norm_out, void* h, void* out, float* out_f32,
+                      float* acc_out, int small, void* dev_scratch, size_t scratch_bytes, int* path, void* stream) {
+    return test_linear_run("lg_test_linear_w8", true, dtype, M, N, K, x, norm_in, eps, GemmWeight(wa, wa_scale), GemmWeight(wb, wb_scale), epi,
+                           norm_out, h, out, out_f32, acc_out, small, dev_scratch, scratch_bytes, path, (cudaStream_t)stream);
+}
+
 int lg_test_linear_plan(int dtype, int M, int N, int K, int paired, int small, int epi, int has_norm_in, int* plan) {
     (void)has_norm_in;   // no dispatch rule depends on the RMSNorm prologue
     LG_REQUIRE(plan, "lg_test_linear_plan: null plan");
-    return test_linear_args("lg_test_linear_plan", dtype, M, N, K, paired != 0, small != 0, epi, false, plan);
+    return test_linear_args("lg_test_linear_plan", dtype, M, N, K, paired != 0, small != 0, epi, false, false, plan);
 }
+
+int lg_test_linear_w8_plan(int dtype, int M, int N, int K, int paired, int small, int epi, int has_norm_in, int* plan) {
+    (void)has_norm_in;
+    LG_REQUIRE(plan, "lg_test_linear_w8_plan: null plan");
+    return test_linear_args("lg_test_linear_w8_plan", dtype, M, N, K, paired != 0, small != 0, epi, false, true, plan);
+}
+
+int lg_quantize_rows_e4m3(const void* w, int N, int K, int dtype, uint8_t* codes_out, float* scales_out, void* stream) {
+    return launch_quantize_rows_e4m3(w, N, K, dtype, codes_out, scales_out, (cudaStream_t)stream);
+}
+int lg_weight_fp8_stored_index(int k) { return k < 0 ? -1 : w8_stored_index(k); }
 
 // What lg_test_attention and lg_test_attention_plan (fn) check of the shape-only arguments, then the call's AttnArgs (no QKV slabs
 // attached yet) over a K / V buffer of n_layer layers, with `maps` as the engine builds them (without a buffer: only whether it would),

@@ -89,7 +89,7 @@ __global__ void __launch_bounds__(kSkinnyWarps * 32) gemm_skinny_kernel(const T*
 
 }  // namespace
 
-GemmPlan gemm_plan(int M, int N, int K, int n_split, int dtype) {
+GemmPlan gemm_plan(int M, int N, int K, int n_split, int dtype, bool w8) {
     GemmPlan p;
     if (M <= 0 || N <= 0 || K <= 0) {
         snprintf(p.error, sizeof(p.error), "gemm: bad shape %d %d %d", M, N, K);
@@ -111,6 +111,18 @@ GemmPlan gemm_plan(int M, int N, int K, int n_split, int dtype) {
     // skinny kernel stays for the fp32 exact mode. A wgmma CTA streams one 128-row weight tile from one segment, so the w1 | w3
     // boundary must fall on a tile edge; any other boundary (ffn_dim % 128 != 0) goes to the row-wise loaders of the other kernels.
     const bool one_segment = n_split == 0 || n_split == N;
+    if (w8) {
+        // fp8 weights exist only as e4m3 codes: the wgmma kernel is their one batched kernel, and a call it cannot take is an error
+        if (!lg_dtype_is16(dtype))
+            snprintf(p.error, sizeof(p.error), "gemm: fp8 weights need a bf16 or fp16 model (dtype %d)", dtype);
+        else if (N % 128 != 0 || !(one_segment || n_split % 128 == 0))
+            snprintf(p.error, sizeof(p.error), "gemm: fp8 weights need N=%d and the segment boundary %d on 128-row tiles", N, n_split);
+        else if (K % 64 != 0)
+            snprintf(p.error, sizeof(p.error), "gemm: fp8 weights need K=%d a multiple of 64", K);
+        else if (!lg_env_flag("LG_GEMM_TC", 1))
+            snprintf(p.error, sizeof(p.error), "gemm: fp8 weights run on the wgmma kernel only (LG_GEMM_TC=0)");
+        if (p.error[0]) return p;
+    }
     const bool tc_ok = lg_env_flag("LG_GEMM_TC", 1) && lg_dtype_is16(dtype) && N % 128 == 0 && (one_segment || n_split % 128 == 0);
     if (tc_ok) {
         const int rblk = std::min(M, 256);
@@ -140,17 +152,20 @@ GemmPlan gemm_plan(int M, int N, int K, int n_split, int dtype) {
     return p;
 }
 
-size_t gemm_partial_floats(int M, int N, int K, int n_split, int dtype) {
-    const GemmPlan p = gemm_plan(M, N, K, n_split, dtype);
+size_t gemm_partial_floats(int M, int N, int K, int n_split, int dtype, bool w8) {
+    const GemmPlan p = gemm_plan(M, N, K, n_split, dtype, w8);
     return p.kernel < 0 ? 0 : (size_t)p.ksplit * M * N;
 }
 
-int gemm_partial(const void* X, int ldx, const void* Wa, const void* Wb, int n_split, int M, int N, int K, int dtype,
+int gemm_partial(const void* X, int ldx, const GemmWeight& wa, const GemmWeight& wb_in, int n_split, int M, int N, int K, int dtype,
                  float* partial, GemmPlan* plan, cudaStream_t st, const GemmNext* next) {
-    if (Wb == nullptr || n_split == 0) { Wb = Wa; n_split = N; }
-    const GemmPlan p = gemm_plan(M, N, K, n_split, dtype);
+    GemmWeight wb = wb_in;
+    if (wb.p == nullptr || n_split == 0) { wb = wa; n_split = N; }
+    LG_REQUIRE((wa.scale != nullptr) == (wb.scale != nullptr), "gemm: both weight segments must be fp8 or both 16-bit");
+    const GemmPlan p = gemm_plan(M, N, K, n_split, dtype, wa.scale != nullptr);
     if (plan) *plan = p;
     if (p.kernel < 0) return lg_fail("%s", p.error);
+    const void *Wa = wa.p, *Wb = wb.p;
     if (p.kernel == 0) {
         // kper: multiple of 256 elements so every lane's 16-byte vector stays inside the slab
         int kper = cdiv(cdiv(K, p.ksplit), 256) * 256;
@@ -176,7 +191,7 @@ int gemm_partial(const void* X, int ldx, const void* Wa, const void* Wb, int n_s
         LG_LAUNCH_CHECK();
         return 0;
     }
-    if (p.kernel == 2) return gemm_tc_partial(X, ldx, Wa, Wb, n_split, M, N, K, dtype, p, partial, st, next);
+    if (p.kernel == 2) return gemm_tc_partial(X, ldx, wa, wb, n_split, M, N, K, dtype, p, partial, st, next);
     mma::DenseA al{(const bf16*)X, ldx, 0, M};   // raw 16-bit elements: the same loaders serve fp16
     mma::BRows bw{(const bf16*)Wa, (const bf16*)Wb, n_split, K, 0, N};
     mma::EpiPartial epi{partial, M, N};

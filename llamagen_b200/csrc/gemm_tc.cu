@@ -11,6 +11,15 @@
 //
 // Warp roles (288 threads): warps 0-7 = two consumer warpgroups (features [0, 64) and [64, 128) of the tile), warp 8 = TMA
 // producer (one elected lane). Each consumer warpgroup stores its accumulator straight from registers into the fp32 slab.
+//
+// fp8 weights (W8 instantiations, LG_DTYPE_E4M3 codes + one fp32 power-of-two scale per weight row, see the layout in
+// include/llamagen_b200.h): the weight stage is a [128 x 64] byte tile written by TMA with the 64-byte swizzle, half the bytes of the
+// 16-bit tile. The consumers do not hand it to the MMA through a descriptor: each thread reads the two 16-byte pieces that hold
+// its A fragments of the whole k-block (the stored K order makes them contiguous), widens them exactly to T (e4m3x2_to<T>) and
+// issues the k-block's four wgmma with A from registers as one group, which it waits for before it widens the next k-block (the
+// next k-block's bytes are fetched from shared memory while the group runs); B (activations) and everything else are as in the
+// 16-bit kernel. The drain multiplies
+// accumulator row n by scale[n] before the slab store, so the slabs hold what a 16-bit GEMM on the dequantised weight would.
 #include "kernels.cuh"
 #include "tma_utils.cuh"
 #include "wgmma_utils.cuh"
@@ -26,6 +35,7 @@ constexpr int kRingStages = 4;  // stages the host launches with (fewer when a C
 constexpr int kTargetCtas = 92; // split-K CTA target per GEMM (~0.7 per SM of an H100)
 constexpr int kThreads = 288;   // 2 consumer warpgroups + 1 producer warp
 constexpr int kATileBytes = kBlockN * kBlockK * 2;   // 16 KB
+constexpr int kATileBytesW8 = kBlockN * kBlockK;     // 8 KB of e4m3 codes
 constexpr int kMaxRowsPerCta = 256;                  // wgmma N <= 256
 
 using namespace tma;
@@ -40,17 +50,19 @@ struct TcArgs {
     const char* pf0; unsigned long long pfb0;   // next GEMM's weights to pull into L2 (see GemmNext)
     const char* pf1; unsigned long long pfb1;
     unsigned long long whint;    // L2 eviction hint of the weight tiles (0: default policy)
+    const float* sca; const float* scb;   // fp8 weights: the row scales of the two weight segments
 };
 
 // RP: rows of one row block padded to a power of two (wgmma N); the activation box has RP rows, rows >= M read as zero.
-// T: operand type (bf16 or f16), only the wgmma instruction depends on it.
-template <int RP, typename T>
+// T: operand type (bf16 or f16), only the wgmma instruction depends on it. W8: the weight maps are e4m3 code maps.
+template <int RP, typename T, bool W8>
 __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_constant__ CUtensorMap map_wa,
                                                               const __grid_constant__ CUtensorMap map_wb,
                                                               const __grid_constant__ CUtensorMap map_x, TcArgs a) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     constexpr int b_tile_bytes = RP * kBlockK * 2;
-    constexpr int stage_bytes = kATileBytes + ((b_tile_bytes + 1023) / 1024) * 1024;
+    constexpr int a_tile_bytes = W8 ? kATileBytesW8 : kATileBytes;
+    constexpr int stage_bytes = a_tile_bytes + ((b_tile_bytes + 1023) / 1024) * 1024;
     uint8_t* tiles = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     const int kStages = a.stages;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(tiles + kStages * stage_bytes);
@@ -82,7 +94,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
             const bool second = n0 >= a.n_split;
             const CUtensorMap* wmap = second ? &map_wb : &map_wa;
             const int wrow = second ? n0 - a.n_split : n0;
-            const uint32_t tx = (uint32_t)(kATileBytes + b_tile_bytes);
+            const uint32_t tx = (uint32_t)(a_tile_bytes + b_tile_bytes);
             // Weights do not depend on the previous kernel: the first ring of weight tiles is requested BEFORE
             // the programmatic-dependency wait, so the HBM stream of this GEMM overlaps the tail of its producer.
             const int npre = min(nkb, kStages);
@@ -92,7 +104,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
             }
             lg_pdl_wait();
             for (int i = 0; i < npre; ++i)
-                load_2d(tiles + i * stage_bytes + kATileBytes, &map_x, &full_bar[i], (kb0 + i) * kBlockK, row0);
+                load_2d(tiles + i * stage_bytes + a_tile_bytes, &map_x, &full_bar[i], (kb0 + i) * kBlockK, row0);
             for (int i = npre; i < nkb; ++i) {
                 const int s = i % kStages;
                 const uint32_t ph = (uint32_t)((i / kStages) & 1);
@@ -100,7 +112,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                 mbar_expect_tx(&full_bar[s], tx);
                 uint8_t* sa = tiles + s * stage_bytes;
                 load_2d_hint(sa, wmap, &full_bar[s], (kb0 + i) * kBlockK, wrow, a.whint);
-                load_2d(sa + kATileBytes, &map_x, &full_bar[s], (kb0 + i) * kBlockK, row0);
+                load_2d(sa + a_tile_bytes, &map_x, &full_bar[s], (kb0 + i) * kBlockK, row0);
             }
             // ask L2 for this CTA's share of the next GEMM's weights (static chain: qkv -> wo -> w1|w3 -> w2 -> next qkv)
             {
@@ -129,18 +141,78 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     float acc[RP / 2];
 #pragma unroll
     for (int i = 0; i < RP / 2; ++i) acc[i] = 0.f;
-    for (int i = 0; i < nkb; ++i) {
-        const int s = i % kStages;
-        const uint32_t ph = (uint32_t)((i / kStages) & 1);
-        mbar_wait(&full_bar[s], ph);
-        const uint32_t sa = smem_u32(tiles + s * stage_bytes);
-        wg::fence_regs<RP / 2>(acc);
-        wg::fence();
-        wg::mma_kblock<RP, T>(acc, sa + g * (kATileBytes / 2), sa + kATileBytes);
-        wg::commit();
-        wg::wait<1>();                                  // the previous k-block's MMAs have retired: release its stage
-        wg::fence_regs<RP / 2>(acc);
-        if (i > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[(i - 1) % kStages]);
+    float sc[2] = {1.f, 1.f};   // fp8: the scales of accumulator rows frag_row(i), one per value of (i >> 1) & 1
+    if constexpr (W8) {
+        const bool second = n0 >= a.n_split;
+        const float* sp = (second ? a.scb + (n0 - a.n_split) : a.sca + n0) + 64 * g + wg::frag_row(0);
+        sc[0] = __ldg(sp);
+        sc[1] = __ldg(sp + 8);
+        // This thread's A fragments of one k-block: rows r and r + 8 of the warpgroup's half tile, 16-byte piece q = lane % 4 of the 64-byte row
+        // (TMA's 64-byte swizzle XORs the piece index with bits 7-8 of the address, the same for both rows).
+        const int r = 64 * g + wg::frag_row(0), q = lane & 3;
+        const uint32_t aoff = (uint32_t)(r * kBlockK + ((q ^ ((r >> 1) & 3)) << 4));
+        // One k-block: widen the raw pieces into the A registers, issue its four MMAs as one group, fetch the next k-block's raw pieces from
+        // shared memory while they run, then wait for the group. The A registers are written only while no wgmma is in flight (ptxas
+        // serialises every wgmma of a pipeline stage in which another instruction defines one of its input registers); the raw pieces
+        // are ordinary registers, so the full-barrier wait and the shared-memory latency of k-block i + 1 overlap the MMAs of k-block i.
+        auto fetch = [&](int i, uint4& lo, uint4& hi) {
+            const int s = i % kStages;
+            mbar_wait(&full_bar[s], (uint32_t)((i / kStages) & 1));
+            const uint8_t* wt = tiles + s * stage_bytes;
+            lo = *reinterpret_cast<const uint4*>(wt + aoff);
+            hi = *reinterpret_cast<const uint4*>(wt + aoff + 8 * kBlockK);
+        };
+        uint4 lo = make_uint4(0u, 0u, 0u, 0u), hi = lo;
+        if (nkb > 0) fetch(0, lo, hi);
+        for (int i = 0; i < nkb; ++i) {
+            const uint32_t wl[4] = {lo.x, lo.y, lo.z, lo.w}, wh[4] = {hi.x, hi.y, hi.z, hi.w};
+            const int s = i % kStages;
+            const uint64_t bd = wg::make_desc_sw128(smem_u32(tiles + s * stage_bytes + a_tile_bytes));
+            // MMAs per group: the whole k-block, but two for the 256-row tile, whose 128 accumulators leave room for 8 A registers
+            // under the 168-register ceiling of a 288-thread CTA (with 16, ptxas serialises every wgmma for lack of registers)
+            constexpr int G = RP == 256 ? 2 : 4;
+#pragma unroll
+            for (int k0 = 0; k0 < 4; k0 += G) {
+                uint32_t af[4 * G];
+#pragma unroll
+                for (int k = 0; k < G; ++k) {   // word k: codes of k = 16k + 2q, +1 (low half) and 16k + 8 + 2q, +1 (high half)
+                    af[4 * k + 0] = e4m3x2_to<T>(wl[k0 + k]);
+                    af[4 * k + 1] = e4m3x2_to<T>(wh[k0 + k]);
+                    af[4 * k + 2] = e4m3x2_to<T>(wl[k0 + k] >> 16);
+                    af[4 * k + 3] = e4m3x2_to<T>(wh[k0 + k] >> 16);
+                }
+                wg::fence_regs<RP / 2>(acc);
+                wg::fence();
+#pragma unroll
+                for (int k = 0; k < G; ++k) wg::WgmmaRS<RP, T>::mma(acc, af + 4 * k, bd + (uint64_t)(2 * (k0 + k)));
+                wg::commit();
+                if (k0 + G < 4) {
+                    wg::wait<0>();
+                    wg::fence_regs<RP / 2>(acc);
+                }
+            }
+            // the 256-row tile has no registers to spare for raw pieces beside 128 accumulators (ptxas would serialise its wgmma):
+            // it fetches after the wait
+            if (RP < 256 && i + 1 < nkb) fetch(i + 1, lo, hi);
+            wg::wait<0>();                              // this k-block's MMAs have retired (its weight bytes left the stage before them)
+            wg::fence_regs<RP / 2>(acc);
+            if (RP == 256 && i + 1 < nkb) fetch(i + 1, lo, hi);
+            if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[s]);
+        }
+    } else {
+        for (int i = 0; i < nkb; ++i) {
+            const int s = i % kStages;
+            const uint32_t ph = (uint32_t)((i / kStages) & 1);
+            mbar_wait(&full_bar[s], ph);
+            const uint32_t sa = smem_u32(tiles + s * stage_bytes);
+            wg::fence_regs<RP / 2>(acc);
+            wg::fence();
+            wg::mma_kblock<RP, T>(acc, sa + g * (kATileBytes / 2), sa + kATileBytes);
+            wg::commit();
+            wg::wait<1>();                                  // the previous k-block's MMAs have retired: release its stage
+            wg::fence_regs<RP / 2>(acc);
+            if (i > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[(i - 1) % kStages]);
+        }
     }
     wg::wait<0>();
     wg::fence_regs<RP / 2>(acc);
@@ -149,7 +221,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
 #pragma unroll
     for (int i = 0; i < RP / 2; ++i) {
         const int n = n0 + 64 * g + wg::frag_row(i), r = wg::frag_col(i);
-        if (n < a.N && r < Mb) out[(size_t)r * a.N + n] = acc[i];
+        if (n < a.N && r < Mb) out[(size_t)r * a.N + n] = W8 ? acc[i] * sc[(i >> 1) & 1] : acc[i];
     }
 }
 
@@ -219,11 +291,11 @@ int gemm_tc_ksplit(int M, int N, int K) {
     return std::min(ks, 16);
 }
 
-template <int RP, typename T>
+template <int RP, typename T, bool W8>
 static int gemm_tc_launch_t(const CUtensorMap& mwa, const CUtensorMap& mwb, const CUtensorMap& mx, TcArgs& a, dim3 grid,
                             cudaStream_t st) {
     constexpr int b_tile_bytes = RP * kBlockK * 2;
-    constexpr int stage_bytes = kATileBytes + ((b_tile_bytes + 1023) / 1024) * 1024;
+    constexpr int stage_bytes = (W8 ? kATileBytesW8 : kATileBytes) + ((b_tile_bytes + 1023) / 1024) * 1024;
     // 4 stages instead of filling shared memory: a CTA never owns more than ~8 k-blocks, and the smaller footprint lets the
     // PDL-launched next kernel become resident next to this one.
     static_assert(1024 + kRingStages * stage_bytes + 2 * kMaxStages * sizeof(uint64_t) <= 227 * 1024, "gemm_tc: ring too large");
@@ -231,18 +303,19 @@ static int gemm_tc_launch_t(const CUtensorMap& mwa, const CUtensorMap& mwb, cons
     const size_t smem = 1024 + (size_t)a.stages * stage_bytes + 2 * kMaxStages * sizeof(uint64_t);
     static DevOnce attr;
     if (lg_first_on_device(attr)) {
-        LG_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<RP, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        LG_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<RP, T, W8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     }
-    (void)lg_launch(gemm_tc_kernel<RP, T>, grid, dim3(kThreads), smem, st, mwa, mwb, mx, a);
+    (void)lg_launch(gemm_tc_kernel<RP, T, W8>, grid, dim3(kThreads), smem, st, mwa, mwb, mx, a);
     LG_LAUNCH_CHECK();
     return 0;
 }
 
-template <typename T>
+template <typename T, bool W8>
 static int gemm_tc_launch(const void* X, int ldx, const void* Wa, const void* Wb, int n_split, int M, int N, int K,
-                          const GemmPlan& p, float* partial, cudaStream_t st, const GemmNext* next) {
-    constexpr int dt = ElemTraits<T>::dtype;
-    if (Wb == nullptr) { Wb = Wa; n_split = N; }
+                          const float* sca, const float* scb, const GemmPlan& p, float* partial, cudaStream_t st, const GemmNext* next) {
+    constexpr int dt = ElemTraits<T>::dtype, wdt = W8 ? LG_DTYPE_E4M3 : dt;
+    if (Wb == nullptr) { Wb = Wa; scb = sca; n_split = N; }
+    LG_REQUIRE(!W8 || (sca && scb && K % kBlockK == 0 && N % kBlockN == 0), "gemm_tc: fp8 weights need row scales, K %% 64 == 0 and N %% 128 == 0");
     LG_REQUIRE(p.kernel == 2, "gemm_tc: the call is planned on kernel %d", p.kernel);
     LG_REQUIRE(((uintptr_t)X & 15) == 0 && ((uintptr_t)Wa & 15) == 0 && ((uintptr_t)Wb & 15) == 0 && ldx % 8 == 0,
                "gemm_tc: operands must be 16-byte aligned");
@@ -258,26 +331,31 @@ static int gemm_tc_launch(const void* X, int ldx, const void* Wa, const void* Wb
     a.partial = partial;
 
     CUtensorMap mwa, mwb, mx;
-    LG_TRY(tma::make_map_2d(&mwa, Wa, (uint64_t)std::min(n_split, N), (uint64_t)K, (uint64_t)K, kBlockN, kBlockK, dt));
-    LG_TRY(tma::make_map_2d(&mwb, Wb, (uint64_t)std::max(N - n_split, Wb == Wa ? N : 1), (uint64_t)K, (uint64_t)K, kBlockN, kBlockK, dt));
+    LG_TRY(tma::make_map_2d(&mwa, Wa, (uint64_t)std::min(n_split, N), (uint64_t)K, (uint64_t)K, kBlockN, kBlockK, wdt));
+    LG_TRY(tma::make_map_2d(&mwb, Wb, (uint64_t)std::max(N - n_split, Wb == Wa ? N : 1), (uint64_t)K, (uint64_t)K, kBlockN, kBlockK, wdt));
     LG_TRY(tma::make_map_2d(&mx, X, (uint64_t)M, (uint64_t)K, (uint64_t)ldx, (uint32_t)rpad, kBlockK, dt));   // rows >= M read as zero
 
     a.whint = 0ull;   // the weight tiles take the default L2 policy
+    a.sca = sca; a.scb = scb;
     a.pf0 = next ? (const char*)next->p0 : nullptr; a.pfb0 = next ? next->b0 : 0;
     a.pf1 = next ? (const char*)next->p1 : nullptr; a.pfb1 = next ? next->b1 : 0;
     const dim3 grid(cdiv(N, kBlockN), ks, zblocks);
     switch (rpad) {
-        case 16: return gemm_tc_launch_t<16, T>(mwa, mwb, mx, a, grid, st);
-        case 32: return gemm_tc_launch_t<32, T>(mwa, mwb, mx, a, grid, st);
-        case 64: return gemm_tc_launch_t<64, T>(mwa, mwb, mx, a, grid, st);
-        case 128: return gemm_tc_launch_t<128, T>(mwa, mwb, mx, a, grid, st);
-        default: return gemm_tc_launch_t<256, T>(mwa, mwb, mx, a, grid, st);
+        case 16: return gemm_tc_launch_t<16, T, W8>(mwa, mwb, mx, a, grid, st);
+        case 32: return gemm_tc_launch_t<32, T, W8>(mwa, mwb, mx, a, grid, st);
+        case 64: return gemm_tc_launch_t<64, T, W8>(mwa, mwb, mx, a, grid, st);
+        case 128: return gemm_tc_launch_t<128, T, W8>(mwa, mwb, mx, a, grid, st);
+        default: return gemm_tc_launch_t<256, T, W8>(mwa, mwb, mx, a, grid, st);
     }
 }
 
-int gemm_tc_partial(const void* X, int ldx, const void* Wa, const void* Wb, int n_split, int M, int N, int K, int dtype,
+int gemm_tc_partial(const void* X, int ldx, const GemmWeight& wa, const GemmWeight& wb, int n_split, int M, int N, int K, int dtype,
                     const GemmPlan& p, float* partial, cudaStream_t st, const GemmNext* next) {
-    if (dtype == LG_DTYPE_F16) return gemm_tc_launch<f16>(X, ldx, Wa, Wb, n_split, M, N, K, p, partial, st, next);
-    LG_REQUIRE(dtype == LG_DTYPE_BF16, "gemm_tc: unsupported dtype %d", dtype);
-    return gemm_tc_launch<bf16>(X, ldx, Wa, Wb, n_split, M, N, K, p, partial, st, next);
+    LG_REQUIRE(lg_dtype_is16(dtype), "gemm_tc: unsupported dtype %d", dtype);
+    if (wa.scale) {
+        if (dtype == LG_DTYPE_F16) return gemm_tc_launch<f16, true>(X, ldx, wa.p, wb.p, n_split, M, N, K, wa.scale, wb.scale, p, partial, st, next);
+        return gemm_tc_launch<bf16, true>(X, ldx, wa.p, wb.p, n_split, M, N, K, wa.scale, wb.scale, p, partial, st, next);
+    }
+    if (dtype == LG_DTYPE_F16) return gemm_tc_launch<f16, false>(X, ldx, wa.p, wb.p, n_split, M, N, K, nullptr, nullptr, p, partial, st, next);
+    return gemm_tc_launch<bf16, false>(X, ldx, wa.p, wb.p, n_split, M, N, K, nullptr, nullptr, p, partial, st, next);
 }

@@ -14,19 +14,27 @@
 // memory in a fixed order. Weight loads do not depend on the previous kernel: the first PF chunks are requested before
 // the programmatic-dependency wait.
 //
+// fp8 weights (W8 instantiations: e4m3 codes in the stored K order of include/llamagen_b200.h, one fp32 scale per weight row): a lane's
+// 128-bit load is piece t of a 64-wide k chunk and holds, for each of the chunk's four K = 16 steps, exactly the four codes of its
+// m16n8k16 A fragment; they are widened exactly to T in registers, and the activation fragments are read from shared memory in the
+// plain fragment layout (two 32-bit loads per step). The row scale multiplies the combined fp32 sum before the first rounding.
+//
 // Rounding points are those of the batched path (xf_kernels.cu: residual_norm_kernel, silu_mul_kernel), i.e. of the
 // reference's bf16 / fp16 tensors (gpt.py:143-148,167,255-256).
 #include "kernels.cuh"
+#include <type_traits>
 
 namespace {
 
 constexpr int kWarps = 8, kThreads = 256;
 
-// 16-bit tensors of element type T (bf16 or f16)
-template <typename T>
+// 16-bit tensors of element type T (bf16 or f16); the weights are rows of WT = T, or of WT = e4m3 codes (bytes) with row scales sa / sb
+template <typename T, typename WT>
 struct GemvArgs {
-    const T* Wa;           // [N][K]
-    const T* Wb;           // paired form (SwiGLU): second matrix [N][K], else null
+    const WT* Wa;          // [N][K]
+    const WT* Wb;          // paired form (SwiGLU): second matrix [N][K], else null
+    const float* sa;       // fp8 weights: [N] row scales of Wa and Wb
+    const float* sb;
     int N, K, R;
     int pro;               // 0: x = in    1: x = rmsnorm(in) * normw
     const T* in;           // [R][K]
@@ -39,10 +47,12 @@ struct GemvArgs {
 };
 
 // ROWS weight rows per CTA: 8 (upper half of one m16 tile), 16 (one tile) or 32 (two tiles; in the paired form tile 0 comes
-// from Wa and tile 1 from the same rows of Wb). PF = chunks of 32 k kept in flight per warp.
-template <int ROWS, int PF, typename T>
-__global__ void __launch_bounds__(kThreads) gemv_small_kernel(GemvArgs<T> a) {
+// from Wa and tile 1 from the same rows of Wb). PF = 64-byte weight chunks (32 k of T, 64 k of fp8 codes) kept in flight per warp.
+template <int ROWS, int PF, typename T, bool W8>
+__global__ void __launch_bounds__(kThreads) gemv_small_kernel(GemvArgs<T, std::conditional_t<W8, uint8_t, T>> a) {
     using TR = ElemTraits<T>;
+    using WT = std::conditional_t<W8, uint8_t, T>;
+    constexpr int KC = W8 ? 64 : 32;                // k per chunk: 64 bytes of weight row, 16 per lane
     constexpr int MT = ROWS == 32 ? 2 : 1;          // m16 tiles
     constexpr int HALVES = ROWS == 8 ? 1 : 2;       // row halves (g, g+8) loaded per tile
     extern __shared__ __align__(16) uint8_t smem[];
@@ -54,17 +64,17 @@ __global__ void __launch_bounds__(kThreads) gemv_small_kernel(GemvArgs<T> a) {
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
     const int n0 = blockIdx.x * (a.Wb ? 16 : ROWS);
-    const int nchunks = K / 32;
+    const int nchunks = K / KC;
     const int my_chunks = (nchunks - warp + kWarps - 1) / kWarps;     // chunks warp, warp+8, ...
 
-    const T* wrow[MT][HALVES];
+    const WT* wrow[MT][HALVES];
 #pragma unroll
     for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
         for (int hh = 0; hh < HALVES; ++hh) {
-            const T* base = (a.Wb && mt == 1) ? a.Wb : a.Wa;
+            const WT* base = (a.Wb && mt == 1) ? a.Wb : a.Wa;
             const int row = n0 + ((a.Wb || mt == 0) ? 0 : 16) + g + 8 * hh;
-            wrow[mt][hh] = base + (size_t)row * K + t * 8;
+            wrow[mt][hh] = base + (size_t)row * K + t * (KC / 4);
         }
 
     uint4 wbuf[PF][MT][HALVES];
@@ -74,8 +84,11 @@ __global__ void __launch_bounds__(kThreads) gemv_small_kernel(GemvArgs<T> a) {
         for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
             for (int hh = 0; hh < HALVES; ++hh)
-                wbuf[slot][mt][hh] = it < my_chunks ? __ldg(reinterpret_cast<const uint4*>(wrow[mt][hh] + (size_t)c * 32))
-                                                    : make_uint4(0u, 0u, 0u, 0u);
+            {
+                // fp8: the g + 8 row is addressed from the row-g pointer (8 K bytes on), one pointer register pair less across the loop
+                const WT* wp = W8 ? wrow[mt][0] + (size_t)(8 * hh) * K : wrow[mt][hh];
+                wbuf[slot][mt][hh] = it < my_chunks ? __ldg(reinterpret_cast<const uint4*>(wp + (size_t)c * KC)) : make_uint4(0u, 0u, 0u, 0u);
+            }
     };
     lg_pdl_launch_dependents();
 #pragma unroll
@@ -157,20 +170,41 @@ __global__ void __launch_bounds__(kThreads) gemv_small_kernel(GemvArgs<T> a) {
     for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
         for (int q = 0; q < 4; ++q) acc[mt][q] = 0.f;
-    const uint8_t* xrow = xs + (size_t)min(g, R - 1) * xstride + t * 16;   // lanes of padding rows re-read a real row (columns are independent)
+    // lanes of padding rows re-read a real row (columns are independent)
+    const uint8_t* xrow = xs + (size_t)min(g, R - 1) * xstride + t * (W8 ? 4 : 16);
     for (int it0 = 0; it0 < my_chunks; it0 += PF) {
 #pragma unroll
         for (int s = 0; s < PF; ++s) {
             const int it = it0 + s;
             if (it < my_chunks) {
                 const int c = warp + it * kWarps;
-                const uint4 xb = *reinterpret_cast<const uint4*>(xrow + (size_t)c * 64);
+                if constexpr (W8) {
+                    uint4 c0[MT], c1[MT];
 #pragma unroll
-                for (int mt = 0; mt < MT; ++mt) {
-                    const uint4 w0 = wbuf[s][mt][0];
-                    const uint4 w1 = HALVES == 2 ? wbuf[s][mt][HALVES - 1] : make_uint4(0u, 0u, 0u, 0u);
-                    mma_m16n8k16<T>(acc[mt], w0.x, w1.x, w0.y, w1.y, xb.x, xb.y);
-                    mma_m16n8k16<T>(acc[mt], w0.z, w1.z, w0.w, w1.w, xb.z, xb.w);
+                    for (int mt = 0; mt < MT; ++mt) {
+                        c0[mt] = wbuf[s][mt][0];
+                        c1[mt] = HALVES == 2 ? wbuf[s][mt][HALVES - 1] : make_uint4(0u, 0u, 0u, 0u);
+                    }
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {   // step j: activations k = 16 j + 2 t, + 1 and 16 j + 8 + 2 t, + 1 of the chunk
+                        const uint32_t b0 = *reinterpret_cast<const uint32_t*>(xrow + (size_t)c * 128 + j * 32);
+                        const uint32_t b1 = *reinterpret_cast<const uint32_t*>(xrow + (size_t)c * 128 + j * 32 + 16);
+#pragma unroll
+                        for (int mt = 0; mt < MT; ++mt) {
+                            const uint32_t w0 = j == 0 ? c0[mt].x : j == 1 ? c0[mt].y : j == 2 ? c0[mt].z : c0[mt].w;
+                            const uint32_t w1 = j == 0 ? c1[mt].x : j == 1 ? c1[mt].y : j == 2 ? c1[mt].z : c1[mt].w;
+                            mma_m16n8k16<T>(acc[mt], e4m3x2_to<T>(w0), e4m3x2_to<T>(w1), e4m3x2_to<T>(w0 >> 16), e4m3x2_to<T>(w1 >> 16), b0, b1);
+                        }
+                    }
+                } else {
+                    const uint4 xb = *reinterpret_cast<const uint4*>(xrow + (size_t)c * 64);
+#pragma unroll
+                    for (int mt = 0; mt < MT; ++mt) {
+                        const uint4 w0 = wbuf[s][mt][0];
+                        const uint4 w1 = HALVES == 2 ? wbuf[s][mt][HALVES - 1] : make_uint4(0u, 0u, 0u, 0u);
+                        mma_m16n8k16<T>(acc[mt], w0.x, w1.x, w0.y, w1.y, xb.x, xb.y);
+                        mma_m16n8k16<T>(acc[mt], w0.z, w1.z, w0.w, w1.w, xb.z, xb.w);
+                    }
                 }
             }
             load_chunk(s, it + PF);
@@ -195,6 +229,7 @@ __global__ void __launch_bounds__(kThreads) gemv_small_kernel(GemvArgs<T> a) {
             av += red[((w * MT + 0) * 16 + i) * 8 + r];
             bv += red[((w * MT + (MT - 1)) * 16 + i) * 8 + r];
         }
+        if constexpr (W8) { av *= __ldg(a.sa + n0 + i); bv *= __ldg(a.sb + n0 + i); }
         av = TR::round(av);
         bv = TR::round(bv);
         const float sv = TR::round(av / (1.0f + expf(-av)));  // F.silu(w1 x) * w3 x in T tensors (gpt.py:167)
@@ -206,6 +241,7 @@ __global__ void __launch_bounds__(kThreads) gemv_small_kernel(GemvArgs<T> a) {
     float v = 0.f;
 #pragma unroll
     for (int w = 0; w < kWarps; ++w) v += red[((w * MT + mt) * 16 + ii) * 8 + r];
+    if constexpr (W8) v *= __ldg(a.sa + n0 + i);
     const size_t o = (size_t)r * a.N + n0 + i;
     if (a.epi == 0) {
         a.out_f32[o] = v;
@@ -214,35 +250,37 @@ __global__ void __launch_bounds__(kThreads) gemv_small_kernel(GemvArgs<T> a) {
     }
 }
 
-template <int ROWS, int PF, typename T>
-int launch_t(const GemvArgs<T>& a, cudaStream_t st) {
+template <int ROWS, int PF, typename T, bool W8, typename WT>
+int launch_t(const GemvArgs<T, WT>& a, cudaStream_t st) {
     constexpr int MT = ROWS == 32 ? 2 : 1;
     const size_t smem = (size_t)(kWarps * MT * 16 * 8 + 64) * sizeof(float) + (size_t)a.R * (a.K * 2 + 16);
     static DevOnce attr;
     if (lg_first_on_device(attr)) {
-        LG_CUDA_OK(cudaFuncSetAttribute(gemv_small_kernel<ROWS, PF, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+        LG_CUDA_OK(cudaFuncSetAttribute(gemv_small_kernel<ROWS, PF, T, W8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     }
     LG_REQUIRE(smem <= 100 * 1024, "gemv_small: %zu bytes of shared memory (R=%d K=%d)", smem, a.R, a.K);
     const int rows_per_cta = a.Wb ? 16 : ROWS;
-    (void)lg_launch(gemv_small_kernel<ROWS, PF, T>, dim3(a.N / rows_per_cta), dim3(kThreads), smem, st, a);
+    (void)lg_launch(gemv_small_kernel<ROWS, PF, T, W8>, dim3(a.N / rows_per_cta), dim3(kThreads), smem, st, a);
     LG_LAUNCH_CHECK();
     return 0;
 }
 
-template <typename T>
+template <typename T, bool W8>
 int launch_typed(const GemvSmall& g, const GemvSmallPlan& p, cudaStream_t st) {
-    GemvArgs<T> a;
-    a.Wa = (const T*)g.Wa; a.Wb = (const T*)g.Wb; a.N = g.N; a.K = g.K; a.R = g.R;
+    using WT = std::conditional_t<W8, uint8_t, T>;
+    GemvArgs<T, WT> a;
+    a.Wa = (const WT*)g.Wa.p; a.Wb = (const WT*)g.Wb.p; a.sa = g.Wa.scale; a.sb = g.Wb.scale;
+    a.N = g.N; a.K = g.K; a.R = g.R;
     a.pro = g.normw ? 1 : 0; a.in = (const T*)g.in; a.normw = (const T*)g.normw; a.eps = g.eps;
-    a.epi = g.Wb ? 2 : (g.out_f32 ? 0 : 1); a.out_f32 = g.out_f32; a.h = (T*)g.h; a.ff = (T*)g.ff;
-    if (p.rows == 8) return launch_t<8, 12>(a, st);
-    if (p.rows == 16) return launch_t<16, 4>(a, st);
-    return launch_t<32, 4>(a, st);
+    a.epi = g.Wb.p ? 2 : (g.out_f32 ? 0 : 1); a.out_f32 = g.out_f32; a.h = (T*)g.h; a.ff = (T*)g.ff;
+    if (p.rows == 8) return launch_t<8, 12, T, W8>(a, st);
+    if (p.rows == 16) return launch_t<16, 4, T, W8>(a, st);
+    return launch_t<32, 4, T, W8>(a, st);
 }
 
 }  // namespace
 
-GemvSmallPlan gemv_small_plan(int R, int N, int K, int dtype, bool paired) {
+GemvSmallPlan gemv_small_plan(int R, int N, int K, int dtype, bool paired, bool w8) {
     GemvSmallPlan p;
     if (!lg_dtype_is16(dtype)) {
         snprintf(p.error, sizeof(p.error), "gemv_small: dtype %d is not bf16 / fp16", dtype);
@@ -250,6 +288,8 @@ GemvSmallPlan gemv_small_plan(int R, int N, int K, int dtype, bool paired) {
         snprintf(p.error, sizeof(p.error), "gemv_small: R=%d rows outside 1..8", R);
     } else if (K % 32 != 0 || K < 256) {
         snprintf(p.error, sizeof(p.error), "gemv_small: K=%d must be a multiple of 32 and at least 256", K);
+    } else if (w8 && K % 64 != 0) {
+        snprintf(p.error, sizeof(p.error), "gemv_small: fp8 weights need K=%d a multiple of 64", K);
     } else if ((size_t)R * (K * 2 + 16) > 90 * 1024) {
         snprintf(p.error, sizeof(p.error), "gemv_small: R=%d rows of K=%d exceed 90 KiB of shared memory", R, K);
     } else if (N <= 0 || N % (paired ? 16 : 32) != 0) {      // every row granularity used below divides N
@@ -266,7 +306,10 @@ GemvSmallPlan gemv_small_plan(int R, int N, int K, int dtype, bool paired) {
 }
 
 int launch_gemv_small(const GemvSmall& g, cudaStream_t st) {
-    const GemvSmallPlan p = gemv_small_plan(g.R, g.N, g.K, g.dtype, g.Wb != nullptr);
+    const bool w8 = g.Wa.scale != nullptr;
+    LG_REQUIRE(!g.Wb.p || w8 == (g.Wb.scale != nullptr), "gemv_small: both weights of a pair must be fp8 or both 16-bit");
+    const GemvSmallPlan p = gemv_small_plan(g.R, g.N, g.K, g.dtype, g.Wb.p != nullptr, w8);
     if (p.rows == 0) return lg_fail("%s", p.error);
-    return g.dtype == LG_DTYPE_F16 ? launch_typed<f16>(g, p, st) : launch_typed<bf16>(g, p, st);
+    if (w8) return g.dtype == LG_DTYPE_F16 ? launch_typed<f16, true>(g, p, st) : launch_typed<bf16, true>(g, p, st);
+    return g.dtype == LG_DTYPE_F16 ? launch_typed<f16, false>(g, p, st) : launch_typed<bf16, false>(g, p, st);
 }

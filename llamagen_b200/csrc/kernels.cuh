@@ -86,8 +86,20 @@ int launch_sjd_refresh(const SjdArgs& a, int first, cudaStream_t st);
 //   1 gemm_mma_kernel: every other 16-bit call. tile: 32, 64 or 128 rows (bm).
 // ksplit: fp32 slabs [ksplit][M][N] written (<= 16). kernel -1: the call is not valid, `error` says why. The only reader of
 // LG_GEMM_TC.
+// w8: the weight is fp8 (GemmWeight::scale set). Kernel 2 is the only batched kernel that reads e4m3 codes, so such a call needs a
+// bf16 / fp16 model, N % 128 == 0, a segment boundary on a 128-row tile, K % 64 == 0 and LG_GEMM_TC other than 0; anything else is
+// kernel -1 (there is no 16-bit copy to fall back to). Where both are valid, the fp8 plan equals the 16-bit plan of the shape.
 struct GemmPlan { int kernel = -1; int tile = 0; int ksplit = 0; int row_blocks = 0; char error[96] = {}; };
-GemmPlan gemm_plan(int M, int N, int K, int n_split, int dtype);
+GemmPlan gemm_plan(int M, int N, int K, int n_split, int dtype, bool w8 = false);
+// One GEMM weight [N][K] as the engine holds it: rows in the model dtype (scale null), or fp8 e4m3 codes in the stored K order of
+// include/llamagen_b200.h (LG_DTYPE_E4M3) with one fp32 power-of-two scale per row
+struct GemmWeight {
+    const void* p = nullptr;
+    const float* scale = nullptr;
+    GemmWeight() = default;
+    GemmWeight(const void* w, const float* s = nullptr) : p(w), scale(s) {}
+    size_t bytes(size_t N, size_t K, size_t esz) const { return N * K * (scale ? 1 : esz); }
+};
 // Weights the NEXT GEMM of the decode chain will stream: the current GEMM's CTAs ask the L2 to fetch them
 // (cp.async.bulk.prefetch.L2) so the next kernel's TMA loads hit L2 instead of paying the HBM latency.
 struct GemmNext {
@@ -95,9 +107,9 @@ struct GemmNext {
     const void* p1 = nullptr; size_t b1 = 0;
 };
 // floats of fp32 slabs the call's plan writes (0 for an invalid call); partial must hold that many
-size_t gemm_partial_floats(int M, int N, int K, int n_split, int dtype);
-// runs the call on the kernel gemm_plan picks; *plan (optional) receives that plan
-int gemm_partial(const void* X, int ldx, const void* Wa, const void* Wb, int n_split, int M, int N, int K,
+size_t gemm_partial_floats(int M, int N, int K, int n_split, int dtype, bool w8 = false);
+// runs the call on the kernel gemm_plan picks; *plan (optional) receives that plan. wb.p null: wa alone
+int gemm_partial(const void* X, int ldx, const GemmWeight& wa, const GemmWeight& wb, int n_split, int M, int N, int K,
                  int dtype, float* partial, GemmPlan* plan, cudaStream_t st, const GemmNext* next = nullptr);
 
 // ------------------------------------------------------------------------------------------------
@@ -245,15 +257,15 @@ ConvPlan conv_plan(const ConvCall& c);
 int launch_conv_tc(const ConvCall& c, const ConvPlan& p, cudaStream_t st);   // p.kernel 1 or 2
 void conv_tc_set_cta_budget(int ctas);   // > 0: persistent conv CTAs (at most `ctas`), 0: one CTA per tile (default)
 int conv_tc_make_phase_weights(const float* w_f32, bf16* out, int cout, int cin, cudaStream_t st);
-// gemm_tc.cu — wgmma/TMA weight-streaming GEMM (bf16 or fp16, row blocks of <= 256)
+// gemm_tc.cu — wgmma/TMA weight-streaming GEMM (bf16 or fp16 activations, 16-bit or fp8 weights, row blocks of <= 256)
 int gemm_tc_ksplit(int M, int N, int K);
-int gemm_tc_partial(const void* X, int ldx, const void* Wa, const void* Wb, int n_split, int M, int N, int K, int dtype,
+int gemm_tc_partial(const void* X, int ldx, const GemmWeight& wa, const GemmWeight& wb, int n_split, int M, int N, int K, int dtype,
                     const GemmPlan& p, float* partial, cudaStream_t st, const GemmNext* next = nullptr);   // p.kernel 2
 
 // gemv_small.cu — decode GEMMs for R <= 8 rows: CTA-owned output columns (no split-K), RMSNorm in the prologue (normw != null),
 // epilogue by destination: out_f32 [R][N] | h (in-place residual add) | ff (SwiGLU gate of the Wa/Wb row pair)
 struct GemvSmall {
-    const void* Wa; const void* Wb;   // [N][K]; Wb only for the paired (w1 | w3) form
+    GemmWeight Wa, Wb;                // [N][K]; Wb only for the paired (w1 | w3) form; both fp8 or both 16-bit
     int N, K, R;
     const void* in;                   // [R][K]
     const void* normw; float eps;     // RMSNorm weight [K] or null
@@ -262,11 +274,21 @@ struct GemvSmall {
 };
 // The instantiation a call runs on: rows = weight rows per CTA (8, 16 or 32; the paired form is 32: 16 rows of Wa and of Wb), pf =
 // 32-wide k chunks in flight per warp. rows 0: the call is not supported (bf16 / fp16, 1 <= R <= 8, K % 32 == 0, K >= 256,
-// R * (2K + 16) bytes <= 90 KiB, N > 0 a multiple of 32, or of 16 when paired), `error` says why.
+// R * (2K + 16) bytes <= 90 KiB, N > 0 a multiple of 32, or of 16 when paired), `error` says why. w8 (fp8 weights): a lane's 16-byte
+// weight load spans a 64-wide k chunk, so K % 64 == 0 as well; rows as for 16-bit weights, pf counts 64-wide chunks.
 struct GemvSmallPlan { int rows = 0; int pf = 0; char error[96] = {}; };
-GemvSmallPlan gemv_small_plan(int R, int N, int K, int dtype, bool paired);
-inline bool gemv_small_supported(int R, int N, int K, int dtype, bool paired) { return gemv_small_plan(R, N, K, dtype, paired).rows != 0; }
+GemvSmallPlan gemv_small_plan(int R, int N, int K, int dtype, bool paired, bool w8 = false);
+inline bool gemv_small_supported(int R, int N, int K, int dtype, bool paired, bool w8 = false) {
+    return gemv_small_plan(R, N, K, dtype, paired, w8).rows != 0;
+}
 int launch_gemv_small(const GemvSmall& g, cudaStream_t st);
+
+// weight_fp8.cu — fp8 (e4m3) GEMM weights: W [N][K] in bf16 / fp16 -> codes [N][K] in the stored K order + power-of-two row scales [N]
+int launch_quantize_rows_e4m3(const void* w, int N, int K, int dtype, uint8_t* codes, float* scales, cudaStream_t st);
+int w8_stored_index(int k);                                     // byte of a row that holds column k's code
+void w8_scale_exponents(int dtype, int* emin, int* emax);      // allowed scale exponents of a bf16 / fp16 model
+// copies N device scales to the host (synchronises) and fails unless each is 2^e with e in that range
+int w8_check_scales(const char* name, const float* dev_scales, int N, int dtype);
 
 // *pos += 1; *step += 1  (device-side loop counters for graph replay)
 int launch_advance(int* pos, int* step, cudaStream_t st);

@@ -1,6 +1,7 @@
 // wgmma (Hopper warpgroup MMA) helpers shared by the tensor-core kernels (gemm_tc.cu, conv_tc.cu).
 //
-// Both operands are K-major bf16 (or fp16) tiles in shared memory written by TMA with the 128-byte swizzle: rows of 64 elements
+// Both operands are K-major bf16 (or fp16) tiles in shared memory written by TMA with the 128-byte swizzle (the fp8-weight GEMM passes
+// A in registers instead, WgmmaRS below): rows of 64 elements
 // (128 B), 8-row groups 1024 B apart, tile bases 1024-aligned. One warpgroup (128 threads) computes a 64 x N fp32
 // accumulator held in registers; thread t of the warpgroup owns, for register i of Wgmma<N>,
 //   row = 16 * (warp % 4) + lane / 4 + 8 * ((i >> 1) & 1),   col = 8 * (i >> 2) + 2 * (lane % 4) + (i & 1).
@@ -108,6 +109,88 @@ struct Wgmma<256, T> {
     }
 };
 
+// The same MMA with A from registers ("RS" form): each thread passes its four packed-pair registers of the 64 x 16 A fragment,
+//   a0 = (row, k 2q..2q+1), a1 = (row + 8, same k), a2 = (row, k 8+2q..), a3 = (row + 8, k 8+2q..), row = 16 * (warp % 4) + lane / 4, q = lane % 4
+// (the mma.sync m16n8k16 A layout), B still comes through its shared-memory descriptor. The registers are read asynchronously:
+// they must not be overwritten before wgmma.wait_group has retired the instruction, and ptxas serialises the wgmma of a group when
+// another instruction writes them while a group is open (gemm_tc.cu writes them only after wait_group 0).
+template <int N, typename T = bf16>
+struct WgmmaRS;
+#define LG_WGRS_ASM16(TY) \
+    "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t" \
+    "wgmma.mma_async.sync.aligned.m64n16k16.f32." TY "." TY " {" \
+    "%0,%1,%2,%3,%4,%5,%6,%7" \
+    "}, {%8,%9,%10,%11}, %12, p, 1, 1, 0;\n\t}"
+template <typename T>
+struct WgmmaRS<16, T> {
+    static __device__ __forceinline__ void mma(float* d, const uint32_t* a, uint64_t bdesc) {
+        if constexpr (std::is_same<T, f16>::value)
+            asm volatile(LG_WGRS_ASM16("f16") : LG_WG_R8(0) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1));
+        else
+            asm volatile(LG_WGRS_ASM16("bf16") : LG_WG_R8(0) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1));
+    }
+};
+
+#define LG_WGRS_ASM32(TY) \
+    "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t" \
+    "wgmma.mma_async.sync.aligned.m64n32k16.f32." TY "." TY " {" \
+    "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15" \
+    "}, {%16,%17,%18,%19}, %20, p, 1, 1, 0;\n\t}"
+template <typename T>
+struct WgmmaRS<32, T> {
+    static __device__ __forceinline__ void mma(float* d, const uint32_t* a, uint64_t bdesc) {
+        if constexpr (std::is_same<T, f16>::value)
+            asm volatile(LG_WGRS_ASM32("f16") : LG_WG_R8(0), LG_WG_R8(8) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1));
+        else
+            asm volatile(LG_WGRS_ASM32("bf16") : LG_WG_R8(0), LG_WG_R8(8) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1));
+    }
+};
+
+#define LG_WGRS_ASM64(TY) \
+    "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t" \
+    "wgmma.mma_async.sync.aligned.m64n64k16.f32." TY "." TY " {" \
+    "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31" \
+    "}, {%32,%33,%34,%35}, %36, p, 1, 1, 0;\n\t}"
+template <typename T>
+struct WgmmaRS<64, T> {
+    static __device__ __forceinline__ void mma(float* d, const uint32_t* a, uint64_t bdesc) {
+        if constexpr (std::is_same<T, f16>::value)
+            asm volatile(LG_WGRS_ASM64("f16") : LG_WG_R8(0), LG_WG_R8(8), LG_WG_R8(16), LG_WG_R8(24) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1));
+        else
+            asm volatile(LG_WGRS_ASM64("bf16") : LG_WG_R8(0), LG_WG_R8(8), LG_WG_R8(16), LG_WG_R8(24) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1));
+    }
+};
+
+#define LG_WGRS_ASM128(TY) \
+    "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t" \
+    "wgmma.mma_async.sync.aligned.m64n128k16.f32." TY "." TY " {" \
+    "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63" \
+    "}, {%64,%65,%66,%67}, %68, p, 1, 1, 0;\n\t}"
+template <typename T>
+struct WgmmaRS<128, T> {
+    static __device__ __forceinline__ void mma(float* d, const uint32_t* a, uint64_t bdesc) {
+        if constexpr (std::is_same<T, f16>::value)
+            asm volatile(LG_WGRS_ASM128("f16") : LG_WG_R8(0), LG_WG_R8(8), LG_WG_R8(16), LG_WG_R8(24), LG_WG_R8(32), LG_WG_R8(40), LG_WG_R8(48), LG_WG_R8(56) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1));
+        else
+            asm volatile(LG_WGRS_ASM128("bf16") : LG_WG_R8(0), LG_WG_R8(8), LG_WG_R8(16), LG_WG_R8(24), LG_WG_R8(32), LG_WG_R8(40), LG_WG_R8(48), LG_WG_R8(56) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1));
+    }
+};
+
+#define LG_WGRS_ASM256(TY) \
+    "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %133, 0;\n\t" \
+    "wgmma.mma_async.sync.aligned.m64n256k16.f32." TY "." TY " {" \
+    "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127" \
+    "}, {%128,%129,%130,%131}, %132, p, 1, 1, 0;\n\t}"
+template <typename T>
+struct WgmmaRS<256, T> {
+    static __device__ __forceinline__ void mma(float* d, const uint32_t* a, uint64_t bdesc) {
+        if constexpr (std::is_same<T, f16>::value)
+            asm volatile(LG_WGRS_ASM256("f16") : LG_WG_R8(0), LG_WG_R8(8), LG_WG_R8(16), LG_WG_R8(24), LG_WG_R8(32), LG_WG_R8(40), LG_WG_R8(48), LG_WG_R8(56), LG_WG_R8(64), LG_WG_R8(72), LG_WG_R8(80), LG_WG_R8(88), LG_WG_R8(96), LG_WG_R8(104), LG_WG_R8(112), LG_WG_R8(120) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1));
+        else
+            asm volatile(LG_WGRS_ASM256("bf16") : LG_WG_R8(0), LG_WG_R8(8), LG_WG_R8(16), LG_WG_R8(24), LG_WG_R8(32), LG_WG_R8(40), LG_WG_R8(48), LG_WG_R8(56), LG_WG_R8(64), LG_WG_R8(72), LG_WG_R8(80), LG_WG_R8(88), LG_WG_R8(96), LG_WG_R8(104), LG_WG_R8(112), LG_WG_R8(120) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1));
+    }
+};
+
 // one 64-wide k-block: A = 64 rows at a_addr, B = N rows at b_addr; four K = 16 steps advance 32 bytes inside the
 // swizzle span (+2 in the address field). Issue only: the caller commits and waits.
 template <int N, typename T = bf16>
@@ -116,7 +199,6 @@ __device__ __forceinline__ void mma_kblock(float* d, uint32_t a_addr, uint32_t b
 #pragma unroll
     for (int k = 0; k < 4; ++k) Wgmma<N, T>::mma(d, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k));
 }
-
 __device__ __forceinline__ int frag_row(int i) { return 16 * (((int)threadIdx.x >> 5) & 3) + (((int)threadIdx.x & 31) >> 2) + 8 * ((i >> 1) & 1); }
 __device__ __forceinline__ int frag_col(int i) { return 8 * (i >> 2) + 2 * ((int)threadIdx.x & 3) + (i & 1); }
 

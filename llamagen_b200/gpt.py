@@ -77,6 +77,10 @@ def rope_table_2d(grid_size: int, head_dim: int, base: float, cls_token_num: int
     return torch.cat([torch.zeros(cls_token_num, head_dim // 2, 2), table]).contiguous()
 
 
+# the per-layer GEMM weights `set_weight_dtype("fp8")` stores as e4m3 codes ("output.weight" joins them with head=True)
+FP8_LAYER_WEIGHTS = ("attention.wqkv.weight", "attention.wo.weight", "feed_forward.w1.weight", "feed_forward.w3.weight",
+                     "feed_forward.w2.weight")
+
 SCORE_SCRATCH_CAP = 4 << 30   # bytes of lg_score scratch a model keeps; a batch that needs more is scored in image chunks
 
 
@@ -193,6 +197,8 @@ class Transformer(nn.Module):
         self._workspace = None
         self._ws_shape = (0, 0)
         self._kv_cache = ("auto", None)
+        self._weight_dtype = ("auto", True)
+        self._w8 = {}
         self._score_ws = None
         self._sjd_ws = None
         self.requires_grad_(False)
@@ -213,9 +219,50 @@ class Transformer(nn.Module):
             scales = tuple(float(x) for x in s.reshape(-1))
         self._kv_cache = (dtype, scales)
 
+    def set_weight_dtype(self, dtype: str = "auto", head: bool = True):
+        """Storage of the transformer's GEMM weights inside the engine of a bf16 / fp16 model: "auto" (the parameters themselves)
+        or "fp8": every layer's wqkv, wo, w1, w3, w2 and, with head=True, the output head are quantised by the engine
+        (lg_quantize_rows_e4m3: e4m3 codes with one power-of-two scale per output row) and the engine streams those codes, half
+        the weight bytes. Activations, KV cache, norms and embeddings are untouched. The module's parameters and state_dict() stay
+        the 16-bit tensors; the codes are re-made at the next engine() after a parameter moved (`.to()`) or was written in place
+        through the parameter itself (load_state_dict, `weight.copy_()`: its version counter changes). A write through `weight.data`
+        changes neither and would leave the old codes bound: call requantize() after one. Takes effect at the next engine() /
+        setup_caches() / generate()."""
+        if dtype not in ("auto", "fp8"):
+            raise ValueError(f"weight dtype must be 'auto' or 'fp8', got {dtype!r}")
+        if not isinstance(head, bool):
+            raise ValueError(f"head must be a bool, got {head!r}")
+        self._weight_dtype = (dtype, head if dtype == "fp8" else True)
+
+    def requantize(self):
+        """Drop the engine so that the next use re-makes it, and with it the fp8 codes, from the parameters as they are now. Only
+        needed after a write through `weight.data`, which no tensor attribute records."""
+        self._drop_engine()
+
+    def fp8_weight_names(self):
+        """state_dict names of the weights the current set_weight_dtype() setting stores in fp8 (empty for "auto")."""
+        dtype, head = self._weight_dtype
+        if dtype != "fp8":
+            return []
+        names = [f"layers.{i}.{w}" for i in range(self.n_layer) for w in FP8_LAYER_WEIGHTS]
+        return names + ["output.weight"] if head else names
+
+    def weight_codes(self, name: str, stored: bool = False) -> torch.Tensor:
+        """uint8 e4m3 codes [N, K] the engine bound for fp8 weight `name`, column k at index k (stored=True: in the engine's stored
+        K order, include/llamagen_b200.h)."""
+        codes = self._w8[name][0]
+        return codes if stored else codes[:, _lib.weight_fp8_stored_index(codes.shape[1]).to(codes.device)]
+
+    def weight_scales(self, name: str) -> torch.Tensor:
+        """fp32 row scales [N] the engine bound for fp8 weight `name`."""
+        return self._w8[name][1]
+
     def _signature(self):
         p = self.tok_embeddings.weight
-        return (p.device, p.dtype, tuple(t.data_ptr() for t in self.state_dict().values()), self._kv_cache)
+        sd = self.state_dict()
+        # the engine holds its own codes of an fp8 weight: an in-place write to the parameter (load_state_dict, copy_) must re-make them
+        versions = tuple(sd[n]._version for n in self.fp8_weight_names())
+        return (p.device, p.dtype, tuple(t.data_ptr() for t in sd.values()), self._kv_cache, self._weight_dtype, versions)
 
     def engine(self):
         """Create / refresh the C engine for the parameters' current device + dtype."""
@@ -235,17 +282,39 @@ class Transformer(nn.Module):
         dev_index = p.device.index if p.device.index is not None else torch.cuda.current_device()
         _lib.check(lib.lg_engine_create(ctypes.byref(cfg), dev_index, ctypes.byref(handle)), "lg_engine_create")
         self._keepalive = []
-        for name, t in self.state_dict().items():
-            if not t.is_contiguous():
-                raise _lib.LgError(f"parameter {name} must be contiguous")
-            t_dt = _lib.dtype_code(t.dtype)
-            _lib.check(lib.lg_engine_bind_weight(handle, name.encode(), _lib.ptr(t), _lib.shape_array(t.shape),
-                                                 t.dim(), t_dt), f"bind {name}")
-        self.freqs_cis = self.freqs_cis.to(device=p.device, dtype=torch.float32).contiguous()
-        _lib.check(lib.lg_engine_bind_weight(handle, b"freqs_cis", _lib.ptr(self.freqs_cis),
-                                             _lib.shape_array(self.freqs_cis.shape), 3, _lib.LG_DTYPE_F32),
-                   "bind freqs_cis")
-        _lib.check(lib.lg_engine_finalize(handle), "lg_engine_finalize")
+        fp8 = set(self.fp8_weight_names())
+        self._w8 = {}
+        try:
+            if fp8 and dt == _lib.LG_DTYPE_F32:
+                raise _lib.LgError("fp8 weights need a bf16 or fp16 model (fp32 models keep fp32 weights)")
+            stream = _lib.current_stream(p.device)
+            for name, t in self.state_dict().items():
+                if not t.is_contiguous():
+                    raise _lib.LgError(f"parameter {name} must be contiguous")
+                t_dt = _lib.dtype_code(t.dtype)
+                if name in fp8:
+                    # the engine's quantiser defines the stored bytes; codes and scales live as long as the engine
+                    codes = torch.empty(t.shape, dtype=torch.uint8, device=t.device)
+                    scales = torch.empty(t.shape[0], dtype=torch.float32, device=t.device)
+                    _lib.check(lib.lg_quantize_rows_e4m3(_lib.ptr(t), t.shape[0], t.shape[1], t_dt, _lib.ptr(codes), _lib.ptr(scales),
+                                                         stream), f"quantize {name}")
+                    self._w8[name] = (codes, scales)
+                    _lib.check(lib.lg_engine_bind_weight(handle, (name + "_scale").encode(), _lib.ptr(scales),
+                                                         _lib.shape_array(scales.shape), 1, _lib.LG_DTYPE_F32), f"bind {name}_scale")
+                    t, t_dt = codes, _lib.LG_DTYPE_E4M3
+                _lib.check(lib.lg_engine_bind_weight(handle, name.encode(), _lib.ptr(t), _lib.shape_array(t.shape),
+                                                     t.dim(), t_dt), f"bind {name}")
+            self.freqs_cis = self.freqs_cis.to(device=p.device, dtype=torch.float32).contiguous()
+            _lib.check(lib.lg_engine_bind_weight(handle, b"freqs_cis", _lib.ptr(self.freqs_cis),
+                                                 _lib.shape_array(self.freqs_cis.shape), 3, _lib.LG_DTYPE_F32),
+                       "bind freqs_cis")
+            if fp8:
+                torch.cuda.current_stream(p.device).synchronize()   # lg_engine_finalize reads the scales back
+            _lib.check(lib.lg_engine_finalize(handle), "lg_engine_finalize")
+        except Exception:
+            lib.lg_engine_destroy(handle)
+            self._w8 = {}
+            raise
         kv_dtype, kv_scales = self._kv_cache
         if kv_dtype == "fp8":
             arr = (ctypes.c_float * len(kv_scales))(*kv_scales) if kv_scales is not None else None

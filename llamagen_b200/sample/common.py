@@ -34,6 +34,9 @@ def load_gpt(args, device, latent_size):
     kv_cache_dtype = getattr(args, "kv_cache_dtype", "auto")
     if kv_cache_dtype == "fp8" and precision == torch.float32:
         raise SystemExit("--kv-cache-dtype fp8 needs --precision bf16 or fp16 (fp32 models keep an fp32 KV cache)")
+    weight_dtype = getattr(args, "weight_dtype", "auto")
+    if weight_dtype == "fp8" and precision == torch.float32:
+        raise SystemExit("--weight-dtype fp8 needs --precision bf16 or fp16 (fp32 models keep fp32 weights)")
     gpt_model = GPT_models[args.gpt_model](
         vocab_size=args.codebook_size, block_size=latent_size ** 2, num_classes=args.num_classes,
         cls_token_num=args.cls_token_num, model_type=args.gpt_type).to(device=device, dtype=precision)
@@ -46,6 +49,7 @@ def load_gpt(args, device, latent_size):
         gpt_model.output.weight.data.normal_(std=0.02)
     gpt_model.eval()
     gpt_model.set_kv_cache(kv_cache_dtype)
+    gpt_model.set_weight_dtype(weight_dtype)
     print("gpt model is loaded")
     if args.compile:
         print("--compile is accepted for CLI compatibility; the engine already replays one CUDA graph per decode step")
@@ -73,6 +77,9 @@ def add_common_args(parser, t2i: bool):
     parser.add_argument("--precision", type=str, default="bf16", choices=["none", "fp16", "bf16"])
     parser.add_argument("--kv-cache-dtype", type=str, default="auto", choices=["auto", "fp8"],
                         help="KV-cache storage: the model dtype (auto) or fp8 e4m3 (half the cache bytes; bf16 / fp16 models)")
+    parser.add_argument("--weight-dtype", type=str, default="auto", choices=["auto", "fp8"],
+                        help="storage of the transformer's GEMM weights: the model dtype (auto) or fp8 e4m3 codes with per-row "
+                             "power-of-two scales (half the weight bytes; bf16 / fp16 models)")
     parser.add_argument("--compile", action="store_true", default=False)
     parser.add_argument("--vq-model", type=str, choices=list(VQ_models.keys()), default="VQ-16")
     parser.add_argument("--vq-ckpt", type=str, default=None, help="ckpt path for vq model")

@@ -65,13 +65,17 @@ class _Request:
 
 class LLM:
     def __init__(self, gpt_model, cfg_scale: float = 1.0, num_classes: int = 1000, max_num_seqs: int = 64, seed: Optional[int] = None,
-                 kv_cache_dtype: Optional[str] = None):
+                 kv_cache_dtype: Optional[str] = None, weight_dtype: Optional[str] = None):
         """kv_cache_dtype: None keeps the model's KV-cache setting (Transformer.set_kv_cache, scales included); "auto" (the model
-        dtype) or "fp8" (e4m3) sets it. Passing the dtype the model already has keeps its scales."""
+        dtype) or "fp8" (e4m3) sets it. Passing the dtype the model already has keeps its scales.
+        weight_dtype: None keeps the model's GEMM-weight storage (Transformer.set_weight_dtype, its head choice included); "auto" or
+        "fp8" sets it."""
         if gpt_model.model_type != "c2i":
             raise ValueError("serve.LLM handles class-conditional models (the reference's serve path is c2i only)")
         if kv_cache_dtype is not None and kv_cache_dtype != getattr(gpt_model, "_kv_cache", ("auto", None))[0]:
             gpt_model.set_kv_cache(kv_cache_dtype)
+        if weight_dtype is not None and weight_dtype != getattr(gpt_model, "_weight_dtype", ("auto", True))[0]:
+            gpt_model.set_weight_dtype(weight_dtype)
         self.model = gpt_model
         self.cfg_scale = float(cfg_scale)
         self.num_classes = int(num_classes)
