@@ -321,6 +321,31 @@ int  lg_test_attention_plan(int dtype, int kv_dtype, int R, int Tq, int H, int h
 int  lg_test_sjd_verify(int B, int S, int L, int V, int greedy, uint64_t seed, const float* p, const float* q, const int32_t* qflag,
                         const int32_t* x, const int32_t* win, int32_t* nfin, int32_t* start, int32_t* out, void* stream);
 
+/* One launch of the sample kernel with every input the engine can give it (dev buffers). logits, B, V, mix_cfg, round_dtype, sc as
+ * lg_sample; the step is step, or *step_dev when step_dev is given, or step_rows[b] with seed_rows[b] as the seed (lg_sample_rows);
+ * row_offset is added to the image index of the RNG stream and of the dbg_logits row. Optional outputs: out_idx [B], out_probs [B][V],
+ * out_seq [B][seq_stride] (element step), next_tokens [B] (the pick, or teacher[b][step] with teacher [B][seq_stride]),
+ * dbg_logits [step + 1][dbg_batch or B][V] (the mixed logits before temperature, row row_offset + b).
+ * Fused tail (16-bit round_dtype, emb_table [V][D] in that type, D even): rows b, B + b, ... < emb_rows of emb_h [emb_rows][D] take
+ * the next token's embedding and, with emb_xn / emb_norm_w [D], of emb_xn its RMSNorm (emb_eps) times emb_norm_w.
+ * adv_pos / adv_step (int32 [1] or NULL): advanced by one after every CTA has read the step, through an arrival ticket this call
+ * owns; the call then synchronises and fails if the ticket was not left at zero.
+ * path: NULL or dev int32 [B][3]: top-k select (0 none, 1 histogram, 2 radix fallback), whether the nucleus trimmed ties at its
+ * boundary value (0 / 1), draw ending (0 greedy, 1 claimed by a segment, 2 past-the-end fallback). vec_loads: NULL or host int, 1
+ * when the row is staged with 16-byte loads (V % 4 == 0 and logits, dbg_logits 16-byte aligned), 0 for element-wise loads.
+ * Every argument is checked before any launch. */
+int  lg_test_sample(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc, uint64_t step,
+                    const int32_t* step_dev, int row_offset, const uint64_t* seed_rows, const int32_t* step_rows, int32_t* out_idx,
+                    float* out_probs, int32_t* out_seq, int seq_stride, const int32_t* teacher, int32_t* next_tokens,
+                    float* dbg_logits, int dbg_batch, const void* emb_table, void* emb_h, void* emb_xn, const void* emb_norm_w,
+                    float emb_eps, int D, int emb_rows, int32_t* adv_pos, int32_t* adv_step, int32_t* path, int* vec_loads,
+                    void* stream);
+/* The score head of lg_score on caller slabs: partial dev f32 [ks][P * nh][V] (row p * nh + h, h = 1 the unconditional twin).
+ * logits (dev f32 [P][V] or NULL): the slabs summed in slab order, rounded to dtype, CFG-mixed with cfg_scale when nh == 2.
+ * nll (dev f32 [P] or NULL, needs targets dev int32 [P]): logsumexp(logits[p]) - logits[p][target], NaN for a target outside [0, V). */
+int  lg_test_score_head(const float* partial, int ks, int P, int V, int nh, float cfg_scale, int dtype, const int32_t* targets,
+                        float* logits, float* nll, void* stream);
+
 /* One VQ decoder/encoder convolution through the decoder's own dispatch (the mma.sync gather kernel or either wgmma kernel,
  * honouring LG_CONV_TC, LG_CONV_SWAP, LG_GN_FUSE and the CTA budget), optionally followed by GroupNorm(32, eps 1e-6)
  * [+ swish] of its output the way a ResnetBlock hands one to the other (statistics taken from the conv's drain when it wrote them).

@@ -79,6 +79,10 @@ SIGNATURES = {
                                 c_void_p, c_void_p, c_void_p, c_void_p]),
     "lg_test_sjd_verify": (c_int, [c_int, c_int, c_int, c_int, c_int, c_uint64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                    c_void_p, c_void_p, c_void_p, c_void_p]),
+    "lg_test_sample": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(SampleCfg), c_uint64, c_void_p, c_int, c_void_p, c_void_p,
+                               c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                               c_void_p, c_float, c_int, c_int, c_void_p, c_void_p, c_void_p, POINTER(c_int), c_void_p]),
+    "lg_test_score_head": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "lg_vq_create": (c_int, [POINTER(VqCfg), c_int, POINTER(c_void_p)]),
     "lg_vq_destroy": (None, [c_void_p]),
     "lg_vq_bind_weight": (c_int, [c_void_p, c_char_p, c_void_p, POINTER(c_int64), c_int]),

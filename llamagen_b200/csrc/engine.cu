@@ -1209,6 +1209,69 @@ int lg_test_sjd_verify(int B, int S, int L, int V, int greedy, uint64_t seed, co
     return rc;
 }
 
+int lg_test_sample(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc, uint64_t step,
+                   const int32_t* step_dev, int row_offset, const uint64_t* seed_rows, const int32_t* step_rows, int32_t* out_idx,
+                   float* out_probs, int32_t* out_seq, int seq_stride, const int32_t* teacher, int32_t* next_tokens, float* dbg_logits,
+                   int dbg_batch, const void* emb_table, void* emb_h, void* emb_xn, const void* emb_norm_w, float emb_eps, int D,
+                   int emb_rows, int32_t* adv_pos, int32_t* adv_step, int32_t* path, int* vec_loads, void* stream) {
+    static const char* fn = "lg_test_sample";
+    cudaStream_t st = (cudaStream_t)stream;
+    LG_REQUIRE(logits && sc, "%s: null logits or config", fn);
+    LG_REQUIRE(B > 0 && V > 0, "%s: bad shape B=%d V=%d", fn, B, V);
+    LG_REQUIRE((size_t)V * sizeof(float) <= 200 * 1024, "lg_sample: vocab %d too large for the shared-memory row stage", V);
+    LG_REQUIRE(round_dtype == LG_DTYPE_F32 || lg_dtype_is16(round_dtype), "%s: unsupported round dtype %d", fn, round_dtype);
+    LG_REQUIRE(((uintptr_t)logits & 3) == 0 && ((uintptr_t)out_probs & 3) == 0 && ((uintptr_t)dbg_logits & 3) == 0,
+               "%s: misaligned (4 bytes) f32 buffer", fn);
+    LG_REQUIRE(!(step_dev && seed_rows), "%s: step_dev and step_rows both give the step", fn);
+    LG_REQUIRE((seed_rows != nullptr) == (step_rows != nullptr), "%s: seed_rows and step_rows go together", fn);
+    LG_REQUIRE(row_offset >= 0, "%s: row_offset %d < 0", fn, row_offset);
+    LG_REQUIRE(!(out_seq || teacher) || seq_stride > 0, "%s: out_seq / teacher need seq_stride > 0", fn);
+    LG_REQUIRE(!teacher || next_tokens || emb_table, "%s: teacher only changes next_tokens and the fused tail", fn);
+    LG_REQUIRE(!dbg_logits || (dbg_batch >= 0 && (dbg_batch == 0 ? row_offset == 0 : row_offset + B <= dbg_batch)),
+               "%s: dbg rows row_offset + b must lie in dbg_batch (%d)", fn, dbg_batch);
+    if (emb_table) {
+        LG_REQUIRE(lg_dtype_is16(round_dtype), "lg_sample: the fused tail needs a 16-bit round dtype");
+        LG_REQUIRE(emb_h && D > 0 && D % 2 == 0 && emb_rows >= B && (!emb_xn || emb_norm_w),
+                   "%s: the fused tail needs emb_h, an even D > 0, emb_rows >= B and emb_norm_w with emb_xn", fn);
+        LG_REQUIRE(((uintptr_t)emb_table & 3) == 0 && ((uintptr_t)emb_h & 3) == 0 && ((uintptr_t)emb_xn & 3) == 0 &&
+                   ((uintptr_t)emb_norm_w & 3) == 0, "%s: misaligned (4 bytes) fused-tail buffer", fn);
+    } else {
+        LG_REQUIRE(!emb_h && !emb_xn && !emb_norm_w, "%s: emb_h / emb_xn / emb_norm_w without emb_table", fn);
+    }
+    SampleArgs a = make_sample_args(*sc, logits, B, V, mix_cfg, round_dtype);
+    a.step = step; a.step_dev = step_dev; a.row_offset = row_offset; a.seed_rows = seed_rows; a.step_rows = step_rows;
+    a.out_idx = out_idx; a.out_probs = out_probs; a.out_seq = out_seq; a.seq_stride = seq_stride; a.teacher = teacher;
+    a.next_tokens = next_tokens; a.dbg_logits = dbg_logits; a.dbg_batch = dbg_batch;
+    a.emb_table = emb_table; a.emb_h = emb_h; a.emb_xn = emb_xn; a.emb_norm_w = emb_norm_w; a.emb_eps = emb_eps; a.emb_D = D;
+    a.emb_rows = emb_rows; a.adv_pos = adv_pos; a.adv_step = adv_step; a.dbg_path = path;
+    if (vec_loads) *vec_loads = sample_vec_loads(a);
+    if (!adv_pos && !adv_step) return launch_sample(a, st);
+    // the arrival ticket: zeroed here, and it must be back at zero once the launch is done (synchronises)
+    unsigned int* ticket = nullptr;
+    LG_CUDA_OK(cudaMallocAsync((void**)&ticket, sizeof(unsigned int), st));
+    LG_CUDA_OK(cudaMemsetAsync(ticket, 0, sizeof(unsigned int), st));
+    a.adv_ticket = ticket;
+    const int rc = launch_sample(a, st);
+    unsigned int left = 0;
+    const cudaError_t ce = cudaMemcpyAsync(&left, ticket, sizeof(left), cudaMemcpyDeviceToHost, st);
+    cudaFreeAsync(ticket, st);
+    LG_TRY(rc);
+    LG_CUDA_OK(ce);
+    LG_CUDA_OK(cudaStreamSynchronize(st));
+    LG_REQUIRE(left == 0, "%s: the counter ticket was left at %u", fn, left);
+    return 0;
+}
+
+int lg_test_score_head(const float* partial, int ks, int P, int V, int nh, float cfg_scale, int dtype, const int32_t* targets,
+                       float* logits, float* nll, void* stream) {
+    static const char* fn = "lg_test_score_head";
+    LG_REQUIRE(partial && (logits || nll), "%s: null slabs, or neither logits nor nll", fn);
+    LG_REQUIRE(!nll || targets, "%s: nll needs targets", fn);
+    LG_REQUIRE(ks >= 1 && P > 0 && V > 0 && (nh == 1 || nh == 2), "%s: bad shape ks=%d P=%d V=%d nh=%d", fn, ks, P, V, nh);
+    LG_REQUIRE(dtype == LG_DTYPE_F32 || lg_dtype_is16(dtype), "%s: unsupported dtype %d", fn, dtype);
+    return launch_score_head(partial, ks, P, V, nh, cfg_scale, dtype, targets, logits, nll, (cudaStream_t)stream);
+}
+
 int lg_vq_set_cta_budget(int ctas) {
     conv_tc_set_cta_budget(ctas < 0 ? 0 : ctas);
     return 0;

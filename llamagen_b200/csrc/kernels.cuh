@@ -46,7 +46,14 @@ struct SampleArgs {
     int* adv_pos = nullptr;                // incremented once per launch by the last CTA (null: no advance)
     int* adv_step = nullptr;
     unsigned int* adv_ticket = nullptr;    // zero-initialised arrival counter, left at zero
+    // lg_test_sample only: [B][3] per image, written by thread 0 of its CTA: top-k select (0 none, 1 histogram, 2 radix fallback),
+    // nucleus tie trim (0 / 1), draw ending (0 greedy, 1 claimed by a segment, 2 the past-the-end fallback). Null in production.
+    int32_t* dbg_path = nullptr;
 };
+// The sample kernel stages the row with 16-byte loads (and dbg_logits with 16-byte stores) iff this holds, else element by element
+__host__ __device__ inline bool sample_vec_loads(const SampleArgs& a) {
+    return (a.V & 3) == 0 && ((uintptr_t)a.logits & 15) == 0 && ((uintptr_t)a.dbg_logits & 15) == 0;
+}
 int launch_sample(const SampleArgs& a, cudaStream_t st);
 
 // Speculative Jacobi decoding (lg_generate_sjd). Image b's window has L slots; slot i feeds token start[b] + i - 1 (win) and its

@@ -31,6 +31,20 @@ __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
     return x ^ (x >> 31);
 }
 
+// Highest thread index of the block (kThreads threads) for which pred holds, -1 if none; returned to every thread. s_w: 32 ints.
+template <int kThreads>
+__device__ __forceinline__ int block_last_true(bool pred, int* s_w) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const unsigned bal = __ballot_sync(0xffffffffu, pred);
+    if (lane == 0) s_w[warp] = bal ? warp * 32 + 31 - __clz((int)bal) : -1;
+    __syncthreads();
+    int r = lane < kThreads / 32 ? s_w[lane] : -1;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) r = max(r, __shfl_xor_sync(0xffffffffu, r, o));
+    __syncthreads();   // s_w may be reused
+    return r;
+}
+
 // E: the 16-bit type of the rounding (a.round_dtype != LG_DTYPE_F32) and of the fused tail's rows
 template <typename E>
 __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
@@ -42,8 +56,9 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
     __shared__ float mhist[256];
     __shared__ uint32_t s_prefix, s_remaining;
     __shared__ float s_acc;
-    __shared__ int s_pick;
+    __shared__ int s_pick, s_end;
     __shared__ float s_wtot[32];
+    __shared__ int s_own[32];
 
     const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int V = a.V, B = a.B;
@@ -65,9 +80,9 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
         if (a.round_dtype) u = TR::round(u);
         return __fadd_rn(u, __fmul_rn(__fsub_rn(c, u), a.cfg_scale));
     };
-    if ((V & 3) == 0) {
+    if (sample_vec_loads(a)) {
         // 128-bit loads, several requests of a thread in flight before the first use (the scalar loop was
-        // latency-bound: 16 dependent L2 round trips per thread)
+        // latency-bound: 16 dependent L2 round trips per thread); a caller's row that is not 16-byte aligned takes the scalar loop
         const float4* lc4 = reinterpret_cast<const float4*>(lc);
         const float4* lu4 = reinterpret_cast<const float4*>(lu);
         const int V4 = V >> 2;
@@ -97,6 +112,7 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
     // holding the k-th largest, then an exact rank count among that bucket's few members. The bucket map is monotone in x, so
     // the selected VALUE is exact. The 4-pass 8-bit radix select below stays as the fallback for degenerate rows (its first
     // pass hashes sign+exponent: ~6 live buckets -> 16384 colliding atomics, measured 26.5 us per row).
+    int path_topk = 0, path_trim = 0;   // dbg_path (lg_test_sample); the draw ending is s_end
     if (a.top_k > 0) {
         const int k = min(max(a.top_k, 1), V);
         if (k < V) {
@@ -199,6 +215,7 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
                 }
                 thr = fkey_inv(prefix);
             }
+            path_topk = fast ? 1 : 2;
             for (int v = tid; v < V; v += kSampleThreads)
                 if (sh[v] < thr) sh[v] = -INFINITY;
             __syncthreads();
@@ -289,6 +306,7 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
         if (nties > 1) {
             int nkeep = 1;
             while (nkeep < nties && acc + (float)nkeep * pstar <= a.top_p) ++nkeep;
+            path_trim = nkeep < nties;
             if (nkeep < nties && tid == 0) {
                 int seen = 0;
                 for (int v = 0; v < V; ++v)
@@ -314,7 +332,7 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
         for (int v = tid; v < V; v += kSampleThreads) op[v] = sh[v] / Z;
     }
 
-    if (tid == 0) s_pick = -1;
+    if (tid == 0) { s_pick = -1; s_end = 0; }
     __syncthreads();
 
     if (a.greedy) {
@@ -380,7 +398,12 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
         const uint64_t r = splitmix64(splitmix64(seed ^ (0xA0761D6478BD642Full * (step + 1))) ^ (0xE7037ED1A0B428DBull * rrow));
         const float u = (float)(r >> 40) * (1.0f / 16777216.0f);
         const float target = u * total;
-        if (local > 0.f && target >= excl && target < excl + local) {
+        // The fp32 prefixes are not additive across threads (excl + local, rounded, need not equal the next thread's excl), so
+        // "excl <= target < excl + local" would give some targets to no thread and others to two. The target belongs instead to the
+        // highest thread with a non-zero segment that starts at or below it: exactly one owner for every target.
+        const int owner = block_last_true<kSampleThreads>(local > 0.f && excl <= target, s_own);
+        const int lastseg = a.dbg_path ? block_last_true<kSampleThreads>(local > 0.f, s_own) : -1;
+        if (tid == owner) {
             float c = excl;
             int pick = -1, lastnz = -1;
             for (int v = v0; v < v1; ++v) {
@@ -389,10 +412,14 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
                 c += e;
                 if (c > target && e > 0.f) { pick = v; break; }
             }
+            // a walk that never passes the target (the target past the total, or in the rounding gap before the next segment's
+            // start) takes the segment's last non-zero weight
             s_pick = pick >= 0 ? pick : lastnz;
+            s_end = pick < 0 && tid == lastseg ? 2 : 1;
         }
         __syncthreads();
-        if (s_pick < 0) {  // rounding pushed the target past the total: take the last non-zero weight
+        if (s_pick < 0) {  // no owner (no segment with a positive sum: a NaN row): the last non-zero weight, if any
+            if (tid == 0) s_end = 2;
             int cand = -1;
             for (int v = tid; v < V; v += kSampleThreads)
                 if (sh[v] > 0.f) cand = max(cand, v);
@@ -410,6 +437,11 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
         const int nxt = a.teacher ? a.teacher[(size_t)b * a.seq_stride + step] : pick;
         if (a.next_tokens) a.next_tokens[b] = nxt;
         s_next = nxt;
+        if (a.dbg_path) {
+            a.dbg_path[3 * b] = path_topk;
+            a.dbg_path[3 * b + 1] = path_trim;
+            a.dbg_path[3 * b + 2] = s_end;
+        }
     }
     // ---------------- fused tail: next step's input rows (embedding lookup + layer-0 RMSNorm) and the counter advance ----------
     if (a.emb_table) {
@@ -507,7 +539,7 @@ __global__ void __launch_bounds__(kSjdThreads) sjd_verify_kernel(SjdArgs a) {
     lg_pdl_sync();
     __shared__ float red[33];
     __shared__ float s_wtot[32];
-    __shared__ int s_i, s_pick;
+    __shared__ int s_i, s_pick, s_own[32];
     const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int L = a.L, V = a.V, S = a.S;
     const int n = a.nfin[b], s = a.start[b];
@@ -568,20 +600,19 @@ __global__ void __launch_bounds__(kSjdThreads) sjd_verify_kernel(SjdArgs a) {
             if (total > 0.f) {
                 const float target = sjd_uniform(a.seed, b + a.row_offset, s + i, kSjdResidual) * total;
                 const float excl = s_wtot[warp] + (incl - local);
-                int last = -1;
-                for (int v = tid; v < V; v += kSjdThreads)
-                    if (pr[v] - (uni ? qu : qr[v]) > 0.f) last = max(last, v);
-                last = (int)block_max((float)last, red);
-                __syncthreads();
-                if (tid == 0) s_pick = last;   // the target past the rounded total: the last positive weight
-                __syncthreads();
-                if (local > 0.f && target >= excl && target < excl + local) {
+                // one owner for every target, as in sample_kernel: the highest thread with a positive segment starting at or below
+                // it; a walk that never passes the target takes the segment's last positive weight
+                const int owner = block_last_true<kSjdThreads>(local > 0.f && excl <= target, s_own);
+                if (tid == owner) {
                     float c = excl;
+                    int pick = -1, lastnz = -1;
                     for (int v = v0; v < v1; ++v) {
                         const float e = fmaxf(0.f, pr[v] - (uni ? qu : qr[v]));
+                        if (e > 0.f) lastnz = v;
                         c += e;
-                        if (c > target && e > 0.f) { s_pick = v; break; }
+                        if (c > target && e > 0.f) { pick = v; break; }
                     }
+                    s_pick = pick >= 0 ? pick : lastnz;
                 }
             }
             __syncthreads();

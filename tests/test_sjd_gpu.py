@@ -1,6 +1,7 @@
 """Speculative Jacobi decoding on the GPU: the window attention kernel against a float64 reference, the acceptance kernel against the
 test oracle (tests/sjd_oracle.py), and lg_generate_sjd end to end (greedy equality with generate(), replay of sampled runs from the
 p rows the engine dumps, determinism, and isolation from generate() and score())."""
+import math
 import zlib
 
 import numpy as np
@@ -124,6 +125,62 @@ def test_verify_kernel_matches_oracle(greedy, V):
         assert (n2[b], s2[b]) == (im.n, im.s)
         accepted += len(made) - 1
     assert accepted > B // 4
+
+
+def _residual_uniforms(seed, B, k):
+    """u_res(k) of images 0 .. B - 1 (sjd_oracle.uniform, vectorised)."""
+    def sm(x):
+        x = x + np.uint64(0x9E3779B97F4A7C15)
+        x = (x ^ (x >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+        x = (x ^ (x >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+        return x ^ (x >> np.uint64(31))
+    with np.errstate(over="ignore"):
+        b = np.arange(1, B + 1, dtype=np.uint64)
+        c1, c3 = np.uint64((so.C1 * (k + 1)) & so.M64), np.uint64((so.C3 * so.RESIDUAL) & so.M64)
+        r = sm(sm(sm(np.uint64(seed) ^ c1) ^ (np.uint64(so.C2) * b)) ^ c3)
+    return (r >> np.uint64(40)).astype(np.float64) * 2.0 ** -24
+
+
+@pytest.mark.gpu
+def test_verify_residual_draw_intervals():
+    """About 1.5 million residual draws of normalize(max(0, p - q)) at V = 16384 (1024 images x 1500 seeds; every draft has p = 0 and
+    is rejected): each pick's float64 CDF interval over the fp32 residual weights holds u_res within (ceil(V / 512) + 16) 2^-24, and
+    its weight is > 0. The fp32 segment prefixes of the 512 threads have gaps and overlaps; a target there must still go to a
+    neighbouring segment, never to an unrelated token."""
+    from llamagen_b200 import _lib
+    lib = _lib.load()
+    B, L, S, V, seeds = 1024, 2, 3, 16384, 1500
+    g = torch.Generator(device=DEV).manual_seed(4)
+    p = torch.softmax(torch.randn(B, L, V, device=DEV, generator=g) * 2.0, -1)
+    q = torch.softmax(torch.randn(B, L, V, device=DEV, generator=g) * 2.0, -1)
+    p[:, 0, 0] = 0                                     # the draft (token 0) has p = 0: rejected
+    p, q = p.contiguous(), q.contiguous()
+    w = torch.clamp_min(p[:, 0] - q[:, 0], 0).double()   # the kernel's fp32 weights fmaxf(0, p - q), exactly
+    C = w.cumsum(1)
+    C = C / C[:, -1:]
+    zi = torch.zeros(B, L, dtype=torch.int32, device=DEV)
+    nfin = torch.empty(B, dtype=torch.int32, device=DEV)
+    start = torch.empty(B, dtype=torch.int32, device=DEV)
+    out = torch.empty(B, S, dtype=torch.int32, device=DEV)
+    picks = torch.empty(seeds, B, dtype=torch.long, device=DEV)
+    P = _lib.ptr
+    for j in range(seeds):
+        nfin.fill_(1)
+        start.fill_(1)
+        out.fill_(-1)
+        _lib.check(lib.lg_test_sjd_verify(B, S, L, V, 0, 1000 + j, P(p), P(q), P(zi), P(zi), P(zi), P(nfin), P(start), P(out),
+                                          _lib.current_stream(DEV)), "lg_test_sjd_verify")
+        picks[j] = out[:, 1].long()
+    u = torch.from_numpy(np.stack([_residual_uniforms(1000 + j, B, 1) for j in range(seeds)])).to(DEV)   # [seeds][B]
+    pk = picks.t().contiguous()                                                                          # [B][seeds]
+    assert (pk >= 0).all() and (w.gather(1, pk) > 0).all()
+    hi = C.gather(1, pk)
+    lo = torch.where(pk > 0, C.gather(1, (pk - 1).clamp(min=0)), torch.zeros_like(hi))
+    band = (math.ceil(V / 512) + 16) * 2.0 ** -24
+    ut = u.t()
+    bad = (ut < lo - band) | (ut > hi + band)
+    print(f"[residual sweep] {B * seeds} draws, {int(bad.sum())} outside their interval")
+    assert int(bad.sum()) == 0, bad.nonzero()[:10].tolist()
 
 
 @pytest.mark.gpu
