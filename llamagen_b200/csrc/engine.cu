@@ -166,22 +166,79 @@ SampleArgs make_sample_args(const lg_sample_cfg& sc, const float* logits, int B,
     return a;
 }
 
-// The workspace (lg_engine::carve), or one decode chain's view of it
-struct Workspace {
-    char* base = nullptr;     // start of the whole workspace
-    int rows = 0, max_seq = 0;
+// A K / V cache pair laid out [layer][rows, H, max_seq, hdp] (DESIGN §3) and its tensor maps
+struct KvCache {
     char *kcache = nullptr, *vcache = nullptr;
     size_t cache_bytes = 0;   // the K and V regions together, from kcache on (what the first use zero-fills)
+    int rows = 0, max_seq = 0;
+    int layers = 0;           // n_layer, or 1 for a cache that every layer rewrites before its attention reads it
+    bool kv_f8 = false;       // e4m3 with the engine's per-layer scales, else the model dtype
+    KvMaps maps;
+};
+
+// The activations, GEMM split-K partials and logits of a forward pass
+struct RowBuffers {
     char *h = nullptr, *xn = nullptr, *q = nullptr, *attn = nullptr, *ff = nullptr, *x0 = nullptr;
     float *partial = nullptr, *logits = nullptr;
     size_t partial_floats = 0;
+};
+
+// The workspace (lg_engine::carve), one decode chain's view of it, or a scratch view (lg_score, lg_generate_sjd)
+struct Workspace : KvCache, RowBuffers {
+    char* base = nullptr;     // start of the whole workspace
     int32_t* tokens = nullptr;
     int* counters = nullptr;  // [0] = pos, [1] = step, [64] = the fused sampler tail's ticket
-    KvMaps maps;
-    // lg_score's view (lg_engine::carve_score): K / V of ONE layer in the model dtype, rewritten by every layer (a teacher-forced pass
-    // never decodes afterwards), and the rows of one head GEMM
-    bool score = false;
-    int head_rows = 0;
+    int head_rows = 0;        // lg_score: rows per head GEMM
+};
+
+// Bump allocator over a workspace from `base` (null: sizes only), 256-byte aligned regions, for chain g of n
+struct Carver {
+    char* base;
+    int g = 0, n = 1;
+    size_t off = 0;
+    // a region of `bytes`, of which chain g takes the part from g * chain_stride on
+    char* shared(size_t bytes, size_t chain_stride) {
+        char* p = base ? base + off + g * chain_stride : nullptr;
+        off += align_up(bytes);
+        return p;
+    }
+    // a region that scales with rows: chain g takes its g-th n-th
+    char* split(size_t bytes) { return shared(bytes, bytes / n); }
+};
+
+// A captured CUDA graph of one stream's work and its executable graph
+struct Graph {
+    cudaGraph_t graph = nullptr;
+    cudaGraphExec_t exec = nullptr;
+    uint64_t launches = 0;    // kernel launches per replay
+    Graph() = default;
+    Graph(const Graph&) = delete;
+    Graph& operator=(const Graph&) = delete;
+    ~Graph() {
+        if (exec) cudaGraphExecDestroy(exec);
+        if (graph) cudaGraphDestroy(graph);
+    }
+    template <class Body>
+    int capture(cudaStream_t st, Body&& body) {
+        cudaError_t ce = cudaStreamBeginCapture(st, cudaStreamCaptureModeRelaxed);
+        if (ce != cudaSuccess) return lg_fail("cudaStreamBeginCapture failed: %s", cudaGetErrorString(ce));
+        const uint64_t before = g_lg_launches.load();
+        const int rc = body();
+        launches = g_lg_launches.load() - before;
+        ce = cudaStreamEndCapture(st, &graph);
+        g_lg_launches.fetch_sub(launches);   // the capture pass launched nothing
+        if (rc < 0) return rc;
+        if (ce != cudaSuccess || !graph) return lg_fail("stream capture failed: %s", cudaGetErrorString(ce));
+        ce = cudaGraphInstantiate(&exec, graph, 0);
+        if (ce != cudaSuccess) return lg_fail("cudaGraphInstantiate failed: %s", cudaGetErrorString(ce));
+        return 0;
+    }
+    int launch(cudaStream_t st) {
+        const cudaError_t ce = cudaGraphLaunch(exec, st);
+        if (ce != cudaSuccess) return lg_fail("cudaGraphLaunch failed: %s", cudaGetErrorString(ce));
+        g_lg_launches.fetch_add(launches);
+        return 0;
+    }
 };
 
 struct Layer {
@@ -200,7 +257,6 @@ struct lg_engine {
     size_t esz = 2;
     // KV-cache storage (lg_engine_set_kv_cache): the model dtype, or fp8 e4m3 with per-layer power-of-two (k, v) scales
     bool kv_f8 = false;
-    size_t kv_esz = 2;                    // bytes per cached element
     std::vector<float> kv_scales;         // [n_layer][2] (fp8 only)
     std::unordered_map<std::string, Tensor> w;
     std::vector<Layer> layers;
@@ -243,6 +299,22 @@ struct lg_engine {
         LG_CUDA_OK(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
         return 0;
     }
+    // Runs body(works[0]) with works[0..n) forked from and joined to the caller's stream by events: the caller's stream may be the
+    // legacy default stream (torch's default), which cannot be captured into a CUDA graph. Semantics for the caller stay
+    // "asynchronous on the given stream".
+    template <class Body>
+    int run_forked(cudaStream_t caller, int n, Body&& body) {
+        LG_TRY(ensure_streams());
+        LG_TRY(zero_fill_if_needed(caller));
+        LG_CUDA_OK(cudaEventRecord(ev_fork, caller));
+        for (int i = 0; i < n; ++i) LG_CUDA_OK(cudaStreamWaitEvent(works[i], ev_fork, 0));
+        const int rc = body(works[0]);
+        for (int i = 0; i < n; ++i) {
+            cudaEventRecord(ev_joins[i], works[i]);
+            cudaStreamWaitEvent(caller, ev_joins[i], 0);
+        }
+        return rc;
+    }
 
     // R <= 8 decode steps on the column-owner GEMV path (gemv_small.cu); shared by forward() and the decode loop's fused tail
     bool small_row_path(int M, const AttnArgs& aa) const {
@@ -259,17 +331,23 @@ struct lg_engine {
     }
     size_t carve(Workspace& o, char* base, int rows, int max_seq, int g = 0, int n = 1) const;
     size_t carve_score(Workspace& o, char* base, int rows, int seq) const;
-    size_t carve_sjd(Workspace& o, SjdArgs& sa, char* base, int B, int nh, int L) const;
-    // K / V tensor maps over every layer of a workspace or chain view (one layer in the model dtype for a scoring view)
-    int make_maps(Workspace& w) const {
-        if (w.score) return make_kv_maps(w.maps, cfg.dtype, hd, hdp, cfg.dtype, w.kcache, w.vcache, (long long)w.rows * cfg.n_head * w.max_seq);
-        return make_kv_maps(w.maps, cfg.dtype, hd, hdp, kv_f8 ? LG_DTYPE_E4M3 : cfg.dtype, w.kcache, w.vcache,
-                            (long long)cfg.n_layer * w.rows * cfg.n_head * w.max_seq);
+    size_t carve_sjd(RowBuffers& o, SjdArgs& sa, char* base, int B, int nh, int L) const;
+    void carve_kv(Carver& c, KvCache& o, int rows, int max_seq, int layers, bool f8) const;
+    void carve_rows(Carver& c, RowBuffers& o, size_t M, size_t x0_rows, size_t partial_floats, size_t logits_rows) const;
+    // the most partial floats one of a layer's four GEMMs needs at M rows
+    size_t layer_partial_floats(int M) const {
+        const int D = cfg.dim, F = cfg.ffn_dim, dt = cfg.dtype;
+        return std::max({gemm_partial_floats(M, 3 * D, D, 0, dt), gemm_partial_floats(M, D, D, 0, dt),
+                         gemm_partial_floats(M, 2 * F, D, F, dt), gemm_partial_floats(M, D, F, 0, dt)});
     }
-    AttnArgs attn_args(const Workspace& w, int l, int R, int Tq) const {
-        if (w.score) return make_attn_args(cfg.dtype, cfg.n_head, hd, hdp, w.rows, w.max_seq, w.kcache, w.vcache, w.maps, nullptr, 0, R, Tq);
-        return make_attn_args(cfg.dtype, cfg.n_head, hd, hdp, w.rows, w.max_seq, w.kcache, w.vcache, w.maps,
-                              kv_f8 ? &kv_scales[2 * l] : nullptr, l, R, Tq);
+    // K / V tensor maps over every layer the cache holds
+    int make_maps(KvCache& kv) const {
+        return make_kv_maps(kv.maps, cfg.dtype, hd, hdp, kv.kv_f8 ? LG_DTYPE_E4M3 : cfg.dtype, kv.kcache, kv.vcache,
+                            (long long)kv.layers * kv.rows * cfg.n_head * kv.max_seq);
+    }
+    AttnArgs attn_args(const KvCache& kv, int l, int R, int Tq) const {
+        return make_attn_args(cfg.dtype, cfg.n_head, hd, hdp, kv.rows, kv.max_seq, kv.kcache, kv.vcache, kv.maps,
+                              kv.kv_f8 ? &kv_scales[2 * l] : nullptr, l % kv.layers, R, Tq);
     }
     AttnArgs layer_attn(const Workspace& w, int l, int R, int Tq, PosArg pos, const float* emb_mask, int B) const {
         AttnArgs aa = attn_args(w, l, R, Tq);
@@ -291,52 +369,54 @@ struct lg_engine {
     int embed_cond(const Workspace& w, const void* cond, int B, int R, int T, cudaStream_t st);
     int gemm(const Workspace& w, const void* x, int M, int N, int K, const GemmWeight& wa, const GemmWeight& wb, int n_split, int* ksplit,
              float* direct_out, cudaStream_t st, const GemmNext* next = nullptr);
+    int head(const Workspace& w, const void* x, int M, float* logits_out, const GemmNext* next, cudaStream_t st);
 };
 
 // Lays out the workspace for `rows` rows and max_seq positions from `base` (null: sizes only) and returns its bytes. With n > 1, `o`
 // becomes chain g's view of that same layout: the g-th n-th of every region that scales with rows (rows / n rows each), a 64-float
 // aligned n-th of the GEMM partials, and the counters from 2g on.
 size_t lg_engine::carve(Workspace& o, char* base, int rows, int max_seq, int g, int n) const {
-    const int L = cfg.n_layer, D = cfg.dim, F = cfg.ffn_dim, V = cfg.vocab_size, H = cfg.n_head;
-    const int Tc = cfg.model_type == LG_MODEL_T2I ? cfg.cls_token_num : 1;
-    const size_t Mmax = (size_t)rows * Tc;
-    size_t off = 0;
-    auto take = [&](size_t bytes, size_t chain_stride) {
-        char* p = base ? base + off + g * chain_stride : nullptr;
-        off += align_up(bytes);
-        return p;
-    };
-    auto split = [&](size_t bytes) { return take(bytes, bytes / n); };
-    const size_t cache = (size_t)rows * H * max_seq * hdp * kv_esz * L;
-    o.kcache = split(cache);
-    o.vcache = split(cache);
-    o.cache_bytes = off;
-    o.h = split(Mmax * D * esz);
-    o.xn = split(Mmax * D * esz);
-    o.q = split(Mmax * D * esz);
-    o.attn = split(Mmax * D * esz);
-    o.ff = split(Mmax * F * esz);
-    o.x0 = split(cfg.model_type == LG_MODEL_T2I ? Mmax * cfg.caption_dim * esz : 0);
-    size_t pf = 0;
-    const int Ms[2] = {rows, (int)Mmax};
-    for (int i = 0; i < 2; ++i) {
-        const int M = Ms[i];
-        pf = std::max(pf, gemm_partial_floats(M, 3 * D, D, 0, cfg.dtype));
-        pf = std::max(pf, gemm_partial_floats(M, D, D, 0, cfg.dtype));
-        pf = std::max(pf, gemm_partial_floats(M, 2 * F, D, F, cfg.dtype));
-        pf = std::max(pf, gemm_partial_floats(M, D, F, 0, cfg.dtype));
-        if (cfg.model_type == LG_MODEL_T2I) pf = std::max(pf, gemm_partial_floats(M, D, cfg.caption_dim, 0, cfg.dtype));
+    const int D = cfg.dim, V = cfg.vocab_size, dt = cfg.dtype;
+    const bool t2i = cfg.model_type == LG_MODEL_T2I;
+    const int Mmax = rows * (t2i ? cfg.cls_token_num : 1);
+    size_t pf = gemm_partial_floats(rows, V, D, 0, dt);
+    for (int M : {rows, Mmax}) {
+        pf = std::max(pf, layer_partial_floats(M));
+        if (t2i) pf = std::max(pf, gemm_partial_floats(M, D, cfg.caption_dim, 0, dt));
     }
-    pf = std::max(pf, gemm_partial_floats(rows, V, D, 0, cfg.dtype));
-    o.partial_floats = n == 1 ? pf : pf / n / 64 * 64;
-    o.partial = (float*)take(pf * sizeof(float), o.partial_floats * sizeof(float));
-    o.logits = (float*)split((size_t)rows * V * sizeof(float));
-    o.tokens = (int32_t*)split((size_t)rows * sizeof(int32_t));
-    o.counters = (int*)take(kCounterInts * sizeof(int), 2 * sizeof(int));
+    Carver c{base, g, n};
+    carve_kv(c, o, rows, max_seq, cfg.n_layer, kv_f8);
+    carve_rows(c, o, Mmax, t2i ? Mmax : 0, pf, rows);
+    o.tokens = (int32_t*)c.split((size_t)rows * sizeof(int32_t));
+    o.counters = (int*)c.shared(kCounterInts * sizeof(int), 2 * sizeof(int));
     o.base = base;
-    o.rows = rows / n;
+    return c.off;
+}
+
+// K and V of `layers` layers of [rows, H, max_seq, hdp] elements, in e4m3 (f8) or the model dtype
+void lg_engine::carve_kv(Carver& c, KvCache& o, int rows, int max_seq, int layers, bool f8) const {
+    const size_t bytes = (size_t)rows * cfg.n_head * max_seq * hdp * (f8 ? 1 : esz) * layers, start = c.off;
+    o.kcache = c.split(bytes);
+    o.vcache = c.split(bytes);
+    o.cache_bytes = c.off - start;
+    o.rows = rows / c.n;
     o.max_seq = max_seq;
-    return off;
+    o.layers = layers;
+    o.kv_f8 = f8;
+}
+
+// The row buffers of M activation rows, x0_rows caption rows, partial_floats GEMM partials (a 64-float aligned n-th of them for each
+// chain) and logits_rows rows of logits
+void lg_engine::carve_rows(Carver& c, RowBuffers& o, size_t M, size_t x0_rows, size_t partial_floats, size_t logits_rows) const {
+    o.h = c.split(M * cfg.dim * esz);
+    o.xn = c.split(M * cfg.dim * esz);
+    o.q = c.split(M * cfg.dim * esz);
+    o.attn = c.split(M * cfg.dim * esz);
+    o.ff = c.split(M * cfg.ffn_dim * esz);
+    o.x0 = c.split(x0_rows * cfg.caption_dim * esz);
+    o.partial_floats = c.n == 1 ? partial_floats : partial_floats / c.n / 64 * 64;
+    o.partial = (float*)c.shared(partial_floats * sizeof(float), o.partial_floats * sizeof(float));
+    o.logits = (float*)c.split(logits_rows * cfg.vocab_size * sizeof(float));
 }
 
 constexpr int kScoreHeadRows = 2048;   // rows per head GEMM of lg_score: its fp32 slabs stay ~kScoreHeadRows * V floats
@@ -345,84 +425,39 @@ constexpr int kScoreHeadRows = 2048;   // rows per head GEMM of lg_score: its fp
 // the GEMM partials of that M (and of the caption MLP and one head chunk), and K / V of ONE layer ([rows, H, round8(seq), hdp] in the
 // model dtype, also after lg_engine_set_kv_cache): every layer rewrites it before its attention reads it.
 size_t lg_engine::carve_score(Workspace& o, char* base, int rows, int seq) const {
-    const int D = cfg.dim, F = cfg.ffn_dim, V = cfg.vocab_size, H = cfg.n_head, Tc = cfg.cls_token_num;
+    const int D = cfg.dim, V = cfg.vocab_size, Tc = cfg.cls_token_num, dt = cfg.dtype;
     const bool t2i = cfg.model_type == LG_MODEL_T2I;
-    const int seq8 = (seq + 7) / 8 * 8, M = rows * seq;
-    size_t off = 0;
-    auto take = [&](size_t bytes) {
-        char* p = base ? base + off : nullptr;
-        off += align_up(bytes);
-        return p;
-    };
-    const size_t kv = (size_t)rows * H * seq8 * hdp * esz;
-    o.kcache = take(kv);
-    o.vcache = take(kv);
-    o.cache_bytes = off;
-    o.h = take((size_t)M * D * esz);
-    o.xn = take((size_t)M * D * esz);
-    o.q = take((size_t)M * D * esz);
-    o.attn = take((size_t)M * D * esz);
-    o.ff = take((size_t)M * F * esz);
-    o.x0 = take(t2i ? (size_t)rows * Tc * cfg.caption_dim * esz : 0);
-    size_t pf = 0;
-    pf = std::max(pf, gemm_partial_floats(M, 3 * D, D, 0, cfg.dtype));
-    pf = std::max(pf, gemm_partial_floats(M, D, D, 0, cfg.dtype));
-    pf = std::max(pf, gemm_partial_floats(M, 2 * F, D, F, cfg.dtype));
-    pf = std::max(pf, gemm_partial_floats(M, D, F, 0, cfg.dtype));
-    if (t2i) {
-        pf = std::max(pf, gemm_partial_floats(rows * Tc, D, cfg.caption_dim, 0, cfg.dtype));
-        pf = std::max(pf, gemm_partial_floats(rows * Tc, D, D, 0, cfg.dtype));
-    }
+    const int M = rows * seq;
     o.head_rows = std::min(rows * std::max(seq - Tc + 1, 1), kScoreHeadRows);
-    pf = std::max(pf, gemm_partial_floats(o.head_rows, V, D, 0, cfg.dtype));
-    o.partial_floats = pf;
-    o.partial = (float*)take(pf * sizeof(float));
+    size_t pf = std::max(layer_partial_floats(M), gemm_partial_floats(o.head_rows, V, D, 0, dt));
+    if (t2i) pf = std::max({pf, gemm_partial_floats(rows * Tc, D, cfg.caption_dim, 0, dt), gemm_partial_floats(rows * Tc, D, D, 0, dt)});
+    Carver c{base};
+    carve_kv(c, o, rows, (seq + 7) / 8 * 8, 1, false);
+    carve_rows(c, o, M, t2i ? rows * Tc : 0, pf, 0);
     o.base = base;
-    o.rows = rows;
-    o.max_seq = seq8;
-    o.score = true;
-    return off;
+    return c.off;
 }
 
-// lg_generate_sjd's scratch for B images (nh rows each) and window L, from `base` (null: sizes only): the activations, GEMM partials
-// and logits of nh * B * L rows, and the loop state (sa's buffers). `o` takes only the row-scaled regions; the caller adds the KV
-// cache of the full workspace.
-size_t lg_engine::carve_sjd(Workspace& o, SjdArgs& sa, char* base, int B, int nh, int L) const {
-    const int D = cfg.dim, F = cfg.ffn_dim, V = cfg.vocab_size;
+// lg_generate_sjd's scratch for B images (nh rows each) and window L, from `base` (null: sizes only): the row buffers of nh * B * L
+// rows, and the loop state (sa's buffers). The caller pairs `o` with the KV cache of the full workspace.
+size_t lg_engine::carve_sjd(RowBuffers& o, SjdArgs& sa, char* base, int B, int nh, int L) const {
+    const int V = cfg.vocab_size;
     const size_t M = (size_t)nh * B * L, BL = (size_t)B * L;
-    size_t off = 0;
-    auto take = [&](size_t bytes) {
-        char* p = base ? base + off : nullptr;
-        off += align_up(bytes);
-        return p;
-    };
-    o.h = take(M * D * esz);
-    o.xn = take(M * D * esz);
-    o.q = take(M * D * esz);
-    o.attn = take(M * D * esz);
-    o.ff = take(M * F * esz);
-    size_t pf = 0;
-    pf = std::max(pf, gemm_partial_floats((int)M, 3 * D, D, 0, cfg.dtype));
-    pf = std::max(pf, gemm_partial_floats((int)M, D, D, 0, cfg.dtype));
-    pf = std::max(pf, gemm_partial_floats((int)M, 2 * F, D, F, cfg.dtype));
-    pf = std::max(pf, gemm_partial_floats((int)M, D, F, 0, cfg.dtype));
-    pf = std::max(pf, gemm_partial_floats((int)M, V, D, 0, cfg.dtype));
-    o.partial_floats = pf;
-    o.partial = (float*)take(pf * sizeof(float));
-    o.logits = (float*)take(M * V * sizeof(float));
-    sa.p = (const float*)take(BL * V * sizeof(float));
-    sa.q = (float*)take(BL * V * sizeof(float));
-    sa.seed_rows = (uint64_t*)take(BL * sizeof(uint64_t));
-    sa.qflag = (int32_t*)take(BL * sizeof(int32_t));
-    sa.x = (const int32_t*)take(BL * sizeof(int32_t));
-    sa.win = (int32_t*)take(BL * sizeof(int32_t));
-    sa.step_rows = (int32_t*)take(BL * sizeof(int32_t));
-    sa.nfin = (int32_t*)take(B * sizeof(int32_t));
-    sa.start = (int32_t*)take(B * sizeof(int32_t));
-    sa.shift = (int32_t*)take(B * sizeof(int32_t));
-    sa.pos_rows = (int32_t*)take((size_t)nh * B * sizeof(int32_t));
-    sa.state = (int32_t*)take(kSjdStateInts * sizeof(int32_t));
-    return off;
+    Carver c{base};
+    carve_rows(c, o, M, 0, std::max(layer_partial_floats((int)M), gemm_partial_floats((int)M, V, cfg.dim, 0, cfg.dtype)), M);
+    sa.p = (const float*)c.split(BL * V * sizeof(float));
+    sa.q = (float*)c.split(BL * V * sizeof(float));
+    sa.seed_rows = (uint64_t*)c.split(BL * sizeof(uint64_t));
+    sa.qflag = (int32_t*)c.split(BL * sizeof(int32_t));
+    sa.x = (const int32_t*)c.split(BL * sizeof(int32_t));
+    sa.win = (int32_t*)c.split(BL * sizeof(int32_t));
+    sa.step_rows = (int32_t*)c.split(BL * sizeof(int32_t));
+    sa.nfin = (int32_t*)c.split(B * sizeof(int32_t));
+    sa.start = (int32_t*)c.split(B * sizeof(int32_t));
+    sa.shift = (int32_t*)c.split(B * sizeof(int32_t));
+    sa.pos_rows = (int32_t*)c.split((size_t)nh * B * sizeof(int32_t));
+    sa.state = (int32_t*)c.split(kSjdStateInts * sizeof(int32_t));
+    return c.off;
 }
 
 int lg_engine::gemm(const Workspace& w, const void* x, int M, int N, int K, const GemmWeight& wa, const GemmWeight& wb, int n_split, int* ksplit,
@@ -446,7 +481,6 @@ int lg_engine::forward(const Workspace& w, int M, int Tq, PosArg pos, const floa
     const int L = cfg.n_layer, D = cfg.dim, F = cfg.ffn_dim, V = cfg.vocab_size;
     const int R = M / Tq;
     const int dt = cfg.dtype;
-    int ks = 1;
     // ---- R <= 8 decode step (batch-1 latency path, gemv_small.cu): 5 dependent kernels per layer, no slabs
     if (Tq == 1 && small_row_path(M, attn_args(w, 0, R, Tq))) {
         for (int l = 0; l < L; ++l) {
@@ -474,12 +508,19 @@ int lg_engine::forward(const Workspace& w, int M, int Tq, PosArg pos, const floa
         LG_TRY(launch_gather_last(w.xn, R, Tq, D, dt, w.q, st));
         xlast = w.q;
     }
-    prof_begin(PC_GEMM_HEAD, st);
     GemmNext nx_first{layers[0].wqkv.p, layers[0].wqkv.bytes(3 * D, D, esz), nullptr, 0};   // the next decode step starts with layer 0
-    const int direct = gemm(w, xlast, R, V, D, output, nullptr, 0, &ks, logits_out, st, &nx_first);
+    return head(w, xlast, R, logits_out, &nx_first, st);
+}
+
+// The head GEMM over M rows of x: straight into logits_out when the plan has one slab, otherwise through the partials
+int lg_engine::head(const Workspace& w, const void* x, int M, float* logits_out, const GemmNext* next, cudaStream_t st) {
+    const int V = cfg.vocab_size;
+    int ks = 1;
+    prof_begin(PC_GEMM_HEAD, st);
+    const int direct = gemm(w, x, M, V, cfg.dim, output, nullptr, 0, &ks, logits_out, st, next);
     prof_end(st);
     if (direct < 0) return direct;
-    if (direct == 0) LG_TRY(launch_reduce_f32(w.partial, ks, R, V, logits_out, st));
+    if (direct == 0) LG_TRY(launch_reduce_f32(w.partial, ks, M, V, logits_out, st));
     return 0;
 }
 
@@ -533,6 +574,34 @@ int lg_engine::embed_cond(const Workspace& w, const void* cond, int B, int R, in
     return 0;
 }
 
+static int check_ready(lg_engine* e, int rows, int seq) {
+    LG_REQUIRE(e && e->finalized, "engine not finalized");
+    LG_REQUIRE(e->full.base, "workspace not set");
+    LG_REQUIRE(rows <= e->full.rows, "rows %d exceed workspace rows %d", rows, e->full.rows);
+    LG_REQUIRE(seq <= e->full.max_seq, "sequence %d exceeds workspace max_seq %d", seq, e->full.max_seq);
+    LG_REQUIRE(seq <= e->cfg.cls_token_num + e->cfg.block_size, "sequence %d exceeds the RoPE table (%d)", seq,
+               e->cfg.cls_token_num + e->cfg.block_size);
+    return 0;
+}
+
+// 16-bit engines: the head's logits are a bf16 / fp16 tensor in the reference (gpt.py:368 `.float()` of it); no-op for fp32
+static int round_logits_inplace(float* logits, size_t n, int dtype, cudaStream_t st);
+
+// One eager forward of R rows of Tq positions each (up to position seq) on the full workspace for the entry point fn: `embed` checks
+// fn's own arguments and writes the rows of h, then the forward writes the logits as the reference's head rounds them
+template <class Embed>
+static int eager_forward(const char* fn, lg_engine* e, int R, int Tq, int seq, PosArg pos, const float* emb_mask, int B, float* logits_out,
+                         void* stream, Embed&& embed) {
+    cudaStream_t st = (cudaStream_t)stream;
+    LG_REQUIRE(e, "%s: null engine", fn);
+    DeviceGuard guard(e->device);
+    LG_TRY(check_ready(e, R, seq));
+    LG_TRY(e->zero_fill_if_needed(st));
+    LG_TRY(embed(st));
+    LG_TRY(e->forward(e->full, R * Tq, Tq, pos, emb_mask, B, logits_out, false, st));
+    return round_logits_inplace(logits_out, (size_t)R * e->cfg.vocab_size, e->cfg.dtype, st);
+}
+
 // ---------------------------------------------------------------------------------------------------
 extern "C" {
 
@@ -555,7 +624,6 @@ int lg_engine_create(const lg_model_cfg* cfg, int device, lg_engine** out) {
     e->hd = hd;
     e->hdp = attn_kv_row_width(cfg->dtype, hd);
     e->esz = (size_t)lg_dtype_info(cfg->dtype).esz;
-    e->kv_esz = e->esz;
     const char* ng = getenv("LG_NO_GRAPH");
     e->use_graph = !(ng && ng[0] == '1');
     *out = e;
@@ -738,7 +806,6 @@ int lg_engine_set_kv_cache(lg_engine* e, int kv_dtype, const float* scales) {
     }
     // the carving and the tensor maps depend on the element size: the caller sets a new workspace
     e->kv_f8 = kv_dtype == LG_DTYPE_E4M3;
-    e->kv_esz = e->kv_f8 ? 1 : e->esz;
     e->kv_scales = sc;
     e->full = Workspace();
     e->n_sub = 0;
@@ -746,67 +813,37 @@ int lg_engine_set_kv_cache(lg_engine* e, int kv_dtype, const float* scales) {
     return 0;
 }
 
-static int check_ready(lg_engine* e, int rows, int seq) {
-    LG_REQUIRE(e && e->finalized, "engine not finalized");
-    LG_REQUIRE(e->full.base, "workspace not set");
-    LG_REQUIRE(rows <= e->full.rows, "rows %d exceed workspace rows %d", rows, e->full.rows);
-    LG_REQUIRE(seq <= e->full.max_seq, "sequence %d exceeds workspace max_seq %d", seq, e->full.max_seq);
-    LG_REQUIRE(seq <= e->cfg.cls_token_num + e->cfg.block_size, "sequence %d exceeds the RoPE table (%d)", seq,
-               e->cfg.cls_token_num + e->cfg.block_size);
-    return 0;
-}
-
-// 16-bit engines: the head's logits are a bf16 / fp16 tensor in the reference (gpt.py:368 `.float()` of it); no-op for fp32
-static int round_logits_inplace(float* logits, size_t n, int dtype, cudaStream_t st);
-
 int lg_prefill(lg_engine* e, const void* cond, const float* emb_mask, int B, int T, int use_cfg, float* logits_out,
                void* stream) {
-    cudaStream_t st = (cudaStream_t)stream;
     const int R = use_cfg ? 2 * B : B;
-    LG_REQUIRE(e, "lg_prefill: null engine");
-    DeviceGuard guard(e->device);
-    LG_TRY(check_ready(e, R, T));
-    LG_TRY(e->zero_fill_if_needed(st));
-    LG_REQUIRE(cond && logits_out && B > 0, "lg_prefill: bad argument");
-    LG_REQUIRE(T == e->cfg.cls_token_num, "lg_prefill: T=%d must equal cls_token_num=%d", T, e->cfg.cls_token_num);
-    LG_TRY(e->embed_cond(e->full, cond, B, R, T, st));
-    PosArg pos{nullptr, 0};
-    LG_TRY(e->forward(e->full, R * T, T, pos, emb_mask, B, logits_out, false, st));
-    LG_TRY(round_logits_inplace(logits_out, (size_t)R * e->cfg.vocab_size, e->cfg.dtype, st));
-    return 0;
+    auto embed = [&](cudaStream_t st) -> int {
+        LG_REQUIRE(cond && logits_out && B > 0, "lg_prefill: bad argument");
+        LG_REQUIRE(T == e->cfg.cls_token_num, "lg_prefill: T=%d must equal cls_token_num=%d", T, e->cfg.cls_token_num);
+        return e->embed_cond(e->full, cond, B, R, T, st);
+    };
+    return eager_forward("lg_prefill", e, R, T, T, PosArg{nullptr, 0}, emb_mask, B, logits_out, stream, embed);
 }
 
 int lg_decode_step(lg_engine* e, const int32_t* tokens, int B, int pos, int use_cfg, float* logits_out, void* stream) {
-    cudaStream_t st = (cudaStream_t)stream;
     const int R = use_cfg ? 2 * B : B;
-    LG_REQUIRE(e, "lg_decode_step: null engine");
-    DeviceGuard guard(e->device);
-    LG_TRY(check_ready(e, R, pos + 1));
-    LG_TRY(e->zero_fill_if_needed(st));
-    LG_REQUIRE(tokens && logits_out && B > 0 && pos >= 0, "lg_decode_step: bad argument");
-    LG_TRY(launch_embed(e->tok_emb, tokens, B, R, -1, e->cfg.dim, e->cfg.dtype, e->full.h, st));
-    PosArg p{nullptr, pos};
-    LG_TRY(e->forward(e->full, R, 1, p, nullptr, B, logits_out, false, st));
-    LG_TRY(round_logits_inplace(logits_out, (size_t)R * e->cfg.vocab_size, e->cfg.dtype, st));
-    return 0;
+    auto embed = [&](cudaStream_t st) -> int {
+        LG_REQUIRE(tokens && logits_out && B > 0 && pos >= 0, "lg_decode_step: bad argument");
+        return launch_embed(e->tok_emb, tokens, B, R, -1, e->cfg.dim, e->cfg.dtype, e->full.h, st);
+    };
+    return eager_forward("lg_decode_step", e, R, 1, pos + 1, PosArg{nullptr, pos}, nullptr, B, logits_out, stream, embed);
 }
 
 int lg_decode_rows(lg_engine* e, const int32_t* tokens, const int32_t* pos_rows, int B, int use_cfg, float* logits_out, void* stream) {
     // Iteration-level scheduling (serve/llm_engine.py:511 step()): one forward for R rows that sit at DIFFERENT depths. A row at
     // position 0 is a request that has just joined: it takes its class embedding (the c2i "prefill" is that single position).
-    cudaStream_t st = (cudaStream_t)stream;
     const int R = use_cfg ? 2 * B : B;
-    LG_REQUIRE(e, "lg_decode_rows: null engine");
-    DeviceGuard guard(e->device);
-    LG_TRY(check_ready(e, R, 1));
-    LG_TRY(e->zero_fill_if_needed(st));
-    LG_REQUIRE(tokens && pos_rows && logits_out && B > 0, "lg_decode_rows: bad argument");
-    LG_REQUIRE(e->cfg.model_type == LG_MODEL_C2I && e->cfg.cls_token_num == 1, "lg_decode_rows: class-conditional models only");
-    LG_TRY(launch_embed_rows(e->cls_table, e->tok_emb, tokens, pos_rows, B, R, e->cfg.num_classes, e->cfg.dim, e->cfg.dtype, e->full.h, st));
-    PosArg p{nullptr, 0, pos_rows};
-    LG_TRY(e->forward(e->full, R, 1, p, nullptr, B, logits_out, false, st));
-    LG_TRY(round_logits_inplace(logits_out, (size_t)R * e->cfg.vocab_size, e->cfg.dtype, st));
-    return 0;
+    auto embed = [&](cudaStream_t st) -> int {
+        LG_REQUIRE(tokens && pos_rows && logits_out && B > 0, "lg_decode_rows: bad argument");
+        LG_REQUIRE(e->cfg.model_type == LG_MODEL_C2I && e->cfg.cls_token_num == 1, "lg_decode_rows: class-conditional models only");
+        const lg_model_cfg& c = e->cfg;
+        return launch_embed_rows(e->cls_table, e->tok_emb, tokens, pos_rows, B, R, c.num_classes, c.dim, c.dtype, e->full.h, st);
+    };
+    return eager_forward("lg_decode_rows", e, R, 1, 1, PosArg{nullptr, 0, pos_rows}, nullptr, B, logits_out, stream, embed);
 }
 
 int lg_score_workspace_bytes(lg_engine* e, int rows, int seq, size_t* bytes) {
@@ -909,22 +946,11 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
 
 int lg_generate(lg_engine* e, const void* cond, const float* emb_mask, int B, int T, int S, const lg_sample_cfg* sc,
                 int32_t* out_tokens, float* dbg_logits, const int32_t* teacher, void* stream) {
-    // The loop runs on engine-owned non-blocking streams forked from / joined to the caller's stream with
-    // events: the caller's stream may be the legacy default stream (torch's default), which cannot be captured
-    // into a CUDA graph. Semantics for the caller stay "asynchronous on the given stream".
-    cudaStream_t caller = (cudaStream_t)stream;
     LG_REQUIRE(e, "lg_generate: null engine");
     DeviceGuard guard(e->device);
-    LG_TRY(e->ensure_streams());
-    LG_TRY(e->zero_fill_if_needed(caller));
-    LG_CUDA_OK(cudaEventRecord(e->ev_fork, caller));
-    for (int i = 0; i < lg_engine::kMaxChains; ++i) LG_CUDA_OK(cudaStreamWaitEvent(e->works[i], e->ev_fork, 0));
-    const int rc = generate_impl(e, cond, emb_mask, B, T, S, sc, out_tokens, dbg_logits, teacher, e->works[0]);
-    for (int i = 0; i < lg_engine::kMaxChains; ++i) {
-        cudaEventRecord(e->ev_joins[i], e->works[i]);
-        cudaStreamWaitEvent(caller, e->ev_joins[i], 0);
-    }
-    return rc;
+    return e->run_forked((cudaStream_t)stream, lg_engine::kMaxChains, [&](cudaStream_t st) {
+        return generate_impl(e, cond, emb_mask, B, T, S, sc, out_tokens, dbg_logits, teacher, st);
+    });
 }
 
 namespace {
@@ -936,9 +962,7 @@ struct Chain {
     const float* emb_mask = nullptr;
     int B = 0, R = 0;
     SampleArgs sa{};
-    cudaGraph_t graph = nullptr;
-    cudaGraphExec_t exec = nullptr;
-    uint64_t per_step = 0;
+    Graph graph;
 };
 }  // namespace
 
@@ -1029,34 +1053,10 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
     // ---- decode loop (generate.py:105-123): per chain one captured graph of one decode step (the loop state is
     // device-resident, so every step has identical kernel arguments), replayed, chains interleaved: with two chains the
     // gap between graph launches of one chain is covered by the other chain's kernels.
-    int ret = 0;
-    auto capture = [&](Chain& k, cudaGraph_t* graph, cudaGraphExec_t* exec, uint64_t* launches) -> int {
-        cudaError_t ce = cudaStreamBeginCapture(k.st, cudaStreamCaptureModeRelaxed);
-        if (ce != cudaSuccess) return lg_fail("cudaStreamBeginCapture failed: %s", cudaGetErrorString(ce));
-        const uint64_t before = g_lg_launches.load();
-        const int rc = body(k);
-        *launches = g_lg_launches.load() - before;
-        ce = cudaStreamEndCapture(k.st, graph);
-        g_lg_launches.fetch_sub(*launches);  // the capture pass launched nothing
-        if (rc < 0) return rc;
-        if (ce != cudaSuccess || !*graph) return lg_fail("stream capture failed: %s", cudaGetErrorString(ce));
-        ce = cudaGraphInstantiate(exec, *graph, 0);
-        if (ce != cudaSuccess) return lg_fail("cudaGraphInstantiate failed: %s", cudaGetErrorString(ce));
-        return 0;
-    };
-    for (int g = 0; g < nchains && ret == 0; ++g) ret = capture(ch[g], &ch[g].graph, &ch[g].exec, &ch[g].per_step);
-    for (int i = 0; i < remaining && ret == 0; ++i) {
-        for (int g = 0; g < nchains; ++g) {
-            const cudaError_t ce = cudaGraphLaunch(ch[g].exec, ch[g].st);
-            if (ce != cudaSuccess) { ret = lg_fail("cudaGraphLaunch failed: %s", cudaGetErrorString(ce)); break; }
-            g_lg_launches.fetch_add(ch[g].per_step);
-        }
-    }
-    for (int g = 0; g < nchains; ++g) {
-        if (ch[g].exec) cudaGraphExecDestroy(ch[g].exec);
-        if (ch[g].graph) cudaGraphDestroy(ch[g].graph);
-    }
-    return ret;
+    for (int g = 0; g < nchains; ++g) LG_TRY(ch[g].graph.capture(ch[g].st, [&] { return body(ch[g]); }));
+    for (int i = 0; i < remaining; ++i)
+        for (int g = 0; g < nchains; ++g) LG_TRY(ch[g].graph.launch(ch[g].st));
+    return 0;
 }
 
 int lg_sjd_workspace_bytes(lg_engine* e, int B, int use_cfg, int L, size_t* bytes) {
@@ -1089,12 +1089,7 @@ static int generate_sjd_impl(lg_engine* e, const Workspace& w, SjdArgs& sa, cons
     auto pass = [&]() -> int {
         LG_PROF(PC_EMBED_MISC, st, launch_embed(e->tok_emb, sa.win, B * L, M, -1, D, dt, w.h, st));
         LG_TRY(e->run_layers(w, M, L, PosArg{nullptr, 0, sa.pos_rows}, emb_mask, B, false, st));
-        int ks = 1;
-        prof_begin(PC_GEMM_HEAD, st);
-        const int direct = e->gemm(w, w.xn, M, V, D, e->output, nullptr, 0, &ks, w.logits, st);
-        prof_end(st);
-        if (direct < 0) return direct;
-        if (direct == 0) LG_TRY(launch_reduce_f32(w.partial, ks, M, V, w.logits, st));
+        LG_TRY(e->head(w, w.xn, M, w.logits, nullptr, st));
         LG_PROF(PC_SAMPLE, st, launch_sample(sp, st));
         LG_PROF(PC_SAMPLE, st, launch_sjd_verify(sa, st));
         LG_PROF(PC_SAMPLE, st, launch_sjd_refresh(sa, 0, st));
@@ -1106,49 +1101,22 @@ static int generate_sjd_impl(lg_engine* e, const Workspace& w, SjdArgs& sa, cons
     // image finished (a no-op: finished images are frozen). At most S - 1 passes: each one makes at least one token final.
     LG_TRY(pass());   // eagerly first: sets every kernel attribute outside capture
     LG_CUDA_OK(cudaEventRecord(e->ev_pass[0], st));
-    const bool graph = e->use_graph && !prof_enabled() && !lg_debug_sync() && S - 1 > 2;
-    cudaGraph_t g = nullptr;
-    cudaGraphExec_t exec = nullptr;
-    uint64_t per_pass = 0;
-    int ret = 0;
-    if (graph) {
-        cudaError_t ce = cudaStreamBeginCapture(st, cudaStreamCaptureModeRelaxed);
-        if (ce != cudaSuccess) return lg_fail("cudaStreamBeginCapture failed: %s", cudaGetErrorString(ce));
-        const uint64_t before = g_lg_launches.load();
-        ret = pass();
-        per_pass = g_lg_launches.load() - before;
-        ce = cudaStreamEndCapture(st, &g);
-        g_lg_launches.fetch_sub(per_pass);   // the capture pass launched nothing
-        if (ret == 0 && (ce != cudaSuccess || !g)) ret = lg_fail("stream capture failed: %s", cudaGetErrorString(ce));
-        if (ret == 0) {
-            ce = cudaGraphInstantiate(&exec, g, 0);
-            if (ce != cudaSuccess) ret = lg_fail("cudaGraphInstantiate failed: %s", cudaGetErrorString(ce));
-        }
-    }
-    for (int launched = 1; ret == 0 && launched < S - 1; ++launched) {
-        if (graph) {
-            const cudaError_t ce = cudaGraphLaunch(exec, st);
-            if (ce != cudaSuccess) { ret = lg_fail("cudaGraphLaunch failed: %s", cudaGetErrorString(ce)); break; }
-            g_lg_launches.fetch_add(per_pass);
-        } else {
-            ret = pass();
-            if (ret) break;
-        }
+    const bool use_graph = e->use_graph && !prof_enabled() && !lg_debug_sync() && S - 1 > 2;
+    Graph graph;
+    if (use_graph) LG_TRY(graph.capture(st, pass));
+    for (int launched = 1; launched < S - 1; ++launched) {
+        LG_TRY(use_graph ? graph.launch(st) : pass());
         cudaError_t ce = cudaEventRecord(e->ev_pass[launched & 1], st);
         if (ce == cudaSuccess) ce = cudaEventSynchronize(e->ev_pass[(launched - 1) & 1]);
-        if (ce != cudaSuccess) { ret = lg_fail("lg_generate_sjd: waiting for a pass failed: %s", cudaGetErrorString(ce)); break; }
+        if (ce != cudaSuccess) return lg_fail("lg_generate_sjd: waiting for a pass failed: %s", cudaGetErrorString(ce));
         if (*(volatile int*)e->sjd_done_host == sa.done_token) break;
     }
-    if (exec) cudaGraphExecDestroy(exec);
-    if (g) cudaGraphDestroy(g);
-    if (ret) return ret;
     LG_CUDA_OK(cudaMemcpyAsync(iters_out, sa.state + kSjdIters, sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
     return 0;
 }
 
 int lg_generate_sjd(lg_engine* e, const void* cond, const float* emb_mask, int B, int T, int S, const lg_sample_cfg* sc, int L,
                     void* dev_ws, size_t ws_bytes, int32_t* out_tokens, int32_t* iters_out, float* dbg_probs, void* stream) {
-    cudaStream_t caller = (cudaStream_t)stream;
     LG_REQUIRE(e && e->finalized, "lg_generate_sjd: engine not finalized");
     DeviceGuard guard(e->device);
     const lg_model_cfg& c = e->cfg;
@@ -1163,32 +1131,22 @@ int lg_generate_sjd(lg_engine* e, const void* cond, const float* emb_mask, int B
     LG_TRY(check_ready(e, R, T + S));
     LG_REQUIRE((long long)R * L <= 65535, "lg_generate_sjd: %d rows x window %d exceed 65535 query rows", R, L);
     LG_REQUIRE(dev_ws && ((uintptr_t)dev_ws & 255) == 0, "lg_generate_sjd: scratch must be non-null and 256-byte aligned");
-    Workspace scr;
+    Workspace w;   // the KV cache and its maps of the workspace, the row buffers of the scratch
     SjdArgs sa{};
-    const size_t need = e->carve_sjd(scr, sa, (char*)dev_ws, B, nh, L);
+    const size_t need = e->carve_sjd(w, sa, (char*)dev_ws, B, nh, L);
     LG_REQUIRE(ws_bytes >= need, "lg_generate_sjd: scratch of %zu bytes is too small (%zu)", ws_bytes, need);
-    Workspace w = e->full;   // the KV cache and its maps of the workspace, everything else from the scratch
-    w.h = scr.h; w.xn = scr.xn; w.q = scr.q; w.attn = scr.attn; w.ff = scr.ff; w.x0 = nullptr;
-    w.partial = scr.partial; w.partial_floats = scr.partial_floats; w.logits = scr.logits;
-    w.tokens = nullptr; w.counters = nullptr;
+    static_cast<KvCache&>(w) = e->full;
     sa.B = B; sa.S = S; sa.L = L; sa.V = c.vocab_size; sa.T = T; sa.nh = nh;
     sa.greedy = sc->greedy; sa.seed = sc->seed; sa.row_offset = 0;
     sa.out = out_tokens; sa.dbg = dbg_probs;
-    LG_TRY(e->ensure_streams());
     if (!e->sjd_done_host) {
         LG_CUDA_OK(cudaHostAlloc((void**)&e->sjd_done_host, sizeof(int), cudaHostAllocDefault));
         *e->sjd_done_host = 0;
         for (cudaEvent_t& ev : e->ev_pass) LG_CUDA_OK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
     }
-    // on an engine-owned stream, as lg_generate: the caller's stream may be the legacy default stream, which cannot be captured
-    cudaStream_t st = e->works[0];
-    LG_TRY(e->zero_fill_if_needed(caller));
-    LG_CUDA_OK(cudaEventRecord(e->ev_fork, caller));
-    LG_CUDA_OK(cudaStreamWaitEvent(st, e->ev_fork, 0));
-    const int rc = generate_sjd_impl(e, w, sa, cond, emb_mask, *sc, use_cfg, iters_out, st);
-    cudaEventRecord(e->ev_joins[0], st);
-    cudaStreamWaitEvent(caller, e->ev_joins[0], 0);
-    return rc;
+    return e->run_forked((cudaStream_t)stream, 1, [&](cudaStream_t st) {
+        return generate_sjd_impl(e, w, sa, cond, emb_mask, *sc, use_cfg, iters_out, st);
+    });
 }
 
 int lg_test_sjd_verify(int B, int S, int L, int V, int greedy, uint64_t seed, const float* p, const float* q, const int32_t* qflag,

@@ -350,15 +350,25 @@ class Transformer(nn.Module):
             nbytes = ctypes.c_size_t()
             _lib.check(lib.lg_engine_workspace_bytes(handle, max_batch_size, max_seq_length, ctypes.byref(nbytes)),
                        "lg_engine_workspace_bytes")
-            dev = self.tok_embeddings.weight.device
-            self._workspace = None
-            self._workspace = torch.empty(nbytes.value + 256, dtype=torch.uint8, device=dev)
-            base = (self._workspace.data_ptr() + 255) // 256 * 256
-            _lib.check(lib.lg_engine_set_workspace(handle, ctypes.c_void_p(base), nbytes.value, max_batch_size,
+            base, _ = self._device_buffer("_workspace", nbytes.value, grow=True)
+            _lib.check(lib.lg_engine_set_workspace(handle, base, nbytes.value, max_batch_size,
                                                    max_seq_length), "lg_engine_set_workspace")
             self._ws_shape = (max_batch_size, max_seq_length)
         self.max_batch_size = max_batch_size
         self.max_seq_length = max_seq_length
+
+    def _device_buffer(self, attr: str, nbytes: int, grow: bool = False):
+        """The torch byte buffer self.<attr> with room for nbytes from a 256-byte aligned address (the engine's alignment), kept
+        while it is on the model's device and large enough unless `grow`; the old buffer is dropped before the new one is allocated.
+        Returns (aligned device pointer, usable bytes)."""
+        dev = self.tok_embeddings.weight.device
+        buf = getattr(self, attr)
+        if grow or buf is None or buf.numel() < nbytes + 256 or buf.device != dev:
+            setattr(self, attr, None)
+            buf = torch.empty(nbytes + 256, dtype=torch.uint8, device=dev)
+            setattr(self, attr, buf)
+        base = (buf.data_ptr() + 255) // 256 * 256
+        return ctypes.c_void_p(base), buf.numel() - (base - buf.data_ptr())
 
     # ------------------------------------------------------------------ teacher-forced scoring (lg_score)
     def _score_scratch(self, rows: int, seq: int, nh: int):
@@ -368,13 +378,7 @@ class Transformer(nn.Module):
         need, one = ctypes.c_size_t(), ctypes.c_size_t()
         _lib.check(lib.lg_score_workspace_bytes(handle, rows, seq, ctypes.byref(need)), "lg_score_workspace_bytes")
         _lib.check(lib.lg_score_workspace_bytes(handle, nh, seq, ctypes.byref(one)), "lg_score_workspace_bytes")
-        nbytes = need.value if need.value <= SCORE_SCRATCH_CAP else max(SCORE_SCRATCH_CAP, one.value)
-        dev = self.tok_embeddings.weight.device
-        if self._score_ws is None or self._score_ws.numel() < nbytes + 256 or self._score_ws.device != dev:
-            self._score_ws = None
-            self._score_ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=dev)
-        base = (self._score_ws.data_ptr() + 255) // 256 * 256
-        return ctypes.c_void_p(base), self._score_ws.numel() - (base - self._score_ws.data_ptr())
+        return self._device_buffer("_score_ws", need.value if need.value <= SCORE_SCRATCH_CAP else max(SCORE_SCRATCH_CAP, one.value))
 
     def _sjd_scratch(self, B: int, use_cfg: bool, L: int):
         """The lg_generate_sjd scratch for B images and window L, kept on the model like the setup_caches() workspace.
@@ -382,12 +386,7 @@ class Transformer(nn.Module):
         lib, handle = _lib.load(), self.engine()
         need = ctypes.c_size_t()
         _lib.check(lib.lg_sjd_workspace_bytes(handle, B, int(use_cfg), L, ctypes.byref(need)), "lg_sjd_workspace_bytes")
-        dev = self.tok_embeddings.weight.device
-        if self._sjd_ws is None or self._sjd_ws.numel() < need.value + 256 or self._sjd_ws.device != dev:
-            self._sjd_ws = None
-            self._sjd_ws = torch.empty(need.value + 256, dtype=torch.uint8, device=dev)
-        base = (self._sjd_ws.data_ptr() + 255) // 256 * 256
-        return ctypes.c_void_p(base), self._sjd_ws.numel() - (base - self._sjd_ws.data_ptr())
+        return self._device_buffer("_sjd_ws", need.value)
 
     def _score(self, cond, idx, targets, emb_masks, cfg_scale: float, want_logits: bool, want_nll: bool):
         """lg_score over complete sequences: cond (c2i labels [B] / t2i features [B, T, C]), idx [B, S-1] or None (S = 1),
