@@ -151,6 +151,24 @@ int  lg_generate(lg_engine* e, const void* cond, const float* emb_mask, int B, i
                  const lg_sample_cfg* sc, int32_t* out_tokens, float* dbg_logits,
                  const int32_t* teacher, void* stream);
 
+/* ---- image completion: generate() after a given prefix of every image's tokens ---------------------------------------------- */
+/* Bytes of caller-provided scratch for lg_generate_prefix's prefill of `rows` rows (2 per image under CFG) of `seq` = T + P positions. */
+int  lg_prefix_workspace_bytes(lg_engine* e, int rows, int seq, size_t* bytes);
+/* generate() that continues given images: token indices 0 .. P - 1 of image b are prefix[b, 0 .. P - 1] (dev int32 [B, P],
+ * 1 <= P <= S - 1) and are copied to out_tokens[b, 0 .. P - 1]. Positions 0 .. T + P - 1 (the condition as lg_prefill embeds it, with
+ * the null condition for CFG rows and emb_mask as in lg_prefill, then the prefix embeddings) are written into the KV cache of
+ * lg_engine_set_workspace in one forward pass, not P decode steps. Token P is sampled from the logits of position T + P - 1 with step
+ * P; decoding then continues at position T + P with steps P + 1 .. S - 1 exactly as in lg_generate (graph, fused tail, chains). Token
+ * k >= P is drawn with lg_generate's RNG key and cfg_interval rule for index k. dbg_logits: NULL or dev f32 [S, B, V]; rows k >= P
+ * are written, rows k < P are left as they are. The prefix ids must lie in [0, vocab_size): they index the token embedding table on
+ * the device unchecked (generate(prefix=...) checks them on the host). The workspace needs rows >= R and max_seq >= T + S, as for
+ * lg_generate. dev_ws
+ * (256-byte aligned, at least lg_prefix_workspace_bytes of one image's rows) holds the prefill's activations only; the prefill runs
+ * in chunks of cache rows that fit ws_bytes and the attention grid. */
+int  lg_generate_prefix(lg_engine* e, const void* cond, const float* emb_mask, int B, int T, int S, const lg_sample_cfg* sc,
+                        const int32_t* prefix, int P, void* dev_ws, size_t ws_bytes, int32_t* out_tokens, float* dbg_logits,
+                        void* stream);
+
 /* ---- teacher-forced scoring: Transformer.forward(idx, cond_idx, targets) (gpt.py:341-382, eval mode) ----------------------- */
 /* Bytes of caller-provided scratch for lg_score over `rows` sequences (rows = 2B under CFG) of `seq` positions (T + S - 1). */
 int  lg_score_workspace_bytes(lg_engine* e, int rows, int seq, size_t* bytes);
@@ -316,6 +334,9 @@ int  lg_test_attention(int dtype, int kv_dtype, float k_scale, float v_scale, in
 int  lg_test_attention_plan(int dtype, int kv_dtype, int R, int Tq, int H, int hd, int hdp, int max_seq, int n_layer, int pos_kind,
                             int pos_value, int input, int* plan);
 
+/* Chunks the prefill of the engine's last lg_generate_prefix call ran in (over all chains); -1 for a null engine. chains: NULL or
+ * receives the number of decode chains that call ran (1, or 2 under a multi-chain split). */
+int  lg_test_prefix_chunks(lg_engine* e, int* chains);
 /* The acceptance step of lg_generate_sjd alone, on caller buffers (dev): p, q f32 [B * L][V], qflag, x, win int32 [B * L], nfin,
  * start int32 [B] (updated), out int32 [B][S] (accepted tokens written). Every image must have nfin < S. */
 int  lg_test_sjd_verify(int B, int S, int L, int V, int greedy, uint64_t seed, const float* p, const float* q, const int32_t* qflag,

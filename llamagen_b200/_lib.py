@@ -71,6 +71,10 @@ SIGNATURES = {
                           c_void_p, c_void_p]),
     "lg_generate": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p,
                             c_void_p, c_void_p, c_void_p]),
+    "lg_prefix_workspace_bytes": (c_int, [c_void_p, c_int, c_int, POINTER(c_size_t)]),
+    "lg_generate_prefix": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p, c_int, c_void_p,
+                                   c_size_t, c_void_p, c_void_p, c_void_p]),
+    "lg_test_prefix_chunks": (c_int, [c_void_p, POINTER(c_int)]),
     "lg_score_workspace_bytes": (c_int, [c_void_p, c_int, c_int, POINTER(c_size_t)]),
     "lg_score": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_size_t,
                          c_void_p, c_void_p, c_void_p]),

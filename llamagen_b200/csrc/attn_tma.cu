@@ -676,6 +676,11 @@ __global__ void __launch_bounds__(256, 2) attn_prefill_tc_kernel(const __grid_co
 // S = Q K^T and O += P V run on mma.sync m16n8k16 with ldmatrix operands, the softmax is online in fp32 registers and P is reused
 // from the score fragments (FlashAttention-2). Q comes straight from global memory into A fragments (rows of 64, 128 or the 100
 // dims of GPT-3B, whose K / V rows are 112 wide: the maps read dims 112..127 as zeros). No R * Tq grid limit.
+//
+// F8 = true: fp8 e4m3 cache (kernel 2 only: attn_causal_tc_f8_kernel). A stage holds [kCqKeys keys][64 or 128 bytes] (one box covers
+// a whole row, 64-byte swizzle for hd 64, 128-byte otherwise) and the B operands are decoded in registers as in attn_tma_kernel<..,
+// F8>: q.K^T visits the head dims in the f8_qdim order (Q's A fragments are read in that order), P.V transposes key bytes with prmt
+// and leaves the output dims permuted (put back in the store). The K scale is in a.scale, the V scale multiplies O / L.
 // ---------------------------------------------------------------------------------------------------
 constexpr int kCqRows = 64;       // query rows per CTA
 constexpr int kCqKeys = 64;       // keys per ring stage
@@ -684,10 +689,12 @@ constexpr int kCqStages = 2;
 //
 // The speculative (Jacobi) decoding window runs the same body with a per-row start (attn_window_tc_kernel): row r's Tq <= kCqRows
 // queries sit at positions a.pos_rows[r] + t and attend keys [0, a.pos_rows[r] + t]; q and out stay [R * Tq, D].
-template <typename T, int HD, bool WINDOW>
-__device__ __forceinline__ void causal_tc_body(const CUtensorMap& kmap, const CUtensorMap& vmap, const AttnTmaArgs& a, int Tq) {
-    constexpr int NSUB = HD / 64;
-    constexpr int SUB_BYTES = kCqKeys * 128;      // [kCqKeys keys][64 dims], 128-byte swizzle
+template <typename T, int HD, bool WINDOW, bool F8 = false>
+__device__ __forceinline__ void causal_tc_body(const CUtensorMap& kmap, const CUtensorMap& vmap, const AttnTmaArgs& a, int Tq,
+                                               KvScales f8s = KvScales{1.f, 1.f, 1.f}) {
+    constexpr int RB = F8 ? (HD == 64 ? 64 : 128) : 128;   // bytes per tile row of one box
+    constexpr int NSUB = F8 ? 1 : HD / 64;        // 64-dim sub-tiles per row (fp8: one box covers the whole row)
+    constexpr int SUB_BYTES = kCqKeys * RB;       // [kCqKeys keys][64 dims] 16-bit, 128-byte swizzle (fp8: [kCqKeys][RB bytes])
     constexpr int TILE_BYTES = NSUB * SUB_BYTES;
     constexpr int NT = kCqKeys / 8;               // n8 score tiles per stage
     extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -722,8 +729,8 @@ __device__ __forceinline__ void causal_tc_body(const CUtensorMap& kmap, const CU
 #pragma unroll
             for (int i = 0; i < kCqKeys / kKC; ++i) {
                 const int row = (int)(row0 + (long long)kb * kCqKeys + i * kKC);
-                load_2d(kt + sub * SUB_BYTES + i * kKC * 128, &kmap, &full_bar[s], sub * 64, row);
-                load_2d(vt + sub * SUB_BYTES + i * kKC * 128, &vmap, &full_bar[s], sub * 64, row);
+                load_2d(kt + sub * SUB_BYTES + i * kKC * RB, &kmap, &full_bar[s], sub * 64, row);
+                load_2d(vt + sub * SUB_BYTES + i * kKC * RB, &vmap, &full_bar[s], sub * 64, row);
             }
     };
     if (threadIdx.x == 0)
@@ -739,7 +746,8 @@ __device__ __forceinline__ void causal_tc_body(const CUtensorMap& kmap, const CU
         const T* r1p = qp + ((size_t)r * Tq + t1) * D;
 #pragma unroll
         for (int kk = 0; kk < HD / 16; ++kk) {
-            const int d0 = kk * 16 + tg * 2, d1 = d0 + 8;
+            // fp8: the k16 step's pairs are dims d, d + 1 (a0 / a1) and d + 2, d + 3 (a2 / a3) of f8_qdim, all real or all padding
+            const int d0 = F8 ? f8_qdim<HD>(tg, kk) : kk * 16 + tg * 2, d1 = F8 ? d0 + 2 : d0 + 8;
             qa[kk][0] = (t0 < Tq && d0 < hdr) ? *reinterpret_cast<const uint32_t*>(r0p + d0) : 0u;
             qa[kk][1] = (t1 < Tq && d0 < hdr) ? *reinterpret_cast<const uint32_t*>(r1p + d0) : 0u;
             qa[kk][2] = (t0 < Tq && d1 < hdr) ? *reinterpret_cast<const uint32_t*>(r0p + d1) : 0u;
@@ -762,15 +770,33 @@ __device__ __forceinline__ void causal_tc_body(const CUtensorMap& kmap, const CU
             float sc[NT][4];
 #pragma unroll
             for (int i = 0; i < NT; ++i) { sc[i][0] = 0.f; sc[i][1] = 0.f; sc[i][2] = 0.f; sc[i][3] = 0.f; }
+            if constexpr (F8) {
+                // key nt * 8 + g of n8 tile nt: 16 dims (4 k16 steps) per 16-byte chunk f8_kchunk of each 64-dim block
+                const uint8_t* ktp = tiles + s * 2 * TILE_BYTES;
 #pragma unroll
-            for (int kk = 0; kk < HD / 16; ++kk) {
+                for (int nt = 0; nt < NT; ++nt) {
 #pragma unroll
-                for (int np = 0; np < NT / 2; ++np) {
-                    uint32_t b0, b1, b2, b3;
-                    const int row = np * 16 + (lane & 7) + ((lane >> 4) << 3);
-                    ldsm_x4(kt + (kk / 4) * SUB_BYTES + swz(row, (kk * 2 + ((lane >> 3) & 1)) & 7), b0, b1, b2, b3);
-                    mma16816<T>(sc[2 * np], qa[kk][0], qa[kk][1], qa[kk][2], qa[kk][3], b0, b1);
-                    mma16816<T>(sc[2 * np + 1], qa[kk][0], qa[kk][1], qa[kk][2], qa[kk][3], b2, b3);
+                    for (int j = 0; j < HD / 64; ++j) {
+                        const uint4 kw = *reinterpret_cast<const uint4*>(ktp + swz8<RB>(nt * 8 + g, f8_kchunk<HD>(tg, j)));
+                        const uint32_t w[4] = {kw.x, kw.y, kw.z, kw.w};
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) {
+                            const int kk = j * 4 + i;
+                            mma16816<T>(sc[nt], qa[kk][0], qa[kk][1], qa[kk][2], qa[kk][3], e4m3x2_to<T>(w[i]), e4m3x2_to<T>(w[i] >> 16));
+                        }
+                    }
+                }
+            } else {
+#pragma unroll
+                for (int kk = 0; kk < HD / 16; ++kk) {
+#pragma unroll
+                    for (int np = 0; np < NT / 2; ++np) {
+                        uint32_t b0, b1, b2, b3;
+                        const int row = np * 16 + (lane & 7) + ((lane >> 4) << 3);
+                        ldsm_x4(kt + (kk / 4) * SUB_BYTES + swz(row, (kk * 2 + ((lane >> 3) & 1)) & 7), b0, b1, b2, b3);
+                        mma16816<T>(sc[2 * np], qa[kk][0], qa[kk][1], qa[kk][2], qa[kk][3], b0, b1);
+                        mma16816<T>(sc[2 * np + 1], qa[kk][0], qa[kk][1], qa[kk][2], qa[kk][3], b2, b3);
+                    }
                 }
             }
             // ---- mask + online softmax; values [..][0..1] belong to row t0, [..][2..3] to row t1
@@ -815,13 +841,43 @@ __device__ __forceinline__ void causal_tc_body(const CUtensorMap& kmap, const CU
                 const uint32_t pa0 = pack16<T>(sc[2 * kb16][0], sc[2 * kb16][1]), pa1 = pack16<T>(sc[2 * kb16][2], sc[2 * kb16][3]);
                 const uint32_t pa2 = pack16<T>(sc[2 * kb16 + 1][0], sc[2 * kb16 + 1][1]);
                 const uint32_t pa3 = pack16<T>(sc[2 * kb16 + 1][2], sc[2 * kb16 + 1][3]);
+                if constexpr (F8) {
+                    // n8 tile i, column n <-> head dim DPT * n + i; the lane reads DPT bytes (dims DPT * g ..) of keys 2tg, 2tg + 1,
+                    // + 8, + 9 (odd tg swap the rows of a pair so a half warp hits distinct banks), prmt pairs the keys' bytes
+                    constexpr int DPT = HD / 8, NWD = DPT / 4;
+                    const uint8_t* vtp = tiles + s * 2 * TILE_BYTES + TILE_BYTES;
+                    const int sw = tg & 1, rb = kb16 * 16 + 2 * tg;
+                    uint32_t w[4][NWD];
 #pragma unroll
-                for (int np = 0; np < HD / 16; ++np) {
-                    uint32_t b0, b1, b2, b3;
-                    const int row = kb16 * 16 + (lane & 7) + (((lane >> 3) & 1) << 3);
-                    ldsm_x4_t(vt + (np / 4) * SUB_BYTES + swz(row, (np * 2 + (lane >> 4)) & 7), b0, b1, b2, b3);
-                    mma16816<T>(o[2 * np], pa0, pa1, pa2, pa3, b0, b1);
-                    mma16816<T>(o[2 * np + 1], pa0, pa1, pa2, pa3, b2, b3);
+                    for (int q = 0; q < 4; ++q) {
+                        const int row = rb + (q >> 1) * 8 + ((q & 1) ^ sw);
+                        if constexpr (RB == 64) {
+                            const uint2 u = *reinterpret_cast<const uint2*>(vtp + swz8<RB>(row, g >> 1) + (g & 1) * 8);
+                            w[q][0] = u.x; w[q][NWD - 1] = u.y;
+                        } else {
+                            const uint4 u = *reinterpret_cast<const uint4*>(vtp + swz8<RB>(row, g));
+                            w[q][0] = u.x; w[q][1 % NWD] = u.y; w[q][2 % NWD] = u.z; w[q][3 % NWD] = u.w;
+                        }
+                    }
+                    const uint32_t sel_lo = sw ? 0x1504u : 0x5140u, sel_hi = sw ? 0x3726u : 0x7362u;
+#pragma unroll
+                    for (int wd = 0; wd < NWD; ++wd) {
+                        const uint32_t x01 = __byte_perm(w[0][wd], w[1][wd], sel_lo), x23 = __byte_perm(w[0][wd], w[1][wd], sel_hi);
+                        const uint32_t y01 = __byte_perm(w[2][wd], w[3][wd], sel_lo), y23 = __byte_perm(w[2][wd], w[3][wd], sel_hi);
+                        mma16816<T>(o[4 * wd + 0], pa0, pa1, pa2, pa3, e4m3x2_to<T>(x01), e4m3x2_to<T>(y01));
+                        mma16816<T>(o[4 * wd + 1], pa0, pa1, pa2, pa3, e4m3x2_to<T>(x01 >> 16), e4m3x2_to<T>(y01 >> 16));
+                        mma16816<T>(o[4 * wd + 2], pa0, pa1, pa2, pa3, e4m3x2_to<T>(x23), e4m3x2_to<T>(y23));
+                        mma16816<T>(o[4 * wd + 3], pa0, pa1, pa2, pa3, e4m3x2_to<T>(x23 >> 16), e4m3x2_to<T>(y23 >> 16));
+                    }
+                } else {
+#pragma unroll
+                    for (int np = 0; np < HD / 16; ++np) {
+                        uint32_t b0, b1, b2, b3;
+                        const int row = kb16 * 16 + (lane & 7) + (((lane >> 3) & 1) << 3);
+                        ldsm_x4_t(vt + (np / 4) * SUB_BYTES + swz(row, (np * 2 + (lane >> 4)) & 7), b0, b1, b2, b3);
+                        mma16816<T>(o[2 * np], pa0, pa1, pa2, pa3, b0, b1);
+                        mma16816<T>(o[2 * np + 1], pa0, pa1, pa2, pa3, b2, b3);
+                    }
                 }
             }
         }
@@ -839,9 +895,21 @@ __device__ __forceinline__ void causal_tc_body(const CUtensorMap& kmap, const CU
         if (t < Tq) {
             const float inv = 1.0f / l[hh];          // the diagonal key is always visible: l > 0
             T* op = reinterpret_cast<T*>(a.out) + ((size_t)r * Tq + t) * D + (size_t)h * hdr;
+            if constexpr (F8) {   // o[i][2hh] -> dim DPT * 2tg + i, o[i][2hh + 1] -> dim DPT * (2tg + 1) + i (O / L * v_scale)
+                constexpr int DPT = HD / 8;
+                const float f = inv * f8s.v_scale;
 #pragma unroll
-            for (int i = 0; i < HD / 8; ++i)
-                if (i * 8 + tg * 2 < hdr) *reinterpret_cast<uint32_t*>(op + i * 8 + tg * 2) = pack16<T>(o[i][2 * hh] * inv, o[i][2 * hh + 1] * inv);
+                for (int i = 0; i < DPT; i += 2)
+#pragma unroll
+                    for (int c = 0; c < 2; ++c) {
+                        const int d = DPT * (2 * tg + c) + i;
+                        if (d < hdr) *reinterpret_cast<uint32_t*>(op + d) = pack16<T>(o[i][2 * hh + c] * f, o[i + 1][2 * hh + c] * f);
+                    }
+            } else {
+#pragma unroll
+                for (int i = 0; i < HD / 8; ++i)
+                    if (i * 8 + tg * 2 < hdr) *reinterpret_cast<uint32_t*>(op + i * 8 + tg * 2) = pack16<T>(o[i][2 * hh] * inv, o[i][2 * hh + 1] * inv);
+            }
         }
     }
 }
@@ -850,6 +918,15 @@ template <typename T, int HD>
 __global__ void __launch_bounds__(128) attn_causal_tc_kernel(const __grid_constant__ CUtensorMap kmap,
                                                              const __grid_constant__ CUtensorMap vmap, AttnTmaArgs a, int Tq) {
     causal_tc_body<T, HD, false>(kmap, vmap, a, Tq);
+}
+
+// kernel 2 over an fp8 cache: the same body with F8 = true; the scales are a separate last argument so that the 16-bit kernel above
+// keeps its argument layout and its code
+template <typename T, int HD>
+__global__ void __launch_bounds__(128) attn_causal_tc_f8_kernel(const __grid_constant__ CUtensorMap kmap,
+                                                                const __grid_constant__ CUtensorMap vmap, AttnTmaArgs a, int Tq,
+                                                                KvScales f8s) {
+    causal_tc_body<T, HD, false, true>(kmap, vmap, a, Tq, f8s);
 }
 
 template <typename T, int HD>
@@ -893,8 +970,8 @@ AttnPlan attn_plan(const AttnArgs& a) {
     if (tma && !fused && a.hd == 64 && (a.hdp == 0 || a.hdp == 64) && a.Tq > 1 && a.Tq <= kPfRows && from0 && a.maxS >= kPfBoxes * kKC &&
         lg_env_flag("LG_ATTN_PREFILL_TC", 1))
         return plan(3, 1);
-    const bool tc16 = tma && !fused && !a.kv_f8;   // kernels 2 and 4: a 16-bit cache in the model dtype
-    if (tc16 && a.Tq > kPfRows && from0 && a.maxS >= a.Tq) return plan(2, kCqStages);
+    if (tma && !fused && a.Tq > kPfRows && from0 && a.maxS >= a.Tq) return plan(2, kCqStages);   // kernel 2 reads fp8 caches too
+    const bool tc16 = tma && !fused && !a.kv_f8;   // kernel 4: a 16-bit cache in the model dtype
     if (tc16 && a.Tq >= 2 && a.Tq <= kCqRows && a.pos.rows) return plan(4, kCqStages);
     if (fused) snprintf(p.error, sizeof(p.error), "attention: fused QKV epilogue requested on a path that does not support it");
     else if ((long long)a.R * a.Tq > 65535) snprintf(p.error, sizeof(p.error), "attention: too many query rows (%d x %d)", a.R, a.Tq);
@@ -933,16 +1010,14 @@ static int launch_prefill_tc(const AttnArgs& a, cudaStream_t st) {
     return 0;
 }
 
-// window = true: attn_window_tc_kernel (one query block per row, at the row's own position), else attn_causal_tc_kernel
-static int launch_causal_tc(const AttnArgs& a, cudaStream_t st, bool window) {
+// attn_window_tc_kernel (one query block per row, at the row's own position; caches in the model dtype)
+static int launch_window_tc(const AttnArgs& a, cudaStream_t st) {
     const bool half = a.dtype == LG_DTYPE_F16, wide = a.hd != 64;
-    auto kern = window ? (wide ? (half ? attn_window_tc_kernel<f16, 128> : attn_window_tc_kernel<bf16, 128>)
-                               : (half ? attn_window_tc_kernel<f16, 64> : attn_window_tc_kernel<bf16, 64>))
-                       : (wide ? (half ? attn_causal_tc_kernel<f16, 128> : attn_causal_tc_kernel<bf16, 128>)
-                               : (half ? attn_causal_tc_kernel<f16, 64> : attn_causal_tc_kernel<bf16, 64>));
+    auto kern = wide ? (half ? attn_window_tc_kernel<f16, 128> : attn_window_tc_kernel<bf16, 128>)
+                     : (half ? attn_window_tc_kernel<f16, 64> : attn_window_tc_kernel<bf16, 64>);
     const size_t smem = 1024 + (size_t)kCqStages * 2 * (wide ? 2 : 1) * kCqKeys * 128 + kCqStages * sizeof(uint64_t);
-    static DevOnce attr[8];
-    if (lg_first_on_device(attr[(half ? 1 : 0) + (wide ? 2 : 0) + (window ? 4 : 0)])) {
+    static DevOnce attr[4];
+    if (lg_first_on_device(attr[(half ? 1 : 0) + (wide ? 2 : 0)])) {
         LG_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
     dim3 grid(a.H, a.R, (a.Tq + kCqRows - 1) / kCqRows);
@@ -952,15 +1027,44 @@ static int launch_causal_tc(const AttnArgs& a, cudaStream_t st, bool window) {
     return 0;
 }
 
+// attn_causal_tc_kernel (attn_causal_tc_f8_kernel for an fp8 cache) at the call's dtype and head dim
+template <typename T, int HD, bool F8>
+static int launch_causal_t(const AttnArgs& a, cudaStream_t st) {
+    constexpr int TILE_BYTES = F8 ? kCqKeys * (HD == 64 ? 64 : 128) : (HD / 64) * kCqKeys * 128;
+    const size_t smem = 1024 + (size_t)kCqStages * 2 * TILE_BYTES + kCqStages * sizeof(uint64_t);
+    static DevOnce attr;
+    const auto& kmap = *reinterpret_cast<const CUtensorMap*>(a.kmap);
+    const auto& vmap = *reinterpret_cast<const CUtensorMap*>(a.vmap);
+    dim3 grid(a.H, a.R, (a.Tq + kCqRows - 1) / kCqRows);
+    if constexpr (F8) {
+        if (lg_first_on_device(attr))
+            LG_CUDA_OK(cudaFuncSetAttribute(attn_causal_tc_f8_kernel<T, HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        (void)lg_launch(attn_causal_tc_f8_kernel<T, HD>, dim3(grid), dim3(128), smem, st, kmap, vmap, tma_args(a), a.Tq,
+                        KvScales{a.k_inv, a.v_inv, a.v_scale});
+    } else {
+        if (lg_first_on_device(attr))
+            LG_CUDA_OK(cudaFuncSetAttribute(attn_causal_tc_kernel<T, HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        (void)lg_launch(attn_causal_tc_kernel<T, HD>, dim3(grid), dim3(128), smem, st, kmap, vmap, tma_args(a), a.Tq);
+    }
+    LG_LAUNCH_CHECK();
+    return 0;
+}
+
+template <typename T>
+static int launch_causal_tc(const AttnArgs& a, cudaStream_t st) {
+    if (a.hd == 64) return a.kv_f8 ? launch_causal_t<T, 64, true>(a, st) : launch_causal_t<T, 64, false>(a, st);
+    return a.kv_f8 ? launch_causal_t<T, 128, true>(a, st) : launch_causal_t<T, 128, false>(a, st);
+}
+
 int launch_attention_tma(const AttnArgs& a, const AttnPlan& p, cudaStream_t st) {
     const bool half = a.dtype == LG_DTYPE_F16;
     switch (p.kernel) {
         case 1:
             if (a.kv_f8) return half ? launch_decode<f16, true>(a, p, st) : launch_decode<bf16, true>(a, p, st);
             return half ? launch_decode<f16, false>(a, p, st) : launch_decode<bf16, false>(a, p, st);
-        case 2: return launch_causal_tc(a, st, false);
+        case 2: return half ? launch_causal_tc<f16>(a, st) : launch_causal_tc<bf16>(a, st);
         case 3: return launch_prefill_tc(a, st);
-        case 4: return launch_causal_tc(a, st, true);
+        case 4: return launch_window_tc(a, st);
     }
     return lg_fail("attention: kernel %d is not one of the TMA kernels", p.kernel);
 }

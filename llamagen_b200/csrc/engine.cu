@@ -123,11 +123,12 @@ int make_kv_maps(KvMaps& m, int dtype, int hd, int hdp, int kv_dtype, const void
 
 // One attention call over layer `layer` of a K / V cache pair laid out [layer][rows, H, max_seq, hdp] (DESIGN §3): the geometry, the
 // softmax scale with an fp8 cache's scales folded in (kv_scales: this layer's {K, V} scales, null for a cache in the model dtype) and
-// the tensor maps over the whole pair. The caller sets q, out, the positions and the emb-mask.
+// the tensor maps over the whole pair. The call's row r is cache row first_row + r: the cache pointers and the maps' first row move
+// alike. The caller sets q, out, the positions and the emb-mask.
 AttnArgs make_attn_args(int dtype, int H, int hd, int hdp, int rows, int max_seq, char* kcache, char* vcache, const KvMaps& maps,
-                        const float* kv_scales, int layer, int R, int Tq) {
+                        const float* kv_scales, int layer, int R, int Tq, int first_row = 0) {
     AttnArgs aa{};
-    const long long row0 = (long long)layer * rows * H * max_seq;
+    const long long row0 = ((long long)layer * rows + first_row) * H * max_seq;
     const size_t row_bytes = (size_t)hdp * (kv_scales ? 1 : lg_dtype_info(dtype).esz);
     aa.kcache = kcache + (size_t)row0 * row_bytes; aa.vcache = vcache + (size_t)row0 * row_bytes;
     aa.R = R; aa.Tq = Tq; aa.H = H; aa.hd = hd; aa.hdp = hdp; aa.maxS = max_seq; aa.dtype = dtype;
@@ -173,6 +174,7 @@ struct KvCache {
     int rows = 0, max_seq = 0;
     int layers = 0;           // n_layer, or 1 for a cache that every layer rewrites before its attention reads it
     bool kv_f8 = false;       // e4m3 with the engine's per-layer scales, else the model dtype
+    int first_row = 0;        // attention row 0 of a forward through this view is this cache row (a chunk of a prefix prefill)
     KvMaps maps;
 };
 
@@ -273,6 +275,9 @@ struct lg_engine {
     bool ws_needs_zero = false;           // KV cache + counters of `full` still have to be zero-filled (done on the caller's stream)
     cudaStream_t works[kMaxChains] = {};   // engine-owned streams (one per chain)
     cudaEvent_t ev_fork = nullptr, ev_joins[kMaxChains] = {};
+    cudaEvent_t ev_prefill = nullptr;     // lg_generate_prefix: every chain's prefill (one scratch) is done
+    int prefix_chunks = 0;                // chunks the last lg_generate_prefix ran its prefill in (lg_test_prefix_chunks)
+    int prefix_chains = 0;                // decode chains of that call
     int* sjd_done_host = nullptr;         // pinned copy of lg_generate_sjd's done flag
     cudaEvent_t ev_pass[2] = {};
     ~lg_engine() {
@@ -281,6 +286,7 @@ struct lg_engine {
             if (ev_joins[i]) cudaEventDestroy(ev_joins[i]);
         }
         if (ev_fork) cudaEventDestroy(ev_fork);
+        if (ev_prefill) cudaEventDestroy(ev_prefill);
         for (cudaEvent_t ev : ev_pass)
             if (ev) cudaEventDestroy(ev);
         if (sjd_done_host) cudaFreeHost(sjd_done_host);
@@ -297,6 +303,7 @@ struct lg_engine {
             LG_CUDA_OK(cudaEventCreateWithFlags(&ev_joins[i], cudaEventDisableTiming));
         }
         LG_CUDA_OK(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
+        LG_CUDA_OK(cudaEventCreateWithFlags(&ev_prefill, cudaEventDisableTiming));
         return 0;
     }
     // Runs body(works[0]) with works[0..n) forked from and joined to the caller's stream by events: the caller's stream may be the
@@ -332,6 +339,7 @@ struct lg_engine {
     size_t carve(Workspace& o, char* base, int rows, int max_seq, int g = 0, int n = 1) const;
     size_t carve_score(Workspace& o, char* base, int rows, int seq) const;
     size_t carve_sjd(RowBuffers& o, SjdArgs& sa, char* base, int B, int nh, int L) const;
+    size_t carve_prefix(RowBuffers& o, char* base, int rows, int seq) const;
     void carve_kv(Carver& c, KvCache& o, int rows, int max_seq, int layers, bool f8) const;
     void carve_rows(Carver& c, RowBuffers& o, size_t M, size_t x0_rows, size_t partial_floats, size_t logits_rows) const;
     // the most partial floats one of a layer's four GEMMs needs at M rows
@@ -347,7 +355,7 @@ struct lg_engine {
     }
     AttnArgs attn_args(const KvCache& kv, int l, int R, int Tq) const {
         return make_attn_args(cfg.dtype, cfg.n_head, hd, hdp, kv.rows, kv.max_seq, kv.kcache, kv.vcache, kv.maps,
-                              kv.kv_f8 ? &kv_scales[2 * l] : nullptr, l % kv.layers, R, Tq);
+                              kv.kv_f8 ? &kv_scales[2 * l] : nullptr, l % kv.layers, R, Tq, kv.first_row);
     }
     AttnArgs layer_attn(const Workspace& w, int l, int R, int Tq, PosArg pos, const float* emb_mask, int B) const {
         AttnArgs aa = attn_args(w, l, R, Tq);
@@ -457,6 +465,19 @@ size_t lg_engine::carve_sjd(RowBuffers& o, SjdArgs& sa, char* base, int B, int n
     sa.shift = (int32_t*)c.split(B * sizeof(int32_t));
     sa.pos_rows = (int32_t*)c.split((size_t)nh * B * sizeof(int32_t));
     sa.state = (int32_t*)c.split(kSjdStateInts * sizeof(int32_t));
+    return c.off;
+}
+
+// lg_generate_prefix's scratch for a chunk of `rows` cache rows of `seq` positions (the condition and the prefix), from `base` (null:
+// sizes only): the row buffers of rows * seq positions and the GEMM partials of that M and of the caption MLP. The K / V rows go to
+// the workspace's cache, the last positions to its row buffers.
+size_t lg_engine::carve_prefix(RowBuffers& o, char* base, int rows, int seq) const {
+    const int D = cfg.dim, Tc = cfg.cls_token_num, dt = cfg.dtype;
+    const bool t2i = cfg.model_type == LG_MODEL_T2I;
+    size_t pf = layer_partial_floats(rows * seq);
+    if (t2i) pf = std::max({pf, gemm_partial_floats(rows * Tc, D, cfg.caption_dim, 0, dt), gemm_partial_floats(rows * Tc, D, D, 0, dt)});
+    Carver c{base};
+    carve_rows(c, o, (size_t)rows * seq, t2i ? (size_t)rows * Tc : 0, pf, 0);
     return c.off;
 }
 
@@ -940,17 +961,58 @@ int lg_sample(const float* logits, int B, int V, int mix_cfg, int round_dtype, c
     return launch_sample(a, (cudaStream_t)stream);
 }
 
+struct PrefixArgs {              // lg_generate_prefix: prefix [B, P] and the prefill's scratch (P = 0: lg_generate)
+    const int32_t* prefix = nullptr;
+    int P = 0;
+    char* scratch = nullptr;
+    size_t scratch_bytes = 0;
+};
 static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, int B, int T, int S,
                          const lg_sample_cfg* sc, int32_t* out_tokens, float* dbg_logits, const int32_t* teacher,
-                         cudaStream_t st);
+                         const PrefixArgs& pa, cudaStream_t st);
 
 int lg_generate(lg_engine* e, const void* cond, const float* emb_mask, int B, int T, int S, const lg_sample_cfg* sc,
                 int32_t* out_tokens, float* dbg_logits, const int32_t* teacher, void* stream) {
     LG_REQUIRE(e, "lg_generate: null engine");
     DeviceGuard guard(e->device);
     return e->run_forked((cudaStream_t)stream, lg_engine::kMaxChains, [&](cudaStream_t st) {
-        return generate_impl(e, cond, emb_mask, B, T, S, sc, out_tokens, dbg_logits, teacher, st);
+        return generate_impl(e, cond, emb_mask, B, T, S, sc, out_tokens, dbg_logits, teacher, PrefixArgs{}, st);
     });
+}
+
+int lg_prefix_workspace_bytes(lg_engine* e, int rows, int seq, size_t* bytes) {
+    LG_REQUIRE(e && bytes && rows > 0 && seq > 0, "lg_prefix_workspace_bytes: bad argument");
+    RowBuffers tmp;
+    *bytes = e->carve_prefix(tmp, nullptr, rows, seq);
+    return 0;
+}
+
+int lg_generate_prefix(lg_engine* e, const void* cond, const float* emb_mask, int B, int T, int S, const lg_sample_cfg* sc,
+                       const int32_t* prefix, int P, void* dev_ws, size_t ws_bytes, int32_t* out_tokens, float* dbg_logits, void* stream) {
+    LG_REQUIRE(e && e->finalized, "lg_generate_prefix: engine not finalized");
+    DeviceGuard guard(e->device);
+    const lg_model_cfg& c = e->cfg;
+    LG_REQUIRE(cond && sc && out_tokens && B > 0 && S > 0, "lg_generate_prefix: null argument or B=%d S=%d", B, S);
+    LG_REQUIRE(prefix, "lg_generate_prefix: null prefix");
+    LG_REQUIRE(P >= 1 && P <= S - 1, "lg_generate_prefix: prefix length P=%d outside [1, S - 1] (S=%d)", P, S);
+    LG_REQUIRE(T == c.cls_token_num, "lg_generate_prefix: T=%d must equal cls_token_num=%d", T, c.cls_token_num);
+    LG_REQUIRE(!emb_mask || c.model_type == LG_MODEL_T2I, "lg_generate_prefix: emb_mask only applies to t2i models");
+    const int nh = sc->cfg_scale > 1.0f ? 2 : 1;   // generate.py:128
+    LG_TRY(check_ready(e, nh * B, T + S));
+    LG_REQUIRE(dev_ws && ((uintptr_t)dev_ws & 255) == 0, "lg_generate_prefix: scratch must be non-null and 256-byte aligned");
+    RowBuffers one;
+    const size_t need1 = e->carve_prefix(one, nullptr, nh, T + P);
+    LG_REQUIRE(ws_bytes >= need1, "lg_generate_prefix: scratch of %zu bytes is too small for one image (%zu)", ws_bytes, need1);
+    const PrefixArgs pa{prefix, P, (char*)dev_ws, ws_bytes};
+    return e->run_forked((cudaStream_t)stream, lg_engine::kMaxChains, [&](cudaStream_t st) {
+        return generate_impl(e, cond, emb_mask, B, T, S, sc, out_tokens, dbg_logits, nullptr, pa, st);
+    });
+}
+
+int lg_test_prefix_chunks(lg_engine* e, int* chains) {
+    if (!e) return -1;
+    if (chains) *chains = e->prefix_chains;
+    return e->prefix_chunks;
 }
 
 namespace {
@@ -960,15 +1022,50 @@ struct Chain {
     cudaStream_t st = nullptr;
     const void* cond = nullptr;
     const float* emb_mask = nullptr;
+    const int32_t* prefix = nullptr;   // [B, P] of this chain's images (lg_generate_prefix)
     int B = 0, R = 0;
     SampleArgs sa{};
     Graph graph;
 };
 }  // namespace
 
+// lg_generate_prefix's prefill of chain k: positions 0 .. T + P - 1 (the condition, then the prefix embeddings) of every row in one
+// forward, its K / V written into the chain's cache. The rows go in chunks of at most `nr` contiguous cache rows of the chain's view
+// that stay inside its conditional rows [0, B) or its unconditional rows [B, 2B): a chunk is then images img0 .. img0 + n - 1 of one
+// half, embedded with the condition of those images or the null condition, and its attention runs at first_row = its first cache
+// row over the maps of the whole view. Chunks also never cross a block of `blk` images (the images of one chain under the largest
+// split), so one and two chains run the same chunks with the same GEMM plans: the results are bit-identical. The chunk's last
+// positions are gathered into k.w.q rows, and one head GEMM over the R rows leaves the logits of token P in k.w.logits.
+static int prefix_prefill(lg_engine* e, Chain& k, int nh, int T, int P, int nr, int blk, const PrefixArgs& pa, cudaStream_t st) {
+    const lg_model_cfg& c = e->cfg;
+    const int D = c.dim, dt = c.dtype, seq = T + P;
+    const size_t esz = e->esz;
+    for (int half = 0; half < nh; ++half)
+        for (int b0 = 0; b0 < k.B; b0 += blk)
+        for (int img0 = b0, b1 = std::min(b0 + blk, k.B); img0 < b1; img0 += nr) {
+            const int n = std::min(nr, b1 - img0), r0 = half * k.B + img0;
+            Workspace w;
+            static_cast<KvCache&>(w) = k.w;
+            w.first_row = r0;
+            LG_REQUIRE(e->carve_prefix(w, pa.scratch, n, seq) <= pa.scratch_bytes, "lg_generate_prefix: a chunk of %d rows outgrows the scratch", n);
+            const void* cond_c = c.model_type == LG_MODEL_C2I ? (const void*)((const int32_t*)k.cond + img0)
+                                                              : (const void*)((const char*)k.cond + (size_t)img0 * T * c.caption_dim * esz);
+            Workspace wc = w;   // the condition rows [n * T, D] go to ff first, then the sequence embedding assembles h
+            wc.h = w.ff;
+            LG_TRY(e->embed_cond(wc, cond_c, half ? 0 : n, n, T, st));   // B = 0: every row takes the null condition
+            LG_TRY(launch_embed_seq(w.ff, e->tok_emb, k.prefix + (size_t)img0 * P, n, n, T, seq, D, dt, w.h, st));
+            const float* em = k.emb_mask ? k.emb_mask + (size_t)img0 * T : nullptr;
+            LG_TRY(e->run_layers(w, n * seq, seq, PosArg{nullptr, 0}, em, n, false, st));
+            LG_TRY(launch_gather_last(w.xn, n, seq, D, dt, k.w.q + (size_t)r0 * D * esz, st));
+            ++e->prefix_chunks;
+        }
+    GemmNext nx_first{e->layers[0].wqkv.p, e->layers[0].wqkv.bytes(3 * D, D, esz), nullptr, 0};
+    return e->head(k.w, k.w.q, k.R, k.w.logits, &nx_first, st);
+}
+
 static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, int B, int T, int S,
                          const lg_sample_cfg* sc, int32_t* out_tokens, float* dbg_logits, const int32_t* teacher,
-                         cudaStream_t st0) {
+                         const PrefixArgs& pa, cudaStream_t st0) {
     LG_REQUIRE(cond && sc && out_tokens && B > 0 && S > 0, "lg_generate: bad argument");
     const bool use_cfg = sc->cfg_scale > 1.0f;  // generate.py:128
     const int R = use_cfg ? 2 * B : B;
@@ -995,6 +1092,7 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
         k.cond = c.model_type == LG_MODEL_C2I ? (const void*)((const int32_t*)cond + boff)
                                               : (const void*)((const char*)cond + boff * T * c.caption_dim * e->esz);
         k.emb_mask = emb_mask ? emb_mask + boff * T : nullptr;
+        k.prefix = pa.prefix ? pa.prefix + boff * pa.P : nullptr;
         k.sa = make_sample_args(*sc, k.w.logits, k.B, c.vocab_size, use_cfg, c.dtype);
         SampleArgs& sa = k.sa;
         sa.row_offset = (int)boff;
@@ -1028,22 +1126,51 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
         return 0;
     };
 
-    // ---- prefill (generate.py:167-169) + first decode step, eagerly, per chain
+    // ---- prefix prefill (lg_generate_prefix): tokens 0 .. P - 1 are the prefix; every chain's prefill shares the one scratch, so all
+    // of them run on the caller's stream, in chunks of the most rows that fit the scratch and the attention kernel's grid
+    const int P = pa.P;
+    if (P > 0) {
+        const int nh = use_cfg ? 2 : 1, seq = T + P;
+        auto fits = [&](int n) {
+            RowBuffers rb;
+            if (e->carve_prefix(rb, nullptr, n, seq) > pa.scratch_bytes) return false;
+            return attn_plan(e->attn_args(ch[0].w, 0, n, seq)).kernel >= 0;
+        };
+        const int blk = B % lg_engine::kMaxChains == 0 ? B / lg_engine::kMaxChains : B;   // one chain's images under the largest split
+        int lo = 1, hi = blk;       // largest chunk that fits
+        while (lo < hi) {
+            const int mid = lo + (hi - lo + 1) / 2;
+            if (fits(mid)) lo = mid; else hi = mid - 1;
+        }
+        LG_REQUIRE(fits(lo), "lg_generate_prefix: no chunk of rows fits the scratch (%zu bytes) and the attention grid", pa.scratch_bytes);
+        LG_CUDA_OK(cudaMemcpy2DAsync(out_tokens, (size_t)S * sizeof(int32_t), pa.prefix, (size_t)P * sizeof(int32_t),
+                                     (size_t)P * sizeof(int32_t), B, cudaMemcpyDeviceToDevice, st0));
+        e->prefix_chunks = 0;
+        e->prefix_chains = nchains;
+        for (int g = 0; g < nchains; ++g) LG_TRY(prefix_prefill(e, ch[g], nh, T, P, lo, blk, pa, st0));
+        if (nchains > 1) {
+            LG_CUDA_OK(cudaEventRecord(e->ev_prefill, st0));
+            for (int g = 1; g < nchains; ++g) LG_CUDA_OK(cudaStreamWaitEvent(ch[g].st, e->ev_prefill, 0));
+        }
+    }
+    // ---- prefill (generate.py:167-169) + first decode step, eagerly, per chain; token P is sampled first (0 without a prefix)
     for (int g = 0; g < nchains; ++g) {
         Chain& k = ch[g];
-        LG_TRY(e->embed_cond(k.w, k.cond, k.B, k.R, T, k.st));
-        LG_TRY(e->forward(k.w, k.R * T, T, PosArg{nullptr, 0}, k.emb_mask, k.B, k.w.logits, false, k.st));
-        k.sa.step = 0; k.sa.step_dev = nullptr;
-        const bool tail = S > 1 && fuse_tail;
+        if (P == 0) {
+            LG_TRY(e->embed_cond(k.w, k.cond, k.B, k.R, T, k.st));
+            LG_TRY(e->forward(k.w, k.R * T, T, PosArg{nullptr, 0}, k.emb_mask, k.B, k.w.logits, false, k.st));
+        }
+        k.sa.step = P; k.sa.step_dev = nullptr;
+        const bool tail = S > P + 1 && fuse_tail;
         if (tail) arm_tail(k, false);            // the prefill's sample prepares the first decode step's rows; counters are set below
         LG_TRY(launch_sample(k.sa, k.st));
-        if (S == 1) continue;
-        LG_TRY(launch_set_counters(k.w.counters, T, k.w.counters + 1, 1, k.st));
+        if (S == P + 1) continue;
+        LG_TRY(launch_set_counters(k.w.counters, T + P, k.w.counters + 1, P + 1, k.st));
         k.sa.step_dev = k.w.counters + 1;
         if (tail) arm_tail(k, true);
         LG_TRY(body(k));   // first decode step runs eagerly (also sets every kernel attribute outside capture)
     }
-    const int remaining = S - 2;
+    const int remaining = S - P - 2;
     if (remaining <= 0) return 0;
     if (!e->use_graph || remaining < 3 || prof_enabled() || lg_debug_sync()) {
         for (int i = 0; i < remaining; ++i)

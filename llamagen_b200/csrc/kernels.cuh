@@ -211,10 +211,11 @@ inline int attn_kv_row_width(int dtype, int hd) { return hd == 100 && lg_dtype_i
 //     LG_ATTN_NST=3, 2 otherwise.
 //   3 attn_prefill_tc_kernel: the t2i condition prefill, 1 < Tq <= 128 from position 0, hd 64, fp8 caches too (LG_ATTN_PREFILL_TC).
 //     TMA-staged Q/K/V, mma.sync QK^T and PV, one CTA per (row, head); stages 1.
-//   2 attn_causal_tc_kernel: teacher-forced sequences, Tq > 128 from position 0 on a cache in the model dtype: a CTA per (head, row,
-//     64-query block), K / V blocks through a 2-stage TMA ring, mma.sync QK^T and PV with an online softmax; no R * Tq limit.
-//   4 attn_window_tc_kernel: speculative-decoding windows, 2 <= Tq <= 64 queries per row at pos.rows[r] + t, same caches as kernel 2,
-//     through the same ring.
+//   2 attn_causal_tc_kernel (attn_causal_tc_f8_kernel for an fp8 cache): teacher-forced sequences and prefix prefills, Tq > 128 from
+//     position 0, on a cache in the model dtype or fp8: a CTA per (head, row, 64-query block), K / V blocks through a 2-stage TMA ring, mma.sync QK^T and PV with an online
+//     softmax; no R * Tq limit.
+//   4 attn_window_tc_kernel: speculative-decoding windows, 2 <= Tq <= 64 queries per row at pos.rows[r] + t, caches in the model
+//     dtype only, through kernel 2's ring.
 //   0 attention_kernel (xf_kernels.cu): CUDA cores, no fused slabs, R * Tq <= 65535, rows attn_kv_row_width wide; stages 0.
 // kernel -1: no kernel takes the call, `error` says why. The only reader of LG_ATTN_TMA, LG_ATTN_PREFILL_TC, LG_ATTN_DEEP and
 // LG_ATTN_NST.

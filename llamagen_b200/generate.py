@@ -45,6 +45,10 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
                            max_new_tokens - 1 is shortened to it). The same distribution as plain sampling but other draws for a
                            seed, except token 0; greedy decoding gives the same tokens.
       return_stats=True    with sjd_window: return (tokens, {"iterations": passes, "tokens_per_iteration": ...})
+      prefix=int tensor    [B, P] tokens 0 .. P - 1 of every image (1 <= P <= max_new_tokens - 1; e.g. the first rows of an encoded
+                           image): the condition and the prefix are prefilled in one forward pass and tokens P .. are sampled as
+                           plain generation samples them (same RNG key per token index), so out[:, :P] == prefix. With
+                           return_logits, rows k < P of the logits are zero.
     """
     if not isinstance(model, Transformer):
         raise TypeError("llamagen_b200.generate needs a llamagen_b200 GPT_models[...] instance")
@@ -57,6 +61,7 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
     teacher = sampling_kwargs.pop("teacher", None)
     sjd_window = sampling_kwargs.pop("sjd_window", None)
     return_stats = bool(sampling_kwargs.pop("return_stats", False))
+    prefix = sampling_kwargs.pop("prefix", None)
     if sampling_kwargs:
         raise TypeError(f"unexpected sampling kwargs: {sorted(sampling_kwargs)}")
     if sjd_window is not None:
@@ -66,6 +71,9 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
             raise ValueError("sjd_window cannot be combined with teacher or return_logits")
     elif return_stats:
         raise ValueError("return_stats needs sjd_window")
+    if prefix is not None and (teacher is not None or sjd_window is not None):
+        raise ValueError("prefix cannot be combined with teacher or sjd_window")
+    pf = _check_prefix(prefix, cond.shape[0], int(max_new_tokens), model.vocab_size) if prefix is not None else None
 
     dev = model.tok_embeddings.weight.device
     _lib.require_cuda(model.tok_embeddings.weight, "generate")
@@ -99,6 +107,18 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
         return _generate_sjd(model, lib, handle, cond, cond_dev, em, B, T, S, out, min(int(sjd_window), S - 1), use_cfg, return_stats,
                              _lib.SampleCfg(float(cfg_scale), int(cfg_interval), temperature, top_k, top_p, 0 if sample_logits else 1,
                                             _draw_seed() if seed is None else int(seed)))
+    if pf is not None:
+        P = pf.shape[1]
+        dbg = torch.zeros((S, B, model.vocab_size), dtype=torch.float32, device=dev) if return_logits else None
+        pf_dev = pf.to(device=dev, dtype=torch.int32).contiguous()
+        ws, ws_bytes = model._prefix_scratch(rows, T + P, 2 if use_cfg else 1)
+        sc = _lib.SampleCfg(float(cfg_scale), int(cfg_interval), temperature, top_k, top_p, 0 if sample_logits else 1,
+                            _draw_seed() if seed is None else int(seed))
+        _lib.check(lib.lg_generate_prefix(handle, _lib.ptr(cond_dev), _lib.ptr(em), B, T, S, ctypes.byref(sc), _lib.ptr(pf_dev), P, ws,
+                                          ws_bytes, _lib.ptr(out), _lib.ptr(dbg), _lib.current_stream(dev)), "lg_generate_prefix")
+        if cond.device != dev:
+            out = out.to(cond.device)
+        return (out, dbg) if return_logits else out
     dbg = torch.empty((S, B, model.vocab_size), dtype=torch.float32, device=dev) if return_logits else None
     tf = teacher.to(device=dev, dtype=torch.int32).contiguous() if teacher is not None else None
     if tf is not None and tuple(tf.shape) != (B, S):
@@ -110,6 +130,21 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
     if cond.device != dev:
         out = out.to(cond.device)
     return (out, dbg) if return_logits else out
+
+
+def _check_prefix(prefix, B, S, V):
+    """The prefix as an int64 host tensor [B, P], checked on the host (it is outside input): integer ids in [0, V), 1 <= P <= S - 1."""
+    pf = torch.as_tensor(prefix)
+    if pf.dtype.is_floating_point or pf.dtype.is_complex or pf.dtype == torch.bool:
+        raise ValueError(f"prefix must be an integer tensor of token ids, got dtype {pf.dtype}")
+    if pf.dim() != 2 or pf.shape[0] != B:
+        raise ValueError(f"prefix must be [B, P] = [{B}, P], got {tuple(pf.shape)}")
+    if not 1 <= pf.shape[1] <= S - 1:
+        raise ValueError(f"prefix length P={pf.shape[1]} must lie in [1, max_new_tokens - 1 = {S - 1}]")
+    pf = pf.detach().to("cpu", torch.int64)
+    if bool(((pf < 0) | (pf >= V)).any()):
+        raise ValueError(f"prefix token ids must lie in [0, vocab_size={V})")
+    return pf
 
 
 def _generate_sjd(model, lib, handle, cond, cond_dev, em, B, T, S, out, L, use_cfg, return_stats, sc, dbg_probs=None):

@@ -82,6 +82,7 @@ FP8_LAYER_WEIGHTS = ("attention.wqkv.weight", "attention.wo.weight", "feed_forwa
                      "feed_forward.w2.weight")
 
 SCORE_SCRATCH_CAP = 4 << 30   # bytes of lg_score scratch a model keeps; a batch that needs more is scored in image chunks
+PREFIX_SCRATCH_CAP = 4 << 30  # bytes of prefix-prefill scratch (generate(prefix=...)); a batch that needs more is prefilled in chunks
 
 
 def t2i_attn_mask(emb_masks: torch.Tensor, seq: int) -> torch.Tensor:
@@ -201,6 +202,7 @@ class Transformer(nn.Module):
         self._w8 = {}
         self._score_ws = None
         self._sjd_ws = None
+        self._prefix_ws = None
         self.requires_grad_(False)
 
     # ------------------------------------------------------------------ engine plumbing
@@ -379,6 +381,18 @@ class Transformer(nn.Module):
         _lib.check(lib.lg_score_workspace_bytes(handle, rows, seq, ctypes.byref(need)), "lg_score_workspace_bytes")
         _lib.check(lib.lg_score_workspace_bytes(handle, nh, seq, ctypes.byref(one)), "lg_score_workspace_bytes")
         return self._device_buffer("_score_ws", need.value if need.value <= SCORE_SCRATCH_CAP else max(SCORE_SCRATCH_CAP, one.value))
+
+    def _prefix_scratch(self, rows: int, seq: int, nh: int):
+        """The scratch of generate(prefix=...)'s prefill of `rows` rows of `seq` = T + P positions, capped at PREFIX_SCRATCH_CAP bytes
+        (the engine then prefills in chunks of rows); kept on the model like the setup_caches() workspace. Returns (device pointer,
+        bytes), the bytes at most what was asked for."""
+        lib, handle = _lib.load(), self.engine()
+        need, one = ctypes.c_size_t(), ctypes.c_size_t()
+        _lib.check(lib.lg_prefix_workspace_bytes(handle, rows, seq, ctypes.byref(need)), "lg_prefix_workspace_bytes")
+        _lib.check(lib.lg_prefix_workspace_bytes(handle, nh, seq, ctypes.byref(one)), "lg_prefix_workspace_bytes")
+        want = need.value if need.value <= PREFIX_SCRATCH_CAP else max(PREFIX_SCRATCH_CAP, one.value)
+        base, nbytes = self._device_buffer("_prefix_ws", want)
+        return base, min(nbytes, want)
 
     def _sjd_scratch(self, B: int, use_cfg: bool, L: int):
         """The lg_generate_sjd scratch for B images and window L, kept on the model like the setup_caches() workspace.

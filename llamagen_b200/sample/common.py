@@ -1,6 +1,9 @@
 """Shared CLI helpers: checkpoint key dispatch (sample_c2i.py:48-58) and model construction."""
 from __future__ import annotations
 
+import os
+
+import numpy as np
 import torch
 
 from .. import GPT_models, VQ_models
@@ -65,6 +68,42 @@ def add_sjd_arg(parser):
 def sjd_kwargs(args) -> dict:
     """generate() keywords of --sjd-window (none when it is not given, so the default path is unchanged)."""
     return {} if args.sjd_window is None else {"sjd_window": args.sjd_window}
+
+
+def add_prefix_args(parser):
+    parser.add_argument("--prefix-image", type=str, default=None,
+                        help="extension: complete this image: it is centre-cropped to --image-size and encoded, the first "
+                             "--prefix-rows rows of its latent grid are kept for every image of the batch and the rest is generated")
+    parser.add_argument("--prefix-rows", type=int, default=None, help="extension: latent rows of --prefix-image kept (1 .. grid - 1)")
+    return parser
+
+
+def check_prefix_args(args, latent_size: int):
+    """Rejects a --prefix-image / --prefix-rows combination that generate() cannot run, before any model is loaded."""
+    if args.prefix_image is None and args.prefix_rows is None:
+        return
+    if args.prefix_image is None or args.prefix_rows is None:
+        raise SystemExit("--prefix-image and --prefix-rows go together")
+    if not 1 <= args.prefix_rows <= latent_size - 1:
+        raise SystemExit(f"--prefix-rows must lie in [1, {latent_size - 1}] (the latent grid has {latent_size} rows)")
+    if getattr(args, "sjd_window", None) is not None:
+        raise SystemExit("--prefix-image cannot be combined with --sjd-window")
+    if not os.path.isfile(args.prefix_image):
+        raise SystemExit(f"--prefix-image {args.prefix_image!r} is not a file")
+
+
+def prefix_kwargs(args, vq_model, batch: int, latent_size: int, device) -> dict:
+    """generate() keywords of --prefix-image / --prefix-rows: the first rows * grid codes of the encoded image (raster order), the
+    same for every image of the batch; none when no prefix is given, so the default path is unchanged."""
+    if args.prefix_image is None:
+        return {}
+    from PIL import Image
+    from .vq_demo import center_crop
+    img = center_crop(Image.open(args.prefix_image).convert("RGB"), args.image_size)
+    x = torch.from_numpy(2.0 * (np.array(img) / 255.0) - 1.0).permute(2, 0, 1)[None].float().to(device)
+    _, _, [_, _, indices] = vq_model.encode(x)
+    codes = indices.reshape(-1)[: args.prefix_rows * latent_size]
+    return {"prefix": codes.view(1, -1).expand(batch, -1).contiguous()}
 
 
 def add_common_args(parser, t2i: bool):

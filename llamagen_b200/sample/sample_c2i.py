@@ -6,7 +6,7 @@ import time
 import torch
 
 from .. import generate
-from .common import add_common_args, add_sjd_arg, sjd_kwargs, load_gpt, load_vq
+from .common import add_common_args, add_prefix_args, add_sjd_arg, check_prefix_args, load_gpt, load_vq, prefix_kwargs, sjd_kwargs
 
 
 def main(args):
@@ -15,19 +15,21 @@ def main(args):
     if not torch.cuda.is_available():
         raise SystemExit("llamagen_b200 has no CPU path: a CUDA (sm_90a) device is required")
     device = "cuda"
-    vq_model = load_vq(args, device)
     latent_size = args.image_size // args.downsample_size
+    check_prefix_args(args, latent_size)
+    vq_model = load_vq(args, device)
     gpt_model = load_gpt(args, device, latent_size)
 
     class_labels = args.class_labels or [207, 360, 387, 974, 88, 979, 417, 279]      # sample_c2i.py:77
     c_indices = torch.tensor(class_labels, device=device)
     qzshape = [len(class_labels), args.codebook_embed_dim, latent_size, latent_size]
 
+    pk = prefix_kwargs(args, vq_model, len(class_labels), latent_size, device)
     torch.cuda.synchronize()
     t1 = time.time()
     index_sample = generate(gpt_model, c_indices, latent_size ** 2, cfg_scale=args.cfg_scale, cfg_interval=args.cfg_interval,
                             temperature=args.temperature, top_k=args.top_k, top_p=args.top_p, sample_logits=True,
-                            **sjd_kwargs(args))
+                            **sjd_kwargs(args), **pk)
     torch.cuda.synchronize()
     print(f"gpt sampling takes about {time.time() - t1:.2f} seconds.")
     t2 = time.time()
@@ -40,7 +42,7 @@ def main(args):
 
 
 def build_parser():
-    parser = add_sjd_arg(add_common_args(argparse.ArgumentParser(), t2i=False))
+    parser = add_prefix_args(add_sjd_arg(add_common_args(argparse.ArgumentParser(), t2i=False)))
     parser.add_argument("--cfg-interval", type=float, default=-1)
     parser.add_argument("--class-labels", type=int, nargs="+", default=None,
                         help="extension: override the 8 hard-coded ImageNet labels (batch size = number of labels)")

@@ -12,7 +12,7 @@ import torch
 
 from .. import generate
 from ..cond import HFT5Encoder, load_t5_feature_files, prepare_condition, synthetic_features
-from .common import add_common_args, add_sjd_arg, sjd_kwargs, load_gpt, load_vq
+from .common import add_common_args, add_prefix_args, add_sjd_arg, check_prefix_args, load_gpt, load_vq, prefix_kwargs, sjd_kwargs
 
 PROMPTS = [
     "A portrait photo of a kangaroo wearing an orange hoodie and blue sunglasses standing on the grassin front of the Sydney Opera House holding a sign on the chest that says Welcome Friends!",
@@ -39,8 +39,9 @@ def main(args):
     if not torch.cuda.is_available():
         raise SystemExit("llamagen_b200 has no CPU path: a CUDA (sm_90a) device is required")
     device = "cuda"
-    vq_model = load_vq(args, device)
     latent_size = args.image_size // args.downsample_size
+    check_prefix_args(args, latent_size)
+    vq_model = load_vq(args, device)
     gpt_model = load_gpt(args, device, latent_size)
     precision = gpt_model.tok_embeddings.weight.dtype
     caption_embs, emb_masks = t5_features(args, device, precision)
@@ -52,11 +53,12 @@ def main(args):
     c_indices, emb_masks = prepare_condition(caption_embs, emb_masks, left_padding=not args.no_left_padding)
     qzshape = [len(c_indices), args.codebook_embed_dim, latent_size, latent_size]
 
+    pk = prefix_kwargs(args, vq_model, len(c_indices), latent_size, device)
     torch.cuda.synchronize()
     t1 = time.time()
     index_sample = generate(gpt_model, c_indices, latent_size ** 2, emb_masks, cfg_scale=args.cfg_scale,
                             temperature=args.temperature, top_k=args.top_k, top_p=args.top_p, sample_logits=True,
-                            **sjd_kwargs(args))
+                            **sjd_kwargs(args), **pk)
     torch.cuda.synchronize()
     print(f"Full sampling takes about {time.time() - t1:.2f} seconds.")
     t2 = time.time()
@@ -69,7 +71,7 @@ def main(args):
 
 
 def build_parser():
-    parser = add_sjd_arg(add_common_args(argparse.ArgumentParser(), t2i=True))
+    parser = add_prefix_args(add_sjd_arg(add_common_args(argparse.ArgumentParser(), t2i=True)))
     parser.add_argument("--t5-path", type=str, default="pretrained_models/t5-ckpt")
     parser.add_argument("--t5-model-type", type=str, default="flan-t5-xl")
     parser.add_argument("--t5-feature-max-len", type=int, default=120)
