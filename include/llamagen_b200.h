@@ -133,6 +133,24 @@ int  lg_decode_step(lg_engine* e, const int32_t* tokens, int B, int pos, int use
  * null class), any other row the embedding of tokens[b]. Writes row r's K/V at pos_rows[r] and attends over [0, pos_rows[r]].
  * logits_out dev f32 [R, V]. */
 int  lg_decode_rows(lg_engine* e, const int32_t* tokens, const int32_t* pos_rows, int B, int use_cfg, float* logits_out, void* stream);
+/* Text-conditional serving. The lg_engine_set_workspace workspace holds B request slots: slot s owns cache row s and, with use_cfg,
+ * row B + s. Bytes of caller-provided scratch for lg_prefill_slot (t2i models only). */
+int  lg_slot_workspace_bytes(lg_engine* e, int use_cfg, size_t* bytes);
+/* Start one request in slot `slot`: cond dev [T, caption_dim] in the model dtype (left-padded, padding zeroed, as
+ * cond.prepare_condition makes it), T == cls_token_num; emb_mask dev f32 [T] or NULL. Writes the K / V of positions 0 .. T - 1 of
+ * the slot's rows (the CFG row with the null condition, uncond_embedding, and the same emb_mask, as lg_generate does) and nothing
+ * else of the workspace. logits_out dev f32 [nh, V] (nh = 2 with use_cfg, cond row first): the head output at position T - 1, rounded
+ * as lg_prefill rounds it. The arithmetic depends on neither slot, B, nor the contents of any other row, including the rows' own
+ * stale K / V from an earlier request: each row is prefilled alone (lg_generate_prefix's prefill chunk of one row, P = 0), then one
+ * head GEMM runs over the request's nh rows. dev_ws: 256-byte aligned, at least lg_slot_workspace_bytes. Every argument is checked
+ * before any launch; the workspace needs rows >= nh * B and max_seq >= T. */
+int  lg_prefill_slot(lg_engine* e, const void* cond, const float* emb_mask, int T, int slot, int B, int use_cfg, void* dev_ws,
+                     size_t ws_bytes, float* logits_out, void* stream);
+/* lg_decode_rows for t2i models: row r takes the token embedding of tokens[r % B] at position pos_rows[r] (every row is past its
+ * condition), writes its K / V there and attends over [0, pos_rows[r]]. emb_mask dev f32 [B, T] or NULL: row r attends to condition
+ * key j < T iff emb_mask[r % B][j] != 0 or j is its own position (lg_generate's rule). logits_out dev f32 [R, V]. */
+int  lg_decode_rows_t2i(lg_engine* e, const int32_t* tokens, const int32_t* pos_rows, const float* emb_mask, int B, int use_cfg,
+                        float* logits_out, void* stream);
 /* lg_sample with per-request RNG streams: image b draws with seed_rows[b] at token index step_rows[b] (exactly the draw a
  * batch-of-one lg_generate with that seed makes), result -> out_idx[b] and/or out_seq[b*seq_stride + step_rows[b]]. */
 int  lg_sample_rows(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc, const uint64_t* seed_rows,

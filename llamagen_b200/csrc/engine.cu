@@ -340,6 +340,7 @@ struct lg_engine {
     size_t carve_score(Workspace& o, char* base, int rows, int seq) const;
     size_t carve_sjd(RowBuffers& o, SjdArgs& sa, char* base, int B, int nh, int L) const;
     size_t carve_prefix(RowBuffers& o, char* base, int rows, int seq) const;
+    size_t carve_slot(RowBuffers& head, char* base, int nh) const;
     void carve_kv(Carver& c, KvCache& o, int rows, int max_seq, int layers, bool f8) const;
     void carve_rows(Carver& c, RowBuffers& o, size_t M, size_t x0_rows, size_t partial_floats, size_t logits_rows) const;
     // the most partial floats one of a layer's four GEMMs needs at M rows
@@ -478,6 +479,18 @@ size_t lg_engine::carve_prefix(RowBuffers& o, char* base, int rows, int seq) con
     if (t2i) pf = std::max({pf, gemm_partial_floats(rows * Tc, D, cfg.caption_dim, 0, dt), gemm_partial_floats(rows * Tc, D, D, 0, dt)});
     Carver c{base};
     carve_rows(c, o, (size_t)rows * seq, t2i ? (size_t)rows * Tc : 0, pf, 0);
+    return c.off;
+}
+
+// lg_prefill_slot's scratch for one request of nh rows, from `base` (null: sizes only): one prefill chunk of one row of cls_token_num
+// positions (carve_prefix, from base on), then the request's nh last positions (head.q) and the partials of the head GEMM over them
+size_t lg_engine::carve_slot(RowBuffers& head, char* base, int nh) const {
+    const int D = cfg.dim, V = cfg.vocab_size, dt = cfg.dtype;
+    RowBuffers chunk;
+    Carver c{base, 0, 1, carve_prefix(chunk, nullptr, 1, cfg.cls_token_num)};
+    head.q = c.split((size_t)nh * D * esz);
+    head.partial_floats = std::max(gemm_partial_floats(nh, V, D, 0, dt), gemm_partial_floats(nh, V, D, 0, dt, output.scale != nullptr));
+    head.partial = (float*)c.split(head.partial_floats * sizeof(float));
     return c.off;
 }
 
@@ -867,6 +880,20 @@ int lg_decode_rows(lg_engine* e, const int32_t* tokens, const int32_t* pos_rows,
     return eager_forward("lg_decode_rows", e, R, 1, 1, PosArg{nullptr, 0, pos_rows}, nullptr, B, logits_out, stream, embed);
 }
 
+int lg_decode_rows_t2i(lg_engine* e, const int32_t* tokens, const int32_t* pos_rows, const float* emb_mask, int B, int use_cfg,
+                       float* logits_out, void* stream) {
+    // lg_decode_rows for text-conditional serving: every row is past its condition (lg_prefill_slot wrote positions 0 .. T - 1), so
+    // every row takes a token embedding; the emb-mask rows follow the rows' slots (row r reads mask row r % B)
+    const int R = use_cfg ? 2 * B : B;
+    LG_REQUIRE(e, "lg_decode_rows_t2i: null engine");
+    LG_REQUIRE(e->cfg.model_type == LG_MODEL_T2I, "lg_decode_rows_t2i: text-conditional models only");
+    LG_REQUIRE(tokens && pos_rows && logits_out && B > 0, "lg_decode_rows_t2i: bad argument");
+    auto embed = [&](cudaStream_t st) -> int {
+        return launch_embed(e->tok_emb, tokens, B, R, -1, e->cfg.dim, e->cfg.dtype, e->full.h, st);
+    };
+    return eager_forward("lg_decode_rows_t2i", e, R, 1, 1, PosArg{nullptr, 0, pos_rows}, emb_mask, B, logits_out, stream, embed);
+}
+
 int lg_score_workspace_bytes(lg_engine* e, int rows, int seq, size_t* bytes) {
     LG_REQUIRE(e && bytes && rows > 0 && seq > 0, "lg_score_workspace_bytes: bad argument");
     LG_REQUIRE(seq >= e->cfg.cls_token_num && seq <= e->cfg.cls_token_num + e->cfg.block_size - 1,
@@ -1029,6 +1056,27 @@ struct Chain {
 };
 }  // namespace
 
+// One chunk of a condition (+ prefix) prefill: positions 0 .. T + P - 1 of n contiguous cache rows of `kv` from row r0 on, in one
+// forward over the row buffers of `scratch`. The rows are n images embedded with their condition (cond: the chunk's first image's),
+// or with the null condition when `uncond`, then their prefix embeddings (prefix [n, P], unread when P = 0); emb_mask [n, T] or null.
+// The attention runs at first_row = r0 over the maps of the whole view, so only rows r0 .. r0 + n - 1 of the cache are written. The
+// last position of every row is gathered to `last` [n, D].
+static int prefill_chunk(lg_engine* e, const KvCache& kv, int r0, int n, const void* cond, bool uncond, const int32_t* prefix,
+                         const float* emb_mask, int T, int P, char* scratch, size_t scratch_bytes, void* last, const char* fn,
+                         cudaStream_t st) {
+    const int D = e->cfg.dim, dt = e->cfg.dtype, seq = T + P;
+    Workspace w;
+    static_cast<KvCache&>(w) = kv;
+    w.first_row = r0;
+    LG_REQUIRE(e->carve_prefix(w, scratch, n, seq) <= scratch_bytes, "%s: a chunk of %d rows outgrows the scratch", fn, n);
+    Workspace wc = w;   // the condition rows [n * T, D] go to ff first, then the sequence embedding assembles h
+    wc.h = w.ff;
+    LG_TRY(e->embed_cond(wc, cond, uncond ? 0 : n, n, T, st));   // B = 0: every row takes the null condition
+    LG_TRY(launch_embed_seq(w.ff, e->tok_emb, prefix, n, n, T, seq, D, dt, w.h, st));
+    LG_TRY(e->run_layers(w, n * seq, seq, PosArg{nullptr, 0}, emb_mask, n, false, st));
+    return launch_gather_last(w.xn, n, seq, D, dt, last, st);
+}
+
 // lg_generate_prefix's prefill of chain k: positions 0 .. T + P - 1 (the condition, then the prefix embeddings) of every row in one
 // forward, its K / V written into the chain's cache. The rows go in chunks of at most `nr` contiguous cache rows of the chain's view
 // that stay inside its conditional rows [0, B) or its unconditional rows [B, 2B): a chunk is then images img0 .. img0 + n - 1 of one
@@ -1038,29 +1086,61 @@ struct Chain {
 // positions are gathered into k.w.q rows, and one head GEMM over the R rows leaves the logits of token P in k.w.logits.
 static int prefix_prefill(lg_engine* e, Chain& k, int nh, int T, int P, int nr, int blk, const PrefixArgs& pa, cudaStream_t st) {
     const lg_model_cfg& c = e->cfg;
-    const int D = c.dim, dt = c.dtype, seq = T + P;
+    const int D = c.dim;
     const size_t esz = e->esz;
     for (int half = 0; half < nh; ++half)
         for (int b0 = 0; b0 < k.B; b0 += blk)
         for (int img0 = b0, b1 = std::min(b0 + blk, k.B); img0 < b1; img0 += nr) {
             const int n = std::min(nr, b1 - img0), r0 = half * k.B + img0;
-            Workspace w;
-            static_cast<KvCache&>(w) = k.w;
-            w.first_row = r0;
-            LG_REQUIRE(e->carve_prefix(w, pa.scratch, n, seq) <= pa.scratch_bytes, "lg_generate_prefix: a chunk of %d rows outgrows the scratch", n);
             const void* cond_c = c.model_type == LG_MODEL_C2I ? (const void*)((const int32_t*)k.cond + img0)
                                                               : (const void*)((const char*)k.cond + (size_t)img0 * T * c.caption_dim * esz);
-            Workspace wc = w;   // the condition rows [n * T, D] go to ff first, then the sequence embedding assembles h
-            wc.h = w.ff;
-            LG_TRY(e->embed_cond(wc, cond_c, half ? 0 : n, n, T, st));   // B = 0: every row takes the null condition
-            LG_TRY(launch_embed_seq(w.ff, e->tok_emb, k.prefix + (size_t)img0 * P, n, n, T, seq, D, dt, w.h, st));
             const float* em = k.emb_mask ? k.emb_mask + (size_t)img0 * T : nullptr;
-            LG_TRY(e->run_layers(w, n * seq, seq, PosArg{nullptr, 0}, em, n, false, st));
-            LG_TRY(launch_gather_last(w.xn, n, seq, D, dt, k.w.q + (size_t)r0 * D * esz, st));
+            LG_TRY(prefill_chunk(e, k.w, r0, n, cond_c, half != 0, k.prefix + (size_t)img0 * P, em, T, P, pa.scratch, pa.scratch_bytes,
+                                 k.w.q + (size_t)r0 * D * esz, "lg_generate_prefix", st));
             ++e->prefix_chunks;
         }
     GemmNext nx_first{e->layers[0].wqkv.p, e->layers[0].wqkv.bytes(3 * D, D, esz), nullptr, 0};
     return e->head(k.w, k.w.q, k.R, k.w.logits, &nx_first, st);
+}
+
+int lg_slot_workspace_bytes(lg_engine* e, int use_cfg, size_t* bytes) {
+    LG_REQUIRE(e && bytes, "lg_slot_workspace_bytes: null argument");
+    LG_REQUIRE(e->cfg.model_type == LG_MODEL_T2I, "lg_slot_workspace_bytes: text-conditional models only");
+    RowBuffers tmp;
+    *bytes = e->carve_slot(tmp, nullptr, use_cfg ? 2 : 1);
+    return 0;
+}
+
+// A join of text-conditional serving: lg_generate_prefix's prefill chunk with P = 0 over one request, once for its conditional row
+// `slot` and once, under CFG, for its unconditional row B + slot. Every call runs the same chunks at the same shapes (one row of T
+// positions, then a head GEMM over the request's nh rows), whatever the slot, B or the other requests, so a request's logits do not
+// depend on which requests join in the same step or are running.
+int lg_prefill_slot(lg_engine* e, const void* cond, const float* emb_mask, int T, int slot, int B, int use_cfg, void* dev_ws,
+                    size_t ws_bytes, float* logits_out, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    LG_REQUIRE(e, "lg_prefill_slot: null engine");
+    const lg_model_cfg& c = e->cfg;
+    LG_REQUIRE(c.model_type == LG_MODEL_T2I, "lg_prefill_slot: text-conditional models only");
+    LG_REQUIRE(cond && logits_out, "lg_prefill_slot: null cond or logits_out");
+    LG_REQUIRE(T == c.cls_token_num, "lg_prefill_slot: T=%d must equal cls_token_num=%d", T, c.cls_token_num);
+    LG_REQUIRE(B > 0 && slot >= 0 && slot < B, "lg_prefill_slot: slot %d outside [0, B=%d)", slot, B);
+    const int nh = use_cfg ? 2 : 1, D = c.dim, V = c.vocab_size;
+    LG_REQUIRE(dev_ws && ((uintptr_t)dev_ws & 255) == 0, "lg_prefill_slot: scratch must be non-null and 256-byte aligned");
+    LG_TRY(check_ready(e, nh * B, T));
+    RowBuffers hb;
+    const size_t need = e->carve_slot(hb, (char*)dev_ws, nh);
+    LG_REQUIRE(ws_bytes >= need, "lg_prefill_slot: scratch of %zu bytes is too small (%zu)", ws_bytes, need);
+    LG_REQUIRE(attn_plan(e->attn_args(e->full, 0, 1, T)).kernel >= 0, "lg_prefill_slot: %s", attn_plan(e->attn_args(e->full, 0, 1, T)).error);
+    DeviceGuard guard(e->device);
+    LG_TRY(e->zero_fill_if_needed(st));
+    for (int half = 0; half < nh; ++half)
+        LG_TRY(prefill_chunk(e, e->full, half * B + slot, 1, cond, half != 0, nullptr, emb_mask, T, 0, (char*)dev_ws, ws_bytes,
+                             hb.q + (size_t)half * D * e->esz, "lg_prefill_slot", st));
+    Workspace w;
+    static_cast<RowBuffers&>(w) = hb;
+    GemmNext nx_first{e->layers[0].wqkv.p, e->layers[0].wqkv.bytes(3 * D, D, e->esz), nullptr, 0};
+    LG_TRY(e->head(w, hb.q, nh, logits_out, &nx_first, st));
+    return round_logits_inplace(logits_out, (size_t)nh * V, c.dtype, st);
 }
 
 static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, int B, int T, int S,

@@ -203,6 +203,7 @@ class Transformer(nn.Module):
         self._score_ws = None
         self._sjd_ws = None
         self._prefix_ws = None
+        self._slot_ws = None
         self.requires_grad_(False)
 
     # ------------------------------------------------------------------ engine plumbing
@@ -393,6 +394,14 @@ class Transformer(nn.Module):
         want = need.value if need.value <= PREFIX_SCRATCH_CAP else max(PREFIX_SCRATCH_CAP, one.value)
         base, nbytes = self._device_buffer("_prefix_ws", want)
         return base, min(nbytes, want)
+
+    def _slot_scratch(self, use_cfg: bool):
+        """The lg_prefill_slot scratch (serve.LLM's join of one t2i request), kept on the model like the setup_caches() workspace.
+        Returns (device pointer, bytes)."""
+        lib, handle = _lib.load(), self.engine()
+        need = ctypes.c_size_t()
+        _lib.check(lib.lg_slot_workspace_bytes(handle, int(use_cfg), ctypes.byref(need)), "lg_slot_workspace_bytes")
+        return self._device_buffer("_slot_ws", need.value)
 
     def _sjd_scratch(self, B: int, use_cfg: bool, L: int):
         """The lg_generate_sjd scratch for B images and window L, kept on the model like the setup_caches() workspace.

@@ -16,6 +16,15 @@ caller appends one `[num_classes]` (null-class) prompt per conditional prompt; t
 unconditional twins, the pair is sampled once, and both requests receive the same tokens (the reference samples the two
 copies of the mixed logits independently and the caller discards the second half, serve/sample_c2i.py:66-67).
 
+Text-conditional models are served the same way, with one caption's T5 features per request (`add_request(prompt_embeds=...)`,
+`LLM.generate(prompt_embeds=[...])`). The condition is built as the samplers build it (cond.pack_t5_features, then
+cond.prepare_condition with left padding). A step (1) decodes and samples the running slots through `lg_decode_rows_t2i` and
+`lg_sample_rows`, then (2) admits waiting requests into free slots: `lg_prefill_slot` prefills the caption (and, under CFG, the
+null condition) into the slot's cache rows alone, and token 0 is drawn from its logits with step 0. A join has the same shapes
+whatever else joins or runs, so a request's tokens do not depend on the schedule, and request r draws token k with the key
+`generate(seed=base_seed + r)` uses for image 0. CFG is internal: the unconditional row takes the learned null condition, and no
+twin requests are involved. temperature=0 decodes greedily (generate's sample_logits=False) on this path.
+
 While requests are in flight the LLM owns the model's KV-cache workspace (a `generate()` call on the same model would reset it)."""
 from __future__ import annotations
 
@@ -26,9 +35,11 @@ from typing import List, Optional, Sequence
 
 import ctypes
 
+import numpy as np
 import torch
 
 from . import _lib
+from .cond import pack_t5_features, prepare_condition
 
 
 @dataclass(frozen=True)
@@ -61,6 +72,8 @@ class _Request:
     prompt_token_ids: List[int]
     params: SamplingParams
     twin_of: Optional[str] = None      # request id of the conditional request this null-class request mirrors
+    cond: Optional[torch.Tensor] = None   # t2i: the prepared condition, fp32 [T, caption_dim] on the host
+    mask: Optional[torch.Tensor] = None   # t2i: its emb-mask, fp32 [T]
 
 
 class LLM:
@@ -69,9 +82,11 @@ class LLM:
         """kv_cache_dtype: None keeps the model's KV-cache setting (Transformer.set_kv_cache, scales included); "auto" (the model
         dtype) or "fp8" (e4m3) sets it. Passing the dtype the model already has keeps its scales.
         weight_dtype: None keeps the model's GEMM-weight storage (Transformer.set_weight_dtype, its head choice included); "auto" or
-        "fp8" sets it."""
-        if gpt_model.model_type != "c2i":
-            raise ValueError("serve.LLM handles class-conditional models (the reference's serve path is c2i only)")
+        "fp8" sets it.
+        A t2i model serves caption requests (prompt_embeds); num_classes does not apply to it."""
+        if gpt_model.model_type not in ("c2i", "t2i"):
+            raise ValueError(f"serve.LLM handles c2i and t2i models, got model_type {gpt_model.model_type!r}")
+        self.t2i = gpt_model.model_type == "t2i"
         if kv_cache_dtype is not None and kv_cache_dtype != getattr(gpt_model, "_kv_cache", ("auto", None))[0]:
             gpt_model.set_kv_cache(kv_cache_dtype)
         if weight_dtype is not None and weight_dtype != getattr(gpt_model, "_weight_dtype", ("auto", True))[0]:
@@ -91,7 +106,18 @@ class LLM:
         self.steps_run = 0
 
     # ------------------------------------------------------------------ engine-style surface (llm_engine.py)
-    def add_request(self, prompt_token_ids: Sequence[int], sampling_params: Optional[SamplingParams] = None, twin_of=None) -> str:
+    def add_request(self, prompt_token_ids: Optional[Sequence[int]] = None, sampling_params: Optional[SamplingParams] = None, twin_of=None,
+                    prompt_embeds=None) -> str:
+        """c2i: prompt_token_ids = [class id] (twin_of: see LLM.generate). t2i: prompt_embeds = one caption's T5 features, [n, caption_dim]
+        or the .npy layout [1, n, caption_dim] (array or tensor, n >= 1, truncated at cls_token_num)."""
+        if self.t2i:
+            if prompt_token_ids is not None or twin_of is not None:
+                raise ValueError("a t2i LLM takes prompt_embeds (T5 caption features), not prompt_token_ids; CFG needs no twin requests")
+            return self._enqueue_t2i(self._caption(prompt_embeds), sampling_params)
+        if prompt_embeds is not None:
+            raise ValueError("prompt_embeds apply to text-conditional (t2i) models; a c2i prompt is prompt_token_ids = [class id]")
+        if prompt_token_ids is None:
+            raise ValueError("a c2i request needs prompt_token_ids = [class id]")
         if len(prompt_token_ids) != 1 or not (0 <= int(prompt_token_ids[0]) <= self.num_classes):
             raise ValueError(f"a c2i prompt is one class id in [0, {self.num_classes}], got {list(prompt_token_ids)}")
         rid = str(next(self.request_counter))
@@ -100,6 +126,28 @@ class LLM:
             self._waiting.append(req)
         else:
             self._twins[twin_of] = req
+        return rid
+
+    def _caption(self, feats):
+        """One caption's (condition fp32 [T, caption_dim], emb-mask fp32 [T]) on the host, exactly as the samplers build a batch row:
+        cond.pack_t5_features (truncation at T), then cond.prepare_condition with left padding."""
+        T, C = self.model.cls_token_num, self.model.config.caption_dim
+        if feats is None:
+            raise ValueError("a t2i request needs prompt_embeds (one caption's T5 features)")
+        f = feats.detach().cpu() if torch.is_tensor(feats) else torch.as_tensor(np.asarray(feats))
+        if f.dim() == 3 and f.shape[0] == 1:
+            f = f[0]
+        if f.dim() != 2 or f.shape[1] != C:
+            raise ValueError(f"prompt_embeds must be [n, {C}] or [1, n, {C}], got {tuple(f.shape)}")
+        if f.shape[0] == 0:
+            raise ValueError("prompt_embeds holds an empty caption (n = 0)")
+        embs, masks = pack_t5_features([f], max_len=T, dim=C)
+        cond, mask = prepare_condition(embs, masks, left_padding=True)
+        return cond[0], mask[0]
+
+    def _enqueue_t2i(self, caption, sampling_params: Optional[SamplingParams]) -> str:
+        rid = str(next(self.request_counter))
+        self._waiting.append(_Request(rid, [], sampling_params or SamplingParams(), cond=caption[0], mask=caption[1]))
         return rid
 
     def _running(self) -> int:
@@ -127,7 +175,101 @@ class LLM:
             seeds=torch.zeros(B, dtype=torch.int64, device=dev),
             out=torch.zeros(B, S, dtype=torch.int32, device=dev),
             logits=torch.empty(R, m.vocab_size, dtype=torch.float32, device=dev))
+        if self.t2i:
+            T, C = m.cls_token_num, m.config.caption_dim
+            self._state.update(
+                step=torch.zeros(B, dtype=torch.int32, device=dev),       # index of the token every slot samples next
+                cond=torch.zeros(B, T, C, dtype=m.tok_embeddings.weight.dtype, device=dev),   # every slot's condition
+                mask=torch.zeros(B, T, dtype=torch.float32, device=dev),   # and emb-mask (row r of a decode reads mask row r % B)
+                step0=torch.zeros(1, dtype=torch.int32, device=dev),      # the step of token 0, drawn by a join
+                join_logits=torch.empty(R // B, m.vocab_size, dtype=torch.float32, device=dev))
         return self._state
+
+    def _sample_cfg(self, params: SamplingParams):
+        """t2i path: temperature 0 is greedy decoding (the argmax of the mixed logits)."""
+        greedy = 1 if params.temperature == 0 else 0
+        return _lib.SampleCfg(self.cfg_scale, -1, float(params.temperature), max(0, int(params.top_k)), float(params.top_p), greedy, 0)
+
+    def _device_decode_t2i(self, st, params: SamplingParams):
+        """lg_decode_rows_t2i + lg_sample_rows on every slot: the logits of every row at its own position under its slot's emb-mask, then
+        one draw per slot with step st["step"][slot], written to st["out"][slot, step] and, in place, to st["tok"][slot]."""
+        B, R, S, dev = self.max_num_seqs, st["R"], st["S"], st["dev"]
+        lib, handle = _lib.load(), self.model.engine()
+        use_cfg = 1 if R == 2 * B else 0
+        stream = _lib.current_stream(dev)
+        _lib.check(lib.lg_decode_rows_t2i(handle, _lib.ptr(st["tok"]), _lib.ptr(st["pos"]), _lib.ptr(st["mask"]), B, use_cfg,
+                                          _lib.ptr(st["logits"]), stream), "lg_decode_rows_t2i")
+        sc = self._sample_cfg(params)
+        dt = _lib.dtype_code(self.model.tok_embeddings.weight.dtype)
+        _lib.check(lib.lg_sample_rows(_lib.ptr(st["logits"]), B, self.model.vocab_size, use_cfg, dt, ctypes.byref(sc), _lib.ptr(st["seeds"]),
+                                      _lib.ptr(st["step"]), _lib.ptr(st["tok"]), _lib.ptr(st["out"]), S, stream), "lg_sample_rows")
+
+    def _device_join_t2i(self, st, params: SamplingParams, slot: int):
+        """lg_prefill_slot of the condition and mask in st["cond"][slot], st["mask"][slot], then token 0 drawn from its logits
+        (lg_sample_rows, one image, the slot's seed, step 0) into st["out"][slot, 0] and st["tok"][slot]."""
+        B, R, S, dev = self.max_num_seqs, st["R"], st["S"], st["dev"]
+        m = self.model
+        lib, handle = _lib.load(), m.engine()
+        use_cfg = 1 if R == 2 * B else 0
+        stream = _lib.current_stream(dev)
+        ws, ws_bytes = m._slot_scratch(use_cfg)
+        _lib.check(lib.lg_prefill_slot(handle, _lib.ptr(st["cond"][slot]), _lib.ptr(st["mask"][slot]), m.cls_token_num, slot, B, use_cfg,
+                                       ws, ws_bytes, _lib.ptr(st["join_logits"]), stream), "lg_prefill_slot")
+        sc = self._sample_cfg(params)
+        dt = _lib.dtype_code(m.tok_embeddings.weight.dtype)
+        _lib.check(lib.lg_sample_rows(_lib.ptr(st["join_logits"]), 1, m.vocab_size, use_cfg, dt, ctypes.byref(sc),
+                                      _lib.ptr(st["seeds"][slot:slot + 1]), _lib.ptr(st["step0"]), _lib.ptr(st["tok"][slot:slot + 1]),
+                                      _lib.ptr(st["out"][slot]), S, stream), "lg_sample_rows")
+
+    def _step_t2i(self, st, params: SamplingParams) -> List[RequestOutput]:
+        """step() of a t2i LLM: decode the running slots, then admit waiting requests (their prefill draws token 0), then return the
+        requests that reached max_tokens."""
+        B, R, S, dev = self.max_num_seqs, st["R"], st["S"], st["dev"]
+        T = self.model.cls_token_num
+        # (1) one decode step for every slot; free slots run too (their rows are never read) so that the row count stays fixed
+        if self._running():
+            self._device_decode_t2i(st, params)
+            st["pos"] += st["active"]
+            st["step"] += st["active"][:B]
+            for i in range(B):
+                if self._slots[i] is not None:
+                    self._depth[i] += 1
+        # (2) admission: the conditions and masks go to their slots' rows, then each request is prefilled alone and draws token 0
+        joined = []
+        for i in range(B):
+            if not self._waiting or self._waiting[0].params != params:
+                break
+            if self._slots[i] is None:
+                req = self._waiting.popleft()
+                self._slots[i], self._depth[i] = req, 1
+                joined.append((i, req))
+        if joined:
+            idx = torch.tensor([i for i, _ in joined], dtype=torch.long, device=dev)
+            st["seeds"][idx] = torch.tensor([self._seed + int(r.request_id) for _, r in joined], dtype=torch.int64, device=dev)
+            for i, r in joined:
+                st["cond"][i].copy_(r.cond)
+                st["mask"][i].copy_(r.mask)
+                self._device_join_t2i(st, params, i)
+            rows = torch.cat([idx, idx + B]) if R == 2 * B else idx
+            st["pos"][rows] = T
+            st["active"][rows] = 1
+            st["step"][idx] = 1
+        self.steps_run += 1
+        # (3) the finished requests: the only device->host copy is their token rows
+        done = [i for i in range(B) if self._slots[i] is not None and self._depth[i] >= S]
+        outs: List[RequestOutput] = []
+        if done:
+            idx = torch.tensor(done, dtype=torch.long, device=dev)
+            toks = st["out"][idx].cpu().tolist()
+            rows = torch.cat([idx, idx + B]) if R == 2 * B else idx
+            st["active"][rows] = 0
+            st["pos"][rows] = 0
+            st["step"][idx] = 0                                # a free slot's draw goes to out[slot, 0], which its next request rewrites
+            for i, t in zip(done, toks):
+                req = self._slots[i]
+                self._slots[i] = None
+                outs.append(RequestOutput(req.request_id, [], [CompletionOutput(0, t)], True))
+        return outs
 
     def _device_step(self, st, params: SamplingParams):
         """lg_decode_rows + lg_sample_rows on the slots' device state: logits of every row at its own position, then one draw per
@@ -154,6 +296,8 @@ class LLM:
             self._params = self._waiting[0].params           # a new running set may change the sampling parameters
         params = self._params
         st = self._ensure_state(params)
+        if self.t2i:
+            return self._step_t2i(st, params)
         B, R, S, dev = self.max_num_seqs, st["R"], st["S"], st["dev"]
         # (1) admission: requests that share the running set's sampling parameters join at position 0, mid-sequence of the others
         joined = []
@@ -203,9 +347,27 @@ class LLM:
 
     # ------------------------------------------------------------------ LLM.generate (llm.py:138-266)
     def generate(self, prompts=None, sampling_params=None, prompt_token_ids: Optional[List[List[int]]] = None,
-                 use_tqdm: bool = False) -> List[RequestOutput]:
+                 use_tqdm: bool = False, prompt_embeds=None) -> List[RequestOutput]:
+        """c2i: prompt_token_ids, one [class id] per request (with CFG followed by one [num_classes] twin each). t2i: prompt_embeds, one
+        caption's T5 features per request (see add_request). Returns the RequestOutputs sorted by request id."""
         if prompts is not None:
             raise ValueError("prompts must be None: the image models have no tokenizer (skip_tokenizer_init=True)")
+        if self.t2i:
+            if prompt_token_ids is not None or prompt_embeds is None:
+                raise ValueError("a t2i LLM takes prompt_embeds (one caption's T5 features per request), not prompt_token_ids")
+            n = len(prompt_embeds)
+            if isinstance(sampling_params, list) and len(sampling_params) != n:
+                raise ValueError("The lengths of prompts and sampling_params must be the same.")
+            per = sampling_params if isinstance(sampling_params, list) else [sampling_params or SamplingParams()] * n
+            captions = [self._caption(f) for f in prompt_embeds]       # every caption is checked before any is queued
+            for c, p in zip(captions, per):
+                self._enqueue_t2i(c, p)
+            outputs = []
+            while self.has_unfinished_requests():
+                outputs.extend(o for o in self.step() if o.finished)
+            return sorted(outputs, key=lambda o: int(o.request_id))
+        if prompt_embeds is not None:
+            raise ValueError("prompt_embeds apply to text-conditional (t2i) models")
         if prompt_token_ids is None:
             raise ValueError("Either prompts or prompt_token_ids must be provided.")
         n = len(prompt_token_ids)
