@@ -146,6 +146,20 @@ int  lg_slot_workspace_bytes(lg_engine* e, int use_cfg, size_t* bytes);
  * before any launch; the workspace needs rows >= nh * B and max_seq >= T. */
 int  lg_prefill_slot(lg_engine* e, const void* cond, const float* emb_mask, int T, int slot, int B, int use_cfg, void* dev_ws,
                      size_t ws_bytes, float* logits_out, void* stream);
+/* Bytes of caller-provided scratch for lg_prefill_slot_prefix with a prefix of P tokens, P in [0, block_size - 1] (c2i and t2i models).
+ * P = 0 gives lg_slot_workspace_bytes' size. */
+int  lg_slot_prefix_workspace_bytes(lg_engine* e, int use_cfg, int P, size_t* bytes);
+/* Start one image-completion request in slot `slot` (c2i and t2i models): lg_prefill_slot with the request's first P image tokens.
+ * cond: c2i dev int32 [1] (the class id), t2i as for lg_prefill_slot; emb_mask: t2i only (dev f32 [T] or NULL), NULL for c2i.
+ * prefix dev int32 [P], ids in [0, vocab_size), P in [0, block_size - 1] (NULL allowed only with P = 0). Writes the K / V of
+ * positions 0 .. T + P - 1 of row `slot` and, with use_cfg, of row B + slot (the null condition there), and nothing else of the
+ * workspace. logits_out dev f32 [nh, V]: the head output at position T + P - 1 (the logits of token P), rounded as lg_prefill_slot
+ * rounds them. Each row is one prefill chunk of T + P positions (lg_generate_prefix's chunk of one row), then one head GEMM over the
+ * nh rows: the arithmetic depends on neither slot, B nor any other row. dev_ws: 256-byte aligned, at least
+ * lg_slot_prefix_workspace_bytes. Every argument is checked before any launch; the workspace needs rows >= nh * B and
+ * max_seq >= T + P. lg_prefill_slot is the P = 0 case of this function (t2i only). */
+int  lg_prefill_slot_prefix(lg_engine* e, const void* cond, const float* emb_mask, int T, const int32_t* prefix, int P, int slot, int B,
+                            int use_cfg, void* dev_ws, size_t ws_bytes, float* logits_out, void* stream);
 /* lg_decode_rows for t2i models: row r takes the token embedding of tokens[r % B] at position pos_rows[r] (every row is past its
  * condition), writes its K / V there and attends over [0, pos_rows[r]]. emb_mask dev f32 [B, T] or NULL: row r attends to condition
  * key j < T iff emb_mask[r % B][j] != 0 or j is its own position (lg_generate's rule). logits_out dev f32 [R, V]. */

@@ -67,6 +67,9 @@ SIGNATURES = {
     "lg_decode_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "lg_slot_workspace_bytes": (c_int, [c_void_p, c_int, POINTER(c_size_t)]),
     "lg_prefill_slot": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "lg_slot_prefix_workspace_bytes": (c_int, [c_void_p, c_int, c_int, POINTER(c_size_t)]),
+    "lg_prefill_slot_prefix": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_size_t,
+                                       c_void_p, c_void_p]),
     "lg_decode_rows_t2i": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "lg_sample_rows": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                c_void_p]),

@@ -340,7 +340,7 @@ struct lg_engine {
     size_t carve_score(Workspace& o, char* base, int rows, int seq) const;
     size_t carve_sjd(RowBuffers& o, SjdArgs& sa, char* base, int B, int nh, int L) const;
     size_t carve_prefix(RowBuffers& o, char* base, int rows, int seq) const;
-    size_t carve_slot(RowBuffers& head, char* base, int nh) const;
+    size_t carve_slot(RowBuffers& head, char* base, int nh, int seq) const;
     void carve_kv(Carver& c, KvCache& o, int rows, int max_seq, int layers, bool f8) const;
     void carve_rows(Carver& c, RowBuffers& o, size_t M, size_t x0_rows, size_t partial_floats, size_t logits_rows) const;
     // the most partial floats one of a layer's four GEMMs needs at M rows
@@ -482,12 +482,13 @@ size_t lg_engine::carve_prefix(RowBuffers& o, char* base, int rows, int seq) con
     return c.off;
 }
 
-// lg_prefill_slot's scratch for one request of nh rows, from `base` (null: sizes only): one prefill chunk of one row of cls_token_num
-// positions (carve_prefix, from base on), then the request's nh last positions (head.q) and the partials of the head GEMM over them
-size_t lg_engine::carve_slot(RowBuffers& head, char* base, int nh) const {
+// lg_prefill_slot_prefix's scratch for one request of nh rows, from `base` (null: sizes only): one prefill chunk of one row of `seq`
+// = T + P positions (carve_prefix, from base on), then the request's nh last positions (head.q) and the partials of the head GEMM over
+// them. lg_prefill_slot's is the seq = cls_token_num case.
+size_t lg_engine::carve_slot(RowBuffers& head, char* base, int nh, int seq) const {
     const int D = cfg.dim, V = cfg.vocab_size, dt = cfg.dtype;
     RowBuffers chunk;
-    Carver c{base, 0, 1, carve_prefix(chunk, nullptr, 1, cfg.cls_token_num)};
+    Carver c{base, 0, 1, carve_prefix(chunk, nullptr, 1, seq)};
     head.q = c.split((size_t)nh * D * esz);
     head.partial_floats = std::max(gemm_partial_floats(nh, V, D, 0, dt), gemm_partial_floats(nh, V, D, 0, dt, output.scale != nullptr));
     head.partial = (float*)c.split(head.partial_floats * sizeof(float));
@@ -1107,40 +1108,65 @@ int lg_slot_workspace_bytes(lg_engine* e, int use_cfg, size_t* bytes) {
     LG_REQUIRE(e && bytes, "lg_slot_workspace_bytes: null argument");
     LG_REQUIRE(e->cfg.model_type == LG_MODEL_T2I, "lg_slot_workspace_bytes: text-conditional models only");
     RowBuffers tmp;
-    *bytes = e->carve_slot(tmp, nullptr, use_cfg ? 2 : 1);
+    *bytes = e->carve_slot(tmp, nullptr, use_cfg ? 2 : 1, e->cfg.cls_token_num);
     return 0;
 }
 
-// A join of text-conditional serving: lg_generate_prefix's prefill chunk with P = 0 over one request, once for its conditional row
-// `slot` and once, under CFG, for its unconditional row B + slot. Every call runs the same chunks at the same shapes (one row of T
-// positions, then a head GEMM over the request's nh rows), whatever the slot, B or the other requests, so a request's logits do not
-// depend on which requests join in the same step or are running.
-int lg_prefill_slot(lg_engine* e, const void* cond, const float* emb_mask, int T, int slot, int B, int use_cfg, void* dev_ws,
-                    size_t ws_bytes, float* logits_out, void* stream) {
+int lg_slot_prefix_workspace_bytes(lg_engine* e, int use_cfg, int P, size_t* bytes) {
+    LG_REQUIRE(e && bytes, "lg_slot_prefix_workspace_bytes: null argument");
+    LG_REQUIRE(P >= 0 && P <= e->cfg.block_size - 1, "lg_slot_prefix_workspace_bytes: prefix length P=%d outside [0, block_size - 1 = %d]",
+               P, e->cfg.block_size - 1);
+    RowBuffers tmp;
+    *bytes = e->carve_slot(tmp, nullptr, use_cfg ? 2 : 1, e->cfg.cls_token_num + P);
+    return 0;
+}
+
+// A join of serving: lg_generate_prefix's prefill chunk over one request, once for its conditional row `slot` and once, under CFG,
+// for its unconditional row B + slot, each one row of T + P positions (the condition, then the prefix embeddings). Every call runs the
+// same chunks at the same shapes (one row of T + P positions, then a head GEMM over the request's nh rows), whatever the slot, B or
+// the other requests, so a request's logits do not depend on which requests join in the same step or are running. lg_prefill_slot
+// is the P = 0 case; fn names the entry point in the messages.
+static int prefill_slot_impl(const char* fn, lg_engine* e, const void* cond, const float* emb_mask, int T, const int32_t* prefix, int P,
+                             int slot, int B, int use_cfg, void* dev_ws, size_t ws_bytes, float* logits_out, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
-    LG_REQUIRE(e, "lg_prefill_slot: null engine");
+    LG_REQUIRE(e, "%s: null engine", fn);
     const lg_model_cfg& c = e->cfg;
-    LG_REQUIRE(c.model_type == LG_MODEL_T2I, "lg_prefill_slot: text-conditional models only");
-    LG_REQUIRE(cond && logits_out, "lg_prefill_slot: null cond or logits_out");
-    LG_REQUIRE(T == c.cls_token_num, "lg_prefill_slot: T=%d must equal cls_token_num=%d", T, c.cls_token_num);
-    LG_REQUIRE(B > 0 && slot >= 0 && slot < B, "lg_prefill_slot: slot %d outside [0, B=%d)", slot, B);
-    const int nh = use_cfg ? 2 : 1, D = c.dim, V = c.vocab_size;
-    LG_REQUIRE(dev_ws && ((uintptr_t)dev_ws & 255) == 0, "lg_prefill_slot: scratch must be non-null and 256-byte aligned");
-    LG_TRY(check_ready(e, nh * B, T));
+    LG_REQUIRE(cond && logits_out, "%s: null cond or logits_out", fn);
+    LG_REQUIRE(T == c.cls_token_num, "%s: T=%d must equal cls_token_num=%d", fn, T, c.cls_token_num);
+    LG_REQUIRE(P == 0 || prefix, "%s: null prefix with P=%d", fn, P);
+    LG_REQUIRE(P >= 0 && P <= c.block_size - 1, "%s: prefix length P=%d outside [0, block_size - 1 = %d]", fn, P, c.block_size - 1);
+    LG_REQUIRE(B > 0 && slot >= 0 && slot < B, "%s: slot %d outside [0, B=%d)", fn, slot, B);
+    LG_REQUIRE(!emb_mask || c.model_type == LG_MODEL_T2I, "%s: emb_mask only applies to t2i models", fn);
+    const int nh = use_cfg ? 2 : 1, D = c.dim, V = c.vocab_size, seq = T + P;
+    LG_REQUIRE(dev_ws && ((uintptr_t)dev_ws & 255) == 0, "%s: scratch must be non-null and 256-byte aligned", fn);
+    LG_TRY(check_ready(e, nh * B, seq));
     RowBuffers hb;
-    const size_t need = e->carve_slot(hb, (char*)dev_ws, nh);
-    LG_REQUIRE(ws_bytes >= need, "lg_prefill_slot: scratch of %zu bytes is too small (%zu)", ws_bytes, need);
-    LG_REQUIRE(attn_plan(e->attn_args(e->full, 0, 1, T)).kernel >= 0, "lg_prefill_slot: %s", attn_plan(e->attn_args(e->full, 0, 1, T)).error);
+    const size_t need = e->carve_slot(hb, (char*)dev_ws, nh, seq);
+    LG_REQUIRE(ws_bytes >= need, "%s: scratch of %zu bytes is too small (%zu)", fn, ws_bytes, need);
+    LG_REQUIRE(attn_plan(e->attn_args(e->full, 0, 1, seq)).kernel >= 0, "%s: %s", fn, attn_plan(e->attn_args(e->full, 0, 1, seq)).error);
     DeviceGuard guard(e->device);
     LG_TRY(e->zero_fill_if_needed(st));
     for (int half = 0; half < nh; ++half)
-        LG_TRY(prefill_chunk(e, e->full, half * B + slot, 1, cond, half != 0, nullptr, emb_mask, T, 0, (char*)dev_ws, ws_bytes,
-                             hb.q + (size_t)half * D * e->esz, "lg_prefill_slot", st));
+        LG_TRY(prefill_chunk(e, e->full, half * B + slot, 1, cond, half != 0, prefix, emb_mask, T, P, (char*)dev_ws, ws_bytes,
+                             hb.q + (size_t)half * D * e->esz, fn, st));
     Workspace w;
     static_cast<RowBuffers&>(w) = hb;
     GemmNext nx_first{e->layers[0].wqkv.p, e->layers[0].wqkv.bytes(3 * D, D, e->esz), nullptr, 0};
     LG_TRY(e->head(w, hb.q, nh, logits_out, &nx_first, st));
     return round_logits_inplace(logits_out, (size_t)nh * V, c.dtype, st);
+}
+
+int lg_prefill_slot_prefix(lg_engine* e, const void* cond, const float* emb_mask, int T, const int32_t* prefix, int P, int slot, int B,
+                           int use_cfg, void* dev_ws, size_t ws_bytes, float* logits_out, void* stream) {
+    return prefill_slot_impl("lg_prefill_slot_prefix", e, cond, emb_mask, T, prefix, P, slot, B, use_cfg, dev_ws, ws_bytes, logits_out,
+                             stream);
+}
+
+int lg_prefill_slot(lg_engine* e, const void* cond, const float* emb_mask, int T, int slot, int B, int use_cfg, void* dev_ws,
+                    size_t ws_bytes, float* logits_out, void* stream) {
+    LG_REQUIRE(e, "lg_prefill_slot: null engine");
+    LG_REQUIRE(e->cfg.model_type == LG_MODEL_T2I, "lg_prefill_slot: text-conditional models only");
+    return prefill_slot_impl("lg_prefill_slot", e, cond, emb_mask, T, nullptr, 0, slot, B, use_cfg, dev_ws, ws_bytes, logits_out, stream);
 }
 
 static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, int B, int T, int S,

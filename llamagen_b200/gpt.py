@@ -204,6 +204,7 @@ class Transformer(nn.Module):
         self._sjd_ws = None
         self._prefix_ws = None
         self._slot_ws = None
+        self._slot_prefix_ws = None
         self.requires_grad_(False)
 
     # ------------------------------------------------------------------ engine plumbing
@@ -402,6 +403,14 @@ class Transformer(nn.Module):
         need = ctypes.c_size_t()
         _lib.check(lib.lg_slot_workspace_bytes(handle, int(use_cfg), ctypes.byref(need)), "lg_slot_workspace_bytes")
         return self._device_buffer("_slot_ws", need.value)
+
+    def _slot_prefix_scratch(self, use_cfg: bool, P: int):
+        """The lg_prefill_slot_prefix scratch (serve.LLM's join of one image-completion request with P given tokens), kept on the model
+        like _slot_scratch and grown to the longest prefix seen. Returns (device pointer, bytes)."""
+        lib, handle = _lib.load(), self.engine()
+        need = ctypes.c_size_t()
+        _lib.check(lib.lg_slot_prefix_workspace_bytes(handle, int(use_cfg), int(P), ctypes.byref(need)), "lg_slot_prefix_workspace_bytes")
+        return self._device_buffer("_slot_prefix_ws", need.value)
 
     def _sjd_scratch(self, B: int, use_cfg: bool, L: int):
         """The lg_generate_sjd scratch for B images and window L, kept on the model like the setup_caches() workspace.

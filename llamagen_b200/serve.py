@@ -25,6 +25,14 @@ whatever else joins or runs, so a request's tokens do not depend on the schedule
 `generate(seed=base_seed + r)` uses for image 0. CFG is internal: the unconditional row takes the learned null condition, and no
 twin requests are involved. temperature=0 decodes greedily (generate's sample_logits=False) on this path.
 
+Image completion: a request may bring its first P image tokens (`add_request(..., prefix=ids)`, `LLM.generate(..., prefixes=[...])`,
+1 <= P <= max_tokens - 1). Its join is `lg_prefill_slot_prefix`: the condition and the P tokens are prefilled into the slot's cache rows
+alone (one row of T + P positions each), token P is drawn from its logits with step P, and the request continues from position T + P
+with token index P + 1 — the draws generate(prefix=..., seed=base_seed + r) makes for image 0. A t2i completion request joins where a
+caption request joins; a c2i one joins in the admission phase (a c2i request without a prefix still starts at position 0 in the
+decode) and takes part in the same step's decode. A request whose join draws its last token (P = max_tokens - 1) finishes at its join.
+Null-class twins mirror their conditional request's prefix.
+
 While requests are in flight the LLM owns the model's KV-cache workspace (a `generate()` call on the same model would reset it)."""
 from __future__ import annotations
 
@@ -40,6 +48,7 @@ import torch
 
 from . import _lib
 from .cond import pack_t5_features, prepare_condition
+from .generate import _check_prefix
 
 
 @dataclass(frozen=True)
@@ -74,6 +83,12 @@ class _Request:
     twin_of: Optional[str] = None      # request id of the conditional request this null-class request mirrors
     cond: Optional[torch.Tensor] = None   # t2i: the prepared condition, fp32 [T, caption_dim] on the host
     mask: Optional[torch.Tensor] = None   # t2i: its emb-mask, fp32 [T]
+    prefix: Optional[torch.Tensor] = None  # image completion: the given tokens 0 .. P - 1, int64 [P] on the host
+
+
+def _plen(req: _Request) -> int:
+    """P, the number of given image tokens of a request (0 without a prefix)."""
+    return 0 if req.prefix is None else int(req.prefix.numel())
 
 
 class LLM:
@@ -107,21 +122,25 @@ class LLM:
 
     # ------------------------------------------------------------------ engine-style surface (llm_engine.py)
     def add_request(self, prompt_token_ids: Optional[Sequence[int]] = None, sampling_params: Optional[SamplingParams] = None, twin_of=None,
-                    prompt_embeds=None) -> str:
+                    prompt_embeds=None, prefix=None) -> str:
         """c2i: prompt_token_ids = [class id] (twin_of: see LLM.generate). t2i: prompt_embeds = one caption's T5 features, [n, caption_dim]
-        or the .npy layout [1, n, caption_dim] (array or tensor, n >= 1, truncated at cls_token_num)."""
+        or the .npy layout [1, n, caption_dim] (array or tensor, n >= 1, truncated at cls_token_num).
+        prefix: image completion, the first P image tokens (1-D integer ids in [0, vocab_size), 1 <= P <= max_tokens - 1); the
+        request's token_ids start with them. A null-class twin takes its conditional request's prefix (passing another one is an error)."""
         if self.t2i:
             if prompt_token_ids is not None or twin_of is not None:
                 raise ValueError("a t2i LLM takes prompt_embeds (T5 caption features), not prompt_token_ids; CFG needs no twin requests")
-            return self._enqueue_t2i(self._caption(prompt_embeds), sampling_params)
+            caption = self._caption(prompt_embeds)
+            return self._enqueue_t2i(caption, sampling_params, self._prefix(prefix, sampling_params))
         if prompt_embeds is not None:
             raise ValueError("prompt_embeds apply to text-conditional (t2i) models; a c2i prompt is prompt_token_ids = [class id]")
         if prompt_token_ids is None:
             raise ValueError("a c2i request needs prompt_token_ids = [class id]")
         if len(prompt_token_ids) != 1 or not (0 <= int(prompt_token_ids[0]) <= self.num_classes):
             raise ValueError(f"a c2i prompt is one class id in [0, {self.num_classes}], got {list(prompt_token_ids)}")
+        pf = self._prefix(prefix, sampling_params) if twin_of is None else self._twin_prefix(twin_of, prefix, sampling_params)
         rid = str(next(self.request_counter))
-        req = _Request(rid, [int(prompt_token_ids[0])], sampling_params or SamplingParams(), twin_of)
+        req = _Request(rid, [int(prompt_token_ids[0])], sampling_params or SamplingParams(), twin_of, prefix=pf)
         if twin_of is None:
             self._waiting.append(req)
         else:
@@ -145,9 +164,30 @@ class LLM:
         cond, mask = prepare_condition(embs, masks, left_padding=True)
         return cond[0], mask[0]
 
-    def _enqueue_t2i(self, caption, sampling_params: Optional[SamplingParams]) -> str:
+    def _prefix(self, prefix, sampling_params: Optional[SamplingParams]) -> Optional[torch.Tensor]:
+        """A request's prefix as int64 [P] on the host, checked as generate(prefix=...) checks it: integer ids in [0, vocab_size),
+        1 <= P <= max_tokens - 1. None stays None."""
+        if prefix is None:
+            return None
+        pf = prefix if torch.is_tensor(prefix) else torch.as_tensor(np.asarray(prefix))
+        if pf.dim() != 1:
+            raise ValueError(f"a request's prefix is 1-D, [P] image token ids, got shape {tuple(pf.shape)}")
+        S = int((sampling_params or SamplingParams()).max_tokens)
+        return _check_prefix(pf[None], 1, S, self.model.vocab_size)[0]
+
+    def _twin_prefix(self, twin_of, prefix, sampling_params: Optional[SamplingParams]) -> Optional[torch.Tensor]:
+        """The prefix of a null-class twin: its conditional request's. A prefix passed for the twin must equal it."""
+        owner = next((r for r in itertools.chain(self._waiting, self._slots) if r is not None and r.request_id == twin_of), None)
+        mine = None if owner is None else owner.prefix
+        if prefix is not None:
+            pf = self._prefix(prefix, sampling_params)
+            if mine is None or not torch.equal(pf, mine):
+                raise ValueError(f"a null-class twin mirrors the prefix of its conditional request {twin_of!r}; it was given another one")
+        return mine
+
+    def _enqueue_t2i(self, caption, sampling_params: Optional[SamplingParams], prefix: Optional[torch.Tensor] = None) -> str:
         rid = str(next(self.request_counter))
-        self._waiting.append(_Request(rid, [], sampling_params or SamplingParams(), cond=caption[0], mask=caption[1]))
+        self._waiting.append(_Request(rid, [], sampling_params or SamplingParams(), cond=caption[0], mask=caption[1], prefix=prefix))
         return rid
 
     def _running(self) -> int:
@@ -174,20 +214,21 @@ class LLM:
             active=torch.zeros(R, dtype=torch.int32, device=dev),       # 1 for rows of occupied slots
             seeds=torch.zeros(B, dtype=torch.int64, device=dev),
             out=torch.zeros(B, S, dtype=torch.int32, device=dev),
-            logits=torch.empty(R, m.vocab_size, dtype=torch.float32, device=dev))
+            logits=torch.empty(R, m.vocab_size, dtype=torch.float32, device=dev),
+            join_logits=torch.empty(R // B, m.vocab_size, dtype=torch.float32, device=dev),   # a join's logits (one request's rows)
+            join_step=torch.zeros(1, dtype=torch.int32, device=dev))  # a completion request's join draws token P: its step
         if self.t2i:
             T, C = m.cls_token_num, m.config.caption_dim
             self._state.update(
                 step=torch.zeros(B, dtype=torch.int32, device=dev),       # index of the token every slot samples next
                 cond=torch.zeros(B, T, C, dtype=m.tok_embeddings.weight.dtype, device=dev),   # every slot's condition
                 mask=torch.zeros(B, T, dtype=torch.float32, device=dev),   # and emb-mask (row r of a decode reads mask row r % B)
-                step0=torch.zeros(1, dtype=torch.int32, device=dev),      # the step of token 0, drawn by a join
-                join_logits=torch.empty(R // B, m.vocab_size, dtype=torch.float32, device=dev))
+                step0=torch.zeros(1, dtype=torch.int32, device=dev))      # the step of token 0, drawn by a join
         return self._state
 
     def _sample_cfg(self, params: SamplingParams):
-        """t2i path: temperature 0 is greedy decoding (the argmax of the mixed logits)."""
-        greedy = 1 if params.temperature == 0 else 0
+        """t2i path: temperature 0 is greedy decoding (the argmax of the mixed logits); the c2i path keeps the reference's temperature."""
+        greedy = 1 if self.t2i and params.temperature == 0 else 0
         return _lib.SampleCfg(self.cfg_scale, -1, float(params.temperature), max(0, int(params.top_k)), float(params.top_p), greedy, 0)
 
     def _device_decode_t2i(self, st, params: SamplingParams):
@@ -221,6 +262,28 @@ class LLM:
                                       _lib.ptr(st["seeds"][slot:slot + 1]), _lib.ptr(st["step0"]), _lib.ptr(st["tok"][slot:slot + 1]),
                                       _lib.ptr(st["out"][slot]), S, stream), "lg_sample_rows")
 
+    def _device_join_prefix(self, st, params: SamplingParams, slot: int, P: int):
+        """The join of a completion request with P given tokens, already in st["out"][slot, :P]: lg_prefill_slot_prefix of the slot's
+        condition (c2i: the class id in st["tok"][slot]; t2i: st["cond"][slot] and st["mask"][slot]) and the prefix, then token P drawn
+        from its logits (lg_sample_rows, one image, the slot's seed, step P) into st["out"][slot, P] and st["tok"][slot]."""
+        B, R, S, dev = self.max_num_seqs, st["R"], st["S"], st["dev"]
+        m = self.model
+        lib, handle = _lib.load(), m.engine()
+        use_cfg = 1 if R == 2 * B else 0
+        stream = _lib.current_stream(dev)
+        ws, ws_bytes = m._slot_prefix_scratch(use_cfg, P)
+        # c2i: the prefill reads the class id from tok[slot] before the draw below overwrites it (one stream)
+        cond = _lib.ptr(st["cond"][slot]) if self.t2i else _lib.ptr(st["tok"][slot:slot + 1])
+        mask = _lib.ptr(st["mask"][slot]) if self.t2i else None
+        _lib.check(lib.lg_prefill_slot_prefix(handle, cond, mask, m.cls_token_num, _lib.ptr(st["out"][slot]), P, slot, B, use_cfg, ws,
+                                              ws_bytes, _lib.ptr(st["join_logits"]), stream), "lg_prefill_slot_prefix")
+        st["join_step"].fill_(P)
+        sc = self._sample_cfg(params)
+        dt = _lib.dtype_code(m.tok_embeddings.weight.dtype)
+        _lib.check(lib.lg_sample_rows(_lib.ptr(st["join_logits"]), 1, m.vocab_size, use_cfg, dt, ctypes.byref(sc),
+                                      _lib.ptr(st["seeds"][slot:slot + 1]), _lib.ptr(st["join_step"]), _lib.ptr(st["tok"][slot:slot + 1]),
+                                      _lib.ptr(st["out"][slot]), S, stream), "lg_sample_rows")
+
     def _step_t2i(self, st, params: SamplingParams) -> List[RequestOutput]:
         """step() of a t2i LLM: decode the running slots, then admit waiting requests (their prefill draws token 0), then return the
         requests that reached max_tokens."""
@@ -234,14 +297,15 @@ class LLM:
             for i in range(B):
                 if self._slots[i] is not None:
                     self._depth[i] += 1
-        # (2) admission: the conditions and masks go to their slots' rows, then each request is prefilled alone and draws token 0
+        # (2) admission: the conditions and masks go to their slots' rows, then each request is prefilled alone and draws token 0, or,
+        # with P given tokens (written to its out row first), token P
         joined = []
         for i in range(B):
             if not self._waiting or self._waiting[0].params != params:
                 break
             if self._slots[i] is None:
                 req = self._waiting.popleft()
-                self._slots[i], self._depth[i] = req, 1
+                self._slots[i], self._depth[i] = req, _plen(req) + 1
                 joined.append((i, req))
         if joined:
             idx = torch.tensor([i for i, _ in joined], dtype=torch.long, device=dev)
@@ -249,11 +313,16 @@ class LLM:
             for i, r in joined:
                 st["cond"][i].copy_(r.cond)
                 st["mask"][i].copy_(r.mask)
-                self._device_join_t2i(st, params, i)
+                if r.prefix is None:
+                    self._device_join_t2i(st, params, i)
+                else:
+                    st["out"][i, :_plen(r)] = r.prefix.to(device=dev, dtype=torch.int32)
+                    self._device_join_prefix(st, params, i, _plen(r))
+            P = torch.tensor([_plen(r) for _, r in joined], dtype=torch.int32, device=dev)
             rows = torch.cat([idx, idx + B]) if R == 2 * B else idx
-            st["pos"][rows] = T
+            st["pos"][rows] = T + (torch.cat([P, P]) if R == 2 * B else P)
             st["active"][rows] = 1
-            st["step"][idx] = 1
+            st["step"][idx] = P + 1
         self.steps_run += 1
         # (3) the finished requests: the only device->host copy is their token rows
         done = [i for i in range(B) if self._slots[i] is not None and self._depth[i] >= S]
@@ -280,7 +349,7 @@ class LLM:
         stream = _lib.current_stream(dev)
         _lib.check(lib.lg_decode_rows(handle, _lib.ptr(st["tok"]), _lib.ptr(st["pos"]), B, use_cfg, _lib.ptr(st["logits"]), stream),
                    "lg_decode_rows")
-        sc = _lib.SampleCfg(self.cfg_scale, -1, float(params.temperature), max(0, int(params.top_k)), float(params.top_p), 0, 0)
+        sc = self._sample_cfg(params)
         dt = _lib.dtype_code(self.model.tok_embeddings.weight.dtype)   # 16-bit models round the head's logits to their dtype
         _lib.check(lib.lg_sample_rows(_lib.ptr(st["logits"]), B, self.model.vocab_size, use_cfg, dt, ctypes.byref(sc),
                                       _lib.ptr(st["seeds"]), _lib.ptr(st["pos"]), _lib.ptr(st["tok"]), _lib.ptr(st["out"]), S, stream),
@@ -315,10 +384,22 @@ class LLM:
             rows = torch.cat([idx, idx + B]) if R == 2 * B else idx
             st["pos"][rows] = 0
             st["active"][rows] = 1
+            # a completion request is prefilled through its P given tokens (written to its out row first) and draws token P here; its
+            # rows then sit at position 1 + P and this step's decode draws token P + 1
+            for i, r in joined:
+                if r.prefix is not None:
+                    P = _plen(r)
+                    st["out"][i, :P] = r.prefix.to(device=dev, dtype=torch.int32)
+                    self._device_join_prefix(st, params, i, P)
+                    st["pos"][[i, B + i] if R == 2 * B else [i]] = self.model.cls_token_num + P
+                    self._depth[i] = P + 1
+        # a request whose join drew its last token (P = max_tokens - 1) finishes now, before a decode could write past its out row
+        outs = self._finish_c2i(st, [i for i, _ in joined if self._depth[i] >= S])
         # (2) one decode step for every slot, (3) per-request sampling; the sampled token becomes the slot's next input in place
-        self._device_step(st, params)
-        st["pos"] += st["active"]
-        st["tok"] *= st["active"][:B]                        # free slots keep a valid (class 0) input; their rows are never read
+        if self._running():
+            self._device_step(st, params)
+            st["pos"] += st["active"]
+            st["tok"] *= st["active"][:B]                    # free slots keep a valid (class 0) input; their rows are never read
         self.steps_run += 1
         # (4) bookkeeping on the host (no EOS: depths are known without reading the device)
         done = []
@@ -327,6 +408,11 @@ class LLM:
                 self._depth[i] += 1
                 if self._depth[i] >= S:
                     done.append(i)
+        return outs + self._finish_c2i(st, done)
+
+    def _finish_c2i(self, st, done: List[int]) -> List[RequestOutput]:
+        """Free the c2i slots in `done` and return their requests' outputs (with their null-class twins')."""
+        B, R, dev = self.max_num_seqs, st["R"], st["dev"]
         outs: List[RequestOutput] = []
         if done:
             idx = torch.tensor(done, dtype=torch.long, device=dev)
@@ -346,10 +432,19 @@ class LLM:
         return outs
 
     # ------------------------------------------------------------------ LLM.generate (llm.py:138-266)
+    def _prefixes(self, prefixes, n: int, per: List[SamplingParams]) -> List[Optional[torch.Tensor]]:
+        """LLM.generate's prefixes, one per request (or None), each checked as add_request checks it."""
+        if prefixes is None:
+            return [None] * n
+        if len(prefixes) != n:
+            raise ValueError(f"prefixes holds {len(prefixes)} entries for {n} requests (c2i with CFG: one per conditional prompt)")
+        return [self._prefix(p, sp) for p, sp in zip(prefixes, per)]
+
     def generate(self, prompts=None, sampling_params=None, prompt_token_ids: Optional[List[List[int]]] = None,
-                 use_tqdm: bool = False, prompt_embeds=None) -> List[RequestOutput]:
+                 use_tqdm: bool = False, prompt_embeds=None, prefixes=None) -> List[RequestOutput]:
         """c2i: prompt_token_ids, one [class id] per request (with CFG followed by one [num_classes] twin each). t2i: prompt_embeds, one
-        caption's T5 features per request (see add_request). Returns the RequestOutputs sorted by request id."""
+        caption's T5 features per request (see add_request). prefixes: None, or one prefix (see add_request) or None per request; under
+        c2i CFG one per conditional prompt, which its twin mirrors. Returns the RequestOutputs sorted by request id."""
         if prompts is not None:
             raise ValueError("prompts must be None: the image models have no tokenizer (skip_tokenizer_init=True)")
         if self.t2i:
@@ -359,9 +454,10 @@ class LLM:
             if isinstance(sampling_params, list) and len(sampling_params) != n:
                 raise ValueError("The lengths of prompts and sampling_params must be the same.")
             per = sampling_params if isinstance(sampling_params, list) else [sampling_params or SamplingParams()] * n
-            captions = [self._caption(f) for f in prompt_embeds]       # every caption is checked before any is queued
-            for c, p in zip(captions, per):
-                self._enqueue_t2i(c, p)
+            captions = [self._caption(f) for f in prompt_embeds]       # every caption and prefix is checked before any is queued
+            pfx = self._prefixes(prefixes, n, per)
+            for c, p, pf in zip(captions, per, pfx):
+                self._enqueue_t2i(c, p, pf)
             outputs = []
             while self.has_unfinished_requests():
                 outputs.extend(o for o in self.step() if o.finished)
@@ -381,7 +477,8 @@ class LLM:
         if self.cfg_scale > 1.0 and not paired:
             raise ValueError("cfg_scale > 1 expects the serving protocol of serve/sample_c2i.py:35-37: the conditional prompts "
                              "followed by one [num_classes] prompt each")
-        ids = [self.add_request(prompt_token_ids[i], per[i]) for i in range(half if paired else n)]
+        pfx = self._prefixes(prefixes, half if paired else n, per)
+        ids = [self.add_request(prompt_token_ids[i], per[i], prefix=pfx[i]) for i in range(half if paired else n)]
         if paired:
             for i in range(half):
                 self.add_request(prompt_token_ids[half + i], per[half + i], twin_of=ids[i])
