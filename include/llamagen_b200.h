@@ -304,7 +304,48 @@ const char* lg_profile_class_name(int cls);   /* NULL past the last class */
  * (the reference runs the two back to back, sample_c2i_ddp.py:128-143). */
 int         lg_vq_set_cta_budget(int ctas);
 
+/* ---- T5 text encoder (transformers T5EncoderModel: Flan-T5, T5 v1.1) ------------------------------- */
+typedef struct lg_t5 lg_t5;
+typedef struct {
+    int32_t n_layer, d_model, d_kv, n_head, d_ff, vocab_size;
+    int32_t num_buckets;     /* relative_attention_num_buckets (the bucket table itself comes with every call) */
+    int32_t gated_gelu;      /* 1: feed_forward_proj "gated-gelu" (wi_0 | wi_1); 0 is refused */
+    int32_t dtype;           /* LG_DTYPE_F32 or LG_DTYPE_BF16; LG_DTYPE_F16 is refused (T5 overflows fp16 without HF's clamps) */
+    float eps;               /* layer_norm_epsilon */
+} lg_t5_cfg;
+
+/* Refuses d_kv != 64, a non-gated feed-forward, fp16 and any other dtype, with a message. */
+int  lg_t5_create(const lg_t5_cfg* cfg, int device, lg_t5** out);
+void lg_t5_destroy(lg_t5* t5);
+/* Weights by their transformers names, dev pointers in the model dtype that stay valid while the encoder lives:
+ * shared.weight [vocab][d_model]; encoder.block.{i}.layer.0.SelfAttention.{q,k,v}.weight [n_head * d_kv][d_model],
+ * .o.weight [d_model][n_head * d_kv]; encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight [num_buckets][n_head]
+ * (shared by every layer); encoder.block.{i}.layer.0.layer_norm.weight, encoder.block.{i}.layer.1.layer_norm.weight [d_model];
+ * encoder.block.{i}.layer.1.DenseReluDense.wi_0.weight, wi_1.weight [d_ff][d_model], wo.weight [d_model][d_ff];
+ * encoder.final_layer_norm.weight [d_model]. */
+int  lg_t5_bind_weight(lg_t5* t5, const char* name, const void* dev_ptr, const int64_t* shape, int ndim, int dtype);
+/* Checks every weight's name, dtype, shape and alignment. The encoder borrows the bound tensors and copies none of them, so a later
+ * in-place write to one is used by the next lg_t5_encode. Launches nothing and allocates nothing. */
+int  lg_t5_finalize(lg_t5* t5);
+/* Scratch lg_t5_encode needs for B captions of T tokens (1 <= T <= 512). Needs no GPU. */
+int  lg_t5_workspace_bytes(lg_t5* t5, int B, int T, size_t* bytes);
+/* last_hidden_state of T5EncoderModel: out (dev [B][T][d_model], model dtype) for ids and mask (dev int32 [B][T]; ids in
+ * [0, vocab), mask 1 for a valid token, 0 for padding) and buckets (dev int32 [2T - 1]: entry (j - i) + T - 1 is the relative
+ * position bucket of key j seen from query i, values in [0, num_buckets)). Every query row is computed, padded ones too; a row
+ * whose mask has no valid key yields finite values. A caption's output does not depend on B or on the other captions of the call:
+ * every GEMM runs over fixed 256-row chunks with a plan that depends on its weight shape alone. ws: 256-byte aligned, at least
+ * lg_t5_workspace_bytes. Every argument is checked before any launch. */
+int  lg_t5_encode(lg_t5* t5, const int32_t* ids, const int32_t* mask, const int32_t* buckets, int B, int T, void* ws,
+                  size_t ws_bytes, void* out, void* stream);
+
 /* ---- stand-alone kernels exported for unit parity tests ------------------------------------------- */
+/* T5 self-attention alone: out [B * T][H * 64] = softmax(q k^T + bias[bucket(j - i)][h] + mask) v per (caption, head), no 1/sqrt(d)
+ * scaling, read from qkv (dev [B * T][3 * H * 64]: q | k | v). mask (dev int32 [B][T], 0 = padded key, which weighs exactly 0),
+ * buckets (dev int32 [2T - 1]), bias (dev [num_buckets][H]); every tensor but the int32 ones in dtype. dtype LG_DTYPE_BF16 runs
+ * t5_attn_tc_kernel (mma.sync), LG_DTYPE_F32 t5_attn_kernel (CUDA cores, fp32 throughout). path: NULL or receives 1 / 0 for those. */
+int  lg_test_t5_attention(int dtype, int B, int T, int H, const void* qkv, const int32_t* mask, const int32_t* buckets, const void* bias,
+                          int num_buckets, void* out, int* path, void* stream);
+
 /* y[M,N] (f32) = x[M,K] * w[N,K]^T, operands in `dtype` (LG_DTYPE_F32, _BF16 or _F16); the same dispatch the engine uses. */
 int  lg_test_gemm(const void* x, const void* w, int M, int N, int K, int dtype, float* y,
                   void* dev_scratch, size_t scratch_bytes, void* stream);
@@ -316,6 +357,7 @@ int  lg_test_gemm(const void* x, const void* w, int M, int N, int K, int dtype, 
  *   epi 0: out_f32 [M][N] f32 = the slabs summed (reduce_f32_kernel)        epi 1: h [M][N] += T(acc) (residual_norm_kernel);
  *   with norm_out also out [M][N] = RMSNorm(h) * norm_out                  epi 2: out [M][N] = silu(T(acc_a)) * T(acc_b)
  *   epi 3: out [M][N] = T(acc)                                              epi 4: out [M][N] = gelu_tanh(T(acc)) (store_act_kernel)
+ *   epi 6 (with wb, like epi 2): out [M][N] = T(gelu_tanh(T(acc_a))) * T(acc_b) (gelu_mul_kernel: T5's gated-GELU feed-forward)
  * acc_out (f32 [M][N or 2N], optional): the slabs summed in slab order, as the epilogues sum them.
  * small = 1: one gemv_small call (bf16 / fp16, M <= 8; norm_in is its RMSNorm prologue; epi 0, 1 without norm_out, or 2; no acc_out).
  * path (int[4], optional): {kernel, tile, ksplit, row blocks or PF}; kernel 0 = gemm_skinny_kernel, 1 = gemm_mma_kernel,

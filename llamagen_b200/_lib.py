@@ -43,6 +43,11 @@ class SampleCfg(Structure):
                 ("top_k", c_int32), ("top_p", c_float), ("greedy", c_int32), ("seed", c_uint64)]
 
 
+class T5Cfg(Structure):
+    _fields_ = [("n_layer", c_int32), ("d_model", c_int32), ("d_kv", c_int32), ("n_head", c_int32), ("d_ff", c_int32),
+                ("vocab_size", c_int32), ("num_buckets", c_int32), ("gated_gelu", c_int32), ("dtype", c_int32), ("eps", c_float)]
+
+
 class VqCfg(Structure):
     _fields_ = [("codebook_size", c_int32), ("codebook_embed_dim", c_int32), ("z_channels", c_int32),
                 ("ch", c_int32), ("num_res_blocks", c_int32), ("n_mult", c_int32),
@@ -93,6 +98,14 @@ SIGNATURES = {
                                c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                                c_void_p, c_float, c_int, c_int, c_void_p, c_void_p, c_void_p, POINTER(c_int), c_void_p]),
     "lg_test_score_head": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "lg_t5_create": (c_int, [POINTER(T5Cfg), c_int, POINTER(c_void_p)]),
+    "lg_t5_destroy": (None, [c_void_p]),
+    "lg_t5_bind_weight": (c_int, [c_void_p, c_char_p, c_void_p, POINTER(c_int64), c_int, c_int]),
+    "lg_t5_finalize": (c_int, [c_void_p]),
+    "lg_t5_workspace_bytes": (c_int, [c_void_p, c_int, c_int, POINTER(c_size_t)]),
+    "lg_t5_encode": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "lg_test_t5_attention": (c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, POINTER(c_int),
+                                     c_void_p]),
     "lg_vq_create": (c_int, [POINTER(VqCfg), c_int, POINTER(c_void_p)]),
     "lg_vq_destroy": (None, [c_void_p]),
     "lg_vq_bind_weight": (c_int, [c_void_p, c_char_p, c_void_p, POINTER(c_int64), c_int]),

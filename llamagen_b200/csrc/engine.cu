@@ -1510,8 +1510,9 @@ int lg_test_gemm(const void* x, const void* w, int M, int N, int K, int dtype, f
 // tile, ksplit, row blocks or PF}
 static int test_linear_args(const char* fn, int dtype, int M, int N, int K, bool paired, bool small, int epi, bool norm_out, bool w8,
                             int* path) {
-    LG_REQUIRE(epi >= 0 && epi <= 4, "%s: epilogue %d outside 0..4", fn, epi);
-    LG_REQUIRE(paired == (epi == 2), "%s: wb goes with the SwiGLU epilogue (2) alone, epilogue %d", fn, epi);
+    LG_REQUIRE((epi >= 0 && epi <= 4) || epi == 6, "%s: epilogue %d outside 0..4 and 6", fn, epi);
+    const bool gated = epi == 2 || epi == 6;
+    LG_REQUIRE(paired == gated, "%s: wb goes with the SwiGLU epilogue (2) and the gated-GELU epilogue (6) alone, epilogue %d", fn, epi);
     LG_REQUIRE(!norm_out || (epi == 1 && !small), "%s: norm_out goes with the batched residual epilogue alone", fn);
     if (small) {
         LG_REQUIRE(epi <= 2, "%s: the small path has no store or gelu epilogue (%d)", fn, epi);
@@ -1523,7 +1524,7 @@ static int test_linear_args(const char* fn, int dtype, int M, int N, int K, bool
     const GemmPlan p = gemm_plan(M, paired ? 2 * N : N, K, paired ? N : 0, dtype, w8);
     LG_REQUIRE(p.kernel >= 0, "%s: %s", fn, p.error);
     LG_REQUIRE(epi != 1 || (N % 4 == 0 && N <= 4096), "%s: the residual epilogue needs N %% 4 == 0 and N <= 4096 (N=%d)", fn, N);
-    LG_REQUIRE(epi != 2 || N % 4 == 0, "%s: the SwiGLU epilogue needs N %% 4 == 0 (N=%d)", fn, N);
+    LG_REQUIRE(!gated || N % 4 == 0, "%s: the SwiGLU and gated-GELU epilogues need N %% 4 == 0 (N=%d)", fn, N);
     path[0] = p.kernel; path[1] = p.tile; path[2] = p.ksplit; path[3] = p.row_blocks;
     return 0;
 }
@@ -1568,6 +1569,7 @@ static int test_linear_run(const char* fn, bool w8, int dtype, int M, int N, int
         case 0: return launch_reduce_f32(partial, p.ksplit, M, N, out_f32, st);
         case 1: return launch_residual_norm(partial, p.ksplit, M, N, h, norm_out, norm_out ? out : nullptr, eps, dtype, st);
         case 2: return launch_silu_mul(partial, p.ksplit, M, N, out, dtype, st);
+        case 6: return launch_gelu_mul(partial, p.ksplit, M, N, out, dtype, st);
         default: return launch_store_act(partial, p.ksplit, M, N, out, epi == 4, dtype, st);
     }
 }

@@ -162,6 +162,8 @@ int launch_residual_norm(const float* partial, int ksplit, int M, int D, void* h
                          float eps, int dtype, cudaStream_t st);
 // out[m, j] = silu(T(p[m, j])) * T(p[m, F + j])   (gpt.py:167)
 int launch_silu_mul(const float* partial, int ksplit, int M, int F, void* out, int dtype, cudaStream_t st);
+// out[m, j] = T(gelu_tanh(T(p[m, j]))) * T(p[m, F + j])   (T5's gated-GELU feed-forward; the rounding points of launch_silu_mul)
+int launch_gelu_mul(const float* partial, int ksplit, int M, int F, void* out, int dtype, cudaStream_t st);
 // out = gelu_tanh(T(p))  (gpt.py:122-131)   /   out = T(p)
 int launch_store_act(const float* partial, int ksplit, int M, int N, void* out, int gelu, int dtype, cudaStream_t st);
 // logits f32 [R, V] = sum partial rows (only needed when ksplit > 1 or rows are strided)

@@ -217,17 +217,38 @@ __global__ void silu_mul_kernel(const float* __restrict__ partial, int ks, int M
     }
 }
 
+__device__ __forceinline__ float gelu_tanh(float v) {   // nn.GELU(approximate='tanh'), gpt.py:122; T5's NewGELUActivation
+    const float kBeta = 0.7978845608028654f, kKappa = 0.044715f;
+    const float inner = kBeta * (v + kKappa * v * v * v);
+    return 0.5f * v * (1.0f + tanhf(inner));
+}
+
+// ---------------------------------------------------------------- gated-GELU (T5DenseGatedActDense: gelu_new(wi_0 x) * wi_1 x)
+// The rounding points of silu_mul_kernel: each GEMM output is a T tensor, so is the activation, and the product is rounded on store.
+template <typename T>
+__global__ void gelu_mul_kernel(const float* __restrict__ partial, int ks, int M, int F, T* __restrict__ out) {
+    lg_pdl_sync();
+    const size_t total4 = (size_t)M * F / 4, slab = (size_t)M * 2 * F;
+    const int f4 = F / 4;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total4; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t m = i / f4, j = (i - m * f4) * 4;
+        const float4 a4 = sum_partials4(partial, m * 2 * F + j, ks, slab);
+        const float4 b4 = sum_partials4(partial, m * 2 * F + F + j, ks, slab);
+        const float a[4] = {a4.x, a4.y, a4.z, a4.w}, b[4] = {b4.x, b4.y, b4.z, b4.w};
+        float o[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) o[k] = TR<T>::round(gelu_tanh(TR<T>::round(a[k]))) * TR<T>::round(b[k]);
+        store4<T>(out + m * F + j, o[0], o[1], o[2], o[3]);
+    }
+}
+
 template <typename T>
 __global__ void store_act_kernel(const float* __restrict__ partial, int ks, size_t total, int gelu,
                                  T* __restrict__ out) {
     lg_pdl_sync();
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
         float v = TR<T>::round(sum_partials(partial, i, ks, total));
-        if (gelu) {  // nn.GELU(approximate='tanh'), gpt.py:122
-            const float kBeta = 0.7978845608028654f, kKappa = 0.044715f;
-            const float inner = kBeta * (v + kKappa * v * v * v);
-            v = 0.5f * v * (1.0f + tanhf(inner));
-        }
+        if (gelu) v = gelu_tanh(v);
         out[i] = TR<T>::from_f(v);
     }
 }
@@ -525,6 +546,18 @@ int launch_silu_mul(const float* partial, int ksplit, int M, int F, void* out, i
         dtype, [&](auto z) {
             using E = decltype(z);
             (void)lg_launch(silu_mul_kernel<E>, dim3(blocks), dim3(256), 0, st, partial, ksplit, M, F, (E*)out);
+            LG_LAUNCH_CHECK();
+            return 0;
+        });
+}
+
+int launch_gelu_mul(const float* partial, int ksplit, int M, int F, void* out, int dtype, cudaStream_t st) {
+    LG_REQUIRE(F % 4 == 0, "ffn dim %d must be a multiple of 4", F);
+    const int blocks = (int)std::min<long long>(((long long)M * F / 4 + 255) / 256, 132 * 16);
+    return dispatch_dtype(
+        dtype, [&](auto z) {
+            using E = decltype(z);
+            (void)lg_launch(gelu_mul_kernel<E>, dim3(blocks), dim3(256), 0, st, partial, ksplit, M, F, (E*)out);
             LG_LAUNCH_CHECK();
             return 0;
         });

@@ -25,6 +25,10 @@ whatever else joins or runs, so a request's tokens do not depend on the schedule
 `generate(seed=base_seed + r)` uses for image 0. CFG is internal: the unconditional row takes the learned null condition, and no
 twin requests are involved. temperature=0 decodes greedily (generate's sample_logits=False) on this path.
 
+With a text encoder (`LLM(gpt_t2i, text_encoder=t5.T5Encoder)`), a t2i request may bring its caption as a string
+(`LLM.generate(prompts=[...])`, `add_request(prompt=...)`): the batch of strings is one encoder call on the device, and each request is
+enqueued exactly as `prompt_embeds` = its valid feature rows would be, so its tokens equal those of that path.
+
 Image completion: a request may bring its first P image tokens (`add_request(..., prefix=ids)`, `LLM.generate(..., prefixes=[...])`,
 1 <= P <= max_tokens - 1). Its join is `lg_prefill_slot_prefix`: the condition and the P tokens are prefilled into the slot's cache rows
 alone (one row of T + P positions each), token P is drawn from its logits with step P, and the request continues from position T + P
@@ -93,15 +97,24 @@ def _plen(req: _Request) -> int:
 
 class LLM:
     def __init__(self, gpt_model, cfg_scale: float = 1.0, num_classes: int = 1000, max_num_seqs: int = 64, seed: Optional[int] = None,
-                 kv_cache_dtype: Optional[str] = None, weight_dtype: Optional[str] = None):
+                 kv_cache_dtype: Optional[str] = None, weight_dtype: Optional[str] = None, text_encoder=None):
         """kv_cache_dtype: None keeps the model's KV-cache setting (Transformer.set_kv_cache, scales included); "auto" (the model
         dtype) or "fp8" (e4m3) sets it. Passing the dtype the model already has keeps its scales.
         weight_dtype: None keeps the model's GEMM-weight storage (Transformer.set_weight_dtype, its head choice included); "auto" or
         "fp8" sets it.
-        A t2i model serves caption requests (prompt_embeds); num_classes does not apply to it."""
+        A t2i model serves caption requests (prompt_embeds); num_classes does not apply to it.
+        text_encoder (t2i only): a t5.T5Encoder whose d_model is the model's caption_dim. Requests may then bring caption strings
+        (generate(prompts=...), add_request(prompt=...)); each is encoded on the device and enqueued exactly as prompt_embeds = its
+        valid feature rows would be."""
         if gpt_model.model_type not in ("c2i", "t2i"):
             raise ValueError(f"serve.LLM handles c2i and t2i models, got model_type {gpt_model.model_type!r}")
         self.t2i = gpt_model.model_type == "t2i"
+        if text_encoder is not None:
+            if not self.t2i:
+                raise ValueError("a text_encoder goes with a text-conditional (t2i) model; a c2i model takes class ids")
+            if int(text_encoder.d_model) != gpt_model.config.caption_dim:
+                raise ValueError(f"text_encoder.d_model {text_encoder.d_model} != the model's caption_dim {gpt_model.config.caption_dim}")
+        self.text_encoder = text_encoder
         if kv_cache_dtype is not None and kv_cache_dtype != getattr(gpt_model, "_kv_cache", ("auto", None))[0]:
             gpt_model.set_kv_cache(kv_cache_dtype)
         if weight_dtype is not None and weight_dtype != getattr(gpt_model, "_weight_dtype", ("auto", True))[0]:
@@ -122,11 +135,14 @@ class LLM:
 
     # ------------------------------------------------------------------ engine-style surface (llm_engine.py)
     def add_request(self, prompt_token_ids: Optional[Sequence[int]] = None, sampling_params: Optional[SamplingParams] = None, twin_of=None,
-                    prompt_embeds=None, prefix=None) -> str:
+                    prompt_embeds=None, prefix=None, prompt: Optional[str] = None) -> str:
         """c2i: prompt_token_ids = [class id] (twin_of: see LLM.generate). t2i: prompt_embeds = one caption's T5 features, [n, caption_dim]
         or the .npy layout [1, n, caption_dim] (array or tensor, n >= 1, truncated at cls_token_num).
         prefix: image completion, the first P image tokens (1-D integer ids in [0, vocab_size), 1 <= P <= max_tokens - 1); the
-        request's token_ids start with them. A null-class twin takes its conditional request's prefix (passing another one is an error)."""
+        request's token_ids start with them. A null-class twin takes its conditional request's prefix (passing another one is an error).
+        prompt: a caption string, with a text_encoder only (instead of prompt_embeds)."""
+        if prompt is not None:
+            prompt_embeds = self._encode_prompts([prompt], prompt_embeds)[0]
         if self.t2i:
             if prompt_token_ids is not None or twin_of is not None:
                 raise ValueError("a t2i LLM takes prompt_embeds (T5 caption features), not prompt_token_ids; CFG needs no twin requests")
@@ -146,6 +162,18 @@ class LLM:
         else:
             self._twins[twin_of] = req
         return rid
+
+    def _encode_prompts(self, prompts, prompt_embeds=None):
+        """Caption strings -> one [valid_len, d_model] feature tensor each (one text_encoder call for the batch)."""
+        if self.text_encoder is None:
+            raise ValueError("prompts must be None: the image models have no tokenizer (skip_tokenizer_init=True)")
+        if prompt_embeds is not None:
+            raise ValueError("pass caption strings (prompts) or their features (prompt_embeds), not both")
+        prompts = [prompts] if isinstance(prompts, str) else list(prompts)
+        if not prompts or not all(isinstance(p, str) for p in prompts):
+            raise ValueError("prompts must be a non-empty list of caption strings")
+        embs, mask = self.text_encoder(prompts)
+        return [embs[i][mask[i] != 0] for i in range(len(prompts))]
 
     def _caption(self, feats):
         """One caption's (condition fp32 [T, caption_dim], emb-mask fp32 [T]) on the host, exactly as the samplers build a batch row:
@@ -446,7 +474,7 @@ class LLM:
         caption's T5 features per request (see add_request). prefixes: None, or one prefix (see add_request) or None per request; under
         c2i CFG one per conditional prompt, which its twin mirrors. Returns the RequestOutputs sorted by request id."""
         if prompts is not None:
-            raise ValueError("prompts must be None: the image models have no tokenizer (skip_tokenizer_init=True)")
+            prompt_embeds = self._encode_prompts(prompts, prompt_embeds)
         if self.t2i:
             if prompt_token_ids is not None or prompt_embeds is None:
                 raise ValueError("a t2i LLM takes prompt_embeds (one caption's T5 features per request), not prompt_token_ids")
