@@ -165,6 +165,33 @@ int  lg_prefill_slot_prefix(lg_engine* e, const void* cond, const float* emb_mas
  * key j < T iff emb_mask[r % B][j] != 0 or j is its own position (lg_generate's rule). logits_out dev f32 [R, V]. */
 int  lg_decode_rows_t2i(lg_engine* e, const int32_t* tokens, const int32_t* pos_rows, const float* emb_mask, int B, int use_cfg,
                         float* logits_out, void* stream);
+
+/* ---- negative prompts: a caption in place of the null condition of CFG ---------------------------------------------------------
+ * Every *_neg entry point is its sibling without the suffix plus one pair (neg_cond, neg_mask), and the sibling is the call with
+ * both NULL. neg_cond: NULL (the unconditional rows take uncond_embedding, as in the sibling) or dev [B, T, caption_dim] in the model
+ * dtype, one negative per image (lg_prefill_slot_prefix_neg: [T, caption_dim], the request's), prepared as cond is (left-padded,
+ * padding zeroed); the unconditional row of image b embeds neg_cond[b] instead of uncond_embedding. neg_mask: NULL (the
+ * unconditional rows attend with emb_mask's rows, as in the sibling) or dev f32 [B, T] (lg_prefill_slot_prefix_neg: [T]); the
+ * unconditional row of image b attends to condition key j < T iff neg_mask[b][j] != 0 or j is its own position. A pair that is not
+ * NULL needs a t2i model and CFG (cfg_scale > 1, or use_cfg); neg_mask needs neg_cond (lg_decode_rows_t2i_neg takes neg_mask alone)
+ * and emb_mask (all ones for an unmasked condition). Every argument is checked before any launch. The negative of
+ * uncond_embedding with neg_mask = emb_mask computes exactly what the sibling computes. */
+int  lg_generate_neg(lg_engine* e, const void* cond, const float* emb_mask, const void* neg_cond, const float* neg_mask, int B, int T, int S,
+                     const lg_sample_cfg* sc, int32_t* out_tokens, float* dbg_logits, const int32_t* teacher, void* stream);
+int  lg_generate_prefix_neg(lg_engine* e, const void* cond, const float* emb_mask, const void* neg_cond, const float* neg_mask, int B,
+                            int T, int S, const lg_sample_cfg* sc, const int32_t* prefix, int P, void* dev_ws, size_t ws_bytes,
+                            int32_t* out_tokens, float* dbg_logits, void* stream);
+int  lg_generate_sjd_neg(lg_engine* e, const void* cond, const float* emb_mask, const void* neg_cond, const float* neg_mask, int B, int T,
+                         int S, const lg_sample_cfg* sc, int L, void* dev_ws, size_t ws_bytes, int32_t* out_tokens, int32_t* iters_out,
+                         float* dbg_probs, void* stream);
+/* The join of a request with a negative (t2i): row B + slot is prefilled with neg_cond [T, caption_dim] and neg_mask [T]. */
+int  lg_prefill_slot_prefix_neg(lg_engine* e, const void* cond, const float* emb_mask, const void* neg_cond, const float* neg_mask, int T,
+                                const int32_t* prefix, int P, int slot, int B, int use_cfg, void* dev_ws, size_t ws_bytes,
+                                float* logits_out, void* stream);
+/* neg_mask dev f32 [B, T] or NULL: row B + s reads neg_mask[s] instead of emb_mask[s] (needs use_cfg and emb_mask). A serving slot
+ * without a negative keeps its emb_mask row there. */
+int  lg_decode_rows_t2i_neg(lg_engine* e, const int32_t* tokens, const int32_t* pos_rows, const float* emb_mask, const float* neg_mask,
+                            int B, int use_cfg, float* logits_out, void* stream);
 /* lg_sample with per-request RNG streams: image b draws with seed_rows[b] at token index step_rows[b] (exactly the draw a
  * batch-of-one lg_generate with that seed makes), result -> out_idx[b] and/or out_seq[b*seq_stride + step_rows[b]]. */
 int  lg_sample_rows(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc, const uint64_t* seed_rows,
@@ -400,6 +427,13 @@ int  lg_test_attention(int dtype, int kv_dtype, float k_scale, float v_scale, in
                        void* kcache, void* vcache, int n_layer, int layer, int pos_value, const int32_t* pos_dev,
                        const int32_t* pos_rows, const float* emb_mask, int B, int Tc, const void* q, const float* qkv_partial,
                        int ksplit, const float* freqs, int fuse, void* q_out, void* out, int* path, void* stream);
+/* lg_test_attention with emb_mask_uncond (dev f32 [B, Tc] or NULL, needs emb_mask): the mask rows r >= B read, row r % B of it (a
+ * negative prompt's mask); NULL is lg_test_attention. */
+int  lg_test_attention_neg(int dtype, int kv_dtype, float k_scale, float v_scale, int R, int Tq, int H, int hd, int hdp, int max_seq,
+                           void* kcache, void* vcache, int n_layer, int layer, int pos_value, const int32_t* pos_dev,
+                           const int32_t* pos_rows, const float* emb_mask, const float* emb_mask_uncond, int B, int Tc, const void* q,
+                           const float* qkv_partial, int ksplit, const float* freqs, int fuse, void* q_out, void* out, int* path,
+                           void* stream);
 /* The dispatch of lg_test_attention without buffers or a GPU: after the same checks of the shape-only arguments, plan (int[3])
  * receives the (kernel, ring depth, fused) that lg_test_attention reports for the call over an n_layer-layer buffer. pos_kind: 0 =
  * pos_value alone, 1 = a device counter plus pos_value, 2 = per-row positions (pos_value 0). input: 0 = q, 1 = QKV slabs with

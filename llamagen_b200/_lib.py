@@ -76,6 +76,15 @@ SIGNATURES = {
     "lg_prefill_slot_prefix": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_size_t,
                                        c_void_p, c_void_p]),
     "lg_decode_rows_t2i": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "lg_decode_rows_t2i_neg": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "lg_prefill_slot_prefix_neg": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int,
+                                           c_void_p, c_size_t, c_void_p, c_void_p]),
+    "lg_generate_neg": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p,
+                                c_void_p, c_void_p, c_void_p]),
+    "lg_generate_prefix_neg": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p,
+                                       c_int, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p]),
+    "lg_generate_sjd_neg": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(SampleCfg), c_int,
+                                    c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p]),
     "lg_sample_rows": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                c_void_p]),
     "lg_sample": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(SampleCfg), c_uint64, c_void_p,
@@ -136,6 +145,9 @@ SIGNATURES = {
     "lg_test_attention": (c_int, [c_int, c_int, c_float, c_float, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                                   c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int,
                                   c_void_p, c_int, c_void_p, c_void_p, POINTER(c_int), c_void_p]),
+    "lg_test_attention_neg": (c_int, [c_int, c_int, c_float, c_float, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                      c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
+                                      c_int, c_void_p, c_int, c_void_p, c_void_p, POINTER(c_int), c_void_p]),
     "lg_test_attention_plan": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
                                        POINTER(c_int)]),
     "lg_test_vq_conv": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,

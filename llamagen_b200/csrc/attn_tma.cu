@@ -58,6 +58,7 @@ struct AttnTmaArgs {   // the 16-bit tensors are bf16 or fp16 (the kernel's T); 
     const int* pos_rows;         // per-row positions [R] or null (continuous batching)
     long long row_base;          // first cache row of this layer inside the tensor maps
     const float* emb_mask; int B, Tc;
+    const float* emb_mask_uncond;   // the mask rows r >= B read, or null (attn_mask_row)
     float scale;
     // fused QKV epilogue (FUSED kernels): split-K slabs of the QKV GEMM, RoPE table, this layer's cache bases
     const float* partial; int ksplit;
@@ -258,7 +259,7 @@ __global__ void __launch_bounds__(kWarps * 32 * (PAR_ ? NST : 1), PAR_ ? 1 : (HD
             }
         }
     }
-    const float* mrow = a.emb_mask ? a.emb_mask + (size_t)(r % a.B) * a.Tc : nullptr;
+    const float* mrow = attn_mask_row(a, r);
 
     float o[HD / 8][4];
 #pragma unroll
@@ -442,7 +443,7 @@ AttnTmaArgs tma_args(const AttnArgs& a) {
     AttnTmaArgs t{};
     t.q = (const bf16*)a.q; t.out = (bf16*)a.out; t.R = a.R; t.H = a.H; t.maxS = a.maxS;
     t.pos_dev = a.pos.dev; t.pos_value = a.pos.value; t.pos_rows = a.pos.rows; t.row_base = a.cache_row_base;
-    t.emb_mask = a.emb_mask; t.B = a.B; t.Tc = a.Tc; t.scale = a.scale;
+    t.emb_mask = a.emb_mask; t.B = a.B; t.Tc = a.Tc; t.emb_mask_uncond = a.emb_mask_uncond; t.scale = a.scale;
     t.partial = a.qkv_partial; t.ksplit = a.qkv_ksplit; t.freqs = a.freqs;
     t.kcache = (bf16*)const_cast<void*>(a.kcache); t.vcache = (bf16*)const_cast<void*>(a.vcache);
     t.hd = a.hd; t.hdp = a.hdp ? a.hdp : a.hd;
@@ -571,7 +572,7 @@ __global__ void __launch_bounds__(256, 2) attn_prefill_tc_kernel(const __grid_co
         }
     }
     // ---- mask + softmax; this thread holds rows t0 = q0 + g (values [..][0..1]) and t1 = t0 + 8 (values [..][2..3])
-    const float* mrow = a.emb_mask ? a.emb_mask + (size_t)(r % a.B) * a.Tc : nullptr;
+    const float* mrow = attn_mask_row(a, r);
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int nt = 0; nt < 16; ++nt) {
@@ -754,7 +755,7 @@ __device__ __forceinline__ void causal_tc_body(const CUtensorMap& kmap, const CU
             qa[kk][3] = (t1 < Tq && d1 < hdr) ? *reinterpret_cast<const uint32_t*>(r1p + d1) : 0u;
         }
     }
-    const float* mrow = a.emb_mask ? a.emb_mask + (size_t)(r % a.B) * a.Tc : nullptr;
+    const float* mrow = attn_mask_row(a, r);
     float o[HD / 8][4];
 #pragma unroll
     for (int i = 0; i < HD / 8; ++i) { o[i][0] = 0.f; o[i][1] = 0.f; o[i][2] = 0.f; o[i][3] = 0.f; }

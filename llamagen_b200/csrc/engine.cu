@@ -243,6 +243,14 @@ struct Graph {
     }
 };
 
+// A negative prompt of the *_neg entry points: the condition of the unconditional CFG rows, cond [B, T, caption_dim] in the model
+// dtype (one per image), and their emb-mask [B, T] (null: the rows read emb_mask's, as without a negative). cond null: the null
+// condition uncond_embedding, today's unconditional rows.
+struct Negative {
+    const void* cond = nullptr;
+    const float* mask = nullptr;
+};
+
 struct Layer {
     GemmWeight wqkv, wo, w1, w3, w2;   // each in the model dtype or fp8 (w1 and w3 alike: one GEMM streams both)
     const void *attn_norm, *ffn_norm;
@@ -358,9 +366,10 @@ struct lg_engine {
         return make_attn_args(cfg.dtype, cfg.n_head, hd, hdp, kv.rows, kv.max_seq, kv.kcache, kv.vcache, kv.maps,
                               kv.kv_f8 ? &kv_scales[2 * l] : nullptr, l % kv.layers, R, Tq, kv.first_row);
     }
-    AttnArgs layer_attn(const Workspace& w, int l, int R, int Tq, PosArg pos, const float* emb_mask, int B) const {
+    AttnArgs layer_attn(const Workspace& w, int l, int R, int Tq, PosArg pos, const float* emb_mask, const float* neg_mask, int B) const {
         AttnArgs aa = attn_args(w, l, R, Tq);
         aa.q = w.q; aa.out = w.attn; aa.pos = pos; aa.emb_mask = emb_mask; aa.B = B; aa.Tc = cfg.cls_token_num;
+        aa.emb_mask_uncond = neg_mask;
         return aa;
     }
     int zero_fill_if_needed(cudaStream_t st) {
@@ -370,12 +379,15 @@ struct lg_engine {
         ws_needs_zero = false;
         return 0;
     }
-    // xn_ready: xn already holds RMSNorm_0(h) (the fused tail of the previous decode step's sample kernel wrote it)
-    int forward(const Workspace& w, int M, int Tq, PosArg pos, const float* emb_mask, int B, float* logits_out, bool xn_ready,
-                cudaStream_t st);
+    // xn_ready: xn already holds RMSNorm_0(h) (the fused tail of the previous decode step's sample kernel wrote it). Rows r < B attend
+    // with emb_mask, rows r >= B with neg_mask when it is set (a negative prompt's), else with emb_mask.
+    int forward(const Workspace& w, int M, int Tq, PosArg pos, const float* emb_mask, const float* neg_mask, int B, float* logits_out,
+                bool xn_ready, cudaStream_t st);
     // the transformer blocks over M = R * Tq rows of w.h, leaving RMSNorm_final(h) in w.xn (batched GEMM path)
-    int run_layers(const Workspace& w, int M, int Tq, PosArg pos, const float* emb_mask, int B, bool xn_ready, cudaStream_t st);
-    int embed_cond(const Workspace& w, const void* cond, int B, int R, int T, cudaStream_t st);
+    int run_layers(const Workspace& w, int M, int Tq, PosArg pos, const float* emb_mask, const float* neg_mask, int B, bool xn_ready,
+                   cudaStream_t st);
+    // the condition rows of R rows: rows r < B from cond, rows r >= B from neg_cond [R - B, T, C] (t2i) or the null condition
+    int embed_cond(const Workspace& w, const void* cond, const void* neg_cond, int B, int R, int T, cudaStream_t st);
     int gemm(const Workspace& w, const void* x, int M, int N, int K, const GemmWeight& wa, const GemmWeight& wb, int n_split, int* ksplit,
              float* direct_out, cudaStream_t st, const GemmNext* next = nullptr);
     int head(const Workspace& w, const void* x, int M, float* logits_out, const GemmNext* next, cudaStream_t st);
@@ -511,8 +523,8 @@ int lg_engine::gemm(const Workspace& w, const void* x, int M, int N, int K, cons
     return dst == direct_out ? 1 : 0;
 }
 
-int lg_engine::forward(const Workspace& w, int M, int Tq, PosArg pos, const float* emb_mask, int B, float* logits_out, bool xn_ready,
-                       cudaStream_t st) {
+int lg_engine::forward(const Workspace& w, int M, int Tq, PosArg pos, const float* emb_mask, const float* neg_mask, int B, float* logits_out,
+                       bool xn_ready, cudaStream_t st) {
     const int L = cfg.n_layer, D = cfg.dim, F = cfg.ffn_dim, V = cfg.vocab_size;
     const int R = M / Tq;
     const int dt = cfg.dtype;
@@ -522,7 +534,7 @@ int lg_engine::forward(const Workspace& w, int M, int Tq, PosArg pos, const floa
             const Layer& ly = layers[l];
             GemvSmall gq{ly.wqkv, nullptr, 3 * D, D, M, w.h, ly.attn_norm, cfg.norm_eps, w.partial, nullptr, nullptr, dt};
             LG_PROF(PC_GEMM_QKV, st, launch_gemv_small(gq, st));
-            AttnArgs aa = layer_attn(w, l, R, Tq, pos, emb_mask, B);
+            AttnArgs aa = layer_attn(w, l, R, Tq, pos, emb_mask, neg_mask, B);
             aa.qkv_partial = w.partial; aa.qkv_ksplit = 1; aa.freqs = freqs;
             LG_PROF(PC_ATTENTION, st, launch_attention(aa, st));
             GemvSmall go{ly.wo, nullptr, D, D, M, w.attn, nullptr, 0.f, nullptr, w.h, nullptr, dt};
@@ -536,7 +548,7 @@ int lg_engine::forward(const Workspace& w, int M, int Tq, PosArg pos, const floa
         LG_PROF(PC_GEMM_HEAD, st, launch_gemv_small(gh, st));
         return 0;
     }
-    LG_TRY(run_layers(w, M, Tq, pos, emb_mask, B, xn_ready, st));
+    LG_TRY(run_layers(w, M, Tq, pos, emb_mask, neg_mask, B, xn_ready, st));
     // head on the last position only (generate.py:58 reads logits[:, -1])
     const void* xlast = w.xn;
     if (Tq > 1) {
@@ -559,7 +571,8 @@ int lg_engine::head(const Workspace& w, const void* x, int M, float* logits_out,
     return 0;
 }
 
-int lg_engine::run_layers(const Workspace& w, int M, int Tq, PosArg pos, const float* emb_mask, int B, bool xn_ready, cudaStream_t st) {
+int lg_engine::run_layers(const Workspace& w, int M, int Tq, PosArg pos, const float* emb_mask, const float* neg_mask, int B, bool xn_ready,
+                          cudaStream_t st) {
     const int L = cfg.n_layer, D = cfg.dim, F = cfg.ffn_dim, V = cfg.vocab_size;
     const int R = M / Tq;
     const int dt = cfg.dtype;
@@ -574,7 +587,7 @@ int lg_engine::run_layers(const Workspace& w, int M, int Tq, PosArg pos, const f
         GemmNext nx_w2{ly.w2.p, ly.w2.bytes(D, F, eb), nullptr, 0};
         GemmNext nx_qkv{last ? output.p : layers[l + 1].wqkv.p, last ? output.bytes(V, D, eb) : layers[l + 1].wqkv.bytes(3 * D, D, eb), nullptr, 0};
         LG_PROF(PC_GEMM_QKV, st, gemm(w, w.xn, M, 3 * D, D, ly.wqkv, nullptr, 0, &ks, nullptr, st, &nx_wo));
-        AttnArgs aa = layer_attn(w, l, R, Tq, pos, emb_mask, B);
+        AttnArgs aa = layer_attn(w, l, R, Tq, pos, emb_mask, neg_mask, B);
         if (fuse_qkv(aa)) {
             aa.qkv_partial = w.partial; aa.qkv_ksplit = ks; aa.freqs = freqs;
         } else {
@@ -592,16 +605,16 @@ int lg_engine::run_layers(const Workspace& w, int M, int Tq, PosArg pos, const f
     return 0;
 }
 
-int lg_engine::embed_cond(const Workspace& w, const void* cond, int B, int R, int T, cudaStream_t st) {
+int lg_engine::embed_cond(const Workspace& w, const void* cond, const void* neg_cond, int B, int R, int T, cudaStream_t st) {
     const int D = cfg.dim, dt = cfg.dtype;
     if (cfg.model_type == LG_MODEL_C2I) {
         // LabelEmbedder (gpt.py:78-83); null class = num_classes (generate.py:130)
         return launch_embed(cls_table, (const int32_t*)cond, B, R, cfg.num_classes, D, dt, w.h, st);
     }
-    // CaptionEmbedder: cap_proj = fc2(gelu_tanh(fc1(x))) (gpt.py:110-131); uncond rows = uncond_embedding
+    // CaptionEmbedder: cap_proj = fc2(gelu_tanh(fc1(x))) (gpt.py:110-131); uncond rows = uncond_embedding, or one negative per image
     const int C = cfg.caption_dim, M = R * T;
     int ks = 1;
-    LG_TRY(launch_build_caption_rows(cond, uncond, B, R, T, C, dt, w.x0, st));
+    LG_TRY(launch_build_caption_rows(cond, neg_cond ? neg_cond : uncond, neg_cond ? (size_t)T * C : 0, B, R, T, C, dt, w.x0, st));
     LG_TRY(gemm(w, w.x0, M, D, C, cap_fc1, nullptr, 0, &ks, nullptr, st));
     LG_TRY(launch_store_act(w.partial, ks, M, D, w.attn, 1, dt, st));
     LG_TRY(gemm(w, w.attn, M, D, D, cap_fc2, nullptr, 0, &ks, nullptr, st));
@@ -625,15 +638,15 @@ static int round_logits_inplace(float* logits, size_t n, int dtype, cudaStream_t
 // One eager forward of R rows of Tq positions each (up to position seq) on the full workspace for the entry point fn: `embed` checks
 // fn's own arguments and writes the rows of h, then the forward writes the logits as the reference's head rounds them
 template <class Embed>
-static int eager_forward(const char* fn, lg_engine* e, int R, int Tq, int seq, PosArg pos, const float* emb_mask, int B, float* logits_out,
-                         void* stream, Embed&& embed) {
+static int eager_forward(const char* fn, lg_engine* e, int R, int Tq, int seq, PosArg pos, const float* emb_mask, const float* neg_mask, int B,
+                         float* logits_out, void* stream, Embed&& embed) {
     cudaStream_t st = (cudaStream_t)stream;
     LG_REQUIRE(e, "%s: null engine", fn);
     DeviceGuard guard(e->device);
     LG_TRY(check_ready(e, R, seq));
     LG_TRY(e->zero_fill_if_needed(st));
     LG_TRY(embed(st));
-    LG_TRY(e->forward(e->full, R * Tq, Tq, pos, emb_mask, B, logits_out, false, st));
+    LG_TRY(e->forward(e->full, R * Tq, Tq, pos, emb_mask, neg_mask, B, logits_out, false, st));
     return round_logits_inplace(logits_out, (size_t)R * e->cfg.vocab_size, e->cfg.dtype, st);
 }
 
@@ -854,9 +867,9 @@ int lg_prefill(lg_engine* e, const void* cond, const float* emb_mask, int B, int
     auto embed = [&](cudaStream_t st) -> int {
         LG_REQUIRE(cond && logits_out && B > 0, "lg_prefill: bad argument");
         LG_REQUIRE(T == e->cfg.cls_token_num, "lg_prefill: T=%d must equal cls_token_num=%d", T, e->cfg.cls_token_num);
-        return e->embed_cond(e->full, cond, B, R, T, st);
+        return e->embed_cond(e->full, cond, nullptr, B, R, T, st);
     };
-    return eager_forward("lg_prefill", e, R, T, T, PosArg{nullptr, 0}, emb_mask, B, logits_out, stream, embed);
+    return eager_forward("lg_prefill", e, R, T, T, PosArg{nullptr, 0}, emb_mask, nullptr, B, logits_out, stream, embed);
 }
 
 int lg_decode_step(lg_engine* e, const int32_t* tokens, int B, int pos, int use_cfg, float* logits_out, void* stream) {
@@ -865,7 +878,7 @@ int lg_decode_step(lg_engine* e, const int32_t* tokens, int B, int pos, int use_
         LG_REQUIRE(tokens && logits_out && B > 0 && pos >= 0, "lg_decode_step: bad argument");
         return launch_embed(e->tok_emb, tokens, B, R, -1, e->cfg.dim, e->cfg.dtype, e->full.h, st);
     };
-    return eager_forward("lg_decode_step", e, R, 1, pos + 1, PosArg{nullptr, pos}, nullptr, B, logits_out, stream, embed);
+    return eager_forward("lg_decode_step", e, R, 1, pos + 1, PosArg{nullptr, pos}, nullptr, nullptr, B, logits_out, stream, embed);
 }
 
 int lg_decode_rows(lg_engine* e, const int32_t* tokens, const int32_t* pos_rows, int B, int use_cfg, float* logits_out, void* stream) {
@@ -878,21 +891,47 @@ int lg_decode_rows(lg_engine* e, const int32_t* tokens, const int32_t* pos_rows,
         const lg_model_cfg& c = e->cfg;
         return launch_embed_rows(e->cls_table, e->tok_emb, tokens, pos_rows, B, R, c.num_classes, c.dim, c.dtype, e->full.h, st);
     };
-    return eager_forward("lg_decode_rows", e, R, 1, 1, PosArg{nullptr, 0, pos_rows}, nullptr, B, logits_out, stream, embed);
+    return eager_forward("lg_decode_rows", e, R, 1, 1, PosArg{nullptr, 0, pos_rows}, nullptr, nullptr, B, logits_out, stream, embed);
 }
 
-int lg_decode_rows_t2i(lg_engine* e, const int32_t* tokens, const int32_t* pos_rows, const float* emb_mask, int B, int use_cfg,
-                       float* logits_out, void* stream) {
-    // lg_decode_rows for text-conditional serving: every row is past its condition (lg_prefill_slot wrote positions 0 .. T - 1), so
-    // every row takes a token embedding; the emb-mask rows follow the rows' slots (row r reads mask row r % B)
+}  // extern "C"
+
+// The checks an entry point fn that takes a negative makes of it before any launch (e non-null)
+static int check_negative(const char* fn, const lg_engine* e, const Negative& neg, const float* emb_mask, bool use_cfg) {
+    if (!neg.cond && !neg.mask) return 0;
+    LG_REQUIRE(e->cfg.model_type == LG_MODEL_T2I, "%s: a negative condition applies to t2i models only", fn);
+    LG_REQUIRE(neg.cond, "%s: neg_mask without neg_cond", fn);
+    LG_REQUIRE(use_cfg, "%s: a negative condition replaces the unconditional CFG rows and needs CFG (cfg_scale > 1)", fn);
+    LG_REQUIRE(!neg.mask || emb_mask, "%s: neg_mask needs emb_mask (all ones for an unmasked condition)", fn);
+    return 0;
+}
+
+// lg_decode_rows for text-conditional serving: every row is past its condition (lg_prefill_slot wrote positions 0 .. T - 1), so every
+// row takes a token embedding; the emb-mask rows follow the rows' slots (row r reads mask row r % B, of neg_mask when set for r >= B)
+static int decode_rows_t2i_impl(const char* fn, lg_engine* e, const int32_t* tokens, const int32_t* pos_rows, const float* emb_mask,
+                                const float* neg_mask, int B, int use_cfg, float* logits_out, void* stream) {
     const int R = use_cfg ? 2 * B : B;
-    LG_REQUIRE(e, "lg_decode_rows_t2i: null engine");
-    LG_REQUIRE(e->cfg.model_type == LG_MODEL_T2I, "lg_decode_rows_t2i: text-conditional models only");
-    LG_REQUIRE(tokens && pos_rows && logits_out && B > 0, "lg_decode_rows_t2i: bad argument");
+    LG_REQUIRE(e, "%s: null engine", fn);
+    LG_REQUIRE(e->cfg.model_type == LG_MODEL_T2I, "%s: text-conditional models only", fn);
+    LG_REQUIRE(tokens && pos_rows && logits_out && B > 0, "%s: bad argument", fn);
+    LG_REQUIRE(!neg_mask || use_cfg, "%s: neg_mask masks the unconditional CFG rows and needs use_cfg", fn);
+    LG_REQUIRE(!neg_mask || emb_mask, "%s: neg_mask needs emb_mask (all ones for an unmasked condition)", fn);
     auto embed = [&](cudaStream_t st) -> int {
         return launch_embed(e->tok_emb, tokens, B, R, -1, e->cfg.dim, e->cfg.dtype, e->full.h, st);
     };
-    return eager_forward("lg_decode_rows_t2i", e, R, 1, 1, PosArg{nullptr, 0, pos_rows}, emb_mask, B, logits_out, stream, embed);
+    return eager_forward(fn, e, R, 1, 1, PosArg{nullptr, 0, pos_rows}, emb_mask, neg_mask, B, logits_out, stream, embed);
+}
+
+extern "C" {
+
+int lg_decode_rows_t2i(lg_engine* e, const int32_t* tokens, const int32_t* pos_rows, const float* emb_mask, int B, int use_cfg,
+                       float* logits_out, void* stream) {
+    return decode_rows_t2i_impl("lg_decode_rows_t2i", e, tokens, pos_rows, emb_mask, nullptr, B, use_cfg, logits_out, stream);
+}
+
+int lg_decode_rows_t2i_neg(lg_engine* e, const int32_t* tokens, const int32_t* pos_rows, const float* emb_mask, const float* neg_mask, int B,
+                           int use_cfg, float* logits_out, void* stream) {
+    return decode_rows_t2i_impl("lg_decode_rows_t2i_neg", e, tokens, pos_rows, emb_mask, neg_mask, B, use_cfg, logits_out, stream);
 }
 
 int lg_score_workspace_bytes(lg_engine* e, int rows, int seq, size_t* bytes) {
@@ -952,9 +991,9 @@ int lg_score(lg_engine* e, const void* cond, const float* emb_mask, const int32_
         const float* em = emb_mask ? emb_mask + (size_t)b0 * T : nullptr;
         Workspace wc = w;   // the condition rows [R * T, D] go to ff first, then the sequence embedding assembles h
         wc.h = w.ff;
-        LG_TRY(e->embed_cond(wc, cond_c, nb, R, T, st));
+        LG_TRY(e->embed_cond(wc, cond_c, nullptr, nb, R, T, st));
         LG_TRY(launch_embed_seq(w.ff, e->tok_emb, idx ? idx + (size_t)b0 * (S - 1) : nullptr, nb, R, T, seq, D, dt, w.h, st));
-        LG_TRY(e->run_layers(w, R * seq, seq, PosArg{nullptr, 0}, em, nb, false, st));
+        LG_TRY(e->run_layers(w, R * seq, seq, PosArg{nullptr, 0}, em, nullptr, nb, false, st));
         LG_TRY(launch_gather_scored(w.xn, nb, nh, seq, T, S, D, dt, w.q, st));
         // the head in chunks of at most w.head_rows rows (a CFG pair never splits)
         const int P = nb * S, per = std::max(1, w.head_rows / nh);
@@ -995,17 +1034,33 @@ struct PrefixArgs {              // lg_generate_prefix: prefix [B, P] and the pr
     char* scratch = nullptr;
     size_t scratch_bytes = 0;
 };
-static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, int B, int T, int S,
+static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, const Negative& neg, int B, int T, int S,
                          const lg_sample_cfg* sc, int32_t* out_tokens, float* dbg_logits, const int32_t* teacher,
                          const PrefixArgs& pa, cudaStream_t st);
 
-int lg_generate(lg_engine* e, const void* cond, const float* emb_mask, int B, int T, int S, const lg_sample_cfg* sc,
-                int32_t* out_tokens, float* dbg_logits, const int32_t* teacher, void* stream) {
-    LG_REQUIRE(e, "lg_generate: null engine");
+}  // extern "C"
+
+static int generate_entry(const char* fn, lg_engine* e, const void* cond, const float* emb_mask, const Negative& neg, int B, int T, int S,
+                          const lg_sample_cfg* sc, int32_t* out_tokens, float* dbg_logits, const int32_t* teacher, void* stream) {
+    LG_REQUIRE(e, "%s: null engine", fn);
+    LG_TRY(check_negative(fn, e, neg, emb_mask, sc && sc->cfg_scale > 1.0f));
     DeviceGuard guard(e->device);
     return e->run_forked((cudaStream_t)stream, lg_engine::kMaxChains, [&](cudaStream_t st) {
-        return generate_impl(e, cond, emb_mask, B, T, S, sc, out_tokens, dbg_logits, teacher, PrefixArgs{}, st);
+        return generate_impl(e, cond, emb_mask, neg, B, T, S, sc, out_tokens, dbg_logits, teacher, PrefixArgs{}, st);
     });
+}
+
+extern "C" {
+
+int lg_generate(lg_engine* e, const void* cond, const float* emb_mask, int B, int T, int S, const lg_sample_cfg* sc,
+                int32_t* out_tokens, float* dbg_logits, const int32_t* teacher, void* stream) {
+    return generate_entry("lg_generate", e, cond, emb_mask, Negative{}, B, T, S, sc, out_tokens, dbg_logits, teacher, stream);
+}
+
+int lg_generate_neg(lg_engine* e, const void* cond, const float* emb_mask, const void* neg_cond, const float* neg_mask, int B, int T, int S,
+                    const lg_sample_cfg* sc, int32_t* out_tokens, float* dbg_logits, const int32_t* teacher, void* stream) {
+    return generate_entry("lg_generate_neg", e, cond, emb_mask, Negative{neg_cond, neg_mask}, B, T, S, sc, out_tokens, dbg_logits, teacher,
+                          stream);
 }
 
 int lg_prefix_workspace_bytes(lg_engine* e, int rows, int seq, size_t* bytes) {
@@ -1015,26 +1070,45 @@ int lg_prefix_workspace_bytes(lg_engine* e, int rows, int seq, size_t* bytes) {
     return 0;
 }
 
-int lg_generate_prefix(lg_engine* e, const void* cond, const float* emb_mask, int B, int T, int S, const lg_sample_cfg* sc,
-                       const int32_t* prefix, int P, void* dev_ws, size_t ws_bytes, int32_t* out_tokens, float* dbg_logits, void* stream) {
-    LG_REQUIRE(e && e->finalized, "lg_generate_prefix: engine not finalized");
+}  // extern "C"
+
+static int generate_prefix_entry(const char* fn, lg_engine* e, const void* cond, const float* emb_mask, const Negative& neg, int B, int T,
+                                 int S, const lg_sample_cfg* sc, const int32_t* prefix, int P, void* dev_ws, size_t ws_bytes,
+                                 int32_t* out_tokens, float* dbg_logits, void* stream) {
+    LG_REQUIRE(e && e->finalized, "%s: engine not finalized", fn);
     DeviceGuard guard(e->device);
     const lg_model_cfg& c = e->cfg;
-    LG_REQUIRE(cond && sc && out_tokens && B > 0 && S > 0, "lg_generate_prefix: null argument or B=%d S=%d", B, S);
-    LG_REQUIRE(prefix, "lg_generate_prefix: null prefix");
-    LG_REQUIRE(P >= 1 && P <= S - 1, "lg_generate_prefix: prefix length P=%d outside [1, S - 1] (S=%d)", P, S);
-    LG_REQUIRE(T == c.cls_token_num, "lg_generate_prefix: T=%d must equal cls_token_num=%d", T, c.cls_token_num);
-    LG_REQUIRE(!emb_mask || c.model_type == LG_MODEL_T2I, "lg_generate_prefix: emb_mask only applies to t2i models");
+    LG_REQUIRE(cond && sc && out_tokens && B > 0 && S > 0, "%s: null argument or B=%d S=%d", fn, B, S);
+    LG_REQUIRE(prefix, "%s: null prefix", fn);
+    LG_REQUIRE(P >= 1 && P <= S - 1, "%s: prefix length P=%d outside [1, S - 1] (S=%d)", fn, P, S);
+    LG_REQUIRE(T == c.cls_token_num, "%s: T=%d must equal cls_token_num=%d", fn, T, c.cls_token_num);
+    LG_REQUIRE(!emb_mask || c.model_type == LG_MODEL_T2I, "%s: emb_mask only applies to t2i models", fn);
     const int nh = sc->cfg_scale > 1.0f ? 2 : 1;   // generate.py:128
+    LG_TRY(check_negative(fn, e, neg, emb_mask, nh == 2));
     LG_TRY(check_ready(e, nh * B, T + S));
-    LG_REQUIRE(dev_ws && ((uintptr_t)dev_ws & 255) == 0, "lg_generate_prefix: scratch must be non-null and 256-byte aligned");
+    LG_REQUIRE(dev_ws && ((uintptr_t)dev_ws & 255) == 0, "%s: scratch must be non-null and 256-byte aligned", fn);
     RowBuffers one;
     const size_t need1 = e->carve_prefix(one, nullptr, nh, T + P);
-    LG_REQUIRE(ws_bytes >= need1, "lg_generate_prefix: scratch of %zu bytes is too small for one image (%zu)", ws_bytes, need1);
+    LG_REQUIRE(ws_bytes >= need1, "%s: scratch of %zu bytes is too small for one image (%zu)", fn, ws_bytes, need1);
     const PrefixArgs pa{prefix, P, (char*)dev_ws, ws_bytes};
     return e->run_forked((cudaStream_t)stream, lg_engine::kMaxChains, [&](cudaStream_t st) {
-        return generate_impl(e, cond, emb_mask, B, T, S, sc, out_tokens, dbg_logits, nullptr, pa, st);
+        return generate_impl(e, cond, emb_mask, neg, B, T, S, sc, out_tokens, dbg_logits, nullptr, pa, st);
     });
+}
+
+extern "C" {
+
+int lg_generate_prefix(lg_engine* e, const void* cond, const float* emb_mask, int B, int T, int S, const lg_sample_cfg* sc,
+                       const int32_t* prefix, int P, void* dev_ws, size_t ws_bytes, int32_t* out_tokens, float* dbg_logits, void* stream) {
+    return generate_prefix_entry("lg_generate_prefix", e, cond, emb_mask, Negative{}, B, T, S, sc, prefix, P, dev_ws, ws_bytes, out_tokens,
+                                 dbg_logits, stream);
+}
+
+int lg_generate_prefix_neg(lg_engine* e, const void* cond, const float* emb_mask, const void* neg_cond, const float* neg_mask, int B, int T,
+                           int S, const lg_sample_cfg* sc, const int32_t* prefix, int P, void* dev_ws, size_t ws_bytes, int32_t* out_tokens,
+                           float* dbg_logits, void* stream) {
+    return generate_prefix_entry("lg_generate_prefix_neg", e, cond, emb_mask, Negative{neg_cond, neg_mask}, B, T, S, sc, prefix, P, dev_ws,
+                                 ws_bytes, out_tokens, dbg_logits, stream);
 }
 
 int lg_test_prefix_chunks(lg_engine* e, int* chains) {
@@ -1050,6 +1124,7 @@ struct Chain {
     cudaStream_t st = nullptr;
     const void* cond = nullptr;
     const float* emb_mask = nullptr;
+    Negative neg;                      // this chain's images' negatives (null: the null condition)
     const int32_t* prefix = nullptr;   // [B, P] of this chain's images (lg_generate_prefix)
     int B = 0, R = 0;
     SampleArgs sa{};
@@ -1059,12 +1134,13 @@ struct Chain {
 
 // One chunk of a condition (+ prefix) prefill: positions 0 .. T + P - 1 of n contiguous cache rows of `kv` from row r0 on, in one
 // forward over the row buffers of `scratch`. The rows are n images embedded with their condition (cond: the chunk's first image's),
-// or with the null condition when `uncond`, then their prefix embeddings (prefix [n, P], unread when P = 0); emb_mask [n, T] or null.
+// or, when `uncond`, with their negatives (neg_cond [n, T, C], the chunk's first image's) or without one the null condition, then
+// their prefix embeddings (prefix [n, P], unread when P = 0); emb_mask [n, T] (the mask of the rows' half) or null.
 // The attention runs at first_row = r0 over the maps of the whole view, so only rows r0 .. r0 + n - 1 of the cache are written. The
 // last position of every row is gathered to `last` [n, D].
-static int prefill_chunk(lg_engine* e, const KvCache& kv, int r0, int n, const void* cond, bool uncond, const int32_t* prefix,
-                         const float* emb_mask, int T, int P, char* scratch, size_t scratch_bytes, void* last, const char* fn,
-                         cudaStream_t st) {
+static int prefill_chunk(lg_engine* e, const KvCache& kv, int r0, int n, const void* cond, bool uncond, const void* neg_cond,
+                         const int32_t* prefix, const float* emb_mask, int T, int P, char* scratch, size_t scratch_bytes, void* last,
+                         const char* fn, cudaStream_t st) {
     const int D = e->cfg.dim, dt = e->cfg.dtype, seq = T + P;
     Workspace w;
     static_cast<KvCache&>(w) = kv;
@@ -1072,16 +1148,16 @@ static int prefill_chunk(lg_engine* e, const KvCache& kv, int r0, int n, const v
     LG_REQUIRE(e->carve_prefix(w, scratch, n, seq) <= scratch_bytes, "%s: a chunk of %d rows outgrows the scratch", fn, n);
     Workspace wc = w;   // the condition rows [n * T, D] go to ff first, then the sequence embedding assembles h
     wc.h = w.ff;
-    LG_TRY(e->embed_cond(wc, cond, uncond ? 0 : n, n, T, st));   // B = 0: every row takes the null condition
+    LG_TRY(e->embed_cond(wc, cond, neg_cond, uncond ? 0 : n, n, T, st));   // B = 0: every row takes the negative or null condition
     LG_TRY(launch_embed_seq(w.ff, e->tok_emb, prefix, n, n, T, seq, D, dt, w.h, st));
-    LG_TRY(e->run_layers(w, n * seq, seq, PosArg{nullptr, 0}, emb_mask, n, false, st));
+    LG_TRY(e->run_layers(w, n * seq, seq, PosArg{nullptr, 0}, emb_mask, nullptr, n, false, st));
     return launch_gather_last(w.xn, n, seq, D, dt, last, st);
 }
 
 // lg_generate_prefix's prefill of chain k: positions 0 .. T + P - 1 (the condition, then the prefix embeddings) of every row in one
 // forward, its K / V written into the chain's cache. The rows go in chunks of at most `nr` contiguous cache rows of the chain's view
 // that stay inside its conditional rows [0, B) or its unconditional rows [B, 2B): a chunk is then images img0 .. img0 + n - 1 of one
-// half, embedded with the condition of those images or the null condition, and its attention runs at first_row = its first cache
+// half, embedded with the condition of those images or their negatives (the null condition without), and its attention runs at first_row = its first cache
 // row over the maps of the whole view. Chunks also never cross a block of `blk` images (the images of one chain under the largest
 // split), so one and two chains run the same chunks with the same GEMM plans: the results are bit-identical. The chunk's last
 // positions are gathered into k.w.q rows, and one head GEMM over the R rows leaves the logits of token P in k.w.logits.
@@ -1095,9 +1171,11 @@ static int prefix_prefill(lg_engine* e, Chain& k, int nh, int T, int P, int nr, 
             const int n = std::min(nr, b1 - img0), r0 = half * k.B + img0;
             const void* cond_c = c.model_type == LG_MODEL_C2I ? (const void*)((const int32_t*)k.cond + img0)
                                                               : (const void*)((const char*)k.cond + (size_t)img0 * T * c.caption_dim * esz);
-            const float* em = k.emb_mask ? k.emb_mask + (size_t)img0 * T : nullptr;
-            LG_TRY(prefill_chunk(e, k.w, r0, n, cond_c, half != 0, k.prefix + (size_t)img0 * P, em, T, P, pa.scratch, pa.scratch_bytes,
-                                 k.w.q + (size_t)r0 * D * esz, "lg_generate_prefix", st));
+            const float* mask = half != 0 && k.neg.mask ? k.neg.mask : k.emb_mask;
+            const float* em = mask ? mask + (size_t)img0 * T : nullptr;
+            const void* neg_c = k.neg.cond ? (const char*)k.neg.cond + (size_t)img0 * T * c.caption_dim * esz : nullptr;
+            LG_TRY(prefill_chunk(e, k.w, r0, n, cond_c, half != 0, neg_c, k.prefix + (size_t)img0 * P, em, T, P, pa.scratch,
+                                 pa.scratch_bytes, k.w.q + (size_t)r0 * D * esz, "lg_generate_prefix", st));
             ++e->prefix_chunks;
         }
     GemmNext nx_first{e->layers[0].wqkv.p, e->layers[0].wqkv.bytes(3 * D, D, esz), nullptr, 0};
@@ -1126,8 +1204,9 @@ int lg_slot_prefix_workspace_bytes(lg_engine* e, int use_cfg, int P, size_t* byt
 // same chunks at the same shapes (one row of T + P positions, then a head GEMM over the request's nh rows), whatever the slot, B or
 // the other requests, so a request's logits do not depend on which requests join in the same step or are running. lg_prefill_slot
 // is the P = 0 case; fn names the entry point in the messages.
-static int prefill_slot_impl(const char* fn, lg_engine* e, const void* cond, const float* emb_mask, int T, const int32_t* prefix, int P,
-                             int slot, int B, int use_cfg, void* dev_ws, size_t ws_bytes, float* logits_out, void* stream) {
+static int prefill_slot_impl(const char* fn, lg_engine* e, const void* cond, const float* emb_mask, const Negative& neg, int T,
+                             const int32_t* prefix, int P, int slot, int B, int use_cfg, void* dev_ws, size_t ws_bytes, float* logits_out,
+                             void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     LG_REQUIRE(e, "%s: null engine", fn);
     const lg_model_cfg& c = e->cfg;
@@ -1137,6 +1216,7 @@ static int prefill_slot_impl(const char* fn, lg_engine* e, const void* cond, con
     LG_REQUIRE(P >= 0 && P <= c.block_size - 1, "%s: prefix length P=%d outside [0, block_size - 1 = %d]", fn, P, c.block_size - 1);
     LG_REQUIRE(B > 0 && slot >= 0 && slot < B, "%s: slot %d outside [0, B=%d)", fn, slot, B);
     LG_REQUIRE(!emb_mask || c.model_type == LG_MODEL_T2I, "%s: emb_mask only applies to t2i models", fn);
+    LG_TRY(check_negative(fn, e, neg, emb_mask, use_cfg != 0));
     const int nh = use_cfg ? 2 : 1, D = c.dim, V = c.vocab_size, seq = T + P;
     LG_REQUIRE(dev_ws && ((uintptr_t)dev_ws & 255) == 0, "%s: scratch must be non-null and 256-byte aligned", fn);
     LG_TRY(check_ready(e, nh * B, seq));
@@ -1147,8 +1227,8 @@ static int prefill_slot_impl(const char* fn, lg_engine* e, const void* cond, con
     DeviceGuard guard(e->device);
     LG_TRY(e->zero_fill_if_needed(st));
     for (int half = 0; half < nh; ++half)
-        LG_TRY(prefill_chunk(e, e->full, half * B + slot, 1, cond, half != 0, prefix, emb_mask, T, P, (char*)dev_ws, ws_bytes,
-                             hb.q + (size_t)half * D * e->esz, fn, st));
+        LG_TRY(prefill_chunk(e, e->full, half * B + slot, 1, cond, half != 0, neg.cond, prefix, half != 0 && neg.mask ? neg.mask : emb_mask,
+                             T, P, (char*)dev_ws, ws_bytes, hb.q + (size_t)half * D * e->esz, fn, st));
     Workspace w;
     static_cast<RowBuffers&>(w) = hb;
     GemmNext nx_first{e->layers[0].wqkv.p, e->layers[0].wqkv.bytes(3 * D, D, e->esz), nullptr, 0};
@@ -1158,18 +1238,26 @@ static int prefill_slot_impl(const char* fn, lg_engine* e, const void* cond, con
 
 int lg_prefill_slot_prefix(lg_engine* e, const void* cond, const float* emb_mask, int T, const int32_t* prefix, int P, int slot, int B,
                            int use_cfg, void* dev_ws, size_t ws_bytes, float* logits_out, void* stream) {
-    return prefill_slot_impl("lg_prefill_slot_prefix", e, cond, emb_mask, T, prefix, P, slot, B, use_cfg, dev_ws, ws_bytes, logits_out,
-                             stream);
+    return prefill_slot_impl("lg_prefill_slot_prefix", e, cond, emb_mask, Negative{}, T, prefix, P, slot, B, use_cfg, dev_ws, ws_bytes,
+                             logits_out, stream);
+}
+
+int lg_prefill_slot_prefix_neg(lg_engine* e, const void* cond, const float* emb_mask, const void* neg_cond, const float* neg_mask, int T,
+                               const int32_t* prefix, int P, int slot, int B, int use_cfg, void* dev_ws, size_t ws_bytes, float* logits_out,
+                               void* stream) {
+    return prefill_slot_impl("lg_prefill_slot_prefix_neg", e, cond, emb_mask, Negative{neg_cond, neg_mask}, T, prefix, P, slot, B, use_cfg,
+                             dev_ws, ws_bytes, logits_out, stream);
 }
 
 int lg_prefill_slot(lg_engine* e, const void* cond, const float* emb_mask, int T, int slot, int B, int use_cfg, void* dev_ws,
                     size_t ws_bytes, float* logits_out, void* stream) {
     LG_REQUIRE(e, "lg_prefill_slot: null engine");
     LG_REQUIRE(e->cfg.model_type == LG_MODEL_T2I, "lg_prefill_slot: text-conditional models only");
-    return prefill_slot_impl("lg_prefill_slot", e, cond, emb_mask, T, nullptr, 0, slot, B, use_cfg, dev_ws, ws_bytes, logits_out, stream);
+    return prefill_slot_impl("lg_prefill_slot", e, cond, emb_mask, Negative{}, T, nullptr, 0, slot, B, use_cfg, dev_ws, ws_bytes, logits_out,
+                             stream);
 }
 
-static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, int B, int T, int S,
+static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, const Negative& neg, int B, int T, int S,
                          const lg_sample_cfg* sc, int32_t* out_tokens, float* dbg_logits, const int32_t* teacher,
                          const PrefixArgs& pa, cudaStream_t st0) {
     LG_REQUIRE(cond && sc && out_tokens && B > 0 && S > 0, "lg_generate: bad argument");
@@ -1198,6 +1286,8 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
         k.cond = c.model_type == LG_MODEL_C2I ? (const void*)((const int32_t*)cond + boff)
                                               : (const void*)((const char*)cond + boff * T * c.caption_dim * e->esz);
         k.emb_mask = emb_mask ? emb_mask + boff * T : nullptr;
+        k.neg.cond = neg.cond ? (const void*)((const char*)neg.cond + boff * T * c.caption_dim * e->esz) : nullptr;
+        k.neg.mask = neg.mask ? neg.mask + boff * T : nullptr;
         k.prefix = pa.prefix ? pa.prefix + boff * pa.P : nullptr;
         k.sa = make_sample_args(*sc, k.w.logits, k.B, c.vocab_size, use_cfg, c.dtype);
         SampleArgs& sa = k.sa;
@@ -1226,7 +1316,7 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
         // with the fused tail the previous iteration's sample kernel left h (and xn) in place
         if (!fuse_tail) LG_PROF(PC_EMBED_MISC, k.st, launch_embed(e->tok_emb, k.w.tokens, k.B, k.R, -1, c.dim, c.dtype, k.w.h, k.st));
         const bool xn_ready = fuse_tail && k.sa.emb_xn != nullptr;
-        LG_TRY(e->forward(k.w, k.R, 1, PosArg{d_pos, 0}, k.emb_mask, k.B, k.w.logits, xn_ready, k.st));
+        LG_TRY(e->forward(k.w, k.R, 1, PosArg{d_pos, 0}, k.emb_mask, k.neg.mask, k.B, k.w.logits, xn_ready, k.st));
         LG_PROF(PC_SAMPLE, k.st, launch_sample(k.sa, k.st));
         if (!fuse_tail) LG_PROF(PC_EMBED_MISC, k.st, launch_advance(d_pos, d_step, k.st));
         return 0;
@@ -1263,8 +1353,8 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
     for (int g = 0; g < nchains; ++g) {
         Chain& k = ch[g];
         if (P == 0) {
-            LG_TRY(e->embed_cond(k.w, k.cond, k.B, k.R, T, k.st));
-            LG_TRY(e->forward(k.w, k.R * T, T, PosArg{nullptr, 0}, k.emb_mask, k.B, k.w.logits, false, k.st));
+            LG_TRY(e->embed_cond(k.w, k.cond, k.neg.cond, k.B, k.R, T, k.st));
+            LG_TRY(e->forward(k.w, k.R * T, T, PosArg{nullptr, 0}, k.emb_mask, k.neg.mask, k.B, k.w.logits, false, k.st));
         }
         k.sa.step = P; k.sa.step_dev = nullptr;
         const bool tail = S > P + 1 && fuse_tail;
@@ -1300,16 +1390,16 @@ int lg_sjd_workspace_bytes(lg_engine* e, int B, int use_cfg, int L, size_t* byte
     return 0;
 }
 
-static int generate_sjd_impl(lg_engine* e, const Workspace& w, SjdArgs& sa, const void* cond, const float* emb_mask, const lg_sample_cfg& sc,
-                             bool use_cfg, int32_t* iters_out, cudaStream_t st) {
+static int generate_sjd_impl(lg_engine* e, const Workspace& w, SjdArgs& sa, const void* cond, const float* emb_mask, const Negative& neg,
+                             const lg_sample_cfg& sc, bool use_cfg, int32_t* iters_out, cudaStream_t st) {
     const lg_model_cfg& c = e->cfg;
     const int B = sa.B, S = sa.S, L = sa.L, T = sa.T, V = c.vocab_size, D = c.dim, dt = c.dtype, R = sa.nh * B, M = R * L;
     static int calls = 0;
     sa.done_token = ++calls;   // a pass still in flight from an earlier call cannot end this one
     LG_CUDA_OK(cudaMemsetAsync(sa.state, 0, kSjdStateInts * sizeof(int32_t), st));
     // prefill and token 0, drawn as lg_generate draws it
-    LG_TRY(e->embed_cond(e->full, cond, B, R, T, st));
-    LG_TRY(e->forward(e->full, R * T, T, PosArg{nullptr, 0}, emb_mask, B, e->full.logits, false, st));
+    LG_TRY(e->embed_cond(e->full, cond, neg.cond, B, R, T, st));
+    LG_TRY(e->forward(e->full, R * T, T, PosArg{nullptr, 0}, emb_mask, neg.mask, B, e->full.logits, false, st));
     SampleArgs s0 = make_sample_args(sc, e->full.logits, B, V, use_cfg, dt);
     s0.step = 0; s0.out_seq = sa.out; s0.seq_stride = S;
     LG_TRY(launch_sample(s0, st));
@@ -1321,7 +1411,7 @@ static int generate_sjd_impl(lg_engine* e, const Workspace& w, SjdArgs& sa, cons
     sp.out_idx = const_cast<int32_t*>(sa.x); sp.out_probs = const_cast<float*>(sa.p);
     auto pass = [&]() -> int {
         LG_PROF(PC_EMBED_MISC, st, launch_embed(e->tok_emb, sa.win, B * L, M, -1, D, dt, w.h, st));
-        LG_TRY(e->run_layers(w, M, L, PosArg{nullptr, 0, sa.pos_rows}, emb_mask, B, false, st));
+        LG_TRY(e->run_layers(w, M, L, PosArg{nullptr, 0, sa.pos_rows}, emb_mask, neg.mask, B, false, st));
         LG_TRY(e->head(w, w.xn, M, w.logits, nullptr, st));
         LG_PROF(PC_SAMPLE, st, launch_sample(sp, st));
         LG_PROF(PC_SAMPLE, st, launch_sjd_verify(sa, st));
@@ -1348,26 +1438,30 @@ static int generate_sjd_impl(lg_engine* e, const Workspace& w, SjdArgs& sa, cons
     return 0;
 }
 
-int lg_generate_sjd(lg_engine* e, const void* cond, const float* emb_mask, int B, int T, int S, const lg_sample_cfg* sc, int L,
-                    void* dev_ws, size_t ws_bytes, int32_t* out_tokens, int32_t* iters_out, float* dbg_probs, void* stream) {
-    LG_REQUIRE(e && e->finalized, "lg_generate_sjd: engine not finalized");
+}  // extern "C"
+
+static int generate_sjd_entry(const char* fn, lg_engine* e, const void* cond, const float* emb_mask, const Negative& neg, int B, int T, int S,
+                              const lg_sample_cfg* sc, int L, void* dev_ws, size_t ws_bytes, int32_t* out_tokens, int32_t* iters_out,
+                              float* dbg_probs, void* stream) {
+    LG_REQUIRE(e && e->finalized, "%s: engine not finalized", fn);
     DeviceGuard guard(e->device);
     const lg_model_cfg& c = e->cfg;
-    LG_REQUIRE(cond && sc && out_tokens && iters_out && B > 0, "lg_generate_sjd: null argument or B=%d", B);
-    LG_REQUIRE(L >= 2 && L <= 64, "lg_generate_sjd: window L=%d outside [2, 64]", L);
-    LG_REQUIRE(S > L && S <= c.block_size, "lg_generate_sjd: S=%d must lie in [L + 1, block_size=%d] (L=%d)", S, c.block_size, L);
-    LG_REQUIRE(T == c.cls_token_num, "lg_generate_sjd: T=%d must equal cls_token_num=%d", T, c.cls_token_num);
-    LG_REQUIRE(!emb_mask || c.model_type == LG_MODEL_T2I, "lg_generate_sjd: emb_mask only applies to t2i models");
-    LG_REQUIRE((size_t)c.vocab_size * sizeof(float) <= 200 * 1024, "lg_generate_sjd: vocab %d too large for the sampler", c.vocab_size);
+    LG_REQUIRE(cond && sc && out_tokens && iters_out && B > 0, "%s: null argument or B=%d", fn, B);
+    LG_REQUIRE(L >= 2 && L <= 64, "%s: window L=%d outside [2, 64]", fn, L);
+    LG_REQUIRE(S > L && S <= c.block_size, "%s: S=%d must lie in [L + 1, block_size=%d] (L=%d)", fn, S, c.block_size, L);
+    LG_REQUIRE(T == c.cls_token_num, "%s: T=%d must equal cls_token_num=%d", fn, T, c.cls_token_num);
+    LG_REQUIRE(!emb_mask || c.model_type == LG_MODEL_T2I, "%s: emb_mask only applies to t2i models", fn);
+    LG_REQUIRE((size_t)c.vocab_size * sizeof(float) <= 200 * 1024, "%s: vocab %d too large for the sampler", fn, c.vocab_size);
     const bool use_cfg = sc->cfg_scale > 1.0f;   // generate.py:128
+    LG_TRY(check_negative(fn, e, neg, emb_mask, use_cfg));
     const int nh = use_cfg ? 2 : 1, R = nh * B;
     LG_TRY(check_ready(e, R, T + S));
-    LG_REQUIRE((long long)R * L <= 65535, "lg_generate_sjd: %d rows x window %d exceed 65535 query rows", R, L);
-    LG_REQUIRE(dev_ws && ((uintptr_t)dev_ws & 255) == 0, "lg_generate_sjd: scratch must be non-null and 256-byte aligned");
+    LG_REQUIRE((long long)R * L <= 65535, "%s: %d rows x window %d exceed 65535 query rows", fn, R, L);
+    LG_REQUIRE(dev_ws && ((uintptr_t)dev_ws & 255) == 0, "%s: scratch must be non-null and 256-byte aligned", fn);
     Workspace w;   // the KV cache and its maps of the workspace, the row buffers of the scratch
     SjdArgs sa{};
     const size_t need = e->carve_sjd(w, sa, (char*)dev_ws, B, nh, L);
-    LG_REQUIRE(ws_bytes >= need, "lg_generate_sjd: scratch of %zu bytes is too small (%zu)", ws_bytes, need);
+    LG_REQUIRE(ws_bytes >= need, "%s: scratch of %zu bytes is too small (%zu)", fn, ws_bytes, need);
     static_cast<KvCache&>(w) = e->full;
     sa.B = B; sa.S = S; sa.L = L; sa.V = c.vocab_size; sa.T = T; sa.nh = nh;
     sa.greedy = sc->greedy; sa.seed = sc->seed; sa.row_offset = 0;
@@ -1378,8 +1472,23 @@ int lg_generate_sjd(lg_engine* e, const void* cond, const float* emb_mask, int B
         for (cudaEvent_t& ev : e->ev_pass) LG_CUDA_OK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
     }
     return e->run_forked((cudaStream_t)stream, 1, [&](cudaStream_t st) {
-        return generate_sjd_impl(e, w, sa, cond, emb_mask, *sc, use_cfg, iters_out, st);
+        return generate_sjd_impl(e, w, sa, cond, emb_mask, neg, *sc, use_cfg, iters_out, st);
     });
+}
+
+extern "C" {
+
+int lg_generate_sjd(lg_engine* e, const void* cond, const float* emb_mask, int B, int T, int S, const lg_sample_cfg* sc, int L,
+                    void* dev_ws, size_t ws_bytes, int32_t* out_tokens, int32_t* iters_out, float* dbg_probs, void* stream) {
+    return generate_sjd_entry("lg_generate_sjd", e, cond, emb_mask, Negative{}, B, T, S, sc, L, dev_ws, ws_bytes, out_tokens, iters_out,
+                              dbg_probs, stream);
+}
+
+int lg_generate_sjd_neg(lg_engine* e, const void* cond, const float* emb_mask, const void* neg_cond, const float* neg_mask, int B, int T,
+                        int S, const lg_sample_cfg* sc, int L, void* dev_ws, size_t ws_bytes, int32_t* out_tokens, int32_t* iters_out,
+                        float* dbg_probs, void* stream) {
+    return generate_sjd_entry("lg_generate_sjd_neg", e, cond, emb_mask, Negative{neg_cond, neg_mask}, B, T, S, sc, L, dev_ws, ws_bytes,
+                              out_tokens, iters_out, dbg_probs, stream);
 }
 
 int lg_test_sjd_verify(int B, int S, int L, int V, int greedy, uint64_t seed, const float* p, const float* q, const int32_t* qflag,
@@ -1637,28 +1746,33 @@ static int test_attention_args(const char* fn, KvMaps& maps, AttnArgs& aa, int d
     return 0;
 }
 
-int lg_test_attention(int dtype, int kv_dtype, float k_scale, float v_scale, int R, int Tq, int H, int hd, int hdp, int max_seq,
-                      void* kcache, void* vcache, int n_layer, int layer, int pos_value, const int32_t* pos_dev,
-                      const int32_t* pos_rows, const float* emb_mask, int B, int Tc, const void* q, const float* qkv_partial,
-                      int ksplit, const float* freqs, int fuse, void* q_out, void* out, int* path, void* stream) {
+}  // extern "C"
+
+// lg_test_attention (fn) with emb_mask_uncond, the mask rows r >= B read (null: emb_mask's)
+static int test_attention_impl(const char* fn, int dtype, int kv_dtype, float k_scale, float v_scale, int R, int Tq, int H, int hd, int hdp,
+                               int max_seq, void* kcache, void* vcache, int n_layer, int layer, int pos_value, const int32_t* pos_dev,
+                               const int32_t* pos_rows, const float* emb_mask, const float* emb_mask_uncond, int B, int Tc, const void* q,
+                               const float* qkv_partial, int ksplit, const float* freqs, int fuse, void* q_out, void* out, int* path,
+                               void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     auto a16 = [](const void* p) { return ((uintptr_t)p & 15) == 0; };
     LG_REQUIRE(kv_dtype == LG_DTYPE_E4M3 ? kv_scale_ok(k_scale) && kv_scale_ok(v_scale) : k_scale == 1.f && v_scale == 1.f,
-               "lg_test_attention: K / V scales %g / %g (fp8: powers of two in [2^-8, 2^7], otherwise 1)", (double)k_scale, (double)v_scale);
+               "%s: K / V scales %g / %g (fp8: powers of two in [2^-8, 2^7], otherwise 1)", fn, (double)k_scale, (double)v_scale);
     LG_REQUIRE(kcache && vcache && out && a16(kcache) && a16(vcache) && a16(out) && a16(q) && a16(q_out) && a16(qkv_partial) && a16(freqs),
-               "lg_test_attention: null or misaligned (16 bytes) buffer");
-    LG_REQUIRE(!emb_mask || (B > 0 && Tc > 0 && Tc <= max_seq), "lg_test_attention: emb_mask needs B > 0 and 0 < Tc <= max_seq (B=%d Tc=%d)",
+               "%s: null or misaligned (16 bytes) buffer", fn);
+    LG_REQUIRE(!emb_mask || (B > 0 && Tc > 0 && Tc <= max_seq), "%s: emb_mask needs B > 0 and 0 < Tc <= max_seq (B=%d Tc=%d)", fn,
                B, Tc);
-    LG_REQUIRE((q != nullptr) != (qkv_partial != nullptr), "lg_test_attention: pass exactly one of q and qkv_partial");
+    LG_REQUIRE((q != nullptr) != (qkv_partial != nullptr), "%s: pass exactly one of q and qkv_partial", fn);
     LG_REQUIRE(q ? fuse == 0 : (ksplit > 0 && freqs && (fuse == 1 || (fuse == 0 && q_out))),
-               "lg_test_attention: q takes fuse = 0; qkv_partial needs ksplit > 0, freqs and fuse = 1 or q_out");
+               "%s: q takes fuse = 0; qkv_partial needs ksplit > 0, freqs and fuse = 1 or q_out", fn);
     KvMaps maps;
     AttnArgs aa;
     const float scales[2] = {k_scale, v_scale};
-    LG_TRY(test_attention_args("lg_test_attention", maps, aa, dtype, kv_dtype, scales, R, Tq, H, hd, hdp, max_seq, kcache, vcache, n_layer,
+    LG_REQUIRE(!emb_mask_uncond || emb_mask, "%s: emb_mask_uncond needs emb_mask", fn);
+    LG_TRY(test_attention_args(fn, maps, aa, dtype, kv_dtype, scales, R, Tq, H, hd, hdp, max_seq, kcache, vcache, n_layer,
                                layer, PosArg{pos_dev, pos_value, pos_rows}, qkv_partial && fuse));
     aa.q = q ? q : q_out; aa.out = out;
-    aa.emb_mask = emb_mask; aa.B = emb_mask ? B : 1; aa.Tc = emb_mask ? Tc : 0;
+    aa.emb_mask = emb_mask; aa.B = emb_mask ? B : 1; aa.Tc = emb_mask ? Tc : 0; aa.emb_mask_uncond = emb_mask_uncond;
     if (qkv_partial) {
         if (fuse) {
             aa.qkv_partial = qkv_partial; aa.qkv_ksplit = ksplit; aa.freqs = freqs;
@@ -1667,6 +1781,27 @@ int lg_test_attention(int dtype, int kv_dtype, float k_scale, float v_scale, int
         }
     }
     return launch_attention(aa, st, path);
+}
+
+extern "C" {
+
+int lg_test_attention(int dtype, int kv_dtype, float k_scale, float v_scale, int R, int Tq, int H, int hd, int hdp, int max_seq,
+                      void* kcache, void* vcache, int n_layer, int layer, int pos_value, const int32_t* pos_dev,
+                      const int32_t* pos_rows, const float* emb_mask, int B, int Tc, const void* q, const float* qkv_partial,
+                      int ksplit, const float* freqs, int fuse, void* q_out, void* out, int* path, void* stream) {
+    return test_attention_impl("lg_test_attention", dtype, kv_dtype, k_scale, v_scale, R, Tq, H, hd, hdp, max_seq, kcache, vcache, n_layer,
+                               layer, pos_value, pos_dev, pos_rows, emb_mask, nullptr, B, Tc, q, qkv_partial, ksplit, freqs, fuse, q_out, out,
+                               path, stream);
+}
+
+int lg_test_attention_neg(int dtype, int kv_dtype, float k_scale, float v_scale, int R, int Tq, int H, int hd, int hdp, int max_seq,
+                          void* kcache, void* vcache, int n_layer, int layer, int pos_value, const int32_t* pos_dev,
+                          const int32_t* pos_rows, const float* emb_mask, const float* emb_mask_uncond, int B, int Tc, const void* q,
+                          const float* qkv_partial, int ksplit, const float* freqs, int fuse, void* q_out, void* out, int* path,
+                          void* stream) {
+    return test_attention_impl("lg_test_attention_neg", dtype, kv_dtype, k_scale, v_scale, R, Tq, H, hd, hdp, max_seq, kcache, vcache,
+                               n_layer, layer, pos_value, pos_dev, pos_rows, emb_mask, emb_mask_uncond, B, Tc, q, qkv_partial, ksplit, freqs,
+                               fuse, q_out, out, path, stream);
 }
 
 int lg_test_attention_plan(int dtype, int kv_dtype, int R, int Tq, int H, int hd, int hdp, int max_seq, int n_layer, int pos_kind,

@@ -135,8 +135,9 @@ int launch_embed(const void* table, const int32_t* src, int B, int R, int null_i
 // at any other position the token embedding of src[r % B]
 int launch_embed_rows(const void* cls_table, const void* tok_table, const int32_t* src, const int* pos_rows, int B, int R, int null_idx,
                       int D, int dtype, void* out, cudaStream_t st);
-// t2i cond rows: out[(r*T+t),:] = r < B ? cond[r,t,:] : uncond[t,:]   (generate.py:137)
-int launch_build_caption_rows(const void* cond, const void* uncond, int B, int R, int T, int C, int dtype,
+// t2i cond rows: out[(r*T+t),:] = r < B ? cond[r,t,:] : uncond[(r-B)*uncond_stride + t*C + :]   (generate.py:137). uncond_stride 0:
+// every unconditional row is uncond_embedding [T, C]; T * C: uncond holds one negative condition [T, C] per image
+int launch_build_caption_rows(const void* cond, const void* uncond, size_t uncond_stride, int B, int R, int T, int C, int dtype,
                               void* out, cudaStream_t st);
 // xn = rmsnorm(x) * w   (gpt.py:143-148)
 int launch_rmsnorm(const void* x, const void* w, void* xn, int M, int D, float eps, int dtype, cudaStream_t st);
@@ -191,6 +192,7 @@ struct AttnArgs {
     int B, Tc;
     float scale;
     int dtype;
+    const float* emb_mask_uncond = nullptr;   // [B, Tc]: the mask rows r >= B read (a negative prompt's); null: emb_mask's
     int hdp = 0;            // elements between consecutive cache rows (0: hd); q / out stay [M, H*hd]
     // TMA path (attn_tma.cu): tensor maps over the whole K / V cache regions + this layer's first row
     const void* kmap = nullptr; const void* vmap = nullptr;        // kKC-row boxes
@@ -203,6 +205,13 @@ struct AttnArgs {
     int kv_f8 = 0;
     float k_inv = 1.f, v_inv = 1.f, v_scale = 1.f;
 };
+// The emb-mask row attention row r reads (AttnArgs or attn_tma.cu's AttnTmaArgs): row r % B of emb_mask for the conditional rows
+// r < B, and of emb_mask_uncond, when it is set, for the rows r >= B; null without a mask
+template <class A>
+__device__ __forceinline__ const float* attn_mask_row(const A& a, int r) {
+    if (!a.emb_mask) return nullptr;
+    return (r >= a.B && a.emb_mask_uncond ? a.emb_mask_uncond : a.emb_mask) + (size_t)(r % a.B) * a.Tc;
+}
 // KV-cache row width in elements: head_dim 100 of a bf16 / fp16 model (GPT-3B) is stored in 112-wide rows, 16-byte multiples that
 // the TMA attention kernels can stream (dims 100..111 stay zero); every other cache row is hd wide
 inline int attn_kv_row_width(int dtype, int hd) { return hd == 100 && lg_dtype_is16(dtype) ? 112 : hd; }

@@ -47,11 +47,11 @@ __global__ void embed_rows_kernel(const T* __restrict__ cls_table, const T* __re
 }
 
 template <typename T>
-__global__ void caption_rows_kernel(const T* __restrict__ cond, const T* __restrict__ uncond, int B, int T_,
+__global__ void caption_rows_kernel(const T* __restrict__ cond, const T* __restrict__ uncond, size_t ustride, int B, int T_,
                                     int C, T* __restrict__ out) {
     lg_pdl_sync();
     const int row = blockIdx.x, r = row / T_, t = row % T_;
-    const T* s = r < B ? cond + ((size_t)r * T_ + t) * C : uncond + (size_t)t * C;
+    const T* s = r < B ? cond + ((size_t)r * T_ + t) * C : uncond + (size_t)(r - B) * ustride + (size_t)t * C;
     T* d = out + (size_t)row * C;
     for (int i = threadIdx.x; i < C; i += blockDim.x) d[i] = s[i];
 }
@@ -263,7 +263,8 @@ __global__ void reduce_f32_kernel(const float* __restrict__ partial, int ks, siz
 // One CTA per (query row m = r*Tq + t, head h). A key is owned by a group of LPK lanes, each holding VEC
 // contiguous head elements (128-bit loads for hd=64 bf16); every lane group runs an independent online
 // softmax over its keys; groups merge by shuffles, warps merge through shared memory.
-// Mask (gpt.py:354 + generate.py:154-163): key j visible iff j <= qpos and (j >= Tc or emb_mask[r%B, j] != 0 or j == qpos).
+// Mask (gpt.py:354 + generate.py:154-163): key j visible iff j <= qpos and (j >= Tc or mask[r%B, j] != 0 or j == qpos), mask the
+// emb_mask of the row's half (attn_mask_row).
 // KV = e4m3 (fp8 cache): K and V are read as their e4m3 codes; a.scale carries the K scale and the output is multiplied by a.v_scale.
 template <typename T, int HD, int VEC, int LPK, int HDP = HD, typename KV = T>
 __global__ void __launch_bounds__(256) attention_kernel(AttnArgs a) {
@@ -284,7 +285,7 @@ __global__ void __launch_bounds__(256) attention_kernel(AttnArgs a) {
     const T* qp = reinterpret_cast<const T*>(a.q) + (size_t)m * D + (size_t)h * HD;
     const KV* kbase = reinterpret_cast<const KV*>(a.kcache) + ((size_t)r * a.H + h) * (size_t)a.maxS * hdp;
     const KV* vbase = reinterpret_cast<const KV*>(a.vcache) + ((size_t)r * a.H + h) * (size_t)a.maxS * hdp;
-    const float* mrow = a.emb_mask ? a.emb_mask + (size_t)(r % a.B) * a.Tc : nullptr;
+    const float* mrow = attn_mask_row(a, r);
 
     float qv[VEC];
 #pragma unroll
@@ -476,12 +477,13 @@ int launch_embed_rows(const void* cls_table, const void* tok_table, const int32_
         });
 }
 
-int launch_build_caption_rows(const void* cond, const void* uncond, int B, int R, int T, int C, int dtype, void* out,
+int launch_build_caption_rows(const void* cond, const void* uncond, size_t uncond_stride, int B, int R, int T, int C, int dtype, void* out,
                               cudaStream_t st) {
     return dispatch_dtype(
         dtype, [&](auto z) {
             using E = decltype(z);
-            (void)lg_launch(caption_rows_kernel<E>, dim3(R * T), dim3(128), 0, st, (const E*)cond, (const E*)uncond, B, T, C, (E*)out);
+            (void)lg_launch(caption_rows_kernel<E>, dim3(R * T), dim3(128), 0, st, (const E*)cond, (const E*)uncond, uncond_stride, B, T, C,
+                            (E*)out);
             LG_LAUNCH_CHECK();
             return 0;
         });

@@ -49,6 +49,12 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
                            image): the condition and the prefix are prefilled in one forward pass and tokens P .. are sampled as
                            plain generation samples them (same RNG key per token index), so out[:, :P] == prefix. With
                            return_logits, rows k < P of the logits are zero.
+      negative_cond=tensor t2i with cfg_scale > 1: a negative prompt, [1, T, C] (one for every image) or [B, T, C], prepared as cond
+                           is (cond.pack_t5_features + cond.prepare_condition). It replaces the null condition of the unconditional
+                           rows, so the mix uncond + (cond - uncond) * cfg_scale pushes away from it. Works on the plain, prefix and
+                           sjd_window paths; not with teacher.
+      negative_emb_masks=tensor  [1, T] or [B, T]: the negative's emb-mask (the unconditional rows attend with it). Either of
+                           emb_masks / negative_emb_masks left out counts as all ones.
     """
     if not isinstance(model, Transformer):
         raise TypeError("llamagen_b200.generate needs a llamagen_b200 GPT_models[...] instance")
@@ -62,6 +68,8 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
     sjd_window = sampling_kwargs.pop("sjd_window", None)
     return_stats = bool(sampling_kwargs.pop("return_stats", False))
     prefix = sampling_kwargs.pop("prefix", None)
+    negative_cond = sampling_kwargs.pop("negative_cond", None)
+    negative_emb_masks = sampling_kwargs.pop("negative_emb_masks", None)
     if sampling_kwargs:
         raise TypeError(f"unexpected sampling kwargs: {sorted(sampling_kwargs)}")
     if sjd_window is not None:
@@ -74,6 +82,8 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
     if prefix is not None and (teacher is not None or sjd_window is not None):
         raise ValueError("prefix cannot be combined with teacher or sjd_window")
     pf = _check_prefix(prefix, cond.shape[0], int(max_new_tokens), model.vocab_size) if prefix is not None else None
+    if negative_cond is not None or negative_emb_masks is not None:
+        _check_negative(model, cond, emb_masks, negative_cond, negative_emb_masks, cfg_scale, teacher)
 
     dev = model.tok_embeddings.weight.device
     _lib.require_cuda(model.tok_embeddings.weight, "generate")
@@ -97,6 +107,12 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
         assert emb_masks.shape[0] == B                          # generate.py:155-156
         assert emb_masks.shape[-1] == T
         em = emb_masks.to(device=dev, dtype=torch.float32).contiguous()
+    neg = nm = None
+    if negative_cond is not None:                                # both halves get a mask: a missing one is all ones
+        neg = negative_cond.to(device=dev, dtype=cond_dev.dtype).expand(B, T, cond_dev.shape[2]).contiguous()
+        ones = torch.ones(B, T, dtype=torch.float32, device=dev)
+        em = ones if em is None else em
+        nm = ones if negative_emb_masks is None else negative_emb_masks.to(device=dev, dtype=torch.float32).expand(B, T).contiguous()
 
     if sjd_window is not None and S < 3:
         raise ValueError(f"sjd_window needs max_new_tokens >= 3, got {S}")
@@ -106,7 +122,7 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
     if sjd_window is not None:
         return _generate_sjd(model, lib, handle, cond, cond_dev, em, B, T, S, out, min(int(sjd_window), S - 1), use_cfg, return_stats,
                              _lib.SampleCfg(float(cfg_scale), int(cfg_interval), temperature, top_k, top_p, 0 if sample_logits else 1,
-                                            _draw_seed() if seed is None else int(seed)))
+                                            _draw_seed() if seed is None else int(seed)), neg=neg, nm=nm)
     if pf is not None:
         P = pf.shape[1]
         dbg = torch.zeros((S, B, model.vocab_size), dtype=torch.float32, device=dev) if return_logits else None
@@ -114,8 +130,13 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
         ws, ws_bytes = model._prefix_scratch(rows, T + P, 2 if use_cfg else 1)
         sc = _lib.SampleCfg(float(cfg_scale), int(cfg_interval), temperature, top_k, top_p, 0 if sample_logits else 1,
                             _draw_seed() if seed is None else int(seed))
-        _lib.check(lib.lg_generate_prefix(handle, _lib.ptr(cond_dev), _lib.ptr(em), B, T, S, ctypes.byref(sc), _lib.ptr(pf_dev), P, ws,
-                                          ws_bytes, _lib.ptr(out), _lib.ptr(dbg), _lib.current_stream(dev)), "lg_generate_prefix")
+        if neg is None:
+            _lib.check(lib.lg_generate_prefix(handle, _lib.ptr(cond_dev), _lib.ptr(em), B, T, S, ctypes.byref(sc), _lib.ptr(pf_dev), P, ws,
+                                              ws_bytes, _lib.ptr(out), _lib.ptr(dbg), _lib.current_stream(dev)), "lg_generate_prefix")
+        else:
+            _lib.check(lib.lg_generate_prefix_neg(handle, _lib.ptr(cond_dev), _lib.ptr(em), _lib.ptr(neg), _lib.ptr(nm), B, T, S,
+                                                  ctypes.byref(sc), _lib.ptr(pf_dev), P, ws, ws_bytes, _lib.ptr(out), _lib.ptr(dbg),
+                                                  _lib.current_stream(dev)), "lg_generate_prefix_neg")
         if cond.device != dev:
             out = out.to(cond.device)
         return (out, dbg) if return_logits else out
@@ -125,11 +146,34 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
         raise ValueError("teacher must be [B, max_new_tokens]")
     sc = _lib.SampleCfg(float(cfg_scale), int(cfg_interval), temperature, top_k, top_p, 0 if sample_logits else 1,
                         _draw_seed() if seed is None else int(seed))
-    _lib.check(lib.lg_generate(handle, _lib.ptr(cond_dev), _lib.ptr(em), B, T, S, ctypes.byref(sc), _lib.ptr(out),
-                               _lib.ptr(dbg), _lib.ptr(tf), _lib.current_stream(dev)), "lg_generate")
+    if neg is None:
+        _lib.check(lib.lg_generate(handle, _lib.ptr(cond_dev), _lib.ptr(em), B, T, S, ctypes.byref(sc), _lib.ptr(out),
+                                   _lib.ptr(dbg), _lib.ptr(tf), _lib.current_stream(dev)), "lg_generate")
+    else:
+        _lib.check(lib.lg_generate_neg(handle, _lib.ptr(cond_dev), _lib.ptr(em), _lib.ptr(neg), _lib.ptr(nm), B, T, S, ctypes.byref(sc),
+                                       _lib.ptr(out), _lib.ptr(dbg), None, _lib.current_stream(dev)), "lg_generate_neg")
     if cond.device != dev:
         out = out.to(cond.device)
     return (out, dbg) if return_logits else out
+
+
+def _check_negative(model, cond, emb_masks, negative_cond, negative_emb_masks, cfg_scale, teacher):
+    """generate()'s checks of a negative prompt, before anything reaches the device."""
+    if model.model_type != "t2i":
+        raise ValueError("negative_cond applies to text-conditional (t2i) models; a c2i model has no negative class")
+    if negative_cond is None:
+        raise ValueError("negative_emb_masks needs negative_cond")
+    if not cfg_scale > 1.0:
+        raise ValueError(f"a negative prompt replaces the unconditional half of classifier-free guidance: it needs cfg_scale > 1, "
+                         f"got {cfg_scale}")
+    if teacher is not None:
+        raise ValueError("negative_cond cannot be combined with teacher")
+    B, T, C = cond.shape[0], cond.shape[1], cond.shape[2]
+    if negative_cond.dim() != 3 or negative_cond.shape[0] not in (1, B) or tuple(negative_cond.shape[1:]) != (T, C):
+        raise ValueError(f"negative_cond must be [1, T, C] or [B, T, C] = [{B}, {T}, {C}], got {tuple(negative_cond.shape)}")
+    if negative_emb_masks is not None and (negative_emb_masks.dim() != 2 or negative_emb_masks.shape[0] not in (1, B)
+                                           or negative_emb_masks.shape[1] != T):
+        raise ValueError(f"negative_emb_masks must be [1, T] or [B, T] = [{B}, {T}], got {tuple(negative_emb_masks.shape)}")
 
 
 def _check_prefix(prefix, B, S, V):
@@ -147,13 +191,19 @@ def _check_prefix(prefix, B, S, V):
     return pf
 
 
-def _generate_sjd(model, lib, handle, cond, cond_dev, em, B, T, S, out, L, use_cfg, return_stats, sc, dbg_probs=None):
-    """lg_generate_sjd with window L (already clamped to S - 1); dbg_probs: None or f32 [S - 1, B, L, V] for replay tests."""
+def _generate_sjd(model, lib, handle, cond, cond_dev, em, B, T, S, out, L, use_cfg, return_stats, sc, dbg_probs=None, neg=None, nm=None):
+    """lg_generate_sjd with window L (already clamped to S - 1); dbg_probs: None or f32 [S - 1, B, L, V] for replay tests; neg, nm:
+    a negative prompt and its mask, [B, T, C] and [B, T] on the device (lg_generate_sjd_neg), or None."""
     dev = out.device
     ws, ws_bytes = model._sjd_scratch(B, use_cfg, L)
     iters = torch.zeros(1, dtype=torch.int32, device=dev)
-    _lib.check(lib.lg_generate_sjd(handle, _lib.ptr(cond_dev), _lib.ptr(em), B, T, S, ctypes.byref(sc), L, ws, ws_bytes, _lib.ptr(out),
-                                   _lib.ptr(iters), _lib.ptr(dbg_probs), _lib.current_stream(dev)), "lg_generate_sjd")
+    if neg is None:
+        _lib.check(lib.lg_generate_sjd(handle, _lib.ptr(cond_dev), _lib.ptr(em), B, T, S, ctypes.byref(sc), L, ws, ws_bytes, _lib.ptr(out),
+                                       _lib.ptr(iters), _lib.ptr(dbg_probs), _lib.current_stream(dev)), "lg_generate_sjd")
+    else:
+        _lib.check(lib.lg_generate_sjd_neg(handle, _lib.ptr(cond_dev), _lib.ptr(em), _lib.ptr(neg), _lib.ptr(nm), B, T, S, ctypes.byref(sc),
+                                           L, ws, ws_bytes, _lib.ptr(out), _lib.ptr(iters), _lib.ptr(dbg_probs), _lib.current_stream(dev)),
+                   "lg_generate_sjd_neg")
     if cond.device != dev:
         out = out.to(cond.device)
     if not return_stats:

@@ -3,7 +3,10 @@
 The Flan-T5 encoder is upstream of the hot path (SURVEY §2 row 7): with `--t5-path` the HF encoder produces the
 [B,120,2048] features exactly like language/t5.py; `--cond-npy` takes features precomputed by
 language/extract_t5_feature.py (fp32 [1, valid_len, 2048] .npy, one file per prompt); `--synthetic-cond`
-draws seeded random features (what the benchmarks use, there are no T5 weights offline)."""
+draws seeded random features (what the benchmarks use, there are no T5 weights offline).
+
+A negative prompt (`--negative-prompt TEXT`, encoded by the `--t5-path` encoder, or `--negative-cond-npy FILE` in
+extract_t5_feature's layout) takes the place of the null condition in classifier-free guidance for every prompt."""
 import argparse
 import os
 import time
@@ -29,8 +32,37 @@ def t5_features(args, device, precision):
         return embs.to(device, precision), masks.to(device)
     if args.synthetic_cond:
         return synthetic_features(len(PROMPTS), T, C, args.seed, device, precision)
-    assert os.path.exists(args.t5_path), "--t5-path not found (use --cond-npy or --synthetic-cond without T5 weights)"
-    return HFT5Encoder(args.t5_path, args.t5_model_type, T, device, precision)(PROMPTS)
+    return _hf_encoder(args, device, precision)(PROMPTS)
+
+
+def negative_features(args, device, precision):
+    """The negative prompt's (features [1, T, C], mask [1, T]), or None without one."""
+    T, C = args.t5_feature_max_len, args.t5_feature_dim
+    if args.negative_cond_npy:
+        embs, masks = load_t5_feature_files([args.negative_cond_npy], T, C)
+        return embs.to(device, precision), masks.to(device)
+    if args.negative_prompt:
+        return _hf_encoder(args, device, precision)([args.negative_prompt])
+    return None
+
+
+_ENCODERS = {}
+
+
+def _hf_encoder(args, device, precision):
+    """The --t5-path encoder, loaded once for the prompts and the negative prompt."""
+    key = (args.t5_path, args.t5_model_type, args.t5_feature_max_len, str(device), precision)
+    if key not in _ENCODERS:
+        assert os.path.exists(args.t5_path), "--t5-path not found (use --cond-npy or --synthetic-cond without T5 weights)"
+        _ENCODERS[key] = HFT5Encoder(args.t5_path, args.t5_model_type, args.t5_feature_max_len, device, precision)
+    return _ENCODERS[key]
+
+
+def check_negative_args(args):
+    if args.negative_prompt and args.negative_cond_npy:
+        raise SystemExit("pass --negative-prompt or --negative-cond-npy, not both")
+    if (args.negative_prompt or args.negative_cond_npy) and not args.cfg_scale > 1.0:
+        raise SystemExit("a negative prompt replaces the unconditional half of classifier-free guidance: it needs --cfg-scale > 1")
 
 
 def main(args):
@@ -41,6 +73,7 @@ def main(args):
     device = "cuda"
     latent_size = args.image_size // args.downsample_size
     check_prefix_args(args, latent_size)
+    check_negative_args(args)
     vq_model = load_vq(args, device)
     gpt_model = load_gpt(args, device, latent_size)
     precision = gpt_model.tok_embeddings.weight.dtype
@@ -51,6 +84,10 @@ def main(args):
         for idx, valid in enumerate(emb_masks.sum(dim=-1).tolist()):
             print(f"  prompt {idx} token len: {int(valid)}")
     c_indices, emb_masks = prepare_condition(caption_embs, emb_masks, left_padding=not args.no_left_padding)
+    neg = negative_features(args, device, precision)
+    nk = {}
+    if neg is not None:   # prepared as the prompts are; one negative for every prompt
+        nk["negative_cond"], nk["negative_emb_masks"] = prepare_condition(*neg, left_padding=not args.no_left_padding)
     qzshape = [len(c_indices), args.codebook_embed_dim, latent_size, latent_size]
 
     pk = prefix_kwargs(args, vq_model, len(c_indices), latent_size, device)
@@ -58,7 +95,7 @@ def main(args):
     t1 = time.time()
     index_sample = generate(gpt_model, c_indices, latent_size ** 2, emb_masks, cfg_scale=args.cfg_scale,
                             temperature=args.temperature, top_k=args.top_k, top_p=args.top_p, sample_logits=True,
-                            **sjd_kwargs(args), **pk)
+                            **sjd_kwargs(args), **pk, **nk)
     torch.cuda.synchronize()
     print(f"Full sampling takes about {time.time() - t1:.2f} seconds.")
     t2 = time.time()
@@ -79,6 +116,10 @@ def build_parser():
     parser.add_argument("--no-left-padding", action="store_true", default=False)
     parser.add_argument("--cond-npy", type=str, nargs="+", default=None, help="extension: precomputed T5 feature files")
     parser.add_argument("--synthetic-cond", action="store_true", help="extension: seeded random T5-shaped features")
+    parser.add_argument("--negative-prompt", type=str, default=None,
+                        help="extension: a negative prompt for every image, encoded by the --t5-path encoder (needs --cfg-scale > 1)")
+    parser.add_argument("--negative-cond-npy", type=str, default=None,
+                        help="extension: the negative prompt's T5 features, one .npy in extract_t5_feature's layout")
     return parser
 
 

@@ -37,6 +37,13 @@ caption request joins; a c2i one joins in the admission phase (a c2i request wit
 decode) and takes part in the same step's decode. A request whose join draws its last token (P = max_tokens - 1) finishes at its join.
 Null-class twins mirror their conditional request's prefix.
 
+Negative prompts (t2i with cfg_scale > 1): a request may bring a negative caption (`add_request(..., negative_prompt_embeds=...)`,
+`LLM.generate(..., negative_prompt_embeds=[...])`, and with a text encoder `negative_prompt=` / `negative_prompts=`, encoded in the same
+encoder call as the prompts). It is prepared as the condition is, and the request's unconditional row is prefilled with it and attends
+with its mask (`lg_prefill_slot_prefix_neg`, `lg_decode_rows_t2i_neg`), so the request draws what generate(negative_cond=...,
+seed=base_seed + r) draws for image 0. Requests with and without a negative share the running batch: a slot without one keeps the null
+condition and its caption's mask in its unconditional row.
+
 While requests are in flight the LLM owns the model's KV-cache workspace (a `generate()` call on the same model would reset it)."""
 from __future__ import annotations
 
@@ -88,6 +95,8 @@ class _Request:
     cond: Optional[torch.Tensor] = None   # t2i: the prepared condition, fp32 [T, caption_dim] on the host
     mask: Optional[torch.Tensor] = None   # t2i: its emb-mask, fp32 [T]
     prefix: Optional[torch.Tensor] = None  # image completion: the given tokens 0 .. P - 1, int64 [P] on the host
+    neg: Optional[torch.Tensor] = None     # t2i: a negative prompt's prepared condition, fp32 [T, caption_dim] on the host, or None
+    neg_mask: Optional[torch.Tensor] = None   # and its emb-mask, fp32 [T]
 
 
 def _plen(req: _Request) -> int:
@@ -135,19 +144,37 @@ class LLM:
 
     # ------------------------------------------------------------------ engine-style surface (llm_engine.py)
     def add_request(self, prompt_token_ids: Optional[Sequence[int]] = None, sampling_params: Optional[SamplingParams] = None, twin_of=None,
-                    prompt_embeds=None, prefix=None, prompt: Optional[str] = None) -> str:
+                    prompt_embeds=None, prefix=None, prompt: Optional[str] = None, negative_prompt_embeds=None,
+                    negative_prompt: Optional[str] = None) -> str:
         """c2i: prompt_token_ids = [class id] (twin_of: see LLM.generate). t2i: prompt_embeds = one caption's T5 features, [n, caption_dim]
         or the .npy layout [1, n, caption_dim] (array or tensor, n >= 1, truncated at cls_token_num).
         prefix: image completion, the first P image tokens (1-D integer ids in [0, vocab_size), 1 <= P <= max_tokens - 1); the
         request's token_ids start with them. A null-class twin takes its conditional request's prefix (passing another one is an error).
-        prompt: a caption string, with a text_encoder only (instead of prompt_embeds)."""
-        if prompt is not None:
-            prompt_embeds = self._encode_prompts([prompt], prompt_embeds)[0]
+        prompt: a caption string, with a text_encoder only (instead of prompt_embeds).
+        negative_prompt_embeds (t2i, cfg_scale > 1): a negative caption's T5 features, shaped as prompt_embeds; the request's
+        unconditional row takes it instead of the null condition. negative_prompt: its string, with a text_encoder only (one encoder
+        call with prompt)."""
+        if prompt is not None or negative_prompt is not None:
+            texts = [t for t in (prompt, negative_prompt) if t is not None]
+            if prompt is not None and prompt_embeds is not None:
+                raise ValueError("pass caption strings (prompts) or their features (prompt_embeds), not both")
+            if negative_prompt is not None and negative_prompt_embeds is not None:
+                raise ValueError("pass negative_prompt or negative_prompt_embeds, not both")
+            feats = self._encode_prompts(texts)
+            if prompt is not None:
+                prompt_embeds = feats.pop(0)
+            if negative_prompt is not None:
+                negative_prompt_embeds = feats.pop(0)
         if self.t2i:
             if prompt_token_ids is not None or twin_of is not None:
                 raise ValueError("a t2i LLM takes prompt_embeds (T5 caption features), not prompt_token_ids; CFG needs no twin requests")
             caption = self._caption(prompt_embeds)
-            return self._enqueue_t2i(caption, sampling_params, self._prefix(prefix, sampling_params))
+            negative = self._negative(negative_prompt_embeds)
+            pf = self._prefix(prefix, sampling_params)
+            return self._enqueue_t2i(caption, sampling_params, pf) if negative is None else self._enqueue_t2i(caption, sampling_params, pf,
+                                                                                                              negative)
+        if negative_prompt_embeds is not None:
+            raise ValueError("negative prompts apply to text-conditional (t2i) models")
         if prompt_embeds is not None:
             raise ValueError("prompt_embeds apply to text-conditional (t2i) models; a c2i prompt is prompt_token_ids = [class id]")
         if prompt_token_ids is None:
@@ -192,6 +219,16 @@ class LLM:
         cond, mask = prepare_condition(embs, masks, left_padding=True)
         return cond[0], mask[0]
 
+    def _negative(self, feats):
+        """A negative caption's (condition fp32 [T, caption_dim], emb-mask fp32 [T]) on the host, prepared as _caption prepares the
+        condition; None stays None. A negative replaces the null condition of CFG: it needs cfg_scale > 1."""
+        if feats is None:
+            return None
+        if not self.cfg_scale > 1.0:
+            raise ValueError(f"a negative prompt replaces the unconditional half of classifier-free guidance: it needs cfg_scale > 1, "
+                             f"this LLM has {self.cfg_scale}")
+        return self._caption(feats)
+
     def _prefix(self, prefix, sampling_params: Optional[SamplingParams]) -> Optional[torch.Tensor]:
         """A request's prefix as int64 [P] on the host, checked as generate(prefix=...) checks it: integer ids in [0, vocab_size),
         1 <= P <= max_tokens - 1. None stays None."""
@@ -213,9 +250,11 @@ class LLM:
                 raise ValueError(f"a null-class twin mirrors the prefix of its conditional request {twin_of!r}; it was given another one")
         return mine
 
-    def _enqueue_t2i(self, caption, sampling_params: Optional[SamplingParams], prefix: Optional[torch.Tensor] = None) -> str:
+    def _enqueue_t2i(self, caption, sampling_params: Optional[SamplingParams], prefix: Optional[torch.Tensor] = None, negative=None) -> str:
         rid = str(next(self.request_counter))
-        self._waiting.append(_Request(rid, [], sampling_params or SamplingParams(), cond=caption[0], mask=caption[1], prefix=prefix))
+        neg, neg_mask = negative if negative is not None else (None, None)
+        self._waiting.append(_Request(rid, [], sampling_params or SamplingParams(), cond=caption[0], mask=caption[1], prefix=prefix,
+                                      neg=neg, neg_mask=neg_mask))
         return rid
 
     def _running(self) -> int:
@@ -251,7 +290,12 @@ class LLM:
                 step=torch.zeros(B, dtype=torch.int32, device=dev),       # index of the token every slot samples next
                 cond=torch.zeros(B, T, C, dtype=m.tok_embeddings.weight.dtype, device=dev),   # every slot's condition
                 mask=torch.zeros(B, T, dtype=torch.float32, device=dev),   # and emb-mask (row r of a decode reads mask row r % B)
-                step0=torch.zeros(1, dtype=torch.int32, device=dev))      # the step of token 0, drawn by a join
+                step0=torch.zeros(1, dtype=torch.int32, device=dev),      # the step of token 0, drawn by a join
+                # negative prompts: a slot's negative condition and the mask its unconditional row B + s attends with (the slot's own
+                # mask without a negative); has_neg: on the host, whether the slot's request brought one
+                neg=torch.zeros(B, T, C, dtype=m.tok_embeddings.weight.dtype, device=dev),
+                neg_mask=torch.zeros(B, T, dtype=torch.float32, device=dev),
+                has_neg=[False] * B)
         return self._state
 
     def _sample_cfg(self, params: SamplingParams):
@@ -266,8 +310,12 @@ class LLM:
         lib, handle = _lib.load(), self.model.engine()
         use_cfg = 1 if R == 2 * B else 0
         stream = _lib.current_stream(dev)
-        _lib.check(lib.lg_decode_rows_t2i(handle, _lib.ptr(st["tok"]), _lib.ptr(st["pos"]), _lib.ptr(st["mask"]), B, use_cfg,
-                                          _lib.ptr(st["logits"]), stream), "lg_decode_rows_t2i")
+        if use_cfg:   # row B + s reads neg_mask[s]: a negative's mask, or the slot's own mask
+            _lib.check(lib.lg_decode_rows_t2i_neg(handle, _lib.ptr(st["tok"]), _lib.ptr(st["pos"]), _lib.ptr(st["mask"]), _lib.ptr(st["neg_mask"]),
+                                                  B, use_cfg, _lib.ptr(st["logits"]), stream), "lg_decode_rows_t2i_neg")
+        else:
+            _lib.check(lib.lg_decode_rows_t2i(handle, _lib.ptr(st["tok"]), _lib.ptr(st["pos"]), _lib.ptr(st["mask"]), B, use_cfg,
+                                              _lib.ptr(st["logits"]), stream), "lg_decode_rows_t2i")
         sc = self._sample_cfg(params)
         dt = _lib.dtype_code(self.model.tok_embeddings.weight.dtype)
         _lib.check(lib.lg_sample_rows(_lib.ptr(st["logits"]), B, self.model.vocab_size, use_cfg, dt, ctypes.byref(sc), _lib.ptr(st["seeds"]),
@@ -281,9 +329,15 @@ class LLM:
         lib, handle = _lib.load(), m.engine()
         use_cfg = 1 if R == 2 * B else 0
         stream = _lib.current_stream(dev)
-        ws, ws_bytes = m._slot_scratch(use_cfg)
-        _lib.check(lib.lg_prefill_slot(handle, _lib.ptr(st["cond"][slot]), _lib.ptr(st["mask"][slot]), m.cls_token_num, slot, B, use_cfg,
-                                       ws, ws_bytes, _lib.ptr(st["join_logits"]), stream), "lg_prefill_slot")
+        if st["has_neg"][slot]:   # the unconditional row takes the slot's negative and its mask
+            ws, ws_bytes = m._slot_prefix_scratch(use_cfg, 0)
+            _lib.check(lib.lg_prefill_slot_prefix_neg(handle, _lib.ptr(st["cond"][slot]), _lib.ptr(st["mask"][slot]), _lib.ptr(st["neg"][slot]),
+                                                      _lib.ptr(st["neg_mask"][slot]), m.cls_token_num, None, 0, slot, B, use_cfg, ws, ws_bytes,
+                                                      _lib.ptr(st["join_logits"]), stream), "lg_prefill_slot_prefix_neg")
+        else:
+            ws, ws_bytes = m._slot_scratch(use_cfg)
+            _lib.check(lib.lg_prefill_slot(handle, _lib.ptr(st["cond"][slot]), _lib.ptr(st["mask"][slot]), m.cls_token_num, slot, B, use_cfg,
+                                           ws, ws_bytes, _lib.ptr(st["join_logits"]), stream), "lg_prefill_slot")
         sc = self._sample_cfg(params)
         dt = _lib.dtype_code(m.tok_embeddings.weight.dtype)
         _lib.check(lib.lg_sample_rows(_lib.ptr(st["join_logits"]), 1, m.vocab_size, use_cfg, dt, ctypes.byref(sc),
@@ -303,8 +357,13 @@ class LLM:
         # c2i: the prefill reads the class id from tok[slot] before the draw below overwrites it (one stream)
         cond = _lib.ptr(st["cond"][slot]) if self.t2i else _lib.ptr(st["tok"][slot:slot + 1])
         mask = _lib.ptr(st["mask"][slot]) if self.t2i else None
-        _lib.check(lib.lg_prefill_slot_prefix(handle, cond, mask, m.cls_token_num, _lib.ptr(st["out"][slot]), P, slot, B, use_cfg, ws,
-                                              ws_bytes, _lib.ptr(st["join_logits"]), stream), "lg_prefill_slot_prefix")
+        if self.t2i and st["has_neg"][slot]:
+            _lib.check(lib.lg_prefill_slot_prefix_neg(handle, cond, mask, _lib.ptr(st["neg"][slot]), _lib.ptr(st["neg_mask"][slot]),
+                                                      m.cls_token_num, _lib.ptr(st["out"][slot]), P, slot, B, use_cfg, ws, ws_bytes,
+                                                      _lib.ptr(st["join_logits"]), stream), "lg_prefill_slot_prefix_neg")
+        else:
+            _lib.check(lib.lg_prefill_slot_prefix(handle, cond, mask, m.cls_token_num, _lib.ptr(st["out"][slot]), P, slot, B, use_cfg, ws,
+                                                  ws_bytes, _lib.ptr(st["join_logits"]), stream), "lg_prefill_slot_prefix")
         st["join_step"].fill_(P)
         sc = self._sample_cfg(params)
         dt = _lib.dtype_code(m.tok_embeddings.weight.dtype)
@@ -341,6 +400,10 @@ class LLM:
             for i, r in joined:
                 st["cond"][i].copy_(r.cond)
                 st["mask"][i].copy_(r.mask)
+                st["has_neg"][i] = r.neg is not None
+                if r.neg is not None:
+                    st["neg"][i].copy_(r.neg)
+                st["neg_mask"][i].copy_(r.mask if r.neg_mask is None else r.neg_mask)
                 if r.prefix is None:
                     self._device_join_t2i(st, params, i)
                 else:
@@ -469,29 +532,55 @@ class LLM:
         return [self._prefix(p, sp) for p, sp in zip(prefixes, per)]
 
     def generate(self, prompts=None, sampling_params=None, prompt_token_ids: Optional[List[List[int]]] = None,
-                 use_tqdm: bool = False, prompt_embeds=None, prefixes=None) -> List[RequestOutput]:
+                 use_tqdm: bool = False, prompt_embeds=None, prefixes=None, negative_prompt_embeds=None,
+                 negative_prompts=None) -> List[RequestOutput]:
         """c2i: prompt_token_ids, one [class id] per request (with CFG followed by one [num_classes] twin each). t2i: prompt_embeds, one
         caption's T5 features per request (see add_request). prefixes: None, or one prefix (see add_request) or None per request; under
-        c2i CFG one per conditional prompt, which its twin mirrors. Returns the RequestOutputs sorted by request id."""
-        if prompts is not None:
-            prompt_embeds = self._encode_prompts(prompts, prompt_embeds)
+        c2i CFG one per conditional prompt, which its twin mirrors. negative_prompt_embeds (t2i, cfg_scale > 1): None, or one negative
+        caption's features or None per request; negative_prompts: the same as strings (or None), with a text_encoder, encoded in one call
+        with prompts. Returns the RequestOutputs sorted by request id."""
+        if negative_prompts is not None:
+            if negative_prompt_embeds is not None:
+                raise ValueError("pass negative_prompts or negative_prompt_embeds, not both")
+            negative_prompts = [negative_prompts] if isinstance(negative_prompts, str) else list(negative_prompts)
+            if not all(t is None or isinstance(t, str) for t in negative_prompts):
+                raise ValueError("negative_prompts must hold caption strings or None")
+        if prompts is not None or negative_prompts is not None:
+            plist = [] if prompts is None else ([prompts] if isinstance(prompts, str) else list(prompts))
+            if prompts is not None and prompt_embeds is not None:
+                raise ValueError("pass caption strings (prompts) or their features (prompt_embeds), not both")
+            nlist = [t for t in (negative_prompts or []) if t is not None]
+            feats = self._encode_prompts(plist + nlist) if prompts is not None or nlist else []
+            if prompts is not None:
+                prompt_embeds = feats[:len(plist)]
+            if negative_prompts is not None:
+                it = iter(feats[len(plist):])
+                negative_prompt_embeds = [None if t is None else next(it) for t in negative_prompts]
         if self.t2i:
             if prompt_token_ids is not None or prompt_embeds is None:
                 raise ValueError("a t2i LLM takes prompt_embeds (one caption's T5 features per request), not prompt_token_ids")
             n = len(prompt_embeds)
             if isinstance(sampling_params, list) and len(sampling_params) != n:
                 raise ValueError("The lengths of prompts and sampling_params must be the same.")
+            if negative_prompt_embeds is not None and len(negative_prompt_embeds) != n:
+                raise ValueError(f"negative prompts hold {len(negative_prompt_embeds)} entries for {n} requests")
             per = sampling_params if isinstance(sampling_params, list) else [sampling_params or SamplingParams()] * n
-            captions = [self._caption(f) for f in prompt_embeds]       # every caption and prefix is checked before any is queued
+            captions = [self._caption(f) for f in prompt_embeds]       # every caption, negative and prefix is checked before any is queued
+            negs = [self._negative(f) for f in (negative_prompt_embeds or [None] * n)]
             pfx = self._prefixes(prefixes, n, per)
-            for c, p, pf in zip(captions, per, pfx):
-                self._enqueue_t2i(c, p, pf)
+            for c, p, pf, ng in zip(captions, per, pfx, negs):
+                if ng is None:
+                    self._enqueue_t2i(c, p, pf)
+                else:
+                    self._enqueue_t2i(c, p, pf, ng)
             outputs = []
             while self.has_unfinished_requests():
                 outputs.extend(o for o in self.step() if o.finished)
             return sorted(outputs, key=lambda o: int(o.request_id))
         if prompt_embeds is not None:
             raise ValueError("prompt_embeds apply to text-conditional (t2i) models")
+        if negative_prompt_embeds is not None:
+            raise ValueError("negative prompts apply to text-conditional (t2i) models")
         if prompt_token_ids is None:
             raise ValueError("Either prompts or prompt_token_ids must be provided.")
         n = len(prompt_token_ids)
