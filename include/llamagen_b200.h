@@ -196,6 +196,15 @@ int  lg_decode_rows_t2i_neg(lg_engine* e, const int32_t* tokens, const int32_t* 
  * batch-of-one lg_generate with that seed makes), result -> out_idx[b] and/or out_seq[b*seq_stride + step_rows[b]]. */
 int  lg_sample_rows(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc, const uint64_t* seed_rows,
                     const int32_t* step_rows, int32_t* out_idx, int32_t* out_seq, int seq_stride, void* stream);
+/* lg_sample_rows with per-request guidance. cfg_rows dev f32 [B] or NULL: image b mixes with scale cfg_rows[b] in place of
+ * sc->cfg_scale, and only when cfg_rows[b] > 1 (a row at scale <= 1 takes its conditional logits and never reads row B + b).
+ * interval_rows dev int32 [B] or NULL: image b drops the mix after decode iteration interval_rows[b] in place of sc->cfg_interval
+ * (-1 = never). A row given scale s > 1 and interval k draws exactly what lg_sample_rows with cfg_scale = s, cfg_interval = k and
+ * mix_cfg draws for it; a row at s <= 1 what lg_sample_rows without mix_cfg draws from its conditional row. A non-NULL cfg_rows or
+ * interval_rows needs mix_cfg (logits of 2B rows). lg_sample_rows is this call with both NULL. */
+int  lg_sample_rows_guided(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc,
+                           const uint64_t* seed_rows, const int32_t* step_rows, const float* cfg_rows, const int32_t* interval_rows,
+                           int32_t* out_idx, int32_t* out_seq, int seq_stride, void* stream);
 /* Fused CFG-mix + temperature + top-k + top-p + softmax + (argmax | multinomial): generate.py:57-66,95-97.
  * logits f32 [rows, V] (rows = 2B when mix_cfg, cond rows first); writes out_idx int32 [B] and, when
  * non-NULL, out_probs f32 [B, V] (the post-filter softmax the reference returns as `probs`).

@@ -87,6 +87,8 @@ SIGNATURES = {
                                     c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p]),
     "lg_sample_rows": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                c_void_p]),
+    "lg_sample_rows_guided": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p, c_void_p, c_void_p, c_void_p,
+                                      c_void_p, c_void_p, c_int, c_void_p]),
     "lg_sample": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(SampleCfg), c_uint64, c_void_p,
                           c_void_p, c_void_p]),
     "lg_generate": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p,

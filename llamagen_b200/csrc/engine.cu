@@ -1011,13 +1011,34 @@ int lg_score(lg_engine* e, const void* cond, const float* emb_mask, const int32_
     return 0;
 }
 
-int lg_sample_rows(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc, const uint64_t* seed_rows,
-                   const int32_t* step_rows, int32_t* out_idx, int32_t* out_seq, int seq_stride, void* stream) {
-    LG_REQUIRE(logits && sc && seed_rows && step_rows && (out_idx || out_seq), "lg_sample_rows: null argument");
+}  // extern "C"
+
+// lg_sample_rows (cfg_rows = interval_rows = null) and lg_sample_rows_guided; fn names the entry point in messages
+static int sample_rows_impl(const char* fn, const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc,
+                            const uint64_t* seed_rows, const int32_t* step_rows, const float* cfg_rows, const int32_t* interval_rows,
+                            int32_t* out_idx, int32_t* out_seq, int seq_stride, void* stream) {
+    LG_REQUIRE(logits && sc && seed_rows && step_rows && (out_idx || out_seq), "%s: null argument", fn);
+    LG_REQUIRE(mix_cfg || (!cfg_rows && !interval_rows), "%s: per-row cfg_rows / interval_rows need mix_cfg (2B logits rows)", fn);
     SampleArgs a = make_sample_args(*sc, logits, B, V, mix_cfg, round_dtype);
     a.seed_rows = seed_rows; a.step_rows = step_rows;
+    a.cfg_rows = cfg_rows; a.interval_rows = interval_rows;
     a.out_idx = out_idx; a.out_seq = out_seq; a.seq_stride = seq_stride;
     return launch_sample(a, (cudaStream_t)stream);
+}
+
+extern "C" {
+
+int lg_sample_rows(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc, const uint64_t* seed_rows,
+                   const int32_t* step_rows, int32_t* out_idx, int32_t* out_seq, int seq_stride, void* stream) {
+    return sample_rows_impl("lg_sample_rows", logits, B, V, mix_cfg, round_dtype, sc, seed_rows, step_rows, nullptr, nullptr, out_idx,
+                            out_seq, seq_stride, stream);
+}
+
+int lg_sample_rows_guided(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc,
+                          const uint64_t* seed_rows, const int32_t* step_rows, const float* cfg_rows, const int32_t* interval_rows,
+                          int32_t* out_idx, int32_t* out_seq, int seq_stride, void* stream) {
+    return sample_rows_impl("lg_sample_rows_guided", logits, B, V, mix_cfg, round_dtype, sc, seed_rows, step_rows, cfg_rows,
+                            interval_rows, out_idx, out_seq, seq_stride, stream);
 }
 
 int lg_sample(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc, uint64_t step,

@@ -33,6 +33,10 @@ struct SampleArgs {
     // continuous batching (lg_sample_rows): every image is its own request with its own RNG seed and token index
     const uint64_t* seed_rows = nullptr;   // [B] or null
     const int* step_rows = nullptr;        // [B] or null
+    // per-request guidance (lg_sample_rows_guided; needs mix_cfg): image b takes cfg_rows[b] / interval_rows[b] in place of
+    // cfg_scale / cfg_interval, and mixes only when its scale is > 1 (generate.py's `if cfg_scale > 1.0`)
+    const float* cfg_rows = nullptr;       // [B] or null
+    const int32_t* interval_rows = nullptr;// [B] or null
     // fused tail of a decode iteration (16-bit models; rows in round_dtype): the CTA that picked image b's token also writes the next step's input rows b and
     // B + b (token embedding, gpt.py:352; optionally its RMSNorm for layer 0, gpt.py:143-148) and the last CTA to finish advances the
     // device-resident position / step counters - three dependent kernels (embed, rmsnorm, advance) fewer per token

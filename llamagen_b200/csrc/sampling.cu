@@ -64,9 +64,13 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
     const int V = a.V, B = a.B;
     const uint64_t step = a.step_rows ? (uint64_t)a.step_rows[b] : (a.step_dev ? (uint64_t)(*a.step_dev) : a.step);
 
-    bool mix = a.mix_cfg != 0;
+    const float cfg_scale = a.cfg_rows ? a.cfg_rows[b] : a.cfg_scale;
+    const int cfg_interval = a.interval_rows ? a.interval_rows[b] : a.cfg_interval;
+    // a row with its own scale mixes only above 1 (generate.py:79 `if cfg_scale > 1.0`; a NaN scale does not mix either): it then
+    // reads only its conditional row
+    bool mix = a.mix_cfg != 0 && (!a.cfg_rows || cfg_scale > 1.0f);
     // generate.py:113-114 — decode iteration i = step-1; once i > cfg_interval the mix is dropped.
-    if (mix && a.cfg_interval > -1 && step >= 1 && (long long)(step - 1) > (long long)a.cfg_interval) mix = false;
+    if (mix && cfg_interval > -1 && step >= 1 && (long long)(step - 1) > (long long)cfg_interval) mix = false;
 
     const float* lc = a.logits + (size_t)b * V;
     const float* lu = a.logits + (size_t)(B + b) * V;
@@ -78,7 +82,7 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
         if (a.round_dtype) c = TR::round(c);
         if (!mix) return c;
         if (a.round_dtype) u = TR::round(u);
-        return __fadd_rn(u, __fmul_rn(__fsub_rn(c, u), a.cfg_scale));
+        return __fadd_rn(u, __fmul_rn(__fsub_rn(c, u), cfg_scale));
     };
     if (sample_vec_loads(a)) {
         // 128-bit loads, several requests of a thread in flight before the first use (the scalar loop was

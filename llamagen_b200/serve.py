@@ -44,10 +44,20 @@ with its mask (`lg_prefill_slot_prefix_neg`, `lg_decode_rows_t2i_neg`), so the r
 seed=base_seed + r) draws for image 0. Requests with and without a negative share the running batch: a slot without one keeps the null
 condition and its caption's mask in its unconditional row.
 
+Per-request guidance and seeds: SamplingParams(cfg_scale=, cfg_interval=, seed=) (None: the LLM's cfg_scale, -1, base_seed + r). The
+running set shares only (temperature, top_p, top_k, max_tokens); a change of these waits for the set to drain, a change of cfg_scale,
+cfg_interval or seed does not. Under CFG every slot's scale and interval sit in device arrays (st["cfg"], st["interval"]) that its
+request's join writes before its first draw, and every draw is lg_sample_rows_guided over them: a row mixes only when its scale is > 1
+and its interval allows it, so a request draws the tokens it draws alone in an LLM built with its cfg_scale (generate(cfg_scale=c,
+cfg_interval=k, seed=s) for image 0). A request's seed replaces base_seed + r in st["seeds"]. A scale > 1 needs an LLM built with
+cfg_scale > 1 (the unconditional rows); a request at scale <= 1 in such an LLM keeps its unconditional row running, unread.
+
 While requests are in flight the LLM owns the model's KV-cache workspace (a `generate()` call on the same model would reset it)."""
 from __future__ import annotations
 
 import itertools
+import math
+import numbers
 from collections import deque
 from dataclasses import dataclass, field
 from typing import List, Optional, Sequence
@@ -64,11 +74,27 @@ from .generate import _check_prefix
 
 @dataclass(frozen=True)
 class SamplingParams:
-    """The vllm.SamplingParams fields the reference sets (serve/sample_c2i.py:47-49). top_k=-1 / 0 disables top-k."""
+    """The vllm.SamplingParams fields the reference sets (serve/sample_c2i.py:47-49). top_k=-1 / 0 disables top-k.
+    Per-request guidance and seed (requests that differ only in these share the running batch):
+    cfg_scale: None = the LLM's cfg_scale; a finite number, > 1 only on an LLM built with cfg_scale > 1 (it has the unconditional rows).
+    cfg_interval: None = -1; an integer >= -1, generate()'s cfg_interval (the mix is dropped after decode iteration cfg_interval).
+    seed: None = the LLM's seed + request id; an integer in [0, 2**63), the key generate(seed=...) draws image 0 with."""
     temperature: float = 1.0
     top_p: float = 1.0
     top_k: int = -1
     max_tokens: int = 256
+    cfg_scale: Optional[float] = None
+    cfg_interval: Optional[int] = None
+    seed: Optional[int] = None
+
+
+def _batch_key(p: SamplingParams):
+    """The parameters every request of a running set shares; a change of these waits for the set to drain."""
+    return (p.temperature, p.top_p, p.top_k, p.max_tokens)
+
+
+def _is_int(x) -> bool:
+    return isinstance(x, (int, np.integer)) and not isinstance(x, (bool, np.bool_))
 
 
 @dataclass
@@ -97,6 +123,9 @@ class _Request:
     prefix: Optional[torch.Tensor] = None  # image completion: the given tokens 0 .. P - 1, int64 [P] on the host
     neg: Optional[torch.Tensor] = None     # t2i: a negative prompt's prepared condition, fp32 [T, caption_dim] on the host, or None
     neg_mask: Optional[torch.Tensor] = None   # and its emb-mask, fp32 [T]
+    cfg: float = 1.0                       # the request's guidance scale, cfg_interval and RNG seed, resolved at enqueue
+    interval: int = -1
+    seed: int = 0
 
 
 def _plen(req: _Request) -> int:
@@ -168,8 +197,9 @@ class LLM:
         if self.t2i:
             if prompt_token_ids is not None or twin_of is not None:
                 raise ValueError("a t2i LLM takes prompt_embeds (T5 caption features), not prompt_token_ids; CFG needs no twin requests")
+            scale = self._guidance(sampling_params)[0]
             caption = self._caption(prompt_embeds)
-            negative = self._negative(negative_prompt_embeds)
+            negative = self._negative(negative_prompt_embeds, scale)
             pf = self._prefix(prefix, sampling_params)
             return self._enqueue_t2i(caption, sampling_params, pf) if negative is None else self._enqueue_t2i(caption, sampling_params, pf,
                                                                                                               negative)
@@ -181,9 +211,14 @@ class LLM:
             raise ValueError("a c2i request needs prompt_token_ids = [class id]")
         if len(prompt_token_ids) != 1 or not (0 <= int(prompt_token_ids[0]) <= self.num_classes):
             raise ValueError(f"a c2i prompt is one class id in [0, {self.num_classes}], got {list(prompt_token_ids)}")
-        pf = self._prefix(prefix, sampling_params) if twin_of is None else self._twin_prefix(twin_of, prefix, sampling_params)
+        self._guidance(sampling_params)
+        if twin_of is None:
+            pf = self._prefix(prefix, sampling_params)
+        else:
+            pf = self._twin_prefix(twin_of, prefix, sampling_params)
+            self._twin_guidance(twin_of, sampling_params)
         rid = str(next(self.request_counter))
-        req = _Request(rid, [int(prompt_token_ids[0])], sampling_params or SamplingParams(), twin_of, prefix=pf)
+        req = self._guided(_Request(rid, [int(prompt_token_ids[0])], sampling_params or SamplingParams(), twin_of, prefix=pf))
         if twin_of is None:
             self._waiting.append(req)
         else:
@@ -219,15 +254,51 @@ class LLM:
         cond, mask = prepare_condition(embs, masks, left_padding=True)
         return cond[0], mask[0]
 
-    def _negative(self, feats):
+    def _negative(self, feats, scale: Optional[float] = None):
         """A negative caption's (condition fp32 [T, caption_dim], emb-mask fp32 [T]) on the host, prepared as _caption prepares the
-        condition; None stays None. A negative replaces the null condition of CFG: it needs cfg_scale > 1."""
+        condition; None stays None. A negative replaces the null condition of CFG: it needs cfg_scale > 1, the LLM's and the request's
+        (scale, its effective cfg_scale; None: the LLM's)."""
         if feats is None:
             return None
         if not self.cfg_scale > 1.0:
             raise ValueError(f"a negative prompt replaces the unconditional half of classifier-free guidance: it needs cfg_scale > 1, "
                              f"this LLM has {self.cfg_scale}")
+        if scale is not None and not scale > 1.0:
+            raise ValueError(f"a negative prompt replaces the unconditional half of classifier-free guidance: it needs cfg_scale > 1, "
+                             f"the request has {scale}")
         return self._caption(feats)
+
+    def _guidance(self, sampling_params: Optional[SamplingParams]):
+        """A request's (cfg_scale, cfg_interval, seed or None) with the LLM's defaults applied, checked before anything is queued."""
+        sp = sampling_params or SamplingParams()
+        scale = self.cfg_scale if sp.cfg_scale is None else sp.cfg_scale
+        if isinstance(scale, (bool, np.bool_)) or not isinstance(scale, numbers.Real) or not math.isfinite(scale):
+            raise ValueError(f"SamplingParams.cfg_scale must be a finite number, got {sp.cfg_scale!r}")
+        scale = float(scale)
+        if scale > 1.0 and not self.cfg_scale > 1.0:
+            raise ValueError(f"SamplingParams.cfg_scale {scale} > 1 needs an LLM built with cfg_scale > 1 (this one has {self.cfg_scale} and "
+                             f"runs no unconditional rows)")
+        interval = -1 if sp.cfg_interval is None else sp.cfg_interval
+        if not _is_int(interval) or interval < -1:
+            raise ValueError(f"SamplingParams.cfg_interval must be an integer >= -1, got {sp.cfg_interval!r}")
+        if sp.seed is not None and (not _is_int(sp.seed) or not 0 <= sp.seed < 2 ** 63):
+            raise ValueError(f"SamplingParams.seed must be an integer in [0, 2**63), got {sp.seed!r}")
+        return scale, int(interval), None if sp.seed is None else int(sp.seed)
+
+    def _guided(self, req: _Request) -> _Request:
+        """req with its guidance and seed resolved (seed None: the LLM's seed + request id)."""
+        req.cfg, req.interval, seed = self._guidance(req.params)
+        req.seed = self._seed + int(req.request_id) if seed is None else seed
+        return req
+
+    def _twin_guidance(self, twin_of, sampling_params: Optional[SamplingParams]):
+        """A null-class twin mirrors its conditional request: its params may not carry another cfg_scale, cfg_interval or seed."""
+        owner = self._owner(twin_of)
+        sp = sampling_params or SamplingParams()
+        if owner is not None and (sp.cfg_scale, sp.cfg_interval, sp.seed) != (owner.params.cfg_scale, owner.params.cfg_interval,
+                                                                               owner.params.seed):
+            raise ValueError(f"a null-class twin mirrors its conditional request {twin_of!r}: its cfg_scale, cfg_interval and seed must be "
+                             f"the request's")
 
     def _prefix(self, prefix, sampling_params: Optional[SamplingParams]) -> Optional[torch.Tensor]:
         """A request's prefix as int64 [P] on the host, checked as generate(prefix=...) checks it: integer ids in [0, vocab_size),
@@ -240,9 +311,13 @@ class LLM:
         S = int((sampling_params or SamplingParams()).max_tokens)
         return _check_prefix(pf[None], 1, S, self.model.vocab_size)[0]
 
+    def _owner(self, twin_of) -> Optional[_Request]:
+        """The waiting or running conditional request a null-class twin mirrors, or None."""
+        return next((r for r in itertools.chain(self._waiting, self._slots) if r is not None and r.request_id == twin_of), None)
+
     def _twin_prefix(self, twin_of, prefix, sampling_params: Optional[SamplingParams]) -> Optional[torch.Tensor]:
         """The prefix of a null-class twin: its conditional request's. A prefix passed for the twin must equal it."""
-        owner = next((r for r in itertools.chain(self._waiting, self._slots) if r is not None and r.request_id == twin_of), None)
+        owner = self._owner(twin_of)
         mine = None if owner is None else owner.prefix
         if prefix is not None:
             pf = self._prefix(prefix, sampling_params)
@@ -253,8 +328,8 @@ class LLM:
     def _enqueue_t2i(self, caption, sampling_params: Optional[SamplingParams], prefix: Optional[torch.Tensor] = None, negative=None) -> str:
         rid = str(next(self.request_counter))
         neg, neg_mask = negative if negative is not None else (None, None)
-        self._waiting.append(_Request(rid, [], sampling_params or SamplingParams(), cond=caption[0], mask=caption[1], prefix=prefix,
-                                      neg=neg, neg_mask=neg_mask))
+        self._waiting.append(self._guided(_Request(rid, [], sampling_params or SamplingParams(), cond=caption[0], mask=caption[1],
+                                                   prefix=prefix, neg=neg, neg_mask=neg_mask)))
         return rid
 
     def _running(self) -> int:
@@ -284,6 +359,9 @@ class LLM:
             logits=torch.empty(R, m.vocab_size, dtype=torch.float32, device=dev),
             join_logits=torch.empty(R // B, m.vocab_size, dtype=torch.float32, device=dev),   # a join's logits (one request's rows)
             join_step=torch.zeros(1, dtype=torch.int32, device=dev))  # a completion request's join draws token P: its step
+        if R == 2 * B:   # every slot's guidance scale and cfg_interval (lg_sample_rows_guided), written by its request's join
+            self._state.update(cfg=torch.full((B,), self.cfg_scale, dtype=torch.float32, device=dev),
+                               interval=torch.full((B,), -1, dtype=torch.int32, device=dev))
         if self.t2i:
             T, C = m.cls_token_num, m.config.caption_dim
             self._state.update(
@@ -303,10 +381,34 @@ class LLM:
         greedy = 1 if self.t2i and params.temperature == 0 else 0
         return _lib.SampleCfg(self.cfg_scale, -1, float(params.temperature), max(0, int(params.top_k)), float(params.top_p), greedy, 0)
 
+    def _write_guidance(self, st, idx, reqs: List[_Request]):
+        """The joining requests' seeds and, under CFG, guidance scales and cfg_intervals, to their slots idx (before their draws)."""
+        dev = st["dev"]
+        st["seeds"][idx] = torch.tensor([r.seed for r in reqs], dtype=torch.int64, device=dev)
+        if "cfg" in st:
+            st["cfg"][idx] = torch.tensor([r.cfg for r in reqs], dtype=torch.float32, device=dev)
+            st["interval"][idx] = torch.tensor([r.interval for r in reqs], dtype=torch.int32, device=dev)
+
+    def _draw(self, st, params: SamplingParams, logits, slots: slice, step_rows, out):
+        """One draw for each slot in `slots` from logits (its rows, cond rows first) with the slot's seed at token index step_rows:
+        result -> st["tok"][slots] and out[slot, step] (out: st["out"] rows from slots.start). Under CFG each slot mixes with its own
+        scale and cfg_interval (lg_sample_rows_guided with st["cfg"], st["interval"]), otherwise lg_sample_rows."""
+        lib, m, n = _lib.load(), self.model, slots.stop - slots.start
+        use_cfg = 1 if st["R"] == 2 * self.max_num_seqs else 0
+        sc = self._sample_cfg(params)
+        dt = _lib.dtype_code(m.tok_embeddings.weight.dtype)   # 16-bit models round the head's logits to their dtype
+        head = (_lib.ptr(logits), n, m.vocab_size, use_cfg, dt, ctypes.byref(sc), _lib.ptr(st["seeds"][slots]), _lib.ptr(step_rows))
+        tail = (_lib.ptr(st["tok"][slots]), _lib.ptr(out), st["S"], _lib.current_stream(st["dev"]))
+        if use_cfg:
+            _lib.check(lib.lg_sample_rows_guided(*head, _lib.ptr(st["cfg"][slots]), _lib.ptr(st["interval"][slots]), *tail),
+                       "lg_sample_rows_guided")
+        else:
+            _lib.check(lib.lg_sample_rows(*head, *tail), "lg_sample_rows")
+
     def _device_decode_t2i(self, st, params: SamplingParams):
-        """lg_decode_rows_t2i + lg_sample_rows on every slot: the logits of every row at its own position under its slot's emb-mask, then
+        """lg_decode_rows_t2i + a draw (_draw) on every slot: the logits of every row at its own position under its slot's emb-mask, then
         one draw per slot with step st["step"][slot], written to st["out"][slot, step] and, in place, to st["tok"][slot]."""
-        B, R, S, dev = self.max_num_seqs, st["R"], st["S"], st["dev"]
+        B, R, dev = self.max_num_seqs, st["R"], st["dev"]
         lib, handle = _lib.load(), self.model.engine()
         use_cfg = 1 if R == 2 * B else 0
         stream = _lib.current_stream(dev)
@@ -316,15 +418,12 @@ class LLM:
         else:
             _lib.check(lib.lg_decode_rows_t2i(handle, _lib.ptr(st["tok"]), _lib.ptr(st["pos"]), _lib.ptr(st["mask"]), B, use_cfg,
                                               _lib.ptr(st["logits"]), stream), "lg_decode_rows_t2i")
-        sc = self._sample_cfg(params)
-        dt = _lib.dtype_code(self.model.tok_embeddings.weight.dtype)
-        _lib.check(lib.lg_sample_rows(_lib.ptr(st["logits"]), B, self.model.vocab_size, use_cfg, dt, ctypes.byref(sc), _lib.ptr(st["seeds"]),
-                                      _lib.ptr(st["step"]), _lib.ptr(st["tok"]), _lib.ptr(st["out"]), S, stream), "lg_sample_rows")
+        self._draw(st, params, st["logits"], slice(0, B), st["step"], st["out"])
 
     def _device_join_t2i(self, st, params: SamplingParams, slot: int):
         """lg_prefill_slot of the condition and mask in st["cond"][slot], st["mask"][slot], then token 0 drawn from its logits
-        (lg_sample_rows, one image, the slot's seed, step 0) into st["out"][slot, 0] and st["tok"][slot]."""
-        B, R, S, dev = self.max_num_seqs, st["R"], st["S"], st["dev"]
+        (_draw: one image, the slot's seed, guidance, step 0) into st["out"][slot, 0] and st["tok"][slot]."""
+        B, R, dev = self.max_num_seqs, st["R"], st["dev"]
         m = self.model
         lib, handle = _lib.load(), m.engine()
         use_cfg = 1 if R == 2 * B else 0
@@ -338,17 +437,13 @@ class LLM:
             ws, ws_bytes = m._slot_scratch(use_cfg)
             _lib.check(lib.lg_prefill_slot(handle, _lib.ptr(st["cond"][slot]), _lib.ptr(st["mask"][slot]), m.cls_token_num, slot, B, use_cfg,
                                            ws, ws_bytes, _lib.ptr(st["join_logits"]), stream), "lg_prefill_slot")
-        sc = self._sample_cfg(params)
-        dt = _lib.dtype_code(m.tok_embeddings.weight.dtype)
-        _lib.check(lib.lg_sample_rows(_lib.ptr(st["join_logits"]), 1, m.vocab_size, use_cfg, dt, ctypes.byref(sc),
-                                      _lib.ptr(st["seeds"][slot:slot + 1]), _lib.ptr(st["step0"]), _lib.ptr(st["tok"][slot:slot + 1]),
-                                      _lib.ptr(st["out"][slot]), S, stream), "lg_sample_rows")
+        self._draw(st, params, st["join_logits"], slice(slot, slot + 1), st["step0"], st["out"][slot])
 
     def _device_join_prefix(self, st, params: SamplingParams, slot: int, P: int):
         """The join of a completion request with P given tokens, already in st["out"][slot, :P]: lg_prefill_slot_prefix of the slot's
         condition (c2i: the class id in st["tok"][slot]; t2i: st["cond"][slot] and st["mask"][slot]) and the prefix, then token P drawn
-        from its logits (lg_sample_rows, one image, the slot's seed, step P) into st["out"][slot, P] and st["tok"][slot]."""
-        B, R, S, dev = self.max_num_seqs, st["R"], st["S"], st["dev"]
+        from its logits (_draw: one image, the slot's seed, guidance, step P) into st["out"][slot, P] and st["tok"][slot]."""
+        B, R, dev = self.max_num_seqs, st["R"], st["dev"]
         m = self.model
         lib, handle = _lib.load(), m.engine()
         use_cfg = 1 if R == 2 * B else 0
@@ -365,11 +460,7 @@ class LLM:
             _lib.check(lib.lg_prefill_slot_prefix(handle, cond, mask, m.cls_token_num, _lib.ptr(st["out"][slot]), P, slot, B, use_cfg, ws,
                                                   ws_bytes, _lib.ptr(st["join_logits"]), stream), "lg_prefill_slot_prefix")
         st["join_step"].fill_(P)
-        sc = self._sample_cfg(params)
-        dt = _lib.dtype_code(m.tok_embeddings.weight.dtype)
-        _lib.check(lib.lg_sample_rows(_lib.ptr(st["join_logits"]), 1, m.vocab_size, use_cfg, dt, ctypes.byref(sc),
-                                      _lib.ptr(st["seeds"][slot:slot + 1]), _lib.ptr(st["join_step"]), _lib.ptr(st["tok"][slot:slot + 1]),
-                                      _lib.ptr(st["out"][slot]), S, stream), "lg_sample_rows")
+        self._draw(st, params, st["join_logits"], slice(slot, slot + 1), st["join_step"], st["out"][slot])
 
     def _step_t2i(self, st, params: SamplingParams) -> List[RequestOutput]:
         """step() of a t2i LLM: decode the running slots, then admit waiting requests (their prefill draws token 0), then return the
@@ -388,7 +479,7 @@ class LLM:
         # with P given tokens (written to its out row first), token P
         joined = []
         for i in range(B):
-            if not self._waiting or self._waiting[0].params != params:
+            if not self._waiting or _batch_key(self._waiting[0].params) != _batch_key(params):
                 break
             if self._slots[i] is None:
                 req = self._waiting.popleft()
@@ -396,7 +487,7 @@ class LLM:
                 joined.append((i, req))
         if joined:
             idx = torch.tensor([i for i, _ in joined], dtype=torch.long, device=dev)
-            st["seeds"][idx] = torch.tensor([self._seed + int(r.request_id) for _, r in joined], dtype=torch.int64, device=dev)
+            self._write_guidance(st, idx, [r for _, r in joined])
             for i, r in joined:
                 st["cond"][i].copy_(r.cond)
                 st["mask"][i].copy_(r.mask)
@@ -432,19 +523,15 @@ class LLM:
         return outs
 
     def _device_step(self, st, params: SamplingParams):
-        """lg_decode_rows + lg_sample_rows on the slots' device state: logits of every row at its own position, then one draw per
+        """lg_decode_rows + a draw (_draw) on the slots' device state: logits of every row at its own position, then one draw per
         slot written to st["out"][slot, depth] and, in place, to st["tok"][slot] (the next step's input)."""
-        B, R, S, dev = self.max_num_seqs, st["R"], st["S"], st["dev"]
+        B, R, dev = self.max_num_seqs, st["R"], st["dev"]
         lib, handle = _lib.load(), self.model.engine()
         use_cfg = 1 if R == 2 * B else 0
         stream = _lib.current_stream(dev)
         _lib.check(lib.lg_decode_rows(handle, _lib.ptr(st["tok"]), _lib.ptr(st["pos"]), B, use_cfg, _lib.ptr(st["logits"]), stream),
                    "lg_decode_rows")
-        sc = self._sample_cfg(params)
-        dt = _lib.dtype_code(self.model.tok_embeddings.weight.dtype)   # 16-bit models round the head's logits to their dtype
-        _lib.check(lib.lg_sample_rows(_lib.ptr(st["logits"]), B, self.model.vocab_size, use_cfg, dt, ctypes.byref(sc),
-                                      _lib.ptr(st["seeds"]), _lib.ptr(st["pos"]), _lib.ptr(st["tok"]), _lib.ptr(st["out"]), S, stream),
-                   "lg_sample_rows")
+        self._draw(st, params, st["logits"], slice(0, B), st["pos"], st["out"])
 
     @torch.no_grad()
     def step(self) -> List[RequestOutput]:
@@ -462,7 +549,7 @@ class LLM:
         # (1) admission: requests that share the running set's sampling parameters join at position 0, mid-sequence of the others
         joined = []
         for i in range(B):
-            if not self._waiting or self._waiting[0].params != params:
+            if not self._waiting or _batch_key(self._waiting[0].params) != _batch_key(params):
                 break
             if self._slots[i] is None:
                 req = self._waiting.popleft()
@@ -471,7 +558,7 @@ class LLM:
         if joined:
             idx = torch.tensor([i for i, _ in joined], dtype=torch.long, device=dev)
             st["tok"][idx] = torch.tensor([r.prompt_token_ids[0] for _, r in joined], dtype=torch.int32, device=dev)
-            st["seeds"][idx] = torch.tensor([self._seed + int(r.request_id) for _, r in joined], dtype=torch.int64, device=dev)
+            self._write_guidance(st, idx, [r for _, r in joined])
             rows = torch.cat([idx, idx + B]) if R == 2 * B else idx
             st["pos"][rows] = 0
             st["active"][rows] = 1
@@ -565,8 +652,9 @@ class LLM:
             if negative_prompt_embeds is not None and len(negative_prompt_embeds) != n:
                 raise ValueError(f"negative prompts hold {len(negative_prompt_embeds)} entries for {n} requests")
             per = sampling_params if isinstance(sampling_params, list) else [sampling_params or SamplingParams()] * n
-            captions = [self._caption(f) for f in prompt_embeds]       # every caption, negative and prefix is checked before any is queued
-            negs = [self._negative(f) for f in (negative_prompt_embeds or [None] * n)]
+            scales = [self._guidance(p)[0] for p in per]             # every guidance, caption, negative and prefix is checked before any
+            captions = [self._caption(f) for f in prompt_embeds]       # is queued
+            negs = [self._negative(f, s) for f, s in zip(negative_prompt_embeds or [None] * n, scales)]
             pfx = self._prefixes(prefixes, n, per)
             for c, p, pf, ng in zip(captions, per, pfx, negs):
                 if ng is None:
@@ -587,6 +675,8 @@ class LLM:
         if isinstance(sampling_params, list) and len(sampling_params) != n:
             raise ValueError("The lengths of prompts and sampling_params must be the same.")
         per = sampling_params if isinstance(sampling_params, list) else [sampling_params or SamplingParams()] * n
+        for p in per:
+            self._guidance(p)
         half = n // 2
         paired = (self.cfg_scale > 1.0 and n % 2 == 0 and n > 0 and
                   all(list(p) == [self.num_classes] for p in prompt_token_ids[half:]) and
