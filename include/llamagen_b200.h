@@ -278,6 +278,26 @@ int  lg_sjd_workspace_bytes(lg_engine* e, int B, int use_cfg, int L, size_t* byt
 int  lg_generate_sjd(lg_engine* e, const void* cond, const float* emb_mask, int B, int T, int S, const lg_sample_cfg* sc, int L,
                      void* dev_ws, size_t ws_bytes, int32_t* out_tokens, int32_t* iters_out, float* dbg_probs, void* stream);
 
+/* ---- SJD over serving slots (serve.LLM(sjd_window=L)): the state of lg_generate_sjd per slot instead of per call ------------------
+ * Slot b (KV-cache rows b and, with use_cfg, B + b) is one request with its own seed and pass counter, keyed as image 0 of
+ * lg_generate_sjd with that seed: u_purpose(k) and pass_seed(0, pass) with the slot's seed, pass counting the passes since the slot's
+ * start (0 at the start). A slot with nfin >= S is frozen: a pass writes nothing of it (out row, window, q, counters); its rows keep
+ * running. The state lives in dev_ws (lg_sjd_slots_workspace_bytes, 256-byte aligned); the KV cache is the workspace's
+ * (rows >= (use_cfg ? 2 : 1) * B, max_seq >= T + S). Every argument is checked before any launch. */
+int  lg_sjd_slots_workspace_bytes(lg_engine* e, int B, int use_cfg, int L, size_t* bytes);
+/* Every slot free (frozen for any S): run once on a new scratch and whenever S changes. */
+int  lg_sjd_slots_reset(lg_engine* e, int B, int use_cfg, int L, void* dev_ws, size_t ws_bytes, void* stream);
+/* Start slot `slot` after its join drew token 0 into out_tokens[slot * S] (dev int32 [B, S]): nfin = 1, its rows at position T, pass
+ * counter 0, window [token 0, u_init drafts of `seed`], and its L window rows' guidance (cfg_scale, cfg_interval; read with use_cfg). */
+int  lg_sjd_slot_start(lg_engine* e, int slot, int B, int use_cfg, int L, int S, uint64_t seed, float cfg_scale, int cfg_interval,
+                       const int32_t* out_tokens, void* dev_ws, size_t ws_bytes, void* stream);
+/* One pass over every slot: the window rows (nh * B * L, at the slots' positions; emb_mask [B, T] and neg_mask [B, T] as in
+ * lg_decode_rows_t2i_neg) through the layers and the head, p and x of every row with its slot's seed, token index and guidance (sc: the
+ * rest of the sampling configuration), acceptance and the next window, as one pass of lg_generate_sjd. nfin_out: host-pinned or dev
+ * int32 [B], every slot's final count after the pass (copied on `stream`). dbg_p: NULL or dev f32 [B][L][V], this pass's p rows. */
+int  lg_sjd_pass_slots(lg_engine* e, const lg_sample_cfg* sc, const float* emb_mask, const float* neg_mask, int B, int use_cfg, int S,
+                       int L, void* dev_ws, size_t ws_bytes, int32_t* out_tokens, int32_t* nfin_out, float* dbg_p, void* stream);
+
 /* ---- VQ tokenizer: replaces VQModel.decode_code / VectorQuantizer (vq_model.py) ------------------- */
 typedef struct lg_vq_cfg {
     int32_t codebook_size;
@@ -458,6 +478,12 @@ int  lg_test_prefix_chunks(lg_engine* e, int* chains);
  * start int32 [B] (updated), out int32 [B][S] (accepted tokens written). Every image must have nfin < S. */
 int  lg_test_sjd_verify(int B, int S, int L, int V, int greedy, uint64_t seed, const float* p, const float* q, const int32_t* qflag,
                         const int32_t* x, const int32_t* win, int32_t* nfin, int32_t* start, int32_t* out, void* stream);
+/* Test entry: one per-slot pass's verify + refresh (lg_sjd_pass_slots without the forward) on given rows: p dev f32 [B][L][V], x dev
+ * int32 [B][L]; the slot state q [B][L][V], qflag, win [B][L], nfin, start [B], seed_slots (uint64) and pass_slots [B] in and out;
+ * seed_rows (uint64) / step_rows [B][L] and out [B][S] out. Frozen slots (nfin >= S) are left as they are. */
+int  lg_test_sjd_slots(int B, int S, int L, int V, int greedy, const float* p, const int32_t* x, float* q, int32_t* qflag, int32_t* win,
+                       int32_t* nfin, int32_t* start, uint64_t* seed_slots, int32_t* pass_slots, uint64_t* seed_rows, int32_t* step_rows,
+                       int32_t* out, void* stream);
 
 /* One launch of the sample kernel with every input the engine can give it (dev buffers). logits, B, V, mix_cfg, round_dtype, sc as
  * lg_sample; the step is step, or *step_dev when step_dev is given, or step_rows[b] with seed_rows[b] as the seed (lg_sample_rows);

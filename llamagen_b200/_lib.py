@@ -103,8 +103,16 @@ SIGNATURES = {
     "lg_sjd_workspace_bytes": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(c_size_t)]),
     "lg_generate_sjd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(SampleCfg), c_int, c_void_p, c_size_t,
                                 c_void_p, c_void_p, c_void_p, c_void_p]),
-    "lg_test_sjd_verify": (c_int, [c_int, c_int, c_int, c_int, c_int, c_uint64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+    "lg_sjd_slots_workspace_bytes": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(c_size_t)]),
+    "lg_sjd_slots_reset": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
+    "lg_sjd_slot_start": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_uint64, c_float, c_int, c_void_p, c_void_p, c_size_t,
+                                  c_void_p]),
+    "lg_sjd_pass_slots": (c_int, [c_void_p, POINTER(SampleCfg), c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_size_t,
+                                  c_void_p, c_void_p, c_void_p, c_void_p]),
+    "lg_test_sjd_verify": (c_int,[c_int, c_int, c_int, c_int, c_int, c_uint64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                    c_void_p, c_void_p, c_void_p, c_void_p]),
+    "lg_test_sjd_slots": (c_int, [c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "lg_test_sample": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(SampleCfg), c_uint64, c_void_p, c_int, c_void_p, c_void_p,
                                c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                                c_void_p, c_float, c_int, c_int, c_void_p, c_void_p, c_void_p, POINTER(c_int), c_void_p]),

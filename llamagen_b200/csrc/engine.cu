@@ -347,6 +347,7 @@ struct lg_engine {
     size_t carve(Workspace& o, char* base, int rows, int max_seq, int g = 0, int n = 1) const;
     size_t carve_score(Workspace& o, char* base, int rows, int seq) const;
     size_t carve_sjd(RowBuffers& o, SjdArgs& sa, char* base, int B, int nh, int L) const;
+    size_t carve_sjd_slots(RowBuffers& o, SjdArgs& sa, char* base, int B, int nh, int L) const;
     size_t carve_prefix(RowBuffers& o, char* base, int rows, int seq) const;
     size_t carve_slot(RowBuffers& head, char* base, int nh, int seq) const;
     void carve_kv(Carver& c, KvCache& o, int rows, int max_seq, int layers, bool f8) const;
@@ -478,6 +479,18 @@ size_t lg_engine::carve_sjd(RowBuffers& o, SjdArgs& sa, char* base, int B, int n
     sa.shift = (int32_t*)c.split(B * sizeof(int32_t));
     sa.pos_rows = (int32_t*)c.split((size_t)nh * B * sizeof(int32_t));
     sa.state = (int32_t*)c.split(kSjdStateInts * sizeof(int32_t));
+    return c.off;
+}
+
+// Serving's SJD state for B slots (lg_sjd_slots_workspace_bytes), from `base` (null: sizes only): carve_sjd's scratch, then every slot's
+// seed and pass counter and the guidance of every window row
+size_t lg_engine::carve_sjd_slots(RowBuffers& o, SjdArgs& sa, char* base, int B, int nh, int L) const {
+    Carver c{base, 0, 1, carve_sjd(o, sa, base, B, nh, L)};
+    const size_t BL = (size_t)B * L;
+    sa.seed_slots = (uint64_t*)c.split(B * sizeof(uint64_t));
+    sa.pass_slots = (int32_t*)c.split(B * sizeof(int32_t));
+    sa.cfg_rows = (float*)c.split(BL * sizeof(float));
+    sa.interval_rows = (int32_t*)c.split(BL * sizeof(int32_t));
     return c.off;
 }
 
@@ -1247,6 +1260,19 @@ static int prefill_slot_impl(const char* fn, lg_engine* e, const void* cond, con
     LG_REQUIRE(attn_plan(e->attn_args(e->full, 0, 1, seq)).kernel >= 0, "%s: %s", fn, attn_plan(e->attn_args(e->full, 0, 1, seq)).error);
     DeviceGuard guard(e->device);
     LG_TRY(e->zero_fill_if_needed(st));
+    // a c2i join without a prefix is one position per row: where lg_prefill of one image takes the small-row decode path, the join
+    // takes it too, one row at a time, so that a one-slot server draws token 0 from the logits generate() draws it from at B = 1
+    if (seq == 1 && c.model_type == LG_MODEL_C2I && e->small_row_path(1, e->attn_args(e->full, 0, 1, 1))) {
+        for (int half = 0; half < nh; ++half) {
+            Workspace w;
+            static_cast<KvCache&>(w) = e->full;
+            w.first_row = half * B + slot;
+            e->carve_prefix(w, (char*)dev_ws, 1, 1);
+            LG_TRY(e->embed_cond(w, cond, nullptr, half != 0 ? 0 : 1, 1, T, st));
+            LG_TRY(e->forward(w, 1, 1, PosArg{nullptr, 0}, nullptr, nullptr, 1, logits_out + (size_t)half * V, false, st));
+        }
+        return round_logits_inplace(logits_out, (size_t)nh * V, c.dtype, st);
+    }
     for (int half = 0; half < nh; ++half)
         LG_TRY(prefill_chunk(e, e->full, half * B + slot, 1, cond, half != 0, neg.cond, prefix, half != 0 && neg.mask ? neg.mask : emb_mask,
                              T, P, (char*)dev_ws, ws_bytes, hb.q + (size_t)half * D * e->esz, fn, st));
@@ -1512,6 +1538,106 @@ int lg_generate_sjd_neg(lg_engine* e, const void* cond, const float* emb_mask, c
                               out_tokens, iters_out, dbg_probs, stream);
 }
 
+}  // extern "C"
+
+// The checks every per-slot SJD entry fn makes of its shape (S: 0 when the entry takes none) and scratch, then sa and w over dev_ws:
+// the slot state and row buffers of the scratch, the KV cache of the workspace
+static int sjd_slots_view(const char* fn, lg_engine* e, int B, int use_cfg, int L, int S, void* dev_ws, size_t ws_bytes, Workspace& w,
+                          SjdArgs& sa) {
+    LG_REQUIRE(B > 0, "%s: B=%d", fn, B);
+    LG_REQUIRE(L >= 2 && L <= 64, "%s: window L=%d outside [2, 64]", fn, L);
+    LG_REQUIRE(S == 0 || S > L, "%s: S=%d must exceed the window L=%d", fn, S, L);
+    LG_REQUIRE(dev_ws && ((uintptr_t)dev_ws & 255) == 0, "%s: scratch must be non-null and 256-byte aligned", fn);
+    LG_REQUIRE(e && e->finalized, "%s: engine not finalized", fn);
+    const lg_model_cfg& c = e->cfg;
+    const int nh = use_cfg ? 2 : 1;
+    LG_REQUIRE(S <= c.block_size, "%s: S=%d exceeds block_size=%d", fn, S, c.block_size);
+    LG_REQUIRE((size_t)c.vocab_size * sizeof(float) <= 200 * 1024, "%s: vocab %d too large for the sampler", fn, c.vocab_size);
+    LG_REQUIRE((long long)nh * B * L <= 65535, "%s: %d rows x window %d exceed 65535 query rows", fn, nh * B, L);
+    LG_TRY(check_ready(e, nh * B, c.cls_token_num + std::max(S, L + 1)));
+    const size_t need = e->carve_sjd_slots(w, sa, (char*)dev_ws, B, nh, L);
+    LG_REQUIRE(ws_bytes >= need, "%s: scratch of %zu bytes is too small (%zu)", fn, ws_bytes, need);
+    static_cast<KvCache&>(w) = e->full;
+    sa.B = B; sa.S = S; sa.L = L; sa.V = c.vocab_size; sa.T = c.cls_token_num; sa.nh = nh; sa.row_offset = 0;
+    if (!use_cfg) { sa.cfg_rows = nullptr; sa.interval_rows = nullptr; }
+    return 0;
+}
+
+extern "C" {
+
+int lg_sjd_slots_workspace_bytes(lg_engine* e, int B, int use_cfg, int L, size_t* bytes) {
+    LG_REQUIRE(e && bytes && B > 0 && L >= 2 && L <= 64, "lg_sjd_slots_workspace_bytes: bad argument (B=%d L=%d)", B, L);
+    Workspace w;
+    SjdArgs sa{};
+    *bytes = e->carve_sjd_slots(w, sa, nullptr, B, use_cfg ? 2 : 1, L);
+    return 0;
+}
+
+int lg_sjd_slots_reset(lg_engine* e, int B, int use_cfg, int L, void* dev_ws, size_t ws_bytes, void* stream) {
+    Workspace w;
+    SjdArgs sa{};
+    LG_TRY(sjd_slots_view("lg_sjd_slots_reset", e, B, use_cfg, L, 0, dev_ws, ws_bytes, w, sa));
+    cudaStream_t st = (cudaStream_t)stream;
+    DeviceGuard guard(e->device);
+    // zeros everywhere (valid window tokens and positions for the rows of free slots), then nfin = 0x7f7f7f7f: every slot frozen
+    RowBuffers rb;
+    SjdArgs sizes{};
+    LG_CUDA_OK(cudaMemsetAsync(dev_ws, 0, e->carve_sjd_slots(rb, sizes, nullptr, B, sa.nh, L), st));
+    LG_CUDA_OK(cudaMemsetAsync(sa.nfin, 0x7f, (size_t)B * sizeof(int32_t), st));
+    return 0;
+}
+
+int lg_sjd_slot_start(lg_engine* e, int slot, int B, int use_cfg, int L, int S, uint64_t seed, float cfg_scale, int cfg_interval,
+                      const int32_t* out_tokens, void* dev_ws, size_t ws_bytes, void* stream) {
+    static const char* fn = "lg_sjd_slot_start";
+    LG_REQUIRE(out_tokens, "%s: null out_tokens", fn);
+    LG_REQUIRE(slot >= 0 && slot < B, "%s: slot %d outside [0, B=%d)", fn, slot, B);
+    LG_REQUIRE(S > 0, "%s: S=%d", fn, S);
+    LG_REQUIRE(std::isfinite(cfg_scale) && cfg_interval >= -1, "%s: cfg_scale %g must be finite and cfg_interval %d >= -1", fn,
+               (double)cfg_scale, cfg_interval);
+    Workspace w;
+    SjdArgs sa{};
+    LG_TRY(sjd_slots_view(fn, e, B, use_cfg, L, S, dev_ws, ws_bytes, w, sa));
+    DeviceGuard guard(e->device);
+    sa.seed = seed; sa.start_cfg = cfg_scale; sa.start_interval = cfg_interval;
+    sa.out = const_cast<int32_t*>(out_tokens);   // read only: token 0 of the slot's row
+    return launch_sjd_refresh(sa, 1, (cudaStream_t)stream, slot);
+}
+
+int lg_sjd_pass_slots(lg_engine* e, const lg_sample_cfg* sc, const float* emb_mask, const float* neg_mask, int B, int use_cfg, int S, int L,
+                      void* dev_ws, size_t ws_bytes, int32_t* out_tokens, int32_t* nfin_out, float* dbg_p, void* stream) {
+    static const char* fn = "lg_sjd_pass_slots";
+    LG_REQUIRE(sc && out_tokens && nfin_out, "%s: null argument", fn);
+    LG_REQUIRE(S > 0, "%s: S=%d", fn, S);
+    LG_REQUIRE(!neg_mask || use_cfg, "%s: neg_mask masks the unconditional CFG rows and needs use_cfg", fn);
+    LG_REQUIRE(!neg_mask || emb_mask, "%s: neg_mask needs emb_mask (all ones for an unmasked condition)", fn);
+    Workspace w;
+    SjdArgs sa{};
+    LG_TRY(sjd_slots_view(fn, e, B, use_cfg, L, S, dev_ws, ws_bytes, w, sa));
+    const lg_model_cfg& c = e->cfg;
+    LG_REQUIRE(!emb_mask || c.model_type == LG_MODEL_T2I, "%s: emb_mask only applies to t2i models", fn);
+    const int V = c.vocab_size, D = c.dim, dt = c.dtype, M = sa.nh * B * L;
+    cudaStream_t st = (cudaStream_t)stream;
+    DeviceGuard guard(e->device);
+    LG_TRY(e->zero_fill_if_needed(st));
+    sa.greedy = sc->greedy; sa.out = out_tokens;
+    // generate_sjd_impl's pass over the slots: window embedding, the layers over nh * B * L rows at the slots' positions, the head, p and
+    // x of every row with the row's seed, token index and guidance, acceptance, next window
+    LG_PROF(PC_EMBED_MISC, st, launch_embed(e->tok_emb, sa.win, B * L, M, -1, D, dt, w.h, st));
+    LG_TRY(e->run_layers(w, M, L, PosArg{nullptr, 0, sa.pos_rows}, emb_mask, neg_mask, B, false, st));
+    LG_TRY(e->head(w, w.xn, M, w.logits, nullptr, st));
+    SampleArgs sp = make_sample_args(*sc, w.logits, B * L, V, use_cfg, dt);
+    sp.seed_rows = sa.seed_rows; sp.step_rows = sa.step_rows;
+    sp.cfg_rows = sa.cfg_rows; sp.interval_rows = sa.interval_rows;
+    sp.out_idx = const_cast<int32_t*>(sa.x); sp.out_probs = const_cast<float*>(sa.p);
+    LG_PROF(PC_SAMPLE, st, launch_sample(sp, st));
+    if (dbg_p) LG_CUDA_OK(cudaMemcpyAsync(dbg_p, sa.p, (size_t)B * L * V * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    LG_PROF(PC_SAMPLE, st, launch_sjd_verify(sa, st));
+    LG_PROF(PC_SAMPLE, st, launch_sjd_refresh(sa, 0, st));
+    LG_CUDA_OK(cudaMemcpyAsync(nfin_out, sa.nfin, (size_t)B * sizeof(int32_t), cudaMemcpyDefault, st));
+    return 0;
+}
+
 int lg_test_sjd_verify(int B, int S, int L, int V, int greedy, uint64_t seed, const float* p, const float* q, const int32_t* qflag,
                        const int32_t* x, const int32_t* win, int32_t* nfin, int32_t* start, int32_t* out, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
@@ -1526,6 +1652,27 @@ int lg_test_sjd_verify(int B, int S, int L, int V, int greedy, uint64_t seed, co
     LG_CUDA_OK(cudaMemsetAsync(tmp, 0, (2 * (size_t)B + kSjdStateInts) * sizeof(int32_t), st));
     sa.shift = tmp; sa.pos_rows = tmp + B; sa.state = tmp + 2 * B;
     const int rc = launch_sjd_verify(sa, st);
+    cudaFreeAsync(tmp, st);
+    return rc;
+}
+
+int lg_test_sjd_slots(int B, int S, int L, int V, int greedy, const float* p, const int32_t* x, float* q, int32_t* qflag, int32_t* win,
+                      int32_t* nfin, int32_t* start, uint64_t* seed_slots, int32_t* pass_slots, uint64_t* seed_rows, int32_t* step_rows,
+                      int32_t* out, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    LG_REQUIRE(p && x && q && qflag && win && nfin && start && seed_slots && pass_slots && seed_rows && step_rows && out,
+               "lg_test_sjd_slots: null argument");
+    LG_REQUIRE(B > 0 && V > 0 && L >= 2 && L <= 64 && S > L, "lg_test_sjd_slots: bad shape B=%d S=%d L=%d V=%d", B, S, L, V);
+    SjdArgs sa{};
+    sa.B = B; sa.S = S; sa.L = L; sa.V = V; sa.T = 0; sa.nh = 1; sa.greedy = greedy;
+    sa.p = p; sa.q = q; sa.qflag = qflag; sa.x = x; sa.win = win; sa.nfin = nfin; sa.start = start; sa.out = out; sa.done_token = 1;
+    sa.seed_slots = seed_slots; sa.pass_slots = pass_slots; sa.seed_rows = seed_rows; sa.step_rows = step_rows;
+    int32_t* tmp = nullptr;   // shift [B], pos_rows [B], loop state
+    LG_CUDA_OK(cudaMallocAsync((void**)&tmp, (2 * (size_t)B + kSjdStateInts) * sizeof(int32_t), st));
+    LG_CUDA_OK(cudaMemsetAsync(tmp, 0, (2 * (size_t)B + kSjdStateInts) * sizeof(int32_t), st));
+    sa.shift = tmp; sa.pos_rows = tmp + B; sa.state = tmp + 2 * B;
+    int rc = launch_sjd_verify(sa, st);
+    if (rc == 0) rc = launch_sjd_refresh(sa, 0, st);
     cudaFreeAsync(tmp, st);
     return rc;
 }

@@ -83,9 +83,18 @@ struct SjdArgs {
     int32_t* state;              // [kSjdStateInts], zero-initialised
     float* dbg;                  // [passes][B][L][V] copy of every pass's p rows, or null
     int done_token;              // written to state[kSjdDone] once every image has S tokens (unique per call)
+    // Per-slot mode (serving, lg_sjd_pass_slots): every image b is a slot with its own seed and pass counter, keyed as image 0 of a
+    // call with that seed (seed and row_offset unused). A slot with nfin >= S is frozen: verify and refresh write nothing of it.
+    uint64_t* seed_slots = nullptr;   // [B] or null (per-call mode)
+    int32_t* pass_slots = nullptr;    // [B] passes the slot has run since its start; verify advances it, refresh keys with it
+    float* cfg_rows = nullptr;        // [B * L] per-row guidance of the window rows (a start writes its slot's L rows), or null
+    int32_t* interval_rows = nullptr; // [B * L]
+    float start_cfg = 1.f;            // a start's (first = 1, one slot) seed is `seed`; its guidance scale and cfg_interval
+    int start_interval = -1;
 };
 int launch_sjd_verify(const SjdArgs& a, cudaStream_t st);
-int launch_sjd_refresh(const SjdArgs& a, int first, cudaStream_t st);
+// slot >= 0: only image `slot` (a per-slot start, with first = 1)
+int launch_sjd_refresh(const SjdArgs& a, int first, cudaStream_t st, int slot = -1);
 
 // ------------------------------------------------------------------------------------------------
 // gemm.cu — y_partial[ks][M][N] (f32) = x[M,K] * W[N,K]^T ; W may be two row segments (w1 | w3).

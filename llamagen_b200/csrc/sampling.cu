@@ -548,6 +548,8 @@ __global__ void __launch_bounds__(kSjdThreads) sjd_verify_kernel(SjdArgs a) {
     const int L = a.L, V = a.V, S = a.S;
     const int n = a.nfin[b], s = a.start[b];
     const bool active = n < S;
+    const uint64_t seed = a.seed_slots ? a.seed_slots[b] : a.seed;   // per-slot mode: the slot's seed, image 0
+    const int img = a.seed_slots ? 0 : b + a.row_offset;
     if (active) {
         const size_t row0 = (size_t)b * L;
         if (tid == 0) {
@@ -560,7 +562,7 @@ __global__ void __launch_bounds__(kSjdThreads) sjd_verify_kernel(SjdArgs a) {
                 } else {
                     const float pd = a.p[(row0 + i) * V + d];
                     const float qd = a.qflag[row0 + i] ? 1.0f / (float)V : a.q[(row0 + i) * V + d];
-                    acc = sjd_uniform(a.seed, b + a.row_offset, k, kSjdAccept) * qd < pd;
+                    acc = sjd_uniform(seed, img, k, kSjdAccept) * qd < pd;
                 }
                 if (!acc) break;
                 a.out[(size_t)b * S + k] = d;
@@ -602,7 +604,7 @@ __global__ void __launch_bounds__(kSjdThreads) sjd_verify_kernel(SjdArgs a) {
             __syncthreads();
             const float total = red[32];
             if (total > 0.f) {
-                const float target = sjd_uniform(a.seed, b + a.row_offset, s + i, kSjdResidual) * total;
+                const float target = sjd_uniform(seed, img, s + i, kSjdResidual) * total;
                 const float excl = s_wtot[warp] + (incl - local);
                 // one owner for every target, as in sample_kernel: the highest thread with a positive segment starting at or below
                 // it; a walk that never passes the target takes the segment's last positive weight
@@ -628,6 +630,7 @@ __global__ void __launch_bounds__(kSjdThreads) sjd_verify_kernel(SjdArgs a) {
             a.start[b] = s2;
             a.shift[b] = s2 - s;
             for (int hh = 0; hh < a.nh; ++hh) a.pos_rows[hh * a.B + b] = a.T + s2 - 1;
+            if (a.pass_slots) a.pass_slots[b] += 1;
             atomicAdd(&a.state[kSjdActive], 1);
             if (n2 >= S) atomicAdd(&a.state[kSjdFinished], 1);
         }
@@ -644,13 +647,17 @@ __global__ void __launch_bounds__(kSjdThreads) sjd_verify_kernel(SjdArgs a) {
     }
 }
 
-// grid (B, L): slot i of image b's next window. first = 1 sets up the window after the prefill (token 0 final, all drafts new).
-__global__ void __launch_bounds__(256) sjd_refresh_kernel(SjdArgs a, int first) {
+// grid (B, L), or (1, L) for image `slot` >= 0: slot i of image b's next window. first = 1 sets up the window after the prefill (token
+// 0 final, all drafts new); in per-slot mode it also sets the slot's seed, pass counter and window rows' guidance.
+__global__ void __launch_bounds__(256) sjd_refresh_kernel(SjdArgs a, int first, int only) {
     lg_pdl_sync();
-    const int b = blockIdx.x, i = blockIdx.y, L = a.L, V = a.V, S = a.S;
+    const int b = only >= 0 ? only : blockIdx.x, i = blockIdx.y, L = a.L, V = a.V, S = a.S;
     const size_t slot = (size_t)b * L + i;
     if (!first && !a.state[kSjdLive]) return;   // a pass after every image finished changes nothing
-    const int pass = a.state[kSjdIters];        // index of the next pass
+    // index of the next pass: the call's, or the slot's own (0 at its start)
+    const int pass = a.pass_slots ? (first ? 0 : a.pass_slots[b]) : a.state[kSjdIters];
+    const uint64_t seed = a.seed_slots && !first ? a.seed_slots[b] : a.seed;
+    const int img = a.seed_slots ? 0 : b + a.row_offset;
     if (!first && a.dbg) {
         float* d = a.dbg + ((size_t)(pass - 1) * a.B * L + slot) * V;
         for (int v = threadIdx.x; v < V; v += blockDim.x) d[v] = a.p[slot * V + v];
@@ -661,14 +668,16 @@ __global__ void __launch_bounds__(256) sjd_refresh_kernel(SjdArgs a, int first) 
         if (i == 0 && threadIdx.x == 0) {
             a.nfin[b] = 1; a.start[b] = 1;
             for (int hh = 0; hh < a.nh; ++hh) a.pos_rows[hh * a.B + b] = a.T;
+            if (a.seed_slots) { a.seed_slots[b] = a.seed; a.pass_slots[b] = 0; }
         }
+        if (a.cfg_rows && threadIdx.x == 0) { a.cfg_rows[slot] = a.start_cfg; a.interval_rows[slot] = a.start_interval; }
     } else {
         n = a.nfin[b]; s = a.start[b]; shift = a.shift[b];
         if (n >= S) return;                      // finished: its rows keep running on the old window, their outputs unused
     }
     const int k = s + i - 1;                     // the token this slot feeds
     if (threadIdx.x == 0) {
-        a.seed_rows[slot] = sjd_pass_seed(a.seed, b + a.row_offset, pass);
+        a.seed_rows[slot] = sjd_pass_seed(seed, img, pass);
         a.step_rows[slot] = s + i;
     }
     if (k < n) {
@@ -683,7 +692,7 @@ __global__ void __launch_bounds__(256) sjd_refresh_kernel(SjdArgs a, int first) 
         for (int v = threadIdx.x; v < V; v += blockDim.x) dst[v] = src[v];
         if (threadIdx.x == 0) { a.win[slot] = a.x[(size_t)b * L + j]; a.qflag[qs] = 0; }
     } else if (threadIdx.x == 0) {               // a new index: uniform over the vocabulary, q = 1 / V
-        const int t = (int)(sjd_uniform(a.seed, b + a.row_offset, k, kSjdInit) * (float)V);
+        const int t = (int)(sjd_uniform(seed, img, k, kSjdInit) * (float)V);
         a.win[slot] = min(t, V - 1);
         a.qflag[qs] = 1;
     }
@@ -698,9 +707,10 @@ int launch_sjd_verify(const SjdArgs& a, cudaStream_t st) {
     return 0;
 }
 
-int launch_sjd_refresh(const SjdArgs& a, int first, cudaStream_t st) {
+int launch_sjd_refresh(const SjdArgs& a, int first, cudaStream_t st, int slot) {
     LG_REQUIRE(a.B > 0 && a.L >= 1 && a.L <= 64 && a.S > a.L && a.V > 0, "sjd: bad shape B=%d L=%d S=%d V=%d", a.B, a.L, a.S, a.V);
-    (void)lg_launch(sjd_refresh_kernel, dim3(a.B, a.L), dim3(256), 0, st, a, first);
+    LG_REQUIRE(slot < a.B && (slot < 0 || first), "sjd: a refresh of one slot (%d of B=%d) is a start (first = 1)", slot, a.B);
+    (void)lg_launch(sjd_refresh_kernel, dim3(slot >= 0 ? 1 : a.B, a.L), dim3(256), 0, st, a, first, slot);
     LG_LAUNCH_CHECK();
     return 0;
 }

@@ -52,6 +52,14 @@ and its interval allows it, so a request draws the tokens it draws alone in an L
 cfg_interval=k, seed=s) for image 0). A request's seed replaces base_seed + r in st["seeds"]. A scale > 1 needs an LLM built with
 cfg_scale > 1 (the unconditional rows); a request at scale <= 1 in such an LLM keeps its unconditional row running, unread.
 
+Speculative Jacobi decoding (LLM(..., sjd_window=L), 2 <= L <= 64): every step() runs one SJD pass over all slots instead of one decode
+step, and makes up to L tokens of every running request final (generate(sjd_window=L)'s pass on per-slot state: lg_sjd_pass_slots).
+A request's window is min(L, max_tokens - 1); it draws token 0 at its join as a plain request does (a c2i join is
+lg_prefill_slot_prefix with P = 0), then lg_sjd_slot_start keys its window with its own seed and a pass counter from 0, so request r draws
+what generate(cond_r, sjd_window=L, seed=s_r) draws for image 0, whatever ran beside it. A step enqueues its pass, then reads the
+previous pass's final counts (a pinned copy and an event): a finished request leaves, and its slot is reused, one step after its last
+pass; its slot is frozen meanwhile. prefix= requests are refused (as generate() refuses prefix with sjd_window).
+
 While requests are in flight the LLM owns the model's KV-cache workspace (a `generate()` call on the same model would reset it)."""
 from __future__ import annotations
 
@@ -135,7 +143,7 @@ def _plen(req: _Request) -> int:
 
 class LLM:
     def __init__(self, gpt_model, cfg_scale: float = 1.0, num_classes: int = 1000, max_num_seqs: int = 64, seed: Optional[int] = None,
-                 kv_cache_dtype: Optional[str] = None, weight_dtype: Optional[str] = None, text_encoder=None):
+                 kv_cache_dtype: Optional[str] = None, weight_dtype: Optional[str] = None, text_encoder=None, sjd_window: Optional[int] = None):
         """kv_cache_dtype: None keeps the model's KV-cache setting (Transformer.set_kv_cache, scales included); "auto" (the model
         dtype) or "fp8" (e4m3) sets it. Passing the dtype the model already has keeps its scales.
         weight_dtype: None keeps the model's GEMM-weight storage (Transformer.set_weight_dtype, its head choice included); "auto" or
@@ -143,7 +151,16 @@ class LLM:
         A t2i model serves caption requests (prompt_embeds); num_classes does not apply to it.
         text_encoder (t2i only): a t5.T5Encoder whose d_model is the model's caption_dim. Requests may then bring caption strings
         (generate(prompts=...), add_request(prompt=...)); each is encoded on the device and enqueued exactly as prompt_embeds = its
-        valid feature rows would be."""
+        valid feature rows would be.
+        sjd_window: None, or an integer L in [2, 64]: every step() runs one speculative Jacobi decoding pass over all slots (up to
+        min(L, max_tokens - 1) tokens of every running request per step; max_tokens >= 3, no prefix requests). sjd_passes counts the
+        passes run, sjd_tokens the tokens they made final, sjd_request_passes the passes of every finished request."""
+        if sjd_window is not None and (not _is_int(sjd_window) or not 2 <= int(sjd_window) <= 64):
+            raise ValueError(f"sjd_window must be an integer in [2, 64], got {sjd_window!r}")
+        self.sjd_window = None if sjd_window is None else int(sjd_window)
+        self.sjd_passes = 0
+        self.sjd_tokens = 0
+        self.sjd_request_passes: dict[str, int] = {}
         if gpt_model.model_type not in ("c2i", "t2i"):
             raise ValueError(f"serve.LLM handles c2i and t2i models, got model_type {gpt_model.model_type!r}")
         self.t2i = gpt_model.model_type == "t2i"
@@ -283,6 +300,8 @@ class LLM:
             raise ValueError(f"SamplingParams.cfg_interval must be an integer >= -1, got {sp.cfg_interval!r}")
         if sp.seed is not None and (not _is_int(sp.seed) or not 0 <= sp.seed < 2 ** 63):
             raise ValueError(f"SamplingParams.seed must be an integer in [0, 2**63), got {sp.seed!r}")
+        if self.sjd_window is not None and int(sp.max_tokens) < 3:
+            raise ValueError(f"sjd_window needs max_tokens >= 3, got {sp.max_tokens}")
         return scale, int(interval), None if sp.seed is None else int(sp.seed)
 
     def _guided(self, req: _Request) -> _Request:
@@ -305,6 +324,8 @@ class LLM:
         1 <= P <= max_tokens - 1. None stays None."""
         if prefix is None:
             return None
+        if self.sjd_window is not None:
+            raise ValueError("prefix cannot be combined with sjd_window")
         pf = prefix if torch.is_tensor(prefix) else torch.as_tensor(np.asarray(prefix))
         if pf.dim() != 1:
             raise ValueError(f"a request's prefix is 1-D, [P] image token ids, got shape {tuple(pf.shape)}")
@@ -374,6 +395,12 @@ class LLM:
                 neg=torch.zeros(B, T, C, dtype=m.tok_embeddings.weight.dtype, device=dev),
                 neg_mask=torch.zeros(B, T, dtype=torch.float32, device=dev),
                 has_neg=[False] * B)
+        if self.sjd_window is not None:
+            # the window, this LLM's own per-slot SJD scratch (every slot free) and the host's pass bookkeeping: passes enqueued, and the
+            # first pass of every slot's request
+            self._state.update(L=min(self.sjd_window, S - 1), passes=0, first_pass=[0] * B, nfin_host=None, events=None, sjd_ws=None,
+                               copy_stream=None)
+            self._device_sjd_reset(self._state)
         return self._state
 
     def _sample_cfg(self, params: SamplingParams):
@@ -462,6 +489,116 @@ class LLM:
         st["join_step"].fill_(P)
         self._draw(st, params, st["join_logits"], slice(slot, slot + 1), st["join_step"], st["out"][slot])
 
+    def _load_caption(self, st, i: int, r: _Request):
+        """A t2i request's condition, mask and negative to slot i's device rows (before its join)."""
+        st["cond"][i].copy_(r.cond)
+        st["mask"][i].copy_(r.mask)
+        st["has_neg"][i] = r.neg is not None
+        if r.neg is not None:
+            st["neg"][i].copy_(r.neg)
+        st["neg_mask"][i].copy_(r.mask if r.neg_mask is None else r.neg_mask)
+
+    # ------------------------------------------------------------------ speculative Jacobi decoding (sjd_window)
+    def _sjd_scratch(self, st):
+        """(device pointer, bytes) of this LLM's per-slot SJD scratch: 256-byte aligned in st["sjd_ws"]."""
+        buf = st["sjd_ws"]
+        base = (buf.data_ptr() + 255) // 256 * 256
+        return ctypes.c_void_p(base), buf.numel() - (base - buf.data_ptr())
+
+    def _device_sjd_reset(self, st):
+        """A new state's SJD scratch (lg_sjd_slots_workspace_bytes), then lg_sjd_slots_reset: every slot free. The slot state lives
+        across steps, so the scratch belongs to this LLM's state, not to the model: another LLM on the same model cannot overwrite it."""
+        B, use_cfg = self.max_num_seqs, 1 if st["R"] == 2 * self.max_num_seqs else 0
+        lib, handle = _lib.load(), self.model.engine()
+        need = ctypes.c_size_t()
+        _lib.check(lib.lg_sjd_slots_workspace_bytes(handle, B, use_cfg, st["L"], ctypes.byref(need)), "lg_sjd_slots_workspace_bytes")
+        st["sjd_ws"] = torch.empty(need.value + 256, dtype=torch.uint8, device=st["dev"])
+        ws, ws_bytes = self._sjd_scratch(st)
+        _lib.check(_lib.load().lg_sjd_slots_reset(self.model.engine(), B, use_cfg, st["L"], ws, ws_bytes, _lib.current_stream(st["dev"])),
+                   "lg_sjd_slots_reset")
+
+    def _device_sjd_start(self, st, slot: int, req: _Request):
+        """lg_sjd_slot_start of slot, after its join drew token 0: the request's seed, guidance and pass counter 0."""
+        B, use_cfg = self.max_num_seqs, 1 if st["R"] == 2 * self.max_num_seqs else 0
+        ws, ws_bytes = self._sjd_scratch(st)
+        _lib.check(_lib.load().lg_sjd_slot_start(self.model.engine(), slot, B, use_cfg, st["L"], st["S"], req.seed, req.cfg, req.interval,
+                                                 _lib.ptr(st["out"]), ws, ws_bytes, _lib.current_stream(st["dev"])), "lg_sjd_slot_start")
+
+    def _device_sjd_pass(self, st, params: SamplingParams, dbg=None):
+        """Enqueue pass st["passes"] (lg_sjd_pass_slots) over every slot; its final counts go to a pinned buffer behind an event.
+        dbg: None or f32 [B, L, V] on the device, this pass's p rows."""
+        B, dev = self.max_num_seqs, st["dev"]
+        use_cfg = 1 if st["R"] == 2 * B else 0
+        if st["events"] is None:
+            st["nfin_host"] = torch.zeros(2, B, dtype=torch.int32).pin_memory()
+            st["events"] = [torch.cuda.Event(), torch.cuda.Event()]
+        j = st["passes"] & 1
+        ws, ws_bytes = self._sjd_scratch(st)
+        sc = self._sample_cfg(params)
+        mask = _lib.ptr(st["mask"]) if self.t2i else None
+        neg_mask = _lib.ptr(st["neg_mask"]) if self.t2i and use_cfg else None
+        _lib.check(_lib.load().lg_sjd_pass_slots(self.model.engine(), ctypes.byref(sc), mask, neg_mask, B, use_cfg, st["S"], st["L"], ws,
+                                                 ws_bytes, _lib.ptr(st["out"]), _lib.ptr(st["nfin_host"][j]), _lib.ptr(dbg),
+                                                 _lib.current_stream(dev)), "lg_sjd_pass_slots")
+        st["events"][j].record(torch.cuda.current_stream(dev))
+
+    def _sjd_nfin(self, st, p: int) -> List[int]:
+        """Every slot's final count after pass p (the pass before the one last enqueued): waits for that pass only."""
+        st["events"][p & 1].synchronize()
+        return st["nfin_host"][p & 1].tolist()
+
+    def _sjd_rows(self, st, done: List[int], p: int) -> List[List[int]]:
+        """The token rows of the slots in `done`, final after pass p: copied on a side stream behind pass p's event, so that the host
+        does not wait for the pass enqueued after it (that pass writes nothing of a frozen slot)."""
+        dev = st["dev"]
+        if st["copy_stream"] is None:
+            st["copy_stream"] = torch.cuda.Stream(dev)
+        side = st["copy_stream"]
+        side.wait_event(st["events"][p & 1])
+        with torch.cuda.stream(side):
+            rows = st["out"][torch.tensor(done, dtype=torch.long, device=dev)].cpu().tolist()
+        return rows
+
+    def _step_sjd(self, st, params: SamplingParams) -> List[RequestOutput]:
+        """step() with sjd_window: (1) admit waiting requests (their join draws token 0, then their slot starts), (2) enqueue one pass
+        over every slot, (3) finish the requests whose final count reached max_tokens in the pass before it. The host never waits for
+        the pass it just enqueued: a finished slot stays frozen until then, which changes no request's tokens."""
+        B, S, dev = self.max_num_seqs, st["S"], st["dev"]
+        joined = []
+        for i in range(B):
+            if not self._waiting or _batch_key(self._waiting[0].params) != _batch_key(params):
+                break
+            if self._slots[i] is None:
+                req = self._waiting.popleft()
+                self._slots[i] = req
+                joined.append((i, req))
+        if joined:
+            idx = torch.tensor([i for i, _ in joined], dtype=torch.long, device=dev)
+            self._write_guidance(st, idx, [r for _, r in joined])
+            for i, r in joined:
+                if self.t2i:
+                    self._load_caption(st, i, r)
+                    self._device_join_t2i(st, params, i)
+                else:   # one row with the class token (lg_prefill_slot_prefix, P = 0), token 0 drawn with step 0
+                    st["tok"][i] = r.prompt_token_ids[0]
+                    self._device_join_prefix(st, params, i, 0)
+                self._device_sjd_start(st, i, r)
+                st["first_pass"][i] = st["passes"]
+        done = []
+        if self._running():
+            self._device_sjd_pass(st, params)
+            p = st["passes"]
+            st["passes"] += 1
+            self.sjd_passes += 1
+            if p > 0:
+                nfin = self._sjd_nfin(st, p - 1)
+                done = [i for i in range(B) if self._slots[i] is not None and st["first_pass"][i] <= p - 1 and nfin[i] >= S]
+                for i in done:
+                    self.sjd_request_passes[self._slots[i].request_id] = p - st["first_pass"][i]
+                self.sjd_tokens += len(done) * (S - 1)
+        self.steps_run += 1
+        return self._finish_c2i(st, done, self._sjd_rows(st, done, p - 1) if done else None)
+
     def _step_t2i(self, st, params: SamplingParams) -> List[RequestOutput]:
         """step() of a t2i LLM: decode the running slots, then admit waiting requests (their prefill draws token 0), then return the
         requests that reached max_tokens."""
@@ -489,12 +626,7 @@ class LLM:
             idx = torch.tensor([i for i, _ in joined], dtype=torch.long, device=dev)
             self._write_guidance(st, idx, [r for _, r in joined])
             for i, r in joined:
-                st["cond"][i].copy_(r.cond)
-                st["mask"][i].copy_(r.mask)
-                st["has_neg"][i] = r.neg is not None
-                if r.neg is not None:
-                    st["neg"][i].copy_(r.neg)
-                st["neg_mask"][i].copy_(r.mask if r.neg_mask is None else r.neg_mask)
+                self._load_caption(st, i, r)
                 if r.prefix is None:
                     self._device_join_t2i(st, params, i)
                 else:
@@ -543,6 +675,8 @@ class LLM:
             self._params = self._waiting[0].params           # a new running set may change the sampling parameters
         params = self._params
         st = self._ensure_state(params)
+        if self.sjd_window is not None:
+            return self._step_sjd(st, params)
         if self.t2i:
             return self._step_t2i(st, params)
         B, R, S, dev = self.max_num_seqs, st["R"], st["S"], st["dev"]
@@ -588,13 +722,15 @@ class LLM:
                     done.append(i)
         return outs + self._finish_c2i(st, done)
 
-    def _finish_c2i(self, st, done: List[int]) -> List[RequestOutput]:
-        """Free the c2i slots in `done` and return their requests' outputs (with their null-class twins')."""
+    def _finish_c2i(self, st, done: List[int], toks: Optional[List[List[int]]] = None) -> List[RequestOutput]:
+        """Free the c2i slots in `done` (or, with sjd_window, any slots) and return their requests' outputs (with their null-class
+        twins'). toks: their token rows, already on the host, or None (copied here)."""
         B, R, dev = self.max_num_seqs, st["R"], st["dev"]
         outs: List[RequestOutput] = []
         if done:
             idx = torch.tensor(done, dtype=torch.long, device=dev)
-            toks = st["out"][idx].cpu().tolist()              # the only device->host copy: token rows of finished requests
+            if toks is None:
+                toks = st["out"][idx].cpu().tolist()          # the only device->host copy: token rows of finished requests
             rows = torch.cat([idx, idx + B]) if R == 2 * B else idx
             st["active"][rows] = 0
             st["pos"][rows] = 0
