@@ -528,6 +528,24 @@ int  lg_test_vq_conv(const void* x, int B, int Hin, int Win, int Cin, const floa
  * gamma / beta f32 [C]. Scratch: at least B * 64 * 64 floats. */
 int  lg_test_group_norm(const void* x, int B, int HW, int C, const float* gamma, const float* beta, int swish, void* y,
                         void* dev_scratch, size_t scratch_bytes, void* stream);
+/* One AttnBlock (vq_model.py:327-351) through the decoder's own run_attn: x bf16 NHWC [B,H,W,C] is read and overwritten with
+ * x + proj_out(softmax(q k^T / sqrt(C)) v). The checkpoint tensors (f32; convs [C,C,1,1], vectors [C]) are packed by the engine's own
+ * weight setup. attn_bc: images per score chunk, 0 = the engine's rule (S of a chunk <= 256 MiB). Optional outputs (NULL or dev):
+ * hn bf16 [B*N,C] (GroupNorm), qk bf16 [B*N,2C] (q | k), vt bf16 [B,C,N] (v transposed), o bf16 [B*N,C] (softmax(.) v of every
+ * image), s f32 and p bf16 [bc,N,N]: scores and probabilities of the last chunk (bc images). N = H*W. Synchronises the stream.
+ * Scratch: 256-byte aligned; the call fails with the size it needs when it is too small. */
+int  lg_test_vq_attn(void* x, int B, int H, int W, int C, const float* norm_w, const float* norm_b, const float* q_w, const float* q_b,
+                     const float* k_w, const float* k_b, const float* v_w, const float* v_b, const float* proj_w, const float* proj_b,
+                     int attn_bc, void* hn, void* qk, void* vt, void* o, float* s, void* p, void* dev_scratch, size_t scratch_bytes,
+                     void* stream);
+/* The first layer of lg_vq_decode: codebook cb f32 [n_e,ed] normalised as lg_vq_finalize does (l2 = 0: copied) into cb_out [n_e,ed]
+ * with squared row norms sq_out [n_e], then rows cb_out[codes[i]] (codes dev int32 [n]) through post_quant_conv (pq_w f32 [Z,ed,1,1],
+ * pq_b [Z]) into out bf16 NHWC [n,Z]. */
+int  lg_test_vq_lookup(const int32_t* codes, int n, const float* cb, int n_e, int ed, int l2, const float* pq_w, const float* pq_b, int Z,
+                       float* cb_out, float* sq_out, void* out, void* stream);
+/* The encoder's first conv as lg_vq_encode runs it: x f32 NCHW [B,3,H,W] (W % 4 == 0), w f32 [ch,3,3,3], bias [ch], ch % 8 == 0
+ * -> out bf16 NHWC [B,H,W,ch], 3x3 pad 1 in fp32. */
+int  lg_test_vq_conv_in_rgb(const float* x, int B, int H, int W, const float* w, const float* bias, int ch, void* out, void* stream);
 
 #ifdef __cplusplus
 }

@@ -165,6 +165,12 @@ SIGNATURES = {
                                 c_void_p, c_size_t, POINTER(c_int), POINTER(c_int), c_void_p]),
     "lg_test_group_norm": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_size_t,
                                    c_void_p]),
+    "lg_test_vq_attn": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                c_void_p, c_void_p, c_size_t, c_void_p]),
+    "lg_test_vq_lookup": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
+                                  c_void_p, c_void_p]),
+    "lg_test_vq_conv_in_rgb": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
 }
 
 _lib = None

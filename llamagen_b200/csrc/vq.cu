@@ -262,10 +262,15 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restri
 
 // argmin-L2 (vq_model.py:215-233): one thread per latent vector, codebook staged through shared memory in
 // tiles; running (min, idx) in registers; d = (|z|^2 + |e|^2) - 2 z.e in fp32 like the reference.
-constexpr int kArgminTile = 2048;
+// Codebook rows per shared-memory tile: 2048 up to ED = 16, 1024 at ED = 32 so that [tile][ED + 1] floats fit the 227 KiB a block
+// can opt into. Every thread scans the rows in ascending order with a strict <, so the tile size does not change any index.
+template <int ED> constexpr int argmin_tile() { return ED <= 16 ? 2048 : 1024; }
+template <int ED> constexpr size_t argmin_smem_bytes() { return (size_t)argmin_tile<ED>() * (ED + 1) * sizeof(float); }
 template <int ED>
 __global__ void __launch_bounds__(128) argmin_kernel(const float* __restrict__ z_nchw, int B, int g, const float* __restrict__ cb,
                                                      const float* __restrict__ cbsq, int n_e, int l2, int64_t* __restrict__ out) {
+    constexpr int kArgminTile = argmin_tile<ED>();
+    static_assert(argmin_smem_bytes<ED>() <= 227 * 1024, "argmin codebook tile exceeds the shared memory of an sm_90 block");
     extern __shared__ float sm[];  // [tile][ED] + [tile]
     float* se = sm;
     float* sq = sm + kArgminTile * ED;
@@ -645,6 +650,9 @@ struct VqWs {
 
 size_t a256(size_t v) { return (v + 255) / 256 * 256; }
 
+// attention scores: chunk Bc images of N tokens so that S (fp32) stays <= 256 MiB
+int attn_chunk_images(int Bc, size_t N) { return (int)std::max<size_t>(1, std::min<size_t>(Bc, (256ull << 20) / (N * N * 4))); }
+
 VqWs carve_vq(const lg_vq* v, char* base, int Bc, int g) {
     const lg_vq_cfg& c = v->cfg;
     size_t maxact = 0;
@@ -658,8 +666,7 @@ VqWs carve_vq(const lg_vq* v, char* base, int Bc, int g) {
     const size_t Cd = (size_t)c.ch * c.ch_mult[c.n_mult - 1];
     const size_t N = (size_t)g * g;
     maxact = std::max(maxact, (size_t)Bc * N * std::max((size_t)c.z_channels, 2 * Cd));
-    // attention scores: chunk images so S (fp32) stays <= 256 MiB
-    int abc = (int)std::max<size_t>(1, std::min<size_t>(Bc, (256ull << 20) / (N * N * 4)));
+    const int abc = attn_chunk_images(Bc, N);
     VqWs w;
     size_t off = 0;
     auto take = [&](size_t b) { char* p = base ? base + off : nullptr; off += a256(b); return p; };
@@ -717,6 +724,32 @@ int run_conv(const ConvCall& c, cudaStream_t st, int* path = nullptr) {
     e.N = c.cout;
     if (c.out_nchw) { e.out_f32 = c.out_nchw; e.nchw = 1; e.hw = Hout * Wout; e.out_bf = nullptr; }
     LG_PROF(PC_VQ_CONV, st, launch_vq_gemm(al, bw, M, c.cout, K, 1, e, st));
+    return 0;
+}
+
+// the codebook as get_codebook_entry reads it (L2-normalised rows when l2) and its squared row norms, from the raw [n, d] table
+int run_normalize_codebook(const float* e, float* out, float* sq, int n, int d, int l2, cudaStream_t st) {
+    normalize_codebook_kernel<<<cdiv(n, 256), 256, 0, st>>>(e, out, sq, n, d, l2);
+    LG_LAUNCH_CHECK();
+    return 0;
+}
+
+// decode_code's first layer: codebook rows of npix codes through post_quant_conv, bf16 NHWC [npix, Z]
+int run_lookup_postquant(const int32_t* codes, int npix, const float* cb, int n_e, int ed, const float* w, const float* bias, int Z,
+                         bf16* out, cudaStream_t st) {
+    lookup_postquant_kernel<<<npix, 256, 0, st>>>(codes, cb, n_e, ed, w, bias, Z, out);
+    LG_LAUNCH_CHECK();
+    return 0;
+}
+
+// Encoder.conv_in over fp32 NCHW x [B,3,H,W] (W % 4 == 0, ch % 8 == 0) into bf16 NHWC; at most 132 * 8 persistent CTAs
+int run_conv_in_rgb(const float* x, const float* w, const float* bias, bf16* out, int B, int H, int W, int ch, cudaStream_t st) {
+    const long long items = (long long)B * H * (W / 4) * (ch / 8);
+    const size_t smem = (size_t)28 * ch * sizeof(float);
+    prof_begin(PC_VQ_CONV, st);
+    conv_in_rgb_kernel<<<(unsigned)std::min<long long>(cdiv(items, 256), 132 * 8), 256, smem, st>>>(x, w, bias, out, B, H, W, ch);
+    prof_end(st);
+    LG_LAUNCH_CHECK();
     return 0;
 }
 
@@ -867,9 +900,7 @@ int lg_vq_finalize(lg_vq* v, void* stream) {
     LG_TRY(get(v, "quantize.embedding.weight", {c.codebook_size, c.codebook_embed_dim}, &e));
     LG_TRY(dev_alloc(v, (size_t)c.codebook_size * c.codebook_embed_dim, &v->codebook));
     LG_TRY(dev_alloc(v, (size_t)c.codebook_size, &v->codebook_sq));
-    normalize_codebook_kernel<<<cdiv(c.codebook_size, 256), 256, 0, st>>>(e, v->codebook, v->codebook_sq, c.codebook_size,
-                                                                           c.codebook_embed_dim, c.l2_norm);
-    LG_LAUNCH_CHECK();
+    LG_TRY(run_normalize_codebook(e, v->codebook, v->codebook_sq, c.codebook_size, c.codebook_embed_dim, c.l2_norm, st));
     LG_TRY(get(v, "post_quant_conv.weight", {c.z_channels, c.codebook_embed_dim, 1, 1}, &v->pq_w));
     LG_TRY(get(v, "post_quant_conv.bias", {c.z_channels}, &v->pq_b));
     LG_TRY(make_conv(v, "decoder.conv_in", block_in, c.z_channels, 3, &v->conv_in, st));
@@ -928,9 +959,8 @@ static int vq_decode_impl(lg_vq* v, const int32_t* codes, int B, int grid, void*
     for (int b0 = 0; b0 < B; b0 += Bc) {
         const int bc = std::min(Bc, B - b0);
         int H = grid, W = grid;
-        lookup_postquant_kernel<<<bc * grid * grid, 256, 0, st>>>(codes + (size_t)b0 * grid * grid, v->codebook, c.codebook_size,
-                                                                  c.codebook_embed_dim, v->pq_w, v->pq_b, c.z_channels, w.T);
-        LG_LAUNCH_CHECK();
+        LG_TRY(run_lookup_postquant(codes + (size_t)b0 * grid * grid, bc * grid * grid, v->codebook, c.codebook_size,
+                                    c.codebook_embed_dim, v->pq_w, v->pq_b, c.z_channels, w.T, st));
         int xs;   // drain-statistics splits of w.X
         LG_TRY(xs = run_conv(w.stats(conv_call(v->conv_in, w.T, bc, H, W, w.X)), st));
         LG_TRY(xs = run_mid(v->dec.mid, w, bc, H, W, xs, st));
@@ -959,11 +989,11 @@ int lg_vq_argmin(lg_vq* v, const float* z_nchw, int B, int grid, int64_t* out_id
     LG_REQUIRE(z_nchw && out_idx && B > 0 && grid > 0, "lg_vq_argmin: bad argument");
     const lg_vq_cfg& c = v->cfg;
     const int nz = B * grid * grid, ed = c.codebook_embed_dim;
-    const size_t smem = (size_t)kArgminTile * (ed + 1) * sizeof(float);
 #define LG_ARGMIN(ED)                                                                                              \
     do {                                                                                                           \
+        constexpr size_t smem = argmin_smem_bytes<ED>();                                                           \
         static DevOnce attr;                                                                                  \
-        if (lg_first_on_device(attr)) { LG_CUDA_OK(cudaFuncSetAttribute(argmin_kernel<ED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)kArgminTile * (ED + 1) * 4))); } \
+        if (lg_first_on_device(attr)) { LG_CUDA_OK(cudaFuncSetAttribute(argmin_kernel<ED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); } \
         argmin_kernel<ED><<<cdiv(nz, 128), 128, smem, st>>>(z_nchw, B, grid, v->codebook, v->codebook_sq, c.codebook_size, c.l2_norm, out_idx); \
     } while (0)
     if (ed == 8) LG_ARGMIN(8);
@@ -993,15 +1023,7 @@ int lg_vq_encode(lg_vq* v, const float* x_nchw, int B, int H, int W, void* dev_w
     for (int b0 = 0; b0 < B; b0 += Bc) {
         const int bc = std::min(Bc, B - b0);
         int h = H, wd = W;
-        {
-            const long long items = (long long)bc * h * (wd / 4) * (c.ch / 8);
-            const size_t smem = (size_t)28 * c.ch * sizeof(float);
-            prof_begin(PC_VQ_CONV, st);
-            conv_in_rgb_kernel<<<(unsigned)std::min<long long>(cdiv(items, 256), 132 * 8), 256, smem, st>>>(x_nchw + (size_t)b0 * 3 * H * W, v->enc_in_w,
-                                                                                v->enc_in_b, w.X, bc, h, wd, c.ch);
-            prof_end(st);
-            LG_LAUNCH_CHECK();
-        }
+        LG_TRY(run_conv_in_rgb(x_nchw + (size_t)b0 * 3 * H * W, v->enc_in_w, v->enc_in_b, w.X, bc, h, wd, c.ch, st));
         int xs = 0;   // drain-statistics splits of w.X: conv_in_rgb_kernel writes none
         for (const LevelW& lv : v->enc.levels) LG_TRY(xs = run_level(lv, 2, w, bc, h, wd, xs, st));
         LG_TRY(xs = run_mid(v->enc.mid, w, bc, h, wd, xs, st));
@@ -1089,6 +1111,70 @@ int lg_test_group_norm(const void* x, int B, int HW, int C, const float* gamma, 
     LG_REQUIRE(scratch_bytes >= need, "lg_test_group_norm: scratch %zu < %zu", scratch_bytes, need);
     const NormW nw{gamma, beta, C};
     return run_gn(nw, (const bf16*)x, 0, (bf16*)y, B, HW, swish, (float*)dev_scratch, (cudaStream_t)stream);
+}
+
+int lg_test_vq_attn(void* x, int B, int H, int W, int C, const float* norm_w, const float* norm_b, const float* q_w, const float* q_b,
+                    const float* k_w, const float* k_b, const float* v_w, const float* v_b, const float* proj_w, const float* proj_b,
+                    int attn_bc, void* hn, void* qk, void* vt, void* o, float* s, void* p, void* dev_scratch, size_t scratch_bytes,
+                    void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    LG_REQUIRE(x && norm_w && norm_b && q_w && q_b && k_w && k_b && v_w && v_b && proj_w && proj_b && dev_scratch && B > 0 && H > 0 &&
+               W > 0 && attn_bc >= 0, "lg_test_vq_attn: bad argument");
+    LG_REQUIRE(((uintptr_t)dev_scratch & 255) == 0, "lg_test_vq_attn: scratch must be 256-byte aligned");
+    // the AttnW packs through make_attn from tensors bound to a throwaway engine, which frees the packed copies on return
+    lg_vq tmp;
+    auto bind = [&](const char* name, const float* ptr, int ndim) {
+        HostTensor h;
+        h.p = ptr; h.ndim = ndim; h.shape[0] = C;
+        if (ndim == 4) { h.shape[1] = C; h.shape[2] = 1; h.shape[3] = 1; }
+        tmp.t[name] = h;
+    };
+    bind("attn.norm.weight", norm_w, 1); bind("attn.norm.bias", norm_b, 1);
+    bind("attn.q.weight", q_w, 4); bind("attn.q.bias", q_b, 1);
+    bind("attn.k.weight", k_w, 4); bind("attn.k.bias", k_b, 1);
+    bind("attn.v.weight", v_w, 4); bind("attn.v.bias", v_b, 1);
+    bind("attn.proj_out.weight", proj_w, 4); bind("attn.proj_out.bias", proj_b, 1);
+    AttnW a;
+    LG_TRY(make_attn(&tmp, "attn", C, &a, st));
+    const size_t N = (size_t)H * W;
+    VqWs w{};
+    w.attn_bc = attn_bc > 0 ? std::min(attn_bc, B) : attn_chunk_images(B, N);
+    w.gn_floats = gn_partial_capacity(B, H, W);
+    size_t off = 0;
+    auto take = [&](size_t b) { char* q = (char*)dev_scratch + off; off += a256(b); return q; };
+    w.X = (bf16*)x;
+    w.T = (bf16*)take((size_t)B * N * C * 2);
+    w.U = (bf16*)take((size_t)B * N * 2 * C * 2);
+    w.VT = (bf16*)take((size_t)B * C * N * 2);
+    w.S = (float*)take((size_t)w.attn_bc * N * N * 4);
+    w.P = (bf16*)take((size_t)w.attn_bc * N * N * 2);
+    w.gn = (float*)take(w.gn_floats * 4);
+    LG_REQUIRE(scratch_bytes >= off, "lg_test_vq_attn: scratch %zu < %zu", scratch_bytes, off);
+    if (hn) LG_TRY(run_gn(a.norm, w.X, 0, (bf16*)hn, B, (int)N, 0, w.gn, st));   // the same statistics + apply run_attn starts with
+    LG_TRY(run_attn(a, w, B, H, W, 0, st));
+    const size_t bc_last = (size_t)B - (size_t)(B - 1) / w.attn_bc * w.attn_bc;
+    if (qk) LG_CUDA_OK(cudaMemcpyAsync(qk, w.U, (size_t)B * N * 2 * C * 2, cudaMemcpyDeviceToDevice, st));
+    if (vt) LG_CUDA_OK(cudaMemcpyAsync(vt, w.VT, (size_t)B * C * N * 2, cudaMemcpyDeviceToDevice, st));
+    if (o) LG_CUDA_OK(cudaMemcpyAsync(o, w.T, (size_t)B * N * C * 2, cudaMemcpyDeviceToDevice, st));
+    if (s) LG_CUDA_OK(cudaMemcpyAsync(s, w.S, bc_last * N * N * 4, cudaMemcpyDeviceToDevice, st));
+    if (p) LG_CUDA_OK(cudaMemcpyAsync(p, w.P, bc_last * N * N * 2, cudaMemcpyDeviceToDevice, st));
+    LG_CUDA_OK(cudaStreamSynchronize(st));
+    return 0;
+}
+
+int lg_test_vq_lookup(const int32_t* codes, int n, const float* cb, int n_e, int ed, int l2, const float* pq_w, const float* pq_b, int Z,
+                      float* cb_out, float* sq_out, void* out, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    LG_REQUIRE(codes && cb && pq_w && pq_b && cb_out && sq_out && out && n > 0 && n_e > 0 && ed > 0 && Z > 0,
+               "lg_test_vq_lookup: bad argument");
+    LG_TRY(run_normalize_codebook(cb, cb_out, sq_out, n_e, ed, l2, st));
+    return run_lookup_postquant(codes, n, cb_out, n_e, ed, pq_w, pq_b, Z, (bf16*)out, st);
+}
+
+int lg_test_vq_conv_in_rgb(const float* x, int B, int H, int W, const float* w, const float* bias, int ch, void* out, void* stream) {
+    LG_REQUIRE(x && w && bias && out && B > 0 && H > 0 && W > 0 && W % 4 == 0 && ch > 0 && ch % 8 == 0,
+               "lg_test_vq_conv_in_rgb: bad argument (W %% 4 == 0 and ch %% 8 == 0 required)");
+    return run_conv_in_rgb(x, w, bias, (bf16*)out, B, H, W, ch, (cudaStream_t)stream);
 }
 
 }  // extern "C"
