@@ -205,6 +205,20 @@ int  lg_sample_rows(const float* logits, int B, int V, int mix_cfg, int round_dt
 int  lg_sample_rows_guided(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc,
                            const uint64_t* seed_rows, const int32_t* step_rows, const float* cfg_rows, const int32_t* interval_rows,
                            int32_t* out_idx, int32_t* out_seq, int seq_stride, void* stream);
+/* lg_sample_rows_guided with per-row image indices (parallel sampling: several images of one request). img_rows dev int32 [B], values
+ * >= 0, or NULL: image b draws what image img_rows[b] of a lg_generate call with seed seed_rows[b] draws at token index step_rows[b]
+ * (lg_sample of that image at that step), where NULL keys every row as image 0 (a batch-of-one call). lg_sample_rows_guided is this
+ * call with img_rows NULL. */
+int  lg_sample_rows_keyed(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc,
+                          const uint64_t* seed_rows, const int32_t* step_rows, const float* cfg_rows, const int32_t* interval_rows,
+                          const int32_t* img_rows, int32_t* out_idx, int32_t* out_seq, int seq_stride, void* stream);
+/* KV fan-out of a parallel-sampling join: copies positions [0, len) of every layer's K and V from the rows of slot src_slot (row
+ * src_slot and, with use_cfg, row B + src_slot) to the same rows of every slot in dst_slots (host int32 [n_dst]), on `stream`, in
+ * whatever the cache stores (the model dtype or e4m3 codes; an fp8 cache's scales are per layer and shared by every row, so they need
+ * no copy). Nothing else of the workspace changes. lg_prefill_slot* write the same bytes whatever the slot, so a destination holds
+ * what a prefill of it would have written. Refused before any launch: a slot outside [0, B), a destination equal to the source or
+ * repeated, len outside [0, max_seq], and a workspace with fewer than nh * B rows. One launch per 64 destinations. */
+int  lg_copy_slot_kv(lg_engine* e, int src_slot, const int32_t* dst_slots, int n_dst, int B, int use_cfg, int len, void* stream);
 /* Fused CFG-mix + temperature + top-k + top-p + softmax + (argmax | multinomial): generate.py:57-66,95-97.
  * logits f32 [rows, V] (rows = 2B when mix_cfg, cond rows first); writes out_idx int32 [B] and, when
  * non-NULL, out_probs f32 [B, V] (the post-filter softmax the reference returns as `probs`).
@@ -279,8 +293,9 @@ int  lg_generate_sjd(lg_engine* e, const void* cond, const float* emb_mask, int 
                      void* dev_ws, size_t ws_bytes, int32_t* out_tokens, int32_t* iters_out, float* dbg_probs, void* stream);
 
 /* ---- SJD over serving slots (serve.LLM(sjd_window=L)): the state of lg_generate_sjd per slot instead of per call ------------------
- * Slot b (KV-cache rows b and, with use_cfg, B + b) is one request with its own seed and pass counter, keyed as image 0 of
- * lg_generate_sjd with that seed: u_purpose(k) and pass_seed(0, pass) with the slot's seed, pass counting the passes since the slot's
+ * Slot b (KV-cache rows b and, with use_cfg, B + b) is one image of a request with its own seed, image index j (0 unless its start
+ * says otherwise) and pass counter, keyed as image j of lg_generate_sjd with that seed: u_purpose(k) and pass_seed(j, pass) with the
+ * slot's seed, pass counting the passes since the slot's
  * start (0 at the start). A slot with nfin >= S is frozen: a pass writes nothing of it (out row, window, q, counters); its rows keep
  * running. The state lives in dev_ws (lg_sjd_slots_workspace_bytes, 256-byte aligned); the KV cache is the workspace's
  * (rows >= (use_cfg ? 2 : 1) * B, max_seq >= T + S). Every argument is checked before any launch. */
@@ -291,6 +306,10 @@ int  lg_sjd_slots_reset(lg_engine* e, int B, int use_cfg, int L, void* dev_ws, s
  * counter 0, window [token 0, u_init drafts of `seed`], and its L window rows' guidance (cfg_scale, cfg_interval; read with use_cfg). */
 int  lg_sjd_slot_start(lg_engine* e, int slot, int B, int use_cfg, int L, int S, uint64_t seed, float cfg_scale, int cfg_interval,
                        const int32_t* out_tokens, void* dev_ws, size_t ws_bytes, void* stream);
+/* lg_sjd_slot_start keyed as image `image` (>= 0) of the call: the slot draws what image `image` of lg_generate_sjd with `seed`
+ * draws. lg_sjd_slot_start is this call with image 0. */
+int  lg_sjd_slot_start_image(lg_engine* e, int slot, int B, int use_cfg, int L, int S, uint64_t seed, float cfg_scale, int cfg_interval,
+                             int image, const int32_t* out_tokens, void* dev_ws, size_t ws_bytes, void* stream);
 /* One pass over every slot: the window rows (nh * B * L, at the slots' positions; emb_mask [B, T] and neg_mask [B, T] as in
  * lg_decode_rows_t2i_neg) through the layers and the head, p and x of every row with its slot's seed, token index and guidance (sc: the
  * rest of the sampling configuration), acceptance and the next window, as one pass of lg_generate_sjd. nfin_out: host-pinned or dev

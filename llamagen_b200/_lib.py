@@ -89,6 +89,9 @@ SIGNATURES = {
                                c_void_p]),
     "lg_sample_rows_guided": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p, c_void_p, c_void_p, c_void_p,
                                       c_void_p, c_void_p, c_int, c_void_p]),
+    "lg_sample_rows_keyed": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p, c_void_p, c_void_p, c_void_p,
+                                     c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
+    "lg_copy_slot_kv": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "lg_sample": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(SampleCfg), c_uint64, c_void_p,
                           c_void_p, c_void_p]),
     "lg_generate": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p,
@@ -107,6 +110,8 @@ SIGNATURES = {
     "lg_sjd_slots_reset": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "lg_sjd_slot_start": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_uint64, c_float, c_int, c_void_p, c_void_p, c_size_t,
                                   c_void_p]),
+    "lg_sjd_slot_start_image": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_uint64, c_float, c_int, c_int, c_void_p, c_void_p,
+                                        c_size_t, c_void_p]),
     "lg_sjd_pass_slots": (c_int, [c_void_p, POINTER(SampleCfg), c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_size_t,
                                   c_void_p, c_void_p, c_void_p, c_void_p]),
     "lg_test_sjd_verify": (c_int,[c_int, c_int, c_int, c_int, c_int, c_uint64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,

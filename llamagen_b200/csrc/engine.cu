@@ -483,7 +483,7 @@ size_t lg_engine::carve_sjd(RowBuffers& o, SjdArgs& sa, char* base, int B, int n
 }
 
 // Serving's SJD state for B slots (lg_sjd_slots_workspace_bytes), from `base` (null: sizes only): carve_sjd's scratch, then every slot's
-// seed and pass counter and the guidance of every window row
+// seed, pass counter and image index and the guidance of every window row
 size_t lg_engine::carve_sjd_slots(RowBuffers& o, SjdArgs& sa, char* base, int B, int nh, int L) const {
     Carver c{base, 0, 1, carve_sjd(o, sa, base, B, nh, L)};
     const size_t BL = (size_t)B * L;
@@ -491,6 +491,7 @@ size_t lg_engine::carve_sjd_slots(RowBuffers& o, SjdArgs& sa, char* base, int B,
     sa.pass_slots = (int32_t*)c.split(B * sizeof(int32_t));
     sa.cfg_rows = (float*)c.split(BL * sizeof(float));
     sa.interval_rows = (int32_t*)c.split(BL * sizeof(int32_t));
+    sa.img_slots = (int32_t*)c.split(B * sizeof(int32_t));
     return c.off;
 }
 
@@ -1026,15 +1027,16 @@ int lg_score(lg_engine* e, const void* cond, const float* emb_mask, const int32_
 
 }  // extern "C"
 
-// lg_sample_rows (cfg_rows = interval_rows = null) and lg_sample_rows_guided; fn names the entry point in messages
+// lg_sample_rows (cfg_rows = interval_rows = img_rows = null), lg_sample_rows_guided (img_rows = null) and lg_sample_rows_keyed; fn
+// names the entry point in messages
 static int sample_rows_impl(const char* fn, const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc,
                             const uint64_t* seed_rows, const int32_t* step_rows, const float* cfg_rows, const int32_t* interval_rows,
-                            int32_t* out_idx, int32_t* out_seq, int seq_stride, void* stream) {
+                            const int32_t* img_rows, int32_t* out_idx, int32_t* out_seq, int seq_stride, void* stream) {
     LG_REQUIRE(logits && sc && seed_rows && step_rows && (out_idx || out_seq), "%s: null argument", fn);
     LG_REQUIRE(mix_cfg || (!cfg_rows && !interval_rows), "%s: per-row cfg_rows / interval_rows need mix_cfg (2B logits rows)", fn);
     SampleArgs a = make_sample_args(*sc, logits, B, V, mix_cfg, round_dtype);
     a.seed_rows = seed_rows; a.step_rows = step_rows;
-    a.cfg_rows = cfg_rows; a.interval_rows = interval_rows;
+    a.cfg_rows = cfg_rows; a.interval_rows = interval_rows; a.img_rows = img_rows;
     a.out_idx = out_idx; a.out_seq = out_seq; a.seq_stride = seq_stride;
     return launch_sample(a, (cudaStream_t)stream);
 }
@@ -1043,15 +1045,22 @@ extern "C" {
 
 int lg_sample_rows(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc, const uint64_t* seed_rows,
                    const int32_t* step_rows, int32_t* out_idx, int32_t* out_seq, int seq_stride, void* stream) {
-    return sample_rows_impl("lg_sample_rows", logits, B, V, mix_cfg, round_dtype, sc, seed_rows, step_rows, nullptr, nullptr, out_idx,
-                            out_seq, seq_stride, stream);
+    return sample_rows_impl("lg_sample_rows", logits, B, V, mix_cfg, round_dtype, sc, seed_rows, step_rows, nullptr, nullptr, nullptr,
+                            out_idx, out_seq, seq_stride, stream);
 }
 
 int lg_sample_rows_guided(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc,
                           const uint64_t* seed_rows, const int32_t* step_rows, const float* cfg_rows, const int32_t* interval_rows,
                           int32_t* out_idx, int32_t* out_seq, int seq_stride, void* stream) {
     return sample_rows_impl("lg_sample_rows_guided", logits, B, V, mix_cfg, round_dtype, sc, seed_rows, step_rows, cfg_rows,
-                            interval_rows, out_idx, out_seq, seq_stride, stream);
+                            interval_rows, nullptr, out_idx, out_seq, seq_stride, stream);
+}
+
+int lg_sample_rows_keyed(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc,
+                         const uint64_t* seed_rows, const int32_t* step_rows, const float* cfg_rows, const int32_t* interval_rows,
+                         const int32_t* img_rows, int32_t* out_idx, int32_t* out_seq, int seq_stride, void* stream) {
+    return sample_rows_impl("lg_sample_rows_keyed", logits, B, V, mix_cfg, round_dtype, sc, seed_rows, step_rows, cfg_rows,
+                            interval_rows, img_rows, out_idx, out_seq, seq_stride, stream);
 }
 
 int lg_sample(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc, uint64_t step,
@@ -1587,11 +1596,14 @@ int lg_sjd_slots_reset(lg_engine* e, int B, int use_cfg, int L, void* dev_ws, si
     return 0;
 }
 
-int lg_sjd_slot_start(lg_engine* e, int slot, int B, int use_cfg, int L, int S, uint64_t seed, float cfg_scale, int cfg_interval,
-                      const int32_t* out_tokens, void* dev_ws, size_t ws_bytes, void* stream) {
-    static const char* fn = "lg_sjd_slot_start";
+}  // extern "C"
+
+// lg_sjd_slot_start (image 0) and lg_sjd_slot_start_image; fn names the entry point in messages
+static int sjd_slot_start_impl(const char* fn, lg_engine* e, int slot, int B, int use_cfg, int L, int S, uint64_t seed, float cfg_scale,
+                               int cfg_interval, int image, const int32_t* out_tokens, void* dev_ws, size_t ws_bytes, void* stream) {
     LG_REQUIRE(out_tokens, "%s: null out_tokens", fn);
     LG_REQUIRE(slot >= 0 && slot < B, "%s: slot %d outside [0, B=%d)", fn, slot, B);
+    LG_REQUIRE(image >= 0 && image < 0x7fffffff, "%s: image %d outside [0, 2^31 - 1)", fn, image);
     LG_REQUIRE(S > 0, "%s: S=%d", fn, S);
     LG_REQUIRE(std::isfinite(cfg_scale) && cfg_interval >= -1, "%s: cfg_scale %g must be finite and cfg_interval %d >= -1", fn,
                (double)cfg_scale, cfg_interval);
@@ -1599,10 +1611,61 @@ int lg_sjd_slot_start(lg_engine* e, int slot, int B, int use_cfg, int L, int S, 
     SjdArgs sa{};
     LG_TRY(sjd_slots_view(fn, e, B, use_cfg, L, S, dev_ws, ws_bytes, w, sa));
     DeviceGuard guard(e->device);
-    sa.seed = seed; sa.start_cfg = cfg_scale; sa.start_interval = cfg_interval;
+    sa.seed = seed; sa.start_cfg = cfg_scale; sa.start_interval = cfg_interval; sa.start_img = image;
     sa.out = const_cast<int32_t*>(out_tokens);   // read only: token 0 of the slot's row
     return launch_sjd_refresh(sa, 1, (cudaStream_t)stream, slot);
 }
+
+extern "C" {
+
+int lg_sjd_slot_start(lg_engine* e, int slot, int B, int use_cfg, int L, int S, uint64_t seed, float cfg_scale, int cfg_interval,
+                      const int32_t* out_tokens, void* dev_ws, size_t ws_bytes, void* stream) {
+    return sjd_slot_start_impl("lg_sjd_slot_start", e, slot, B, use_cfg, L, S, seed, cfg_scale, cfg_interval, 0, out_tokens, dev_ws,
+                               ws_bytes, stream);
+}
+
+int lg_sjd_slot_start_image(lg_engine* e, int slot, int B, int use_cfg, int L, int S, uint64_t seed, float cfg_scale, int cfg_interval,
+                            int image, const int32_t* out_tokens, void* dev_ws, size_t ws_bytes, void* stream) {
+    return sjd_slot_start_impl("lg_sjd_slot_start_image", e, slot, B, use_cfg, L, S, seed, cfg_scale, cfg_interval, image, out_tokens,
+                               dev_ws, ws_bytes, stream);
+}
+
+int lg_copy_slot_kv(lg_engine* e, int src_slot, const int32_t* dst_slots, int n_dst, int B, int use_cfg, int len, void* stream) {
+    static const char* fn = "lg_copy_slot_kv";
+    LG_REQUIRE(n_dst >= 0 && (n_dst == 0 || dst_slots), "%s: n_dst=%d with %s dst_slots", fn, n_dst, dst_slots ? "non-null" : "null");
+    LG_REQUIRE(B > 0 && src_slot >= 0 && src_slot < B, "%s: source slot %d outside [0, B=%d)", fn, src_slot, B);
+    for (int i = 0; i < n_dst; ++i) {
+        const int d = dst_slots[i];
+        LG_REQUIRE(d >= 0 && d < B, "%s: destination slot %d outside [0, B=%d)", fn, d, B);
+        LG_REQUIRE(d != src_slot, "%s: destination slot %d is the source", fn, d);
+        for (int j = 0; j < i; ++j) LG_REQUIRE(dst_slots[j] != d, "%s: destination slot %d repeated", fn, d);
+    }
+    LG_REQUIRE(len >= 0, "%s: len %d < 0", fn, len);
+    LG_REQUIRE(e && e->finalized, "%s: engine not finalized", fn);
+    LG_REQUIRE(e->full.base, "%s: workspace not set", fn);
+    const int nh = use_cfg ? 2 : 1;
+    LG_REQUIRE(nh * B <= e->full.rows, "%s: %d rows (nh=%d, B=%d) exceed the workspace's %d", fn, nh * B, nh, B, e->full.rows);
+    LG_REQUIRE(len <= e->full.max_seq, "%s: len %d exceeds the workspace's max_seq %d", fn, len, e->full.max_seq);
+    cudaStream_t st = (cudaStream_t)stream;
+    DeviceGuard guard(e->device);
+    LG_TRY(e->zero_fill_if_needed(st));
+    // fp8 scales are per layer, shared by every row: the codes alone are copied
+    KvCopyArgs a{};
+    a.kcache = e->full.kcache; a.vcache = e->full.vcache;
+    a.layers = e->full.layers; a.rows = e->full.rows; a.H = e->cfg.n_head; a.max_seq = e->full.max_seq;
+    a.row_bytes = e->hdp * (e->full.kv_f8 ? 1 : (int)e->esz);
+    a.B = B; a.nh = nh; a.len = len; a.src = src_slot;
+    for (int d0 = 0; d0 < n_dst; d0 += kKvCopyMaxDst) {
+        a.n_dst = std::min(kKvCopyMaxDst, n_dst - d0);
+        for (int i = 0; i < a.n_dst; ++i) a.dst[i] = dst_slots[d0 + i];
+        LG_TRY(launch_copy_slot_kv(a, st));
+    }
+    return 0;
+}
+
+}  // extern "C"
+
+extern "C" {
 
 int lg_sjd_pass_slots(lg_engine* e, const lg_sample_cfg* sc, const float* emb_mask, const float* neg_mask, int B, int use_cfg, int S, int L,
                       void* dev_ws, size_t ws_bytes, int32_t* out_tokens, int32_t* nfin_out, float* dbg_p, void* stream) {

@@ -37,6 +37,9 @@ struct SampleArgs {
     // cfg_scale / cfg_interval, and mixes only when its scale is > 1 (generate.py's `if cfg_scale > 1.0`)
     const float* cfg_rows = nullptr;       // [B] or null
     const int32_t* interval_rows = nullptr;// [B] or null
+    // parallel sampling (lg_sample_rows_keyed; needs seed_rows): image b keys its draw as image img_rows[b] of a call with seed
+    // seed_rows[b], where null keys every row as image 0
+    const int32_t* img_rows = nullptr;     // [B] or null
     // fused tail of a decode iteration (16-bit models; rows in round_dtype): the CTA that picked image b's token also writes the next step's input rows b and
     // B + b (token embedding, gpt.py:352; optionally its RMSNorm for layer 0, gpt.py:143-148) and the last CTA to finish advances the
     // device-resident position / step counters - three dependent kernels (embed, rmsnorm, advance) fewer per token
@@ -83,10 +86,13 @@ struct SjdArgs {
     int32_t* state;              // [kSjdStateInts], zero-initialised
     float* dbg;                  // [passes][B][L][V] copy of every pass's p rows, or null
     int done_token;              // written to state[kSjdDone] once every image has S tokens (unique per call)
-    // Per-slot mode (serving, lg_sjd_pass_slots): every image b is a slot with its own seed and pass counter, keyed as image 0 of a
-    // call with that seed (seed and row_offset unused). A slot with nfin >= S is frozen: verify and refresh write nothing of it.
+    // Per-slot mode (serving, lg_sjd_pass_slots): every image b is a slot with its own seed and pass counter, keyed as image
+    // img_slots[b] (0 when img_slots is null) of a call with that seed (seed and row_offset unused). A slot with nfin >= S is frozen:
+    // verify and refresh write nothing of it.
     uint64_t* seed_slots = nullptr;   // [B] or null (per-call mode)
     int32_t* pass_slots = nullptr;    // [B] passes the slot has run since its start; verify advances it, refresh keys with it
+    int32_t* img_slots = nullptr;     // [B] or null: the image index every slot keys as, written by its start (start_img)
+    int start_img = 0;
     float* cfg_rows = nullptr;        // [B * L] per-row guidance of the window rows (a start writes its slot's L rows), or null
     int32_t* interval_rows = nullptr; // [B * L]
     float start_cfg = 1.f;            // a start's (first = 1, one slot) seed is `seed`; its guidance scale and cfg_interval
@@ -184,6 +190,17 @@ int launch_store_act(const float* partial, int ksplit, int M, int N, void* out, 
 int launch_reduce_f32(const float* partial, int ksplit, int M, int N, float* out, cudaStream_t st);
 // gather last-position rows: out[r,:] = in[(r*T + T-1),:]
 int launch_gather_last(const void* in, int R, int T, int D, int dtype, void* out, cudaStream_t st);
+// KV fan-out of serving (lg_copy_slot_kv): in a cache laid out [layers][rows, H, max_seq, row_bytes] (K at kcache, V at vcache),
+// positions [0, len) of row half * B + src (half < nh) are copied to row half * B + dst[d] for every destination d, in every layer, K
+// and V. One launch for up to kKvCopyMaxDst destinations, 16-byte copies when every segment allows them.
+constexpr int kKvCopyMaxDst = 64;
+struct KvCopyArgs {
+    char *kcache, *vcache;
+    int layers, rows, H, max_seq, row_bytes;   // row_bytes: bytes per position of one head (hdp elements of the stored type)
+    int B, nh, len, src, n_dst;
+    int dst[kKvCopyMaxDst];
+};
+int launch_copy_slot_kv(const KvCopyArgs& a, cudaStream_t st);
 
 // lg_score: h[r, t] = t < T ? cond_rows[r * T + t] : table[idx[r % B][t - T]] over R * seq rows (idx [B][seq - T])
 int launch_embed_seq(const void* cond_rows, const void* table, const int32_t* idx, int B, int R, int T, int seq, int D, int dtype, void* out,

@@ -396,9 +396,10 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
         __syncthreads();
         const float total = red[32];
         const float excl = s_wtot[warp] + (incl - local);
-        // per-request streams (seed_rows): every image draws exactly what a batch-of-one generate() with its seed would draw
+        // per-request streams (seed_rows): every image draws exactly what a batch-of-one generate() with its seed would draw, or, with
+        // img_rows, what image img_rows[b] of a generate() with its seed draws
         const uint64_t seed = a.seed_rows ? a.seed_rows[b] : a.seed;
-        const uint64_t rrow = a.seed_rows ? 1ull : (uint64_t)(b + 1 + a.row_offset);
+        const uint64_t rrow = a.seed_rows ? (a.img_rows ? (uint64_t)a.img_rows[b] + 1 : 1ull) : (uint64_t)(b + 1 + a.row_offset);
         const uint64_t r = splitmix64(splitmix64(seed ^ (0xA0761D6478BD642Full * (step + 1))) ^ (0xE7037ED1A0B428DBull * rrow));
         const float u = (float)(r >> 40) * (1.0f / 16777216.0f);
         const float target = u * total;
@@ -548,8 +549,8 @@ __global__ void __launch_bounds__(kSjdThreads) sjd_verify_kernel(SjdArgs a) {
     const int L = a.L, V = a.V, S = a.S;
     const int n = a.nfin[b], s = a.start[b];
     const bool active = n < S;
-    const uint64_t seed = a.seed_slots ? a.seed_slots[b] : a.seed;   // per-slot mode: the slot's seed, image 0
-    const int img = a.seed_slots ? 0 : b + a.row_offset;
+    const uint64_t seed = a.seed_slots ? a.seed_slots[b] : a.seed;   // per-slot mode: the slot's seed and image index
+    const int img = a.seed_slots ? (a.img_slots ? a.img_slots[b] : 0) : b + a.row_offset;
     if (active) {
         const size_t row0 = (size_t)b * L;
         if (tid == 0) {
@@ -648,7 +649,7 @@ __global__ void __launch_bounds__(kSjdThreads) sjd_verify_kernel(SjdArgs a) {
 }
 
 // grid (B, L), or (1, L) for image `slot` >= 0: slot i of image b's next window. first = 1 sets up the window after the prefill (token
-// 0 final, all drafts new); in per-slot mode it also sets the slot's seed, pass counter and window rows' guidance.
+// 0 final, all drafts new); in per-slot mode it also sets the slot's seed, pass counter, image index and window rows' guidance.
 __global__ void __launch_bounds__(256) sjd_refresh_kernel(SjdArgs a, int first, int only) {
     lg_pdl_sync();
     const int b = only >= 0 ? only : blockIdx.x, i = blockIdx.y, L = a.L, V = a.V, S = a.S;
@@ -657,7 +658,7 @@ __global__ void __launch_bounds__(256) sjd_refresh_kernel(SjdArgs a, int first, 
     // index of the next pass: the call's, or the slot's own (0 at its start)
     const int pass = a.pass_slots ? (first ? 0 : a.pass_slots[b]) : a.state[kSjdIters];
     const uint64_t seed = a.seed_slots && !first ? a.seed_slots[b] : a.seed;
-    const int img = a.seed_slots ? 0 : b + a.row_offset;
+    const int img = !a.seed_slots ? b + a.row_offset : first ? a.start_img : a.img_slots ? a.img_slots[b] : 0;
     if (!first && a.dbg) {
         float* d = a.dbg + ((size_t)(pass - 1) * a.B * L + slot) * V;
         for (int v = threadIdx.x; v < V; v += blockDim.x) d[v] = a.p[slot * V + v];
@@ -669,6 +670,7 @@ __global__ void __launch_bounds__(256) sjd_refresh_kernel(SjdArgs a, int first, 
             a.nfin[b] = 1; a.start[b] = 1;
             for (int hh = 0; hh < a.nh; ++hh) a.pos_rows[hh * a.B + b] = a.T;
             if (a.seed_slots) { a.seed_slots[b] = a.seed; a.pass_slots[b] = 0; }
+            if (a.img_slots) a.img_slots[b] = a.start_img;
         }
         if (a.cfg_rows && threadIdx.x == 0) { a.cfg_rows[slot] = a.start_cfg; a.interval_rows[slot] = a.start_interval; }
     } else {

@@ -444,6 +444,28 @@ __global__ void set_counters_kernel(int* pos, int pv, int* step, int sv) {
     if (step) *step = sv;
 }
 
+// One CTA column per (layer, K | V, half, head) segment: positions [0, len) of the source row, read once in W-wide words and written
+// to every destination row; blockIdx.y strides over the segment
+template <typename W>
+__global__ void __launch_bounds__(256) copy_slot_kv_kernel(KvCopyArgs a) {
+    lg_pdl_sync();
+    int seg = blockIdx.x;
+    const int head = seg % a.H;
+    seg /= a.H;
+    const int half = seg % a.nh;
+    seg /= a.nh;
+    char* base = (seg & 1) ? a.vcache : a.kcache;
+    const int layer = seg >> 1;
+    const size_t seg_bytes = (size_t)a.max_seq * a.row_bytes, n = (size_t)a.len * a.row_bytes / sizeof(W);
+    const size_t row0 = (size_t)layer * a.rows + (size_t)half * a.B;
+    const W* src = reinterpret_cast<const W*>(base + ((row0 + a.src) * a.H + head) * seg_bytes);
+    for (size_t i = (size_t)blockIdx.y * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.y * blockDim.x) {
+        const W v = src[i];
+        for (int d = 0; d < a.n_dst; ++d)
+            reinterpret_cast<W*>(base + ((row0 + a.dst[d]) * a.H + head) * seg_bytes)[i] = v;
+    }
+}
+
 // f is called with a value of the element type: f(T{}) for T = float, bf16 or f16
 template <typename F>
 int dispatch_dtype(int dtype, F f) {
@@ -670,6 +692,24 @@ int launch_advance(int* pos, int* step, cudaStream_t st) {
 }
 int launch_set_counters(int* pos, int pos_v, int* step, int step_v, cudaStream_t st) {
     (void)lg_launch(set_counters_kernel, dim3(1), dim3(1), 0, st, pos, pos_v, step, step_v);
+    LG_LAUNCH_CHECK();
+    return 0;
+}
+
+int launch_copy_slot_kv(const KvCopyArgs& a, cudaStream_t st) {
+    LG_REQUIRE(a.n_dst >= 0 && a.n_dst <= kKvCopyMaxDst && a.len >= 0 && a.len <= a.max_seq && a.row_bytes > 0,
+               "copy_slot_kv: bad shape (n_dst=%d len=%d max_seq=%d)", a.n_dst, a.len, a.max_seq);
+    if (a.n_dst == 0 || a.len == 0) return 0;
+    const size_t segs = (size_t)a.layers * 2 * a.nh * a.H, words16 = (size_t)a.len * a.row_bytes / 16;
+    LG_REQUIRE(segs <= 0x7fffffffu, "copy_slot_kv: %zu segments", segs);
+    // 16-byte words when every segment's start and length allow them (hdp-wide rows are 16-byte multiples in every cache the engine
+    // stores), else 4-byte or single-byte words
+    const size_t seg_bytes = (size_t)a.max_seq * a.row_bytes, len_bytes = (size_t)a.len * a.row_bytes;
+    const uintptr_t al = (uintptr_t)a.kcache | (uintptr_t)a.vcache | seg_bytes | len_bytes;
+    const dim3 block(256), grid((unsigned)segs, (unsigned)std::max<size_t>(1, std::min<size_t>(8, words16 / (4 * 256))));
+    if ((al & 15) == 0) (void)lg_launch(copy_slot_kv_kernel<uint4>, grid, block, 0, st, a);
+    else if ((al & 3) == 0) (void)lg_launch(copy_slot_kv_kernel<uint32_t>, grid, block, 0, st, a);
+    else (void)lg_launch(copy_slot_kv_kernel<uint8_t>, grid, block, 0, st, a);
     LG_LAUNCH_CHECK();
     return 0;
 }

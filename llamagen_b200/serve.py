@@ -60,6 +60,16 @@ what generate(cond_r, sjd_window=L, seed=s_r) draws for image 0, whatever ran be
 previous pass's final counts (a pinned copy and an event): a finished request leaves, and its slot is reused, one step after its last
 pass; its slot is frozen meanwhile. prefix= requests are refused (as generate() refuses prefix with sjd_window).
 
+Parallel sampling (SamplingParams(n=k), 1 <= k <= max_num_seqs; vLLM's `n`): a request takes k sequence slots (max_num_seqs counts
+sequences) and returns one RequestOutput whose outputs are k CompletionOutputs, index 0 .. k - 1. Sample j draws what image j of
+generate(cond repeated k times, seed=s) draws (s: the request's seed), with the same guidance, prefix, negative and sjd_window; n = 1 is
+image 0, as before. The request joins when k slots are free, all at once, in FIFO order (a later request does not overtake it). A join
+that prefills (t2i, a prefix, every SJD join) prefills once, into the first slot; lg_copy_slot_kv then copies positions [0, T + P) of
+its K / V rows to the other k - 1 slots (a prefill writes the same bytes whatever the slot), their host-side state is copied too, and the
+join's logits are drawn once per slot with the slot's image index (lg_sample_rows_keyed). A plain c2i join has no prefill: its k slots
+start at position 0 with the same class. Samples finish independently (under SJD at different passes); a finished sample frees its slot
+at once, and the request is returned when its last sample finishes. Null-class twins mirror the request's k outputs.
+
 While requests are in flight the LLM owns the model's KV-cache workspace (a `generate()` call on the same model would reset it)."""
 from __future__ import annotations
 
@@ -86,7 +96,9 @@ class SamplingParams:
     Per-request guidance and seed (requests that differ only in these share the running batch):
     cfg_scale: None = the LLM's cfg_scale; a finite number, > 1 only on an LLM built with cfg_scale > 1 (it has the unconditional rows).
     cfg_interval: None = -1; an integer >= -1, generate()'s cfg_interval (the mix is dropped after decode iteration cfg_interval).
-    seed: None = the LLM's seed + request id; an integer in [0, 2**63), the key generate(seed=...) draws image 0 with."""
+    seed: None = the LLM's seed + request id; an integer in [0, 2**63), the key generate(seed=...) draws image 0 with.
+    n: the number of images of the request, an integer in [1, max_num_seqs]; image j is what image j of generate(cond repeated n times,
+    seed=seed) draws. Requests that differ in n share the running batch."""
     temperature: float = 1.0
     top_p: float = 1.0
     top_k: int = -1
@@ -94,6 +106,7 @@ class SamplingParams:
     cfg_scale: Optional[float] = None
     cfg_interval: Optional[int] = None
     seed: Optional[int] = None
+    n: int = 1
 
 
 def _batch_key(p: SamplingParams):
@@ -134,6 +147,8 @@ class _Request:
     cfg: float = 1.0                       # the request's guidance scale, cfg_interval and RNG seed, resolved at enqueue
     interval: int = -1
     seed: int = 0
+    n: int = 1                             # its images (sequence slots)
+    done: dict = field(default_factory=dict)   # image index -> token ids of every finished sample
 
 
 def _plen(req: _Request) -> int:
@@ -184,6 +199,7 @@ class LLM:
         self._seed = int(torch.randint(0, 2 ** 31, (1,)).item()) if seed is None else int(seed)
         self._slots: List[Optional[_Request]] = [None] * self.max_num_seqs
         self._depth = [0] * self.max_num_seqs          # tokens sampled so far per slot (== position of the next input)
+        self._img = [0] * self.max_num_seqs            # image index of every slot's sample within its request
         self._params: Optional[SamplingParams] = None  # sampling parameters of the running set
         self._state = None                             # device tensors, allocated for (max_num_seqs, max_tokens)
         self.steps_run = 0
@@ -302,22 +318,25 @@ class LLM:
             raise ValueError(f"SamplingParams.seed must be an integer in [0, 2**63), got {sp.seed!r}")
         if self.sjd_window is not None and int(sp.max_tokens) < 3:
             raise ValueError(f"sjd_window needs max_tokens >= 3, got {sp.max_tokens}")
+        if not _is_int(sp.n) or not 1 <= sp.n <= self.max_num_seqs:
+            raise ValueError(f"SamplingParams.n must be an integer in [1, max_num_seqs = {self.max_num_seqs}], got {sp.n!r}")
         return scale, int(interval), None if sp.seed is None else int(sp.seed)
 
     def _guided(self, req: _Request) -> _Request:
-        """req with its guidance and seed resolved (seed None: the LLM's seed + request id)."""
+        """req with its guidance, seed (None: the LLM's seed + request id) and image count resolved."""
         req.cfg, req.interval, seed = self._guidance(req.params)
         req.seed = self._seed + int(req.request_id) if seed is None else seed
+        req.n = int(req.params.n)
         return req
 
     def _twin_guidance(self, twin_of, sampling_params: Optional[SamplingParams]):
-        """A null-class twin mirrors its conditional request: its params may not carry another cfg_scale, cfg_interval or seed."""
+        """A null-class twin mirrors its conditional request: its params may not carry another cfg_scale, cfg_interval, seed or n."""
         owner = self._owner(twin_of)
         sp = sampling_params or SamplingParams()
-        if owner is not None and (sp.cfg_scale, sp.cfg_interval, sp.seed) != (owner.params.cfg_scale, owner.params.cfg_interval,
-                                                                               owner.params.seed):
-            raise ValueError(f"a null-class twin mirrors its conditional request {twin_of!r}: its cfg_scale, cfg_interval and seed must be "
-                             f"the request's")
+        if owner is not None and (sp.cfg_scale, sp.cfg_interval, sp.seed, sp.n) != (owner.params.cfg_scale, owner.params.cfg_interval,
+                                                                                     owner.params.seed, owner.params.n):
+            raise ValueError(f"a null-class twin mirrors its conditional request {twin_of!r}: its cfg_scale, cfg_interval, seed and n "
+                             f"must be the request's")
 
     def _prefix(self, prefix, sampling_params: Optional[SamplingParams]) -> Optional[torch.Tensor]:
         """A request's prefix as int64 [P] on the host, checked as generate(prefix=...) checks it: integer ids in [0, vocab_size),
@@ -360,7 +379,20 @@ class LLM:
         return bool(self._waiting) or self._running() > 0
 
     def get_num_unfinished_requests(self) -> int:
-        return len(self._waiting) + self._running() + len(self._twins)
+        return len(self._waiting) + len({id(r) for r in self._slots if r is not None}) + len(self._twins)
+
+    def _admit(self, params: SamplingParams):
+        """Admission: the waiting requests that share the running set's sampling parameters, in FIFO order, each into its n lowest free
+        slots (image j in the j-th); the first request without n free slots waits, and every request behind it. Returns [(slots, req)]."""
+        free = [i for i in range(self.max_num_seqs) if self._slots[i] is None]
+        joined = []
+        while self._waiting and _batch_key(self._waiting[0].params) == _batch_key(params) and len(free) >= self._waiting[0].n:
+            req = self._waiting.popleft()
+            slots, free = free[:req.n], free[req.n:]
+            for j, i in enumerate(slots):
+                self._slots[i], self._img[i] = req, j
+            joined.append((slots, req))
+        return joined
 
     def _ensure_state(self, params: SamplingParams):
         m, B = self.model, self.max_num_seqs
@@ -376,6 +408,8 @@ class LLM:
             pos=torch.zeros(R, dtype=torch.int32, device=dev),          # per-row positions
             active=torch.zeros(R, dtype=torch.int32, device=dev),       # 1 for rows of occupied slots
             seeds=torch.zeros(B, dtype=torch.int64, device=dev),
+            img=torch.zeros(B, dtype=torch.int32, device=dev),          # every slot's image index (lg_sample_rows_keyed)
+            img_host=[0] * B,                                           # what st["img"] holds
             out=torch.zeros(B, S, dtype=torch.int32, device=dev),
             logits=torch.empty(R, m.vocab_size, dtype=torch.float32, device=dev),
             join_logits=torch.empty(R // B, m.vocab_size, dtype=torch.float32, device=dev),   # a join's logits (one request's rows)
@@ -408,25 +442,38 @@ class LLM:
         greedy = 1 if self.t2i and params.temperature == 0 else 0
         return _lib.SampleCfg(self.cfg_scale, -1, float(params.temperature), max(0, int(params.top_k)), float(params.top_p), greedy, 0)
 
-    def _write_guidance(self, st, idx, reqs: List[_Request]):
-        """The joining requests' seeds and, under CFG, guidance scales and cfg_intervals, to their slots idx (before their draws)."""
+    def _write_guidance(self, st, flat: List[tuple]):
+        """The joining requests' seeds, image indices and, under CFG, guidance scales and cfg_intervals, to their slots (flat: [(slot,
+        request)]) before their draws. The image indices are written only when one of them changes (a slot at image 0 that held image 0
+        writes nothing). Returns the slots as a device index."""
         dev = st["dev"]
-        st["seeds"][idx] = torch.tensor([r.seed for r in reqs], dtype=torch.int64, device=dev)
+        idx = torch.tensor([i for i, _ in flat], dtype=torch.long, device=dev)
+        st["seeds"][idx] = torch.tensor([r.seed for _, r in flat], dtype=torch.int64, device=dev)
         if "cfg" in st:
-            st["cfg"][idx] = torch.tensor([r.cfg for r in reqs], dtype=torch.float32, device=dev)
-            st["interval"][idx] = torch.tensor([r.interval for r in reqs], dtype=torch.int32, device=dev)
+            st["cfg"][idx] = torch.tensor([r.cfg for _, r in flat], dtype=torch.float32, device=dev)
+            st["interval"][idx] = torch.tensor([r.interval for _, r in flat], dtype=torch.int32, device=dev)
+        slots = [i for i, _ in flat]
+        if any(st["img_host"][i] != self._img[i] for i in slots):
+            st["img"][idx] = torch.tensor([self._img[i] for i in slots], dtype=torch.int32, device=dev)
+            for i in slots:
+                st["img_host"][i] = self._img[i]
+        return idx
 
     def _draw(self, st, params: SamplingParams, logits, slots: slice, step_rows, out):
         """One draw for each slot in `slots` from logits (its rows, cond rows first) with the slot's seed at token index step_rows:
         result -> st["tok"][slots] and out[slot, step] (out: st["out"] rows from slots.start). Under CFG each slot mixes with its own
-        scale and cfg_interval (lg_sample_rows_guided with st["cfg"], st["interval"]), otherwise lg_sample_rows."""
+        scale and cfg_interval (lg_sample_rows_guided with st["cfg"], st["interval"]), otherwise lg_sample_rows. When a running slot
+        among them holds an image index > 0 (parallel sampling), every slot draws as its image (lg_sample_rows_keyed with st["img"])."""
         lib, m, n = _lib.load(), self.model, slots.stop - slots.start
         use_cfg = 1 if st["R"] == 2 * self.max_num_seqs else 0
         sc = self._sample_cfg(params)
         dt = _lib.dtype_code(m.tok_embeddings.weight.dtype)   # 16-bit models round the head's logits to their dtype
         head = (_lib.ptr(logits), n, m.vocab_size, use_cfg, dt, ctypes.byref(sc), _lib.ptr(st["seeds"][slots]), _lib.ptr(step_rows))
         tail = (_lib.ptr(st["tok"][slots]), _lib.ptr(out), st["S"], _lib.current_stream(st["dev"]))
-        if use_cfg:
+        if any(self._slots[i] is not None and self._img[i] > 0 for i in range(slots.start, slots.stop)):
+            guide = (_lib.ptr(st["cfg"][slots]), _lib.ptr(st["interval"][slots])) if use_cfg else (None, None)
+            _lib.check(lib.lg_sample_rows_keyed(*head, *guide, _lib.ptr(st["img"][slots]), *tail), "lg_sample_rows_keyed")
+        elif use_cfg:
             _lib.check(lib.lg_sample_rows_guided(*head, _lib.ptr(st["cfg"][slots]), _lib.ptr(st["interval"][slots]), *tail),
                        "lg_sample_rows_guided")
         else:
@@ -498,6 +545,39 @@ class LLM:
             st["neg"][i].copy_(r.neg)
         st["neg_mask"][i].copy_(r.mask if r.neg_mask is None else r.neg_mask)
 
+    # ------------------------------------------------------------------ parallel sampling (SamplingParams.n)
+    def _device_copy_kv(self, st, src: int, dsts: List[int], length: int):
+        """lg_copy_slot_kv: positions [0, length) of slot src's K / V rows (and, under CFG, row B + src) to every slot in dsts."""
+        B, use_cfg = self.max_num_seqs, 1 if st["R"] == 2 * self.max_num_seqs else 0
+        arr = (ctypes.c_int32 * len(dsts))(*dsts)
+        _lib.check(_lib.load().lg_copy_slot_kv(self.model.engine(), src, arr, len(dsts), B, use_cfg, length, _lib.current_stream(st["dev"])),
+                   "lg_copy_slot_kv")
+
+    def _device_join_draws(self, st, params: SamplingParams, slots: List[int], P: int):
+        """Token P of every slot in `slots` drawn from the join's logits (st["join_logits"]) with the slot's seed, guidance and image
+        index (_draw at step P) into st["out"][slot, P] and st["tok"][slot]."""
+        st["join_step"].fill_(P)
+        for i in slots:
+            self._draw(st, params, st["join_logits"], slice(i, i + 1), st["join_step"], st["out"][i])
+
+    def _fan_out(self, st, params: SamplingParams, slots: List[int], P: int):
+        """After the join of a request with several samples prefilled its first slot: its K / V over [0, T + P) to the other slots, then
+        their draws of token P from the same logits."""
+        if len(slots) > 1:
+            self._device_copy_kv(st, slots[0], slots[1:], self.model.cls_token_num + P)
+            self._device_join_draws(st, params, slots[1:], P)
+
+    def _sample_done(self, i: int, toks: List[int]) -> Optional[_Request]:
+        """Free slot i, whose sample finished with tokens toks; returns its request when that was the request's last sample."""
+        req = self._slots[i]
+        self._slots[i] = None
+        req.done[self._img[i]] = toks
+        return req if len(req.done) == req.n else None
+
+    @staticmethod
+    def _completions(req: _Request) -> List[CompletionOutput]:
+        return [CompletionOutput(j, list(req.done[j])) for j in range(req.n)]
+
     # ------------------------------------------------------------------ speculative Jacobi decoding (sjd_window)
     def _sjd_scratch(self, st):
         """(device pointer, bytes) of this LLM's per-slot SJD scratch: 256-byte aligned in st["sjd_ws"]."""
@@ -518,11 +598,16 @@ class LLM:
                    "lg_sjd_slots_reset")
 
     def _device_sjd_start(self, st, slot: int, req: _Request):
-        """lg_sjd_slot_start of slot, after its join drew token 0: the request's seed, guidance and pass counter 0."""
+        """lg_sjd_slot_start of slot, after its join drew token 0: the request's seed, guidance and pass counter 0; a sample j > 0 of a
+        parallel-sampling request keys as image j (lg_sjd_slot_start_image)."""
         B, use_cfg = self.max_num_seqs, 1 if st["R"] == 2 * self.max_num_seqs else 0
         ws, ws_bytes = self._sjd_scratch(st)
-        _lib.check(_lib.load().lg_sjd_slot_start(self.model.engine(), slot, B, use_cfg, st["L"], st["S"], req.seed, req.cfg, req.interval,
-                                                 _lib.ptr(st["out"]), ws, ws_bytes, _lib.current_stream(st["dev"])), "lg_sjd_slot_start")
+        lib, args = _lib.load(), (self.model.engine(), slot, B, use_cfg, st["L"], st["S"], req.seed, req.cfg, req.interval)
+        tail = (_lib.ptr(st["out"]), ws, ws_bytes, _lib.current_stream(st["dev"]))
+        if self._img[slot] > 0:
+            _lib.check(lib.lg_sjd_slot_start_image(*args, self._img[slot], *tail), "lg_sjd_slot_start_image")
+        else:
+            _lib.check(lib.lg_sjd_slot_start(*args, *tail), "lg_sjd_slot_start")
 
     def _device_sjd_pass(self, st, params: SamplingParams, dbg=None):
         """Enqueue pass st["passes"] (lg_sjd_pass_slots) over every slot; its final counts go to a pinned buffer behind an event.
@@ -564,26 +649,23 @@ class LLM:
         over every slot, (3) finish the requests whose final count reached max_tokens in the pass before it. The host never waits for
         the pass it just enqueued: a finished slot stays frozen until then, which changes no request's tokens."""
         B, S, dev = self.max_num_seqs, st["S"], st["dev"]
-        joined = []
-        for i in range(B):
-            if not self._waiting or _batch_key(self._waiting[0].params) != _batch_key(params):
-                break
-            if self._slots[i] is None:
-                req = self._waiting.popleft()
-                self._slots[i] = req
-                joined.append((i, req))
+        joined = self._admit(params)
         if joined:
-            idx = torch.tensor([i for i, _ in joined], dtype=torch.long, device=dev)
-            self._write_guidance(st, idx, [r for _, r in joined])
-            for i, r in joined:
+            flat = [(i, r) for slots, r in joined for i in slots]
+            idx = self._write_guidance(st, flat)
+            for slots, r in joined:
+                i = slots[0]
                 if self.t2i:
-                    self._load_caption(st, i, r)
+                    for s in slots:
+                        self._load_caption(st, s, r)
                     self._device_join_t2i(st, params, i)
                 else:   # one row with the class token (lg_prefill_slot_prefix, P = 0), token 0 drawn with step 0
                     st["tok"][i] = r.prompt_token_ids[0]
                     self._device_join_prefix(st, params, i, 0)
-                self._device_sjd_start(st, i, r)
-                st["first_pass"][i] = st["passes"]
+                self._fan_out(st, params, slots, 0)
+                for s in slots:
+                    self._device_sjd_start(st, s, r)
+                    st["first_pass"][s] = st["passes"]
         done = []
         if self._running():
             self._device_sjd_pass(st, params)
@@ -614,25 +696,24 @@ class LLM:
                     self._depth[i] += 1
         # (2) admission: the conditions and masks go to their slots' rows, then each request is prefilled alone and draws token 0, or,
         # with P given tokens (written to its out row first), token P
-        joined = []
-        for i in range(B):
-            if not self._waiting or _batch_key(self._waiting[0].params) != _batch_key(params):
-                break
-            if self._slots[i] is None:
-                req = self._waiting.popleft()
-                self._slots[i], self._depth[i] = req, _plen(req) + 1
-                joined.append((i, req))
+        joined = self._admit(params)
+        flat = [(i, r) for slots, r in joined for i in slots]
+        for i, r in flat:
+            self._depth[i] = _plen(r) + 1
         if joined:
-            idx = torch.tensor([i for i, _ in joined], dtype=torch.long, device=dev)
-            self._write_guidance(st, idx, [r for _, r in joined])
-            for i, r in joined:
-                self._load_caption(st, i, r)
+            idx = self._write_guidance(st, flat)
+            for slots, r in joined:
+                i = slots[0]
+                for s in slots:
+                    self._load_caption(st, s, r)
                 if r.prefix is None:
                     self._device_join_t2i(st, params, i)
                 else:
-                    st["out"][i, :_plen(r)] = r.prefix.to(device=dev, dtype=torch.int32)
+                    for s in slots:
+                        st["out"][s, :_plen(r)] = r.prefix.to(device=dev, dtype=torch.int32)
                     self._device_join_prefix(st, params, i, _plen(r))
-            P = torch.tensor([_plen(r) for _, r in joined], dtype=torch.int32, device=dev)
+                self._fan_out(st, params, slots, _plen(r))
+            P = torch.tensor([_plen(r) for _, r in flat], dtype=torch.int32, device=dev)
             rows = torch.cat([idx, idx + B]) if R == 2 * B else idx
             st["pos"][rows] = T + (torch.cat([P, P]) if R == 2 * B else P)
             st["active"][rows] = 1
@@ -649,9 +730,9 @@ class LLM:
             st["pos"][rows] = 0
             st["step"][idx] = 0                                # a free slot's draw goes to out[slot, 0], which its next request rewrites
             for i, t in zip(done, toks):
-                req = self._slots[i]
-                self._slots[i] = None
-                outs.append(RequestOutput(req.request_id, [], [CompletionOutput(0, t)], True))
+                req = self._sample_done(i, t)
+                if req is not None:
+                    outs.append(RequestOutput(req.request_id, [], self._completions(req), True))
         return outs
 
     def _device_step(self, st, params: SamplingParams):
@@ -681,32 +762,30 @@ class LLM:
             return self._step_t2i(st, params)
         B, R, S, dev = self.max_num_seqs, st["R"], st["S"], st["dev"]
         # (1) admission: requests that share the running set's sampling parameters join at position 0, mid-sequence of the others
-        joined = []
-        for i in range(B):
-            if not self._waiting or _batch_key(self._waiting[0].params) != _batch_key(params):
-                break
-            if self._slots[i] is None:
-                req = self._waiting.popleft()
-                self._slots[i], self._depth[i] = req, 0
-                joined.append((i, req))
+        joined = self._admit(params)
+        flat = [(i, r) for slots, r in joined for i in slots]
+        for i, _ in flat:
+            self._depth[i] = 0
         if joined:
-            idx = torch.tensor([i for i, _ in joined], dtype=torch.long, device=dev)
-            st["tok"][idx] = torch.tensor([r.prompt_token_ids[0] for _, r in joined], dtype=torch.int32, device=dev)
-            self._write_guidance(st, idx, [r for _, r in joined])
+            idx = self._write_guidance(st, flat)
+            st["tok"][idx] = torch.tensor([r.prompt_token_ids[0] for _, r in flat], dtype=torch.int32, device=dev)
             rows = torch.cat([idx, idx + B]) if R == 2 * B else idx
             st["pos"][rows] = 0
             st["active"][rows] = 1
-            # a completion request is prefilled through its P given tokens (written to its out row first) and draws token P here; its
+            # a completion request is prefilled through its P given tokens (written to its out rows first) and draws token P here; its
             # rows then sit at position 1 + P and this step's decode draws token P + 1
-            for i, r in joined:
+            for slots, r in joined:
                 if r.prefix is not None:
                     P = _plen(r)
-                    st["out"][i, :P] = r.prefix.to(device=dev, dtype=torch.int32)
-                    self._device_join_prefix(st, params, i, P)
-                    st["pos"][[i, B + i] if R == 2 * B else [i]] = self.model.cls_token_num + P
-                    self._depth[i] = P + 1
+                    for i in slots:
+                        st["out"][i, :P] = r.prefix.to(device=dev, dtype=torch.int32)
+                    self._device_join_prefix(st, params, slots[0], P)
+                    self._fan_out(st, params, slots, P)
+                    for i in slots:
+                        st["pos"][[i, B + i] if R == 2 * B else [i]] = self.model.cls_token_num + P
+                        self._depth[i] = P + 1
         # a request whose join drew its last token (P = max_tokens - 1) finishes now, before a decode could write past its out row
-        outs = self._finish_c2i(st, [i for i, _ in joined if self._depth[i] >= S])
+        outs = self._finish_c2i(st, [i for i, _ in flat if self._depth[i] >= S])
         # (2) one decode step for every slot, (3) per-request sampling; the sampled token becomes the slot's next input in place
         if self._running():
             self._device_step(st, params)
@@ -737,12 +816,13 @@ class LLM:
             st["tok"][idx] = 0                                # a free slot sits at position 0 = the class branch: its input must be a valid
                                                               # class id, not the last sampled token (which indexed past the class table)
             for i, t in zip(done, toks):
-                req = self._slots[i]
-                self._slots[i] = None
-                outs.append(RequestOutput(req.request_id, req.prompt_token_ids, [CompletionOutput(0, t)], True))
+                req = self._sample_done(i, t)
+                if req is None:
+                    continue
+                outs.append(RequestOutput(req.request_id, req.prompt_token_ids, self._completions(req), True))
                 twin = self._twins.pop(req.request_id, None)
                 if twin is not None:
-                    outs.append(RequestOutput(twin.request_id, twin.prompt_token_ids, [CompletionOutput(0, list(t))], True))
+                    outs.append(RequestOutput(twin.request_id, twin.prompt_token_ids, self._completions(req), True))
         return outs
 
     # ------------------------------------------------------------------ LLM.generate (llm.py:138-266)
