@@ -219,6 +219,39 @@ int  lg_sample_rows_keyed(const float* logits, int B, int V, int mix_cfg, int ro
  * what a prefill of it would have written. Refused before any launch: a slot outside [0, B), a destination equal to the source or
  * repeated, len outside [0, max_seq], and a workspace with fewer than nh * B rows. One launch per 64 destinations. */
 int  lg_copy_slot_kv(lg_engine* e, int src_slot, const int32_t* dst_slots, int n_dst, int B, int use_cfg, int len, void* stream);
+/* ---- token log-probabilities of the sample kernel's draws ----------------------------------------------------------------------
+ * x is the f32 row a draw takes its token from: the logits rounded to round_dtype, CFG-mixed with the row's scale and interval,
+ * divided by max(temperature, 1e-5), tokens removed by top-k / top-p at -inf. With m = max x and Z = sum exp(x - m) (the kernel's own),
+ * the logprob of token v is (x_v - m) - logf(Z), so exp(logprob) is, up to rounding, lg_sample's out_probs. A greedy draw reports the
+ * distribution it took the argmax of. Every member is NULL (off) or dev memory indexed as the token row out_seq, element
+ * b * seq_stride + step (lg_generate_logprobs: b * S + k):
+ *   logprob      f32: the drawn token's logprob;
+ *   rank         int32: 1 + #{v : x_v > x_drawn} (on x: distinct logits can round to the same expf);
+ *   top_ids      int32 [.., top_n]: the top_n kept tokens by (x descending, id ascending); -1 past the last kept token;
+ *   top_logprob  f32 [.., top_n]: their logprobs; -inf past the last kept token.
+ * 0 <= top_n <= 20; top_n > 0 needs both top_ids and top_logprob (top_n = 0 ignores them). A NULL lg_logprobs, or one with every
+ * member NULL, is off. Turning logprobs on changes no draw. */
+typedef struct lg_logprobs {
+    float*   logprob;
+    int32_t* rank;
+    int32_t* top_ids;
+    float*   top_logprob;
+    int32_t  top_n;
+} lg_logprobs;
+/* lg_sample_rows_keyed (cfg_rows, interval_rows and img_rows may each be NULL) plus token log-probabilities; lp NULL or off is that
+ * call. Logprobs need out_seq (they are indexed as it is). */
+int  lg_sample_rows_logprobs(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc,
+                             const uint64_t* seed_rows, const int32_t* step_rows, const float* cfg_rows, const int32_t* interval_rows,
+                             const int32_t* img_rows, const lg_logprobs* lp, int32_t* out_idx, int32_t* out_seq, int seq_stride,
+                             void* stream);
+/* generate() with token log-probabilities [B, S] (top: [B, S, top_n]), in one call covering lg_generate (neg_cond NULL, P = 0),
+ * lg_generate_neg (neg_cond, neg_mask as there) and lg_generate_prefix(_neg) (1 <= P <= S - 1, prefix and dev_ws as there; P = 0
+ * needs neither and ignores them). The tokens are those of that call. Rows k < P (given tokens) get logprob 0, rank 0, top ids -1 and
+ * top logprobs -inf, so the row sum of logprob is the cumulative logprob of the drawn tokens. No teacher or dbg_logits: lg_generate
+ * and lg_score cover those. */
+int  lg_generate_logprobs(lg_engine* e, const void* cond, const float* emb_mask, const void* neg_cond, const float* neg_mask, int B, int T,
+                          int S, const lg_sample_cfg* sc, const int32_t* prefix, int P, void* dev_ws, size_t ws_bytes,
+                          const lg_logprobs* lp, int32_t* out_tokens, void* stream);
 /* Fused CFG-mix + temperature + top-k + top-p + softmax + (argmax | multinomial): generate.py:57-66,95-97.
  * logits f32 [rows, V] (rows = 2B when mix_cfg, cond rows first); writes out_idx int32 [B] and, when
  * non-NULL, out_probs f32 [B, V] (the post-filter softmax the reference returns as `probs`).

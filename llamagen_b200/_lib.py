@@ -43,6 +43,14 @@ class SampleCfg(Structure):
                 ("top_k", c_int32), ("top_p", c_float), ("greedy", c_int32), ("seed", c_uint64)]
 
 
+class Logprobs(Structure):
+    """lg_logprobs: device pointers (0 = off) of the logprob outputs, and top_n in [0, 20]."""
+    _fields_ = [("logprob", c_void_p), ("rank", c_void_p), ("top_ids", c_void_p), ("top_logprob", c_void_p), ("top_n", c_int32)]
+
+
+MAX_TOP_LOGPROBS = 20
+
+
 class T5Cfg(Structure):
     _fields_ = [("n_layer", c_int32), ("d_model", c_int32), ("d_kv", c_int32), ("n_head", c_int32), ("d_ff", c_int32),
                 ("vocab_size", c_int32), ("num_buckets", c_int32), ("gated_gelu", c_int32), ("dtype", c_int32), ("eps", c_float)]
@@ -91,6 +99,10 @@ SIGNATURES = {
                                       c_void_p, c_void_p, c_int, c_void_p]),
     "lg_sample_rows_keyed": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p, c_void_p, c_void_p, c_void_p,
                                      c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
+    "lg_sample_rows_logprobs": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p, c_void_p, c_void_p, c_void_p,
+                                        c_void_p, POINTER(Logprobs), c_void_p, c_void_p, c_int, c_void_p]),
+    "lg_generate_logprobs": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p,
+                                     c_int, c_void_p, c_size_t, POINTER(Logprobs), c_void_p, c_void_p]),
     "lg_copy_slot_kv": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "lg_sample": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(SampleCfg), c_uint64, c_void_p,
                           c_void_p, c_void_p]),

@@ -1027,17 +1027,43 @@ int lg_score(lg_engine* e, const void* cond, const float* emb_mask, const int32_
 
 }  // extern "C"
 
-// lg_sample_rows (cfg_rows = interval_rows = img_rows = null), lg_sample_rows_guided (img_rows = null) and lg_sample_rows_keyed; fn
-// names the entry point in messages
+// A caller's lg_logprobs: NULL or every member NULL is off; on, 0 <= top_n <= kMaxTopLogprobs and top_n > 0 needs both top arrays
+static int check_logprobs(const char* fn, const lg_logprobs* lp, bool* on) {
+    *on = lp && (lp->logprob || lp->rank || (lp->top_n > 0 && (lp->top_ids || lp->top_logprob)));
+    if (!lp) return 0;
+    LG_REQUIRE(lp->top_n >= 0 && lp->top_n <= kMaxTopLogprobs, "%s: top_n=%d outside [0, %d]", fn, lp->top_n, kMaxTopLogprobs);
+    LG_REQUIRE(lp->top_n == 0 || (lp->top_ids && lp->top_logprob), "%s: top_n=%d needs both top_ids and top_logprob", fn, lp->top_n);
+    return 0;
+}
+
+// The logprob outputs of `lp` (checked by check_logprobs, or NULL) into a, offset by `off` elements of the token row
+static void apply_logprobs(SampleArgs& a, const lg_logprobs* lp, size_t off) {
+    if (!lp) return;
+    a.lp_out = lp->logprob ? lp->logprob + off : nullptr;
+    a.rank_out = lp->rank ? lp->rank + off : nullptr;
+    if (lp->top_n > 0) {
+        a.top_n = lp->top_n;
+        a.top_ids = lp->top_ids + off * lp->top_n;
+        a.top_lp = lp->top_logprob + off * lp->top_n;
+    }
+}
+
+// lg_sample_rows (cfg_rows = interval_rows = img_rows = null), lg_sample_rows_guided (img_rows = null), lg_sample_rows_keyed and
+// lg_sample_rows_logprobs (lp: NULL for the others); fn names the entry point in messages
 static int sample_rows_impl(const char* fn, const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc,
                             const uint64_t* seed_rows, const int32_t* step_rows, const float* cfg_rows, const int32_t* interval_rows,
-                            const int32_t* img_rows, int32_t* out_idx, int32_t* out_seq, int seq_stride, void* stream) {
+                            const int32_t* img_rows, const lg_logprobs* lp, int32_t* out_idx, int32_t* out_seq, int seq_stride,
+                            void* stream) {
     LG_REQUIRE(logits && sc && seed_rows && step_rows && (out_idx || out_seq), "%s: null argument", fn);
     LG_REQUIRE(mix_cfg || (!cfg_rows && !interval_rows), "%s: per-row cfg_rows / interval_rows need mix_cfg (2B logits rows)", fn);
+    bool lp_on = false;
+    LG_TRY(check_logprobs(fn, lp, &lp_on));
+    LG_REQUIRE(!lp_on || out_seq, "%s: logprobs are indexed as out_seq and need it", fn);
     SampleArgs a = make_sample_args(*sc, logits, B, V, mix_cfg, round_dtype);
     a.seed_rows = seed_rows; a.step_rows = step_rows;
     a.cfg_rows = cfg_rows; a.interval_rows = interval_rows; a.img_rows = img_rows;
     a.out_idx = out_idx; a.out_seq = out_seq; a.seq_stride = seq_stride;
+    if (lp_on) apply_logprobs(a, lp, 0);
     return launch_sample(a, (cudaStream_t)stream);
 }
 
@@ -1046,21 +1072,29 @@ extern "C" {
 int lg_sample_rows(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc, const uint64_t* seed_rows,
                    const int32_t* step_rows, int32_t* out_idx, int32_t* out_seq, int seq_stride, void* stream) {
     return sample_rows_impl("lg_sample_rows", logits, B, V, mix_cfg, round_dtype, sc, seed_rows, step_rows, nullptr, nullptr, nullptr,
-                            out_idx, out_seq, seq_stride, stream);
+                            nullptr, out_idx, out_seq, seq_stride, stream);
 }
 
 int lg_sample_rows_guided(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc,
                           const uint64_t* seed_rows, const int32_t* step_rows, const float* cfg_rows, const int32_t* interval_rows,
                           int32_t* out_idx, int32_t* out_seq, int seq_stride, void* stream) {
     return sample_rows_impl("lg_sample_rows_guided", logits, B, V, mix_cfg, round_dtype, sc, seed_rows, step_rows, cfg_rows,
-                            interval_rows, nullptr, out_idx, out_seq, seq_stride, stream);
+                            interval_rows, nullptr, nullptr, out_idx, out_seq, seq_stride, stream);
 }
 
 int lg_sample_rows_keyed(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc,
                          const uint64_t* seed_rows, const int32_t* step_rows, const float* cfg_rows, const int32_t* interval_rows,
                          const int32_t* img_rows, int32_t* out_idx, int32_t* out_seq, int seq_stride, void* stream) {
     return sample_rows_impl("lg_sample_rows_keyed", logits, B, V, mix_cfg, round_dtype, sc, seed_rows, step_rows, cfg_rows,
-                            interval_rows, img_rows, out_idx, out_seq, seq_stride, stream);
+                            interval_rows, img_rows, nullptr, out_idx, out_seq, seq_stride, stream);
+}
+
+int lg_sample_rows_logprobs(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc,
+                            const uint64_t* seed_rows, const int32_t* step_rows, const float* cfg_rows, const int32_t* interval_rows,
+                            const int32_t* img_rows, const lg_logprobs* lp, int32_t* out_idx, int32_t* out_seq, int seq_stride,
+                            void* stream) {
+    return sample_rows_impl("lg_sample_rows_logprobs", logits, B, V, mix_cfg, round_dtype, sc, seed_rows, step_rows, cfg_rows,
+                            interval_rows, img_rows, lp, out_idx, out_seq, seq_stride, stream);
 }
 
 int lg_sample(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc, uint64_t step,
@@ -1079,17 +1113,18 @@ struct PrefixArgs {              // lg_generate_prefix: prefix [B, P] and the pr
 };
 static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, const Negative& neg, int B, int T, int S,
                          const lg_sample_cfg* sc, int32_t* out_tokens, float* dbg_logits, const int32_t* teacher,
-                         const PrefixArgs& pa, cudaStream_t st);
+                         const PrefixArgs& pa, const lg_logprobs* lp, cudaStream_t st);
 
 }  // extern "C"
 
 static int generate_entry(const char* fn, lg_engine* e, const void* cond, const float* emb_mask, const Negative& neg, int B, int T, int S,
-                          const lg_sample_cfg* sc, int32_t* out_tokens, float* dbg_logits, const int32_t* teacher, void* stream) {
+                          const lg_sample_cfg* sc, int32_t* out_tokens, float* dbg_logits, const int32_t* teacher, void* stream,
+                          const lg_logprobs* lp = nullptr) {
     LG_REQUIRE(e, "%s: null engine", fn);
     LG_TRY(check_negative(fn, e, neg, emb_mask, sc && sc->cfg_scale > 1.0f));
     DeviceGuard guard(e->device);
     return e->run_forked((cudaStream_t)stream, lg_engine::kMaxChains, [&](cudaStream_t st) {
-        return generate_impl(e, cond, emb_mask, neg, B, T, S, sc, out_tokens, dbg_logits, teacher, PrefixArgs{}, st);
+        return generate_impl(e, cond, emb_mask, neg, B, T, S, sc, out_tokens, dbg_logits, teacher, PrefixArgs{}, lp, st);
     });
 }
 
@@ -1117,7 +1152,7 @@ int lg_prefix_workspace_bytes(lg_engine* e, int rows, int seq, size_t* bytes) {
 
 static int generate_prefix_entry(const char* fn, lg_engine* e, const void* cond, const float* emb_mask, const Negative& neg, int B, int T,
                                  int S, const lg_sample_cfg* sc, const int32_t* prefix, int P, void* dev_ws, size_t ws_bytes,
-                                 int32_t* out_tokens, float* dbg_logits, void* stream) {
+                                 int32_t* out_tokens, float* dbg_logits, void* stream, const lg_logprobs* lp = nullptr) {
     LG_REQUIRE(e && e->finalized, "%s: engine not finalized", fn);
     DeviceGuard guard(e->device);
     const lg_model_cfg& c = e->cfg;
@@ -1135,7 +1170,7 @@ static int generate_prefix_entry(const char* fn, lg_engine* e, const void* cond,
     LG_REQUIRE(ws_bytes >= need1, "%s: scratch of %zu bytes is too small for one image (%zu)", fn, ws_bytes, need1);
     const PrefixArgs pa{prefix, P, (char*)dev_ws, ws_bytes};
     return e->run_forked((cudaStream_t)stream, lg_engine::kMaxChains, [&](cudaStream_t st) {
-        return generate_impl(e, cond, emb_mask, neg, B, T, S, sc, out_tokens, dbg_logits, nullptr, pa, st);
+        return generate_impl(e, cond, emb_mask, neg, B, T, S, sc, out_tokens, dbg_logits, nullptr, pa, lp, st);
     });
 }
 
@@ -1152,6 +1187,18 @@ int lg_generate_prefix_neg(lg_engine* e, const void* cond, const float* emb_mask
                            float* dbg_logits, void* stream) {
     return generate_prefix_entry("lg_generate_prefix_neg", e, cond, emb_mask, Negative{neg_cond, neg_mask}, B, T, S, sc, prefix, P, dev_ws,
                                  ws_bytes, out_tokens, dbg_logits, stream);
+}
+
+int lg_generate_logprobs(lg_engine* e, const void* cond, const float* emb_mask, const void* neg_cond, const float* neg_mask, int B, int T,
+                         int S, const lg_sample_cfg* sc, const int32_t* prefix, int P, void* dev_ws, size_t ws_bytes,
+                         const lg_logprobs* lp, int32_t* out_tokens, void* stream) {
+    const char* fn = "lg_generate_logprobs";
+    bool lp_on = false;
+    LG_TRY(check_logprobs(fn, lp, &lp_on));
+    const Negative neg{neg_cond, neg_mask};
+    if (P == 0) return generate_entry(fn, e, cond, emb_mask, neg, B, T, S, sc, out_tokens, nullptr, nullptr, stream, lp_on ? lp : nullptr);
+    return generate_prefix_entry(fn, e, cond, emb_mask, neg, B, T, S, sc, prefix, P, dev_ws, ws_bytes, out_tokens, nullptr, stream,
+                                 lp_on ? lp : nullptr);
 }
 
 int lg_test_prefix_chunks(lg_engine* e, int* chains) {
@@ -1315,7 +1362,7 @@ int lg_prefill_slot(lg_engine* e, const void* cond, const float* emb_mask, int T
 
 static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, const Negative& neg, int B, int T, int S,
                          const lg_sample_cfg* sc, int32_t* out_tokens, float* dbg_logits, const int32_t* teacher,
-                         const PrefixArgs& pa, cudaStream_t st0) {
+                         const PrefixArgs& pa, const lg_logprobs* lp, cudaStream_t st0) {
     LG_REQUIRE(cond && sc && out_tokens && B > 0 && S > 0, "lg_generate: bad argument");
     const bool use_cfg = sc->cfg_scale > 1.0f;  // generate.py:128
     const int R = use_cfg ? 2 * B : B;
@@ -1351,6 +1398,7 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
         sa.out_seq = out_tokens + boff * S; sa.seq_stride = S; sa.next_tokens = k.w.tokens;
         sa.teacher = teacher ? teacher + boff * S : nullptr;
         sa.dbg_logits = dbg_logits; sa.dbg_batch = B;
+        apply_logprobs(sa, lp, boff * S);
     }
 
     // Fused tail (bf16 / fp16): the sample kernel writes the next step's input rows (token embedding, and on the batched path the layer-0
@@ -1397,6 +1445,8 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
         LG_REQUIRE(fits(lo), "lg_generate_prefix: no chunk of rows fits the scratch (%zu bytes) and the attention grid", pa.scratch_bytes);
         LG_CUDA_OK(cudaMemcpy2DAsync(out_tokens, (size_t)S * sizeof(int32_t), pa.prefix, (size_t)P * sizeof(int32_t),
                                      (size_t)P * sizeof(int32_t), B, cudaMemcpyDeviceToDevice, st0));
+        if (lp) LG_TRY(launch_given_logprobs(lp->logprob, lp->rank, lp->top_n > 0 ? lp->top_ids : nullptr,
+                                             lp->top_n > 0 ? lp->top_logprob : nullptr, lp->top_n, B, S, P, st0));
         e->prefix_chunks = 0;
         e->prefix_chains = nchains;
         for (int g = 0; g < nchains; ++g) LG_TRY(prefix_prefill(e, ch[g], nh, T, P, lo, blk, pa, st0));

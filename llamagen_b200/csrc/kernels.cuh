@@ -56,12 +56,24 @@ struct SampleArgs {
     // lg_test_sample only: [B][3] per image, written by thread 0 of its CTA: top-k select (0 none, 1 histogram, 2 radix fallback),
     // nucleus tie trim (0 / 1), draw ending (0 greedy, 1 claimed by a segment, 2 the past-the-end fallback). Null in production.
     int32_t* dbg_path = nullptr;
+    // token log-probabilities (lg_sample_rows_logprobs, lg_generate_logprobs), each null or indexed as out_seq: element
+    // b * seq_stride + step (top_ids / top_lp: that element's row of top_n). Any of them non-null selects the logprob instantiation.
+    float* lp_out = nullptr;               // logprob of the drawn token: (x_pick - m) - log(Z) on the processed row x
+    int32_t* rank_out = nullptr;           // 1 + #{v : x_v > x_pick}
+    int32_t* top_ids = nullptr;            // the top_n kept tokens by (x desc, id asc); -1 past the kept ones
+    float* top_lp = nullptr;               // their logprobs; -inf past the kept ones
+    int top_n = 0;                         // 0 .. kMaxTopLogprobs
 };
+constexpr int kMaxTopLogprobs = 20;
+inline bool sample_wants_logprobs(const SampleArgs& a) { return a.lp_out || a.rank_out || a.top_ids || a.top_lp; }
 // The sample kernel stages the row with 16-byte loads (and dbg_logits with 16-byte stores) iff this holds, else element by element
 __host__ __device__ inline bool sample_vec_loads(const SampleArgs& a) {
     return (a.V & 3) == 0 && ((uintptr_t)a.logits & 15) == 0 && ((uintptr_t)a.dbg_logits & 15) == 0;
 }
 int launch_sample(const SampleArgs& a, cudaStream_t st);
+// Logprob rows of given tokens (lg_generate_logprobs' prefix): element b * S + k, k < P, of every non-null array gets logprob 0, rank 0,
+// top ids -1 and top logprobs -inf
+int launch_given_logprobs(float* lp, int32_t* rank, int32_t* top_ids, float* top_lp, int top_n, int B, int S, int P, cudaStream_t st);
 
 // Speculative Jacobi decoding (lg_generate_sjd). Image b's window has L slots; slot i feeds token start[b] + i - 1 (win) and its
 // output p (the sample kernel's out_probs) is the distribution of token start[b] + i. Rows of image b are b * L + i.

@@ -45,8 +45,85 @@ __device__ __forceinline__ int block_last_true(bool pred, int* s_w) {
     return r;
 }
 
-// E: the 16-bit type of the rounding (a.round_dtype != LG_DTYPE_F32) and of the fused tail's rows
-template <typename E>
+// Dynamic shared memory of the logprob instantiation: the working row, a copy of the processed row x (the exp pass overwrites the
+// working row), then every warp's top-N candidates (x, id)
+__host__ __device__ constexpr size_t sample_lp_smem(int V) {
+    return (size_t)2 * V * sizeof(float) + (size_t)(kSampleThreads / 32) * kMaxTopLogprobs * (sizeof(float) + sizeof(int));
+}
+
+// Logprob, rank and top-N of the row x (xs, V floats) the draw took `pick` from; m, Z: the final softmax's max and sum, so that
+// exp(logprob) is the kernel's own probability. o: the output element (out_seq's index). Called by every thread after the draw.
+__device__ void sample_logprobs(const SampleArgs& a, const float* xs, float* cx, int* ci, int V, float m, float Z, int pick, size_t o) {
+    __shared__ int s_gt[kSampleThreads / 32];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const float lz = logf(Z);
+    const float xp = pick >= 0 ? xs[pick] : __int_as_float(0x7fffffff);
+    if (a.rank_out) {   // on x, not on exp values: distinct logits can round to the same expf
+        int gt = 0;
+        for (int v = tid; v < V; v += kSampleThreads) gt += xs[v] > xp;
+        gt = __reduce_add_sync(0xffffffffu, gt);
+        if (lane == 0) s_gt[warp] = gt;
+        __syncthreads();
+        if (tid == 0) {
+            int r = 1;
+            for (int w = 0; w < kSampleThreads / 32; ++w) r += s_gt[w];
+            a.rank_out[o] = r;
+        }
+    }
+    if (tid == 0 && a.lp_out) a.lp_out[o] = (xp - m) - lz;
+    const int N = a.top_n;
+    if (N <= 0) return;
+    // order (x desc, id asc); (bx, bi) is better than (x, i); kept tokens only, so an empty slot (-inf, INT_MAX) loses to all of them
+    auto better = [](float x, int i, float bx, int bi) { return x > bx || (x == bx && i < bi); };
+    auto warp_best = [&](float& bx, int& bi) {
+#pragma unroll
+        for (int s = 16; s > 0; s >>= 1) {
+            const float ox = __shfl_xor_sync(0xffffffffu, bx, s);
+            const int oi = __shfl_xor_sync(0xffffffffu, bi, s);
+            if (better(ox, oi, bx, bi)) { bx = ox; bi = oi; }
+        }
+    };
+    // each lane: the best kept entry of its columns (v = 32 warp + lane + 1024 j) strictly after (lx, li) in the order
+    auto scan = [&](float lx, int li, float& bx, int& bi) {
+        bx = -INFINITY; bi = 0x7fffffff;
+        for (int v = warp * 32 + lane; v < V; v += kSampleThreads) {
+            const float x = xs[v];
+            if ((x < lx || (x == lx && v > li)) && x > -INFINITY && better(x, v, bx, bi)) { bx = x; bi = v; }
+        }
+    };
+    // each warp: its N best in N shuffle-argmax rounds; the other lanes' candidates stay valid, so only the winner's lane rescans
+    float bx, wx;
+    int bi, wi;
+    scan(INFINITY, -1, bx, bi);
+    for (int r = 0; r < N; ++r) {
+        wx = bx; wi = bi;
+        warp_best(wx, wi);
+        if (lane == 0) { cx[warp * N + r] = wx; ci[warp * N + r] = wi; }
+        if (wi != 0x7fffffff && bi == wi) scan(wx, wi, bx, bi);
+    }
+    __syncthreads();
+    // warp 0 merges the 32 sorted lists: lane w holds the head of warp w's, and the winner's lane advances
+    static_assert(kSampleThreads / 32 == 32, "one list per lane");
+    if (warp == 0) {
+        int p = 0;
+        for (int r = 0; r < N; ++r) {
+            const float x = p < N ? cx[lane * N + p] : -INFINITY;
+            const int id = p < N ? ci[lane * N + p] : 0x7fffffff;
+            wx = x; wi = id;
+            warp_best(wx, wi);
+            if (lane == 0) {
+                const bool kept = wi != 0x7fffffff;
+                a.top_ids[o * N + r] = kept ? wi : -1;
+                a.top_lp[o * N + r] = kept ? (wx - m) - lz : -INFINITY;
+            }
+            if (wi != 0x7fffffff && id == wi) ++p;
+        }
+    }
+}
+
+// E: the 16-bit type of the rounding (a.round_dtype != LG_DTYPE_F32) and of the fused tail's rows. kLogprobs: also write the token
+// log-probabilities (SampleArgs.lp_out ...); the draw is the same
+template <typename E, bool kLogprobs>
 __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
     using TR = ElemTraits<E>;
     lg_pdl_sync();
@@ -326,6 +403,7 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
     const float m = block_max(lm, red);
     float ls = 0.f;
     for (int v = tid; v < V; v += kSampleThreads) {
+        if constexpr (kLogprobs) sh[V + v] = sh[v];
         const float e = expf(sh[v] - m);
         sh[v] = e;
         ls += e;
@@ -434,6 +512,11 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
         }
     }
 
+    if constexpr (kLogprobs) {
+        float* cx = sh + 2 * (size_t)V;
+        sample_logprobs(a, sh + V, cx, reinterpret_cast<int*>(cx + (kSampleThreads / 32) * kMaxTopLogprobs), V, m, Z, s_pick,
+                        (size_t)b * a.seq_stride + step);
+    }
     __shared__ int s_next;
     if (tid == 0) {
         const int pick = s_pick;
@@ -502,17 +585,47 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
 
 int launch_sample(const SampleArgs& a, cudaStream_t st) {
     LG_REQUIRE(a.B > 0 && a.V > 0, "lg_sample: bad shape B=%d V=%d", a.B, a.V);
-    const size_t smem = (size_t)a.V * sizeof(float);
-    LG_REQUIRE(smem <= 200 * 1024, "lg_sample: vocab %d too large for the shared-memory row stage", a.V);
+    const bool lp = sample_wants_logprobs(a);
+    const size_t smem = lp ? sample_lp_smem(a.V) : (size_t)a.V * sizeof(float);
+    LG_REQUIRE(smem <= 200 * 1024, "lg_sample: vocab %d too large for the shared-memory row stage%s", a.V, lp ? " with logprobs" : "");
     LG_REQUIRE(a.round_dtype == LG_DTYPE_F32 || lg_dtype_is16(a.round_dtype), "lg_sample: unsupported round dtype %d", a.round_dtype);
     LG_REQUIRE(!a.emb_table || a.round_dtype != LG_DTYPE_F32, "lg_sample: the fused tail needs a 16-bit round dtype");
+    LG_REQUIRE(a.top_n >= 0 && a.top_n <= kMaxTopLogprobs && (a.top_n == 0) == (!a.top_ids && !a.top_lp) &&
+                   (a.top_n == 0 || (a.top_ids && a.top_lp)),
+               "lg_sample: top_n=%d outside [0, %d], or top_ids / top_logprob not both given exactly when top_n > 0", a.top_n,
+               kMaxTopLogprobs);
     const bool half = a.round_dtype == LG_DTYPE_F16;
-    auto kern = half ? sample_kernel<f16> : sample_kernel<bf16>;
-    static DevOnce attr_set[2];
-    if (lg_first_on_device(attr_set[half])) {
+    auto kern = lp ? (half ? sample_kernel<f16, true> : sample_kernel<bf16, true>)
+                   : (half ? sample_kernel<f16, false> : sample_kernel<bf16, false>);
+    static DevOnce attr_set[4];
+    if (lg_first_on_device(attr_set[2 * lp + half])) {
         LG_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     }
     (void)lg_launch(kern, dim3(a.B), dim3(kSampleThreads), smem, st, a);
+    LG_LAUNCH_CHECK();
+    return 0;
+}
+
+namespace {
+__global__ void given_logprobs_kernel(float* lp, int32_t* rank, int32_t* top_ids, float* top_lp, int top_n, int S, int P) {
+    lg_pdl_sync();
+    const int b = blockIdx.x;
+    for (int k = threadIdx.x; k < P; k += blockDim.x) {
+        const size_t o = (size_t)b * S + k;
+        if (lp) lp[o] = 0.f;
+        if (rank) rank[o] = 0;
+        for (int j = 0; j < top_n; ++j) {
+            if (top_ids) top_ids[o * top_n + j] = -1;
+            if (top_lp) top_lp[o * top_n + j] = -INFINITY;
+        }
+    }
+}
+}  // namespace
+
+int launch_given_logprobs(float* lp, int32_t* rank, int32_t* top_ids, float* top_lp, int top_n, int B, int S, int P, cudaStream_t st) {
+    LG_REQUIRE(B > 0 && P >= 0 && P <= S && top_n >= 0, "given logprobs: bad shape B=%d S=%d P=%d top_n=%d", B, S, P, top_n);
+    if (P == 0) return 0;
+    (void)lg_launch(given_logprobs_kernel, dim3(B), dim3(128), 0, st, lp, rank, top_ids, top_lp, top_n, S, P);
     LG_LAUNCH_CHECK();
     return 0;
 }

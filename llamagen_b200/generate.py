@@ -55,6 +55,16 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
                            sjd_window paths; not with teacher.
       negative_emb_masks=tensor  [1, T] or [B, T]: the negative's emb-mask (the unconditional rows attend with it). Either of
                            emb_masks / negative_emb_masks left out counts as all ones.
+      return_logprobs=True return (tokens, logprobs): f32 [B, S], the log-probability of every drawn token under the distribution the
+                           sampler drew it from (logits rounded to the model dtype, CFG-mixed with cfg_interval, divided by
+                           temperature, top-k / top-p applied; a greedy draw reports that distribution's value too). Rows k < P of a
+                           prefix are 0, so logprobs.sum(1) is the cumulative logprob of the drawn tokens. The tokens are those of the
+                           same call without it. Works on the plain, CFG, negative and prefix paths; not with sjd_window, teacher (use
+                           score() for given tokens) or return_logits.
+      top_logprobs=N       1 <= N <= 20, with return_logprobs: return (tokens, logprobs, {"ranks": int32 [B, S], "top_ids": int32
+                           [B, S, N], "top_logprobs": f32 [B, S, N]}). rank = 1 + the number of tokens with a larger processed logit;
+                           the top ids are the N kept tokens with the largest logits (ties: lower id first), -1 with logprob -inf past
+                           the last kept token. Prefix rows: rank 0, ids -1, logprobs -inf.
     """
     if not isinstance(model, Transformer):
         raise TypeError("llamagen_b200.generate needs a llamagen_b200 GPT_models[...] instance")
@@ -70,8 +80,22 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
     prefix = sampling_kwargs.pop("prefix", None)
     negative_cond = sampling_kwargs.pop("negative_cond", None)
     negative_emb_masks = sampling_kwargs.pop("negative_emb_masks", None)
+    return_logprobs = bool(sampling_kwargs.pop("return_logprobs", False))
+    top_logprobs = sampling_kwargs.pop("top_logprobs", None)
     if sampling_kwargs:
         raise TypeError(f"unexpected sampling kwargs: {sorted(sampling_kwargs)}")
+    if top_logprobs is not None:
+        if not return_logprobs:
+            raise ValueError("top_logprobs needs return_logprobs=True")
+        if not _is_int(top_logprobs) or not 1 <= int(top_logprobs) <= _lib.MAX_TOP_LOGPROBS:
+            raise ValueError(f"top_logprobs must be an integer in [1, {_lib.MAX_TOP_LOGPROBS}], got {top_logprobs!r}")
+    if return_logprobs:
+        if sjd_window is not None:
+            raise ValueError("return_logprobs cannot be combined with sjd_window")
+        if teacher is not None:
+            raise ValueError("return_logprobs cannot be combined with teacher: score() gives the log-likelihood of given tokens")
+        if return_logits:
+            raise ValueError("return_logprobs cannot be combined with return_logits")
     if sjd_window is not None:
         if isinstance(sjd_window, bool) or int(sjd_window) != sjd_window or not 2 <= int(sjd_window) <= 64:
             raise ValueError(f"sjd_window must be an integer in [2, 64], got {sjd_window!r}")
@@ -123,6 +147,11 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
         return _generate_sjd(model, lib, handle, cond, cond_dev, em, B, T, S, out, min(int(sjd_window), S - 1), use_cfg, return_stats,
                              _lib.SampleCfg(float(cfg_scale), int(cfg_interval), temperature, top_k, top_p, 0 if sample_logits else 1,
                                             _draw_seed() if seed is None else int(seed)), neg=neg, nm=nm)
+    if return_logprobs:
+        sc = _lib.SampleCfg(float(cfg_scale), int(cfg_interval), temperature, top_k, top_p, 0 if sample_logits else 1,
+                            _draw_seed() if seed is None else int(seed))
+        return _generate_logprobs(model, lib, handle, cond, cond_dev, em, neg, nm, pf, B, T, S, sc, out, use_cfg,
+                                  None if top_logprobs is None else int(top_logprobs))
     if pf is not None:
         P = pf.shape[1]
         dbg = torch.zeros((S, B, model.vocab_size), dtype=torch.float32, device=dev) if return_logits else None
@@ -155,6 +184,35 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
     if cond.device != dev:
         out = out.to(cond.device)
     return (out, dbg) if return_logits else out
+
+
+def _is_int(x) -> bool:
+    return isinstance(x, int) and not isinstance(x, bool)
+
+
+def _generate_logprobs(model, lib, handle, cond, cond_dev, em, neg, nm, pf, B, T, S, sc, out, use_cfg, top_n):
+    """lg_generate_logprobs: generate() with return_logprobs (top_n: None or top_logprobs)."""
+    dev = out.device
+    lp = torch.empty((B, S), dtype=torch.float32, device=dev)
+    extra = None
+    if top_n is not None:
+        extra = {"ranks": torch.empty((B, S), dtype=torch.int32, device=dev),
+                 "top_ids": torch.empty((B, S, top_n), dtype=torch.int32, device=dev),
+                 "top_logprobs": torch.empty((B, S, top_n), dtype=torch.float32, device=dev)}
+    spec = _lib.Logprobs(lp.data_ptr(), *((extra["ranks"].data_ptr(), extra["top_ids"].data_ptr(), extra["top_logprobs"].data_ptr(),
+                                           top_n) if extra else (0, 0, 0, 0)))
+    P, pf_dev, ws, ws_bytes = 0, None, None, 0
+    if pf is not None:
+        P = pf.shape[1]
+        pf_dev = pf.to(device=dev, dtype=torch.int32).contiguous()
+        ws, ws_bytes = model._prefix_scratch(2 * B if use_cfg else B, T + P, 2 if use_cfg else 1)
+    _lib.check(lib.lg_generate_logprobs(handle, _lib.ptr(cond_dev), _lib.ptr(em), _lib.ptr(neg), _lib.ptr(nm), B, T, S, ctypes.byref(sc),
+                                        _lib.ptr(pf_dev), P, ws, ws_bytes, ctypes.byref(spec), _lib.ptr(out), _lib.current_stream(dev)),
+               "lg_generate_logprobs")
+    if cond.device != dev:
+        out, lp = out.to(cond.device), lp.to(cond.device)
+        extra = None if extra is None else {k: v.to(cond.device) for k, v in extra.items()}
+    return (out, lp) if extra is None else (out, lp, extra)
 
 
 def _check_negative(model, cond, emb_masks, negative_cond, negative_emb_masks, cfg_scale, teacher):

@@ -70,6 +70,19 @@ join's logits are drawn once per slot with the slot's image index (lg_sample_row
 start at position 0 with the same class. Samples finish independently (under SJD at different passes); a finished sample frees its slot
 at once, and the request is returned when its last sample finishes. Null-class twins mirror the request's k outputs.
 
+Token log-probabilities (SamplingParams(logprobs=N), 0 <= N <= 20; vLLM's field): every CompletionOutput then carries
+cumulative_logprob and one dict per token_ids entry, None for a given prefix token, otherwise {drawn token: Logprob(logprob, rank)} plus
+the N kept tokens with the largest processed logits (Logprob(logprob, 1 .. N)). The numbers are the sample kernel's own, on the
+distribution the token was drawn from: the logits rounded to the model dtype, mixed with the request's guidance, divided by temperature
+and filtered by top-k / top-p (generate(return_logprobs=True, top_logprobs=N) for image j of the request). Two differences from vLLM:
+a greedy (temperature 0, t2i) draw reports that distribution, not the temperature-1 one, and a slot past the last token top-k / top-p
+keep is left out rather than filled with arbitrary -inf tokens. Requests with and without logprobs share the running batch; a draw
+switches to lg_sample_rows_logprobs only while a running or joining slot needs logprobs, and asks for 20 alternatives whenever one asks
+for any (the device rows hold 20 per token). best_of = m (n <= m <= max_num_seqs) draws images 0 .. m - 1 as n = m would and returns
+the n with the largest cumulative_logprob, sorted descending (ties: the lower image index first), each with its image index; without
+best_of the outputs stay in index order (vLLM always sorts). cumulative_logprob is filled whenever logprobs or best_of is set: the sum of
+the drawn tokens' logprobs in float64. Neither field goes with sjd_window.
+
 While requests are in flight the LLM owns the model's KV-cache workspace (a `generate()` call on the same model would reset it)."""
 from __future__ import annotations
 
@@ -78,7 +91,7 @@ import math
 import numbers
 from collections import deque
 from dataclasses import dataclass, field
-from typing import List, Optional, Sequence
+from typing import Dict, List, Optional, Sequence
 
 import ctypes
 
@@ -98,7 +111,10 @@ class SamplingParams:
     cfg_interval: None = -1; an integer >= -1, generate()'s cfg_interval (the mix is dropped after decode iteration cfg_interval).
     seed: None = the LLM's seed + request id; an integer in [0, 2**63), the key generate(seed=...) draws image 0 with.
     n: the number of images of the request, an integer in [1, max_num_seqs]; image j is what image j of generate(cond repeated n times,
-    seed=seed) draws. Requests that differ in n share the running batch."""
+    seed=seed) draws. Requests that differ in n share the running batch.
+    logprobs: None, or an integer in [0, 20]: return every drawn token's logprob and rank and its `logprobs` most likely alternatives.
+    best_of: None, or an integer in [n, max_num_seqs]: draw best_of images and return the n with the largest cumulative_logprob.
+    Requests that differ in logprobs or best_of share the running batch."""
     temperature: float = 1.0
     top_p: float = 1.0
     top_k: int = -1
@@ -107,6 +123,13 @@ class SamplingParams:
     cfg_interval: Optional[int] = None
     seed: Optional[int] = None
     n: int = 1
+    logprobs: Optional[int] = None
+    best_of: Optional[int] = None
+
+
+def _wants_logprobs(p: SamplingParams) -> bool:
+    """Whether a request's draws need the device's logprob outputs."""
+    return p.logprobs is not None or p.best_of is not None
 
 
 def _batch_key(p: SamplingParams):
@@ -119,10 +142,19 @@ def _is_int(x) -> bool:
 
 
 @dataclass
+class Logprob:
+    """vLLM's Logprob without the decoded text: a token's log-probability and its rank among the processed logits (1 = largest)."""
+    logprob: float
+    rank: int
+
+
+@dataclass
 class CompletionOutput:
     index: int
     token_ids: List[int]
     finish_reason: str = "length"
+    cumulative_logprob: Optional[float] = None
+    logprobs: Optional[List[Optional[Dict[int, Logprob]]]] = None
 
 
 @dataclass
@@ -147,8 +179,9 @@ class _Request:
     cfg: float = 1.0                       # the request's guidance scale, cfg_interval and RNG seed, resolved at enqueue
     interval: int = -1
     seed: int = 0
-    n: int = 1                             # its images (sequence slots)
+    n: int = 1                             # its images (sequence slots): best_of, else n
     done: dict = field(default_factory=dict)   # image index -> token ids of every finished sample
+    done_lp: dict = field(default_factory=dict)   # image index -> (logprob, rank, top ids, top logprobs) rows, when it wants them
 
 
 def _plen(req: _Request) -> int:
@@ -320,23 +353,31 @@ class LLM:
             raise ValueError(f"sjd_window needs max_tokens >= 3, got {sp.max_tokens}")
         if not _is_int(sp.n) or not 1 <= sp.n <= self.max_num_seqs:
             raise ValueError(f"SamplingParams.n must be an integer in [1, max_num_seqs = {self.max_num_seqs}], got {sp.n!r}")
+        if sp.logprobs is not None and (not _is_int(sp.logprobs) or not 0 <= sp.logprobs <= _lib.MAX_TOP_LOGPROBS):
+            raise ValueError(f"SamplingParams.logprobs must be None or an integer in [0, {_lib.MAX_TOP_LOGPROBS}], got {sp.logprobs!r}")
+        if sp.best_of is not None and (not _is_int(sp.best_of) or not sp.n <= sp.best_of <= self.max_num_seqs):
+            raise ValueError(f"SamplingParams.best_of must be None or an integer in [n = {sp.n}, max_num_seqs = {self.max_num_seqs}], "
+                             f"got {sp.best_of!r}")
+        if self.sjd_window is not None and _wants_logprobs(sp):
+            raise ValueError("logprobs and best_of cannot be combined with sjd_window")
         return scale, int(interval), None if sp.seed is None else int(sp.seed)
 
     def _guided(self, req: _Request) -> _Request:
         """req with its guidance, seed (None: the LLM's seed + request id) and image count resolved."""
         req.cfg, req.interval, seed = self._guidance(req.params)
         req.seed = self._seed + int(req.request_id) if seed is None else seed
-        req.n = int(req.params.n)
+        req.n = int(req.params.n if req.params.best_of is None else req.params.best_of)
         return req
 
     def _twin_guidance(self, twin_of, sampling_params: Optional[SamplingParams]):
-        """A null-class twin mirrors its conditional request: its params may not carry another cfg_scale, cfg_interval, seed or n."""
+        """A null-class twin mirrors its conditional request: its params may not carry another cfg_scale, cfg_interval, seed, n,
+        logprobs or best_of."""
         owner = self._owner(twin_of)
         sp = sampling_params or SamplingParams()
-        if owner is not None and (sp.cfg_scale, sp.cfg_interval, sp.seed, sp.n) != (owner.params.cfg_scale, owner.params.cfg_interval,
-                                                                                     owner.params.seed, owner.params.n):
-            raise ValueError(f"a null-class twin mirrors its conditional request {twin_of!r}: its cfg_scale, cfg_interval, seed and n "
-                             f"must be the request's")
+        mirror = lambda p: (p.cfg_scale, p.cfg_interval, p.seed, p.n, p.logprobs, p.best_of)   # noqa: E731
+        if owner is not None and mirror(sp) != mirror(owner.params):
+            raise ValueError(f"a null-class twin mirrors its conditional request {twin_of!r}: its cfg_scale, cfg_interval, seed, n, "
+                             f"logprobs and best_of must be the request's")
 
     def _prefix(self, prefix, sampling_params: Optional[SamplingParams]) -> Optional[torch.Tensor]:
         """A request's prefix as int64 [P] on the host, checked as generate(prefix=...) checks it: integer ids in [0, vocab_size),
@@ -463,14 +504,23 @@ class LLM:
         """One draw for each slot in `slots` from logits (its rows, cond rows first) with the slot's seed at token index step_rows:
         result -> st["tok"][slots] and out[slot, step] (out: st["out"] rows from slots.start). Under CFG each slot mixes with its own
         scale and cfg_interval (lg_sample_rows_guided with st["cfg"], st["interval"]), otherwise lg_sample_rows. When a running slot
-        among them holds an image index > 0 (parallel sampling), every slot draws as its image (lg_sample_rows_keyed with st["img"])."""
+        among them holds an image index > 0 (parallel sampling), every slot draws as its image (lg_sample_rows_keyed with st["img"]).
+        While a slot among them wants logprobs, the draw is lg_sample_rows_logprobs into st["lp"] ... at the same index as out."""
         lib, m, n = _lib.load(), self.model, slots.stop - slots.start
         use_cfg = 1 if st["R"] == 2 * self.max_num_seqs else 0
         sc = self._sample_cfg(params)
         dt = _lib.dtype_code(m.tok_embeddings.weight.dtype)   # 16-bit models round the head's logits to their dtype
         head = (_lib.ptr(logits), n, m.vocab_size, use_cfg, dt, ctypes.byref(sc), _lib.ptr(st["seeds"][slots]), _lib.ptr(step_rows))
         tail = (_lib.ptr(st["tok"][slots]), _lib.ptr(out), st["S"], _lib.current_stream(st["dev"]))
-        if any(self._slots[i] is not None and self._img[i] > 0 for i in range(slots.start, slots.stop)):
+        keyed = any(self._slots[i] is not None and self._img[i] > 0 for i in range(slots.start, slots.stop))
+        wants = [self._slots[i].params for i in range(slots.start, slots.stop)
+                 if self._slots[i] is not None and _wants_logprobs(self._slots[i].params)]
+        if wants:
+            spec = self._logprob_spec(st, slots.start, any(p.logprobs for p in wants))
+            guide = (_lib.ptr(st["cfg"][slots]), _lib.ptr(st["interval"][slots])) if use_cfg else (None, None)
+            _lib.check(lib.lg_sample_rows_logprobs(*head, *guide, _lib.ptr(st["img"][slots]) if keyed else None, ctypes.byref(spec), *tail),
+                       "lg_sample_rows_logprobs")
+        elif keyed:
             guide = (_lib.ptr(st["cfg"][slots]), _lib.ptr(st["interval"][slots])) if use_cfg else (None, None)
             _lib.check(lib.lg_sample_rows_keyed(*head, *guide, _lib.ptr(st["img"][slots]), *tail), "lg_sample_rows_keyed")
         elif use_cfg:
@@ -478,6 +528,31 @@ class LLM:
                        "lg_sample_rows_guided")
         else:
             _lib.check(lib.lg_sample_rows(*head, *tail), "lg_sample_rows")
+
+    def _logprob_spec(self, st, row: int, top: bool):
+        """lg_logprobs over the state's logprob rows from slot `row` on (allocated at the first draw that needs them: [B, S], and
+        [B, S, 20] for the alternatives, which a draw asks for whenever a request wants any)."""
+        B, S, dev, N = self.max_num_seqs, st["S"], st["dev"], _lib.MAX_TOP_LOGPROBS
+        if "lp" not in st:
+            st.update(lp=torch.zeros(B, S, dtype=torch.float32, device=dev), rank=torch.zeros(B, S, dtype=torch.int32, device=dev),
+                      top_ids=torch.full((B, S, N), -1, dtype=torch.int32, device=dev),
+                      top_lp=torch.full((B, S, N), -math.inf, dtype=torch.float32, device=dev))
+        return _lib.Logprobs(st["lp"][row].data_ptr(), st["rank"][row].data_ptr(), st["top_ids"][row].data_ptr() if top else 0,
+                             st["top_lp"][row].data_ptr() if top else 0, N if top else 0)
+
+    def _host_rows(self, st, done: List[int]):
+        """The token rows of the slots in `done` on the host, and for each the logprob rows of its request ((logprob, rank, top ids,
+        top logprobs), all [S] / [S, 20]) or None when it did not ask: one device->host copy each."""
+        idx = torch.tensor(done, dtype=torch.long, device=st["dev"])
+        toks = st["out"][idx].cpu().tolist()
+        want = [_wants_logprobs(self._slots[i].params) for i in done]
+        lps: List[Optional[tuple]] = [None] * len(done)
+        if any(want):
+            sel = [j for j, w in enumerate(want) if w]
+            rows = [st[k][idx[sel]].cpu().numpy() for k in ("lp", "rank", "top_ids", "top_lp")]
+            for n, j in enumerate(sel):
+                lps[j] = tuple(r[n] for r in rows)
+        return toks, lps
 
     def _device_decode_t2i(self, st, params: SamplingParams):
         """lg_decode_rows_t2i + a draw (_draw) on every slot: the logits of every row at its own position under its slot's emb-mask, then
@@ -567,16 +642,43 @@ class LLM:
             self._device_copy_kv(st, slots[0], slots[1:], self.model.cls_token_num + P)
             self._device_join_draws(st, params, slots[1:], P)
 
-    def _sample_done(self, i: int, toks: List[int]) -> Optional[_Request]:
-        """Free slot i, whose sample finished with tokens toks; returns its request when that was the request's last sample."""
+    def _sample_done(self, i: int, toks: List[int], lp: Optional[tuple] = None) -> Optional[_Request]:
+        """Free slot i, whose sample finished with tokens toks (and logprob rows lp); returns its request when that was the request's
+        last sample."""
         req = self._slots[i]
         self._slots[i] = None
         req.done[self._img[i]] = toks
+        if lp is not None:
+            req.done_lp[self._img[i]] = lp
         return req if len(req.done) == req.n else None
 
     @staticmethod
     def _completions(req: _Request) -> List[CompletionOutput]:
-        return [CompletionOutput(j, list(req.done[j])) for j in range(req.n)]
+        """The request's outputs: every image in index order, or with best_of the n with the largest cumulative logprob (descending,
+        ties: the lower index first). With logprobs, one dict per token: None for a given prefix token, else the drawn token's Logprob
+        and the N most likely kept tokens' (rank 1 .. N)."""
+        sp, P = req.params, _plen(req)
+        if not _wants_logprobs(sp):
+            return [CompletionOutput(j, list(req.done[j])) for j in range(req.n)]
+        outs = []
+        for j in range(req.n):
+            lp, rank, top_ids, top_lp = req.done_lp[j]
+            toks = list(req.done[j])
+            c = CompletionOutput(j, toks, cumulative_logprob=float(np.sum(lp[P:].astype(np.float64))))
+            if sp.logprobs is not None:
+                N = sp.logprobs
+                lps, ranks, ids, tlps = lp.tolist(), rank.tolist(), top_ids[:, :N].tolist(), top_lp[:, :N].tolist()
+                c.logprobs = [None] * P
+                for k in range(P, len(toks)):
+                    d = {toks[k]: Logprob(lps[k], ranks[k])}
+                    for r, (t, x) in enumerate(zip(ids[k], tlps[k])):
+                        if t >= 0:
+                            d.setdefault(t, Logprob(x, r + 1))
+                    c.logprobs.append(d)
+            outs.append(c)
+        if sp.best_of is not None:
+            outs = sorted(outs, key=lambda c: (-c.cumulative_logprob, c.index))[:sp.n]
+        return outs
 
     # ------------------------------------------------------------------ speculative Jacobi decoding (sjd_window)
     def _sjd_scratch(self, st):
@@ -724,13 +826,13 @@ class LLM:
         outs: List[RequestOutput] = []
         if done:
             idx = torch.tensor(done, dtype=torch.long, device=dev)
-            toks = st["out"][idx].cpu().tolist()
+            toks, lps = self._host_rows(st, done)
             rows = torch.cat([idx, idx + B]) if R == 2 * B else idx
             st["active"][rows] = 0
             st["pos"][rows] = 0
             st["step"][idx] = 0                                # a free slot's draw goes to out[slot, 0], which its next request rewrites
-            for i, t in zip(done, toks):
-                req = self._sample_done(i, t)
+            for i, t, lp in zip(done, toks, lps):
+                req = self._sample_done(i, t, lp)
                 if req is not None:
                     outs.append(RequestOutput(req.request_id, [], self._completions(req), True))
         return outs
@@ -808,15 +910,16 @@ class LLM:
         outs: List[RequestOutput] = []
         if done:
             idx = torch.tensor(done, dtype=torch.long, device=dev)
-            if toks is None:
-                toks = st["out"][idx].cpu().tolist()          # the only device->host copy: token rows of finished requests
+            lps = [None] * len(done)
+            if toks is None:                                  # the only device->host copy: token (and logprob) rows of finished requests
+                toks, lps = self._host_rows(st, done)
             rows = torch.cat([idx, idx + B]) if R == 2 * B else idx
             st["active"][rows] = 0
             st["pos"][rows] = 0
             st["tok"][idx] = 0                                # a free slot sits at position 0 = the class branch: its input must be a valid
                                                               # class id, not the last sampled token (which indexed past the class table)
-            for i, t in zip(done, toks):
-                req = self._sample_done(i, t)
+            for i, t, lp in zip(done, toks, lps):
+                req = self._sample_done(i, t, lp)
                 if req is None:
                     continue
                 outs.append(RequestOutput(req.request_id, req.prompt_token_ids, self._completions(req), True))
