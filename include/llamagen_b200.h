@@ -284,6 +284,31 @@ int  lg_generate_prefix(lg_engine* e, const void* cond, const float* emb_mask, i
                         const int32_t* prefix, int P, void* dev_ws, size_t ws_bytes, int32_t* out_tokens, float* dbg_logits,
                         void* stream);
 
+/* ---- inpainting: generate() that keeps any given tokens of every image and draws the rest ----------------------------------------
+ * given: HOST int32 [B, S]; given[b][k] in [0, vocab_size) is image b's token k, -1 means token k of image b is drawn. At least one
+ * token must be drawn. The call cuts [0, S) into segments, one rule and no option:
+ *   LEAD    the leading run of tokens given to every image (length P >= 0): prefilled with the condition in one pass, as
+ *           lg_generate_prefix (P > 0) or lg_generate (P = 0) prefill; its head draws token P;
+ *   DECODE  one decode step (lg_generate's graph, fused tail and chains) per token that some image draws; images whose token is
+ *           given there take it;
+ *   EXTEND  each interior run of K tokens given to every image: one window pass feeds tokens k .. k + K (k: the drawn token before the
+ *           run) at positions T + k .. in chunks of at most 64 rows, writes their K / V, and the head over its last row gives the
+ *           logits of token k + K + 1;
+ *   TAIL    a trailing run given to every image: copied, no forward pass.
+ * A drawn token k of image b is drawn as lg_generate draws it (RNG key (seed, b, k), cfg_interval by token index, the same
+ * temperature / top-k / top-p), from logits that have seen every token before k, given or drawn; never a given token after k.
+ * out_tokens dev int32 [B, S]: given tokens where given, drawn ones elsewhere. A mask that gives only a leading run of P tokens is
+ * lg_generate_prefix's call, and one that gives nothing is lg_generate's, bit for bit. neg_cond, neg_mask: NULL, or a negative
+ * prompt as for lg_generate_neg. dev_ws: 256-byte aligned, lg_given_workspace_bytes of this given array; the call uploads given into
+ * it once, on `stream` before any other work of the call, from the engine's pinned staging buffer: the host waits only until the
+ * previous call's upload has read that buffer, never for the rest of the stream. Bytes past what lg_given_workspace_bytes counts before the prefill go to the prefill, which runs in chunks of rows as
+ * lg_generate_prefix's does (at least one image's rows must fit). Every argument is checked before any launch; the workspace needs
+ * rows >= nh * B and max_seq >= T + S. */
+int  lg_given_workspace_bytes(lg_engine* e, const int32_t* given, int B, int S, int use_cfg, size_t* bytes);
+int  lg_generate_given(lg_engine* e, const void* cond, const float* emb_mask, const void* neg_cond, const float* neg_mask, int B, int T,
+                       int S, const lg_sample_cfg* sc, const int32_t* given, void* dev_ws, size_t ws_bytes, int32_t* out_tokens,
+                       void* stream);
+
 /* ---- teacher-forced scoring: Transformer.forward(idx, cond_idx, targets) (gpt.py:341-382, eval mode) ----------------------- */
 /* Bytes of caller-provided scratch for lg_score over `rows` sequences (rows = 2B under CFG) of `seq` positions (T + S - 1). */
 int  lg_score_workspace_bytes(lg_engine* e, int rows, int seq, size_t* bytes);
@@ -526,6 +551,17 @@ int  lg_test_attention_plan(int dtype, int kv_dtype, int R, int Tq, int H, int h
 /* Chunks the prefill of the engine's last lg_generate_prefix call ran in (over all chains); -1 for a null engine. chains: NULL or
  * receives the number of decode chains that call ran (1, or 2 under a multi-chain split). */
 int  lg_test_prefix_chunks(lg_engine* e, int* chains);
+/* Test hook: the segments of lg_generate_given's plan for given (host int32 [B, S]) as {kind (0 LEAD, 1 DECODE, 2 EXTEND, 3 TAIL),
+ * start, length} triples, the first max_segs of them into segs_out; returns the number of segments, or -1. DECODE [start, start +
+ * length) draws those tokens; EXTEND [start, start + length) holds the given run and draws token start + length; LEAD [0, length)
+ * draws token length. */
+int  lg_test_given_plan(const int32_t* given, int B, int S, int32_t* segs_out, int max_segs);
+/* Test hook: lg_sample_rows (seed_rows, step_rows dev, as there) with the inpainting select: given dev int32 [B, seq_stride]; where
+ * given[b][step_rows[b]] >= 0 that token replaces image b's draw in out_idx (NULL allowed), out_seq (dev [B, seq_stride]) and
+ * next_tokens (dev [B] or NULL). Given all -1, every draw is lg_sample_rows' draw. */
+int  lg_test_sample_given(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc,
+                          const uint64_t* seed_rows, const int32_t* step_rows, const int32_t* given, int32_t* out_idx, int32_t* out_seq,
+                          int seq_stride, int32_t* next_tokens, void* stream);
 /* The acceptance step of lg_generate_sjd alone, on caller buffers (dev): p, q f32 [B * L][V], qflag, x, win int32 [B * L], nfin,
  * start int32 [B] (updated), out int32 [B][S] (accepted tokens written). Every image must have nfin < S. */
 int  lg_test_sjd_verify(int B, int S, int L, int V, int greedy, uint64_t seed, const float* p, const float* q, const int32_t* qflag,

@@ -112,6 +112,12 @@ SIGNATURES = {
     "lg_generate_prefix": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p, c_int, c_void_p,
                                    c_size_t, c_void_p, c_void_p, c_void_p]),
     "lg_test_prefix_chunks": (c_int, [c_void_p, POINTER(c_int)]),
+    "lg_given_workspace_bytes": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_size_t)]),
+    "lg_generate_given": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p,
+                                  c_void_p, c_size_t, c_void_p, c_void_p]),
+    "lg_test_given_plan": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int]),
+    "lg_test_sample_given": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p, c_void_p, c_void_p, c_void_p,
+                                     c_void_p, c_int, c_void_p, c_void_p]),
     "lg_score_workspace_bytes": (c_int, [c_void_p, c_int, c_int, POINTER(c_size_t)]),
     "lg_score": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_size_t,
                          c_void_p, c_void_p, c_void_p]),

@@ -288,6 +288,21 @@ struct lg_engine {
     int prefix_chains = 0;                // decode chains of that call
     int* sjd_done_host = nullptr;         // pinned copy of lg_generate_sjd's done flag
     cudaEvent_t ev_pass[2] = {};
+    int32_t* given_host = nullptr;        // lg_generate_given's pinned staging of the head of its scratch (given_host_bytes)
+    size_t given_host_bytes = 0;
+    cudaEvent_t ev_given = nullptr;       // the last upload from given_host has been read
+    // given_host with room for `bytes`, once the previous upload from it has read it
+    int stage_given(size_t bytes) {
+        if (!ev_given) LG_CUDA_OK(cudaEventCreateWithFlags(&ev_given, cudaEventDisableTiming));
+        else LG_CUDA_OK(cudaEventSynchronize(ev_given));
+        if (bytes <= given_host_bytes) return 0;
+        if (given_host) LG_CUDA_OK(cudaFreeHost(given_host));
+        given_host = nullptr;
+        given_host_bytes = 0;
+        LG_CUDA_OK(cudaHostAlloc((void**)&given_host, bytes, cudaHostAllocDefault));
+        given_host_bytes = bytes;
+        return 0;
+    }
     ~lg_engine() {
         for (int i = 0; i < kMaxChains; ++i) {
             if (works[i]) cudaStreamDestroy(works[i]);
@@ -298,6 +313,8 @@ struct lg_engine {
         for (cudaEvent_t ev : ev_pass)
             if (ev) cudaEventDestroy(ev);
         if (sjd_done_host) cudaFreeHost(sjd_done_host);
+        if (given_host) cudaFreeHost(given_host);
+        if (ev_given) cudaEventDestroy(ev_given);
     }
     // the engine-owned streams the loops run on, created on first use
     int ensure_streams() {
@@ -350,6 +367,7 @@ struct lg_engine {
     size_t carve_sjd_slots(RowBuffers& o, SjdArgs& sa, char* base, int B, int nh, int L) const;
     size_t carve_prefix(RowBuffers& o, char* base, int rows, int seq) const;
     size_t carve_slot(RowBuffers& head, char* base, int nh, int seq) const;
+    size_t carve_given_window(RowBuffers& o, int32_t** win, int32_t** pos_rows, char* base, int B, int nh, int W) const;
     void carve_kv(Carver& c, KvCache& o, int rows, int max_seq, int layers, bool f8) const;
     void carve_rows(Carver& c, RowBuffers& o, size_t M, size_t x0_rows, size_t partial_floats, size_t logits_rows) const;
     // the most partial floats one of a layer's four GEMMs needs at M rows
@@ -518,6 +536,21 @@ size_t lg_engine::carve_slot(RowBuffers& head, char* base, int nh, int seq) cons
     head.q = c.split((size_t)nh * D * esz);
     head.partial_floats = std::max(gemm_partial_floats(nh, V, D, 0, dt), gemm_partial_floats(nh, V, D, 0, dt, output.scale != nullptr));
     head.partial = (float*)c.split(head.partial_floats * sizeof(float));
+    return c.off;
+}
+
+// lg_generate_given's extend pass of one chain of B images (nh rows each), from `base` (null: sizes only): the row buffers of nh * B
+// windows of W rows, the GEMM partials of that M and of the head over the nh * B last rows, then the window's tokens [B, W] and its
+// rows' positions [nh * B]. The K / V rows go to the chain's cache, the logits to its row buffers.
+size_t lg_engine::carve_given_window(RowBuffers& o, int32_t** win, int32_t** pos_rows, char* base, int B, int nh, int W) const {
+    const int R = nh * B, V = cfg.vocab_size, D = cfg.dim, dt = cfg.dtype;
+    const size_t M = (size_t)R * W;
+    const size_t pf = std::max({layer_partial_floats((int)M), gemm_partial_floats(R, V, D, 0, dt),
+                                gemm_partial_floats(R, V, D, 0, dt, output.scale != nullptr)});
+    Carver c{base};
+    carve_rows(c, o, M, 0, pf, 0);
+    *win = (int32_t*)c.split((size_t)B * W * sizeof(int32_t));
+    *pos_rows = (int32_t*)c.split((size_t)R * sizeof(int32_t));
     return c.off;
 }
 
@@ -1105,17 +1138,82 @@ int lg_sample(const float* logits, int B, int V, int mix_cfg, int round_dtype, c
     return launch_sample(a, (cudaStream_t)stream);
 }
 
+// The segments generate_impl runs, in token order. A plan starts with one LEAD and draws every token that is not given to all images:
+//   LEAD   [0, len): tokens given to every image, prefilled with the condition in one pass (len = 0: the condition alone); its head
+//          draws token len
+//   DECODE [start, start + len): one decode step per token; images with a given token there take it
+//   EXTEND [start, start + len): tokens given to every image between two drawn ones; one window pass over tokens start - 1 ..
+//          start + len - 1 writes their K / V, and its last row's head draws token start + len
+//   TAIL   [start, S): tokens given to every image after the last drawn one; no forward pass
+enum GivenSegKind { kSegLead = 0, kSegDecode = 1, kSegExtend = 2, kSegTail = 3 };
+struct GivenSeg {
+    int kind, start, len;
+};
+constexpr int kGivenWindowRows = 64;   // rows of an extend pass's window chunk per image (the windowed tensor-core attention's limit)
+
+// The plan of given [B, S] (host, -1: drawn), or an error when every token is given or a value is below -1
+static int given_plan(const char* fn, const int32_t* given, int B, int S, std::vector<GivenSeg>& segs) {
+    std::vector<char> all(S, 1);   // token k is given to every image
+    for (int b = 0; b < B; ++b)
+        for (int k = 0; k < S; ++k) {
+            const int32_t v = given[(size_t)b * S + k];
+            LG_REQUIRE(v >= -1, "%s: given[%d][%d] = %d (token ids, or -1 for a drawn token)", fn, b, k, v);
+            if (v < 0) all[k] = 0;
+        }
+    int P = 0;
+    while (P < S && all[P]) ++P;
+    LG_REQUIRE(P < S, "%s: every token is given; nothing to draw", fn);
+    segs.clear();
+    segs.push_back({kSegLead, 0, P});
+    for (int k = P + 1; k < S;) {
+        const int a = k;
+        const char g = all[k];
+        while (k < S && all[k] == g) ++k;
+        if (!g) segs.push_back({kSegDecode, a, k - a});
+        else if (k == S) segs.push_back({kSegTail, a, k - a});
+        else segs.push_back({kSegExtend, a, k++ - a});   // the window draws token k
+    }
+    return 0;
+}
+
+// The rows of the longest extend window of a plan, capped at one chunk (0: no extend)
+static int given_window_rows(const std::vector<GivenSeg>& segs) {
+    int W = 0;
+    for (const GivenSeg& s : segs)
+        if (s.kind == kSegExtend) W = std::max(W, std::min(s.len + 1, kGivenWindowRows));
+    return W;
+}
+
 struct PrefixArgs {              // lg_generate_prefix: prefix [B, P] and the prefill's scratch (P = 0: lg_generate)
     const int32_t* prefix = nullptr;
     int P = 0;
     char* scratch = nullptr;
     size_t scratch_bytes = 0;
+    // lg_generate_given: the plan (null: LEAD P, then DECODE to the end), the given tokens dev [B, S] (-1: drawn) and the extend
+    // passes' scratch (given_window_bytes) for window chunks of W rows
+    const std::vector<GivenSeg>* segs = nullptr;
+    const int32_t* given = nullptr;
+    char* window = nullptr;
+    int W = 0;
 };
 static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, const Negative& neg, int B, int T, int S,
                          const lg_sample_cfg* sc, int32_t* out_tokens, float* dbg_logits, const int32_t* teacher,
                          const PrefixArgs& pa, const lg_logprobs* lp, cudaStream_t st);
 
 }  // extern "C"
+
+// Bytes of the extend passes' scratch for B images (nh rows each) and window chunks of W rows: the windows of every chain, one after
+// the other, for each chain count generate_impl may run (0 without an extend)
+static size_t given_window_bytes(const lg_engine* e, int B, int nh, int W) {
+    size_t most = 0;
+    for (int n = 1; W > 0 && n <= lg_engine::kMaxChains; ++n) {
+        if (B % n) continue;
+        RowBuffers rb;
+        int32_t *win, *pos;
+        most = std::max(most, n * e->carve_given_window(rb, &win, &pos, nullptr, B / n, nh, W));
+    }
+    return most;
+}
 
 static int generate_entry(const char* fn, lg_engine* e, const void* cond, const float* emb_mask, const Negative& neg, int B, int T, int S,
                           const lg_sample_cfg* sc, int32_t* out_tokens, float* dbg_logits, const int32_t* teacher, void* stream,
@@ -1207,6 +1305,99 @@ int lg_test_prefix_chunks(lg_engine* e, int* chains) {
     return e->prefix_chunks;
 }
 
+}  // extern "C"
+
+// lg_generate_given's scratch before the prefill's: the given tokens [B, S], the leading run [B, P] and the extend passes' windows
+static size_t given_fixed_bytes(const lg_engine* e, int B, int S, int nh, int P, int W) {
+    return align_up((size_t)B * S * sizeof(int32_t)) + align_up((size_t)B * P * sizeof(int32_t)) + given_window_bytes(e, B, nh, W);
+}
+
+// The checks lg_generate_given and lg_given_workspace_bytes (fn) make of given [B, S] (host) before any launch, then its plan and the
+// bytes of its scratch: fixed (given_fixed_bytes) and the prefill's (lg_prefix_workspace_bytes of every row, 0 without a LEAD)
+static int given_layout(const char* fn, const lg_engine* e, const int32_t* given, int B, int S, int nh, std::vector<GivenSeg>& segs,
+                        size_t* fixed, size_t* prefill) {
+    const lg_model_cfg& c = e->cfg;
+    LG_REQUIRE(given, "%s: null given", fn);
+    LG_REQUIRE(B > 0 && S >= 1 && S <= c.block_size, "%s: B=%d, or S=%d outside [1, block_size=%d]", fn, B, S, c.block_size);
+    for (size_t i = 0; i < (size_t)B * S; ++i)
+        LG_REQUIRE(given[i] < c.vocab_size, "%s: given[%zu][%zu] = %d is not below vocab_size=%d", fn, i / S, i % S, given[i],
+                   c.vocab_size);
+    LG_TRY(given_plan(fn, given, B, S, segs));
+    const int P = segs[0].len, W = given_window_rows(segs);
+    LG_REQUIRE((long long)nh * B * W <= 65535, "%s: %d rows x window %d exceed 65535 query rows", fn, nh * B, W);
+    *fixed = given_fixed_bytes(e, B, S, nh, P, W);
+    RowBuffers rb;
+    *prefill = P > 0 ? e->carve_prefix(rb, nullptr, nh * B, c.cls_token_num + P) : 0;
+    return 0;
+}
+
+extern "C" {
+
+int lg_given_workspace_bytes(lg_engine* e, const int32_t* given, int B, int S, int use_cfg, size_t* bytes) {
+    LG_REQUIRE(e && bytes, "lg_given_workspace_bytes: null argument");
+    std::vector<GivenSeg> segs;
+    size_t fixed = 0, prefill = 0;
+    LG_TRY(given_layout("lg_given_workspace_bytes", e, given, B, S, use_cfg ? 2 : 1, segs, &fixed, &prefill));
+    *bytes = fixed + prefill;
+    return 0;
+}
+
+int lg_generate_given(lg_engine* e, const void* cond, const float* emb_mask, const void* neg_cond, const float* neg_mask, int B, int T, int S,
+                      const lg_sample_cfg* sc, const int32_t* given, void* dev_ws, size_t ws_bytes, int32_t* out_tokens, void* stream) {
+    static const char* fn = "lg_generate_given";
+    LG_REQUIRE(e && e->finalized, "%s: engine not finalized", fn);
+    const lg_model_cfg& c = e->cfg;
+    LG_REQUIRE(cond && sc && out_tokens, "%s: null cond, sc or out_tokens", fn);
+    LG_REQUIRE(T == c.cls_token_num, "%s: T=%d must equal cls_token_num=%d", fn, T, c.cls_token_num);
+    LG_REQUIRE(!emb_mask || c.model_type == LG_MODEL_T2I, "%s: emb_mask only applies to t2i models", fn);
+    const int nh = sc->cfg_scale > 1.0f ? 2 : 1;   // generate.py:128
+    const Negative neg{neg_cond, neg_mask};
+    LG_TRY(check_negative(fn, e, neg, emb_mask, nh == 2));
+    std::vector<GivenSeg> segs;
+    size_t fixed = 0, prefill = 0;
+    LG_TRY(given_layout(fn, e, given, B, S, nh, segs, &fixed, &prefill));
+    const int P = segs[0].len, W = given_window_rows(segs);
+    LG_TRY(check_ready(e, nh * B, T + S));
+    LG_REQUIRE(dev_ws && ((uintptr_t)dev_ws & 255) == 0, "%s: scratch must be non-null and 256-byte aligned", fn);
+    RowBuffers one;
+    const size_t need1 = fixed + (P > 0 ? e->carve_prefix(one, nullptr, nh, T + P) : 0);
+    LG_REQUIRE(ws_bytes >= need1, "%s: scratch of %zu bytes is too small (%zu with the prefill of one image)", fn, ws_bytes, need1);
+    // the scratch: given [B, S], the leading run [B, P], the extend windows, then the prefill's activations
+    char* base = (char*)dev_ws;
+    int32_t* given_dev = (int32_t*)base;
+    int32_t* lead_dev = (int32_t*)(base + align_up((size_t)B * S * sizeof(int32_t)));
+    PrefixArgs pa{P > 0 ? lead_dev : nullptr, P, base + fixed, ws_bytes - fixed};
+    pa.segs = &segs; pa.given = given_dev; pa.W = W;
+    pa.window = (char*)lead_dev + align_up((size_t)B * P * sizeof(int32_t));
+    DeviceGuard guard(e->device);
+    // given [B, S] and the leading run [B, P] go up in one copy from the engine's pinned staging buffer (laid out as the scratch's head,
+    // so the host never waits for earlier work on the stream), then out_tokens starts as given: every drawn token overwrites its -1.
+    // The copies run on the caller's stream before the fork, so every chain's stream is ordered after them.
+    const cudaStream_t caller = (cudaStream_t)stream;
+    const size_t up = (char*)lead_dev - base + (size_t)B * P * sizeof(int32_t);
+    LG_TRY(e->stage_given(up));
+    std::copy(given, given + (size_t)B * S, e->given_host);
+    int32_t* lead_host = e->given_host + ((char*)lead_dev - base) / sizeof(int32_t);
+    for (int b = 0; b < B; ++b) std::copy(given + (size_t)b * S, given + (size_t)b * S + P, lead_host + (size_t)b * P);
+    LG_CUDA_OK(cudaMemcpyAsync(base, e->given_host, up, cudaMemcpyHostToDevice, caller));
+    LG_CUDA_OK(cudaEventRecord(e->ev_given, caller));
+    LG_CUDA_OK(cudaMemcpyAsync(out_tokens, given_dev, (size_t)B * S * sizeof(int32_t), cudaMemcpyDeviceToDevice, caller));
+    return e->run_forked(caller, lg_engine::kMaxChains, [&](cudaStream_t st) {
+        return generate_impl(e, cond, emb_mask, neg, B, T, S, sc, out_tokens, nullptr, nullptr, pa, nullptr, st);
+    });
+}
+
+int lg_test_given_plan(const int32_t* given, int B, int S, int32_t* segs_out, int max_segs) {
+    static const char* fn = "lg_test_given_plan";
+    LG_REQUIRE(given && B > 0 && S > 0 && (segs_out || max_segs == 0) && max_segs >= 0, "%s: bad argument", fn);
+    std::vector<GivenSeg> segs;
+    LG_TRY(given_plan(fn, given, B, S, segs));
+    for (int i = 0; i < (int)segs.size() && i < max_segs; ++i) {
+        segs_out[3 * i] = segs[i].kind; segs_out[3 * i + 1] = segs[i].start; segs_out[3 * i + 2] = segs[i].len;
+    }
+    return (int)segs.size();
+}
+
 namespace {
 // One independent decode chain (a contiguous group of images with its own workspace view, stream and graph).
 struct Chain {
@@ -1219,6 +1410,9 @@ struct Chain {
     int B = 0, R = 0;
     SampleArgs sa{};
     Graph graph;
+    RowBuffers win;                    // the extend passes' row buffers (lg_generate_given)
+    int32_t* win_tokens = nullptr;     // [B, W]
+    int32_t* win_pos = nullptr;        // [R]
 };
 }  // namespace
 
@@ -1397,8 +1591,19 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
         sa.row_offset = (int)boff;
         sa.out_seq = out_tokens + boff * S; sa.seq_stride = S; sa.next_tokens = k.w.tokens;
         sa.teacher = teacher ? teacher + boff * S : nullptr;
+        sa.given = pa.given ? pa.given + boff * S : nullptr;
         sa.dbg_logits = dbg_logits; sa.dbg_batch = B;
         apply_logprobs(sa, lp, boff * S);
+    }
+    std::vector<GivenSeg> lead_decode;   // lg_generate and lg_generate_prefix: LEAD P, then one DECODE run to the end
+    if (!pa.segs) {
+        lead_decode.push_back({kSegLead, 0, pa.P});
+        if (S > pa.P + 1) lead_decode.push_back({kSegDecode, pa.P + 1, S - pa.P - 1});
+    }
+    const std::vector<GivenSeg>& segs = pa.segs ? *pa.segs : lead_decode;
+    for (int g = 0, off = 0; pa.W > 0 && g < nchains; ++g) {
+        Chain& k = ch[g];
+        off += (int)e->carve_given_window(k.win, &k.win_tokens, &k.win_pos, pa.window + off, k.B, use_cfg ? 2 : 1, pa.W);
     }
 
     // Fused tail (bf16 / fp16): the sample kernel writes the next step's input rows (token embedding, and on the batched path the layer-0
@@ -1424,6 +1629,30 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
         LG_PROF(PC_SAMPLE, k.st, launch_sample(k.sa, k.st));
         if (!fuse_tail) LG_PROF(PC_EMBED_MISC, k.st, launch_advance(d_pos, d_step, k.st));
         return 0;
+    };
+    // An extend pass (lg_generate_given): tokens a - 1 .. a + K - 1 of every row, at positions T + a - 1 .., through the layers in
+    // window chunks of at most pa.W rows (their K / V go to the chain's cache); the head over the last row of every image's window
+    // gives the logits of token a + K, which is drawn (or taken as given) with its own step, and the counters move past it
+    auto extend = [&](Chain& k, int a, int K) -> int {
+        const int D = c.dim, dt = c.dtype, nh = use_cfg ? 2 : 1;
+        Workspace w;
+        static_cast<KvCache&>(w) = k.w;
+        static_cast<RowBuffers&>(w) = k.win;
+        int n = 0;
+        for (int c0 = 0; c0 < K + 1; c0 += n) {
+            n = std::min(pa.W, K + 1 - c0);
+            const int j0 = a - 1 + c0;
+            LG_TRY(launch_given_window(k.w.tokens, k.sa.given, k.B, nh, S, j0, n, c0 == 0, T + j0, k.win_tokens, k.win_pos, k.st));
+            LG_PROF(PC_EMBED_MISC, k.st, launch_embed(e->tok_emb, k.win_tokens, k.B * n, k.R * n, -1, D, dt, w.h, k.st));
+            LG_TRY(e->run_layers(w, k.R * n, n, PosArg{nullptr, 0, k.win_pos}, k.emb_mask, k.neg.mask, k.B, false, k.st));
+        }
+        LG_TRY(launch_gather_last(w.xn, k.R, n, D, dt, w.q, k.st));
+        GemmNext nx_first{e->layers[0].wqkv.p, e->layers[0].wqkv.bytes(3 * D, D, e->esz), nullptr, 0};
+        LG_TRY(e->head(w, w.q, k.R, k.w.logits, &nx_first, k.st));
+        SampleArgs sa = k.sa;   // the decode step's draw at a fixed step; the counters are set, not advanced
+        sa.step = a + K; sa.step_dev = nullptr; sa.adv_pos = nullptr; sa.adv_step = nullptr; sa.adv_ticket = nullptr;
+        LG_PROF(PC_SAMPLE, k.st, launch_sample(sa, k.st));
+        return launch_set_counters(k.w.counters, T + a + K, k.w.counters + 1, a + K + 1, k.st);
     };
 
     // ---- prefix prefill (lg_generate_prefix): tokens 0 .. P - 1 are the prefix; every chain's prefill shares the one scratch, so all
@@ -1470,21 +1699,32 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
         LG_TRY(launch_set_counters(k.w.counters, T + P, k.w.counters + 1, P + 1, k.st));
         k.sa.step_dev = k.w.counters + 1;
         if (tail) arm_tail(k, true);
-        LG_TRY(body(k));   // first decode step runs eagerly (also sets every kernel attribute outside capture)
     }
-    const int remaining = S - P - 2;
-    if (remaining <= 0) return 0;
-    if (!e->use_graph || remaining < 3 || prof_enabled() || lg_debug_sync()) {
-        for (int i = 0; i < remaining; ++i)
-            for (int g = 0; g < nchains; ++g) LG_TRY(body(ch[g]));
-        return 0;
+    // ---- the plan's other segments, every chain in turn. The first decode step runs eagerly (it also sets every kernel attribute
+    // outside capture); the later ones replay, per chain, one captured graph of one decode step (generate.py:105-123; the loop state is
+    // device-resident, so every step has identical kernel arguments), chains interleaved: with two chains the gap between graph
+    // launches of one chain is covered by the other chain's kernels.
+    int remaining = -1;   // decode steps after the first
+    for (const GivenSeg& sg : segs)
+        if (sg.kind == kSegDecode) remaining += sg.len;
+    const bool graph = e->use_graph && remaining >= 3 && !prof_enabled() && !lg_debug_sync();
+    bool eager_done = false, captured = false;
+    for (const GivenSeg& sg : segs) {
+        if (sg.kind == kSegExtend)
+            for (int g = 0; g < nchains; ++g) LG_TRY(extend(ch[g], sg.start, sg.len));
+        if (sg.kind != kSegDecode) continue;
+        for (int i = 0; i < sg.len; ++i) {
+            if (!eager_done || !graph) {
+                for (int g = 0; g < nchains; ++g) LG_TRY(body(ch[g]));
+                eager_done = true;
+                continue;
+            }
+            if (!captured)
+                for (int g = 0; g < nchains; ++g) LG_TRY(ch[g].graph.capture(ch[g].st, [&] { return body(ch[g]); }));
+            captured = true;
+            for (int g = 0; g < nchains; ++g) LG_TRY(ch[g].graph.launch(ch[g].st));
+        }
     }
-    // ---- decode loop (generate.py:105-123): per chain one captured graph of one decode step (the loop state is
-    // device-resident, so every step has identical kernel arguments), replayed, chains interleaved: with two chains the
-    // gap between graph launches of one chain is covered by the other chain's kernels.
-    for (int g = 0; g < nchains; ++g) LG_TRY(ch[g].graph.capture(ch[g].st, [&] { return body(ch[g]); }));
-    for (int i = 0; i < remaining; ++i)
-        for (int g = 0; g < nchains; ++g) LG_TRY(ch[g].graph.launch(ch[g].st));
     return 0;
 }
 
@@ -1841,6 +2081,18 @@ int lg_test_sample(const float* logits, int B, int V, int mix_cfg, int round_dty
     LG_CUDA_OK(cudaStreamSynchronize(st));
     LG_REQUIRE(left == 0, "%s: the counter ticket was left at %u", fn, left);
     return 0;
+}
+
+int lg_test_sample_given(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc, const uint64_t* seed_rows,
+                         const int32_t* step_rows, const int32_t* given, int32_t* out_idx, int32_t* out_seq, int seq_stride,
+                         int32_t* next_tokens, void* stream) {
+    static const char* fn = "lg_test_sample_given";
+    LG_REQUIRE(logits && sc && seed_rows && step_rows && given && out_seq && seq_stride > 0, "%s: null argument or seq_stride=%d", fn,
+               seq_stride);
+    SampleArgs a = make_sample_args(*sc, logits, B, V, mix_cfg, round_dtype);
+    a.seed_rows = seed_rows; a.step_rows = step_rows; a.given = given;
+    a.out_idx = out_idx; a.out_seq = out_seq; a.seq_stride = seq_stride; a.next_tokens = next_tokens;
+    return launch_sample(a, (cudaStream_t)stream);
 }
 
 int lg_test_score_head(const float* partial, int ks, int P, int V, int nh, float cfg_scale, int dtype, const int32_t* targets,

@@ -63,6 +63,9 @@ struct SampleArgs {
     int32_t* top_ids = nullptr;            // the top_n kept tokens by (x desc, id asc); -1 past the kept ones
     float* top_lp = nullptr;               // their logprobs; -inf past the kept ones
     int top_n = 0;                         // 0 .. kMaxTopLogprobs
+    // inpainting (lg_generate_given): [B, seq_stride] or null; a value >= 0 at element b * seq_stride + step is image b's given token
+    // there: it goes to out_idx, out_seq, next_tokens and the fused tail in place of the draw (-1: the draw)
+    const int32_t* given = nullptr;
 };
 constexpr int kMaxTopLogprobs = 20;
 inline bool sample_wants_logprobs(const SampleArgs& a) { return a.lp_out || a.rank_out || a.top_ids || a.top_lp; }
@@ -74,6 +77,11 @@ int launch_sample(const SampleArgs& a, cudaStream_t st);
 // Logprob rows of given tokens (lg_generate_logprobs' prefix): element b * S + k, k < P, of every non-null array gets logprob 0, rank 0,
 // top ids -1 and top logprobs -inf
 int launch_given_logprobs(float* lp, int32_t* rank, int32_t* top_ids, float* top_lp, int top_n, int B, int S, int P, cudaStream_t st);
+// One chunk of an inpainting window (lg_generate_given's extend pass): image b's rows feed tokens j0 .. j0 + n - 1, token j0 from
+// tokens[b] when `from_tokens` (the token the previous sample fed forward), the others from given [B, S]; win [B, n] gets them and
+// pos_rows [nh * B] the position T + j0 of the chunk's first row (CFG twins included)
+int launch_given_window(const int32_t* tokens, const int32_t* given, int B, int nh, int S, int j0, int n, int from_tokens, int pos0,
+                        int32_t* win, int32_t* pos_rows, cudaStream_t st);
 
 // Speculative Jacobi decoding (lg_generate_sjd). Image b's window has L slots; slot i feeds token start[b] + i - 1 (win) and its
 // output p (the sample kernel's out_probs) is the distribution of token start[b] + i. Rows of image b are b * L + i.

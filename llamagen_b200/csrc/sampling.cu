@@ -519,7 +519,11 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
     }
     __shared__ int s_next;
     if (tid == 0) {
-        const int pick = s_pick;
+        int pick = s_pick;
+        if (a.given) {   // a given token of an inpainting call replaces the draw
+            const int g = a.given[(size_t)b * a.seq_stride + step];
+            if (g >= 0) pick = g;
+        }
         if (a.out_idx) a.out_idx[b] = pick;
         if (a.out_seq) a.out_seq[(size_t)b * a.seq_stride + step] = pick;
         const int nxt = a.teacher ? a.teacher[(size_t)b * a.seq_stride + step] : pick;
@@ -626,6 +630,27 @@ int launch_given_logprobs(float* lp, int32_t* rank, int32_t* top_ids, float* top
     LG_REQUIRE(B > 0 && P >= 0 && P <= S && top_n >= 0, "given logprobs: bad shape B=%d S=%d P=%d top_n=%d", B, S, P, top_n);
     if (P == 0) return 0;
     (void)lg_launch(given_logprobs_kernel, dim3(B), dim3(128), 0, st, lp, rank, top_ids, top_lp, top_n, S, P);
+    LG_LAUNCH_CHECK();
+    return 0;
+}
+
+namespace {
+__global__ void given_window_kernel(const int32_t* tokens, const int32_t* given, int B, int nh, int S, int j0, int n, int from_tokens,
+                                    int pos0, int32_t* win, int32_t* pos_rows) {
+    lg_pdl_sync();
+    const int b = blockIdx.x;
+    for (int i = threadIdx.x; i < n; i += blockDim.x)
+        win[(size_t)b * n + i] = i == 0 && from_tokens ? tokens[b] : given[(size_t)b * S + j0 + i];
+    if (threadIdx.x == 0)
+        for (int h = 0; h < nh; ++h) pos_rows[h * B + b] = pos0;
+}
+}  // namespace
+
+int launch_given_window(const int32_t* tokens, const int32_t* given, int B, int nh, int S, int j0, int n, int from_tokens, int pos0,
+                        int32_t* win, int32_t* pos_rows, cudaStream_t st) {
+    LG_REQUIRE(B > 0 && (nh == 1 || nh == 2) && n >= 1 && j0 >= 0 && j0 + n <= S, "given window: bad shape B=%d nh=%d S=%d j0=%d n=%d", B,
+               nh, S, j0, n);
+    (void)lg_launch(given_window_kernel, dim3(B), dim3(64), 0, st, tokens, given, B, nh, S, j0, n, from_tokens, pos0, win, pos_rows);
     LG_LAUNCH_CHECK();
     return 0;
 }

@@ -61,6 +61,18 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
                            prefix are 0, so logprobs.sum(1) is the cumulative logprob of the drawn tokens. The tokens are those of the
                            same call without it. Works on the plain, CFG, negative and prefix paths; not with sjd_window, teacher (use
                            score() for given tokens) or return_logits.
+      given=int tensor, given_mask=bool tensor
+                           inpainting: given [B, S] or [1, S] (one for every image) holds token ids, read only where given_mask
+                           ([B, S], [1, S] or [S]) is True; those ids must lie in [0, vocab_size) and at least one mask entry must be
+                           False. out[b, k] == given[b, k] wherever the mask is True; every other token is drawn as plain generation
+                           draws token k of image b (same RNG key per token index, cfg_interval by token index, the same filters), from
+                           a model that has seen every token before k, given or drawn. A raster-order model never sees the given tokens
+                           after k (e.g. the rows below a hole): a redrawn region follows what lies above and left of it. The leading
+                           run given to every image is prefilled in one pass (as prefix), and every later run given to every image is
+                           appended in one window pass instead of one decode step per token. An all-False mask gives exactly the tokens
+                           of the call without it, and a mask of the first P columns exactly those of prefix=given[:, :P]. Works with
+                           c2i and t2i, emb_masks, negative prompts, fp8 KV caches and fp8 weights; not with prefix, teacher,
+                           sjd_window, return_logits or return_logprobs.
       top_logprobs=N       1 <= N <= 20, with return_logprobs: return (tokens, logprobs, {"ranks": int32 [B, S], "top_ids": int32
                            [B, S, N], "top_logprobs": f32 [B, S, N]}). rank = 1 + the number of tokens with a larger processed logit;
                            the top ids are the N kept tokens with the largest logits (ties: lower id first), -1 with logprob -inf past
@@ -82,6 +94,8 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
     negative_emb_masks = sampling_kwargs.pop("negative_emb_masks", None)
     return_logprobs = bool(sampling_kwargs.pop("return_logprobs", False))
     top_logprobs = sampling_kwargs.pop("top_logprobs", None)
+    given = sampling_kwargs.pop("given", None)
+    given_mask = sampling_kwargs.pop("given_mask", None)
     if sampling_kwargs:
         raise TypeError(f"unexpected sampling kwargs: {sorted(sampling_kwargs)}")
     if top_logprobs is not None:
@@ -106,6 +120,13 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
     if prefix is not None and (teacher is not None or sjd_window is not None):
         raise ValueError("prefix cannot be combined with teacher or sjd_window")
     pf = _check_prefix(prefix, cond.shape[0], int(max_new_tokens), model.vocab_size) if prefix is not None else None
+    gv = None
+    if given is not None or given_mask is not None:
+        for name, on in (("prefix", prefix is not None), ("teacher", teacher is not None), ("sjd_window", sjd_window is not None),
+                         ("return_logits", return_logits), ("return_logprobs", return_logprobs)):
+            if on:
+                raise ValueError(f"given / given_mask cannot be combined with {name}")
+        gv = _check_given(given, given_mask, cond.shape[0], int(max_new_tokens), model.vocab_size)
     if negative_cond is not None or negative_emb_masks is not None:
         _check_negative(model, cond, emb_masks, negative_cond, negative_emb_masks, cfg_scale, teacher)
 
@@ -143,6 +164,13 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
     model.setup_caches(max_batch_size=rows, max_seq_length=T + S, dtype=model.tok_embeddings.weight.dtype)
     lib, handle = _lib.load(), model.engine()
     out = torch.empty((B, S), dtype=torch.int32, device=dev)
+    if gv is not None:
+        sc = _lib.SampleCfg(float(cfg_scale), int(cfg_interval), temperature, top_k, top_p, 0 if sample_logits else 1,
+                            _draw_seed() if seed is None else int(seed))
+        ws, ws_bytes = model._given_scratch(gv, T, use_cfg)
+        _lib.check(lib.lg_generate_given(handle, _lib.ptr(cond_dev), _lib.ptr(em), _lib.ptr(neg), _lib.ptr(nm), B, T, S, ctypes.byref(sc),
+                                         _lib.ptr(gv), ws, ws_bytes, _lib.ptr(out), _lib.current_stream(dev)), "lg_generate_given")
+        return out.to(cond.device) if cond.device != dev else out
     if sjd_window is not None:
         return _generate_sjd(model, lib, handle, cond, cond_dev, em, B, T, S, out, min(int(sjd_window), S - 1), use_cfg, return_stats,
                              _lib.SampleCfg(float(cfg_scale), int(cfg_interval), temperature, top_k, top_p, 0 if sample_logits else 1,
@@ -247,6 +275,31 @@ def _check_prefix(prefix, B, S, V):
     if bool(((pf < 0) | (pf >= V)).any()):
         raise ValueError(f"prefix token ids must lie in [0, vocab_size={V})")
     return pf
+
+
+def _check_given(given, given_mask, B, S, V):
+    """given / given_mask as one int32 host tensor [B, S]: the given token where the mask is True, -1 where the token is drawn; checked
+    on the host (it is outside input): integer ids in [0, V) where given, shapes [B, S] / [1, S] (and [S] for the mask), at least one
+    drawn token."""
+    if given is None or given_mask is None:
+        raise ValueError("given and given_mask go together")
+    g = torch.as_tensor(given)
+    m = torch.as_tensor(given_mask)
+    if g.dtype.is_floating_point or g.dtype.is_complex or g.dtype == torch.bool:
+        raise ValueError(f"given must be an integer tensor of token ids, got dtype {g.dtype}")
+    if m.dtype != torch.bool:
+        raise ValueError(f"given_mask must be a bool tensor, got dtype {m.dtype}")
+    if g.dim() != 2 or g.shape[0] not in (1, B) or g.shape[1] != S:
+        raise ValueError(f"given must be [B, S] or [1, S] = [{B}, {S}], got {tuple(g.shape)}")
+    if m.dim() not in (1, 2) or (m.dim() == 2 and m.shape[0] not in (1, B)) or m.shape[-1] != S:
+        raise ValueError(f"given_mask must be [B, S], [1, S] or [S] = [{B}, {S}], got {tuple(m.shape)}")
+    g = g.detach().to("cpu", torch.int64).expand(B, S)
+    m = m.detach().to("cpu").reshape(-1, S).expand(B, S)
+    if bool(m.all()):
+        raise ValueError("given_mask is True everywhere: at least one token must be drawn")
+    if bool((m & ((g < 0) | (g >= V))).any()):
+        raise ValueError(f"given token ids must lie in [0, vocab_size={V}) where given_mask is True")
+    return torch.where(m, g, torch.full_like(g, -1)).to(torch.int32).contiguous()
 
 
 def _generate_sjd(model, lib, handle, cond, cond_dev, em, B, T, S, out, L, use_cfg, return_stats, sc, dbg_probs=None, neg=None, nm=None):

@@ -203,6 +203,7 @@ class Transformer(nn.Module):
         self._score_ws = None
         self._sjd_ws = None
         self._prefix_ws = None
+        self._given_ws = None
         self._slot_ws = None
         self._slot_prefix_ws = None
         self.requires_grad_(False)
@@ -394,6 +395,27 @@ class Transformer(nn.Module):
         _lib.check(lib.lg_prefix_workspace_bytes(handle, nh, seq, ctypes.byref(one)), "lg_prefix_workspace_bytes")
         want = need.value if need.value <= PREFIX_SCRATCH_CAP else max(PREFIX_SCRATCH_CAP, one.value)
         base, nbytes = self._device_buffer("_prefix_ws", want)
+        return base, min(nbytes, want)
+
+    def _given_scratch(self, given, T: int, use_cfg: bool):
+        """The scratch of generate(given=..., given_mask=...) for given (int32 host [B, S], -1: drawn): the given tokens, the window
+        passes' rows and the prefill of the leading run given to every image, the prefill part capped as _prefix_scratch caps it (so a
+        mask of the first P columns prefills as generate(prefix=...) does); kept on the model like the setup_caches() workspace.
+        Returns (device pointer, bytes)."""
+        lib, handle = _lib.load(), self.engine()
+        B, S = given.shape
+        need = ctypes.c_size_t()
+        _lib.check(lib.lg_given_workspace_bytes(handle, _lib.ptr(given), B, S, int(use_cfg), ctypes.byref(need)), "lg_given_workspace_bytes")
+        want = need.value
+        lead = (given >= 0).all(0).tolist() + [False]
+        P = lead.index(False)
+        if P > 0:
+            nh = 2 if use_cfg else 1
+            pneed, pone = ctypes.c_size_t(), ctypes.c_size_t()
+            _lib.check(lib.lg_prefix_workspace_bytes(handle, nh * B, T + P, ctypes.byref(pneed)), "lg_prefix_workspace_bytes")
+            _lib.check(lib.lg_prefix_workspace_bytes(handle, nh, T + P, ctypes.byref(pone)), "lg_prefix_workspace_bytes")
+            want += (pneed.value if pneed.value <= PREFIX_SCRATCH_CAP else max(PREFIX_SCRATCH_CAP, pone.value)) - pneed.value
+        base, nbytes = self._device_buffer("_given_ws", want)
         return base, min(nbytes, want)
 
     def _slot_scratch(self, use_cfg: bool):

@@ -97,13 +97,63 @@ def prefix_kwargs(args, vq_model, batch: int, latent_size: int, device) -> dict:
     same for every image of the batch; none when no prefix is given, so the default path is unchanged."""
     if args.prefix_image is None:
         return {}
+    codes = _encode_image(args.prefix_image, args.image_size, vq_model, device)[: args.prefix_rows * latent_size]
+    return {"prefix": codes.view(1, -1).expand(batch, -1).contiguous()}
+
+
+def _encode_image(path, image_size: int, vq_model, device):
+    """The latent codes of the image at `path`, centre-cropped to image_size and encoded, in raster order."""
     from PIL import Image
     from .vq_demo import center_crop
-    img = center_crop(Image.open(args.prefix_image).convert("RGB"), args.image_size)
+    img = center_crop(Image.open(path).convert("RGB"), image_size)
     x = torch.from_numpy(2.0 * (np.array(img) / 255.0) - 1.0).permute(2, 0, 1)[None].float().to(device)
     _, _, [_, _, indices] = vq_model.encode(x)
-    codes = indices.reshape(-1)[: args.prefix_rows * latent_size]
-    return {"prefix": codes.view(1, -1).expand(batch, -1).contiguous()}
+    return indices.reshape(-1)
+
+
+def add_inpaint_args(parser):
+    parser.add_argument("--inpaint-image", type=str, default=None,
+                        help="extension: redraw one box of this image: it is centre-cropped to --image-size and encoded, every latent "
+                             "cell outside --inpaint-box is kept for every image of the batch and the box is generated")
+    parser.add_argument("--inpaint-box", type=int, nargs=4, default=None, metavar=("TOP", "LEFT", "BOTTOM", "RIGHT"),
+                        help="extension: the latent-grid cells to redraw, rows TOP .. BOTTOM - 1 and columns LEFT .. RIGHT - 1 (a "
+                             "redrawn cell sees the cells above and to its left, not the rows below the box)")
+    return parser
+
+
+def check_inpaint_args(args, latent_size: int):
+    """Rejects an --inpaint-image / --inpaint-box combination that generate() cannot run, before any model is loaded."""
+    if args.inpaint_image is None and args.inpaint_box is None:
+        return
+    if args.inpaint_image is None or args.inpaint_box is None:
+        raise SystemExit("--inpaint-image and --inpaint-box go together")
+    top, left, bottom, right = args.inpaint_box
+    if not (0 <= top < bottom <= latent_size and 0 <= left < right <= latent_size):
+        raise SystemExit(f"--inpaint-box TOP LEFT BOTTOM RIGHT must satisfy 0 <= TOP < BOTTOM <= {latent_size} and "
+                         f"0 <= LEFT < RIGHT <= {latent_size} (the latent grid is {latent_size} x {latent_size})")
+    if getattr(args, "prefix_image", None) is not None:
+        raise SystemExit("--inpaint-image cannot be combined with --prefix-image")
+    if getattr(args, "sjd_window", None) is not None:
+        raise SystemExit("--inpaint-image cannot be combined with --sjd-window")
+    if not os.path.isfile(args.inpaint_image):
+        raise SystemExit(f"--inpaint-image {args.inpaint_image!r} is not a file")
+
+
+def inpaint_mask(box, latent_size: int) -> torch.Tensor:
+    """given_mask [grid * grid] of --inpaint-box: True (kept) outside the box, False (redrawn) inside, raster order."""
+    top, left, bottom, right = box
+    m = torch.ones(latent_size, latent_size, dtype=torch.bool)
+    m[top:bottom, left:right] = False
+    return m.reshape(-1)
+
+
+def inpaint_kwargs(args, vq_model, batch: int, latent_size: int, device) -> dict:
+    """generate() keywords of --inpaint-image / --inpaint-box: the encoded image's codes, the same for every image of the batch, and the
+    mask that keeps every cell outside the box; none when no image is given, so the default path is unchanged."""
+    if args.inpaint_image is None:
+        return {}
+    codes = _encode_image(args.inpaint_image, args.image_size, vq_model, device)
+    return {"given": codes.view(1, -1), "given_mask": inpaint_mask(args.inpaint_box, latent_size)}
 
 
 def add_common_args(parser, t2i: bool):

@@ -6,7 +6,8 @@ import time
 import torch
 
 from .. import generate
-from .common import add_common_args, add_prefix_args, add_sjd_arg, check_prefix_args, load_gpt, load_vq, prefix_kwargs, sjd_kwargs
+from .common import (add_common_args, add_inpaint_args, add_prefix_args, add_sjd_arg, check_inpaint_args, check_prefix_args,
+                     inpaint_kwargs, load_gpt, load_vq, prefix_kwargs, sjd_kwargs)
 
 
 def main(args):
@@ -17,6 +18,7 @@ def main(args):
     device = "cuda"
     latent_size = args.image_size // args.downsample_size
     check_prefix_args(args, latent_size)
+    check_inpaint_args(args, latent_size)
     vq_model = load_vq(args, device)
     gpt_model = load_gpt(args, device, latent_size)
 
@@ -24,7 +26,8 @@ def main(args):
     c_indices = torch.tensor(class_labels, device=device)
     qzshape = [len(class_labels), args.codebook_embed_dim, latent_size, latent_size]
 
-    pk = prefix_kwargs(args, vq_model, len(class_labels), latent_size, device)
+    pk = {**prefix_kwargs(args, vq_model, len(class_labels), latent_size, device),
+          **inpaint_kwargs(args, vq_model, len(class_labels), latent_size, device)}
     torch.cuda.synchronize()
     t1 = time.time()
     index_sample = generate(gpt_model, c_indices, latent_size ** 2, cfg_scale=args.cfg_scale, cfg_interval=args.cfg_interval,
@@ -42,7 +45,7 @@ def main(args):
 
 
 def build_parser():
-    parser = add_prefix_args(add_sjd_arg(add_common_args(argparse.ArgumentParser(), t2i=False)))
+    parser = add_inpaint_args(add_prefix_args(add_sjd_arg(add_common_args(argparse.ArgumentParser(), t2i=False))))
     parser.add_argument("--cfg-interval", type=float, default=-1)
     parser.add_argument("--class-labels", type=int, nargs="+", default=None,
                         help="extension: override the 8 hard-coded ImageNet labels (batch size = number of labels)")

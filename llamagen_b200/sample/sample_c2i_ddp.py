@@ -14,7 +14,7 @@ import torch.distributed as dist
 from .. import distributed as lgd
 from ..pipeline import SamplePipeline
 from ..postprocess import AsyncPngWriter
-from .common import add_common_args, load_gpt, load_vq
+from .common import add_common_args, add_inpaint_args, check_inpaint_args, inpaint_kwargs, load_gpt, load_vq
 
 
 def create_npz_from_sample_folder(sample_dir, num=50_000):
@@ -36,6 +36,7 @@ def main(args):
     torch.manual_seed(args.global_seed)            # identical init on every rank before the broadcast
     print(f"Starting rank={rank}, seed={seed}, world_size={world}.")
     latent_size = args.image_size // args.downsample_size
+    check_inpaint_args(args, latent_size)
     if rank != 0:                                   # only rank 0 touches the disk
         args_nockpt = argparse.Namespace(**{**vars(args), "vq_ckpt": None, "gpt_ckpt": None})
         vq_model, gpt_model = load_vq(args_nockpt, device), load_gpt(args_nockpt, device, latent_size)
@@ -44,6 +45,8 @@ def main(args):
     nbytes = lgd.broadcast_module(gpt_model) + lgd.broadcast_module(vq_model)
     if rank == 0:
         print(f"broadcast {nbytes / 1e6:.1f} MB of weights over NCCL")
+    # every rank keeps the same cells of the same image (none without --inpaint-image)
+    ik = inpaint_kwargs(args, vq_model, args.per_proc_batch_size, latent_size, device)
     torch.manual_seed(seed)
 
     # folder name of sample_c2i_ddp.py:100-107 (model, checkpoint name, sizes, sampling knobs); "random-init" when no ckpt is given
@@ -70,7 +73,7 @@ def main(args):
     # D2H of batch i run on a second stream under the AR sampling of batch i+1, and the PNG encoders run on host
     # threads; file names and contents are the reference's.
     pipe = SamplePipeline(gpt_model, vq_model, args.codebook_embed_dim, cfg_scale=args.cfg_scale, cfg_interval=args.cfg_interval,
-                          temperature=args.temperature, top_k=args.top_k, top_p=args.top_p, sample_logits=True)
+                          temperature=args.temperature, top_k=args.top_k, top_p=args.top_p, sample_logits=True, **ik)
     eval_px = args.image_size_eval
     host = [torch.empty(n, eval_px, eval_px, 3, dtype=torch.uint8).pin_memory() for _ in range(2)]
 
@@ -105,7 +108,7 @@ def main(args):
 
 
 def build_parser():
-    parser = add_common_args(argparse.ArgumentParser(), t2i=False)
+    parser = add_inpaint_args(add_common_args(argparse.ArgumentParser(), t2i=False))
     parser.add_argument("--cfg-interval", type=float, default=-1)
     parser.add_argument("--image-size-eval", type=int, choices=[256, 384, 512], default=256)
     parser.add_argument("--sample-dir", type=str, default="samples")

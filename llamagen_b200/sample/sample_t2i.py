@@ -15,7 +15,8 @@ import torch
 
 from .. import generate
 from ..cond import HFT5Encoder, load_t5_feature_files, prepare_condition, synthetic_features
-from .common import add_common_args, add_prefix_args, add_sjd_arg, check_prefix_args, load_gpt, load_vq, prefix_kwargs, sjd_kwargs
+from .common import (add_common_args, add_inpaint_args, add_prefix_args, add_sjd_arg, check_inpaint_args, check_prefix_args,
+                     inpaint_kwargs, load_gpt, load_vq, prefix_kwargs, sjd_kwargs)
 
 PROMPTS = [
     "A portrait photo of a kangaroo wearing an orange hoodie and blue sunglasses standing on the grassin front of the Sydney Opera House holding a sign on the chest that says Welcome Friends!",
@@ -73,6 +74,7 @@ def main(args):
     device = "cuda"
     latent_size = args.image_size // args.downsample_size
     check_prefix_args(args, latent_size)
+    check_inpaint_args(args, latent_size)
     check_negative_args(args)
     vq_model = load_vq(args, device)
     gpt_model = load_gpt(args, device, latent_size)
@@ -90,7 +92,8 @@ def main(args):
         nk["negative_cond"], nk["negative_emb_masks"] = prepare_condition(*neg, left_padding=not args.no_left_padding)
     qzshape = [len(c_indices), args.codebook_embed_dim, latent_size, latent_size]
 
-    pk = prefix_kwargs(args, vq_model, len(c_indices), latent_size, device)
+    pk = {**prefix_kwargs(args, vq_model, len(c_indices), latent_size, device),
+          **inpaint_kwargs(args, vq_model, len(c_indices), latent_size, device)}
     torch.cuda.synchronize()
     t1 = time.time()
     index_sample = generate(gpt_model, c_indices, latent_size ** 2, emb_masks, cfg_scale=args.cfg_scale,
@@ -108,7 +111,7 @@ def main(args):
 
 
 def build_parser():
-    parser = add_prefix_args(add_sjd_arg(add_common_args(argparse.ArgumentParser(), t2i=True)))
+    parser = add_inpaint_args(add_prefix_args(add_sjd_arg(add_common_args(argparse.ArgumentParser(), t2i=True))))
     parser.add_argument("--t5-path", type=str, default="pretrained_models/t5-ckpt")
     parser.add_argument("--t5-model-type", type=str, default="flan-t5-xl")
     parser.add_argument("--t5-feature-max-len", type=int, default=120)

@@ -20,7 +20,7 @@ from .. import distributed as lgd
 from ..cond import HFT5Encoder, load_t5_feature_files, prepare_condition, synthetic_features
 from ..pipeline import SamplePipeline
 from ..postprocess import AsyncPngWriter
-from .common import add_common_args, load_gpt, load_vq
+from .common import add_common_args, add_inpaint_args, check_inpaint_args, inpaint_kwargs, load_gpt, load_vq
 
 FALLBACK_PROMPT = "a cute dog"      # sample_t2i_ddp.py:138
 
@@ -45,6 +45,7 @@ def main(args):
     torch.manual_seed(args.global_seed)            # identical init on every rank before the broadcast
     print(f"Starting rank={rank}, seed={seed}, world_size={world}.")
     latent_size = args.image_size // args.downsample_size
+    check_inpaint_args(args, latent_size)
     if rank != 0:
         args_nockpt = argparse.Namespace(**{**vars(args), "gpt_ckpt": None, "vq_ckpt": None})
         vq_model, gpt_model = load_vq(args_nockpt, device), load_gpt(args_nockpt, device, latent_size)
@@ -53,6 +54,8 @@ def main(args):
     nbytes = lgd.broadcast_module(gpt_model) + lgd.broadcast_module(vq_model)
     if rank == 0:
         print(f"broadcast {nbytes / 1e6:.1f} MB of weights over NCCL")
+    # every rank keeps the same cells of the same image (none without --inpaint-image)
+    ik = inpaint_kwargs(args, vq_model, args.per_proc_batch_size, latent_size, device)
     torch.manual_seed(seed)
     precision = gpt_model.tok_embeddings.weight.dtype
     T, C = args.t5_feature_max_len, args.t5_feature_dim
@@ -93,7 +96,7 @@ def main(args):
         return t5([prompt_list[i] if i < len(prompt_list) else FALLBACK_PROMPT for i in indices])
 
     pipe = SamplePipeline(gpt_model, vq_model, args.codebook_embed_dim, cfg_scale=args.cfg_scale, temperature=args.temperature,
-                          top_k=args.top_k, top_p=args.top_p, sample_logits=True)
+                          top_k=args.top_k, top_p=args.top_p, sample_logits=True, **ik)
     px = args.image_size
     host = [torch.empty(n, px, px, 3, dtype=torch.uint8).pin_memory() for _ in range(2)]
 
@@ -138,7 +141,7 @@ def main(args):
 
 
 def build_parser():
-    parser = add_common_args(argparse.ArgumentParser(), t2i=True)
+    parser = add_inpaint_args(add_common_args(argparse.ArgumentParser(), t2i=True))
     parser.add_argument("--prompt-csv", type=str, default="evaluations/t2i/PartiPrompts.tsv")
     parser.add_argument("--t5-path", type=str, default="pretrained_models/t5-ckpt")
     parser.add_argument("--t5-model-type", type=str, default="flan-t5-xl")
