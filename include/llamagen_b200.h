@@ -244,6 +244,13 @@ int  lg_sample_rows_logprobs(const float* logits, int B, int V, int mix_cfg, int
                              const uint64_t* seed_rows, const int32_t* step_rows, const float* cfg_rows, const int32_t* interval_rows,
                              const int32_t* img_rows, const lg_logprobs* lp, int32_t* out_idx, int32_t* out_seq, int seq_stride,
                              void* stream);
+/* lg_sample_rows_logprobs with the inpainting select (serving's inpainting requests): given dev int32 [B, seq_stride] or NULL, indexed
+ * as out_seq; where given[b][step_rows[b]] >= 0 that token replaces image b's draw in out_idx and out_seq, and every other row draws
+ * what lg_sample_rows_logprobs draws. cfg_rows, interval_rows, img_rows, given and lp may each be NULL; given needs out_seq. */
+int  lg_sample_rows_given(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc,
+                          const uint64_t* seed_rows, const int32_t* step_rows, const float* cfg_rows, const int32_t* interval_rows,
+                          const int32_t* img_rows, const int32_t* given, const lg_logprobs* lp, int32_t* out_idx, int32_t* out_seq,
+                          int seq_stride, void* stream);
 /* generate() with token log-probabilities [B, S] (top: [B, S, top_n]), in one call covering lg_generate (neg_cond NULL, P = 0),
  * lg_generate_neg (neg_cond, neg_mask as there) and lg_generate_prefix(_neg) (1 <= P <= S - 1, prefix and dev_ws as there; P = 0
  * needs neither and ignores them). The tokens are those of that call. Rows k < P (given tokens) get logprob 0, rank 0, top ids -1 and
@@ -308,6 +315,19 @@ int  lg_given_workspace_bytes(lg_engine* e, const int32_t* given, int B, int S, 
 int  lg_generate_given(lg_engine* e, const void* cond, const float* emb_mask, const void* neg_cond, const float* neg_mask, int B, int T,
                        int S, const lg_sample_cfg* sc, const int32_t* given, void* dev_ws, size_t ws_bytes, int32_t* out_tokens,
                        void* stream);
+/* Bytes of caller-provided scratch for lg_extend_slot with a run of K given tokens, K in [1, block_size - 2] (c2i and t2i models). */
+int  lg_slot_extend_workspace_bytes(lg_engine* e, int use_cfg, int K, size_t* bytes);
+/* The EXTEND of one serving slot (an inpainting request): tokens dev int32 [S], the slot's token row, holds the drawn token a - 1 and
+ * the given tokens a .. a + K - 1 (1 <= a, K >= 1, a + K <= S - 1). Feeds tokens a - 1 .. a + K - 1 at positions T + a - 1 .. of row
+ * `slot` and, with use_cfg, of row B + slot, each row alone in window chunks of at most 64 positions (lg_generate_given's extend pass of
+ * one image and one row), and writes the K / V of positions T + a - 1 .. T + a + K - 1 of those rows and nothing else of the workspace.
+ * emb_mask (t2i only): dev f32 [T] or NULL, the conditional row's mask; neg_mask: dev f32 [T] or NULL, the unconditional row's (needs
+ * use_cfg and emb_mask; NULL: emb_mask). logits_out dev f32 [nh, V]: the head output at position T + a + K - 1 (the logits of token
+ * a + K), one head GEMM over the request's nh rows, rounded as lg_prefill_slot rounds them. The arithmetic depends on neither slot, B
+ * nor any other row. dev_ws: 256-byte aligned, at least lg_slot_extend_workspace_bytes. Every argument, and the attention kernel of
+ * every chunk, is checked before any launch; the workspace needs rows >= nh * B and max_seq >= T + a + K. */
+int  lg_extend_slot(lg_engine* e, const int32_t* tokens, int S, int a, int K, int slot, int B, int use_cfg, const float* emb_mask,
+                    const float* neg_mask, void* dev_ws, size_t ws_bytes, float* logits_out, void* stream);
 
 /* ---- teacher-forced scoring: Transformer.forward(idx, cond_idx, targets) (gpt.py:341-382, eval mode) ----------------------- */
 /* Bytes of caller-provided scratch for lg_score over `rows` sequences (rows = 2B under CFG) of `seq` positions (T + S - 1). */

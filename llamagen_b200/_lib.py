@@ -101,6 +101,8 @@ SIGNATURES = {
                                      c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "lg_sample_rows_logprobs": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p, c_void_p, c_void_p, c_void_p,
                                         c_void_p, POINTER(Logprobs), c_void_p, c_void_p, c_int, c_void_p]),
+    "lg_sample_rows_given": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p, c_void_p, c_void_p, c_void_p,
+                                     c_void_p, c_void_p, POINTER(Logprobs), c_void_p, c_void_p, c_int, c_void_p]),
     "lg_generate_logprobs": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p,
                                      c_int, c_void_p, c_size_t, POINTER(Logprobs), c_void_p, c_void_p]),
     "lg_copy_slot_kv": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
@@ -115,6 +117,9 @@ SIGNATURES = {
     "lg_given_workspace_bytes": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_size_t)]),
     "lg_generate_given": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p,
                                   c_void_p, c_size_t, c_void_p, c_void_p]),
+    "lg_slot_extend_workspace_bytes": (c_int, [c_void_p, c_int, c_int, POINTER(c_size_t)]),
+    "lg_extend_slot": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t,
+                               c_void_p, c_void_p]),
     "lg_test_given_plan": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int]),
     "lg_test_sample_given": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p, c_void_p, c_void_p, c_void_p,
                                      c_void_p, c_int, c_void_p, c_void_p]),

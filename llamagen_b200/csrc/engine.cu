@@ -1086,8 +1086,9 @@ static void apply_logprobs(SampleArgs& a, const lg_logprobs* lp, size_t off) {
 static int sample_rows_impl(const char* fn, const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc,
                             const uint64_t* seed_rows, const int32_t* step_rows, const float* cfg_rows, const int32_t* interval_rows,
                             const int32_t* img_rows, const lg_logprobs* lp, int32_t* out_idx, int32_t* out_seq, int seq_stride,
-                            void* stream) {
+                            void* stream, const int32_t* given = nullptr) {
     LG_REQUIRE(logits && sc && seed_rows && step_rows && (out_idx || out_seq), "%s: null argument", fn);
+    LG_REQUIRE(!given || (out_seq && seq_stride > 0), "%s: given tokens are indexed as out_seq and need it", fn);
     LG_REQUIRE(mix_cfg || (!cfg_rows && !interval_rows), "%s: per-row cfg_rows / interval_rows need mix_cfg (2B logits rows)", fn);
     bool lp_on = false;
     LG_TRY(check_logprobs(fn, lp, &lp_on));
@@ -1095,7 +1096,7 @@ static int sample_rows_impl(const char* fn, const float* logits, int B, int V, i
     SampleArgs a = make_sample_args(*sc, logits, B, V, mix_cfg, round_dtype);
     a.seed_rows = seed_rows; a.step_rows = step_rows;
     a.cfg_rows = cfg_rows; a.interval_rows = interval_rows; a.img_rows = img_rows;
-    a.out_idx = out_idx; a.out_seq = out_seq; a.seq_stride = seq_stride;
+    a.out_idx = out_idx; a.out_seq = out_seq; a.seq_stride = seq_stride; a.given = given;
     if (lp_on) apply_logprobs(a, lp, 0);
     return launch_sample(a, (cudaStream_t)stream);
 }
@@ -1128,6 +1129,14 @@ int lg_sample_rows_logprobs(const float* logits, int B, int V, int mix_cfg, int 
                             void* stream) {
     return sample_rows_impl("lg_sample_rows_logprobs", logits, B, V, mix_cfg, round_dtype, sc, seed_rows, step_rows, cfg_rows,
                             interval_rows, img_rows, lp, out_idx, out_seq, seq_stride, stream);
+}
+
+int lg_sample_rows_given(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc,
+                         const uint64_t* seed_rows, const int32_t* step_rows, const float* cfg_rows, const int32_t* interval_rows,
+                         const int32_t* img_rows, const int32_t* given, const lg_logprobs* lp, int32_t* out_idx, int32_t* out_seq,
+                         int seq_stride, void* stream) {
+    return sample_rows_impl("lg_sample_rows_given", logits, B, V, mix_cfg, round_dtype, sc, seed_rows, step_rows, cfg_rows,
+                            interval_rows, img_rows, lp, out_idx, out_seq, seq_stride, stream, given);
 }
 
 int lg_sample(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc, uint64_t step,
@@ -1554,6 +1563,102 @@ int lg_prefill_slot(lg_engine* e, const void* cond, const float* emb_mask, int T
                              stream);
 }
 
+// The chunk loop of an extend pass: tokens a - 1 .. a + K - 1 of nb images (nh cache rows each, from w.first_row on) at positions
+// T + a - 1 .., through the layers in window chunks of at most W rows; their K / V go to w's cache, the activations to w's row buffers.
+// Token a - 1 is tokens[b] when tokens is set (the token the previous draw fed forward), every other token given[b][k] ([nb, S]). Rows
+// r < nb attend with emb_mask, the others with neg_mask when set. The last row of every cache row's window is gathered to `last`
+// [nh * nb, D]. lg_generate_given's extend (every chain's images) and lg_extend_slot (one row of one slot per call) share it, so one
+// image at nh = 1 runs the same chunks and GEMM plans in both.
+static int extend_window(lg_engine* e, const Workspace& w, int32_t* win_tokens, int32_t* win_pos, const int32_t* tokens,
+                         const int32_t* given, int nb, int nh, int S, int T, int a, int K, int W, const float* emb_mask,
+                         const float* neg_mask, void* last, cudaStream_t st) {
+    const int D = e->cfg.dim, dt = e->cfg.dtype, R = nh * nb;
+    int n = 0;
+    for (int c0 = 0; c0 < K + 1; c0 += n) {
+        n = std::min(W, K + 1 - c0);
+        const int j0 = a - 1 + c0;
+        LG_TRY(launch_given_window(tokens, given, nb, nh, S, j0, n, tokens && c0 == 0, T + j0, win_tokens, win_pos, st));
+        LG_PROF(PC_EMBED_MISC, st, launch_embed(e->tok_emb, win_tokens, nb * n, R * n, -1, D, dt, w.h, st));
+        LG_TRY(e->run_layers(w, R * n, n, PosArg{nullptr, 0, win_pos}, emb_mask, neg_mask, nb, false, st));
+    }
+    return launch_gather_last(w.xn, R, n, D, dt, last, st);
+}
+
+// lg_extend_slot's scratch for a request of nh rows and window chunks of W rows, from `base` (null: sizes only): the rows of one cache
+// row's window (carve_given_window of one image, one row), then the request's nh last rows (head.q) and the partials of the head GEMM
+// over them.
+static size_t carve_slot_extend(const lg_engine* e, RowBuffers& win, int32_t** win_tokens, int32_t** win_pos, RowBuffers& head, char* base,
+                                int nh, int W) {
+    const int D = e->cfg.dim, V = e->cfg.vocab_size, dt = e->cfg.dtype;
+    Carver c{base, 0, 1, e->carve_given_window(win, win_tokens, win_pos, base, 1, 1, W)};
+    head.q = c.split((size_t)nh * D * e->esz);
+    head.partial_floats = std::max(gemm_partial_floats(nh, V, D, 0, dt), gemm_partial_floats(nh, V, D, 0, dt, e->output.scale != nullptr));
+    head.partial = (float*)c.split(head.partial_floats * sizeof(float));
+    return c.off;
+}
+
+int lg_slot_extend_workspace_bytes(lg_engine* e, int use_cfg, int K, size_t* bytes) {
+    static const char* fn = "lg_slot_extend_workspace_bytes";
+    LG_REQUIRE(e && bytes, "%s: null argument", fn);
+    LG_REQUIRE(K >= 1 && K <= e->cfg.block_size - 2, "%s: K=%d outside [1, block_size - 2 = %d]", fn, K, e->cfg.block_size - 2);
+    RowBuffers win, head;
+    int32_t *t, *p;
+    *bytes = carve_slot_extend(e, win, &t, &p, head, nullptr, use_cfg ? 2 : 1, std::min(K + 1, kGivenWindowRows));
+    return 0;
+}
+
+// An extend of serving: lg_generate_given's extend pass over one request, once for its conditional row `slot` and once, under CFG, for
+// its unconditional row B + slot, each one cache row in chunks of at most kGivenWindowRows positions, then one head GEMM over the
+// request's nh rows. Every call runs the same chunks at the same shapes whatever the slot, B or the other requests.
+int lg_extend_slot(lg_engine* e, const int32_t* tokens, int S, int a, int K, int slot, int B, int use_cfg, const float* emb_mask,
+                   const float* neg_mask, void* dev_ws, size_t ws_bytes, float* logits_out, void* stream) {
+    static const char* fn = "lg_extend_slot";
+    cudaStream_t st = (cudaStream_t)stream;
+    LG_REQUIRE(e, "%s: null engine", fn);
+    const lg_model_cfg& c = e->cfg;
+    LG_REQUIRE(tokens && logits_out, "%s: null tokens or logits_out", fn);
+    LG_REQUIRE(S >= 3 && S <= c.block_size, "%s: S=%d outside [3, block_size=%d]", fn, S, c.block_size);
+    LG_REQUIRE(a >= 1 && K >= 1 && a + K <= S - 1, "%s: extend [a=%d, a + K=%d) must lie in [1, S - 1 = %d)", fn, a, a + K, S - 1);
+    LG_REQUIRE(B > 0 && slot >= 0 && slot < B, "%s: slot %d outside [0, B=%d)", fn, slot, B);
+    LG_REQUIRE(!emb_mask || c.model_type == LG_MODEL_T2I, "%s: emb_mask only applies to t2i models", fn);
+    LG_REQUIRE(!neg_mask || use_cfg, "%s: neg_mask masks the unconditional CFG row and needs use_cfg", fn);
+    LG_REQUIRE(!neg_mask || emb_mask, "%s: neg_mask needs emb_mask (all ones for an unmasked condition)", fn);
+    const int nh = use_cfg ? 2 : 1, D = c.dim, V = c.vocab_size, T = c.cls_token_num, W = std::min(K + 1, kGivenWindowRows);
+    LG_REQUIRE(dev_ws && ((uintptr_t)dev_ws & 255) == 0, "%s: scratch must be non-null and 256-byte aligned", fn);
+    LG_REQUIRE(e->finalized, "%s: engine not finalized", fn);
+    LG_TRY(check_ready(e, nh * B, T + a + K));
+    RowBuffers win, hb;
+    int32_t *win_tokens, *win_pos;
+    const size_t need = carve_slot_extend(e, win, &win_tokens, &win_pos, hb, (char*)dev_ws, nh, W);
+    LG_REQUIRE(ws_bytes >= need, "%s: scratch of %zu bytes is too small (%zu)", fn, ws_bytes, need);
+    // every chunk's attention at first_row = the slot's row: the window kernel (16-bit cache), the CUDA-core kernel (fp32 or fp8 cache)
+    // and, for a chunk of one row, the decode kernel all address the cache from first_row through make_attn_args
+    for (int c0 = 0, n = 0; c0 < K + 1; c0 += n) {
+        n = std::min(W, K + 1 - c0);
+        KvCache kv = e->full;
+        kv.first_row = slot;
+        AttnArgs aa = e->attn_args(kv, 0, 1, n);
+        aa.pos = PosArg{nullptr, 0, win_pos};
+        const AttnPlan p = attn_plan(aa);
+        LG_REQUIRE(p.kernel >= 0, "%s: %s", fn, p.error);
+    }
+    DeviceGuard guard(e->device);
+    LG_TRY(e->zero_fill_if_needed(st));
+    for (int half = 0; half < nh; ++half) {
+        Workspace w;
+        static_cast<KvCache&>(w) = e->full;
+        static_cast<RowBuffers&>(w) = win;
+        w.first_row = half * B + slot;
+        LG_TRY(extend_window(e, w, win_tokens, win_pos, nullptr, tokens, 1, 1, S, T, a, K, W, half != 0 && neg_mask ? neg_mask : emb_mask,
+                             nullptr, hb.q + (size_t)half * D * e->esz, st));
+    }
+    Workspace w;
+    static_cast<RowBuffers&>(w) = hb;
+    GemmNext nx_first{e->layers[0].wqkv.p, e->layers[0].wqkv.bytes(3 * D, D, e->esz), nullptr, 0};
+    LG_TRY(e->head(w, hb.q, nh, logits_out, &nx_first, st));
+    return round_logits_inplace(logits_out, (size_t)nh * V, c.dtype, st);
+}
+
 static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, const Negative& neg, int B, int T, int S,
                          const lg_sample_cfg* sc, int32_t* out_tokens, float* dbg_logits, const int32_t* teacher,
                          const PrefixArgs& pa, const lg_logprobs* lp, cudaStream_t st0) {
@@ -1634,19 +1739,12 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
     // window chunks of at most pa.W rows (their K / V go to the chain's cache); the head over the last row of every image's window
     // gives the logits of token a + K, which is drawn (or taken as given) with its own step, and the counters move past it
     auto extend = [&](Chain& k, int a, int K) -> int {
-        const int D = c.dim, dt = c.dtype, nh = use_cfg ? 2 : 1;
+        const int D = c.dim;
         Workspace w;
         static_cast<KvCache&>(w) = k.w;
         static_cast<RowBuffers&>(w) = k.win;
-        int n = 0;
-        for (int c0 = 0; c0 < K + 1; c0 += n) {
-            n = std::min(pa.W, K + 1 - c0);
-            const int j0 = a - 1 + c0;
-            LG_TRY(launch_given_window(k.w.tokens, k.sa.given, k.B, nh, S, j0, n, c0 == 0, T + j0, k.win_tokens, k.win_pos, k.st));
-            LG_PROF(PC_EMBED_MISC, k.st, launch_embed(e->tok_emb, k.win_tokens, k.B * n, k.R * n, -1, D, dt, w.h, k.st));
-            LG_TRY(e->run_layers(w, k.R * n, n, PosArg{nullptr, 0, k.win_pos}, k.emb_mask, k.neg.mask, k.B, false, k.st));
-        }
-        LG_TRY(launch_gather_last(w.xn, k.R, n, D, dt, w.q, k.st));
+        LG_TRY(extend_window(e, w, k.win_tokens, k.win_pos, k.w.tokens, k.sa.given, k.B, use_cfg ? 2 : 1, S, T, a, K, pa.W, k.emb_mask,
+                             k.neg.mask, w.q, k.st));
         GemmNext nx_first{e->layers[0].wqkv.p, e->layers[0].wqkv.bytes(3 * D, D, e->esz), nullptr, 0};
         LG_TRY(e->head(w, w.q, k.R, k.w.logits, &nx_first, k.st));
         SampleArgs sa = k.sa;   // the decode step's draw at a fixed step; the counters are set, not advanced

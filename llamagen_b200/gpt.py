@@ -206,6 +206,7 @@ class Transformer(nn.Module):
         self._given_ws = None
         self._slot_ws = None
         self._slot_prefix_ws = None
+        self._slot_extend_ws = None
         self.requires_grad_(False)
 
     # ------------------------------------------------------------------ engine plumbing
@@ -433,6 +434,14 @@ class Transformer(nn.Module):
         need = ctypes.c_size_t()
         _lib.check(lib.lg_slot_prefix_workspace_bytes(handle, int(use_cfg), int(P), ctypes.byref(need)), "lg_slot_prefix_workspace_bytes")
         return self._device_buffer("_slot_prefix_ws", need.value)
+
+    def _slot_extend_scratch(self, use_cfg: bool, K: int):
+        """The lg_extend_slot scratch (serve.LLM's window pass over a run of K given tokens of one inpainting request), kept on the model
+        like _slot_scratch and grown to the largest seen. Returns (device pointer, bytes)."""
+        lib, handle = _lib.load(), self.engine()
+        need = ctypes.c_size_t()
+        _lib.check(lib.lg_slot_extend_workspace_bytes(handle, int(use_cfg), int(K), ctypes.byref(need)), "lg_slot_extend_workspace_bytes")
+        return self._device_buffer("_slot_extend_ws", need.value)
 
     def _sjd_scratch(self, B: int, use_cfg: bool, L: int):
         """The lg_generate_sjd scratch for B images and window L, kept on the model like the setup_caches() workspace.

@@ -83,6 +83,20 @@ the n with the largest cumulative_logprob, sorted descending (ties: the lower im
 best_of the outputs stay in index order (vLLM always sorts). cumulative_logprob is filled whenever logprobs or best_of is set: the sum of
 the drawn tokens' logprobs in float64. Neither field goes with sjd_window.
 
+Inpainting (add_request(..., given=ids, given_mask=mask), LLM.generate(..., givens=[...], given_masks=[...]); c2i and t2i): ids and
+mask have shape [max_tokens], checked as generate()'s given / given_mask at B = 1, and the request's token_ids hold ids[k] wherever
+mask[k] is True. The request follows the engine's own plan of generate(given=...) at B = 1 (lg_test_given_plan): its leading given run
+of P tokens is its prefix (a join through lg_prefill_slot_prefix, P = 0: a plain join); its drawn tokens are drawn by the running
+batch's decode and draw; each interior given run [a, a + K) is one window pass over the slot alone (lg_extend_slot: tokens a - 1 ..
+a + K - 1 at positions T + a - 1 ..), enqueued after the step's batched decode, whose row for the slot is rewritten by it, and token
+a + K is drawn from its logits with the slot's seed, guidance and image index at step a + K; a trailing given run needs no step, the
+request finishes when its last drawn token is drawn. While a running or joining slot has given tokens, every draw is
+lg_sample_rows_given over the slots' given rows, so a row whose token is given takes it; requests without given draw as before. A
+request's passes and their shapes depend only on the request, whatever ran beside it. At cfg_scale 1 they are the passes of
+generate(cond, given=ids, given_mask=mask, seed=base_seed + r) at B = 1, so the tokens are that call's bit for bit; under CFG each half
+runs its own window pass, so the logits agree with that call's up to rounding. With n = k, sample j is keyed as image j. given goes with everything generate(given=) goes with; prefix=, sjd_window, logprobs and best_of are refused.
+Null-class twins mirror their conditional request's given tokens.
+
 While requests are in flight the LLM owns the model's KV-cache workspace (a `generate()` call on the same model would reset it)."""
 from __future__ import annotations
 
@@ -100,7 +114,7 @@ import torch
 
 from . import _lib
 from .cond import pack_t5_features, prepare_condition
-from .generate import _check_prefix
+from .generate import _check_given, _check_prefix
 
 
 @dataclass(frozen=True)
@@ -182,11 +196,27 @@ class _Request:
     n: int = 1                             # its images (sequence slots): best_of, else n
     done: dict = field(default_factory=dict)   # image index -> token ids of every finished sample
     done_lp: dict = field(default_factory=dict)   # image index -> (logprob, rank, top ids, top logprobs) rows, when it wants them
+    given: Optional[torch.Tensor] = None   # inpainting: int32 [S] on the host, the given token where given, -1 where drawn
+    extends: dict = field(default_factory=dict)   # inpainting: start a of every interior given run -> its length K
+    end: int = 0                           # the index after the last drawn token (max_tokens without a trailing given run)
 
 
 def _plen(req: _Request) -> int:
     """P, the number of given image tokens of a request (0 without a prefix)."""
     return 0 if req.prefix is None else int(req.prefix.numel())
+
+
+def _given_plan(given: torch.Tensor):
+    """The engine's plan of generate(given=...) at B = 1 for one request's given row (int32 [S], -1: drawn), lg_test_given_plan:
+    (P, {a: K} of every EXTEND, the index after the last drawn token)."""
+    S = int(given.numel())
+    row = np.ascontiguousarray(given.numpy(), dtype=np.int32)
+    segs = np.zeros((S + 1, 3), dtype=np.int32)
+    n = _lib.load().lg_test_given_plan(row.ctypes.data_as(ctypes.c_void_p), 1, S, segs.ctypes.data_as(ctypes.c_void_p), S + 1)
+    _lib.check(n, "lg_test_given_plan")
+    segs = segs[:n].tolist()
+    tail = [ln for kind, _, ln in segs if kind == 3]
+    return segs[0][2], {a: K for kind, a, K in segs if kind == 2}, S - sum(tail)
 
 
 class LLM:
@@ -240,7 +270,7 @@ class LLM:
     # ------------------------------------------------------------------ engine-style surface (llm_engine.py)
     def add_request(self, prompt_token_ids: Optional[Sequence[int]] = None, sampling_params: Optional[SamplingParams] = None, twin_of=None,
                     prompt_embeds=None, prefix=None, prompt: Optional[str] = None, negative_prompt_embeds=None,
-                    negative_prompt: Optional[str] = None) -> str:
+                    negative_prompt: Optional[str] = None, given=None, given_mask=None) -> str:
         """c2i: prompt_token_ids = [class id] (twin_of: see LLM.generate). t2i: prompt_embeds = one caption's T5 features, [n, caption_dim]
         or the .npy layout [1, n, caption_dim] (array or tensor, n >= 1, truncated at cls_token_num).
         prefix: image completion, the first P image tokens (1-D integer ids in [0, vocab_size), 1 <= P <= max_tokens - 1); the
@@ -248,7 +278,10 @@ class LLM:
         prompt: a caption string, with a text_encoder only (instead of prompt_embeds).
         negative_prompt_embeds (t2i, cfg_scale > 1): a negative caption's T5 features, shaped as prompt_embeds; the request's
         unconditional row takes it instead of the null condition. negative_prompt: its string, with a text_encoder only (one encoder
-        call with prompt)."""
+        call with prompt).
+        given, given_mask: inpainting, token ids [max_tokens] and a bool mask [max_tokens] with at least one False (generate()'s checks
+        at B = 1); the request keeps given[k] wherever given_mask[k] is True and draws the rest. Not with prefix, sjd_window, logprobs
+        or best_of. A null-class twin takes its conditional request's (passing other ones is an error)."""
         if prompt is not None or negative_prompt is not None:
             texts = [t for t in (prompt, negative_prompt) if t is not None]
             if prompt is not None and prompt_embeds is not None:
@@ -267,6 +300,9 @@ class LLM:
             caption = self._caption(prompt_embeds)
             negative = self._negative(negative_prompt_embeds, scale)
             pf = self._prefix(prefix, sampling_params)
+            gv = self._given(given, given_mask, sampling_params, pf)
+            if gv is not None:
+                return self._enqueue_t2i(caption, sampling_params, pf, negative, gv)
             return self._enqueue_t2i(caption, sampling_params, pf) if negative is None else self._enqueue_t2i(caption, sampling_params, pf,
                                                                                                               negative)
         if negative_prompt_embeds is not None:
@@ -280,11 +316,14 @@ class LLM:
         self._guidance(sampling_params)
         if twin_of is None:
             pf = self._prefix(prefix, sampling_params)
+            gv = self._given(given, given_mask, sampling_params, pf)
         else:
+            gv = self._twin_given(twin_of, given, given_mask, sampling_params, prefix)
             pf = self._twin_prefix(twin_of, prefix, sampling_params)
             self._twin_guidance(twin_of, sampling_params)
         rid = str(next(self.request_counter))
         req = self._guided(_Request(rid, [int(prompt_token_ids[0])], sampling_params or SamplingParams(), twin_of, prefix=pf))
+        self._set_given(req, gv)
         if twin_of is None:
             self._waiting.append(req)
         else:
@@ -392,6 +431,44 @@ class LLM:
         S = int((sampling_params or SamplingParams()).max_tokens)
         return _check_prefix(pf[None], 1, S, self.model.vocab_size)[0]
 
+    def _given(self, given, given_mask, sampling_params: Optional[SamplingParams], prefix) -> Optional[torch.Tensor]:
+        """A request's given tokens as int32 [max_tokens] on the host, -1 where drawn, checked as generate(given=, given_mask=) checks
+        them at B = 1; None without them."""
+        if given is None and given_mask is None:
+            return None
+        if self.sjd_window is not None:
+            raise ValueError("given / given_mask cannot be combined with sjd_window")
+        if prefix is not None:
+            raise ValueError("given / given_mask cannot be combined with prefix (a leading given run already is a prefix)")
+        sp = sampling_params or SamplingParams()
+        if _wants_logprobs(sp):
+            raise ValueError("given / given_mask cannot be combined with SamplingParams.logprobs or best_of")
+        S = int(sp.max_tokens)
+        g, m = [None if x is None else x.detach().cpu() if torch.is_tensor(x) else torch.as_tensor(np.asarray(x)) for x in (given, given_mask)]
+        for name, x in (("given", g), ("given_mask", m)):
+            if x is not None and x.dim() != 1:
+                raise ValueError(f"a request's {name} is 1-D, [max_tokens = {S}], got shape {tuple(x.shape)}")
+        return _check_given(None if g is None else g[None], m, 1, S, self.model.vocab_size)[0]
+
+    def _set_given(self, req: _Request, gv: Optional[torch.Tensor]) -> _Request:
+        """req with its given tokens and plan (_given_plan); the leading given run becomes its prefix (its join is a prefix join)."""
+        req.end = int(req.params.max_tokens)
+        if gv is not None:
+            P, req.extends, req.end = _given_plan(gv)
+            req.given = gv
+            req.prefix = gv[:P].to(torch.int64) if P > 0 else None
+        return req
+
+    def _twin_given(self, twin_of, given, given_mask, sampling_params: Optional[SamplingParams], prefix) -> Optional[torch.Tensor]:
+        """The given tokens of a null-class twin: its conditional request's. Given tokens passed for the twin must equal them."""
+        owner = self._owner(twin_of)
+        mine = None if owner is None else owner.given
+        if given is not None or given_mask is not None:
+            gv = self._given(given, given_mask, sampling_params, prefix)
+            if mine is None or not torch.equal(gv, mine):
+                raise ValueError(f"a null-class twin mirrors the given tokens of its conditional request {twin_of!r}; it was given other ones")
+        return mine
+
     def _owner(self, twin_of) -> Optional[_Request]:
         """The waiting or running conditional request a null-class twin mirrors, or None."""
         return next((r for r in itertools.chain(self._waiting, self._slots) if r is not None and r.request_id == twin_of), None)
@@ -399,18 +476,19 @@ class LLM:
     def _twin_prefix(self, twin_of, prefix, sampling_params: Optional[SamplingParams]) -> Optional[torch.Tensor]:
         """The prefix of a null-class twin: its conditional request's. A prefix passed for the twin must equal it."""
         owner = self._owner(twin_of)
-        mine = None if owner is None else owner.prefix
+        mine = None if owner is None or owner.given is not None else owner.prefix
         if prefix is not None:
             pf = self._prefix(prefix, sampling_params)
             if mine is None or not torch.equal(pf, mine):
                 raise ValueError(f"a null-class twin mirrors the prefix of its conditional request {twin_of!r}; it was given another one")
         return mine
 
-    def _enqueue_t2i(self, caption, sampling_params: Optional[SamplingParams], prefix: Optional[torch.Tensor] = None, negative=None) -> str:
+    def _enqueue_t2i(self, caption, sampling_params: Optional[SamplingParams], prefix: Optional[torch.Tensor] = None, negative=None,
+                     given: Optional[torch.Tensor] = None) -> str:
         rid = str(next(self.request_counter))
         neg, neg_mask = negative if negative is not None else (None, None)
-        self._waiting.append(self._guided(_Request(rid, [], sampling_params or SamplingParams(), cond=caption[0], mask=caption[1],
-                                                   prefix=prefix, neg=neg, neg_mask=neg_mask)))
+        self._waiting.append(self._set_given(self._guided(_Request(rid, [], sampling_params or SamplingParams(), cond=caption[0],
+                                                                   mask=caption[1], prefix=prefix, neg=neg, neg_mask=neg_mask)), given))
         return rid
 
     def _running(self) -> int:
@@ -505,7 +583,8 @@ class LLM:
         result -> st["tok"][slots] and out[slot, step] (out: st["out"] rows from slots.start). Under CFG each slot mixes with its own
         scale and cfg_interval (lg_sample_rows_guided with st["cfg"], st["interval"]), otherwise lg_sample_rows. When a running slot
         among them holds an image index > 0 (parallel sampling), every slot draws as its image (lg_sample_rows_keyed with st["img"]).
-        While a slot among them wants logprobs, the draw is lg_sample_rows_logprobs into st["lp"] ... at the same index as out."""
+        While a slot among them wants logprobs, the draw is lg_sample_rows_logprobs into st["lp"] ... at the same index as out. While a
+        slot among them has given tokens, it is lg_sample_rows_given over st["given"] (a row whose token is given takes it)."""
         lib, m, n = _lib.load(), self.model, slots.stop - slots.start
         use_cfg = 1 if st["R"] == 2 * self.max_num_seqs else 0
         sc = self._sample_cfg(params)
@@ -515,7 +594,12 @@ class LLM:
         keyed = any(self._slots[i] is not None and self._img[i] > 0 for i in range(slots.start, slots.stop))
         wants = [self._slots[i].params for i in range(slots.start, slots.stop)
                  if self._slots[i] is not None and _wants_logprobs(self._slots[i].params)]
-        if wants:
+        if any(self._slots[i] is not None and self._slots[i].given is not None for i in range(slots.start, slots.stop)):
+            spec = self._logprob_spec(st, slots.start, any(p.logprobs for p in wants)) if wants else None
+            guide = (_lib.ptr(st["cfg"][slots]), _lib.ptr(st["interval"][slots])) if use_cfg else (None, None)
+            _lib.check(lib.lg_sample_rows_given(*head, *guide, _lib.ptr(st["img"][slots]) if keyed else None, _lib.ptr(st["given"][slots]),
+                                                None if spec is None else ctypes.byref(spec), *tail), "lg_sample_rows_given")
+        elif wants:
             spec = self._logprob_spec(st, slots.start, any(p.logprobs for p in wants))
             guide = (_lib.ptr(st["cfg"][slots]), _lib.ptr(st["interval"][slots])) if use_cfg else (None, None)
             _lib.check(lib.lg_sample_rows_logprobs(*head, *guide, _lib.ptr(st["img"][slots]) if keyed else None, ctypes.byref(spec), *tail),
@@ -619,6 +703,52 @@ class LLM:
         if r.neg is not None:
             st["neg"][i].copy_(r.neg)
         st["neg_mask"][i].copy_(r.mask if r.neg_mask is None else r.neg_mask)
+
+    # ------------------------------------------------------------------ inpainting (given=, given_mask=)
+    def _load_given(self, st, slots: List[int], r: _Request):
+        """A joining request's given tokens to its slots' token rows st["out"] and given rows st["given"] (allocated, all -1, when the
+        first request with given tokens joins; from then on every join rewrites its slots' given rows)."""
+        if r.given is None and "given" not in st:
+            return
+        if "given" not in st:
+            st["given"] = torch.full((self.max_num_seqs, st["S"]), -1, dtype=torch.int32, device=st["dev"])
+        row = torch.full((st["S"],), -1, dtype=torch.int32) if r.given is None else r.given
+        row = row.to(st["dev"])
+        for s in slots:
+            st["given"][s] = row
+            if r.given is not None:
+                st["out"][s] = row
+
+    def _extends(self) -> List[tuple]:
+        """(slot, a, K) of every running slot whose next token starts an interior given run: this step's decode row for it draws the
+        given token a (the given select), and its extend follows the decode."""
+        return [(i, self._depth[i], r.extends[self._depth[i]]) for i, r in enumerate(self._slots)
+                if r is not None and self._depth[i] in r.extends]
+
+    def _device_extend(self, st, params: SamplingParams, slot: int, a: int, K: int):
+        """lg_extend_slot over the given run [a, a + K) of slot: tokens a - 1 .. a + K - 1 of st["out"][slot] at positions T + a - 1 ..,
+        then token a + K drawn from its logits (_draw: the slot's seed, guidance and image index, step a + K) into st["out"][slot, a + K]
+        and st["tok"][slot]."""
+        B, m = self.max_num_seqs, self.model
+        use_cfg = 1 if st["R"] == 2 * B else 0
+        ws, ws_bytes = m._slot_extend_scratch(use_cfg, K)
+        mask = _lib.ptr(st["mask"][slot]) if self.t2i else None
+        neg_mask = _lib.ptr(st["neg_mask"][slot]) if self.t2i and use_cfg else None
+        _lib.check(_lib.load().lg_extend_slot(m.engine(), _lib.ptr(st["out"][slot]), st["S"], a, K, slot, B, use_cfg, mask, neg_mask, ws,
+                                              ws_bytes, _lib.ptr(st["join_logits"]), _lib.current_stream(st["dev"])), "lg_extend_slot")
+        st["join_step"].fill_(a + K)
+        self._draw(st, params, st["join_logits"], slice(slot, slot + 1), st["join_step"], st["out"][slot])
+
+    def _run_extends(self, st, params: SamplingParams, ext: List[tuple]):
+        """After a step's decode: every extend of `ext` ((slot, a, K), from _extends before the decode), then the slot's rows sit at
+        position T + a + K with token a + K as input, and it has drawn a + K + 1 tokens."""
+        B, R, T = self.max_num_seqs, st["R"], self.model.cls_token_num
+        for i, a, K in ext:
+            self._device_extend(st, params, i, a, K)
+            st["pos"][[i, B + i] if R == 2 * B else [i]] = T + a + K
+            if self.t2i:
+                st["step"][i] = a + K + 1
+            self._depth[i] = a + K + 1
 
     # ------------------------------------------------------------------ parallel sampling (SamplingParams.n)
     def _device_copy_kv(self, st, src: int, dsts: List[int], length: int):
@@ -788,14 +918,17 @@ class LLM:
         requests that reached max_tokens."""
         B, R, S, dev = self.max_num_seqs, st["R"], st["S"], st["dev"]
         T = self.model.cls_token_num
-        # (1) one decode step for every slot; free slots run too (their rows are never read) so that the row count stays fixed
+        # (1) one decode step for every slot; free slots run too (their rows are never read) so that the row count stays fixed; then the
+        # extends of the slots whose decode row drew the first token of a given run
         if self._running():
+            ext = self._extends()
             self._device_decode_t2i(st, params)
             st["pos"] += st["active"]
             st["step"] += st["active"][:B]
             for i in range(B):
                 if self._slots[i] is not None:
                     self._depth[i] += 1
+            self._run_extends(st, params, ext)
         # (2) admission: the conditions and masks go to their slots' rows, then each request is prefilled alone and draws token 0, or,
         # with P given tokens (written to its out row first), token P
         joined = self._admit(params)
@@ -808,6 +941,7 @@ class LLM:
                 i = slots[0]
                 for s in slots:
                     self._load_caption(st, s, r)
+                self._load_given(st, slots, r)
                 if r.prefix is None:
                     self._device_join_t2i(st, params, i)
                 else:
@@ -821,8 +955,8 @@ class LLM:
             st["active"][rows] = 1
             st["step"][idx] = P + 1
         self.steps_run += 1
-        # (3) the finished requests: the only device->host copy is their token rows
-        done = [i for i in range(B) if self._slots[i] is not None and self._depth[i] >= S]
+        # (3) the finished requests (their last drawn token is drawn): the only device->host copy is their token rows
+        done = [i for i in range(B) if self._slots[i] is not None and self._depth[i] >= self._slots[i].end]
         outs: List[RequestOutput] = []
         if done:
             idx = torch.tensor(done, dtype=torch.long, device=dev)
@@ -874,6 +1008,8 @@ class LLM:
             rows = torch.cat([idx, idx + B]) if R == 2 * B else idx
             st["pos"][rows] = 0
             st["active"][rows] = 1
+            for slots, r in joined:
+                self._load_given(st, slots, r)
             # a completion request is prefilled through its P given tokens (written to its out rows first) and draws token P here; its
             # rows then sit at position 1 + P and this step's decode draws token P + 1
             for slots, r in joined:
@@ -886,20 +1022,27 @@ class LLM:
                     for i in slots:
                         st["pos"][[i, B + i] if R == 2 * B else [i]] = self.model.cls_token_num + P
                         self._depth[i] = P + 1
-        # a request whose join drew its last token (P = max_tokens - 1) finishes now, before a decode could write past its out row
-        outs = self._finish_c2i(st, [i for i, _ in flat if self._depth[i] >= S])
-        # (2) one decode step for every slot, (3) per-request sampling; the sampled token becomes the slot's next input in place
+        # a request whose join drew its last drawn token (P = max_tokens - 1, or a given tail after P) finishes now, before a decode could
+        # write past its out row
+        outs = self._finish_c2i(st, [i for i, r in flat if self._depth[i] >= r.end])
+        # (2) one decode step for every slot, (3) per-request sampling; the sampled token becomes the slot's next input in place; then the
+        # extends of the slots whose decode row drew the first token of a given run
+        ext = []
         if self._running():
+            ext = self._extends()
             self._device_step(st, params)
             st["pos"] += st["active"]
             st["tok"] *= st["active"][:B]                    # free slots keep a valid (class 0) input; their rows are never read
+            self._run_extends(st, params, ext)
         self.steps_run += 1
         # (4) bookkeeping on the host (no EOS: depths are known without reading the device)
         done = []
+        extended = {i for i, _, _ in ext}
         for i in range(B):
             if self._slots[i] is not None:
-                self._depth[i] += 1
-                if self._depth[i] >= S:
+                if i not in extended:
+                    self._depth[i] += 1
+                if self._depth[i] >= self._slots[i].end:
                     done.append(i)
         return outs + self._finish_c2i(st, done)
 
@@ -937,14 +1080,26 @@ class LLM:
             raise ValueError(f"prefixes holds {len(prefixes)} entries for {n} requests (c2i with CFG: one per conditional prompt)")
         return [self._prefix(p, sp) for p, sp in zip(prefixes, per)]
 
+    def _givens(self, givens, given_masks, n: int, per: List[SamplingParams], pfx) -> List[Optional[torch.Tensor]]:
+        """LLM.generate's givens / given_masks, one per request (or None), each pair checked as add_request checks it."""
+        if givens is None and given_masks is None:
+            return [None] * n
+        givens = [None] * n if givens is None else list(givens)
+        given_masks = [None] * n if given_masks is None else list(given_masks)
+        if len(givens) != n or len(given_masks) != n:
+            raise ValueError(f"givens / given_masks hold {len(givens)} / {len(given_masks)} entries for {n} requests (c2i with CFG: one "
+                             f"per conditional prompt)")
+        return [self._given(g, m, sp, pf) for g, m, sp, pf in zip(givens, given_masks, per, pfx)]
+
     def generate(self, prompts=None, sampling_params=None, prompt_token_ids: Optional[List[List[int]]] = None,
                  use_tqdm: bool = False, prompt_embeds=None, prefixes=None, negative_prompt_embeds=None,
-                 negative_prompts=None) -> List[RequestOutput]:
+                 negative_prompts=None, givens=None, given_masks=None) -> List[RequestOutput]:
         """c2i: prompt_token_ids, one [class id] per request (with CFG followed by one [num_classes] twin each). t2i: prompt_embeds, one
         caption's T5 features per request (see add_request). prefixes: None, or one prefix (see add_request) or None per request; under
         c2i CFG one per conditional prompt, which its twin mirrors. negative_prompt_embeds (t2i, cfg_scale > 1): None, or one negative
         caption's features or None per request; negative_prompts: the same as strings (or None), with a text_encoder, encoded in one call
-        with prompts. Returns the RequestOutputs sorted by request id."""
+        with prompts. givens, given_masks: None, or one inpainting request's given tokens and mask (see add_request) or None per request;
+        under c2i CFG one per conditional prompt, which its twin mirrors. Returns the RequestOutputs sorted by request id."""
         if negative_prompts is not None:
             if negative_prompt_embeds is not None:
                 raise ValueError("pass negative_prompts or negative_prompt_embeds, not both")
@@ -975,8 +1130,11 @@ class LLM:
             captions = [self._caption(f) for f in prompt_embeds]       # is queued
             negs = [self._negative(f, s) for f, s in zip(negative_prompt_embeds or [None] * n, scales)]
             pfx = self._prefixes(prefixes, n, per)
-            for c, p, pf, ng in zip(captions, per, pfx, negs):
-                if ng is None:
+            gvs = self._givens(givens, given_masks, n, per, pfx)
+            for c, p, pf, ng, gv in zip(captions, per, pfx, negs, gvs):
+                if gv is not None:
+                    self._enqueue_t2i(c, p, pf, ng, gv)
+                elif ng is None:
                     self._enqueue_t2i(c, p, pf)
                 else:
                     self._enqueue_t2i(c, p, pf, ng)
@@ -1004,7 +1162,10 @@ class LLM:
             raise ValueError("cfg_scale > 1 expects the serving protocol of serve/sample_c2i.py:35-37: the conditional prompts "
                              "followed by one [num_classes] prompt each")
         pfx = self._prefixes(prefixes, half if paired else n, per)
-        ids = [self.add_request(prompt_token_ids[i], per[i], prefix=pfx[i]) for i in range(half if paired else n)]
+        gvs = self._givens(givens, given_masks, half if paired else n, per, pfx)
+        ids = [self.add_request(prompt_token_ids[i], per[i], prefix=pfx[i]) if gvs[i] is None else
+               self.add_request(prompt_token_ids[i], per[i], prefix=pfx[i], given=gvs[i], given_mask=gvs[i] >= 0)
+               for i in range(half if paired else n)]
         if paired:
             for i in range(half):
                 self.add_request(prompt_token_ids[half + i], per[half + i], twin_of=ids[i])
