@@ -315,6 +315,26 @@ int  lg_given_workspace_bytes(lg_engine* e, const int32_t* given, int B, int S, 
 int  lg_generate_given(lg_engine* e, const void* cond, const float* emb_mask, const void* neg_cond, const float* neg_mask, int B, int T,
                        int S, const lg_sample_cfg* sc, const int32_t* given, void* dev_ws, size_t ws_bytes, int32_t* out_tokens,
                        void* stream);
+/* ---- composable guidance: generate() that steers every image with K weighted conditions -------------------------------------------
+ * B images, K conditions each (1 <= K <= 8, B * K <= 65535). Image j's K conditions are rows j K + i of R = B K conditional rows
+ * (image-major), paired with R unconditional rows; the prefill, decode, attention, masks and KV cache run on them as on R images of
+ * lg_generate (the workspace needs rows >= 2R and max_seq >= T + S). Per row (R rows, image-major): cond (c2i: int32 [R] class ids in
+ * [0, num_classes), unchecked on the device; t2i: [R, T, caption_dim]), emb_mask [R, T] or NULL, neg_cond / neg_mask as for
+ * lg_generate_neg or NULL, prefix dev int32 [R, P], given HOST int32 [R, S] (as lg_generate_given's): the caller repeats an image's
+ * negative, prefix and given row K times (the call refuses given rows of an image that differ). weights: dev f32 [B, K], finite.
+ * Every token of image j is drawn from x = u + d, d = w_1 (c_1 - u) + w_2 (c_2 - u) + ... accumulated left to right in fp32, where
+ * c_i is the logit row of row j K + i and u that of unconditional row R + j K (the null condition, or the negative; it attends with
+ * row j K's emb_mask, or its neg_mask), each row rounded to the model dtype first. Temperature, top-k, top-p, greedy and the RNG key
+ * (seed, token index, image j) are lg_generate's; sc->cfg_scale is unused (the weights are the scales) and sc->cfg_interval must be
+ * < 0 unless K = 1, where it drops the mix as in lg_generate. So K = 1 with weight s > 1 draws lg_generate's tokens at cfg_scale = s,
+ * and a zero weight drops its condition. The other R - B unconditional rows are computed and never read.
+ * out_tokens dev int32 [B, S]; lp: NULL or logprobs as for lg_generate_logprobs, [B, S] (of the composed distribution). P = 0 and
+ * given NULL: lg_generate's plan; 1 <= P <= S - 1: lg_generate_prefix's (dev_ws as there, for 2R rows); given: lg_generate_given's
+ * (dev_ws: lg_given_workspace_bytes of the R given rows with use_cfg; no prefix, no logprobs). Every argument is checked before any
+ * launch. */
+int  lg_generate_composed(lg_engine* e, const void* cond, const float* emb_mask, const void* neg_cond, const float* neg_mask, int B, int K,
+                          int T, int S, const lg_sample_cfg* sc, const float* weights, const int32_t* prefix, int P, const int32_t* given,
+                          void* dev_ws, size_t ws_bytes, const lg_logprobs* lp, int32_t* out_tokens, void* stream);
 /* Bytes of caller-provided scratch for lg_extend_slot with a run of K given tokens, K in [1, block_size - 2] (c2i and t2i models). */
 int  lg_slot_extend_workspace_bytes(lg_engine* e, int use_cfg, int K, size_t* bytes);
 /* The EXTEND of one serving slot (an inpainting request): tokens dev int32 [S], the slot's token row, holds the drawn token a - 1 and
@@ -582,6 +602,11 @@ int  lg_test_given_plan(const int32_t* given, int B, int S, int32_t* segs_out, i
 int  lg_test_sample_given(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc,
                           const uint64_t* seed_rows, const int32_t* step_rows, const int32_t* given, int32_t* out_idx, int32_t* out_seq,
                           int seq_stride, int32_t* next_tokens, void* stream);
+/* Test hook: the sample kernel's composable-guidance mix alone. logits f32 [2 B K, V]: image b's conditional rows b K + i and its
+ * unconditional row B K + b K (the other unconditional rows are not read); weights dev f32 [B, K]; seed_rows / step_rows dev [B] (both
+ * NULL: sc->seed, step 0, image b). out_idx dev int32 [B]; next_tokens dev int32 [B K] or NULL (image b's token in all K rows). */
+int  lg_test_sample_groups(const float* logits, int B, int K, int V, int round_dtype, const lg_sample_cfg* sc, const float* weights,
+                           const uint64_t* seed_rows, const int32_t* step_rows, int32_t* out_idx, int32_t* next_tokens, void* stream);
 /* The acceptance step of lg_generate_sjd alone, on caller buffers (dev): p, q f32 [B * L][V], qflag, x, win int32 [B * L], nfin,
  * start int32 [B] (updated), out int32 [B][S] (accepted tokens written). Every image must have nfin < S. */
 int  lg_test_sjd_verify(int B, int S, int L, int V, int greedy, uint64_t seed, const float* p, const float* q, const int32_t* qflag,

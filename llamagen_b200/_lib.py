@@ -49,6 +49,7 @@ class Logprobs(Structure):
 
 
 MAX_TOP_LOGPROBS = 20
+MAX_COMPOSE = 8     # conditions per image of composable guidance (lg_generate_composed)
 
 
 class T5Cfg(Structure):
@@ -117,6 +118,10 @@ SIGNATURES = {
     "lg_given_workspace_bytes": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_size_t)]),
     "lg_generate_given": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p,
                                   c_void_p, c_size_t, c_void_p, c_void_p]),
+    "lg_generate_composed": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, POINTER(SampleCfg),
+                                     c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_size_t, POINTER(Logprobs), c_void_p, c_void_p]),
+    "lg_test_sample_groups": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p, c_void_p, c_void_p, c_void_p,
+                                      c_void_p, c_void_p]),
     "lg_slot_extend_workspace_bytes": (c_int, [c_void_p, c_int, c_int, POINTER(c_size_t)]),
     "lg_extend_slot": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t,
                                c_void_p, c_void_p]),

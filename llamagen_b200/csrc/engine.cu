@@ -1205,9 +1205,18 @@ struct PrefixArgs {              // lg_generate_prefix: prefix [B, P] and the pr
     char* window = nullptr;
     int W = 0;
 };
+// lg_generate_composed: every image is K consecutive rows of each half (its K conditions, and K copies of its unconditional row), mixed
+// by the sample kernel's grouped mode with weights dev f32 [B / K][K]. Every per-row input (cond, masks, negatives, prefix, given) has
+// a row per row; out_tokens and the logprobs have one per image. K = 1 with null weights: one row per image, plain CFG.
+struct Compose {
+    int K = 1;
+    const float* weights = nullptr;
+};
 static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, const Negative& neg, int B, int T, int S,
                          const lg_sample_cfg* sc, int32_t* out_tokens, float* dbg_logits, const int32_t* teacher,
-                         const PrefixArgs& pa, const lg_logprobs* lp, cudaStream_t st);
+                         const PrefixArgs& pa, const lg_logprobs* lp, cudaStream_t st, const Compose& cp = Compose{});
+// Whether a call runs the unconditional rows: CFG (generate.py:128), or a composed call, which always mixes
+static bool uses_cfg(const lg_sample_cfg* sc, const Compose& cp) { return cp.weights || sc->cfg_scale > 1.0f; }
 
 }  // extern "C"
 
@@ -1226,12 +1235,12 @@ static size_t given_window_bytes(const lg_engine* e, int B, int nh, int W) {
 
 static int generate_entry(const char* fn, lg_engine* e, const void* cond, const float* emb_mask, const Negative& neg, int B, int T, int S,
                           const lg_sample_cfg* sc, int32_t* out_tokens, float* dbg_logits, const int32_t* teacher, void* stream,
-                          const lg_logprobs* lp = nullptr) {
+                          const lg_logprobs* lp = nullptr, const Compose& cp = Compose{}) {
     LG_REQUIRE(e, "%s: null engine", fn);
-    LG_TRY(check_negative(fn, e, neg, emb_mask, sc && sc->cfg_scale > 1.0f));
+    LG_TRY(check_negative(fn, e, neg, emb_mask, sc && uses_cfg(sc, cp)));
     DeviceGuard guard(e->device);
     return e->run_forked((cudaStream_t)stream, lg_engine::kMaxChains, [&](cudaStream_t st) {
-        return generate_impl(e, cond, emb_mask, neg, B, T, S, sc, out_tokens, dbg_logits, teacher, PrefixArgs{}, lp, st);
+        return generate_impl(e, cond, emb_mask, neg, B, T, S, sc, out_tokens, dbg_logits, teacher, PrefixArgs{}, lp, st, cp);
     });
 }
 
@@ -1259,7 +1268,8 @@ int lg_prefix_workspace_bytes(lg_engine* e, int rows, int seq, size_t* bytes) {
 
 static int generate_prefix_entry(const char* fn, lg_engine* e, const void* cond, const float* emb_mask, const Negative& neg, int B, int T,
                                  int S, const lg_sample_cfg* sc, const int32_t* prefix, int P, void* dev_ws, size_t ws_bytes,
-                                 int32_t* out_tokens, float* dbg_logits, void* stream, const lg_logprobs* lp = nullptr) {
+                                 int32_t* out_tokens, float* dbg_logits, void* stream, const lg_logprobs* lp = nullptr,
+                                 const Compose& cp = Compose{}) {
     LG_REQUIRE(e && e->finalized, "%s: engine not finalized", fn);
     DeviceGuard guard(e->device);
     const lg_model_cfg& c = e->cfg;
@@ -1268,7 +1278,7 @@ static int generate_prefix_entry(const char* fn, lg_engine* e, const void* cond,
     LG_REQUIRE(P >= 1 && P <= S - 1, "%s: prefix length P=%d outside [1, S - 1] (S=%d)", fn, P, S);
     LG_REQUIRE(T == c.cls_token_num, "%s: T=%d must equal cls_token_num=%d", fn, T, c.cls_token_num);
     LG_REQUIRE(!emb_mask || c.model_type == LG_MODEL_T2I, "%s: emb_mask only applies to t2i models", fn);
-    const int nh = sc->cfg_scale > 1.0f ? 2 : 1;   // generate.py:128
+    const int nh = uses_cfg(sc, cp) ? 2 : 1;   // generate.py:128
     LG_TRY(check_negative(fn, e, neg, emb_mask, nh == 2));
     LG_TRY(check_ready(e, nh * B, T + S));
     LG_REQUIRE(dev_ws && ((uintptr_t)dev_ws & 255) == 0, "%s: scratch must be non-null and 256-byte aligned", fn);
@@ -1277,7 +1287,7 @@ static int generate_prefix_entry(const char* fn, lg_engine* e, const void* cond,
     LG_REQUIRE(ws_bytes >= need1, "%s: scratch of %zu bytes is too small for one image (%zu)", fn, ws_bytes, need1);
     const PrefixArgs pa{prefix, P, (char*)dev_ws, ws_bytes};
     return e->run_forked((cudaStream_t)stream, lg_engine::kMaxChains, [&](cudaStream_t st) {
-        return generate_impl(e, cond, emb_mask, neg, B, T, S, sc, out_tokens, dbg_logits, nullptr, pa, lp, st);
+        return generate_impl(e, cond, emb_mask, neg, B, T, S, sc, out_tokens, dbg_logits, nullptr, pa, lp, st, cp);
     });
 }
 
@@ -1351,16 +1361,18 @@ int lg_given_workspace_bytes(lg_engine* e, const int32_t* given, int B, int S, i
     return 0;
 }
 
-int lg_generate_given(lg_engine* e, const void* cond, const float* emb_mask, const void* neg_cond, const float* neg_mask, int B, int T, int S,
-                      const lg_sample_cfg* sc, const int32_t* given, void* dev_ws, size_t ws_bytes, int32_t* out_tokens, void* stream) {
-    static const char* fn = "lg_generate_given";
+}  // extern "C"
+
+// lg_generate_given, and lg_generate_composed with given tokens (B: rows per half, given [B, S] per row, out_tokens [B / K, S])
+static int generate_given_impl(const char* fn, lg_engine* e, const void* cond, const float* emb_mask, const Negative& neg, int B, int T,
+                               int S, const lg_sample_cfg* sc, const int32_t* given, void* dev_ws, size_t ws_bytes, int32_t* out_tokens,
+                               void* stream, const Compose& cp = Compose{}) {
     LG_REQUIRE(e && e->finalized, "%s: engine not finalized", fn);
     const lg_model_cfg& c = e->cfg;
     LG_REQUIRE(cond && sc && out_tokens, "%s: null cond, sc or out_tokens", fn);
     LG_REQUIRE(T == c.cls_token_num, "%s: T=%d must equal cls_token_num=%d", fn, T, c.cls_token_num);
     LG_REQUIRE(!emb_mask || c.model_type == LG_MODEL_T2I, "%s: emb_mask only applies to t2i models", fn);
-    const int nh = sc->cfg_scale > 1.0f ? 2 : 1;   // generate.py:128
-    const Negative neg{neg_cond, neg_mask};
+    const int nh = uses_cfg(sc, cp) ? 2 : 1;   // generate.py:128
     LG_TRY(check_negative(fn, e, neg, emb_mask, nh == 2));
     std::vector<GivenSeg> segs;
     size_t fixed = 0, prefill = 0;
@@ -1390,10 +1402,22 @@ int lg_generate_given(lg_engine* e, const void* cond, const float* emb_mask, con
     for (int b = 0; b < B; ++b) std::copy(given + (size_t)b * S, given + (size_t)b * S + P, lead_host + (size_t)b * P);
     LG_CUDA_OK(cudaMemcpyAsync(base, e->given_host, up, cudaMemcpyHostToDevice, caller));
     LG_CUDA_OK(cudaEventRecord(e->ev_given, caller));
-    LG_CUDA_OK(cudaMemcpyAsync(out_tokens, given_dev, (size_t)B * S * sizeof(int32_t), cudaMemcpyDeviceToDevice, caller));
+    if (cp.K == 1)
+        LG_CUDA_OK(cudaMemcpyAsync(out_tokens, given_dev, (size_t)B * S * sizeof(int32_t), cudaMemcpyDeviceToDevice, caller));
+    else   // an image's K rows hold the same given tokens: row j K of each image
+        LG_CUDA_OK(cudaMemcpy2DAsync(out_tokens, (size_t)S * sizeof(int32_t), given_dev, (size_t)cp.K * S * sizeof(int32_t),
+                                     (size_t)S * sizeof(int32_t), B / cp.K, cudaMemcpyDeviceToDevice, caller));
     return e->run_forked(caller, lg_engine::kMaxChains, [&](cudaStream_t st) {
-        return generate_impl(e, cond, emb_mask, neg, B, T, S, sc, out_tokens, nullptr, nullptr, pa, nullptr, st);
+        return generate_impl(e, cond, emb_mask, neg, B, T, S, sc, out_tokens, nullptr, nullptr, pa, nullptr, st, cp);
     });
+}
+
+extern "C" {
+
+int lg_generate_given(lg_engine* e, const void* cond, const float* emb_mask, const void* neg_cond, const float* neg_mask, int B, int T, int S,
+                      const lg_sample_cfg* sc, const int32_t* given, void* dev_ws, size_t ws_bytes, int32_t* out_tokens, void* stream) {
+    return generate_given_impl("lg_generate_given", e, cond, emb_mask, Negative{neg_cond, neg_mask}, B, T, S, sc, given, dev_ws, ws_bytes,
+                               out_tokens, stream);
 }
 
 int lg_test_given_plan(const int32_t* given, int B, int S, int32_t* segs_out, int max_segs) {
@@ -1405,6 +1429,40 @@ int lg_test_given_plan(const int32_t* given, int B, int S, int32_t* segs_out, in
         segs_out[3 * i] = segs[i].kind; segs_out[3 * i + 1] = segs[i].start; segs_out[3 * i + 2] = segs[i].len;
     }
     return (int)segs.size();
+}
+
+int lg_generate_composed(lg_engine* e, const void* cond, const float* emb_mask, const void* neg_cond, const float* neg_mask, int B, int K,
+                         int T, int S, const lg_sample_cfg* sc, const float* weights, const int32_t* prefix, int P, const int32_t* given,
+                         void* dev_ws, size_t ws_bytes, const lg_logprobs* lp, int32_t* out_tokens, void* stream) {
+    static const char* fn = "lg_generate_composed";
+    LG_REQUIRE(e && e->finalized, "%s: engine not finalized", fn);
+    LG_REQUIRE(cond && sc && weights && out_tokens, "%s: null cond, sc, weights or out_tokens", fn);
+    LG_REQUIRE(B > 0 && K >= 1 && K <= kMaxMixGroups && (long long)B * K <= 65535 && S > 0,
+               "%s: B=%d, K=%d outside [1, %d], or S=%d", fn, B, K, kMaxMixGroups, S);
+    LG_REQUIRE(K == 1 || sc->cfg_interval < 0, "%s: cfg_interval=%d needs K = 1 (got K=%d)", fn, sc->cfg_interval, K);
+    LG_REQUIRE(P >= 0 && P <= S - 1 && (P > 0) == (prefix != nullptr), "%s: prefix length P=%d outside [0, S - 1], or prefix %s", fn, P,
+               prefix ? "given with P = 0" : "null");
+    bool lp_on = false;
+    LG_TRY(check_logprobs(fn, lp, &lp_on));
+    LG_REQUIRE(!given || (P == 0 && !lp_on), "%s: given tokens take no prefix and no logprobs", fn);
+    const int R = B * K;   // rows per half
+    const Compose cp{K, weights};
+    const Negative neg{neg_cond, neg_mask};
+    if (given) {
+        // the rows of an image carry one token row: refuse rows that disagree before the upload
+        for (int j = 0; j < B; ++j)
+            for (int i = 1; i < K; ++i)
+                LG_REQUIRE(std::equal(given + (size_t)j * K * S, given + ((size_t)j * K + 1) * S, given + ((size_t)j * K + i) * S),
+                           "%s: given row %d of image %d differs from its row 0", fn, i, j);
+        return generate_given_impl(fn, e, cond, emb_mask, neg, R, T, S, sc, given, dev_ws, ws_bytes, out_tokens, stream, cp);
+    }
+    LG_REQUIRE(T == e->cfg.cls_token_num, "%s: T=%d must equal cls_token_num=%d", fn, T, e->cfg.cls_token_num);
+    LG_REQUIRE(!emb_mask || e->cfg.model_type == LG_MODEL_T2I, "%s: emb_mask only applies to t2i models", fn);
+    LG_TRY(check_negative(fn, e, neg, emb_mask, true));
+    LG_TRY(check_ready(e, 2 * R, T + S));
+    if (P == 0) return generate_entry(fn, e, cond, emb_mask, neg, R, T, S, sc, out_tokens, nullptr, nullptr, stream, lp_on ? lp : nullptr, cp);
+    return generate_prefix_entry(fn, e, cond, emb_mask, neg, R, T, S, sc, prefix, P, dev_ws, ws_bytes, out_tokens, nullptr, stream,
+                                 lp_on ? lp : nullptr, cp);
 }
 
 namespace {
@@ -1661,9 +1719,10 @@ int lg_extend_slot(lg_engine* e, const int32_t* tokens, int S, int a, int K, int
 
 static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, const Negative& neg, int B, int T, int S,
                          const lg_sample_cfg* sc, int32_t* out_tokens, float* dbg_logits, const int32_t* teacher,
-                         const PrefixArgs& pa, const lg_logprobs* lp, cudaStream_t st0) {
-    LG_REQUIRE(cond && sc && out_tokens && B > 0 && S > 0, "lg_generate: bad argument");
-    const bool use_cfg = sc->cfg_scale > 1.0f;  // generate.py:128
+                         const PrefixArgs& pa, const lg_logprobs* lp, cudaStream_t st0, const Compose& cp) {
+    LG_REQUIRE(cond && sc && out_tokens && B > 0 && S > 0 && cp.K >= 1 && B % cp.K == 0, "lg_generate: bad argument");
+    const bool use_cfg = uses_cfg(sc, cp);  // generate.py:128
+    const int K = cp.K;   // rows per image and half; B rows per half are B / K images
     const int R = use_cfg ? 2 * B : B;
     LG_TRY(check_ready(e, R, T + S));
     LG_REQUIRE(T == e->cfg.cls_token_num, "lg_generate: T=%d must equal cls_token_num=%d", T, e->cfg.cls_token_num);
@@ -1673,8 +1732,8 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
     // Multi-chain decode: at large batch every kernel of a decode step is latency-bound (a few microseconds of
     // dependent load -> compute -> store), so the batch is cut into n_sub independent chains (the chain-count policy of
     // lg_engine_set_workspace, which LG_SPLIT overrides; each chain has its own KV-cache slice, stream and CUDA graph) whose kernels interleave on the GPU. Each image's arithmetic is unchanged, so the result
-    // is bit-identical to the single-chain run.
-    const bool split = e->n_sub >= 2 && lg_env_flag("LG_SPLIT", 2) >= 2 && R == e->full.rows && B % e->n_sub == 0 &&
+    // is bit-identical to the single-chain run. A chain never splits an image's K rows.
+    const bool split = e->n_sub >= 2 && lg_env_flag("LG_SPLIT", 2) >= 2 && R == e->full.rows && (B / K) % e->n_sub == 0 &&
                        !prof_enabled() && !lg_debug_sync();
     const int nchains = split ? e->n_sub : 1;
     Chain ch[lg_engine::kMaxChains];
@@ -1684,7 +1743,7 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
         k.st = g == 0 ? st0 : e->works[g];
         k.B = B / nchains;
         k.R = R / nchains;
-        const size_t boff = (size_t)g * k.B;
+        const size_t boff = (size_t)g * k.B, ioff = boff / K;   // the chain's first row and first image
         k.cond = c.model_type == LG_MODEL_C2I ? (const void*)((const int32_t*)cond + boff)
                                               : (const void*)((const char*)cond + boff * T * c.caption_dim * e->esz);
         k.emb_mask = emb_mask ? emb_mask + boff * T : nullptr;
@@ -1694,11 +1753,12 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
         k.sa = make_sample_args(*sc, k.w.logits, k.B, c.vocab_size, use_cfg, c.dtype);
         SampleArgs& sa = k.sa;
         sa.row_offset = (int)boff;
-        sa.out_seq = out_tokens + boff * S; sa.seq_stride = S; sa.next_tokens = k.w.tokens;
-        sa.teacher = teacher ? teacher + boff * S : nullptr;
+        sa.out_seq = out_tokens + ioff * S; sa.seq_stride = S; sa.next_tokens = k.w.tokens;
+        sa.teacher = teacher ? teacher + ioff * S : nullptr;
         sa.given = pa.given ? pa.given + boff * S : nullptr;
         sa.dbg_logits = dbg_logits; sa.dbg_batch = B;
-        apply_logprobs(sa, lp, boff * S);
+        if (cp.weights) { sa.mix_groups = K; sa.mix_weights = cp.weights + boff; }
+        apply_logprobs(sa, lp, ioff * S);
     }
     std::vector<GivenSeg> lead_decode;   // lg_generate and lg_generate_prefix: LEAD P, then one DECODE run to the end
     if (!pa.segs) {
@@ -1763,17 +1823,17 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
             if (e->carve_prefix(rb, nullptr, n, seq) > pa.scratch_bytes) return false;
             return attn_plan(e->attn_args(ch[0].w, 0, n, seq)).kernel >= 0;
         };
-        const int blk = B % lg_engine::kMaxChains == 0 ? B / lg_engine::kMaxChains : B;   // one chain's images under the largest split
+        const int blk = (B / K) % lg_engine::kMaxChains == 0 ? B / lg_engine::kMaxChains : B;   // one chain's rows under the largest split
         int lo = 1, hi = blk;       // largest chunk that fits
         while (lo < hi) {
             const int mid = lo + (hi - lo + 1) / 2;
             if (fits(mid)) lo = mid; else hi = mid - 1;
         }
         LG_REQUIRE(fits(lo), "lg_generate_prefix: no chunk of rows fits the scratch (%zu bytes) and the attention grid", pa.scratch_bytes);
-        LG_CUDA_OK(cudaMemcpy2DAsync(out_tokens, (size_t)S * sizeof(int32_t), pa.prefix, (size_t)P * sizeof(int32_t),
-                                     (size_t)P * sizeof(int32_t), B, cudaMemcpyDeviceToDevice, st0));
+        LG_CUDA_OK(cudaMemcpy2DAsync(out_tokens, (size_t)S * sizeof(int32_t), pa.prefix, (size_t)K * P * sizeof(int32_t),
+                                     (size_t)P * sizeof(int32_t), B / K, cudaMemcpyDeviceToDevice, st0));   // row j K of image j
         if (lp) LG_TRY(launch_given_logprobs(lp->logprob, lp->rank, lp->top_n > 0 ? lp->top_ids : nullptr,
-                                             lp->top_n > 0 ? lp->top_logprob : nullptr, lp->top_n, B, S, P, st0));
+                                             lp->top_n > 0 ? lp->top_logprob : nullptr, lp->top_n, B / K, S, P, st0));
         e->prefix_chunks = 0;
         e->prefix_chains = nchains;
         for (int g = 0; g < nchains; ++g) LG_TRY(prefix_prefill(e, ch[g], nh, T, P, lo, blk, pa, st0));
@@ -2190,6 +2250,20 @@ int lg_test_sample_given(const float* logits, int B, int V, int mix_cfg, int rou
     SampleArgs a = make_sample_args(*sc, logits, B, V, mix_cfg, round_dtype);
     a.seed_rows = seed_rows; a.step_rows = step_rows; a.given = given;
     a.out_idx = out_idx; a.out_seq = out_seq; a.seq_stride = seq_stride; a.next_tokens = next_tokens;
+    return launch_sample(a, (cudaStream_t)stream);
+}
+
+int lg_test_sample_groups(const float* logits, int B, int K, int V, int round_dtype, const lg_sample_cfg* sc, const float* weights,
+                          const uint64_t* seed_rows, const int32_t* step_rows, int32_t* out_idx, int32_t* next_tokens, void* stream) {
+    static const char* fn = "lg_test_sample_groups";
+    LG_REQUIRE(logits && sc && weights && out_idx, "%s: null logits, sc, weights or out_idx", fn);
+    LG_REQUIRE(B > 0 && K >= 1 && K <= kMaxMixGroups && V > 0, "%s: bad shape B=%d K=%d V=%d", fn, B, K, V);
+    LG_REQUIRE((seed_rows != nullptr) == (step_rows != nullptr), "%s: seed_rows and step_rows go together", fn);
+    LG_REQUIRE(round_dtype == LG_DTYPE_F32 || lg_dtype_is16(round_dtype), "%s: unsupported round dtype %d", fn, round_dtype);
+    SampleArgs a = make_sample_args(*sc, logits, B * K, V, 1, round_dtype);
+    a.mix_groups = K; a.mix_weights = weights;
+    a.seed_rows = seed_rows; a.step_rows = step_rows;
+    a.out_idx = out_idx; a.next_tokens = next_tokens;
     return launch_sample(a, (cudaStream_t)stream);
 }
 

@@ -66,8 +66,16 @@ struct SampleArgs {
     // inpainting (lg_generate_given): [B, seq_stride] or null; a value >= 0 at element b * seq_stride + step is image b's given token
     // there: it goes to out_idx, out_seq, next_tokens and the fused tail in place of the draw (-1: the draw)
     const int32_t* given = nullptr;
+    // composable guidance (lg_generate_composed): mix_groups = K > 0 makes the B rows of each half B / K images of K rows, image j's
+    // rows j K .. j K + K - 1; one CTA per image mixes x = u + w_1 (c_1 - u) + ... + w_K (c_K - u) (left to right, in fp32) from its
+    // conditional rows and the unconditional row B + j K, with mix_weights [B / K][K]. Image j's draw keys as image j + row_offset / K;
+    // out_idx, out_probs, out_seq, the logprobs, teacher, seed_rows, step_rows and img_rows are per image, given is read at row j K
+    // ([B][seq_stride]), and the token goes to next_tokens and the fused tail's rows of all 2K rows. 0: one row per image, as above
+    int mix_groups = 0;
+    const float* mix_weights = nullptr;
 };
 constexpr int kMaxTopLogprobs = 20;
+constexpr int kMaxMixGroups = 8;
 inline bool sample_wants_logprobs(const SampleArgs& a) { return a.lp_out || a.rank_out || a.top_ids || a.top_lp; }
 // The sample kernel stages the row with 16-byte loads (and dbg_logits with 16-byte stores) iff this holds, else element by element
 __host__ __device__ inline bool sample_vec_loads(const SampleArgs& a) {

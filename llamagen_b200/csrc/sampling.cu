@@ -122,8 +122,10 @@ __device__ void sample_logprobs(const SampleArgs& a, const float* xs, float* cx,
 }
 
 // E: the 16-bit type of the rounding (a.round_dtype != LG_DTYPE_F32) and of the fused tail's rows. kLogprobs: also write the token
-// log-probabilities (SampleArgs.lp_out ...); the draw is the same
-template <typename E, bool kLogprobs>
+// log-probabilities (SampleArgs.lp_out ...); the draw is the same. kGroups: composable guidance (SampleArgs.mix_groups = K): CTA b is
+// image b, which reads its K conditional rows b K .. b K + K - 1 and the unconditional row B + b K and mixes them with its weights;
+// every per-image output, input and key is image b's, and its token feeds all 2K of its rows
+template <typename E, bool kLogprobs, bool kGroups>
 __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
     using TR = ElemTraits<E>;
     lg_pdl_sync();
@@ -149,8 +151,9 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
     // generate.py:113-114 — decode iteration i = step-1; once i > cfg_interval the mix is dropped.
     if (mix && cfg_interval > -1 && step >= 1 && (long long)(step - 1) > (long long)cfg_interval) mix = false;
 
-    const float* lc = a.logits + (size_t)b * V;
-    const float* lu = a.logits + (size_t)(B + b) * V;
+    const int G = kGroups ? a.mix_groups : 1;   // rows per image and half
+    const float* lc = a.logits + (size_t)b * G * V;
+    const float* lu = a.logits + (size_t)(B + b * G) * V;
     const float tdiv = fmaxf(a.temperature, 1e-5f);
     const int dbgB = a.dbg_batch > 0 ? a.dbg_batch : B;
     float* dbg = a.dbg_logits ? a.dbg_logits + ((size_t)step * dbgB + a.row_offset + b) * V : nullptr;
@@ -161,7 +164,51 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
         if (a.round_dtype) u = TR::round(u);
         return __fadd_rn(u, __fmul_rn(__fsub_rn(c, u), cfg_scale));
     };
-    if (sample_vec_loads(a)) {
+    if constexpr (kGroups) {
+        // x = u + d, d = w_1 (c_1 - u) + ... + w_K (c_K - u) accumulated left to right, every row rounded first; K = 1 is mix1 with
+        // cfg_scale = w_1 exactly. Without the mix (cfg_interval passed, K = 1 only) x = c_1, as mix1
+        float w[kMaxMixGroups];
+#pragma unroll
+        for (int i = 0; i < kMaxMixGroups; ++i) w[i] = i < G ? a.mix_weights[(size_t)b * G + i] : 0.f;
+        auto rd = [&](float x) -> float { return a.round_dtype ? TR::round(x) : x; };
+        auto mixg = [&](int v) -> float {
+            const float c1 = rd(lc[v]);
+            if (!mix) return c1;
+            const float u = rd(lu[v]);
+            float d = __fmul_rn(__fsub_rn(c1, u), w[0]);
+#pragma unroll
+            for (int i = 1; i < kMaxMixGroups; ++i)
+                if (i < G) d = __fadd_rn(d, __fmul_rn(__fsub_rn(rd(lc[(size_t)i * V + v]), u), w[i]));
+            return __fadd_rn(u, d);
+        };
+        if (sample_vec_loads(a)) {   // 128-bit loads, as below
+            const float4* lc4 = reinterpret_cast<const float4*>(lc);
+            const float4* lu4 = reinterpret_cast<const float4*>(lu);
+            const int V4 = V >> 2;
+            auto rd4 = [&](float4 x) -> float4 { return make_float4(rd(x.x), rd(x.y), rd(x.z), rd(x.w)); };
+            auto term = [](float c, float u, float wi) { return __fmul_rn(__fsub_rn(c, u), wi); };
+#pragma unroll 2
+            for (int v4 = tid; v4 < V4; v4 += kSampleThreads) {
+                float4 x = rd4(lc4[v4]);
+                if (mix) {
+                    const float4 u = rd4(lu4[v4]);
+                    float4 d = make_float4(term(x.x, u.x, w[0]), term(x.y, u.y, w[0]), term(x.z, u.z, w[0]), term(x.w, u.w, w[0]));
+#pragma unroll
+                    for (int i = 1; i < kMaxMixGroups; ++i)
+                        if (i < G) {
+                            const float4 c = rd4(lc4[(size_t)i * V4 + v4]);
+                            d.x = __fadd_rn(d.x, term(c.x, u.x, w[i])); d.y = __fadd_rn(d.y, term(c.y, u.y, w[i]));
+                            d.z = __fadd_rn(d.z, term(c.z, u.z, w[i])); d.w = __fadd_rn(d.w, term(c.w, u.w, w[i]));
+                        }
+                    x = make_float4(__fadd_rn(u.x, d.x), __fadd_rn(u.y, d.y), __fadd_rn(u.z, d.z), __fadd_rn(u.w, d.w));
+                }
+                x.x = __fdiv_rn(x.x, tdiv); x.y = __fdiv_rn(x.y, tdiv); x.z = __fdiv_rn(x.z, tdiv); x.w = __fdiv_rn(x.w, tdiv);
+                reinterpret_cast<float4*>(sh)[v4] = x;
+            }
+        } else {
+            for (int v = tid; v < V; v += kSampleThreads) sh[v] = __fdiv_rn(mixg(v), tdiv);
+        }
+    } else if (sample_vec_loads(a)) {
         // 128-bit loads, several requests of a thread in flight before the first use (the scalar loop was
         // latency-bound: 16 dependent L2 round trips per thread); a caller's row that is not 16-byte aligned takes the scalar loop
         const float4* lc4 = reinterpret_cast<const float4*>(lc);
@@ -477,7 +524,8 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
         // per-request streams (seed_rows): every image draws exactly what a batch-of-one generate() with its seed would draw, or, with
         // img_rows, what image img_rows[b] of a generate() with its seed draws
         const uint64_t seed = a.seed_rows ? a.seed_rows[b] : a.seed;
-        const uint64_t rrow = a.seed_rows ? (a.img_rows ? (uint64_t)a.img_rows[b] + 1 : 1ull) : (uint64_t)(b + 1 + a.row_offset);
+        const uint64_t rrow = a.seed_rows ? (a.img_rows ? (uint64_t)a.img_rows[b] + 1 : 1ull)
+                                          : (uint64_t)(b + 1 + (kGroups ? a.row_offset / G : a.row_offset));
         const uint64_t r = splitmix64(splitmix64(seed ^ (0xA0761D6478BD642Full * (step + 1))) ^ (0xE7037ED1A0B428DBull * rrow));
         const float u = (float)(r >> 40) * (1.0f / 16777216.0f);
         const float target = u * total;
@@ -521,13 +569,19 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
     if (tid == 0) {
         int pick = s_pick;
         if (a.given) {   // a given token of an inpainting call replaces the draw
-            const int g = a.given[(size_t)b * a.seq_stride + step];
+            const int g = a.given[(size_t)b * G * a.seq_stride + step];
             if (g >= 0) pick = g;
         }
         if (a.out_idx) a.out_idx[b] = pick;
         if (a.out_seq) a.out_seq[(size_t)b * a.seq_stride + step] = pick;
         const int nxt = a.teacher ? a.teacher[(size_t)b * a.seq_stride + step] : pick;
-        if (a.next_tokens) a.next_tokens[b] = nxt;
+        if (a.next_tokens) {
+            if constexpr (kGroups) {
+                for (int i = 0; i < G; ++i) a.next_tokens[b * G + i] = nxt;
+            } else {
+                a.next_tokens[b] = nxt;
+            }
+        }
         s_next = nxt;
         if (a.dbg_path) {
             a.dbg_path[3 * b] = path_topk;
@@ -543,8 +597,9 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
         // thread -> 2 consecutive elements per pass (D even); the same token feeds the cond and the uncond row (generate.py:91)
         for (int i = tid * 2; i < D; i += kSampleThreads * 2) {
             const uint32_t w = *reinterpret_cast<const uint32_t*>(src + i);
-            for (int row = b; row < a.emb_rows; row += B)
-                *reinterpret_cast<uint32_t*>(reinterpret_cast<E*>(a.emb_h) + (size_t)row * D + i) = w;
+            for (int row = b * G; row < a.emb_rows; row += B)
+                for (int j = 0; j < G; ++j)   // G = 1 without kGroups
+                    *reinterpret_cast<uint32_t*>(reinterpret_cast<E*>(a.emb_h) + (size_t)(row + j) * D + i) = w;
         }
         if (a.emb_xn) {
             // sum of squares in rmsnorm_kernel's order (256 threads striding the row, then the same block reduction tree: the other
@@ -565,8 +620,9 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
                 const float lo = TR::round(TR::lo(w) * rinv) * TR::lo(g2);
                 const float hi = TR::round(TR::hi(w) * rinv) * TR::hi(g2);
                 const uint32_t pk = TR::pack2(lo, hi);
-                for (int row = b; row < a.emb_rows; row += B)
-                    *reinterpret_cast<uint32_t*>(reinterpret_cast<E*>(a.emb_xn) + (size_t)row * D + i) = pk;
+                for (int row = b * G; row < a.emb_rows; row += B)
+                    for (int j = 0; j < G; ++j)
+                        *reinterpret_cast<uint32_t*>(reinterpret_cast<E*>(a.emb_xn) + (size_t)(row + j) * D + i) = pk;
             }
         }
     }
@@ -598,14 +654,25 @@ int launch_sample(const SampleArgs& a, cudaStream_t st) {
                    (a.top_n == 0 || (a.top_ids && a.top_lp)),
                "lg_sample: top_n=%d outside [0, %d], or top_ids / top_logprob not both given exactly when top_n > 0", a.top_n,
                kMaxTopLogprobs);
+    const bool grp = a.mix_groups > 0;
+    if (grp) {
+        LG_REQUIRE(a.mix_groups <= kMaxMixGroups && a.B % a.mix_groups == 0 && a.mix_cfg && a.mix_weights,
+                   "lg_sample: composable guidance needs 1 <= K=%d <= %d dividing B=%d rows, mix_cfg and weights", a.mix_groups,
+                   kMaxMixGroups, a.B);
+        LG_REQUIRE(!a.cfg_rows && !a.interval_rows && !a.dbg_logits,
+                   "lg_sample: composable guidance takes no per-row guidance or dbg_logits");
+        LG_REQUIRE(!a.emb_table || a.emb_rows == a.B || a.emb_rows == 2 * a.B, "lg_sample: the fused tail of groups needs emb_rows B or 2B");
+    }
     const bool half = a.round_dtype == LG_DTYPE_F16;
-    auto kern = lp ? (half ? sample_kernel<f16, true> : sample_kernel<bf16, true>)
-                   : (half ? sample_kernel<f16, false> : sample_kernel<bf16, false>);
-    static DevOnce attr_set[4];
-    if (lg_first_on_device(attr_set[2 * lp + half])) {
+    auto kern = grp ? (lp ? (half ? sample_kernel<f16, true, true> : sample_kernel<bf16, true, true>)
+                          : (half ? sample_kernel<f16, false, true> : sample_kernel<bf16, false, true>))
+                    : lp ? (half ? sample_kernel<f16, true, false> : sample_kernel<bf16, true, false>)
+                         : (half ? sample_kernel<f16, false, false> : sample_kernel<bf16, false, false>);
+    static DevOnce attr_set[8];
+    if (lg_first_on_device(attr_set[4 * grp + 2 * lp + half])) {
         LG_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     }
-    (void)lg_launch(kern, dim3(a.B), dim3(kSampleThreads), smem, st, a);
+    (void)lg_launch(kern, dim3(grp ? a.B / a.mix_groups : a.B), dim3(kSampleThreads), smem, st, a);
     LG_LAUNCH_CHECK();
     return 0;
 }

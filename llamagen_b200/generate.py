@@ -77,6 +77,19 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
                            [B, S, N], "top_logprobs": f32 [B, S, N]}). rank = 1 + the number of tokens with a larger processed logit;
                            the top ids are the N kept tokens with the largest logits (ties: lower id first), -1 with logprob -inf past
                            the last kept token. Prefix rows: rank 0, ids -1, logprobs -inf.
+      cond_weights=floats  composable guidance (Liu et al. 2022 on logits): K weighted conditions per image, 1 <= K <= 8. cond is
+                           int [B, K] class ids in [0, num_classes) (c2i) or [B, K, T, C] captions prepared as cond is (t2i; emb_masks
+                           [B, K, T] or None); cond_weights is [K] (every image) or [B, K] (per image, e.g. an interpolation strip),
+                           finite, any sign, zeros allowed. Every token is drawn from x = u + d, d = w_1 (c_1 - u) + w_2 (c_2 - u) + ...
+                           accumulated left to right in fp32, c_i the logits under condition i and u those of the null condition (or
+                           negative_cond), every row rounded to the model dtype first; u attends with the emb-mask of condition 1, or
+                           with negative_emb_masks when a negative is given. Temperature, top-k / top-p, greedy and the RNG key (seed,
+                           token index, image index) are those of plain generation, so K = 1 with cond_weights=[s], s > 1, gives the
+                           tokens of cfg_scale=s bit for bit, and a zero weight drops its condition exactly. The call always mixes:
+                           cfg_scale must stay at its default; cfg_interval only with K = 1. Combines with negative_cond /
+                           negative_emb_masks ([1 or B, T, C] / [1 or B, T]), prefix ([B, P]), given / given_mask, return_logprobs /
+                           top_logprobs (of the composed distribution), fp16, fp8 KV caches and fp8 weights; not with sjd_window,
+                           teacher or return_logits. An image runs 2K rows through the model, of which K + 1 are read.
     """
     if not isinstance(model, Transformer):
         raise TypeError("llamagen_b200.generate needs a llamagen_b200 GPT_models[...] instance")
@@ -96,6 +109,7 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
     top_logprobs = sampling_kwargs.pop("top_logprobs", None)
     given = sampling_kwargs.pop("given", None)
     given_mask = sampling_kwargs.pop("given_mask", None)
+    cond_weights = sampling_kwargs.pop("cond_weights", None)
     if sampling_kwargs:
         raise TypeError(f"unexpected sampling kwargs: {sorted(sampling_kwargs)}")
     if top_logprobs is not None:
@@ -117,6 +131,15 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
             raise ValueError("sjd_window cannot be combined with teacher or return_logits")
     elif return_stats:
         raise ValueError("return_stats needs sjd_window")
+    if cond_weights is not None:
+        for name, on in (("sjd_window", sjd_window is not None), ("teacher", teacher is not None), ("return_logits", return_logits),
+                         ("return_stats", return_stats)):
+            if on:
+                raise ValueError(f"cond_weights cannot be combined with {name}")
+        return _generate_composed(model, cond, int(max_new_tokens), emb_masks, cfg_scale, cfg_interval, cond_weights,
+                                  temperature=temperature, top_k=top_k, top_p=top_p, sample_logits=sample_logits, seed=seed,
+                                  prefix=prefix, negative_cond=negative_cond, negative_emb_masks=negative_emb_masks,
+                                  return_logprobs=return_logprobs, top_logprobs=top_logprobs, given=given, given_mask=given_mask)
     if prefix is not None and (teacher is not None or sjd_window is not None):
         raise ValueError("prefix cannot be combined with teacher or sjd_window")
     pf = _check_prefix(prefix, cond.shape[0], int(max_new_tokens), model.vocab_size) if prefix is not None else None
@@ -212,6 +235,127 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
     if cond.device != dev:
         out = out.to(cond.device)
     return (out, dbg) if return_logits else out
+
+
+def _check_compose(model, cond, S, emb_masks, cfg_scale, cfg_interval, cond_weights, negative_cond, negative_emb_masks):
+    """generate(cond_weights=...)'s checks, before anything reaches the device. Returns (B, K, T, weights f32 host [B, K])."""
+    if not isinstance(model, Transformer):
+        raise TypeError("llamagen_b200.generate needs a llamagen_b200 GPT_models[...] instance")
+    if cfg_scale != 1.0:
+        raise ValueError(f"cond_weights are the guidance scales of a composed call; leave cfg_scale at its default (got {cfg_scale})")
+    w = torch.as_tensor(cond_weights)
+    if w.dtype == torch.bool or w.dtype.is_complex:
+        raise ValueError(f"cond_weights must be real numbers, got dtype {w.dtype}")
+    w = w.detach().to("cpu", torch.float64)
+    if w.dim() not in (1, 2):
+        raise ValueError(f"cond_weights must be [K] or [B, K], got {tuple(w.shape)}")
+    K = w.shape[-1]
+    if not 1 <= K <= _lib.MAX_COMPOSE:
+        raise ValueError(f"cond_weights has K={K} conditions per image; K must lie in [1, {_lib.MAX_COMPOSE}]")
+    if not bool(torch.isfinite(w).all()) or not bool(torch.isfinite(w.float()).all()):
+        raise ValueError("cond_weights must be finite (in fp32)")
+    if cfg_interval != -1 and K > 1:
+        raise ValueError(f"cfg_interval applies to a composed call only with K = 1 (got K={K}, cfg_interval={cfg_interval})")
+    if not torch.is_tensor(cond):
+        raise ValueError("cond must be a tensor")
+    if model.model_type == "c2i":
+        if cond.dtype.is_floating_point or cond.dtype.is_complex or cond.dtype == torch.bool:
+            raise ValueError(f"c2i cond of a composed call must be an integer tensor of class ids, got dtype {cond.dtype}")
+        if cond.dim() != 2 or cond.shape[1] != K or cond.shape[0] < 1:
+            raise ValueError(f"c2i cond of a composed call must be [B, K] = [B, {K}], got {tuple(cond.shape)}")
+        c = cond.detach().to("cpu", torch.int64)
+        if bool(((c < 0) | (c >= model.num_classes)).any()):
+            raise ValueError(f"class ids must lie in [0, num_classes={model.num_classes})")
+        if emb_masks is not None or negative_cond is not None or negative_emb_masks is not None:
+            raise ValueError("emb_masks and negative prompts apply to text-conditional (t2i) models")
+        T = 1
+    elif model.model_type == "t2i":
+        T, C = model.cls_token_num, model.config.caption_dim
+        if cond.dim() != 4 or cond.shape[0] < 1 or tuple(cond.shape[1:]) != (K, T, C):
+            raise ValueError(f"t2i cond of a composed call must be [B, K, T, C] = [B, {K}, {T}, {C}], got {tuple(cond.shape)}")
+        B = cond.shape[0]
+        if emb_masks is not None and tuple(emb_masks.shape) != (B, K, T):
+            raise ValueError(f"emb_masks of a composed call must be [B, K, T] = [{B}, {K}, {T}], got {tuple(emb_masks.shape)}")
+        if negative_emb_masks is not None and negative_cond is None:
+            raise ValueError("negative_emb_masks needs negative_cond")
+        if negative_cond is not None and (negative_cond.dim() != 3 or negative_cond.shape[0] not in (1, B)
+                                          or tuple(negative_cond.shape[1:]) != (T, C)):
+            raise ValueError(f"negative_cond must be [1, T, C] or [B, T, C] = [{B}, {T}, {C}], got {tuple(negative_cond.shape)}")
+        if negative_emb_masks is not None and (negative_emb_masks.dim() != 2 or negative_emb_masks.shape[0] not in (1, B)
+                                               or negative_emb_masks.shape[1] != T):
+            raise ValueError(f"negative_emb_masks must be [1, T] or [B, T] = [{B}, {T}], got {tuple(negative_emb_masks.shape)}")
+    else:
+        raise Exception("please check model type")
+    B = cond.shape[0]
+    if w.dim() == 2 and w.shape[0] != B:
+        raise ValueError(f"cond_weights must be [K] or [B, K] = [{B}, {K}], got {tuple(w.shape)}")
+    if S < 1:
+        raise ValueError(f"max_new_tokens must be >= 1, got {S}")
+    return B, K, T, w.float().expand(B, K).contiguous()
+
+
+def _generate_composed(model, cond, S, emb_masks, cfg_scale, cfg_interval, cond_weights, *, temperature, top_k, top_p, sample_logits,
+                       seed, prefix, negative_cond, negative_emb_masks, return_logprobs, top_logprobs, given, given_mask):
+    """generate(cond_weights=...): lg_generate_composed over B * K conditional rows (image-major) and as many unconditional rows."""
+    B, K, T, w = _check_compose(model, cond, S, emb_masks, cfg_scale, cfg_interval, cond_weights, negative_cond, negative_emb_masks)
+    if prefix is not None and (given is not None or given_mask is not None):
+        raise ValueError("given / given_mask cannot be combined with prefix")
+    if return_logprobs and (given is not None or given_mask is not None):
+        raise ValueError("given / given_mask cannot be combined with return_logprobs")
+    pf = _check_prefix(prefix, B, S, model.vocab_size) if prefix is not None else None
+    gv = _check_given(given, given_mask, B, S, model.vocab_size) if given is not None or given_mask is not None else None
+
+    dev = model.tok_embeddings.weight.device
+    _lib.require_cuda(model.tok_embeddings.weight, "generate")
+    R = B * K
+    if model.model_type == "c2i":
+        cond_dev = cond.reshape(R).to(device=dev, dtype=torch.int32).contiguous()
+    else:
+        cond_dev = cond.reshape(R, T, cond.shape[3]).to(device=dev, dtype=model.tok_embeddings.weight.dtype).contiguous()
+    em = None if emb_masks is None else emb_masks.reshape(R, T).to(device=dev, dtype=torch.float32).contiguous()
+    neg = nm = None
+    if negative_cond is not None:   # an image's negative and its mask repeat on its K rows; a missing mask is all ones
+        neg = negative_cond.to(device=dev, dtype=cond_dev.dtype).expand(B, T, cond_dev.shape[2]).repeat_interleave(K, 0).contiguous()
+        ones = torch.ones(R, T, dtype=torch.float32, device=dev)
+        em = ones if em is None else em
+        nm = ones if negative_emb_masks is None else \
+            negative_emb_masks.to(device=dev, dtype=torch.float32).expand(B, T).repeat_interleave(K, 0).contiguous()
+    w_dev = w.to(dev)
+    model.setup_caches(max_batch_size=2 * R, max_seq_length=T + S, dtype=model.tok_embeddings.weight.dtype)
+    lib, handle = _lib.load(), model.engine()
+    out = torch.empty((B, S), dtype=torch.int32, device=dev)
+    sc = _lib.SampleCfg(float(cfg_scale), int(cfg_interval), temperature, top_k, top_p, 0 if sample_logits else 1,
+                        _draw_seed() if seed is None else int(seed))
+    P, pf_dev, g_rows, ws, ws_bytes = 0, None, None, None, 0
+    if pf is not None:
+        P = pf.shape[1]
+        pf_dev = pf.repeat_interleave(K, 0).to(device=dev, dtype=torch.int32).contiguous()
+        ws, ws_bytes = model._prefix_scratch(2 * R, T + P, 2)
+    if gv is not None:
+        g_rows = gv.repeat_interleave(K, 0).contiguous()
+        ws, ws_bytes = model._given_scratch(g_rows, T, True)
+    extra, spec = None, None
+    if return_logprobs:
+        top_n = None if top_logprobs is None else int(top_logprobs)
+        lp = torch.empty((B, S), dtype=torch.float32, device=dev)
+        if top_n is not None:
+            extra = {"ranks": torch.empty((B, S), dtype=torch.int32, device=dev),
+                     "top_ids": torch.empty((B, S, top_n), dtype=torch.int32, device=dev),
+                     "top_logprobs": torch.empty((B, S, top_n), dtype=torch.float32, device=dev)}
+        spec = _lib.Logprobs(lp.data_ptr(), *((extra["ranks"].data_ptr(), extra["top_ids"].data_ptr(), extra["top_logprobs"].data_ptr(),
+                                               top_n) if extra else (0, 0, 0, 0)))
+    _lib.check(lib.lg_generate_composed(handle, _lib.ptr(cond_dev), _lib.ptr(em), _lib.ptr(neg), _lib.ptr(nm), B, K, T, S,
+                                        ctypes.byref(sc), _lib.ptr(w_dev), _lib.ptr(pf_dev), P, _lib.ptr(g_rows), ws, ws_bytes,
+                                        None if spec is None else ctypes.byref(spec), _lib.ptr(out), _lib.current_stream(dev)),
+               "lg_generate_composed")
+    if cond.device != dev:
+        out = out.to(cond.device)
+    if not return_logprobs:
+        return out
+    lp = lp.to(out.device)
+    if extra is None:
+        return out, lp
+    return out, lp, {k: v.to(out.device) for k, v in extra.items()}
 
 
 def _is_int(x) -> bool:

@@ -156,6 +156,111 @@ def inpaint_kwargs(args, vq_model, batch: int, latent_size: int, device) -> dict
     return {"given": codes.view(1, -1), "given_mask": inpaint_mask(args.inpaint_box, latent_size)}
 
 
+def add_compose_class_arg(parser):
+    parser.add_argument("--compose-class", type=str, nargs=2, action="append", default=None, metavar=("LABEL", "WEIGHT"),
+                        help="extension: composable guidance: add this class to every image with this weight (any sign; repeatable, "
+                             "up to 7 times); each image's own class keeps weight --cfg-scale")
+    return parser
+
+
+def add_compose_prompt_args(parser):
+    parser.add_argument("--compose-prompt", type=str, nargs=2, action="append", default=None, metavar=("TEXT", "WEIGHT"),
+                        help="extension: composable guidance: add this caption to every image with this weight (any sign; "
+                             "repeatable), encoded by the --t5-path encoder; each image's own caption keeps weight --cfg-scale")
+    parser.add_argument("--compose-cond-npy", type=str, nargs=2, action="append", default=None, metavar=("PATH", "WEIGHT"),
+                        help="extension: as --compose-prompt, with the caption's T5 features in one .npy (extract_t5_feature's "
+                             "layout); these conditions follow the --compose-prompt ones")
+    return parser
+
+
+def compose_entries(args) -> list:
+    """The (value, weight string) pairs of --compose-class, or of --compose-prompt then --compose-cond-npy; [] without them."""
+    return (list(getattr(args, "compose_class", None) or []) + list(getattr(args, "compose_prompt", None) or [])
+            + list(getattr(args, "compose_cond_npy", None) or []))
+
+
+def check_compose_args(args, num_classes: int = 0):
+    """Rejects --compose-* flags that generate() cannot run, before any model is loaded: weights that are not finite numbers, more
+    than 7 added conditions, class labels outside [0, num_classes), missing feature files, --sjd-window, and --cfg-interval with
+    added conditions."""
+    from .. import _lib
+    entries = compose_entries(args)
+    if not entries:
+        return
+    if len(entries) > _lib.MAX_COMPOSE - 1:
+        raise SystemExit(f"at most {_lib.MAX_COMPOSE - 1} --compose-* conditions (every image has {_lib.MAX_COMPOSE} at most), "
+                         f"got {len(entries)}")
+    for value, w in entries:
+        try:
+            wf = float(w)
+        except ValueError:
+            raise SystemExit(f"--compose-* weight {w!r} is not a number") from None
+        if not (np.isfinite(wf) and abs(wf) <= float(np.finfo(np.float32).max)):
+            raise SystemExit(f"--compose-* weight {w!r} is not finite")
+    for label, _ in getattr(args, "compose_class", None) or []:
+        try:
+            lab = int(label)
+        except ValueError:
+            raise SystemExit(f"--compose-class label {label!r} is not an integer") from None
+        if not 0 <= lab < num_classes:
+            raise SystemExit(f"--compose-class label {lab} must lie in [0, {num_classes})")
+    for path, _ in getattr(args, "compose_cond_npy", None) or []:
+        if not os.path.isfile(path):
+            raise SystemExit(f"--compose-cond-npy {path!r} is not a file")
+    if getattr(args, "sjd_window", None) is not None:
+        raise SystemExit("--compose-* cannot be combined with --sjd-window")
+    if getattr(args, "cfg_interval", -1) != -1:
+        raise SystemExit("--cfg-interval applies to plain guidance only; it cannot be combined with --compose-*")
+
+
+def guidance_kwargs(args, cfg_interval: bool = True) -> dict:
+    """generate()'s guidance keywords: cfg_scale (and cfg_interval) as before without --compose-*, else cond_weights: --cfg-scale for
+    each image's own condition, then the added conditions' weights in flag order."""
+    entries = compose_entries(args)
+    if not entries:
+        return {"cfg_scale": args.cfg_scale, **({"cfg_interval": args.cfg_interval} if cfg_interval else {})}
+    return {"cond_weights": [float(args.cfg_scale)] + [float(w) for _, w in entries]}
+
+
+def compose_class_cond(args, c_indices):
+    """c2i cond of generate(): the labels [B] as they are without --compose-class, else [B, K] with the added classes after each
+    image's own."""
+    extra = [int(label) for label, _ in getattr(args, "compose_class", None) or []]
+    if not extra:
+        return c_indices
+    add = torch.tensor(extra, dtype=c_indices.dtype, device=c_indices.device).view(1, -1).expand(len(c_indices), -1)
+    return torch.cat([c_indices.view(-1, 1), add], 1)
+
+
+def compose_caption_cond(cond, emb_masks, extra):
+    """t2i cond / emb_masks of generate(): as they are without added captions (extra empty), else [B, K, T, C] / [B, K, T] with the
+    added prepared captions (each ([1, T, C], [1, T])) after each image's own."""
+    if not extra:
+        return cond, emb_masks
+    B = cond.shape[0]
+    c = torch.stack([cond] + [e.to(cond.dtype).expand(B, -1, -1) for e, _ in extra], 1)
+    m = torch.stack([emb_masks] + [mk.to(emb_masks.dtype).expand(B, -1) for _, mk in extra], 1)
+    return c, m
+
+
+def compose_caption_features(args, encode, device, precision) -> list:
+    """The added captions of --compose-prompt (encoded by `encode`, a list-of-strings -> (features, masks) text encoder, or None when
+    the sampler has none) then --compose-cond-npy, each prepared as the prompts are: [(cond [1, T, C], mask [1, T]), ...]."""
+    from ..cond import load_t5_feature_files, prepare_condition
+    T, C = args.t5_feature_max_len, args.t5_feature_dim
+    feats = []
+    prompts = [text for text, _ in getattr(args, "compose_prompt", None) or []]
+    if prompts:
+        if encode is None:
+            raise SystemExit("--compose-prompt needs the text encoder (--t5-path); use --compose-cond-npy with precomputed features")
+        embs, masks = encode(prompts)
+        feats += [(embs[i:i + 1], masks[i:i + 1]) for i in range(len(prompts))]
+    for path, _ in getattr(args, "compose_cond_npy", None) or []:
+        embs, masks = load_t5_feature_files([path], T, C)
+        feats.append((embs.to(device, precision), masks.to(device)))
+    return [prepare_condition(e, mk, left_padding=not args.no_left_padding) for e, mk in feats]
+
+
 def add_common_args(parser, t2i: bool):
     parser.add_argument("--gpt-model", type=str, choices=list(GPT_models.keys()), default="GPT-XL" if t2i else "GPT-B")
     parser.add_argument("--gpt-ckpt", type=str, default=None)

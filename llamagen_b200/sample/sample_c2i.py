@@ -6,8 +6,9 @@ import time
 import torch
 
 from .. import generate
-from .common import (add_common_args, add_inpaint_args, add_prefix_args, add_sjd_arg, check_inpaint_args, check_prefix_args,
-                     inpaint_kwargs, load_gpt, load_vq, prefix_kwargs, sjd_kwargs)
+from .common import (add_common_args, add_compose_class_arg, add_inpaint_args, add_prefix_args, add_sjd_arg, check_compose_args,
+                     check_inpaint_args, check_prefix_args, compose_class_cond, guidance_kwargs, inpaint_kwargs, load_gpt, load_vq,
+                     prefix_kwargs, sjd_kwargs)
 
 
 def main(args):
@@ -19,6 +20,7 @@ def main(args):
     latent_size = args.image_size // args.downsample_size
     check_prefix_args(args, latent_size)
     check_inpaint_args(args, latent_size)
+    check_compose_args(args, args.num_classes)
     vq_model = load_vq(args, device)
     gpt_model = load_gpt(args, device, latent_size)
 
@@ -30,7 +32,7 @@ def main(args):
           **inpaint_kwargs(args, vq_model, len(class_labels), latent_size, device)}
     torch.cuda.synchronize()
     t1 = time.time()
-    index_sample = generate(gpt_model, c_indices, latent_size ** 2, cfg_scale=args.cfg_scale, cfg_interval=args.cfg_interval,
+    index_sample = generate(gpt_model, compose_class_cond(args, c_indices), latent_size ** 2, **guidance_kwargs(args),
                             temperature=args.temperature, top_k=args.top_k, top_p=args.top_p, sample_logits=True,
                             **sjd_kwargs(args), **pk)
     torch.cuda.synchronize()
@@ -45,7 +47,7 @@ def main(args):
 
 
 def build_parser():
-    parser = add_inpaint_args(add_prefix_args(add_sjd_arg(add_common_args(argparse.ArgumentParser(), t2i=False))))
+    parser = add_compose_class_arg(add_inpaint_args(add_prefix_args(add_sjd_arg(add_common_args(argparse.ArgumentParser(), t2i=False)))))
     parser.add_argument("--cfg-interval", type=float, default=-1)
     parser.add_argument("--class-labels", type=int, nargs="+", default=None,
                         help="extension: override the 8 hard-coded ImageNet labels (batch size = number of labels)")

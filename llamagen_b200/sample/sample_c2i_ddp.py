@@ -14,7 +14,8 @@ import torch.distributed as dist
 from .. import distributed as lgd
 from ..pipeline import SamplePipeline
 from ..postprocess import AsyncPngWriter
-from .common import add_common_args, add_inpaint_args, check_inpaint_args, inpaint_kwargs, load_gpt, load_vq
+from .common import (add_common_args, add_compose_class_arg, add_inpaint_args, check_compose_args, check_inpaint_args, compose_class_cond,
+                     guidance_kwargs, inpaint_kwargs, load_gpt, load_vq)
 
 
 def create_npz_from_sample_folder(sample_dir, num=50_000):
@@ -37,6 +38,7 @@ def main(args):
     print(f"Starting rank={rank}, seed={seed}, world_size={world}.")
     latent_size = args.image_size // args.downsample_size
     check_inpaint_args(args, latent_size)
+    check_compose_args(args, args.num_classes)
     if rank != 0:                                   # only rank 0 touches the disk
         args_nockpt = argparse.Namespace(**{**vars(args), "vq_ckpt": None, "gpt_ckpt": None})
         vq_model, gpt_model = load_vq(args_nockpt, device), load_gpt(args_nockpt, device, latent_size)
@@ -72,8 +74,7 @@ def main(args):
     # Steady-state loop of sample_c2i_ddp.py:128-149, reorganised (SURVEY §8 f-1): the VQ decode + pixel finishing +
     # D2H of batch i run on a second stream under the AR sampling of batch i+1, and the PNG encoders run on host
     # threads; file names and contents are the reference's.
-    pipe = SamplePipeline(gpt_model, vq_model, args.codebook_embed_dim, cfg_scale=args.cfg_scale, cfg_interval=args.cfg_interval,
-                          temperature=args.temperature, top_k=args.top_k, top_p=args.top_p, sample_logits=True, **ik)
+    pipe = SamplePipeline(gpt_model, vq_model, args.codebook_embed_dim, **guidance_kwargs(args), temperature=args.temperature, top_k=args.top_k, top_p=args.top_p, sample_logits=True, **ik)
     eval_px = args.image_size_eval
     host = [torch.empty(n, eval_px, eval_px, 3, dtype=torch.uint8).pin_memory() for _ in range(2)]
 
@@ -88,7 +89,7 @@ def main(args):
         for it in range(iterations):
             c_indices = torch.randint(0, args.num_classes, (n,), device=device)
             buf = host[it % 2]
-            pipe.submit(c_indices, latent_size, to_uint8_host=buf)
+            pipe.submit(compose_class_cond(args, c_indices), latent_size, to_uint8_host=buf)
             done = torch.cuda.Event()
             done.record(pipe.decode_stream)
             if pending is not None:
@@ -108,7 +109,7 @@ def main(args):
 
 
 def build_parser():
-    parser = add_inpaint_args(add_common_args(argparse.ArgumentParser(), t2i=False))
+    parser = add_compose_class_arg(add_inpaint_args(add_common_args(argparse.ArgumentParser(), t2i=False)))
     parser.add_argument("--cfg-interval", type=float, default=-1)
     parser.add_argument("--image-size-eval", type=int, choices=[256, 384, 512], default=256)
     parser.add_argument("--sample-dir", type=str, default="samples")

@@ -6,7 +6,10 @@ language/extract_t5_feature.py (fp32 [1, valid_len, 2048] .npy, one file per pro
 draws seeded random features (what the benchmarks use, there are no T5 weights offline).
 
 A negative prompt (`--negative-prompt TEXT`, encoded by the `--t5-path` encoder, or `--negative-cond-npy FILE` in
-extract_t5_feature's layout) takes the place of the null condition in classifier-free guidance for every prompt."""
+extract_t5_feature's layout) takes the place of the null condition in classifier-free guidance for every prompt.
+
+Composable guidance (`--compose-prompt TEXT WEIGHT`, `--compose-cond-npy FILE WEIGHT`, repeatable) adds weighted captions to every
+image; each image's own caption keeps weight --cfg-scale."""
 import argparse
 import os
 import time
@@ -15,8 +18,9 @@ import torch
 
 from .. import generate
 from ..cond import HFT5Encoder, load_t5_feature_files, prepare_condition, synthetic_features
-from .common import (add_common_args, add_inpaint_args, add_prefix_args, add_sjd_arg, check_inpaint_args, check_prefix_args,
-                     inpaint_kwargs, load_gpt, load_vq, prefix_kwargs, sjd_kwargs)
+from .common import (add_common_args, add_compose_prompt_args, add_inpaint_args, add_prefix_args, add_sjd_arg, check_compose_args,
+                     check_inpaint_args, check_prefix_args, compose_caption_cond, compose_caption_features, compose_entries,
+                     guidance_kwargs, inpaint_kwargs, load_gpt, load_vq, prefix_kwargs, sjd_kwargs)
 
 PROMPTS = [
     "A portrait photo of a kangaroo wearing an orange hoodie and blue sunglasses standing on the grassin front of the Sydney Opera House holding a sign on the chest that says Welcome Friends!",
@@ -62,8 +66,9 @@ def _hf_encoder(args, device, precision):
 def check_negative_args(args):
     if args.negative_prompt and args.negative_cond_npy:
         raise SystemExit("pass --negative-prompt or --negative-cond-npy, not both")
-    if (args.negative_prompt or args.negative_cond_npy) and not args.cfg_scale > 1.0:
-        raise SystemExit("a negative prompt replaces the unconditional half of classifier-free guidance: it needs --cfg-scale > 1")
+    if (args.negative_prompt or args.negative_cond_npy) and not args.cfg_scale > 1.0 and not compose_entries(args):
+        raise SystemExit("a negative prompt replaces the unconditional half of classifier-free guidance: it needs --cfg-scale > 1 "
+                         "(or --compose-*)")
 
 
 def main(args):
@@ -76,6 +81,7 @@ def main(args):
     check_prefix_args(args, latent_size)
     check_inpaint_args(args, latent_size)
     check_negative_args(args)
+    check_compose_args(args)
     vq_model = load_vq(args, device)
     gpt_model = load_gpt(args, device, latent_size)
     precision = gpt_model.tok_embeddings.weight.dtype
@@ -90,13 +96,15 @@ def main(args):
     nk = {}
     if neg is not None:   # prepared as the prompts are; one negative for every prompt
         nk["negative_cond"], nk["negative_emb_masks"] = prepare_condition(*neg, left_padding=not args.no_left_padding)
+    encode = (lambda texts: _hf_encoder(args, device, precision)(texts)) if args.compose_prompt else None
+    c_indices, emb_masks = compose_caption_cond(c_indices, emb_masks, compose_caption_features(args, encode, device, precision))
     qzshape = [len(c_indices), args.codebook_embed_dim, latent_size, latent_size]
 
     pk = {**prefix_kwargs(args, vq_model, len(c_indices), latent_size, device),
           **inpaint_kwargs(args, vq_model, len(c_indices), latent_size, device)}
     torch.cuda.synchronize()
     t1 = time.time()
-    index_sample = generate(gpt_model, c_indices, latent_size ** 2, emb_masks, cfg_scale=args.cfg_scale,
+    index_sample = generate(gpt_model, c_indices, latent_size ** 2, emb_masks, **guidance_kwargs(args, cfg_interval=False),
                             temperature=args.temperature, top_k=args.top_k, top_p=args.top_p, sample_logits=True,
                             **sjd_kwargs(args), **pk, **nk)
     torch.cuda.synchronize()
@@ -111,7 +119,7 @@ def main(args):
 
 
 def build_parser():
-    parser = add_inpaint_args(add_prefix_args(add_sjd_arg(add_common_args(argparse.ArgumentParser(), t2i=True))))
+    parser = add_compose_prompt_args(add_inpaint_args(add_prefix_args(add_sjd_arg(add_common_args(argparse.ArgumentParser(), t2i=True)))))
     parser.add_argument("--t5-path", type=str, default="pretrained_models/t5-ckpt")
     parser.add_argument("--t5-model-type", type=str, default="flan-t5-xl")
     parser.add_argument("--t5-feature-max-len", type=int, default=120)

@@ -20,7 +20,8 @@ from .. import distributed as lgd
 from ..cond import HFT5Encoder, load_t5_feature_files, prepare_condition, synthetic_features
 from ..pipeline import SamplePipeline
 from ..postprocess import AsyncPngWriter
-from .common import add_common_args, add_inpaint_args, check_inpaint_args, inpaint_kwargs, load_gpt, load_vq
+from .common import (add_common_args, add_compose_prompt_args, add_inpaint_args, check_compose_args, check_inpaint_args,
+                     compose_caption_cond, compose_caption_features, guidance_kwargs, inpaint_kwargs, load_gpt, load_vq)
 
 FALLBACK_PROMPT = "a cute dog"      # sample_t2i_ddp.py:138
 
@@ -46,6 +47,7 @@ def main(args):
     print(f"Starting rank={rank}, seed={seed}, world_size={world}.")
     latent_size = args.image_size // args.downsample_size
     check_inpaint_args(args, latent_size)
+    check_compose_args(args)
     if rank != 0:
         args_nockpt = argparse.Namespace(**{**vars(args), "gpt_ckpt": None, "vq_ckpt": None})
         vq_model, gpt_model = load_vq(args_nockpt, device), load_gpt(args_nockpt, device, latent_size)
@@ -63,6 +65,8 @@ def main(args):
     if not (args.synthetic_cond or args.t5_feature_dir):
         assert os.path.exists(args.t5_path), "--t5-path not found (use --t5-feature-dir or --synthetic-cond without T5 weights)"
         t5 = HFT5Encoder(args.t5_path, args.t5_model_type, T, device, precision)
+    # the added captions of --compose-*, the same for every image of every rank (none without them)
+    extra = compose_caption_features(args, t5, device, precision)
 
     prompt_list = read_prompts(args.prompt_csv)
     ckpt_name = os.path.basename(args.gpt_ckpt or "random-init").replace(".pth", "").replace(".pt", "")
@@ -95,7 +99,8 @@ def main(args):
             return embs.to(device, precision), masks.to(device)
         return t5([prompt_list[i] if i < len(prompt_list) else FALLBACK_PROMPT for i in indices])
 
-    pipe = SamplePipeline(gpt_model, vq_model, args.codebook_embed_dim, cfg_scale=args.cfg_scale, temperature=args.temperature,
+    pipe = SamplePipeline(gpt_model, vq_model, args.codebook_embed_dim, **guidance_kwargs(args, cfg_interval=False),
+                          temperature=args.temperature,
                           top_k=args.top_k, top_p=args.top_p, sample_logits=True, **ik)
     px = args.image_size
     host = [torch.empty(n, px, px, 3, dtype=torch.uint8).pin_memory() for _ in range(2)]
@@ -114,6 +119,7 @@ def main(args):
             caption_embs, emb_masks = features(indices)
             c_indices, c_emb_masks = prepare_condition(caption_embs, emb_masks, left_padding=not args.no_left_padding)
             buf = host[it % 2]
+            c_indices, c_emb_masks = compose_caption_cond(c_indices, c_emb_masks, extra)
             pipe.submit(c_indices, latent_size, to_uint8_host=buf, emb_masks=c_emb_masks)
             done = torch.cuda.Event()
             done.record(pipe.decode_stream)
@@ -141,7 +147,7 @@ def main(args):
 
 
 def build_parser():
-    parser = add_inpaint_args(add_common_args(argparse.ArgumentParser(), t2i=True))
+    parser = add_compose_prompt_args(add_inpaint_args(add_common_args(argparse.ArgumentParser(), t2i=True)))
     parser.add_argument("--prompt-csv", type=str, default="evaluations/t2i/PartiPrompts.tsv")
     parser.add_argument("--t5-path", type=str, default="pretrained_models/t5-ckpt")
     parser.add_argument("--t5-model-type", type=str, default="flan-t5-xl")
