@@ -251,6 +251,23 @@ int  lg_sample_rows_given(const float* logits, int B, int V, int mix_cfg, int ro
                           const uint64_t* seed_rows, const int32_t* step_rows, const float* cfg_rows, const int32_t* interval_rows,
                           const int32_t* img_rows, const int32_t* given, const lg_logprobs* lp, int32_t* out_idx, int32_t* out_seq,
                           int seq_stride, void* stream);
+/* Composable guidance inside a mixed batch (serving's composed requests): lg_sample_rows_given with mix_cfg = 1, plus a gather table.
+ * logits f32 [rows, V], rows >= 2B. mix_rows dev int32 [B][1 + 8] and mix_weights dev f32 [B][8], both NULL or both given; entry 0 of
+ * row b is its role:
+ *   -2      a condition row: nothing of row b is written (its logits are read by the lead row that names them);
+ *   -1      a plain row: conditional row b and unconditional row B + b, cfg_rows[b] / interval_rows[b], exactly what
+ *           lg_sample_rows_given draws for it;
+ *   u >= 0  a lead row: x = u + w_1 (c_1 - u) + ... + w_K (c_K - u) with u = logits row u, c_i = logits row mix_rows[b][i] for
+ *           i = 1 .. K (1 <= K <= 8; entry K + 1, if any, is -1) and w_i = mix_weights[b][i - 1], every row rounded to round_dtype
+ *           first and the sum accumulated left to right in fp32, as in lg_generate_composed; always mixed, except that interval_rows[b]
+ *           drops the mix as for a plain row (sc->cfg_scale and cfg_rows[b] are unused).
+ * The RNG key (seed_rows[b], step_rows[b], img_rows[b]), the given select, the logprobs and out_idx[b] / out_seq[b, step] are row b's.
+ * The row indices inside mix_rows are unchecked on the device (the caller's contract: in [0, rows)). With mix_rows NULL this is
+ * lg_sample_rows_given with mix_cfg = 1. Every argument the host can check is checked before any launch. */
+int  lg_sample_rows_composed(const float* logits, int rows, int B, int V, int round_dtype, const lg_sample_cfg* sc,
+                             const uint64_t* seed_rows, const int32_t* step_rows, const float* cfg_rows, const int32_t* interval_rows,
+                             const int32_t* img_rows, const int32_t* given, const int32_t* mix_rows, const float* mix_weights,
+                             const lg_logprobs* lp, int32_t* out_idx, int32_t* out_seq, int seq_stride, void* stream);
 /* generate() with token log-probabilities [B, S] (top: [B, S, top_n]), in one call covering lg_generate (neg_cond NULL, P = 0),
  * lg_generate_neg (neg_cond, neg_mask as there) and lg_generate_prefix(_neg) (1 <= P <= S - 1, prefix and dev_ws as there; P = 0
  * needs neither and ignores them). The tokens are those of that call. Rows k < P (given tokens) get logprob 0, rank 0, top ids -1 and

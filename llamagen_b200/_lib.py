@@ -104,6 +104,8 @@ SIGNATURES = {
                                         c_void_p, POINTER(Logprobs), c_void_p, c_void_p, c_int, c_void_p]),
     "lg_sample_rows_given": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p, c_void_p, c_void_p, c_void_p,
                                      c_void_p, c_void_p, POINTER(Logprobs), c_void_p, c_void_p, c_int, c_void_p]),
+    "lg_sample_rows_composed": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p, c_void_p, c_void_p, c_void_p,
+                                        c_void_p, c_void_p, c_void_p, c_void_p, POINTER(Logprobs), c_void_p, c_void_p, c_int, c_void_p]),
     "lg_generate_logprobs": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(SampleCfg), c_void_p,
                                      c_int, c_void_p, c_size_t, POINTER(Logprobs), c_void_p, c_void_p]),
     "lg_copy_slot_kv": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),

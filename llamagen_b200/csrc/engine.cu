@@ -1082,11 +1082,13 @@ static void apply_logprobs(SampleArgs& a, const lg_logprobs* lp, size_t off) {
 }
 
 // lg_sample_rows (cfg_rows = interval_rows = img_rows = null), lg_sample_rows_guided (img_rows = null), lg_sample_rows_keyed and
-// lg_sample_rows_logprobs (lp: NULL for the others); fn names the entry point in messages
+// lg_sample_rows_logprobs (lp: NULL for the others), lg_sample_rows_given (given) and lg_sample_rows_composed (mix_rows, mix_weights: a
+// gather table, needs mix_cfg); fn names the entry point in messages
 static int sample_rows_impl(const char* fn, const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc,
                             const uint64_t* seed_rows, const int32_t* step_rows, const float* cfg_rows, const int32_t* interval_rows,
                             const int32_t* img_rows, const lg_logprobs* lp, int32_t* out_idx, int32_t* out_seq, int seq_stride,
-                            void* stream, const int32_t* given = nullptr) {
+                            void* stream, const int32_t* given = nullptr, const int32_t* mix_rows = nullptr,
+                            const float* mix_weights = nullptr) {
     LG_REQUIRE(logits && sc && seed_rows && step_rows && (out_idx || out_seq), "%s: null argument", fn);
     LG_REQUIRE(!given || (out_seq && seq_stride > 0), "%s: given tokens are indexed as out_seq and need it", fn);
     LG_REQUIRE(mix_cfg || (!cfg_rows && !interval_rows), "%s: per-row cfg_rows / interval_rows need mix_cfg (2B logits rows)", fn);
@@ -1097,6 +1099,7 @@ static int sample_rows_impl(const char* fn, const float* logits, int B, int V, i
     a.seed_rows = seed_rows; a.step_rows = step_rows;
     a.cfg_rows = cfg_rows; a.interval_rows = interval_rows; a.img_rows = img_rows;
     a.out_idx = out_idx; a.out_seq = out_seq; a.seq_stride = seq_stride; a.given = given;
+    a.mix_rows = mix_rows; a.mix_weights = mix_rows ? mix_weights : nullptr;
     if (lp_on) apply_logprobs(a, lp, 0);
     return launch_sample(a, (cudaStream_t)stream);
 }
@@ -1137,6 +1140,19 @@ int lg_sample_rows_given(const float* logits, int B, int V, int mix_cfg, int rou
                          int seq_stride, void* stream) {
     return sample_rows_impl("lg_sample_rows_given", logits, B, V, mix_cfg, round_dtype, sc, seed_rows, step_rows, cfg_rows,
                             interval_rows, img_rows, lp, out_idx, out_seq, seq_stride, stream, given);
+}
+
+int lg_sample_rows_composed(const float* logits, int rows, int B, int V, int round_dtype, const lg_sample_cfg* sc, const uint64_t* seed_rows,
+                            const int32_t* step_rows, const float* cfg_rows, const int32_t* interval_rows, const int32_t* img_rows,
+                            const int32_t* given, const int32_t* mix_rows, const float* mix_weights, const lg_logprobs* lp,
+                            int32_t* out_idx, int32_t* out_seq, int seq_stride, void* stream) {
+    static const char* fn = "lg_sample_rows_composed";
+    // every row may be plain (the roles live on the device), and a plain row reads rows b and B + b
+    LG_REQUIRE(B > 0 && V > 0 && rows >= 2 * B, "%s: bad shape rows=%d B=%d V=%d (rows >= 2B)", fn, rows, B, V);
+    LG_REQUIRE((mix_rows != nullptr) == (mix_weights != nullptr), "%s: mix_rows and mix_weights go together", fn);
+    LG_REQUIRE(round_dtype == LG_DTYPE_F32 || lg_dtype_is16(round_dtype), "%s: unsupported round dtype %d", fn, round_dtype);
+    return sample_rows_impl(fn, logits, B, V, 1, round_dtype, sc, seed_rows, step_rows, cfg_rows, interval_rows, img_rows, lp, out_idx,
+                            out_seq, seq_stride, stream, given, mix_rows, mix_weights);
 }
 
 int lg_sample(const float* logits, int B, int V, int mix_cfg, int round_dtype, const lg_sample_cfg* sc, uint64_t step,

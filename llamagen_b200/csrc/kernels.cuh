@@ -73,6 +73,12 @@ struct SampleArgs {
     // ([B][seq_stride]), and the token goes to next_tokens and the fused tail's rows of all 2K rows. 0: one row per image, as above
     int mix_groups = 0;
     const float* mix_weights = nullptr;
+    // composed draws inside a mixed batch (lg_sample_rows_composed; mix_groups = 0, needs mix_cfg and seed_rows): int32
+    // [B][1 + kMaxMixGroups], one CTA per row, and mix_weights becomes per row, [B][kMaxMixGroups]. Entry 0 of row b is its role:
+    // -2, a condition row: the CTA writes nothing; -1, a plain row: conditional row b, unconditional row B + b, cfg_rows / interval_rows
+    // as in lg_sample_rows_guided; u >= 0, a lead row: unconditional row u, conditional rows in entries 1 .. K (then -1), always mixed
+    // (interval_rows still drops the mix). Keys, given, logprobs and outputs are row b's. No fused tail, no dbg_logits
+    const int32_t* mix_rows = nullptr;
 };
 constexpr int kMaxTopLogprobs = 20;
 constexpr int kMaxMixGroups = 8;

@@ -143,17 +143,23 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
     const int V = a.V, B = a.B;
     const uint64_t step = a.step_rows ? (uint64_t)a.step_rows[b] : (a.step_dev ? (uint64_t)(*a.step_dev) : a.step);
 
+    // a gather table (mix_rows, grouped instantiation only): row b's role, -2 condition row, -1 plain row, u >= 0 lead row mixing
+    // unconditional row u; without one, -1
+    const int32_t* mr = kGroups && a.mix_rows ? a.mix_rows + (size_t)b * (1 + kMaxMixGroups) : nullptr;
+    const int role = mr ? mr[0] : -1;
+    if (role == -2) return;   // a condition row: its logits are read by its lead's CTA
+
     const float cfg_scale = a.cfg_rows ? a.cfg_rows[b] : a.cfg_scale;
     const int cfg_interval = a.interval_rows ? a.interval_rows[b] : a.cfg_interval;
     // a row with its own scale mixes only above 1 (generate.py:79 `if cfg_scale > 1.0`; a NaN scale does not mix either): it then
-    // reads only its conditional row
-    bool mix = a.mix_cfg != 0 && (!a.cfg_rows || cfg_scale > 1.0f);
+    // reads only its conditional row. A lead row always mixes (its weights are the scales)
+    bool mix = a.mix_cfg != 0 && (role >= 0 || !a.cfg_rows || cfg_scale > 1.0f);
     // generate.py:113-114 — decode iteration i = step-1; once i > cfg_interval the mix is dropped.
     if (mix && cfg_interval > -1 && step >= 1 && (long long)(step - 1) > (long long)cfg_interval) mix = false;
 
-    const int G = kGroups ? a.mix_groups : 1;   // rows per image and half
+    const int G = kGroups ? (mr ? 1 : a.mix_groups) : 1;   // rows per image and half (a gather table: one row per CTA)
     const float* lc = a.logits + (size_t)b * G * V;
-    const float* lu = a.logits + (size_t)(B + b * G) * V;
+    const float* lu = a.logits + (size_t)(role >= 0 ? role : B + b * G) * V;
     const float tdiv = fmaxf(a.temperature, 1e-5f);
     const int dbgB = a.dbg_batch > 0 ? a.dbg_batch : B;
     float* dbg = a.dbg_logits ? a.dbg_logits + ((size_t)step * dbgB + a.row_offset + b) * V : nullptr;
@@ -166,37 +172,48 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
     };
     if constexpr (kGroups) {
         // x = u + d, d = w_1 (c_1 - u) + ... + w_K (c_K - u) accumulated left to right, every row rounded first; K = 1 is mix1 with
-        // cfg_scale = w_1 exactly. Without the mix (cfg_interval passed, K = 1 only) x = c_1, as mix1
+        // cfg_scale = w_1 exactly. Without the mix (cfg_interval passed, K = 1 only) x = c_1, as mix1. With a gather table a lead row
+        // mixes the nc conditional rows its entries name, and a plain row is one condition at its own scale (mix1 bit for bit)
+        int nc = G;
+        if (role >= 0) {
+            nc = 0;
+            while (nc < kMaxMixGroups && mr[1 + nc] >= 0) ++nc;
+        }
+        int crow[kMaxMixGroups];   // the conditional rows
         float w[kMaxMixGroups];
 #pragma unroll
-        for (int i = 0; i < kMaxMixGroups; ++i) w[i] = i < G ? a.mix_weights[(size_t)b * G + i] : 0.f;
+        for (int i = 0; i < kMaxMixGroups; ++i) {
+            crow[i] = role >= 0 ? mr[1 + min(i, nc - 1)] : b * G + i;
+            w[i] = i >= nc ? 0.f : !mr ? a.mix_weights[(size_t)b * G + i] : role >= 0 ? a.mix_weights[(size_t)b * kMaxMixGroups + i] : cfg_scale;
+        }
+        auto crow_ptr = [&](int i) { return a.logits + (size_t)crow[i] * V; };
         auto rd = [&](float x) -> float { return a.round_dtype ? TR::round(x) : x; };
         auto mixg = [&](int v) -> float {
-            const float c1 = rd(lc[v]);
+            const float c1 = rd(crow_ptr(0)[v]);
             if (!mix) return c1;
             const float u = rd(lu[v]);
             float d = __fmul_rn(__fsub_rn(c1, u), w[0]);
 #pragma unroll
             for (int i = 1; i < kMaxMixGroups; ++i)
-                if (i < G) d = __fadd_rn(d, __fmul_rn(__fsub_rn(rd(lc[(size_t)i * V + v]), u), w[i]));
+                if (i < nc) d = __fadd_rn(d, __fmul_rn(__fsub_rn(rd(crow_ptr(i)[v]), u), w[i]));
             return __fadd_rn(u, d);
         };
         if (sample_vec_loads(a)) {   // 128-bit loads, as below
-            const float4* lc4 = reinterpret_cast<const float4*>(lc);
             const float4* lu4 = reinterpret_cast<const float4*>(lu);
             const int V4 = V >> 2;
+            auto row4 = [&](int i) { return reinterpret_cast<const float4*>(crow_ptr(i)); };
             auto rd4 = [&](float4 x) -> float4 { return make_float4(rd(x.x), rd(x.y), rd(x.z), rd(x.w)); };
             auto term = [](float c, float u, float wi) { return __fmul_rn(__fsub_rn(c, u), wi); };
 #pragma unroll 2
             for (int v4 = tid; v4 < V4; v4 += kSampleThreads) {
-                float4 x = rd4(lc4[v4]);
+                float4 x = rd4(row4(0)[v4]);
                 if (mix) {
                     const float4 u = rd4(lu4[v4]);
                     float4 d = make_float4(term(x.x, u.x, w[0]), term(x.y, u.y, w[0]), term(x.z, u.z, w[0]), term(x.w, u.w, w[0]));
 #pragma unroll
                     for (int i = 1; i < kMaxMixGroups; ++i)
-                        if (i < G) {
-                            const float4 c = rd4(lc4[(size_t)i * V4 + v4]);
+                        if (i < nc) {
+                            const float4 c = rd4(row4(i)[v4]);
                             d.x = __fadd_rn(d.x, term(c.x, u.x, w[i])); d.y = __fadd_rn(d.y, term(c.y, u.y, w[i]));
                             d.z = __fadd_rn(d.z, term(c.z, u.z, w[i])); d.w = __fadd_rn(d.w, term(c.w, u.w, w[i]));
                         }
@@ -654,8 +671,14 @@ int launch_sample(const SampleArgs& a, cudaStream_t st) {
                    (a.top_n == 0 || (a.top_ids && a.top_lp)),
                "lg_sample: top_n=%d outside [0, %d], or top_ids / top_logprob not both given exactly when top_n > 0", a.top_n,
                kMaxTopLogprobs);
-    const bool grp = a.mix_groups > 0;
-    if (grp) {
+    const bool table = a.mix_rows != nullptr;
+    const bool grp = a.mix_groups > 0 || table;
+    if (table) {
+        LG_REQUIRE(a.mix_groups == 0 && a.mix_cfg && a.mix_weights && a.seed_rows,
+                   "lg_sample: a gather table (mix_rows) needs mix_groups 0, mix_cfg, per-row weights and seed_rows");
+        LG_REQUIRE(!a.emb_table && !a.adv_pos && !a.adv_step && !a.dbg_logits,
+                   "lg_sample: a gather table (mix_rows) takes no fused tail or dbg_logits");
+    } else if (grp) {
         LG_REQUIRE(a.mix_groups <= kMaxMixGroups && a.B % a.mix_groups == 0 && a.mix_cfg && a.mix_weights,
                    "lg_sample: composable guidance needs 1 <= K=%d <= %d dividing B=%d rows, mix_cfg and weights", a.mix_groups,
                    kMaxMixGroups, a.B);
@@ -672,7 +695,7 @@ int launch_sample(const SampleArgs& a, cudaStream_t st) {
     if (lg_first_on_device(attr_set[4 * grp + 2 * lp + half])) {
         LG_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     }
-    (void)lg_launch(kern, dim3(grp ? a.B / a.mix_groups : a.B), dim3(kSampleThreads), smem, st, a);
+    (void)lg_launch(kern, dim3(grp && !table ? a.B / a.mix_groups : a.B), dim3(kSampleThreads), smem, st, a);
     LG_LAUNCH_CHECK();
     return 0;
 }

@@ -237,10 +237,9 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
     return (out, dbg) if return_logits else out
 
 
-def _check_compose(model, cond, S, emb_masks, cfg_scale, cfg_interval, cond_weights, negative_cond, negative_emb_masks):
-    """generate(cond_weights=...)'s checks, before anything reaches the device. Returns (B, K, T, weights f32 host [B, K])."""
-    if not isinstance(model, Transformer):
-        raise TypeError("llamagen_b200.generate needs a llamagen_b200 GPT_models[...] instance")
+def _check_cond_weights(cfg_scale, cfg_interval, cond_weights):
+    """The checks of cond_weights, and of the cfg_scale / cfg_interval beside it, that do not depend on cond (serve.LLM makes them on
+    a request's SamplingParams). Returns (weights f64 host [K] or [B, K], K)."""
     if cfg_scale != 1.0:
         raise ValueError(f"cond_weights are the guidance scales of a composed call; leave cfg_scale at its default (got {cfg_scale})")
     w = torch.as_tensor(cond_weights)
@@ -256,6 +255,14 @@ def _check_compose(model, cond, S, emb_masks, cfg_scale, cfg_interval, cond_weig
         raise ValueError("cond_weights must be finite (in fp32)")
     if cfg_interval != -1 and K > 1:
         raise ValueError(f"cfg_interval applies to a composed call only with K = 1 (got K={K}, cfg_interval={cfg_interval})")
+    return w, K
+
+
+def _check_compose(model, cond, S, emb_masks, cfg_scale, cfg_interval, cond_weights, negative_cond, negative_emb_masks):
+    """generate(cond_weights=...)'s checks, before anything reaches the device. Returns (B, K, T, weights f32 host [B, K])."""
+    if not isinstance(model, Transformer):
+        raise TypeError("llamagen_b200.generate needs a llamagen_b200 GPT_models[...] instance")
+    w, K = _check_cond_weights(cfg_scale, cfg_interval, cond_weights)
     if not torch.is_tensor(cond):
         raise ValueError("cond must be a tensor")
     if model.model_type == "c2i":

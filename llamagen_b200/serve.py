@@ -97,6 +97,19 @@ generate(cond, given=ids, given_mask=mask, seed=base_seed + r) at B = 1, so the 
 runs its own window pass, so the logits agree with that call's up to rounding. With n = k, sample j is keyed as image j. given goes with everything generate(given=) goes with; prefix=, sjd_window, logprobs and best_of are refused.
 Null-class twins mirror their conditional request's given tokens.
 
+Composable guidance (SamplingParams(cond_weights=(w_1, .., w_K)), 1 <= K <= 8, on an LLM built with cfg_scale > 1): a c2i request brings
+K class ids (prompt_token_ids=[c_1, .., c_K]), a t2i request K captions (prompt_embeds=[f_1, .., f_K], or prompt=[s_1, .., s_K] with a
+text encoder; a bare one when K = 1), and every token is drawn from u + w_1 (c_1 - u) + .. + w_K (c_K - u), as generate(cond_weights=)
+draws it: sample j draws what image j of generate(cond repeated n times, cond_weights=w, seed=s) draws, whatever runs beside it. The
+request takes n K slots, the lowest free ones at once (sample j's condition i in the (j K + i)-th); condition 1's slot is the sample's
+lead (its seed, image index, token row and unconditional row: the null condition or the negative), the others are condition slots
+whose unconditional rows run unread. A t2i or prefix join prefills sample 0's K slots alone, fans their K / V out to the other samples
+and draws token P once per sample; a c2i join without a prefix enters its K classes at position 0. While a running or joining slot is
+composed, every draw is lg_sample_rows_composed over a gather table (st["mix_rows"], st["mix_w"]: -2 for a condition slot, -1 for a
+plain one, the lead's rows and weights otherwise), and the leads' tokens become their condition slots' inputs on the device. A sample
+frees its K slots together. Not with cfg_scale (the weights are the scales), cfg_interval when K > 1, given / given_mask or sjd_window.
+Null-class twins mirror their conditional request's cond_weights and keep the single null class as their prompt.
+
 While requests are in flight the LLM owns the model's KV-cache workspace (a `generate()` call on the same model would reset it)."""
 from __future__ import annotations
 
@@ -114,7 +127,7 @@ import torch
 
 from . import _lib
 from .cond import pack_t5_features, prepare_condition
-from .generate import _check_given, _check_prefix
+from .generate import _check_cond_weights, _check_given, _check_prefix
 
 
 @dataclass(frozen=True)
@@ -128,7 +141,11 @@ class SamplingParams:
     seed=seed) draws. Requests that differ in n share the running batch.
     logprobs: None, or an integer in [0, 20]: return every drawn token's logprob and rank and its `logprobs` most likely alternatives.
     best_of: None, or an integer in [n, max_num_seqs]: draw best_of images and return the n with the largest cumulative_logprob.
-    Requests that differ in logprobs or best_of share the running batch."""
+    Requests that differ in logprobs or best_of share the running batch.
+    cond_weights: None, or K finite weights (1 <= K <= 8, any sign, zeros allowed; stored as a tuple): composable guidance, every token
+    drawn from u + w_1 (c_1 - u) + ... + w_K (c_K - u) over the request's K conditions (generate(cond_weights=)). Needs an LLM built
+    with cfg_scale > 1 and no sjd_window; not with cfg_scale (the weights are the scales), given / given_mask, or cfg_interval when
+    K > 1. A request takes n * K sequence slots. Requests that differ in cond_weights share the running batch."""
     temperature: float = 1.0
     top_p: float = 1.0
     top_k: int = -1
@@ -139,6 +156,14 @@ class SamplingParams:
     n: int = 1
     logprobs: Optional[int] = None
     best_of: Optional[int] = None
+    cond_weights: Optional[Sequence[float]] = None
+
+    def __post_init__(self):
+        if self.cond_weights is not None and not isinstance(self.cond_weights, (str, bytes)):
+            try:
+                object.__setattr__(self, "cond_weights", tuple(self.cond_weights))
+            except TypeError:   # not a sequence: refused when a request is added
+                pass
 
 
 def _wants_logprobs(p: SamplingParams) -> bool:
@@ -199,6 +224,13 @@ class _Request:
     given: Optional[torch.Tensor] = None   # inpainting: int32 [S] on the host, the given token where given, -1 where drawn
     extends: dict = field(default_factory=dict)   # inpainting: start a of every interior given run -> its length K
     end: int = 0                           # the index after the last drawn token (max_tokens without a trailing given run)
+    weights: Optional[tuple] = None        # composable guidance: the K weights (fp32 values), or None
+    conds: Optional[list] = None           # t2i composed: the K prepared (condition, emb-mask) pairs; conds[0] is (cond, mask)
+
+    @property
+    def K(self) -> int:
+        """Conditions per image: a sample takes K sequence slots."""
+        return 1 if self.weights is None else len(self.weights)
 
 
 def _plen(req: _Request) -> int:
@@ -263,6 +295,7 @@ class LLM:
         self._slots: List[Optional[_Request]] = [None] * self.max_num_seqs
         self._depth = [0] * self.max_num_seqs          # tokens sampled so far per slot (== position of the next input)
         self._img = [0] * self.max_num_seqs            # image index of every slot's sample within its request
+        self._lead = list(range(self.max_num_seqs))    # the lead slot of every slot's sample (itself, except for condition slots)
         self._params: Optional[SamplingParams] = None  # sampling parameters of the running set
         self._state = None                             # device tensors, allocated for (max_num_seqs, max_tokens)
         self.steps_run = 0
@@ -281,22 +314,33 @@ class LLM:
         call with prompt).
         given, given_mask: inpainting, token ids [max_tokens] and a bool mask [max_tokens] with at least one False (generate()'s checks
         at B = 1); the request keeps given[k] wherever given_mask[k] is True and draws the rest. Not with prefix, sjd_window, logprobs
-        or best_of. A null-class twin takes its conditional request's (passing other ones is an error)."""
+        or best_of. A null-class twin takes its conditional request's (passing other ones is an error).
+        With SamplingParams.cond_weights of K weights: c2i prompt_token_ids = [c_1, .., c_K] (class ids in [0, num_classes); a twin's
+        prompt stays [num_classes]); t2i prompt_embeds = a list of K captions (or one when K = 1), prompt = a list of K strings."""
+        composed = sampling_params is not None and sampling_params.cond_weights is not None
         if prompt is not None or negative_prompt is not None:
-            texts = [t for t in (prompt, negative_prompt) if t is not None]
+            many = composed and isinstance(prompt, (list, tuple))   # a composed request's K caption strings
+            texts = (list(prompt) if many else [t for t in (prompt,) if t is not None]) + [t for t in (negative_prompt,) if t is not None]
             if prompt is not None and prompt_embeds is not None:
                 raise ValueError("pass caption strings (prompts) or their features (prompt_embeds), not both")
             if negative_prompt is not None and negative_prompt_embeds is not None:
                 raise ValueError("pass negative_prompt or negative_prompt_embeds, not both")
             feats = self._encode_prompts(texts)
             if prompt is not None:
-                prompt_embeds = feats.pop(0)
+                prompt_embeds = feats[:len(prompt)] if many else feats.pop(0)
+                feats = feats[len(prompt):] if many else feats
             if negative_prompt is not None:
                 negative_prompt_embeds = feats.pop(0)
         if self.t2i:
             if prompt_token_ids is not None or twin_of is not None:
                 raise ValueError("a t2i LLM takes prompt_embeds (T5 caption features), not prompt_token_ids; CFG needs no twin requests")
             scale = self._guidance(sampling_params)[0]
+            if composed:
+                conds = self._captions(prompt_embeds, sampling_params)
+                negative = self._negative(negative_prompt_embeds, scale)
+                pf = self._prefix(prefix, sampling_params)
+                self._given(given, given_mask, sampling_params, pf)
+                return self._enqueue_t2i(conds[0], sampling_params, pf, negative, conds=conds)
             caption = self._caption(prompt_embeds)
             negative = self._negative(negative_prompt_embeds, scale)
             pf = self._prefix(prefix, sampling_params)
@@ -311,8 +355,7 @@ class LLM:
             raise ValueError("prompt_embeds apply to text-conditional (t2i) models; a c2i prompt is prompt_token_ids = [class id]")
         if prompt_token_ids is None:
             raise ValueError("a c2i request needs prompt_token_ids = [class id]")
-        if len(prompt_token_ids) != 1 or not (0 <= int(prompt_token_ids[0]) <= self.num_classes):
-            raise ValueError(f"a c2i prompt is one class id in [0, {self.num_classes}], got {list(prompt_token_ids)}")
+        ids = self._class_ids(prompt_token_ids, sampling_params, twin_of)
         self._guidance(sampling_params)
         if twin_of is None:
             pf = self._prefix(prefix, sampling_params)
@@ -322,13 +365,32 @@ class LLM:
             pf = self._twin_prefix(twin_of, prefix, sampling_params)
             self._twin_guidance(twin_of, sampling_params)
         rid = str(next(self.request_counter))
-        req = self._guided(_Request(rid, [int(prompt_token_ids[0])], sampling_params or SamplingParams(), twin_of, prefix=pf))
+        req = self._guided(_Request(rid, ids, sampling_params or SamplingParams(), twin_of, prefix=pf))
         self._set_given(req, gv)
         if twin_of is None:
             self._waiting.append(req)
         else:
             self._twins[twin_of] = req
         return rid
+
+    def _class_ids(self, prompt_token_ids, sampling_params: Optional[SamplingParams], twin_of=None) -> List[int]:
+        """A c2i prompt's class ids: one id in [0, num_classes] (num_classes: the null class), or for a composed request (not a twin,
+        which keeps the single null class) K ids in [0, num_classes), one per weight."""
+        if sampling_params is not None and sampling_params.cond_weights is not None and twin_of is None:
+            K = len(self._weights(sampling_params, self._guidance(sampling_params)[1]))
+            ids = list(prompt_token_ids)
+            if len(ids) != K or not all(_is_int(c) and 0 <= int(c) < self.num_classes for c in ids):
+                raise ValueError(f"a composed c2i prompt is K = {K} class ids in [0, {self.num_classes}), one per weight, got {ids}")
+            return [int(c) for c in ids]
+        if len(prompt_token_ids) != 1 or not (0 <= int(prompt_token_ids[0]) <= self.num_classes):
+            raise ValueError(f"a c2i prompt is one class id in [0, {self.num_classes}], got {list(prompt_token_ids)}")
+        return [int(prompt_token_ids[0])]
+
+    @staticmethod
+    def _composed(sampling_params, i: int) -> bool:
+        """Whether request i of an LLM.generate call (sampling_params: one SamplingParams, a list, or None) has cond_weights."""
+        sp = sampling_params[i] if isinstance(sampling_params, list) and i < len(sampling_params) else sampling_params
+        return isinstance(sp, SamplingParams) and sp.cond_weights is not None
 
     def _encode_prompts(self, prompts, prompt_embeds=None):
         """Caption strings -> one [valid_len, d_model] feature tensor each (one text_encoder call for the batch)."""
@@ -358,6 +420,20 @@ class LLM:
         embs, masks = pack_t5_features([f], max_len=T, dim=C)
         cond, mask = prepare_condition(embs, masks, left_padding=True)
         return cond[0], mask[0]
+
+    def _captions(self, feats, sampling_params: SamplingParams) -> list:
+        """A composed t2i request's K captions, [(condition, emb-mask)] prepared as _caption prepares one: feats is a list of K
+        prompt_embeds, or, when K = 1, one bare prompt_embeds."""
+        K = len(self._weights(sampling_params, -1 if sampling_params.cfg_interval is None else sampling_params.cfg_interval))
+        if feats is None:
+            raise ValueError(f"a composed t2i request needs prompt_embeds = a list of K = {K} captions' T5 features")
+        many = isinstance(feats, (list, tuple))
+        if not many and K != 1:
+            raise ValueError(f"a composed t2i request takes a list of K = {K} captions, one per weight; got one caption")
+        feats = list(feats) if many else [feats]
+        if len(feats) != K:
+            raise ValueError(f"a composed t2i request takes K = {K} captions, one per weight; got {len(feats)}")
+        return [self._caption(f) for f in feats]
 
     def _negative(self, feats, scale: Optional[float] = None):
         """A negative caption's (condition fp32 [T, caption_dim], emb-mask fp32 [T]) on the host, prepared as _caption prepares the
@@ -399,13 +475,41 @@ class LLM:
                              f"got {sp.best_of!r}")
         if self.sjd_window is not None and _wants_logprobs(sp):
             raise ValueError("logprobs and best_of cannot be combined with sjd_window")
+        self._weights(sp, int(interval))
         return scale, int(interval), None if sp.seed is None else int(sp.seed)
+
+    def _weights(self, sp: SamplingParams, interval: int) -> Optional[tuple]:
+        """A request's cond_weights as a tuple of fp32 values (None without them), checked as generate(cond_weights=) checks them at
+        B = 1, with the LLM's own conditions: unconditional rows (cfg_scale > 1), no sjd_window, and n * K, best_of * K slots."""
+        if sp.cond_weights is None:
+            return None
+        if not self.cfg_scale > 1.0:
+            raise ValueError(f"SamplingParams.cond_weights mixes each condition with the unconditional rows: it needs an LLM built with "
+                             f"cfg_scale > 1, this one has {self.cfg_scale}")
+        if sp.cfg_scale is not None:
+            raise ValueError("SamplingParams.cond_weights are the request's guidance scales; leave SamplingParams.cfg_scale at None")
+        if self.sjd_window is not None:
+            raise ValueError("SamplingParams.cond_weights cannot be combined with sjd_window")
+        if isinstance(sp.cond_weights, (str, bytes)) or not isinstance(sp.cond_weights, tuple):
+            raise ValueError(f"SamplingParams.cond_weights must be a sequence of K weights, got {sp.cond_weights!r}")
+        try:
+            w, K = _check_cond_weights(1.0, interval, sp.cond_weights)
+        except (TypeError, RuntimeError) as e:
+            raise ValueError(f"SamplingParams.cond_weights must be a sequence of K real numbers, got {sp.cond_weights!r}") from e
+        if w.dim() != 1:
+            raise ValueError(f"SamplingParams.cond_weights must be a sequence of K weights, got shape {tuple(w.shape)}")
+        m = sp.n if sp.best_of is None else sp.best_of
+        if m * K > self.max_num_seqs:
+            raise ValueError(f"a composed request takes {'best_of' if sp.best_of is not None else 'n'} * K = {m} * {K} sequence slots, more "
+                             f"than max_num_seqs = {self.max_num_seqs}")
+        return tuple(float(x) for x in w.float())
 
     def _guided(self, req: _Request) -> _Request:
         """req with its guidance, seed (None: the LLM's seed + request id) and image count resolved."""
         req.cfg, req.interval, seed = self._guidance(req.params)
         req.seed = self._seed + int(req.request_id) if seed is None else seed
         req.n = int(req.params.n if req.params.best_of is None else req.params.best_of)
+        req.weights = self._weights(req.params, req.interval) if req.twin_of is None else None
         return req
 
     def _twin_guidance(self, twin_of, sampling_params: Optional[SamplingParams]):
@@ -413,10 +517,10 @@ class LLM:
         logprobs or best_of."""
         owner = self._owner(twin_of)
         sp = sampling_params or SamplingParams()
-        mirror = lambda p: (p.cfg_scale, p.cfg_interval, p.seed, p.n, p.logprobs, p.best_of)   # noqa: E731
+        mirror = lambda p: (p.cfg_scale, p.cfg_interval, p.seed, p.n, p.logprobs, p.best_of, p.cond_weights)   # noqa: E731
         if owner is not None and mirror(sp) != mirror(owner.params):
             raise ValueError(f"a null-class twin mirrors its conditional request {twin_of!r}: its cfg_scale, cfg_interval, seed, n, "
-                             f"logprobs and best_of must be the request's")
+                             f"logprobs, best_of and cond_weights must be the request's")
 
     def _prefix(self, prefix, sampling_params: Optional[SamplingParams]) -> Optional[torch.Tensor]:
         """A request's prefix as int64 [P] on the host, checked as generate(prefix=...) checks it: integer ids in [0, vocab_size),
@@ -443,6 +547,8 @@ class LLM:
         sp = sampling_params or SamplingParams()
         if _wants_logprobs(sp):
             raise ValueError("given / given_mask cannot be combined with SamplingParams.logprobs or best_of")
+        if sp.cond_weights is not None:
+            raise ValueError("given / given_mask cannot be combined with SamplingParams.cond_weights")
         S = int(sp.max_tokens)
         g, m = [None if x is None else x.detach().cpu() if torch.is_tensor(x) else torch.as_tensor(np.asarray(x)) for x in (given, given_mask)]
         for name, x in (("given", g), ("given_mask", m)):
@@ -484,11 +590,12 @@ class LLM:
         return mine
 
     def _enqueue_t2i(self, caption, sampling_params: Optional[SamplingParams], prefix: Optional[torch.Tensor] = None, negative=None,
-                     given: Optional[torch.Tensor] = None) -> str:
+                     given: Optional[torch.Tensor] = None, conds: Optional[list] = None) -> str:
         rid = str(next(self.request_counter))
         neg, neg_mask = negative if negative is not None else (None, None)
         self._waiting.append(self._set_given(self._guided(_Request(rid, [], sampling_params or SamplingParams(), cond=caption[0],
-                                                                   mask=caption[1], prefix=prefix, neg=neg, neg_mask=neg_mask)), given))
+                                                                   mask=caption[1], prefix=prefix, neg=neg, neg_mask=neg_mask,
+                                                                   conds=conds)), given))
         return rid
 
     def _running(self) -> int:
@@ -501,17 +608,24 @@ class LLM:
         return len(self._waiting) + len({id(r) for r in self._slots if r is not None}) + len(self._twins)
 
     def _admit(self, params: SamplingParams):
-        """Admission: the waiting requests that share the running set's sampling parameters, in FIFO order, each into its n lowest free
-        slots (image j in the j-th); the first request without n free slots waits, and every request behind it. Returns [(slots, req)]."""
+        """Admission: the waiting requests that share the running set's sampling parameters, in FIFO order, each into its n K lowest free
+        slots (image j's condition i in the (j K + i)-th; K = 1 without cond_weights); the first request without n K free slots waits,
+        and every request behind it. Returns [(slots, req)]."""
         free = [i for i in range(self.max_num_seqs) if self._slots[i] is None]
         joined = []
-        while self._waiting and _batch_key(self._waiting[0].params) == _batch_key(params) and len(free) >= self._waiting[0].n:
+        while (self._waiting and _batch_key(self._waiting[0].params) == _batch_key(params) and
+               len(free) >= self._waiting[0].n * self._waiting[0].K):
             req = self._waiting.popleft()
-            slots, free = free[:req.n], free[req.n:]
-            for j, i in enumerate(slots):
-                self._slots[i], self._img[i] = req, j
+            K = req.K
+            slots, free = free[:req.n * K], free[req.n * K:]
+            for k, i in enumerate(slots):
+                self._slots[i], self._img[i], self._lead[i] = req, k // K, slots[k - k % K]
             joined.append((slots, req))
         return joined
+
+    def _sample_slots(self, lead: int) -> List[int]:
+        """The slots of the sample whose lead slot is `lead`: itself, then its condition slots."""
+        return [lead] + [s for s in range(self.max_num_seqs) if s != lead and self._lead[s] == lead and self._slots[s] is not None]
 
     def _ensure_state(self, params: SamplingParams):
         m, B = self.model, self.max_num_seqs
@@ -578,13 +692,16 @@ class LLM:
                 st["img_host"][i] = self._img[i]
         return idx
 
-    def _draw(self, st, params: SamplingParams, logits, slots: slice, step_rows, out):
+    def _draw(self, st, params: SamplingParams, logits, slots: slice, step_rows, out, mix=None):
         """One draw for each slot in `slots` from logits (its rows, cond rows first) with the slot's seed at token index step_rows:
         result -> st["tok"][slots] and out[slot, step] (out: st["out"] rows from slots.start). Under CFG each slot mixes with its own
         scale and cfg_interval (lg_sample_rows_guided with st["cfg"], st["interval"]), otherwise lg_sample_rows. When a running slot
         among them holds an image index > 0 (parallel sampling), every slot draws as its image (lg_sample_rows_keyed with st["img"]).
         While a slot among them wants logprobs, the draw is lg_sample_rows_logprobs into st["lp"] ... at the same index as out. While a
-        slot among them has given tokens, it is lg_sample_rows_given over st["given"] (a row whose token is given takes it)."""
+        slot among them has given tokens, it is lg_sample_rows_given over st["given"] (a row whose token is given takes it). While a slot
+        among them is composed, or for a composed join (mix: its gather table, weights and logits row count), it is
+        lg_sample_rows_composed over the gather table st["mix_rows"], st["mix_w"]; a batch draw then hands every lead's token to its
+        condition slots' next input (st["lead"]), on the device."""
         lib, m, n = _lib.load(), self.model, slots.stop - slots.start
         use_cfg = 1 if st["R"] == 2 * self.max_num_seqs else 0
         sc = self._sample_cfg(params)
@@ -594,7 +711,17 @@ class LLM:
         keyed = any(self._slots[i] is not None and self._img[i] > 0 for i in range(slots.start, slots.stop))
         wants = [self._slots[i].params for i in range(slots.start, slots.stop)
                  if self._slots[i] is not None and _wants_logprobs(self._slots[i].params)]
-        if any(self._slots[i] is not None and self._slots[i].given is not None for i in range(slots.start, slots.stop)):
+        if mix is not None or any(self._slots[i] is not None and self._slots[i].weights is not None for i in range(slots.start, slots.stop)):
+            rows, weights, nrows = mix if mix is not None else (st["mix_rows"][slots], st["mix_w"][slots], st["R"])
+            spec = self._logprob_spec(st, slots.start, any(p.logprobs for p in wants)) if wants else None
+            _lib.check(lib.lg_sample_rows_composed(_lib.ptr(logits), nrows, n, m.vocab_size, dt, ctypes.byref(sc), *head[6:],
+                                                   _lib.ptr(st["cfg"][slots]), _lib.ptr(st["interval"][slots]),
+                                                   _lib.ptr(st["img"][slots]), _lib.ptr(st["given"][slots]) if "given" in st else None,
+                                                   _lib.ptr(rows), _lib.ptr(weights), None if spec is None else ctypes.byref(spec), *tail),
+                       "lg_sample_rows_composed")
+            if mix is None:
+                st["tok"].copy_(st["tok"][st["lead"]])
+        elif any(self._slots[i] is not None and self._slots[i].given is not None for i in range(slots.start, slots.stop)):
             spec = self._logprob_spec(st, slots.start, any(p.logprobs for p in wants)) if wants else None
             guide = (_lib.ptr(st["cfg"][slots]), _lib.ptr(st["interval"][slots])) if use_cfg else (None, None)
             _lib.check(lib.lg_sample_rows_given(*head, *guide, _lib.ptr(st["img"][slots]) if keyed else None, _lib.ptr(st["given"][slots]),
@@ -653,56 +780,120 @@ class LLM:
                                               _lib.ptr(st["logits"]), stream), "lg_decode_rows_t2i")
         self._draw(st, params, st["logits"], slice(0, B), st["step"], st["out"])
 
-    def _device_join_t2i(self, st, params: SamplingParams, slot: int):
-        """lg_prefill_slot of the condition and mask in st["cond"][slot], st["mask"][slot], then token 0 drawn from its logits
-        (_draw: one image, the slot's seed, guidance, step 0) into st["out"][slot, 0] and st["tok"][slot]."""
+    def _device_prefill(self, st, slot: int, P: int, logits):
+        """The prefill of a join into slot's cache rows alone, its logits ([2, V] under CFG, else [1, V]) to `logits`: t2i without a
+        prefix, lg_prefill_slot of st["cond"][slot], st["mask"][slot]; otherwise lg_prefill_slot_prefix of the slot's condition (c2i: the
+        class id in st["tok"][slot]; t2i: st["cond"][slot] and st["mask"][slot]) and the P given tokens in st["out"][slot, :P]. A t2i slot
+        with a negative prefills its unconditional row with it and its mask (lg_prefill_slot_prefix_neg)."""
         B, R, dev = self.max_num_seqs, st["R"], st["dev"]
         m = self.model
         lib, handle = _lib.load(), m.engine()
         use_cfg = 1 if R == 2 * B else 0
         stream = _lib.current_stream(dev)
-        if st["has_neg"][slot]:   # the unconditional row takes the slot's negative and its mask
-            ws, ws_bytes = m._slot_prefix_scratch(use_cfg, 0)
-            _lib.check(lib.lg_prefill_slot_prefix_neg(handle, _lib.ptr(st["cond"][slot]), _lib.ptr(st["mask"][slot]), _lib.ptr(st["neg"][slot]),
-                                                      _lib.ptr(st["neg_mask"][slot]), m.cls_token_num, None, 0, slot, B, use_cfg, ws, ws_bytes,
-                                                      _lib.ptr(st["join_logits"]), stream), "lg_prefill_slot_prefix_neg")
-        else:
-            ws, ws_bytes = m._slot_scratch(use_cfg)
-            _lib.check(lib.lg_prefill_slot(handle, _lib.ptr(st["cond"][slot]), _lib.ptr(st["mask"][slot]), m.cls_token_num, slot, B, use_cfg,
-                                           ws, ws_bytes, _lib.ptr(st["join_logits"]), stream), "lg_prefill_slot")
-        self._draw(st, params, st["join_logits"], slice(slot, slot + 1), st["step0"], st["out"][slot])
-
-    def _device_join_prefix(self, st, params: SamplingParams, slot: int, P: int):
-        """The join of a completion request with P given tokens, already in st["out"][slot, :P]: lg_prefill_slot_prefix of the slot's
-        condition (c2i: the class id in st["tok"][slot]; t2i: st["cond"][slot] and st["mask"][slot]) and the prefix, then token P drawn
-        from its logits (_draw: one image, the slot's seed, guidance, step P) into st["out"][slot, P] and st["tok"][slot]."""
-        B, R, dev = self.max_num_seqs, st["R"], st["dev"]
-        m = self.model
-        lib, handle = _lib.load(), m.engine()
-        use_cfg = 1 if R == 2 * B else 0
-        stream = _lib.current_stream(dev)
+        if self.t2i and P == 0:
+            if st["has_neg"][slot]:   # the unconditional row takes the slot's negative and its mask
+                ws, ws_bytes = m._slot_prefix_scratch(use_cfg, 0)
+                _lib.check(lib.lg_prefill_slot_prefix_neg(handle, _lib.ptr(st["cond"][slot]), _lib.ptr(st["mask"][slot]),
+                                                          _lib.ptr(st["neg"][slot]), _lib.ptr(st["neg_mask"][slot]), m.cls_token_num, None, 0,
+                                                          slot, B, use_cfg, ws, ws_bytes, _lib.ptr(logits), stream), "lg_prefill_slot_prefix_neg")
+            else:
+                ws, ws_bytes = m._slot_scratch(use_cfg)
+                _lib.check(lib.lg_prefill_slot(handle, _lib.ptr(st["cond"][slot]), _lib.ptr(st["mask"][slot]), m.cls_token_num, slot, B,
+                                               use_cfg, ws, ws_bytes, _lib.ptr(logits), stream), "lg_prefill_slot")
+            return
         ws, ws_bytes = m._slot_prefix_scratch(use_cfg, P)
-        # c2i: the prefill reads the class id from tok[slot] before the draw below overwrites it (one stream)
+        # c2i: the prefill reads the class id from tok[slot] before a draw overwrites it (one stream)
         cond = _lib.ptr(st["cond"][slot]) if self.t2i else _lib.ptr(st["tok"][slot:slot + 1])
         mask = _lib.ptr(st["mask"][slot]) if self.t2i else None
         if self.t2i and st["has_neg"][slot]:
             _lib.check(lib.lg_prefill_slot_prefix_neg(handle, cond, mask, _lib.ptr(st["neg"][slot]), _lib.ptr(st["neg_mask"][slot]),
                                                       m.cls_token_num, _lib.ptr(st["out"][slot]), P, slot, B, use_cfg, ws, ws_bytes,
-                                                      _lib.ptr(st["join_logits"]), stream), "lg_prefill_slot_prefix_neg")
+                                                      _lib.ptr(logits), stream), "lg_prefill_slot_prefix_neg")
         else:
             _lib.check(lib.lg_prefill_slot_prefix(handle, cond, mask, m.cls_token_num, _lib.ptr(st["out"][slot]), P, slot, B, use_cfg, ws,
-                                                  ws_bytes, _lib.ptr(st["join_logits"]), stream), "lg_prefill_slot_prefix")
+                                                  ws_bytes, _lib.ptr(logits), stream), "lg_prefill_slot_prefix")
+
+    def _device_join_t2i(self, st, params: SamplingParams, slot: int):
+        """lg_prefill_slot of the condition and mask in st["cond"][slot], st["mask"][slot] (_device_prefill), then token 0 drawn from
+        its logits (_draw: one image, the slot's seed, guidance, step 0) into st["out"][slot, 0] and st["tok"][slot]."""
+        self._device_prefill(st, slot, 0, st["join_logits"])
+        self._draw(st, params, st["join_logits"], slice(slot, slot + 1), st["step0"], st["out"][slot])
+
+    def _device_join_prefix(self, st, params: SamplingParams, slot: int, P: int):
+        """The join of a completion request with P given tokens, already in st["out"][slot, :P]: lg_prefill_slot_prefix of the slot's
+        condition and the prefix (_device_prefill), then token P drawn from its logits (_draw: one image, the slot's seed, guidance,
+        step P) into st["out"][slot, P] and st["tok"][slot]."""
+        self._device_prefill(st, slot, P, st["join_logits"])
         st["join_step"].fill_(P)
         self._draw(st, params, st["join_logits"], slice(slot, slot + 1), st["join_step"], st["out"][slot])
 
-    def _load_caption(self, st, i: int, r: _Request):
-        """A t2i request's condition, mask and negative to slot i's device rows (before its join)."""
-        st["cond"][i].copy_(r.cond)
-        st["mask"][i].copy_(r.mask)
-        st["has_neg"][i] = r.neg is not None
-        if r.neg is not None:
-            st["neg"][i].copy_(r.neg)
-        st["neg_mask"][i].copy_(r.mask if r.neg_mask is None else r.neg_mask)
+    def _load_caption(self, st, i: int, r: _Request, c: int = 0):
+        """A t2i request's condition c (0: its own; a composed request's c-th caption), its mask and, for c = 0, its negative to slot
+        i's device rows (before its join). A condition slot's unconditional row keeps the null condition: it is never read."""
+        cond, mask = (r.cond, r.mask) if c == 0 or r.conds is None else r.conds[c]
+        neg = r.neg if c == 0 else None
+        st["cond"][i].copy_(cond)
+        st["mask"][i].copy_(mask)
+        st["has_neg"][i] = neg is not None
+        if neg is not None:
+            st["neg"][i].copy_(neg)
+        st["neg_mask"][i].copy_(mask if neg is None else r.neg_mask)
+
+    # ------------------------------------------------------------------ composable guidance (SamplingParams.cond_weights)
+    def _write_mix(self, st, joined):
+        """The joining requests' rows of the gather table (st["mix_rows"] [B, 9], st["mix_w"] [B, 8]) and of st["lead"] [B], before
+        their draws. Allocated, every row plain (-1) and every slot its own lead, when the first composed request joins; from then on
+        every join rewrites its slots' rows: a plain slot -1, a condition slot -2, a lead slot [B + lead, its K slots, -1 ...] with the
+        request's weights."""
+        if "mix_rows" not in st and all(r.weights is None for _, r in joined):
+            return
+        B, dev, M = self.max_num_seqs, st["dev"], _lib.MAX_COMPOSE
+        if "mix_rows" not in st:
+            st.update(mix_rows=torch.full((B, 1 + M), -1, dtype=torch.int32, device=dev),
+                      mix_w=torch.zeros(B, M, dtype=torch.float32, device=dev),
+                      lead=torch.arange(B, dtype=torch.long, device=dev),
+                      # a composed join: the [K, 2, V] logits of its K prefills and the gather table of its lead's draw over them
+                      join_logits_k=torch.empty(M, 2, self.model.vocab_size, dtype=torch.float32, device=dev),
+                      join_rows=torch.full((1, 1 + M), -1, dtype=torch.int32, device=dev),
+                      join_w=torch.zeros(1, M, dtype=torch.float32, device=dev))
+        idx, rows, ws = [], [], []
+        for slots, r in joined:
+            for k, s in enumerate(slots):
+                row, w = [-1] * (1 + M), [0.0] * M
+                if r.weights is not None and k % r.K == 0:
+                    row[:1 + r.K] = [B + s] + slots[k:k + r.K]
+                    w[:r.K] = r.weights
+                elif r.weights is not None:
+                    row[0] = -2
+                idx.append(s), rows.append(row), ws.append(w)
+        i = torch.tensor(idx, dtype=torch.long, device=dev)
+        st["mix_rows"][i] = torch.tensor(rows, dtype=torch.int32, device=dev)
+        st["mix_w"][i] = torch.tensor(ws, dtype=torch.float32, device=dev)
+        st["lead"][i] = torch.tensor([self._lead[s] for s in idx], dtype=torch.long, device=dev)
+
+    def _join_composed(self, st, params: SamplingParams, slots: List[int], r: _Request):
+        """The join of a composed request (slots: sample j's condition i in slots[j K + i]). A c2i request without a prefix needs none:
+        its K classes enter at position 0 and the step's decode draws token 0. Otherwise sample 0's K slots are prefilled alone
+        (_device_prefill) into st["join_logits_k"] [K, 2, V], each condition slot's K / V is copied to the same condition's slot of every
+        other sample, and token P of every sample is drawn once from those logits (lg_sample_rows_composed over rows u = 1, c_i = 2 (i - 1),
+        with the lead's seed and image index); the lead's token then becomes its condition slots' next input."""
+        K, n, P, M = r.K, r.n, _plen(r), _lib.MAX_COMPOSE
+        if not self.t2i and P == 0:
+            return
+        dev, T, buf = st["dev"], self.model.cls_token_num, st["join_logits_k"]
+        for i in range(K):
+            self._device_prefill(st, slots[i], P, buf[i])
+        if n > 1:
+            for i in range(K):
+                self._device_copy_kv(st, slots[i], [slots[j * K + i] for j in range(1, n)], T + P)
+        st["join_rows"][0] = torch.tensor([1] + [2 * i for i in range(K)] + [-1] * (M - K), dtype=torch.int32, device=dev)
+        st["join_w"][0] = torch.tensor(list(r.weights) + [0.0] * (M - K), dtype=torch.float32, device=dev)
+        st["join_step"].fill_(P)
+        for j in range(n):
+            lead = slots[j * K]
+            self._draw(st, params, buf, slice(lead, lead + 1), st["join_step"], st["out"][lead], mix=(st["join_rows"], st["join_w"], 2 * K))
+            if K > 1:
+                st["tok"][torch.tensor(slots[j * K + 1:(j + 1) * K], dtype=torch.long, device=dev)] = st["tok"][lead].clone()
 
     # ------------------------------------------------------------------ inpainting (given=, given_mask=)
     def _load_given(self, st, slots: List[int], r: _Request):
@@ -776,11 +967,23 @@ class LLM:
         """Free slot i, whose sample finished with tokens toks (and logprob rows lp); returns its request when that was the request's
         last sample."""
         req = self._slots[i]
+        for s in self._sample_slots(i)[1:]:   # a composed sample's condition slots leave with it
+            self._slots[s], self._lead[s] = None, s
         self._slots[i] = None
         req.done[self._img[i]] = toks
         if lp is not None:
             req.done_lp[self._img[i]] = lp
         return req if len(req.done) == req.n else None
+
+    def _free_rows(self, st, done: List[int]):
+        """The slots of the finished samples whose lead slots are `done` (a composed sample's condition slots too) as a device index,
+        for their rows to be reset; condition slots become their own leads again in st["lead"]."""
+        members = [s for i in done for s in self._sample_slots(i)]
+        idx = torch.tensor(members, dtype=torch.long, device=st["dev"])
+        if len(members) > len(done):
+            conds = torch.tensor([s for s in members if self._lead[s] != s], dtype=torch.long, device=st["dev"])
+            st["lead"][conds] = conds
+        return idx
 
     @staticmethod
     def _completions(req: _Request) -> List[CompletionOutput]:
@@ -937,16 +1140,21 @@ class LLM:
             self._depth[i] = _plen(r) + 1
         if joined:
             idx = self._write_guidance(st, flat)
+            self._write_mix(st, joined)
             for slots, r in joined:
                 i = slots[0]
-                for s in slots:
-                    self._load_caption(st, s, r)
+                for k, s in enumerate(slots):
+                    self._load_caption(st, s, r, k % r.K)
                 self._load_given(st, slots, r)
+                if r.prefix is not None:
+                    for s in slots:
+                        st["out"][s, :_plen(r)] = r.prefix.to(device=dev, dtype=torch.int32)
+                if r.weights is not None:   # K prefills of sample 0, their fan-out and one draw per sample
+                    self._join_composed(st, params, slots, r)
+                    continue
                 if r.prefix is None:
                     self._device_join_t2i(st, params, i)
                 else:
-                    for s in slots:
-                        st["out"][s, :_plen(r)] = r.prefix.to(device=dev, dtype=torch.int32)
                     self._device_join_prefix(st, params, i, _plen(r))
                 self._fan_out(st, params, slots, _plen(r))
             P = torch.tensor([_plen(r) for _, r in flat], dtype=torch.int32, device=dev)
@@ -956,10 +1164,10 @@ class LLM:
             st["step"][idx] = P + 1
         self.steps_run += 1
         # (3) the finished requests (their last drawn token is drawn): the only device->host copy is their token rows
-        done = [i for i in range(B) if self._slots[i] is not None and self._depth[i] >= self._slots[i].end]
+        done = [i for i in range(B) if self._slots[i] is not None and self._lead[i] == i and self._depth[i] >= self._slots[i].end]
         outs: List[RequestOutput] = []
         if done:
-            idx = torch.tensor(done, dtype=torch.long, device=dev)
+            idx = self._free_rows(st, done)
             toks, lps = self._host_rows(st, done)
             rows = torch.cat([idx, idx + B]) if R == 2 * B else idx
             st["active"][rows] = 0
@@ -1004,7 +1212,10 @@ class LLM:
             self._depth[i] = 0
         if joined:
             idx = self._write_guidance(st, flat)
-            st["tok"][idx] = torch.tensor([r.prompt_token_ids[0] for _, r in flat], dtype=torch.int32, device=dev)
+            self._write_mix(st, joined)
+            # every slot's class: a composed request's sample j takes class c_i in its condition i's slot
+            st["tok"][idx] = torch.tensor([r.prompt_token_ids[k % r.K] for slots, r in joined for k in range(len(slots))], dtype=torch.int32,
+                                          device=dev)
             rows = torch.cat([idx, idx + B]) if R == 2 * B else idx
             st["pos"][rows] = 0
             st["active"][rows] = 1
@@ -1017,14 +1228,17 @@ class LLM:
                     P = _plen(r)
                     for i in slots:
                         st["out"][i, :P] = r.prefix.to(device=dev, dtype=torch.int32)
-                    self._device_join_prefix(st, params, slots[0], P)
-                    self._fan_out(st, params, slots, P)
+                    if r.weights is not None:
+                        self._join_composed(st, params, slots, r)
+                    else:
+                        self._device_join_prefix(st, params, slots[0], P)
+                        self._fan_out(st, params, slots, P)
                     for i in slots:
                         st["pos"][[i, B + i] if R == 2 * B else [i]] = self.model.cls_token_num + P
                         self._depth[i] = P + 1
         # a request whose join drew its last drawn token (P = max_tokens - 1, or a given tail after P) finishes now, before a decode could
         # write past its out row
-        outs = self._finish_c2i(st, [i for i, r in flat if self._depth[i] >= r.end])
+        outs = self._finish_c2i(st, [i for i, r in flat if self._lead[i] == i and self._depth[i] >= r.end])
         # (2) one decode step for every slot, (3) per-request sampling; the sampled token becomes the slot's next input in place; then the
         # extends of the slots whose decode row drew the first token of a given run
         ext = []
@@ -1042,7 +1256,7 @@ class LLM:
             if self._slots[i] is not None:
                 if i not in extended:
                     self._depth[i] += 1
-                if self._depth[i] >= self._slots[i].end:
+                if self._lead[i] == i and self._depth[i] >= self._slots[i].end:
                     done.append(i)
         return outs + self._finish_c2i(st, done)
 
@@ -1052,7 +1266,7 @@ class LLM:
         B, R, dev = self.max_num_seqs, st["R"], st["dev"]
         outs: List[RequestOutput] = []
         if done:
-            idx = torch.tensor(done, dtype=torch.long, device=dev)
+            idx = self._free_rows(st, done)
             lps = [None] * len(done)
             if toks is None:                                  # the only device->host copy: token (and logprob) rows of finished requests
                 toks, lps = self._host_rows(st, done)
@@ -1099,7 +1313,9 @@ class LLM:
         c2i CFG one per conditional prompt, which its twin mirrors. negative_prompt_embeds (t2i, cfg_scale > 1): None, or one negative
         caption's features or None per request; negative_prompts: the same as strings (or None), with a text_encoder, encoded in one call
         with prompts. givens, given_masks: None, or one inpainting request's given tokens and mask (see add_request) or None per request;
-        under c2i CFG one per conditional prompt, which its twin mirrors. Returns the RequestOutputs sorted by request id."""
+        under c2i CFG one per conditional prompt, which its twin mirrors. A request whose SamplingParams has cond_weights takes K class
+        ids, K captions' features or K caption strings in its entry (see add_request); every string of the call, negatives included, goes
+        through one encoder call. Returns the RequestOutputs sorted by request id."""
         if negative_prompts is not None:
             if negative_prompt_embeds is not None:
                 raise ValueError("pass negative_prompts or negative_prompt_embeds, not both")
@@ -1111,11 +1327,15 @@ class LLM:
             if prompts is not None and prompt_embeds is not None:
                 raise ValueError("pass caption strings (prompts) or their features (prompt_embeds), not both")
             nlist = [t for t in (negative_prompts or []) if t is not None]
-            feats = self._encode_prompts(plist + nlist) if prompts is not None or nlist else []
+            # a composed request's entry may be a list of its K captions: every string of the call goes through one encoder call
+            sizes = [len(p) if isinstance(p, (list, tuple)) and self._composed(sampling_params, i) else None for i, p in enumerate(plist)]
+            flat = [t for p, k in zip(plist, sizes) for t in (p if k is not None else [p])]
+            feats = self._encode_prompts(flat + nlist) if prompts is not None or nlist else []
             if prompts is not None:
-                prompt_embeds = feats[:len(plist)]
+                it = iter(feats[:len(flat)])
+                prompt_embeds = [next(it) if k is None else [next(it) for _ in range(k)] for k in sizes]
             if negative_prompts is not None:
-                it = iter(feats[len(plist):])
+                it = iter(feats[len(flat):])
                 negative_prompt_embeds = [None if t is None else next(it) for t in negative_prompts]
         if self.t2i:
             if prompt_token_ids is not None or prompt_embeds is None:
@@ -1127,12 +1347,15 @@ class LLM:
                 raise ValueError(f"negative prompts hold {len(negative_prompt_embeds)} entries for {n} requests")
             per = sampling_params if isinstance(sampling_params, list) else [sampling_params or SamplingParams()] * n
             scales = [self._guidance(p)[0] for p in per]             # every guidance, caption, negative and prefix is checked before any
-            captions = [self._caption(f) for f in prompt_embeds]       # is queued
+            captions = [self._captions(f, p) if p.cond_weights is not None else self._caption(f)   # is queued
+                        for f, p in zip(prompt_embeds, per)]
             negs = [self._negative(f, s) for f, s in zip(negative_prompt_embeds or [None] * n, scales)]
             pfx = self._prefixes(prefixes, n, per)
             gvs = self._givens(givens, given_masks, n, per, pfx)
             for c, p, pf, ng, gv in zip(captions, per, pfx, negs, gvs):
-                if gv is not None:
+                if p.cond_weights is not None:   # a composed request's K captions
+                    self._enqueue_t2i(c[0], p, pf, ng, conds=c)
+                elif gv is not None:
                     self._enqueue_t2i(c, p, pf, ng, gv)
                 elif ng is None:
                     self._enqueue_t2i(c, p, pf)
@@ -1163,6 +1386,9 @@ class LLM:
                              "followed by one [num_classes] prompt each")
         pfx = self._prefixes(prefixes, half if paired else n, per)
         gvs = self._givens(givens, given_masks, half if paired else n, per, pfx)
+        for i in range(half if paired else n):   # a composed prompt's K class ids, before any request is queued
+            if per[i].cond_weights is not None:
+                self._class_ids(prompt_token_ids[i], per[i])
         ids = [self.add_request(prompt_token_ids[i], per[i], prefix=pfx[i]) if gvs[i] is None else
                self.add_request(prompt_token_ids[i], per[i], prefix=pfx[i], given=gvs[i], given_mask=gvs[i] >= 0)
                for i in range(half if paired else n)]
