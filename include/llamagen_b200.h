@@ -62,6 +62,15 @@ typedef struct lg_sample_cfg {
     float    top_p;         /* 1.0 = off */
     int32_t  greedy;        /* 1 == sample_logits=False (argmax) */
     uint64_t seed;          /* counter-based RNG seed for the multinomial draw */
+    /* Per-image filters: device arrays, each NULL (every image takes the scalar above) or one entry per image of the call, entry b
+     * replacing temperature, top_k, top_p or greedy for image b with the same semantics (temperature: divide by max(t, 1e-5); top_k:
+     * k <= 0 off, clamped to V; top_p: p >= 1 off, p <= 0 keeps the maximum; greedy: nonzero is argmax). Image b is image b of the call
+     * (c2i with CFG: conditional image b; a composed call: image b, not its K rows), or slot b for lg_sample_rows* and lg_sjd_pass_slots,
+     * whose window rows of slot b all read entry b. The values are not checked on the device: the caller checks them. */
+    const float*   temperature_rows;
+    const int32_t* top_k_rows;
+    const float*   top_p_rows;
+    const int32_t* greedy_rows;
 } lg_sample_cfg;
 
 typedef struct lg_engine lg_engine;

@@ -39,8 +39,11 @@ class ModelCfg(Structure):
 
 
 class SampleCfg(Structure):
+    """lg_sample_cfg. The four trailing device pointers (0 = NULL, the default) give every image its own temperature (f32), top_k
+    (int32), top_p (f32) and greedy flag (int32); positional constructions of the first seven fields keep their meaning."""
     _fields_ = [("cfg_scale", c_float), ("cfg_interval", c_int32), ("temperature", c_float),
-                ("top_k", c_int32), ("top_p", c_float), ("greedy", c_int32), ("seed", c_uint64)]
+                ("top_k", c_int32), ("top_p", c_float), ("greedy", c_int32), ("seed", c_uint64),
+                ("temperature_rows", c_void_p), ("top_k_rows", c_void_p), ("top_p_rows", c_void_p), ("greedy_rows", c_void_p)]
 
 
 class Logprobs(Structure):

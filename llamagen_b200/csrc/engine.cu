@@ -164,6 +164,7 @@ SampleArgs make_sample_args(const lg_sample_cfg& sc, const float* logits, int B,
     a.logits = logits; a.B = B; a.V = V; a.mix_cfg = mix_cfg; a.round_dtype = lg_dtype_is16(round_dtype) ? round_dtype : LG_DTYPE_F32;
     a.cfg_scale = sc.cfg_scale; a.cfg_interval = sc.cfg_interval; a.temperature = sc.temperature;
     a.top_k = sc.top_k; a.top_p = sc.top_p; a.greedy = sc.greedy; a.seed = sc.seed;
+    a.temp_rows = sc.temperature_rows; a.topk_rows = sc.top_k_rows; a.topp_rows = sc.top_p_rows; a.greedy_rows = sc.greedy_rows;
     return a;
 }
 
@@ -1774,6 +1775,11 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
         sa.given = pa.given ? pa.given + boff * S : nullptr;
         sa.dbg_logits = dbg_logits; sa.dbg_batch = B;
         if (cp.weights) { sa.mix_groups = K; sa.mix_weights = cp.weights + boff; }
+        // the chain's image b is image ioff + b of the call
+        if (sa.temp_rows) sa.temp_rows += ioff;
+        if (sa.topk_rows) sa.topk_rows += ioff;
+        if (sa.topp_rows) sa.topp_rows += ioff;
+        if (sa.greedy_rows) sa.greedy_rows += ioff;
         apply_logprobs(sa, lp, ioff * S);
     }
     std::vector<GivenSeg> lead_decode;   // lg_generate and lg_generate_prefix: LEAD P, then one DECODE run to the end
@@ -1927,6 +1933,7 @@ static int generate_sjd_impl(lg_engine* e, const Workspace& w, SjdArgs& sa, cons
     // one pass: window embedding, the layers over R * L rows at per-row positions, the head over every row, p and x for every slot
     // (B * L images, CFG twins at rows b * L + i and (B + b) * L + i), acceptance, next window
     SampleArgs sp = make_sample_args(sc, w.logits, B * L, V, use_cfg, dt);
+    sp.param_div = L;   // window rows b * L .. b * L + L - 1 are image b's
     sp.seed_rows = sa.seed_rows; sp.step_rows = sa.step_rows;
     sp.out_idx = const_cast<int32_t*>(sa.x); sp.out_probs = const_cast<float*>(sa.p);
     auto pass = [&]() -> int {
@@ -1984,7 +1991,7 @@ static int generate_sjd_entry(const char* fn, lg_engine* e, const void* cond, co
     LG_REQUIRE(ws_bytes >= need, "%s: scratch of %zu bytes is too small (%zu)", fn, ws_bytes, need);
     static_cast<KvCache&>(w) = e->full;
     sa.B = B; sa.S = S; sa.L = L; sa.V = c.vocab_size; sa.T = T; sa.nh = nh;
-    sa.greedy = sc->greedy; sa.seed = sc->seed; sa.row_offset = 0;
+    sa.greedy = sc->greedy; sa.greedy_rows = sc->greedy_rows; sa.seed = sc->seed; sa.row_offset = 0;
     sa.out = out_tokens; sa.dbg = dbg_probs;
     if (!e->sjd_done_host) {
         LG_CUDA_OK(cudaHostAlloc((void**)&e->sjd_done_host, sizeof(int), cudaHostAllocDefault));
@@ -2147,13 +2154,14 @@ int lg_sjd_pass_slots(lg_engine* e, const lg_sample_cfg* sc, const float* emb_ma
     cudaStream_t st = (cudaStream_t)stream;
     DeviceGuard guard(e->device);
     LG_TRY(e->zero_fill_if_needed(st));
-    sa.greedy = sc->greedy; sa.out = out_tokens;
+    sa.greedy = sc->greedy; sa.greedy_rows = sc->greedy_rows; sa.out = out_tokens;
     // generate_sjd_impl's pass over the slots: window embedding, the layers over nh * B * L rows at the slots' positions, the head, p and
     // x of every row with the row's seed, token index and guidance, acceptance, next window
     LG_PROF(PC_EMBED_MISC, st, launch_embed(e->tok_emb, sa.win, B * L, M, -1, D, dt, w.h, st));
     LG_TRY(e->run_layers(w, M, L, PosArg{nullptr, 0, sa.pos_rows}, emb_mask, neg_mask, B, false, st));
     LG_TRY(e->head(w, w.xn, M, w.logits, nullptr, st));
     SampleArgs sp = make_sample_args(*sc, w.logits, B * L, V, use_cfg, dt);
+    sp.param_div = L;   // window rows b * L .. b * L + L - 1 are slot b's
     sp.seed_rows = sa.seed_rows; sp.step_rows = sa.step_rows;
     sp.cfg_rows = sa.cfg_rows; sp.interval_rows = sa.interval_rows;
     sp.out_idx = const_cast<int32_t*>(sa.x); sp.out_probs = const_cast<float*>(sa.p);

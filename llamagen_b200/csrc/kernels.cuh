@@ -79,6 +79,15 @@ struct SampleArgs {
     // as in lg_sample_rows_guided; u >= 0, a lead row: unconditional row u, conditional rows in entries 1 .. K (then -1), always mixed
     // (interval_rows still drops the mix). Keys, given, logprobs and outputs are row b's. No fused tail, no dbg_logits
     const int32_t* mix_rows = nullptr;
+    // per-image sampling filters (lg_sample_cfg's *_rows): each null (the scalar above) or one entry per image; CTA b reads entry
+    // b / param_div and uses it in place of temperature, top_k, top_p and greedy, with the scalar semantics. param_div = L for the
+    // B * L window rows of a speculative-decoding pass, so that every window row of image b reads entry b; 1 otherwise (the grouped
+    // instantiation's CTA is the image without a gather table and the row with one)
+    const float* temp_rows = nullptr;      // [images] or null
+    const int32_t* topk_rows = nullptr;    // [images] or null
+    const float* topp_rows = nullptr;      // [images] or null
+    const int32_t* greedy_rows = nullptr;  // [images] or null
+    int param_div = 1;
 };
 constexpr int kMaxTopLogprobs = 20;
 constexpr int kMaxMixGroups = 8;
@@ -131,6 +140,7 @@ struct SjdArgs {
     int32_t* interval_rows = nullptr; // [B * L]
     float start_cfg = 1.f;            // a start's (first = 1, one slot) seed is `seed`; its guidance scale and cfg_interval
     int start_interval = -1;
+    const int32_t* greedy_rows = nullptr;   // [B] or null (greedy): image (slot) b's greedy flag, for acceptance and the residual draw
 };
 int launch_sjd_verify(const SjdArgs& a, cudaStream_t st);
 // slot >= 0: only image `slot` (a per-slot start, with first = 1)

@@ -160,7 +160,12 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
     const int G = kGroups ? (mr ? 1 : a.mix_groups) : 1;   // rows per image and half (a gather table: one row per CTA)
     const float* lc = a.logits + (size_t)b * G * V;
     const float* lu = a.logits + (size_t)(role >= 0 ? role : B + b * G) * V;
-    const float tdiv = fmaxf(a.temperature, 1e-5f);
+    // the image's filters: its entry of the row arrays, or the call's scalars
+    const int fr = b / a.param_div;
+    const float tdiv = fmaxf(a.temp_rows ? a.temp_rows[fr] : a.temperature, 1e-5f);
+    const int top_k = a.topk_rows ? a.topk_rows[fr] : a.top_k;
+    const float top_p = a.topp_rows ? a.topp_rows[fr] : a.top_p;
+    const bool greedy = a.greedy_rows ? a.greedy_rows[fr] != 0 : a.greedy != 0;
     const int dbgB = a.dbg_batch > 0 ? a.dbg_batch : B;
     float* dbg = a.dbg_logits ? a.dbg_logits + ((size_t)step * dbgB + a.row_offset + b) * V : nullptr;
 
@@ -258,8 +263,8 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
     // the selected VALUE is exact. The 4-pass 8-bit radix select below stays as the fallback for degenerate rows (its first
     // pass hashes sign+exponent: ~6 live buckets -> 16384 colliding atomics, measured 26.5 us per row).
     int path_topk = 0, path_trim = 0;   // dbg_path (lg_test_sample); the draw ending is s_end
-    if (a.top_k > 0) {
-        const int k = min(max(a.top_k, 1), V);
+    if (top_k > 0) {
+        const int k = min(max(top_k, 1), V);
         if (k < V) {
             __shared__ uint32_t hist2[kNB];
             __shared__ float cand[kSampleThreads];
@@ -368,7 +373,7 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
     }
 
     // ---------------- top-p (nucleus) ---------------------------------------------------------------
-    if (a.top_p < 1.0f) {
+    if (top_p < 1.0f) {
         float lm = -INFINITY;
         for (int v = tid; v < V; v += kSampleThreads) lm = fmaxf(lm, sh[v]);
         const float m = block_max(lm, red);
@@ -415,7 +420,7 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
                 for (int j = 0; j < 8; ++j) {
                     if (c[j] > 0) {
                         if (first_nonempty < 0) { first_nonempty = 255 - 8 * lane - j; firstG = G; }
-                        if (G <= a.top_p) { cand = 255 - 8 * lane - j; candG = G; }
+                        if (G <= top_p) { cand = 255 - 8 * lane - j; candG = G; }
                     }
                     G += ms[j];
                 }
@@ -450,7 +455,7 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
         const int nties = (int)(block_sum((float)lt, red) + 0.5f);
         if (nties > 1) {
             int nkeep = 1;
-            while (nkeep < nties && acc + (float)nkeep * pstar <= a.top_p) ++nkeep;
+            while (nkeep < nties && acc + (float)nkeep * pstar <= top_p) ++nkeep;
             path_trim = nkeep < nties;
             if (nkeep < nties && tid == 0) {
                 int seen = 0;
@@ -481,7 +486,7 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
     if (tid == 0) { s_pick = -1; s_end = 0; }
     __syncthreads();
 
-    if (a.greedy) {
+    if (greedy) {
         // torch.topk(probs, 1): arg-max of the probabilities; lowest index wins ties.
         float bv = -1.f;
         int bi = 0x7fffffff;
@@ -661,7 +666,7 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
 }  // namespace
 
 int launch_sample(const SampleArgs& a, cudaStream_t st) {
-    LG_REQUIRE(a.B > 0 && a.V > 0, "lg_sample: bad shape B=%d V=%d", a.B, a.V);
+    LG_REQUIRE(a.B > 0 && a.V > 0 && a.param_div >= 1, "lg_sample: bad shape B=%d V=%d param_div=%d", a.B, a.V, a.param_div);
     const bool lp = sample_wants_logprobs(a);
     const size_t smem = lp ? sample_lp_smem(a.V) : (size_t)a.V * sizeof(float);
     LG_REQUIRE(smem <= 200 * 1024, "lg_sample: vocab %d too large for the shared-memory row stage%s", a.V, lp ? " with logprobs" : "");
@@ -778,6 +783,7 @@ __global__ void __launch_bounds__(kSjdThreads) sjd_verify_kernel(SjdArgs a) {
     const int n = a.nfin[b], s = a.start[b];
     const bool active = n < S;
     const uint64_t seed = a.seed_slots ? a.seed_slots[b] : a.seed;   // per-slot mode: the slot's seed and image index
+    const bool greedy = a.greedy_rows ? a.greedy_rows[b] != 0 : a.greedy != 0;
     const int img = a.seed_slots ? (a.img_slots ? a.img_slots[b] : 0) : b + a.row_offset;
     if (active) {
         const size_t row0 = (size_t)b * L;
@@ -786,7 +792,7 @@ __global__ void __launch_bounds__(kSjdThreads) sjd_verify_kernel(SjdArgs a) {
             for (; i <= L - 2; ++i) {   // the draft for token s + i is fed in slot i + 1 and checked against p_{s + i} (slot i)
                 const int d = a.win[row0 + i + 1], k = s + i;
                 bool acc;
-                if (a.greedy) {
+                if (greedy) {
                     acc = d == a.x[row0 + i];
                 } else {
                     const float pd = a.p[(row0 + i) * V + d];
@@ -801,7 +807,7 @@ __global__ void __launch_bounds__(kSjdThreads) sjd_verify_kernel(SjdArgs a) {
         }
         __syncthreads();
         const int i = s_i;
-        if (i <= L - 2 && !a.greedy) {
+        if (i <= L - 2 && !greedy) {
             // residual draw: normalize(max(0, p - q)), inverse CDF over contiguous per-thread segments
             const float* pr = a.p + (row0 + i) * V;
             const float* qr = a.q + (row0 + i) * V;

@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import ctypes
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -19,15 +20,61 @@ def _draw_seed() -> int:
     return int(torch.randint(0, 2 ** 62, (1,), dtype=torch.int64).item())
 
 
+def _is_rows(x) -> bool:
+    """Whether a temperature / top_k / top_p argument is per image (a sequence, array or tensor with a dimension) rather than a number."""
+    return isinstance(x, (list, tuple)) or (isinstance(x, (torch.Tensor, np.ndarray)) and x.ndim > 0)
+
+
+def _filters(temperature, top_k, top_p, B):
+    """generate()'s and sample()'s temperature, top_k and top_p. Plain numbers keep the scalar path: (temperature, top_k, top_p, None)
+    converted as always. When any of them is a 1-D sequence, array or tensor, each is B per-image values (a number is repeated),
+    checked on the host (it is outside input): temperature finite and >= 0, top_k integral (k <= 0: off), top_p not NaN. Returns
+    (temperature, top_k, top_p, rows) with rows = (f32 [B], int32 [B], f32 [B]) on the host; the scalars are then unused."""
+    if not any(_is_rows(x) for x in (temperature, top_k, top_p)):
+        return float(temperature), int(top_k or 0), float(top_p), None
+
+    def rows(name, x):
+        try:
+            t = torch.as_tensor(x.detach().cpu() if torch.is_tensor(x) else np.asarray(0 if x is None else x))
+        except (TypeError, ValueError) as e:
+            raise ValueError(f"{name} must hold real numbers, got {x!r}") from e
+        if t.dtype == torch.bool or t.dtype.is_complex:
+            raise ValueError(f"{name} must hold real numbers, got dtype {t.dtype}")
+        if t.dim() > 1 or (t.dim() == 1 and t.shape[0] != B):
+            raise ValueError(f"{name} must be a number or {B} values, one per image, got shape {tuple(t.shape)}")
+        return t.to(torch.float64).expand(B)
+    t, k, p = rows("temperature", temperature), rows("top_k", top_k), rows("top_p", top_p)
+    if not bool(torch.isfinite(t).all()) or bool((t < 0).any()):
+        raise ValueError(f"temperature must be finite and >= 0, got {t.tolist()}")
+    if not bool(torch.isfinite(k).all()) or not bool((k == k.round()).all()):
+        raise ValueError(f"top_k must hold integers, got {k.tolist()}")
+    if bool(torch.isnan(p).any()):
+        raise ValueError(f"top_p must not be NaN, got {p.tolist()}")
+    return 1.0, 0, 1.0, (t.float().contiguous(), k.clamp(0, 2 ** 31 - 1).to(torch.int32).contiguous(), p.float().contiguous())
+
+
+def _sample_cfg(cfg_scale, cfg_interval, temperature, top_k, top_p, sample_logits, seed, rows, dev):
+    """The call's SampleCfg, and the device copies of its per-image filter rows (None without them), which the caller keeps alive for
+    the call. Draws the seed from torch's generator when seed is None."""
+    sc = _lib.SampleCfg(float(cfg_scale), int(cfg_interval), temperature, top_k, top_p, 0 if sample_logits else 1,
+                        _draw_seed() if seed is None else int(seed))
+    if rows is None:
+        return sc, None
+    keep = tuple(r.to(dev) for r in rows)
+    sc.temperature_rows, sc.top_k_rows, sc.top_p_rows = (r.data_ptr() for r in keep)
+    return sc, keep
+
+
 def sample(logits, temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0, sample_logits=True, seed=None):
-    """generate.py:57-66 on the device: logits [B, T, V] (last position used) -> (idx int64 [B,1], probs [B,V])."""
+    """generate.py:57-66 on the device: logits [B, T, V] (last position used) -> (idx int64 [B,1], probs [B,V]). temperature, top_k
+    and top_p may each be B per-row values (see generate())."""
     lib = _lib.load()
     x = _lib.require_cuda(logits, "sample")[:, -1, :].float().contiguous()
     B, V = x.shape
     idx = torch.empty(B, dtype=torch.int32, device=x.device)
     probs = torch.empty(B, V, dtype=torch.float32, device=x.device)
-    sc = _lib.SampleCfg(1.0, -1, float(temperature), int(top_k), float(top_p), 0 if sample_logits else 1,
-                        _draw_seed() if seed is None else int(seed))
+    temperature, top_k, top_p, rows = _filters(temperature, top_k, top_p, B)
+    sc, keep = _sample_cfg(1.0, -1, temperature, top_k, top_p, sample_logits, seed, rows, x.device)
     _lib.check(lib.lg_sample(_lib.ptr(x), B, V, 0, _lib.LG_DTYPE_F32, ctypes.byref(sc), 0, _lib.ptr(idx),
                              _lib.ptr(probs), _lib.current_stream(x.device)), "lg_sample")
     return idx.long().unsqueeze(-1), probs
@@ -36,6 +83,12 @@ def sample(logits, temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0,
 @torch.no_grad()
 def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_interval=-1, **sampling_kwargs):
     """Same contract as the reference generate() (generate.py:126-176).
+
+    temperature, top_k and top_p may each also be a 1-D sequence, array or tensor of B values, one per image (c2i with CFG: the B
+    conditional images; cond_weights: per image, not per condition). Image b then draws exactly what image b of the same call draws
+    with the plain number set to value b, on every path below (sjd_window, prefix, given, negatives, cond_weights, return_logprobs,
+    teacher, fp16, fp8). Checked on the host with ValueError: B values, temperature finite and >= 0, top_k integral (<= 0: off), top_p
+    not NaN. Plain numbers keep the scalar path.
 
     Extra keyword-only knobs (ignored by the reference signature, all optional):
       seed=int             explicit RNG seed for the multinomial draw
@@ -93,9 +146,9 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
     """
     if not isinstance(model, Transformer):
         raise TypeError("llamagen_b200.generate needs a llamagen_b200 GPT_models[...] instance")
-    temperature = float(sampling_kwargs.pop("temperature", 1.0))
-    top_k = int(sampling_kwargs.pop("top_k", 0) or 0)
-    top_p = float(sampling_kwargs.pop("top_p", 1.0))
+    temperature = sampling_kwargs.pop("temperature", 1.0)
+    top_k = sampling_kwargs.pop("top_k", 0)
+    top_p = sampling_kwargs.pop("top_p", 1.0)
     sample_logits = bool(sampling_kwargs.pop("sample_logits", True))
     seed = sampling_kwargs.pop("seed", None)
     return_logits = bool(sampling_kwargs.pop("return_logits", False))
@@ -168,7 +221,7 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
     B = cond.shape[0]
     S = int(max_new_tokens)
     use_cfg = cfg_scale > 1.0
-    rows = 2 * B if use_cfg else B
+    temperature, top_k, top_p, rows = _filters(temperature, top_k, top_p, B)
 
     em = None
     if emb_masks is not None:
@@ -184,32 +237,29 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
 
     if sjd_window is not None and S < 3:
         raise ValueError(f"sjd_window needs max_new_tokens >= 3, got {S}")
-    model.setup_caches(max_batch_size=rows, max_seq_length=T + S, dtype=model.tok_embeddings.weight.dtype)
+    model.setup_caches(max_batch_size=2 * B if use_cfg else B, max_seq_length=T + S, dtype=model.tok_embeddings.weight.dtype)
     lib, handle = _lib.load(), model.engine()
     out = torch.empty((B, S), dtype=torch.int32, device=dev)
     if gv is not None:
-        sc = _lib.SampleCfg(float(cfg_scale), int(cfg_interval), temperature, top_k, top_p, 0 if sample_logits else 1,
-                            _draw_seed() if seed is None else int(seed))
+        sc, keep = _sample_cfg(cfg_scale, cfg_interval, temperature, top_k, top_p, sample_logits, seed, rows, dev)
         ws, ws_bytes = model._given_scratch(gv, T, use_cfg)
         _lib.check(lib.lg_generate_given(handle, _lib.ptr(cond_dev), _lib.ptr(em), _lib.ptr(neg), _lib.ptr(nm), B, T, S, ctypes.byref(sc),
                                          _lib.ptr(gv), ws, ws_bytes, _lib.ptr(out), _lib.current_stream(dev)), "lg_generate_given")
         return out.to(cond.device) if cond.device != dev else out
     if sjd_window is not None:
+        sc, keep = _sample_cfg(cfg_scale, cfg_interval, temperature, top_k, top_p, sample_logits, seed, rows, dev)
         return _generate_sjd(model, lib, handle, cond, cond_dev, em, B, T, S, out, min(int(sjd_window), S - 1), use_cfg, return_stats,
-                             _lib.SampleCfg(float(cfg_scale), int(cfg_interval), temperature, top_k, top_p, 0 if sample_logits else 1,
-                                            _draw_seed() if seed is None else int(seed)), neg=neg, nm=nm)
+                             sc, neg=neg, nm=nm)
     if return_logprobs:
-        sc = _lib.SampleCfg(float(cfg_scale), int(cfg_interval), temperature, top_k, top_p, 0 if sample_logits else 1,
-                            _draw_seed() if seed is None else int(seed))
+        sc, keep = _sample_cfg(cfg_scale, cfg_interval, temperature, top_k, top_p, sample_logits, seed, rows, dev)
         return _generate_logprobs(model, lib, handle, cond, cond_dev, em, neg, nm, pf, B, T, S, sc, out, use_cfg,
                                   None if top_logprobs is None else int(top_logprobs))
     if pf is not None:
         P = pf.shape[1]
         dbg = torch.zeros((S, B, model.vocab_size), dtype=torch.float32, device=dev) if return_logits else None
         pf_dev = pf.to(device=dev, dtype=torch.int32).contiguous()
-        ws, ws_bytes = model._prefix_scratch(rows, T + P, 2 if use_cfg else 1)
-        sc = _lib.SampleCfg(float(cfg_scale), int(cfg_interval), temperature, top_k, top_p, 0 if sample_logits else 1,
-                            _draw_seed() if seed is None else int(seed))
+        ws, ws_bytes = model._prefix_scratch(2 * B if use_cfg else B, T + P, 2 if use_cfg else 1)
+        sc, keep = _sample_cfg(cfg_scale, cfg_interval, temperature, top_k, top_p, sample_logits, seed, rows, dev)
         if neg is None:
             _lib.check(lib.lg_generate_prefix(handle, _lib.ptr(cond_dev), _lib.ptr(em), B, T, S, ctypes.byref(sc), _lib.ptr(pf_dev), P, ws,
                                               ws_bytes, _lib.ptr(out), _lib.ptr(dbg), _lib.current_stream(dev)), "lg_generate_prefix")
@@ -224,8 +274,7 @@ def generate(model, cond, max_new_tokens, emb_masks=None, cfg_scale=1.0, cfg_int
     tf = teacher.to(device=dev, dtype=torch.int32).contiguous() if teacher is not None else None
     if tf is not None and tuple(tf.shape) != (B, S):
         raise ValueError("teacher must be [B, max_new_tokens]")
-    sc = _lib.SampleCfg(float(cfg_scale), int(cfg_interval), temperature, top_k, top_p, 0 if sample_logits else 1,
-                        _draw_seed() if seed is None else int(seed))
+    sc, keep = _sample_cfg(cfg_scale, cfg_interval, temperature, top_k, top_p, sample_logits, seed, rows, dev)
     if neg is None:
         _lib.check(lib.lg_generate(handle, _lib.ptr(cond_dev), _lib.ptr(em), B, T, S, ctypes.byref(sc), _lib.ptr(out),
                                    _lib.ptr(dbg), _lib.ptr(tf), _lib.current_stream(dev)), "lg_generate")
@@ -305,6 +354,7 @@ def _generate_composed(model, cond, S, emb_masks, cfg_scale, cfg_interval, cond_
                        seed, prefix, negative_cond, negative_emb_masks, return_logprobs, top_logprobs, given, given_mask):
     """generate(cond_weights=...): lg_generate_composed over B * K conditional rows (image-major) and as many unconditional rows."""
     B, K, T, w = _check_compose(model, cond, S, emb_masks, cfg_scale, cfg_interval, cond_weights, negative_cond, negative_emb_masks)
+    temperature, top_k, top_p, rows = _filters(temperature, top_k, top_p, B)   # per image, not per condition
     if prefix is not None and (given is not None or given_mask is not None):
         raise ValueError("given / given_mask cannot be combined with prefix")
     if return_logprobs and (given is not None or given_mask is not None):
@@ -331,8 +381,7 @@ def _generate_composed(model, cond, S, emb_masks, cfg_scale, cfg_interval, cond_
     model.setup_caches(max_batch_size=2 * R, max_seq_length=T + S, dtype=model.tok_embeddings.weight.dtype)
     lib, handle = _lib.load(), model.engine()
     out = torch.empty((B, S), dtype=torch.int32, device=dev)
-    sc = _lib.SampleCfg(float(cfg_scale), int(cfg_interval), temperature, top_k, top_p, 0 if sample_logits else 1,
-                        _draw_seed() if seed is None else int(seed))
+    sc, keep = _sample_cfg(cfg_scale, cfg_interval, temperature, top_k, top_p, sample_logits, seed, rows, dev)
     P, pf_dev, g_rows, ws, ws_bytes = 0, None, None, None, 0
     if pf is not None:
         P = pf.shape[1]

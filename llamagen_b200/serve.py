@@ -45,12 +45,13 @@ seed=base_seed + r) draws for image 0. Requests with and without a negative shar
 condition and its caption's mask in its unconditional row.
 
 Per-request guidance and seeds: SamplingParams(cfg_scale=, cfg_interval=, seed=) (None: the LLM's cfg_scale, -1, base_seed + r). The
-running set shares only (temperature, top_p, top_k, max_tokens); a change of these waits for the set to drain, a change of cfg_scale,
-cfg_interval or seed does not. Under CFG every slot's scale and interval sit in device arrays (st["cfg"], st["interval"]) that its
-request's join writes before its first draw, and every draw is lg_sample_rows_guided over them: a row mixes only when its scale is > 1
-and its interval allows it, so a request draws the tokens it draws alone in an LLM built with its cfg_scale (generate(cfg_scale=c,
-cfg_interval=k, seed=s) for image 0). A request's seed replaces base_seed + r in st["seeds"]. A scale > 1 needs an LLM built with
-cfg_scale > 1 (the unconditional rows); a request at scale <= 1 in such an LLM keeps its unconditional row running, unread.
+running set shares only (temperature, top_p, top_k, max_tokens) (with per_request_sampling, max_tokens alone); a change of these waits
+for the set to drain, a change of cfg_scale, cfg_interval or seed does not. Under CFG every slot's scale and interval sit in device
+arrays (st["cfg"], st["interval"]) that its request's join writes before its first draw, and every draw is lg_sample_rows_guided over
+them: a row mixes only when its scale is > 1 and its interval allows it, so a request draws the tokens it draws alone in an LLM built
+with its cfg_scale (generate(cfg_scale=c, cfg_interval=k, seed=s) for image 0). A request's seed replaces base_seed + r in st["seeds"]. A
+scale > 1 needs an LLM built with cfg_scale > 1 (the unconditional rows); a request at scale <= 1 in such an LLM keeps its
+unconditional row running, unread.
 
 Speculative Jacobi decoding (LLM(..., sjd_window=L), 2 <= L <= 64): every step() runs one SJD pass over all slots instead of one decode
 step, and makes up to L tokens of every running request final (generate(sjd_window=L)'s pass on per-slot state: lg_sjd_pass_slots).
@@ -110,6 +111,15 @@ plain one, the lead's rows and weights otherwise), and the leads' tokens become 
 frees its K slots together. Not with cfg_scale (the weights are the scales), cfg_interval when K > 1, given / given_mask or sjd_window.
 Null-class twins mirror their conditional request's cond_weights and keep the single null class as their prompt.
 
+Per-request sampling filters (LLM(..., per_request_sampling=True)): requests that differ in temperature, top_k or top_p share the running
+batch, as requests that differ in cfg_scale or seed do; only a change of max_tokens (which sizes the KV, token and given rows and the SJD
+window) still waits for the running set to drain. Without the flag a change of any of the four drains, as before. In both modes every
+join writes its slots' temperature, top_k, top_p and greedy flag to device arrays (st["temp"], st["topk"], st["topp"], st["greedy"]) before
+its first draw, and every draw, SJD passes included, reads them through SampleCfg's row arrays, so a request draws what it draws alone in
+an LLM whose running set shares its filters (generate(cond, seed=s, temperature=t, top_k=k, top_p=p) for image j). A t2i request at
+temperature 0 is greedy; c2i keeps the reference's temperature. Under the flag add_request checks the three values as generate() checks
+per-image filters (top_k -1 or 0: off), and a null-class twin must carry its request's filters.
+
 While requests are in flight the LLM owns the model's KV-cache workspace (a `generate()` call on the same model would reset it)."""
 from __future__ import annotations
 
@@ -127,7 +137,7 @@ import torch
 
 from . import _lib
 from .cond import pack_t5_features, prepare_condition
-from .generate import _check_cond_weights, _check_given, _check_prefix
+from .generate import _check_cond_weights, _check_given, _check_prefix, _filters
 
 
 @dataclass(frozen=True)
@@ -145,7 +155,11 @@ class SamplingParams:
     cond_weights: None, or K finite weights (1 <= K <= 8, any sign, zeros allowed; stored as a tuple): composable guidance, every token
     drawn from u + w_1 (c_1 - u) + ... + w_K (c_K - u) over the request's K conditions (generate(cond_weights=)). Needs an LLM built
     with cfg_scale > 1 and no sjd_window; not with cfg_scale (the weights are the scales), given / given_mask, or cfg_interval when
-    K > 1. A request takes n * K sequence slots. Requests that differ in cond_weights share the running batch."""
+    K > 1. A request takes n * K sequence slots. Requests that differ in cond_weights share the running batch.
+    temperature, top_k, top_p: the request's filters (top_k -1 or 0: off; temperature 0 on a t2i LLM: greedy). A change of them waits
+    for the running set to drain, unless the LLM was built with per_request_sampling=True: then they are per request, checked when
+    the request is added (temperature finite and >= 0, top_k an integer, top_p not NaN), and requests that differ in them share the
+    running batch."""
     temperature: float = 1.0
     top_p: float = 1.0
     top_k: int = -1
@@ -253,7 +267,8 @@ def _given_plan(given: torch.Tensor):
 
 class LLM:
     def __init__(self, gpt_model, cfg_scale: float = 1.0, num_classes: int = 1000, max_num_seqs: int = 64, seed: Optional[int] = None,
-                 kv_cache_dtype: Optional[str] = None, weight_dtype: Optional[str] = None, text_encoder=None, sjd_window: Optional[int] = None):
+                 kv_cache_dtype: Optional[str] = None, weight_dtype: Optional[str] = None, text_encoder=None, sjd_window: Optional[int] = None,
+                 per_request_sampling: bool = False):
         """kv_cache_dtype: None keeps the model's KV-cache setting (Transformer.set_kv_cache, scales included); "auto" (the model
         dtype) or "fp8" (e4m3) sets it. Passing the dtype the model already has keeps its scales.
         weight_dtype: None keeps the model's GEMM-weight storage (Transformer.set_weight_dtype, its head choice included); "auto" or
@@ -264,10 +279,14 @@ class LLM:
         valid feature rows would be.
         sjd_window: None, or an integer L in [2, 64]: every step() runs one speculative Jacobi decoding pass over all slots (up to
         min(L, max_tokens - 1) tokens of every running request per step; max_tokens >= 3, no prefix requests). sjd_passes counts the
-        passes run, sjd_tokens the tokens they made final, sjd_request_passes the passes of every finished request."""
+        passes run, sjd_tokens the tokens they made final, sjd_request_passes the passes of every finished request.
+        per_request_sampling: False (the default) keeps one (temperature, top_k, top_p) per running set: a request with other filters
+        waits until every running request finished. True makes them per request: requests that differ in them share the running batch,
+        and only a change of max_tokens drains."""
         if sjd_window is not None and (not _is_int(sjd_window) or not 2 <= int(sjd_window) <= 64):
             raise ValueError(f"sjd_window must be an integer in [2, 64], got {sjd_window!r}")
         self.sjd_window = None if sjd_window is None else int(sjd_window)
+        self.per_request_sampling = bool(per_request_sampling)
         self.sjd_passes = 0
         self.sjd_tokens = 0
         self.sjd_request_passes: dict[str, int] = {}
@@ -476,6 +495,8 @@ class LLM:
         if self.sjd_window is not None and _wants_logprobs(sp):
             raise ValueError("logprobs and best_of cannot be combined with sjd_window")
         self._weights(sp, int(interval))
+        if self.per_request_sampling:   # generate()'s checks of per-image filters, at B = 1
+            _filters((sp.temperature,), (sp.top_k,), (sp.top_p,), 1)
         return scale, int(interval), None if sp.seed is None else int(sp.seed)
 
     def _weights(self, sp: SamplingParams, interval: int) -> Optional[tuple]:
@@ -521,6 +542,10 @@ class LLM:
         if owner is not None and mirror(sp) != mirror(owner.params):
             raise ValueError(f"a null-class twin mirrors its conditional request {twin_of!r}: its cfg_scale, cfg_interval, seed, n, "
                              f"logprobs, best_of and cond_weights must be the request's")
+        filters = lambda p: (p.temperature, p.top_k, p.top_p)   # noqa: E731
+        if self.per_request_sampling and owner is not None and filters(sp) != filters(owner.params):
+            raise ValueError(f"a null-class twin mirrors its conditional request {twin_of!r}: its temperature, top_k and top_p must be "
+                             f"the request's")
 
     def _prefix(self, prefix, sampling_params: Optional[SamplingParams]) -> Optional[torch.Tensor]:
         """A request's prefix as int64 [P] on the host, checked as generate(prefix=...) checks it: integer ids in [0, vocab_size),
@@ -613,7 +638,7 @@ class LLM:
         and every request behind it. Returns [(slots, req)]."""
         free = [i for i in range(self.max_num_seqs) if self._slots[i] is None]
         joined = []
-        while (self._waiting and _batch_key(self._waiting[0].params) == _batch_key(params) and
+        while (self._waiting and self._key(self._waiting[0].params) == self._key(params) and
                len(free) >= self._waiting[0].n * self._waiting[0].K):
             req = self._waiting.popleft()
             K = req.K
@@ -622,6 +647,10 @@ class LLM:
                 self._slots[i], self._img[i], self._lead[i] = req, k // K, slots[k - k % K]
             joined.append((slots, req))
         return joined
+
+    def _key(self, p: SamplingParams):
+        """The parameters every request of the running set shares: _batch_key, or with per_request_sampling max_tokens alone."""
+        return (p.max_tokens,) if self.per_request_sampling else _batch_key(p)
 
     def _sample_slots(self, lead: int) -> List[int]:
         """The slots of the sample whose lead slot is `lead`: itself, then its condition slots."""
@@ -646,7 +675,10 @@ class LLM:
             out=torch.zeros(B, S, dtype=torch.int32, device=dev),
             logits=torch.empty(R, m.vocab_size, dtype=torch.float32, device=dev),
             join_logits=torch.empty(R // B, m.vocab_size, dtype=torch.float32, device=dev),   # a join's logits (one request's rows)
-            join_step=torch.zeros(1, dtype=torch.int32, device=dev))  # a completion request's join draws token P: its step
+            join_step=torch.zeros(1, dtype=torch.int32, device=dev),  # a completion request's join draws token P: its step
+            # every slot's sampling filters (SampleCfg's row arrays), written by its request's join
+            temp=torch.ones(B, dtype=torch.float32, device=dev), topk=torch.zeros(B, dtype=torch.int32, device=dev),
+            topp=torch.ones(B, dtype=torch.float32, device=dev), greedy=torch.zeros(B, dtype=torch.int32, device=dev))
         if R == 2 * B:   # every slot's guidance scale and cfg_interval (lg_sample_rows_guided), written by its request's join
             self._state.update(cfg=torch.full((B,), self.cfg_scale, dtype=torch.float32, device=dev),
                                interval=torch.full((B,), -1, dtype=torch.int32, device=dev))
@@ -670,18 +702,29 @@ class LLM:
             self._device_sjd_reset(self._state)
         return self._state
 
-    def _sample_cfg(self, params: SamplingParams):
-        """t2i path: temperature 0 is greedy decoding (the argmax of the mixed logits); the c2i path keeps the reference's temperature."""
-        greedy = 1 if self.t2i and params.temperature == 0 else 0
-        return _lib.SampleCfg(self.cfg_scale, -1, float(params.temperature), max(0, int(params.top_k)), float(params.top_p), greedy, 0)
+    def _filter_values(self, p: SamplingParams) -> tuple:
+        """A request's (temperature, top_k, top_p, greedy) as its slots hold them: top_k <= 0 is off (0); t2i: temperature 0 is greedy
+        decoding (the argmax of the mixed logits); the c2i path keeps the reference's temperature."""
+        return float(p.temperature), min(max(0, int(p.top_k)), 2 ** 31 - 1), float(p.top_p), 1 if self.t2i and p.temperature == 0 else 0
+
+    def _sample_cfg(self, st, params: SamplingParams, slots: slice):
+        """The SampleCfg of a draw over `slots`: the row arrays point at their slots' filters (st["temp"], st["topk"], st["topp"],
+        st["greedy"]), which the kernel reads in place of the scalars; those stay the running set's."""
+        sc = _lib.SampleCfg(self.cfg_scale, -1, *self._filter_values(params), 0)
+        sc.temperature_rows, sc.top_k_rows, sc.top_p_rows, sc.greedy_rows = (st[k][slots].data_ptr()
+                                                                             for k in ("temp", "topk", "topp", "greedy"))
+        return sc
 
     def _write_guidance(self, st, flat: List[tuple]):
-        """The joining requests' seeds, image indices and, under CFG, guidance scales and cfg_intervals, to their slots (flat: [(slot,
-        request)]) before their draws. The image indices are written only when one of them changes (a slot at image 0 that held image 0
-        writes nothing). Returns the slots as a device index."""
+        """The joining requests' seeds, image indices, sampling filters and, under CFG, guidance scales and cfg_intervals, to their slots
+        (flat: [(slot, request)]) before their draws. The image indices are written only when one of them changes (a slot at image 0
+        that held image 0 writes nothing). Returns the slots as a device index."""
         dev = st["dev"]
         idx = torch.tensor([i for i, _ in flat], dtype=torch.long, device=dev)
         st["seeds"][idx] = torch.tensor([r.seed for _, r in flat], dtype=torch.int64, device=dev)
+        f = [self._filter_values(r.params) for _, r in flat]
+        for j, (k, dt) in enumerate((("temp", torch.float32), ("topk", torch.int32), ("topp", torch.float32), ("greedy", torch.int32))):
+            st[k][idx] = torch.tensor([v[j] for v in f], dtype=dt, device=dev)
         if "cfg" in st:
             st["cfg"][idx] = torch.tensor([r.cfg for _, r in flat], dtype=torch.float32, device=dev)
             st["interval"][idx] = torch.tensor([r.interval for _, r in flat], dtype=torch.int32, device=dev)
@@ -704,7 +747,7 @@ class LLM:
         condition slots' next input (st["lead"]), on the device."""
         lib, m, n = _lib.load(), self.model, slots.stop - slots.start
         use_cfg = 1 if st["R"] == 2 * self.max_num_seqs else 0
-        sc = self._sample_cfg(params)
+        sc = self._sample_cfg(st, params, slots)
         dt = _lib.dtype_code(m.tok_embeddings.weight.dtype)   # 16-bit models round the head's logits to their dtype
         head = (_lib.ptr(logits), n, m.vocab_size, use_cfg, dt, ctypes.byref(sc), _lib.ptr(st["seeds"][slots]), _lib.ptr(step_rows))
         tail = (_lib.ptr(st["tok"][slots]), _lib.ptr(out), st["S"], _lib.current_stream(st["dev"]))
@@ -1054,7 +1097,7 @@ class LLM:
             st["events"] = [torch.cuda.Event(), torch.cuda.Event()]
         j = st["passes"] & 1
         ws, ws_bytes = self._sjd_scratch(st)
-        sc = self._sample_cfg(params)
+        sc = self._sample_cfg(st, params, slice(0, B))
         mask = _lib.ptr(st["mask"]) if self.t2i else None
         neg_mask = _lib.ptr(st["neg_mask"]) if self.t2i and use_cfg else None
         _lib.check(_lib.load().lg_sjd_pass_slots(self.model.engine(), ctypes.byref(sc), mask, neg_mask, B, use_cfg, st["S"], st["L"], ws,
