@@ -123,8 +123,10 @@ __global__ void __launch_bounds__(kWarps * 32 * (PAR_ ? NST : 1), PAR_ ? 1 : (HD
         fence_barrier_init();
     }
     __syncthreads();
-    // Programmatic dependent launch: the position counter and every key row of EARLIER steps were produced at least
-    // one kernel before the predecessor, so their TMA loads are issued before the dependency wait.
+    // Read before the dependency wait: the position (counter or per-row array) and every key row of EARLIER steps. Precondition:
+    // each must be complete when the predecessor (the QKV GEMM, which lets this kernel start before its own wait) STARTS. The
+    // engine guarantees it by launching an eager decode step's first kernel without PDL, after the sample kernel or set_counters
+    // that wrote the counter has completed; graph replay orders the step the same way (DESIGN §4, "Reads before the dependency wait").
     const int qpos = a.pos_rows ? a.pos_rows[r] : (a.pos_dev ? *a.pos_dev : 0) + a.pos_value;
     const int nkeys = FUSED ? qpos : qpos + 1;      // keys streamed from the cache (FUSED: the new key stays on chip)
     const int nchunks = (nkeys + kKC - 1) / kKC;

@@ -107,6 +107,8 @@ struct DeviceGuard {
 // programmaticStreamSerializationAllowed so its CTAs are scheduled (and run their prologue) while the
 // previous kernel drains; lg_pdl_sync() at the top of the kernel blocks until the producer grid's memory
 // is visible. Inside the captured CUDA graph these become programmatic dependency edges.
+// A kernel may read before its wait only what was complete when its predecessor STARTED (DESIGN §4, "Reads before the
+// dependency wait"). lg_launch_pdl(false, ...) launches one kernel without PDL: it starts after the previous kernel completed.
 // ---------------------------------------------------------------------------------------------
 int lg_env_flag(const char* name, int dflt);
 extern int g_lg_pdl;     // -1: read LG_PDL from the environment on first use
@@ -115,7 +117,7 @@ inline bool lg_pdl_enabled() {
     return g_lg_pdl == 1;
 }
 template <typename... KArgs, typename... Args>
-inline cudaError_t lg_launch(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+inline cudaError_t lg_launch_pdl(bool pdl, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = grid;
     cfg.blockDim = block;
@@ -123,10 +125,14 @@ inline cudaError_t lg_launch(void (*kern)(KArgs...), dim3 grid, dim3 block, size
     cfg.stream = st;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = lg_pdl_enabled() ? 1 : 0;
+    attr[0].val.programmaticStreamSerializationAllowed = pdl && lg_pdl_enabled() ? 1 : 0;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
+}
+template <typename... KArgs, typename... Args>
+inline cudaError_t lg_launch(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+    return lg_launch_pdl(true, kern, grid, block, smem, st, static_cast<Args&&>(args)...);
 }
 #ifdef __CUDACC__
 __device__ __forceinline__ void lg_pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }

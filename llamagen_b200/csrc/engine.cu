@@ -400,16 +400,17 @@ struct lg_engine {
         return 0;
     }
     // xn_ready: xn already holds RMSNorm_0(h) (the fused tail of the previous decode step's sample kernel wrote it). Rows r < B attend
-    // with emb_mask, rows r >= B with neg_mask when it is set (a negative prompt's), else with emb_mask.
+    // with emb_mask, rows r >= B with neg_mask when it is set (a negative prompt's), else with emb_mask. pdl_first false: the first
+    // kernel is launched without PDL (generate_impl's eager decode steps).
     int forward(const Workspace& w, int M, int Tq, PosArg pos, const float* emb_mask, const float* neg_mask, int B, float* logits_out,
-                bool xn_ready, cudaStream_t st);
+                bool xn_ready, cudaStream_t st, bool pdl_first = true);
     // the transformer blocks over M = R * Tq rows of w.h, leaving RMSNorm_final(h) in w.xn (batched GEMM path)
     int run_layers(const Workspace& w, int M, int Tq, PosArg pos, const float* emb_mask, const float* neg_mask, int B, bool xn_ready,
-                   cudaStream_t st);
+                   cudaStream_t st, bool pdl_first = true);
     // the condition rows of R rows: rows r < B from cond, rows r >= B from neg_cond [R - B, T, C] (t2i) or the null condition
     int embed_cond(const Workspace& w, const void* cond, const void* neg_cond, int B, int R, int T, cudaStream_t st);
     int gemm(const Workspace& w, const void* x, int M, int N, int K, const GemmWeight& wa, const GemmWeight& wb, int n_split, int* ksplit,
-             float* direct_out, cudaStream_t st, const GemmNext* next = nullptr);
+             float* direct_out, cudaStream_t st, const GemmNext* next = nullptr, bool pdl = true);
     int head(const Workspace& w, const void* x, int M, float* logits_out, const GemmNext* next, cudaStream_t st);
 };
 
@@ -556,7 +557,7 @@ size_t lg_engine::carve_given_window(RowBuffers& o, int32_t** win, int32_t** pos
 }
 
 int lg_engine::gemm(const Workspace& w, const void* x, int M, int N, int K, const GemmWeight& wa, const GemmWeight& wb, int n_split, int* ksplit,
-                    float* direct_out, cudaStream_t st, const GemmNext* next) {
+                    float* direct_out, cudaStream_t st, const GemmNext* next, bool pdl) {
     // when the plan needs a single slab the GEMM can write straight into `direct_out`
     const size_t need = gemm_partial_floats(M, N, K, wb.p ? n_split : 0, cfg.dtype, wa.scale != nullptr);
     LG_REQUIRE(need > 0, "%s", gemm_plan(M, N, K, wb.p ? n_split : 0, cfg.dtype, wa.scale != nullptr).error);
@@ -566,13 +567,13 @@ int lg_engine::gemm(const Workspace& w, const void* x, int M, int N, int K, cons
     LG_REQUIRE(dst == direct_out || need <= w.partial_floats, "gemm %dx%dx%d needs %zu partial floats, workspace holds %zu", M, N, K, need,
                w.partial_floats);
     GemmPlan plan;
-    LG_TRY(gemm_partial(x, K, wa, wb, n_split, M, N, K, cfg.dtype, dst, &plan, st, next));
+    LG_TRY(gemm_partial(x, K, wa, wb, n_split, M, N, K, cfg.dtype, dst, &plan, st, next, pdl));
     *ksplit = plan.ksplit;
     return dst == direct_out ? 1 : 0;
 }
 
 int lg_engine::forward(const Workspace& w, int M, int Tq, PosArg pos, const float* emb_mask, const float* neg_mask, int B, float* logits_out,
-                       bool xn_ready, cudaStream_t st) {
+                       bool xn_ready, cudaStream_t st, bool pdl_first) {
     const int L = cfg.n_layer, D = cfg.dim, F = cfg.ffn_dim, V = cfg.vocab_size;
     const int R = M / Tq;
     const int dt = cfg.dtype;
@@ -581,6 +582,7 @@ int lg_engine::forward(const Workspace& w, int M, int Tq, PosArg pos, const floa
         for (int l = 0; l < L; ++l) {
             const Layer& ly = layers[l];
             GemvSmall gq{ly.wqkv, nullptr, 3 * D, D, M, w.h, ly.attn_norm, cfg.norm_eps, w.partial, nullptr, nullptr, dt};
+            gq.pdl = l > 0 || pdl_first;
             LG_PROF(PC_GEMM_QKV, st, launch_gemv_small(gq, st));
             AttnArgs aa = layer_attn(w, l, R, Tq, pos, emb_mask, neg_mask, B);
             aa.qkv_partial = w.partial; aa.qkv_ksplit = 1; aa.freqs = freqs;
@@ -596,7 +598,7 @@ int lg_engine::forward(const Workspace& w, int M, int Tq, PosArg pos, const floa
         LG_PROF(PC_GEMM_HEAD, st, launch_gemv_small(gh, st));
         return 0;
     }
-    LG_TRY(run_layers(w, M, Tq, pos, emb_mask, neg_mask, B, xn_ready, st));
+    LG_TRY(run_layers(w, M, Tq, pos, emb_mask, neg_mask, B, xn_ready, st, pdl_first));
     // head on the last position only (generate.py:58 reads logits[:, -1])
     const void* xlast = w.xn;
     if (Tq > 1) {
@@ -620,12 +622,12 @@ int lg_engine::head(const Workspace& w, const void* x, int M, float* logits_out,
 }
 
 int lg_engine::run_layers(const Workspace& w, int M, int Tq, PosArg pos, const float* emb_mask, const float* neg_mask, int B, bool xn_ready,
-                          cudaStream_t st) {
+                          cudaStream_t st, bool pdl_first) {
     const int L = cfg.n_layer, D = cfg.dim, F = cfg.ffn_dim, V = cfg.vocab_size;
     const int R = M / Tq;
     const int dt = cfg.dtype;
     int ks = 1;
-    if (!xn_ready) LG_PROF(PC_EMBED_MISC, st, launch_rmsnorm(w.h, layers[0].attn_norm, w.xn, M, D, cfg.norm_eps, dt, st));
+    if (!xn_ready) LG_PROF(PC_EMBED_MISC, st, launch_rmsnorm(w.h, layers[0].attn_norm, w.xn, M, D, cfg.norm_eps, dt, st, pdl_first));
     for (int l = 0; l < L; ++l) {
         const Layer& ly = layers[l];
         const size_t eb = esz;
@@ -634,7 +636,7 @@ int lg_engine::run_layers(const Workspace& w, int M, int Tq, PosArg pos, const f
         GemmNext nx_w13{ly.w1.p, ly.w1.bytes(F, D, eb), ly.w3.p, ly.w3.bytes(F, D, eb)};
         GemmNext nx_w2{ly.w2.p, ly.w2.bytes(D, F, eb), nullptr, 0};
         GemmNext nx_qkv{last ? output.p : layers[l + 1].wqkv.p, last ? output.bytes(V, D, eb) : layers[l + 1].wqkv.bytes(3 * D, D, eb), nullptr, 0};
-        LG_PROF(PC_GEMM_QKV, st, gemm(w, w.xn, M, 3 * D, D, ly.wqkv, nullptr, 0, &ks, nullptr, st, &nx_wo));
+        LG_PROF(PC_GEMM_QKV, st, gemm(w, w.xn, M, 3 * D, D, ly.wqkv, nullptr, 0, &ks, nullptr, st, &nx_wo, l > 0 || !xn_ready || pdl_first));
         AttnArgs aa = layer_attn(w, l, R, Tq, pos, emb_mask, neg_mask, B);
         if (fuse_qkv(aa)) {
             aa.qkv_partial = w.partial; aa.qkv_ksplit = ks; aa.freqs = freqs;
@@ -1806,13 +1808,18 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
         sa.adv_step = advance ? k.w.counters + 1 : nullptr;
         sa.adv_ticket = advance ? reinterpret_cast<unsigned int*>(k.w.counters + 64) : nullptr;
     };
-    auto body = [&](Chain& k) -> int {
+    // eager: the step is launched outside graph capture. Its first kernel is then launched without PDL, so it starts only after the
+    // previous kernel (the sample kernel, whose fused tail advances the position counter at its very end, or set_counters) has
+    // completed; the fused decode attention reads that counter before its dependency wait (DESIGN §4, "Reads before the dependency
+    // wait"). In a captured step the graph orders its first node after everything launched before the graph.
+    auto body = [&](Chain& k, bool eager) -> int {
         int* d_pos = k.w.counters;
         int* d_step = k.w.counters + 1;
         // with the fused tail the previous iteration's sample kernel left h (and xn) in place
-        if (!fuse_tail) LG_PROF(PC_EMBED_MISC, k.st, launch_embed(e->tok_emb, k.w.tokens, k.B, k.R, -1, c.dim, c.dtype, k.w.h, k.st));
+        if (!fuse_tail)
+            LG_PROF(PC_EMBED_MISC, k.st, launch_embed(e->tok_emb, k.w.tokens, k.B, k.R, -1, c.dim, c.dtype, k.w.h, k.st, !eager));
         const bool xn_ready = fuse_tail && k.sa.emb_xn != nullptr;
-        LG_TRY(e->forward(k.w, k.R, 1, PosArg{d_pos, 0}, k.emb_mask, k.neg.mask, k.B, k.w.logits, xn_ready, k.st));
+        LG_TRY(e->forward(k.w, k.R, 1, PosArg{d_pos, 0}, k.emb_mask, k.neg.mask, k.B, k.w.logits, xn_ready, k.st, !eager || !fuse_tail));
         LG_PROF(PC_SAMPLE, k.st, launch_sample(k.sa, k.st));
         if (!fuse_tail) LG_PROF(PC_EMBED_MISC, k.st, launch_advance(d_pos, d_step, k.st));
         return 0;
@@ -1895,12 +1902,12 @@ static int generate_impl(lg_engine* e, const void* cond, const float* emb_mask, 
         if (sg.kind != kSegDecode) continue;
         for (int i = 0; i < sg.len; ++i) {
             if (!eager_done || !graph) {
-                for (int g = 0; g < nchains; ++g) LG_TRY(body(ch[g]));
+                for (int g = 0; g < nchains; ++g) LG_TRY(body(ch[g], true));
                 eager_done = true;
                 continue;
             }
             if (!captured)
-                for (int g = 0; g < nchains; ++g) LG_TRY(ch[g].graph.capture(ch[g].st, [&] { return body(ch[g]); }));
+                for (int g = 0; g < nchains; ++g) LG_TRY(ch[g].graph.capture(ch[g].st, [&] { return body(ch[g], false); }));
             captured = true;
             for (int g = 0; g < nchains; ++g) LG_TRY(ch[g].graph.launch(ch[g].st));
         }

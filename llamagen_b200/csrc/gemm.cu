@@ -158,7 +158,7 @@ size_t gemm_partial_floats(int M, int N, int K, int n_split, int dtype, bool w8)
 }
 
 int gemm_partial(const void* X, int ldx, const GemmWeight& wa, const GemmWeight& wb_in, int n_split, int M, int N, int K, int dtype,
-                 float* partial, GemmPlan* plan, cudaStream_t st, const GemmNext* next) {
+                 float* partial, GemmPlan* plan, cudaStream_t st, const GemmNext* next, bool pdl) {
     GemmWeight wb = wb_in;
     if (wb.p == nullptr || n_split == 0) { wb = wa; n_split = N; }
     LG_REQUIRE((wa.scale != nullptr) == (wb.scale != nullptr), "gemm: both weight segments must be fp8 or both 16-bit");
@@ -177,30 +177,30 @@ int gemm_partial(const void* X, int ldx, const GemmWeight& wa, const GemmWeight&
             if (lg_first_on_device(attr)) {
                 LG_CUDA_OK(cudaFuncSetAttribute(gemm_skinny_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             }
-            (void)lg_launch(gemm_skinny_kernel<float>, dim3(grid), dim3(kSkinnyWarps * 32), smem, st, 
+            (void)lg_launch_pdl(pdl, gemm_skinny_kernel<float>, dim3(grid), dim3(kSkinnyWarps * 32), smem, st, 
                 (const float*)X, ldx, (const float*)Wa, (const float*)Wb, n_split, M, N, K, kper, partial);
         } else if (dtype == LG_DTYPE_F16) {
             const size_t smem = (size_t)kSkinnyRT * kSkinnyKC * sizeof(f16);
-            (void)lg_launch(gemm_skinny_kernel<f16>, dim3(grid), dim3(kSkinnyWarps * 32), smem, st,
+            (void)lg_launch_pdl(pdl, gemm_skinny_kernel<f16>, dim3(grid), dim3(kSkinnyWarps * 32), smem, st,
                 (const f16*)X, ldx, (const f16*)Wa, (const f16*)Wb, n_split, M, N, K, kper, partial);
         } else {
             const size_t smem = (size_t)kSkinnyRT * kSkinnyKC * sizeof(bf16);
-            (void)lg_launch(gemm_skinny_kernel<bf16>, dim3(grid), dim3(kSkinnyWarps * 32), smem, st, 
+            (void)lg_launch_pdl(pdl, gemm_skinny_kernel<bf16>, dim3(grid), dim3(kSkinnyWarps * 32), smem, st, 
                 (const bf16*)X, ldx, (const bf16*)Wa, (const bf16*)Wb, n_split, M, N, K, kper, partial);
         }
         LG_LAUNCH_CHECK();
         return 0;
     }
-    if (p.kernel == 2) return gemm_tc_partial(X, ldx, wa, wb, n_split, M, N, K, dtype, p, partial, st, next);
+    if (p.kernel == 2) return gemm_tc_partial(X, ldx, wa, wb, n_split, M, N, K, dtype, p, partial, st, next, pdl);
     mma::DenseA al{(const bf16*)X, ldx, 0, M};   // raw 16-bit elements: the same loaders serve fp16
     mma::BRows bw{(const bf16*)Wa, (const bf16*)Wb, n_split, K, 0, N};
     mma::EpiPartial epi{partial, M, N};
     if (dtype == LG_DTYPE_F16) {
-        if (p.tile == 32) return mma::launch_gemm_mma<32, 128, 1, 8, 4, f16>(al, bw, M, N, K, p.ksplit, 1, epi, st);
-        if (p.tile == 64) return mma::launch_gemm_mma<64, 128, 2, 4, 4, f16>(al, bw, M, N, K, p.ksplit, 1, epi, st);
-        return mma::launch_gemm_mma<128, 128, 2, 4, 3, f16>(al, bw, M, N, K, p.ksplit, 1, epi, st);
+        if (p.tile == 32) return mma::launch_gemm_mma<32, 128, 1, 8, 4, f16>(al, bw, M, N, K, p.ksplit, 1, epi, st, pdl);
+        if (p.tile == 64) return mma::launch_gemm_mma<64, 128, 2, 4, 4, f16>(al, bw, M, N, K, p.ksplit, 1, epi, st, pdl);
+        return mma::launch_gemm_mma<128, 128, 2, 4, 3, f16>(al, bw, M, N, K, p.ksplit, 1, epi, st, pdl);
     }
-    if (p.tile == 32) return mma::launch_gemm_mma<32, 128, 1, 8, 4>(al, bw, M, N, K, p.ksplit, 1, epi, st);
-    if (p.tile == 64) return mma::launch_gemm_mma<64, 128, 2, 4, 4>(al, bw, M, N, K, p.ksplit, 1, epi, st);
-    return mma::launch_gemm_mma<128, 128, 2, 4, 3>(al, bw, M, N, K, p.ksplit, 1, epi, st);
+    if (p.tile == 32) return mma::launch_gemm_mma<32, 128, 1, 8, 4>(al, bw, M, N, K, p.ksplit, 1, epi, st, pdl);
+    if (p.tile == 64) return mma::launch_gemm_mma<64, 128, 2, 4, 4>(al, bw, M, N, K, p.ksplit, 1, epi, st, pdl);
+    return mma::launch_gemm_mma<128, 128, 2, 4, 3>(al, bw, M, N, K, p.ksplit, 1, epi, st, pdl);
 }

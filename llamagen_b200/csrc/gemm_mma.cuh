@@ -225,7 +225,7 @@ __global__ void __launch_bounds__(kThreads) gemm_mma_kernel(AL al, BRows bw, int
 
 template <int BM, int BN, int WARPS_M, int WARPS_N, int STAGES, typename T = bf16, class AL, class Epi>
 int launch_gemm_mma(const AL& al, const BRows& bw, int M, int N, int K, int ksplit, int nbatch, const Epi& epi,
-                    cudaStream_t st) {
+                    cudaStream_t st, bool pdl = true) {
     auto kern = gemm_mma_kernel<BM, BN, WARPS_M, WARPS_N, STAGES, AL, Epi, T>;
     constexpr int smem = STAGES * (BM + BN) * 128;
     static DevOnce attr_set;
@@ -237,7 +237,7 @@ int launch_gemm_mma(const AL& al, const BRows& bw, int M, int N, int K, int kspl
     const int kper = ((kt_total + ksplit - 1) / ksplit) * BK;
     dim3 grid((M + BM - 1) / BM, (N + BN - 1) / BN, nbatch * ksplit);
     LG_REQUIRE(grid.y <= 65535 && grid.z <= 65535, "gemm: grid too large (%u, %u)", grid.y, grid.z);
-    (void)lg_launch(kern, grid, dim3(kThreads), smem, st, al, bw, M, N, K, kper, ksplit, epi);
+    (void)lg_launch_pdl(pdl, kern, grid, dim3(kThreads), smem, st, al, bw, M, N, K, kper, ksplit, epi);
     LG_LAUNCH_CHECK();
     return 0;
 }

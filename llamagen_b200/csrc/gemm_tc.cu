@@ -293,7 +293,7 @@ int gemm_tc_ksplit(int M, int N, int K) {
 
 template <int RP, typename T, bool W8>
 static int gemm_tc_launch_t(const CUtensorMap& mwa, const CUtensorMap& mwb, const CUtensorMap& mx, TcArgs& a, dim3 grid,
-                            cudaStream_t st) {
+                            bool pdl, cudaStream_t st) {
     constexpr int b_tile_bytes = RP * kBlockK * 2;
     constexpr int stage_bytes = (W8 ? kATileBytesW8 : kATileBytes) + ((b_tile_bytes + 1023) / 1024) * 1024;
     // 4 stages instead of filling shared memory: a CTA never owns more than ~8 k-blocks, and the smaller footprint lets the
@@ -305,14 +305,15 @@ static int gemm_tc_launch_t(const CUtensorMap& mwa, const CUtensorMap& mwb, cons
     if (lg_first_on_device(attr)) {
         LG_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<RP, T, W8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     }
-    (void)lg_launch(gemm_tc_kernel<RP, T, W8>, grid, dim3(kThreads), smem, st, mwa, mwb, mx, a);
+    (void)lg_launch_pdl(pdl, gemm_tc_kernel<RP, T, W8>, grid, dim3(kThreads), smem, st, mwa, mwb, mx, a);
     LG_LAUNCH_CHECK();
     return 0;
 }
 
 template <typename T, bool W8>
 static int gemm_tc_launch(const void* X, int ldx, const void* Wa, const void* Wb, int n_split, int M, int N, int K,
-                          const float* sca, const float* scb, const GemmPlan& p, float* partial, cudaStream_t st, const GemmNext* next) {
+                          const float* sca, const float* scb, const GemmPlan& p, float* partial, cudaStream_t st, const GemmNext* next,
+                          bool pdl) {
     constexpr int dt = ElemTraits<T>::dtype, wdt = W8 ? LG_DTYPE_E4M3 : dt;
     if (Wb == nullptr) { Wb = Wa; scb = sca; n_split = N; }
     LG_REQUIRE(!W8 || (sca && scb && K % kBlockK == 0 && N % kBlockN == 0), "gemm_tc: fp8 weights need row scales, K %% 64 == 0 and N %% 128 == 0");
@@ -341,21 +342,21 @@ static int gemm_tc_launch(const void* X, int ldx, const void* Wa, const void* Wb
     a.pf1 = next ? (const char*)next->p1 : nullptr; a.pfb1 = next ? next->b1 : 0;
     const dim3 grid(cdiv(N, kBlockN), ks, zblocks);
     switch (rpad) {
-        case 16: return gemm_tc_launch_t<16, T, W8>(mwa, mwb, mx, a, grid, st);
-        case 32: return gemm_tc_launch_t<32, T, W8>(mwa, mwb, mx, a, grid, st);
-        case 64: return gemm_tc_launch_t<64, T, W8>(mwa, mwb, mx, a, grid, st);
-        case 128: return gemm_tc_launch_t<128, T, W8>(mwa, mwb, mx, a, grid, st);
-        default: return gemm_tc_launch_t<256, T, W8>(mwa, mwb, mx, a, grid, st);
+        case 16: return gemm_tc_launch_t<16, T, W8>(mwa, mwb, mx, a, grid, pdl, st);
+        case 32: return gemm_tc_launch_t<32, T, W8>(mwa, mwb, mx, a, grid, pdl, st);
+        case 64: return gemm_tc_launch_t<64, T, W8>(mwa, mwb, mx, a, grid, pdl, st);
+        case 128: return gemm_tc_launch_t<128, T, W8>(mwa, mwb, mx, a, grid, pdl, st);
+        default: return gemm_tc_launch_t<256, T, W8>(mwa, mwb, mx, a, grid, pdl, st);
     }
 }
 
 int gemm_tc_partial(const void* X, int ldx, const GemmWeight& wa, const GemmWeight& wb, int n_split, int M, int N, int K, int dtype,
-                    const GemmPlan& p, float* partial, cudaStream_t st, const GemmNext* next) {
+                    const GemmPlan& p, float* partial, cudaStream_t st, const GemmNext* next, bool pdl) {
     LG_REQUIRE(lg_dtype_is16(dtype), "gemm_tc: unsupported dtype %d", dtype);
     if (wa.scale) {
-        if (dtype == LG_DTYPE_F16) return gemm_tc_launch<f16, true>(X, ldx, wa.p, wb.p, n_split, M, N, K, wa.scale, wb.scale, p, partial, st, next);
-        return gemm_tc_launch<bf16, true>(X, ldx, wa.p, wb.p, n_split, M, N, K, wa.scale, wb.scale, p, partial, st, next);
+        if (dtype == LG_DTYPE_F16) return gemm_tc_launch<f16, true>(X, ldx, wa.p, wb.p, n_split, M, N, K, wa.scale, wb.scale, p, partial, st, next, pdl);
+        return gemm_tc_launch<bf16, true>(X, ldx, wa.p, wb.p, n_split, M, N, K, wa.scale, wb.scale, p, partial, st, next, pdl);
     }
-    if (dtype == LG_DTYPE_F16) return gemm_tc_launch<f16, false>(X, ldx, wa.p, wb.p, n_split, M, N, K, nullptr, nullptr, p, partial, st, next);
-    return gemm_tc_launch<bf16, false>(X, ldx, wa.p, wb.p, n_split, M, N, K, nullptr, nullptr, p, partial, st, next);
+    if (dtype == LG_DTYPE_F16) return gemm_tc_launch<f16, false>(X, ldx, wa.p, wb.p, n_split, M, N, K, nullptr, nullptr, p, partial, st, next, pdl);
+    return gemm_tc_launch<bf16, false>(X, ldx, wa.p, wb.p, n_split, M, N, K, nullptr, nullptr, p, partial, st, next, pdl);
 }

@@ -251,7 +251,7 @@ __global__ void __launch_bounds__(kThreads) gemv_small_kernel(GemvArgs<T, std::c
 }
 
 template <int ROWS, int PF, typename T, bool W8, typename WT>
-int launch_t(const GemvArgs<T, WT>& a, cudaStream_t st) {
+int launch_t(const GemvArgs<T, WT>& a, bool pdl, cudaStream_t st) {
     constexpr int MT = ROWS == 32 ? 2 : 1;
     const size_t smem = (size_t)(kWarps * MT * 16 * 8 + 64) * sizeof(float) + (size_t)a.R * (a.K * 2 + 16);
     static DevOnce attr;
@@ -260,7 +260,7 @@ int launch_t(const GemvArgs<T, WT>& a, cudaStream_t st) {
     }
     LG_REQUIRE(smem <= 100 * 1024, "gemv_small: %zu bytes of shared memory (R=%d K=%d)", smem, a.R, a.K);
     const int rows_per_cta = a.Wb ? 16 : ROWS;
-    (void)lg_launch(gemv_small_kernel<ROWS, PF, T, W8>, dim3(a.N / rows_per_cta), dim3(kThreads), smem, st, a);
+    (void)lg_launch_pdl(pdl, gemv_small_kernel<ROWS, PF, T, W8>, dim3(a.N / rows_per_cta), dim3(kThreads), smem, st, a);
     LG_LAUNCH_CHECK();
     return 0;
 }
@@ -273,9 +273,9 @@ int launch_typed(const GemvSmall& g, const GemvSmallPlan& p, cudaStream_t st) {
     a.N = g.N; a.K = g.K; a.R = g.R;
     a.pro = g.normw ? 1 : 0; a.in = (const T*)g.in; a.normw = (const T*)g.normw; a.eps = g.eps;
     a.epi = g.Wb.p ? 2 : (g.out_f32 ? 0 : 1); a.out_f32 = g.out_f32; a.h = (T*)g.h; a.ff = (T*)g.ff;
-    if (p.rows == 8) return launch_t<8, 12, T, W8>(a, st);
-    if (p.rows == 16) return launch_t<16, 4, T, W8>(a, st);
-    return launch_t<32, 4, T, W8>(a, st);
+    if (p.rows == 8) return launch_t<8, 12, T, W8>(a, g.pdl, st);
+    if (p.rows == 16) return launch_t<16, 4, T, W8>(a, g.pdl, st);
+    return launch_t<32, 4, T, W8>(a, g.pdl, st);
 }
 
 }  // namespace

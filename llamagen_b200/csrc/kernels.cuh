@@ -179,8 +179,9 @@ struct GemmNext {
 // floats of fp32 slabs the call's plan writes (0 for an invalid call); partial must hold that many
 size_t gemm_partial_floats(int M, int N, int K, int n_split, int dtype, bool w8 = false);
 // runs the call on the kernel gemm_plan picks; *plan (optional) receives that plan. wb.p null: wa alone
+// pdl false: launched without PDL (lg_launch_pdl), so it starts after the stream's previous kernel completed
 int gemm_partial(const void* X, int ldx, const GemmWeight& wa, const GemmWeight& wb, int n_split, int M, int N, int K,
-                 int dtype, float* partial, GemmPlan* plan, cudaStream_t st, const GemmNext* next = nullptr);
+                 int dtype, float* partial, GemmPlan* plan, cudaStream_t st, const GemmNext* next = nullptr, bool pdl = true);
 
 // ------------------------------------------------------------------------------------------------
 // xf_kernels.cu — transformer glue kernels (all templated on the activation dtype internally)
@@ -193,7 +194,7 @@ struct PosArg {            // position of row-block: pos = (rows ? rows[r] : (de
 
 // out[r,:] = table[idx(r),:]; idx(r) = r < B ? src[r] : (null_idx >= 0 ? null_idx : src[r-B])
 int launch_embed(const void* table, const int32_t* src, int B, int R, int null_idx, int D, int dtype,
-                 void* out, cudaStream_t st);
+                 void* out, cudaStream_t st, bool pdl = true);
 // continuous batching, c2i: row r at position 0 takes the class embedding (cond rows: label src[r], uncond rows: null_idx),
 // at any other position the token embedding of src[r % B]
 int launch_embed_rows(const void* cls_table, const void* tok_table, const int32_t* src, const int* pos_rows, int B, int R, int null_idx,
@@ -203,7 +204,7 @@ int launch_embed_rows(const void* cls_table, const void* tok_table, const int32_
 int launch_build_caption_rows(const void* cond, const void* uncond, size_t uncond_stride, int B, int R, int T, int C, int dtype,
                               void* out, cudaStream_t st);
 // xn = rmsnorm(x) * w   (gpt.py:143-148)
-int launch_rmsnorm(const void* x, const void* w, void* xn, int M, int D, float eps, int dtype, cudaStream_t st);
+int launch_rmsnorm(const void* x, const void* w, void* xn, int M, int D, float eps, int dtype, cudaStream_t st, bool pdl = true);
 
 struct QkvEpiArgs {
     const float* partial; int ksplit;   // [ks][M][3D]
@@ -353,7 +354,7 @@ int conv_tc_make_phase_weights(const float* w_f32, bf16* out, int cout, int cin,
 // gemm_tc.cu — wgmma/TMA weight-streaming GEMM (bf16 or fp16 activations, 16-bit or fp8 weights, row blocks of <= 256)
 int gemm_tc_ksplit(int M, int N, int K);
 int gemm_tc_partial(const void* X, int ldx, const GemmWeight& wa, const GemmWeight& wb, int n_split, int M, int N, int K, int dtype,
-                    const GemmPlan& p, float* partial, cudaStream_t st, const GemmNext* next = nullptr);   // p.kernel 2
+                    const GemmPlan& p, float* partial, cudaStream_t st, const GemmNext* next = nullptr, bool pdl = true);   // p.kernel 2
 
 // gemv_small.cu — decode GEMMs for R <= 8 rows: CTA-owned output columns (no split-K), RMSNorm in the prologue (normw != null),
 // epilogue by destination: out_f32 [R][N] | h (in-place residual add) | ff (SwiGLU gate of the Wa/Wb row pair)
@@ -364,6 +365,7 @@ struct GemvSmall {
     const void* normw; float eps;     // RMSNorm weight [K] or null
     float* out_f32; void* h; void* ff;
     int dtype;                        // LG_DTYPE_BF16 or LG_DTYPE_F16: every 16-bit tensor above
+    bool pdl = true;                  // false: launched without PDL, it starts after the stream's previous kernel completed
 };
 // The instantiation a call runs on: rows = weight rows per CTA (8, 16 or 32; the paired form is 32: 16 rows of Wa and of Wb), pf =
 // 32-wide k chunks in flight per warp. rows 0: the call is not supported (bf16 / fp16, 1 <= R <= 8, K % 32 == 0, K >= 256,

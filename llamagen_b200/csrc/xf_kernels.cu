@@ -478,11 +478,11 @@ int dispatch_dtype(int dtype, F f) {
 }  // namespace
 
 int launch_embed(const void* table, const int32_t* src, int B, int R, int null_idx, int D, int dtype, void* out,
-                 cudaStream_t st) {
+                 cudaStream_t st, bool pdl) {
     return dispatch_dtype(
         dtype, [&](auto z) {
             using E = decltype(z);
-            (void)lg_launch(embed_kernel<E>, dim3(R), dim3(128), 0, st, (const E*)table, src, B, null_idx, D, (E*)out);
+            (void)lg_launch_pdl(pdl, embed_kernel<E>, dim3(R), dim3(128), 0, st, (const E*)table, src, B, null_idx, D, (E*)out);
             LG_LAUNCH_CHECK();
             return 0;
         });
@@ -521,11 +521,11 @@ int launch_gather_last(const void* in, int R, int T, int D, int dtype, void* out
         });
 }
 
-int launch_rmsnorm(const void* x, const void* w, void* xn, int M, int D, float eps, int dtype, cudaStream_t st) {
+int launch_rmsnorm(const void* x, const void* w, void* xn, int M, int D, float eps, int dtype, cudaStream_t st, bool pdl) {
     return dispatch_dtype(
         dtype, [&](auto z) {
             using E = decltype(z);
-            (void)lg_launch(rmsnorm_kernel<E>, dim3(M), dim3(256), 0, st, (const E*)x, (const E*)w, (E*)xn, D, eps);
+            (void)lg_launch_pdl(pdl, rmsnorm_kernel<E>, dim3(M), dim3(256), 0, st, (const E*)x, (const E*)w, (E*)xn, D, eps);
             LG_LAUNCH_CHECK();
             return 0;
         });

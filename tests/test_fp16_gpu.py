@@ -151,9 +151,8 @@ def test_f16_is_closer_to_fp32_than_bf16():
 
 def test_f16_paths_agree(monkeypatch):
     """CUDA-core attention and the mma.sync GEMM stay within the calibrated bound of the default path; the default path (CUDA-graph
-    replay, fused sampling tail) is bit-identical to two-chain decode, to the unfused tail and to eager launches of the unfused
-    tail. Eager launches WITH the fused tail are left out: under programmatic dependent launch the next step's attention kernel
-    can read the position counter before the sample kernel that advances it has finished (bf16 is affected the same way)."""
+    replay, fused sampling tail) is bit-identical to two-chain decode, to the unfused tail and to eager launches with the tail off
+    and on (with it, the sample kernel advances the position counter that the next step's fused attention reads)."""
     g = load_golden("gpt_c2i.pt")
     B, S = 48, 8
     cond = torch.randint(0, 10, (B,), generator=torch.Generator().manual_seed(3))
@@ -176,7 +175,8 @@ def test_f16_paths_agree(monkeypatch):
     for env in ({"LG_ATTN_TMA": "0", "LG_SPLIT": "1"}, {"LG_GEMM_TC": "0", "LG_SPLIT": "1"}):
         _, logits, _ = run(env)
         assert (logits - base[1]).abs().max().item() <= tol, env
-    for env in ({"LG_SPLIT": "2"}, {"LG_FUSE_TAIL": "0", "LG_SPLIT": "1"}, {"LG_NO_GRAPH": "1", "LG_FUSE_TAIL": "0", "LG_SPLIT": "1"}):
+    for env in ({"LG_SPLIT": "2"}, {"LG_FUSE_TAIL": "0", "LG_SPLIT": "1"}, {"LG_NO_GRAPH": "1", "LG_FUSE_TAIL": "0", "LG_SPLIT": "1"},
+                {"LG_NO_GRAPH": "1", "LG_SPLIT": "1"}):
         other = run(env)
         for i in range(3):
             assert torch.equal(other[i], base[i]), (env, i)

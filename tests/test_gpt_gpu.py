@@ -55,8 +55,12 @@ def test_graph_replay_equals_eager(name, monkeypatch):
     assert torch.equal(t_graph, t_eager) and torch.equal(l_graph, l_eager)
 
 
-@pytest.mark.parametrize("name", ["gpt_c2i.pt", "gpt_t2i.pt"])
-def test_bf16_teacher_forced_vs_oracle(name):
+@pytest.mark.parametrize("name,eager", [("gpt_c2i.pt", False), ("gpt_t2i.pt", False), ("gpt_c2i.pt", True), ("gpt_t2i.pt", True)],
+                         ids=["gpt_c2i.pt", "gpt_t2i.pt", "gpt_c2i.pt-eager", "gpt_t2i.pt-eager"])
+def test_bf16_teacher_forced_vs_oracle(name, eager, monkeypatch):
+    """eager: LG_NO_GRAPH=1, every decode step launched eagerly with the fused sampling tail (graph replay otherwise)."""
+    if eager:
+        monkeypatch.setenv("LG_NO_GRAPH", "1")
     g = load_golden(name)
     m = build_gpt(g["cfg"], g["state_dict"], torch.bfloat16)
     sd = cpu_state(m)                                   # bf16 weights

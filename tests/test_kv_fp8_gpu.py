@@ -219,7 +219,9 @@ def _run_env(monkeypatch, env, build, cond, S, teacher):
 
 
 def test_fp8_paths_agree(monkeypatch):
-    """CUDA-core attention within the bound of the default; the ring-depth, chain-count, tail and graph switches bit-identical to it."""
+    """CUDA-core attention within the bound of the default; the ring-depth, chain-count, tail and graph switches bit-identical to it.
+    The eager runs (LG_NO_GRAPH=1) cover the fused tail on and off: with it, every step's position counter is advanced by the sample
+    kernel right before the next step."""
     S, B = 8, 24
     cond = torch.randint(0, 1000, (B,), generator=torch.Generator().manual_seed(3))
 
@@ -234,7 +236,7 @@ def test_fp8_paths_agree(monkeypatch):
     _, logits, _ = _run_env(monkeypatch, {"LG_ATTN_TMA": "0", "LG_SPLIT": "1"}, build, cond, S, teacher)
     assert (logits - base[1]).abs().max().item() <= tol
     for env in ({"LG_ATTN_NST": "3", "LG_SPLIT": "1"}, {"LG_SPLIT": "2"}, {"LG_FUSE_TAIL": "0", "LG_SPLIT": "1"},
-                {"LG_NO_GRAPH": "1", "LG_FUSE_TAIL": "0", "LG_SPLIT": "1"}):
+                {"LG_NO_GRAPH": "1", "LG_FUSE_TAIL": "0", "LG_SPLIT": "1"}, {"LG_NO_GRAPH": "1", "LG_SPLIT": "1"}):
         other = _run_env(monkeypatch, env, build, cond, S, teacher)
         for i in range(3):
             assert torch.equal(other[i], base[i]), (env, i)
