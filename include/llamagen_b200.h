@@ -622,6 +622,14 @@ int  lg_test_prefix_chunks(lg_engine* e, int* chains);
  * length) draws those tokens; EXTEND [start, start + length) holds the given run and draws token start + length; LEAD [0, length)
  * draws token length. */
 int  lg_test_given_plan(const int32_t* given, int B, int S, int32_t* segs_out, int max_segs);
+/* Test hook: the regions of one scratch layout, as the engine carves it, without a GPU. kind names a *_workspace_bytes function and
+ * args (int64 [nargs]) its arguments: 0 lg_engine_workspace_bytes (rows, max_seq), or (rows, max_seq, g, n) for chain g's view of it
+ * when n chains split it; 1 lg_score (rows, seq); 2 lg_prefix (rows, seq); 3 lg_slot (use_cfg); 4 lg_slot_prefix (use_cfg, P);
+ * 5 lg_slot_extend (use_cfg, K); 6 lg_given (B, S, use_cfg, chains) with given (host int32 [B, S]), the extend windows laid out for
+ * that many decode chains; 7 lg_sjd (B, use_cfg, L); 8 lg_sjd_slots (B, use_cfg, L). The first cap regions go to out (int64 [cap][4])
+ * as {offset from the scratch's start, bytes, class (0 float or 16-bit data, 1 int32 / uint64 state, 2 KV cache), chain}, in carving
+ * order; a chain view reports chain g's part of each region. Returns the number of regions, or -1 after the kind's own checks. */
+int  lg_test_scratch_regions(lg_engine* e, int kind, const int64_t* args, int nargs, const int32_t* given, int64_t* out, int cap);
 /* Test hook: lg_sample_rows (seed_rows, step_rows dev, as there) with the inpainting select: given dev int32 [B, seq_stride]; where
  * given[b][step_rows[b]] >= 0 that token replaces image b's draw in out_idx (NULL allowed), out_seq (dev [B, seq_stride]) and
  * next_tokens (dev [B] or NULL). Given all -1, every draw is lg_sample_rows' draw. */

@@ -141,6 +141,7 @@ SIGNATURES = {
                                 c_void_p, c_void_p, c_void_p, c_void_p]),
     "lg_sjd_slots_workspace_bytes": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(c_size_t)]),
     "lg_sjd_slots_reset": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
+    "lg_test_scratch_regions": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int]),
     "lg_sjd_slot_start": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_uint64, c_float, c_int, c_void_p, c_void_p, c_size_t,
                                   c_void_p]),
     "lg_sjd_slot_start_image": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_uint64, c_float, c_int, c_int, c_void_p, c_void_p,

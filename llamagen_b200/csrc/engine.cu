@@ -194,19 +194,36 @@ struct Workspace : KvCache, RowBuffers {
     int head_rows = 0;        // lg_score: rows per head GEMM
 };
 
+// The class of a scratch region (lg_test_scratch_regions): float or 16-bit data, int32 / uint64 state, KV cache
+enum RegionClass { kRegionData = 0, kRegionInt = 1, kRegionKv = 2 };
+
+// lg_test_scratch_regions' log of the regions carved while it is set: {offset, bytes, class, chain} per region, offsets from the
+// scratch's start (`shift` is added: a layout carved from a point inside the scratch)
+struct RegionLog {
+    std::vector<int64_t> rows;
+    size_t shift = 0;
+    int chain = -1;   // >= 0: the chain of every region logged (one chain's layout carved on its own), else the carver's g
+};
+thread_local RegionLog* t_region_log = nullptr;
+
 // Bump allocator over a workspace from `base` (null: sizes only), 256-byte aligned regions, for chain g of n
 struct Carver {
     char* base;
     int g = 0, n = 1;
     size_t off = 0;
-    // a region of `bytes`, of which chain g takes the part from g * chain_stride on
-    char* shared(size_t bytes, size_t chain_stride) {
+    // a region of `bytes`, of which chain g takes the part from g * chain_stride on (chain_stride bytes of it with n > 1; `used` bytes
+    // of it with n = 1, when less than the whole region is ever used)
+    char* shared(size_t bytes, size_t chain_stride, int cls = kRegionData, size_t used = SIZE_MAX) {
         char* p = base ? base + off + g * chain_stride : nullptr;
+        if (t_region_log)
+            t_region_log->rows.insert(t_region_log->rows.end(), {(int64_t)(t_region_log->shift + off + g * chain_stride),
+                                                                 (int64_t)(n > 1 ? chain_stride : std::min(bytes, used)), cls,
+                                                                 t_region_log->chain >= 0 ? t_region_log->chain : g});
         off += align_up(bytes);
         return p;
     }
     // a region that scales with rows: chain g takes its g-th n-th
-    char* split(size_t bytes) { return shared(bytes, bytes / n); }
+    char* split(size_t bytes, int cls = kRegionData) { return shared(bytes, bytes / n, cls); }
 };
 
 // A captured CUDA graph of one stream's work and its executable graph
@@ -277,7 +294,7 @@ struct lg_engine {
     size_t layer_weight_bytes = 0;        // GEMM weight bytes of the largest layer as bound (the chain-count policy's measure)
     const float* freqs = nullptr;
     bool finalized = false;
-    static constexpr int kMaxChains = 2;
+    static constexpr int kMaxChains = 2;   // carve_rows' chain slices are exact while every chain count divides this
     Workspace full, sub[kMaxChains];      // sub[g]: chain g's view of `full` (multi-chain decode)
     int n_sub = 0;                        // 0: no split available
     bool use_graph = true;
@@ -370,7 +387,7 @@ struct lg_engine {
     size_t carve_slot(RowBuffers& head, char* base, int nh, int seq) const;
     size_t carve_given_window(RowBuffers& o, int32_t** win, int32_t** pos_rows, char* base, int B, int nh, int W) const;
     void carve_kv(Carver& c, KvCache& o, int rows, int max_seq, int layers, bool f8) const;
-    void carve_rows(Carver& c, RowBuffers& o, size_t M, size_t x0_rows, size_t partial_floats, size_t logits_rows) const;
+    void carve_rows(Carver& c, RowBuffers& o, size_t M, size_t x0_rows, size_t partial_floats, size_t logits_rows, int chains = 1) const;
     // the most partial floats one of a layer's four GEMMs needs at M rows
     size_t layer_partial_floats(int M) const {
         const int D = cfg.dim, F = cfg.ffn_dim, dt = cfg.dtype;
@@ -428,9 +445,9 @@ size_t lg_engine::carve(Workspace& o, char* base, int rows, int max_seq, int g, 
     }
     Carver c{base, g, n};
     carve_kv(c, o, rows, max_seq, cfg.n_layer, kv_f8);
-    carve_rows(c, o, Mmax, t2i ? Mmax : 0, pf, rows);
-    o.tokens = (int32_t*)c.split((size_t)rows * sizeof(int32_t));
-    o.counters = (int*)c.shared(kCounterInts * sizeof(int), 2 * sizeof(int));
+    carve_rows(c, o, Mmax, t2i ? Mmax : 0, pf, rows, kMaxChains);
+    o.tokens = (int32_t*)c.split((size_t)rows * sizeof(int32_t), kRegionInt);
+    o.counters = (int*)c.shared(kCounterInts * sizeof(int), 2 * sizeof(int), kRegionInt);
     o.base = base;
     return c.off;
 }
@@ -438,8 +455,8 @@ size_t lg_engine::carve(Workspace& o, char* base, int rows, int max_seq, int g, 
 // K and V of `layers` layers of [rows, H, max_seq, hdp] elements, in e4m3 (f8) or the model dtype
 void lg_engine::carve_kv(Carver& c, KvCache& o, int rows, int max_seq, int layers, bool f8) const {
     const size_t bytes = (size_t)rows * cfg.n_head * max_seq * hdp * (f8 ? 1 : esz) * layers, start = c.off;
-    o.kcache = c.split(bytes);
-    o.vcache = c.split(bytes);
+    o.kcache = c.split(bytes, kRegionKv);
+    o.vcache = c.split(bytes, kRegionKv);
     o.cache_bytes = c.off - start;
     o.rows = rows / c.n;
     o.max_seq = max_seq;
@@ -447,17 +464,19 @@ void lg_engine::carve_kv(Carver& c, KvCache& o, int rows, int max_seq, int layer
     o.kv_f8 = f8;
 }
 
-// The row buffers of M activation rows, x0_rows caption rows, partial_floats GEMM partials (a 64-float aligned n-th of them for each
-// chain) and logits_rows rows of logits
-void lg_engine::carve_rows(Carver& c, RowBuffers& o, size_t M, size_t x0_rows, size_t partial_floats, size_t logits_rows) const {
+// The row buffers of M activation rows, x0_rows caption rows, partial_floats GEMM partials and logits_rows rows of logits. The partials
+// region holds a whole number of 64-float slices for each of `chains` chains, so that chain g of n takes its n-th, 64-float aligned and
+// at least an n-th of partial_floats.
+void lg_engine::carve_rows(Carver& c, RowBuffers& o, size_t M, size_t x0_rows, size_t partial_floats, size_t logits_rows, int chains) const {
     o.h = c.split(M * cfg.dim * esz);
     o.xn = c.split(M * cfg.dim * esz);
     o.q = c.split(M * cfg.dim * esz);
     o.attn = c.split(M * cfg.dim * esz);
     o.ff = c.split(M * cfg.ffn_dim * esz);
     o.x0 = c.split(x0_rows * cfg.caption_dim * esz);
-    o.partial_floats = c.n == 1 ? partial_floats : partial_floats / c.n / 64 * 64;
-    o.partial = (float*)c.shared(partial_floats * sizeof(float), o.partial_floats * sizeof(float));
+    const size_t region = chains == 1 ? partial_floats : (partial_floats + 64 * chains - 1) / (64 * chains) * (64 * chains);
+    o.partial_floats = c.n == 1 ? partial_floats : region / c.n / 64 * 64;
+    o.partial = (float*)c.shared(region * sizeof(float), o.partial_floats * sizeof(float), kRegionData, partial_floats * sizeof(float));
     o.logits = (float*)c.split(logits_rows * cfg.vocab_size * sizeof(float));
 }
 
@@ -489,16 +508,16 @@ size_t lg_engine::carve_sjd(RowBuffers& o, SjdArgs& sa, char* base, int B, int n
     carve_rows(c, o, M, 0, std::max(layer_partial_floats((int)M), gemm_partial_floats((int)M, V, cfg.dim, 0, cfg.dtype)), M);
     sa.p = (const float*)c.split(BL * V * sizeof(float));
     sa.q = (float*)c.split(BL * V * sizeof(float));
-    sa.seed_rows = (uint64_t*)c.split(BL * sizeof(uint64_t));
-    sa.qflag = (int32_t*)c.split(BL * sizeof(int32_t));
-    sa.x = (const int32_t*)c.split(BL * sizeof(int32_t));
-    sa.win = (int32_t*)c.split(BL * sizeof(int32_t));
-    sa.step_rows = (int32_t*)c.split(BL * sizeof(int32_t));
-    sa.nfin = (int32_t*)c.split(B * sizeof(int32_t));
-    sa.start = (int32_t*)c.split(B * sizeof(int32_t));
-    sa.shift = (int32_t*)c.split(B * sizeof(int32_t));
-    sa.pos_rows = (int32_t*)c.split((size_t)nh * B * sizeof(int32_t));
-    sa.state = (int32_t*)c.split(kSjdStateInts * sizeof(int32_t));
+    sa.seed_rows = (uint64_t*)c.split(BL * sizeof(uint64_t), kRegionInt);
+    sa.qflag = (int32_t*)c.split(BL * sizeof(int32_t), kRegionInt);
+    sa.x = (const int32_t*)c.split(BL * sizeof(int32_t), kRegionInt);
+    sa.win = (int32_t*)c.split(BL * sizeof(int32_t), kRegionInt);
+    sa.step_rows = (int32_t*)c.split(BL * sizeof(int32_t), kRegionInt);
+    sa.nfin = (int32_t*)c.split(B * sizeof(int32_t), kRegionInt);
+    sa.start = (int32_t*)c.split(B * sizeof(int32_t), kRegionInt);
+    sa.shift = (int32_t*)c.split(B * sizeof(int32_t), kRegionInt);
+    sa.pos_rows = (int32_t*)c.split((size_t)nh * B * sizeof(int32_t), kRegionInt);
+    sa.state = (int32_t*)c.split(kSjdStateInts * sizeof(int32_t), kRegionInt);
     return c.off;
 }
 
@@ -507,11 +526,11 @@ size_t lg_engine::carve_sjd(RowBuffers& o, SjdArgs& sa, char* base, int B, int n
 size_t lg_engine::carve_sjd_slots(RowBuffers& o, SjdArgs& sa, char* base, int B, int nh, int L) const {
     Carver c{base, 0, 1, carve_sjd(o, sa, base, B, nh, L)};
     const size_t BL = (size_t)B * L;
-    sa.seed_slots = (uint64_t*)c.split(B * sizeof(uint64_t));
-    sa.pass_slots = (int32_t*)c.split(B * sizeof(int32_t));
+    sa.seed_slots = (uint64_t*)c.split(B * sizeof(uint64_t), kRegionInt);
+    sa.pass_slots = (int32_t*)c.split(B * sizeof(int32_t), kRegionInt);
     sa.cfg_rows = (float*)c.split(BL * sizeof(float));
-    sa.interval_rows = (int32_t*)c.split(BL * sizeof(int32_t));
-    sa.img_slots = (int32_t*)c.split(B * sizeof(int32_t));
+    sa.interval_rows = (int32_t*)c.split(BL * sizeof(int32_t), kRegionInt);
+    sa.img_slots = (int32_t*)c.split(B * sizeof(int32_t), kRegionInt);
     return c.off;
 }
 
@@ -551,8 +570,8 @@ size_t lg_engine::carve_given_window(RowBuffers& o, int32_t** win, int32_t** pos
                                 gemm_partial_floats(R, V, D, 0, dt, output.scale != nullptr)});
     Carver c{base};
     carve_rows(c, o, M, 0, pf, 0);
-    *win = (int32_t*)c.split((size_t)B * W * sizeof(int32_t));
-    *pos_rows = (int32_t*)c.split((size_t)R * sizeof(int32_t));
+    *win = (int32_t*)c.split((size_t)B * W * sizeof(int32_t), kRegionInt);
+    *pos_rows = (int32_t*)c.split((size_t)R * sizeof(int32_t), kRegionInt);
     return c.off;
 }
 
@@ -1034,7 +1053,9 @@ int lg_score(lg_engine* e, const void* cond, const float* emb_mask, const int32_
         Workspace w;
         e->carve_score(w, (char*)dev_ws, R, seq);
         LG_TRY(e->make_maps(w));
-        // K / V rows past the sequence and dims hd..hdp-1 are never written; the tensor-core attention multiplies them by exact zeros
+        // K / V rows past the sequence and dims hd..hdp-1 are never written. The tensor-core attentions read them: the hd-64 prefill
+        // kernel (seq 121..128) stages keys up to 128 and the windowed kernel (seq > 128) whole 64-key blocks, and both multiply the
+        // masked probabilities (exact zeros) by those V rows; the CUDA-core kernel of shorter sequences reads only keys it wrote
         LG_CUDA_OK(cudaMemsetAsync(w.kcache, 0, w.cache_bytes, st));
         const void* cond_c = c.model_type == LG_MODEL_C2I ? (const void*)((const int32_t*)cond + b0)
                                                           : (const void*)((const char*)cond + (size_t)b0 * T * c.caption_dim * esz);
@@ -2072,6 +2093,74 @@ int lg_sjd_slots_reset(lg_engine* e, int B, int use_cfg, int L, void* dev_ws, si
     LG_CUDA_OK(cudaMemsetAsync(dev_ws, 0, e->carve_sjd_slots(rb, sizes, nullptr, B, sa.nh, L), st));
     LG_CUDA_OK(cudaMemsetAsync(sa.nfin, 0x7f, (size_t)B * sizeof(int32_t), st));
     return 0;
+}
+
+int lg_test_scratch_regions(lg_engine* e, int kind, const int64_t* args, int nargs, const int32_t* given, int64_t* out, int cap) {
+    static const char* fn = "lg_test_scratch_regions";
+    static const int kArgs[] = {2, 2, 2, 1, 2, 2, 4, 3, 3};   // arguments of each kind (the workspace also takes 4: its chain view)
+    LG_REQUIRE(e && args && (out || cap == 0) && cap >= 0, "%s: bad argument", fn);
+    LG_REQUIRE(kind >= 0 && kind <= 8 && (nargs == kArgs[kind] || (kind == 0 && nargs == 4)), "%s: kind %d with %d arguments", fn, kind,
+               nargs);
+    int a[4] = {0, 0, 0, 0};
+    for (int i = 0; i < nargs; ++i) {
+        LG_REQUIRE(args[i] >= 0 && args[i] <= INT32_MAX, "%s: argument %d = %lld", fn, i, (long long)args[i]);
+        a[i] = (int)args[i];
+    }
+    // the same checks as the kind's *_workspace_bytes, before anything is logged
+    size_t bytes = 0;
+    std::vector<GivenSeg> segs;
+    size_t fixed = 0, prefill = 0;
+    switch (kind) {
+        case 0: LG_TRY(lg_engine_workspace_bytes(e, a[0], a[1], &bytes));
+                LG_REQUIRE(nargs == 2 || (a[3] >= 1 && a[3] <= lg_engine::kMaxChains && a[2] < a[3] && a[0] % a[3] == 0),
+                           "%s: chain %d of %d over %d rows", fn, a[2], a[3], a[0]);
+                break;
+        case 1: LG_TRY(lg_score_workspace_bytes(e, a[0], a[1], &bytes)); break;
+        case 2: LG_TRY(lg_prefix_workspace_bytes(e, a[0], a[1], &bytes)); break;
+        case 3: LG_TRY(lg_slot_workspace_bytes(e, a[0], &bytes)); break;
+        case 4: LG_TRY(lg_slot_prefix_workspace_bytes(e, a[0], a[1], &bytes)); break;
+        case 5: LG_TRY(lg_slot_extend_workspace_bytes(e, a[0], a[1], &bytes)); break;
+        case 6: LG_TRY(given_layout(fn, e, given, a[0], a[1], a[2] ? 2 : 1, segs, &fixed, &prefill));
+                LG_REQUIRE(a[3] >= 1 && a[3] <= lg_engine::kMaxChains && a[0] % a[3] == 0, "%s: %d chains over B=%d", fn, a[3], a[0]);
+                break;
+        case 7: LG_TRY(lg_sjd_workspace_bytes(e, a[0], a[1], a[2], &bytes)); break;
+        case 8: LG_TRY(lg_sjd_slots_workspace_bytes(e, a[0], a[1], a[2], &bytes)); break;
+    }
+    RegionLog log;
+    t_region_log = &log;
+    Workspace w;
+    SjdArgs sa{};
+    RowBuffers rb, head;
+    int32_t *win = nullptr, *pos = nullptr;
+    switch (kind) {
+        case 0: e->carve(w, nullptr, a[0], a[1], a[2], nargs == 4 ? a[3] : 1); break;
+        case 1: e->carve_score(w, nullptr, a[0], a[1]); break;
+        case 2: e->carve_prefix(rb, nullptr, a[0], a[1]); break;
+        case 3: e->carve_slot(rb, nullptr, a[0] ? 2 : 1, e->cfg.cls_token_num); break;
+        case 4: e->carve_slot(rb, nullptr, a[0] ? 2 : 1, e->cfg.cls_token_num + a[1]); break;
+        case 5: carve_slot_extend(e, rb, &win, &pos, head, nullptr, a[0] ? 2 : 1, std::min(a[1] + 1, kGivenWindowRows)); break;
+        case 6: {   // generate_given_impl's scratch: given [B, S], the leading run [B, P], the windows of a[3] chains, the prefill
+            const int B = a[0], S = a[1], nh = a[2] ? 2 : 1, n = a[3], P = segs[0].len, W = given_window_rows(segs);
+            Carver c{nullptr};
+            c.split((size_t)B * S * sizeof(int32_t), kRegionInt);
+            c.split((size_t)B * P * sizeof(int32_t), kRegionInt);
+            for (int g = 0; W > 0 && g < n; ++g) {
+                log.shift = c.off;
+                log.chain = g;
+                c.off += e->carve_given_window(rb, &win, &pos, nullptr, B / n, nh, W);
+            }
+            log.shift = fixed;
+            log.chain = -1;
+            if (P > 0) e->carve_prefix(rb, nullptr, nh * B, e->cfg.cls_token_num + P);
+            break;
+        }
+        case 7: e->carve_sjd(rb, sa, nullptr, a[0], a[1] ? 2 : 1, a[2]); break;
+        case 8: e->carve_sjd_slots(rb, sa, nullptr, a[0], a[1] ? 2 : 1, a[2]); break;
+    }
+    t_region_log = nullptr;
+    const int count = (int)(log.rows.size() / 4);
+    std::copy(log.rows.begin(), log.rows.begin() + 4 * std::min(count, cap), out);
+    return count;
 }
 
 }  // extern "C"
